@@ -2,11 +2,11 @@
 """Benchmark of the VoiceFixer inference hot path (BASELINE.json metric: clips/sec on 44.1 kHz 10 s clips).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
-                    [--workload gsr|ssr|longform] [--batch B] [--seconds S] [--minutes M]
+                    [--workload gsr|ssr|longform] [--batch B] [--seconds S] [--minutes M] [--dump-outputs DIR]
 
-Default workload `gsr` (what the driver runs): a step = one pass of the whole hot path (STFT+mel -> ResUNet ->
+Default workload `gsr`: a step = one pass of the whole hot path (STFT+mel -> ResUNet ->
 vocoder -> peak-normalise -> trim) over one batch of B synthetic clips per GPU (configs[1] of BASELINE.json: batch
-32 x 10 s, 1 x B200; at N GPUs each rank runs its own 32 clips = configs[3], weak scaling, the only collective being
+32 x 10 s, 1 x H100; at N GPUs each rank runs its own 32 clips = configs[3], weak scaling, the only collective being
 the start-up weight broadcast).  `ssr` = BASELINE configs[2] (SSR_UNet denoising, unet_v2 + ISTFT, batch 64);
 `longform` = configs[4] (one 30-minute stream as 60 s segments, handler() hard cuts and the margin mode).
 
@@ -14,8 +14,11 @@ Prints ONE JSON line (rank 0).  `value` = clips/s with inputs resident in HBM; `
 host-buffer entry point (pinned host buffers, H2D + D2H inside the timed region); `roofline` = the dominant kernel
 (live CUDA events) plus one entry per stage against SURVEY.md 8(d)'s algorithmic work; `parity` = the reference's
 golden clip riding in row 0 of the benchmarked batch; `cpu_baseline` = the oracle timed on host cores.
-`--impl reference` times the reference algorithm on the host CPU (the oracle port - the reference itself is a Python
-tree that cannot travel to the GPU box) on a bounded sample of the same workload.
+`--impl reference` times the reference algorithm on the host CPU (the oracle port of the reference's Python code) on a
+bounded sample of the same workload.
+`--dump-outputs DIR` writes what the last timed step returned to its caller as DIR/<name>.npy (float32; at most 64 MB in
+all - a larger output is written as a fixed, seeded sample of its elements plus DIR/<name>_index.npy).  The inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -43,11 +46,12 @@ def load_peaks():
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tflops": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "tflops_burst": d["bf16_tflops"], "source": "measured"}
-    return {"hbm_gbs": 6650.0, "tflops": 1400.0, "tflops_burst": 1590.0, "source": "fallback"}
+    # H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense fp16 - not reached figures, the denominators
+    return {"hbm_gbs": 3350.0, "tflops": 989.0, "tflops_burst": 989.0, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region (read-only queries)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -77,6 +81,26 @@ class ClockSampler(threading.Thread):
         mx = [float(r[1]) for r in self.rows if len(r) > 1 and r[1].replace(".", "").isdigit()]
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": mx[0] if mx else None,
                 "reasons": sorted(reasons), "samples": len(self.rows)}
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Write {name: tensor} as out_dir/<name>.npy in float32; past DUMP_LIMIT_BYTES in all, every array is replaced by the
+    same fraction of its elements, chosen by a fixed seed and stored with their flat indices (<name>_index.npy)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: v.detach().float().cpu().contiguous() for k, v in arrays.items()}
+    total = sum(v.numel() * 4 for v in arrays.values())
+    for name, v in arrays.items():
+        if total > DUMP_LIMIT_BYTES:
+            keep = max(1, int(v.numel() * (DUMP_LIMIT_BYTES / 2) / total))        # index + value both stored
+            g = torch.Generator().manual_seed(12345)
+            idx = torch.randperm(v.numel(), generator=g)[:keep].sort().values
+            np.save(os.path.join(out_dir, f"{name}_index.npy"), idx.numpy().astype(np.int64 if v.numel() >= 2**31 else np.int32))
+            v = v.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), v.numpy())
 
 
 def synth_batch(batch, n, seed):
@@ -229,9 +253,8 @@ def stage_roofline(prof, stage_ms, peaks, clips, n_samples, frames, ssr=False):
 def dominant_kernel(prof, peaks):
     groups = {}
     for r in prof:
-        pair = r["label"].endswith(".pair")        # pair_tc_kernel (fused residual pair) is its own kernel class
-        if r["bn"] or pair:
-            key = ("pair", 64, 1) if pair else (r["bn"], r["bk"], r.get("terms", 0))
+        if r["bn"]:
+            key = (r["bn"], r["bk"], r.get("terms", 0))
             g = groups.setdefault(key, {"ms": 0.0, "flops": 0.0, "exec": 0.0, "bytes": 0.0, "n": 0, "ops": []})
             g["ms"] += r["ms"]; g["flops"] += r["flops"]; g["exec"] += r.get("exec_flops", 0.0); g["bytes"] += r["bytes"]; g["n"] += 1; g["ops"].append(r)
     total_ms = sum(r["ms"] for r in prof)
@@ -244,31 +267,18 @@ def dominant_kernel(prof, peaks):
     (bn, bk, terms), top = max(groups.items(), key=lambda kv: kv[1]["ms"])
     tf, gb, f_t, f_h = rates(top)
     bound = "hbm" if f_h > f_t else "tensor"
-    # dram__bytes of the ncu --set full capture of ONE launch of this group (profiles/traffic.json, regenerated from
-    # this build by tools/run_profile.sh + tools/summarize_profiles.py), beside the engine's figure for the SAME label
-    traffic, traffic_detail = None, None
-    tpath = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tpath):
-        tj = json.load(open(tpath))
-        for r in top["ops"]:
-            if r["label"] in tj:
-                traffic = tj[r["label"]]["dram_bytes"]
-                traffic_detail = {"label": r["label"], "ncu_dram_bytes_per_launch": traffic, "algorithmic_bytes_this_launch": r["bytes"],
-                                  "ratio": traffic / r["bytes"] if r["bytes"] else None, "source": "profiles/traffic.json (ncu --set full, tools/run_profile.sh)"}
-                break
     labels = [r["label"] for r in top["ops"]]
-    kname = (f"pair_tc_kernel (tcgen05 fused residual pair, C = 64, hi-only; layers: {labels[0]} ... {labels[-1]})" if bn == "pair" else
-             f"gemm_tc_kernel<BN={bn},BK={bk},{'3-term' if terms == 3 else 'hi-only'}> (tcgen05 flat-shift conv GEMM; layers: {labels[0]} ... {labels[-1]})")
+    kname = f"gemm_tc_kernel<BN={bn},BK={bk},{'3-term' if terms == 3 else 'hi-only'}> (wgmma flat-shift conv GEMM; layers: {labels[0]} ... {labels[-1]})"
     return {
         "kernel": kname,
         "bound": bound,
         "achieved": gb if bound == "hbm" else tf, "peak": peaks["hbm_gbs"] if bound == "hbm" else peaks["tflops"],
         "unit": "GB/s" if bound == "hbm" else "TFLOP/s", "frac": f_h if bound == "hbm" else f_t,
         "peak_source": peaks["source"] + (" STREAM copy" if bound == "hbm" else " bf16 dense (== fp16 rate), sustained"),
-        "traffic": traffic, "traffic_detail": traffic_detail, "launches": top["n"], "avg_launch_ms": top["ms"] / top["n"], "share_of_step": top["ms"] / total_ms,
+        "launches": top["n"], "avg_launch_ms": top["ms"] / top["n"], "share_of_step": top["ms"] / total_ms,
         "algorithmic_gflop_per_launch": top["flops"] / top["n"] / 1e9, "algorithmic_gb_per_launch": top["bytes"] / top["n"] / 1e9,
         "tensor_frac": f_t, "tensor_frac_executed": top["exec"] / (top["ms"] * 1e-3) / 1e12 / peaks["tflops"], "hbm_frac": f_h,
-        "all_kernels": {("pair_tc<64>" if k[0] == "pair" else f"gemm<{k[0]},{k[1]},{'3t' if k[2] == 3 else '1t'}>"): {"ms": v["ms"], "launches": v["n"], "tflops": rates(v)[0], "min_gbs": rates(v)[1],
+        "all_kernels": {f"gemm<{k[0]},{k[1]},{'3t' if k[2] == 3 else '1t'}>": {"ms": v["ms"], "launches": v["n"], "tflops": rates(v)[0], "min_gbs": rates(v)[1],
                                                                    "tensor_frac": rates(v)[2], "hbm_frac": rates(v)[3]}
                         for k, v in sorted(groups.items(), key=lambda kv: -kv[1]["ms"])},
     }
@@ -355,6 +365,8 @@ def run_b200(args):
     l0 = eng.launch_count()
     ms = timed_loop(step_dev, args.steps, barrier, dev, vdist)
     launches = eng.launch_count() - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"wav": dev_out})        # restore()'s result in the last timed step
     # ---- end to end through the public host API (pinned host in/out, copies inside the timed region)
     for _ in range(min(2, args.warmup)):
         step_host()
@@ -411,7 +423,7 @@ def run_b200(args):
                    "parallelism": f"dp{world} (independent clips, one NCCL weight broadcast at start-up)",
                    "startup": {"weight_broadcast_ms": bcast_ms, "process_group_init_and_first_barrier_ms": (t_init - t0) * 1e3,
                                "payload_mb": sum(x[2] for x in layout) * 4 / 1e6},
-                   "l2": "activation working set per step (tens of GB) far exceeds the 126 MB L2; no explicit flush needed",
+                   "l2": "activation working set per step (GBs) far exceeds the 50 MB L2; no explicit flush needed",
                    "weights": "seeded synthetic (no checkpoint/network)", "workspace_gb": eng.workspace_bytes(B, n) / 1e9 if not ssr else eng.plan_cache_info()["bytes"] / 1e9,
                    "cuda_graphs": not args.no_graphs},
         "e2e": {"value": e2e, "unit": "clips/s", "h2d_bytes_per_step": B * n * 4, "d2h_bytes_per_step": B * n * 4,
@@ -429,7 +441,7 @@ def run_b200(args):
 
 # ---------------------------------------------------------------------------------------------- long form (configs[4])
 def run_longform(args):
-    """BASELINE configs[4]: one 30-minute stream on 1 x B200.  Three schedules over the same engine:
+    """BASELINE configs[4]: one 30-minute stream on 1 x H100.  Three schedules over the same engine:
     (a) handler(): independent 60 s segments one at a time, hard cuts (eval_gsr_voicefixer.py:47-75) - bit-compatible;
     (b) the same segments batched `--batch` at a time (they are independent, so the bits do not change);
     (c) 30 s windows with 2 s context margins (tools/dsp/overlapadd_boxcar.py:416-510), middle windows batched."""
@@ -477,6 +489,8 @@ def run_longform(args):
         if not name.startswith("handler"):
             res[name]["bit_identical_to_hard_cuts"] = bool(torch.equal(out_host, res["handler_hard_cuts_batch1"]["keep"]))
     ref_out = res["handler_hard_cuts_batch1"].pop("keep")
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"wav": ref_out})           # the handler schedule's stream, last timed step
     res[f"segments_batched_{gb}"].pop("keep")
     ws_seg = eng.workspace_bytes(1, seg) / 1e9
     ws_b = eng.workspace_bytes(gb, seg) / 1e9
@@ -507,7 +521,7 @@ def run_longform(args):
     line = {"metric": "rtf_30min_longform_44k1", "value": res["handler_hard_cuts_batch1"]["rtf"], "unit": "x real time", "n_gpus": 1, "steps": args.steps, "warmup": 1,
             "ms_per_step": res["handler_hard_cuts_batch1"]["ms_per_stream"], "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "f16 tensor-core (UNet hi/lo split; vocoder hi-only), f32 accumulate", "data": "synthetic",
-            "config": {"workload": f"{n_seg}-minute long-form restoration as {n_seg} x 60 s segments (T = 6001 -> T' = 6016), 1 x B200 (BASELINE configs[4]); value = handler() schedule "
+            "config": {"workload": f"{n_seg}-minute long-form restoration as {n_seg} x 60 s segments (T = 6001 -> T' = 6016), 1 x H100 (BASELINE configs[4]); value = handler() schedule "
                                    "through the host entry point (H2D + D2H inside)", "minutes": n_seg, "segment_batch": gb,
                        "workspace_gb_batch1": ws_seg, f"workspace_gb_batch{gb}": ws_b, "plan_cache": eng.plan_cache_info()},
             "schedules": res, "best_rtf": best["rtf"], "parity": parity,
@@ -530,6 +544,8 @@ def main():
     ap.add_argument("--no-graphs", action="store_true", help="launch every kernel individually instead of replaying CUDA graphs")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--profile-out", default="", help="write the per-launch profile (JSON) to this file")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write what the last timed step computed as DIR/<name>.npy (float32, at most 64 MB in all)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     if args.impl == "reference":

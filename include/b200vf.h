@@ -1,4 +1,4 @@
-/* b200vf.h - C ABI of libb200vf.so: the B200-native VoiceFixer inference hot path.
+/* b200vf.h - C ABI of libb200vf.so: the H100-native (sm_90a) VoiceFixer inference hot path.
  *
  * The reference (haoheliu/voicefixer_main) has no FFI for this path; its boundary is the Python object
  * protocol that eval_gsr_voicefixer.py:handler() consumes (SURVEY.md 8(b)).  Each entry point below
@@ -203,7 +203,7 @@ VF_API int vf_check_errors(vf_ctx* ctx, void* stream);
  * held by cached per-shape plans, least recently used evicted first; 0 = half of the free device memory),
  * "graphs" (default 1: the fixed-pointer launch chain of a plan is captured on its second use and replayed as one CUDA graph from then on),
  * "host_pipeline" (default 1, see vf_restore_host),
- * "validate_simt" (1: run every GEMM on the SIMT validation kernel instead of tcgen05 - tests only). */
+ * "validate_simt" (1: run every GEMM on the SIMT validation kernel instead of the wgmma kernel - tests only). */
 VF_API int vf_set_option(vf_ctx* ctx, const char* key, int value);
 /* Plans are cached per (path, batch, frames); the cache is bounded (see "plan_cache_mb").  A batch whose plan would not fit
  * the budget is processed in sub-batches through a smaller plan (same results: rows are independent); the *_stages accessors
@@ -220,14 +220,14 @@ VF_API int vf_stage_times(vf_ctx* ctx, float ms[4]);
 /* Per-launch profile: with op timing enabled, the next vf_restore records a CUDA event before every kernel of
  * the UNet and vocoder launch chains.  vf_op_info(i) synchronises and returns the device time of launch i
  * together with its ALGORITHMIC flops / minimum HBM bytes (the reference op's own counts), the flops the tensor
- * cores actually executed for it (3 MMAs per product in 3-term mode, tile / phase padding, identity taps), the tcgen05 tile
+ * cores actually executed for it (3 MMAs per product in 3-term mode, tile / phase padding, identity taps), the tensor-core tile
  * (bn, bk, fp16 split terms; 0 for non-GEMM kernels) and a label such as "enc3.b2.conv1".  For roofline reporting only. */
 VF_API int vf_enable_op_timing(vf_ctx* ctx, int enable);
 VF_API int vf_op_count(vf_ctx* ctx);
 VF_API int vf_op_info(vf_ctx* ctx, int i, float* ms, double* flops, double* bytes, int* bn, int* bk, int* terms,
                       char* label, int label_cap, double* exec_flops /* nullable: tensor-core flops actually issued */);
 
-/* Self-test of one flat-shift GEMM configuration: random fp16 hi/lo planes through the tcgen05 kernel and
+/* Self-test of one flat-shift GEMM configuration: random fp16 hi/lo planes through the wgmma kernel and
  * the SIMT validation kernel; returns max |difference| and max |value|.  Synchronous. */
 VF_API int vf_selftest_gemm(vf_ctx* ctx, int n_img, int rows, int cin, int cout, int ntaps, int dilation, int terms,
                      double* max_abs_diff, double* max_abs_ref);

@@ -1,8 +1,7 @@
 """Import the reference's own modules UNMODIFIED from /root/reference.  TEST INFRASTRUCTURE ONLY.
 
-Works only in the build container (the GPU box has no /root/reference); used by
-oracle/make_golden.py to generate tests/golden/ and by
-tests/test_oracle_vs_reference.py to pin oracle/vf_oracle.py against the real code.
+Works only where the reference tree exists; used by the golden generators oracle/make_golden.py and
+oracle/make_ref_vectors.py, which write tests/golden/.  The tests themselves read only those stored vectors.
 
 Third-party packages the reference imports but this image lacks are replaced by
 stubs in sys.modules *before* the import:

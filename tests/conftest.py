@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     # the CPU oracle (torch convs) gets slower, not faster, beyond ~16 threads on the many-core GPU hosts
     import torch
     torch.set_num_threads(min(16, os.cpu_count() or 1))

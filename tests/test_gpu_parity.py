@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box).  Everything goes through the C ABI
+"""GPU parity tests (run with -m gpu on an H100).  Everything goes through the C ABI
 (libb200vf.so via ctypes); the oracle and the golden files are only the checker."""
 import numpy as np
 import pytest
@@ -21,7 +21,7 @@ def model(state):
     m._engine().check_errors()
 
 
-# ------------------------------------------------------------------ tcgen05 GEMM vs SIMT validation kernel
+# ------------------------------------------------------------------ tensor-core (wgmma) GEMM vs SIMT validation kernel
 GEMM_CASES = [
     # n_img, rows, cin, cout, ntaps, dilation        (BN, BK) exercised
     (2, 300, 32, 32, 9, 1),      # (32, 32)  SW64
@@ -32,7 +32,7 @@ GEMM_CASES = [
     (2, 500, 128, 128, 3, 27),   # (128, 64), dilated taps, OOB rows
     (3, 40, 384, 384, 9, 2),     # tiny image, 3 N tiles, long K
     (1, 1000, 64, 192, 2, 1),    # N = 192 -> BN 64
-    (2, 700, 128, 512, 3, 3),    # terms = 1 -> BN 256
+    (2, 700, 128, 512, 3, 3),    # terms = 1 -> BN 128, terms = 3 -> BN 64
 ]
 
 
@@ -95,7 +95,7 @@ def test_unet_simt_validation_path_agrees(model, state):
         eng.set_option("validate_simt", 0)
     ref = torch.from_numpy(g["log_mel"])[:1]
     e_tc, e_simt, e_x = float((tc.cpu() - ref).abs().max()), float((simt.cpu() - ref).abs().max()), float((tc - simt).abs().max())
-    print("T=101: tcgen05 vs golden", e_tc, " simt vs golden", e_simt, " tcgen05 vs simt", e_x)
+    print("T=101: wgmma vs golden", e_tc, " simt vs golden", e_simt, " wgmma vs simt", e_x)
     assert e_simt < MEL_TOL and e_tc < MEL_TOL and e_x < MEL_TOL
 
 
@@ -335,8 +335,11 @@ def test_vocoder_fused_pair_vs_two_launch_path(state, monkeypatch):
     m = VoiceFixer().load_state_dict(state).eval().to("cuda:0")
     out = m.vocoder(mel.cuda()).cpu()
     m._engine().check_errors()
+    n_fused = m._engine().launch_count()
     monkeypatch.setenv("VF_TUNE_FUSED_PAIR", "0")
-    plain = VoiceFixer().load_state_dict(state).eval().to("cuda:0").vocoder(mel.cuda()).cpu()
+    mp = VoiceFixer().load_state_dict(state).eval().to("cuda:0")
+    plain = mp.vocoder(mel.cuda()).cpu()
+    assert n_fused < mp._engine().launch_count()                  # one launch per pair instead of two: the fused kernel ran
     assert out.shape == ref.shape
     print("fused pair rms vs oracle", float((out - ref).pow(2).mean().sqrt()), "vs two-launch path", float((out - plain).pow(2).mean().sqrt()))
     assert float((out - ref).pow(2).mean().sqrt()) < WAV_RMS_TOL * 0.2

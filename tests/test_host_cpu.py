@@ -66,13 +66,11 @@ def test_unsupported_configs_fail_loudly():
 
 
 def test_arch_keys_match_reference_state_dict():
-    from oracle import ref_import
-    if not ref_import.available():
-        pytest.skip("reference tree not present")
+    """Against the reference model's state-dict keys and shapes, in registration order (tests/golden/ref_oracle.npz)."""
+    from conftest import load_golden
     from voicefixer_main_b200.arch import UNET_PREFIX, unet_keys
-    from voicefixer_main_b200.weights import make_state
-    model, _ = ref_import.build_reference_model(make_state(1234))
-    own = {k: tuple(v.shape) for k, v in model.state_dict().items() if k.startswith(UNET_PREFIX)}
+    ref = load_golden("ref_oracle.npz")
+    own = {str(k): tuple(int(v) for v in s.split(",") if v) for k, s in zip(ref["sd_keys"], ref["sd_shapes"])}
     mine = {UNET_PREFIX + k: tuple(s) for k, s in unet_keys()}
     assert own == mine
     assert list(own) == list(mine)          # same registration order

@@ -1,20 +1,20 @@
 """Long-form overlap-add with context margins (voicefixer_main_b200/longform.py) - host logic, CPU only.
 
-The mirror is checked (a) against the reference's own LambdaOverlapAdd (tools/dsp/overlapadd_boxcar.py:338-534),
-imported unmodified where /root/reference exists, with identical toy networks, and (b) through properties that
-need no reference: the batched schedule equals the sequential one, and with a margin at least as long as the
+The mirror is checked (a) against the outputs of the reference's own LambdaOverlapAdd (tools/dsp/overlapadd_boxcar.py:338-534)
+with identical toy networks, stored in tests/golden/ref_ola.npz by oracle/make_ref_vectors.py, and (b) through properties
+that need no reference: the batched schedule equals the sequential one, and with a margin at least as long as the
 network's receptive field the chunking is invisible."""
-import importlib.util
 import os
 import types
 
+import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
 from voicefixer_main_b200.longform import BoxcarOverlapAdd, WindowedOverlapAdd
 
-REF = "/root/reference/tools/dsp/overlapadd_boxcar.py"
+GOLDEN_OLA = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_ola.npz")
 CASES = [(1000, 256, 32), (1024, 256, 32), (200, 256, 32), (256, 256, 64), (513, 256, 255), (2049, 512, 100)]
 
 
@@ -41,29 +41,29 @@ def _signal(n, batch=2):
     return torch.randn(batch, 1, n, generator=g)
 
 
-def _load_reference_class():
-    spec = importlib.util.spec_from_file_location("ref_overlapadd_boxcar", REF)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod.LambdaOverlapAdd
+def ref_key(kind, n, w, m, windowed):
+    return f"{kind}_{n}_{w}_{m}_{int(windowed)}"
 
 
-@pytest.mark.skipif(not os.path.exists(REF), reason="reference tree not present")
+def _reference(kind, n, w, m, windowed):
+    """Output and network calls of the reference's LambdaOverlapAdd on _signal(n) with a ToyNet (oracle/make_ref_vectors.py)."""
+    g = np.load(GOLDEN_OLA)
+    key = ref_key(kind, n, w, m, windowed)
+    return torch.from_numpy(g[key + "_out"]), [tuple(int(v) for v in c) for c in g[key + "_calls"]]
+
+
 @pytest.mark.parametrize("n,w,m", CASES)
 @pytest.mark.parametrize("windowed", [False, True])
 def test_matches_reference_lambda_overlap_add(n, w, m, windowed):
-    Ref = _load_reference_class()
     x = _signal(n)
-    ref_net, our_net = ToyNet(), ToyNet()
-    # the reference constructor only survives with a window name (None.type_as fails at :411); the boxcar path is
-    # then selected the way its own ola_forward does, through use_window
-    ref = Ref(nnet=ref_net, n_src=1, window_size=w, in_margin=m, window="hann", reorder_chunks=False)
-    ref.use_window = windowed
+    our_net = ToyNet()
+    # the reference ran with window="hann" and its boxcar path selected through use_window, as its own ola_forward does
+    a, ref_calls = _reference("boxcar", n, w, m, windowed)
     ours = BoxcarOverlapAdd(our_net, n_src=1, window_size=w, in_margin=m, window="hann" if windowed else None)
-    a, b = ref(x), ours(x)
+    b = ours(x)
     assert a.shape == b.shape == (2, 1, n)
     assert torch.equal(a, b)
-    assert sorted(ref_net.calls) == sorted(our_net.calls)          # same chunks reach the network
+    assert sorted(ref_calls) == sorted(our_net.calls)              # same chunks reach the network
 
 
 @pytest.mark.parametrize("n,w,m", CASES)
@@ -104,27 +104,22 @@ def test_plan_and_argument_checks():
 
 
 # ------------------------------------------------------------------ windowed overlap-add (tools/dsp/overlapadd.py)
-REF_OLA = "/root/reference/tools/dsp/overlapadd.py"
 OLA_CASES = [(1000, 256, None), (1024, 256, 128), (300, 256, 64), (2049, 512, 256), (777, 128, 32)]
 
 
-@pytest.mark.skipif(not os.path.exists(REF_OLA), reason="reference tree not present")
 @pytest.mark.parametrize("n,w,hop", OLA_CASES)
 @pytest.mark.parametrize("windowed", [True, False])
 def test_windowed_ola_matches_reference(n, w, hop, windowed):
-    spec = importlib.util.spec_from_file_location("ref_overlapadd", REF_OLA)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
+    """Against the reference's tools/dsp/overlapadd.py LambdaOverlapAdd (window="hann", use_window = windowed)."""
     x = _signal(n)
-    ref_net, our_net = ToyNet(), ToyNet()
-    ref = mod.LambdaOverlapAdd(nnet=ref_net, n_src=1, window_size=w, hop_size=hop, window="hann", reorder_chunks=False)
-    ref.use_window = windowed
+    our_net = ToyNet()
+    a, ref_calls = _reference("ola", n, w, hop, windowed)
     ours = WindowedOverlapAdd(our_net, n_src=1, window_size=w, hop_size=hop, window="hann" if windowed else None,
                               reorder_chunks=False)
-    a, b = ref(x), ours(x)
+    b = ours(x)
     assert a.shape == b.shape == (2, 1, n)
     assert torch.equal(a, b)
-    assert ref_net.calls == our_net.calls
+    assert ref_calls == our_net.calls
 
 
 @pytest.mark.parametrize("n,w,hop", OLA_CASES)

@@ -1,6 +1,6 @@
 """Design check for the fused residual-pair kernel (voicefixer_main_b200/csrc/pair_tc.cu), CPU only.
 
-The kernel itself has not run on hardware yet; what can be checked here is its tiling arithmetic: tiles of 126
+What can be checked here is its tiling arithmetic: tiles of 126
 output rows with m0 = t0 - 1, conv_a evaluated on 128 rows m0 .. m0+127 from zero-filled out-of-range input rows,
 h forced to zero outside the clip, conv_b evaluated on the 128-row tile with one undefined row on either side (only
 rows 1..126 kept), the row masks of the two epilogues.  The emulation below follows the kernel's index expressions

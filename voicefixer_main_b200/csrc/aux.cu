@@ -1,7 +1,7 @@
 // HBM-bound helper kernels around the GEMMs: first UNet layer (Cin = 1), 2x2 average pooling, log/exp
 // maps, vocoder conditioning, reflection padding, the Cout = 1 tail conv + tanh + peak, peak-normalise + trim.
 // All of them are one-pass, vectorised (16-byte accesses on the channel-innermost planes) and write the
-// fp16 hi/lo planes the next tcgen05 GEMM consumes, so no tensor is re-read for an elementwise step.
+// fp16 hi/lo planes the next tensor-core GEMM consumes, so no tensor is re-read for an elementwise step.
 #include "gemm.cuh"
 #include "kernels.cuh"
 

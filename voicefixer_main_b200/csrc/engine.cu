@@ -27,10 +27,10 @@
 namespace vf {
 cudaError_t launch_gemm_tc(const GemmTcParams& p, int bn, int bk, cudaStream_t stream);
 size_t gemm_tc_smem_bytes(int bn, int bk, int stages, int planes_a, int terms, int a_box_rows, int gmax, int tile_chunks, int resid_tma = 0);
-int gemm_tc_max_ctas(int bn);
-uint32_t gemm_tc_magic(uint32_t d, uint64_t nmax);
+int gemm_tc_max_bn(int terms);
 cudaError_t launch_pair_tc(const PairParams& p, cudaStream_t stream);
-size_t pair_tc_smem_bytes(int C, int stages);
+size_t pair_tc_smem_bytes(int C);
+uint32_t gemm_tc_magic(uint32_t d, uint64_t nmax);
 cudaError_t launch_gemm_simt(const GemmSimtParams& p, cudaStream_t stream);
 }  // namespace vf
 
@@ -163,7 +163,7 @@ struct vf_ctx {
   size_t weight_bytes = 0;
   bool loaded = false;
   EncodeTiledFn encode = nullptr;
-  int sm_count = 148;
+  int sm_count = 132;
   int unet_terms = 3, voc_terms = 1, validate_simt = 0, unify_energy = 0;
   int64_t launches = 0;
   int* d_err = nullptr;      // [0] device error code, [1] negative-input count
@@ -571,7 +571,7 @@ struct Builder {
     if (r != CUDA_SUCCESS) return fail(ctx, VF_ECUDA, "cuTensorMapEncodeTiled(A: C=%d rows=%d img_rows=%d n=%d box=%d) -> %d", C, rows, img_rows, n_img, box_c, (int)r);
     return VF_OK;
   }
-  // generic [C, rows, image] map with SWIZZLE_128B (inner box = 128 bytes): TMA loads / stores of the fused pair kernel
+  // generic [C, rows, image] map with SWIZZLE_128B (inner box = 128 bytes): epilogue TMA loads / stores
   int make_map3_any(CUtensorMap* m, const void* base, CUtensorMapDataType dt, int esize, int C, int rows, size_t img_rows, int n_img,
                     int box_c, int box_rows) {
     cuuint64_t dims[3] = {(cuuint64_t)C, (cuuint64_t)rows, (cuuint64_t)n_img};
@@ -675,9 +675,9 @@ struct Builder {
       if (ksum <= maxk) bk = 32;
     }
     const int N = W.N;
-    // 1-term (hi-only) GEMMs stream half the operand bytes per MMA, so they are L2-bandwidth bound at 128-wide
-    // tiles: use 256-wide N tiles where the accumulator budget allows (one accumulator, double buffered)
-    const int bn = (terms == 1 && N % 256 == 0) ? 256 : (N % 128 == 0) ? 128 : (N % 64 == 0) ? 64 : 32;
+    // widest N tile the register-resident accumulator allows (gemm_tc.cu): 128 hi-only, 64 in 3-term mode
+    const int bn_max = gemm_tc_max_bn(terms);
+    const int bn = (bn_max >= 128 && N % 128 == 0) ? 128 : (N % 64 == 0) ? 64 : 32;
     if (N % 32) { rc = fail(ctx, VF_EINVAL, "GEMM N=%d not a multiple of 32", N); return; }
     if (terms == 1 && (epi.a_scale || epi.head_w || epi.out_raw || epi.resid)) {
       rc = fail(ctx, VF_EINVAL, "1-term GEMM with an affine / head / fp32 stream epilogue (3-term kernels only)");
@@ -697,55 +697,9 @@ struct Builder {
       t.g = 1; t.shift[0] = t.shift[1] = t.shift[2] = 0; t.kstride = padded;
       if (ctx->validate_simt == 0) t.nch = padded;
     }
-    // Halo groups: up to 3 consecutive taps reading row-adjacent windows of the same planes share one A load of
-    // 128 + 2 rows; each tap is then an MMA on a row-shifted view (tools/probe_desc_shift.cu).  Worth it where the
-    // layer is bound by shared-memory / L2 feed traffic (narrow N); wide-N tiles keep the finer-grained ring.
-    int gmax = 1;
-    {
-      // measured (B = 32 x 10 s, same box): BN = 64 layers gain 8-17 %, BN = 32 layers 15-25 % (9x L2->SM re-reads of
-      // the taps become 3x); a grouping whose stage no longer fits twice falls back to single taps
-      bool want = ctx->validate_simt == 0;
-      if (const char* ov = getenv("VF_TUNE_HALO")) {      // 0: never, 1: only BN = 64 and hi-only BN = 128 tiles
-        if (atoi(ov) == 0) want = false;
-        if (atoi(ov) == 1) want = want && (bn == 64 || (terms == 1 && bn == 128));
-      }
-      if (want) {
-        std::vector<GemmTap> grouped;
-        int gm = 1;
-        bool any_both = false;
-        for (auto& t : taps) any_both |= t.both != 0;
-        for (size_t i = 0; i < taps.size();) {
-          GemmTap gt = taps[i];
-          size_t n = 1;
-          int step = 0;
-          while (n < 3 && i + n < taps.size()) {
-            const GemmTap& a = taps[i + n - 1];
-            const GemmTap& b2 = taps[i + n];
-            const int d = b2.a_off - a.a_off;
-            if (b2.src != gt.src || b2.c_off != gt.c_off || b2.nch != gt.nch || b2.both || gt.both || (d != 1 && d != -1)) break;
-            if (n == 1) step = d; else if (d != step) break;
-            ++n;
-          }
-          const int lo = std::min(taps[i].a_off, taps[i + n - 1].a_off);
-          for (size_t j = 0; j < n; ++j) gt.shift[j] = taps[i + j].a_off - lo;
-          gt.a_off = lo;
-          gt.g = (int)n;
-          gm = std::max(gm, gt.g);
-          grouped.push_back(gt);
-          i += n;
-        }
-        // a grouped stage holds up to 3 weight tiles: keep the grouping only if a 2-deep ring still fits
-        int gchunks = 0;
-        for (auto& t : grouped) gchunks += t.nch / bk;
-        if (gm > 1 && gemm_tc_smem_bytes(bn, bk, 2, (terms == 3 || any_both) ? 2 : 1, terms, GEMM_BM + 2, gm, gchunks, resid_tma) <= (size_t)226 * 1024) {
-          taps.swap(grouped);
-          gmax = gm;
-        }
-      }
-    }
-    // halo boxes: 128 + 2 rows; 3-term GEMMs fetch the hi and lo planes in one 4-D box, whose planes land back to
-    // back in shared memory, so the box is grown to a whole number of 1024-byte swizzle atoms (136 / 144 rows)
-    const int a_box_rows = gmax > 1 ? (terms == 3 ? (bk == 64 ? 136 : 144) : GEMM_BM + 2) : GEMM_BM;
+    // every tap has its own A load of 128 rows starting on a whole swizzle pattern (gemm_tc.cu): no row-shifted tap groups
+    const int gmax = 1;
+    const int a_box_rows = GEMM_BM;
     if (k != W.K && k != W.K - W.k_tail) { rc = fail(ctx, VF_EINVAL, "GEMM K mismatch: taps cover %d, packed weight has %d", k, W.K); return; }
     GemmProblem pr;
     memset(&pr, 0, sizeof pr);
@@ -797,58 +751,33 @@ struct Builder {
       }
       // accumulation segments (see gemm_tc.cu): a bounded chain of truncating MMAs, then promotion to registers
       tp.tile_chunks = 0;
-      for (auto& t : taps) tp.tile_chunks += t.nch / bk;           // ring slots (group chunks) per tile
-      // K steps per truncating accumulation chain.  Longer chains = fewer promotion drains and a longer run-ahead of
-      // the MMA thread while the epilogue warps are in their output phase (two TMEM buffers = two segments), but
-      // more truncation drift.  Measured on the T = 1001 golden (max log-mel error, UNet ms): 16: 3.1e-5, 33.8;
-      // 24: 3.8e-5, 32.0; 32: 4.1e-5, 31.0; 48: 5.5e-5, 30.1 (bar 1e-4).
+      for (auto& t : taps) tp.tile_chunks += t.nch / bk * ((terms == 1 && t.both) ? 2 : 1);   // ring slots per tile (a hi-only
+                                                                    // identity tap is a hi pass and a lo pass, gemm_tc.cu)
+      // K steps per accumulation chain before promotion: longer chains = fewer promotion drains, shorter ones = less
+      // drift of the tensor core's fp32 accumulation (the 3-term UNet carries a 1e-4 log-mel bar).
       int seg_mmas = 24;
       if (const char* ov = getenv("VF_TUNE_SEG_MMAS")) seg_mmas = std::max(4, atoi(ov));
       tp.seg_chunks = std::max(1, seg_mmas / ((bk / 16) * gmax));
       tp.a_box_rows = a_box_rows;
       tp.gmax = gmax;
-      bool any_both = false;
-      for (auto& t : taps) any_both |= t.both != 0;
-      tp.planes_a = (terms == 3 || any_both) ? 2 : 1;
-      auto pow2 = [](int x) { int c = 32; while (c < x) c *= 2; return c; };
+      tp.planes_a = terms == 3 ? 2 : 1;
       // occupancy: small-K tiles are bound by loads/stores -> several persistent CTAs per SM; large-K -> one
-      const int reg_limit = gemm_tc_max_ctas(bn);
-      int ctas = (k <= 1024) ? reg_limit : 1;
-      if (const char* ov = getenv("VF_TUNE_SMALLK_CTAS")) { if (k <= 1024) ctas = std::max(1, std::min(reg_limit, atoi(ov))); }
-      {   // per tile shape: VF_TUNE_CTAS_<bn>_<terms>=n
-        char key[48];
-        snprintf(key, sizeof key, "VF_TUNE_CTAS_%d_%d", bn, terms);
-        if (const char* ov = getenv(key)) { if (k <= 1024) ctas = std::max(1, std::min(reg_limit, atoi(ov))); }
-      }
+      // one persistent CTA of 384 threads per SM (the accumulators take the register file): the deepest operand ring that fits
+      const size_t smem_cap = (size_t)227 * 1024 - 1024;
+      auto fit = [&](int ring) {
+        int st = 8;
+        for (; st >= 2; --st)
+          if (gemm_tc_smem_bytes(bn, bk, st, tp.planes_a, terms, a_box_rows, gmax, tp.tile_chunks, ring) <= smem_cap) break;
+        return st;
+      };
       tp.resid_tma = resid_tma;
-      int stages = 0;
-      for (; ctas >= 1; --ctas) {
-        // accumulator buffers: four where TMEM allows (run-ahead of the MMA thread over the epilogue's output phase)
-        const int acc_w = (terms == 3 ? 2 : 1) * bn;
-        int nb_log = 1;
-        if (pow2(4 * acc_w) * ctas <= 512) nb_log = 2;
-        if (const char* ov = getenv("VF_TUNE_NBUF")) { if (atoi(ov) == 2) nb_log = 1; }
-        tp.nbuf_log = nb_log;
-        tp.tmem_cols = pow2((1 << nb_log) * acc_w);
-        if (tp.tmem_cols * ctas > 512) continue;
-        const size_t per_cta = (size_t)227 * 1024 / ctas - 1024;
-        auto fit = [&](int ring) {
-          int st = 8;
-          for (; st >= 2; --st)
-            if (gemm_tc_smem_bytes(bn, bk, st, tp.planes_a, terms, a_box_rows, gmax, tp.tile_chunks, ring) <= per_cta) break;
-          return st;
-        };
-        stages = fit(tp.resid_tma);
-        if (tp.resid_tma == 1 && resid_want == 2) {      // a second residual tile in flight if the operand ring stays deep enough
-          const int st2 = fit(2);
-          if (st2 >= 2 && (st2 == stages || st2 >= 4)) { tp.resid_tma = 2; stages = st2; }
-        }
-        if (stages >= 2) break;
-        tp.resid_tma = resid_tma;
+      int stages = fit(tp.resid_tma);
+      if (tp.resid_tma == 1 && resid_want == 2) {      // a second residual tile in flight if the operand ring stays deep enough
+        const int st2 = fit(2);
+        if (st2 >= 2 && (st2 == stages || st2 >= 4)) { tp.resid_tma = 2; stages = st2; }
       }
-      if (ctas < 1 || stages < 2) { rc = fail(ctx, VF_EINVAL, "no tcgen05 tile configuration fits (bn=%d bk=%d terms=%d)", bn, bk, terms); return; }
+      if (stages < 2) { rc = fail(ctx, VF_EINVAL, "no wgmma tile configuration fits (bn=%d bk=%d terms=%d)", bn, bk, terms); return; }
       tp.stages = stages;
-      tp.ctas_per_sm = ctas;
       // MAP_PLAIN outputs leave the epilogue's staging tiles by TMA store (gemm_tc.cu); VF_TUNE_TMA_STORE=0 keeps LDS + STG
       {
         const char* tenv = getenv("VF_TUNE_TMA_STORE");
@@ -886,7 +815,7 @@ struct Builder {
         }
       }
       const long total_tiles = (long)n_img * pr.m_tiles * (N / bn);
-      tp.grid = (int)std::min<long>(total_tiles, (long)ctx->sm_count * ctas);
+      tp.grid = (int)std::min<long>(total_tiles, (long)ctx->sm_count);
       tp.magic_n = gemm_tc_magic((uint32_t)(N / bn), (uint64_t)total_tiles);
       tp.magic_m = gemm_tc_magic((uint32_t)pr.m_tiles, (uint64_t)n_img * pr.m_tiles);
       tp.prob = pr;
@@ -1192,20 +1121,18 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
     const int sc = c.voc_scales[s], cout = cin / 2;
     const long L = Lprev * sc;
     const bool last_stage = s == c.voc_num_stages - 1;
-    // C = 64 stacks in the hi-only mode: one kernel per residual pair (pair_tc.cu), the intermediate h stays in shared
-    // memory and the residual stream of the stack is fp32.  Measured 2.33 vs 2.49 ms per pair against the two GEMM launches
-    // (B = 32 x 10 s); VF_TUNE_FUSED_PAIR=0 selects the two-launch path.  Its activated input and output planes must differ
-    // (a tile reads rows up to `dil` away from the ones another CTA is writing), so the pairs ping-pong between xa and xa2.
-    const char* fenv = getenv("VF_TUNE_FUSED_PAIR");
-    const bool fused = !(fenv && atoi(fenv) == 0) && !ctx->validate_simt && terms == 1 && cout == 64;
     // (a, r) residual stream of the hi-only mode (gemm.cuh): x lives in the activated plane the convs read anyway plus one
     // fp16 correction plane (the otherwise unused lo plane of the same allocation), updated in place by every residual layer:
-    // 10 instead of 12 bytes per element through a two-launch pair, 8 instead of 12 through a fused pair.  VF_TUNE_AR_STREAM=0
-    // keeps separate hi/lo planes of x (and the fp32 stream of the fused stacks).
+    // 10 instead of 12 bytes per element through a residual pair.  VF_TUNE_AR_STREAM=0 keeps separate hi/lo planes of x.
     const char* aenv = getenv("VF_TUNE_AR_STREAM");
     const uint32_t ar = (!(aenv && atoi(aenv) == 0) && !ctx->validate_simt && terms == 1) ? ar_inv_word(c.voc_res_slope) : 0u;
-    // residual stream x as hi/lo planes (ping-pong; a fused stack only reads the first, written by the transposed conv)
-    Planes xr[2] = {ar ? Planes() : b.planes(B, (int)L, cout), (fused || ar) ? Planes() : b.planes(B, (int)L, cout)};
+    // C = 64 stacks of the hi-only mode with the (a, r) stream: one kernel per residual pair (pair_tc.cu), the intermediate h
+    // stays in shared memory; VF_TUNE_FUSED_PAIR=0 selects the two-launch path.  A pair's activated input and output planes
+    // must differ (a tile reads rows up to `dil` away from the ones another CTA is writing): the pairs ping-pong between xa and xa2.
+    const char* fenv = getenv("VF_TUNE_FUSED_PAIR");
+    const bool fused = !(fenv && atoi(fenv) == 0) && ar != 0 && cout == 64 && pair_tc_smem_bytes(cout) != 0;
+    // residual stream x as hi/lo planes (ping-pong)
+    Planes xr[2] = {ar ? Planes() : b.planes(B, (int)L, cout), ar ? Planes() : b.planes(B, (int)L, cout)};
     Planes xa = b.planes(B, (int)L, cout), ha = fused ? Planes() : b.planes(B, (int)L, cout);
     Planes tail_in;
     if (last_stage) tail_in = b.planes(B, (int)L + 6, cout);
@@ -1223,18 +1150,10 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
       b.label = "voc.up" + std::to_string(s);
       b.gemm(ops, ctx->voc_up[s], ASrc{prev, (int)Lprev, 0}, nullptr, taps, e, B, terms);
     }
-    int curx = 0;
+    int curx = 0, cura = 0;
     Planes xa2;
-    float* xf[2] = {nullptr, nullptr};       // fp32 residual stream of a fused stack (ping-pong)
-    if (fused) {
-      xa2 = b.planes(B, (int)L, cout);
-      if (!ar) {
-        xf[0] = b.alloc<float>((size_t)B * L * cout);
-        xf[1] = b.alloc<float>((size_t)B * L * cout);
-      }
-    }
+    if (fused) xa2 = b.planes(B, (int)L, cout);
     if (b.rc) return b.rc;
-    int cura = 0;
     for (int i = 0; i < c.voc_depth[s]; ++i) {
       int dil = 1;
       for (int q = 0; q < i % 10; ++q) dil *= 3;
@@ -1249,50 +1168,35 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
         int mrc = b.make_map3(&pp.a_map, src.p.hi, cout, (int)L, src.img_rows, B, 64, true, GEMM_BM);
         if (!mrc) mrc = b.make_map2(&pp.wa_map, ctx->voc_res_a[s][i].hi, ctx->voc_res_a[s][i].K, cout, 64, cout, true);
         if (!mrc) mrc = b.make_map2(&pp.wb_map, ctx->voc_res_b[s][i].hi, ctx->voc_res_b[s][i].K, cout, 64, cout, true);
+        // the residual is rebuilt from the activated plane (an L2 hit: the centre tap just read these rows) and the correction
+        // plane; the new pair leaves as the two planes of `dst`
+        if (!mrc) mrc = b.make_map3_any(&pp.xin_map[0], src.p.hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, cout, (int)L, (size_t)src.img_rows, B, 64, 126);
+        if (!mrc) mrc = b.make_map3_any(&pp.xin_map[1], src.p.lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, cout, (int)L, (size_t)src.img_rows, B, 64, 126);
+        pp.ar_in = ar;
+        if (!mrc && !last) {
+          pp.ar_out = ar;
+          mrc = b.make_map3_any(&pp.xo_map, dst.p.lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, cout, (int)L, (size_t)dst.img_rows, B, 64, 126);
+        }
+        const int orow0 = (last && last_stage) ? 3 : 0;
+        if (!mrc) mrc = b.make_map3_any(&pp.ao_map, dst.p.hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, cout, orow0 + (int)L, (size_t)dst.img_rows, B, 64, 126);
         if (mrc) return mrc;
         pp.bias_a = ctx->voc_res_a[s][i].bias;
         pp.bias_b = ctx->voc_res_b[s][i].bias;
-        const int orow0 = (last && last_stage) ? 3 : 0;
-        if (ar) {            // (a, r) stream: the residual is rebuilt from the activated plane (an L2 hit: the centre tap just read
-          pp.ar_in = ar;     // these rows) and the correction plane; the new pair leaves as the two planes of `dst`
-          mrc = b.make_map3_any(&pp.xin_map[0], src.p.hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, cout, (int)L, (size_t)src.img_rows, B, 64, 126);
-          if (!mrc) mrc = b.make_map3_any(&pp.xin_map[1], src.p.lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, cout, (int)L, (size_t)src.img_rows, B, 64, 126);
-          if (!mrc && !last) {
-            pp.ar_out = ar;
-            mrc = b.make_map3_any(&pp.xo_map, dst.p.lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, cout, (int)L, (size_t)dst.img_rows, B, 64, 126);
-          }
-        } else if (i == 0) {        // the stack's input: hi / lo planes written by the transposed conv above
-          mrc = b.make_map3_any(&pp.xin_map[0], xr[0].p.hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, cout, (int)L, (size_t)L, B, 64, 126);
-          if (!mrc) mrc = b.make_map3_any(&pp.xin_map[1], xr[0].p.lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, cout, (int)L, (size_t)L, B, 64, 126);
-        } else {
-          pp.in_f32 = 1;
-          mrc = b.make_map3_any(&pp.xin_map[0], xf[curx], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, cout, (int)L, (size_t)L, B, 32, 126);
-        }
-        if (!mrc && !last && !ar) {
-          pp.out_f32 = 1;
-          mrc = b.make_map3_any(&pp.xo_map, xf[1 - curx], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, cout, (int)L, (size_t)L, B, 32, 126);
-        }
-        if (!mrc) mrc = b.make_map3_any(&pp.ao_map, dst.p.hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, cout, orow0 + (int)L, (size_t)dst.img_rows, B, 64, 126);
-        if (mrc) return mrc;
         pp.L = (int)L; pp.n_img = B; pp.C = cout; pp.dil = dil;
         pp.out_img_rows = dst.img_rows;
-        pp.out_row0 = (last && last_stage) ? 3 : 0;
+        pp.out_row0 = orow0;
         pp.tiles_per_img = (int)((L + 125) / 126);
         const long total_tiles = (long)B * pp.tiles_per_img;
-        if (pair_tc_smem_bytes(cout, 0) == 0) return fail(ctx, VF_EINVAL, "fused pair: C=%d not built", cout);
-        pp.stages = 2;
-        pp.grid = (int)std::min<long>(total_tiles, (long)ctx->sm_count);      // one persistent CTA per SM (211 KB of shared memory)
+        pp.grid = (int)std::min<long>(total_tiles, (long)ctx->sm_count);      // one persistent CTA per SM (about 225 KB of shared memory)
         pp.magic_t = gemm_tc_magic((uint32_t)pp.tiles_per_img, (uint64_t)total_tiles);
         pp.slope_h = c.voc_res_slope;
         pp.slope_out = last ? c.voc_stage_slope : c.voc_res_slope;
         pp.err = ctx->d_err;
         op.flops = 2.0 * 2.0 * (double)B * L * cout * 3.0 * cout;
         op.exec_flops = 2.0 * 2.0 * (double)B * pp.tiles_per_img * GEMM_BM * cout * 3.0 * cout;
-        op.bytes = ar ? (double)B * L * cout * (2 + 2 + (last ? 0 : 2) + 2)    // act in (operand and residual), r in, r out, act out
-                      : (double)B * L * cout * (2 + 4 + (last ? 0 : 4) + 2);   // act in, x in, x_new out, act out
+        op.bytes = (double)B * L * cout * (2 + 2 + (last ? 0 : 2) + 2);    // act in (operand and residual), r in, r out, act out
         snprintf(op.label, sizeof op.label, "voc.res%d.%d.pair", s, i);
         ops.push_back(op);
-        curx = 1 - curx;
         cura = 1 - cura;
         continue;
       }
@@ -1699,7 +1603,7 @@ VF_API int vf_create(vf_ctx** out, int device, const vf_config* cfg) {
   if (device < 0 || device >= ndev) return fail(nullptr, VF_EINVAL, "device %d out of range (%d devices)", device, ndev);
   cudaDeviceProp prop;
   if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return fail(nullptr, VF_ECUDA, "%s", cudaGetErrorString(e));
-  if (prop.major != 10) return fail(nullptr, VF_ENODEVICE, "device %d is sm_%d%d; libb200vf is built for sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) return fail(nullptr, VF_ENODEVICE, "device %d is sm_%d%d; libb200vf is built for sm_90a only", device, prop.major, prop.minor);
   if ((e = cudaSetDevice(device)) != cudaSuccess) return fail(nullptr, VF_ECUDA, "%s", cudaGetErrorString(e));
   std::unique_ptr<vf_ctx> ctx(new vf_ctx);
   ctx->device = device;

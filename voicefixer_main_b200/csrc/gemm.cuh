@@ -41,9 +41,8 @@ struct GemmTap {   // one tap, or a GROUP of up to 3 taps that read row-adjacent
   int nch;     // channels contracted by each tap (multiple of the kernel's BK)
   int both;    // 1: contract hi AND lo planes of A even in 1-term mode (identity tap carrying the fp32-grade
                //    residual stream through the accumulator)
-  int g;       // taps in the group (1..3).  Halo load: the A window (128 + 2 rows) is fetched once and tap i is
-               // an MMA on the view shifted by shift[i] rows - a descriptor whose start address is advanced by
-               // shift * row_bytes; the hardware swizzles on absolute address bits (tools/probe_desc_shift.cu)
+  int g;       // taps in the group (1..3; the engine builds groups of 1 for the wgmma kernel).  Halo load: the A
+               // window (128 + 2 rows) fetched once, tap i an MMA on the view shifted by shift[i] rows
   int shift[3];
   int kstride; // columns between consecutive taps' weight segments
 };
@@ -116,32 +115,26 @@ struct GemmTcParams {
   int stages;
   int tile_chunks; // BK-wide K chunks per output tile
   int seg_chunks;  // 3-term mode: chunks per accumulation segment (promotion to registers in between)
-  int tmem_cols;   // power of two >= (1 << nbuf_log) accumulator buffers of BN (1-term) or 2 * BN (3-term: [main | correction]) columns
-  int nbuf_log;    // log2 of the number of accumulator buffers rotating in TMEM (1 or 2)
   int planes_a;    // smem slots per stage for A: 2 when any tap contracts the lo plane
   int a_box_rows;  // rows per A TMA box: 128, or 130 when taps are grouped (halo)
-  int gmax;        // largest tap group: B slots per stage
+  int gmax;        // largest tap group: B slots per stage (1: the wgmma kernel loads every tap on its own)
   int grid;        // persistent CTAs
   uint32_t magic_n, magic_m;   // gemm_tc_magic() of N / BN and m_tiles: division-free tile decoding
-  int ctas_per_sm; // co-resident CTAs the launch is sized for (selects the register budget of the kernel variant)
   GemmProblem prob;
 };
 
-// Fused residual pair of the C = 64 vocoder stacks (pair_tc.cu): x_new = x + conv_b(lrelu(conv_a(xa) + bias_a)) + bias_b
+// Fused residual pair of the C = 64 vocoder stacks (pair_tc.cu): x_new = x + conv_b(lrelu(conv_a(xa) + bias_a)) + bias_b, with the
+// residual stream x kept as the (a, r) pair of GemmEpilogue
 struct PairParams {
   CUtensorMap a_map;             // activated input plane lrelu(x), hi: [C, L, clips], box 64 x 128 x 1, SWIZZLE_128B
   CUtensorMap wa_map, wb_map;    // packed K-major hi weights [K >= 3C, C], box 64 x C
-  CUtensorMap xin_map[2];        // residual x.  in_f32: [0] = the stack's fp32 stream [C, L, clips] (box 32 x 126 x 1, used for
-                                 // both channel halves); else [0] / [1] = its hi / lo fp16 planes (box 64 x 126 x 1), written
-                                 // by the up-sampling GEMM in front of the stack
-  CUtensorMap xo_map;            // x_new, fp32 stream (box 32 x 126 x 1); unused when out_f32 == 0 (last pair of a stage)
+  CUtensorMap xin_map[2];        // the activated and the correction plane of the source (box 64 x 126 x 1)
+  CUtensorMap xo_map;            // the correction plane of the destination (box 64 x 126 x 1); unused when ar_out == 0
   CUtensorMap ao_map;            // lrelu(x_new, slope_out), hi plane [C, out_row0 + L, clips] (box 64 x 126 x 1)
   const float* bias_a;
   const float* bias_b;
-  int in_f32, out_f32;
-  uint32_t ar_in, ar_out;        // (a, r) stream (see GemmEpilogue): xin_map = the activated and the correction plane of the source,
-                                 // xo_map = the correction plane of the destination (fp16, box 64 x 126 x 1); ar_out = 0 on the last pair
-  int L, n_img, C, dil, out_img_rows, out_row0, tiles_per_img, stages, grid;
+  uint32_t ar_in, ar_out;        // fp16(1 / slope) words of the (a, r) stream; ar_out = 0 on the last pair of a stack
+  int L, n_img, C, dil, out_img_rows, out_row0, tiles_per_img, grid;
   uint32_t magic_t;              // gemm_tc_magic(tiles_per_img, ...)
   float slope_h, slope_out;
   int* err;

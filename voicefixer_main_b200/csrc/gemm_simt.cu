@@ -1,5 +1,5 @@
 // SIMT fp32 implementation of the flat-shift multi-tap GEMM contract (gemm.cuh).
-// VALIDATION KERNEL: it exists so every tcgen05 launch can be cross-checked element by element on the
+// VALIDATION KERNEL: it exists so every tensor-core GEMM launch can be cross-checked element by element on the
 // device (tests/test_gemm_gpu.py, VF_DEBUG_SIMT=1); the product path always runs gemm_tc.cu.
 // One thread per output row, 32 output columns per pass; the weight tile is staged in shared memory as
 // fp32 (hi + lo), the activation row is read straight from the hi/lo planes.

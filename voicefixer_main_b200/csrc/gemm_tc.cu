@@ -1,29 +1,27 @@
-// tcgen05 implementation of the flat-shift multi-tap GEMM (see gemm.cuh).
+// wgmma implementation of the flat-shift multi-tap GEMM (see gemm.cuh), sm_90a.
 //
 // Persistent, warp-specialised: each CTA loops over 128 x BN output tiles (tile = blockIdx.x + i * gridDim.x,
-// N tiles of one M tile adjacent so co-running CTAs share the A rows in L2).
-//   warp 0     : TMA producer - streams A (activation rows, shifted per tap; one 130..144-row "halo" box serves up to
-//                three row-adjacent taps) and B (packed weights) tiles into a `stages`-deep shared-memory ring that
-//                runs ahead across tile boundaries (SWIZZLE_128B rows for BK = 64, SWIZZLE_64B for BK = 32); in
-//                3-term mode the hi and lo planes of an operand arrive in one 4-D / 3-D box
-//   warp 1     : TMEM owner + single-thread tcgen05.mma issuer; 2 or 4 accumulator buffers rotate in TMEM
-//   warps 2..  : epilogue (4 or 8 warps; one TMEM lane = output row per thread, two warps share a lane quarter
-//                and split the column chunks)
-// Both issue loops are run by ONE elected thread each and read the flattened per-chunk table the CTA builds in
-// shared memory at start-up (ChunkDesc); their per-chunk instruction count bounds every small-tile layer, which
-// is what the table, the 32-bit descriptor arithmetic and the specialised issue bodies (issue_mmas) are for.
+// N tiles of one M tile adjacent so co-running CTAs share the A rows in L2).  384 threads:
+//   warp group 0 : TMA producer (one elected thread of warp 0) - streams A (activation rows, shifted per tap) and B (packed
+//                  weights) tiles into a `stages`-deep shared-memory ring that runs ahead across tile boundaries
+//                  (SWIZZLE_128B rows for BK = 64, SWIZZLE_64B for BK = 32); in 3-term mode the hi and lo planes of an
+//                  operand arrive in one 4-D / 3-D box
+//   warp groups 1, 2 : MMA + epilogue.  Warp group g issues the wgmma of tile rows [64 g, 64 g + 64) with its fp32
+//                  accumulator in registers, then runs the epilogue on the same rows.  The producer keeps loading the next
+//                  tile's operands while the epilogue runs.
+// Both loops read the flattened per-chunk table the CTA builds in shared memory at start-up (ChunkDesc).
 //
-// Accumulation precision.  The tensor core adds into its fp32 accumulator with truncation, so one long chain
-// of K/16 MMAs drifts by ~0.5 ulp per instruction (measured 2e-4 on the UNet log-mel with one accumulator per
-// tile).  In 3-term mode the K loop is therefore cut into segments of 24 K steps that rotate through the TMEM
-// accumulator buffers; the epilogue warps add each finished segment into registers in fp32 round-to-nearest
-// ("promotion") while the tensor core already works on the next one.  Each buffer is [main | correction]: the
-// two small correction products (hi*lo, lo*hi) never mix into the main chain.  The same ping-pong is the tile double buffering
-// of the 1-term mode (one segment per tile): tile i+1 accumulates while tile i drains.
+// Accumulation precision.  In 3-term mode the K loop is cut into segments of about 24 K steps; every finished segment
+// is added into a second register fragment in fp32 round-to-nearest ("promotion"), so no chain of tensor-core adds is
+// longer than one segment.  The accumulator is [main | correction]: hi*hi and hi*lo come from ONE MMA of width 2*BN
+// against the stacked [B_hi; B_lo] tile, lo*hi is a second MMA of width BN into the correction half, so the two small
+// correction products never mix into the main chain.
 //
 // Epilogue I/O.  A thread owns a row, but global stores are issued row-major by the whole warp: values are
 // transposed through a swizzled shared-memory staging tile so every LDG/STG instruction touches whole
-// 64/128-byte row segments.  Per-tile constants (bias, BN scale/shift, head weights) live in shared memory.
+// 64/128-byte row segments.  The accumulator fragments reach the row-per-thread layout through the same staging tiles
+// (64 columns of the warp group's 64 rows per round).  Per-tile constants (bias, BN scale/shift, head weights) live in
+// shared memory.
 #include "gemm.cuh"
 #include "ptx.cuh"
 
@@ -44,20 +42,23 @@ struct RowInfo {        // published per epilogue thread for its own row, read b
 __device__ __forceinline__ void epi_bar_sync(int nthreads) {
   asm volatile("bar.sync 1, %0;" ::"r"(nthreads) : "memory");
 }
+__device__ __forceinline__ void wg_bar_sync(int wg) {      // the 128 threads of consumer warp group wg
+  asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory");
+}
 
-// One K chunk (= one ring slot) of a tile, as the two issue threads need it: the tap structure is flattened once per
+// One K chunk (= one ring slot) of a tile, as the producer thread and the MMA warp groups need it: the tap structure is flattened once per
 // CTA into this table, so the per-chunk work of the producer / MMA loops is one 16-byte shared-memory load instead
 // of a walk over the tap list in constant memory.
 struct ChunkDesc {
   int a_c;          // channel coordinate of the A box
   int a_off;        // row offset of the A box relative to the tile's first row
   uint32_t kk;      // K coordinate of the first weight tile | kstride << 16 (stride between the weight tiles of a group)
-  uint32_t flags;   // bit 0 src, bit 1 lo plane of A is needed, bits 2-3 g, bit 4 both, bits 5-6 / 7-8 / 9-10 row shifts
+  uint32_t flags;   // bit 0 src, bit 4 (hi-only kernels) the A tile is the lo plane: the second pass of an identity tap
 };
 
 // Tile coordinates without loop-carried state: tile = (img * m_tiles + mi) * n_tiles + nt, decoded per tile with the
 // host's multiply-high magic numbers (gemm_tc_magic): a handful of instructions instead of two integer divisions,
-// and no registers held across the tile loop (the hi-only epilogue runs at a 96-register budget).
+// and no registers held across the tile loop (the accumulators take most of the register file).
 __device__ __forceinline__ uint32_t fast_div(uint32_t n, uint32_t d, uint32_t magic) {
   if (magic == 0u) return n;                    // d == 1
   if (magic == 0xffffffffu) return n / d;       // range too large for the 32-bit magic (host decides)
@@ -94,7 +95,7 @@ __device__ __forceinline__ void pack_hi_lo(const float (&v)[32], uint32_t (&hi)[
 }
 
 // Eight columns (v[8 i .. 8 i + 7]) -> one 16-byte word of the hi plane (and of the lo plane): packing straight into the
-// staging tiles keeps 8 instead of 32 packed words live - the two- and three-CTA variants have no registers to spare.
+// staging tiles keeps 8 instead of 32 packed words live next to the register-resident accumulators.
 template <bool TWO>
 __device__ __forceinline__ void pack8(const float (&v)[32], const int i, uint4& h, uint4& l) {
   uint32_t hw[4], lw[4];
@@ -108,43 +109,20 @@ __device__ __forceinline__ void pack8(const float (&v)[32], const int i, uint4& 
   if (TWO) l = make_uint4(lw[0], lw[1], lw[2], lw[3]);
 }
 
-// The MMAs of one K chunk: G taps (row shifts packed 2 bits each in `shifts`) x BK/16 K steps; 3-term mode adds
-// lo(A) x hi(B) into the correction half, BOTH (hi-only identity tap) contracts the lo plane into the same accumulator.
-template <int BN, int BK, bool THREE, int G, bool BOTH>
-__device__ __forceinline__ void issue_mmas(uint32_t d_main, uint32_t da_hi0, uint32_t da_lo0, uint32_t db00, uint32_t shifts,
-                                           uint32_t started) {
-  constexpr uint32_t idesc = make_idesc_f16(GEMM_BM, BN);
-  constexpr uint32_t idesc2 = make_idesc_f16(GEMM_BM, THREE ? 2 * BN : BN);   // hi x [hi | lo]
-  constexpr uint32_t dhi = make_smem_desc_hi(BK * 2);
-  constexpr uint32_t ROW_UNITS = BK * 2 / 16;
-  constexpr uint32_t B_SLOT_UNITS = (THREE ? 2 : 1) * BN * BK * 2 / 16;
-  // the tap loop is unrolled where the kernel's register budget has room (narrow tiles): every rolled iteration costs
-  // the single issue thread ~25 instructions of loop and shift bookkeeping per 2-4 MMAs
-  constexpr int UNROLL_G = BN <= 64 ? G : 1;
-#pragma unroll UNROLL_G
-  for (int gi = 0; gi < G; ++gi) {
-    const uint32_t sh = G == 1 ? 0u : ((shifts >> (2 * gi)) & 3u) * ROW_UNITS;
-    const uint32_t db0 = db00 + gi * B_SLOT_UNITS;
-#pragma unroll
-    for (int k = 0; k < BK / 16; ++k) {
-      umma_f16_lo(d_main, da_hi0 + sh + 2 * k, db0 + 2 * k, dhi, idesc2, (gi == 0 && k == 0) ? started : 1u);
-      if (THREE) umma_f16_lo(d_main + BN, da_lo0 + sh + 2 * k, db0 + 2 * k, dhi, idesc, 1u);
-      else if (BOTH) umma_f16_lo(d_main, da_lo0 + sh + 2 * k, db0 + 2 * k, dhi, idesc, 1u);
-    }
-  }
-}
+// 8 consumer warps (two warp groups); epilogue warp ew = 4 g + w owns rows [32 (2 g + (w & 1)), +32) of the tile ("row quarter"
+// q) and, per round of 64 columns, the 32-column chunk 2 round + (w >> 1).
+constexpr int GEMM_THREADS = 384;
+constexpr int EPI_WARPS = 8;
 
-// MINB = co-resident CTAs per SM the register allocation is budgeted for (the engine picks the variant that
-// matches the occupancy shared memory allows: fewer CTAs -> more registers -> no spills in the 3-term epilogue).
-template <int BN, int BK, int EPI_WARPS, bool THREE, int MINB>
-__global__ void __launch_bounds__(64 + 32 * EPI_WARPS, MINB)
+template <int BN, int BK, bool THREE>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
     gemm_tc_kernel(const __grid_constant__ GemmTcParams P) {
   constexpr int B_BYTES = BN * BK * 2;
   constexpr int ROW_BYTES = BK * 2;
   constexpr int EPI_THREADS = 32 * EPI_WARPS;
-  constexpr int CHUNK_STEP = EPI_WARPS / 4;             // column chunks are dealt to the warps of a lane quarter
-  constexpr int NJ = (BN / 32 + CHUNK_STEP - 1) / CHUNK_STEP;   // chunks per epilogue warp
-  constexpr bool PREFETCH = !THREE && MINB == 1;        // residual planes one chunk ahead (needs 32 registers)
+  constexpr int CHUNK_STEP = 2;                         // column chunks are dealt to the two warps of a row quarter
+  constexpr int ACC_N = THREE ? 2 * BN : BN;            // [main | correction] in 3-term mode
+  constexpr uint32_t DHI = make_smem_desc_hi(ROW_BYTES);
 
   extern __shared__ __align__(16) uint8_t smem_raw[];
   // 1024-byte alignment by offset arithmetic (keeps the pointer in the shared address space: LDS/STS, not generic)
@@ -153,7 +131,7 @@ __global__ void __launch_bounds__(64 + 32 * EPI_WARPS, MINB)
   const int planes_a = P.planes_a;                      // 2 when any tap contracts the lo plane of A
   constexpr int B_SLOT = (THREE ? 2 : 1) * B_BYTES;      // [B_hi][B_lo] of one tap, contiguous
   const int a_box_bytes = P.a_box_rows * ROW_BYTES;     // bytes one A TMA box delivers
-  const int a_slot = (a_box_bytes + 1023) & ~1023;      // halo rows spill into one more swizzle atom
+  const int a_slot = (a_box_bytes + 1023) & ~1023;
   const int off_b = planes_a * a_slot;
   const int stage_bytes = off_b + P.gmax * B_SLOT;
   uint8_t* stg_base = smem + (size_t)stages * stage_bytes;          // EPI_WARPS x 4 KB staging
@@ -161,11 +139,8 @@ __global__ void __launch_bounds__(64 + 32 * EPI_WARPS, MINB)
   uint8_t* tail = rstg_base + (size_t)P.resid_tma * EPI_WARPS * 4096;  // P.resid_tma = tiles in flight per warp (0, 1 or 2)
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);
   uint64_t* empty_bar = full_bar + stages;
-  uint64_t* seg_full_bar = empty_bar + stages;           // [nbuf <= 4] accumulator buffer holds a finished segment
-  uint64_t* seg_empty_bar = seg_full_bar + 4;            // [nbuf <= 4] ... has been drained by every epilogue thread
-  uint64_t* resid_bar = seg_empty_bar + 4;               // [8][2] per epilogue warp and ring slot: the residual tile has landed
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(resid_bar + 16);   // keep the float arrays 16-byte aligned
-  float* s_bias = reinterpret_cast<float*>(tmem_holder + 4);   // [BN]  (16-byte aligned: float4 reads)
+  uint64_t* resid_bar = empty_bar + stages;              // [8][2] per epilogue warp and ring slot: the residual tile has landed
+  float* s_bias = reinterpret_cast<float*>(resid_bar + 16);    // [BN]  (16-byte aligned: float4 reads)
   float* s_scale = s_bias + BN;                                // [BN]
   float* s_shift = s_scale + BN;                                // [BN]
   float* s_head = s_shift + BN;                                // [32]
@@ -174,26 +149,17 @@ __global__ void __launch_bounds__(64 + 32 * EPI_WARPS, MINB)
 
   const GemmProblem& pr = P.prob;
   const GemmEpilogue& e = pr.epi;
-  const int warp = threadIdx.x >> 5;
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // warp-uniform for the compiler (wgmma paths)
   const int lane = threadIdx.x & 31;
   const int n_tiles = pr.N / BN;
   const int total_tiles = pr.n_img * pr.m_tiles * n_tiles;
   const int tile_chunks = P.tile_chunks;                 // K chunks per tile
   const int seg_chunks = THREE ? P.seg_chunks : tile_chunks;   // K chunks per accumulation segment
-  const int nbuf_log = P.nbuf_log, nbuf_mask = (1 << nbuf_log) - 1;   // 2 or 4 accumulator buffers rotate in TMEM
-  // TMEM columns: 2 or 4 accumulator buffers rotate (as many as 512 columns / co-resident CTAs allow: the MMA
-  // thread can run that many segments ahead of the epilogue warps).  1-term: M0 [0,BN) M1 [BN,2BN) ...  3-term: [M0|C0] [M1|C1] ..., each
-  // 2*BN wide: hi*hi and hi*lo come from ONE MMA of width 2*BN against the stacked [B_hi; B_lo] tile (A_hi is read
-  // from shared memory once instead of twice), lo*hi is a second MMA of width BN into the C half.
 
   if (warp == 0 && lane == 0) {
     for (int s = 0; s < stages; ++s) {
       mbar_init(full_bar + s, 1);
-      mbar_init(empty_bar + s, 1);
-    }
-    for (int i = 0; i <= nbuf_mask; ++i) {
-      mbar_init(seg_full_bar + i, 1);
-      mbar_init(seg_empty_bar + i, EPI_THREADS);
+      mbar_init(empty_bar + s, EPI_WARPS);               // one arrival per consumer warp
     }
     for (int i = 0; i < 16; ++i) mbar_init(resid_bar + i, 1);
     fence_mbar_init();
@@ -201,37 +167,35 @@ __global__ void __launch_bounds__(64 + 32 * EPI_WARPS, MINB)
     tma_prefetch_desc(&P.b_hi);
     if (!THREE) tma_prefetch_desc(&P.a_lo[0]);
   }
-  if (warp == 1) tmem_alloc_dyn(tmem_holder, P.tmem_cols);
-  for (int ci = threadIdx.x; ci < tile_chunks; ci += blockDim.x) {   // flatten taps x K chunks (see ChunkDesc)
+  // flatten taps x K chunks (see ChunkDesc).  In hi-only kernels a `both` tap (identity weights carrying the hi/lo residual
+  // stream) is two passes over the same weight chunks, the second with the lo plane of A as its A tile: every chunk is then one
+  // and the same MMA body (a data-dependent extra MMA per chunk would make the compiler serialise the wgmma pipeline).
+  for (int ci = threadIdx.x; ci < tile_chunks; ci += blockDim.x) {
     int t = 0, first = 0;
     for (; t < pr.ntaps - 1; ++t) {
-      const int n = pr.taps[t].nch / BK;
+      const int n = pr.taps[t].nch / BK * ((!THREE && pr.taps[t].both) ? 2 : 1);
       if (ci < first + n) break;
       first += n;
     }
     const GemmTap& tap = pr.taps[t];
-    const int c = (ci - first) * BK;
+    const int nk = tap.nch / BK;
+    const bool lo_pass = !THREE && tap.both && ci - first >= nk;
+    const int c = (ci - first - (lo_pass ? nk : 0)) * BK;
     ChunkDesc cd;
     cd.a_c = tap.c_off + c;
     cd.a_off = tap.a_off;
     cd.kk = (uint32_t)(tap.k_off + c) | ((uint32_t)tap.kstride << 16);
-    cd.flags = (uint32_t)(tap.src & 1) | ((THREE || tap.both) ? 2u : 0u) | ((uint32_t)tap.g << 2) | (tap.both ? 16u : 0u) |
-               ((uint32_t)tap.shift[0] << 5) | ((uint32_t)tap.shift[1] << 7) | ((uint32_t)tap.shift[2] << 9);
+    cd.flags = (uint32_t)(tap.src & 1) | (lo_pass ? 16u : 0u);
     s_tab[ci] = cd;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
 
-  // Each issue warp elects ONE thread (elect.sync) that runs the whole loop.  Running it under `if (lane == 0)`
-  // instead makes the compiler wrap every UTMALDG / UTCHMMA / UTCBAR in an ELECT + BRA.U.ANY loop (it cannot prove a
-  // single active thread), which measured ~1300 cycles per K chunk on the issue path (ncu, voc.res3.1.a) - the
-  // bottleneck of small-chunk layers.  Measured alternatives: all 32 lanes polling (small-chunk layers -17 %, but
-  // MMA-bound layers +8 %), lane-0 polling with a shuffle broadcast (+12 % overall).
-  if (warp == 0) {
+  if (warp < 4) {
     // ------------------------------------------------------------------ TMA producer
-    if (elect_one()) {      // ONE elected thread runs the whole loop (see above)
+    // the producer warp group hands its registers to the consumers (128 x 40 + 256 x 232 <= 64 K)
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
+    // ONE elected thread runs the whole loop (elect.sync lets the compiler see a single active thread)
+    if (warp == 0 && elect_one()) {
     int s = 0;              // ring slot and its phase bit advance by increment: no division on the issue path
     uint32_t ph = 0;
     bool ok = true;
@@ -245,104 +209,51 @@ __global__ void __launch_bounds__(64 + 32 * EPI_WARPS, MINB)
         const ChunkDesc cur = cd;
         cd = s_tab[ci + 1 < tile_chunks ? ci + 1 : 0];     // next entry: its load latency hides behind the wait
         if (!mbar_wait(empty_bar + s, ph ^ 1, e.err, ERR_PIPE_PRODUCER)) { ok = false; break; }
-        const bool a_lo = (cur.flags & 2u) != 0;
+        const bool lo_pass = (cur.flags & 16u) != 0;
         const int src = cur.flags & 1u;
-        const int tg = (cur.flags >> 2) & 3u;
         uint8_t* st = smem + (size_t)s * stage_bytes;
-        mbar_expect_tx(full_bar + s, (a_lo ? 2u : 1u) * a_box_bytes + tg * B_SLOT);
-        const int k0 = cur.kk & 0xffffu, ks = cur.kk >> 16;
+        mbar_expect_tx(full_bar + s, (THREE ? 2u : 1u) * a_box_bytes + B_SLOT);
+        const int k0 = cur.kk & 0xffffu;
         if (THREE) {      // hi and lo planes of A in one 4-D box, [B_hi][B_lo] of a tap in one 3-D box (a_slot == box bytes)
           tma_load_4d(st, &P.a_hi[src], full_bar + s, cur.a_c, m0 + cur.a_off, img, 0);
-          for (int gi = 0; gi < tg; ++gi) tma_load_3d(st + off_b + gi * B_SLOT, &P.b_hi, full_bar + s, k0 + gi * ks, n0, 0);
+          tma_load_3d(st + off_b, &P.b_hi, full_bar + s, k0, n0, 0);
         } else {
-          tma_load_3d(st, &P.a_hi[src], full_bar + s, cur.a_c, m0 + cur.a_off, img);
-          if (a_lo) tma_load_3d(st + a_slot, &P.a_lo[src], full_bar + s, cur.a_c, m0 + cur.a_off, img);
-          for (int gi = 0; gi < tg; ++gi) tma_load_2d(st + off_b + gi * B_SLOT, &P.b_hi, full_bar + s, k0 + gi * ks, n0);
+          tma_load_3d(st, lo_pass ? &P.a_lo[src] : &P.a_hi[src], full_bar + s, cur.a_c, m0 + cur.a_off, img);
+          tma_load_2d(st + off_b, &P.b_hi, full_bar + s, k0, n0);
         }
-        if (++s == stages) { s = 0; ph ^= 1; }
-      }
-    }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (elect_one()) {
-    constexpr int ACC_W = THREE ? 2 * BN : BN;
-    int s = 0, g = 0;               // smem ring slot, accumulation-segment counter
-    uint32_t ph = 0;                // phase bit of the ring slot
-    bool ok = true;
-    for (int tile = blockIdx.x; tile < total_tiles && ok; tile += gridDim.x) {
-      uint32_t d_main = 0, started = 0;
-      int left_in_seg = 0, buf = 0;                      // countdown: no division on the issue path
-      if (!THREE) {                                      // hi-only: one segment per tile, opened here, closed after the loop
-        buf = g & nbuf_mask;
-        if (!mbar_wait(seg_empty_bar + buf, ((g >> nbuf_log) & 1) ^ 1, e.err, ERR_PIPE_MMA)) { ok = false; break; }
-        d_main = tmem_base + buf * ACC_W;
-      }
-      uint32_t fl = s_tab[0].flags;
-      for (int ci = 0; ci < tile_chunks; ++ci) {
-        const uint32_t cur = fl;
-        fl = s_tab[ci + 1 < tile_chunks ? ci + 1 : 0].flags;
-        if (THREE && left_in_seg == 0) {       // open a segment: its accumulator buffer must have been drained
-          left_in_seg = min(seg_chunks, tile_chunks - ci);
-          buf = g & nbuf_mask;
-          if (!mbar_wait(seg_empty_bar + buf, ((g >> nbuf_log) & 1) ^ 1, e.err, ERR_PIPE_MMA)) { ok = false; break; }
-          d_main = tmem_base + buf * ACC_W;
-          started = 0;
-        }
-        if (!mbar_wait(full_bar + s, ph, e.err, ERR_PIPE_MMA)) { ok = false; break; }
-        tc_fence_after();
-        const bool close_seg = THREE ? (--left_in_seg == 0) : (ci + 1 == tile_chunks);
-        // descriptors differ only in the 14-bit start-address field of their low word (units of 16 B): +2 per
-        // 32-byte K step, +ROW_BYTES/16 per row of halo shift, +B_SLOT/16 per weight tile of a tap group
-        const uint32_t da_hi0 = make_smem_desc_lo(smem_u32(smem + (size_t)s * stage_bytes));
-        const uint32_t da_lo0 = da_hi0 + (uint32_t)(a_slot >> 4);
-        const uint32_t db00 = da_hi0 + (uint32_t)(off_b >> 4);                 // spans [B_hi; B_lo]
-        // one straight-line body per chunk kind (the generic loop with its per-MMA predication costs the single
-        // issue thread ~2x the instructions of the common single-tap case)
-        const uint32_t kind = (cur >> 2) & 7u;                                 // g | both << 2
-        if (kind == 1u) {
-          issue_mmas<BN, BK, THREE, 1, false>(d_main, da_hi0, da_lo0, db00, 0u, started);
-        } else if (kind == 3u) {
-          issue_mmas<BN, BK, THREE, 3, false>(d_main, da_hi0, da_lo0, db00, cur >> 5, started);
-        } else if (kind == 2u) {
-          issue_mmas<BN, BK, THREE, 2, false>(d_main, da_hi0, da_lo0, db00, cur >> 5, started);
-        } else {
-          issue_mmas<BN, BK, THREE, 1, true>(d_main, da_hi0, da_lo0, db00, 0u, started);
-        }
-        started = 1;
-        umma_commit(empty_bar + s);              // frees the smem slot once these MMAs have read it
-        if (close_seg) { umma_commit(seg_full_bar + buf); ++g; }
         if (++s == stages) { s = 0; ph ^= 1; }
       }
     }
     }
     __syncwarp();
   } else {
-    // ------------------------------------------------------------------ epilogue
-    const int ew = warp - 2;
-    const int q = warp & 3;             // TMEM lane quarter this warp may access
-    const int half = ew >> 2;           // with 8 epilogue warps: which column chunks this warp takes
+    // ------------------------------------------------------------------ MMA + epilogue (consumer warp groups)
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
+    const int ew = warp - 4;            // consumer warp 0..7
+    const int wg = ew >> 2;             // consumer warp group: tile rows [64 wg, 64 wg + 64)
+    const int wq = ew & 3;              // warp inside its group: fragment rows [16 wq, 16 wq + 16) of the group's 64
+    const int q = 2 * wg + (wq & 1);    // row quarter of the tile this warp's epilogue owns
+    const int half = wq >> 1;           // which column chunk of each 64-column round it takes
     float4* stg_f = reinterpret_cast<float4*>(stg_base) + (size_t)ew * 256;            // 4 KB per warp
     uint4* stg_h = reinterpret_cast<uint4*>(stg_f);                                    // halves alias the same 4 KB
     uint4* stg_l = stg_h + 128;
     RowInfo* rows = s_rows + ew * 32;
-    const int et = threadIdx.x - 64;
-    const uint32_t lane_bits = static_cast<uint32_t>(q * 32) << 16;
+    const int et = threadIdx.x - 128;
+    float* stg_wg = reinterpret_cast<float*>(stg_base) + (size_t)wg * 4 * 1024;       // the 4 staging tiles of this warp group
     // loop-invariant epilogue configuration in registers
     const int map = e.map, Wp = e.Wp, cout = e.cout, rows_in = e.rows_in;
-    // hi-only (1-term) kernels serve the vocoder: no BN affine, no fused head, no fp32 streams - compiled out, the
-    // 96-register budget of the two-CTA variants has no room for their state
+    // hi-only (1-term) kernels serve the vocoder: no BN affine, no fused head, no fp32 streams - compiled out, so their
+    // state takes no registers next to the 128-column accumulator
     const bool has_affine = THREE && e.a_scale != nullptr, has_bias = e.bias != nullptr;
     const bool want_a = e.out_a.hi != nullptr, want_r = e.out_r.hi != nullptr, want_raw = THREE && e.out_raw != nullptr;
     const bool has_resid = THREE && e.resid != nullptr, has_resid_planes = e.resid_hi != nullptr, has_head = THREE && e.head_w != nullptr;
+    constexpr bool PREFETCH = false;     // residual planes of the next chunk in registers: no room next to the accumulator
     const int act = e.act;
     const float slope = e.slope;
     const uint32_t resid_ar = THREE ? 0u : e.resid_ar, out_ar = THREE ? 0u : e.out_ar;      // (a, r) residual stream, gemm.cuh
     // lane roles for the row-major global accesses
     const int f_row = lane >> 3, f_c16 = lane & 7;       // fp32: 4 rows x 128 B per instruction
     const int h_row = lane >> 2, h_c16 = lane & 3;       // fp16: 8 rows x 64 B per instruction
-    const int nseg = (tile_chunks + seg_chunks - 1) / seg_chunks;
     // staging slots: own row (so_*) and row-major role (sr_*); the swizzle terms are lane constants
     const int so_h0 = lane * 4, so_hx = (lane >> 1) & 3;            // sw64(lane, i)      = so_h0 + (i ^ so_hx)
     const int sr_h0 = h_row * 4, sr_hx = h_c16;                     // sw64(8i+h_row, c)  = 32 i + sr_h0 + (c ^ ((h_row >> 1) & 3)) (8i keeps bits 1-2)
@@ -395,10 +306,12 @@ __global__ void __launch_bounds__(64 + 32 * EPI_WARPS, MINB)
     };
     if (resid_tma && half < BN / 32)
       for (int i = 0; i < resid_ring; ++i) issue_resid();
-    int prev_n0 = -1, g = 0;
+    int prev_n0 = -1, s = 0;            // operand ring slot and its phase bit (the same sequence the producer walks)
+    uint32_t ph = 0;
     float amax = 0.f;
-    bool ok = true;
-    for (int tile = blockIdx.x; tile < total_tiles && ok; tile += gridDim.x) {
+    bool ok = true;     // a timed-out wait is recorded and its later waits skipped; the loop still runs to the end (the
+                        // warp-group barriers need every warp)
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const TileCoord it((uint32_t)tile, P, n_tiles, pr.m_tiles);
       const int img = it.img;
       const int m0 = it.mi * GEMM_BM;
@@ -527,7 +440,7 @@ __global__ void __launch_bounds__(64 + 32 * EPI_WARPS, MINB)
         }
         if (THREE && has_resid && resid_tma) {      // the tile was requested one chunk ago (or at the start of the tile)
           const uint32_t slot = r_cons & (uint32_t)(resid_ring - 1);
-          if (!mbar_wait(rbar + slot, (r_cons >> (resid_ring >> 1)) & 1u, e.err, ERR_PIPE_EPILOGUE)) ok = false;
+          if (ok && !mbar_wait(rbar + slot, (r_cons >> (resid_ring >> 1)) & 1u, e.err, ERR_PIPE_EPILOGUE)) ok = false;
           ++r_cons;
           const float4* rt = reinterpret_cast<const float4*>(rstg + slot * 4096);
 #pragma unroll
@@ -558,7 +471,7 @@ __global__ void __launch_bounds__(64 + 32 * EPI_WARPS, MINB)
         }
         if (has_resid_planes && resid_tma) {
           const uint32_t slot = r_cons & (uint32_t)(resid_ring - 1);
-          if (!mbar_wait(rbar + slot, (r_cons >> (resid_ring >> 1)) & 1u, e.err, ERR_PIPE_EPILOGUE)) ok = false;
+          if (ok && !mbar_wait(rbar + slot, (r_cons >> (resid_ring >> 1)) & 1u, e.err, ERR_PIPE_EPILOGUE)) ok = false;
           ++r_cons;
           const uint4* rth = reinterpret_cast<const uint4*>(rstg + slot * 4096);
           const uint4* rtl = rth + 128;
@@ -717,7 +630,7 @@ __global__ void __launch_bounds__(64 + 32 * EPI_WARPS, MINB)
             }
           }
           __syncwarp();
-          // A TMA store whose box STARTS at a negative coordinate faults (illegal instruction; tools/probe_tma5d.cu - boxes that
+          // A TMA store box may not START at a negative coordinate (boxes that
           // run past the upper bound are clipped as documented): the one warp per image and early phase whose first output row
           // would be q = -1 keeps the LDS + STG path.
           if ((tma_out & 8) && !(wrow0 == 0 && nb / cout < e.ct_pad)) {      // t = stride * r + phase - pad = stride * (r - up) + (phase - pad + up * stride)
@@ -736,71 +649,91 @@ __global__ void __launch_bounds__(64 + 32 * EPI_WARPS, MINB)
         }
       };
 
-      if (THREE) {
-        // Promotion: every finished K segment is added into registers in fp32 round-to-nearest, so no chain of
-        // truncating tensor-core adds is longer than one segment; the small hi*lo + lo*hi sums join at the end.
-        float acc[NJ][32];
-        for (int sg = 0; sg < nseg && ok; ++sg, ++g) {
-          const int buf = g & nbuf_mask;
-          if (!mbar_wait(seg_full_bar + buf, (g >> nbuf_log) & 1, e.err, ERR_PIPE_EPILOGUE)) { ok = false; break; }
-          tc_fence_after();
+      // ---- MMA: this warp group's 64 rows x BN, K chunks from the operand ring
+      float acc[ACC_N / 2];                 // hi x [hi | lo]: [main | correction]
+      float acc2[THREE ? BN / 2 : 1];       // lo x hi, the second correction product
+      float tot[THREE ? BN / 2 : 1];
+      {
+        int left_in_seg = 0, prev_s = -1;
+        uint32_t started = 0;
+        bool first_seg = true;
+        for (int ci = 0; ci < tile_chunks; ++ci) {
+          if (THREE && left_in_seg == 0) {
+            left_in_seg = min(seg_chunks, tile_chunks - ci);
+            started = 0;
+          }
+          if (ok && !mbar_wait(full_bar + s, ph, e.err, ERR_PIPE_EPILOGUE)) ok = false;
+          const uint32_t da_hi = make_smem_desc_lo(smem_u32(smem + (size_t)s * stage_bytes + wg * 64 * ROW_BYTES));
+          const uint32_t da_lo = da_hi + (uint32_t)(a_slot >> 4);
+          const uint32_t db = make_smem_desc_lo(smem_u32(smem + (size_t)s * stage_bytes + off_b));     // spans [B_hi; B_lo]
+          wgmma_fence_regs(acc, ACC_N / 2);
+          if (THREE) wgmma_fence_regs(acc2, BN / 2);
+          wgmma_fence();
 #pragma unroll
-          for (int jj = 0; jj < NJ; ++jj) {
-            const int j = half + jj * CHUNK_STEP;
-            if (j < BN / 32) {
-              if constexpr (MINB >= 2) {      // register-capped variants: 16 columns of both accumulators at a time
-#pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                  float w[16], c[16];
-                  const uint32_t ta = tmem_base + lane_bits + buf * 2 * BN + j * 32 + hh * 16;
-                  tmem_ld2_32x16(ta, ta + BN, w, c);
-                  if (sg == 0) {
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) acc[jj][hh * 16 + i] = w[i] + c[i];
-                  } else {
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) acc[jj][hh * 16 + i] += w[i] + c[i];
-                  }
-                }
-              } else {
-                float w[32], c[32];
-                tmem_ld_32x32(tmem_base + lane_bits + buf * 2 * BN + j * 32, w);
-                tmem_ld_32x32(tmem_base + lane_bits + buf * 2 * BN + BN + j * 32, c);
-                if (sg == 0) {
-#pragma unroll
-                  for (int i = 0; i < 32; ++i) acc[jj][i] = w[i] + c[i];
-                } else {
-#pragma unroll
-                  for (int i = 0; i < 32; ++i) acc[jj][i] += w[i] + c[i];
-                }
-              }
+          for (int k = 0; k < BK / 16; ++k) {
+            Wgmma<ACC_N>::mma(acc, smem_desc(da_hi + 2 * k, DHI), smem_desc(db + 2 * k, DHI), k == 0 ? started : 1u);
+            if (THREE) Wgmma<BN>::mma(acc2, smem_desc(da_lo + 2 * k, DHI), smem_desc(db + 2 * k, DHI), k == 0 ? started : 1u);
+          }
+          wgmma_commit();
+          started = 1;
+          const bool close_seg = THREE ? (--left_in_seg == 0) : (ci + 1 == tile_chunks);
+          // the group of the previous chunk has completed: its slot may be refilled (and this one at a segment's end)
+          if (close_seg) {
+            wgmma_wait<0>();
+            wgmma_fence_regs(acc, ACC_N / 2);
+            if (THREE) wgmma_fence_regs(acc2, BN / 2);
+            __syncwarp();
+            if (lane == 0) {
+              if (prev_s >= 0) mbar_arrive(empty_bar + prev_s);
+              mbar_arrive(empty_bar + s);
             }
-          }
-          tc_fence_before();
-          mbar_arrive(seg_empty_bar + buf);
-        }
-        if (ok) {
+            prev_s = -1;
+            if (THREE) {       // promotion of the finished segment: main + corrections, fp32 round-to-nearest
 #pragma unroll
-          for (int jj = 0; jj < NJ; ++jj) {
-            const int j = half + jj * CHUNK_STEP;
-            if (j < BN / 32) process_chunk(j, acc[jj]);
+              for (int i = 0; i < BN / 2; ++i) tot[i] = (first_seg ? 0.f : tot[i]) + (acc[i] + (acc[BN / 2 + i] + acc2[i]));
+              first_seg = false;
+            }
+          } else {
+            wgmma_wait<1>();
+            wgmma_fence_regs(acc, ACC_N / 2);
+            if (THREE) wgmma_fence_regs(acc2, BN / 2);
+            __syncwarp();
+            if (prev_s >= 0 && lane == 0) mbar_arrive(empty_bar + prev_s);
+            prev_s = s;
           }
+          if (++s == stages) { s = 0; ph ^= 1; }
         }
-      } else {
-        const int buf = g & nbuf_mask;
-        if (!mbar_wait(seg_full_bar + buf, (g >> nbuf_log) & 1, e.err, ERR_PIPE_EPILOGUE)) { ok = false; break; }
-        tc_fence_after();
-#pragma unroll 1
-        for (int j = half; j < BN / 32; j += CHUNK_STEP) {
+        wgmma_wait<0>();                  // already drained at the tile's last chunk; states it for the compiler
+        wgmma_fence_regs(acc, ACC_N / 2);
+      }
+      // ---- accumulator fragments -> row-per-thread chunks, 64 columns per round through the group's staging tiles
+      const float* fin = THREE ? tot : acc;
+#pragma unroll
+      for (int rd = 0; rd < (BN + 63) / 64; ++rd) {
+        stg_release();                    // every tile of the group may be overwritten: no TMA store still reads it
+        wg_bar_sync(wg);
+#pragma unroll
+        for (int i = 0; i < BN / 2; i += 2) {
+          const int col = 8 * (i / 4) + 2 * (lane & 3);
+          if ((8 * (i / 4)) / 64 != rd) continue;
+          const int row = 16 * wq + (lane >> 2) + 8 * ((i / 2) & 1);        // of the group's 64
+          const int cc = (col >> 5) & 1, c32 = col & 31;
+          const int rr = row & 31;
+          float* tile_p = stg_wg + (size_t)(2 * cc + (row >> 5)) * 1024;
+          *reinterpret_cast<float2*>(tile_p + rr * 32 + ((((c32 >> 2) ^ (rr & 7)) << 2) | (c32 & 3))) = make_float2(fin[i], fin[i + 1]);
+        }
+        wg_bar_sync(wg);
+        const int j = 2 * rd + half;
+        if (j < BN / 32) {
           float v[32];
-          tmem_ld_32x32(tmem_base + lane_bits + buf * BN + j * 32, v);
-          if (j + CHUNK_STEP >= BN / 32) {   // last chunk is in registers: hand the accumulator back before the math / stores
-            tc_fence_before();
-            mbar_arrive(seg_empty_bar + buf);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const float4 x = stg_f[SO_F(i)];
+            v[4 * i] = x.x; v[4 * i + 1] = x.y; v[4 * i + 2] = x.z; v[4 * i + 3] = x.w;
           }
+          __syncwarp();
           process_chunk(j, v);
         }
-        ++g;
       }
       if (THREE && half == 0) epilogue_head(e, img, r, head_acc);
     }
@@ -808,47 +741,37 @@ __global__ void __launch_bounds__(64 + 32 * EPI_WARPS, MINB)
     // NaN compares false against everything, inf exceeds the bound
     if (!(amax <= 65504.f) && e.err) atomicCAS(e.err, 0, ERR_FP16_OVERFLOW);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_dyn(tmem_base, P.tmem_cols);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------- host side
-static int epi_warps_for(int bn, int /*terms*/) { return bn == 32 ? 4 : 8; }
-
 size_t gemm_tc_smem_bytes(int bn, int bk, int stages, int planes_a, int terms, int a_box_rows, int gmax, int tile_chunks, int resid_tma) {
   const size_t a_slot = ((size_t)a_box_rows * bk * 2 + 1023) & ~(size_t)1023;
   const size_t stage = planes_a * a_slot + (size_t)gmax * (terms == 3 ? 2 : 1) * bn * bk * 2;
-  const int ew = epi_warps_for(bn, terms);
-  return stages * stage + ew * 4096 * (1 + resid_tma) + (2 * stages + 24) * 8 + 32 + (3 * bn + 32) * 4 + ew * 32 * 8 + (size_t)tile_chunks * 16 + 1024;
+  return stages * stage + EPI_WARPS * 4096 * (1 + resid_tma) + (2 * stages + 16) * 8 + (3 * bn + 32) * 4 + EPI_WARPS * 32 * 8 +
+         (size_t)tile_chunks * 16 + 1024;
 }
 
-template <int BN, int BK, int EW, bool THREE, int MINB>
+template <int BN, int BK, bool THREE>
 static cudaError_t launch_cfg(const GemmTcParams& p, cudaStream_t stream) {
   const size_t smem = gemm_tc_smem_bytes(BN, BK, p.stages, p.planes_a, p.prob.terms, p.a_box_rows, p.gmax, p.tile_chunks, p.resid_tma);
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BN, BK, EW, THREE, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BN, BK, THREE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  gemm_tc_kernel<BN, BK, EW, THREE, MINB><<<p.grid, 64 + 32 * EW, smem, stream>>>(p);
+  gemm_tc_kernel<BN, BK, THREE><<<p.grid, GEMM_THREADS, smem, stream>>>(p);
   return cudaGetLastError();
 }
-template <int BN, int BK, int EW, int MINB>
-static cudaError_t launch_one(const GemmTcParams& p, cudaStream_t stream) {
-  return p.prob.terms == 3 ? launch_cfg<BN, BK, EW, true, MINB>(p, stream) : launch_cfg<BN, BK, EW, false, MINB>(p, stream);
-}
+// tile widths: up to 128 columns hi-only (64 accumulator registers per thread), up to 64 in 3-term mode ([main | correction]
+// = 64 registers plus the 32 of the promoted sum)
 template <int BK>
 static cudaError_t launch_bk(const GemmTcParams& p, int bn, cudaStream_t stream) {
-  const int c = p.ctas_per_sm;
-  if (bn == 256) return p.prob.terms == 1 ? launch_cfg<256, BK, 8, false, 1>(p, stream) : cudaErrorInvalidValue;
-  if (bn == 128) return launch_one<128, BK, 8, 1>(p, stream);
-  if (bn == 64) return c >= 2 ? launch_one<64, BK, 8, 2>(p, stream) : launch_one<64, BK, 8, 1>(p, stream);
-  if (bn == 32) return c >= 3 ? launch_one<32, BK, 4, 3>(p, stream) : launch_one<32, BK, 4, 2>(p, stream);
+  const bool three = p.prob.terms == 3;
+  if (p.gmax != 1) return cudaErrorInvalidValue;
+  if (bn == 128) return three ? cudaErrorInvalidValue : launch_cfg<128, BK, false>(p, stream);
+  if (bn == 64) return three ? launch_cfg<64, BK, true>(p, stream) : launch_cfg<64, BK, false>(p, stream);
+  if (bn == 32) return three ? launch_cfg<32, BK, true>(p, stream) : launch_cfg<32, BK, false>(p, stream);
   return cudaErrorInvalidValue;
 }
 
@@ -859,8 +782,8 @@ uint32_t gemm_tc_magic(uint32_t d, uint64_t nmax) {
   return (uint32_t)(((1ull << 32) + d - 1) / d);
 }
 
-// register-limited CTAs per SM of the variants above (the engine sizes shared memory and the grid against it)
-int gemm_tc_max_ctas(int bn) { return bn == 32 ? 3 : (bn == 64 ? 2 : 1); }
+// widest N tile of the kernel variants above
+int gemm_tc_max_bn(int terms) { return terms == 3 ? 64 : 128; }
 
 cudaError_t launch_gemm_tc(const GemmTcParams& p, int bn, int bk, cudaStream_t stream) {
   if (bk == 64) return launch_bk<64>(p, bn, stream);

@@ -1,4 +1,4 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (UMMA + TMEM).
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma.
 // Every wait is bounded: a broken pipeline sets a sticky error word and returns instead of
 // hanging the GPU (a hung box is a strike on the shared pool).
 #pragma once
@@ -107,86 +107,65 @@ __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_holder) {   // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {        // whole warp, same warp as alloc
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_dyn(uint32_t* smem_holder, uint32_t cols) {   // whole warp; cols = 32..512, power of 2
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)), "r"(cols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_dyn(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem], kind::f16 (fp16 operands, fp32 accumulate), issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Same, with the descriptors given as their low words plus the shared high word (make_smem_desc_hi): all per-MMA
-// descriptor arithmetic (K step, halo row shift, weight tile) touches only the 14-bit start-address field, so the
-// issue loop advances 32-bit values instead of 64-bit ones with carries.
-__device__ __forceinline__ void umma_f16_lo(uint32_t tmem_d, uint32_t a_lo, uint32_t b_lo, uint32_t desc_hi, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %5};\n\t"
-      "mov.b64 db, {%2, %5};\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(a_lo), "r"(b_lo), "r"(idesc), "r"(accumulate), "r"(desc_hi)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued MMAs of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives lane (base+i), columns c..c+31.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Keeps the compiler from moving reads / writes of an accumulator fragment across the asynchronous MMAs that own it.
+__device__ __forceinline__ void wgmma_fence_regs(float* d, int n) {
+#pragma unroll
+  for (int i = 0; i < n; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// 32 lanes x 16 consecutive fp32 columns.
-// Mixed-precision adds (PTX ISA 8.6, sm_100+; SASS FHADD): fp16 + fp32 -> fp32 in ONE instruction, the half selected by a
-// register sub-word modifier - replaces a conversion plus an FADD wherever an epilogue mixes fp16 planes with fp32 values.
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], fp16 operands from shared memory (both K-major), fp32 accumulator in registers,
+// issued by the whole warp group.  Fragment of thread t (warp w = t / 32, lane l): d[i] holds row 16 w + l / 4 + 8 ((i / 2) & 1),
+// column 8 (i / 4) + 2 (l & 3) + (i & 1).  scale_d == 0 starts a new sum.
+template <int N>
+struct Wgmma;
+template <>
+struct Wgmma<32> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(scale_d));
+  }
+};
+template <>
+struct Wgmma<64> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d));
+  }
+};
+template <>
+struct Wgmma<128> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t scale_d) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(scale_d));
+  }
+};
+
+// Mixed fp16 + fp32 arithmetic of the epilogues: the fp16 value is widened exactly, then one fp32 add / subtract.
 __device__ __forceinline__ float add_f32_f16(const unsigned short h, const float c) {      // h + c
-  float d;
-  asm("add.rn.f32.f16 %0, %1, %2;" : "=f"(d) : "h"(h), "f"(c));
-  return d;
+  return __half2float(__ushort_as_half(h)) + c;
 }
 __device__ __forceinline__ float sub_f32_f16(const unsigned short h, const float c) {      // h - c
-  float d;
-  asm("sub.rn.f32.f16 %0, %1, %2;" : "=f"(d) : "h"(h), "f"(c));
-  return d;
+  return __half2float(__ushort_as_half(h)) - c;
 }
 // v0 += lo half of w, v1 += hi half of w (w = a packed half2)
 __device__ __forceinline__ void add_h2(float& v0, float& v1, const uint32_t w) {
@@ -223,61 +202,16 @@ __device__ __forceinline__ void add_planes(float& v0, float& v1, const uint32_t 
   add_h2(v0, v1, lbits);
 }
 
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// two 16-column loads (e.g. the main and the correction accumulator of a 3-term segment), one wait
-__device__ __forceinline__ void tmem_ld2_32x16(uint32_t taddr_a, uint32_t taddr_b, float* a, float* b) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(a);
-  uint32_t* q = reinterpret_cast<uint32_t*>(b);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr_a)
-      : "memory");
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(q[0]), "=r"(q[1]), "=r"(q[2]), "=r"(q[3]), "=r"(q[4]), "=r"(q[5]), "=r"(q[6]), "=r"(q[7]), "=r"(q[8]),
-        "=r"(q[9]), "=r"(q[10]), "=r"(q[11]), "=r"(q[12]), "=r"(q[13]), "=r"(q[14]), "=r"(q[15])
-      : "r"(taddr_b)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// Shared-memory matrix descriptor for a K-major operand tile whose rows are `row_bytes`
-// (64 or 128) wide and swizzled the way TMA SWIZZLE_64B / SWIZZLE_128B writes them
-// (cute::UMMA::SmemDescriptor: start>>4 [0,14), LBO>>4 [16,30), SBO>>4 [32,46), version=1 [46,48),
-// layout_type [61,64): 2 = SWIZZLE_128B, 4 = SWIZZLE_64B).  SBO = 8 rows.
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, int row_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;                                   // LBO (unused for swizzled K-major)
-  d |= static_cast<uint64_t>((8 * row_bytes) >> 4) << 32;                // SBO
-  d |= static_cast<uint64_t>(1) << 46;                                   // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(row_bytes == 128 ? 2 : 4) << 61;            // swizzle mode
-  return d;
-}
+// Shared-memory matrix descriptor of wgmma for a K-major operand tile whose rows are `row_bytes` (64 or 128) wide and
+// swizzled the way TMA SWIZZLE_64B / SWIZZLE_128B writes them: start >> 4 [0,14), LBO >> 4 [16,30) (unused for swizzled
+// K-major), SBO >> 4 [32,46) = 8 rows, layout [62,64): 1 = SWIZZLE_128B, 2 = SWIZZLE_64B.  The tile starts on a whole
+// swizzle pattern (base offset 0); a K step of 16 elements advances the start address by 32 bytes.
 __device__ __forceinline__ uint32_t make_smem_desc_lo(uint32_t smem_addr) {      // start address >> 4 | LBO
   return ((smem_addr & 0x3FFFF) >> 4) | (1u << 16);
 }
-__host__ __device__ constexpr uint32_t make_smem_desc_hi(int row_bytes) {        // SBO | version | swizzle mode
-  return static_cast<uint32_t>((8 * row_bytes) >> 4) | (1u << 14) | (static_cast<uint32_t>(row_bytes == 128 ? 2 : 4) << 29);
+__host__ __device__ constexpr uint32_t make_smem_desc_hi(int row_bytes) {        // SBO | swizzle mode
+  return static_cast<uint32_t>((8 * row_bytes) >> 4) | (static_cast<uint32_t>(row_bytes == 128 ? 1 : 2) << 30);
 }
-// cute::UMMA::InstrDescriptor for kind::f16: C=F32 (1<<4), A=B=F16 (0), both K-major, N>>3 at [17,23), M>>4 at [24,29).
-__host__ __device__ constexpr uint32_t make_idesc_f16(int m, int n) {
-  return (1u << 4) | (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
-}
+__device__ __forceinline__ uint64_t smem_desc(uint32_t lo, uint32_t hi) { return (static_cast<uint64_t>(hi) << 32) | lo; }
 
 }  // namespace vf

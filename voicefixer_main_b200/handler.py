@@ -1,4 +1,4 @@
-"""Mirror of eval_gsr_voicefixer.py (pre :19-25, refresh_model :31-35, handler :37-77) over the B200 engine.
+"""Mirror of eval_gsr_voicefixer.py (pre :19-25, refresh_model :31-35, handler :37-77) over the CUDA engine.
 
 Same signature and contract as the reference handler that evaluation_proc/eval.py:128-132 calls:
     handler(input, output, target, ckpt, device, needrefresh=False, meta={}) -> dict of metrics

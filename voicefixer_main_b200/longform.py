@@ -6,9 +6,9 @@ centre is kept), with the same constructor arguments, the same `ola_forward` / `
 special cases (first chunk has no left margin, last chunk may be short, the signal is zero-padded to a multiple of
 the window).  What differs is the schedule: the reference runs the chunks one by one through `nnet`; here all
 middle chunks of all batch items have the same length and go through `nnet` as ONE batch when the network says it
-is batch-invariant (`nnet.batch_invariant`, true for the B200 engine, whose per-row peak normalisation and
+is batch-invariant (`nnet.batch_invariant`, true for the CUDA engine, whose per-row peak normalisation and
 vocoder are independent across rows), `max_batch` rows at a time: the engine's workspace grows linearly with
-batch x length (~0.14 GB per clip-second), so an unbounded stack of a 20-minute file would not fit a B200, and a
+batch x length (~0.14 GB per clip-second), so an unbounded stack of a 20-minute file would not fit one GPU, and a
 fixed group size also lets the per-shape plans be reused.  A 10-minute file is three launches of batch 8.
 
 `RestoreNet` adapts `VoiceFixer.restore` to the `nnet(x[B, C, L]) -> {key: [B, n_src, L]}` protocol the class expects.

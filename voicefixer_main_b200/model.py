@@ -15,7 +15,7 @@ Same names, arguments and error behaviour as the objects eval_gsr_voicefixer.py:
       .restore_host(pinned_in, pinned_out)
 
 PyTorch is used only to own device memory and streams; every tensor handed back is written by a
-hand-written sm_100a kernel.  Tensors must be fp32 CUDA tensors on the model's device.
+hand-written sm_90a kernel.  Tensors must be fp32 CUDA tensors on the model's device.
 """
 import ctypes
 import json
