@@ -14,6 +14,7 @@
  *   vf_vocoder                    model.vocoder(mel) eval_gsr_voicefixer.py:66 (third-party voicefixer.Vocoder)
  *   vf_restore / vf_restore_host  one iteration of the segment loop of handler(), eval_gsr_voicefixer.py:49-74:
  *                                 pre -> model -> from_log -> vocoder -> peak normalise -> trim_center
+ *   vf_restore_varlen             the same for clips of different lengths in one call (handler() run over a test set)
  *   vf_to_log / vf_from_log       tools/pytorch/pytorch_util.py:157-163
  *   vf_to_pcm16                   the int16 conversion of save_wave, tools/file/wav.py:22-24 (SURVEY.md 8(f) row 3)
  *   vf_mel                        MelScale.forward on any spectrogram, tools/pytorch/mel_scale.py:52-64
@@ -128,6 +129,16 @@ VF_API int vf_restore(vf_ctx* ctx, const float* wav, int batch, int64_t n_sample
                                         meta["unify_energy"] is set, eval_gsr_voicefixer.py:54-55 */
 VF_API int vf_restore_ex(vf_ctx* ctx, const float* wav, int batch, int64_t n_samples, float* wav_out, unsigned flags,
                          void* stream);
+/* Clips of different lengths in one call.  wav: packed device buffer, clip i = wav[offsets[i] .. offsets[i+1]);
+ * offsets: HOST array of batch + 1 increasing int64, offsets[0] = 0 (read during the call only); wav_out: packed the same
+ * way.  flags as vf_restore_ex.  Clip i's output is bit-identical to vf_restore_ex on that clip alone (batch 1, same flags,
+ * same options).  Every clip needs more than 1024 samples and a length trim_center accepts (as vf_restore_ex); a bad
+ * argument fails before any work is queued.  Plans are cached per (batch, bucket), bucket = the longest clip's frames
+ * rounded up to a multiple of 64, so any mix of lengths under one bucket reuses one plan and its CUDA graph; the clips'
+ * lengths reach the device through a kernel parameter on `stream`.  Large calls run as consecutive sub-batches of at most
+ * 256 clips (fewer under the plan budget), each with its own bucket; clips keep their order. */
+VF_API int vf_restore_varlen(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out,
+                             unsigned flags, void* stream);
 /* Same through HOST buffers (pinned for true asynchrony).  The copies and the compute run on library-owned streams with
  * two staging buffer pairs, so back-to-back calls overlap (the H2D of call i+1 and the D2H of call i-1 run under the
  * compute of call i); `stream` only receives a wait on this call's D2H.  Contract: wav_host holds its data when the
@@ -205,7 +216,7 @@ VF_API int vf_check_errors(vf_ctx* ctx, void* stream);
  * "host_pipeline" (default 1, see vf_restore_host),
  * "validate_simt" (1: run every GEMM on the SIMT validation kernel instead of the wgmma kernel - tests only). */
 VF_API int vf_set_option(vf_ctx* ctx, const char* key, int value);
-/* Plans are cached per (path, batch, frames); the cache is bounded (see "plan_cache_mb").  A batch whose plan would not fit
+/* Plans are cached per (path, batch, frames) - vf_restore_varlen: (batch, bucket) - ; the cache is bounded (see "plan_cache_mb").  A batch whose plan would not fit
  * the budget is processed in sub-batches through a smaller plan (same results: rows are independent); the *_stages accessors
  * then only see the last sub-batch. */
 VF_API int vf_plan_cache_info(vf_ctx* ctx, int* n_plans, size_t* bytes, size_t* budget, int64_t* evicted);

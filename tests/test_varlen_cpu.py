@@ -1,0 +1,51 @@
+"""VoiceFixer.restore_batch host logic with a stub engine: the clips are packed into one call in order, the result comes back
+as one view per clip, and bad arguments raise before anything is called."""
+import pytest
+import torch
+
+
+class StubEngine:
+    device = torch.device("cpu")
+    loaded = True
+
+    def __init__(self):
+        self.calls = []
+
+    def restore_varlen(self, packed, lengths, unify_energy=False):
+        self.calls.append((packed.clone(), list(lengths), unify_energy))
+        return packed * 0.5
+
+
+def _model():
+    from voicefixer_main_b200 import VoiceFixer
+    m = VoiceFixer()
+    m._eng = StubEngine()
+    return m
+
+
+def test_restore_batch_packs_in_order_and_splits_into_views():
+    m = _model()
+    clips = [torch.arange(n, dtype=torch.float32) + 10 * i for i, n in enumerate([1025, 3000, 2048])]
+    out = m.restore_batch(clips, unify_energy=True)
+    (packed, lengths, unify), = m._eng.calls
+    assert lengths == [1025, 3000, 2048] and unify is True
+    assert torch.equal(packed, torch.cat(clips))
+    assert [o.shape for o in out] == [c.shape for c in clips]
+    for o, c in zip(out, clips):
+        assert torch.equal(o, c * 0.5)
+    assert all(o.untyped_storage().data_ptr() == out[0].untyped_storage().data_ptr() for o in out)   # views of one output
+
+
+@pytest.mark.parametrize("bad, exc", [
+    ([], ValueError),                                                        # empty list
+    ("not a list", ValueError),
+    ([torch.zeros(2, 2000)], ValueError),                                    # not 1-D
+    ([torch.zeros(2000), torch.zeros(1024)], ValueError),                    # too short for the reflect padding
+    ([torch.zeros(2000, dtype=torch.float64)], TypeError),                   # dtype
+    ([torch.zeros(2000, device="meta")], TypeError),                         # device
+])
+def test_restore_batch_rejects_bad_arguments_before_calling(bad, exc):
+    m = _model()
+    with pytest.raises(exc):
+        m.restore_batch(bad)
+    assert m._eng.calls == []

@@ -19,8 +19,10 @@ __global__ void __launch_bounds__(128) unet_first_kernel(UnetFirstParams p) {
   const int f = (int)(pix - row * Wp);
   const int t = (int)(row % p.Tp);
   const int b = (int)(row / p.Tp);
+  const int T = p.vl_T ? __ldg(p.vl_T + b) : p.T;        // this clip's frames and UNet extent (varlen plans)
+  const int Tp = p.vl_Tp ? __ldg(p.vl_Tp + b) : p.Tp;
   float out_a[32], out_r[32];
-  if (f == p.W) {
+  if (f == p.W || t >= Tp) {
 #pragma unroll
     for (int c = 0; c < 32; ++c) { out_a[c] = 0.f; out_r[c] = 0.f; }
   } else {
@@ -32,8 +34,8 @@ __global__ void __launch_bounds__(128) unet_first_kernel(UnetFirstParams p) {
       for (int dw = 0; dw < 3; ++dw) {
         const int tt = t + dh - 1, ff = f + dw - 1;
         float v = 0.f;
-        if (tt >= 0 && tt < p.Tp && ff >= 0 && ff < p.W) {
-          const float x = tt < p.T ? __ldg(p.logmel + ((size_t)b * p.T + tt) * p.in_ld + ff) : 0.f;
+        if (tt >= 0 && tt < Tp && ff >= 0 && ff < p.W) {
+          const float x = tt < T ? __ldg(p.logmel + ((size_t)b * p.T + tt) * p.in_ld + ff) : 0.f;
           if (dh == 1 && dw == 1) xc = x;
           v = lrelu(fmaf(x, p.bn1_scale, p.bn1_shift), p.slope);
         }
@@ -77,7 +79,7 @@ __global__ void __launch_bounds__(256) pool_kernel(PoolParams p) {
   const int h = (opix / Wpo) % Ho;
   const int b = opix / ((size_t)Wpo * Ho);
   float v[8], a[8];
-  if (w == Wpo - 1) {
+  if (w == Wpo - 1 || (p.row_valid && h * Wpo + w >= __ldg(p.row_valid + b))) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) { v[i] = 0.f; a[i] = 0.f; }
   } else {
@@ -145,8 +147,12 @@ __global__ void __launch_bounds__(256) voc_condition_kernel(VocCondParams p) {
   const int g = idx & 15;
   const int tv = (idx >> 4) % p.Tv;
   const int b = (idx >> 4) / p.Tv;
+  const int T = p.vl_T ? __ldg(p.vl_T + b) : p.T;
   float c[8];
-  if (tv >= p.T) {
+  if (p.vl_Tv && tv >= __ldg(p.vl_Tv + b)) {               // past this clip's vocoder frames (varlen): the conv's zero padding
+#pragma unroll
+    for (int i = 0; i < 8; ++i) c[i] = 0.f;
+  } else if (tv >= T) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) c[i] = p.tail_value;
   } else {
@@ -165,11 +171,12 @@ __global__ void __launch_bounds__(256) voc_condition_kernel(VocCondParams p) {
 }
 // One CTA per clip, fixed reduction order: the scale amp_to_original_f applies (and with it every output sample) is
 // reproducible run to run (a multi-CTA atomicAdd version differed in the last bits between identical calls).
-__global__ void __launch_bounds__(256) band_energy_kernel(const float* tgt, const float* logest, int T, float* sums) {
+__global__ void __launch_bounds__(256) band_energy_kernel(const float* tgt, const float* logest, int T, float* sums, const int* vl_T) {
   __shared__ float sh[2][8];
   const int b = blockIdx.x;
+  const int Tb = vl_T ? __ldg(vl_T + b) : T;
   float st = 0.f, se = 0.f;
-  for (int i = threadIdx.x; i < T * 20; i += 256) {
+  for (int i = threadIdx.x; i < Tb * 20; i += 256) {
     const size_t idx = ((size_t)b * T + i / 20) * 128 + 5 + i % 20;
     st += __ldg(tgt + idx);
     se += exp10f(fminf(__ldg(logest + idx), 5.f));
@@ -189,8 +196,8 @@ __global__ void __launch_bounds__(256) band_energy_kernel(const float* tgt, cons
   }
 }
 cudaError_t launch_band_energy(const float* mel_target_lin, const float* logmel_est, int batch, int T, float* sums,
-                               cudaStream_t stream) {
-  band_energy_kernel<<<batch, 256, 0, stream>>>(mel_target_lin, logmel_est, T, sums);
+                               cudaStream_t stream, const int* vl_T) {
+  band_energy_kernel<<<batch, 256, 0, stream>>>(mel_target_lin, logmel_est, T, sums, vl_T);
   return cudaGetLastError();
 }
 
@@ -235,7 +242,7 @@ cudaError_t launch_voc_condition(const VocCondParams& p, cudaStream_t stream) {
 }
 
 // ---------------------------------------------------------------------------------------------
-__global__ void reflect_fill_kernel(PlanePtr pl, int batch, int L, int C, int pad) {
+__global__ void reflect_fill_kernel(PlanePtr pl, int batch, int L, int C, int pad, const int* vl_L) {
   const int cg = C / 8;
   const size_t total = (size_t)batch * 2 * pad * cg;
   const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -243,17 +250,18 @@ __global__ void reflect_fill_kernel(PlanePtr pl, int batch, int L, int C, int pa
   const int g = idx % cg;
   const int j = (idx / cg) % (2 * pad);
   const int b = idx / ((size_t)cg * 2 * pad);
+  const int Lb = vl_L ? __ldg(vl_L + b) : L;
   int dst, src;
   if (j < pad) { dst = j; src = 2 * pad - j; }
-  else { const int i = j - pad; dst = L + pad + i; src = L - 2 - i + pad; }
+  else { const int i = j - pad; dst = Lb + pad + i; src = Lb - 2 - i + pad; }
   const size_t rows = (size_t)L + 2 * pad;
   const size_t d = ((size_t)b * rows + dst) * C + g * 8, s = ((size_t)b * rows + src) * C + g * 8;
   *reinterpret_cast<uint4*>(pl.hi + d) = *reinterpret_cast<const uint4*>(pl.hi + s);
   *reinterpret_cast<uint4*>(pl.lo + d) = *reinterpret_cast<const uint4*>(pl.lo + s);
 }
-cudaError_t launch_reflect_fill(PlanePtr planes, int batch, int L, int C, int pad, cudaStream_t stream) {
+cudaError_t launch_reflect_fill(PlanePtr planes, int batch, int L, int C, int pad, cudaStream_t stream, const int* vl_L) {
   const size_t total = (size_t)batch * 2 * pad * (C / 8);
-  reflect_fill_kernel<<<(unsigned)((total + 127) / 128), 128, 0, stream>>>(planes, batch, L, C, pad);
+  reflect_fill_kernel<<<(unsigned)((total + 127) / 128), 128, 0, stream>>>(planes, batch, L, C, pad, vl_L);
   return cudaGetLastError();
 }
 
@@ -278,6 +286,8 @@ __global__ void __launch_bounds__(TAIL_THREADS) voc_tail_kernel(VocTailParams p)
   __half* x_l = x_h + (size_t)(TAIL_TILE + 6) * pitch;                    // THREE only
   const int b = blockIdx.y;
   const long t0 = (long)blockIdx.x * TAIL_TILE;
+  const long Lb = p.vl_L ? __ldg(p.vl_L + b) : p.L;        // samples of this clip (varlen plans)
+  if (t0 >= Lb) return;                                    // block-uniform: a tile wholly past the clip
   const size_t rows = (size_t)p.L + 6;
   const int nrows = (int)min((long)TAIL_TILE + 6, (long)rows - t0);
   const int cg = C / 8;
@@ -338,7 +348,7 @@ __global__ void __launch_bounds__(TAIL_THREADS) voc_tail_kernel(VocTailParams p)
 #pragma unroll
   for (int o = 0; o < TAIL_RT; ++o) {
     const long t = t0 + r0 + o;
-    if (t < p.L) {
+    if (t < Lb) {
       const float y = p.tanh_out ? tanhf(acc[o] + p.bias) : acc[o] + p.bias;
       p.wav[(size_t)b * p.L + t] = y;
       mag = fmaxf(mag, fabsf(y));
@@ -375,11 +385,18 @@ cudaError_t launch_voc_tail(const VocTailParams& p, cudaStream_t stream) {
 __global__ void finalize_kernel(FinalizeParams p) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   const int b = blockIdx.y;
-  if (i >= p.n) return;
+  long n = p.n, skip = p.skip;
+  size_t o = (size_t)b * p.out_ld + p.out_off;
+  if (p.vl_off) {
+    n = (long)(__ldg(p.vl_off + b + 1) - __ldg(p.vl_off + b));
+    skip = (__ldg(p.vl_L + b) - n) / 2;
+    o = (size_t)__ldg(p.vl_off + b);
+  }
+  if (i >= n) return;
   const float peak = __uint_as_float(p.peak_bits[b]);
-  float v = p.wav[(size_t)b * p.L + p.skip + i];
+  float v = p.wav[(size_t)b * p.L + skip + i];
   if (peak > 1.0f) v = v / peak;
-  p.out[(size_t)b * p.out_ld + p.out_off + i] = v;
+  p.out[o + i] = v;
 }
 cudaError_t launch_finalize(const FinalizeParams& p, cudaStream_t stream) {
   dim3 grid((unsigned)((p.n + 255) / 256), p.batch);
@@ -399,6 +416,32 @@ __global__ void pcm16_kernel(const float* __restrict__ in, int16_t* __restrict__
     out[i] = static_cast<int16_t>(static_cast<uint16_t>(static_cast<uint32_t>(__float2int_rz(v)) & 0xffffu));
   }
 }
+// ---------------------------------------------------------------------------------------------
+// The lengths table of a varlen plan (kernels.cuh), one thread per clip.
+__global__ void varlen_setup_kernel(const __grid_constant__ VarlenSetupParams p) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b > p.batch) return;
+  p.d_off[b] = p.off[b];
+  if (b == p.batch) return;
+  const int n = (int)(p.off[b + 1] - p.off[b]);
+  const int T = 1 + n / p.hop, Tp = (T + 63) / 64 * 64;
+  int* rows = p.d_rows + b;
+  rows[VL_T * p.batch] = T;
+  rows[VL_TP * p.batch] = Tp;
+  for (int l = 0; l < 7; ++l) rows[(VL_UNET + l) * p.batch] = (Tp >> l) * ((p.w0 >> l) + 1);
+  const int Tv = T + T % 2 + p.tail_base;
+  rows[VL_TV * p.batch] = Tv;
+  int L = Tv;
+  for (int s = 0; s < p.n_stages; ++s) {
+    L *= p.scales[s];
+    rows[(VL_VOC + s) * p.batch] = L;
+  }
+}
+cudaError_t launch_varlen_setup(const VarlenSetupParams& p, cudaStream_t stream) {
+  varlen_setup_kernel<<<(p.batch + 128) / 128, 128, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
 cudaError_t launch_pcm16(const float* in, int16_t* out, size_t n, int saturate, cudaStream_t stream) {
   const unsigned blocks = (unsigned)std::min<size_t>((n + 255) / 256, 148 * 16);
   pcm16_kernel<<<blocks, 256, 0, stream>>>(in, out, n, saturate);

@@ -87,7 +87,7 @@ struct Op {
   UnetFirstParams first;
   PoolParams pool;
   VocCondParams cond;
-  struct { PlanePtr pl; int batch, L, C, pad; } refl;
+  struct { PlanePtr pl; int batch, L, C, pad; const int* vl_L; } refl;
   VocTailParams tail;
   FinalizeParams fin;
   struct { void* p; size_t bytes; } ms;
@@ -114,12 +114,18 @@ struct UnetW {
   float head_b = 0;
 };
 
-enum PlanKind { PLAN_GSR = 0, PLAN_SSR = 1 };
+// PLAN_VARLEN: the GSR path for clips of different lengths (vf_restore_varlen), keyed by (batch, bucket): T = the bucket, a
+// multiple of 64 frames (the UNet's time granularity) that holds the call's longest clip
+enum PlanKind { PLAN_GSR = 0, PLAN_SSR = 1, PLAN_VARLEN = 2 };
 
 struct Plan {
   int kind = PLAN_GSR;
   uint64_t last_use = 0;
   int batch = 0, T = 0;
+  // varlen plans: the per-clip lengths table (kernels.cuh), rewritten on the stream by every call; null otherwise
+  int64_t* d_vl_off = nullptr;   // [batch + 1] sample offsets of the clips
+  int* d_vl_rows = nullptr;      // [VL_ROWS][batch]
+  const int* vl(int row) const { return d_vl_rows ? d_vl_rows + (size_t)row * batch : nullptr; }
   long n_samples = 0;
   std::vector<void*> allocs;
   size_t bytes = 0;
@@ -880,6 +886,7 @@ std::vector<GemmTap> taps3x3(int Wp, int cin) {
 
 struct Level {
   int H, W, Wp, C, rows;
+  const int* valid;      // varlen plans: per clip valid rows of this level (the rest are zero), else null
   float* raw[2];
   Planes aX, aT, cat_r, cat_a, P_r, P_a;   // P_* : pooled output of this level (input of the next)
   float* P_raw = nullptr;
@@ -906,6 +913,7 @@ int build_unet(vf_ctx* ctx, Builder& b, Plan* plan, const UnetW& U, const UnetGe
   for (int l = 0; l < 7; ++l) {
     Level& L = lv[l];
     L.H = Tp >> l; L.W = G.W0 >> l; L.Wp = L.W + 1; L.C = l < 6 ? ENC_C[l] : 384; L.rows = L.H * L.Wp;
+    L.valid = plan->vl(VL_UNET + l);
     L.raw[0] = b.alloc<float>((size_t)B * L.rows * L.C);
     L.raw[1] = b.alloc<float>((size_t)B * L.rows * L.C);
     L.aX = b.planes(B, L.rows, L.C);
@@ -928,6 +936,7 @@ int build_unet(vf_ctx* ctx, Builder& b, Plan* plan, const UnetW& U, const UnetGe
   auto conv1 = [&](const ConvBlockW& w, Level& L, const Planes& in) {
     b.label = tag + ".conv1";
     GemmEpilogue e = epi_plain(L.rows, L.Wp, w.cout, L.rows);
+    e.row_valid = L.valid;
     set_out_a(e, L.aT, 0, w.bn2.scale, w.bn2.shift, ACT_LRELU, S);
     b.gemm(ops, w.conv1, ASrc{in, L.rows, 0}, nullptr, taps3x3(L.Wp, w.cin), e, B, terms);
   };
@@ -942,6 +951,7 @@ int build_unet(vf_ctx* ctx, Builder& b, Plan* plan, const UnetW& U, const UnetGe
     }
     e.resid = resid;
     e.resid_ld = w.cout;
+    e.row_valid = L.valid;
     b.label = tag + (sc_src ? ".conv2+sc" : ".conv2");
     b.gemm(ops, w.conv2, ASrc{L.aT, L.rows, 0}, sc_src ? &s1 : nullptr, taps, e, B, terms);
   };
@@ -964,6 +974,7 @@ int build_unet(vf_ctx* ctx, Builder& b, Plan* plan, const UnetW& U, const UnetGe
         f.w1 = U.d_first_w1; f.bn2_scale = w.bn2.scale; f.bn2_shift = w.bn2.shift;
         f.w_sc = U.d_first_wsc; f.b_sc = U.d_first_bsc; f.slope = S;
         f.a2 = L.aT.p; f.sc_raw = L.raw[0]; f.err = ctx->d_err;
+        f.vl_T = plan->vl(VL_T); f.vl_Tp = plan->vl(VL_TP);
         ops.push_back(op);
         resid = L.raw[0];      // precomputed shortcut(x) acts as the residual
         cur = 0;
@@ -1000,6 +1011,7 @@ int build_unet(vf_ctx* ctx, Builder& b, Plan* plan, const UnetW& U, const UnetGe
     p.in = L.raw[cur]; p.batch = B; p.H = L.H; p.Wp = L.Wp; p.C = L.C; p.Wpo = (L.W >> 1) + 1;
     p.out_r = L.P_r.p; p.out_a = L.P_a.p; p.out_raw = L.P_raw;
     p.a_scale = nx.bn1.scale; p.a_shift = nx.bn1.shift; p.slope = S; p.err = ctx->d_err;
+    p.row_valid = lv[l + 1].valid;
     ops.push_back(op);
   }
   // ---------------- bottleneck (conv_block7, identity shortcut) -> decoder_block1.bn1 + ReLU
@@ -1021,6 +1033,7 @@ int build_unet(vf_ctx* ctx, Builder& b, Plan* plan, const UnetW& U, const UnetGe
       memset(&e, 0, sizeof e);
       e.map = MAP_CONVT2D; e.rows_in = Lin.rows; e.Wp = Lin.Wp; e.cout = cout; e.out_img_rows = L.rows;
       e.out_rows_valid = L.rows;
+      e.row_valid = Lin.valid;
       e.ct_out_wp = L.Wp;      // 2 * Lin.Wp (time-only prune, modules.py:209) or 2 * Lin.Wp - 1 (both=True, modules.py:207-208)
       const ConvBlockW& blk = U.dec[k][0];
       e.out_r = OutPlane{L.cat_r.p.hi, L.cat_r.p.lo, 2 * L.C, 0};
@@ -1059,7 +1072,7 @@ int build_unet(vf_ctx* ctx, Builder& b, Plan* plan, const UnetW& U, const UnetGe
       conv1(U.post, L, L.aX);
       GemmEpilogue e = epi_plain(L.rows, L.Wp, 32, L.rows);
       e.head_w = U.d_head_w; e.head_b = U.head_b;
-      e.head_in = G.head_in; e.head_out = G.head_out; e.head_T = T;
+      e.head_in = G.head_in; e.head_out = G.head_out; e.head_T = T; e.head_valid = plan->vl(VL_T);
       conv2(U.post, L, nullptr, L.raw[cur], e);
     }
   }
@@ -1086,6 +1099,7 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
     p.mel = plan->d_logmel_out; p.is_log = 1; p.batch = B; p.T = T; p.Tv = Tv; p.weight = ctx->d_melw;
     p.amp_floor = c.voc_amp_floor; p.ref_db = c.voc_ref_db; p.min_db = c.voc_min_db; p.tail_value = c.voc_tail_value;
     p.out = cond.p;
+    p.vl_T = plan->vl(VL_T); p.vl_Tv = plan->vl(VL_TV);
     plan->cond_op = (int)ops.size();
     ops.push_back(op);
   }
@@ -1100,15 +1114,17 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
     Planes dst = last ? cpad : (i % 2 ? c1 : c0);
     GemmEpilogue e = epi_plain(Tv, 0, CC, dst.img_rows);
     e.out_row0 = last ? 3 : 0;
+    e.row_valid = plan->vl(VL_TV);
     e.bias = ctx->voc_cond[i].bias;
     set_out_a(e, dst, 0, nullptr, nullptr, ACT_ELU, 0.f);
     b.label = "voc.cond" + std::to_string(i);
     b.gemm(ops, ctx->voc_cond[i], ASrc{cur, Tv, 0}, nullptr, taps1d(3, 1, cur.C, true), e, B, terms);
     cur = dst;
   }
-  { Op op; op.kind = OP_REFLECT; op.refl.pl = cpad.p; op.refl.batch = B; op.refl.L = Tv; op.refl.C = CC; op.refl.pad = 3; ops.push_back(op); }
+  { Op op; op.kind = OP_REFLECT; op.refl.pl = cpad.p; op.refl.batch = B; op.refl.L = Tv; op.refl.C = CC; op.refl.pad = 3; op.refl.vl_L = plan->vl(VL_TV); ops.push_back(op); }
   {
     GemmEpilogue e = epi_plain(Tv, 0, c.voc_channels, Tv);
+    e.row_valid = plan->vl(VL_TV);
     e.bias = ctx->voc_stem.bias;
     set_out_a(e, stem, 0, nullptr, nullptr, ACT_LRELU, c.voc_stage_slope);
     b.label = "voc.stem";
@@ -1142,6 +1158,7 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
       memset(&e, 0, sizeof e);
       e.map = MAP_CONVT1D; e.rows_in = (int)Lprev + 1; e.cout = cout; e.out_img_rows = (int)L; e.out_rows_valid = (int)L;
       e.ct_stride = sc; e.ct_pad = sc / 2 + sc % 2;
+      e.row_valid = plan->vl(VL_VOC + s);
       e.bias = ctx->voc_up[s].bias;
       if (ar) e.out_ar = ar;
       else e.out_r = OutPlane{xr[0].p.hi, xr[0].p.lo, cout, 0};
@@ -1191,6 +1208,7 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
         pp.magic_t = gemm_tc_magic((uint32_t)pp.tiles_per_img, (uint64_t)total_tiles);
         pp.slope_h = c.voc_res_slope;
         pp.slope_out = last ? c.voc_stage_slope : c.voc_res_slope;
+        pp.row_valid = plan->vl(VL_VOC + s);
         pp.err = ctx->d_err;
         op.flops = 2.0 * 2.0 * (double)B * L * cout * 3.0 * cout;
         op.exec_flops = 2.0 * 2.0 * (double)B * pp.tiles_per_img * GEMM_BM * cout * 3.0 * cout;
@@ -1202,6 +1220,7 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
       }
       {
         GemmEpilogue e = epi_plain((int)L, 0, cout, (int)L);
+        e.row_valid = plan->vl(VL_VOC + s);
         e.bias = ctx->voc_res_a[s][i].bias;
         set_out_a(e, ha, 0, nullptr, nullptr, ACT_LRELU, c.voc_res_slope);
         b.label = "voc.res" + std::to_string(s) + "." + std::to_string(i) + ".a";
@@ -1211,6 +1230,7 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
         Planes dst = (last && last_stage) ? tail_in : xa;
         GemmEpilogue e = epi_plain((int)L, 0, cout, dst.img_rows);
         e.out_row0 = (last && last_stage) ? 3 : 0;
+        e.row_valid = plan->vl(VL_VOC + s);
         e.bias = ctx->voc_res_b[s][i].bias;
         if (!last) {
           if (ar) e.out_ar = ar;
@@ -1239,7 +1259,7 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
       }
     }
     if (last_stage) {
-      { Op op; op.kind = OP_REFLECT; op.refl.pl = tail_in.p; op.refl.batch = B; op.refl.L = (int)L; op.refl.C = cout; op.refl.pad = 3; ops.push_back(op); }
+      { Op op; op.kind = OP_REFLECT; op.refl.pl = tail_in.p; op.refl.batch = B; op.refl.L = (int)L; op.refl.C = cout; op.refl.pad = 3; op.refl.vl_L = plan->vl(VL_VOC + s); ops.push_back(op); }
       plan->L = L;
       plan->d_voc_wav = b.alloc<float>((size_t)B * L);
       plan->d_peak = b.alloc<unsigned int>(B);
@@ -1249,7 +1269,7 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
       VocTailParams& p = op.tail;
       memset(&p, 0, sizeof p);
       p.in = tail_in.p; p.batch = B; p.L = (int)L; p.C = cout; p.terms = terms; p.w = ctx->d_tail_w; p.bias = ctx->tail_b;
-      p.wav = plan->d_voc_wav; p.peak_bits = plan->d_peak; p.tanh_out = c.voc_tail_tanh;
+      p.wav = plan->d_voc_wav; p.peak_bits = plan->d_peak; p.tanh_out = c.voc_tail_tanh; p.vl_L = plan->vl(VL_VOC + s);
       ops.push_back(op);
     }
     prev = (fused && cura) ? xa2 : xa;
@@ -1322,7 +1342,7 @@ int get_plan(vf_ctx* ctx, int kind, int batch, int frames, Plan** out) {
   auto it = ctx->plans.find(key);
   if (it != ctx->plans.end()) { it->second->last_use = ++ctx->use_clock; *out = it->second.get(); return VF_OK; }
   if (!ctx->loaded) return fail(ctx, VF_ESTATE, "weights not loaded");
-  if (kind == PLAN_GSR && !(ctx->gsr.loaded && ctx->voc_loaded))
+  if (kind != PLAN_SSR && !(ctx->gsr.loaded && ctx->voc_loaded))
     return fail(ctx, VF_ESTATE, "this entry point needs the analysis module (generator.analysis_module.*) and the vocoder (vocoder.*) weights");
   if (kind == PLAN_SSR && !ctx->ssr.loaded)
     return fail(ctx, VF_ESTATE, "this entry point needs the unet_v2 weights (generator.unet.*)");
@@ -1342,7 +1362,11 @@ int get_plan(vf_ctx* ctx, int kind, int batch, int frames, Plan** out) {
   plan->kind = kind; plan->batch = batch; plan->T = frames;
   Builder b{ctx, plan.get()};
   int rc = VF_OK;
-  if (kind == PLAN_GSR) {
+  if (kind == PLAN_VARLEN) {
+    plan->d_vl_off = b.alloc<int64_t>((size_t)batch + 1);
+    plan->d_vl_rows = b.alloc<int>((size_t)VL_ROWS * batch);
+  }
+  if (kind != PLAN_SSR) {
     const size_t mel_n = (size_t)batch * frames * 128;
     plan->d_mel = b.alloc<float>(mel_n);
     plan->d_logmel_in = b.alloc<float>(mel_n);
@@ -1470,7 +1494,7 @@ int run_ops(vf_ctx* ctx, std::vector<Op>& ops, cudaStream_t st) {
       case OP_FIRST: e = launch_unet_first(op.first, st); break;
       case OP_POOL: e = launch_pool(op.pool, st); break;
       case OP_COND: e = launch_voc_condition(op.cond, st); break;
-      case OP_REFLECT: e = launch_reflect_fill(op.refl.pl, op.refl.batch, op.refl.L, op.refl.C, op.refl.pad, st); break;
+      case OP_REFLECT: e = launch_reflect_fill(op.refl.pl, op.refl.batch, op.refl.L, op.refl.C, op.refl.pad, st, op.refl.vl_L); break;
       case OP_TAIL: e = launch_voc_tail(op.tail, st); break;
       case OP_FINALIZE: e = launch_finalize(op.fin, st); break;
       case OP_MEMSET32: e = cudaMemsetAsync(op.ms.p, 0, op.ms.bytes, st); break;
@@ -1526,12 +1550,14 @@ int run_chain(vf_ctx* ctx, Plan* plan, int slot, cudaStream_t st, int64_t n_laun
 
 int frames_of(vf_ctx* ctx, long n) { return 1 + (int)(n / ctx->cfg.hop); }
 
+// vl_plan: a varlen plan whose lengths table holds the clips of `wav` (n is then the longest clip, T the plan's frames)
 int run_frontend(vf_ctx* ctx, const float* wav, int batch, long n, float* mel, float* logmel, float* sp, float* co,
-                 float* si, cudaStream_t st) {
+                 float* si, cudaStream_t st, const Plan* vl_plan = nullptr) {
   if (n <= 1024) return fail(ctx, VF_EINVAL, "reflect padding needs more than n_fft/2 = 1024 samples (got %ld)", n);
   FrontendParams p;
   memset(&p, 0, sizeof p);
   p.wav = wav; p.n = n; p.batch = batch; p.T = frames_of(ctx, n);
+  if (vl_plan) { p.T = vl_plan->T; p.vl_off = vl_plan->d_vl_off; }
   p.window = ctx->d_window; p.tw1024 = ctx->d_tw1024; p.tw2048 = ctx->d_tw2048;
   p.fb_f0 = ctx->d_fb_f0; p.fb_len = ctx->d_fb_len; p.fb_ofs = ctx->d_fb_ofs; p.fb_val = ctx->d_fb_val;
   p.sp_out = sp; p.cos_out = co; p.sin_out = si; p.mel_out = mel; p.logmel_out = logmel;
@@ -1721,10 +1747,14 @@ VF_API int vf_vocoder(vf_ctx* ctx, const float* mel_lin, int batch, int frames, 
   return plan_exit(ctx, plan, st);
 }
 
-static int restore_impl(vf_ctx* ctx, const float* wav, int batch, int64_t n, float* wav_out, unsigned flags, cudaStream_t st) {
-  const int frames = frames_of(ctx, (long)n);
+// One restore chain.  off == nullptr: `batch` clips of n samples (PLAN_GSR).  Otherwise clips of different lengths
+// (vf_restore_varlen): clip i = wav[off[i] .. off[i + 1]) (host offsets, off[0] = 0, validated by the caller), n = the longest
+// clip, one PLAN_VARLEN plan for the bucket of its frames; the output is packed like the input.
+static int restore_impl(vf_ctx* ctx, const float* wav, int batch, int64_t n, float* wav_out, unsigned flags, cudaStream_t st,
+                        const int64_t* off = nullptr) {
+  const int frames = off ? round_up(frames_of(ctx, (long)n), 64) : frames_of(ctx, (long)n);
   Plan* plan;
-  int rc = get_plan(ctx, PLAN_GSR, batch, frames, &plan);
+  int rc = get_plan(ctx, off ? PLAN_VARLEN : PLAN_GSR, batch, frames, &plan);
   if (rc) return rc;
   if (ctx->op_timing) ctx->prof.clear();
   rc = plan_enter(ctx, plan, st);
@@ -1735,7 +1765,18 @@ static int restore_impl(vf_ctx* ctx, const float* wav, int batch, int64_t n, flo
       if (!e) CK(cudaEventCreate(&e));
     CK(cudaEventRecord(ctx->ev[0], st));
   }
-  rc = run_frontend(ctx, wav, batch, (long)n, plan->d_mel, plan->d_logmel_in, nullptr, nullptr, nullptr, st);
+  if (off) {   // this call's lengths -> the plan's table, in stream order ahead of every kernel that reads it
+    VarlenSetupParams vp;
+    memset(&vp, 0, sizeof vp);
+    for (int i = 0; i <= batch; ++i) vp.off[i] = off[i];
+    vp.batch = batch; vp.hop = ctx->cfg.hop; vp.tail_base = ctx->cfg.voc_tail_base; vp.w0 = 127;
+    vp.n_stages = ctx->cfg.voc_num_stages;
+    for (int s = 0; s < vp.n_stages; ++s) vp.scales[s] = ctx->cfg.voc_scales[s];
+    vp.d_off = plan->d_vl_off; vp.d_rows = plan->d_vl_rows;
+    CK(launch_varlen_setup(vp, st));
+    ctx->launches++;
+  }
+  rc = run_frontend(ctx, wav, batch, (long)n, plan->d_mel, plan->d_logmel_in, nullptr, nullptr, nullptr, st, off ? plan : nullptr);
   if (rc) return rc;
   if (tm) CK(cudaEventRecord(ctx->ev[1], st));
   const bool unify = (flags & VF_RESTORE_UNIFY_ENERGY) != 0;
@@ -1750,7 +1791,7 @@ static int restore_impl(vf_ctx* ctx, const float* wav, int batch, int64_t n, flo
     cop.cond.band_sums = nullptr;
     if (unify) {
       CK(cudaMemsetAsync(plan->d_band, 0, 2 * (size_t)batch * sizeof(float), s));
-      CK(launch_band_energy(plan->d_mel, plan->d_logmel_out, batch, frames, plan->d_band, s));
+      CK(launch_band_energy(plan->d_mel, plan->d_logmel_out, batch, frames, plan->d_band, s, plan->vl(VL_T)));
       ctx->launches++;
       cop.cond.band_sums = plan->d_band;
     }
@@ -1763,9 +1804,10 @@ static int restore_impl(vf_ctx* ctx, const float* wav, int batch, int64_t n, flo
   FinalizeParams f;
   memset(&f, 0, sizeof f);
   const long d = plan->L - (long)n;
-  if (d < 0 || d == 1) return fail(ctx, VF_EINVAL, "vocoder output length %ld incompatible with input %ld (trim_center)", plan->L, (long)n);
+  if (!off && (d < 0 || d == 1)) return fail(ctx, VF_EINVAL, "vocoder output length %ld incompatible with input %ld (trim_center)", plan->L, (long)n);
   f.wav = plan->d_voc_wav; f.peak_bits = plan->d_peak; f.batch = batch; f.L = plan->L; f.n = (long)n; f.skip = d / 2;
   f.out = wav_out; f.out_ld = (long)n; f.out_off = 0;
+  if (off) { f.vl_off = plan->d_vl_off; f.vl_L = plan->vl(VL_VOC + ctx->cfg.voc_num_stages - 1); }
   CK(launch_finalize(f, st));
   ctx->launches++;
   if (tm) { CK(cudaEventRecord(ctx->ev[4], st)); ctx->ev_valid = true; }
@@ -1780,6 +1822,43 @@ VF_API int vf_restore_ex(vf_ctx* ctx, const float* wav, int batch, int64_t n, fl
   const int cb = choose_sub_batch(ctx, PLAN_GSR, batch, frames_of(ctx, (long)n));
   for (int off = 0; off < batch; off += cb) {
     rc = restore_impl(ctx, wav + (size_t)off * n, std::min(cb, batch - off), n, wav_out + (size_t)off * n, flags, (cudaStream_t)stream);
+    if (rc) return rc;
+  }
+  return VF_OK;
+}
+
+VF_API int vf_restore_varlen(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out, unsigned flags,
+                             void* stream) {
+  int rc = check_ready(ctx);
+  if (rc) return rc;
+  if (!wav || !wav_out || !offsets || batch <= 0) return fail(ctx, VF_EINVAL, "vf_restore_varlen: bad arguments");
+  if (flags & ~(unsigned)VF_RESTORE_UNIFY_ENERGY) return fail(ctx, VF_EINVAL, "vf_restore_varlen: unknown flag bits 0x%x", flags);
+  if (offsets[0] != 0) return fail(ctx, VF_EINVAL, "vf_restore_varlen: offsets[0] must be 0 (got %ld)", (long)offsets[0]);
+  if (!(ctx->gsr.loaded && ctx->voc_loaded))
+    return fail(ctx, VF_ESTATE, "this entry point needs the analysis module (generator.analysis_module.*) and the vocoder (vocoder.*) weights");
+  // every clip is checked before anything is launched: a rejected call leaves no partial output and no work queued
+  long scale = 1;
+  for (int s = 0; s < ctx->cfg.voc_num_stages; ++s) scale *= ctx->cfg.voc_scales[s];
+  int max_frames = 0;
+  for (int i = 0; i < batch; ++i) {
+    const int64_t n = offsets[i + 1] - offsets[i];
+    if (n <= 0) return fail(ctx, VF_EINVAL, "vf_restore_varlen: offsets must increase (clip %d: %ld -> %ld)", i, (long)offsets[i], (long)offsets[i + 1]);
+    if (n <= 1024) return fail(ctx, VF_EINVAL, "clip %d: reflect padding needs more than n_fft/2 = 1024 samples (got %ld)", i, (long)n);
+    if (n > (int64_t)1 << 30) return fail(ctx, VF_EINVAL, "clip %d: %ld samples is too long for one restore", i, (long)n);
+    const int T = frames_of(ctx, (long)n);
+    const long d = (long)(T + T % 2 + ctx->cfg.voc_tail_base) * scale - (long)n;
+    if (d < 0 || d == 1) return fail(ctx, VF_EINVAL, "clip %d: vocoder output length %ld incompatible with input %ld (trim_center)", i, (long)n + d, (long)n);
+    max_frames = std::max(max_frames, T);
+  }
+  // consecutive clips form sub-batches (plan budget, and the lengths table's per-launch cap); each has its own bucket
+  const int cb = std::min(choose_sub_batch(ctx, PLAN_VARLEN, batch, max_frames), VL_MAX_CLIPS);
+  for (int s = 0; s < batch; s += cb) {
+    const int b = std::min(cb, batch - s);
+    int64_t rel[VL_MAX_CLIPS + 1];
+    int64_t n_max = 0;
+    for (int i = 0; i <= b; ++i) rel[i] = offsets[s + i] - offsets[s];
+    for (int i = 0; i < b; ++i) n_max = std::max(n_max, rel[i + 1] - rel[i]);
+    rc = restore_impl(ctx, wav + offsets[s], b, n_max, wav_out + offsets[s], flags, (cudaStream_t)stream, rel);
     if (rc) return rc;
   }
   return VF_OK;

@@ -21,9 +21,15 @@ __global__ void __launch_bounds__(256) frontend_kernel(FrontendParams p) {
   __shared__ float2 buf1[1024];
   const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
   const float* x = p.wav + (size_t)b * p.n;
+  long n = p.n;
+  if (p.vl_off) {        // clips of different lengths: this clip's samples, reflect padded at its own ends
+    x = p.wav + __ldg(p.vl_off + b);
+    n = (long)(__ldg(p.vl_off + b + 1) - __ldg(p.vl_off + b));
+    if (t >= 1 + n / 441) return;      // block-uniform
+  }
 
   // windowed, reflect-padded frame packed as z[n] = x[2n] + i x[2n+1]; 1024-point FFT (fft.cuh)
-  load_frame_packed(buf0, x, p.n, t, p.window, tid);
+  load_frame_packed(buf0, x, n, t, p.window, tid);
   __syncthreads();
   const float2* src = fft1024_forward(buf0, buf1, p.tw1024, tid);
   // src == buf1 now holds Z[0..1023]; buf0 is free and becomes the magnitude row

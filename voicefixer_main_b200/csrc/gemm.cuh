@@ -91,8 +91,25 @@ struct GemmEpilogue {
   uint32_t out_ar;       // out_a is written as (hi plane = a, lo plane = r); 1-term kernels, ACT_LRELU, no affine
   int tma_out;           // bit 3: MAP_CONVT1D out_a through a 5-D map (see gemm_tc.cu).  MAP_PLAIN layers: bit 0 out_raw, bit 1 out_r, bit 2 out_a leave the staging tiles by TMA store
                          // (GemmTcParams::o_raw / o_r / o_a) instead of LDS + STG: half the LSU wavefronts of the store path
+  // Clips of different lengths in one plan (vf_restore_varlen): per image, the count of valid rows - GEMM rows for MAP_PLAIN /
+  // MAP_CONVT2D, output rows for MAP_CONVT1D.  Rows past it are written as zeros in every output, like the pad column, so the
+  // next conv reads the zero padding it would see past the end of a clip-sized tensor.  nullptr: every row is valid.
+  const int* row_valid;
+  const int* head_valid;   // per image, frames the fused head writes (t < head_valid[img]); nullptr: head_T
   int* err;
 };
+
+// Per image valid-row limit of a varlen plan, or "no limit".
+__device__ __forceinline__ int valid_rows(const int* row_valid, int img) {
+  return row_valid ? __ldg(row_valid + img) : 0x7fffffff;
+}
+// A tile of a varlen plan whose rows are all past its image's valid rows: the GEMM issues no loads and no MMAs for it and only
+// stores its zeros.  The producer and the consumers evaluate the same predicate, so the operand ring stays in step.
+__device__ __forceinline__ bool tile_is_empty(const GemmEpilogue& e, int img, int m0) {
+  if (!e.row_valid) return false;
+  const int v = __ldg(e.row_valid + img);
+  return e.map == MAP_CONVT1D ? (long)m0 * e.ct_stride - e.ct_pad >= v : m0 >= v;
+}
 
 struct GemmProblem {
   int n_img;
@@ -137,6 +154,7 @@ struct PairParams {
   int L, n_img, C, dil, out_img_rows, out_row0, tiles_per_img, grid;
   uint32_t magic_t;              // gemm_tc_magic(tiles_per_img, ...)
   float slope_h, slope_out;
+  const int* row_valid;          // varlen plans: per clip valid rows (<= L); rows past it are written as zeros.  nullptr: L
   int* err;
 };
 
@@ -184,20 +202,23 @@ __device__ __forceinline__ void epilogue_chunk(const GemmEpilogue& e, int img, i
   }
   size_t orow;
   bool pad = false;
+  const int vrows = valid_rows(e.row_valid, img);
   if (e.map == MAP_PLAIN) {
     orow = (size_t)img * e.out_img_rows + e.out_row0 + r;
     if (e.Wp > 0) pad = (r % e.Wp) == e.Wp - 1;
+    pad |= r >= vrows;
   } else if (e.map == MAP_CONVT2D) {
     const int h = r / e.Wp, w = r - h * e.Wp;
     const int ph = phase >> 1, pw = phase & 1;
     const int col = 2 * w + pw;
     if (col >= e.ct_out_wp) return;          // both=True prune: column past the output pitch
     orow = (size_t)img * e.out_img_rows + (size_t)(2 * h + ph) * e.ct_out_wp + col;
-    pad = col == e.ct_out_wp - 1;
+    pad = col == e.ct_out_wp - 1 || r >= vrows;
   } else {
     const long t = (long)r * e.ct_stride + phase - e.ct_pad;
     if (t < 0 || t >= e.out_rows_valid) return;
     orow = (size_t)img * e.out_img_rows + e.out_row0 + t;
+    pad = t >= vrows;
   }
   if (e.bias) {
 #pragma unroll
@@ -258,7 +279,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmEpilogue& e, int img, i
 __device__ __forceinline__ void epilogue_head(const GemmEpilogue& e, int img, int r, float head_acc) {
   if (!e.head_w || r >= e.rows_in) return;
   const int t = r / e.Wp, f = r - t * e.Wp;
-  if (t >= e.head_T) return;
+  if (t >= e.head_T || (e.head_valid && t >= __ldg(e.head_valid + img))) return;
   const size_t idx = ((size_t)img * e.head_T + t) * e.Wp + f;
   const float y = (f < e.Wp - 1) ? head_acc + e.head_b : 0.f;
   e.head_out[idx] = e.head_in ? y + __ldg(e.head_in + idx) : y;

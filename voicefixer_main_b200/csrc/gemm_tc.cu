@@ -204,8 +204,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       const int img = it.img;
       const int m0 = it.mi * GEMM_BM;
       const int n0 = it.nt * BN;
+      const int nchunks = tile_is_empty(e, img, m0) ? 0 : tile_chunks;
       ChunkDesc cd = s_tab[0];
-      for (int ci = 0; ci < tile_chunks; ++ci) {
+      for (int ci = 0; ci < nchunks; ++ci) {
         const ChunkDesc cur = cd;
         cd = s_tab[ci + 1 < tile_chunks ? ci + 1 : 0];     // next entry: its load latency hides behind the wait
         if (!mbar_wait(empty_bar + s, ph ^ 1, e.err, ERR_PIPE_PRODUCER)) { ok = false; break; }
@@ -342,7 +343,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       if (map == MAP_PLAIN) {
         if (row_ok) {
           orow = obase + lane;
-          flags = kRowValid | ((Wp > 0 && (r % Wp) == Wp - 1) ? kRowPad : 0);
+          flags = kRowValid | (((Wp > 0 && (r % Wp) == Wp - 1) || r >= valid_rows(e.row_valid, img)) ? kRowPad : 0);
         }
       } else if (map == MAP_CONVT2D) {
         cth = r / Wp;
@@ -412,18 +413,19 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           co0 = nb - phase * cout;
           orow = 0; flags = 0;
           if (row_ok) {
+            const int vrows = valid_rows(e.row_valid, img);
             if (map == MAP_CONVT2D) {
               const int ph = phase >> 1, pw = phase & 1;
               const int col = 2 * ctw + pw;
               if (col < e.ct_out_wp) {         // both=True pruning drops the column past the output pitch
                 orow = (uint32_t)((size_t)img * e.out_img_rows + (size_t)(2 * cth + ph) * e.ct_out_wp + col);
-                flags = kRowValid | (col == e.ct_out_wp - 1 ? kRowPad : 0);
+                flags = kRowValid | ((col == e.ct_out_wp - 1 || r >= vrows) ? kRowPad : 0);
               }
             } else {
               const long t = (long)r * e.ct_stride + phase - e.ct_pad;
               if (t >= 0 && t < e.out_rows_valid) {
                 orow = (uint32_t)((size_t)img * e.out_img_rows + e.out_row0 + t);
-                flags = kRowValid;
+                flags = kRowValid | (t >= vrows ? kRowPad : 0);
               }
             }
           }
@@ -657,7 +659,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         int left_in_seg = 0, prev_s = -1;
         uint32_t started = 0;
         bool first_seg = true;
-        for (int ci = 0; ci < tile_chunks; ++ci) {
+        const int nchunks = tile_is_empty(e, img, m0) ? 0 : tile_chunks;   // the producer's predicate: the ring stays in step
+        for (int ci = 0; ci < nchunks; ++ci) {
           if (THREE && left_in_seg == 0) {
             left_in_seg = min(seg_chunks, tile_chunks - ci);
             started = 0;

@@ -22,8 +22,30 @@ struct FrontendParams {
   float* sin_out;
   float* mel_out;        // [batch, T, 128] linear mel or null
   float* logmel_out;     // [batch, T, 128] log10(clip(mel, 1e-8)) or null
+  const int64_t* vl_off; // varlen: clip b = wav[vl_off[b] .. vl_off[b + 1]) (device), 1 + n_b / 441 frames at row stride T; or null
 };
 cudaError_t launch_frontend(const FrontendParams& p, cudaStream_t stream);
+
+// Varlen plans (vf_restore_varlen): per clip lengths in a plan-owned device table, written on the call's stream by
+// varlen_setup_kernel from the call's offsets (a kernel parameter: no host memory is read after the call returns), so a
+// captured launch chain with fixed pointers serves any mix of lengths.  Rows of the table, VL_ROWS x batch ints:
+enum {
+  VL_T = 0,          // frames T = 1 + n / hop
+  VL_TP = 1,         // UNet time extent Tp = 64 * ceil(T / 64)
+  VL_UNET = 2,       // + l (l = 0..6): UNet rows of level l, (Tp >> l) * ((w0 >> l) + 1)
+  VL_TV = 9,         // vocoder frames Tv = T + T % 2 + tail_base
+  VL_VOC = 10,       // + s: samples of vocoder stage s, Tv * scales[0] * ... * scales[s]
+  VL_ROWS = 18
+};
+constexpr int VL_MAX_CLIPS = 256;  // clips per launch chain: keeps the setup kernel's parameters within 4 KB
+struct VarlenSetupParams {
+  int64_t off[VL_MAX_CLIPS + 1];   // relative sample offsets of the chain's clips
+  int batch, hop, tail_base, w0, n_stages;
+  int scales[8];
+  int64_t* d_off;                  // [batch + 1]
+  int* d_rows;                     // [VL_ROWS][batch]
+};
+cudaError_t launch_varlen_setup(const VarlenSetupParams& p, cudaStream_t stream);
 
 struct PlanePtr {
   __half* hi;
@@ -46,6 +68,8 @@ struct UnetFirstParams {
   float slope;
   PlanePtr a2;           // [batch, Tp*Wp, 32] act(bn2(conv1(...))), pad column zero
   float* sc_raw;         // [batch, Tp*Wp, 32] fp32 shortcut(x), pad column zero
+  const int* vl_T;       // varlen: per clip T and Tp (rows t >= Tp_b are written as zeros), or null: T, Tp for every clip
+  const int* vl_Tp;
   int* err;
 };
 cudaError_t launch_unet_first(const UnetFirstParams& p, cudaStream_t stream);
@@ -61,6 +85,7 @@ struct PoolParams {
   const float* a_scale;
   const float* a_shift;
   float slope;
+  const int* row_valid;  // varlen: per clip valid output rows (of H/2 * Wpo), the rest written as zeros; or null
   int* err;
 };
 cudaError_t launch_pool(const PoolParams& p, cudaStream_t stream);
@@ -79,19 +104,23 @@ struct VocCondParams {
   const float* band_sums;    // [batch][2] (target, estimate) low-band sums from launch_band_energy, or null:
                              // amp_to_original_f (tools/utils.py:50-55) scales the estimate by target/estimate
   PlanePtr out;          // [batch, Tv, 128]
+  const int* vl_T;       // varlen: per clip T and Tv (rows tv >= Tv_b are written as zeros), or null
+  const int* vl_Tv;
 };
 cudaError_t launch_voc_condition(const VocCondParams& p, cudaStream_t stream);
 
 // amp_to_original_f, reduction half: per clip, sums over frames and mel bins [5, int(128*0.2)) of the noisy
 // linear mel (target) and of from_log(restored log-mel) (estimate).  sums must be zeroed before the launch.
+// vl_T (varlen, or null): clip b sums its first vl_T[b] frames of the [batch, T, 128] buffers, in the order of a T = vl_T[b] launch.
 cudaError_t launch_band_energy(const float* mel_target_lin, const float* logmel_est, int batch, int T, float* sums,
-                               cudaStream_t stream);
+                               cudaStream_t stream, const int* vl_T = nullptr);
 
 // amp_to_original_f as a stand-alone op: out = est * (low-band mean of target / low-band mean of est), linear mels [batch, T, 128].
 cudaError_t launch_amp_to_original(const float* est, const float* tgt, int batch, int T, float* out, cudaStream_t stream);
 
 // nn.ReflectionPad1d(3): rows [3, L+3) of each image are already written; fill 3 + 3 mirrored rows.
-cudaError_t launch_reflect_fill(PlanePtr planes, int batch, int L, int C, int pad, cudaStream_t stream);
+// vl_L (varlen, or null): clip b is vl_L[b] rows long and mirrors at its own end (images keep their L + 6 row stride).
+cudaError_t launch_reflect_fill(PlanePtr planes, int batch, int L, int C, int pad, cudaStream_t stream, const int* vl_L = nullptr);
 
 // Tail: ReflectionPad(3) (pre-filled) + Conv1d(C -> 1, k7) + tanh, plus the per-clip peak |out|.
 struct VocTailParams {
@@ -102,6 +131,7 @@ struct VocTailParams {
   float bias;
   float* wav;            // [batch, L]
   unsigned int* peak_bits;   // [batch] max |out| as float bits (non-negative floats order like uints)
+  const int* vl_L;       // varlen: clip b writes (and peaks over) its first vl_L[b] samples; or null
 };
 cudaError_t launch_voc_tail(const VocTailParams& p, cudaStream_t stream);
 
@@ -113,6 +143,10 @@ struct FinalizeParams {
   long L, n, skip;       // out[b, i] = wav[b, skip + i], i < n
   float* out;            // [batch, out_ld]
   long out_ld, out_off;
+  // varlen (or null): clip b has n_b = vl_off[b + 1] - vl_off[b] samples and a vl_L[b]-sample vocoder output; it is
+  // trimmed by skip_b = (vl_L[b] - n_b) / 2 and written to out[vl_off[b] ..]  (n then bounds every n_b)
+  const int64_t* vl_off;
+  const int* vl_L;
 };
 cudaError_t launch_finalize(const FinalizeParams& p, cudaStream_t stream);
 cudaError_t launch_pcm16(const float* in, int16_t* out, size_t n, int saturate, cudaStream_t stream);

@@ -94,17 +94,20 @@ __global__ void __launch_bounds__(PAIR_THREADS, 1) pair_tc_kernel(const __grid_c
         tma_load_2d(w_base + t * PAIR_W_TAP, &P.wa_map, w_full, t * C, 0);
         tma_load_2d(w_base + (3 + t) * PAIR_W_TAP, &P.wb_map, w_full, t * C, 0);
       }
+      int jl = 0;                              // tiles loaded: the parity of the A slots (empty tiles load nothing)
       for (int j = 0; j < n_local; ++j) {
         const int tile = blockIdx.x + j * gridDim.x;
         const int img = (int)fast_div_pair((uint32_t)tile, (uint32_t)P.tiles_per_img, P.magic_t);
         const int m0 = (tile - img * P.tiles_per_img) * PAIR_ROWS - 1;
+        if (m0 + 1 >= valid_rows(P.row_valid, img)) continue;
         bool ok = true;
         for (int t = 0; t < 3 && ok; ++t) {
-          if (!mbar_wait(a_empty + t, (j & 1) ^ 1u, P.err, ERR_PIPE_PRODUCER)) { ok = false; break; }
+          if (!mbar_wait(a_empty + t, (jl & 1) ^ 1u, P.err, ERR_PIPE_PRODUCER)) { ok = false; break; }
           mbar_expect_tx(a_full + t, PAIR_TILE);
           tma_load_3d(a_base + t * PAIR_TILE, &P.a_map, a_full + t, 0, m0 + (t - 1) * P.dil, img);
         }
         if (!ok) break;
+        ++jl;
       }
     }
     __syncwarp();
@@ -116,6 +119,7 @@ __global__ void __launch_bounds__(PAIR_THREADS, 1) pair_tc_kernel(const __grid_c
         const int img = (int)fast_div_pair((uint32_t)tile, (uint32_t)P.tiles_per_img, P.magic_t);
         const int t0 = (tile - img * P.tiles_per_img) * PAIR_ROWS;
         uint8_t* xs = x_base + st * 2 * PAIR_TILE;
+        if (t0 >= valid_rows(P.row_valid, img)) { mbar_expect_tx(x_full + st, 0); return; }   // empty tile: E2 reads no residual
         mbar_expect_tx(x_full + st, 2 * PAIR_ROWS * 128);
         tma_load_3d(xs, &P.xin_map[0], x_full + st, 0, t0, img);                  // activated plane a
         tma_load_3d(xs + PAIR_TILE, &P.xin_map[1], x_full + st, 0, t0, img);      // correction plane r
@@ -149,13 +153,17 @@ __global__ void __launch_bounds__(PAIR_THREADS, 1) pair_tc_kernel(const __grid_c
     bool ok = mbar_wait(w_full, 0, P.err, ERR_PIPE_MMA);
     const uint32_t dw = make_smem_desc_lo(smem_u32(w_base));
     float acc[C / 2];
+    int jl = 0;                                // tiles computed (the producer's count of loaded tiles)
     for (int j = 0; j < n_local; ++j) {
       const int tile = blockIdx.x + j * gridDim.x;
       const int img = (int)fast_div_pair((uint32_t)tile, (uint32_t)P.tiles_per_img, P.magic_t);
       const int m0 = (tile - img * P.tiles_per_img) * PAIR_ROWS - 1;
+      const int L = min(P.L, valid_rows(P.row_valid, img));   // rows of this clip; a varlen plan zeroes the rest
+      const bool empty = m0 + 1 >= L;          // no valid row: no loads, no MMAs, E2 stores zeros
+      if (!empty) {
       // ---- P1: conv_a, three taps from the A slots
       for (int t = 0; t < 3; ++t) {
-        if (ok && !mbar_wait(a_full + t, j & 1, P.err, ERR_PIPE_MMA)) ok = false;
+        if (ok && !mbar_wait(a_full + t, jl & 1, P.err, ERR_PIPE_MMA)) ok = false;
         const uint32_t da = make_smem_desc_lo(smem_u32(a_base + t * PAIR_TILE + wg * 64 * 128));
         wgmma_fence_regs(acc, C / 2);
         wgmma_fence();
@@ -177,7 +185,7 @@ __global__ void __launch_bounds__(PAIR_THREADS, 1) pair_tc_kernel(const __grid_c
         const int tm = m0 + r;
         float a0 = acc[i] + s_bias_a[c], a1 = acc[i + 1] + s_bias_a[c + 1];
         a0 = fmaxf(a0, a0 * slope_h); a1 = fmaxf(a1, a1 * slope_h);
-        if (tm < 0 || tm >= P.L) { a0 = 0.f; a1 = 0.f; }      // conv_b pads h with zeros outside the clip
+        if (tm < 0 || tm >= L) { a0 = 0.f; a1 = 0.f; }        // conv_b pads h with zeros outside the clip
         amax = fmaxf(amax, fmaxf(fabsf(a0), fabsf(a1)));
         const __half2 hv = __floats2half2_rn(a0, a1);
         const uint32_t bits = *reinterpret_cast<const uint32_t*>(&hv);
@@ -202,7 +210,9 @@ __global__ void __launch_bounds__(PAIR_THREADS, 1) pair_tc_kernel(const __grid_c
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_fence_regs(acc, C / 2);
-      // ---- E2: + bias_b + x, x_new as (a, r)
+      ++jl;
+      }
+      // ---- E2: + bias_b + x, x_new as (a, r); rows past the clip are written as zeros
       const int s = j % PAIR_X_STAGES;
       uint8_t* xa = x_base + s * 2 * PAIR_TILE;
       uint8_t* xr = xa + PAIR_TILE;
@@ -215,6 +225,11 @@ __global__ void __launch_bounds__(PAIR_THREADS, 1) pair_tc_kernel(const __grid_c
         const int xrow = r - 1;
         const int c = 8 * (i >> 2) + cbase;
         const uint32_t off = sw128_off(xrow, c);
+        if (m0 + r >= L) {
+          if (ar_out) *reinterpret_cast<uint32_t*>(xr + off) = 0u;
+          *reinterpret_cast<uint32_t*>(act_base + off) = 0u;
+          continue;
+        }
         float v0 = acc[i] + s_bias_b[c], v1 = acc[i + 1] + s_bias_b[c + 1];
         add_planes(v0, v1, *reinterpret_cast<const uint32_t*>(xa + off), *reinterpret_cast<const uint32_t*>(xr + off), ar_in);
         uint32_t a_bits;

@@ -13,14 +13,16 @@ Same names, arguments and error behaviour as the objects eval_gsr_voicefixer.py:
     plus the batched fused entry points the reference lacks:
       .restore(wav[B,N]) -> wav[B,N]             one launch chain for stages A -> B -> C + normalise + trim
       .restore_host(pinned_in, pinned_out)
+      .restore_batch([wav_i]) -> [out_i]         clips of different lengths in one launch chain
 
 PyTorch is used only to own device memory and streams; every tensor handed back is written by a
 hand-written sm_90a kernel.  Tensors must be fp32 CUDA tensors on the model's device.
 """
 import ctypes
+import itertools
 import json
 import math
-from typing import Dict, Optional
+from typing import Dict, List, Optional, Sequence
 
 import torch
 
@@ -199,6 +201,21 @@ class Engine:
         flags = L.VF_RESTORE_UNIFY_ENERGY if unify_energy else 0
         with torch.cuda.device(self.device):
             self._ck(self.lib.vf_restore_ex(self.ctx, _ptr(wav), b, n, _ptr(out), flags, _stream()))
+        return out
+
+    def restore_varlen(self, wav_packed: torch.Tensor, lengths, out: Optional[torch.Tensor] = None,
+                       unify_energy: bool = False) -> torch.Tensor:
+        """Clips of different lengths in one call (vf_restore_varlen): wav_packed [sum(lengths)] holds the clips back to back;
+        the result is packed the same way, and clip i is bit-identical to restore(clip_i[None])[0]."""
+        wav_packed = _check_in(wav_packed, self.device, "wav_packed")
+        lengths = [int(n) for n in lengths]
+        if wav_packed.dim() != 1 or not lengths or sum(lengths) != wav_packed.numel():
+            raise ValueError("wav_packed must be 1-D and hold exactly sum(lengths) samples of at least one clip")
+        offsets = (ctypes.c_int64 * (len(lengths) + 1))(0, *itertools.accumulate(lengths))
+        out = torch.empty_like(wav_packed) if out is None else out
+        flags = L.VF_RESTORE_UNIFY_ENERGY if unify_energy else 0
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_restore_varlen(self.ctx, _ptr(wav_packed), offsets, len(lengths), _ptr(out), flags, _stream()))
         return out
 
     def mel(self, specgram: torch.Tensor) -> torch.Tensor:
@@ -611,6 +628,24 @@ class VoiceFixer(_EngineModel):
         if pip_kwargs:
             raise TypeError(f"restore(tensor): unexpected arguments {sorted(pip_kwargs)}")
         return self._engine().restore(wav, out, unify_energy=unify_energy)
+
+    def restore_batch(self, wavs: Sequence[torch.Tensor], unify_energy: bool = False) -> List[torch.Tensor]:
+        """Clips of different lengths - a test set, a request queue - restored in one packed call: wavs is a list of 1-D fp32
+        tensors on the model's device, each longer than 1024 samples; returns one view per clip into a packed output.
+        Every clip gets exactly the bits restore(clip[None]) would give it (no zero-padding to a common length)."""
+        eng = self._engine()
+        if not isinstance(wavs, (list, tuple)) or not wavs:
+            raise ValueError("restore_batch: expected a non-empty list of 1-D tensors")
+        for i, w in enumerate(wavs):
+            if not isinstance(w, torch.Tensor) or w.dim() != 1:
+                raise ValueError(f"restore_batch: clip {i} must be a 1-D tensor")
+            if w.dtype != torch.float32 or w.device != eng.device:
+                raise TypeError(f"restore_batch: clip {i} must be float32 on {eng.device} (got {w.dtype} on {w.device})")
+            if w.numel() <= 1024:
+                raise ValueError(f"restore_batch: clip {i} has {w.numel()} samples; reflect padding needs more than 1024")
+        lengths = [w.numel() for w in wavs]
+        out = eng.restore_varlen(torch.cat(wavs), lengths, unify_energy=unify_energy)
+        return list(torch.split(out, lengths))
 
     def restore_inmem(self, wav_10k, cuda=True, mode=0, your_vocoder_func=None):
         """The pip package's in-memory entry point: 44.1 kHz samples -> restored [1, N] numpy (handler.restore_inmem)."""
