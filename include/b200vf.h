@@ -23,6 +23,7 @@
  *                                 SSR_UNet / GSR_UNet inference (BASELINE config 3): models/ssr_unet.py:140-155 ->
  *                                 Generator.forward :51-54 -> unet_v2 UNetResComplex_100Mb.forward
  *                                 models/components/unet_v2.py:86-148 (magnitude net, input phase, ISTFT)
+ *   vf_ssr_restore_varlen         the same for clips of different lengths in one call (eval_ssr_unet.py:handler()'s test set)
  *   vf_istft                      FDomainHelper.istft tools/pytorch/modules/fDomainHelper.py:30-32,127 (torchlibrosa ISTFT)
  *   vf_resample_poly              load_wav's rate conversion, tools/utils.py:46-48
  *   vf_lsd / vf_sispec            AudioMetrics.lsd / .sispec evaluation_proc/metrics.py:83-95 (handler's mel metrics,
@@ -139,6 +140,14 @@ VF_API int vf_restore_ex(vf_ctx* ctx, const float* wav, int batch, int64_t n_sam
  * 256 clips (fewer under the plan budget), each with its own bucket; clips keep their order. */
 VF_API int vf_restore_varlen(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out,
                              unsigned flags, void* stream);
+/* The same for the SSR_UNet / GSR_UNet path: clips of different lengths, packed and with HOST offsets as in
+ * vf_restore_varlen, no flags.  Clip i's output is bit-identical to vf_ssr_restore on that clip alone (batch 1, same
+ * options).  Every clip needs more than 1024 samples and at most 2^30 (no trim_center constraint: there is no vocoder); a
+ * bad argument fails with VF_EINVAL before any work is queued, and a context without the unet_v2 weights
+ * (generator.unet.*) with VF_ESTATE.  Plans, buckets, sub-batches and the lengths' path to the device as in
+ * vf_restore_varlen. */
+VF_API int vf_ssr_restore_varlen(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out,
+                                 void* stream);
 /* Same through HOST buffers (pinned for true asynchrony).  The copies and the compute run on library-owned streams with
  * two staging buffer pairs, so back-to-back calls overlap (the H2D of call i+1 and the D2H of call i-1 run under the
  * compute of call i); `stream` only receives a wait on this call's D2H.  Contract: wav_host holds its data when the
@@ -216,7 +225,7 @@ VF_API int vf_check_errors(vf_ctx* ctx, void* stream);
  * "host_pipeline" (default 1, see vf_restore_host),
  * "validate_simt" (1: run every GEMM on the SIMT validation kernel instead of the wgmma kernel - tests only). */
 VF_API int vf_set_option(vf_ctx* ctx, const char* key, int value);
-/* Plans are cached per (path, batch, frames) - vf_restore_varlen: (batch, bucket) - ; the cache is bounded (see "plan_cache_mb").  A batch whose plan would not fit
+/* Plans are cached per (path, batch, frames) - vf_restore_varlen and vf_ssr_restore_varlen: (path, batch, bucket) - ; the cache is bounded (see "plan_cache_mb").  A batch whose plan would not fit
  * the budget is processed in sub-batches through a smaller plan (same results: rows are independent); the *_stages accessors
  * then only see the last sub-batch. */
 VF_API int vf_plan_cache_info(vf_ctx* ctx, int* n_plans, size_t* bytes, size_t* budget, int64_t* evicted);

@@ -61,10 +61,12 @@ bool init_plan_budget(vf_ctx* ctx) {
   return true;
 }
 
-// The cached plan that size estimates for `kind` scale from (bytes scale with batch * padded frames), or null
+// The cached plan that size estimates for `kind` scale from (bytes scale with batch * padded frames), or null.  An SSR varlen
+// plan without a cached plan of its kind scales from an SSR plan: the same network and buffers per padded frame.
 const Plan* size_reference(vf_ctx* ctx, int kind) {
   for (auto& kv : ctx->plans)
     if (std::get<0>(kv.first) == kind) return kv.second.get();
+  if (kind == PLAN_SSR_VARLEN) return size_reference(ctx, PLAN_SSR);
   return nullptr;
 }
 
@@ -91,9 +93,9 @@ int evict_plans(vf_ctx* ctx, size_t incoming, const Plan* keep) {
 
 // The networks a plan of `kind` runs must have been loaded
 int check_networks(vf_ctx* ctx, int kind) {
-  if (kind != PLAN_SSR && !(ctx->gsr.loaded && ctx->voc_loaded))
+  if (!is_ssr_plan(kind) && !(ctx->gsr.loaded && ctx->voc_loaded))
     return fail(ctx, VF_ESTATE, "this entry point needs the analysis module (generator.analysis_module.*) and the vocoder (vocoder.*) weights");
-  if (kind == PLAN_SSR && !ctx->ssr.loaded)
+  if (is_ssr_plan(kind) && !ctx->ssr.loaded)
     return fail(ctx, VF_ESTATE, "this entry point needs the unet_v2 weights (generator.unet.*)");
   return VF_OK;
 }
@@ -142,7 +144,7 @@ int get_plan(vf_ctx* ctx, int kind, int batch, int frames, Plan** out) {
 int choose_sub_batch(vf_ctx* ctx, int kind, int batch, int frames) {
   init_plan_budget(ctx);
   const double tp = (frames + 63) / 64 * 64;
-  double per_frame = kind == PLAN_SSR ? 2.4e6 : 1.7e6;      // bytes per clip and padded frame (measured 2.19e6 / 1.52e6) + margin
+  double per_frame = is_ssr_plan(kind) ? 2.4e6 : 1.7e6;     // bytes per clip and padded frame (measured 2.19e6 / 1.52e6) + margin
   if (const Plan* ref = size_reference(ctx, kind))
     per_frame = 1.05 * (double)ref->bytes / ((double)ref->batch * ((ref->T + 63) / 64 * 64));
   const double fit = (double)ctx->plan_budget / (per_frame * tp);
@@ -351,6 +353,21 @@ int stage_mark(vf_ctx* ctx, int i, cudaStream_t st) {
   return VF_OK;
 }
 
+// This call's lengths -> the lengths table of a varlen plan (host offsets off[0..batch]), in stream order ahead of every
+// kernel that reads it.  w0: the valid frequency bins of the plan's UNet, 127 (mel UNet) or 1024 (unet_v2).
+int write_lengths_table(vf_ctx* ctx, Plan* plan, const int64_t* off, int batch, int w0, cudaStream_t st) {
+  VarlenSetupParams vp;
+  memset(&vp, 0, sizeof vp);
+  for (int i = 0; i <= batch; ++i) vp.off[i] = off[i];
+  vp.batch = batch; vp.hop = ctx->cfg.hop; vp.tail_base = ctx->cfg.voc_tail_base; vp.w0 = w0;
+  vp.n_stages = ctx->cfg.voc_num_stages;
+  for (int s = 0; s < vp.n_stages; ++s) vp.scales[s] = ctx->cfg.voc_scales[s];
+  vp.d_off = plan->d_vl_off; vp.d_rows = plan->d_vl_rows;
+  CK(launch_varlen_setup(vp, st));
+  ctx->launches++;
+  return VF_OK;
+}
+
 // One restore chain on `plan`.  off == nullptr: `batch` clips of n samples (PLAN_GSR).  Otherwise clips of different
 // lengths (vf_restore_varlen): clip i = wav[off[i] .. off[i + 1]) (host offsets, off[0] = 0, validated by the caller), n = the
 // longest clip, `plan` the PLAN_VARLEN plan for the bucket of its frames; the output is packed like the input.
@@ -361,16 +378,9 @@ int restore_impl(vf_ctx* ctx, Plan* plan, const float* wav, int batch, int64_t n
   int rc = plan_enter(ctx, plan, st);
   if (rc) return rc;
   rc = stage_mark(ctx, 0, st); if (rc) return rc;
-  if (off) {   // this call's lengths -> the plan's table, in stream order ahead of every kernel that reads it
-    VarlenSetupParams vp;
-    memset(&vp, 0, sizeof vp);
-    for (int i = 0; i <= batch; ++i) vp.off[i] = off[i];
-    vp.batch = batch; vp.hop = ctx->cfg.hop; vp.tail_base = ctx->cfg.voc_tail_base; vp.w0 = 127;
-    vp.n_stages = ctx->cfg.voc_num_stages;
-    for (int s = 0; s < vp.n_stages; ++s) vp.scales[s] = ctx->cfg.voc_scales[s];
-    vp.d_off = plan->d_vl_off; vp.d_rows = plan->d_vl_rows;
-    CK(launch_varlen_setup(vp, st));
-    ctx->launches++;
+  if (off) {
+    rc = write_lengths_table(ctx, plan, off, batch, 127, st);
+    if (rc) return rc;
   }
   rc = run_frontend(ctx, wav, batch, (long)n, plan->d_mel, plan->d_logmel_in, nullptr, nullptr, nullptr, st, off ? plan : nullptr);
   if (rc) return rc;
@@ -410,15 +420,22 @@ int restore_impl(vf_ctx* ctx, Plan* plan, const float* wav, int batch, int64_t n
   return plan_exit(ctx, plan, st);
 }
 
-// One SSR / GSR-UNet chain on `plan`: `batch` clips of n samples, magnitudes from the clips themselves (sp == nullptr) or sp
-int ssr_impl(vf_ctx* ctx, Plan* plan, const float* sp, const float* wav, int batch, int64_t n, float* wav_out, cudaStream_t st) {
+// One SSR / GSR-UNet chain on `plan`: `batch` clips of n samples, magnitudes from the clips themselves (sp == nullptr) or sp.
+// off != nullptr: clips of different lengths (vf_ssr_restore_varlen) as in restore_impl, sp == nullptr, `plan` the
+// PLAN_SSR_VARLEN plan for the bucket of the longest clip's frames; rows t >= T_i of d_sp, d_mag and d_frames are never read.
+int ssr_impl(vf_ctx* ctx, Plan* plan, const float* sp, const float* wav, int batch, int64_t n, float* wav_out, cudaStream_t st,
+             const int64_t* off = nullptr) {
   const int frames = plan->T;
   if (ctx->op_timing) ctx->prof.clear();
   int rc = plan_enter(ctx, plan, st);
   if (rc) return rc;
   rc = stage_mark(ctx, 0, st); if (rc) return rc;
+  if (off) {
+    rc = write_lengths_table(ctx, plan, off, batch, 1024, st);
+    if (rc) return rc;
+  }
   if (!sp) {     // SSR_UNet.pre (ssr_unet.py:140-143): the magnitude of the input itself
-    rc = run_frontend(ctx, wav, batch, (long)n, nullptr, nullptr, plan->d_sp, nullptr, nullptr, st);
+    rc = run_frontend(ctx, wav, batch, (long)n, nullptr, nullptr, plan->d_sp, nullptr, nullptr, st, off ? plan : nullptr);
     if (rc) return rc;
   }
   rc = stage_mark(ctx, 1, st); if (rc) return rc;
@@ -431,11 +448,13 @@ int ssr_impl(vf_ctx* ctx, Plan* plan, const float* sp, const float* wav, int bat
   memset(&fp, 0, sizeof fp);
   fp.mag = plan->d_mag; fp.wav = wav; fp.n = (long)n; fp.batch = batch; fp.T = frames;
   fp.window = ctx->d_window; fp.tw1024 = ctx->d_tw1024; fp.tw2048 = ctx->d_tw2048; fp.frames = plan->d_frames;
+  fp.vl_off = plan->d_vl_off; fp.vl_T = plan->vl(VL_T);       // null unless varlen
   CK(launch_istft_frames(fp, st));
   IstftOlaParams op;
   memset(&op, 0, sizeof op);
   op.frames = plan->d_frames; op.batch = batch; op.T = frames; op.length = (long)n; op.window = ctx->d_window;
   op.out = wav_out; op.out_ld = (long)n;
+  op.vl_off = plan->d_vl_off; op.vl_T = plan->vl(VL_T);
   CK(launch_istft_ola(op, st));
   ctx->launches += 2;
   rc = stage_mark(ctx, 3, st); if (rc) return rc;
@@ -457,6 +476,43 @@ int run_sub_batches(vf_ctx* ctx, int kind, int batch, Frames frames, F body, int
     if (rc) return rc;
   }
   return VF_OK;
+}
+
+// Argument checks of a varlen entry point (`fn`) on plans of `kind`, all before anything is launched, so a rejected call
+// leaves no partial output and no work queued: offsets[0] == 0, the networks, then every clip (offsets increase, more than
+// n_fft/2 samples, at most 2^30, and per_clip(i, n) for checks of the entry point's own).
+template <typename F>
+int check_varlen_call(vf_ctx* ctx, const char* fn, int kind, const int64_t* offsets, int batch, F per_clip) {
+  if (offsets[0] != 0) return fail(ctx, VF_EINVAL, "%s: offsets[0] must be 0 (got %ld)", fn, (long)offsets[0]);
+  int rc = check_networks(ctx, kind);
+  if (rc) return rc;
+  for (int i = 0; i < batch; ++i) {
+    const int64_t n = offsets[i + 1] - offsets[i];
+    if (n <= 0) return fail(ctx, VF_EINVAL, "%s: offsets must increase (clip %d: %ld -> %ld)", fn, i, (long)offsets[i], (long)offsets[i + 1]);
+    if (n <= 1024) return fail(ctx, VF_EINVAL, "clip %d: reflect padding needs more than n_fft/2 = 1024 samples (got %ld)", i, (long)n);
+    if (n > (int64_t)1 << 30) return fail(ctx, VF_EINVAL, "clip %d: %ld samples is too long for one restore", i, (long)n);
+    rc = per_clip(i, n);
+    if (rc) return rc;
+  }
+  return VF_OK;
+}
+
+// A varlen call (offsets validated by check_varlen_call) as consecutive sub-batches on plans of `kind` (plan budget, and the
+// lengths table's per-launch cap), each with its own bucket: body(plan, s, b, rel, n_max) runs clips [s, s + b), whose
+// offsets rebased to the sub-batch are rel[0..b] and whose longest clip has n_max samples.
+template <typename F>
+int run_varlen_sub_batches(vf_ctx* ctx, int kind, const int64_t* offsets, int batch, F body) {
+  auto longest = [&](int s, int b) {
+    int64_t n_max = 0;
+    for (int i = s; i < s + b; ++i) n_max = std::max(n_max, offsets[i + 1] - offsets[i]);
+    return n_max;
+  };
+  auto bucket = [&](int s, int b) { return round_up(frames_of(ctx, (long)longest(s, b)), 64); };
+  return run_sub_batches(ctx, kind, batch, bucket, [&](Plan* plan, int s, int b) {
+    int64_t rel[VL_MAX_CLIPS + 1];
+    for (int i = 0; i <= b; ++i) rel[i] = offsets[s + i] - offsets[s];
+    return body(plan, s, b, rel, longest(s, b));
+  }, VL_MAX_CLIPS);
 }
 
 }  // namespace
@@ -623,33 +679,18 @@ VF_API int vf_restore_varlen(vf_ctx* ctx, const float* wav, const int64_t* offse
   if (rc) return rc;
   if (!wav || !wav_out || !offsets || batch <= 0) return fail(ctx, VF_EINVAL, "vf_restore_varlen: bad arguments");
   if (flags & ~(unsigned)VF_RESTORE_UNIFY_ENERGY) return fail(ctx, VF_EINVAL, "vf_restore_varlen: unknown flag bits 0x%x", flags);
-  if (offsets[0] != 0) return fail(ctx, VF_EINVAL, "vf_restore_varlen: offsets[0] must be 0 (got %ld)", (long)offsets[0]);
-  rc = check_networks(ctx, PLAN_VARLEN);
-  if (rc) return rc;
-  // every clip is checked before anything is launched: a rejected call leaves no partial output and no work queued
   long scale = 1;
   for (int s = 0; s < ctx->cfg.voc_num_stages; ++s) scale *= ctx->cfg.voc_scales[s];
-  for (int i = 0; i < batch; ++i) {
-    const int64_t n = offsets[i + 1] - offsets[i];
-    if (n <= 0) return fail(ctx, VF_EINVAL, "vf_restore_varlen: offsets must increase (clip %d: %ld -> %ld)", i, (long)offsets[i], (long)offsets[i + 1]);
-    if (n <= 1024) return fail(ctx, VF_EINVAL, "clip %d: reflect padding needs more than n_fft/2 = 1024 samples (got %ld)", i, (long)n);
-    if (n > (int64_t)1 << 30) return fail(ctx, VF_EINVAL, "clip %d: %ld samples is too long for one restore", i, (long)n);
+  rc = check_varlen_call(ctx, "vf_restore_varlen", PLAN_VARLEN, offsets, batch, [&](int i, int64_t n) {
     const int T = frames_of(ctx, (long)n);
     const long d = (long)(T + T % 2 + ctx->cfg.voc_tail_base) * scale - (long)n;
     if (d < 0 || d == 1) return fail(ctx, VF_EINVAL, "clip %d: vocoder output length %ld incompatible with input %ld (trim_center)", i, (long)n + d, (long)n);
-  }
-  // consecutive clips form sub-batches (plan budget, and the lengths table's per-launch cap); each has its own bucket
-  auto longest = [&](int s, int b) {
-    int64_t n_max = 0;
-    for (int i = s; i < s + b; ++i) n_max = std::max(n_max, offsets[i + 1] - offsets[i]);
-    return n_max;
-  };
-  auto bucket = [&](int s, int b) { return round_up(frames_of(ctx, (long)longest(s, b)), 64); };
-  return run_sub_batches(ctx, PLAN_VARLEN, batch, bucket, [&](Plan* plan, int s, int b) {
-    int64_t rel[VL_MAX_CLIPS + 1];
-    for (int i = 0; i <= b; ++i) rel[i] = offsets[s + i] - offsets[s];
-    return restore_impl(ctx, plan, wav + offsets[s], b, longest(s, b), wav_out + offsets[s], flags, (cudaStream_t)stream, rel);
-  }, VL_MAX_CLIPS);
+    return VF_OK;
+  });
+  if (rc) return rc;
+  return run_varlen_sub_batches(ctx, PLAN_VARLEN, offsets, batch, [&](Plan* plan, int s, int b, const int64_t* rel, int64_t n_max) {
+    return restore_impl(ctx, plan, wav + offsets[s], b, n_max, wav_out + offsets[s], flags, (cudaStream_t)stream, rel);
+  });
 }
 
 VF_API int vf_restore(vf_ctx* ctx, const float* wav, int batch, int64_t n, float* wav_out, void* stream) {
@@ -683,6 +724,17 @@ VF_API int vf_ssr_forward(vf_ctx* ctx, const float* sp, const float* wav, int ba
 
 VF_API int vf_ssr_restore(vf_ctx* ctx, const float* wav, int batch, int64_t n, float* wav_out, void* stream) {
   return vf_ssr_forward(ctx, nullptr, wav, batch, n, wav_out, stream);
+}
+
+VF_API int vf_ssr_restore_varlen(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out, void* stream) {
+  int rc = check_ready(ctx);
+  if (rc) return rc;
+  if (!wav || !wav_out || !offsets || batch <= 0) return fail(ctx, VF_EINVAL, "vf_ssr_restore_varlen: bad arguments");
+  rc = check_varlen_call(ctx, "vf_ssr_restore_varlen", PLAN_SSR_VARLEN, offsets, batch, [](int, int64_t) { return VF_OK; });
+  if (rc) return rc;
+  return run_varlen_sub_batches(ctx, PLAN_SSR_VARLEN, offsets, batch, [&](Plan* plan, int s, int b, const int64_t* rel, int64_t n_max) {
+    return ssr_impl(ctx, plan, nullptr, wav + offsets[s], b, n_max, wav_out + offsets[s], (cudaStream_t)stream, rel);
+  });
 }
 
 VF_API int vf_ssr_restore_host(vf_ctx* ctx, const float* wav_host, int batch, int64_t n, float* out_host, void* stream) {

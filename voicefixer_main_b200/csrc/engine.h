@@ -102,8 +102,13 @@ struct UnetW {
 };
 
 // PLAN_VARLEN: the GSR path for clips of different lengths (vf_restore_varlen), keyed by (batch, bucket): T = the bucket, a
-// multiple of 64 frames (the UNet's time granularity) that holds the call's longest clip
-enum PlanKind { PLAN_GSR = 0, PLAN_SSR = 1, PLAN_VARLEN = 2 };
+// multiple of 64 frames (the UNet's time granularity) that holds the call's longest clip.  PLAN_SSR_VARLEN: the same for
+// the SSR / GSR-UNet path (vf_ssr_restore_varlen)
+enum PlanKind { PLAN_GSR = 0, PLAN_SSR = 1, PLAN_VARLEN = 2, PLAN_SSR_VARLEN = 3 };
+// Plans of these kinds run unet_v2 + ISTFT (build_ssr); the others run the mel UNet + vocoder
+inline bool is_ssr_plan(int kind) { return kind == PLAN_SSR || kind == PLAN_SSR_VARLEN; }
+// Plans of these kinds own a lengths table (kernels.cuh)
+inline bool is_varlen_plan(int kind) { return kind == PLAN_VARLEN || kind == PLAN_SSR_VARLEN; }
 
 struct Plan {
   int kind = PLAN_GSR;

@@ -420,6 +420,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
               if (col < e.ct_out_wp) {         // both=True pruning drops the column past the output pitch
                 orow = (uint32_t)((size_t)img * e.out_img_rows + (size_t)(2 * cth + ph) * e.ct_out_wp + col);
                 flags = kRowValid | ((col == e.ct_out_wp - 1 || r >= vrows) ? kRowPad : 0);
+              } else if (r >= vrows) {         // a dropped column past a varlen clip's rows is not stored, and its value
+                flags = kRowPad;               // (an empty tile's accumulator is never written) must not reach the range check
               }
             } else {
               const long t = (long)r * e.ct_stride + phase - e.ct_pad;

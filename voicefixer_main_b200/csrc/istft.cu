@@ -22,8 +22,15 @@ __global__ void __launch_bounds__(256) istft_frames_kernel(IstftFramesParams p) 
   __shared__ float2 Y[1025];
   const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
   const size_t frame = (size_t)b * p.T + t;
+  if (p.vl_T && t >= __ldg(p.vl_T + b)) return;      // block-uniform: a frame past this clip (varlen)
   if (p.mag) {
-    load_frame_packed(buf0, p.wav + (size_t)b * p.n, p.n, t, p.window, tid);
+    const float* x = p.wav + (size_t)b * p.n;
+    long n = p.n;
+    if (p.vl_off) {      // clips of different lengths: this clip's samples, reflect padded at its own ends
+      x = p.wav + __ldg(p.vl_off + b);
+      n = (long)(__ldg(p.vl_off + b + 1) - __ldg(p.vl_off + b));
+    }
+    load_frame_packed(buf0, x, n, t, p.window, tid);
     __syncthreads();
     const float2* Z = fft1024_forward(buf0, buf1, p.tw1024, tid);
     for (int k = tid; k <= 1024; k += 256) {
@@ -64,16 +71,25 @@ cudaError_t launch_istft_frames(const IstftFramesParams& p, cudaStream_t stream)
   return cudaGetLastError();
 }
 
-// y[p] = sum_t frames[t][p - 441 t] / clamp(sum_t win^2[p - 441 t], 1e-11), p = i + 1024; ascending t (deterministic)
+// y[p] = sum_t frames[t][p - 441 t] / clamp(sum_t win^2[p - 441 t], 1e-11), p = i + 1024; ascending t (deterministic).
+// A varlen clip runs the loop of a one-clip launch over its own frames and samples, so its sums are the same.
 __global__ void __launch_bounds__(256) istft_ola_kernel(IstftOlaParams p) {
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   const int b = blockIdx.y;
-  if (i >= p.length) return;
+  long length = p.length;
+  int T = p.T;
+  size_t o = (size_t)b * p.out_ld;
+  if (p.vl_off) {
+    length = (long)(__ldg(p.vl_off + b + 1) - __ldg(p.vl_off + b));
+    T = __ldg(p.vl_T + b);
+    o = (size_t)__ldg(p.vl_off + b);
+  }
+  if (i >= length) return;
   const long pos = i + 1024;
   long t_lo = (pos - 2047 + 440) / 441;       // ceil((pos - 2047) / 441), pos >= 1024 so the numerator may be negative
   if (pos - 2047 <= 0) t_lo = 0;
   long t_hi = pos / 441;
-  if (t_hi > p.T - 1) t_hi = p.T - 1;
+  if (t_hi > T - 1) t_hi = T - 1;
   float acc = 0.f, ws = 0.f;
   for (long t = t_lo; t <= t_hi; ++t) {
     const int off = (int)(pos - 441 * t);
@@ -81,7 +97,7 @@ __global__ void __launch_bounds__(256) istft_ola_kernel(IstftOlaParams p) {
     const float w = __ldg(p.window + off);
     ws = fmaf(w, w, ws);
   }
-  p.out[(size_t)b * p.out_ld + i] = acc / fmaxf(ws, 1e-11f);
+  p.out[o + i] = acc / fmaxf(ws, 1e-11f);
 }
 cudaError_t launch_istft_ola(const IstftOlaParams& p, cudaStream_t stream) {
   dim3 grid((unsigned)((p.length + 255) / 256), p.batch);

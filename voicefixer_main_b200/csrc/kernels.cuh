@@ -26,13 +26,13 @@ struct FrontendParams {
 };
 cudaError_t launch_frontend(const FrontendParams& p, cudaStream_t stream);
 
-// Varlen plans (vf_restore_varlen): per clip lengths in a plan-owned device table, written on the call's stream by
-// varlen_setup_kernel from the call's offsets (a kernel parameter: no host memory is read after the call returns), so a
-// captured launch chain with fixed pointers serves any mix of lengths.  Rows of the table, VL_ROWS x batch ints:
+// Varlen plans (vf_restore_varlen, vf_ssr_restore_varlen): per clip lengths in a plan-owned device table, written on the
+// call's stream by varlen_setup_kernel from the call's offsets (a kernel parameter: no host memory is read after the call
+// returns), so a captured launch chain with fixed pointers serves any mix of lengths.  Rows of the table, VL_ROWS x batch ints:
 enum {
   VL_T = 0,          // frames T = 1 + n / hop
   VL_TP = 1,         // UNet time extent Tp = 64 * ceil(T / 64)
-  VL_UNET = 2,       // + l (l = 0..6): UNet rows of level l, (Tp >> l) * ((w0 >> l) + 1)
+  VL_UNET = 2,       // + l (l = 0..6): UNet rows of level l, (Tp >> l) * ((w0 >> l) + 1); w0 = 127 (mel UNet) or 1024 (unet_v2)
   VL_TV = 9,         // vocoder frames Tv = T + T % 2 + tail_base
   VL_VOC = 10,       // + s: samples of vocoder stage s, Tv * scales[0] * ... * scales[s]
   VL_ROWS = 18
@@ -184,6 +184,10 @@ struct IstftFramesParams {
   const float2* tw1024;
   const float2* tw2048;
   float* frames;         // [batch, T, 2048]
+  // varlen (with mag, or null): clip b = wav[vl_off[b] .. vl_off[b + 1]) (device), reflect padded at its own ends; only its
+  // first vl_T[b] frames are computed (mag and frames keep the row stride T, the rows past vl_T[b] are not touched)
+  const int64_t* vl_off;
+  const int* vl_T;
 };
 cudaError_t launch_istft_frames(const IstftFramesParams& p, cudaStream_t stream);
 struct IstftOlaParams {
@@ -193,6 +197,10 @@ struct IstftOlaParams {
   const float* window;
   float* out;            // [batch, out_ld]
   long out_ld;
+  // varlen (or null): clip b produces n_b = vl_off[b + 1] - vl_off[b] samples from its first vl_T[b] frames, in the
+  // order of a one-clip launch, written to out[vl_off[b] ..]  (length then bounds every n_b)
+  const int64_t* vl_off;
+  const int* vl_T;
 };
 cudaError_t launch_istft_ola(const IstftOlaParams& p, cudaStream_t stream);
 

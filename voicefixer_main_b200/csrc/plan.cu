@@ -730,11 +730,11 @@ int build_plan(vf_ctx* ctx, Plan* plan) {
   const int kind = plan->kind, batch = plan->batch, frames = plan->T;
   Builder b{ctx, plan};
   int rc = VF_OK;
-  if (kind == PLAN_VARLEN) {
+  if (is_varlen_plan(kind)) {
     plan->d_vl_off = b.alloc<int64_t>((size_t)batch + 1);
     plan->d_vl_rows = b.alloc<int>((size_t)VL_ROWS * batch);
   }
-  if (kind != PLAN_SSR) {
+  if (!is_ssr_plan(kind)) {
     const size_t mel_n = (size_t)batch * frames * 128;
     plan->d_mel = b.alloc<float>(mel_n);
     plan->d_logmel_in = b.alloc<float>(mel_n);

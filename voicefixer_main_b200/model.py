@@ -14,6 +14,7 @@ Same names, arguments and error behaviour as the objects eval_gsr_voicefixer.py:
       .restore(wav[B,N]) -> wav[B,N]             one launch chain for stages A -> B -> C + normalise + trim
       .restore_host(pinned_in, pinned_out)
       .restore_batch([wav_i]) -> [out_i]         clips of different lengths in one launch chain
+    SSR_UNet / GSR_UNet (models/ssr_unet.py) have .restore(wav[B,N]), .restore_host and .restore_batch([wav_i]) the same way.
 
 PyTorch is used only to own device memory and streams; every tensor handed back is written by a
 hand-written sm_90a kernel.  Tensors must be fp32 CUDA tensors on the model's device.
@@ -207,16 +208,20 @@ class Engine:
                        unify_energy: bool = False) -> torch.Tensor:
         """Clips of different lengths in one call (vf_restore_varlen): wav_packed [sum(lengths)] holds the clips back to back;
         the result is packed the same way, and clip i is bit-identical to restore(clip_i[None])[0]."""
+        wav_packed, offsets = self._varlen_args(wav_packed, lengths)
+        out = torch.empty_like(wav_packed) if out is None else out
+        flags = L.VF_RESTORE_UNIFY_ENERGY if unify_energy else 0
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_restore_varlen(self.ctx, _ptr(wav_packed), offsets, len(offsets) - 1, _ptr(out), flags, _stream()))
+        return out
+
+    def _varlen_args(self, wav_packed: torch.Tensor, lengths):
+        """Checked packed input and the host offsets array (0, then the running sum of lengths) of a varlen call."""
         wav_packed = _check_in(wav_packed, self.device, "wav_packed")
         lengths = [int(n) for n in lengths]
         if wav_packed.dim() != 1 or not lengths or sum(lengths) != wav_packed.numel():
             raise ValueError("wav_packed must be 1-D and hold exactly sum(lengths) samples of at least one clip")
-        offsets = (ctypes.c_int64 * (len(lengths) + 1))(0, *itertools.accumulate(lengths))
-        out = torch.empty_like(wav_packed) if out is None else out
-        flags = L.VF_RESTORE_UNIFY_ENERGY if unify_energy else 0
-        with torch.cuda.device(self.device):
-            self._ck(self.lib.vf_restore_varlen(self.ctx, _ptr(wav_packed), offsets, len(lengths), _ptr(out), flags, _stream()))
-        return out
+        return wav_packed, (ctypes.c_int64 * (len(lengths) + 1))(0, *itertools.accumulate(lengths))
 
     def mel(self, specgram: torch.Tensor) -> torch.Tensor:
         """MelScale.forward: specgram [..., 1025, time] (any strides) -> [..., 128, time]."""
@@ -262,6 +267,15 @@ class Engine:
         out = torch.empty_like(wav) if out is None else out
         with torch.cuda.device(self.device):
             self._ck(self.lib.vf_ssr_forward(self.ctx, _ptr(sp), _ptr(wav), b, n, _ptr(out), _stream()))
+        return out
+
+    def ssr_restore_varlen(self, wav_packed: torch.Tensor, lengths, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """restore_varlen for the SSR / GSR-UNet path (vf_ssr_restore_varlen): clip i of the packed result is bit-identical
+        to ssr_forward(None, clip_i[None])[0]."""
+        wav_packed, offsets = self._varlen_args(wav_packed, lengths)
+        out = torch.empty_like(wav_packed) if out is None else out
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_ssr_restore_varlen(self.ctx, _ptr(wav_packed), offsets, len(offsets) - 1, _ptr(out), _stream()))
         return out
 
     def ssr_restore_host(self, wav_host: torch.Tensor, out_host: torch.Tensor):
@@ -524,6 +538,21 @@ class _EngineModel:
     def _need(self):
         return self._NEED
 
+    def _batch_engine(self, wavs):
+        """The engine and the clip lengths for restore_batch(wavs), after checking the clips before anything is launched: a
+        non-empty list of 1-D float32 tensors on the model's device, each longer than 1024 samples."""
+        eng = self._engine()
+        if not isinstance(wavs, (list, tuple)) or not wavs:
+            raise ValueError("restore_batch: expected a non-empty list of 1-D tensors")
+        for i, w in enumerate(wavs):
+            if not isinstance(w, torch.Tensor) or w.dim() != 1:
+                raise ValueError(f"restore_batch: clip {i} must be a 1-D tensor")
+            if w.dtype != torch.float32 or w.device != eng.device:
+                raise TypeError(f"restore_batch: clip {i} must be float32 on {eng.device} (got {w.dtype} on {w.device})")
+            if w.numel() <= 1024:
+                raise ValueError(f"restore_batch: clip {i} has {w.numel()} samples; reflect padding needs more than 1024")
+        return eng, [w.numel() for w in wavs]
+
     def load_state_dict(self, state_dict, strict=True, vocoder_state=None):
         """state_dict: reference names for the analysis network (generator.analysis_module.* / generator.unet.*).
         The vocoder is NOT part of what a reference Lightning checkpoint can provide in loadable form (see
@@ -633,17 +662,7 @@ class VoiceFixer(_EngineModel):
         """Clips of different lengths - a test set, a request queue - restored in one packed call: wavs is a list of 1-D fp32
         tensors on the model's device, each longer than 1024 samples; returns one view per clip into a packed output.
         Every clip gets exactly the bits restore(clip[None]) would give it (no zero-padding to a common length)."""
-        eng = self._engine()
-        if not isinstance(wavs, (list, tuple)) or not wavs:
-            raise ValueError("restore_batch: expected a non-empty list of 1-D tensors")
-        for i, w in enumerate(wavs):
-            if not isinstance(w, torch.Tensor) or w.dim() != 1:
-                raise ValueError(f"restore_batch: clip {i} must be a 1-D tensor")
-            if w.dtype != torch.float32 or w.device != eng.device:
-                raise TypeError(f"restore_batch: clip {i} must be float32 on {eng.device} (got {w.dtype} on {w.device})")
-            if w.numel() <= 1024:
-                raise ValueError(f"restore_batch: clip {i} has {w.numel()} samples; reflect padding needs more than 1024")
-        lengths = [w.numel() for w in wavs]
+        eng, lengths = self._batch_engine(wavs)
         out = eng.restore_varlen(torch.cat(wavs), lengths, unify_energy=unify_energy)
         return list(torch.split(out, lengths))
 
@@ -702,6 +721,14 @@ class SSR_UNet(_EngineModel):
     def restore(self, wav: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """pre + forward fused: wav [B,N] -> denoised [B,N] (the magnitude never leaves the device plan)."""
         return self._engine().ssr_forward(None, wav, out)
+
+    def restore_batch(self, wavs: Sequence[torch.Tensor]) -> List[torch.Tensor]:
+        """Clips of different lengths - eval_ssr_unet.py:handler()'s test set, a request queue - in one packed call: wavs is a
+        list of 1-D fp32 tensors on the model's device, each longer than 1024 samples; returns one view per clip into a packed
+        output.  Every clip gets exactly the bits restore(clip[None]) would give it (no zero-padding to a common length)."""
+        eng, lengths = self._batch_engine(wavs)
+        out = eng.ssr_restore_varlen(torch.cat(wavs), lengths)
+        return list(torch.split(out, lengths))
 
     def restore_host(self, wav_host: torch.Tensor, out_host: torch.Tensor):
         self._engine().ssr_restore_host(wav_host, out_host)
