@@ -345,3 +345,28 @@ def test_vocoder_fused_pair_vs_two_launch_path(state, monkeypatch):
     assert float((out - ref).pow(2).mean().sqrt()) < WAV_RMS_TOL * 0.2
     assert float((plain - ref).pow(2).mean().sqrt()) < WAV_RMS_TOL * 0.2
     assert float((out - plain).pow(2).mean().sqrt()) < WAV_RMS_TOL * 0.2
+
+
+def test_vocoder_separate_planes_without_ar_inverse(model, state):
+    """A residual slope with no fp16 inverse (0: ReLU) cannot use the (a, r) stream: the stacks keep x as separate hi/lo
+    planes, added through identity taps with a lo pass (C <= 128) or in the epilogue (C > 128), and the C = 64 stacks take
+    two launches per residual pair."""
+    from voicefixer_main_b200 import VocoderConfig, VoiceFixer
+    cfg = VocoderConfig(res_slope=0.0)
+    gen = torch.Generator().manual_seed(17)
+    mel = 10 ** (torch.randn(2, 1, 37, 128, generator=gen) * 0.7 - 1.5)
+    with torch.no_grad():
+        ref = O.vocoder_forward(state, mel, cfg)
+    m = VoiceFixer(vocoder_config=cfg).load_state_dict(state).eval().to("cuda:0")
+    eng, eng_ar = m._engine(), model._engine()
+    n0 = eng_ar.launch_count()
+    model.vocoder(mel.cuda())
+    n_ar = eng_ar.launch_count() - n0
+    n1 = eng.launch_count()
+    out = m.vocoder(mel.cuda()).cpu()
+    eng.check_errors()
+    assert eng.launch_count() - n1 > n_ar                         # no fused pair ran
+    assert out.shape == ref.shape
+    rms = float((out - ref).pow(2).mean().sqrt())
+    print("separate-planes vocoder rms err", rms, "ref rms", float(ref.pow(2).mean().sqrt()))
+    assert rms < WAV_RMS_TOL * 0.2

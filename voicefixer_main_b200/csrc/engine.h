@@ -20,7 +20,7 @@
 
 namespace vf {
 cudaError_t launch_gemm_tc(const GemmTcParams& p, int bn, int bk, cudaStream_t stream);
-size_t gemm_tc_smem_bytes(int bn, int bk, int stages, int planes_a, int terms, int a_box_rows, int gmax, int tile_chunks, int resid_tma = 0);
+size_t gemm_tc_smem_bytes(int bn, int bk, int stages, int planes_a, int terms, int tile_chunks, int resid_tma);
 int gemm_tc_max_bn(int terms);
 cudaError_t launch_pair_tc(const PairParams& p, cudaStream_t stream);
 size_t pair_tc_smem_bytes(int C);
@@ -234,7 +234,9 @@ inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 int upload_gemm(vf_ctx* ctx, GemmW* w, const std::vector<float>& m, int N, int K, const std::vector<float>* bias);
 int build_tables(vf_ctx* ctx);
 int load_all(vf_ctx* ctx);
-int ident_max_c();
+// Residual add of a vocoder stack as an identity tap (through the accumulator, no epilogue loads) up to this channel count;
+// above it the epilogue adds the hi/lo planes.  The packer appends the identity block and the plan builder adds the tap.
+constexpr int IDENT_MAX_C = 128;
 
 // plan.cu
 struct Builder {

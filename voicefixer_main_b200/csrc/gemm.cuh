@@ -33,18 +33,14 @@ enum { ACT_NONE = 0, ACT_LRELU = 1, ACT_ELU = 2 };
 enum { MAP_PLAIN = 0, MAP_CONVT2D = 1, MAP_CONVT1D = 2 };
 enum { ERR_FP16_OVERFLOW = 100, ERR_PIPE_PRODUCER = 201, ERR_PIPE_MMA = 202, ERR_PIPE_EPILOGUE = 203 };
 
-struct GemmTap {   // one tap, or a GROUP of up to 3 taps that read row-adjacent windows of the same source
-  int a_off;   // row offset of the (group's) window start relative to the output row
+struct GemmTap {
+  int a_off;   // row offset of the tap's window relative to the output row
   int src;     // which A source (0/1)
   int c_off;   // first channel inside the source
-  int k_off;   // first column of the (first) tap's segment in the packed weight matrix
-  int nch;     // channels contracted by each tap (multiple of the kernel's BK)
+  int k_off;   // first column of the tap's segment in the packed weight matrix
+  int nch;     // channels contracted by the tap (multiple of the kernel's BK)
   int both;    // 1: contract hi AND lo planes of A even in 1-term mode (identity tap carrying the fp32-grade
                //    residual stream through the accumulator)
-  int g;       // taps in the group (1..3; the engine builds groups of 1 for the wgmma kernel).  Halo load: the A
-               // window (128 + 2 rows) fetched once, tap i an MMA on the view shifted by shift[i] rows
-  int shift[3];
-  int kstride; // columns between consecutive taps' weight segments
 };
 
 struct OutPlane {
@@ -89,8 +85,8 @@ struct GemmEpilogue {
   // instead of 6 bytes per element out of every residual layer (no separate hi plane of x).
   uint32_t resid_ar;     // the residual planes (resid_hi, resid_lo) hold (a, r): add U(a) + r
   uint32_t out_ar;       // out_a is written as (hi plane = a, lo plane = r); 1-term kernels, ACT_LRELU, no affine
-  int tma_out;           // bit 3: MAP_CONVT1D out_a through a 5-D map (see gemm_tc.cu).  MAP_PLAIN layers: bit 0 out_raw, bit 1 out_r, bit 2 out_a leave the staging tiles by TMA store
-                         // (GemmTcParams::o_raw / o_r / o_a) instead of LDS + STG: half the LSU wavefronts of the store path
+  int tma_out;           // 1: MAP_CONVT1D out_a leaves the staging tiles by TMA store through a 5-D map (see gemm_tc.cu).
+                         // MAP_PLAIN outputs always do (GemmTcParams::o_raw / o_r / o_a)
   // Clips of different lengths in one plan (vf_restore_varlen): per image, the count of valid rows - GEMM rows for MAP_PLAIN /
   // MAP_CONVT2D, output rows for MAP_CONVT1D.  Rows past it are written as zeros in every output, like the pad column, so the
   // next conv reads the zero padding it would see past the end of a clip-sized tensor.  nullptr: every row is valid.
@@ -124,17 +120,15 @@ struct GemmProblem {
 struct GemmTcParams {
   CUtensorMap a_hi[2], a_lo[2];   // [C, rows, n_img] fp16
   CUtensorMap b_hi, b_lo;         // [Ktot, N] fp16 (K-major)
-  CUtensorMap i_res;              // epilogue residual by TMA load (resid_tma): fp32 [resid_ld, rows_in, n_img] box 32 x 32 x 1
+  CUtensorMap i_res;              // epilogue residual by TMA load (MAP_PLAIN only): fp32 [resid_ld, rows_in, n_img] box 32 x 32 x 1
                                   // SWIZZLE_128B (3-term), or fp16 planes [resid_ld, rows_in, n_img, 2] box 32 x 32 x 1 x 2 SWIZZLE_64B
-  int resid_tma;                  // 1: each epilogue warp owns a second 4 KB tile + an mbarrier for it
-  CUtensorMap o_raw;              // fp32 [raw_ld, rows, n_img], box 32 x 32 x 1, SWIZZLE_128B (epilogue TMA stores, see tma_out)
-  CUtensorMap o_r, o_a;           // fp16 [ld, rows, n_img, planes], box 32 x 32 x 1 x planes, SWIZZLE_64B
+  int resid_tma;                  // residual tiles in flight per epilogue warp (4 KB and an mbarrier each): 1 or 2; 0 without a residual
+  CUtensorMap o_raw;              // MAP_PLAIN epilogue TMA stores: fp32 [raw_ld, rows, n_img], box 32 x 32 x 1, SWIZZLE_128B
+  CUtensorMap o_r, o_a;           // fp16 [ld, rows, n_img, planes], box 32 x 32 x 1 x planes, SWIZZLE_64B (o_a: also see tma_out)
   int stages;
   int tile_chunks; // BK-wide K chunks per output tile
   int seg_chunks;  // 3-term mode: chunks per accumulation segment (promotion to registers in between)
   int planes_a;    // smem slots per stage for A: 2 when any tap contracts the lo plane
-  int a_box_rows;  // rows per A TMA box: 128, or 130 when taps are grouped (halo)
-  int gmax;        // largest tap group: B slots per stage (1: the wgmma kernel loads every tap on its own)
   int grid;        // persistent CTAs
   uint32_t magic_n, magic_m;   // gemm_tc_magic() of N / BN and m_tiles: division-free tile decoding
   GemmProblem prob;
@@ -158,15 +152,11 @@ struct PairParams {
   int* err;
 };
 
-__host__ __device__ inline uint32_t fast_div_pair(uint32_t n, uint32_t d, uint32_t magic) {
-#ifdef __CUDA_ARCH__
-  if (magic == 0u) return n;
-  if (magic == 0xffffffffu) return n / d;
+// n / d with the host's multiply-high magic number (gemm_tc_magic): a handful of instructions instead of an integer division
+__device__ __forceinline__ uint32_t fast_div(uint32_t n, uint32_t d, uint32_t magic) {
+  if (magic == 0u) return n;                    // d == 1
+  if (magic == 0xffffffffu) return n / d;       // range too large for the 32-bit magic (host decides)
   return __umulhi(n, magic);
-#else
-  (void)magic;
-  return n / d;
-#endif
 }
 
 struct GemmSimtParams {            // validation kernel: same contract, plain pointers

@@ -1,6 +1,6 @@
 // SIMT fp32 implementation of the flat-shift multi-tap GEMM contract (gemm.cuh).
 // VALIDATION KERNEL: it exists so every tensor-core GEMM launch can be cross-checked element by element on the
-// device (tests/test_gemm_gpu.py, VF_DEBUG_SIMT=1); the product path always runs gemm_tc.cu.
+// device (vf_selftest_gemm, and whole plans under the option validate_simt); the product path always runs gemm_tc.cu.
 // One thread per output row, 32 output columns per pass; the weight tile is staged in shared memory as
 // fp32 (hi + lo), the activation row is read straight from the hi/lo planes.
 #include "gemm.cuh"
@@ -21,32 +21,29 @@ __global__ void __launch_bounds__(128) gemm_simt_kernel(const GemmSimtParams P) 
 
   for (int t = 0; t < pr.ntaps; ++t) {
     const GemmTap tap = pr.taps[t];
-    for (int gi = 0; gi < tap.g; ++gi) {
-      const int row = r + tap.a_off + tap.shift[gi];
-      const int koff = tap.k_off + gi * tap.kstride;
-      const bool in = row >= 0 && row < P.a_rows[tap.src];
-      const size_t abase = ((size_t)img * P.a_img_rows[tap.src] + (in ? row : 0)) * P.a_ld[tap.src] + tap.c_off;
-      for (int c0 = 0; c0 < tap.nch; c0 += 64) {
-        const int cw = min(64, tap.nch - c0);
-        __syncthreads();
-        for (int idx = threadIdx.x; idx < 32 * 64; idx += 128) {
-          const int n = idx >> 6, k = idx & 63;
-          float w = 0.f;
-          if (k < cw) {
-            const size_t wi = (size_t)(n0 + n) * P.ktot + koff + c0 + k;
-            w = __half2float(P.b_hi[wi]);
-            if (three) w += __half2float(P.b_lo[wi]);
-          }
-          w_s[n][k] = w;
+    const int row = r + tap.a_off;
+    const bool in = row >= 0 && row < P.a_rows[tap.src];
+    const size_t abase = ((size_t)img * P.a_img_rows[tap.src] + (in ? row : 0)) * P.a_ld[tap.src] + tap.c_off;
+    for (int c0 = 0; c0 < tap.nch; c0 += 64) {
+      const int cw = min(64, tap.nch - c0);
+      __syncthreads();
+      for (int idx = threadIdx.x; idx < 32 * 64; idx += 128) {
+        const int n = idx >> 6, k = idx & 63;
+        float w = 0.f;
+        if (k < cw) {
+          const size_t wi = (size_t)(n0 + n) * P.ktot + tap.k_off + c0 + k;
+          w = __half2float(P.b_hi[wi]);
+          if (three) w += __half2float(P.b_lo[wi]);
         }
-        __syncthreads();
-        if (in) {
-          for (int k = 0; k < cw; ++k) {
-            float a = __half2float(P.a_hi[tap.src][abase + c0 + k]);
-            if (three || tap.both) a += __half2float(P.a_lo[tap.src][abase + c0 + k]);
+        w_s[n][k] = w;
+      }
+      __syncthreads();
+      if (in) {
+        for (int k = 0; k < cw; ++k) {
+          float a = __half2float(P.a_hi[tap.src][abase + c0 + k]);
+          if (three || tap.both) a += __half2float(P.a_lo[tap.src][abase + c0 + k]);
 #pragma unroll
-            for (int n = 0; n < 32; ++n) acc[n] = fmaf(a, w_s[n][k], acc[n]);
-          }
+          for (int n = 0; n < 32; ++n) acc[n] = fmaf(a, w_s[n][k], acc[n]);
         }
       }
     }

@@ -17,11 +17,11 @@
 // against the stacked [B_hi; B_lo] tile, lo*hi is a second MMA of width BN into the correction half, so the two small
 // correction products never mix into the main chain.
 //
-// Epilogue I/O.  A thread owns a row, but global stores are issued row-major by the whole warp: values are
-// transposed through a swizzled shared-memory staging tile so every LDG/STG instruction touches whole
-// 64/128-byte row segments.  The accumulator fragments reach the row-per-thread layout through the same staging tiles
-// (64 columns of the warp group's 64 rows per round).  Per-tile constants (bias, BN scale/shift, head weights) live in
-// shared memory.
+// Epilogue I/O.  A thread owns a row; a warp's 32 rows x 32 columns pass through its swizzled shared-memory staging tile.
+// Residual tiles arrive there by TMA load, and MAP_PLAIN outputs leave by TMA store.  The transposed convs scatter their
+// rows, so the whole warp stores them row-major from the staging tile, every STG touching whole 64-byte row segments.
+// The accumulator fragments reach the row-per-thread layout through the same staging tiles (64 columns of the warp
+// group's 64 rows per round).  Per-tile constants (bias, BN scale/shift, head weights) live in shared memory.
 #include "gemm.cuh"
 #include "ptx.cuh"
 
@@ -52,18 +52,13 @@ __device__ __forceinline__ void wg_bar_sync(int wg) {      // the 128 threads of
 struct ChunkDesc {
   int a_c;          // channel coordinate of the A box
   int a_off;        // row offset of the A box relative to the tile's first row
-  uint32_t kk;      // K coordinate of the first weight tile | kstride << 16 (stride between the weight tiles of a group)
+  uint32_t kk;      // K coordinate of the weight tile
   uint32_t flags;   // bit 0 src, bit 4 (hi-only kernels) the A tile is the lo plane: the second pass of an identity tap
 };
 
 // Tile coordinates without loop-carried state: tile = (img * m_tiles + mi) * n_tiles + nt, decoded per tile with the
-// host's multiply-high magic numbers (gemm_tc_magic): a handful of instructions instead of two integer divisions,
-// and no registers held across the tile loop (the accumulators take most of the register file).
-__device__ __forceinline__ uint32_t fast_div(uint32_t n, uint32_t d, uint32_t magic) {
-  if (magic == 0u) return n;                    // d == 1
-  if (magic == 0xffffffffu) return n / d;       // range too large for the 32-bit magic (host decides)
-  return __umulhi(n, magic);
-}
+// host's multiply-high magic numbers (fast_div): no registers held across the tile loop (the accumulators take most of
+// the register file).
 struct TileCoord {
   int nt, mi, img;
   __device__ __forceinline__ TileCoord(uint32_t tile, const GemmTcParams& P, int n_tiles, int m_tiles) {
@@ -130,10 +125,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
   const int stages = P.stages;
   const int planes_a = P.planes_a;                      // 2 when any tap contracts the lo plane of A
   constexpr int B_SLOT = (THREE ? 2 : 1) * B_BYTES;      // [B_hi][B_lo] of one tap, contiguous
-  const int a_box_bytes = P.a_box_rows * ROW_BYTES;     // bytes one A TMA box delivers
-  const int a_slot = (a_box_bytes + 1023) & ~1023;
-  const int off_b = planes_a * a_slot;
-  const int stage_bytes = off_b + P.gmax * B_SLOT;
+  constexpr int A_BOX_BYTES = GEMM_BM * ROW_BYTES;      // bytes one A TMA box delivers: a whole number of 1 KB swizzle atoms
+  const int off_b = planes_a * A_BOX_BYTES;
+  const int stage_bytes = off_b + B_SLOT;
   uint8_t* stg_base = smem + (size_t)stages * stage_bytes;          // EPI_WARPS x 4 KB staging
   uint8_t* rstg_base = stg_base + EPI_WARPS * 4096;                  // resid_tma: EPI_WARPS x 4 KB residual tiles (TMA destination)
   uint8_t* tail = rstg_base + (size_t)P.resid_tma * EPI_WARPS * 4096;  // P.resid_tma = tiles in flight per warp (0, 1 or 2)
@@ -184,7 +178,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     ChunkDesc cd;
     cd.a_c = tap.c_off + c;
     cd.a_off = tap.a_off;
-    cd.kk = (uint32_t)(tap.k_off + c) | ((uint32_t)tap.kstride << 16);
+    cd.kk = (uint32_t)(tap.k_off + c);
     cd.flags = (uint32_t)(tap.src & 1) | (lo_pass ? 16u : 0u);
     s_tab[ci] = cd;
   }
@@ -213,9 +207,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         const bool lo_pass = (cur.flags & 16u) != 0;
         const int src = cur.flags & 1u;
         uint8_t* st = smem + (size_t)s * stage_bytes;
-        mbar_expect_tx(full_bar + s, (THREE ? 2u : 1u) * a_box_bytes + B_SLOT);
-        const int k0 = cur.kk & 0xffffu;
-        if (THREE) {      // hi and lo planes of A in one 4-D box, [B_hi][B_lo] of a tap in one 3-D box (a_slot == box bytes)
+        mbar_expect_tx(full_bar + s, (THREE ? 2u : 1u) * A_BOX_BYTES + B_SLOT);
+        const int k0 = cur.kk;
+        if (THREE) {      // hi and lo planes of A in one 4-D box, [B_hi][B_lo] of a tap in one 3-D box
           tma_load_4d(st, &P.a_hi[src], full_bar + s, cur.a_c, m0 + cur.a_off, img, 0);
           tma_load_3d(st + off_b, &P.b_hi, full_bar + s, k0, n0, 0);
         } else {
@@ -248,29 +242,25 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     const bool has_affine = THREE && e.a_scale != nullptr, has_bias = e.bias != nullptr;
     const bool want_a = e.out_a.hi != nullptr, want_r = e.out_r.hi != nullptr, want_raw = THREE && e.out_raw != nullptr;
     const bool has_resid = THREE && e.resid != nullptr, has_resid_planes = e.resid_hi != nullptr, has_head = THREE && e.head_w != nullptr;
-    constexpr bool PREFETCH = false;     // residual planes of the next chunk in registers: no room next to the accumulator
     const int act = e.act;
     const float slope = e.slope;
     const uint32_t resid_ar = THREE ? 0u : e.resid_ar, out_ar = THREE ? 0u : e.out_ar;      // (a, r) residual stream, gemm.cuh
-    // lane roles for the row-major global accesses
-    const int f_row = lane >> 3, f_c16 = lane & 7;       // fp32: 4 rows x 128 B per instruction
-    const int h_row = lane >> 2, h_c16 = lane & 3;       // fp16: 8 rows x 64 B per instruction
+    // lane roles for the row-major stores of the transposed convs: 8 rows x 64 B of fp16 per instruction
+    const int h_row = lane >> 2, h_c16 = lane & 3;
     // staging slots: own row (so_*) and row-major role (sr_*); the swizzle terms are lane constants
     const int so_h0 = lane * 4, so_hx = (lane >> 1) & 3;            // sw64(lane, i)      = so_h0 + (i ^ so_hx)
     const int sr_h0 = h_row * 4, sr_hx = h_c16;                     // sw64(8i+h_row, c)  = 32 i + sr_h0 + (c ^ ((h_row >> 1) & 3)) (8i keeps bits 1-2)
     const int so_f0 = lane * 8, so_fx = lane & 7;                   // sw128(lane, i)     = so_f0 + (i ^ so_fx)
-    const int sr_f0 = f_row * 8;                                    // sw128(4i+f_row, c) = 32 i + sr_f0 + (c ^ ((4i + f_row) & 7))
 #define SO_H(i) (so_h0 + ((i) ^ so_hx))
 #define SR_H(i) (32 * (i) + sr_h0 + (sr_hx ^ ((h_row >> 1) & 3)))
 #define SO_F(i) (so_f0 + ((i) ^ so_fx))
-#define SR_F(i) (32 * (i) + sr_f0 + (f_c16 ^ ((4 * (i) + f_row) & 7)))
-    // TMA-store output path (MAP_PLAIN layers, e.tma_out): the staging tiles are written in the layouts SWIZZLE_128B (fp32,
+    // TMA-store output path (every MAP_PLAIN output): the staging tiles are written in the layouts SWIZZLE_128B (fp32,
     // 128-byte rows) / SWIZZLE_64B (fp16, 64-byte rows) expect - chunk ^ (row & 7) and chunk ^ ((row >> 1) & 3) are exactly the
     // SO_F / SO_H slots - so lane 0 hands a finished tile to the copy engine instead of the warp reading it back row-major and
     // storing it with 12 STG per lane: half the LSU wavefronts of the store path, which bounds the narrow layers (ncu l1tex 60-86 %)
-    // (bit 3: the activated planes of a MAP_CONVT1D layer through a 5-D map [C, phase, q, image, plane] - output row
+    // (e.tma_out: the activated planes of a MAP_CONVT1D layer through a 5-D map [C, phase, q, image, plane] - output row
     // stride * q + phase - the 32 rows of a warp are one box per column chunk)
-    const int tma_out = (map == MAP_PLAIN) ? (e.tma_out & 7) : (map == MAP_CONVT1D ? (e.tma_out & 8) : 0);
+    const bool convt1d_tma = map == MAP_CONVT1D && e.tma_out != 0;
     bool st_pending = false;             // a TMA store of this warp may still be reading its staging tile (warp-uniform)
     auto stg_release = [&]() {
       if (st_pending) {
@@ -279,14 +269,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         st_pending = false;
       }
     };
-    // Residual by TMA (P.resid_tma): lane 0 asks the copy engine for the warp's next [32 rows x 32 columns] residual tiles (fp32,
-    // or the hi and lo planes) while earlier chunks are processed; the threads read their own rows from the swizzled tile.
-    // No LDG, no STS for the residual - the other half of the epilogue's LSU traffic (see tma_out above).  The requests run
-    // P.resid_tma (1 or 2) chunks ahead ACROSS tiles: a warp's chunk sequence is known up front (persistent tile loop), and a
-    // request issued only at the start of its own tile exposes one HBM round trip per tile (ncu on voc.res2.*.b: 4.8 us per
-    // 2-chunk tile, every unit below 62 %).
-    const int resid_ring = (map == MAP_PLAIN) ? P.resid_tma : 0;
-    const bool resid_tma = resid_ring != 0;
+    // Residual by TMA (MAP_PLAIN layers only): lane 0 asks the copy engine for the warp's next [32 rows x 32 columns] residual
+    // tiles (fp32, or the hi and lo planes) while earlier chunks are processed; the threads read their own rows from the swizzled
+    // tile.  No LDG, no STS for the residual - the other half of the epilogue's LSU traffic (see the TMA stores above).  The
+    // requests run P.resid_tma (1 or 2) chunks ahead ACROSS tiles: a warp's chunk sequence is known up front (persistent tile
+    // loop), and a request issued only at the start of its own tile exposes one HBM round trip per tile (ncu on voc.res2.*.b:
+    // 4.8 us per 2-chunk tile, every unit below 62 %).
+    const int resid_ring = P.resid_tma;
     uint8_t* rstg = rstg_base + (size_t)ew * resid_ring * 4096;
     uint64_t* rbar = resid_bar + ew * 2;
     uint32_t r_cons = 0, r_issued = 0;       // chunks consumed / requested by this warp
@@ -305,7 +294,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       pf_j += CHUNK_STEP;
       if (pf_j >= BN / 32) { pf_j = half; pf_tile += gridDim.x; }
     };
-    if (resid_tma && half < BN / 32)
+    if (half < BN / 32)
       for (int i = 0; i < resid_ring; ++i) issue_resid();
     int prev_n0 = -1, s = 0;            // operand ring slot and its phase bit (the same sequence the producer walks)
     uint32_t ph = 0;
@@ -336,22 +325,18 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       float head_acc = 0.f;
       int cth = 0, ctw = 0;
       uint32_t orow = 0, flags = 0;
-      // MAP_PLAIN (everything but the transposed convs): output rows follow the GEMM rows, so the lanes that store
-      // row rr of this warp need no exchange: row = obase + rr, valid iff rr < lim.
-      const int lim = rows_in - wrow0;
-      const uint32_t obase = (uint32_t)((size_t)img * e.out_img_rows + e.out_row0 + wrow0);
+      // MAP_PLAIN (everything but the transposed convs): output rows follow the GEMM rows, and the TMA stores clip the rows
+      // past rows_in; only the pad flag is needed
       if (map == MAP_PLAIN) {
-        if (row_ok) {
-          orow = obase + lane;
-          flags = kRowValid | (((Wp > 0 && (r % Wp) == Wp - 1) || r >= valid_rows(e.row_valid, img)) ? kRowPad : 0);
-        }
+        if (row_ok) flags = kRowValid | (((Wp > 0 && (r % Wp) == Wp - 1) || r >= valid_rows(e.row_valid, img)) ? kRowPad : 0);
       } else if (map == MAP_CONVT2D) {
         cth = r / Wp;
         ctw = r - cth * Wp;
       }
-      // store this warp's staged 32 rows x 32 columns of fp16 (hi [+ lo]) row-major: 8 rows x 64 B per instruction
+      // store this warp's staged 32 rows x 32 columns of fp16 (hi [+ lo]): by TMA through the map `tm` of a MAP_PLAIN output,
+      // else row-major to the rows published in `rows`, 8 rows x 64 B per instruction
       auto store_rows_h = [&](const OutPlane& op, const int co0, const bool two, const CUtensorMap* tm) {
-        if (tm) {                         // staged tile(s) -> TMA store; rows past rows_in are clipped by the tensor map
+        if (map == MAP_PLAIN) {           // staged tile(s) -> TMA store; rows past rows_in are clipped by the tensor map
           fence_proxy_async();
           __syncwarp();
           if (lane == 0) {
@@ -359,17 +344,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
             tma_store_commit();
           }
           st_pending = true;
-        } else if (map == MAP_PLAIN) {
-          const size_t o0 = (size_t)(obase + h_row) * op.ld + op.c_off + co0;   // one wide multiply per chunk
-          uint4* ph = reinterpret_cast<uint4*>(op.hi + o0) + h_c16;
-          uint4* pl = reinterpret_cast<uint4*>(op.lo + o0) + h_c16;
-          const int step = op.ld;       // 8 rows further, in 16-byte units
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-            if (8 * i + h_row < lim) {
-              ph[i * step] = stg_h[SR_H(i)];
-              if (two) pl[i * step] = stg_l[SR_H(i)];
-            }
         } else {
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
@@ -382,27 +356,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           }
         }
       };
-
-      // Residual planes of the NEXT column chunk are fetched into registers while the current one is processed
-      // (1-term kernels with a register budget for it): an epilogue warp otherwise has one exposed global-load
-      // round trip per chunk, which bounded voc.res*.b (ncu: 31 % of all samples on the first STS after the loads).
-      uint4 pre_h[4], pre_l[4];
-      auto load_resid = [&](const int j) {     // MAP_PLAIN only (the residual stream follows the GEMM rows)
-        const size_t rbase = ((size_t)img * rows_in + wrow0 + h_row) * e.resid_ld + n0 + j * 32;
-        const uint4* gh = reinterpret_cast<const uint4*>(e.resid_hi + rbase) + h_c16;
-        const uint4* gl = reinterpret_cast<const uint4*>(e.resid_lo + rbase) + h_c16;
-        const int step = e.resid_ld;     // 8 rows further, in 16-byte units
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          pre_h[i] = make_uint4(0, 0, 0, 0);
-          pre_l[i] = make_uint4(0, 0, 0, 0);
-          if (8 * i + h_row < lim) {
-            pre_h[i] = __ldg(gh + i * step);
-            pre_l[i] = __ldg(gl + i * step);
-          }
-        }
-      };
-      if (!resid_tma && PREFETCH && has_resid_planes) load_resid(half);
 
       // One 32-column chunk of this thread's row: bias, residual, outputs (see gemm.cuh for the semantics).
       auto process_chunk = [&](const int j, float (&v)[32]) {
@@ -442,7 +395,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
             v[4 * i] += b4.x; v[4 * i + 1] += b4.y; v[4 * i + 2] += b4.z; v[4 * i + 3] += b4.w;
           }
         }
-        if (THREE && has_resid && resid_tma) {      // the tile was requested one chunk ago (or at the start of the tile)
+        if (THREE && has_resid) {         // the tile was requested one chunk ago (or at the start of the tile)
           const uint32_t slot = r_cons & (uint32_t)(resid_ring - 1);
           if (ok && !mbar_wait(rbar + slot, (r_cons >> (resid_ring >> 1)) & 1u, e.err, ERR_PIPE_EPILOGUE)) ok = false;
           ++r_cons;
@@ -454,26 +407,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           }
           __syncwarp();                   // every lane has read the tile: it may be refilled
           issue_resid();                  // the slot just read is free again: request the chunk `resid_ring` ahead
-        } else if (THREE && has_resid) {         // coalesced global -> staging -> own row (MAP_PLAIN only; fp32 streams exist in 3-term mode only)
-          const size_t rbase = ((size_t)img * rows_in + m0 + q * 32) * e.resid_ld + co0;
-          stg_release();
-          __syncwarp();
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rr = 4 * i + f_row;
-            float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (m0 + q * 32 + rr < rows_in)
-              x = __ldg(reinterpret_cast<const float4*>(e.resid + rbase + (size_t)rr * e.resid_ld) + f_c16);
-            stg_f[SR_F(i)] = x;
-          }
-          __syncwarp();
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 x = stg_f[SO_F(i)];
-            v[4 * i] += x.x; v[4 * i + 1] += x.y; v[4 * i + 2] += x.z; v[4 * i + 3] += x.w;
-          }
         }
-        if (has_resid_planes && resid_tma) {
+        if (has_resid_planes) {
           const uint32_t slot = r_cons & (uint32_t)(resid_ring - 1);
           if (ok && !mbar_wait(rbar + slot, (r_cons >> (resid_ring >> 1)) & 1u, e.err, ERR_PIPE_EPILOGUE)) ok = false;
           ++r_cons;
@@ -490,76 +425,24 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           }
           __syncwarp();
           issue_resid();                  // the slot just read is free again: request the chunk `resid_ring` ahead
-        } else if (has_resid_planes) {           // residual stream kept as hi/lo planes: coalesced load, sum in fp32
-          stg_release();
-          __syncwarp();
-          if (PREFETCH) {                 // loaded one chunk ahead (see load_resid below): no exposed load latency
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              stg_h[SR_H(i)] = pre_h[i];
-              stg_l[SR_H(i)] = pre_l[i];
-            }
-            if (j + CHUNK_STEP < BN / 32) load_resid(j + CHUNK_STEP);
-          } else {
-            const size_t rbase = ((size_t)img * rows_in + wrow0) * e.resid_ld + co0;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int rr = 8 * i + h_row;
-              uint4 xh = make_uint4(0, 0, 0, 0), xl = make_uint4(0, 0, 0, 0);
-              if (rr < lim) {
-                xh = __ldg(reinterpret_cast<const uint4*>(e.resid_hi + rbase + (size_t)rr * e.resid_ld) + h_c16);
-                xl = __ldg(reinterpret_cast<const uint4*>(e.resid_lo + rbase + (size_t)rr * e.resid_ld) + h_c16);
-              }
-              stg_h[SR_H(i)] = xh;
-              stg_l[SR_H(i)] = xl;
-            }
-          }
-          __syncwarp();
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const uint4 xh = stg_h[SO_H(i)], xl = stg_l[SO_H(i)];
-            const __half2* ph = reinterpret_cast<const __half2*>(&xh);
-            const __half2* pl = reinterpret_cast<const __half2*>(&xl);
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              add_planes(v[8 * i + 2 * k], v[8 * i + 2 * k + 1], reinterpret_cast<const uint32_t*>(ph)[k], reinterpret_cast<const uint32_t*>(pl)[k], resid_ar);
-          }
         }
         const bool pad = (flags & kRowPad) != 0;
         if (pad) {
 #pragma unroll
           for (int i = 0; i < 32; ++i) v[i] = 0.f;
         }
-        if (THREE && want_raw) {          // fp32 output
+        if (THREE && want_raw) {          // fp32 output (MAP_PLAIN layers only)
           stg_release();
           __syncwarp();
 #pragma unroll
           for (int i = 0; i < 8; ++i) stg_f[SO_F(i)] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-          if (tma_out & 1) {
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) {
-              tma_store_3d(&P.o_raw, stg_f, co0, e.out_row0 + wrow0, img);
-              tma_store_commit();
-            }
-            st_pending = true;
-          } else {
+          fence_proxy_async();
           __syncwarp();
-          if (map == MAP_PLAIN) {
-            float4* pr4 = reinterpret_cast<float4*>(e.out_raw + (size_t)(obase + f_row) * e.raw_ld + co0) + f_c16;
-            const int step = e.raw_ld;    // 4 rows further, in 16-byte units
-#pragma unroll
-            for (int i = 0; i < 8; ++i)
-              if (4 * i + f_row < lim) pr4[i * step] = stg_f[SR_F(i)];
-          } else {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const RowInfo ri = rows[4 * i + f_row];
-              if (ri.flags & kRowValid)
-                reinterpret_cast<float4*>(e.out_raw + (size_t)ri.orow * e.raw_ld + co0)[f_c16] = stg_f[SR_F(i)];
-            }
+          if (lane == 0) {
+            tma_store_3d(&P.o_raw, stg_f, co0, e.out_row0 + wrow0, img);
+            tma_store_commit();
           }
-          }
+          st_pending = true;
         }
         if (want_r) {                     // raw hi/lo planes
           stg_release();
@@ -572,7 +455,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
             stg_l[SO_H(i)] = l;
           }
           __syncwarp();
-          store_rows_h(e.out_r, co0, true, (tma_out & 2) ? &P.o_r : nullptr);
+          store_rows_h(e.out_r, co0, true, &P.o_r);
         }
         if (has_head) {                   // fused 1x1 head (N == 32)
 #pragma unroll
@@ -637,7 +520,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           // A TMA store box may not START at a negative coordinate (boxes that
           // run past the upper bound are clipped as documented): the one warp per image and early phase whose first output row
           // would be q = -1 keeps the LDS + STG path.
-          if ((tma_out & 8) && !(wrow0 == 0 && nb / cout < e.ct_pad)) {      // t = stride * r + phase - pad = stride * (r - up) + (phase - pad + up * stride)
+          if (convt1d_tma && !(wrow0 == 0 && nb / cout < e.ct_pad)) {      // t = stride * r + phase - pad = stride * (r - up) + (phase - pad + up * stride)
             fence_proxy_async();
             __syncwarp();
             if (lane == 0) {
@@ -648,7 +531,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
             }
             st_pending = true;
           } else {
-            store_rows_h(e.out_a, co0, THREE || out_ar, (tma_out & 4) ? &P.o_a : nullptr);
+            store_rows_h(e.out_a, co0, THREE || out_ar, &P.o_a);
           }
         }
       };
@@ -669,7 +552,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           }
           if (ok && !mbar_wait(full_bar + s, ph, e.err, ERR_PIPE_EPILOGUE)) ok = false;
           const uint32_t da_hi = make_smem_desc_lo(smem_u32(smem + (size_t)s * stage_bytes + wg * 64 * ROW_BYTES));
-          const uint32_t da_lo = da_hi + (uint32_t)(a_slot >> 4);
+          const uint32_t da_lo = da_hi + (uint32_t)(A_BOX_BYTES >> 4);
           const uint32_t db = make_smem_desc_lo(smem_u32(smem + (size_t)s * stage_bytes + off_b));     // spans [B_hi; B_lo]
           wgmma_fence_regs(acc, ACC_N / 2);
           if (THREE) wgmma_fence_regs(acc2, BN / 2);
@@ -742,23 +625,22 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       }
       if (THREE && half == 0) epilogue_head(e, img, r, head_acc);
     }
-    if (tma_out && lane == 0) tma_store_wait_all();      // this thread's bulk stores have completed before the CTA exits
+    if ((map == MAP_PLAIN || convt1d_tma) && lane == 0) tma_store_wait_all();      // this thread's bulk stores have completed before the CTA exits
     // NaN compares false against everything, inf exceeds the bound
     if (!(amax <= 65504.f) && e.err) atomicCAS(e.err, 0, ERR_FP16_OVERFLOW);
   }
 }
 
 // ---------------------------------------------------------------------------------------------- host side
-size_t gemm_tc_smem_bytes(int bn, int bk, int stages, int planes_a, int terms, int a_box_rows, int gmax, int tile_chunks, int resid_tma) {
-  const size_t a_slot = ((size_t)a_box_rows * bk * 2 + 1023) & ~(size_t)1023;
-  const size_t stage = planes_a * a_slot + (size_t)gmax * (terms == 3 ? 2 : 1) * bn * bk * 2;
+size_t gemm_tc_smem_bytes(int bn, int bk, int stages, int planes_a, int terms, int tile_chunks, int resid_tma) {
+  const size_t stage = (size_t)planes_a * GEMM_BM * bk * 2 + (size_t)(terms == 3 ? 2 : 1) * bn * bk * 2;
   return stages * stage + EPI_WARPS * 4096 * (1 + resid_tma) + (2 * stages + 16) * 8 + (3 * bn + 32) * 4 + EPI_WARPS * 32 * 8 +
          (size_t)tile_chunks * 16 + 1024;
 }
 
 template <int BN, int BK, bool THREE>
 static cudaError_t launch_cfg(const GemmTcParams& p, cudaStream_t stream) {
-  const size_t smem = gemm_tc_smem_bytes(BN, BK, p.stages, p.planes_a, p.prob.terms, p.a_box_rows, p.gmax, p.tile_chunks, p.resid_tma);
+  const size_t smem = gemm_tc_smem_bytes(BN, BK, p.stages, p.planes_a, p.prob.terms, p.tile_chunks, p.resid_tma);
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BN, BK, THREE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
@@ -773,7 +655,6 @@ static cudaError_t launch_cfg(const GemmTcParams& p, cudaStream_t stream) {
 template <int BK>
 static cudaError_t launch_bk(const GemmTcParams& p, int bn, cudaStream_t stream) {
   const bool three = p.prob.terms == 3;
-  if (p.gmax != 1) return cudaErrorInvalidValue;
   if (bn == 128) return three ? cudaErrorInvalidValue : launch_cfg<128, BK, false>(p, stream);
   if (bn == 64) return three ? launch_cfg<64, BK, true>(p, stream) : launch_cfg<64, BK, false>(p, stream);
   if (bn == 32) return three ? launch_cfg<32, BK, true>(p, stream) : launch_cfg<32, BK, false>(p, stream);

@@ -1,7 +1,6 @@
 // Weight ingestion: the state dict's fp32 tensors become packed fp16 hi/lo GEMM operands, folded BatchNorm affines and
 // the small tables the kernels read, uploaded once per context.
 #include <cmath>
-#include <cstdlib>
 
 #include "engine.h"
 
@@ -41,13 +40,6 @@ int upload_gemm(vf_ctx* ctx, GemmW* w, const std::vector<float>& m, int N, int K
   w->lo = w->hi + m.size();
   if (bias) return upload(ctx, &w->bias, *bias);
   return VF_OK;
-}
-
-// Residual add of a vocoder stack as an identity tap (through the accumulator, no epilogue loads) up to this channel count;
-// above it the epilogue adds the hi/lo planes.  VF_TUNE_IDENT_MAXC overrides (read at weight-load AND plan-build time).
-int ident_max_c() {
-  if (const char* ov = getenv("VF_TUNE_IDENT_MAXC")) return atoi(ov);
-  return 128;
 }
 
 int build_tables(vf_ctx* ctx) {
@@ -253,7 +245,7 @@ int load_vocoder(vf_ctx* ctx) {
       const std::string p = "vocoder.res." + std::to_string(s) + "." + std::to_string(i);
       NEED(wa, p + ".a.weight"); NEED(ba, p + ".a.bias"); NEED(wb, p + ".b.weight"); NEED(bb, p + ".b.bias");
       rc = pack_conv1d(ctx, &ctx->voc_res_a[s][i], *wa, *ba); if (rc) return rc;
-      rc = pack_conv1d(ctx, &ctx->voc_res_b[s][i], *wb, *bb, (int)wb->shape[0] <= ident_max_c()); if (rc) return rc;
+      rc = pack_conv1d(ctx, &ctx->voc_res_b[s][i], *wb, *bb, (int)wb->shape[0] <= IDENT_MAX_C); if (rc) return rc;
     }
   }
   {

@@ -97,7 +97,7 @@ __global__ void __launch_bounds__(PAIR_THREADS, 1) pair_tc_kernel(const __grid_c
       int jl = 0;                              // tiles loaded: the parity of the A slots (empty tiles load nothing)
       for (int j = 0; j < n_local; ++j) {
         const int tile = blockIdx.x + j * gridDim.x;
-        const int img = (int)fast_div_pair((uint32_t)tile, (uint32_t)P.tiles_per_img, P.magic_t);
+        const int img = (int)fast_div((uint32_t)tile, (uint32_t)P.tiles_per_img, P.magic_t);
         const int m0 = (tile - img * P.tiles_per_img) * PAIR_ROWS - 1;
         if (m0 + 1 >= valid_rows(P.row_valid, img)) continue;
         bool ok = true;
@@ -116,7 +116,7 @@ __global__ void __launch_bounds__(PAIR_THREADS, 1) pair_tc_kernel(const __grid_c
     if (elect_one()) {
       auto load_x = [&](int jj, int st) {       // rows t0 .. t0+125 (rows past the clip are zero filled, and clipped on the way out)
         const int tile = blockIdx.x + jj * gridDim.x;
-        const int img = (int)fast_div_pair((uint32_t)tile, (uint32_t)P.tiles_per_img, P.magic_t);
+        const int img = (int)fast_div((uint32_t)tile, (uint32_t)P.tiles_per_img, P.magic_t);
         const int t0 = (tile - img * P.tiles_per_img) * PAIR_ROWS;
         uint8_t* xs = x_base + st * 2 * PAIR_TILE;
         if (t0 >= valid_rows(P.row_valid, img)) { mbar_expect_tx(x_full + st, 0); return; }   // empty tile: E2 reads no residual
@@ -128,7 +128,7 @@ __global__ void __launch_bounds__(PAIR_THREADS, 1) pair_tc_kernel(const __grid_c
       for (int j = 0; j < n_local; ++j) {
         const int s = j % PAIR_X_STAGES;
         const int tile = blockIdx.x + j * gridDim.x;
-        const int img = (int)fast_div_pair((uint32_t)tile, (uint32_t)P.tiles_per_img, P.magic_t);
+        const int img = (int)fast_div((uint32_t)tile, (uint32_t)P.tiles_per_img, P.magic_t);
         const int t0 = (tile - img * P.tiles_per_img) * PAIR_ROWS;
         if (!mbar_wait(out_ready + s, (j / PAIR_X_STAGES) & 1, P.err, ERR_PIPE_EPILOGUE)) break;
         if (P.ar_out) tma_store_3d(&P.xo_map, x_base + s * 2 * PAIR_TILE + PAIR_TILE, 0, t0, img);   // correction plane, in place
@@ -156,7 +156,7 @@ __global__ void __launch_bounds__(PAIR_THREADS, 1) pair_tc_kernel(const __grid_c
     int jl = 0;                                // tiles computed (the producer's count of loaded tiles)
     for (int j = 0; j < n_local; ++j) {
       const int tile = blockIdx.x + j * gridDim.x;
-      const int img = (int)fast_div_pair((uint32_t)tile, (uint32_t)P.tiles_per_img, P.magic_t);
+      const int img = (int)fast_div((uint32_t)tile, (uint32_t)P.tiles_per_img, P.magic_t);
       const int m0 = (tile - img * P.tiles_per_img) * PAIR_ROWS - 1;
       const int L = min(P.L, valid_rows(P.row_valid, img));   // rows of this clip; a varlen plan zeroes the rest
       const bool empty = m0 + 1 >= L;          // no valid row: no loads, no MMAs, E2 stores zeros

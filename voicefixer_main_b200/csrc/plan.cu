@@ -80,12 +80,14 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
   if (rc) return;
   Op op;
   op.kind = OP_GEMM;
+  // K chunk width: 64 wherever the taps allow it.  Every chunk costs the two single-thread issue loops a fixed ~0.5 us
+  // round (barrier wait, TMA / MMA operand set-up), so wide chunks win even where narrow ones would allow one more
+  // co-resident CTA (measured: voc.res3.a 1.43 -> 0.96 ms)
   int bk = 64;
   for (auto& t : taps)
     if (t.nch % 64) bk = 32;
   // a short tail segment (the 32-channel shortcut of a 64-channel conv) may be zero-padded to BK = 64 when
   // the source has exactly that many channels: the TMA box then runs out of bounds and is zero-filled.
-  bool promoted = false;
   if (bk == 32) {
     bool main64 = true, padok = true;
     for (auto& t : taps) {
@@ -95,16 +97,7 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
         if (&t != &taps.back()) main64 = false;
       }
     }
-    if (main64 && padok && taps.size() > 1) { bk = 64; promoted = true; }
-  }
-  // K chunk width: every chunk costs the two single-thread issue loops a fixed ~0.5 us round (barrier wait, TMA /
-  // MMA operand set-up), so wide chunks win even where narrow ones would allow one more co-resident CTA
-  if (bk == 64 && !promoted) {
-    int ksum = 0;
-    for (auto& t : taps) ksum += t.nch;
-    int maxk = 0;   // measured: halving the chunk count beats the extra co-resident CTA (voc.res3.a 1.43 -> 0.96 ms)
-    if (const char* ov = getenv("VF_TUNE_BK32_MAXK")) maxk = atoi(ov);
-    if (ksum <= maxk) bk = 32;
+    if (main64 && padok && taps.size() > 1) bk = 64;
   }
   const int N = W.N;
   // widest N tile the register-resident accumulator allows (gemm_tc.cu): 128 hi-only, 64 in 3-term mode
@@ -115,23 +108,13 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
     rc = fail(ctx, VF_EINVAL, "1-term GEMM with an affine / head / fp32 stream epilogue (3-term kernels only)");
     return;
   }
-  // epilogue residual by TMA (gemm_tc.cu): one or two more 4 KB tiles per epilogue warp, requested that many chunks ahead;
-  // VF_TUNE_TMA_RESID=0 keeps LDG + staging, =1 pins one tile in flight (default: two where the operand ring keeps its depth)
-  const char* renv = getenv("VF_TUNE_TMA_RESID");
-  const int resid_want = renv ? std::max(0, std::min(2, atoi(renv))) : 2;
-  const int resid_tma = (resid_want && !ctx->validate_simt && epi.map == MAP_PLAIN &&
-                         ((terms == 3 && epi.resid != nullptr) != (epi.resid_hi != nullptr))) ? 1 : 0;      // exactly one residual source
   int k = 0;
   for (auto& t : taps) {
     t.k_off = k;
     const int padded = round_up(t.nch, bk);
     k += padded;
-    t.g = 1; t.shift[0] = t.shift[1] = t.shift[2] = 0; t.kstride = padded;
     if (ctx->validate_simt == 0) t.nch = padded;
   }
-  // every tap has its own A load of 128 rows starting on a whole swizzle pattern (gemm_tc.cu): no row-shifted tap groups
-  const int gmax = 1;
-  const int a_box_rows = GEMM_BM;
   if (k != W.K && k != W.K - W.k_tail) { rc = fail(ctx, VF_EINVAL, "GEMM K mismatch: taps cover %d, packed weight has %d", k, W.K); return; }
   GemmProblem pr;
   memset(&pr, 0, sizeof pr);
@@ -186,11 +169,8 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
                                                                   // identity tap is a hi pass and a lo pass, gemm_tc.cu)
     // K steps per accumulation chain before promotion: longer chains = fewer promotion drains, shorter ones = less
     // drift of the tensor core's fp32 accumulation (the 3-term UNet carries a 1e-4 log-mel bar).
-    int seg_mmas = 24;
-    if (const char* ov = getenv("VF_TUNE_SEG_MMAS")) seg_mmas = std::max(4, atoi(ov));
-    tp.seg_chunks = std::max(1, seg_mmas / ((bk / 16) * gmax));
-    tp.a_box_rows = a_box_rows;
-    tp.gmax = gmax;
+    const int seg_mmas = 24;
+    tp.seg_chunks = std::max(1, seg_mmas / (bk / 16));
     tp.planes_a = terms == 3 ? 2 : 1;
     // occupancy: small-K tiles are bound by loads/stores -> several persistent CTAs per SM; large-K -> one
     // one persistent CTA of 384 threads per SM (the accumulators take the register file): the deepest operand ring that fits
@@ -198,51 +178,55 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
     auto fit = [&](int ring) {
       int st = 8;
       for (; st >= 2; --st)
-        if (gemm_tc_smem_bytes(bn, bk, st, tp.planes_a, terms, a_box_rows, gmax, tp.tile_chunks, ring) <= smem_cap) break;
+        if (gemm_tc_smem_bytes(bn, bk, st, tp.planes_a, terms, tp.tile_chunks, ring) <= smem_cap) break;
       return st;
     };
-    tp.resid_tma = resid_tma;
+    // The residual and the fp32 output follow the GEMM rows, which only MAP_PLAIN layers store in order (gemm_tc.cu).
+    GemmEpilogue& pe = pr.epi;
+    const bool has_resid = pe.resid || pe.resid_hi;
+    if (pe.map != MAP_PLAIN && (has_resid || pe.out_raw)) {
+      rc = fail(ctx, VF_EINVAL, "GEMM residual or fp32 output on a transposed conv (MAP_PLAIN layers only)");
+      return;
+    }
+    if (pe.resid && pe.resid_hi) { rc = fail(ctx, VF_EINVAL, "GEMM with both an fp32 and a hi/lo residual"); return; }
+    // The epilogue reads its residual by TMA, one or two 4 KB tiles per epilogue warp requested that many chunks ahead:
+    // two where the operand ring keeps its depth.
+    tp.resid_tma = has_resid ? 1 : 0;
     int stages = fit(tp.resid_tma);
-    if (tp.resid_tma == 1 && resid_want == 2) {      // a second residual tile in flight if the operand ring stays deep enough
+    if (tp.resid_tma) {
       const int st2 = fit(2);
       if (st2 >= 2 && (st2 == stages || st2 >= 4)) { tp.resid_tma = 2; stages = st2; }
     }
     if (stages < 2) { rc = fail(ctx, VF_EINVAL, "no wgmma tile configuration fits (bn=%d bk=%d terms=%d)", bn, bk, terms); return; }
     tp.stages = stages;
-    // MAP_PLAIN outputs leave the epilogue's staging tiles by TMA store (gemm_tc.cu); VF_TUNE_TMA_STORE=0 keeps LDS + STG
-    {
-      const char* tenv = getenv("VF_TUNE_TMA_STORE");
-      const int want = tenv ? atoi(tenv) : 7;
-      GemmEpilogue& pe = pr.epi;
+    if (tp.resid_tma) {
+      if (pe.resid) rc = map_rows(ctx, &tp.i_res, pe.resid, 4, pe.resid_ld, pe.rows_in, (size_t)pe.rows_in, n_img, 32, 32);
+      else rc = map_out_planes(ctx, &tp.i_res, pe.resid_hi, pe.resid_lo, 2, pe.resid_ld, pe.rows_in, (size_t)pe.rows_in, n_img);
+      if (rc) return;
+    }
+    // Every MAP_PLAIN output leaves the epilogue's staging tiles by TMA store (gemm_tc.cu), and so does the activated output
+    // of a transposed 1-D conv that fills its output rows exactly; the other transposed-conv outputs are scattered by STG.
+    pe.tma_out = 0;
+    if (pe.map == MAP_CONVT1D && pe.out_a.hi && !pe.out_r.hi && pe.out_row0 == 0 &&
+        pe.out_rows_valid == pe.out_img_rows && pe.out_img_rows % pe.ct_stride == 0 && pe.out_a.ld % 8 == 0) {
+      rc = map_convt1d_out(ctx, &tp.o_a, pe.out_a.hi, pe.out_a.lo, (terms == 3 || pe.out_ar) ? 2 : 1, pe.out_a.ld, pe.ct_stride, pe.out_img_rows, n_img);
+      if (rc) return;
+      pe.tma_out = 1;
+    }
+    if (pe.map == MAP_PLAIN) {
       const int orows = pe.out_row0 + pe.rows_in;
-      pe.tma_out = 0;
-      if (tp.resid_tma) {
-        if (terms == 3 && pe.resid) rc = map_rows(ctx, &tp.i_res, pe.resid, 4, pe.resid_ld, pe.rows_in, (size_t)pe.rows_in, n_img, 32, 32);
-        else rc = map_out_planes(ctx, &tp.i_res, pe.resid_hi, pe.resid_lo, 2, pe.resid_ld, pe.rows_in, (size_t)pe.rows_in, n_img);
+      if (pe.out_raw) {
+        if (pe.raw_ld % 4) { rc = fail(ctx, VF_EINVAL, "fp32 GEMM output row of %d floats: the TMA store needs 16-byte rows", pe.raw_ld); return; }
+        rc = map_rows(ctx, &tp.o_raw, pe.out_raw, 4, pe.raw_ld, orows, (size_t)pe.out_img_rows, n_img, 32, 32);
         if (rc) return;
       }
-      if (pe.map == MAP_CONVT1D && (want & 4) && !ctx->validate_simt && pe.out_a.hi && !pe.out_r.hi && !pe.out_raw && pe.out_row0 == 0 &&
-          pe.out_rows_valid == pe.out_img_rows && pe.out_img_rows % pe.ct_stride == 0 && pe.out_a.ld % 8 == 0) {
-        rc = map_convt1d_out(ctx, &tp.o_a, pe.out_a.hi, pe.out_a.lo, (terms == 3 || pe.out_ar) ? 2 : 1, pe.out_a.ld, pe.ct_stride, pe.out_img_rows, n_img);
+      if (pe.out_r.hi) {
+        rc = map_out_planes(ctx, &tp.o_r, pe.out_r.hi, pe.out_r.lo, 2, pe.out_r.ld, orows, (size_t)pe.out_img_rows, n_img);
         if (rc) return;
-        pe.tma_out |= 8;
       }
-      if (pe.map == MAP_PLAIN && want) {
-        if ((want & 1) && terms == 3 && pe.out_raw && pe.raw_ld % 4 == 0) {
-          rc = map_rows(ctx, &tp.o_raw, pe.out_raw, 4, pe.raw_ld, orows, (size_t)pe.out_img_rows, n_img, 32, 32);
-          if (rc) return;
-          pe.tma_out |= 1;
-        }
-        if ((want & 2) && pe.out_r.hi) {
-          rc = map_out_planes(ctx, &tp.o_r, pe.out_r.hi, pe.out_r.lo, 2, pe.out_r.ld, orows, (size_t)pe.out_img_rows, n_img);
-          if (rc) return;
-          pe.tma_out |= 2;
-        }
-        if ((want & 4) && pe.out_a.hi) {
-          rc = map_out_planes(ctx, &tp.o_a, pe.out_a.hi, pe.out_a.lo, (terms == 3 || pe.out_ar) ? 2 : 1, pe.out_a.ld, orows, (size_t)pe.out_img_rows, n_img);
-          if (rc) return;
-          pe.tma_out |= 4;
-        }
+      if (pe.out_a.hi) {
+        rc = map_out_planes(ctx, &tp.o_a, pe.out_a.hi, pe.out_a.lo, (terms == 3 || pe.out_ar) ? 2 : 1, pe.out_a.ld, orows, (size_t)pe.out_img_rows, n_img);
+        if (rc) return;
       }
     }
     const long total_tiles = (long)n_img * pr.m_tiles * (N / bn);
@@ -253,7 +237,7 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
   }
   {   // algorithmic work: the reference op's own MAC count and the minimum HBM traffic of this launch
     double kreal = 0;
-    for (auto& t : taps) if (!t.both) kreal += (double)t.g * std::min(t.nch, (t.src ? s1 : &s0)->pl.C);
+    for (auto& t : taps) if (!t.both) kreal += (double)std::min(t.nch, (t.src ? s1 : &s0)->pl.C);
     const double wfrac = (epi.Wp > 1) ? double(epi.Wp - 1) / epi.Wp : 1.0;
     double rows = (double)n_img * (epi.map == MAP_CONVT1D ? epi.rows_in - 1 : epi.rows_in) * wfrac;
     op.flops = 2.0 * rows * N * kreal * (epi.map == MAP_CONVT2D ? 9.0 / 16.0 : 1.0);
@@ -264,7 +248,7 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
     double a_bytes = (double)n_img * s0.rows * s0.pl.C * (terms == 3 ? 4 : 2);
     if (s1) a_bytes += (double)n_img * s1->rows * s1->pl.C * ((terms == 3 || s1_both) ? 4 : 2);
     double kexec = 0;
-    for (auto& t : taps) kexec += (double)t.g * round_up(t.nch, bk) * (terms == 3 ? 3 : (t.both ? 2 : 1));
+    for (auto& t : taps) kexec += (double)round_up(t.nch, bk) * (terms == 3 ? 3 : (t.both ? 2 : 1));
     op.exec_flops = 2.0 * (double)n_img * pr.m_tiles * GEMM_BM * N * kexec;
     const double out_elems = (double)n_img * (epi.map == MAP_CONVT1D ? (double)epi.out_rows_valid * epi.cout
                                               : (epi.map == MAP_CONVT2D ? 4.0 * epi.rows_in * epi.cout : (double)epi.rows_in * N));
@@ -570,9 +554,9 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
     const bool last_stage = s == c.voc_num_stages - 1;
     // (a, r) residual stream of the hi-only mode (gemm.cuh): x lives in the activated plane the convs read anyway plus one
     // fp16 correction plane (the otherwise unused lo plane of the same allocation), updated in place by every residual layer:
-    // 10 instead of 12 bytes per element through a residual pair.  VF_TUNE_AR_STREAM=0 keeps separate hi/lo planes of x.
-    const char* aenv = getenv("VF_TUNE_AR_STREAM");
-    const uint32_t ar = (!(aenv && atoi(aenv) == 0) && !ctx->validate_simt && terms == 1) ? ar_inv_word(c.voc_res_slope) : 0u;
+    // 10 instead of 12 bytes per element through a residual pair.  A slope with no fp16 inverse (ar_inv_word) keeps separate
+    // hi/lo planes of x.
+    const uint32_t ar = (!ctx->validate_simt && terms == 1) ? ar_inv_word(c.voc_res_slope) : 0u;
     // C = 64 stacks of the hi-only mode with the (a, r) stream: one kernel per residual pair (pair_tc.cu), the intermediate h
     // stays in shared memory; VF_TUNE_FUSED_PAIR=0 selects the two-launch path.  A pair's activated input and output planes
     // must differ (a tile reads rows up to `dil` away from the ones another CTA is writing): the pairs ping-pong between xa and xa2.
@@ -676,7 +660,7 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
           // the "a" conv of the next pair (a later launch) looks at neighbouring rows
           e.resid_hi = xa.p.hi; e.resid_lo = xa.p.lo; e.resid_ld = cout; e.resid_ar = ar;
           b.gemm(ops, ctx->voc_res_b[s][i], ASrc{ha, (int)L, 0}, nullptr, taps, e, B, terms);
-        } else if (cout <= ident_max_c()) {
+        } else if (cout <= IDENT_MAX_C) {
           // load/store-bound stacks: x rides through the accumulator (identity weights, both planes) and the
           // epilogue issues no global loads
           taps.push_back(GemmTap{0, 1, 0, 0, cout, 1});
