@@ -15,6 +15,7 @@
  *   vf_restore / vf_restore_host  one iteration of the segment loop of handler(), eval_gsr_voicefixer.py:49-74:
  *                                 pre -> model -> from_log -> vocoder -> peak normalise -> trim_center
  *   vf_restore_varlen             the same for clips of different lengths in one call (handler() run over a test set)
+ *   vf_restore_varlen_mels        + each clip's stage A / B mels, the inputs of handler()'s metrics (handler_batch)
  *   vf_to_log / vf_from_log       tools/pytorch/pytorch_util.py:157-163
  *   vf_to_pcm16                   the int16 conversion of save_wave, tools/file/wav.py:22-24 (SURVEY.md 8(f) row 3)
  *   vf_mel                        MelScale.forward on any spectrogram, tools/pytorch/mel_scale.py:52-64
@@ -140,6 +141,12 @@ VF_API int vf_restore_ex(vf_ctx* ctx, const float* wav, int batch, int64_t n_sam
  * 256 clips (fewer under the plan budget), each with its own bucket; clips keep their order. */
 VF_API int vf_restore_varlen(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out,
                              unsigned flags, void* stream);
+/* vf_restore_varlen, and in addition: clip i's linear mel (stage A) and restored log10 mel (stage B), T_i = 1 + n_i / hop
+ * frames of 128 bins, written at frame offset F_i = sum_{j<i} T_j of mel_out / log_mel_out ([sum T_i, 128], device,
+ * either may be NULL).  Bit-identical to what vf_restore_stages returns after vf_restore_ex on that clip alone.  Each
+ * sub-batch adds one copy kernel on `stream` (none when both are NULL: the call is then vf_restore_varlen). */
+VF_API int vf_restore_varlen_mels(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out,
+                                  unsigned flags, float* mel_out, float* log_mel_out, void* stream);
 /* The same for the SSR_UNet / GSR_UNet path: clips of different lengths, packed and with HOST offsets as in
  * vf_restore_varlen, no flags.  Clip i's output is bit-identical to vf_ssr_restore on that clip alone (batch 1, same
  * options).  Every clip needs more than 1024 samples and at most 2^30 (no trim_center constraint: there is no vocoder); a

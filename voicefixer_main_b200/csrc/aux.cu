@@ -442,6 +442,20 @@ cudaError_t launch_varlen_setup(const VarlenSetupParams& p, cudaStream_t stream)
   return cudaGetLastError();
 }
 
+// One thread per mel value of the packed outputs; blocks past clip b's frames return.
+__global__ void gather_mels_kernel(const __grid_constant__ MelGatherParams p) {
+  const int b = blockIdx.y;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)(p.frame_off[b + 1] - p.frame_off[b]) * 128) return;
+  const size_t src = (size_t)b * p.T * 128 + i, dst = (size_t)p.frame_off[b] * 128 + i;
+  if (p.mel_out) p.mel_out[dst] = p.mel[src];
+  if (p.logmel_out) p.logmel_out[dst] = p.logmel[src];
+}
+cudaError_t launch_gather_mels(const MelGatherParams& p, cudaStream_t stream) {
+  gather_mels_kernel<<<dim3((unsigned)(((size_t)p.T * 128 + 255) / 256), p.batch), 256, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
 cudaError_t launch_pcm16(const float* in, int16_t* out, size_t n, int saturate, cudaStream_t stream) {
   const unsigned blocks = (unsigned)std::min<size_t>((n + 255) / 256, 148 * 16);
   pcm16_kernel<<<blocks, 256, 0, stream>>>(in, out, n, saturate);

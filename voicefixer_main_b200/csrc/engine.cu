@@ -515,6 +515,41 @@ int run_varlen_sub_batches(vf_ctx* ctx, int kind, const int64_t* offsets, int ba
   }, VL_MAX_CLIPS);
 }
 
+// vf_restore_varlen (`fn`) and vf_restore_varlen_mels.  With mel_out or log_mel_out, each sub-batch's restore is followed by
+// one gather of its clips' rows t < T_i into the packed outputs at frame offsets F_i = sum_{j<i} T_j, still inside the
+// plan's use on `stream` (plan_exit again after it).
+int restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t* offsets, int batch, float* wav_out,
+                   unsigned flags, float* mel_out, float* log_mel_out, cudaStream_t st) {
+  int rc = check_ready(ctx);
+  if (rc) return rc;
+  if (!wav || !wav_out || !offsets || batch <= 0) return fail(ctx, VF_EINVAL, "%s: bad arguments", fn);
+  if (flags & ~(unsigned)VF_RESTORE_UNIFY_ENERGY) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
+  long scale = 1;
+  for (int s = 0; s < ctx->cfg.voc_num_stages; ++s) scale *= ctx->cfg.voc_scales[s];
+  rc = check_varlen_call(ctx, fn, PLAN_VARLEN, offsets, batch, [&](int i, int64_t n) {
+    const int T = frames_of(ctx, (long)n);
+    const long d = (long)(T + T % 2 + ctx->cfg.voc_tail_base) * scale - (long)n;
+    if (d < 0 || d == 1) return fail(ctx, VF_EINVAL, "clip %d: vocoder output length %ld incompatible with input %ld (trim_center)", i, (long)n + d, (long)n);
+    return VF_OK;
+  });
+  if (rc) return rc;
+  const bool mels = mel_out || log_mel_out;
+  std::vector<int64_t> frame_off(mels ? batch + 1 : 0, 0);
+  for (int i = 0; mels && i < batch; ++i) frame_off[i + 1] = frame_off[i] + frames_of(ctx, (long)(offsets[i + 1] - offsets[i]));
+  return run_varlen_sub_batches(ctx, PLAN_VARLEN, offsets, batch, [&](Plan* plan, int s, int b, const int64_t* rel, int64_t n_max) {
+    int r = restore_impl(ctx, plan, wav + offsets[s], b, n_max, wav_out + offsets[s], flags, st, rel);
+    if (r || !mels) return r;
+    MelGatherParams g;
+    memset(&g, 0, sizeof g);
+    g.mel = plan->d_mel; g.logmel = plan->d_logmel_out; g.mel_out = mel_out; g.logmel_out = log_mel_out;
+    g.batch = b; g.T = plan->T;
+    for (int i = 0; i <= b; ++i) g.frame_off[i] = frame_off[s + i];
+    CK(launch_gather_mels(g, st));
+    ctx->launches++;
+    return plan_exit(ctx, plan, st);
+  });
+}
+
 }  // namespace
 
 // =============================================================================================== C ABI
@@ -675,22 +710,13 @@ VF_API int vf_restore_ex(vf_ctx* ctx, const float* wav, int batch, int64_t n, fl
 
 VF_API int vf_restore_varlen(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out, unsigned flags,
                              void* stream) {
-  int rc = check_ready(ctx);
-  if (rc) return rc;
-  if (!wav || !wav_out || !offsets || batch <= 0) return fail(ctx, VF_EINVAL, "vf_restore_varlen: bad arguments");
-  if (flags & ~(unsigned)VF_RESTORE_UNIFY_ENERGY) return fail(ctx, VF_EINVAL, "vf_restore_varlen: unknown flag bits 0x%x", flags);
-  long scale = 1;
-  for (int s = 0; s < ctx->cfg.voc_num_stages; ++s) scale *= ctx->cfg.voc_scales[s];
-  rc = check_varlen_call(ctx, "vf_restore_varlen", PLAN_VARLEN, offsets, batch, [&](int i, int64_t n) {
-    const int T = frames_of(ctx, (long)n);
-    const long d = (long)(T + T % 2 + ctx->cfg.voc_tail_base) * scale - (long)n;
-    if (d < 0 || d == 1) return fail(ctx, VF_EINVAL, "clip %d: vocoder output length %ld incompatible with input %ld (trim_center)", i, (long)n + d, (long)n);
-    return VF_OK;
-  });
-  if (rc) return rc;
-  return run_varlen_sub_batches(ctx, PLAN_VARLEN, offsets, batch, [&](Plan* plan, int s, int b, const int64_t* rel, int64_t n_max) {
-    return restore_impl(ctx, plan, wav + offsets[s], b, n_max, wav_out + offsets[s], flags, (cudaStream_t)stream, rel);
-  });
+  return restore_varlen(ctx, "vf_restore_varlen", wav, offsets, batch, wav_out, flags, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+VF_API int vf_restore_varlen_mels(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out,
+                                  unsigned flags, float* mel_out, float* log_mel_out, void* stream) {
+  return restore_varlen(ctx, "vf_restore_varlen_mels", wav, offsets, batch, wav_out, flags, mel_out, log_mel_out,
+                        (cudaStream_t)stream);
 }
 
 VF_API int vf_restore(vf_ctx* ctx, const float* wav, int batch, int64_t n, float* wav_out, void* stream) {

@@ -46,6 +46,18 @@ struct VarlenSetupParams {
   int* d_rows;                     // [VL_ROWS][batch]
 };
 cudaError_t launch_varlen_setup(const VarlenSetupParams& p, cudaStream_t stream);
+// vf_restore_varlen_mels: rows t < T_b of clip b in a varlen plan's [batch, T, 128] mel buffers (row stride T = the bucket)
+// -> rows [frame_off[b], frame_off[b + 1]) of packed caller buffers (either output may be null).  The frame offsets are a
+// kernel parameter, as the lengths table's sample offsets are.
+struct MelGatherParams {
+  const float* mel;
+  const float* logmel;
+  float* mel_out;
+  float* logmel_out;
+  int batch, T;
+  int64_t frame_off[VL_MAX_CLIPS + 1];
+};
+cudaError_t launch_gather_mels(const MelGatherParams& p, cudaStream_t stream);
 
 struct PlanePtr {
   __half* hi;

@@ -9,12 +9,16 @@ per-segment mel metrics of eval_gsr_voicefixer.py:56-64 are computed on the GPU 
 is a CPU skimage call in the reference, evaluation_proc/metrics.py:97-106, and is not reported).
 The segment loop, from_log, peak normalisation, trim_center, concat and the int16 conversion of
 tools/file/wav.py:22-24 are reproduced exactly; the per-segment stages run as one fused launch chain.
+handler_batch(items, ...) is handler() over a whole list of files, with the same files and dicts, as batched restores.
 """
 import wave
+from fractions import Fraction
 
 import numpy as np
 import torch
 
+from ._lib import VF_EINVAL, EngineError
+from .arch import frames_for
 from .model import VoiceFixer, default_hparams
 
 model = None
@@ -35,13 +39,25 @@ def read_pcm16(path):
 def load_wav(path, sample_rate=44100, engine=None):
     """tools/utils.py:46-48 (librosa.load(path, sr=sample_rate)): decode + convert to `sample_rate`.  Rate conversion
     runs on the GPU (`engine`, edges.resample_to); a file already at the target rate needs no engine."""
-    wav, rate = read_pcm16(path)
+    return _to_rate(path, *read_pcm16(path), sample_rate, engine)
+
+
+def _to_rate(path, wav, rate, sample_rate, engine):
+    """load_wav's conversion of decoded samples `wav` at `rate` to `sample_rate`."""
     if rate == sample_rate:
         return wav
     if engine is None:
         raise ValueError(f"{path}: {rate} Hz input needs an engine for the GPU resampler (pass engine=model._engine())")
     from .edges import resample_to
     return resample_to(engine, torch.from_numpy(wav)[None].to(engine.device), rate, sample_rate)[0].cpu().numpy()
+
+
+def _rate_len(n, rate, sample_rate=44100):
+    """Length of what load_wav returns for n samples at `rate`: resample_poly's ceil(n * up / down)."""
+    if rate == sample_rate:
+        return n
+    fr = Fraction(sample_rate, rate)
+    return (n * fr.numerator + fr.denominator - 1) // fr.denominator
 
 
 def save_wave(frames: np.ndarray, fname, sample_rate=44100):
@@ -85,23 +101,55 @@ def restore_array(mdl: VoiceFixer, wav_10k: np.ndarray, device, unify_energy: bo
         seg = torch.from_numpy(np.ascontiguousarray(segment))[None, :].to(device)
         res.append(mdl.restore(seg, unify_energy=unify_energy))
         if target is not None and metrics is not None:
-            from .edges import AudioMetrics
-            am = AudioMetrics(mdl)
-            eng = mdl._engine()
             tseg = torch.from_numpy(np.ascontiguousarray(target[break_point - SEG_LENGTH:break_point]))[None, None, :].to(device)
-            _, target_mel = mdl.pre(tseg)
-            mel_noisy, log_mel = eng.restore_stages(1, seg.shape[1])
-            log_mel, mel_noisy = log_mel[:, None], mel_noisy[:, None]
-            denoised = eng.from_log(log_mel)
-            if unify_energy:                     # eval_gsr_voicefixer.py:54-55 (tools/utils.py:50-55) before the lsd
-                denoised = eng.amp_to_original_f(denoised[:, 0].contiguous(), mel_noisy[:, 0].contiguous())[:, None]
-            metrics.update({
-                "mel-lsd": float(am.lsd(denoised.contiguous(), target_mel.contiguous())),
-                "mel-sispec": float(am.sispec(log_mel, target_mel.contiguous(), target_map=1)),             # in log scale
-                "mel-non-log-sispec": float(am.sispec(log_mel, target_mel.contiguous(), est_map=2)),
-            })
+            mel_noisy, log_mel = mdl._engine().restore_stages(1, seg.shape[1])
+            metrics.update(_mel_metrics(mdl, tseg, mel_noisy[:, None], log_mel[:, None], unify_energy))
         break_point += SEG_LENGTH
     return torch.cat(res, -1)
+
+
+def _mel_metrics(mdl: VoiceFixer, tseg, mel_noisy, log_mel, unify_energy: bool) -> dict:
+    """eval_gsr_voicefixer.py:56-64 for one segment: tseg [1, 1, n] the clean target on the device, mel_noisy / log_mel
+    [1, 1, T, 128] the restore's linear mel (stage A) and restored log10 mel (stage B)."""
+    from .edges import AudioMetrics
+    am = AudioMetrics(mdl)
+    eng = mdl._engine()
+    _, target_mel = mdl.pre(tseg)
+    denoised = eng.from_log(log_mel)
+    if unify_energy:                     # eval_gsr_voicefixer.py:54-55 (tools/utils.py:50-55) before the lsd
+        denoised = eng.amp_to_original_f(denoised[:, 0].contiguous(), mel_noisy[:, 0].contiguous())[:, None]
+    return {
+        "mel-lsd": float(am.lsd(denoised.contiguous(), target_mel.contiguous())),
+        "mel-sispec": float(am.sispec(log_mel, target_mel.contiguous(), target_map=1)),             # in log scale
+        "mel-non-log-sispec": float(am.sispec(log_mel, target_mel.contiguous(), est_map=2)),
+    }
+
+
+def segment_bounds(n):
+    """(start, end) of the segments restore_array cuts a file of n samples into: SEG_LENGTH each, the last one ragged."""
+    return [(bp - SEG_LENGTH, min(bp, n)) for bp in range(SEG_LENGTH, n + SEG_LENGTH, SEG_LENGTH)]
+
+
+def _check_file(path, n, n_target=None):
+    """Raises what handler() would raise on a file of n samples (at 44.1 kHz) with a target of n_target samples (None: no
+    target), without touching the GPU: nothing to concatenate (RuntimeError); a segment, or the target slice of one, of at
+    most 1024 samples, which the front end's reflect padding rejects (EngineError); a target slice with another frame count
+    than its segment, which the metrics' shape check rejects (AssertionError).  Segments are checked in handler()'s order."""
+    bounds = segment_bounds(n)
+    if not bounds:
+        raise RuntimeError(f"{path}: no samples to restore")
+    for s, e in bounds:
+        if e - s <= 1024:
+            raise EngineError(VF_EINVAL, f"{path}: segment [{s}, {e}) has {e - s} samples; reflect padding needs more than 1024")
+        if n_target is None:
+            continue
+        t = max(0, min(s + SEG_LENGTH, n_target) - s)
+        if t <= 1024:
+            raise EngineError(VF_EINVAL, f"{path}: the target slice of segment [{s}, {e}) has {t} samples; reflect padding "
+                                         f"needs more than 1024")
+        if frames_for(t) != frames_for(e - s):
+            raise AssertionError(f"{path}: the target slice of segment [{s}, {e}) has {frames_for(t)} frames, the segment "
+                                 f"{frames_for(e - s)}")
 
 
 def handler(input, output, target, ckpt, device, needrefresh=False, meta={}):
@@ -119,6 +167,74 @@ def handler(input, output, target, ckpt, device, needrefresh=False, meta={}):
     pcm = model._engine().to_pcm16(out[0], saturate=bool(meta.get("saturate", False)))
     save_pcm16(pcm.cpu().numpy(), fname=output, sample_rate=44100)
     return metrics
+
+
+def handler_batch(items, ckpt, device, needrefresh=False, meta={}):
+    """handler(input, output, target, ckpt, device, needrefresh, meta) for every (input, output, target) of `items`, in
+    order, as one batched restore: returns the list of metrics dicts, and every output file and dict is exactly what
+    handler() gives that item.  The segments of all files go through vf_restore_varlen_mels, longest first so that each
+    sub-batch's bucket fits its clips: one call for the full 60 s segments and one for the others, instead of one restore
+    (and one plan per distinct length) per segment.  Every file is decoded and checked before any GPU work: an item
+    handler() would reject fails the whole call with handler()'s exception class, naming the file, and no file is written.
+    needrefresh reloads the model once.  All segments and their mels are held on the device at once: split a test set too
+    large for that into several calls."""
+    if needrefresh:
+        refresh_model(ckpt)
+    global model
+    model = model.to(device)
+    eng = model._engine()
+    items = [tuple(it) for it in items]
+    if not items:
+        return []
+    decoded = []
+    for inp, _, tgt in items:
+        x = read_pcm16(inp)
+        t = read_pcm16(tgt) if tgt is not None else None
+        _check_file(inp, _rate_len(len(x[0]), x[1]), None if t is None else _rate_len(len(t[0]), t[1]))
+        decoded.append((x, t))
+    sigs = [_to_rate(inp, *x, 44100, eng) for (inp, _, _), (x, _) in zip(items, decoded)]
+    tgts = [None if t is None else _to_rate(tgt, *t, 44100, eng) for (_, _, tgt), (_, t) in zip(items, decoded)]
+    segs = [(f, s, e) for f, x in enumerate(sigs) for s, e in segment_bounds(len(x))]    # (file, start, end), file order
+    unify, want_mels = bool(meta.get("unify_energy", False)), any(t is not None for t in tgts)
+    pcm, mels = [None] * len(segs), [None] * len(segs)   # per segment: int16 samples; (mel, log_mel) [1, 1, T, 128] views
+    # Full 60 s segments get a call of their own.  A call's longest clip sizes all of its sub-batches (plan budget), and a
+    # 60 s segment needs the plan memory of about six 10 s clips: next to short clips it would cap every sub-batch at a few
+    # clips, each sub-batch a plan of its own shape.
+    full = [k for k, (_, s, e) in enumerate(segs) if e - s == SEG_LENGTH]
+    rest = [k for k, (_, s, e) in enumerate(segs) if e - s < SEG_LENGTH]
+    for group in (full, rest):
+        if not group:
+            continue
+        order = sorted(group, key=lambda k: segs[k][1] - segs[k][2])                    # longest first, stable
+        lengths = [segs[k][2] - segs[k][1] for k in order]
+        off = np.concatenate([[0], np.cumsum(lengths)])
+        f_off = np.concatenate([[0], np.cumsum([frames_for(n) for n in lengths])])
+        packed = torch.from_numpy(np.concatenate([sigs[f][s:e] for f, s, e in (segs[k] for k in order)])).to(model.device)
+        mel = torch.empty(int(f_off[-1]), 128, device=model.device) if want_mels else None
+        log_mel = torch.empty_like(mel) if want_mels else None
+        out = eng.restore_varlen(packed, lengths, unify_energy=unify, mel_out=mel, log_mel_out=log_mel)
+        # to_pcm16 is elementwise: one conversion of the packed output gives every file the bytes of its own conversion
+        out16 = eng.to_pcm16(out, saturate=bool(meta.get("saturate", False))).cpu().numpy()
+        for p, k in enumerate(order):
+            pcm[k] = out16[off[p]:off[p + 1]]
+            if want_mels:
+                rows = slice(int(f_off[p]), int(f_off[p + 1]))
+                mels[k] = (mel[rows][None, None], log_mel[rows][None, None])
+    file_segs = [[] for _ in items]
+    for k, (f, _, _) in enumerate(segs):
+        file_segs[f].append(k)
+    results = []
+    for f, tgt in enumerate(tgts):                 # restore_array leaves the metrics of a file's last segment
+        if tgt is None:
+            results.append({})
+            continue
+        k = file_segs[f][-1]
+        s = segs[k][1]
+        tseg = torch.from_numpy(np.ascontiguousarray(tgt[s:s + SEG_LENGTH]))[None, None, :].to(model.device)
+        results.append(_mel_metrics(model, tseg, *mels[k], unify))
+    for (_, output, _), ks in zip(items, file_segs):
+        save_pcm16(np.concatenate([pcm[k] for k in ks]), fname=output, sample_rate=44100)
+    return results
 
 
 # ---- the pip package's entry points (SURVEY.md 8(b): `VoiceFixer.restore(input, output, cuda, mode, your_vocoder_func)` /

@@ -205,14 +205,25 @@ class Engine:
         return out
 
     def restore_varlen(self, wav_packed: torch.Tensor, lengths, out: Optional[torch.Tensor] = None,
-                       unify_energy: bool = False) -> torch.Tensor:
+                       unify_energy: bool = False, mel_out: Optional[torch.Tensor] = None,
+                       log_mel_out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Clips of different lengths in one call (vf_restore_varlen): wav_packed [sum(lengths)] holds the clips back to back;
-        the result is packed the same way, and clip i is bit-identical to restore(clip_i[None])[0]."""
+        the result is packed the same way, and clip i is bit-identical to restore(clip_i[None])[0].
+        mel_out / log_mel_out (vf_restore_varlen_mels), each [sum(frames_for(n_i)), 128] or None: clip i's linear mel and
+        restored log10 mel land in rows sum_{j<i} frames_for(n_j) onwards, the bits restore_stages(1, n_i) gives after
+        restore(clip_i[None])."""
         wav_packed, offsets = self._varlen_args(wav_packed, lengths)
         out = torch.empty_like(wav_packed) if out is None else out
+        rows = sum(frames_for(offsets[i + 1] - offsets[i]) for i in range(len(offsets) - 1))
+        for name, t in (("mel_out", mel_out), ("log_mel_out", log_mel_out)):
+            if t is not None:
+                _check_in(t, self.device, name)
+                if not t.is_contiguous() or tuple(t.shape) != (rows, 128):
+                    raise ValueError(f"{name} must be a contiguous [{rows}, 128] tensor (the clips' frames, packed)")
         flags = L.VF_RESTORE_UNIFY_ENERGY if unify_energy else 0
         with torch.cuda.device(self.device):
-            self._ck(self.lib.vf_restore_varlen(self.ctx, _ptr(wav_packed), offsets, len(offsets) - 1, _ptr(out), flags, _stream()))
+            self._ck(self.lib.vf_restore_varlen_mels(self.ctx, _ptr(wav_packed), offsets, len(offsets) - 1, _ptr(out), flags,
+                                                     _ptr(mel_out), _ptr(log_mel_out), _stream()))
         return out
 
     def _varlen_args(self, wav_packed: torch.Tensor, lengths):
