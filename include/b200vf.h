@@ -29,6 +29,9 @@
  *   vf_resample_poly              load_wav's rate conversion, tools/utils.py:46-48
  *   vf_lsd / vf_sispec            AudioMetrics.lsd / .sispec evaluation_proc/metrics.py:83-95 (handler's mel metrics,
  *                                 eval_gsr_voicefixer.py:56-64)
+ *   vf_metric_spectrogram         AudioMetrics.wav_to_spectrogram metrics.py:37-51 (librosa STFT magnitude + mel) at 44.1 kHz
+ *   vf_ssim                       AudioMetrics.ssim metrics.py:97-106 (scikit-image structural_similarity, win_size 7)
+ *   vf_score_varlen               the spectral part of AudioMetrics.evaluation metrics.py:53-81 for a set of file pairs
  *
  * Conventions: every function returns 0 on success or a negative VF_E* code and never throws; the message is
  * available from vf_last_error().  All tensor arguments are contiguous fp32.  Unless a name ends in `_host`,
@@ -109,7 +112,8 @@ VF_API const char* vf_last_error(vf_ctx* ctx);   /* ctx may be NULL: error of th
  * matrices, mel filterbank to its sparse form).  Synchronous.  "mel.fb" is required; of the three networks -
  * "generator.analysis_module.*" (VoiceFixer's mel UNet; unet.py and unet_small.py share its keys), "vocoder.*",
  * "generator.unet.*" (unet_v2 of SSR_UNet / GSR_UNet) - whichever are present are loaded, and a network that is
- * present must be complete (missing key -> VF_ESTATE).  Entry points that need an absent network fail with VF_ESTATE. */
+ * present must be complete (missing key -> VF_ESTATE).  Entry points that need an absent network fail with VF_ESTATE; "mel.fb"
+ * alone is enough for the front end and for scoring (vf_metric_spectrogram, vf_score_varlen). */
 VF_API int vf_load_weights(vf_ctx* ctx, const vf_tensor_desc* descs, int n);
 
 /* wav [B,N] -> mel_out [B,T,128] linear mel (T = 1 + N/hop); optional sp/cos/sin [B,T,1025] (NULL to skip). */
@@ -208,6 +212,35 @@ VF_API int vf_lsd(vf_ctx* ctx, const float* est, const float* target, int images
  * the batch).  est_map / target_map: 0 none, 1 to_log, 2 from_log applied on the fly (eval_gsr_voicefixer.py:60-62). */
 VF_API int vf_sispec(vf_ctx* ctx, const float* est, const float* target, int batch, int64_t n, int est_map, int target_map,
                      float* out, void* stream);
+
+/* ---- Scoring a restored file against its target (AudioMetrics.evaluation, evaluation_proc/metrics.py:53-81).
+ * Versions: the STFT is librosa 0.8's default (reflect padding; librosa >= 0.10 pads with zeros, not built), and SSIM is
+ * scikit-image <= 0.18's float64 structural_similarity with data_range 2 (the dtype range of float32; >= 0.19 computes in
+ * float32 and refuses float input without data_range, not built).
+ *
+ * np.abs(librosa.stft(wav, n_fft=2048, hop_length=441)) per clip, transposed: wav and offsets packed as in vf_restore_varlen
+ * (HOST offsets, batch + 1, offsets[0] = 0, every clip 1025 .. 2^30 samples); clip i's T_i = 1 + n_i / 441 frames land at
+ * row F_i = sum_{j<i} T_j of sp_out [sum T_i, 1025].  Float64 window and FFT, the spectrum rounded to complex64, |.| of that;
+ * no clamp (digital silence gives exact zeros).  mel_out [sum T_i, 128] (or NULL): MelScale(n_mels=128, sample_rate=44100,
+ * n_stft=1025) of those rows, the arithmetic of vf_mel; it needs "mel.fb" loaded (VF_ESTATE otherwise). */
+VF_API int vf_metric_spectrogram(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* sp_out, float* mel_out,
+                                 void* stream);
+/* SSIM of each [frames, bins] image pair of est / target ([images, frames, bins] fp32, frames and bins >= 7) -> out[images].
+ * The result is float64, as scikit-image's is: the one exception to the fp32 convention above.  Computed in float64 with a
+ * fixed reduction order (deterministic); identical images give exactly 1.0. */
+VF_API int vf_ssim(vf_ctx* ctx, const float* est, const float* target, int images, int frames, int bins, double* out, void* stream);
+/* The spectral part of AudioMetrics.evaluation for `batch` (est, target) pairs at 44.1 kHz: est and target packed with their
+ * own HOST offsets (as in vf_metric_spectrogram).  out [batch, 8] float64 in the reference's key order: lsd, non_log_sispec,
+ * sispec, ssim on the spectrogram, then final_mel_lsd, final_non_log_mel_sispec, final_mel_sispec, final_mel_ssim on its
+ * mel.  lsd and sispec are the fp32 values of vf_lsd / vf_sispec on each pair alone, widened; sispec is on to_log of both
+ * spectrograms.  (sisdr, stoi and pesq come from the third-party speechmetrics package and are not computed.)  Every pair
+ * is checked before any work is queued: equal frame counts and at least 7 frames, else VF_EINVAL naming the pair.  The
+ * scratch (two spectrograms, two mels, SSIM tile sums) is owned by the context and freed by vf_destroy; it is allocated
+ * stream-ordered, so there is no host synchronisation.  Pairs run in consecutive sub-batches of at most 16384 frames
+ * (about 164 s of audio per side) and 128 pairs; a single longer pair gets a sub-batch, and scratch, of its own.  Ten
+ * launches per sub-batch.  Needs "mel.fb" loaded (no network). */
+VF_API int vf_score_varlen(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target,
+                           const int64_t* target_offsets, int batch, double* out, void* stream);
 
 VF_API int vf_to_log(vf_ctx* ctx, const float* in, float* out, int64_t n, void* stream);
 VF_API int vf_from_log(vf_ctx* ctx, const float* in, float* out, int64_t n, void* stream);

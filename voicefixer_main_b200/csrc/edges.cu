@@ -4,6 +4,7 @@
 //   * the mel metrics handler() reports when a target is given (eval_gsr_voicefixer.py:56-64):
 //     AudioMetrics.lsd / .sispec (evaluation_proc/metrics.py:83-95, energy_unify evaluation_proc/utils.py:81-101)
 #include "kernels.cuh"
+#include "reduce.cuh"
 
 namespace vf {
 
@@ -31,22 +32,11 @@ cudaError_t launch_resample_poly(const float* x, int batch, long n, int up, int 
   return cudaGetLastError();
 }
 
-// One CTA per (clip, channel) image of T x F values; fixed reduction order (deterministic).
-__device__ __forceinline__ double block_sum(double v, double* sh) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0;
-  for (int i = 0; i < (int)(blockDim.x >> 5); ++i) s += sh[i];
-  return s;
-}
-
+// One CTA per (clip, channel) image of T x F values; fixed reduction order (deterministic, block_sum in reduce.cuh).
 // AudioMetrics.lsd (metrics.py:83-87): mean_t sqrt(mean_f log10(target^2 / (est + EPS)^2 + EPS)^2), EPS = 1e-12 (metrics.py:15)
-__global__ void __launch_bounds__(256) lsd_kernel(const float* __restrict__ est, const float* __restrict__ tgt, int T, int F, float* __restrict__ out) {
+// The image at element `base` of est / tgt; the value is returned to every thread.
+__device__ __forceinline__ float lsd_image(const float* __restrict__ est, const float* __restrict__ tgt, size_t base, int T, int F) {
   __shared__ double sh[8];
-  const size_t base = (size_t)blockIdx.x * T * F;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   double acc = 0;
   for (int t = warp; t < T; t += 8) {
@@ -61,7 +51,11 @@ __global__ void __launch_bounds__(256) lsd_kernel(const float* __restrict__ est,
     acc += (double)sqrtf(s / (float)F);
   }
   const double tot = block_sum(lane == 0 ? acc : 0.0, sh);
-  if (threadIdx.x == 0) out[blockIdx.x] = (float)(tot / T);
+  return (float)(tot / T);
+}
+__global__ void __launch_bounds__(256) lsd_kernel(const float* __restrict__ est, const float* __restrict__ tgt, int T, int F, float* __restrict__ out) {
+  const float v = lsd_image(est, tgt, (size_t)blockIdx.x * T * F, T, F);
+  if (threadIdx.x == 0) out[blockIdx.x] = v;
 }
 cudaError_t launch_lsd(const float* est, const float* tgt, int images, int T, int F, float* out, cudaStream_t stream) {
   lsd_kernel<<<images, 256, 0, stream>>>(est, tgt, T, F, out);
@@ -79,10 +73,9 @@ __device__ __forceinline__ float metric_map(float v, int m) {
   if (m == 2) return exp10f(fminf(v, 5.f));
   return v;
 }
-__global__ void __launch_bounds__(256) sispec_kernel(const float* __restrict__ est, const float* __restrict__ tgt, long n, int est_map, int tgt_map,
-                                                     float* __restrict__ out) {
+__device__ __forceinline__ float sispec_image(const float* __restrict__ est, const float* __restrict__ tgt, size_t base, long n, int est_map,
+                                              int tgt_map) {
   __shared__ double sh[8];
-  const size_t base = (size_t)blockIdx.x * n;
   double st = 0, tt = 0;
   for (long i = threadIdx.x; i < n; i += 256) {
     const float e = metric_map(__ldg(est + base + i), est_map), g = metric_map(__ldg(tgt + base + i), tgt_map);
@@ -101,10 +94,40 @@ __global__ void __launch_bounds__(256) sispec_kernel(const float* __restrict__ e
   }
   const float p = (float)block_sum(pn, sh);
   const float q = (float)block_sum(nn, sh);
-  if (threadIdx.x == 0) out[blockIdx.x] = 10.f * log10f(p / (q + 1e-12f) + 1e-12f);
+  return 10.f * log10f(p / (q + 1e-12f) + 1e-12f);
+}
+__global__ void __launch_bounds__(256) sispec_kernel(const float* __restrict__ est, const float* __restrict__ tgt, long n, int est_map, int tgt_map,
+                                                     float* __restrict__ out) {
+  const float v = sispec_image(est, tgt, (size_t)blockIdx.x * n, n, est_map, tgt_map);
+  if (threadIdx.x == 0) out[blockIdx.x] = v;
 }
 cudaError_t launch_sispec(const float* est, const float* tgt, int batch, long n, int est_map, int tgt_map, float* out, cudaStream_t stream) {
   sispec_kernel<<<batch, 256, 0, stream>>>(est, tgt, n, est_map, tgt_map, out);
+  return cudaGetLastError();
+}
+
+// The same metrics over images of different frame counts, one launch for a set: image b is rows [frame_off[b],
+// frame_off[b + 1]) of F bins, with the arithmetic and reduction order of a uniform launch on that image alone.  Results are
+// widened to double at out[b * out_stride] (sispec: blockIdx.y = 0 non-log, 1 to_log of both operands, at + blockIdx.y).
+__global__ void __launch_bounds__(256) lsd_varlen_kernel(const float* __restrict__ est, const float* __restrict__ tgt, int F, ImageSet s,
+                                                         double* __restrict__ out, int out_stride) {
+  const int b = blockIdx.x;
+  const float v = lsd_image(est, tgt, (size_t)s.frame_off[b] * F, (int)(s.frame_off[b + 1] - s.frame_off[b]), F);
+  if (threadIdx.x == 0) out[(size_t)b * out_stride] = (double)v;
+}
+__global__ void __launch_bounds__(256) sispec_varlen_kernel(const float* __restrict__ est, const float* __restrict__ tgt, int F, ImageSet s,
+                                                            double* __restrict__ out, int out_stride) {
+  const int b = blockIdx.x, m = blockIdx.y;
+  const long n = (long)(s.frame_off[b + 1] - s.frame_off[b]) * F;
+  const float v = sispec_image(est, tgt, (size_t)s.frame_off[b] * F, n, m, m);
+  if (threadIdx.x == 0) out[(size_t)b * out_stride + m] = (double)v;
+}
+cudaError_t launch_lsd_varlen(const float* est, const float* tgt, int F, const ImageSet& s, double* out, int out_stride, cudaStream_t stream) {
+  lsd_varlen_kernel<<<s.batch, 256, 0, stream>>>(est, tgt, F, s, out, out_stride);
+  return cudaGetLastError();
+}
+cudaError_t launch_sispec_varlen(const float* est, const float* tgt, int F, const ImageSet& s, double* out, int out_stride, cudaStream_t stream) {
+  sispec_varlen_kernel<<<dim3(s.batch, 2), 256, 0, stream>>>(est, tgt, F, s, out, out_stride);
   return cudaGetLastError();
 }
 

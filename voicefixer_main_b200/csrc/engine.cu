@@ -618,6 +618,8 @@ VF_API void vf_destroy(vf_ctx* ctx) {
     if (st) cudaStreamDestroy(st);
   for (auto& e : ctx->ev)
     if (e) cudaEventDestroy(e);
+  if (ctx->d_score) cudaFree(ctx->d_score);
+  if (ctx->score_ev) cudaEventDestroy(ctx->score_ev);
   delete ctx;
 }
 
@@ -881,6 +883,173 @@ VF_API int vf_sispec(vf_ctx* ctx, const float* est, const float* target, int bat
   CK(cudaSetDevice(ctx->device));
   CK(launch_sispec(est, target, batch, (long)n, est_map, target_map, out, (cudaStream_t)stream));
   ctx->launches++;
+  return VF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------- scoring
+namespace {
+
+constexpr long SCORE_CAP_FRAMES = 16384;   // vf_score_varlen sub-batch cap (frames per side), see b200vf.h
+
+// Host offsets of a packed set: offsets[0] == 0, increasing, every clip > 1024 samples (one reflection of the STFT padding)
+// and at most 2^30 samples.
+int check_clip_offsets(vf_ctx* ctx, const char* fn, const char* what, const int64_t* off, int batch) {
+  if (!off || off[0] != 0) return fail(ctx, VF_EINVAL, "%s: %s offsets must start at 0", fn, what);
+  for (int i = 0; i < batch; ++i) {
+    const int64_t n = off[i + 1] - off[i];
+    if (n <= 1024 || n > (int64_t(1) << 30))
+      return fail(ctx, VF_EINVAL, "%s: %s clip %d has %ld samples (need 1025 .. 2^30)", fn, what, i, (long)n);
+  }
+  return VF_OK;
+}
+
+long stft_frames(int64_t n) { return 1 + (long)(n / 441); }
+
+}  // namespace
+
+VF_API int vf_metric_spectrogram(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* sp_out, float* mel_out,
+                                 void* stream) {
+  if (!ctx || !wav || !sp_out || batch <= 0) return ctx ? fail(ctx, VF_EINVAL, "vf_metric_spectrogram: bad arguments") : VF_EINVAL;
+  int rc = check_clip_offsets(ctx, "vf_metric_spectrogram", "wav", offsets, batch);
+  if (rc) return rc;
+  if (mel_out && !ctx->d_fb_val) return fail(ctx, VF_ESTATE, "mel filterbank not loaded (call vf_load_weights first)");
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  long rows = 0;
+  for (int s = 0; s < batch; s += SCORE_MAX_IMAGES) {
+    MetricStftParams p;
+    memset(&p, 0, sizeof p);
+    p.batch = std::min(SCORE_MAX_IMAGES, batch - s);
+    p.sources = 1;
+    p.wav[0] = wav; p.sp[0] = sp_out + (size_t)rows * 1025;
+    p.window = ctx->d_window64; p.tw1024 = ctx->d_tw1024d; p.tw2048 = ctx->d_tw2048d;
+    for (int i = 0; i <= p.batch; ++i) p.off[0][i] = offsets[s + i];
+    for (int i = 0; i < p.batch; ++i) p.frame_off[i + 1] = p.frame_off[i] + stft_frames(offsets[s + i + 1] - offsets[s + i]);
+    CK(launch_metric_stft(p, st));
+    ctx->launches++;
+    rows += (long)p.frame_off[p.batch];
+  }
+  if (mel_out) {
+    MelParams m;
+    memset(&m, 0, sizeof m);
+    m.in = sp_out; m.n_outer = 1; m.T = rows; m.so = 0; m.sf = 1; m.st = 1025;
+    m.out = mel_out; m.fb_f0 = ctx->d_fb_f0; m.fb_len = ctx->d_fb_len; m.fb_ofs = ctx->d_fb_ofs; m.fb_val = ctx->d_fb_val;
+    CK(launch_mel(m, st));
+    ctx->launches++;
+  }
+  return VF_OK;
+}
+
+VF_API int vf_ssim(vf_ctx* ctx, const float* est, const float* target, int images, int frames, int bins, double* out, void* stream) {
+  if (!ctx || !est || !target || !out || images <= 0) return ctx ? fail(ctx, VF_EINVAL, "vf_ssim: bad arguments") : VF_EINVAL;
+  if (frames < 7 || bins < 7) return fail(ctx, VF_EINVAL, "vf_ssim: a %d x %d image is smaller than the 7 x 7 window", frames, bins);
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  const int per = ssim_tiles(frames, bins);
+  double* partial = nullptr;                 // stream-ordered scratch
+  CK(cudaMallocAsync((void**)&partial, (size_t)per * std::min(images, SCORE_MAX_IMAGES) * sizeof(double), st));
+  cudaError_t e = cudaSuccess;
+  for (int s = 0; s < images && e == cudaSuccess; s += SCORE_MAX_IMAGES) {
+    SsimParams p;
+    memset(&p, 0, sizeof p);
+    p.batch = std::min(SCORE_MAX_IMAGES, images - s);
+    const size_t off = (size_t)s * frames * bins;
+    p.x = est + off; p.y = target + off; p.F = bins; p.partial = partial;
+    for (int i = 0; i <= p.batch; ++i) { p.frame_off[i] = (int64_t)i * frames; p.tile_off[i] = i * per; }
+    e = launch_ssim(p, out + s, 1, st);
+    ctx->launches += 2;
+  }
+  cudaFreeAsync(partial, st);
+  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "ssim launch: %s", cudaGetErrorString(e));
+  return VF_OK;
+}
+
+VF_API int vf_score_varlen(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target, const int64_t* target_offsets,
+                           int batch, double* out, void* stream) {
+  if (!ctx || !est || !target || !out || batch <= 0) return ctx ? fail(ctx, VF_EINVAL, "vf_score_varlen: bad arguments") : VF_EINVAL;
+  int rc = check_clip_offsets(ctx, "vf_score_varlen", "est", est_offsets, batch);
+  if (!rc) rc = check_clip_offsets(ctx, "vf_score_varlen", "target", target_offsets, batch);
+  if (rc) return rc;
+  std::vector<long> T(batch);
+  for (int i = 0; i < batch; ++i) {
+    T[i] = stft_frames(est_offsets[i + 1] - est_offsets[i]);
+    const long tt = stft_frames(target_offsets[i + 1] - target_offsets[i]);
+    if (T[i] != tt) return fail(ctx, VF_EINVAL, "vf_score_varlen: pair %d: est has %ld frames, target %ld", i, T[i], tt);
+    if (T[i] < 7) return fail(ctx, VF_EINVAL, "vf_score_varlen: pair %d has %ld frames, fewer than SSIM's 7", i, T[i]);
+  }
+  if (!ctx->d_fb_val) return fail(ctx, VF_ESTATE, "mel filterbank not loaded (call vf_load_weights first)");
+  CK(cudaSetDevice(ctx->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  // consecutive sub-batches of at most SCORE_MAX_IMAGES pairs and SCORE_CAP_FRAMES frames; a longer pair runs alone
+  std::vector<int> starts{0};
+  long frames = 0;
+  size_t need = 0;
+  auto bytes_of = [](long f, long tiles) { return (size_t)f * (2 * 1025 + 2 * 128) * 4 + (size_t)tiles * 8; };
+  long tiles = 0;
+  for (int i = 0; i < batch; ++i) {
+    const int n_in = i - starts.back();
+    if (n_in == SCORE_MAX_IMAGES || (n_in > 0 && frames + T[i] > SCORE_CAP_FRAMES)) {
+      need = std::max(need, bytes_of(frames, tiles));
+      starts.push_back(i);
+      frames = tiles = 0;
+    }
+    frames += T[i];
+    tiles += (long)ssim_tiles(T[i], 1025) + ssim_tiles(T[i], 128);
+  }
+  need = std::max(need, bytes_of(frames, tiles));
+  starts.push_back(batch);
+  if (ctx->score_used) CK(cudaStreamWaitEvent(st, ctx->score_ev, 0));
+  if (!ctx->score_ev) CK(cudaEventCreateWithFlags(&ctx->score_ev, cudaEventDisableTiming));
+  if (need > ctx->score_bytes) {             // stream-ordered: no host synchronisation
+    if (ctx->d_score) CK(cudaFreeAsync(ctx->d_score, st));
+    ctx->d_score = nullptr;
+    ctx->score_bytes = 0;
+    CK(cudaMallocAsync(&ctx->d_score, need, st));
+    ctx->score_bytes = need;
+  }
+  cudaError_t e = cudaSuccess;
+  for (size_t k = 0; k + 1 < starts.size() && e == cudaSuccess; ++k) {
+    const int s = starts[k], nb = starts[k + 1] - starts[k];
+    MetricStftParams p;
+    memset(&p, 0, sizeof p);
+    ImageSet set;
+    memset(&set, 0, sizeof set);
+    p.batch = set.batch = nb;
+    p.sources = 2;
+    for (int i = 0; i <= nb; ++i) { p.off[0][i] = est_offsets[s + i]; p.off[1][i] = target_offsets[s + i]; }
+    for (int i = 0; i < nb; ++i) p.frame_off[i + 1] = set.frame_off[i + 1] = p.frame_off[i] + T[s + i];
+    const long F = (long)p.frame_off[nb];
+    float* sp_e = static_cast<float*>(ctx->d_score);
+    float* sp_t = sp_e + (size_t)F * 1025;
+    float* mel_e = sp_t + (size_t)F * 1025;
+    float* mel_t = mel_e + (size_t)F * 128;
+    double* partial = reinterpret_cast<double*>(mel_t + (size_t)F * 128);   // F * 2306 floats: 8-byte aligned
+    p.wav[0] = est; p.wav[1] = target; p.sp[0] = sp_e; p.sp[1] = sp_t;
+    p.window = ctx->d_window64; p.tw1024 = ctx->d_tw1024d; p.tw2048 = ctx->d_tw2048d;
+    e = launch_metric_stft(p, st);
+    MelParams m;                              // both spectrograms in one launch: outer index 0 = est, 1 = target
+    memset(&m, 0, sizeof m);
+    m.in = sp_e; m.n_outer = 2; m.T = F; m.so = F * 1025; m.sf = 1; m.st = 1025;
+    m.out = mel_e; m.fb_f0 = ctx->d_fb_f0; m.fb_len = ctx->d_fb_len; m.fb_ofs = ctx->d_fb_ofs; m.fb_val = ctx->d_fb_val;
+    if (e == cudaSuccess) e = launch_mel(m, st);
+    double* o = out + (size_t)s * 8;
+    const float* img[2][2] = {{sp_e, sp_t}, {mel_e, mel_t}};
+    const int bins[2] = {1025, 128};
+    for (int r = 0; r < 2 && e == cudaSuccess; ++r) {        // keys 0-3 on the spectrogram, 4-7 on the mel
+      e = launch_lsd_varlen(img[r][0], img[r][1], bins[r], set, o + 4 * r, 8, st);
+      if (e == cudaSuccess) e = launch_sispec_varlen(img[r][0], img[r][1], bins[r], set, o + 4 * r + 1, 8, st);
+      SsimParams q;
+      memset(&q, 0, sizeof q);
+      q.x = img[r][0]; q.y = img[r][1]; q.F = bins[r]; q.batch = nb; q.partial = partial;
+      for (int i = 0; i <= nb; ++i) q.frame_off[i] = set.frame_off[i];
+      for (int i = 0; i < nb; ++i) q.tile_off[i + 1] = q.tile_off[i] + ssim_tiles(T[s + i], bins[r]);
+      if (e == cudaSuccess) e = launch_ssim(q, o + 4 * r + 3, 8, st);
+    }
+    ctx->launches += 10;
+  }
+  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "score launch: %s", cudaGetErrorString(e));
+  CK(cudaEventRecord(ctx->score_ev, st));
+  ctx->score_used = true;
   return VF_OK;
 }
 

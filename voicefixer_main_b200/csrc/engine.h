@@ -174,6 +174,15 @@ struct vf_ctx {
   int *d_fb_f0 = nullptr, *d_fb_len = nullptr, *d_fb_ofs = nullptr;
   float* d_fb_val = nullptr;
   float* d_melw = nullptr;
+  double* d_window64 = nullptr;    // metric STFT (vf_metric_spectrogram, vf_score_varlen): float64 window and twiddles
+  double2* d_tw1024d = nullptr;
+  double2* d_tw2048d = nullptr;
+  // vf_score_varlen scratch (two spectrograms, two mels, SSIM tile sums), stream-ordered allocation grown on demand and
+  // freed by vf_destroy; uses on different streams are ordered through score_ev
+  void* d_score = nullptr;
+  size_t score_bytes = 0;
+  cudaEvent_t score_ev = nullptr;
+  bool score_used = false;
   // UNet weights: the mel-domain analysis module of VoiceFixer (prefix generator.analysis_module.) and the
   // linear-spectrogram unet_v2 of SSR_UNet / GSR_UNet (prefix generator.unet.); either may be absent
   UnetW gsr, ssr;

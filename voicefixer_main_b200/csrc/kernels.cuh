@@ -222,4 +222,48 @@ cudaError_t launch_resample_poly(const float* x, int batch, long n, int up, int 
 cudaError_t launch_lsd(const float* est, const float* tgt, int images, int T, int F, float* out, cudaStream_t stream);
 cudaError_t launch_sispec(const float* est, const float* tgt, int batch, long n, int est_map, int tgt_map, float* out, cudaStream_t stream);
 
+// Scoring (AudioMetrics.evaluation, evaluation_proc/metrics.py:53-81) over sets of images of different frame counts.  The
+// images' extents are kernel parameters, so one launch serves a set of up to SCORE_MAX_IMAGES images.
+constexpr int SCORE_MAX_IMAGES = 128;
+struct ImageSet {
+  int batch;
+  int64_t frame_off[SCORE_MAX_IMAGES + 1];   // image b = rows [frame_off[b], frame_off[b + 1]) of a packed [rows, F] buffer
+};
+// edges.cu: lsd -> out[b * out_stride]; sispec non-log -> out[b * out_stride], to_log of both -> out[b * out_stride + 1]
+cudaError_t launch_lsd_varlen(const float* est, const float* tgt, int F, const ImageSet& s, double* out, int out_stride, cudaStream_t stream);
+cudaError_t launch_sispec_varlen(const float* est, const float* tgt, int F, const ImageSet& s, double* out, int out_stride, cudaStream_t stream);
+
+// metrics.cu: |librosa.stft(wav, n_fft=2048, hop_length=441)| (librosa 0.8: reflect padding, periodic hann, float64 FFT
+// stored as complex64) of up to two packed sources at once (blockIdx.y = source), one CTA per frame.
+struct MetricStftParams {
+  const float* wav[2];                       // packed samples; clip b of source z = wav[z][off[z][b] .. off[z][b + 1])
+  float* sp[2];                              // [sum T_b, 1025]: clip b's frames at rows frame_off[b] ..
+  const double* window;                      // [2048] periodic hann, float64
+  const double2* tw1024;                     // e^{-2 pi i j / 1024}, float64
+  const double2* tw2048;                     // e^{-2 pi i k / 2048}, k = 0..1024
+  int batch, sources;
+  int64_t off[2][SCORE_MAX_IMAGES + 1];
+  int64_t frame_off[SCORE_MAX_IMAGES + 1];   // T_b = 1 + n_b / 441 (the sources have equal frame counts)
+};
+cudaError_t launch_metric_stft(const MetricStftParams& p, cudaStream_t stream);
+
+// skimage.metrics.structural_similarity(x, y, win_size=7) of scikit-image <= 0.18 on float32 images (data_range 2, 7x7
+// uniform filter, sample covariance, mean over the image cropped by 3), in float64.  Stage 1: one CTA per tile of
+// SSIM_TILE_R x SSIM_TILE_C output pixels writes the tile's sum to partial[]; stage 2: one CTA per image sums its tiles in
+// order and writes the mean to out[b * out_stride].
+constexpr int SSIM_TILE_R = 8, SSIM_TILE_C = 64;
+struct SsimParams {
+  const float* x;                            // packed [rows, F] images (frame_off as in ImageSet)
+  const float* y;
+  int F, batch;
+  double* partial;                           // [tile_off[batch]]
+  int64_t frame_off[SCORE_MAX_IMAGES + 1];
+  int tile_off[SCORE_MAX_IMAGES + 1];        // first tile of image b (ssim_tiles)
+};
+// Tiles of one T x F image (T, F >= 7)
+inline int ssim_tiles(long T, int F) {
+  return (int)((T - 6 + SSIM_TILE_R - 1) / SSIM_TILE_R) * ((F - 6 + SSIM_TILE_C - 1) / SSIM_TILE_C);
+}
+cudaError_t launch_ssim(const SsimParams& p, double* out, int out_stride, cudaStream_t stream);
+
 }  // namespace vf

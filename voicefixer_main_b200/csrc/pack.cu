@@ -55,6 +55,19 @@ int build_tables(vf_ctx* ctx) {
   if (rc) return rc;
   rc = upload(ctx, &ctx->d_tw2048, t2);
   if (rc) return rc;
+  // float64 tables of the metric STFT: scipy.signal.get_window('hann', 2048, fftbins=True) as librosa builds it (a
+  // symmetric 2049-point general_cosine, 0.5 + 0.5 cos(fac) with fac = linspace(-pi, pi, 2049), truncated), twiddles
+  std::vector<double> win64(2048);
+  for (int i = 0; i < 2048; ++i) win64[i] = 0.5 + 0.5 * std::cos(i * (2.0 * PI / 2048.0) + -PI);
+  std::vector<double2> d1(1024), d2(1025);
+  for (int j = 0; j < 1024; ++j) d1[j] = make_double2(std::cos(2 * PI * j / 1024.0), -std::sin(2 * PI * j / 1024.0));
+  for (int k = 0; k <= 1024; ++k) d2[k] = make_double2(std::cos(2 * PI * k / 2048.0), -std::sin(2 * PI * k / 2048.0));
+  rc = upload(ctx, &ctx->d_window64, win64);
+  if (rc) return rc;
+  rc = upload(ctx, &ctx->d_tw1024d, d1);
+  if (rc) return rc;
+  rc = upload(ctx, &ctx->d_tw2048d, d2);
+  if (rc) return rc;
   std::vector<float> mw(128);
   for (int i = 0; i < 128; ++i) mw[i] = (float)(ctx->cfg.voc_mel_weight_a * std::exp(ctx->cfg.voc_mel_weight_b * i));
   return upload(ctx, &ctx->d_melw, mw);
@@ -269,7 +282,8 @@ const char* const SSR_PREFIX = "generator.unet.";              // models/ssr_une
 }  // namespace
 
 // Loads whichever of the three networks the descriptors hold (a VoiceFixer checkpoint: analysis module + vocoder;
-// an SSR_UNet / GSR_UNet checkpoint: generator.unet.*).  A network that is present must be complete.
+// an SSR_UNet / GSR_UNet checkpoint: generator.unet.*).  A network that is present must be complete.  With none, only the
+// filterbank is loaded: enough for scoring (vf_score_varlen) and the front end; the network entry points fail with VF_ESTATE.
 int load_all(vf_ctx* ctx) {
   // mel filterbank -> sparse rows (each triangular filter is one contiguous run of bins)
   {
@@ -292,12 +306,10 @@ int load_all(vf_ctx* ctx) {
     rc = upload(ctx, &ctx->d_fb_ofs, ofs); if (rc) return rc;
     rc = upload(ctx, &ctx->d_fb_val, val); if (rc) return rc;
   }
-  int rc = VF_OK, n_nets = 0;
-  if (has_prefix(ctx, GSR_PREFIX)) { rc = load_unet(ctx, GSR_PREFIX, &ctx->gsr); if (rc) return rc; ++n_nets; }
-  if (has_prefix(ctx, SSR_PREFIX)) { rc = load_unet(ctx, SSR_PREFIX, &ctx->ssr); if (rc) return rc; ++n_nets; }
-  if (has_prefix(ctx, "vocoder.")) { rc = load_vocoder(ctx); if (rc) return rc; ++n_nets; }
-  if (n_nets == 0)
-    return fail(ctx, VF_ESTATE, "no network in the state: expected keys under '%s', '%s' or 'vocoder.'", GSR_PREFIX, SSR_PREFIX);
+  int rc = VF_OK;
+  if (has_prefix(ctx, GSR_PREFIX)) { rc = load_unet(ctx, GSR_PREFIX, &ctx->gsr); if (rc) return rc; }
+  if (has_prefix(ctx, SSR_PREFIX)) { rc = load_unet(ctx, SSR_PREFIX, &ctx->ssr); if (rc) return rc; }
+  if (has_prefix(ctx, "vocoder.")) { rc = load_vocoder(ctx); if (rc) return rc; }
   return VF_OK;
 }
 

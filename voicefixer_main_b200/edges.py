@@ -5,9 +5,13 @@
   itself uses to change rates (tools/dsp/lowpass.py:138-141).  The reference's `load_wav` (tools/utils.py:46-48) calls
   librosa.load(sr=44100), whose resampler depends on the installed librosa (soxr_hq / kaiser_best) and is not available
   offline; the FIR here is of the same class (windowed-sinc, > 60 dB stop band) and is checked against scipy.
-* `AudioMetrics.lsd` / `.sispec`: evaluation_proc/metrics.py:83-95 for [B, C, T, F] tensors on the device, the two
-  metrics handler() logs per segment when a target is given (eval_gsr_voicefixer.py:56-64).  `ssim` is CPU numpy in
-  the reference (skimage, metrics.py:97-106) and is not part of this path.
+* `AudioMetrics.lsd` / `.sispec` / `.ssim`: evaluation_proc/metrics.py:83-106 for [B, C, T, F] tensors on the device, the
+  metrics handler() logs per segment when a target is given (eval_gsr_voicefixer.py:56-64).
+* `AudioMetrics.wav_to_spectrogram` / `.evaluation` / `.evaluation_batch`: scoring a restored file against its clean target
+  (metrics.py:37-81), the second half of evaluation_proc/eval.py's evaluation().  The spectrogram is librosa 0.8's STFT
+  (reflect padding; librosa >= 0.10 pads with zeros, not built) and SSIM is scikit-image <= 0.18's float64
+  structural_similarity with data_range 2 (>= 0.19 computes float32 and needs data_range, not built).  sisdr, stoi and pesq
+  come from the third-party speechmetrics package (CPU) and are not produced.
 
 The filter design is host arithmetic (numpy); every sample / reduction is computed by libb200vf kernels (edges.cu).
 """
@@ -56,8 +60,22 @@ def resample_to(eng: Engine, x: torch.Tensor, rate_in: int, rate_out: int = 4410
     return resample_poly(eng, x, fr.numerator, fr.denominator)
 
 
+# AudioMetrics.evaluation's keys (metrics.py:70-78) in the column order of Engine.score_varlen
+SCORE_KEYS = ("lsd", "non_log_sispec", "sispec", "ssim", "final_mel_lsd", "final_non_log_mel_sispec", "final_mel_sispec",
+              "final_mel_ssim")
+
+
+def check_rate(rate: int, what) -> None:
+    """wav_to_spectrogram's rate branch (metrics.py:38-47): 44100 is built, 16000 (n_fft 743, hop 160, 80 mels) is not."""
+    if rate == 16000:
+        raise NotImplementedError(f"{what}: the 16 kHz metrics (n_fft 743, hop 160, 80 mels) are not built")
+    if rate != 44100:
+        raise ValueError(f"Bad Samplerate: {what} is {rate} Hz")
+
+
 class AudioMetrics:
-    """evaluation_proc/metrics.py:25-106, the parts handler() calls on device tensors: lsd and sispec."""
+    """evaluation_proc/metrics.py:25-106 on the GPU: lsd, sispec and ssim of device tensors, the spectrogram and mel of a
+    signal, and evaluation() of restored files against their targets."""
 
     def __init__(self, owner, rate: int = 44100):
         self.rate = rate
@@ -91,3 +109,63 @@ class AudioMetrics:
         with torch.cuda.device(eng.device):
             eng._ck(eng.lib.vf_sispec(eng.ctx, _ptr(est), _ptr(target), b, n, int(est_map), int(target_map), _ptr(out), _stream()))
         return torch.sum(out) / b
+
+    def ssim(self, est: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
+        """metrics.py:97-106: structural_similarity(est[b, c], target[b, c], win_size=7) of [B, C, T, F] tensors ->
+        float64 [B, C, 1, 1].  T or F below 7 raises ValueError, as scikit-image does."""
+        eng = self._eng()
+        if est.dim() != 4 or est.shape != target.shape:
+            raise ValueError("ssim: est and target must be [B, C, T, F] tensors of one shape")
+        b, c, t, f = est.shape
+        if t < 7 or f < 7:
+            raise ValueError(f"ssim: win_size 7 exceeds the {t} x {f} image")
+        return eng.ssim(est.reshape(b * c, t, f), target.reshape(b * c, t, f)).view(b, c, 1, 1)
+
+    def wav_to_spectrogram(self, wav, rate: int = 44100):
+        """metrics.py:37-51 for one signal (numpy or tensor, 1-D): (sp [1, 1, T, 1025], mel [1, 1, T, 128]) on the device."""
+        check_rate(rate, "wav")
+        eng = self._eng()
+        x = torch.as_tensor(np.ascontiguousarray(wav, dtype=np.float32) if not isinstance(wav, torch.Tensor) else wav)
+        x = x.to(eng.device, torch.float32).reshape(-1).contiguous()
+        sp, mel = eng.metric_spectrogram(x, [x.numel()])
+        return sp[None, None], mel[None, None]
+
+    def evaluation(self, est, target) -> dict:
+        """metrics.py:53-81 for one (est, target) pair of wav paths: the 8 spectral keys; {} when target is None."""
+        return self.evaluation_batch([(est, target)])[0]
+
+    def evaluation_batch(self, pairs) -> list:
+        """evaluation(est, target) of every pair, in order, in one vf_score_varlen call: each dict is float-identical to
+        evaluation() of that pair.  Every file is decoded and checked before any GPU work; a bad pair fails the whole call,
+        naming the file: a target at 16 kHz (NotImplementedError) or at another rate than 44.1 kHz (ValueError), an est
+        whose frame count differs from its target's or a pair of fewer than 7 frames (ValueError)."""
+        from .arch import frames_for
+        from .handler import _rate_len, _to_rate, read_pcm16
+        eng = self._eng()
+        decoded = []
+        for est, target in pairs:
+            if target is None:
+                decoded.append(None)
+                continue
+            t, rate = read_pcm16(target)
+            check_rate(rate, target)
+            e, e_rate = read_pcm16(est)
+            te, tt = frames_for(_rate_len(len(e), e_rate, rate)), frames_for(len(t))
+            if te != tt:
+                raise ValueError(f"{est} has {te} frames at {rate} Hz, its target {target} {tt}")
+            if tt < 7:
+                raise ValueError(f"{est} / {target}: {tt} frames, fewer than SSIM's 7x7 window")
+            decoded.append((est, e, e_rate, t))
+        live = [d for d in decoded if d is not None]
+        results = [{} for _ in decoded]
+        if not live:
+            return results
+        ests = [_to_rate(path, e, e_rate, 44100, eng) for path, e, e_rate, _ in live]
+        tgts = [t for _, _, _, t in live]
+        scores = eng.score_varlen(torch.from_numpy(np.concatenate(ests)).to(eng.device), [len(e) for e in ests],
+                                  torch.from_numpy(np.concatenate(tgts)).to(eng.device), [len(t) for t in tgts]).cpu()
+        rows = iter(scores.tolist())
+        for i, d in enumerate(decoded):
+            if d is not None:
+                results[i] = dict(zip(SCORE_KEYS, next(rows)))
+        return results

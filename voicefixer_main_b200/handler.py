@@ -5,8 +5,8 @@ Same signature and contract as the reference handler that evaluation_proc/eval.p
 It writes a 16-bit wav at `output`.  Differences, all outside the hot path: audio decoding uses the stdlib `wave`
 module (librosa / soundfile are not in this image): PCM16 wav of ANY sample rate, converted to 44.1 kHz on the GPU by
 the polyphase resampler (edges.py; load_wav -> librosa.load(sr=44100), tools/utils.py:46-48).  With a `target` the
-per-segment mel metrics of eval_gsr_voicefixer.py:56-64 are computed on the GPU (lsd, sispec, non-log sispec; `mel-ssim`
-is a CPU skimage call in the reference, evaluation_proc/metrics.py:97-106, and is not reported).
+per-segment mel metrics of eval_gsr_voicefixer.py:56-64 are computed on the GPU (lsd, sispec, non-log sispec, and with
+meta["mel_ssim"] the reference's `mel-ssim`, evaluation_proc/metrics.py:97-106).
 The segment loop, from_log, peak normalisation, trim_center, concat and the int16 conversion of
 tools/file/wav.py:22-24 are reproduced exactly; the per-segment stages run as one fused launch chain.
 handler_batch(items, ...) is handler() over a whole list of files, with the same files and dicts, as batched restores.
@@ -89,7 +89,7 @@ def refresh_model(ckpt):
 
 
 def restore_array(mdl: VoiceFixer, wav_10k: np.ndarray, device, unify_energy: bool = False, target: np.ndarray = None,
-                  metrics: dict = None) -> torch.Tensor:
+                  metrics: dict = None, mel_ssim: bool = False) -> torch.Tensor:
     """The segment loop of handler() for one in-memory file: returns [1, N] on `device`.  With `target` (the clean
     signal, same rate) the mel metrics of the LAST segment land in `metrics`, as the reference's loop leaves them
     (eval_gsr_voicefixer.py:56-64 overwrites the dict every segment)."""
@@ -103,14 +103,15 @@ def restore_array(mdl: VoiceFixer, wav_10k: np.ndarray, device, unify_energy: bo
         if target is not None and metrics is not None:
             tseg = torch.from_numpy(np.ascontiguousarray(target[break_point - SEG_LENGTH:break_point]))[None, None, :].to(device)
             mel_noisy, log_mel = mdl._engine().restore_stages(1, seg.shape[1])
-            metrics.update(_mel_metrics(mdl, tseg, mel_noisy[:, None], log_mel[:, None], unify_energy))
+            metrics.update(_mel_metrics(mdl, tseg, mel_noisy[:, None], log_mel[:, None], unify_energy, mel_ssim))
         break_point += SEG_LENGTH
     return torch.cat(res, -1)
 
 
-def _mel_metrics(mdl: VoiceFixer, tseg, mel_noisy, log_mel, unify_energy: bool) -> dict:
+def _mel_metrics(mdl: VoiceFixer, tseg, mel_noisy, log_mel, unify_energy: bool, mel_ssim: bool = False) -> dict:
     """eval_gsr_voicefixer.py:56-64 for one segment: tseg [1, 1, n] the clean target on the device, mel_noisy / log_mel
-    [1, 1, T, 128] the restore's linear mel (stage A) and restored log10 mel (stage B)."""
+    [1, 1, T, 128] the restore's linear mel (stage A) and restored log10 mel (stage B).  mel_ssim adds "mel-ssim" (:63), the
+    SSIM of the same mels as "mel-lsd"; a segment of fewer than 7 frames then raises ValueError, as skimage does."""
     from .edges import AudioMetrics
     am = AudioMetrics(mdl)
     eng = mdl._engine()
@@ -118,11 +119,14 @@ def _mel_metrics(mdl: VoiceFixer, tseg, mel_noisy, log_mel, unify_energy: bool) 
     denoised = eng.from_log(log_mel)
     if unify_energy:                     # eval_gsr_voicefixer.py:54-55 (tools/utils.py:50-55) before the lsd
         denoised = eng.amp_to_original_f(denoised[:, 0].contiguous(), mel_noisy[:, 0].contiguous())[:, None]
-    return {
+    res = {
         "mel-lsd": float(am.lsd(denoised.contiguous(), target_mel.contiguous())),
         "mel-sispec": float(am.sispec(log_mel, target_mel.contiguous(), target_map=1)),             # in log scale
         "mel-non-log-sispec": float(am.sispec(log_mel, target_mel.contiguous(), est_map=2)),
     }
+    if mel_ssim:
+        res["mel-ssim"] = float(am.ssim(denoised.contiguous(), target_mel.contiguous()))
+    return res
 
 
 def segment_bounds(n):
@@ -130,11 +134,12 @@ def segment_bounds(n):
     return [(bp - SEG_LENGTH, min(bp, n)) for bp in range(SEG_LENGTH, n + SEG_LENGTH, SEG_LENGTH)]
 
 
-def _check_file(path, n, n_target=None):
+def _check_file(path, n, n_target=None, mel_ssim=False):
     """Raises what handler() would raise on a file of n samples (at 44.1 kHz) with a target of n_target samples (None: no
     target), without touching the GPU: nothing to concatenate (RuntimeError); a segment, or the target slice of one, of at
     most 1024 samples, which the front end's reflect padding rejects (EngineError); a target slice with another frame count
-    than its segment, which the metrics' shape check rejects (AssertionError).  Segments are checked in handler()'s order."""
+    than its segment, which the metrics' shape check rejects (AssertionError); with mel_ssim, a segment with a target and
+    fewer than 7 frames, which SSIM's 7x7 window rejects (ValueError).  Segments are checked in handler()'s order."""
     bounds = segment_bounds(n)
     if not bounds:
         raise RuntimeError(f"{path}: no samples to restore")
@@ -150,6 +155,8 @@ def _check_file(path, n, n_target=None):
         if frames_for(t) != frames_for(e - s):
             raise AssertionError(f"{path}: the target slice of segment [{s}, {e}) has {frames_for(t)} frames, the segment "
                                  f"{frames_for(e - s)}")
+        if mel_ssim and frames_for(e - s) < 7:
+            raise ValueError(f"{path}: segment [{s}, {e}) has {frames_for(e - s)} frames; mel-ssim's 7x7 window needs 7")
 
 
 def handler(input, output, target, ckpt, device, needrefresh=False, meta={}):
@@ -160,7 +167,8 @@ def handler(input, output, target, ckpt, device, needrefresh=False, meta={}):
     metrics = {}
     wav_10k = load_wav(input, sample_rate=44100, engine=model._engine())
     tgt = load_wav(target, sample_rate=44100, engine=model._engine()) if target is not None else None
-    out = restore_array(model, wav_10k, model.device, unify_energy=bool(meta.get("unify_energy", False)), target=tgt, metrics=metrics)
+    out = restore_array(model, wav_10k, model.device, unify_energy=bool(meta.get("unify_energy", False)), target=tgt, metrics=metrics,
+                        mel_ssim=bool(meta.get("mel_ssim", False)))
     # save_wave's float -> int16 conversion runs on the GPU (its `max <= 1` condition always holds after the
     # per-segment peak normalisation), so only 2 bytes per sample cross PCIe.  meta["saturate"] (not in the reference)
     # clamps instead of reproducing numpy's +1.0 -> -32768 wrap, see INTEGRATION.md
@@ -190,7 +198,8 @@ def handler_batch(items, ckpt, device, needrefresh=False, meta={}):
     for inp, _, tgt in items:
         x = read_pcm16(inp)
         t = read_pcm16(tgt) if tgt is not None else None
-        _check_file(inp, _rate_len(len(x[0]), x[1]), None if t is None else _rate_len(len(t[0]), t[1]))
+        _check_file(inp, _rate_len(len(x[0]), x[1]), None if t is None else _rate_len(len(t[0]), t[1]),
+                    mel_ssim=bool(meta.get("mel_ssim", False)))
         decoded.append((x, t))
     sigs = [_to_rate(inp, *x, 44100, eng) for (inp, _, _), (x, _) in zip(items, decoded)]
     tgts = [None if t is None else _to_rate(tgt, *t, 44100, eng) for (_, _, tgt), (_, t) in zip(items, decoded)]
@@ -231,7 +240,7 @@ def handler_batch(items, ckpt, device, needrefresh=False, meta={}):
         k = file_segs[f][-1]
         s = segs[k][1]
         tseg = torch.from_numpy(np.ascontiguousarray(tgt[s:s + SEG_LENGTH]))[None, None, :].to(model.device)
-        results.append(_mel_metrics(model, tseg, *mels[k], unify))
+        results.append(_mel_metrics(model, tseg, *mels[k], unify, bool(meta.get("mel_ssim", False))))
     for (_, output, _), ks in zip(items, file_segs):
         save_pcm16(np.concatenate([pcm[k] for k in ks]), fname=output, sample_rate=44100)
     return results

@@ -249,6 +249,42 @@ class Engine:
                                          ctypes.c_void_p(out[o0:].data_ptr()), _stream()))
         return out.view(*lead, t, 128).transpose(-1, -2)     # same memory layout as the reference's matmul result
 
+    def metric_spectrogram(self, wav_packed: torch.Tensor, lengths, want_mel: bool = True):
+        """vf_metric_spectrogram: |librosa.stft(n_fft=2048, hop_length=441)| of each clip of wav_packed (clips back to back,
+        `lengths` samples each) -> (sp [sum T_i, 1025], mel [sum T_i, 128] or None), clip i at rows sum_{j<i} T_i."""
+        wav_packed, offsets = self._varlen_args(wav_packed, lengths)
+        rows = sum(frames_for(offsets[i + 1] - offsets[i]) for i in range(len(offsets) - 1))
+        sp = torch.empty(rows, 1025, device=self.device)
+        mel = torch.empty(rows, 128, device=self.device) if want_mel else None
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_metric_spectrogram(self.ctx, _ptr(wav_packed), offsets, len(offsets) - 1, _ptr(sp), _ptr(mel),
+                                                    _stream()))
+        return sp, mel
+
+    def ssim(self, est: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
+        """vf_ssim: est, target [images, frames, bins] float32 -> float64 [images]."""
+        est, target = _check_in(est, self.device, "est"), _check_in(target, self.device, "target")
+        if est.dim() != 3 or est.shape != target.shape:
+            raise ValueError("ssim: est and target must be [images, frames, bins] tensors of one shape")
+        n, t, f = est.shape
+        out = torch.empty(n, dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_ssim(self.ctx, _ptr(est), _ptr(target), n, t, f, _ptr(out), _stream()))
+        return out
+
+    def score_varlen(self, est_packed: torch.Tensor, est_lengths, target_packed: torch.Tensor, target_lengths) -> torch.Tensor:
+        """vf_score_varlen: the spectral metrics of each (est, target) pair of two packed sets -> float64 [pairs, 8], columns
+        in the order of edges.SCORE_KEYS."""
+        est_packed, est_off = self._varlen_args(est_packed, est_lengths)
+        target_packed, target_off = self._varlen_args(target_packed, target_lengths)
+        if len(est_off) != len(target_off):
+            raise ValueError("score_varlen: est and target must hold the same number of clips")
+        out = torch.empty(len(est_off) - 1, 8, dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_score_varlen(self.ctx, _ptr(est_packed), est_off, _ptr(target_packed), target_off,
+                                              len(est_off) - 1, _ptr(out), _stream()))
+        return out
+
     def amp_to_original_f(self, mel_est: torch.Tensor, mel_target: torch.Tensor) -> torch.Tensor:
         """tools/utils.py:50-55 on linear mels [B,T,128]: the estimate scaled to the target's low-band energy."""
         mel_est, mel_target = _check_in(mel_est, self.device, "mel_est"), _check_in(mel_target, self.device, "mel_target")
