@@ -25,6 +25,8 @@
  *                                 Generator.forward :51-54 -> unet_v2 UNetResComplex_100Mb.forward
  *                                 models/components/unet_v2.py:86-148 (magnitude net, input phase, ISTFT)
  *   vf_ssr_restore_varlen         the same for clips of different lengths in one call (eval_ssr_unet.py:handler()'s test set)
+ *   vf_ssr_restore_varlen_mels    + each clip's output mel and peak normalise, the rest of eval_gsr_unet.py:handler()'s
+ *                                 segment loop (handler_unet.handler_batch)
  *   vf_istft                      FDomainHelper.istft tools/pytorch/modules/fDomainHelper.py:30-32,127 (torchlibrosa ISTFT)
  *   vf_resample_poly              load_wav's rate conversion, tools/utils.py:46-48
  *   vf_lsd / vf_sispec            AudioMetrics.lsd / .sispec evaluation_proc/metrics.py:83-95 (handler's mel metrics,
@@ -159,6 +161,19 @@ VF_API int vf_restore_varlen_mels(vf_ctx* ctx, const float* wav, const int64_t* 
  * vf_restore_varlen. */
 VF_API int vf_ssr_restore_varlen(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out,
                                  void* stream);
+/* vf_ssr_restore_varlen plus the rest of one iteration of the SSR / GSR-UNet handler's segment loop (eval_gsr_unet.py:54-67,
+ * eval_ssr_unet.py:116-136):
+ * - mel_out ([sum T_i, 128], device, or NULL): the linear mel of clip i's restored, un-normalised output,
+ *   mel(wav_to_spectrogram_phase(out)[0]), T_i = 1 + n_i / hop frames at frame offset F_i = sum_{j<i} T_j.  Bit-identical
+ *   to vf_frontend's mel_out on vf_ssr_restore's output for that clip alone.
+ * - flags & VF_SSR_PEAK_NORMALISE: after the mel is taken, clip i of wav_out is divided by its own max |x| when that
+ *   exceeds 1.  Bit-identical to vf_finalize(len = n_i, n_samples = n_i) on vf_ssr_restore's output for that clip alone.
+ * Per sub-batch, on `stream` after the ISTFT: with mel_out one front-end launch and one copy kernel, with the flag one
+ * memset and two kernels.  Unknown flag bits fail with VF_EINVAL before any work is queued.  With mel_out NULL and flags 0
+ * the call is vf_ssr_restore_varlen. */
+#define VF_SSR_PEAK_NORMALISE 1u
+VF_API int vf_ssr_restore_varlen_mels(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out,
+                                      unsigned flags, float* mel_out, void* stream);
 /* Same through HOST buffers (pinned for true asynchrony).  The copies and the compute run on library-owned streams with
  * two staging buffer pairs, so back-to-back calls overlap (the H2D of call i+1 and the D2H of call i-1 run under the
  * compute of call i); `stream` only receives a wait on this call's D2H.  Contract: wav_host holds its data when the

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of a test-set evaluation: handler() once per file against one handler_batch() call, on one GPU.
 
-    python tools/bench_testset.py --out DIR [--files F] [--steps K]
+    python tools/bench_testset.py --out DIR [--files F] [--steps K] [--workload gsr|ssr]
 
 Writes a seeded synthetic test set under DIR/set: F PCM16 files (default 64) of lengths uniform in [1 s, 10 s] at 44.1 kHz,
 plus one 61 s file (two segments) and two 22.05 kHz files, with clean targets for every other file.  In one process it
@@ -11,6 +11,8 @@ over the set, which builds its plans, is timed on its own (first_run_*: one eval
 after one warm-up file); then the two arms alternate for --steps runs with their plans cached as far as the plan budget
 allows.  It checks that the two arms wrote byte-identical files and equal metrics, and prints one JSON line with files/s
 and audio-seconds/s of both arms, the plans each evicted per run, and the card's name and power limit.
+--workload gsr (the default) runs VoiceFixer through handler.py; --workload ssr runs SSR_UNet through handler_unet.py
+(eval_gsr_unet.py / eval_ssr_unet.py's handler) on the same set.
 """
 import argparse
 import json
@@ -53,14 +55,22 @@ def main():
     ap.add_argument("--files", type=int, default=64, help="files of 1 - 10 s (plus the 61 s and the two 22.05 kHz files)")
     ap.add_argument("--steps", type=int, default=3, help="timed runs of each arm")
     ap.add_argument("--seed", type=int, default=4242)
+    ap.add_argument("--workload", choices=("gsr", "ssr"), default="gsr",
+                    help="gsr: VoiceFixer through handler.py; ssr: SSR_UNet through handler_unet.py")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("tools/bench_testset.py needs a CUDA device")
-    from voicefixer_main_b200 import VoiceFixer
-    from voicefixer_main_b200 import handler as H
-    from voicefixer_main_b200.weights import make_state
     dev = torch.device("cuda", 0)
-    H.model = VoiceFixer().load_state_dict(make_state(1234)).eval().to(dev)
+    if args.workload == "ssr":
+        from voicefixer_main_b200 import SSR_UNet
+        from voicefixer_main_b200 import handler_unet as H
+        from voicefixer_main_b200.weights import make_ssr_state
+        H.model = SSR_UNet().load_state_dict(make_ssr_state(1234)).eval().to(dev)
+    else:
+        from voicefixer_main_b200 import VoiceFixer
+        from voicefixer_main_b200 import handler as H
+        from voicefixer_main_b200.weights import make_state
+        H.model = VoiceFixer().load_state_dict(make_state(1234)).eval().to(dev)
     items, audio_s = write_set(H, os.path.join(args.out, "set"), args.files, args.seed)
     dirs = {k: os.path.join(args.out, k) for k in ("per_file", "batch")}
     for d in dirs.values():
@@ -104,10 +114,11 @@ def main():
         res[k] = {"s_median": med, "s_min": min(v), "s_max": max(v), "files_per_sec": len(items) / med,
                   "audio_seconds_per_sec": audio_s / med, "plans_evicted_per_run": evicted[k] / len(v),
                   "first_run_s": first[k], "first_run_files_per_sec": len(items) / first[k]}
-    line = {"metric": "files_per_sec_testset_44k1", "value": res["batch"]["files_per_sec"], "unit": "files/s",
+    line = {"metric": "files_per_sec_testset_44k1" + ("_ssr" if args.workload == "ssr" else ""), "value": res["batch"]["files_per_sec"], "unit": "files/s",
             "steps": args.steps, "higher_is_better": True, "data": "synthetic",
             "config": {"workload": f"{len(items)} PCM16 files ({args.files} of 1 - 10 s, one of 61 s, two at 22.05 kHz), "
-                                   f"targets on every other file; value = one handler_batch call", "files": len(items),
+                                   f"targets on every other file; value = one "
+                                   f"{'handler_unet.' if args.workload == 'ssr' else ''}handler_batch call", "files": len(items),
                        "total_audio_seconds": audio_s, "plan_cache": H.model._engine().plan_cache_info()},
             "arms": res, "speedup_vs_per_file": res["per_file"]["s_median"] / res["batch"]["s_median"],
             "first_run_speedup_vs_per_file": first["per_file"] / first["batch"],

@@ -456,6 +456,36 @@ cudaError_t launch_gather_mels(const MelGatherParams& p, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
+// Segmented peak normalise (kernels.cuh): clip b = wav[off[b] .. off[b + 1]).  The max is order-free and the scale divides as
+// finalize_kernel does, so each clip gets the bits of a one-clip vf_finalize(len = n, n = n).
+__global__ void __launch_bounds__(256) peak_varlen_kernel(const float* __restrict__ wav, const int64_t* __restrict__ off,
+                                                          unsigned int* peak_bits) {
+  const int b = blockIdx.y;
+  const int64_t end = __ldg(off + b + 1);
+  float m = 0.f;
+  for (int64_t i = __ldg(off + b) + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < end; i += (int64_t)gridDim.x * blockDim.x)
+    m = fmaxf(m, fabsf(__ldg(wav + i)));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) atomicMax(peak_bits + b, __float_as_uint(m));
+}
+__global__ void __launch_bounds__(256) scale_varlen_kernel(float* __restrict__ wav, const int64_t* __restrict__ off,
+                                                           const unsigned int* __restrict__ peak_bits) {
+  const int b = blockIdx.y;
+  const float peak = __uint_as_float(__ldg(peak_bits + b));
+  if (!(peak > 1.0f)) return;                              // block-uniform: this clip is left as it is
+  const int64_t end = __ldg(off + b + 1);
+  for (int64_t i = __ldg(off + b) + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < end; i += (int64_t)gridDim.x * blockDim.x)
+    wav[i] = wav[i] / peak;
+}
+cudaError_t launch_peak_normalise_varlen(float* wav, const int64_t* vl_off, int batch, long n_max, unsigned int* peak_bits,
+                                         cudaStream_t stream) {
+  dim3 grid((unsigned)std::min<long>((n_max + 2047) / 2048, 128), batch);
+  peak_varlen_kernel<<<grid, 256, 0, stream>>>(wav, vl_off, peak_bits);
+  scale_varlen_kernel<<<grid, 256, 0, stream>>>(wav, vl_off, peak_bits);
+  return cudaGetLastError();
+}
+
 cudaError_t launch_pcm16(const float* in, int16_t* out, size_t n, int saturate, cudaStream_t stream) {
   const unsigned blocks = (unsigned)std::min<size_t>((n + 255) / 256, 148 * 16);
   pcm16_kernel<<<blocks, 256, 0, stream>>>(in, out, n, saturate);

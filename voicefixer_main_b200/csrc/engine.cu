@@ -515,6 +515,13 @@ int run_varlen_sub_batches(vf_ctx* ctx, int kind, const int64_t* offsets, int ba
   }, VL_MAX_CLIPS);
 }
 
+// Packed frame offsets F_i = sum_{j<i} T_j of a varlen call's clips
+std::vector<int64_t> frame_offsets(vf_ctx* ctx, const int64_t* offsets, int batch) {
+  std::vector<int64_t> f(batch + 1, 0);
+  for (int i = 0; i < batch; ++i) f[i + 1] = f[i] + frames_of(ctx, (long)(offsets[i + 1] - offsets[i]));
+  return f;
+}
+
 // vf_restore_varlen (`fn`) and vf_restore_varlen_mels.  With mel_out or log_mel_out, each sub-batch's restore is followed by
 // one gather of its clips' rows t < T_i into the packed outputs at frame offsets F_i = sum_{j<i} T_j, still inside the
 // plan's use on `stream` (plan_exit again after it).
@@ -534,8 +541,7 @@ int restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t*
   });
   if (rc) return rc;
   const bool mels = mel_out || log_mel_out;
-  std::vector<int64_t> frame_off(mels ? batch + 1 : 0, 0);
-  for (int i = 0; mels && i < batch; ++i) frame_off[i + 1] = frame_off[i] + frames_of(ctx, (long)(offsets[i + 1] - offsets[i]));
+  const std::vector<int64_t> frame_off = mels ? frame_offsets(ctx, offsets, batch) : std::vector<int64_t>();
   return run_varlen_sub_batches(ctx, PLAN_VARLEN, offsets, batch, [&](Plan* plan, int s, int b, const int64_t* rel, int64_t n_max) {
     int r = restore_impl(ctx, plan, wav + offsets[s], b, n_max, wav_out + offsets[s], flags, st, rel);
     if (r || !mels) return r;
@@ -546,6 +552,44 @@ int restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t*
     for (int i = 0; i <= b; ++i) g.frame_off[i] = frame_off[s + i];
     CK(launch_gather_mels(g, st));
     ctx->launches++;
+    return plan_exit(ctx, plan, st);
+  });
+}
+
+// vf_ssr_restore_varlen (`fn`) and vf_ssr_restore_varlen_mels.  After each sub-batch's ISTFT, still inside the plan's use on
+// `stream`: with mel_out, the front end on the restored clips and one gather of their rows into the packed output; with
+// VF_SSR_PEAK_NORMALISE, the per-clip peak normalise of wav_out, after the mel is taken.
+int ssr_restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t* offsets, int batch, float* wav_out,
+                       unsigned flags, float* mel_out, cudaStream_t st) {
+  int rc = check_ready(ctx);
+  if (rc) return rc;
+  if (!wav || !wav_out || !offsets || batch <= 0) return fail(ctx, VF_EINVAL, "%s: bad arguments", fn);
+  if (flags & ~(unsigned)VF_SSR_PEAK_NORMALISE) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
+  rc = check_varlen_call(ctx, fn, PLAN_SSR_VARLEN, offsets, batch, [](int, int64_t) { return VF_OK; });
+  if (rc) return rc;
+  const bool peak = (flags & VF_SSR_PEAK_NORMALISE) != 0;
+  const std::vector<int64_t> frame_off = mel_out ? frame_offsets(ctx, offsets, batch) : std::vector<int64_t>();
+  return run_varlen_sub_batches(ctx, PLAN_SSR_VARLEN, offsets, batch, [&](Plan* plan, int s, int b, const int64_t* rel, int64_t n_max) {
+    float* out = wav_out + offsets[s];
+    int r = ssr_impl(ctx, plan, nullptr, wav + offsets[s], b, n_max, out, st, rel);
+    if (r || (!mel_out && !peak)) return r;
+    if (mel_out) {
+      // mel(wav_to_spectrogram_phase(out)[0]) (eval_gsr_unet.py:54-55).  The ISTFT frames are dead once the overlap-add
+      // has run, so they hold the mels at the bucket's row stride ([b, T, 128] of the [b, T, 2048] buffer).
+      r = run_frontend(ctx, out, b, (long)n_max, plan->d_frames, nullptr, nullptr, nullptr, nullptr, st, plan);
+      if (r) return r;
+      MelGatherParams g;
+      memset(&g, 0, sizeof g);
+      g.mel = plan->d_frames; g.mel_out = mel_out; g.batch = b; g.T = plan->T;
+      for (int i = 0; i <= b; ++i) g.frame_off[i] = frame_off[s + i];
+      CK(launch_gather_mels(g, st));
+      ctx->launches++;
+    }
+    if (peak) {
+      CK(cudaMemsetAsync(plan->d_peak, 0, (size_t)b * sizeof(unsigned int), st));
+      CK(launch_peak_normalise_varlen(out, plan->d_vl_off, b, (long)n_max, plan->d_peak, st));
+      ctx->launches += 2;
+    }
     return plan_exit(ctx, plan, st);
   });
 }
@@ -755,14 +799,13 @@ VF_API int vf_ssr_restore(vf_ctx* ctx, const float* wav, int batch, int64_t n, f
 }
 
 VF_API int vf_ssr_restore_varlen(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out, void* stream) {
-  int rc = check_ready(ctx);
-  if (rc) return rc;
-  if (!wav || !wav_out || !offsets || batch <= 0) return fail(ctx, VF_EINVAL, "vf_ssr_restore_varlen: bad arguments");
-  rc = check_varlen_call(ctx, "vf_ssr_restore_varlen", PLAN_SSR_VARLEN, offsets, batch, [](int, int64_t) { return VF_OK; });
-  if (rc) return rc;
-  return run_varlen_sub_batches(ctx, PLAN_SSR_VARLEN, offsets, batch, [&](Plan* plan, int s, int b, const int64_t* rel, int64_t n_max) {
-    return ssr_impl(ctx, plan, nullptr, wav + offsets[s], b, n_max, wav_out + offsets[s], (cudaStream_t)stream, rel);
-  });
+  return ssr_restore_varlen(ctx, "vf_ssr_restore_varlen", wav, offsets, batch, wav_out, 0u, nullptr, (cudaStream_t)stream);
+}
+
+VF_API int vf_ssr_restore_varlen_mels(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out,
+                                      unsigned flags, float* mel_out, void* stream) {
+  return ssr_restore_varlen(ctx, "vf_ssr_restore_varlen_mels", wav, offsets, batch, wav_out, flags, mel_out,
+                            (cudaStream_t)stream);
 }
 
 VF_API int vf_ssr_restore_host(vf_ctx* ctx, const float* wav_host, int batch, int64_t n, float* out_host, void* stream) {

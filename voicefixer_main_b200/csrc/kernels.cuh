@@ -165,6 +165,11 @@ cudaError_t launch_pcm16(const float* in, int16_t* out, size_t n, int saturate, 
 
 // max |wav| per clip as float bits (atomicMax), for the stand-alone peak normalise + trim entry point.
 cudaError_t launch_peak(const float* wav, int batch, long L, unsigned int* peak_bits, cudaStream_t stream);
+// vf_ssr_restore_varlen_mels: in place, clip b = wav[vl_off[b] .. vl_off[b + 1]) (device offsets, clips of at most n_max
+// samples) is divided by its max |x| when that exceeds 1 (eval_gsr_unet.py:66-67).  Two kernels: the per-clip max as float
+// bits into peak_bits[batch], which must be zeroed before the launch, then the scale.
+cudaError_t launch_peak_normalise_varlen(float* wav, const int64_t* vl_off, int batch, long n_max, unsigned int* peak_bits,
+                                         cudaStream_t stream);
 
 // MelScale.forward (tools/pytorch/mel_scale.py:52-64) as a stand-alone op on any [..., freq, time] view:
 // out[o, t, m] = sum_f in[o * so + f * sf + t * st] * fb[f, m] with the filterbank in its sparse form.

@@ -695,12 +695,14 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
 }
 
 // SSR / GSR-UNet plan (models/ssr_unet.py:145-155 -> unet_v2.py:86-148): STFT magnitude -> unet_v2 on 1024 bins -> the
-// predicted magnitude with the input's phase -> ISTFT.  Frames and the magnitude planes are the only extra buffers.
+// predicted magnitude with the input's phase -> ISTFT.  Frames and the magnitude planes are the only extra buffers (and,
+// in a varlen plan, the per-clip peaks of the output's peak normalise).
 int build_ssr(vf_ctx* ctx, Builder& b, Plan* plan) {
   const size_t sp_n = (size_t)plan->batch * plan->T * 1025;
   plan->d_sp = b.alloc<float>(sp_n);
   plan->d_mag = b.alloc<float>(sp_n);
   plan->d_frames = b.alloc<float>((size_t)plan->batch * plan->T * 2048);
+  if (plan->kind == PLAN_SSR_VARLEN) plan->d_peak = b.alloc<unsigned int>(plan->batch);   // vf_ssr_restore_varlen_mels
   if (b.rc) return b.rc;
   UnetGeom g{1024, plan->d_sp, nullptr, plan->d_mag, "ssr."};
   return build_unet(ctx, b, plan, ctx->ssr, g);

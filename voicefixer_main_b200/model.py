@@ -316,13 +316,24 @@ class Engine:
             self._ck(self.lib.vf_ssr_forward(self.ctx, _ptr(sp), _ptr(wav), b, n, _ptr(out), _stream()))
         return out
 
-    def ssr_restore_varlen(self, wav_packed: torch.Tensor, lengths, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def ssr_restore_varlen(self, wav_packed: torch.Tensor, lengths, out: Optional[torch.Tensor] = None,
+                           mel_out: Optional[torch.Tensor] = None, peak_normalise: bool = False) -> torch.Tensor:
         """restore_varlen for the SSR / GSR-UNet path (vf_ssr_restore_varlen): clip i of the packed result is bit-identical
-        to ssr_forward(None, clip_i[None])[0]."""
+        to ssr_forward(None, clip_i[None])[0].
+        mel_out ([sum(frames_for(n_i)), 128] or None) and peak_normalise (vf_ssr_restore_varlen_mels): clip i's linear mel
+        of that output lands in rows sum_{j<i} frames_for(n_j) onwards, the bits frontend() gives on it; then, with
+        peak_normalise, clip i is divided by its max |x| when that exceeds 1, the bits of finalize(out_i[None], n_i)."""
         wav_packed, offsets = self._varlen_args(wav_packed, lengths)
         out = torch.empty_like(wav_packed) if out is None else out
+        if mel_out is not None:
+            rows = sum(frames_for(offsets[i + 1] - offsets[i]) for i in range(len(offsets) - 1))
+            _check_in(mel_out, self.device, "mel_out")
+            if not mel_out.is_contiguous() or tuple(mel_out.shape) != (rows, 128):
+                raise ValueError(f"mel_out must be a contiguous [{rows}, 128] tensor (the clips' frames, packed)")
+        flags = L.VF_SSR_PEAK_NORMALISE if peak_normalise else 0
         with torch.cuda.device(self.device):
-            self._ck(self.lib.vf_ssr_restore_varlen(self.ctx, _ptr(wav_packed), offsets, len(offsets) - 1, _ptr(out), _stream()))
+            self._ck(self.lib.vf_ssr_restore_varlen_mels(self.ctx, _ptr(wav_packed), offsets, len(offsets) - 1, _ptr(out),
+                                                         flags, _ptr(mel_out), _stream()))
         return out
 
     def ssr_restore_host(self, wav_host: torch.Tensor, out_host: torch.Tensor):
