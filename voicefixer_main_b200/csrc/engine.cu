@@ -479,12 +479,18 @@ int run_sub_batches(vf_ctx* ctx, int kind, int batch, Frames frames, F body, int
 }
 
 // Argument checks of a varlen entry point (`fn`) on plans of `kind`, all before anything is launched, so a rejected call
-// leaves no partial output and no work queued: offsets[0] == 0, the networks, then every clip (offsets increase, more than
-// n_fft/2 samples, at most 2^30, and per_clip(i, n) for checks of the entry point's own).
+// leaves no partial output and no work queued: a ready context, the pointers and batch, no flag bits outside `known_flags`,
+// offsets[0] == 0, the networks, then every clip (offsets increase, more than n_fft/2 samples, at most 2^30, and
+// per_clip(i, n) for checks of the entry point's own).
 template <typename F>
-int check_varlen_call(vf_ctx* ctx, const char* fn, int kind, const int64_t* offsets, int batch, F per_clip) {
+int check_varlen_call(vf_ctx* ctx, const char* fn, int kind, const float* wav, const int64_t* offsets, int batch,
+                      const float* wav_out, unsigned flags, unsigned known_flags, F per_clip) {
+  int rc = check_ready(ctx);
+  if (rc) return rc;
+  if (!wav || !wav_out || !offsets || batch <= 0) return fail(ctx, VF_EINVAL, "%s: bad arguments", fn);
+  if (flags & ~known_flags) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
   if (offsets[0] != 0) return fail(ctx, VF_EINVAL, "%s: offsets[0] must be 0 (got %ld)", fn, (long)offsets[0]);
-  int rc = check_networks(ctx, kind);
+  rc = check_networks(ctx, kind);
   if (rc) return rc;
   for (int i = 0; i < batch; ++i) {
     const int64_t n = offsets[i + 1] - offsets[i];
@@ -522,18 +528,28 @@ std::vector<int64_t> frame_offsets(vf_ctx* ctx, const int64_t* offsets, int batc
   return f;
 }
 
+// One launch that gathers rows t < T_i of the sub-batch's [b, plan->T, 128] mel / logmel (either may be null with its
+// output) into the packed outputs at the frame offsets frame_off[s .. s + b] of its clips.
+int gather_mels(vf_ctx* ctx, const Plan* plan, const std::vector<int64_t>& frame_off, int s, int b, const float* mel,
+                const float* logmel, float* mel_out, float* logmel_out, cudaStream_t st) {
+  MelGatherParams g;
+  memset(&g, 0, sizeof g);
+  g.mel = mel; g.logmel = logmel; g.mel_out = mel_out; g.logmel_out = logmel_out;
+  g.batch = b; g.T = plan->T;
+  for (int i = 0; i <= b; ++i) g.frame_off[i] = frame_off[s + i];
+  CK(launch_gather_mels(g, st));
+  ctx->launches++;
+  return VF_OK;
+}
+
 // vf_restore_varlen (`fn`) and vf_restore_varlen_mels.  With mel_out or log_mel_out, each sub-batch's restore is followed by
 // one gather of its clips' rows t < T_i into the packed outputs at frame offsets F_i = sum_{j<i} T_j, still inside the
 // plan's use on `stream` (plan_exit again after it).
 int restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t* offsets, int batch, float* wav_out,
                    unsigned flags, float* mel_out, float* log_mel_out, cudaStream_t st) {
-  int rc = check_ready(ctx);
-  if (rc) return rc;
-  if (!wav || !wav_out || !offsets || batch <= 0) return fail(ctx, VF_EINVAL, "%s: bad arguments", fn);
-  if (flags & ~(unsigned)VF_RESTORE_UNIFY_ENERGY) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
-  long scale = 1;
-  for (int s = 0; s < ctx->cfg.voc_num_stages; ++s) scale *= ctx->cfg.voc_scales[s];
-  rc = check_varlen_call(ctx, fn, PLAN_VARLEN, offsets, batch, [&](int i, int64_t n) {
+  int rc = check_varlen_call(ctx, fn, PLAN_VARLEN, wav, offsets, batch, wav_out, flags, VF_RESTORE_UNIFY_ENERGY, [&](int i, int64_t n) {
+    long scale = 1;
+    for (int s = 0; s < ctx->cfg.voc_num_stages; ++s) scale *= ctx->cfg.voc_scales[s];
     const int T = frames_of(ctx, (long)n);
     const long d = (long)(T + T % 2 + ctx->cfg.voc_tail_base) * scale - (long)n;
     if (d < 0 || d == 1) return fail(ctx, VF_EINVAL, "clip %d: vocoder output length %ld incompatible with input %ld (trim_center)", i, (long)n + d, (long)n);
@@ -545,13 +561,8 @@ int restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t*
   return run_varlen_sub_batches(ctx, PLAN_VARLEN, offsets, batch, [&](Plan* plan, int s, int b, const int64_t* rel, int64_t n_max) {
     int r = restore_impl(ctx, plan, wav + offsets[s], b, n_max, wav_out + offsets[s], flags, st, rel);
     if (r || !mels) return r;
-    MelGatherParams g;
-    memset(&g, 0, sizeof g);
-    g.mel = plan->d_mel; g.logmel = plan->d_logmel_out; g.mel_out = mel_out; g.logmel_out = log_mel_out;
-    g.batch = b; g.T = plan->T;
-    for (int i = 0; i <= b; ++i) g.frame_off[i] = frame_off[s + i];
-    CK(launch_gather_mels(g, st));
-    ctx->launches++;
+    r = gather_mels(ctx, plan, frame_off, s, b, plan->d_mel, plan->d_logmel_out, mel_out, log_mel_out, st);
+    if (r) return r;
     return plan_exit(ctx, plan, st);
   });
 }
@@ -561,11 +572,8 @@ int restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t*
 // VF_SSR_PEAK_NORMALISE, the per-clip peak normalise of wav_out, after the mel is taken.
 int ssr_restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t* offsets, int batch, float* wav_out,
                        unsigned flags, float* mel_out, cudaStream_t st) {
-  int rc = check_ready(ctx);
-  if (rc) return rc;
-  if (!wav || !wav_out || !offsets || batch <= 0) return fail(ctx, VF_EINVAL, "%s: bad arguments", fn);
-  if (flags & ~(unsigned)VF_SSR_PEAK_NORMALISE) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
-  rc = check_varlen_call(ctx, fn, PLAN_SSR_VARLEN, offsets, batch, [](int, int64_t) { return VF_OK; });
+  int rc = check_varlen_call(ctx, fn, PLAN_SSR_VARLEN, wav, offsets, batch, wav_out, flags, VF_SSR_PEAK_NORMALISE,
+                             [](int, int64_t) { return VF_OK; });
   if (rc) return rc;
   const bool peak = (flags & VF_SSR_PEAK_NORMALISE) != 0;
   const std::vector<int64_t> frame_off = mel_out ? frame_offsets(ctx, offsets, batch) : std::vector<int64_t>();
@@ -578,12 +586,8 @@ int ssr_restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int6
       // has run, so they hold the mels at the bucket's row stride ([b, T, 128] of the [b, T, 2048] buffer).
       r = run_frontend(ctx, out, b, (long)n_max, plan->d_frames, nullptr, nullptr, nullptr, nullptr, st, plan);
       if (r) return r;
-      MelGatherParams g;
-      memset(&g, 0, sizeof g);
-      g.mel = plan->d_frames; g.mel_out = mel_out; g.batch = b; g.T = plan->T;
-      for (int i = 0; i <= b; ++i) g.frame_off[i] = frame_off[s + i];
-      CK(launch_gather_mels(g, st));
-      ctx->launches++;
+      r = gather_mels(ctx, plan, frame_off, s, b, plan->d_frames, nullptr, mel_out, nullptr, st);
+      if (r) return r;
     }
     if (peak) {
       CK(cudaMemsetAsync(plan->d_peak, 0, (size_t)b * sizeof(unsigned int), st));

@@ -94,17 +94,13 @@ def restore_array(mdl: VoiceFixer, wav_10k: np.ndarray, device, unify_energy: bo
     signal, same rate) the mel metrics of the LAST segment land in `metrics`, as the reference's loop leaves them
     (eval_gsr_voicefixer.py:56-64 overwrites the dict every segment)."""
     res = []
-    break_point = SEG_LENGTH
-    n = wav_10k.shape[0]
-    while break_point < n + SEG_LENGTH:
-        segment = wav_10k[break_point - SEG_LENGTH:break_point]
-        seg = torch.from_numpy(np.ascontiguousarray(segment))[None, :].to(device)
+    for s, e in segment_bounds(wav_10k.shape[0]):
+        seg = torch.from_numpy(np.ascontiguousarray(wav_10k[s:e]))[None, :].to(device)
         res.append(mdl.restore(seg, unify_energy=unify_energy))
         if target is not None and metrics is not None:
-            tseg = torch.from_numpy(np.ascontiguousarray(target[break_point - SEG_LENGTH:break_point]))[None, None, :].to(device)
+            tseg = torch.from_numpy(np.ascontiguousarray(target[s:s + SEG_LENGTH]))[None, None, :].to(device)
             mel_noisy, log_mel = mdl._engine().restore_stages(1, seg.shape[1])
             metrics.update(_mel_metrics(mdl, tseg, mel_noisy[:, None], log_mel[:, None], unify_energy, mel_ssim))
-        break_point += SEG_LENGTH
     return torch.cat(res, -1)
 
 
@@ -130,7 +126,8 @@ def _mel_metrics(mdl: VoiceFixer, tseg, mel_noisy, log_mel, unify_energy: bool, 
 
 
 def segment_bounds(n):
-    """(start, end) of the segments restore_array cuts a file of n samples into: SEG_LENGTH each, the last one ragged."""
+    """(start, end) of the segments of a file of n samples, as the reference's break_point loop cuts them
+    (eval_gsr_voicefixer.py:47-74): SEG_LENGTH each, the last one ragged.  A segment's target slice is [start, start + SEG_LENGTH)."""
     return [(bp - SEG_LENGTH, min(bp, n)) for bp in range(SEG_LENGTH, n + SEG_LENGTH, SEG_LENGTH)]
 
 
@@ -191,6 +188,21 @@ def handler_batch(items, ckpt, device, needrefresh=False, meta={}):
     global model
     model = model.to(device)
     eng = model._engine()
+    unify, mel_ssim = bool(meta.get("unify_energy", False)), bool(meta.get("mel_ssim", False))
+    return restore_test_set(
+        model, items, 2, mel_ssim, bool(meta.get("saturate", False)),
+        lambda x, lengths, mel, log_mel: eng.restore_varlen(x, lengths, unify_energy=unify, mel_out=mel, log_mel_out=log_mel),
+        lambda tseg, mel, log_mel: _mel_metrics(model, tseg, mel, log_mel, unify, mel_ssim))
+
+
+def restore_test_set(mdl, items, n_mels, mel_ssim, saturate, restore, score):
+    """The body of handler_batch and handler_unet.handler_batch, which differ only in `restore` and `score`: the list of
+    handler()'s dicts for `items`, and handler()'s output files, from batched restores.  Every item is decoded and checked
+    (_check_file, with `mel_ssim`) before any GPU work.  Segments go longest first through
+    restore(packed, lengths, *mel_bufs) -> the packed restored samples, where mel_bufs are `n_mels` packed [rows, 128]
+    outputs when some item has a target and Nones otherwise.  score(tseg, *mels) -> dict scores a file's last segment: tseg
+    [1, 1, n] its target slice on the device, mels its [1, 1, T, 128] rows of each buffer.  Files are written last."""
+    eng = mdl._engine()
     items = [tuple(it) for it in items]
     if not items:
         return []
@@ -198,14 +210,13 @@ def handler_batch(items, ckpt, device, needrefresh=False, meta={}):
     for inp, _, tgt in items:
         x = read_pcm16(inp)
         t = read_pcm16(tgt) if tgt is not None else None
-        _check_file(inp, _rate_len(len(x[0]), x[1]), None if t is None else _rate_len(len(t[0]), t[1]),
-                    mel_ssim=bool(meta.get("mel_ssim", False)))
+        _check_file(inp, _rate_len(len(x[0]), x[1]), None if t is None else _rate_len(len(t[0]), t[1]), mel_ssim=mel_ssim)
         decoded.append((x, t))
     sigs = [_to_rate(inp, *x, 44100, eng) for (inp, _, _), (x, _) in zip(items, decoded)]
     tgts = [None if t is None else _to_rate(tgt, *t, 44100, eng) for (_, _, tgt), (_, t) in zip(items, decoded)]
     segs = [(f, s, e) for f, x in enumerate(sigs) for s, e in segment_bounds(len(x))]    # (file, start, end), file order
-    unify, want_mels = bool(meta.get("unify_energy", False)), any(t is not None for t in tgts)
-    pcm, mels = [None] * len(segs), [None] * len(segs)   # per segment: int16 samples; (mel, log_mel) [1, 1, T, 128] views
+    want_mels = any(t is not None for t in tgts)
+    pcm, mels = [None] * len(segs), [None] * len(segs)   # per segment: int16 samples; its [1, 1, T, 128] mel views
     # Full 60 s segments get a call of their own.  A call's longest clip sizes all of its sub-batches (plan budget), and a
     # 60 s segment needs the plan memory of about six 10 s clips: next to short clips it would cap every sub-batch at a few
     # clips, each sub-batch a plan of its own shape.
@@ -218,29 +229,27 @@ def handler_batch(items, ckpt, device, needrefresh=False, meta={}):
         lengths = [segs[k][2] - segs[k][1] for k in order]
         off = np.concatenate([[0], np.cumsum(lengths)])
         f_off = np.concatenate([[0], np.cumsum([frames_for(n) for n in lengths])])
-        packed = torch.from_numpy(np.concatenate([sigs[f][s:e] for f, s, e in (segs[k] for k in order)])).to(model.device)
-        mel = torch.empty(int(f_off[-1]), 128, device=model.device) if want_mels else None
-        log_mel = torch.empty_like(mel) if want_mels else None
-        out = eng.restore_varlen(packed, lengths, unify_energy=unify, mel_out=mel, log_mel_out=log_mel)
+        packed = torch.from_numpy(np.concatenate([sigs[f][s:e] for f, s, e in (segs[k] for k in order)])).to(mdl.device)
+        bufs = [torch.empty(int(f_off[-1]), 128, device=mdl.device) if want_mels else None for _ in range(n_mels)]
+        out = restore(packed, lengths, *bufs)
         # to_pcm16 is elementwise: one conversion of the packed output gives every file the bytes of its own conversion
-        out16 = eng.to_pcm16(out, saturate=bool(meta.get("saturate", False))).cpu().numpy()
+        out16 = eng.to_pcm16(out, saturate=saturate).cpu().numpy()
         for p, k in enumerate(order):
             pcm[k] = out16[off[p]:off[p + 1]]
             if want_mels:
-                rows = slice(int(f_off[p]), int(f_off[p + 1]))
-                mels[k] = (mel[rows][None, None], log_mel[rows][None, None])
+                mels[k] = [b[int(f_off[p]):int(f_off[p + 1])][None, None] for b in bufs]
     file_segs = [[] for _ in items]
     for k, (f, _, _) in enumerate(segs):
         file_segs[f].append(k)
     results = []
-    for f, tgt in enumerate(tgts):                 # restore_array leaves the metrics of a file's last segment
+    for f, tgt in enumerate(tgts):                 # handler() leaves the metrics of a file's last segment
         if tgt is None:
             results.append({})
             continue
         k = file_segs[f][-1]
         s = segs[k][1]
-        tseg = torch.from_numpy(np.ascontiguousarray(tgt[s:s + SEG_LENGTH]))[None, None, :].to(model.device)
-        results.append(_mel_metrics(model, tseg, *mels[k], unify, bool(meta.get("mel_ssim", False))))
+        tseg = torch.from_numpy(np.ascontiguousarray(tgt[s:s + SEG_LENGTH]))[None, None, :].to(mdl.device)
+        results.append(score(tseg, *mels[k]))
     for (_, output, _), ks in zip(items, file_segs):
         save_pcm16(np.concatenate([pcm[k] for k in ks]), fname=output, sample_rate=44100)
     return results

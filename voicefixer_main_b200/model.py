@@ -214,12 +214,7 @@ class Engine:
         restore(clip_i[None])."""
         wav_packed, offsets = self._varlen_args(wav_packed, lengths)
         out = torch.empty_like(wav_packed) if out is None else out
-        rows = sum(frames_for(offsets[i + 1] - offsets[i]) for i in range(len(offsets) - 1))
-        for name, t in (("mel_out", mel_out), ("log_mel_out", log_mel_out)):
-            if t is not None:
-                _check_in(t, self.device, name)
-                if not t.is_contiguous() or tuple(t.shape) != (rows, 128):
-                    raise ValueError(f"{name} must be a contiguous [{rows}, 128] tensor (the clips' frames, packed)")
+        self._packed_rows(offsets, mel_out=mel_out, log_mel_out=log_mel_out)
         flags = L.VF_RESTORE_UNIFY_ENERGY if unify_energy else 0
         with torch.cuda.device(self.device):
             self._ck(self.lib.vf_restore_varlen_mels(self.ctx, _ptr(wav_packed), offsets, len(offsets) - 1, _ptr(out), flags,
@@ -233,6 +228,17 @@ class Engine:
         if wav_packed.dim() != 1 or not lengths or sum(lengths) != wav_packed.numel():
             raise ValueError("wav_packed must be 1-D and hold exactly sum(lengths) samples of at least one clip")
         return wav_packed, (ctypes.c_int64 * (len(lengths) + 1))(0, *itertools.accumulate(lengths))
+
+    def _packed_rows(self, offsets, **outs) -> int:
+        """Rows sum_i frames_for(n_i) of a varlen call's packed per-frame outputs (clip i from row sum_{j<i} frames_for(n_j));
+        checks that each output of `outs` (name -> tensor or None) is a contiguous [rows, 128] float32 tensor on the device."""
+        rows = sum(frames_for(offsets[i + 1] - offsets[i]) for i in range(len(offsets) - 1))
+        for name, t in outs.items():
+            if t is not None:
+                _check_in(t, self.device, name)
+                if not t.is_contiguous() or tuple(t.shape) != (rows, 128):
+                    raise ValueError(f"{name} must be a contiguous [{rows}, 128] tensor (the clips' frames, packed)")
+        return rows
 
     def mel(self, specgram: torch.Tensor) -> torch.Tensor:
         """MelScale.forward: specgram [..., 1025, time] (any strides) -> [..., 128, time]."""
@@ -253,7 +259,7 @@ class Engine:
         """vf_metric_spectrogram: |librosa.stft(n_fft=2048, hop_length=441)| of each clip of wav_packed (clips back to back,
         `lengths` samples each) -> (sp [sum T_i, 1025], mel [sum T_i, 128] or None), clip i at rows sum_{j<i} T_i."""
         wav_packed, offsets = self._varlen_args(wav_packed, lengths)
-        rows = sum(frames_for(offsets[i + 1] - offsets[i]) for i in range(len(offsets) - 1))
+        rows = self._packed_rows(offsets)
         sp = torch.empty(rows, 1025, device=self.device)
         mel = torch.empty(rows, 128, device=self.device) if want_mel else None
         with torch.cuda.device(self.device):
@@ -325,11 +331,7 @@ class Engine:
         peak_normalise, clip i is divided by its max |x| when that exceeds 1, the bits of finalize(out_i[None], n_i)."""
         wav_packed, offsets = self._varlen_args(wav_packed, lengths)
         out = torch.empty_like(wav_packed) if out is None else out
-        if mel_out is not None:
-            rows = sum(frames_for(offsets[i + 1] - offsets[i]) for i in range(len(offsets) - 1))
-            _check_in(mel_out, self.device, "mel_out")
-            if not mel_out.is_contiguous() or tuple(mel_out.shape) != (rows, 128):
-                raise ValueError(f"mel_out must be a contiguous [{rows}, 128] tensor (the clips' frames, packed)")
+        self._packed_rows(offsets, mel_out=mel_out)
         flags = L.VF_SSR_PEAK_NORMALISE if peak_normalise else 0
         with torch.cuda.device(self.device):
             self._ck(self.lib.vf_ssr_restore_varlen_mels(self.ctx, _ptr(wav_packed), offsets, len(offsets) - 1, _ptr(out),
