@@ -302,10 +302,64 @@ VF_API int vf_op_count(vf_ctx* ctx);
 VF_API int vf_op_info(vf_ctx* ctx, int i, float* ms, double* flops, double* bytes, int* bn, int* bk, int* terms,
                       char* label, int label_cap, double* exec_flops /* nullable: tensor-core flops actually issued */);
 
-/* Self-test of one flat-shift GEMM configuration: random fp16 hi/lo planes through the wgmma kernel and
- * the SIMT validation kernel; returns max |difference| and max |value|.  Synchronous. */
-VF_API int vf_selftest_gemm(vf_ctx* ctx, int n_img, int rows, int cin, int cout, int ntaps, int dilation, int terms,
-                     double* max_abs_diff, double* max_abs_ref);
+/* TEST ONLY.  One conv layer built the way the plans build it (the product's weight packers and tap lists, the plan
+ * builder's GEMM / fused-pair set-up), run once and copied back.  Synchronous; every pointer is a host pointer.
+ * Activation operands are fp16 bit patterns in the kernels' layout: [plane (hi, lo)][n_img][img_rows][C], rows of a 2-D
+ * layer flattened (h, w) with one pad column (row pitch W + 1).  Output buffers are read AND written: they are uploaded
+ * before the launch, so what the layer must not touch comes back unchanged. */
+enum { VF_LAYER_CONV2D = 0, VF_LAYER_CONVT2D = 1, VF_LAYER_CONV1D = 2, VF_LAYER_CONVT1D = 3, VF_LAYER_PAIR = 4 };
+enum { VF_LAYER_PRODUCT = 0, VF_LAYER_SIMT = 1 };
+enum { VF_RESID_NONE = 0, VF_RESID_FP32 = 1, VF_RESID_PLANES = 2, VF_RESID_AR = 3, VF_RESID_IDENTITY = 4 };
+typedef struct vf_layer_case {
+  int kind, impl, terms;    /* VF_LAYER_*, VF_LAYER_PRODUCT / SIMT (no (a, r) support: VF_EINVAL), 1 or 3 */
+  int n_img;
+  int H, W;                 /* CONV2D / CONVT2D input pixels; GEMM rows per image H * (W + 1) */
+  int L;                    /* CONV1D / CONVT1D / PAIR input rows per image */
+  int cin, cout, sc_cin;    /* sc_cin: CONV2D 1x1 shortcut source channels, 0 = none */
+  int k, dilation, centered;   /* CONV1D */
+  int stride;               /* CONVT1D: stride s, padding s / 2 + s % 2 */
+  int both;                 /* CONVT2D: 1 = prune time and frequency (output pitch 2 (W + 1) - 1), 0 = time only */
+  /* PyTorch layouts, fp32: w [cout][cin][3][3] / [cin][cout][3][3] / [cout][cin][k] / [cin][cout][2 s]; PAIR: w, b = conv_a, w2, b2 = conv_b */
+  const float* w;
+  const float* b;           /* [cout] or NULL */
+  const float* sc_w;        /* [cout][sc_cin] */
+  const float* sc_b;        /* [cout] */
+  const float* w2;
+  const float* b2;
+  const uint16_t* x;        /* [2][n_img][x_img_rows][cin]; rows [x_row0, x_img_rows) of each image are the layer's input
+                               (PAIR: the (a, r) planes of x) */
+  int x_img_rows, x_row0;
+  const uint16_t* sc_x;     /* [2][n_img][rows][sc_cin] */
+  int resid_kind;           /* VF_RESID_*: FP32 [n_img][rows][cout] floats; PLANES / AR / IDENTITY [2][n_img][rows][cout] fp16 */
+  const void* resid;
+  float ar_slope;           /* AR (input and output streams): the LeakyReLU slope whose fp16 inverse the stream uses */
+  float* out_raw;           /* [n_img][out_img_rows][raw_ld] or NULL */
+  int raw_ld;
+  uint16_t* out_r;          /* [2][n_img][out_img_rows][r_ld] or NULL */
+  int r_ld, r_c_off;
+  uint16_t* out_a;          /* [2][n_img][out_img_rows][a_ld] or NULL: act(scale * v + shift) */
+  int a_ld, a_c_off;
+  int out_ar;               /* out_a is written as the (a, r) pair of x itself (1-term, LeakyReLU ar_slope, no affine) */
+  const float* a_scale;     /* [cout] or NULL */
+  const float* a_shift;
+  int act;                  /* 0 none, 1 LeakyReLU (slope), 2 ELU */
+  float slope;
+  int out_row0, out_img_rows;
+  const float* head_w;      /* [32]: fused 1x1 head of a 32-channel CONV2D, or NULL */
+  float head_b;
+  const float* head_in;     /* [n_img][head_T][W + 1] or NULL */
+  float* head_out;          /* [n_img][head_T][W + 1] */
+  int head_T;
+  const int* row_valid;     /* [n_img] or NULL */
+  const int* head_valid;    /* [n_img] or NULL */
+  float pair_slope_h, pair_slope_out;   /* PAIR: activation of h, and of x_new (the stage slope after the last pair) */
+  int pair_last;            /* PAIR: no correction plane out (last pair of a stack) */
+  /* reported: the launch configuration the builder chose */
+  int bn, bk, stages, resid_tma, tma_out, grid;
+  int64_t tiles;
+  int div_fallback;         /* a tile decode divides (its multiply-high magic would not be exact) */
+} vf_layer_case;
+VF_API int vf_selftest_layer(vf_ctx* ctx, vf_layer_case* lc);
 
 #ifdef __cplusplus
 }

@@ -21,30 +21,6 @@ def model(state):
     m._engine().check_errors()
 
 
-# ------------------------------------------------------------------ tensor-core (wgmma) GEMM vs SIMT validation kernel
-GEMM_CASES = [
-    # n_img, rows, cin, cout, ntaps, dilation        (BN, BK) exercised
-    (2, 300, 32, 32, 9, 1),      # (32, 32)  SW64
-    (1, 128, 32, 64, 3, 1),      # (64, 32)
-    (1, 257, 32, 128, 1, 1),     # (128, 32)
-    (2, 200, 64, 32, 3, 1),      # (32, 64)  SW128
-    (1, 129, 64, 64, 9, 1),      # (64, 64)
-    (2, 500, 128, 128, 3, 27),   # (128, 64), dilated taps, OOB rows
-    (3, 40, 384, 384, 9, 2),     # tiny image, 3 N tiles, long K
-    (1, 1000, 64, 192, 2, 1),    # N = 192 -> BN 64
-    (2, 700, 128, 512, 3, 3),    # terms = 1 -> BN 128, terms = 3 -> BN 64
-]
-
-
-@pytest.mark.parametrize("case", GEMM_CASES)
-@pytest.mark.parametrize("terms", [3, 1])
-def test_gemm_tcgen05_matches_simt(model, case, terms):
-    diff, ref = model._engine().selftest_gemm(*case[:5], dilation=case[5], terms=terms)
-    model._engine().check_errors()
-    assert ref > 0.1
-    assert diff <= 2e-5 * ref, (case, terms, diff, ref)
-
-
 # ------------------------------------------------------------------ stage A
 @pytest.mark.parametrize("name", ["stage_a_n4410.npz", "stage_a_n30001.npz"])
 def test_frontend_matches_reference_golden(model, name):

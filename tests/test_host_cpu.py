@@ -157,15 +157,12 @@ def test_ar_residual_stream_arithmetic_keeps_22_bits():
     U(a) = min(a, a * fp16(1/s)) evaluated in fp16 (csrc/ptx.cuh ar_unact / ar_split).  Restated in numpy: U(a) + r recovers
     x to ~2^-21 relative - the precision of a hi/lo split of x itself - for every slope the engine accepts."""
     import numpy as np
+    from oracle.layers import ar_decode, ar_encode
     rng = np.random.default_rng(5)
     x = np.concatenate([rng.standard_normal(200000) * 3.0, rng.standard_normal(1000) * 1e-4, [0.0, -0.0, 65000.0, -65000.0]]).astype(np.float32)
     for s in (0.1, 0.2, 0.01, 1.0):
-        inv = np.float16(1.0 / s)
-        a = np.maximum(x, x * np.float32(s)).astype(np.float16)                      # fmaxf(v, v * slope) -> fp16
-        with np.errstate(over="ignore"):                                              # a * inv may overflow to +inf: min() keeps a
-            u = np.minimum(a, (a * inv).astype(np.float16))                          # __hmin2(a, __hmul2(a, inv))
-        r = (x - u.astype(np.float32)).astype(np.float16)                            # FHADD + pack
-        back = u.astype(np.float32) + r.astype(np.float32)
+        a, r = ar_encode(x, s)
+        back = ar_decode(a, r, s).astype(np.float32)
         hi = x.astype(np.float16)
         lo = (x - hi.astype(np.float32)).astype(np.float16)
         err_ar = np.abs(back - x)

@@ -17,7 +17,7 @@ EXPORTS = [
     "vf_default_config", "vf_create", "vf_destroy", "vf_last_error", "vf_load_weights", "vf_frontend",
     "vf_unet_mel", "vf_vocoder", "vf_vocoder_out_len", "vf_restore", "vf_restore_host", "vf_restore_stages",
     "vf_to_log", "vf_from_log", "vf_to_pcm16", "vf_workspace_bytes", "vf_check_errors", "vf_set_option", "vf_launch_count",
-    "vf_enable_stage_timing", "vf_stage_times", "vf_selftest_gemm", "vf_enable_op_timing", "vf_op_count", "vf_op_info",
+    "vf_enable_stage_timing", "vf_stage_times", "vf_selftest_layer", "vf_enable_op_timing", "vf_op_count", "vf_op_info",
     "vf_restore_ex", "vf_ssr_forward", "vf_ssr_restore", "vf_ssr_restore_host", "vf_ssr_unet", "vf_ssr_stages", "vf_istft",
     "vf_mel", "vf_finalize", "vf_plan_cache_info", "vf_resample_poly", "vf_lsd", "vf_sispec", "vf_to_pcm16_ex", "vf_amp_to_original_f",
     "vf_restore_varlen", "vf_ssr_restore_varlen", "vf_restore_varlen_mels", "vf_metric_spectrogram", "vf_ssim", "vf_score_varlen",
@@ -40,6 +40,22 @@ class VfConfig(Structure):
 class VfTensorDesc(Structure):
     _fields_ = [("name", c_char_p), ("data", c_void_p), ("ndim", c_int), ("shape", c_int64 * 4),
                 ("on_device", c_int)]
+
+
+class VfLayerCase(Structure):
+    """vf_layer_case (include/b200vf.h): one conv layer for vf_selftest_layer (tests only)."""
+    _fields_ = [(f, c_int) for f in ("kind", "impl", "terms", "n_img", "H", "W", "L", "cin", "cout", "sc_cin", "k",
+                                      "dilation", "centered", "stride", "both")] + \
+               [(f, c_void_p) for f in ("w", "b", "sc_w", "sc_b", "w2", "b2", "x")] + \
+               [("x_img_rows", c_int), ("x_row0", c_int), ("sc_x", c_void_p), ("resid_kind", c_int), ("resid", c_void_p),
+                ("ar_slope", c_float), ("out_raw", c_void_p), ("raw_ld", c_int), ("out_r", c_void_p), ("r_ld", c_int),
+                ("r_c_off", c_int), ("out_a", c_void_p), ("a_ld", c_int), ("a_c_off", c_int), ("out_ar", c_int),
+                ("a_scale", c_void_p), ("a_shift", c_void_p), ("act", c_int), ("slope", c_float), ("out_row0", c_int),
+                ("out_img_rows", c_int), ("head_w", c_void_p), ("head_b", c_float), ("head_in", c_void_p),
+                ("head_out", c_void_p), ("head_T", c_int), ("row_valid", c_void_p), ("head_valid", c_void_p),
+                ("pair_slope_h", c_float), ("pair_slope_out", c_float), ("pair_last", c_int)] + \
+               [(f, c_int) for f in ("bn", "bk", "stages", "resid_tma", "tma_out", "grid")] + \
+               [("tiles", c_int64), ("div_fallback", c_int)]
 
 
 class EngineError(RuntimeError):
@@ -89,8 +105,7 @@ def load_library():
     lib.vf_launch_count.restype = c_int64
     lib.vf_enable_stage_timing.argtypes = [P, c_int]
     lib.vf_stage_times.argtypes = [P, POINTER(c_float * 4)]
-    lib.vf_selftest_gemm.argtypes = [P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, POINTER(c_double),
-                                     POINTER(c_double)]
+    lib.vf_selftest_layer.argtypes = [P, POINTER(VfLayerCase)]
     lib.vf_enable_op_timing.argtypes = [P, c_int]
     lib.vf_op_count.argtypes = [P]
     lib.vf_op_info.argtypes = [P, c_int, POINTER(c_float), POINTER(c_double), POINTER(c_double), POINTER(c_int),

@@ -243,6 +243,11 @@ inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 int upload_gemm(vf_ctx* ctx, GemmW* w, const std::vector<float>& m, int N, int K, const std::vector<float>* bias);
 int build_tables(vf_ctx* ctx);
 int load_all(vf_ctx* ctx);
+// PyTorch weight layouts -> packed GEMM operands (upload_gemm), as the loaders pack every conv of the networks
+int pack_conv3x3(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT* sc_w, const HostT* sc_b);
+int pack_convT2d(vf_ctx* ctx, GemmW* out, const HostT& w);
+int pack_conv1d(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT& b, bool identity = false);
+int pack_convT1d(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT& b, int s);
 // Residual add of a vocoder stack as an identity tap (through the accumulator, no epilogue loads) up to this channel count;
 // above it the epilogue adds the hi/lo planes.  The packer appends the identity block and the plan builder adds the tap.
 constexpr int IDENT_MAX_C = 128;
@@ -267,6 +272,19 @@ struct Builder {
             GemmEpilogue epi, int n_img, int terms);
 };
 GemmEpilogue epi_plain(int rows_in, int Wp, int cout, int out_img_rows);
+// (a, r) residual stream (gemm.cuh): fp16(1 / slope) in both halves of a word, 0 when the LeakyReLU is not invertible that way
+uint32_t ar_inv_word(float slope);
+// Tap lists of the plans' convs: Conv2d 3x3 pad 1 on rows of pitch Wp; the four (dh, dw) input shifts of ConvTranspose2d
+// k3 s2 (pack_convT2d); Conv1d k with dilation, centred (pad (k - 1) / 2 * dil) or not (the caller pads); ConvTranspose1d
+// rows q and q - 1 (pack_convT1d)
+std::vector<GemmTap> taps3x3(int Wp, int cin);
+std::vector<GemmTap> taps_convt2d(int Wp, int cin);
+std::vector<GemmTap> taps1d(int k, int dil, int cin, bool centered);
+std::vector<GemmTap> taps_convt1d(int cin);
+// Fused residual pair (pair_tc.cu) of a C = 64 stack: src / dst hold (a, r) planes of L rows per image; dst's activated
+// plane is written from row out_row0; `last`: no correction plane out
+int pair_setup(vf_ctx* ctx, PairParams* pp, const Planes& src, const Planes& dst, const GemmW& wa, const GemmW& wb, int n_img,
+               int L, int dil, uint32_t ar, bool last, int out_row0, float slope_h, float slope_out, const int* row_valid);
 int build_plan(vf_ctx* ctx, Plan* plan);
 
 }  // namespace vf

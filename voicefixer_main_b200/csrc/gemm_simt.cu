@@ -1,6 +1,6 @@
 // SIMT fp32 implementation of the flat-shift multi-tap GEMM contract (gemm.cuh).
 // VALIDATION KERNEL: it exists so every tensor-core GEMM launch can be cross-checked element by element on the
-// device (vf_selftest_gemm, and whole plans under the option validate_simt); the product path always runs gemm_tc.cu.
+// device (vf_selftest_layer, and whole plans under the option validate_simt); the product path always runs gemm_tc.cu.
 // One thread per output row, 32 output columns per pass; the weight tile is staged in shared memory as
 // fp32 (hi + lo), the activation row is read straight from the hi/lo planes.
 #include "gemm.cuh"

@@ -100,6 +100,7 @@ int upload_bn(vf_ctx* ctx, const std::string& p, Affine* a) {
   return upload(ctx, &a->shift, h);
 }
 
+}  // namespace
 
 // Conv2d 3x3 [Cout][Cin][3][3] (+ optional 1x1 shortcut [Cout][Csc]) -> [Cout][9*Cin + pad64(Csc)]
 int pack_conv3x3(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT* sc_w, const HostT* sc_b) {
@@ -138,7 +139,7 @@ int pack_convT2d(vf_ctx* ctx, GemmW* out, const HostT& w) {
 
 // Conv1d [Cout][Cin][k] -> [Cout][k*Cin (+ Cout)]; with `identity` an identity block is appended so the
 // residual stream x (kept as fp16 hi/lo planes) is added inside the same accumulator: x' = x + conv(...)
-int pack_conv1d(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT& b, bool identity = false) {
+int pack_conv1d(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT& b, bool identity) {
   const int cout = (int)w.shape[0], cin = (int)w.shape[1], k = (int)w.shape[2];
   const int K = k * cin + (identity ? cout : 0);
   std::vector<float> m((size_t)cout * K, 0.f);
@@ -165,6 +166,8 @@ int pack_convT1d(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT& b, int s)
     }
   return upload_gemm(ctx, out, m, N, K, &bias);
 }
+
+namespace {
 
 int load_block(vf_ctx* ctx, const std::string& p, ConvBlockW* blk, bool skip_conv1) {
   NEED(w1, p + ".conv1.weight");

@@ -259,6 +259,66 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
   ops.push_back(op);
 }
 
+uint32_t ar_inv_word(float slope) {
+  if (!(slope > 0.f && slope <= 1.f)) return 0;
+  const __half h = __float2half(1.f / slope);
+  const uint32_t b = *reinterpret_cast<const unsigned short*>(&h);
+  return b == 0x7c00u ? 0u : (b | (b << 16));
+}
+
+std::vector<GemmTap> taps3x3(int Wp, int cin) {
+  std::vector<GemmTap> t;
+  for (int kh = 0; kh < 3; ++kh)
+    for (int kw = 0; kw < 3; ++kw) t.push_back(GemmTap{(kh - 1) * Wp + (kw - 1), 0, 0, 0, cin});
+  return t;
+}
+std::vector<GemmTap> taps_convt2d(int Wp, int cin) {
+  std::vector<GemmTap> t;
+  for (int dh = 0; dh < 2; ++dh)
+    for (int dw = 0; dw < 2; ++dw) t.push_back(GemmTap{-(dh * Wp + dw), 0, 0, 0, cin});
+  return t;
+}
+std::vector<GemmTap> taps1d(int k, int dil, int cin, bool centered) {
+  std::vector<GemmTap> t;
+  for (int i = 0; i < k; ++i) t.push_back(GemmTap{centered ? (i - (k - 1) / 2) * dil : i, 0, 0, 0, cin});
+  return t;
+}
+std::vector<GemmTap> taps_convt1d(int cin) { return {GemmTap{0, 0, 0, 0, cin}, GemmTap{-1, 0, 0, 0, cin}}; }
+
+int pair_setup(vf_ctx* ctx, PairParams* pp, const Planes& src, const Planes& dst, const GemmW& wa, const GemmW& wb, int n_img,
+               int L, int dil, uint32_t ar, bool last, int out_row0, float slope_h, float slope_out, const int* row_valid) {
+  memset(pp, 0, sizeof *pp);
+  const int C = wa.N;
+  int rc = map_a(ctx, &pp->a_map, ASrc{src, L, 0}, src.p.hi, n_img, 64, false);
+  if (!rc) rc = map_weights(ctx, &pp->wa_map, wa, wa.hi, 64, C, false);
+  if (!rc) rc = map_weights(ctx, &pp->wb_map, wb, wb.hi, 64, C, false);
+  // the residual is rebuilt from the activated plane (an L2 hit: the centre tap just read these rows) and the correction
+  // plane; the new pair leaves as the two planes of `dst`
+  if (!rc) rc = map_rows(ctx, &pp->xin_map[0], src.p.hi, 2, C, L, (size_t)src.img_rows, n_img, 64, 126);
+  if (!rc) rc = map_rows(ctx, &pp->xin_map[1], src.p.lo, 2, C, L, (size_t)src.img_rows, n_img, 64, 126);
+  pp->ar_in = ar;
+  if (!rc && !last) {
+    pp->ar_out = ar;
+    rc = map_rows(ctx, &pp->xo_map, dst.p.lo, 2, C, L, (size_t)dst.img_rows, n_img, 64, 126);
+  }
+  if (!rc) rc = map_rows(ctx, &pp->ao_map, dst.p.hi, 2, C, out_row0 + L, (size_t)dst.img_rows, n_img, 64, 126);
+  if (rc) return rc;
+  pp->bias_a = wa.bias;
+  pp->bias_b = wb.bias;
+  pp->L = L; pp->n_img = n_img; pp->C = C; pp->dil = dil;
+  pp->out_img_rows = dst.img_rows;
+  pp->out_row0 = out_row0;
+  pp->tiles_per_img = (L + 125) / 126;
+  const long total_tiles = (long)n_img * pp->tiles_per_img;
+  pp->grid = (int)std::min<long>(total_tiles, (long)ctx->sm_count);      // one persistent CTA per SM (about 225 KB of shared memory)
+  pp->magic_t = gemm_tc_magic((uint32_t)pp->tiles_per_img, (uint64_t)total_tiles);
+  pp->slope_h = slope_h;
+  pp->slope_out = slope_out;
+  pp->row_valid = row_valid;
+  pp->err = ctx->d_err;
+  return VF_OK;
+}
+
 GemmEpilogue epi_plain(int rows_in, int Wp, int cout, int out_img_rows) {
   GemmEpilogue e;
   memset(&e, 0, sizeof e);
@@ -277,26 +337,12 @@ const int ENC_C[6] = {32, 64, 128, 256, 384, 384};
 const int DEC_CIN[6] = {384, 384, 384, 256, 128, 64};
 const int DEC_COUT[6] = {384, 384, 256, 128, 64, 32};
 
-// (a, r) residual stream (gemm.cuh): fp16(1 / slope) in both halves of a word, 0 when the LeakyReLU is not invertible that way
-uint32_t ar_inv_word(float slope) {
-  if (!(slope > 0.f && slope <= 1.f)) return 0;
-  const __half h = __float2half(1.f / slope);
-  const uint32_t b = *reinterpret_cast<const unsigned short*>(&h);
-  return b == 0x7c00u ? 0u : (b | (b << 16));
-}
-
 void set_out_a(GemmEpilogue& e, const Planes& pl, int c_off, const float* scale, const float* shift, int act, float slope) {
   e.out_a = OutPlane{pl.p.hi, pl.p.lo, pl.C, c_off};
   e.a_scale = scale;
   e.a_shift = shift;
   e.act = act;
   e.slope = slope;
-}
-std::vector<GemmTap> taps3x3(int Wp, int cin) {
-  std::vector<GemmTap> t;
-  for (int kh = 0; kh < 3; ++kh)
-    for (int kw = 0; kw < 3; ++kw) t.push_back(GemmTap{(kh - 1) * Wp + (kw - 1), 0, 0, 0, cin});
-  return t;
 }
 
 struct Level {
@@ -453,11 +499,8 @@ int build_unet(vf_ctx* ctx, Builder& b, Plan* plan, const UnetW& U, const UnetGe
       const ConvBlockW& blk = U.dec[k][0];
       e.out_r = OutPlane{L.cat_r.p.hi, L.cat_r.p.lo, 2 * L.C, 0};
       set_out_a(e, L.cat_a, 0, blk.bn1.scale, blk.bn1.shift, ACT_LRELU, S);
-      std::vector<GemmTap> taps;
-      for (int dh = 0; dh < 2; ++dh)
-        for (int dw = 0; dw < 2; ++dw) taps.push_back(GemmTap{-(dh * Lin.Wp + dw), 0, 0, 0, cin});
       b.label = pre + "dec" + std::to_string(k + 1) + ".convT";
-      b.gemm(ops, U.dec_up[k], ASrc{Lin.aX, Lin.rows, 0}, nullptr, taps, e, B, terms);
+      b.gemm(ops, U.dec_up[k], ASrc{Lin.aX, Lin.rows, 0}, nullptr, taps_convt2d(Lin.Wp, cin), e, B, terms);
     }
     int cur = 0;
     for (int j = 0; j < 4; ++j) {
@@ -518,11 +561,6 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
     plan->cond_op = (int)ops.size();
     ops.push_back(op);
   }
-  auto taps1d = [](int k, int dil, int cin, bool centered) {
-    std::vector<GemmTap> t;
-    for (int i = 0; i < k; ++i) t.push_back(GemmTap{centered ? (i - (k - 1) / 2) * dil : i, 0, 0, 0, cin});
-    return t;
-  };
   Planes cur = cond;
   for (int i = 0; i < c.voc_cond_layers; ++i) {
     const bool last = i == c.voc_cond_layers - 1;
@@ -578,9 +616,8 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
       if (ar) e.out_ar = ar;
       else e.out_r = OutPlane{xr[0].p.hi, xr[0].p.lo, cout, 0};
       set_out_a(e, xa, 0, nullptr, nullptr, ACT_LRELU, c.voc_res_slope);
-      std::vector<GemmTap> taps = {GemmTap{0, 0, 0, 0, cin}, GemmTap{-1, 0, 0, 0, cin}};
       b.label = "voc.up" + std::to_string(s);
-      b.gemm(ops, ctx->voc_up[s], ASrc{prev, (int)Lprev, 0}, nullptr, taps, e, B, terms);
+      b.gemm(ops, ctx->voc_up[s], ASrc{prev, (int)Lprev, 0}, nullptr, taps_convt1d(cin), e, B, terms);
     }
     int curx = 0, cura = 0;
     Planes xa2;
@@ -596,35 +633,10 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
         Op op;
         op.kind = OP_PAIR;
         PairParams& pp = op.pair;
-        memset(&pp, 0, sizeof pp);
-        int mrc = map_a(ctx, &pp.a_map, ASrc{src, (int)L, 0}, src.p.hi, B, 64, false);
-        if (!mrc) mrc = map_weights(ctx, &pp.wa_map, ctx->voc_res_a[s][i], ctx->voc_res_a[s][i].hi, 64, cout, false);
-        if (!mrc) mrc = map_weights(ctx, &pp.wb_map, ctx->voc_res_b[s][i], ctx->voc_res_b[s][i].hi, 64, cout, false);
-        // the residual is rebuilt from the activated plane (an L2 hit: the centre tap just read these rows) and the correction
-        // plane; the new pair leaves as the two planes of `dst`
-        if (!mrc) mrc = map_rows(ctx, &pp.xin_map[0], src.p.hi, 2, cout, (int)L, (size_t)src.img_rows, B, 64, 126);
-        if (!mrc) mrc = map_rows(ctx, &pp.xin_map[1], src.p.lo, 2, cout, (int)L, (size_t)src.img_rows, B, 64, 126);
-        pp.ar_in = ar;
-        if (!mrc && !last) {
-          pp.ar_out = ar;
-          mrc = map_rows(ctx, &pp.xo_map, dst.p.lo, 2, cout, (int)L, (size_t)dst.img_rows, B, 64, 126);
-        }
-        const int orow0 = (last && last_stage) ? 3 : 0;
-        if (!mrc) mrc = map_rows(ctx, &pp.ao_map, dst.p.hi, 2, cout, orow0 + (int)L, (size_t)dst.img_rows, B, 64, 126);
+        const int mrc = pair_setup(ctx, &pp, src, dst, ctx->voc_res_a[s][i], ctx->voc_res_b[s][i], B, (int)L, dil, ar, last,
+                                   (last && last_stage) ? 3 : 0, c.voc_res_slope, last ? c.voc_stage_slope : c.voc_res_slope,
+                                   plan->vl(VL_VOC + s));
         if (mrc) return mrc;
-        pp.bias_a = ctx->voc_res_a[s][i].bias;
-        pp.bias_b = ctx->voc_res_b[s][i].bias;
-        pp.L = (int)L; pp.n_img = B; pp.C = cout; pp.dil = dil;
-        pp.out_img_rows = dst.img_rows;
-        pp.out_row0 = orow0;
-        pp.tiles_per_img = (int)((L + 125) / 126);
-        const long total_tiles = (long)B * pp.tiles_per_img;
-        pp.grid = (int)std::min<long>(total_tiles, (long)ctx->sm_count);      // one persistent CTA per SM (about 225 KB of shared memory)
-        pp.magic_t = gemm_tc_magic((uint32_t)pp.tiles_per_img, (uint64_t)total_tiles);
-        pp.slope_h = c.voc_res_slope;
-        pp.slope_out = last ? c.voc_stage_slope : c.voc_res_slope;
-        pp.row_valid = plan->vl(VL_VOC + s);
-        pp.err = ctx->d_err;
         op.flops = 2.0 * 2.0 * (double)B * L * cout * 3.0 * cout;
         op.exec_flops = 2.0 * 2.0 * (double)B * pp.tiles_per_img * GEMM_BM * cout * 3.0 * cout;
         op.bytes = (double)B * L * cout * (2 + 2 + (last ? 0 : 2) + 2);    // act in (operand and residual), r in, r out, act out

@@ -460,11 +460,10 @@ class Engine:
                          "exec_flops": ex.value, "bn": bn.value, "bk": bk.value, "terms": tm.value})
         return recs
 
-    def selftest_gemm(self, n_img, rows, cin, cout, ntaps, dilation=1, terms=3):
-        d, r = ctypes.c_double(), ctypes.c_double()
-        self._ck(self.lib.vf_selftest_gemm(self.ctx, n_img, rows, cin, cout, ntaps, dilation, terms,
-                                           ctypes.byref(d), ctypes.byref(r)))
-        return d.value, r.value
+    def selftest_layer(self, case: "L.VfLayerCase"):
+        """Runs one conv layer as the plans build it (vf_selftest_layer; tests only).  Synchronous."""
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_selftest_layer(self.ctx, ctypes.byref(case)))
 
 
 # --------------------------------------------------------------------------------------------------------------
