@@ -361,6 +361,74 @@ typedef struct vf_layer_case {
 } vf_layer_case;
 VF_API int vf_selftest_layer(vf_ctx* ctx, vf_layer_case* lc);
 
+/* TEST ONLY.  One non-GEMM op of the launch chains, set up by the same helpers the plan builders and restore paths use and
+ * launched as they launch it (run_ops or the same launch_* call), then copied back.  Synchronous; every pointer is a host
+ * pointer, and output buffers are read AND written as in vf_selftest_layer.  fp16 planes are bit patterns [2][batch][rows][C].
+ * Fields a kind does not use are zero.  The mel-weight table, window and twiddles are the context's own. */
+enum { VF_OP_FIRST = 0, VF_OP_POOL = 1, VF_OP_COND = 2, VF_OP_REFLECT = 3, VF_OP_TAIL = 4, VF_OP_FINALIZE = 5, VF_OP_ISTFT = 6,
+       VF_OP_PEAK_NORM = 7 };
+typedef struct vf_op_case {
+  int kind, batch;
+  /* Clips of different lengths (any kind; PEAK_NORM needs them): host sample offsets [batch + 1], clip b = [off[b], off[b + 1]).
+   * The hook writes a lengths table with the product's setup kernel (unet_w0: 127 or 1024, the UNet's valid bins) and hands
+   * the kernel the rows its plan would: FIRST T / Tp, POOL the UNet rows of level + 1, COND T / Tv, REFLECT / TAIL the last
+   * vocoder stage's samples (REFLECT with cond_pad: Tv), FINALIZE and ISTFT the offsets and the last stage / T.  The table
+   * comes back in vl_rows [18][batch] when that is not NULL. */
+  const int64_t* clip_off;
+  int unet_w0;
+  int* vl_rows;
+  /* FIRST: x [batch][T][W + 1], w1 [32][9], bn2 / shortcut [32]; out a2 planes [batch][Tp (W + 1)][32], sc_raw floats */
+  int T, W;
+  float bn1_scale, bn1_shift;
+  const float* x;
+  const float* w1;
+  const float* bn2_scale;
+  const float* bn2_shift;
+  const float* w_sc;
+  const float* b_sc;
+  uint16_t* a2;
+  float* sc_raw;
+  /* POOL (H, W, C, level): pin [batch][H (W + 1)][C] floats, the next block's bn1 [C]; out_r / out_a planes and out_raw floats
+   * [batch][(H / 2) Wpo][C] (any of them NULL) */
+  int H, C, level;
+  const float* pin;
+  const float* a_scale;
+  const float* a_shift;
+  uint16_t* out_r;
+  uint16_t* out_a;
+  float* out_raw;
+  /* COND (T): mel [batch][T][128], log10 when is_log; unify: mel_target [batch][T][128] linear, the band sums come back in
+   * band_sums [batch][2]; out cond planes [batch][Tv][128] */
+  int is_log, unify;
+  const float* mel;
+  const float* mel_target;
+  float* band_sums;
+  uint16_t* cond;
+  /* REFLECT (C, L, cond_pad): planes [batch][L + 6][C] in place.  TAIL (C, L, terms, tanh_out): tail_in [batch][L + 6][C]
+   * planes (already reflect padded), tail_w [1][C][7] (PyTorch layout), out wav [batch][L] and peak_bits [batch] */
+  int64_t L;
+  int cond_pad, terms, tanh_out;
+  uint16_t* planes;
+  const uint16_t* tail_in;
+  const float* tail_w;
+  float tail_b;
+  float* wav;
+  uint32_t* peak_bits;
+  /* FINALIZE (L, n): wav [batch][L] and peak_bits [batch] in; out [batch][n] (varlen: packed by clip_off).
+   * ISTFT (T, n): mag [batch][T][1025], wav [batch][n] (varlen: packed by clip_off); frames [batch][T][2048], out as FINALIZE.
+   * PEAK_NORM (n = the longest clip): wav packed by clip_off, normalised in place; the per-clip peaks come back in peak_bits */
+  int64_t n;
+  const float* in_wav;
+  const float* mag;
+  float* frames;
+  float* out;
+  /* reported: what the set-up derived */
+  int Tp, Wpo, Tv;
+  int64_t skip;
+  int64_t tail_smem;
+} vf_op_case;
+VF_API int vf_selftest_op(vf_ctx* ctx, vf_op_case* oc);
+
 #ifdef __cplusplus
 }
 #endif

@@ -21,7 +21,7 @@ EXPORTS = [
     "vf_restore_ex", "vf_ssr_forward", "vf_ssr_restore", "vf_ssr_restore_host", "vf_ssr_unet", "vf_ssr_stages", "vf_istft",
     "vf_mel", "vf_finalize", "vf_plan_cache_info", "vf_resample_poly", "vf_lsd", "vf_sispec", "vf_to_pcm16_ex", "vf_amp_to_original_f",
     "vf_restore_varlen", "vf_ssr_restore_varlen", "vf_restore_varlen_mels", "vf_metric_spectrogram", "vf_ssim", "vf_score_varlen",
-    "vf_ssr_restore_varlen_mels",
+    "vf_ssr_restore_varlen_mels", "vf_selftest_op",
 ]
 VF_RESTORE_UNIFY_ENERGY = 1
 VF_SSR_PEAK_NORMALISE = 1
@@ -56,6 +56,22 @@ class VfLayerCase(Structure):
                 ("pair_slope_h", c_float), ("pair_slope_out", c_float), ("pair_last", c_int)] + \
                [(f, c_int) for f in ("bn", "bk", "stages", "resid_tma", "tma_out", "grid")] + \
                [("tiles", c_int64), ("div_fallback", c_int)]
+
+
+class VfOpCase(Structure):
+    """vf_op_case (include/b200vf.h): one non-GEMM op for vf_selftest_op (tests only)."""
+    _fields_ = [("kind", c_int), ("batch", c_int), ("clip_off", c_void_p), ("unet_w0", c_int), ("vl_rows", c_void_p),
+                ("T", c_int), ("W", c_int), ("bn1_scale", c_float), ("bn1_shift", c_float)] + \
+               [(f, c_void_p) for f in ("x", "w1", "bn2_scale", "bn2_shift", "w_sc", "b_sc", "a2", "sc_raw")] + \
+               [("H", c_int), ("C", c_int), ("level", c_int)] + \
+               [(f, c_void_p) for f in ("pin", "a_scale", "a_shift", "out_r", "out_a", "out_raw")] + \
+               [("is_log", c_int), ("unify", c_int)] + \
+               [(f, c_void_p) for f in ("mel", "mel_target", "band_sums", "cond")] + \
+               [("L", c_int64), ("cond_pad", c_int), ("terms", c_int), ("tanh_out", c_int), ("planes", c_void_p),
+                ("tail_in", c_void_p), ("tail_w", c_void_p), ("tail_b", c_float), ("wav", c_void_p), ("peak_bits", c_void_p),
+                ("n", c_int64)] + \
+               [(f, c_void_p) for f in ("in_wav", "mag", "frames", "out")] + \
+               [("Tp", c_int), ("Wpo", c_int), ("Tv", c_int), ("skip", c_int64), ("tail_smem", c_int64)]
 
 
 class EngineError(RuntimeError):
@@ -106,6 +122,7 @@ def load_library():
     lib.vf_enable_stage_timing.argtypes = [P, c_int]
     lib.vf_stage_times.argtypes = [P, POINTER(c_float * 4)]
     lib.vf_selftest_layer.argtypes = [P, POINTER(VfLayerCase)]
+    lib.vf_selftest_op.argtypes = [P, POINTER(VfOpCase)]
     lib.vf_enable_op_timing.argtypes = [P, c_int]
     lib.vf_op_count.argtypes = [P]
     lib.vf_op_info.argtypes = [P, c_int, POINTER(c_float), POINTER(c_double), POINTER(c_double), POINTER(c_int),

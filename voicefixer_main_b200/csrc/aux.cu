@@ -365,10 +365,13 @@ __global__ void __launch_bounds__(TAIL_THREADS) voc_tail_kernel(VocTailParams p)
     atomicMax(p.peak_bits + b, __float_as_uint(m));
   }
 }
+size_t voc_tail_smem_bytes(int C, int terms) {
+  return (size_t)7 * C * 4 + (size_t)(terms == 3 ? 2 : 1) * (TAIL_TILE + 6) * (C + 8) * 2;
+}
 cudaError_t launch_voc_tail(const VocTailParams& p, cudaStream_t stream) {
   dim3 grid((unsigned)((p.L + TAIL_TILE - 1) / TAIL_TILE), p.batch);
   const bool three = p.terms == 3;
-  const size_t smem = (size_t)7 * p.C * 4 + (size_t)(three ? 2 : 1) * (TAIL_TILE + 6) * (p.C + 8) * 2;
+  const size_t smem = voc_tail_smem_bytes(p.C, p.terms);
   static bool attr_set[2] = {false, false};     // once per variant (not while a graph is being captured)
   if (!attr_set[three]) {
     cudaError_t e = three ? cudaFuncSetAttribute(voc_tail_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)

@@ -396,10 +396,8 @@ int restore_impl(vf_ctx* ctx, Plan* plan, const float* wav, int batch, int64_t n
     cop.cond.is_log = 1;
     cop.cond.band_sums = nullptr;
     if (unify) {
-      CK(cudaMemsetAsync(plan->d_band, 0, 2 * (size_t)batch * sizeof(float), s));
-      CK(launch_band_energy(plan->d_mel, plan->d_logmel_out, batch, frames, plan->d_band, s, plan->vl(VL_T)));
+      CK(unify_energy(plan->d_mel, plan->d_logmel_out, batch, frames, plan->d_band, plan->vl(VL_T), &cop.cond, s));
       ctx->launches++;
-      cop.cond.band_sums = plan->d_band;
     }
     return run_ops(ctx, plan->vocoder, s);
   };
@@ -408,12 +406,9 @@ int restore_impl(vf_ctx* ctx, Plan* plan, const float* wav, int batch, int64_t n
   rc = stage_mark(ctx, 3, st); if (rc) return rc;
   // eval_gsr_voicefixer.py:68-72: peak normalise + trim_center
   FinalizeParams f;
-  memset(&f, 0, sizeof f);
-  const long d = plan->L - (long)n;
-  if (!off && (d < 0 || d == 1)) return fail(ctx, VF_EINVAL, "vocoder output length %ld incompatible with input %ld (trim_center)", plan->L, (long)n);
-  f.wav = plan->d_voc_wav; f.peak_bits = plan->d_peak; f.batch = batch; f.L = plan->L; f.n = (long)n; f.skip = d / 2;
-  f.out = wav_out; f.out_ld = (long)n; f.out_off = 0;
-  if (off) { f.vl_off = plan->d_vl_off; f.vl_L = plan->vl(VL_VOC + ctx->cfg.voc_num_stages - 1); }
+  rc = finalize_params(ctx, &f, plan->d_voc_wav, plan->d_peak, batch, plan->L, (long)n, wav_out, off ? plan->d_vl_off : nullptr,
+                       off ? plan->vl(VL_VOC + ctx->cfg.voc_num_stages - 1) : nullptr);
+  if (rc) return rc;
   CK(launch_finalize(f, st));
   ctx->launches++;
   rc = stage_mark(ctx, 4, st); if (rc) return rc;
@@ -445,16 +440,10 @@ int ssr_impl(vf_ctx* ctx, Plan* plan, const float* sp, const float* wav, int bat
   if (rc) return rc;
   rc = stage_mark(ctx, 2, st); if (rc) return rc;
   IstftFramesParams fp;
-  memset(&fp, 0, sizeof fp);
-  fp.mag = plan->d_mag; fp.wav = wav; fp.n = (long)n; fp.batch = batch; fp.T = frames;
-  fp.window = ctx->d_window; fp.tw1024 = ctx->d_tw1024; fp.tw2048 = ctx->d_tw2048; fp.frames = plan->d_frames;
-  fp.vl_off = plan->d_vl_off; fp.vl_T = plan->vl(VL_T);       // null unless varlen
-  CK(launch_istft_frames(fp, st));
   IstftOlaParams op;
-  memset(&op, 0, sizeof op);
-  op.frames = plan->d_frames; op.batch = batch; op.T = frames; op.length = (long)n; op.window = ctx->d_window;
-  op.out = wav_out; op.out_ld = (long)n;
-  op.vl_off = plan->d_vl_off; op.vl_T = plan->vl(VL_T);
+  istft_params(ctx, &fp, &op, plan->d_mag, wav, batch, (long)n, frames, plan->d_frames, wav_out, plan->d_vl_off,
+               plan->vl(VL_T));       // the lengths table is null unless varlen
+  CK(launch_istft_frames(fp, st));
   CK(launch_istft_ola(op, st));
   ctx->launches += 2;
   rc = stage_mark(ctx, 3, st); if (rc) return rc;
@@ -1512,6 +1501,188 @@ VF_API int vf_selftest_layer(vf_ctx* ctx, vf_layer_case* lc) {
   ctx->allocs.resize(n_weight_allocs);
   ctx->weight_bytes = weight_bytes;
   if (!rc && se != cudaSuccess) rc = fail(ctx, VF_ECUDA, "vf_selftest_layer: %s", cudaGetErrorString(se));
+  return rc;
+}
+
+}  // extern "C"
+
+namespace {
+
+// Builds and runs one vf_op_case with its buffers in `b.plan`; each op's parameter block comes from the helper the plans
+// use, and the buffers are sized from what that helper derived.  Outputs are copied back into the case's host buffers.
+int run_op_case(vf_ctx* ctx, Builder& b, vf_op_case& c) {
+  Plan& plan = *b.plan;
+  const int B = c.batch;
+  plan.batch = B;
+  struct Down { void* host; const void* dev; size_t bytes; };
+  std::vector<Down> downs;
+  auto dev = [&](const void* host, size_t bytes) -> void* {        // device copy of a host buffer (or of nothing)
+    uint8_t* d = b.alloc<uint8_t>(bytes);
+    if (!b.rc && host && bytes) {
+      const cudaError_t e = cudaMemcpy(d, host, bytes, cudaMemcpyHostToDevice);
+      if (e != cudaSuccess) b.rc = fail(ctx, VF_ECUDA, "selftest upload: %s", cudaGetErrorString(e));
+    }
+    return d;
+  };
+  auto out = [&](void* host, size_t bytes) -> void* {             // in/out: uploaded now, copied back after the launch
+    if (!host) return nullptr;
+    void* d = dev(host, bytes);
+    downs.push_back({host, d, bytes});
+    return d;
+  };
+  auto planes_out = [&](uint16_t* host, size_t n) -> PlanePtr {  // [2][n] fp16 planes
+    __half* d = static_cast<__half*>(out(host, 2 * n * sizeof(__half)));
+    return PlanePtr{d, d ? d + n : nullptr};
+  };
+  auto fl = [&](const float* host, size_t n) { return static_cast<float*>(dev(host, n * sizeof(float))); };
+  const int last = VL_VOC + ctx->cfg.voc_num_stages - 1;
+  const int64_t packed = c.clip_off ? c.clip_off[B] : 0;            // samples of all clips when they are packed
+  int rc = VF_OK;
+  if (c.clip_off) {
+    plan.d_vl_off = b.alloc<int64_t>((size_t)B + 1);
+    plan.d_vl_rows = b.alloc<int>((size_t)VL_ROWS * B);
+    if (b.rc) return b.rc;
+    rc = write_lengths_table(ctx, &plan, c.clip_off, B, c.unet_w0, 0);
+    if (rc) return rc;
+  }
+  std::vector<Op> ops;
+  switch (c.kind) {
+    case VF_OP_FIRST: {
+      UnetW U;
+      ConvBlockW blk;
+      U.first_bn1_scale = c.bn1_scale; U.first_bn1_shift = c.bn1_shift;
+      U.d_first_w1 = fl(c.w1, 32 * 9); U.d_first_wsc = fl(c.w_sc, 32); U.d_first_bsc = fl(c.b_sc, 32);
+      blk.bn2 = Affine{fl(c.bn2_scale, 32), fl(c.bn2_shift, 32)};
+      Op op = first_op(ctx, U, blk, fl(c.x, (size_t)B * c.T * (c.W + 1)), B, c.T, c.W, PlanePtr{nullptr, nullptr}, nullptr,
+                       plan.vl(VL_T), plan.vl(VL_TP));
+      UnetFirstParams& f = op.first;
+      const size_t n = (size_t)B * f.Tp * (f.W + 1) * 32;
+      f.a2 = planes_out(c.a2, n);
+      f.sc_raw = static_cast<float*>(out(c.sc_raw, n * sizeof(float)));
+      c.Tp = f.Tp;
+      ops.push_back(op);
+      break;
+    }
+    case VF_OP_POOL: {
+      const Affine bn1{fl(c.a_scale, c.C), fl(c.a_shift, c.C)};
+      Op op = pool_op(ctx, fl(c.pin, (size_t)B * c.H * (c.W + 1) * c.C), B, c.H, c.W, c.C, bn1, PlanePtr{nullptr, nullptr},
+                      PlanePtr{nullptr, nullptr}, nullptr, plan.vl(VL_UNET + c.level + 1));
+      PoolParams& p = op.pool;
+      const size_t n = (size_t)B * (p.H / 2) * p.Wpo * p.C;
+      p.out_r = planes_out(c.out_r, n);
+      p.out_a = planes_out(c.out_a, n);
+      p.out_raw = static_cast<float*>(out(c.out_raw, n * sizeof(float)));
+      c.Wpo = p.Wpo;
+      ops.push_back(op);
+      break;
+    }
+    case VF_OP_COND: {
+      const size_t mel_n = (size_t)B * c.T * 128;
+      Op op = cond_op(ctx, fl(c.mel, mel_n), B, c.T, PlanePtr{nullptr, nullptr}, plan.vl(VL_T), plan.vl(VL_TV));
+      VocCondParams& p = op.cond;
+      p.is_log = c.is_log;
+      p.out = planes_out(c.cond, (size_t)B * p.Tv * 128);
+      c.Tv = p.Tv;
+      if (c.unify) {     // restore_impl: the band sums of the linear input mel and the restored log-mel, then the conditioning
+        float* sums = static_cast<float*>(out(c.band_sums, 2 * (size_t)B * sizeof(float)));
+        if (b.rc) return b.rc;
+        CK(unify_energy(fl(c.mel_target, mel_n), p.mel, B, c.T, sums, plan.vl(VL_T), &p, 0));
+      }
+      ops.push_back(op);
+      break;
+    }
+    case VF_OP_REFLECT:
+      ops.push_back(reflect_op(planes_out(c.planes, (size_t)B * (c.L + 6) * c.C), B, (int)c.L, c.C,
+                               c.cond_pad ? plan.vl(VL_TV) : plan.vl(last)));
+      break;
+    case VF_OP_TAIL: {
+      float* w = nullptr;
+      rc = pack_tail(ctx, &w, host_tensor(c.tail_w, {1, c.C, 7}));
+      if (rc) return rc;
+      const size_t n = (size_t)B * (c.L + 6) * c.C;
+      __half* in = static_cast<__half*>(dev(c.tail_in, 2 * n * sizeof(__half)));
+      float* wav = static_cast<float*>(out(c.wav, (size_t)B * c.L * sizeof(float)));
+      unsigned int* peak = static_cast<unsigned int*>(out(c.peak_bits, (size_t)B * sizeof(unsigned int)));
+      ops.push_back(memset_op(peak, (size_t)B * 4));
+      ops.push_back(tail_op(PlanePtr{in, in + n}, B, c.L, c.C, c.terms, w, c.tail_b, c.tanh_out, wav, peak, plan.vl(last)));
+      c.tail_smem = (int64_t)voc_tail_smem_bytes(c.C, c.terms);
+      break;
+    }
+    case VF_OP_FINALIZE: {
+      Op op;
+      op.kind = OP_FINALIZE;
+      float* o = static_cast<float*>(out(c.out, (c.clip_off ? packed : (int64_t)B * c.n) * sizeof(float)));
+      if (b.rc) return b.rc;
+      rc = finalize_params(ctx, &op.fin, fl(c.in_wav, (size_t)B * c.L), static_cast<unsigned int*>(dev(c.peak_bits, B * 4)), B,
+                           c.L, c.n, o, plan.d_vl_off, plan.vl(last));
+      if (rc) return rc;
+      c.skip = op.fin.skip;
+      ops.push_back(op);
+      break;
+    }
+    case VF_OP_ISTFT: {
+      const int64_t wav_n = c.clip_off ? packed : (int64_t)B * c.n;
+      float* frames = static_cast<float*>(out(c.frames, (size_t)B * c.T * 2048 * sizeof(float)));
+      float* o = static_cast<float*>(out(c.out, wav_n * sizeof(float)));
+      const float* mag = fl(c.mag, (size_t)B * c.T * 1025);
+      const float* wav = fl(c.in_wav, wav_n);
+      if (b.rc) return b.rc;
+      IstftFramesParams fp;
+      IstftOlaParams op;
+      istft_params(ctx, &fp, &op, mag, wav, B, c.n, c.T, frames, o, plan.d_vl_off, plan.vl(VL_T));
+      CK(launch_istft_frames(fp, 0));
+      CK(launch_istft_ola(op, 0));
+      break;
+    }
+    case VF_OP_PEAK_NORM: {      // ssr_restore_varlen's VF_SSR_PEAK_NORMALISE
+      float* wav = static_cast<float*>(out(c.wav, packed * sizeof(float)));
+      unsigned int* peak = static_cast<unsigned int*>(out(c.peak_bits, (size_t)B * sizeof(unsigned int)));
+      if (b.rc) return b.rc;
+      CK(cudaMemsetAsync(peak, 0, (size_t)B * sizeof(unsigned int), 0));
+      CK(launch_peak_normalise_varlen(wav, plan.d_vl_off, B, (long)c.n, peak, 0));
+      break;
+    }
+  }
+  if (b.rc) return b.rc;
+  rc = run_ops(ctx, ops, 0);
+  if (rc) return rc;
+  CK(cudaDeviceSynchronize());
+  for (const Down& d : downs) CK(cudaMemcpy(d.host, d.dev, d.bytes, cudaMemcpyDeviceToHost));
+  if (c.vl_rows && plan.d_vl_rows) CK(cudaMemcpy(c.vl_rows, plan.d_vl_rows, (size_t)VL_ROWS * B * sizeof(int), cudaMemcpyDeviceToHost));
+  return VF_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+VF_API int vf_selftest_op(vf_ctx* ctx, vf_op_case* oc) {
+  if (!ctx || !oc) return VF_EINVAL;
+  vf_op_case& c = *oc;
+  const bool bad_kind = c.kind < VF_OP_FIRST || c.kind > VF_OP_PEAK_NORM;
+  const bool bad_shape =
+      (c.kind == VF_OP_FIRST && (c.T <= 0 || c.W <= 0 || !c.x || !c.w1 || !c.bn2_scale || !c.bn2_shift || !c.w_sc || !c.b_sc)) ||
+      (c.kind == VF_OP_POOL && (c.H < 2 || c.W <= 0 || c.C <= 0 || c.C % 8 || !c.pin || !c.a_scale || !c.a_shift || c.level < 0 || c.level > 5)) ||
+      (c.kind == VF_OP_COND && (c.T <= 0 || !c.mel || !c.cond || (c.unify && (!c.mel_target || !c.band_sums)))) ||
+      (c.kind == VF_OP_REFLECT && (c.L < 4 || c.C <= 0 || c.C % 8 || !c.planes)) ||
+      (c.kind == VF_OP_TAIL && (c.L <= 0 || c.C <= 0 || c.C % 8 || (c.terms != 1 && c.terms != 3) || !c.tail_in || !c.tail_w ||
+                                !c.wav || !c.peak_bits)) ||
+      (c.kind == VF_OP_FINALIZE && (c.L <= 0 || c.n <= 0 || !c.in_wav || !c.peak_bits || !c.out)) ||
+      (c.kind == VF_OP_ISTFT && (c.T <= 0 || c.n <= 1024 || !c.mag || !c.in_wav || !c.frames || !c.out)) ||
+      (c.kind == VF_OP_PEAK_NORM && (!c.clip_off || c.n <= 0 || !c.wav || !c.peak_bits));
+  if (bad_kind || c.batch <= 0 || bad_shape || (c.clip_off && (c.batch > VL_MAX_CLIPS || c.clip_off[0] != 0)))
+    return fail(ctx, VF_EINVAL, "vf_selftest_op: bad case");
+  CK(cudaSetDevice(ctx->device));
+  const size_t n_weight_allocs = ctx->allocs.size(), weight_bytes = ctx->weight_bytes;
+  Plan plan;
+  Builder b{ctx, &plan};
+  int rc = run_op_case(ctx, b, c);
+  const cudaError_t se = cudaDeviceSynchronize();
+  for (void* p : plan.allocs) cudaFree(p);
+  for (size_t i = n_weight_allocs; i < ctx->allocs.size(); ++i) cudaFree(ctx->allocs[i]);
+  ctx->allocs.resize(n_weight_allocs);
+  ctx->weight_bytes = weight_bytes;
+  if (!rc && se != cudaSuccess) rc = fail(ctx, VF_ECUDA, "vf_selftest_op: %s", cudaGetErrorString(se));
   return rc;
 }
 

@@ -248,6 +248,8 @@ int pack_conv3x3(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT* sc_w, con
 int pack_convT2d(vf_ctx* ctx, GemmW* out, const HostT& w);
 int pack_conv1d(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT& b, bool identity = false);
 int pack_convT1d(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT& b, int s);
+// the tail Conv1d(C -> 1, k7) weight [1][C][7] -> the tail kernel's [7][C]
+int pack_tail(vf_ctx* ctx, float** out, const HostT& w);
 // Residual add of a vocoder stack as an identity tap (through the accumulator, no epilogue loads) up to this channel count;
 // above it the epilogue adds the hi/lo planes.  The packer appends the identity block and the plan builder adds the tap.
 constexpr int IDENT_MAX_C = 128;
@@ -285,6 +287,33 @@ std::vector<GemmTap> taps_convt1d(int cin);
 // plane is written from row out_row0; `last`: no correction plane out
 int pair_setup(vf_ctx* ctx, PairParams* pp, const Planes& src, const Planes& dst, const GemmW& wa, const GemmW& wb, int n_img,
                int L, int dil, uint32_t ar, bool last, int out_row0, float slope_h, float slope_out, const int* row_valid);
+// The non-GEMM ops of the launch chains, set up as the plan builders and the restore paths use them (vf_selftest_op runs the
+// same set-up).  LeakyReLU slope of the UNet blocks, modules.py:265-266
+constexpr float UNET_SLOPE = 0.01f;
+// encoder_block1.conv_block1 on a [batch, T, W0 + 1] input: Tp = T padded to a multiple of 64; blk supplies bn2
+Op first_op(vf_ctx* ctx, const UnetW& U, const ConvBlockW& blk, const float* in, int batch, int T, int W0, PlanePtr a2,
+            float* sc_raw, const int* vl_T, const int* vl_Tp);
+// avg_pool2d(2,2) of an [batch, H * (W + 1), C] level + the consumer's bn1 + LeakyReLU: output pitch (W >> 1) + 1
+Op pool_op(vf_ctx* ctx, const float* in, int batch, int H, int W, int C, const Affine& next_bn1, PlanePtr out_r, PlanePtr out_a,
+           float* out_raw, const int* row_valid);
+// vocoder conditioning of the restored log-mel [batch, T, 128]: Tv = T + T % 2 + voc_tail_base rows per clip
+Op cond_op(vf_ctx* ctx, const float* logmel, int batch, int T, PlanePtr out, const int* vl_T, const int* vl_Tv);
+inline int voc_frames(const vf_config& c, int T) { return T + T % 2 + c.voc_tail_base; }
+// amp_to_original_f (VF_RESTORE_UNIFY_ENERGY): zeroes `sums` and launches the low-band reduction on the stream, then points
+// the conditioning op at it
+cudaError_t unify_energy(const float* mel_lin, const float* logmel_est, int batch, int T, float* sums, const int* vl_T,
+                         VocCondParams* cond, cudaStream_t st);
+// ReflectionPad1d(3) of [batch, L + 6, C] planes, the peak memset and the tail conv (the vocoder's last three launches)
+Op reflect_op(PlanePtr pl, int batch, int L, int C, const int* vl_L);
+Op memset_op(void* p, size_t bytes);
+Op tail_op(PlanePtr in, int batch, long L, int C, int terms, const float* w, float bias, int tanh_out, float* wav,
+           unsigned int* peak, const int* vl_L);
+// peak normalise + trim_center of a [batch, L] vocoder output into [batch, n] (varlen: packed by vl_off, trimmed by vl_L)
+int finalize_params(vf_ctx* ctx, FinalizeParams* f, const float* wav, const unsigned int* peak, int batch, long L, long n,
+                    float* out, const int64_t* vl_off, const int* vl_L);
+// the SSR back end: the predicted magnitude with the phase of `wav`'s STFT -> frames -> overlap-add into out [batch, n]
+void istft_params(vf_ctx* ctx, IstftFramesParams* fp, IstftOlaParams* op, const float* mag, const float* wav, int batch, long n,
+                  int T, float* frames, float* out, const int64_t* vl_off, const int* vl_T);
 int build_plan(vf_ctx* ctx, Plan* plan);
 
 }  // namespace vf

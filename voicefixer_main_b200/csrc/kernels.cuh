@@ -146,6 +146,8 @@ struct VocTailParams {
   const int* vl_L;       // varlen: clip b writes (and peaks over) its first vl_L[b] samples; or null
 };
 cudaError_t launch_voc_tail(const VocTailParams& p, cudaStream_t stream);
+// dynamic shared memory of one tail CTA: the [7][C] weights and the fp16 input tile (both planes when terms == 3)
+size_t voc_tail_smem_bytes(int C, int terms);
 
 // eval_gsr_voicefixer.py:68-72: out /= max|out| if it exceeds 1; trim_center (tools/utils.py:57-70).
 struct FinalizeParams {

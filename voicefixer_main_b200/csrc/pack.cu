@@ -237,6 +237,19 @@ int load_unet(vf_ctx* ctx, const std::string& U, UnetW* w) {
   return VF_OK;
 }
 
+}  // namespace
+
+int pack_tail(vf_ctx* ctx, float** out, const HostT& w) {
+  if (w.shape.size() != 3 || w.shape[2] != 7) return fail(ctx, VF_EINVAL, "vocoder tail kernel must be 7");
+  const int cl = (int)w.shape[1];
+  std::vector<float> t((size_t)7 * cl);
+  for (int cch = 0; cch < cl; ++cch)
+    for (int kk = 0; kk < 7; ++kk) t[(size_t)kk * cl + cch] = w.v[(size_t)cch * 7 + kk];
+  return upload(ctx, out, t);
+}
+
+namespace {
+
 int load_vocoder(vf_ctx* ctx) {
   int rc;
   const vf_config& c = ctx->cfg;
@@ -266,14 +279,9 @@ int load_vocoder(vf_ctx* ctx) {
   }
   {
     NEED(w, "vocoder.tail.weight"); NEED(b, "vocoder.tail.bias");
-    const int cl = (int)w->shape[1], k = (int)w->shape[2];
-    if (k != 7) return fail(ctx, VF_EINVAL, "vocoder tail kernel must be 7");
-    std::vector<float> t((size_t)7 * cl);
-    for (int cch = 0; cch < cl; ++cch)
-      for (int kk = 0; kk < 7; ++kk) t[(size_t)kk * cl + cch] = w->v[(size_t)cch * 7 + kk];
-    rc = upload(ctx, &ctx->d_tail_w, t); if (rc) return rc;
+    rc = pack_tail(ctx, &ctx->d_tail_w, *w); if (rc) return rc;
     ctx->tail_b = b->v[0];
-    ctx->voc_last_c = cl;
+    ctx->voc_last_c = (int)w->shape[1];
   }
   ctx->voc_loaded = true;
   return VF_OK;

@@ -331,6 +331,97 @@ GemmEpilogue epi_plain(int rows_in, int Wp, int cout, int out_img_rows) {
   return e;
 }
 
+Op first_op(vf_ctx* ctx, const UnetW& U, const ConvBlockW& blk, const float* in, int batch, int T, int W0, PlanePtr a2,
+            float* sc_raw, const int* vl_T, const int* vl_Tp) {
+  Op op; op.kind = OP_FIRST;
+  UnetFirstParams& f = op.first;
+  memset(&f, 0, sizeof f);
+  f.logmel = in; f.batch = batch; f.T = T; f.Tp = (T + 63) / 64 * 64; f.W = W0; f.in_ld = W0 + 1;
+  f.bn1_scale = U.first_bn1_scale; f.bn1_shift = U.first_bn1_shift;
+  f.w1 = U.d_first_w1; f.bn2_scale = blk.bn2.scale; f.bn2_shift = blk.bn2.shift;
+  f.w_sc = U.d_first_wsc; f.b_sc = U.d_first_bsc; f.slope = UNET_SLOPE;
+  f.a2 = a2; f.sc_raw = sc_raw; f.err = ctx->d_err;
+  f.vl_T = vl_T; f.vl_Tp = vl_Tp;
+  return op;
+}
+
+Op pool_op(vf_ctx* ctx, const float* in, int batch, int H, int W, int C, const Affine& next_bn1, PlanePtr out_r, PlanePtr out_a,
+           float* out_raw, const int* row_valid) {
+  Op op; op.kind = OP_POOL;
+  PoolParams& p = op.pool;
+  memset(&p, 0, sizeof p);
+  p.in = in; p.batch = batch; p.H = H; p.Wp = W + 1; p.C = C; p.Wpo = (W >> 1) + 1;
+  p.out_r = out_r; p.out_a = out_a; p.out_raw = out_raw;
+  p.a_scale = next_bn1.scale; p.a_shift = next_bn1.shift; p.slope = UNET_SLOPE; p.err = ctx->d_err;
+  p.row_valid = row_valid;
+  return op;
+}
+
+Op cond_op(vf_ctx* ctx, const float* logmel, int batch, int T, PlanePtr out, const int* vl_T, const int* vl_Tv) {
+  const vf_config& c = ctx->cfg;
+  Op op; op.kind = OP_COND;
+  VocCondParams& p = op.cond;
+  memset(&p, 0, sizeof p);
+  p.mel = logmel; p.is_log = 1; p.batch = batch; p.T = T; p.Tv = voc_frames(c, T); p.weight = ctx->d_melw;
+  p.amp_floor = c.voc_amp_floor; p.ref_db = c.voc_ref_db; p.min_db = c.voc_min_db; p.tail_value = c.voc_tail_value;
+  p.out = out;
+  p.vl_T = vl_T; p.vl_Tv = vl_Tv;
+  return op;
+}
+
+cudaError_t unify_energy(const float* mel_lin, const float* logmel_est, int batch, int T, float* sums, const int* vl_T,
+                         VocCondParams* cond, cudaStream_t st) {
+  cudaError_t e = cudaMemsetAsync(sums, 0, 2 * (size_t)batch * sizeof(float), st);
+  if (e == cudaSuccess) e = launch_band_energy(mel_lin, logmel_est, batch, T, sums, st, vl_T);
+  cond->band_sums = sums;
+  return e;
+}
+
+Op reflect_op(PlanePtr pl, int batch, int L, int C, const int* vl_L) {
+  Op op; op.kind = OP_REFLECT;
+  op.refl.pl = pl; op.refl.batch = batch; op.refl.L = L; op.refl.C = C; op.refl.pad = 3; op.refl.vl_L = vl_L;
+  return op;
+}
+
+Op memset_op(void* p, size_t bytes) {
+  Op op; op.kind = OP_MEMSET32;
+  op.ms.p = p; op.ms.bytes = bytes;
+  return op;
+}
+
+Op tail_op(PlanePtr in, int batch, long L, int C, int terms, const float* w, float bias, int tanh_out, float* wav,
+           unsigned int* peak, const int* vl_L) {
+  Op op; op.kind = OP_TAIL;
+  VocTailParams& p = op.tail;
+  memset(&p, 0, sizeof p);
+  p.in = in; p.batch = batch; p.L = (int)L; p.C = C; p.terms = terms; p.w = w; p.bias = bias;
+  p.wav = wav; p.peak_bits = peak; p.tanh_out = tanh_out; p.vl_L = vl_L;
+  return op;
+}
+
+int finalize_params(vf_ctx* ctx, FinalizeParams* f, const float* wav, const unsigned int* peak, int batch, long L, long n,
+                    float* out, const int64_t* vl_off, const int* vl_L) {
+  memset(f, 0, sizeof *f);
+  const long d = L - n;
+  if (!vl_off && (d < 0 || d == 1)) return fail(ctx, VF_EINVAL, "vocoder output length %ld incompatible with input %ld (trim_center)", L, n);
+  f->wav = wav; f->peak_bits = peak; f->batch = batch; f->L = L; f->n = n; f->skip = d / 2;
+  f->out = out; f->out_ld = n; f->out_off = 0;
+  f->vl_off = vl_off; f->vl_L = vl_L;
+  return VF_OK;
+}
+
+void istft_params(vf_ctx* ctx, IstftFramesParams* fp, IstftOlaParams* op, const float* mag, const float* wav, int batch, long n,
+                  int T, float* frames, float* out, const int64_t* vl_off, const int* vl_T) {
+  memset(fp, 0, sizeof *fp);
+  fp->mag = mag; fp->wav = wav; fp->n = n; fp->batch = batch; fp->T = T;
+  fp->window = ctx->d_window; fp->tw1024 = ctx->d_tw1024; fp->tw2048 = ctx->d_tw2048; fp->frames = frames;
+  fp->vl_off = vl_off; fp->vl_T = vl_T;
+  memset(op, 0, sizeof *op);
+  op->frames = frames; op->batch = batch; op->T = T; op->length = n; op->window = ctx->d_window;
+  op->out = out; op->out_ld = n;
+  op->vl_off = vl_off; op->vl_T = vl_T;
+}
+
 namespace {
 
 const int ENC_C[6] = {32, 64, 128, 256, 384, 384};
@@ -369,7 +460,7 @@ int build_unet(vf_ctx* ctx, Builder& b, Plan* plan, const UnetW& U, const UnetGe
   const int Tp = (T + 63) / 64 * 64;
   std::vector<Op>& ops = plan->unet;
   const int terms = ctx->unet_terms;
-  const float S = 0.01f;   // LeakyReLU slope, modules.py:265-266
+  const float S = UNET_SLOPE;
   Level lv[7];
   for (int l = 0; l < 7; ++l) {
     Level& L = lv[l];
@@ -427,16 +518,7 @@ int build_unet(vf_ctx* ctx, Builder& b, Plan* plan, const UnetW& U, const UnetGe
       const float* resid = nullptr;
       const Planes* sc = nullptr;
       if (j == 0 && l == 0) {
-        Op op; op.kind = OP_FIRST;
-        UnetFirstParams& f = op.first;
-        memset(&f, 0, sizeof f);
-        f.logmel = G.in; f.batch = B; f.T = T; f.Tp = Tp; f.W = G.W0; f.in_ld = G.W0 + 1;
-        f.bn1_scale = U.first_bn1_scale; f.bn1_shift = U.first_bn1_shift;
-        f.w1 = U.d_first_w1; f.bn2_scale = w.bn2.scale; f.bn2_shift = w.bn2.shift;
-        f.w_sc = U.d_first_wsc; f.b_sc = U.d_first_bsc; f.slope = S;
-        f.a2 = L.aT.p; f.sc_raw = L.raw[0]; f.err = ctx->d_err;
-        f.vl_T = plan->vl(VL_T); f.vl_Tp = plan->vl(VL_TP);
-        ops.push_back(op);
+        ops.push_back(first_op(ctx, U, w, G.in, B, T, G.W0, L.aT.p, L.raw[0], plan->vl(VL_T), plan->vl(VL_TP)));
         resid = L.raw[0];      // precomputed shortcut(x) acts as the residual
         cur = 0;
       } else if (j == 0) {
@@ -465,15 +547,8 @@ int build_unet(vf_ctx* ctx, Builder& b, Plan* plan, const UnetW& U, const UnetGe
       cur = dst;
     }
     // avg_pool2d(2,2) -> next stage's (or the bottleneck's) bn1 + LeakyReLU
-    Op op; op.kind = OP_POOL;
-    PoolParams& p = op.pool;
-    memset(&p, 0, sizeof p);
     const ConvBlockW& nx = l < 5 ? U.enc[l + 1][0] : U.bott;
-    p.in = L.raw[cur]; p.batch = B; p.H = L.H; p.Wp = L.Wp; p.C = L.C; p.Wpo = (L.W >> 1) + 1;
-    p.out_r = L.P_r.p; p.out_a = L.P_a.p; p.out_raw = L.P_raw;
-    p.a_scale = nx.bn1.scale; p.a_shift = nx.bn1.shift; p.slope = S; p.err = ctx->d_err;
-    p.row_valid = lv[l + 1].valid;
-    ops.push_back(op);
+    ops.push_back(pool_op(ctx, L.raw[cur], B, L.H, L.W, L.C, nx.bn1, L.P_r.p, L.P_a.p, L.P_raw, lv[l + 1].valid));
   }
   // ---------------- bottleneck (conv_block7, identity shortcut) -> decoder_block1.bn1 + ReLU
   {
@@ -540,7 +615,7 @@ int build_unet(vf_ctx* ctx, Builder& b, Plan* plan, const UnetW& U, const UnetGe
 int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
   const vf_config& c = ctx->cfg;
   const int B = plan->batch, T = plan->T;
-  const int Tv = T + T % 2 + c.voc_tail_base;
+  const int Tv = voc_frames(c, T);
   const int terms = ctx->voc_terms;
   std::vector<Op>& ops = plan->vocoder;
   const int CC = c.voc_cond_channels;
@@ -550,17 +625,8 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
   Planes cpad = b.planes(B, Tv + 6, CC);
   Planes stem = b.planes(B, Tv, c.voc_channels);
   if (b.rc) return b.rc;
-  {
-    Op op; op.kind = OP_COND;
-    VocCondParams& p = op.cond;
-    memset(&p, 0, sizeof p);
-    p.mel = plan->d_logmel_out; p.is_log = 1; p.batch = B; p.T = T; p.Tv = Tv; p.weight = ctx->d_melw;
-    p.amp_floor = c.voc_amp_floor; p.ref_db = c.voc_ref_db; p.min_db = c.voc_min_db; p.tail_value = c.voc_tail_value;
-    p.out = cond.p;
-    p.vl_T = plan->vl(VL_T); p.vl_Tv = plan->vl(VL_TV);
-    plan->cond_op = (int)ops.size();
-    ops.push_back(op);
-  }
+  plan->cond_op = (int)ops.size();
+  ops.push_back(cond_op(ctx, plan->d_logmel_out, B, T, cond.p, plan->vl(VL_T), plan->vl(VL_TV)));
   Planes cur = cond;
   for (int i = 0; i < c.voc_cond_layers; ++i) {
     const bool last = i == c.voc_cond_layers - 1;
@@ -574,7 +640,7 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
     b.gemm(ops, ctx->voc_cond[i], ASrc{cur, Tv, 0}, nullptr, taps1d(3, 1, cur.C, true), e, B, terms);
     cur = dst;
   }
-  { Op op; op.kind = OP_REFLECT; op.refl.pl = cpad.p; op.refl.batch = B; op.refl.L = Tv; op.refl.C = CC; op.refl.pad = 3; op.refl.vl_L = plan->vl(VL_TV); ops.push_back(op); }
+  ops.push_back(reflect_op(cpad.p, B, Tv, CC, plan->vl(VL_TV)));
   {
     GemmEpilogue e = epi_plain(Tv, 0, c.voc_channels, Tv);
     e.row_valid = plan->vl(VL_TV);
@@ -686,18 +752,14 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
       }
     }
     if (last_stage) {
-      { Op op; op.kind = OP_REFLECT; op.refl.pl = tail_in.p; op.refl.batch = B; op.refl.L = (int)L; op.refl.C = cout; op.refl.pad = 3; op.refl.vl_L = plan->vl(VL_VOC + s); ops.push_back(op); }
+      ops.push_back(reflect_op(tail_in.p, B, (int)L, cout, plan->vl(VL_VOC + s)));
       plan->L = L;
       plan->d_voc_wav = b.alloc<float>((size_t)B * L);
       plan->d_peak = b.alloc<unsigned int>(B);
       if (b.rc) return b.rc;
-      { Op op; op.kind = OP_MEMSET32; op.ms.p = plan->d_peak; op.ms.bytes = (size_t)B * 4; ops.push_back(op); }
-      Op op; op.kind = OP_TAIL;
-      VocTailParams& p = op.tail;
-      memset(&p, 0, sizeof p);
-      p.in = tail_in.p; p.batch = B; p.L = (int)L; p.C = cout; p.terms = terms; p.w = ctx->d_tail_w; p.bias = ctx->tail_b;
-      p.wav = plan->d_voc_wav; p.peak_bits = plan->d_peak; p.tanh_out = c.voc_tail_tanh; p.vl_L = plan->vl(VL_VOC + s);
-      ops.push_back(op);
+      ops.push_back(memset_op(plan->d_peak, (size_t)B * 4));
+      ops.push_back(tail_op(tail_in.p, B, L, cout, terms, ctx->d_tail_w, ctx->tail_b, c.voc_tail_tanh, plan->d_voc_wav,
+                            plan->d_peak, plan->vl(VL_VOC + s)));
     }
     prev = (fused && cura) ? xa2 : xa;
     Lprev = L;

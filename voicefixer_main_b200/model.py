@@ -465,6 +465,11 @@ class Engine:
         with torch.cuda.device(self.device):
             self._ck(self.lib.vf_selftest_layer(self.ctx, ctypes.byref(case)))
 
+    def selftest_op(self, case: "L.VfOpCase"):
+        """Runs one non-GEMM op of the launch chains as the plans set it up (vf_selftest_op; tests only).  Synchronous."""
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_selftest_op(self.ctx, ctypes.byref(case)))
+
 
 # --------------------------------------------------------------------------------------------------------------
 class FDomainHelper:
