@@ -34,6 +34,7 @@
  *   vf_metric_spectrogram         AudioMetrics.wav_to_spectrogram metrics.py:37-51 (librosa STFT magnitude + mel) at 44.1 kHz
  *   vf_ssim                       AudioMetrics.ssim metrics.py:97-106 (scikit-image structural_similarity, win_size 7)
  *   vf_score_varlen               the spectral part of AudioMetrics.evaluation metrics.py:53-81 for a set of file pairs
+ *   vf_score_time_varlen          its sisdr and stoi keys (speechmetrics, metrics.py:58-64) for a set of file pairs
  *
  * Conventions: every function returns 0 on success or a negative VF_E* code and never throws; the message is
  * available from vf_last_error().  All tensor arguments are contiguous fp32.  Unless a name ends in `_host`,
@@ -249,7 +250,7 @@ VF_API int vf_ssim(vf_ctx* ctx, const float* est, const float* target, int image
  * own HOST offsets (as in vf_metric_spectrogram).  out [batch, 8] float64 in the reference's key order: lsd, non_log_sispec,
  * sispec, ssim on the spectrogram, then final_mel_lsd, final_non_log_mel_sispec, final_mel_sispec, final_mel_ssim on its
  * mel.  lsd and sispec are the fp32 values of vf_lsd / vf_sispec on each pair alone, widened; sispec is on to_log of both
- * spectrograms.  (sisdr, stoi and pesq come from the third-party speechmetrics package and are not computed.)  Every pair
+ * spectrograms.  (sisdr and stoi: vf_score_time_varlen; pesq is not computed.)  Every pair
  * is checked before any work is queued: equal frame counts and at least 7 frames, else VF_EINVAL naming the pair.  The
  * scratch (two spectrograms, two mels, SSIM tile sums) is owned by the context and freed by vf_destroy; it is allocated
  * stream-ordered, so there is no host synchronisation.  Pairs run in consecutive sub-batches of at most 16384 frames
@@ -257,6 +258,20 @@ VF_API int vf_ssim(vf_ctx* ctx, const float* est, const float* target, int image
  * launches per sub-batch.  Needs "mel.fb" loaded (no network). */
 VF_API int vf_score_varlen(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target,
                            const int64_t* target_offsets, int batch, double* out, void* stream);
+/* The time-domain keys of AudioMetrics.evaluation for `batch` (est, target) pairs of 44.1 kHz samples, packed with their
+ * own HOST offsets: out [batch, 2] float64 = sisdr, stoi, as speechmetrics computes them with window np.inf (restated in
+ * oracle/speech_metrics.py): the shorter clip of a pair is zero-padded at the end to the longer one; sisdr is the
+ * scale-invariant SDR without mean removal, stoi is pystoi 0.3.3's stoi(target, est, 44100, extended=False) - Octave-window
+ * resampling to 10 kHz, removal of the frames 40 dB below the target's loudest, 512-point STFT, 15 one-third-octave bands,
+ * 30-frame segment correlations; fewer than 30 frames left give 1e-5, as pystoi returns with a warning.  All arithmetic
+ * is float64 with fixed reduction orders: a pair's result does not depend on its batch or position.  Every pair is checked
+ * before any work is queued: each clip 1 .. 2^30 samples, and the padded pair more than 256 samples at 10 kHz (one STOI
+ * frame; pystoi fails on fewer), else VF_EINVAL naming the pair.  The tables (31947 resampling taps and the rest, designed
+ * in float64 on the host on first use) and the scratch are owned by the context and freed by vf_destroy; the scratch is
+ * allocated stream-ordered.  Sub-batches as in vf_score_varlen (at most 128 pairs and 16384 * 441 padded samples; a
+ * longer pair runs alone); eight launches per sub-batch.  Needs no weights.  PESQ is not computed. */
+VF_API int vf_score_time_varlen(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target,
+                                const int64_t* target_offsets, int batch, double* out, void* stream);
 
 VF_API int vf_to_log(vf_ctx* ctx, const float* in, float* out, int64_t n, void* stream);
 VF_API int vf_from_log(vf_ctx* ctx, const float* in, float* out, int64_t n, void* stream);

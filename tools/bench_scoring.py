@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of scoring a test set (AudioMetrics.evaluation over (restored, target) pairs) on one GPU.
 
-    python tools/bench_scoring.py [--files F] [--steps K] [--dir DIR]
+    python tools/bench_scoring.py [--files F] [--steps K] [--dir DIR] [--time-domain]
 
 Writes a seeded set of F PCM16 pairs (default 64) of 1-10 s at 44.1 kHz plus one 61 s pair to DIR (default: a temporary
 directory), then times three arms, alternating, for K rounds: one evaluation_batch() call over the set, evaluation() per
@@ -10,6 +10,10 @@ pair, and the CPU restatement (oracle/scoring.py: numpy / scipy / torch, the ari
 exactly; GPU vs CPU within 1e-3 relative for lsd / sispec - the CPU arm sums up to millions of values in torch fp32, the
 kernels in fp64 - and 1e-6 absolute for ssim), reports the largest deviation per key, and prints one JSON line with files/s
 and audio seconds/s per arm, the host's core count, and the card's name and power limit.
+
+--time-domain scores sisdr and stoi as well: the GPU arms call evaluation(_batch)(..., time_domain=True), the CPU arm adds
+oracle/speech_metrics.py (speechmetrics' sisdr, pystoi 0.3.3's stoi, numpy / scipy float64), and the largest absolute
+sisdr / stoi deviations are reported next to the spectral ones.
 """
 import argparse
 import json
@@ -48,10 +52,12 @@ def main():
     ap.add_argument("--files", type=int, default=64)
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--dir", default=None)
+    ap.add_argument("--time-domain", action="store_true")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_scoring needs a CUDA device")
     from oracle import scoring as S
+    from oracle import speech_metrics as M
     from voicefixer_main_b200.edges import AudioMetrics
     from voicefixer_main_b200.model import Engine
     eng = Engine("cuda:0")
@@ -61,12 +67,14 @@ def main():
         d = args.dir or tmp
         os.makedirs(d, exist_ok=True)
         pairs, seconds = write_pairs(d, args.files, 4242)
+        padded = [max(len(M.load_first_channel(pe)), len(M.load_first_channel(pt))) for pe, pt in pairs]
+        td = args.time_domain
         arms = {
-            "gpu_batch": lambda: am.evaluation_batch(pairs),
-            "gpu_per_file": lambda: [am.evaluation(pe, pt) for pe, pt in pairs],
-            "cpu_per_file": lambda: [S.evaluation(pe, pt) for pe, pt in pairs],
+            "gpu_batch": lambda: am.evaluation_batch(pairs, time_domain=td),
+            "gpu_per_file": lambda: [am.evaluation(pe, pt, time_domain=td) for pe, pt in pairs],
+            "cpu_per_file": lambda: [(M.evaluation if td else S.evaluation)(pe, pt) for pe, pt in pairs],
         }
-        am.evaluation_batch(pairs[:2])          # warm-up: module load, scratch
+        am.evaluation_batch(pairs[:2], time_domain=td)   # warm-up: module load, scratch
         times = {k: [] for k in arms}
         results = {}
         for _ in range(args.steps):
@@ -83,9 +91,19 @@ def main():
             d = abs(g[k] - c[k]) if k.endswith("ssim") else abs(g[k] - c[k]) / max(1.0, abs(c[k]))
             worst[k] = max(worst[k], d)
     assert all(v < (1e-6 if k.endswith("ssim") else 1e-3) for k, v in worst.items()), worst
+    if args.time_domain:                          # absolute, and relative to the test bars of oracle/speech_metrics.py
+        bar_ratio = dict.fromkeys(M.KEYS, 0.0)
+        for n, g, c in zip(padded, results["gpu_batch"], results["cpu_per_file"]):
+            bars = {"sisdr": M.sisdr_bar(n, c["sisdr"]), "stoi": M.stoi_bar(n)}
+            for k in M.KEYS:
+                worst[k] = max(worst.get(k, 0.0), abs(g[k] - c[k]))
+                bar_ratio[k] = max(bar_ratio[k], abs(g[k] - c[k]) / bars[k])
+        assert all(v <= 1 for v in bar_ratio.values()), bar_ratio
     n = len(pairs)
     res = {"files": n, "audio_s": round(seconds, 1), "host_cores": os.cpu_count(), "torch_threads": torch.get_num_threads(),
-           "max_deviation_vs_cpu": worst, **card_info(0)}
+           "time_domain": args.time_domain, "max_deviation_vs_cpu": worst, **card_info(0)}
+    if args.time_domain:
+        res["max_deviation_over_bar"] = bar_ratio
     for k, ts in times.items():
         res[f"{k}_files_per_s"] = [round(n / t, 2) for t in ts]
         res[f"{k}_audio_s_per_s"] = [round(seconds / t, 1) for t in ts]

@@ -21,7 +21,7 @@ EXPORTS = [
     "vf_restore_ex", "vf_ssr_forward", "vf_ssr_restore", "vf_ssr_restore_host", "vf_ssr_unet", "vf_ssr_stages", "vf_istft",
     "vf_mel", "vf_finalize", "vf_plan_cache_info", "vf_resample_poly", "vf_lsd", "vf_sispec", "vf_to_pcm16_ex", "vf_amp_to_original_f",
     "vf_restore_varlen", "vf_ssr_restore_varlen", "vf_restore_varlen_mels", "vf_metric_spectrogram", "vf_ssim", "vf_score_varlen",
-    "vf_ssr_restore_varlen_mels", "vf_selftest_op", "vf_selftest_gru",
+    "vf_ssr_restore_varlen_mels", "vf_selftest_op", "vf_selftest_gru", "vf_score_time_varlen",
 ]
 VF_RESTORE_UNIFY_ENERGY = 1
 VF_SSR_PEAK_NORMALISE = 1
@@ -156,6 +156,7 @@ def load_library():
     lib.vf_metric_spectrogram.argtypes = [P, P, POINTER(c_int64), c_int, P, P, P]
     lib.vf_ssim.argtypes = [P, P, P, c_int, c_int, c_int, P, P]
     lib.vf_score_varlen.argtypes = [P, P, POINTER(c_int64), P, POINTER(c_int64), c_int, P, P]
+    lib.vf_score_time_varlen.argtypes = [P, P, POINTER(c_int64), P, POINTER(c_int64), c_int, P, P]
     _lib = lib
     return lib
 

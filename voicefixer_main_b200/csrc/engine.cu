@@ -5,6 +5,7 @@
 // allocated once, every TMA tensor map is encoded once, and running a stage is a loop of kernel launches on
 // the caller's stream - no allocation, no host synchronisation, no CPU arithmetic on the data path.
 #include <climits>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -660,6 +661,9 @@ VF_API void vf_destroy(vf_ctx* ctx) {
     if (e) cudaEventDestroy(e);
   if (ctx->d_score) cudaFree(ctx->d_score);
   if (ctx->score_ev) cudaEventDestroy(ctx->score_ev);
+  if (ctx->d_stoi_tables) cudaFree(ctx->d_stoi_tables);
+  if (ctx->d_time_score) cudaFree(ctx->d_time_score);
+  if (ctx->time_score_ev) cudaEventDestroy(ctx->time_score_ev);
   delete ctx;
 }
 
@@ -1092,6 +1096,163 @@ VF_API int vf_score_varlen(vf_ctx* ctx, const float* est, const int64_t* est_off
   if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "score launch: %s", cudaGetErrorString(e));
   CK(cudaEventRecord(ctx->score_ev, st));
   ctx->score_used = true;
+  return VF_OK;
+}
+
+namespace {
+
+// d_stoi_tables layout (doubles): taps, window, tw256 (double2), tw512 (double2)
+constexpr size_t STOI_TAPS = 2 * STOI_HALF + 1, STOI_WIN_AT = STOI_TAPS + 1, STOI_TW256_AT = STOI_WIN_AT + 256,
+                 STOI_TW512_AT = STOI_TW256_AT + 2 * 256, STOI_TABLES = STOI_TW512_AT + 2 * 257;
+
+// The float64 tables of vf_score_time_varlen, designed once per context on the host:
+// * pystoi's resample_oct(x, 10000, 44100) window, Octave's resample filter for p / q = 100 / 441: L = ceil((60 - 8) /
+//   (28.714 * roll_off)) with cut-off 1 / 882 and roll_off = cut-off / 10, h = kaiser(2L + 1, 0.1102 * (60 - 8.7)) x
+//   2 * 100 * (1 / 882) * sinc(2 * (1 / 882) * t), t = -L..L; scipy's resample_poly uses window = h / sum(h), times up = 100.
+// * np.hanning(258)[1:-1] (0.5 + 0.5 cos(pi n / 257), n = -255, -253, ..., 255) and the 256 / 512-point twiddles.
+int stoi_tables(vf_ctx* ctx) {
+  if (ctx->d_stoi_tables) return VF_OK;
+  const double PI = 3.14159265358979323846;
+  std::vector<double> t(STOI_TABLES, 0.0);
+  const double fc = 1.0 / (2 * 441.0), roll_off = fc / 10, rejection_db = 60.0;
+  const long L = (long)std::ceil((rejection_db - 8) / (28.714 * roll_off));
+  if (L != STOI_HALF) return fail(ctx, VF_EASSERT, "stoi filter half length %ld != %d", L, STOI_HALF);
+  const double beta = 0.1102 * (rejection_db - 8.7), alpha = (double)L, i0_beta = std::cyl_bessel_i(0.0, beta);
+  double sum = 0;
+  for (long i = 0; i <= 2 * L; ++i) {
+    const double r = (i - alpha) / alpha;
+    const double kaiser = std::cyl_bessel_i(0.0, beta * std::sqrt(1 - r * r)) / i0_beta;
+    const double x = 2 * fc * (double)(i - L), y = PI * (x == 0 ? 1e-20 : x);     // np.sinc
+    t[i] = kaiser * (2 * 100.0 * fc * (std::sin(y) / y));
+    sum += t[i];
+  }
+  for (size_t i = 0; i < STOI_TAPS; ++i) t[i] = t[i] / sum * STOI_UP;
+  for (int i = 0; i < 256; ++i) t[STOI_WIN_AT + i] = 0.5 + 0.5 * std::cos(PI * (2 * i - 255) / 257.0);
+  for (int j = 0; j < 256; ++j) {
+    t[STOI_TW256_AT + 2 * j] = std::cos(2 * PI * j / 256.0);
+    t[STOI_TW256_AT + 2 * j + 1] = -std::sin(2 * PI * j / 256.0);
+  }
+  for (int k = 0; k <= 256; ++k) {
+    t[STOI_TW512_AT + 2 * k] = std::cos(2 * PI * k / 512.0);
+    t[STOI_TW512_AT + 2 * k + 1] = -std::sin(2 * PI * k / 512.0);
+  }
+  CK(cudaMalloc((void**)&ctx->d_stoi_tables, STOI_TABLES * sizeof(double)));
+  CK(cudaMemcpy(ctx->d_stoi_tables, t.data(), STOI_TABLES * sizeof(double), cudaMemcpyHostToDevice));
+  return VF_OK;
+}
+
+// pystoi's thirdoct(10000, 512, 15, 150): band k spans the rfft bins nearest (first of ties) to 150 * 2^((2k -+ 1) / 6)
+void stoi_bands(int* lo, int* hi) {
+  auto nearest = [](double f) {
+    int best = 0;
+    double d = INFINITY;
+    for (int q = 0; q <= 256; ++q) {
+      const double e = (q * (10000.0 / 512) - f) * (q * (10000.0 / 512) - f);
+      if (e < d) { d = e; best = q; }
+    }
+    return best;
+  };
+  for (int k = 0; k < STOI_BANDS; ++k) {
+    lo[k] = nearest(150 * std::pow(2.0, (2 * k - 1) / 6.0));
+    hi[k] = nearest(150 * std::pow(2.0, (2 * k + 1) / 6.0));
+  }
+}
+
+}  // namespace
+
+VF_API int vf_score_time_varlen(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target,
+                                const int64_t* target_offsets, int batch, double* out, void* stream) {
+  if (!ctx || !est || !target || !out || !est_offsets || !target_offsets || batch <= 0)
+    return ctx ? fail(ctx, VF_EINVAL, "vf_score_time_varlen: bad arguments") : VF_EINVAL;
+  if (est_offsets[0] != 0 || target_offsets[0] != 0) return fail(ctx, VF_EINVAL, "vf_score_time_varlen: offsets must start at 0");
+  std::vector<int64_t> N(batch);
+  for (int i = 0; i < batch; ++i) {
+    const int64_t ne = est_offsets[i + 1] - est_offsets[i], nt = target_offsets[i + 1] - target_offsets[i];
+    const int64_t cap = int64_t(1) << 30;
+    if (ne < 1 || nt < 1 || ne > cap || nt > cap)
+      return fail(ctx, VF_EINVAL, "vf_score_time_varlen: pair %d: est has %ld samples, target %ld (need 1 .. 2^30 each)", i,
+                  (long)ne, (long)nt);
+    N[i] = std::max(ne, nt);
+    if (stoi_len10(N[i]) <= STOI_FRAME)
+      return fail(ctx, VF_EINVAL, "vf_score_time_varlen: pair %d: %ld samples give %ld at 10 kHz, STOI needs more than %d", i,
+                  (long)N[i], (long)stoi_len10(N[i]), STOI_FRAME);
+  }
+  CK(cudaSetDevice(ctx->device));
+  int rc = stoi_tables(ctx);
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  // consecutive sub-batches of at most SCORE_MAX_IMAGES pairs and SCORE_CAP_FRAMES * 441 padded samples; a longer pair
+  // runs alone.  Scratch: resampled and compacted signals, energies, band values, tile sums (doubles), then the kept-frame
+  // indices and counts (ints).
+  auto bytes_of = [](int64_t R, int64_t F, int64_t T, int nb) {
+    return (size_t)(4 * R + F + 2 * STOI_BANDS * F + T) * 8 + (size_t)(F + nb) * 4;
+  };
+  std::vector<int> starts{0};
+  int64_t samples = 0, R = 0, F = 0, T = 0;
+  size_t need = 0;
+  for (int i = 0; i < batch; ++i) {
+    const int n_in = i - starts.back();
+    if (n_in == SCORE_MAX_IMAGES || (n_in > 0 && samples + N[i] > SCORE_CAP_FRAMES * 441)) {
+      need = std::max(need, bytes_of(R, F, T, n_in));
+      starts.push_back(i);
+      samples = R = F = T = 0;
+    }
+    samples += N[i];
+    R += stoi_len10(N[i]);
+    F += stoi_frames(stoi_len10(N[i]));
+    T += stoi_tiles(stoi_frames(stoi_len10(N[i])));
+  }
+  need = std::max(need, bytes_of(R, F, T, batch - starts.back()));
+  starts.push_back(batch);
+  if (ctx->time_score_used) CK(cudaStreamWaitEvent(st, ctx->time_score_ev, 0));
+  if (!ctx->time_score_ev) CK(cudaEventCreateWithFlags(&ctx->time_score_ev, cudaEventDisableTiming));
+  if (need > ctx->time_score_bytes) {        // stream-ordered: no host synchronisation
+    if (ctx->d_time_score) CK(cudaFreeAsync(ctx->d_time_score, st));
+    ctx->d_time_score = nullptr;
+    ctx->time_score_bytes = 0;
+    CK(cudaMallocAsync(&ctx->d_time_score, need, st));
+    ctx->time_score_bytes = need;
+  }
+  cudaError_t e = cudaSuccess;
+  for (size_t k = 0; k + 1 < starts.size() && e == cudaSuccess; ++k) {
+    const int s = starts[k], nb = starts[k + 1] - starts[k];
+    TimeScoreParams p;
+    memset(&p, 0, sizeof p);
+    p.batch = nb;
+    p.est = est + est_offsets[s];
+    p.tgt = target + target_offsets[s];
+    for (int i = 0; i <= nb; ++i) {
+      p.e_off[i] = est_offsets[s + i] - est_offsets[s];
+      p.t_off[i] = target_offsets[s + i] - target_offsets[s];
+    }
+    for (int i = 0; i < nb; ++i) {
+      const int64_t n10 = stoi_len10(N[s + i]), nf = stoi_frames(n10);
+      p.r_off[i + 1] = p.r_off[i] + n10;
+      p.f_off[i + 1] = p.f_off[i] + nf;
+      p.tile_off[i + 1] = p.tile_off[i] + stoi_tiles(nf);
+    }
+    stoi_bands(p.band_lo, p.band_hi);
+    p.clip = 1 + std::pow(10.0, 15.0 / 20);
+    p.taps = ctx->d_stoi_tables;
+    p.window = ctx->d_stoi_tables + STOI_WIN_AT;
+    p.tw256 = reinterpret_cast<const double2*>(ctx->d_stoi_tables + STOI_TW256_AT);
+    p.tw512 = reinterpret_cast<const double2*>(ctx->d_stoi_tables + STOI_TW512_AT);
+    const int64_t Rs = p.r_off[nb], Fs = p.f_off[nb], Ts = p.tile_off[nb];
+    double* d = static_cast<double*>(ctx->d_time_score);
+    p.rs = d;
+    p.cs = p.rs + 2 * Rs;
+    p.energy = p.cs + 2 * Rs;
+    p.tob = p.energy + Fs;
+    p.partial = p.tob + 2 * STOI_BANDS * Fs;
+    p.src = reinterpret_cast<int*>(p.partial + Ts);
+    p.kept = p.src + Fs;
+    p.out = out + (size_t)s * 2;
+    e = launch_score_time(p, st);
+    ctx->launches += Ts > 0 ? 8 : 7;
+  }
+  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "time score launch: %s", cudaGetErrorString(e));
+  CK(cudaEventRecord(ctx->time_score_ev, st));
+  ctx->time_score_used = true;
   return VF_OK;
 }
 

@@ -209,6 +209,13 @@ struct vf_ctx {
   size_t score_bytes = 0;
   cudaEvent_t score_ev = nullptr;
   bool score_used = false;
+  // vf_score_time_varlen: its float64 tables (resampling taps, window, twiddles; designed on first use) and its scratch,
+  // held and ordered like d_score's
+  double* d_stoi_tables = nullptr;
+  void* d_time_score = nullptr;
+  size_t time_score_bytes = 0;
+  cudaEvent_t time_score_ev = nullptr;
+  bool time_score_used = false;
   // UNet weights: the mel-domain analysis module of VoiceFixer (prefix generator.analysis_module.) and the
   // linear-spectrogram unet_v2 of SSR_UNet / GSR_UNet (prefix generator.unet.); either may be absent
   UnetW gsr, ssr;

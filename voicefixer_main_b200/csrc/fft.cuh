@@ -113,4 +113,47 @@ __device__ __forceinline__ double2 rfft_split(const double2* Z, const double2* _
   return make_double2(e.x + wo.x, e.y + wo.y);
 }
 
+// ---- fp64 256-point complex FFT and the 512-point real split, for STOI's STFT (speech_metrics.cu).  The same radix-4
+// Stockham passes with 64 threads per transform (tid 0..63); several transforms may share a block, since every thread of
+// the block runs the four passes and their __syncthreads.  tw256[j] = e^{-2 pi i j / 256}.
+__device__ __forceinline__ double2* fft256_forward(double2* buf0, double2* buf1, const double2* __restrict__ tw256, int tid) {
+  double2* src = buf0;
+  double2* dst = buf1;
+#pragma unroll
+  for (int pass = 0; pass < 4; ++pass) {
+    const int ns = 1 << (2 * pass);
+    const int k = tid & (ns - 1);
+    const int tw_step = k * (64 / ns);
+    double2 a = src[tid];
+    double2 bq = src[tid + 64];
+    double2 c = src[tid + 128];
+    double2 d = src[tid + 192];
+    if (pass > 0) {
+      bq = cmul(bq, __ldg(tw256 + tw_step));
+      c = cmul(c, __ldg(tw256 + 2 * tw_step));
+      d = cmul(d, __ldg(tw256 + 3 * tw_step));
+    }
+    const double2 s0 = make_double2(a.x + c.x, a.y + c.y), s1 = make_double2(a.x - c.x, a.y - c.y);
+    const double2 s2 = make_double2(bq.x + d.x, bq.y + d.y), s3 = make_double2(bq.x - d.x, bq.y - d.y);
+    const int o = ((tid - k) << 2) + k;
+    dst[o] = make_double2(s0.x + s2.x, s0.y + s2.y);
+    dst[o + ns] = make_double2(s1.x + s3.y, s1.y - s3.x);          // s1 - i*s3
+    dst[o + 2 * ns] = make_double2(s0.x - s2.x, s0.y - s2.y);
+    dst[o + 3 * ns] = make_double2(s1.x - s3.y, s1.y + s3.x);      // s1 + i*s3
+    __syncthreads();
+    double2* tmp = src; src = dst; dst = tmp;
+  }
+  return src;   // four passes: buf0
+}
+
+// Bin k (0..256) of the 512-point real DFT from the packed 256-point spectrum Z.  tw512[k] = e^{-2 pi i k / 512}.
+__device__ __forceinline__ double2 rfft512_split(const double2* Z, const double2* __restrict__ tw512, int k) {
+  const double2 zk = Z[k & 255];
+  const double2 zr = Z[(256 - k) & 255];
+  const double2 e = make_double2(0.5 * (zk.x + zr.x), 0.5 * (zk.y - zr.y));
+  const double2 o = make_double2(0.5 * (zk.y + zr.y), -0.5 * (zk.x - zr.x));
+  const double2 wo = cmul(o, __ldg(tw512 + k));
+  return make_double2(e.x + wo.x, e.y + wo.y);
+}
+
 }  // namespace vf

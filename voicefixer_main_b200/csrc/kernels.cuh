@@ -300,4 +300,45 @@ inline int ssim_tiles(long T, int F) {
 }
 cudaError_t launch_ssim(const SsimParams& p, double* out, int out_stride, cudaStream_t stream);
 
+// speech_metrics.cu: the time-domain keys of AudioMetrics.evaluation (metrics.py:58-64), speechmetrics' sisdr and stoi
+// (pystoi 0.3.3, extended=False) for pairs of packed 44.1 kHz clips, all in float64.  A pair is zero-padded at the end to
+// its longer clip (N_b samples) by index math.  STOI's pipeline runs at 10 kHz: resample (100/441, Octave's 31947-tap
+// window), the target's frame energies, the silent-frame mask and its kept-frame scan, the overlap-add of the kept frames
+// into a compacted buffer, a 512-point STFT with the 15 one-third-octave band values per frame, and the 30-frame segment
+// correlations, summed per tile and then per pair in a fixed order.  The silence removal makes the frame count of a pair
+// a device value (kept[b] - 1 STFT frames); the buffers and grids are sized by its host-known upper bound, and slots past
+// it are skipped.  Every value depends on its own pair only, so a pair's bits do not depend on its batch.
+constexpr int STOI_UP = 100, STOI_DOWN = 441;   // 44.1 kHz -> 10 kHz
+constexpr int STOI_HALF = 15973;               // half length of the resampling filter (2 * 15973 + 1 taps)
+constexpr int STOI_FRAME = 256, STOI_HOP = 128, STOI_BANDS = 15, STOI_SEG = 30;
+// 10 kHz samples of a pair of padded length n, and its frames before silence removal (starts range(0, n10 - 256, 128))
+inline int64_t stoi_len10(int64_t n) { return (n * STOI_UP + STOI_DOWN - 1) / STOI_DOWN; }
+inline int64_t stoi_frames(int64_t n10) { return n10 > STOI_FRAME ? (n10 - STOI_FRAME + STOI_HOP - 1) / STOI_HOP : 0; }
+// correlation tiles of 256 (segment, band) items for at most nF - 1 STFT frames (nF - 30 segments)
+inline int64_t stoi_tiles(int64_t nF) { return nF > STOI_SEG ? ((nF - STOI_SEG) * STOI_BANDS + 255) / 256 : 0; }
+struct TimeScoreParams {
+  const float* est;                          // packed samples: pair b = est[e_off[b] .. e_off[b + 1]), target likewise
+  const float* tgt;
+  int batch;
+  int64_t e_off[SCORE_MAX_IMAGES + 1], t_off[SCORE_MAX_IMAGES + 1];
+  int64_t r_off[SCORE_MAX_IMAGES + 1];       // 10 kHz samples: stoi_len10(N_b)
+  int64_t f_off[SCORE_MAX_IMAGES + 1];       // frame slots: stoi_frames
+  int64_t tile_off[SCORE_MAX_IMAGES + 1];    // correlation tiles: stoi_tiles
+  int band_lo[STOI_BANDS], band_hi[STOI_BANDS];   // band k = rfft bins [band_lo[k], band_hi[k])
+  double clip;                               // 1 + 10^(15 / 20)
+  const double* taps;                        // [2 * STOI_HALF + 1] Octave's window / its sum * 100
+  const double* window;                      // [256] np.hanning(258)[1:-1]
+  const double2* tw256;                      // e^{-2 pi i j / 256}
+  const double2* tw512;                      // e^{-2 pi i k / 512}, k = 0..256
+  double* rs;                                // [2][r_off[batch]] resampled target (0) and estimate (1)
+  double* cs;                                // [2][r_off[batch]] their compacted signals ((kept + 1) * 128 <= n10 samples)
+  double* energy;                            // [f_off[batch]] the target's frame energies, dB
+  double* tob;                               // [2][f_off[batch]][15] band values of the STFT frames
+  double* partial;                           // [tile_off[batch]] correlation tile sums
+  int* src;                                  // [f_off[batch]] kept frame k of pair b -> its frame index
+  int* kept;                                 // [batch] kept frames
+  double* out;                               // [batch][2]: sisdr, stoi
+};
+cudaError_t launch_score_time(const TimeScoreParams& p, cudaStream_t stream);   // eight launches
+
 }  // namespace vf

@@ -10,12 +10,17 @@
 * `AudioMetrics.wav_to_spectrogram` / `.evaluation` / `.evaluation_batch`: scoring a restored file against its clean target
   (metrics.py:37-81), the second half of evaluation_proc/eval.py's evaluation().  The spectrogram is librosa 0.8's STFT
   (reflect padding; librosa >= 0.10 pads with zeros, not built) and SSIM is scikit-image <= 0.18's float64
-  structural_similarity with data_range 2 (>= 0.19 computes float32 and needs data_range, not built).  sisdr, stoi and pesq
-  come from the third-party speechmetrics package (CPU) and are not produced.
+  structural_similarity with data_range 2 (>= 0.19 computes float32 and needs data_range, not built).
+* `evaluation(..., time_domain=True)` / `evaluation_batch(..., time_domain=True)` add the sisdr and stoi keys, which the
+  reference gets from the third-party speechmetrics package on the CPU (metrics.py:58-64): SI-SDR as speechmetrics
+  computes it and pystoi 0.3.3's STOI, restated in oracle/speech_metrics.py and computed in float64 by
+  vf_score_time_varlen.  pesq (ITU-T P.862, a large reference C program under its own licence) and bsseval are not
+  produced.
 
 The filter design is host arithmetic (numpy); every sample / reduction is computed by libb200vf kernels (edges.cu).
 """
 import ctypes
+import wave
 from fractions import Fraction
 
 import numpy as np
@@ -63,6 +68,18 @@ def resample_to(eng: Engine, x: torch.Tensor, rate_in: int, rate_out: int = 4410
 # AudioMetrics.evaluation's keys (metrics.py:70-78) in the column order of Engine.score_varlen
 SCORE_KEYS = ("lsd", "non_log_sispec", "sispec", "ssim", "final_mel_lsd", "final_non_log_mel_sispec", "final_mel_sispec",
               "final_mel_ssim")
+# its time-domain keys (metrics.py:58-64, without pesq) in the column order of Engine.score_time_varlen
+TIME_KEYS = ("sisdr", "stoi")
+
+
+def first_channel(path) -> np.ndarray:
+    """The first channel of a 16-bit PCM wav as speechmetrics reads it (soundfile, float64 int16 / 32768), held as float32,
+    which represents every such value exactly."""
+    with wave.open(path, "rb") as w:
+        if w.getsampwidth() != 2:
+            raise ValueError(f"{path}: need 16-bit PCM (got {8 * w.getsampwidth()} bit)")
+        data = np.frombuffer(w.readframes(w.getnframes()), dtype=np.int16).reshape(-1, w.getnchannels())
+    return np.ascontiguousarray(data[:, 0].astype(np.float32) / np.float32(32768.0))
 
 
 def check_rate(rate: int, what) -> None:
@@ -130,19 +147,25 @@ class AudioMetrics:
         sp, mel = eng.metric_spectrogram(x, [x.numel()])
         return sp[None, None], mel[None, None]
 
-    def evaluation(self, est, target) -> dict:
-        """metrics.py:53-81 for one (est, target) pair of wav paths: the 8 spectral keys; {} when target is None."""
-        return self.evaluation_batch([(est, target)])[0]
+    def evaluation(self, est, target, time_domain: bool = False) -> dict:
+        """metrics.py:53-81 for one (est, target) pair of wav paths: the 8 spectral keys; {} when target is None.  With
+        time_domain, also sisdr and stoi (see evaluation_batch)."""
+        return self.evaluation_batch([(est, target)], time_domain=time_domain)[0]
 
-    def evaluation_batch(self, pairs) -> list:
+    def evaluation_batch(self, pairs, time_domain: bool = False) -> list:
         """evaluation(est, target) of every pair, in order, in one vf_score_varlen call: each dict is float-identical to
         evaluation() of that pair.  Every file is decoded and checked before any GPU work; a bad pair fails the whole call,
         naming the file: a target at 16 kHz (NotImplementedError) or at another rate than 44.1 kHz (ValueError), an est
-        whose frame count differs from its target's or a pair of fewer than 7 frames (ValueError)."""
+        whose frame count differs from its target's or a pair of fewer than 7 frames (ValueError).
+
+        time_domain=True adds speechmetrics' sisdr and stoi (one more call, vf_score_time_varlen, on each file's first
+        channel as speechmetrics reads it), and each dict is {"sisdr", "stoi", <the 8 spectral keys>} in metrics.py's
+        order, without pesq.  The spectral values are those of time_domain=False.  The est must then be at the target's
+        44.1 kHz (ValueError naming it): speechmetrics would compare samples at two rates, which is not reproduced."""
         from .arch import frames_for
         from .handler import _rate_len, _to_rate, read_pcm16
         eng = self._eng()
-        decoded = []
+        decoded, channels = [], []
         for est, target in pairs:
             if target is None:
                 decoded.append(None)
@@ -150,12 +173,16 @@ class AudioMetrics:
             t, rate = read_pcm16(target)
             check_rate(rate, target)
             e, e_rate = read_pcm16(est)
+            if time_domain and e_rate != rate:
+                raise ValueError(f"{est} is at {e_rate} Hz: sisdr / stoi need it at its target's {rate} Hz")
             te, tt = frames_for(_rate_len(len(e), e_rate, rate)), frames_for(len(t))
             if te != tt:
                 raise ValueError(f"{est} has {te} frames at {rate} Hz, its target {target} {tt}")
             if tt < 7:
                 raise ValueError(f"{est} / {target}: {tt} frames, fewer than SSIM's 7x7 window")
             decoded.append((est, e, e_rate, t))
+            if time_domain:       # 7 frames are more than STOI's one frame at 10 kHz: no check of its own
+                channels.append((first_channel(est), first_channel(target)))
         live = [d for d in decoded if d is not None]
         results = [{} for _ in decoded]
         if not live:
@@ -165,7 +192,13 @@ class AudioMetrics:
         scores = eng.score_varlen(torch.from_numpy(np.concatenate(ests)).to(eng.device), [len(e) for e in ests],
                                   torch.from_numpy(np.concatenate(tgts)).to(eng.device), [len(t) for t in tgts]).cpu()
         rows = iter(scores.tolist())
+        if time_domain:
+            ests, tgts = [e for e, _ in channels], [t for _, t in channels]
+            td = eng.score_time_varlen(torch.from_numpy(np.concatenate(ests)).to(eng.device), [len(e) for e in ests],
+                                       torch.from_numpy(np.concatenate(tgts)).to(eng.device), [len(t) for t in tgts])
+            time_rows = iter(td.cpu().tolist())
         for i, d in enumerate(decoded):
             if d is not None:
-                results[i] = dict(zip(SCORE_KEYS, next(rows)))
+                spectral = dict(zip(SCORE_KEYS, next(rows)))
+                results[i] = dict(zip(TIME_KEYS, next(time_rows)), **spectral) if time_domain else spectral
         return results

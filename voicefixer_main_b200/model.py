@@ -297,6 +297,19 @@ class Engine:
                                               len(est_off) - 1, _ptr(out), _stream()))
         return out
 
+    def score_time_varlen(self, est_packed: torch.Tensor, est_lengths, target_packed: torch.Tensor, target_lengths) -> torch.Tensor:
+        """vf_score_time_varlen: speechmetrics' sisdr and stoi of each (est, target) pair of two packed 44.1 kHz sets ->
+        float64 [pairs, 2], columns sisdr, stoi.  The clips of a pair may differ in length (the shorter is zero-padded)."""
+        est_packed, est_off = self._varlen_args(est_packed, est_lengths)
+        target_packed, target_off = self._varlen_args(target_packed, target_lengths)
+        if len(est_off) != len(target_off):
+            raise ValueError("score_time_varlen: est and target must hold the same number of clips")
+        out = torch.empty(len(est_off) - 1, 2, dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_score_time_varlen(self.ctx, _ptr(est_packed), est_off, _ptr(target_packed), target_off,
+                                                   len(est_off) - 1, _ptr(out), _stream()))
+        return out
+
     def amp_to_original_f(self, mel_est: torch.Tensor, mel_target: torch.Tensor) -> torch.Tensor:
         """tools/utils.py:50-55 on linear mels [B,T,128]: the estimate scaled to the target's low-band energy."""
         mel_est, mel_target = _check_in(mel_est, self.device, "mel_est"), _check_in(mel_target, self.device, "mel_target")
