@@ -35,6 +35,9 @@
  *   vf_ssim                       AudioMetrics.ssim metrics.py:97-106 (scikit-image structural_similarity, win_size 7)
  *   vf_score_varlen               the spectral part of AudioMetrics.evaluation metrics.py:53-81 for a set of file pairs
  *   vf_score_time_varlen          its sisdr and stoi keys (speechmetrics, metrics.py:58-64) for a set of file pairs
+ *   vf_sosfiltfilt_varlen         the IIR types of tools/dsp/lowpass.py lowpass() / bandpass() (scipy sosfiltfilt)
+ *   vf_resample_poly_f64_varlen   its "stft" type (resample_poly down and up), collate_fn_val's SR inputs
+ *                                 dataloaders/data_module.py:130-150
  *
  * Conventions: every function returns 0 on success or a negative VF_E* code and never throws; the message is
  * available from vf_last_error().  All tensor arguments are contiguous fp32.  Unless a name ends in `_host`,
@@ -272,6 +275,33 @@ VF_API int vf_score_varlen(vf_ctx* ctx, const float* est, const int64_t* est_off
  * longer pair runs alone); eight launches per sub-batch.  Needs no weights.  PESQ is not computed. */
 VF_API int vf_score_time_varlen(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target,
                                 const int64_t* target_offsets, int batch, double* out, void* stream);
+
+/* scipy.signal.sosfiltfilt(sos, x) (padtype "odd", default padlen) of `batch` packed FLOAT64 rows, each with its own filter:
+ * x and out are device float64, packed with HOST offsets [batch + 1]; row i uses filter row_filter[i] (host) of
+ * `n_filters` second-order-section filters given on the HOST as sos [n_filters][10][6] and sosfilt_zi(sos)
+ * [n_filters][10][2], filter f using its first n_sections[f] (1 .. 10) rows.  row_f32 (host, or NULL for none) marks rows
+ * whose samples came from float32 input: numpy builds sosfiltfilt's odd extension in the input's dtype, so theirs is
+ * rounded to float32 (the filtering itself is float64 either way, as in scipy).  Filter f's padlen is 3 * (2 n_sections + 1 -
+ * min(#(sos[:, 2] == 0), #(sos[:, 5] == 0))); every row must be longer than its padlen, and sos[:, 3] must be 1, else
+ * VF_EINVAL naming the row or filter before any work is queued.  float64 throughout: the odd extension is index math, each
+ * pass (forward from zi * x_ext[0], backward from zi * y[-1]) is an exact chunked scan whose only error is fp64 rounding, in
+ * scipy's per-sample section order.  A row's bits do not depend on its batch or position.  Each filter's table (sos, zi and
+ * its 1024-step transition matrix) is designed on the device by one more launch per 6 filters, in the call's scratch: no
+ * host synchronisation and nothing kept between calls.  The scratch is owned by the context and allocated stream-ordered.
+ * Rows run in sub-batches of at most 64 rows and 2^24 extended samples (a longer row runs alone); six launches per
+ * sub-batch. */
+VF_API int vf_sosfiltfilt_varlen(vf_ctx* ctx, const double* x, const int64_t* offsets, int batch, const double* sos,
+                                 const double* zi, const int* n_sections, int n_filters, const int* row_filter, const int* row_f32,
+                                 double* out, void* stream);
+/* scipy.signal.resample_poly(x, up, down) of `batch` packed FLOAT64 rows in float64: x packed with HOST in_offsets, y with HOST
+ * out_offsets.  Row i uses filter row_filter[i] (host) of `n_filters`: up[f], down[f] >= 1 (already reduced by their gcd)
+ * and the odd-length float64 taps taps[tap_offsets[f] .. tap_offsets[f + 1]) (device; host tap_offsets), firwin x up as
+ * resample_poly designs them.  Row i writes out_offsets[i + 1] - out_offsets[i] samples: resample_poly's first
+ * ceil(n up / down) and zeros past them, so an output length other than ceil(n up / down) is align_length's pad or cut.
+ * No scratch; one launch per 64 rows. */
+VF_API int vf_resample_poly_f64_varlen(vf_ctx* ctx, const double* x, const int64_t* in_offsets, int batch, const double* taps,
+                                       const int64_t* tap_offsets, const int* up, const int* down, int n_filters,
+                                       const int* row_filter, double* y, const int64_t* out_offsets, void* stream);
 
 VF_API int vf_to_log(vf_ctx* ctx, const float* in, float* out, int64_t n, void* stream);
 VF_API int vf_from_log(vf_ctx* ctx, const float* in, float* out, int64_t n, void* stream);

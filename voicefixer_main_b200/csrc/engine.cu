@@ -664,6 +664,8 @@ VF_API void vf_destroy(vf_ctx* ctx) {
   if (ctx->d_stoi_tables) cudaFree(ctx->d_stoi_tables);
   if (ctx->d_time_score) cudaFree(ctx->d_time_score);
   if (ctx->time_score_ev) cudaEventDestroy(ctx->time_score_ev);
+  if (ctx->d_iir) cudaFree(ctx->d_iir);
+  if (ctx->iir_ev) cudaEventDestroy(ctx->iir_ev);
   delete ctx;
 }
 
@@ -1253,6 +1255,169 @@ VF_API int vf_score_time_varlen(vf_ctx* ctx, const float* est, const int64_t* es
   if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "time score launch: %s", cudaGetErrorString(e));
   CK(cudaEventRecord(ctx->time_score_ev, st));
   ctx->time_score_used = true;
+  return VF_OK;
+}
+
+namespace {
+
+// Checked offsets of `batch` packed rows: start at 0, each row at least `min_len` samples.
+bool rows_ok(vf_ctx* ctx, const char* fn, const int64_t* off, int batch, int64_t min_len, const char* what) {
+  if (off[0] != 0) { fail(ctx, VF_EINVAL, "%s: %s offsets must start at 0", fn, what); return false; }
+  for (int i = 0; i < batch; ++i)
+    if (off[i + 1] - off[i] < min_len) {
+      fail(ctx, VF_EINVAL, "%s: %s row %d has %ld samples (need at least %ld)", fn, what, i, (long)(off[i + 1] - off[i]),
+           (long)min_len);
+      return false;
+    }
+  return true;
+}
+
+}  // namespace
+
+VF_API int vf_sosfiltfilt_varlen(vf_ctx* ctx, const double* x, const int64_t* offsets, int batch, const double* sos,
+                                 const double* zi, const int* n_sections, int n_filters, const int* row_filter, const int* row_f32,
+                                 double* out, void* stream) {
+  static const char* fn = "vf_sosfiltfilt_varlen";
+  if (!ctx || !x || !offsets || !sos || !zi || !n_sections || !row_filter || !out || batch <= 0 || n_filters <= 0)
+    return ctx ? fail(ctx, VF_EINVAL, "%s: bad arguments", fn) : VF_EINVAL;
+  if (!rows_ok(ctx, fn, offsets, batch, 1, "x")) return VF_EINVAL;
+  std::vector<int> edge(n_filters);
+  for (int f = 0; f < n_filters; ++f) {
+    const int ns = n_sections[f];
+    if (ns < 1 || ns > IIR_MAX_SECTIONS) return fail(ctx, VF_EINVAL, "%s: filter %d has %d sections (need 1 .. %d)", fn, f, ns, IIR_MAX_SECTIONS);
+    const double* s = sos + (size_t)f * 6 * IIR_MAX_SECTIONS;
+    int zb = 0, za = 0;
+    for (int k = 0; k < ns; ++k) {
+      if (s[6 * k + 3] != 1.0) return fail(ctx, VF_EINVAL, "%s: filter %d: sos[%d, 3] is not 1", fn, f, k);
+      zb += s[6 * k + 2] == 0.0;
+      za += s[6 * k + 5] == 0.0;
+    }
+    edge[f] = 3 * (2 * ns + 1 - std::min(zb, za));        // sosfiltfilt's default padlen
+  }
+  std::vector<int64_t> ne(batch);
+  for (int i = 0; i < batch; ++i) {
+    const int f = row_filter[i];
+    if (f < 0 || f >= n_filters) return fail(ctx, VF_EINVAL, "%s: row %d: filter %d of %d", fn, i, f, n_filters);
+    const int64_t n = offsets[i + 1] - offsets[i];
+    if (n <= edge[f]) return fail(ctx, VF_EINVAL, "%s: row %d has %ld samples, not more than its padlen %d", fn, i, (long)n, edge[f]);
+    ne[i] = n + 2 * (int64_t)edge[f];
+  }
+  CK(cudaSetDevice(ctx->device));
+  auto chunks = [](int64_t n) { return (n + IIR_CHUNK - 1) / IIR_CHUNK; };
+  auto bytes_of = [](int64_t E, int64_t C) { return (size_t)(E + C * IIR_MAX_STATES) * sizeof(double); };
+  // consecutive sub-batches of at most IIR_MAX_ROWS rows and IIR_CAP_SAMPLES extended samples; a longer row runs alone
+  std::vector<int> starts{0};
+  int64_t E = 0, C = 0;
+  size_t need = 0;
+  for (int i = 0; i < batch; ++i) {
+    const int n_in = i - starts.back();
+    if (n_in == IIR_MAX_ROWS || (n_in > 0 && E + ne[i] > IIR_CAP_SAMPLES)) {
+      need = std::max(need, bytes_of(E, C));
+      starts.push_back(i);
+      E = C = 0;
+    }
+    E += ne[i];
+    C += chunks(ne[i]);
+  }
+  need = std::max(need, bytes_of(E, C));
+  starts.push_back(batch);
+  const size_t table_doubles = (size_t)n_filters * IIR_TABLE;     // the call's filter tables lead the scratch
+  need += table_doubles * sizeof(double);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (ctx->iir_used) CK(cudaStreamWaitEvent(st, ctx->iir_ev, 0));
+  if (!ctx->iir_ev) CK(cudaEventCreateWithFlags(&ctx->iir_ev, cudaEventDisableTiming));
+  if (need > ctx->iir_bytes) {               // stream-ordered: no host synchronisation
+    if (ctx->d_iir) CK(cudaFreeAsync(ctx->d_iir, st));
+    ctx->d_iir = nullptr;
+    ctx->iir_bytes = 0;
+    CK(cudaMallocAsync(&ctx->d_iir, need, st));
+    ctx->iir_bytes = need;
+  }
+  double* tables = static_cast<double*>(ctx->d_iir);
+  cudaError_t e = cudaSuccess;
+  for (int f0 = 0; f0 < n_filters && e == cudaSuccess; f0 += IIR_DESIGN_FILTERS) {   // sos and zi go as kernel parameters
+    IirDesignParams d;
+    memset(&d, 0, sizeof d);
+    d.tables = tables + (size_t)f0 * IIR_TABLE;
+    d.n = std::min(IIR_DESIGN_FILTERS, n_filters - f0);
+    for (int i = 0; i < d.n; ++i) {
+      const int f = f0 + i;
+      d.n_sections[i] = n_sections[f];
+      std::copy(sos + (size_t)f * 6 * IIR_MAX_SECTIONS, sos + (size_t)f * 6 * IIR_MAX_SECTIONS + 6 * n_sections[f], d.sos[i]);
+      std::copy(zi + (size_t)f * 2 * IIR_MAX_SECTIONS, zi + (size_t)f * 2 * IIR_MAX_SECTIONS + 2 * n_sections[f], d.zi[i]);
+    }
+    e = launch_iir_design(d, st);
+    ctx->launches += 1;
+  }
+  for (size_t k = 0; k + 1 < starts.size() && e == cudaSuccess; ++k) {
+    const int s = starts[k], nb = starts[k + 1] - starts[k];
+    SosParams p;
+    memset(&p, 0, sizeof p);
+    p.batch = nb;
+    p.x = x + offsets[s];
+    p.out = out + offsets[s];
+    for (int i = 0; i < nb; ++i) {
+      const int f = row_filter[s + i];
+      p.off[i + 1] = offsets[s + i + 1] - offsets[s];
+      p.ext_off[i + 1] = p.ext_off[i] + ne[s + i];
+      p.chunk_off[i + 1] = p.chunk_off[i] + chunks(ne[s + i]);
+      p.edge[i] = edge[f];
+      p.ext_f32[i] = row_f32 ? row_f32[s + i] != 0 : 0;
+      p.n_sections[i] = n_sections[f];
+      p.table[i] = tables + (size_t)f * IIR_TABLE;
+    }
+    p.yf = tables + table_doubles;
+    p.state = p.yf + p.ext_off[nb];
+    e = launch_sosfiltfilt(p, st);
+    ctx->launches += 6;
+  }
+  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "sosfiltfilt launch: %s", cudaGetErrorString(e));
+  CK(cudaEventRecord(ctx->iir_ev, st));
+  ctx->iir_used = true;
+  return VF_OK;
+}
+
+VF_API int vf_resample_poly_f64_varlen(vf_ctx* ctx, const double* x, const int64_t* in_offsets, int batch, const double* taps,
+                                       const int64_t* tap_offsets, const int* up, const int* down, int n_filters,
+                                       const int* row_filter, double* y, const int64_t* out_offsets, void* stream) {
+  static const char* fn = "vf_resample_poly_f64_varlen";
+  if (!ctx || !x || !in_offsets || !taps || !tap_offsets || !up || !down || !row_filter || !y || !out_offsets || batch <= 0 ||
+      n_filters <= 0)
+    return ctx ? fail(ctx, VF_EINVAL, "%s: bad arguments", fn) : VF_EINVAL;
+  if (!rows_ok(ctx, fn, in_offsets, batch, 1, "x") || !rows_ok(ctx, fn, out_offsets, batch, 0, "y")) return VF_EINVAL;
+  if (tap_offsets[0] != 0) return fail(ctx, VF_EINVAL, "%s: tap offsets must start at 0", fn);
+  for (int f = 0; f < n_filters; ++f) {
+    const int64_t nt = tap_offsets[f + 1] - tap_offsets[f];
+    if (nt < 1 || nt % 2 == 0 || nt > (int64_t(1) << 30))
+      return fail(ctx, VF_EINVAL, "%s: filter %d has %ld taps (need an odd count)", fn, f, (long)nt);
+    if (up[f] < 1 || down[f] < 1) return fail(ctx, VF_EINVAL, "%s: filter %d: up %d, down %d (need >= 1)", fn, f, up[f], down[f]);
+  }
+  for (int i = 0; i < batch; ++i)
+    if (row_filter[i] < 0 || row_filter[i] >= n_filters)
+      return fail(ctx, VF_EINVAL, "%s: row %d: filter %d of %d", fn, i, row_filter[i], n_filters);
+  CK(cudaSetDevice(ctx->device));
+  cudaError_t e = cudaSuccess;
+  for (int s = 0; s < batch && e == cudaSuccess; s += IIR_MAX_ROWS) {
+    const int nb = std::min(IIR_MAX_ROWS, batch - s);
+    ResampleF64Params p;
+    memset(&p, 0, sizeof p);
+    p.batch = nb;
+    p.x = x + in_offsets[s];
+    p.y = y + out_offsets[s];
+    p.taps = taps;
+    for (int i = 0; i < nb; ++i) {
+      const int f = row_filter[s + i];
+      p.in_off[i + 1] = in_offsets[s + i + 1] - in_offsets[s];
+      p.out_off[i + 1] = out_offsets[s + i + 1] - out_offsets[s];
+      p.tap_at[i] = tap_offsets[f];
+      p.half[i] = (int)((tap_offsets[f + 1] - tap_offsets[f] - 1) / 2);
+      p.up[i] = up[f];
+      p.down[i] = down[f];
+    }
+    e = launch_resample_f64(p, (cudaStream_t)stream);
+    ctx->launches += 1;
+  }
+  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "resample launch: %s", cudaGetErrorString(e));
   return VF_OK;
 }
 

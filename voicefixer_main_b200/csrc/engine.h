@@ -216,6 +216,11 @@ struct vf_ctx {
   size_t time_score_bytes = 0;
   cudaEvent_t time_score_ev = nullptr;
   bool time_score_used = false;
+  // vf_sosfiltfilt_varlen: the call's filter tables and the scan scratch, held and ordered like d_score's
+  void* d_iir = nullptr;
+  size_t iir_bytes = 0;
+  cudaEvent_t iir_ev = nullptr;
+  bool iir_used = false;
   // UNet weights: the mel-domain analysis module of VoiceFixer (prefix generator.analysis_module.) and the
   // linear-spectrogram unet_v2 of SSR_UNet / GSR_UNet (prefix generator.unet.); either may be absent
   UnetW gsr, ssr;

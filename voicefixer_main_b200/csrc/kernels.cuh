@@ -341,4 +341,58 @@ struct TimeScoreParams {
 };
 cudaError_t launch_score_time(const TimeScoreParams& p, cudaStream_t stream);   // eight launches
 
+// iir.cu: scipy.signal.sosfiltfilt(sos, x) (padtype "odd") of packed float64 rows, each with its own filter, as an exact
+// chunked scan.  Row b's odd extension (edge[b] samples each side, index math) is cut into IIR_CHUNK-sample chunks.  Phase
+// A runs every chunk but the last from zero state and stores its end state; phase B carries the true chunk-start states
+// along the row, s_{k+1} = M s_k + e_k with M = the cascade's IIR_CHUNK-step zero-input transition (iir_design_kernel);
+// phase C runs every chunk again from its true start state, in scipy's per-sample order (sections inner), and writes it.
+// The forward pass writes yf; the backward pass reads yf reversed and writes the cropped output.  Its only error is fp64
+// rounding: no warm-up truncation.
+constexpr int IIR_MAX_SECTIONS = 10, IIR_MAX_STATES = 2 * IIR_MAX_SECTIONS;
+constexpr int IIR_CHUNK = 1024;
+constexpr int IIR_MAX_ROWS = 64;                       // rows per sub-batch
+constexpr int64_t IIR_CAP_SAMPLES = int64_t(1) << 24;   // extended samples per sub-batch (a longer row runs alone)
+// per-filter device table (doubles): sos [10][6] (rows past n_sections unused), zi [20], M [20][20] (zero past 2 n_sections)
+constexpr int IIR_ZI_AT = 6 * IIR_MAX_SECTIONS, IIR_M_AT = IIR_ZI_AT + IIR_MAX_STATES,
+              IIR_TABLE = IIR_M_AT + IIR_MAX_STATES * IIR_MAX_STATES;
+struct SosParams {
+  const double* x;                           // packed input rows: row b = x[off[b] .. off[b + 1])
+  double* out;                               // packed output, same offsets
+  int batch;
+  int64_t off[IIR_MAX_ROWS + 1];
+  int64_t ext_off[IIR_MAX_ROWS + 1];         // row b's extended samples (n + 2 edge) in yf
+  int64_t chunk_off[IIR_MAX_ROWS + 1];       // row b's chunks (ceil((n + 2 edge) / IIR_CHUNK)) in state
+  int edge[IIR_MAX_ROWS];
+  int ext_f32[IIR_MAX_ROWS];                 // row b was float32: its odd extension is rounded to float32, as numpy makes it
+  int n_sections[IIR_MAX_ROWS];
+  const double* table[IIR_MAX_ROWS];         // row b's filter table (IIR_TABLE doubles)
+  double* yf;                                // [ext_off[batch]] forward pass
+  double* state;                             // [chunk_off[batch]][20] chunk end (phase A) / start (phase B) states
+};
+cudaError_t launch_sosfiltfilt(const SosParams& p, cudaStream_t stream);   // six launches
+// The per-call tables of up to IIR_DESIGN_FILTERS filters (one launch; sos and zi travel in the parameters)
+constexpr int IIR_DESIGN_FILTERS = 6;
+struct IirDesignParams {
+  double* tables;                            // [n][IIR_TABLE]
+  int n;
+  int n_sections[IIR_DESIGN_FILTERS];
+  double sos[IIR_DESIGN_FILTERS][6 * IIR_MAX_SECTIONS];
+  double zi[IIR_DESIGN_FILTERS][2 * IIR_MAX_SECTIONS];
+};
+cudaError_t launch_iir_design(const IirDesignParams& p, cudaStream_t stream);
+
+// iir.cu: scipy.signal.resample_poly(x, up, down) of packed float64 rows with float64 taps (firwin x up, odd length 2 half
+// + 1, designed by the caller), one thread per output sample: y[m] = sum_j x[j] h[m down + half - up j].  Row b writes
+// out_off[b + 1] - out_off[b] samples: resample_poly's first ceil(n up / down), then zeros (align_length's pad).
+struct ResampleF64Params {
+  const double* x;
+  double* y;
+  const double* taps;
+  int batch;
+  int64_t in_off[IIR_MAX_ROWS + 1], out_off[IIR_MAX_ROWS + 1];
+  int64_t tap_at[IIR_MAX_ROWS];              // row b's taps start in `taps`
+  int half[IIR_MAX_ROWS], up[IIR_MAX_ROWS], down[IIR_MAX_ROWS];
+};
+cudaError_t launch_resample_f64(const ResampleF64Params& p, cudaStream_t stream);
+
 }  // namespace vf

@@ -43,6 +43,15 @@ def design_filter(up: int, down: int) -> np.ndarray:
     return (h * up).astype(np.float32)
 
 
+def design_filter_f64(up: int, down: int) -> np.ndarray:
+    """resample_poly's own float64 FIR for (up, down) already reduced by their gcd: scipy.signal.firwin(2 * half + 1,
+    1 / max(up, down), window=('kaiser', 5.0)) * up with half = 10 * max(up, down), the taps of
+    Engine.resample_poly_f64_varlen."""
+    from scipy.signal import firwin
+    max_rate = max(up, down)
+    return firwin(2 * 10 * max_rate + 1, 1.0 / max_rate, window=("kaiser", 5.0)) * up
+
+
 def resample_poly(eng: Engine, x: torch.Tensor, up: int, down: int) -> torch.Tensor:
     """x [B, N] float32 on the engine's device -> [B, ceil(N * up / down)]."""
     x = _check_in(x, eng.device, "x")

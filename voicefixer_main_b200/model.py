@@ -25,6 +25,7 @@ import json
 import math
 from typing import Dict, List, Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import _lib as L
@@ -308,6 +309,58 @@ class Engine:
         with torch.cuda.device(self.device):
             self._ck(self.lib.vf_score_time_varlen(self.ctx, _ptr(est_packed), est_off, _ptr(target_packed), target_off,
                                                    len(est_off) - 1, _ptr(out), _stream()))
+        return out
+
+    def _packed64(self, x_packed: torch.Tensor, lengths):
+        """Checked packed float64 input of the float64 varlen calls and its host offsets."""
+        if not isinstance(x_packed, torch.Tensor) or x_packed.dtype != torch.float64 or x_packed.device != self.device:
+            raise TypeError(f"x_packed must be a float64 CUDA tensor on {self.device}")
+        lengths = [int(n) for n in lengths]
+        if x_packed.dim() != 1 or not lengths or sum(lengths) != x_packed.numel():
+            raise ValueError("x_packed must be 1-D and hold exactly sum(lengths) samples of at least one row")
+        return x_packed.contiguous(), (ctypes.c_int64 * (len(lengths) + 1))(0, *itertools.accumulate(lengths))
+
+    def sosfiltfilt_varlen(self, x_packed: torch.Tensor, lengths, sos, zi, row_filter, row_f32=None) -> torch.Tensor:
+        """vf_sosfiltfilt_varlen: scipy.signal.sosfiltfilt(sos[f], row) of each float64 row of x_packed (rows back to back,
+        `lengths` samples each), row i with filter f = row_filter[i]; sos[f] is an [n_sections <= 10, 6] float64 array and
+        zi[f] its sosfilt_zi.  row_f32[i] true: row i holds float32 input, whose odd extension scipy rounds to float32.
+        -> float64, packed like x_packed."""
+        x_packed, off = self._packed64(x_packed, lengths)
+        nf = len(sos)
+        sos_t = (ctypes.c_double * (nf * 60))()
+        zi_t = (ctypes.c_double * (nf * 20))()
+        ns = (ctypes.c_int * nf)()
+        for f, (s, z) in enumerate(zip(sos, zi)):
+            s, z = np.asarray(s, dtype=np.float64), np.asarray(z, dtype=np.float64)
+            ns[f] = s.shape[0]
+            for k, v in enumerate(s[:10].reshape(-1).tolist()):
+                sos_t[f * 60 + k] = v
+            for k, v in enumerate(z[:10].reshape(-1).tolist()):
+                zi_t[f * 20 + k] = v
+        rows = (ctypes.c_int * len(row_filter))(*[int(f) for f in row_filter])
+        f32 = (ctypes.c_int * len(row_filter))(*[int(bool(v)) for v in row_f32]) if row_f32 is not None else None
+        out = torch.empty_like(x_packed)
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_sosfiltfilt_varlen(self.ctx, _ptr(x_packed), off, len(off) - 1, sos_t, zi_t, ns, nf, rows,
+                                                    f32, _ptr(out), _stream()))
+        return out
+
+    def resample_poly_f64_varlen(self, x_packed: torch.Tensor, lengths, filters, row_filter, out_lengths) -> torch.Tensor:
+        """vf_resample_poly_f64_varlen: scipy.signal.resample_poly of each float64 row of x_packed, row i with filter
+        filters[row_filter[i]] = (up, down, taps: float64 device tensor of odd length) -> float64 rows of out_lengths[i]
+        samples packed back to back (ceil(n up / down) is resample_poly's length; more pads zeros, fewer cuts)."""
+        x_packed, off = self._packed64(x_packed, lengths)
+        out_lengths = [int(n) for n in out_lengths]
+        out_off = (ctypes.c_int64 * (len(out_lengths) + 1))(0, *itertools.accumulate(out_lengths))
+        taps = torch.cat([t.to(self.device, torch.float64).reshape(-1) for _, _, t in filters]).contiguous()
+        tap_off = (ctypes.c_int64 * (len(filters) + 1))(0, *itertools.accumulate(t.numel() for _, _, t in filters))
+        up = (ctypes.c_int * len(filters))(*[int(u) for u, _, _ in filters])
+        down = (ctypes.c_int * len(filters))(*[int(d) for _, d, _ in filters])
+        rows = (ctypes.c_int * len(row_filter))(*[int(f) for f in row_filter])
+        out = torch.empty(sum(out_lengths), dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_resample_poly_f64_varlen(self.ctx, _ptr(x_packed), off, len(off) - 1, _ptr(taps), tap_off, up,
+                                                          down, len(filters), rows, _ptr(out), out_off, _stream()))
         return out
 
     def amp_to_original_f(self, mel_est: torch.Tensor, mel_target: torch.Tensor) -> torch.Tensor:
