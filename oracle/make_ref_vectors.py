@@ -4,10 +4,16 @@ Run where the reference tree exists:  python oracle/make_ref_vectors.py
 Writes tests/golden/ref_oracle.npz (small model-level outputs), tests/golden/ref_unet.npz (UNet and handler outputs)
 and tests/golden/ref_ola.npz (overlap-add outputs and call lists).  The tests then compare against these files and
 need no reference tree.  Inputs come from the seeded helpers below (CPU torch generators), which the tests call too.
+
+torch computes log10 (and tanh, exp, sqrt) through MKL's vector math, whose rounding differs between the code paths MKL
+picks for the CPU (AVX512, AVX2, ...).  So the reference's to_log is also written once per path, each with a log10 probe
+that tells the paths apart, to tests/golden/ref_log10_paths.npz; the test compares against the path its CPU runs.
 """
 import importlib.util
 import os
+import subprocess
 import sys
+import tempfile
 
 import numpy as np
 import torch
@@ -21,6 +27,12 @@ from voicefixer_main_b200.arch import UNET_PREFIX        # noqa: E402
 from voicefixer_main_b200.weights import make_state      # noqa: E402
 
 GOLDEN = os.path.join(ROOT, "tests", "golden")
+MKL_PATHS = ("AVX512", "AVX2", "SSE4_2")                 # values of MKL_ENABLE_INSTRUCTIONS
+
+
+def log10_probe():
+    """torch.log10 on fixed inputs: its bits identify the MKL code path of the CPU that runs it."""
+    return torch.log10(torch.linspace(1e-3, 30.0, 4096))
 
 
 def log_helper_inputs():
@@ -112,10 +124,34 @@ def ola_vectors(out):
                 out[key + "_calls"] = np.array(net.calls, dtype=np.int64)
 
 
+def log10_paths(out):
+    """The reference's to_log on log_helper_inputs() and log10_probe() under each of MKL_PATHS, one process per path."""
+    with tempfile.TemporaryDirectory() as d:
+        for isa in MKL_PATHS:
+            f = os.path.join(d, isa + ".npz")
+            subprocess.run([sys.executable, os.path.abspath(__file__), "--log10-path", f], check=True,
+                           env={**os.environ, "MKL_ENABLE_INSTRUCTIONS": isa})
+            g = np.load(f)
+            out[isa + "_log_to"], out[isa + "_probe"] = g["log_to"], g["probe"]
+    for p in MKL_PATHS:                # equal probes must mean equal outputs, or the probe cannot pick the path
+        for q in MKL_PATHS:
+            if np.array_equal(out[p + "_probe"], out[q + "_probe"]):
+                assert np.array_equal(out[p + "_log_to"], out[q + "_log_to"]), (p, q)
+
+
 def main():
     if not ref_import.available():
         raise SystemExit("reference tree not present at " + ref_import.REFERENCE_ROOT)
     torch.set_num_threads(min(16, os.cpu_count() or 1))
+    if "--log10-path" in sys.argv:
+        ref_import.install_shims()
+        from tools.pytorch.pytorch_util import to_log
+        np.savez(sys.argv[sys.argv.index("--log10-path") + 1], log_to=to_log(log_helper_inputs()[0]).numpy(),
+                 probe=log10_probe().numpy())
+        return
+    c = {}
+    log10_paths(c)
+    np.savez_compressed(os.path.join(GOLDEN, "ref_log10_paths.npz"), **c)
     a, b = {}, {}
     model_vectors(a)
     ola_vectors(b)
@@ -123,7 +159,7 @@ def main():
     np.savez_compressed(os.path.join(GOLDEN, "ref_oracle.npz"), **a)
     np.savez_compressed(os.path.join(GOLDEN, "ref_unet.npz"), **big)
     np.savez_compressed(os.path.join(GOLDEN, "ref_ola.npz"), **b)
-    for f in ("ref_oracle.npz", "ref_unet.npz", "ref_ola.npz"):
+    for f in ("ref_oracle.npz", "ref_unet.npz", "ref_ola.npz", "ref_log10_paths.npz"):
         print(f, os.path.getsize(os.path.join(GOLDEN, f)), "bytes")
 
 

@@ -33,7 +33,8 @@ class ToyNet(torch.nn.Module):
     def forward(self, x):
         self.calls.append(tuple(x.shape))
         y = F.conv1d(x[:, :1, :], self.k, padding=self.k.shape[-1] // 2)
-        return {"wav": torch.tanh(y) + 0.1 * y}
+        # softsign from correctly rounded operations: the same bits on every CPU, where tanh's depend on MKL's code path
+        return {"wav": y / (1 + y.abs()) + 0.1 * y}
 
 
 def _signal(n, batch=2):

@@ -5,7 +5,7 @@ import pytest
 import torch
 
 from oracle import vf_oracle as O
-from oracle.make_ref_vectors import log_helper_inputs, small_input, unet_inputs
+from oracle.make_ref_vectors import MKL_PATHS, log10_probe, log_helper_inputs, small_input, unet_inputs
 from conftest import load_golden
 
 
@@ -30,7 +30,10 @@ def test_mel_filterbank_bit_identical(ref):
 def test_log_helpers_match_reference(ref):
     x, y = log_helper_inputs()
     assert torch.equal(torch.from_numpy(ref["log_x"]), x) and torch.equal(torch.from_numpy(ref["log_y"]), y)
-    assert torch.equal(torch.from_numpy(ref["log_to"]), O.to_log(x))
+    paths = load_golden("ref_log10_paths.npz")        # the reference's to_log on each MKL code path
+    isa = [p for p in MKL_PATHS if torch.equal(torch.from_numpy(paths[p + "_probe"]), log10_probe())]
+    assert isa, "this CPU's log10 matches none of the stored MKL code paths: rerun oracle/make_ref_vectors.py"
+    assert torch.equal(torch.from_numpy(paths[isa[0] + "_log_to"]), O.to_log(x))
     assert torch.equal(torch.from_numpy(ref["log_from"]), O.from_log(y))
     with pytest.raises(AssertionError):             # the reference's to_log asserts on negative input as well
         O.to_log(-x - 1)

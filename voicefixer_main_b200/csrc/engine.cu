@@ -1,5 +1,6 @@
-// Host side of libb200vf.so: the context, the plan cache, the run machinery and the C ABI (include/b200vf.h).  Weight
-// packing is in pack.cu, plan building in plan.cu, and the declarations they share in engine.h.
+// Host side of libb200vf.so: the context, the plan cache, the run machinery and the C ABI (include/b200vf.h) of the restore
+// paths, options, profiling and self-tests.  Weight packing is in pack.cu, plan building in plan.cu, the entry points
+// that use no plan in standalone.cu, and the declarations they share in engine.h.
 //
 // A plan is the full, pre-resolved launch list for one (batch, frames) shape: every activation buffer is
 // allocated once, every TMA tensor map is encoded once, and running a stage is a loop of kernel launches on
@@ -30,6 +31,19 @@ int fail(vf_ctx* c, int code, const char* fmt, ...) {
   return code;
 }
 
+int order_use(vf_ctx* ctx, StreamOrder& o, cudaStream_t st) {
+  if (!o.ev) CK(cudaEventCreateWithFlags(&o.ev, cudaEventDisableTiming));
+  if (o.used && o.last_stream != st) CK(cudaStreamWaitEvent(st, o.ev, 0));
+  return VF_OK;
+}
+
+int mark_use(vf_ctx* ctx, StreamOrder& o, cudaStream_t st) {
+  CK(cudaEventRecord(o.ev, st));
+  o.last_stream = st;
+  o.used = true;
+  return VF_OK;
+}
+
 }  // namespace vf
 
 namespace {
@@ -40,7 +54,7 @@ void free_plan(Plan* plan) {
   for (auto& row : plan->io_ev)
     for (auto& e : row)
       if (e) { cudaEventDestroy(e); e = nullptr; }
-  if (plan->ev_last) { cudaEventDestroy(plan->ev_last); plan->ev_last = nullptr; }
+  if (plan->order.ev) { cudaEventDestroy(plan->order.ev); plan->order.ev = nullptr; }
   for (void* p : plan->allocs) cudaFree(p);
   plan->allocs.clear();
 }
@@ -170,19 +184,6 @@ int ensure_io(vf_ctx* ctx, Plan* plan, long n) {
   plan->n_samples = n;
   ctx->plan_bytes += plan->bytes - before;
   return b.rc;
-}
-
-// Orders this use of the plan's buffers after the previous one when that ran on another stream.
-int plan_enter(vf_ctx* ctx, Plan* plan, cudaStream_t st) {
-  if (plan->used && plan->last_stream != st) CK(cudaStreamWaitEvent(st, plan->ev_last, 0));
-  return VF_OK;
-}
-int plan_exit(vf_ctx* ctx, Plan* plan, cudaStream_t st) {
-  if (!plan->ev_last) CK(cudaEventCreateWithFlags(&plan->ev_last, cudaEventDisableTiming));
-  CK(cudaEventRecord(plan->ev_last, st));
-  plan->last_stream = st;
-  plan->used = true;
-  return VF_OK;
 }
 
 // Host-buffer round trip of plan->batch clips of n samples around `body(d_in, d_out, stream)`.  Pipelined mode: H2D on
@@ -379,7 +380,7 @@ int restore_impl(vf_ctx* ctx, Plan* plan, const float* wav, int batch, int64_t n
                  const int64_t* off = nullptr) {
   const int frames = plan->T;
   if (ctx->op_timing) ctx->prof.clear();
-  int rc = plan_enter(ctx, plan, st);
+  int rc = order_use(ctx, plan->order, st);
   if (rc) return rc;
   rc = stage_mark(ctx, 0, st); if (rc) return rc;
   if (off) {
@@ -416,7 +417,7 @@ int restore_impl(vf_ctx* ctx, Plan* plan, const float* wav, int batch, int64_t n
   CK(launch_finalize(f, st));
   ctx->launches++;
   rc = stage_mark(ctx, 4, st); if (rc) return rc;
-  return plan_exit(ctx, plan, st);
+  return mark_use(ctx, plan->order, st);
 }
 
 // One SSR / GSR-UNet chain on `plan`: `batch` clips of n samples, magnitudes from the clips themselves (sp == nullptr) or sp.
@@ -426,7 +427,7 @@ int ssr_impl(vf_ctx* ctx, Plan* plan, const float* sp, const float* wav, int bat
              const int64_t* off = nullptr) {
   const int frames = plan->T;
   if (ctx->op_timing) ctx->prof.clear();
-  int rc = plan_enter(ctx, plan, st);
+  int rc = order_use(ctx, plan->order, st);
   if (rc) return rc;
   rc = stage_mark(ctx, 0, st); if (rc) return rc;
   if (off) {
@@ -452,7 +453,7 @@ int ssr_impl(vf_ctx* ctx, Plan* plan, const float* sp, const float* wav, int bat
   ctx->launches += 2;
   rc = stage_mark(ctx, 3, st); if (rc) return rc;
   rc = stage_mark(ctx, 4, st); if (rc) return rc;
-  return plan_exit(ctx, plan, st);
+  return mark_use(ctx, plan->order, st);
 }
 
 // A batched call as consecutive sub-batches of at most max_cb clips that fit the plan budget (choose_sub_batch, sized for
@@ -537,7 +538,7 @@ int gather_mels(vf_ctx* ctx, const Plan* plan, const std::vector<int64_t>& frame
 
 // vf_restore_varlen (`fn`) and vf_restore_varlen_mels.  With mel_out or log_mel_out, each sub-batch's restore is followed by
 // one gather of its clips' rows t < T_i into the packed outputs at frame offsets F_i = sum_{j<i} T_j, still inside the
-// plan's use on `stream` (plan_exit again after it).
+// plan's use on `stream` (mark_use again after it).
 int restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t* offsets, int batch, float* wav_out,
                    unsigned flags, float* mel_out, float* log_mel_out, cudaStream_t st) {
   int rc = check_varlen_call(ctx, fn, PLAN_VARLEN, wav, offsets, batch, wav_out, flags, VF_RESTORE_UNIFY_ENERGY, [&](int i, int64_t n) {
@@ -556,7 +557,7 @@ int restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t*
     if (r || !mels) return r;
     r = gather_mels(ctx, plan, frame_off, s, b, plan->d_mel, plan->d_logmel_out, mel_out, log_mel_out, st);
     if (r) return r;
-    return plan_exit(ctx, plan, st);
+    return mark_use(ctx, plan->order, st);
   });
 }
 
@@ -587,7 +588,7 @@ int ssr_restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int6
       CK(launch_peak_normalise_varlen(out, plan->d_vl_off, b, (long)n_max, plan->d_peak, st));
       ctx->launches += 2;
     }
-    return plan_exit(ctx, plan, st);
+    return mark_use(ctx, plan->order, st);
   });
 }
 
@@ -659,13 +660,11 @@ VF_API void vf_destroy(vf_ctx* ctx) {
     if (st) cudaStreamDestroy(st);
   for (auto& e : ctx->ev)
     if (e) cudaEventDestroy(e);
-  if (ctx->d_score) cudaFree(ctx->d_score);
-  if (ctx->score_ev) cudaEventDestroy(ctx->score_ev);
+  for (Scratch* s : {&ctx->score, &ctx->time_score, &ctx->iir}) {
+    if (s->p) cudaFree(s->p);
+    if (s->order.ev) cudaEventDestroy(s->order.ev);
+  }
   if (ctx->d_stoi_tables) cudaFree(ctx->d_stoi_tables);
-  if (ctx->d_time_score) cudaFree(ctx->d_time_score);
-  if (ctx->time_score_ev) cudaEventDestroy(ctx->time_score_ev);
-  if (ctx->d_iir) cudaFree(ctx->d_iir);
-  if (ctx->iir_ev) cudaEventDestroy(ctx->iir_ev);
   delete ctx;
 }
 
@@ -712,14 +711,14 @@ VF_API int vf_unet_mel(vf_ctx* ctx, const float* mel_lin, int batch, int frames,
   rc = get_plan(ctx, PLAN_GSR, batch, frames, &plan);
   if (rc) return rc;
   const size_t n = (size_t)batch * frames * 128;
-  rc = plan_enter(ctx, plan, st);
+  rc = order_use(ctx, plan->order, st);
   if (rc) return rc;
   CK(launch_to_log(mel_lin, plan->d_logmel_in, n, ctx->d_err + 1, st));
   ctx->launches++;
   rc = run_ops(ctx, plan->unet, st);
   if (rc) return rc;
   CK(cudaMemcpyAsync(logmel_out, plan->d_logmel_out, n * 4, cudaMemcpyDeviceToDevice, st));
-  return plan_exit(ctx, plan, st);
+  return mark_use(ctx, plan->order, st);
 }
 
 VF_API int64_t vf_vocoder_out_len(vf_ctx* ctx, int frames) {
@@ -735,7 +734,7 @@ VF_API int vf_vocoder(vf_ctx* ctx, const float* mel_lin, int batch, int frames, 
   Plan* plan;
   rc = get_plan(ctx, PLAN_GSR, batch, frames, &plan);
   if (rc) return rc;
-  rc = plan_enter(ctx, plan, st);
+  rc = order_use(ctx, plan->order, st);
   if (rc) return rc;
   Op& cop = plan->vocoder[plan->cond_op];
   cop.cond.mel = mel_lin;
@@ -746,7 +745,7 @@ VF_API int vf_vocoder(vf_ctx* ctx, const float* mel_lin, int batch, int frames, 
   cop.cond.is_log = 1;
   if (rc) return rc;
   CK(cudaMemcpyAsync(wav_out, plan->d_voc_wav, (size_t)batch * plan->L * 4, cudaMemcpyDeviceToDevice, st));
-  return plan_exit(ctx, plan, st);
+  return mark_use(ctx, plan->order, st);
 }
 
 VF_API int vf_restore_ex(vf_ctx* ctx, const float* wav, int batch, int64_t n, float* wav_out, unsigned flags, void* stream) {
@@ -835,13 +834,13 @@ VF_API int vf_ssr_unet(vf_ctx* ctx, const float* sp, int batch, int frames, floa
   rc = get_plan(ctx, PLAN_SSR, batch, frames, &plan);
   if (rc) return rc;
   if (ctx->op_timing) ctx->prof.clear();
-  rc = plan_enter(ctx, plan, st);
+  rc = order_use(ctx, plan->order, st);
   if (rc) return rc;
   plan->unet[0].first.logmel = sp;
   rc = run_ops(ctx, plan->unet, st);
   if (rc) return rc;
   CK(cudaMemcpyAsync(mag_out, plan->d_mag, (size_t)batch * frames * 1025 * 4, cudaMemcpyDeviceToDevice, st));
-  return plan_exit(ctx, plan, st);
+  return mark_use(ctx, plan->order, st);
 }
 
 VF_API int vf_ssr_stages(vf_ctx* ctx, int batch, int64_t n, float* sp_out, float* mag_out, void* stream) {
@@ -852,596 +851,11 @@ VF_API int vf_ssr_stages(vf_ctx* ctx, int batch, int64_t n, float* sp_out, float
   rc = get_plan(ctx, PLAN_SSR, batch, frames, &plan);
   if (rc) return rc;
   const size_t bytes = (size_t)batch * frames * 1025 * 4;
-  rc = plan_enter(ctx, plan, (cudaStream_t)stream);
+  rc = order_use(ctx, plan->order, (cudaStream_t)stream);
   if (rc) return rc;
   if (sp_out) CK(cudaMemcpyAsync(sp_out, plan->d_sp, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   if (mag_out) CK(cudaMemcpyAsync(mag_out, plan->d_mag, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  return plan_exit(ctx, plan, (cudaStream_t)stream);
-}
-
-VF_API int vf_istft(vf_ctx* ctx, const float* real, const float* imag, int batch, int frames, int64_t length, float* wav_out, void* stream) {
-  if (!ctx || !real || !imag || !wav_out || batch <= 0 || frames <= 0 || length <= 0) return ctx ? fail(ctx, VF_EINVAL, "vf_istft: bad arguments") : VF_EINVAL;
-  CK(cudaSetDevice(ctx->device));
-  if (length + 1024 > (int64_t)(frames - 1) * ctx->cfg.hop + 2048)
-    return fail(ctx, VF_EINVAL, "vf_istft: %d frames cover %ld samples, fewer than length %ld + n_fft/2", frames, (long)(frames - 1) * ctx->cfg.hop + 2048, (long)length);
-  cudaStream_t st = (cudaStream_t)stream;
-  float* frames_buf = nullptr;           // stream-ordered scratch: no plan is tied to a bare ISTFT
-  CK(cudaMallocAsync((void**)&frames_buf, (size_t)batch * frames * 2048 * 4, st));
-  IstftFramesParams fp;
-  memset(&fp, 0, sizeof fp);
-  fp.real = real; fp.imag = imag; fp.batch = batch; fp.T = frames;
-  fp.window = ctx->d_window; fp.tw1024 = ctx->d_tw1024; fp.tw2048 = ctx->d_tw2048; fp.frames = frames_buf;
-  cudaError_t e1 = launch_istft_frames(fp, st);
-  IstftOlaParams op;
-  memset(&op, 0, sizeof op);
-  op.frames = frames_buf; op.batch = batch; op.T = frames; op.length = (long)length; op.window = ctx->d_window;
-  op.out = wav_out; op.out_ld = (long)length;
-  cudaError_t e2 = e1 == cudaSuccess ? launch_istft_ola(op, st) : e1;
-  cudaFreeAsync(frames_buf, st);
-  if (e2 != cudaSuccess) return fail(ctx, VF_ECUDA, "istft launch: %s", cudaGetErrorString(e2));
-  ctx->launches += 2;
-  return VF_OK;
-}
-
-// ---------------------------------------------------------------------------------------------- stand-alone boundary ops
-VF_API int vf_mel(vf_ctx* ctx, const float* specgram, int64_t n_outer, int64_t frames, int64_t stride_outer, int64_t stride_freq,
-                  int64_t stride_time, float* mel_out, void* stream) {
-  if (!ctx || !specgram || !mel_out || n_outer <= 0 || frames <= 0 || n_outer > 65535) return ctx ? fail(ctx, VF_EINVAL, "vf_mel: bad arguments") : VF_EINVAL;
-  if (!ctx->d_fb_val) return fail(ctx, VF_ESTATE, "mel filterbank not loaded (call vf_load_weights first)");
-  CK(cudaSetDevice(ctx->device));
-  MelParams p;
-  memset(&p, 0, sizeof p);
-  p.in = specgram; p.n_outer = (long)n_outer; p.T = (long)frames; p.so = (long)stride_outer; p.sf = (long)stride_freq; p.st = (long)stride_time;
-  p.out = mel_out; p.fb_f0 = ctx->d_fb_f0; p.fb_len = ctx->d_fb_len; p.fb_ofs = ctx->d_fb_ofs; p.fb_val = ctx->d_fb_val;
-  CK(launch_mel(p, (cudaStream_t)stream));
-  ctx->launches++;
-  return VF_OK;
-}
-
-VF_API int vf_resample_poly(vf_ctx* ctx, const float* wav, int batch, int64_t n, int up, int down, const float* taps, int n_taps,
-                            float* out, int64_t n_out, void* stream) {
-  if (!ctx || !wav || !taps || !out || batch <= 0 || n <= 0 || up <= 0 || down <= 0 || n_taps < 1 || (n_taps & 1) == 0)
-    return ctx ? fail(ctx, VF_EINVAL, "vf_resample_poly: bad arguments (n_taps must be odd)") : VF_EINVAL;
-  if (n_out != (n * up + down - 1) / down) return fail(ctx, VF_EINVAL, "vf_resample_poly: n_out must be ceil(n * up / down) = %ld", (long)((n * up + down - 1) / down));
-  CK(cudaSetDevice(ctx->device));
-  CK(launch_resample_poly(wav, batch, (long)n, up, down, taps, n_taps / 2, out, (long)n_out, (cudaStream_t)stream));
-  ctx->launches++;
-  return VF_OK;
-}
-
-VF_API int vf_amp_to_original_f(vf_ctx* ctx, const float* mel_est, const float* mel_target, int batch, int frames, float* mel_out, void* stream) {
-  if (!ctx || !mel_est || !mel_target || !mel_out || batch <= 0 || frames <= 0) return ctx ? fail(ctx, VF_EINVAL, "vf_amp_to_original_f: bad arguments") : VF_EINVAL;
-  CK(cudaSetDevice(ctx->device));
-  CK(launch_amp_to_original(mel_est, mel_target, batch, frames, mel_out, (cudaStream_t)stream));
-  ctx->launches++;
-  return VF_OK;
-}
-
-VF_API int vf_lsd(vf_ctx* ctx, const float* est, const float* target, int images, int frames, int bins, float* out, void* stream) {
-  if (!ctx || !est || !target || !out || images <= 0 || frames <= 0 || bins <= 0) return ctx ? fail(ctx, VF_EINVAL, "vf_lsd: bad arguments") : VF_EINVAL;
-  CK(cudaSetDevice(ctx->device));
-  CK(launch_lsd(est, target, images, frames, bins, out, (cudaStream_t)stream));
-  ctx->launches++;
-  return VF_OK;
-}
-
-VF_API int vf_sispec(vf_ctx* ctx, const float* est, const float* target, int batch, int64_t n, int est_map, int target_map, float* out, void* stream) {
-  if (!ctx || !est || !target || !out || batch <= 0 || n <= 0 || est_map < 0 || est_map > 2 || target_map < 0 || target_map > 2)
-    return ctx ? fail(ctx, VF_EINVAL, "vf_sispec: bad arguments") : VF_EINVAL;
-  CK(cudaSetDevice(ctx->device));
-  CK(launch_sispec(est, target, batch, (long)n, est_map, target_map, out, (cudaStream_t)stream));
-  ctx->launches++;
-  return VF_OK;
-}
-
-// ---------------------------------------------------------------------------------------------------------------- scoring
-namespace {
-
-constexpr long SCORE_CAP_FRAMES = 16384;   // vf_score_varlen sub-batch cap (frames per side), see b200vf.h
-
-// Host offsets of a packed set: offsets[0] == 0, increasing, every clip > 1024 samples (one reflection of the STFT padding)
-// and at most 2^30 samples.
-int check_clip_offsets(vf_ctx* ctx, const char* fn, const char* what, const int64_t* off, int batch) {
-  if (!off || off[0] != 0) return fail(ctx, VF_EINVAL, "%s: %s offsets must start at 0", fn, what);
-  for (int i = 0; i < batch; ++i) {
-    const int64_t n = off[i + 1] - off[i];
-    if (n <= 1024 || n > (int64_t(1) << 30))
-      return fail(ctx, VF_EINVAL, "%s: %s clip %d has %ld samples (need 1025 .. 2^30)", fn, what, i, (long)n);
-  }
-  return VF_OK;
-}
-
-long stft_frames(int64_t n) { return 1 + (long)(n / 441); }
-
-}  // namespace
-
-VF_API int vf_metric_spectrogram(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* sp_out, float* mel_out,
-                                 void* stream) {
-  if (!ctx || !wav || !sp_out || batch <= 0) return ctx ? fail(ctx, VF_EINVAL, "vf_metric_spectrogram: bad arguments") : VF_EINVAL;
-  int rc = check_clip_offsets(ctx, "vf_metric_spectrogram", "wav", offsets, batch);
-  if (rc) return rc;
-  if (mel_out && !ctx->d_fb_val) return fail(ctx, VF_ESTATE, "mel filterbank not loaded (call vf_load_weights first)");
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = (cudaStream_t)stream;
-  long rows = 0;
-  for (int s = 0; s < batch; s += SCORE_MAX_IMAGES) {
-    MetricStftParams p;
-    memset(&p, 0, sizeof p);
-    p.batch = std::min(SCORE_MAX_IMAGES, batch - s);
-    p.sources = 1;
-    p.wav[0] = wav; p.sp[0] = sp_out + (size_t)rows * 1025;
-    p.window = ctx->d_window64; p.tw1024 = ctx->d_tw1024d; p.tw2048 = ctx->d_tw2048d;
-    for (int i = 0; i <= p.batch; ++i) p.off[0][i] = offsets[s + i];
-    for (int i = 0; i < p.batch; ++i) p.frame_off[i + 1] = p.frame_off[i] + stft_frames(offsets[s + i + 1] - offsets[s + i]);
-    CK(launch_metric_stft(p, st));
-    ctx->launches++;
-    rows += (long)p.frame_off[p.batch];
-  }
-  if (mel_out) {
-    MelParams m;
-    memset(&m, 0, sizeof m);
-    m.in = sp_out; m.n_outer = 1; m.T = rows; m.so = 0; m.sf = 1; m.st = 1025;
-    m.out = mel_out; m.fb_f0 = ctx->d_fb_f0; m.fb_len = ctx->d_fb_len; m.fb_ofs = ctx->d_fb_ofs; m.fb_val = ctx->d_fb_val;
-    CK(launch_mel(m, st));
-    ctx->launches++;
-  }
-  return VF_OK;
-}
-
-VF_API int vf_ssim(vf_ctx* ctx, const float* est, const float* target, int images, int frames, int bins, double* out, void* stream) {
-  if (!ctx || !est || !target || !out || images <= 0) return ctx ? fail(ctx, VF_EINVAL, "vf_ssim: bad arguments") : VF_EINVAL;
-  if (frames < 7 || bins < 7) return fail(ctx, VF_EINVAL, "vf_ssim: a %d x %d image is smaller than the 7 x 7 window", frames, bins);
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const int per = ssim_tiles(frames, bins);
-  double* partial = nullptr;                 // stream-ordered scratch
-  CK(cudaMallocAsync((void**)&partial, (size_t)per * std::min(images, SCORE_MAX_IMAGES) * sizeof(double), st));
-  cudaError_t e = cudaSuccess;
-  for (int s = 0; s < images && e == cudaSuccess; s += SCORE_MAX_IMAGES) {
-    SsimParams p;
-    memset(&p, 0, sizeof p);
-    p.batch = std::min(SCORE_MAX_IMAGES, images - s);
-    const size_t off = (size_t)s * frames * bins;
-    p.x = est + off; p.y = target + off; p.F = bins; p.partial = partial;
-    for (int i = 0; i <= p.batch; ++i) { p.frame_off[i] = (int64_t)i * frames; p.tile_off[i] = i * per; }
-    e = launch_ssim(p, out + s, 1, st);
-    ctx->launches += 2;
-  }
-  cudaFreeAsync(partial, st);
-  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "ssim launch: %s", cudaGetErrorString(e));
-  return VF_OK;
-}
-
-VF_API int vf_score_varlen(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target, const int64_t* target_offsets,
-                           int batch, double* out, void* stream) {
-  if (!ctx || !est || !target || !out || batch <= 0) return ctx ? fail(ctx, VF_EINVAL, "vf_score_varlen: bad arguments") : VF_EINVAL;
-  int rc = check_clip_offsets(ctx, "vf_score_varlen", "est", est_offsets, batch);
-  if (!rc) rc = check_clip_offsets(ctx, "vf_score_varlen", "target", target_offsets, batch);
-  if (rc) return rc;
-  std::vector<long> T(batch);
-  for (int i = 0; i < batch; ++i) {
-    T[i] = stft_frames(est_offsets[i + 1] - est_offsets[i]);
-    const long tt = stft_frames(target_offsets[i + 1] - target_offsets[i]);
-    if (T[i] != tt) return fail(ctx, VF_EINVAL, "vf_score_varlen: pair %d: est has %ld frames, target %ld", i, T[i], tt);
-    if (T[i] < 7) return fail(ctx, VF_EINVAL, "vf_score_varlen: pair %d has %ld frames, fewer than SSIM's 7", i, T[i]);
-  }
-  if (!ctx->d_fb_val) return fail(ctx, VF_ESTATE, "mel filterbank not loaded (call vf_load_weights first)");
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = (cudaStream_t)stream;
-  // consecutive sub-batches of at most SCORE_MAX_IMAGES pairs and SCORE_CAP_FRAMES frames; a longer pair runs alone
-  std::vector<int> starts{0};
-  long frames = 0;
-  size_t need = 0;
-  auto bytes_of = [](long f, long tiles) { return (size_t)f * (2 * 1025 + 2 * 128) * 4 + (size_t)tiles * 8; };
-  long tiles = 0;
-  for (int i = 0; i < batch; ++i) {
-    const int n_in = i - starts.back();
-    if (n_in == SCORE_MAX_IMAGES || (n_in > 0 && frames + T[i] > SCORE_CAP_FRAMES)) {
-      need = std::max(need, bytes_of(frames, tiles));
-      starts.push_back(i);
-      frames = tiles = 0;
-    }
-    frames += T[i];
-    tiles += (long)ssim_tiles(T[i], 1025) + ssim_tiles(T[i], 128);
-  }
-  need = std::max(need, bytes_of(frames, tiles));
-  starts.push_back(batch);
-  if (ctx->score_used) CK(cudaStreamWaitEvent(st, ctx->score_ev, 0));
-  if (!ctx->score_ev) CK(cudaEventCreateWithFlags(&ctx->score_ev, cudaEventDisableTiming));
-  if (need > ctx->score_bytes) {             // stream-ordered: no host synchronisation
-    if (ctx->d_score) CK(cudaFreeAsync(ctx->d_score, st));
-    ctx->d_score = nullptr;
-    ctx->score_bytes = 0;
-    CK(cudaMallocAsync(&ctx->d_score, need, st));
-    ctx->score_bytes = need;
-  }
-  cudaError_t e = cudaSuccess;
-  for (size_t k = 0; k + 1 < starts.size() && e == cudaSuccess; ++k) {
-    const int s = starts[k], nb = starts[k + 1] - starts[k];
-    MetricStftParams p;
-    memset(&p, 0, sizeof p);
-    ImageSet set;
-    memset(&set, 0, sizeof set);
-    p.batch = set.batch = nb;
-    p.sources = 2;
-    for (int i = 0; i <= nb; ++i) { p.off[0][i] = est_offsets[s + i]; p.off[1][i] = target_offsets[s + i]; }
-    for (int i = 0; i < nb; ++i) p.frame_off[i + 1] = set.frame_off[i + 1] = p.frame_off[i] + T[s + i];
-    const long F = (long)p.frame_off[nb];
-    float* sp_e = static_cast<float*>(ctx->d_score);
-    float* sp_t = sp_e + (size_t)F * 1025;
-    float* mel_e = sp_t + (size_t)F * 1025;
-    float* mel_t = mel_e + (size_t)F * 128;
-    double* partial = reinterpret_cast<double*>(mel_t + (size_t)F * 128);   // F * 2306 floats: 8-byte aligned
-    p.wav[0] = est; p.wav[1] = target; p.sp[0] = sp_e; p.sp[1] = sp_t;
-    p.window = ctx->d_window64; p.tw1024 = ctx->d_tw1024d; p.tw2048 = ctx->d_tw2048d;
-    e = launch_metric_stft(p, st);
-    MelParams m;                              // both spectrograms in one launch: outer index 0 = est, 1 = target
-    memset(&m, 0, sizeof m);
-    m.in = sp_e; m.n_outer = 2; m.T = F; m.so = F * 1025; m.sf = 1; m.st = 1025;
-    m.out = mel_e; m.fb_f0 = ctx->d_fb_f0; m.fb_len = ctx->d_fb_len; m.fb_ofs = ctx->d_fb_ofs; m.fb_val = ctx->d_fb_val;
-    if (e == cudaSuccess) e = launch_mel(m, st);
-    double* o = out + (size_t)s * 8;
-    const float* img[2][2] = {{sp_e, sp_t}, {mel_e, mel_t}};
-    const int bins[2] = {1025, 128};
-    for (int r = 0; r < 2 && e == cudaSuccess; ++r) {        // keys 0-3 on the spectrogram, 4-7 on the mel
-      e = launch_lsd_varlen(img[r][0], img[r][1], bins[r], set, o + 4 * r, 8, st);
-      if (e == cudaSuccess) e = launch_sispec_varlen(img[r][0], img[r][1], bins[r], set, o + 4 * r + 1, 8, st);
-      SsimParams q;
-      memset(&q, 0, sizeof q);
-      q.x = img[r][0]; q.y = img[r][1]; q.F = bins[r]; q.batch = nb; q.partial = partial;
-      for (int i = 0; i <= nb; ++i) q.frame_off[i] = set.frame_off[i];
-      for (int i = 0; i < nb; ++i) q.tile_off[i + 1] = q.tile_off[i] + ssim_tiles(T[s + i], bins[r]);
-      if (e == cudaSuccess) e = launch_ssim(q, o + 4 * r + 3, 8, st);
-    }
-    ctx->launches += 10;
-  }
-  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "score launch: %s", cudaGetErrorString(e));
-  CK(cudaEventRecord(ctx->score_ev, st));
-  ctx->score_used = true;
-  return VF_OK;
-}
-
-namespace {
-
-// d_stoi_tables layout (doubles): taps, window, tw256 (double2), tw512 (double2)
-constexpr size_t STOI_TAPS = 2 * STOI_HALF + 1, STOI_WIN_AT = STOI_TAPS + 1, STOI_TW256_AT = STOI_WIN_AT + 256,
-                 STOI_TW512_AT = STOI_TW256_AT + 2 * 256, STOI_TABLES = STOI_TW512_AT + 2 * 257;
-
-// The float64 tables of vf_score_time_varlen, designed once per context on the host:
-// * pystoi's resample_oct(x, 10000, 44100) window, Octave's resample filter for p / q = 100 / 441: L = ceil((60 - 8) /
-//   (28.714 * roll_off)) with cut-off 1 / 882 and roll_off = cut-off / 10, h = kaiser(2L + 1, 0.1102 * (60 - 8.7)) x
-//   2 * 100 * (1 / 882) * sinc(2 * (1 / 882) * t), t = -L..L; scipy's resample_poly uses window = h / sum(h), times up = 100.
-// * np.hanning(258)[1:-1] (0.5 + 0.5 cos(pi n / 257), n = -255, -253, ..., 255) and the 256 / 512-point twiddles.
-int stoi_tables(vf_ctx* ctx) {
-  if (ctx->d_stoi_tables) return VF_OK;
-  const double PI = 3.14159265358979323846;
-  std::vector<double> t(STOI_TABLES, 0.0);
-  const double fc = 1.0 / (2 * 441.0), roll_off = fc / 10, rejection_db = 60.0;
-  const long L = (long)std::ceil((rejection_db - 8) / (28.714 * roll_off));
-  if (L != STOI_HALF) return fail(ctx, VF_EASSERT, "stoi filter half length %ld != %d", L, STOI_HALF);
-  const double beta = 0.1102 * (rejection_db - 8.7), alpha = (double)L, i0_beta = std::cyl_bessel_i(0.0, beta);
-  double sum = 0;
-  for (long i = 0; i <= 2 * L; ++i) {
-    const double r = (i - alpha) / alpha;
-    const double kaiser = std::cyl_bessel_i(0.0, beta * std::sqrt(1 - r * r)) / i0_beta;
-    const double x = 2 * fc * (double)(i - L), y = PI * (x == 0 ? 1e-20 : x);     // np.sinc
-    t[i] = kaiser * (2 * 100.0 * fc * (std::sin(y) / y));
-    sum += t[i];
-  }
-  for (size_t i = 0; i < STOI_TAPS; ++i) t[i] = t[i] / sum * STOI_UP;
-  for (int i = 0; i < 256; ++i) t[STOI_WIN_AT + i] = 0.5 + 0.5 * std::cos(PI * (2 * i - 255) / 257.0);
-  for (int j = 0; j < 256; ++j) {
-    t[STOI_TW256_AT + 2 * j] = std::cos(2 * PI * j / 256.0);
-    t[STOI_TW256_AT + 2 * j + 1] = -std::sin(2 * PI * j / 256.0);
-  }
-  for (int k = 0; k <= 256; ++k) {
-    t[STOI_TW512_AT + 2 * k] = std::cos(2 * PI * k / 512.0);
-    t[STOI_TW512_AT + 2 * k + 1] = -std::sin(2 * PI * k / 512.0);
-  }
-  CK(cudaMalloc((void**)&ctx->d_stoi_tables, STOI_TABLES * sizeof(double)));
-  CK(cudaMemcpy(ctx->d_stoi_tables, t.data(), STOI_TABLES * sizeof(double), cudaMemcpyHostToDevice));
-  return VF_OK;
-}
-
-// pystoi's thirdoct(10000, 512, 15, 150): band k spans the rfft bins nearest (first of ties) to 150 * 2^((2k -+ 1) / 6)
-void stoi_bands(int* lo, int* hi) {
-  auto nearest = [](double f) {
-    int best = 0;
-    double d = INFINITY;
-    for (int q = 0; q <= 256; ++q) {
-      const double e = (q * (10000.0 / 512) - f) * (q * (10000.0 / 512) - f);
-      if (e < d) { d = e; best = q; }
-    }
-    return best;
-  };
-  for (int k = 0; k < STOI_BANDS; ++k) {
-    lo[k] = nearest(150 * std::pow(2.0, (2 * k - 1) / 6.0));
-    hi[k] = nearest(150 * std::pow(2.0, (2 * k + 1) / 6.0));
-  }
-}
-
-}  // namespace
-
-VF_API int vf_score_time_varlen(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target,
-                                const int64_t* target_offsets, int batch, double* out, void* stream) {
-  if (!ctx || !est || !target || !out || !est_offsets || !target_offsets || batch <= 0)
-    return ctx ? fail(ctx, VF_EINVAL, "vf_score_time_varlen: bad arguments") : VF_EINVAL;
-  if (est_offsets[0] != 0 || target_offsets[0] != 0) return fail(ctx, VF_EINVAL, "vf_score_time_varlen: offsets must start at 0");
-  std::vector<int64_t> N(batch);
-  for (int i = 0; i < batch; ++i) {
-    const int64_t ne = est_offsets[i + 1] - est_offsets[i], nt = target_offsets[i + 1] - target_offsets[i];
-    const int64_t cap = int64_t(1) << 30;
-    if (ne < 1 || nt < 1 || ne > cap || nt > cap)
-      return fail(ctx, VF_EINVAL, "vf_score_time_varlen: pair %d: est has %ld samples, target %ld (need 1 .. 2^30 each)", i,
-                  (long)ne, (long)nt);
-    N[i] = std::max(ne, nt);
-    if (stoi_len10(N[i]) <= STOI_FRAME)
-      return fail(ctx, VF_EINVAL, "vf_score_time_varlen: pair %d: %ld samples give %ld at 10 kHz, STOI needs more than %d", i,
-                  (long)N[i], (long)stoi_len10(N[i]), STOI_FRAME);
-  }
-  CK(cudaSetDevice(ctx->device));
-  int rc = stoi_tables(ctx);
-  if (rc) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  // consecutive sub-batches of at most SCORE_MAX_IMAGES pairs and SCORE_CAP_FRAMES * 441 padded samples; a longer pair
-  // runs alone.  Scratch: resampled and compacted signals, energies, band values, tile sums (doubles), then the kept-frame
-  // indices and counts (ints).
-  auto bytes_of = [](int64_t R, int64_t F, int64_t T, int nb) {
-    return (size_t)(4 * R + F + 2 * STOI_BANDS * F + T) * 8 + (size_t)(F + nb) * 4;
-  };
-  std::vector<int> starts{0};
-  int64_t samples = 0, R = 0, F = 0, T = 0;
-  size_t need = 0;
-  for (int i = 0; i < batch; ++i) {
-    const int n_in = i - starts.back();
-    if (n_in == SCORE_MAX_IMAGES || (n_in > 0 && samples + N[i] > SCORE_CAP_FRAMES * 441)) {
-      need = std::max(need, bytes_of(R, F, T, n_in));
-      starts.push_back(i);
-      samples = R = F = T = 0;
-    }
-    samples += N[i];
-    R += stoi_len10(N[i]);
-    F += stoi_frames(stoi_len10(N[i]));
-    T += stoi_tiles(stoi_frames(stoi_len10(N[i])));
-  }
-  need = std::max(need, bytes_of(R, F, T, batch - starts.back()));
-  starts.push_back(batch);
-  if (ctx->time_score_used) CK(cudaStreamWaitEvent(st, ctx->time_score_ev, 0));
-  if (!ctx->time_score_ev) CK(cudaEventCreateWithFlags(&ctx->time_score_ev, cudaEventDisableTiming));
-  if (need > ctx->time_score_bytes) {        // stream-ordered: no host synchronisation
-    if (ctx->d_time_score) CK(cudaFreeAsync(ctx->d_time_score, st));
-    ctx->d_time_score = nullptr;
-    ctx->time_score_bytes = 0;
-    CK(cudaMallocAsync(&ctx->d_time_score, need, st));
-    ctx->time_score_bytes = need;
-  }
-  cudaError_t e = cudaSuccess;
-  for (size_t k = 0; k + 1 < starts.size() && e == cudaSuccess; ++k) {
-    const int s = starts[k], nb = starts[k + 1] - starts[k];
-    TimeScoreParams p;
-    memset(&p, 0, sizeof p);
-    p.batch = nb;
-    p.est = est + est_offsets[s];
-    p.tgt = target + target_offsets[s];
-    for (int i = 0; i <= nb; ++i) {
-      p.e_off[i] = est_offsets[s + i] - est_offsets[s];
-      p.t_off[i] = target_offsets[s + i] - target_offsets[s];
-    }
-    for (int i = 0; i < nb; ++i) {
-      const int64_t n10 = stoi_len10(N[s + i]), nf = stoi_frames(n10);
-      p.r_off[i + 1] = p.r_off[i] + n10;
-      p.f_off[i + 1] = p.f_off[i] + nf;
-      p.tile_off[i + 1] = p.tile_off[i] + stoi_tiles(nf);
-    }
-    stoi_bands(p.band_lo, p.band_hi);
-    p.clip = 1 + std::pow(10.0, 15.0 / 20);
-    p.taps = ctx->d_stoi_tables;
-    p.window = ctx->d_stoi_tables + STOI_WIN_AT;
-    p.tw256 = reinterpret_cast<const double2*>(ctx->d_stoi_tables + STOI_TW256_AT);
-    p.tw512 = reinterpret_cast<const double2*>(ctx->d_stoi_tables + STOI_TW512_AT);
-    const int64_t Rs = p.r_off[nb], Fs = p.f_off[nb], Ts = p.tile_off[nb];
-    double* d = static_cast<double*>(ctx->d_time_score);
-    p.rs = d;
-    p.cs = p.rs + 2 * Rs;
-    p.energy = p.cs + 2 * Rs;
-    p.tob = p.energy + Fs;
-    p.partial = p.tob + 2 * STOI_BANDS * Fs;
-    p.src = reinterpret_cast<int*>(p.partial + Ts);
-    p.kept = p.src + Fs;
-    p.out = out + (size_t)s * 2;
-    e = launch_score_time(p, st);
-    ctx->launches += Ts > 0 ? 8 : 7;
-  }
-  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "time score launch: %s", cudaGetErrorString(e));
-  CK(cudaEventRecord(ctx->time_score_ev, st));
-  ctx->time_score_used = true;
-  return VF_OK;
-}
-
-namespace {
-
-// Checked offsets of `batch` packed rows: start at 0, each row at least `min_len` samples.
-bool rows_ok(vf_ctx* ctx, const char* fn, const int64_t* off, int batch, int64_t min_len, const char* what) {
-  if (off[0] != 0) { fail(ctx, VF_EINVAL, "%s: %s offsets must start at 0", fn, what); return false; }
-  for (int i = 0; i < batch; ++i)
-    if (off[i + 1] - off[i] < min_len) {
-      fail(ctx, VF_EINVAL, "%s: %s row %d has %ld samples (need at least %ld)", fn, what, i, (long)(off[i + 1] - off[i]),
-           (long)min_len);
-      return false;
-    }
-  return true;
-}
-
-}  // namespace
-
-VF_API int vf_sosfiltfilt_varlen(vf_ctx* ctx, const double* x, const int64_t* offsets, int batch, const double* sos,
-                                 const double* zi, const int* n_sections, int n_filters, const int* row_filter, const int* row_f32,
-                                 double* out, void* stream) {
-  static const char* fn = "vf_sosfiltfilt_varlen";
-  if (!ctx || !x || !offsets || !sos || !zi || !n_sections || !row_filter || !out || batch <= 0 || n_filters <= 0)
-    return ctx ? fail(ctx, VF_EINVAL, "%s: bad arguments", fn) : VF_EINVAL;
-  if (!rows_ok(ctx, fn, offsets, batch, 1, "x")) return VF_EINVAL;
-  std::vector<int> edge(n_filters);
-  for (int f = 0; f < n_filters; ++f) {
-    const int ns = n_sections[f];
-    if (ns < 1 || ns > IIR_MAX_SECTIONS) return fail(ctx, VF_EINVAL, "%s: filter %d has %d sections (need 1 .. %d)", fn, f, ns, IIR_MAX_SECTIONS);
-    const double* s = sos + (size_t)f * 6 * IIR_MAX_SECTIONS;
-    int zb = 0, za = 0;
-    for (int k = 0; k < ns; ++k) {
-      if (s[6 * k + 3] != 1.0) return fail(ctx, VF_EINVAL, "%s: filter %d: sos[%d, 3] is not 1", fn, f, k);
-      zb += s[6 * k + 2] == 0.0;
-      za += s[6 * k + 5] == 0.0;
-    }
-    edge[f] = 3 * (2 * ns + 1 - std::min(zb, za));        // sosfiltfilt's default padlen
-  }
-  std::vector<int64_t> ne(batch);
-  for (int i = 0; i < batch; ++i) {
-    const int f = row_filter[i];
-    if (f < 0 || f >= n_filters) return fail(ctx, VF_EINVAL, "%s: row %d: filter %d of %d", fn, i, f, n_filters);
-    const int64_t n = offsets[i + 1] - offsets[i];
-    if (n <= edge[f]) return fail(ctx, VF_EINVAL, "%s: row %d has %ld samples, not more than its padlen %d", fn, i, (long)n, edge[f]);
-    ne[i] = n + 2 * (int64_t)edge[f];
-  }
-  CK(cudaSetDevice(ctx->device));
-  auto chunks = [](int64_t n) { return (n + IIR_CHUNK - 1) / IIR_CHUNK; };
-  auto bytes_of = [](int64_t E, int64_t C) { return (size_t)(E + C * IIR_MAX_STATES) * sizeof(double); };
-  // consecutive sub-batches of at most IIR_MAX_ROWS rows and IIR_CAP_SAMPLES extended samples; a longer row runs alone
-  std::vector<int> starts{0};
-  int64_t E = 0, C = 0;
-  size_t need = 0;
-  for (int i = 0; i < batch; ++i) {
-    const int n_in = i - starts.back();
-    if (n_in == IIR_MAX_ROWS || (n_in > 0 && E + ne[i] > IIR_CAP_SAMPLES)) {
-      need = std::max(need, bytes_of(E, C));
-      starts.push_back(i);
-      E = C = 0;
-    }
-    E += ne[i];
-    C += chunks(ne[i]);
-  }
-  need = std::max(need, bytes_of(E, C));
-  starts.push_back(batch);
-  const size_t table_doubles = (size_t)n_filters * IIR_TABLE;     // the call's filter tables lead the scratch
-  need += table_doubles * sizeof(double);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (ctx->iir_used) CK(cudaStreamWaitEvent(st, ctx->iir_ev, 0));
-  if (!ctx->iir_ev) CK(cudaEventCreateWithFlags(&ctx->iir_ev, cudaEventDisableTiming));
-  if (need > ctx->iir_bytes) {               // stream-ordered: no host synchronisation
-    if (ctx->d_iir) CK(cudaFreeAsync(ctx->d_iir, st));
-    ctx->d_iir = nullptr;
-    ctx->iir_bytes = 0;
-    CK(cudaMallocAsync(&ctx->d_iir, need, st));
-    ctx->iir_bytes = need;
-  }
-  double* tables = static_cast<double*>(ctx->d_iir);
-  cudaError_t e = cudaSuccess;
-  for (int f0 = 0; f0 < n_filters && e == cudaSuccess; f0 += IIR_DESIGN_FILTERS) {   // sos and zi go as kernel parameters
-    IirDesignParams d;
-    memset(&d, 0, sizeof d);
-    d.tables = tables + (size_t)f0 * IIR_TABLE;
-    d.n = std::min(IIR_DESIGN_FILTERS, n_filters - f0);
-    for (int i = 0; i < d.n; ++i) {
-      const int f = f0 + i;
-      d.n_sections[i] = n_sections[f];
-      std::copy(sos + (size_t)f * 6 * IIR_MAX_SECTIONS, sos + (size_t)f * 6 * IIR_MAX_SECTIONS + 6 * n_sections[f], d.sos[i]);
-      std::copy(zi + (size_t)f * 2 * IIR_MAX_SECTIONS, zi + (size_t)f * 2 * IIR_MAX_SECTIONS + 2 * n_sections[f], d.zi[i]);
-    }
-    e = launch_iir_design(d, st);
-    ctx->launches += 1;
-  }
-  for (size_t k = 0; k + 1 < starts.size() && e == cudaSuccess; ++k) {
-    const int s = starts[k], nb = starts[k + 1] - starts[k];
-    SosParams p;
-    memset(&p, 0, sizeof p);
-    p.batch = nb;
-    p.x = x + offsets[s];
-    p.out = out + offsets[s];
-    for (int i = 0; i < nb; ++i) {
-      const int f = row_filter[s + i];
-      p.off[i + 1] = offsets[s + i + 1] - offsets[s];
-      p.ext_off[i + 1] = p.ext_off[i] + ne[s + i];
-      p.chunk_off[i + 1] = p.chunk_off[i] + chunks(ne[s + i]);
-      p.edge[i] = edge[f];
-      p.ext_f32[i] = row_f32 ? row_f32[s + i] != 0 : 0;
-      p.n_sections[i] = n_sections[f];
-      p.table[i] = tables + (size_t)f * IIR_TABLE;
-    }
-    p.yf = tables + table_doubles;
-    p.state = p.yf + p.ext_off[nb];
-    e = launch_sosfiltfilt(p, st);
-    ctx->launches += 6;
-  }
-  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "sosfiltfilt launch: %s", cudaGetErrorString(e));
-  CK(cudaEventRecord(ctx->iir_ev, st));
-  ctx->iir_used = true;
-  return VF_OK;
-}
-
-VF_API int vf_resample_poly_f64_varlen(vf_ctx* ctx, const double* x, const int64_t* in_offsets, int batch, const double* taps,
-                                       const int64_t* tap_offsets, const int* up, const int* down, int n_filters,
-                                       const int* row_filter, double* y, const int64_t* out_offsets, void* stream) {
-  static const char* fn = "vf_resample_poly_f64_varlen";
-  if (!ctx || !x || !in_offsets || !taps || !tap_offsets || !up || !down || !row_filter || !y || !out_offsets || batch <= 0 ||
-      n_filters <= 0)
-    return ctx ? fail(ctx, VF_EINVAL, "%s: bad arguments", fn) : VF_EINVAL;
-  if (!rows_ok(ctx, fn, in_offsets, batch, 1, "x") || !rows_ok(ctx, fn, out_offsets, batch, 0, "y")) return VF_EINVAL;
-  if (tap_offsets[0] != 0) return fail(ctx, VF_EINVAL, "%s: tap offsets must start at 0", fn);
-  for (int f = 0; f < n_filters; ++f) {
-    const int64_t nt = tap_offsets[f + 1] - tap_offsets[f];
-    if (nt < 1 || nt % 2 == 0 || nt > (int64_t(1) << 30))
-      return fail(ctx, VF_EINVAL, "%s: filter %d has %ld taps (need an odd count)", fn, f, (long)nt);
-    if (up[f] < 1 || down[f] < 1) return fail(ctx, VF_EINVAL, "%s: filter %d: up %d, down %d (need >= 1)", fn, f, up[f], down[f]);
-  }
-  for (int i = 0; i < batch; ++i)
-    if (row_filter[i] < 0 || row_filter[i] >= n_filters)
-      return fail(ctx, VF_EINVAL, "%s: row %d: filter %d of %d", fn, i, row_filter[i], n_filters);
-  CK(cudaSetDevice(ctx->device));
-  cudaError_t e = cudaSuccess;
-  for (int s = 0; s < batch && e == cudaSuccess; s += IIR_MAX_ROWS) {
-    const int nb = std::min(IIR_MAX_ROWS, batch - s);
-    ResampleF64Params p;
-    memset(&p, 0, sizeof p);
-    p.batch = nb;
-    p.x = x + in_offsets[s];
-    p.y = y + out_offsets[s];
-    p.taps = taps;
-    for (int i = 0; i < nb; ++i) {
-      const int f = row_filter[s + i];
-      p.in_off[i + 1] = in_offsets[s + i + 1] - in_offsets[s];
-      p.out_off[i + 1] = out_offsets[s + i + 1] - out_offsets[s];
-      p.tap_at[i] = tap_offsets[f];
-      p.half[i] = (int)((tap_offsets[f + 1] - tap_offsets[f] - 1) / 2);
-      p.up[i] = up[f];
-      p.down[i] = down[f];
-    }
-    e = launch_resample_f64(p, (cudaStream_t)stream);
-    ctx->launches += 1;
-  }
-  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "resample launch: %s", cudaGetErrorString(e));
-  return VF_OK;
-}
-
-VF_API int vf_finalize(vf_ctx* ctx, const float* wav, int batch, int64_t len, int64_t n, float* wav_out, void* stream) {
-  if (!ctx || !wav || !wav_out || batch <= 0 || len <= 0 || n <= 0) return ctx ? fail(ctx, VF_EINVAL, "vf_finalize: bad arguments") : VF_EINVAL;
-  const long d = (long)len - (long)n;
-  // trim_center (tools/utils.py:57-70) for an estimate at least as long as the reference; d == 1 is the reference's
-  // empty-slice case (est[..., 0:-0])
-  if (d < 0 || d == 1) return fail(ctx, VF_EINVAL, "vf_finalize: estimate length %ld vs reference %ld is not a trim_center case the path produces", (long)len, (long)n);
-  CK(cudaSetDevice(ctx->device));
-  cudaStream_t st = (cudaStream_t)stream;
-  unsigned int* peak = nullptr;
-  CK(cudaMallocAsync((void**)&peak, (size_t)batch * 4, st));
-  CK(cudaMemsetAsync(peak, 0, (size_t)batch * 4, st));
-  cudaError_t e1 = launch_peak(wav, batch, (long)len, peak, st);
-  FinalizeParams f;
-  memset(&f, 0, sizeof f);
-  f.wav = wav; f.peak_bits = peak; f.batch = batch; f.L = (long)len; f.n = (long)n; f.skip = d / 2;
-  f.out = wav_out; f.out_ld = (long)n; f.out_off = 0;
-  cudaError_t e2 = e1 == cudaSuccess ? launch_finalize(f, st) : e1;
-  cudaFreeAsync(peak, st);
-  if (e2 != cudaSuccess) return fail(ctx, VF_ECUDA, "finalize launch: %s", cudaGetErrorString(e2));
-  ctx->launches += 2;
-  return VF_OK;
+  return mark_use(ctx, plan->order, (cudaStream_t)stream);
 }
 
 VF_API int vf_restore_stages(vf_ctx* ctx, int batch, int64_t n, float* mel_lin_out, float* log_mel_out, void* stream) {
@@ -1452,37 +866,11 @@ VF_API int vf_restore_stages(vf_ctx* ctx, int batch, int64_t n, float* mel_lin_o
   rc = get_plan(ctx, PLAN_GSR, batch, frames, &plan);
   if (rc) return rc;
   const size_t bytes = (size_t)batch * frames * 128 * 4;
-  rc = plan_enter(ctx, plan, (cudaStream_t)stream);
+  rc = order_use(ctx, plan->order, (cudaStream_t)stream);
   if (rc) return rc;
   if (mel_lin_out) CK(cudaMemcpyAsync(mel_lin_out, plan->d_mel, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   if (log_mel_out) CK(cudaMemcpyAsync(log_mel_out, plan->d_logmel_out, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  return plan_exit(ctx, plan, (cudaStream_t)stream);
-}
-
-VF_API int vf_to_log(vf_ctx* ctx, const float* in, float* out, int64_t n, void* stream) {
-  if (!ctx || !in || !out || n <= 0) return VF_EINVAL;
-  CK(cudaSetDevice(ctx->device));
-  CK(launch_to_log(in, out, (size_t)n, ctx->d_err + 1, (cudaStream_t)stream));
-  ctx->launches++;
-  return VF_OK;
-}
-VF_API int vf_from_log(vf_ctx* ctx, const float* in, float* out, int64_t n, void* stream) {
-  if (!ctx || !in || !out || n <= 0) return VF_EINVAL;
-  CK(cudaSetDevice(ctx->device));
-  CK(launch_from_log(in, out, (size_t)n, (cudaStream_t)stream));
-  ctx->launches++;
-  return VF_OK;
-}
-
-VF_API int vf_to_pcm16_ex(vf_ctx* ctx, const float* in, int16_t* out, int64_t n, int saturate, void* stream) {
-  if (!ctx || !in || !out || n <= 0) return VF_EINVAL;
-  CK(cudaSetDevice(ctx->device));
-  CK(launch_pcm16(in, out, (size_t)n, saturate ? 1 : 0, (cudaStream_t)stream));
-  ctx->launches++;
-  return VF_OK;
-}
-VF_API int vf_to_pcm16(vf_ctx* ctx, const float* in, int16_t* out, int64_t n, void* stream) {
-  return vf_to_pcm16_ex(ctx, in, out, n, 0, stream);
+  return mark_use(ctx, plan->order, (cudaStream_t)stream);
 }
 
 VF_API int vf_workspace_bytes(vf_ctx* ctx, int batch, int64_t n, size_t* bytes) {

@@ -1,5 +1,6 @@
 // Declarations shared by the host translation units of libb200vf.so: engine.cu (context, plan cache, run machinery, C ABI),
-// pack.cu (weight ingestion and packing) and plan.cu (launch plans).  No kernels are declared or defined here.
+// pack.cu (weight ingestion and packing), plan.cu (launch plans) and standalone.cu (the plan-free entry points).  No
+// kernels are declared or defined here.
 #pragma once
 
 #include <cuda.h>
@@ -136,6 +137,14 @@ inline bool is_ssr_plan(int kind) { return kind == PLAN_SSR || kind == PLAN_SSR_
 // Plans of these kinds own a lengths table (kernels.cuh)
 inline bool is_varlen_plan(int kind) { return kind == PLAN_VARLEN || kind == PLAN_SSR_VARLEN; }
 
+// The previous use of a device buffer that calls on any stream share (a plan's workspace, a scratch): order_use makes
+// this use wait for it when it ran on another stream, mark_use records this one
+struct StreamOrder {
+  cudaEvent_t ev = nullptr;
+  cudaStream_t last_stream = nullptr;
+  bool used = false;
+};
+
 struct Plan {
   int kind = PLAN_GSR;
   uint64_t last_use = 0;
@@ -153,10 +162,7 @@ struct Plan {
   float* d_io[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};   // [buffer][in / out]: double-buffered host staging
   cudaEvent_t io_ev[2][4] = {{nullptr, nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr, nullptr}};   // h2d done, input consumed, compute done, d2h done
   unsigned io_seq = 0;
-  // a plan's buffers are shared by every call of its shape: uses on different streams are ordered through this event
-  cudaEvent_t ev_last = nullptr;
-  cudaStream_t last_stream = nullptr;
-  bool used = false;
+  StreamOrder order;             // a plan's buffers are shared by every call of its shape
   float* d_mel = nullptr;        // [B, T, 128] linear mel
   float* d_logmel_in = nullptr;  // [B, T, 128] log10 mel (UNet input)
   float* d_logmel_out = nullptr; // [B, T, 128]
@@ -174,6 +180,13 @@ struct Plan {
   int uses = 0;
   // op slots patched per call
   int fe_op = -1, cond_op = -1, fin_op = -1;
+};
+
+// Scratch of a plan-free entry point (standalone.cu): a stream-ordered allocation grown on demand and freed by vf_destroy
+struct Scratch {
+  void* p = nullptr;
+  size_t bytes = 0;
+  StreamOrder order;
 };
 
 }  // namespace vf
@@ -203,24 +216,11 @@ struct vf_ctx {
   double* d_window64 = nullptr;    // metric STFT (vf_metric_spectrogram, vf_score_varlen): float64 window and twiddles
   double2* d_tw1024d = nullptr;
   double2* d_tw2048d = nullptr;
-  // vf_score_varlen scratch (two spectrograms, two mels, SSIM tile sums), stream-ordered allocation grown on demand and
-  // freed by vf_destroy; uses on different streams are ordered through score_ev
-  void* d_score = nullptr;
-  size_t score_bytes = 0;
-  cudaEvent_t score_ev = nullptr;
-  bool score_used = false;
-  // vf_score_time_varlen: its float64 tables (resampling taps, window, twiddles; designed on first use) and its scratch,
-  // held and ordered like d_score's
-  double* d_stoi_tables = nullptr;
-  void* d_time_score = nullptr;
-  size_t time_score_bytes = 0;
-  cudaEvent_t time_score_ev = nullptr;
-  bool time_score_used = false;
-  // vf_sosfiltfilt_varlen: the call's filter tables and the scan scratch, held and ordered like d_score's
-  void* d_iir = nullptr;
-  size_t iir_bytes = 0;
-  cudaEvent_t iir_ev = nullptr;
-  bool iir_used = false;
+  // scratch of the packed-set calls of standalone.cu: vf_score_varlen (two spectrograms, two mels, SSIM tile sums),
+  // vf_score_time_varlen (resampled signals, frame and band values, tile sums, kept-frame indices) and
+  // vf_sosfiltfilt_varlen (the call's filter tables, then the scan's extended rows and chunk states)
+  Scratch score, time_score, iir;
+  double* d_stoi_tables = nullptr;   // vf_score_time_varlen's float64 tables (resampling taps, window, twiddles; first use)
   // UNet weights: the mel-domain analysis module of VoiceFixer (prefix generator.analysis_module.) and the
   // linear-spectrogram unet_v2 of SSR_UNet / GSR_UNet (prefix generator.unet.); either may be absent
   UnetW gsr, ssr;
@@ -279,6 +279,11 @@ int dev_alloc(vf_ctx* ctx, std::vector<void*>& pool, size_t& acct, T** out, size
 }
 
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
+
+// engine.cu: StreamOrder around one use on `st`.  After a successful order_use, mark_use must run on every path that may
+// have queued work on the buffer, or the next use on another stream would not wait for that work.
+int order_use(vf_ctx* ctx, StreamOrder& o, cudaStream_t st);
+int mark_use(vf_ctx* ctx, StreamOrder& o, cudaStream_t st);
 
 // pack.cu
 int upload_gemm(vf_ctx* ctx, GemmW* w, const std::vector<float>& m, int N, int K, const std::vector<float>* bias);

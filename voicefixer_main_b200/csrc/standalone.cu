@@ -1,0 +1,595 @@
+// Host side of libb200vf.so's plan-free entry points (include/b200vf.h): the stand-alone boundary ops, the scoring of
+// packed sets, the SR degradations and the element-wise conversions.  None of them uses a plan: each launches on the
+// caller's stream with its own arguments, the context's tables and at most one context-owned Scratch.
+#include <climits>
+#include <cmath>
+#include <cstring>
+
+#include "engine.h"
+
+namespace {
+
+// The opening of plan-free entry point `fn`: `ok` is its argument check (`why` is added to its message); then the
+// context's device is made current.
+int begin_call(vf_ctx* ctx, const char* fn, bool ok, const char* why = "") {
+  if (!ctx) return VF_EINVAL;
+  if (!ok) return fail(ctx, VF_EINVAL, "%s: bad arguments%s", fn, why);
+  CK(cudaSetDevice(ctx->device));
+  return VF_OK;
+}
+
+// Orders this use of `s` after its previous one and grows it to `need` bytes, stream-ordered (no host synchronisation).
+// Once this succeeds, mark_use(ctx, s.order, st) must run on every path, a failed launch included: the sub-batches
+// queued before it read the scratch.
+int acquire_scratch(vf_ctx* ctx, Scratch& s, size_t need, cudaStream_t st) {
+  const int rc = order_use(ctx, s.order, st);
+  if (rc || need <= s.bytes) return rc;
+  if (s.p) CK(cudaFreeAsync(s.p, st));
+  s.p = nullptr;
+  s.bytes = 0;
+  CK(cudaMallocAsync(&s.p, need, st));
+  s.bytes = need;
+  return VF_OK;
+}
+
+// Consecutive sub-batches of a packed set of `batch` items: a sub-batch takes items until it holds max_rows, or until the
+// next item's size_of(i) would take its size past `cap`; an item larger than cap runs alone.  -> the first item of every
+// sub-batch, then `batch`.
+template <typename Size>
+std::vector<int> split(int batch, int max_rows, int64_t cap, Size size_of) {
+  std::vector<int> starts{0};
+  int64_t size = 0;
+  for (int i = 0; i < batch; ++i) {
+    const int64_t n = size_of(i);
+    if (i - starts.back() == max_rows || (i > starts.back() && size + n > cap)) {
+      starts.push_back(i);
+      size = 0;
+    }
+    size += n;
+  }
+  starts.push_back(batch);
+  return starts;
+}
+std::vector<int> split(int batch, int max_rows) { return split(batch, max_rows, INT64_MAX, [](int) { return int64_t(0); }); }
+
+// The scratch a split call needs: the largest sum of bytes_of(i) over the items of one sub-batch of `starts`
+template <typename Bytes>
+size_t max_bytes(const std::vector<int>& starts, Bytes bytes_of) {
+  size_t need = 0;
+  for (size_t k = 0; k + 1 < starts.size(); ++k) {
+    size_t sum = 0;
+    for (int i = starts[k]; i < starts[k + 1]; ++i) sum += bytes_of(i);
+    need = std::max(need, sum);
+  }
+  return need;
+}
+
+constexpr int64_t ITEM_MAX = int64_t(1) << 30;   // samples of one clip of a scored set
+
+// Host offsets of a packed set of `batch` items of `fn`: off[0] == 0, and item i = [off[i], off[i + 1]) holds lo .. hi
+// samples.  A rejection names the set (`side`: est, target, x, y) and the item in the entry point's word (clip, pair, row).
+int check_offsets(vf_ctx* ctx, const char* fn, const char* side, const char* item, const int64_t* off, int batch, int64_t lo,
+                  int64_t hi = INT64_MAX) {
+  if (!off || off[0] != 0) return fail(ctx, VF_EINVAL, "%s: %s offsets must start at 0", fn, side);
+  for (int i = 0; i < batch; ++i) {
+    const long n = (long)(off[i + 1] - off[i]);
+    if (n >= lo && n <= hi) continue;
+    if (hi == INT64_MAX) return fail(ctx, VF_EINVAL, "%s: %s %s %d has %ld samples (need at least %ld)", fn, side, item, i, n, (long)lo);
+    return fail(ctx, VF_EINVAL, "%s: %s %s %d has %ld samples (need %ld .. %ld)", fn, side, item, i, n, (long)lo, (long)hi);
+  }
+  return VF_OK;
+}
+
+constexpr long SCORE_CAP_FRAMES = 16384;   // vf_score_varlen sub-batch cap (frames per side), see b200vf.h
+
+long stft_frames(int64_t n) { return 1 + (long)(n / 441); }
+
+// d_stoi_tables layout (doubles): taps, window, tw256 (double2), tw512 (double2)
+constexpr size_t STOI_TAPS = 2 * STOI_HALF + 1, STOI_WIN_AT = STOI_TAPS + 1, STOI_TW256_AT = STOI_WIN_AT + 256,
+                 STOI_TW512_AT = STOI_TW256_AT + 2 * 256, STOI_TABLES = STOI_TW512_AT + 2 * 257;
+
+// The float64 tables of vf_score_time_varlen, designed once per context on the host:
+// * pystoi's resample_oct(x, 10000, 44100) window, Octave's resample filter for p / q = 100 / 441: L = ceil((60 - 8) /
+//   (28.714 * roll_off)) with cut-off 1 / 882 and roll_off = cut-off / 10, h = kaiser(2L + 1, 0.1102 * (60 - 8.7)) x
+//   2 * 100 * (1 / 882) * sinc(2 * (1 / 882) * t), t = -L..L; scipy's resample_poly uses window = h / sum(h), times up = 100.
+// * np.hanning(258)[1:-1] (0.5 + 0.5 cos(pi n / 257), n = -255, -253, ..., 255) and the 256 / 512-point twiddles.
+int stoi_tables(vf_ctx* ctx) {
+  if (ctx->d_stoi_tables) return VF_OK;
+  const double PI = 3.14159265358979323846;
+  std::vector<double> t(STOI_TABLES, 0.0);
+  const double fc = 1.0 / (2 * 441.0), roll_off = fc / 10, rejection_db = 60.0;
+  const long L = (long)std::ceil((rejection_db - 8) / (28.714 * roll_off));
+  if (L != STOI_HALF) return fail(ctx, VF_EASSERT, "stoi filter half length %ld != %d", L, STOI_HALF);
+  const double beta = 0.1102 * (rejection_db - 8.7), alpha = (double)L, i0_beta = std::cyl_bessel_i(0.0, beta);
+  double sum = 0;
+  for (long i = 0; i <= 2 * L; ++i) {
+    const double r = (i - alpha) / alpha;
+    const double kaiser = std::cyl_bessel_i(0.0, beta * std::sqrt(1 - r * r)) / i0_beta;
+    const double x = 2 * fc * (double)(i - L), y = PI * (x == 0 ? 1e-20 : x);     // np.sinc
+    t[i] = kaiser * (2 * 100.0 * fc * (std::sin(y) / y));
+    sum += t[i];
+  }
+  for (size_t i = 0; i < STOI_TAPS; ++i) t[i] = t[i] / sum * STOI_UP;
+  for (int i = 0; i < 256; ++i) t[STOI_WIN_AT + i] = 0.5 + 0.5 * std::cos(PI * (2 * i - 255) / 257.0);
+  for (int j = 0; j < 256; ++j) {
+    t[STOI_TW256_AT + 2 * j] = std::cos(2 * PI * j / 256.0);
+    t[STOI_TW256_AT + 2 * j + 1] = -std::sin(2 * PI * j / 256.0);
+  }
+  for (int k = 0; k <= 256; ++k) {
+    t[STOI_TW512_AT + 2 * k] = std::cos(2 * PI * k / 512.0);
+    t[STOI_TW512_AT + 2 * k + 1] = -std::sin(2 * PI * k / 512.0);
+  }
+  CK(cudaMalloc((void**)&ctx->d_stoi_tables, STOI_TABLES * sizeof(double)));
+  CK(cudaMemcpy(ctx->d_stoi_tables, t.data(), STOI_TABLES * sizeof(double), cudaMemcpyHostToDevice));
+  return VF_OK;
+}
+
+// pystoi's thirdoct(10000, 512, 15, 150): band k spans the rfft bins nearest (first of ties) to 150 * 2^((2k -+ 1) / 6)
+void stoi_bands(int* lo, int* hi) {
+  auto nearest = [](double f) {
+    int best = 0;
+    double d = INFINITY;
+    for (int q = 0; q <= 256; ++q) {
+      const double e = (q * (10000.0 / 512) - f) * (q * (10000.0 / 512) - f);
+      if (e < d) { d = e; best = q; }
+    }
+    return best;
+  };
+  for (int k = 0; k < STOI_BANDS; ++k) {
+    lo[k] = nearest(150 * std::pow(2.0, (2 * k - 1) / 6.0));
+    hi[k] = nearest(150 * std::pow(2.0, (2 * k + 1) / 6.0));
+  }
+}
+
+}  // namespace
+
+extern "C" {
+
+VF_API int vf_istft(vf_ctx* ctx, const float* real, const float* imag, int batch, int frames, int64_t length, float* wav_out, void* stream) {
+  const int rc = begin_call(ctx, "vf_istft", real && imag && wav_out && batch > 0 && frames > 0 && length > 0);
+  if (rc) return rc;
+  if (length + 1024 > (int64_t)(frames - 1) * ctx->cfg.hop + 2048)
+    return fail(ctx, VF_EINVAL, "vf_istft: %d frames cover %ld samples, fewer than length %ld + n_fft/2", frames, (long)(frames - 1) * ctx->cfg.hop + 2048, (long)length);
+  cudaStream_t st = (cudaStream_t)stream;
+  float* frames_buf = nullptr;           // stream-ordered scratch: no plan is tied to a bare ISTFT
+  CK(cudaMallocAsync((void**)&frames_buf, (size_t)batch * frames * 2048 * 4, st));
+  IstftFramesParams fp;
+  memset(&fp, 0, sizeof fp);
+  fp.real = real; fp.imag = imag; fp.batch = batch; fp.T = frames;
+  fp.window = ctx->d_window; fp.tw1024 = ctx->d_tw1024; fp.tw2048 = ctx->d_tw2048; fp.frames = frames_buf;
+  cudaError_t e1 = launch_istft_frames(fp, st);
+  IstftOlaParams op;
+  memset(&op, 0, sizeof op);
+  op.frames = frames_buf; op.batch = batch; op.T = frames; op.length = (long)length; op.window = ctx->d_window;
+  op.out = wav_out; op.out_ld = (long)length;
+  cudaError_t e2 = e1 == cudaSuccess ? launch_istft_ola(op, st) : e1;
+  cudaFreeAsync(frames_buf, st);
+  if (e2 != cudaSuccess) return fail(ctx, VF_ECUDA, "istft launch: %s", cudaGetErrorString(e2));
+  ctx->launches += 2;
+  return VF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------- stand-alone boundary ops
+VF_API int vf_mel(vf_ctx* ctx, const float* specgram, int64_t n_outer, int64_t frames, int64_t stride_outer, int64_t stride_freq,
+                  int64_t stride_time, float* mel_out, void* stream) {
+  const int rc = begin_call(ctx, "vf_mel", specgram && mel_out && n_outer > 0 && frames > 0 && n_outer <= 65535);
+  if (rc) return rc;
+  if (!ctx->d_fb_val) return fail(ctx, VF_ESTATE, "mel filterbank not loaded (call vf_load_weights first)");
+  MelParams p;
+  memset(&p, 0, sizeof p);
+  p.in = specgram; p.n_outer = (long)n_outer; p.T = (long)frames; p.so = (long)stride_outer; p.sf = (long)stride_freq; p.st = (long)stride_time;
+  p.out = mel_out; p.fb_f0 = ctx->d_fb_f0; p.fb_len = ctx->d_fb_len; p.fb_ofs = ctx->d_fb_ofs; p.fb_val = ctx->d_fb_val;
+  CK(launch_mel(p, (cudaStream_t)stream));
+  ctx->launches++;
+  return VF_OK;
+}
+
+VF_API int vf_resample_poly(vf_ctx* ctx, const float* wav, int batch, int64_t n, int up, int down, const float* taps, int n_taps,
+                            float* out, int64_t n_out, void* stream) {
+  const int rc = begin_call(ctx, "vf_resample_poly", wav && taps && out && batch > 0 && n > 0 && up > 0 && down > 0 && n_taps >= 1 &&
+                                                         (n_taps & 1), " (n_taps must be odd)");
+  if (rc) return rc;
+  if (n_out != (n * up + down - 1) / down) return fail(ctx, VF_EINVAL, "vf_resample_poly: n_out must be ceil(n * up / down) = %ld", (long)((n * up + down - 1) / down));
+  CK(launch_resample_poly(wav, batch, (long)n, up, down, taps, n_taps / 2, out, (long)n_out, (cudaStream_t)stream));
+  ctx->launches++;
+  return VF_OK;
+}
+
+VF_API int vf_amp_to_original_f(vf_ctx* ctx, const float* mel_est, const float* mel_target, int batch, int frames, float* mel_out, void* stream) {
+  const int rc = begin_call(ctx, "vf_amp_to_original_f", mel_est && mel_target && mel_out && batch > 0 && frames > 0);
+  if (rc) return rc;
+  CK(launch_amp_to_original(mel_est, mel_target, batch, frames, mel_out, (cudaStream_t)stream));
+  ctx->launches++;
+  return VF_OK;
+}
+
+VF_API int vf_lsd(vf_ctx* ctx, const float* est, const float* target, int images, int frames, int bins, float* out, void* stream) {
+  const int rc = begin_call(ctx, "vf_lsd", est && target && out && images > 0 && frames > 0 && bins > 0);
+  if (rc) return rc;
+  CK(launch_lsd(est, target, images, frames, bins, out, (cudaStream_t)stream));
+  ctx->launches++;
+  return VF_OK;
+}
+
+VF_API int vf_sispec(vf_ctx* ctx, const float* est, const float* target, int batch, int64_t n, int est_map, int target_map, float* out, void* stream) {
+  const int rc = begin_call(ctx, "vf_sispec", est && target && out && batch > 0 && n > 0 && est_map >= 0 && est_map <= 2 &&
+                                                  target_map >= 0 && target_map <= 2);
+  if (rc) return rc;
+  CK(launch_sispec(est, target, batch, (long)n, est_map, target_map, out, (cudaStream_t)stream));
+  ctx->launches++;
+  return VF_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------- scoring
+VF_API int vf_metric_spectrogram(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* sp_out, float* mel_out,
+                                 void* stream) {
+  static const char* fn = "vf_metric_spectrogram";
+  int rc = begin_call(ctx, fn, wav && sp_out && batch > 0);
+  if (!rc) rc = check_offsets(ctx, fn, "wav", "clip", offsets, batch, 1025, ITEM_MAX);   // one reflection of the STFT padding
+  if (rc) return rc;
+  if (mel_out && !ctx->d_fb_val) return fail(ctx, VF_ESTATE, "mel filterbank not loaded (call vf_load_weights first)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const std::vector<int> starts = split(batch, SCORE_MAX_IMAGES);
+  long rows = 0;
+  for (size_t k = 0; k + 1 < starts.size(); ++k) {
+    const int s = starts[k];
+    MetricStftParams p;
+    memset(&p, 0, sizeof p);
+    p.batch = starts[k + 1] - s;
+    p.sources = 1;
+    p.wav[0] = wav; p.sp[0] = sp_out + (size_t)rows * 1025;
+    p.window = ctx->d_window64; p.tw1024 = ctx->d_tw1024d; p.tw2048 = ctx->d_tw2048d;
+    for (int i = 0; i <= p.batch; ++i) p.off[0][i] = offsets[s + i];
+    for (int i = 0; i < p.batch; ++i) p.frame_off[i + 1] = p.frame_off[i] + stft_frames(offsets[s + i + 1] - offsets[s + i]);
+    CK(launch_metric_stft(p, st));
+    ctx->launches++;
+    rows += (long)p.frame_off[p.batch];
+  }
+  if (mel_out) {
+    MelParams m;
+    memset(&m, 0, sizeof m);
+    m.in = sp_out; m.n_outer = 1; m.T = rows; m.so = 0; m.sf = 1; m.st = 1025;
+    m.out = mel_out; m.fb_f0 = ctx->d_fb_f0; m.fb_len = ctx->d_fb_len; m.fb_ofs = ctx->d_fb_ofs; m.fb_val = ctx->d_fb_val;
+    CK(launch_mel(m, st));
+    ctx->launches++;
+  }
+  return VF_OK;
+}
+
+VF_API int vf_ssim(vf_ctx* ctx, const float* est, const float* target, int images, int frames, int bins, double* out, void* stream) {
+  const int rc = begin_call(ctx, "vf_ssim", est && target && out && images > 0);
+  if (rc) return rc;
+  if (frames < 7 || bins < 7) return fail(ctx, VF_EINVAL, "vf_ssim: a %d x %d image is smaller than the 7 x 7 window", frames, bins);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int per = ssim_tiles(frames, bins);
+  double* partial = nullptr;                 // stream-ordered scratch
+  CK(cudaMallocAsync((void**)&partial, (size_t)per * std::min(images, SCORE_MAX_IMAGES) * sizeof(double), st));
+  const std::vector<int> starts = split(images, SCORE_MAX_IMAGES);
+  cudaError_t e = cudaSuccess;
+  for (size_t k = 0; k + 1 < starts.size() && e == cudaSuccess; ++k) {
+    const int s = starts[k];
+    SsimParams p;
+    memset(&p, 0, sizeof p);
+    p.batch = starts[k + 1] - s;
+    const size_t off = (size_t)s * frames * bins;
+    p.x = est + off; p.y = target + off; p.F = bins; p.partial = partial;
+    for (int i = 0; i <= p.batch; ++i) { p.frame_off[i] = (int64_t)i * frames; p.tile_off[i] = i * per; }
+    e = launch_ssim(p, out + s, 1, st);
+    ctx->launches += 2;
+  }
+  cudaFreeAsync(partial, st);
+  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "ssim launch: %s", cudaGetErrorString(e));
+  return VF_OK;
+}
+
+VF_API int vf_score_varlen(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target, const int64_t* target_offsets,
+                           int batch, double* out, void* stream) {
+  static const char* fn = "vf_score_varlen";
+  int rc = begin_call(ctx, fn, est && target && out && batch > 0);
+  if (!rc) rc = check_offsets(ctx, fn, "est", "clip", est_offsets, batch, 1025, ITEM_MAX);
+  if (!rc) rc = check_offsets(ctx, fn, "target", "clip", target_offsets, batch, 1025, ITEM_MAX);
+  if (rc) return rc;
+  std::vector<long> T(batch);
+  for (int i = 0; i < batch; ++i) {
+    T[i] = stft_frames(est_offsets[i + 1] - est_offsets[i]);
+    const long tt = stft_frames(target_offsets[i + 1] - target_offsets[i]);
+    if (T[i] != tt) return fail(ctx, VF_EINVAL, "vf_score_varlen: pair %d: est has %ld frames, target %ld", i, T[i], tt);
+    if (T[i] < 7) return fail(ctx, VF_EINVAL, "vf_score_varlen: pair %d has %ld frames, fewer than SSIM's 7", i, T[i]);
+  }
+  if (!ctx->d_fb_val) return fail(ctx, VF_ESTATE, "mel filterbank not loaded (call vf_load_weights first)");
+  cudaStream_t st = (cudaStream_t)stream;
+  // sub-batches of at most SCORE_MAX_IMAGES pairs and SCORE_CAP_FRAMES frames per side.  Scratch per pair: two
+  // spectrograms, two mels, its SSIM tile sums.
+  const std::vector<int> starts = split(batch, SCORE_MAX_IMAGES, SCORE_CAP_FRAMES, [&](int i) { return (int64_t)T[i]; });
+  rc = acquire_scratch(ctx, ctx->score, max_bytes(starts, [&](int i) {
+    return (size_t)T[i] * (2 * 1025 + 2 * 128) * 4 + (size_t)(ssim_tiles(T[i], 1025) + ssim_tiles(T[i], 128)) * 8;
+  }), st);
+  if (rc) return rc;
+  cudaError_t e = cudaSuccess;
+  for (size_t k = 0; k + 1 < starts.size() && e == cudaSuccess; ++k) {
+    const int s = starts[k], nb = starts[k + 1] - starts[k];
+    MetricStftParams p;
+    memset(&p, 0, sizeof p);
+    ImageSet set;
+    memset(&set, 0, sizeof set);
+    p.batch = set.batch = nb;
+    p.sources = 2;
+    for (int i = 0; i <= nb; ++i) { p.off[0][i] = est_offsets[s + i]; p.off[1][i] = target_offsets[s + i]; }
+    for (int i = 0; i < nb; ++i) p.frame_off[i + 1] = set.frame_off[i + 1] = p.frame_off[i] + T[s + i];
+    const long F = (long)p.frame_off[nb];
+    float* sp_e = static_cast<float*>(ctx->score.p);
+    float* sp_t = sp_e + (size_t)F * 1025;
+    float* mel_e = sp_t + (size_t)F * 1025;
+    float* mel_t = mel_e + (size_t)F * 128;
+    double* partial = reinterpret_cast<double*>(mel_t + (size_t)F * 128);   // F * 2306 floats: 8-byte aligned
+    p.wav[0] = est; p.wav[1] = target; p.sp[0] = sp_e; p.sp[1] = sp_t;
+    p.window = ctx->d_window64; p.tw1024 = ctx->d_tw1024d; p.tw2048 = ctx->d_tw2048d;
+    e = launch_metric_stft(p, st);
+    MelParams m;                              // both spectrograms in one launch: outer index 0 = est, 1 = target
+    memset(&m, 0, sizeof m);
+    m.in = sp_e; m.n_outer = 2; m.T = F; m.so = F * 1025; m.sf = 1; m.st = 1025;
+    m.out = mel_e; m.fb_f0 = ctx->d_fb_f0; m.fb_len = ctx->d_fb_len; m.fb_ofs = ctx->d_fb_ofs; m.fb_val = ctx->d_fb_val;
+    if (e == cudaSuccess) e = launch_mel(m, st);
+    double* o = out + (size_t)s * 8;
+    const float* img[2][2] = {{sp_e, sp_t}, {mel_e, mel_t}};
+    const int bins[2] = {1025, 128};
+    for (int r = 0; r < 2 && e == cudaSuccess; ++r) {        // keys 0-3 on the spectrogram, 4-7 on the mel
+      e = launch_lsd_varlen(img[r][0], img[r][1], bins[r], set, o + 4 * r, 8, st);
+      if (e == cudaSuccess) e = launch_sispec_varlen(img[r][0], img[r][1], bins[r], set, o + 4 * r + 1, 8, st);
+      SsimParams q;
+      memset(&q, 0, sizeof q);
+      q.x = img[r][0]; q.y = img[r][1]; q.F = bins[r]; q.batch = nb; q.partial = partial;
+      for (int i = 0; i <= nb; ++i) q.frame_off[i] = set.frame_off[i];
+      for (int i = 0; i < nb; ++i) q.tile_off[i + 1] = q.tile_off[i] + ssim_tiles(T[s + i], bins[r]);
+      if (e == cudaSuccess) e = launch_ssim(q, o + 4 * r + 3, 8, st);
+    }
+    ctx->launches += 10;
+  }
+  rc = mark_use(ctx, ctx->score.order, st);
+  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "score launch: %s", cudaGetErrorString(e));
+  return rc;
+}
+
+VF_API int vf_score_time_varlen(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target,
+                                const int64_t* target_offsets, int batch, double* out, void* stream) {
+  static const char* fn = "vf_score_time_varlen";
+  int rc = begin_call(ctx, fn, est && target && out && batch > 0);
+  if (!rc) rc = check_offsets(ctx, fn, "est", "pair", est_offsets, batch, 1, ITEM_MAX);
+  if (!rc) rc = check_offsets(ctx, fn, "target", "pair", target_offsets, batch, 1, ITEM_MAX);
+  if (rc) return rc;
+  std::vector<int64_t> N(batch);
+  for (int i = 0; i < batch; ++i) {
+    N[i] = std::max(est_offsets[i + 1] - est_offsets[i], target_offsets[i + 1] - target_offsets[i]);
+    if (stoi_len10(N[i]) <= STOI_FRAME)
+      return fail(ctx, VF_EINVAL, "vf_score_time_varlen: pair %d: %ld samples give %ld at 10 kHz, STOI needs more than %d", i,
+                  (long)N[i], (long)stoi_len10(N[i]), STOI_FRAME);
+  }
+  rc = stoi_tables(ctx);
+  if (rc) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  // sub-batches of at most SCORE_MAX_IMAGES pairs and SCORE_CAP_FRAMES * 441 padded samples.  Scratch per pair:
+  // resampled and compacted signals, energies, band values, tile sums (doubles), then kept-frame indices and a count (ints).
+  const std::vector<int> starts = split(batch, SCORE_MAX_IMAGES, SCORE_CAP_FRAMES * 441, [&](int i) { return N[i]; });
+  rc = acquire_scratch(ctx, ctx->time_score, max_bytes(starts, [&](int i) {
+    const int64_t n10 = stoi_len10(N[i]), nf = stoi_frames(n10);
+    return (size_t)(4 * n10 + (1 + 2 * STOI_BANDS) * nf + stoi_tiles(nf)) * 8 + (size_t)(nf + 1) * 4;
+  }), st);
+  if (rc) return rc;
+  cudaError_t e = cudaSuccess;
+  for (size_t k = 0; k + 1 < starts.size() && e == cudaSuccess; ++k) {
+    const int s = starts[k], nb = starts[k + 1] - starts[k];
+    TimeScoreParams p;
+    memset(&p, 0, sizeof p);
+    p.batch = nb;
+    p.est = est + est_offsets[s];
+    p.tgt = target + target_offsets[s];
+    for (int i = 0; i <= nb; ++i) {
+      p.e_off[i] = est_offsets[s + i] - est_offsets[s];
+      p.t_off[i] = target_offsets[s + i] - target_offsets[s];
+    }
+    for (int i = 0; i < nb; ++i) {
+      const int64_t n10 = stoi_len10(N[s + i]), nf = stoi_frames(n10);
+      p.r_off[i + 1] = p.r_off[i] + n10;
+      p.f_off[i + 1] = p.f_off[i] + nf;
+      p.tile_off[i + 1] = p.tile_off[i] + stoi_tiles(nf);
+    }
+    stoi_bands(p.band_lo, p.band_hi);
+    p.clip = 1 + std::pow(10.0, 15.0 / 20);
+    p.taps = ctx->d_stoi_tables;
+    p.window = ctx->d_stoi_tables + STOI_WIN_AT;
+    p.tw256 = reinterpret_cast<const double2*>(ctx->d_stoi_tables + STOI_TW256_AT);
+    p.tw512 = reinterpret_cast<const double2*>(ctx->d_stoi_tables + STOI_TW512_AT);
+    const int64_t Rs = p.r_off[nb], Fs = p.f_off[nb], Ts = p.tile_off[nb];
+    double* d = static_cast<double*>(ctx->time_score.p);
+    p.rs = d;
+    p.cs = p.rs + 2 * Rs;
+    p.energy = p.cs + 2 * Rs;
+    p.tob = p.energy + Fs;
+    p.partial = p.tob + 2 * STOI_BANDS * Fs;
+    p.src = reinterpret_cast<int*>(p.partial + Ts);
+    p.kept = p.src + Fs;
+    p.out = out + (size_t)s * 2;
+    e = launch_score_time(p, st);
+    ctx->launches += Ts > 0 ? 8 : 7;
+  }
+  rc = mark_use(ctx, ctx->time_score.order, st);
+  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "time score launch: %s", cudaGetErrorString(e));
+  return rc;
+}
+
+// ------------------------------------------------------------------------------------------------------ SR degradations
+VF_API int vf_sosfiltfilt_varlen(vf_ctx* ctx, const double* x, const int64_t* offsets, int batch, const double* sos,
+                                 const double* zi, const int* n_sections, int n_filters, const int* row_filter, const int* row_f32,
+                                 double* out, void* stream) {
+  static const char* fn = "vf_sosfiltfilt_varlen";
+  int rc = begin_call(ctx, fn, x && sos && zi && n_sections && row_filter && out && batch > 0 && n_filters > 0);
+  if (!rc) rc = check_offsets(ctx, fn, "x", "row", offsets, batch, 1);
+  if (rc) return rc;
+  std::vector<int> edge(n_filters);
+  for (int f = 0; f < n_filters; ++f) {
+    const int ns = n_sections[f];
+    if (ns < 1 || ns > IIR_MAX_SECTIONS) return fail(ctx, VF_EINVAL, "%s: filter %d has %d sections (need 1 .. %d)", fn, f, ns, IIR_MAX_SECTIONS);
+    const double* s = sos + (size_t)f * 6 * IIR_MAX_SECTIONS;
+    int zb = 0, za = 0;
+    for (int k = 0; k < ns; ++k) {
+      if (s[6 * k + 3] != 1.0) return fail(ctx, VF_EINVAL, "%s: filter %d: sos[%d, 3] is not 1", fn, f, k);
+      zb += s[6 * k + 2] == 0.0;
+      za += s[6 * k + 5] == 0.0;
+    }
+    edge[f] = 3 * (2 * ns + 1 - std::min(zb, za));        // sosfiltfilt's default padlen
+  }
+  std::vector<int64_t> ne(batch);
+  for (int i = 0; i < batch; ++i) {
+    const int f = row_filter[i];
+    if (f < 0 || f >= n_filters) return fail(ctx, VF_EINVAL, "%s: row %d: filter %d of %d", fn, i, f, n_filters);
+    const int64_t n = offsets[i + 1] - offsets[i];
+    if (n <= edge[f]) return fail(ctx, VF_EINVAL, "%s: row %d has %ld samples, not more than its padlen %d", fn, i, (long)n, edge[f]);
+    ne[i] = n + 2 * (int64_t)edge[f];
+  }
+  auto chunks = [](int64_t n) { return (n + IIR_CHUNK - 1) / IIR_CHUNK; };
+  // sub-batches of at most IIR_MAX_ROWS rows and IIR_CAP_SAMPLES extended samples; the call's filter tables lead the scratch
+  const std::vector<int> starts = split(batch, IIR_MAX_ROWS, IIR_CAP_SAMPLES, [&](int i) { return ne[i]; });
+  const size_t table_doubles = (size_t)n_filters * IIR_TABLE;
+  cudaStream_t st = (cudaStream_t)stream;
+  rc = acquire_scratch(ctx, ctx->iir, table_doubles * sizeof(double) + max_bytes(starts, [&](int i) {
+    return (size_t)(ne[i] + chunks(ne[i]) * IIR_MAX_STATES) * sizeof(double);   // the row's extended samples and chunk states
+  }), st);
+  if (rc) return rc;
+  double* tables = static_cast<double*>(ctx->iir.p);
+  cudaError_t e = cudaSuccess;
+  for (int f0 = 0; f0 < n_filters && e == cudaSuccess; f0 += IIR_DESIGN_FILTERS) {   // sos and zi go as kernel parameters
+    IirDesignParams d;
+    memset(&d, 0, sizeof d);
+    d.tables = tables + (size_t)f0 * IIR_TABLE;
+    d.n = std::min(IIR_DESIGN_FILTERS, n_filters - f0);
+    for (int i = 0; i < d.n; ++i) {
+      const int f = f0 + i;
+      d.n_sections[i] = n_sections[f];
+      std::copy(sos + (size_t)f * 6 * IIR_MAX_SECTIONS, sos + (size_t)f * 6 * IIR_MAX_SECTIONS + 6 * n_sections[f], d.sos[i]);
+      std::copy(zi + (size_t)f * 2 * IIR_MAX_SECTIONS, zi + (size_t)f * 2 * IIR_MAX_SECTIONS + 2 * n_sections[f], d.zi[i]);
+    }
+    e = launch_iir_design(d, st);
+    ctx->launches += 1;
+  }
+  for (size_t k = 0; k + 1 < starts.size() && e == cudaSuccess; ++k) {
+    const int s = starts[k], nb = starts[k + 1] - starts[k];
+    SosParams p;
+    memset(&p, 0, sizeof p);
+    p.batch = nb;
+    p.x = x + offsets[s];
+    p.out = out + offsets[s];
+    for (int i = 0; i < nb; ++i) {
+      const int f = row_filter[s + i];
+      p.off[i + 1] = offsets[s + i + 1] - offsets[s];
+      p.ext_off[i + 1] = p.ext_off[i] + ne[s + i];
+      p.chunk_off[i + 1] = p.chunk_off[i] + chunks(ne[s + i]);
+      p.edge[i] = edge[f];
+      p.ext_f32[i] = row_f32 ? row_f32[s + i] != 0 : 0;
+      p.n_sections[i] = n_sections[f];
+      p.table[i] = tables + (size_t)f * IIR_TABLE;
+    }
+    p.yf = tables + table_doubles;
+    p.state = p.yf + p.ext_off[nb];
+    e = launch_sosfiltfilt(p, st);
+    ctx->launches += 6;
+  }
+  rc = mark_use(ctx, ctx->iir.order, st);
+  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "sosfiltfilt launch: %s", cudaGetErrorString(e));
+  return rc;
+}
+
+VF_API int vf_resample_poly_f64_varlen(vf_ctx* ctx, const double* x, const int64_t* in_offsets, int batch, const double* taps,
+                                       const int64_t* tap_offsets, const int* up, const int* down, int n_filters,
+                                       const int* row_filter, double* y, const int64_t* out_offsets, void* stream) {
+  static const char* fn = "vf_resample_poly_f64_varlen";
+  int rc = begin_call(ctx, fn, x && taps && tap_offsets && up && down && row_filter && y && batch > 0 && n_filters > 0);
+  if (!rc) rc = check_offsets(ctx, fn, "x", "row", in_offsets, batch, 1);
+  if (!rc) rc = check_offsets(ctx, fn, "y", "row", out_offsets, batch, 0);
+  if (rc) return rc;
+  if (tap_offsets[0] != 0) return fail(ctx, VF_EINVAL, "%s: tap offsets must start at 0", fn);
+  for (int f = 0; f < n_filters; ++f) {
+    const int64_t nt = tap_offsets[f + 1] - tap_offsets[f];
+    if (nt < 1 || nt % 2 == 0 || nt > (int64_t(1) << 30))
+      return fail(ctx, VF_EINVAL, "%s: filter %d has %ld taps (need an odd count)", fn, f, (long)nt);
+    if (up[f] < 1 || down[f] < 1) return fail(ctx, VF_EINVAL, "%s: filter %d: up %d, down %d (need >= 1)", fn, f, up[f], down[f]);
+  }
+  for (int i = 0; i < batch; ++i)
+    if (row_filter[i] < 0 || row_filter[i] >= n_filters)
+      return fail(ctx, VF_EINVAL, "%s: row %d: filter %d of %d", fn, i, row_filter[i], n_filters);
+  const std::vector<int> starts = split(batch, IIR_MAX_ROWS);
+  cudaError_t e = cudaSuccess;
+  for (size_t k = 0; k + 1 < starts.size() && e == cudaSuccess; ++k) {
+    const int s = starts[k], nb = starts[k + 1] - starts[k];
+    ResampleF64Params p;
+    memset(&p, 0, sizeof p);
+    p.batch = nb;
+    p.x = x + in_offsets[s];
+    p.y = y + out_offsets[s];
+    p.taps = taps;
+    for (int i = 0; i < nb; ++i) {
+      const int f = row_filter[s + i];
+      p.in_off[i + 1] = in_offsets[s + i + 1] - in_offsets[s];
+      p.out_off[i + 1] = out_offsets[s + i + 1] - out_offsets[s];
+      p.tap_at[i] = tap_offsets[f];
+      p.half[i] = (int)((tap_offsets[f + 1] - tap_offsets[f] - 1) / 2);
+      p.up[i] = up[f];
+      p.down[i] = down[f];
+    }
+    e = launch_resample_f64(p, (cudaStream_t)stream);
+    ctx->launches += 1;
+  }
+  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "resample launch: %s", cudaGetErrorString(e));
+  return VF_OK;
+}
+
+// ------------------------------------------------------------------------------------------- finalize and conversions
+VF_API int vf_finalize(vf_ctx* ctx, const float* wav, int batch, int64_t len, int64_t n, float* wav_out, void* stream) {
+  const int rc = begin_call(ctx, "vf_finalize", wav && wav_out && batch > 0 && len > 0 && n > 0);
+  if (rc) return rc;
+  const long d = (long)len - (long)n;
+  // trim_center (tools/utils.py:57-70) for an estimate at least as long as the reference; d == 1 is the reference's
+  // empty-slice case (est[..., 0:-0])
+  if (d < 0 || d == 1) return fail(ctx, VF_EINVAL, "vf_finalize: estimate length %ld vs reference %ld is not a trim_center case the path produces", (long)len, (long)n);
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned int* peak = nullptr;
+  CK(cudaMallocAsync((void**)&peak, (size_t)batch * 4, st));
+  CK(cudaMemsetAsync(peak, 0, (size_t)batch * 4, st));
+  cudaError_t e1 = launch_peak(wav, batch, (long)len, peak, st);
+  FinalizeParams f;
+  memset(&f, 0, sizeof f);
+  f.wav = wav; f.peak_bits = peak; f.batch = batch; f.L = (long)len; f.n = (long)n; f.skip = d / 2;
+  f.out = wav_out; f.out_ld = (long)n; f.out_off = 0;
+  cudaError_t e2 = e1 == cudaSuccess ? launch_finalize(f, st) : e1;
+  cudaFreeAsync(peak, st);
+  if (e2 != cudaSuccess) return fail(ctx, VF_ECUDA, "finalize launch: %s", cudaGetErrorString(e2));
+  ctx->launches += 2;
+  return VF_OK;
+}
+
+VF_API int vf_to_log(vf_ctx* ctx, const float* in, float* out, int64_t n, void* stream) {
+  const int rc = begin_call(ctx, "vf_to_log", in && out && n > 0);
+  if (rc) return rc;
+  CK(launch_to_log(in, out, (size_t)n, ctx->d_err + 1, (cudaStream_t)stream));
+  ctx->launches++;
+  return VF_OK;
+}
+VF_API int vf_from_log(vf_ctx* ctx, const float* in, float* out, int64_t n, void* stream) {
+  const int rc = begin_call(ctx, "vf_from_log", in && out && n > 0);
+  if (rc) return rc;
+  CK(launch_from_log(in, out, (size_t)n, (cudaStream_t)stream));
+  ctx->launches++;
+  return VF_OK;
+}
+
+VF_API int vf_to_pcm16_ex(vf_ctx* ctx, const float* in, int16_t* out, int64_t n, int saturate, void* stream) {
+  const int rc = begin_call(ctx, "vf_to_pcm16_ex", in && out && n > 0);
+  if (rc) return rc;
+  CK(launch_pcm16(in, out, (size_t)n, saturate ? 1 : 0, (cudaStream_t)stream));
+  ctx->launches++;
+  return VF_OK;
+}
+VF_API int vf_to_pcm16(vf_ctx* ctx, const float* in, int16_t* out, int64_t n, void* stream) {
+  return vf_to_pcm16_ex(ctx, in, out, n, 0, stream);
+}
+
+}  // extern "C"

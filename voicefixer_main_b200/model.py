@@ -80,6 +80,11 @@ def _stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+def _offsets(lengths):
+    """Host int64 offsets of a packed set: 0, then the running sum of `lengths`."""
+    return (ctypes.c_int64 * (len(lengths) + 1))(0, *itertools.accumulate(lengths))
+
+
 def _check_in(t: torch.Tensor, device, what: str):
     if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or not t.is_cuda or t.device != device:
         raise TypeError(f"{what} must be a float32 CUDA tensor on {device}")
@@ -228,13 +233,14 @@ class Engine:
                                                      _ptr(mel_out), _ptr(log_mel_out), _stream()))
         return out
 
-    def _varlen_args(self, wav_packed: torch.Tensor, lengths):
-        """Checked packed input and the host offsets array (0, then the running sum of lengths) of a varlen call."""
-        wav_packed = _check_in(wav_packed, self.device, "wav_packed")
+    def _varlen_args(self, packed: torch.Tensor, lengths, dtype=torch.float32):
+        """Checked packed `dtype` input and the host offsets array of a varlen call."""
+        if not isinstance(packed, torch.Tensor) or packed.dtype != dtype or packed.device != self.device:
+            raise TypeError(f"the packed input must be a {str(dtype)[6:]} CUDA tensor on {self.device}")
         lengths = [int(n) for n in lengths]
-        if wav_packed.dim() != 1 or not lengths or sum(lengths) != wav_packed.numel():
-            raise ValueError("wav_packed must be 1-D and hold exactly sum(lengths) samples of at least one clip")
-        return wav_packed, (ctypes.c_int64 * (len(lengths) + 1))(0, *itertools.accumulate(lengths))
+        if packed.dim() != 1 or not lengths or sum(lengths) != packed.numel():
+            raise ValueError("the packed input must be 1-D and hold exactly sum(lengths) samples of at least one item")
+        return packed.contiguous(), _offsets(lengths)
 
     def _packed_rows(self, offsets, **outs) -> int:
         """Rows sum_i frames_for(n_i) of a varlen call's packed per-frame outputs (clip i from row sum_{j<i} frames_for(n_j));
@@ -311,21 +317,12 @@ class Engine:
                                                    len(est_off) - 1, _ptr(out), _stream()))
         return out
 
-    def _packed64(self, x_packed: torch.Tensor, lengths):
-        """Checked packed float64 input of the float64 varlen calls and its host offsets."""
-        if not isinstance(x_packed, torch.Tensor) or x_packed.dtype != torch.float64 or x_packed.device != self.device:
-            raise TypeError(f"x_packed must be a float64 CUDA tensor on {self.device}")
-        lengths = [int(n) for n in lengths]
-        if x_packed.dim() != 1 or not lengths or sum(lengths) != x_packed.numel():
-            raise ValueError("x_packed must be 1-D and hold exactly sum(lengths) samples of at least one row")
-        return x_packed.contiguous(), (ctypes.c_int64 * (len(lengths) + 1))(0, *itertools.accumulate(lengths))
-
     def sosfiltfilt_varlen(self, x_packed: torch.Tensor, lengths, sos, zi, row_filter, row_f32=None) -> torch.Tensor:
         """vf_sosfiltfilt_varlen: scipy.signal.sosfiltfilt(sos[f], row) of each float64 row of x_packed (rows back to back,
         `lengths` samples each), row i with filter f = row_filter[i]; sos[f] is an [n_sections <= 10, 6] float64 array and
         zi[f] its sosfilt_zi.  row_f32[i] true: row i holds float32 input, whose odd extension scipy rounds to float32.
         -> float64, packed like x_packed."""
-        x_packed, off = self._packed64(x_packed, lengths)
+        x_packed, off = self._varlen_args(x_packed, lengths, torch.float64)
         nf = len(sos)
         sos_t = (ctypes.c_double * (nf * 60))()
         zi_t = (ctypes.c_double * (nf * 20))()
@@ -349,11 +346,11 @@ class Engine:
         """vf_resample_poly_f64_varlen: scipy.signal.resample_poly of each float64 row of x_packed, row i with filter
         filters[row_filter[i]] = (up, down, taps: float64 device tensor of odd length) -> float64 rows of out_lengths[i]
         samples packed back to back (ceil(n up / down) is resample_poly's length; more pads zeros, fewer cuts)."""
-        x_packed, off = self._packed64(x_packed, lengths)
+        x_packed, off = self._varlen_args(x_packed, lengths, torch.float64)
         out_lengths = [int(n) for n in out_lengths]
-        out_off = (ctypes.c_int64 * (len(out_lengths) + 1))(0, *itertools.accumulate(out_lengths))
+        out_off = _offsets(out_lengths)
         taps = torch.cat([t.to(self.device, torch.float64).reshape(-1) for _, _, t in filters]).contiguous()
-        tap_off = (ctypes.c_int64 * (len(filters) + 1))(0, *itertools.accumulate(t.numel() for _, _, t in filters))
+        tap_off = _offsets([t.numel() for _, _, t in filters])
         up = (ctypes.c_int * len(filters))(*[int(u) for u, _, _ in filters])
         down = (ctypes.c_int * len(filters))(*[int(d) for _, d, _ in filters])
         rows = (ctypes.c_int * len(row_filter))(*[int(f) for f in row_filter])
