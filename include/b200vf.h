@@ -122,7 +122,8 @@ VF_API const char* vf_last_error(vf_ctx* ctx);   /* ctx may be NULL: error of th
  * alone is enough for the front end and for scoring (vf_metric_spectrogram, vf_score_varlen). */
 VF_API int vf_load_weights(vf_ctx* ctx, const vf_tensor_desc* descs, int n);
 
-/* wav [B,N] -> mel_out [B,T,128] linear mel (T = 1 + N/hop); optional sp/cos/sin [B,T,1025] (NULL to skip). */
+/* wav [B,N] -> mel_out [B,T,128] linear mel (T = 1 + N/hop); optional sp/cos/sin [B,T,1025] (NULL to skip).
+ * B <= 65535 (one launch: the clips are the grid's y dimension). */
 VF_API int vf_frontend(vf_ctx* ctx, const float* wav, int batch, int64_t n_samples, float* mel_out, float* sp_out,
                 float* cos_out, float* sin_out, void* stream);
 
@@ -202,7 +203,8 @@ VF_API int vf_ssr_restore_host(vf_ctx* ctx, const float* wav_host, int batch, in
 VF_API int vf_ssr_unet(vf_ctx* ctx, const float* sp, int batch, int frames, float* mag_out, void* stream);
 /* Intermediates of the last vf_ssr_* call of this shape: input magnitude and predicted magnitude [B,T,1025]. */
 VF_API int vf_ssr_stages(vf_ctx* ctx, int batch, int64_t n_samples, float* sp_out, float* mag_out, void* stream);
-/* FDomainHelper.istft(real, imag, length): real, imag [B,T,1025] -> wav_out [B,length]. */
+/* FDomainHelper.istft(real, imag, length): real, imag [B,T,1025] -> wav_out [B,length], B <= 65535, length + n_fft/2 <=
+ * (T - 1) * hop + n_fft. */
 VF_API int vf_istft(vf_ctx* ctx, const float* real, const float* imag, int batch, int frames, int64_t length,
                     float* wav_out, void* stream);
 
@@ -412,7 +414,7 @@ VF_API int vf_selftest_layer(vf_ctx* ctx, vf_layer_case* lc);
  * pointer, and output buffers are read AND written as in vf_selftest_layer.  fp16 planes are bit patterns [2][batch][rows][C].
  * Fields a kind does not use are zero.  The mel-weight table, window and twiddles are the context's own. */
 enum { VF_OP_FIRST = 0, VF_OP_POOL = 1, VF_OP_COND = 2, VF_OP_REFLECT = 3, VF_OP_TAIL = 4, VF_OP_FINALIZE = 5, VF_OP_ISTFT = 6,
-       VF_OP_PEAK_NORM = 7 };
+       VF_OP_PEAK_NORM = 7, VF_OP_FRONTEND = 8 };
 typedef struct vf_op_case {
   int kind, batch;
   /* Clips of different lengths (any kind; PEAK_NORM needs them): host sample offsets [batch + 1], clip b = [off[b], off[b + 1]).
@@ -472,6 +474,16 @@ typedef struct vf_op_case {
   int Tp, Wpo, Tv;
   int64_t skip;
   int64_t tail_smem;
+  /* FRONTEND (n; the mel filterbank must be loaded): the front end as every restore runs it, on in_wav [batch][n] with the
+   * outputs that are not NULL: mel_out / logmel_out [batch][T][128], sp_out / cos_out / sin_out [batch][T][1025] (cos and
+   * sin together, and only with sp).  Uniform: T = 1 + n / hop is reported back.  With clip_off: in_wav packed, n = the
+   * longest clip, T = the caller's rows per clip (the varlen plans' bucket; a clip with more frames, or with 1024 samples
+   * or fewer, fails with VF_EINVAL); rows t >= T_b of clip b are not written. */
+  float* mel_out;
+  float* logmel_out;
+  float* sp_out;
+  float* cos_out;
+  float* sin_out;
 } vf_op_case;
 VF_API int vf_selftest_op(vf_ctx* ctx, vf_op_case* oc);
 

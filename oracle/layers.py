@@ -7,7 +7,9 @@
   bars against mutated references).
 - The non-GEMM kernels of the same launch chains (aux.cu, istft.cu): the UNet's first layer with its input padding,
   pooling, the vocoder conditioning and its low-band sums, reflection padding, the tail conv, peak normalise + trim and the
-  fused ISTFT of the SSR back end.  Used by tests/test_gpu_aux.py and tests/test_aux_cpu.py in the same two ways."""
+  fused ISTFT of the SSR back end.  Used by tests/test_gpu_aux.py and tests/test_aux_cpu.py in the same two ways.
+- The STFT + mel front end (frontend.cu) and the stand-alone mel and ISTFT: used by tests/test_gpu_frontend.py and
+  tests/test_frontend_cpu.py."""
 import numpy as np
 import torch
 import torch.nn.functional as F
@@ -269,6 +271,17 @@ def phase(X, eps=1e-8):
     """fDomainHelper.py:60-65: cos, sin = re / m, im / m with m = sqrt(max(|X|^2, eps))."""
     m = np.sqrt(np.maximum(X.real ** 2 + X.imag ** 2, eps))
     return X.real / m, X.imag / m
+
+
+def frontend64(wav, T, fb):
+    """The front end of one clip (frontend.cu) in float64: the first T frames of the STFT X [T, 1025] and S_t = Σ|x w| per
+    frame, the clamped magnitude and its cos / sin (fDomainHelper.py:62-64, power clamp 1e-8), mel = mag @ fb with the
+    caller's fp32 filterbank [1025, 128] widened, and log-mel = log10(max(mel, 1e-8)) (pytorch_util.py:157-159)."""
+    X, S = stft64(wav, T)
+    mag = np.sqrt(np.maximum(X.real ** 2 + X.imag ** 2, 1e-8))
+    cs, sn = phase(X)
+    mel = mag @ np.asarray(fb, np.float32).astype(np.float64)
+    return dict(X=X, S=S, mag=mag, cos=cs, sin=sn, mel=mel, logmel=np.log10(np.maximum(mel, 1e-8)))
 
 
 def inverse_frames(Y, keep_dc_imag=False):

@@ -72,7 +72,8 @@ class VfOpCase(Structure):
                 ("tail_in", c_void_p), ("tail_w", c_void_p), ("tail_b", c_float), ("wav", c_void_p), ("peak_bits", c_void_p),
                 ("n", c_int64)] + \
                [(f, c_void_p) for f in ("in_wav", "mag", "frames", "out")] + \
-               [("Tp", c_int), ("Wpo", c_int), ("Tv", c_int), ("skip", c_int64), ("tail_smem", c_int64)]
+               [("Tp", c_int), ("Wpo", c_int), ("Tv", c_int), ("skip", c_int64), ("tail_smem", c_int64)] + \
+               [(f, c_void_p) for f in ("mel_out", "logmel_out", "sp_out", "cos_out", "sin_out")]     # VF_OP_FRONTEND
 
 
 class VfGruCase(Structure):

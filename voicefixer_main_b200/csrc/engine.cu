@@ -697,7 +697,7 @@ VF_API int vf_frontend(vf_ctx* ctx, const float* wav, int batch, int64_t n, floa
                 float* sin_out, void* stream) {
   int rc = check_ready(ctx);
   if (rc) return rc;
-  if (!wav || batch <= 0) return fail(ctx, VF_EINVAL, "vf_frontend: bad arguments");
+  if (!wav || batch <= 0 || batch > 65535) return fail(ctx, VF_EINVAL, "vf_frontend: bad arguments (batch must be 1 .. 65535)");
   if ((cos_out || sin_out) && !(sp_out && cos_out && sin_out)) return fail(ctx, VF_EINVAL, "cos/sin need sp, cos and sin");
   return run_frontend(ctx, wav, batch, (long)n, mel_out, nullptr, sp_out, cos_out, sin_out, (cudaStream_t)stream);
 }
@@ -1362,6 +1362,27 @@ int run_op_case(vf_ctx* ctx, Builder& b, vf_op_case& c) {
       CK(launch_peak_normalise_varlen(wav, plan.d_vl_off, B, (long)c.n, peak, 0));
       break;
     }
+    case VF_OP_FRONTEND: {       // run_frontend as restore_impl, ssr_impl, ssr_restore_varlen and vf_frontend call it
+      if (!ctx->d_fb_val) return fail(ctx, VF_ESTATE, "vf_selftest_op: mel filterbank not loaded");
+      if (!c.clip_off) c.T = frames_of(ctx, (long)c.n);
+      for (int i = 0; c.clip_off && i < B; ++i) {
+        const long nb = (long)(c.clip_off[i + 1] - c.clip_off[i]);
+        if (nb <= 1024 || nb > c.n || frames_of(ctx, nb) > c.T)
+          return fail(ctx, VF_EINVAL, "vf_selftest_op: clip %d has %ld samples (need 1025 .. n, at most T = %d frames)", i, nb, c.T);
+      }
+      const size_t rows = (size_t)B * c.T;
+      float* mel = static_cast<float*>(out(c.mel_out, rows * 128 * sizeof(float)));
+      float* logmel = static_cast<float*>(out(c.logmel_out, rows * 128 * sizeof(float)));
+      float* sp = static_cast<float*>(out(c.sp_out, rows * 1025 * sizeof(float)));
+      float* co = static_cast<float*>(out(c.cos_out, rows * 1025 * sizeof(float)));
+      float* si = static_cast<float*>(out(c.sin_out, rows * 1025 * sizeof(float)));
+      const float* wav = fl(c.in_wav, c.clip_off ? packed : (int64_t)B * c.n);
+      if (b.rc) return b.rc;
+      plan.T = c.T;
+      rc = run_frontend(ctx, wav, B, (long)c.n, mel, logmel, sp, co, si, 0, c.clip_off ? &plan : nullptr);
+      if (rc) return rc;
+      break;
+    }
   }
   if (b.rc) return b.rc;
   rc = run_ops(ctx, ops, 0);
@@ -1413,7 +1434,7 @@ VF_API int vf_selftest_gru(vf_ctx* ctx, vf_gru_case* gc) {
 VF_API int vf_selftest_op(vf_ctx* ctx, vf_op_case* oc) {
   if (!ctx || !oc) return VF_EINVAL;
   vf_op_case& c = *oc;
-  const bool bad_kind = c.kind < VF_OP_FIRST || c.kind > VF_OP_PEAK_NORM;
+  const bool bad_kind = c.kind < VF_OP_FIRST || c.kind > VF_OP_FRONTEND;
   const bool bad_shape =
       (c.kind == VF_OP_FIRST && (c.T <= 0 || c.W <= 0 || !c.x || !c.w1 || !c.bn2_scale || !c.bn2_shift || !c.w_sc || !c.b_sc)) ||
       (c.kind == VF_OP_POOL && (c.H < 2 || c.W <= 0 || c.C <= 0 || c.C % 8 || !c.pin || !c.a_scale || !c.a_shift || c.level < 0 || c.level > 5)) ||
@@ -1423,7 +1444,8 @@ VF_API int vf_selftest_op(vf_ctx* ctx, vf_op_case* oc) {
                                 !c.wav || !c.peak_bits)) ||
       (c.kind == VF_OP_FINALIZE && (c.L <= 0 || c.n <= 0 || !c.in_wav || !c.peak_bits || !c.out)) ||
       (c.kind == VF_OP_ISTFT && (c.T <= 0 || c.n <= 1024 || !c.mag || !c.in_wav || !c.frames || !c.out)) ||
-      (c.kind == VF_OP_PEAK_NORM && (!c.clip_off || c.n <= 0 || !c.wav || !c.peak_bits));
+      (c.kind == VF_OP_PEAK_NORM && (!c.clip_off || c.n <= 0 || !c.wav || !c.peak_bits)) ||
+      (c.kind == VF_OP_FRONTEND && (c.n <= 0 || !c.in_wav || (c.clip_off && c.T <= 0) || !c.cos_out != !c.sin_out || (c.cos_out && !c.sp_out)));
   if (bad_kind || c.batch <= 0 || bad_shape || (c.clip_off && (c.batch > VL_MAX_CLIPS || c.clip_off[0] != 0)))
     return fail(ctx, VF_EINVAL, "vf_selftest_op: bad case");
   CK(cudaSetDevice(ctx->device));

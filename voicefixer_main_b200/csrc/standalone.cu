@@ -146,7 +146,8 @@ void stoi_bands(int* lo, int* hi) {
 extern "C" {
 
 VF_API int vf_istft(vf_ctx* ctx, const float* real, const float* imag, int batch, int frames, int64_t length, float* wav_out, void* stream) {
-  const int rc = begin_call(ctx, "vf_istft", real && imag && wav_out && batch > 0 && frames > 0 && length > 0);
+  const int rc = begin_call(ctx, "vf_istft", real && imag && wav_out && batch > 0 && batch <= 65535 && frames > 0 && length > 0,
+                            " (batch must be 1 .. 65535)");
   if (rc) return rc;
   if (length + 1024 > (int64_t)(frames - 1) * ctx->cfg.hop + 2048)
     return fail(ctx, VF_EINVAL, "vf_istft: %d frames cover %ld samples, fewer than length %ld + n_fft/2", frames, (long)(frames - 1) * ctx->cfg.hop + 2048, (long)length);
