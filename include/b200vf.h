@@ -31,7 +31,8 @@
  *   vf_resample_poly              load_wav's rate conversion, tools/utils.py:46-48
  *   vf_lsd / vf_sispec            AudioMetrics.lsd / .sispec evaluation_proc/metrics.py:83-95 (handler's mel metrics,
  *                                 eval_gsr_voicefixer.py:56-64)
- *   vf_metric_spectrogram         AudioMetrics.wav_to_spectrogram metrics.py:37-51 (librosa STFT magnitude + mel) at 44.1 kHz
+ *   vf_metric_spectrogram         AudioMetrics.wav_to_spectrogram metrics.py:37-51 (librosa STFT magnitude + mel) at 44.1 kHz;
+ *                                 the _ex forms of it and the two calls below take the rate (44.1 or 16 kHz)
  *   vf_ssim                       AudioMetrics.ssim metrics.py:97-106 (scikit-image structural_similarity, win_size 7)
  *   vf_score_varlen               the spectral part of AudioMetrics.evaluation metrics.py:53-81 for a set of file pairs
  *   vf_score_time_varlen          its sisdr and stoi keys (speechmetrics, metrics.py:58-64) for a set of file pairs
@@ -119,7 +120,9 @@ VF_API const char* vf_last_error(vf_ctx* ctx);   /* ctx may be NULL: error of th
  * "generator.analysis_module.*" (VoiceFixer's mel UNet; unet.py and unet_small.py share its keys), "vocoder.*",
  * "generator.unet.*" (unet_v2 of SSR_UNet / GSR_UNet) - whichever are present are loaded, and a network that is
  * present must be complete (missing key -> VF_ESTATE).  Entry points that need an absent network fail with VF_ESTATE; "mel.fb"
- * alone is enough for the front end and for scoring (vf_metric_spectrogram, vf_score_varlen). */
+ * alone is enough for the front end and for scoring (vf_metric_spectrogram, vf_score_varlen).  The optional
+ * "metrics.mel_16k.fb" [372, 80] (MelScale(n_mels=80, sample_rate=16000, n_stft=372)) enables 16 kHz scoring (the _ex
+ * scoring calls with rate 16000). */
 VF_API int vf_load_weights(vf_ctx* ctx, const vf_tensor_desc* descs, int n);
 
 /* wav [B,N] -> mel_out [B,T,128] linear mel (T = 1 + N/hop); optional sp/cos/sin [B,T,1025] (NULL to skip).
@@ -277,6 +280,25 @@ VF_API int vf_score_varlen(vf_ctx* ctx, const float* est, const int64_t* est_off
  * longer pair runs alone); eight launches per sub-batch.  Needs no weights.  PESQ is not computed. */
 VF_API int vf_score_time_varlen(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target,
                                 const int64_t* target_offsets, int batch, double* out, void* stream);
+
+/* The three scoring calls above at the rate of a test set: `rate` 44100 is exactly the call without _ex; 16000 is
+ * AudioMetrics' 16 kHz branch (metrics.py:43-46); any other rate is VF_EINVAL.  At 16 kHz:
+ * - the spectrogram is np.abs(librosa.stft(wav, n_fft=743, hop_length=160)): reflect padding by 371, the float64 periodic
+ *   hann of length 743, a direct float64 DFT of the prime length 743 (372 bins) rounded to complex64, |.| of that.  Clip i
+ *   has T_i = 1 + (n_i - 1) / 160 frames and needs at least 372 samples (one reflection of the padding).  The mel is
+ *   MelScale(n_mels=80, sample_rate=16000, n_stft=372), [sum T_i, 80]; it needs "metrics.mel_16k.fb" [372, 80] loaded
+ *   (VF_ESTATE otherwise).
+ * - vf_score_varlen_ex computes the same eight keys on the [T, 372] spectrogram and its [T, 80] mel; every pair needs equal
+ *   frame counts and at least 7 frames (961 samples).
+ * - vf_score_time_varlen_ex runs stoi(target, est, 16000): resample_oct(x, 10000, 16000) is resample_poly by 5 / 8 with
+ *   Octave's 581-tap window (ceil(5 n / 8) samples); the rest is unchanged.  Sub-batches hold at most 16384 * 160 padded
+ *   samples, the same 10 kHz scratch as at 44.1 kHz. */
+VF_API int vf_metric_spectrogram_ex(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* sp_out,
+                                    float* mel_out, int rate, void* stream);
+VF_API int vf_score_varlen_ex(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target,
+                              const int64_t* target_offsets, int batch, double* out, int rate, void* stream);
+VF_API int vf_score_time_varlen_ex(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target,
+                                   const int64_t* target_offsets, int batch, double* out, int rate, void* stream);
 
 /* scipy.signal.sosfiltfilt(sos, x) (padtype "odd", default padlen) of `batch` packed FLOAT64 rows, each with its own filter:
  * x and out are device float64, packed with HOST offsets [batch + 1]; row i uses filter row_filter[i] (host) of

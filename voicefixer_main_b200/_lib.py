@@ -22,7 +22,8 @@ EXPORTS = [
     "vf_mel", "vf_finalize", "vf_plan_cache_info", "vf_resample_poly", "vf_lsd", "vf_sispec", "vf_to_pcm16_ex", "vf_amp_to_original_f",
     "vf_restore_varlen", "vf_ssr_restore_varlen", "vf_restore_varlen_mels", "vf_metric_spectrogram", "vf_ssim", "vf_score_varlen",
     "vf_ssr_restore_varlen_mels", "vf_selftest_op", "vf_selftest_gru", "vf_score_time_varlen",
-    "vf_sosfiltfilt_varlen", "vf_resample_poly_f64_varlen",
+    "vf_sosfiltfilt_varlen", "vf_resample_poly_f64_varlen", "vf_metric_spectrogram_ex", "vf_score_varlen_ex",
+    "vf_score_time_varlen_ex",
 ]
 VF_RESTORE_UNIFY_ENERGY = 1
 VF_SSR_PEAK_NORMALISE = 1
@@ -159,6 +160,9 @@ def load_library():
     lib.vf_ssim.argtypes = [P, P, P, c_int, c_int, c_int, P, P]
     lib.vf_score_varlen.argtypes = [P, P, POINTER(c_int64), P, POINTER(c_int64), c_int, P, P]
     lib.vf_score_time_varlen.argtypes = [P, P, POINTER(c_int64), P, POINTER(c_int64), c_int, P, P]
+    lib.vf_metric_spectrogram_ex.argtypes = [P, P, POINTER(c_int64), c_int, P, P, c_int, P]
+    lib.vf_score_varlen_ex.argtypes = [P, P, POINTER(c_int64), P, POINTER(c_int64), c_int, P, c_int, P]
+    lib.vf_score_time_varlen_ex.argtypes = [P, P, POINTER(c_int64), P, POINTER(c_int64), c_int, P, c_int, P]
     lib.vf_sosfiltfilt_varlen.argtypes = [P, P, POINTER(c_int64), c_int, POINTER(c_double), POINTER(c_double), POINTER(c_int),
                                           c_int, POINTER(c_int), POINTER(c_int), P, P]
     lib.vf_resample_poly_f64_varlen.argtypes = [P, P, POINTER(c_int64), c_int, P, POINTER(c_int64), POINTER(c_int),

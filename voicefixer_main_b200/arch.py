@@ -162,6 +162,16 @@ def frames_for(n_samples: int, hop: int = 441) -> int:
     return 1 + n_samples // hop
 
 
+def metric_frames(n_samples: int, rate: int = 44100) -> int:
+    """Frames of AudioMetrics.wav_to_spectrogram at `rate` (librosa's center=True count 1 + (n + 2 (n_fft // 2) - n_fft) //
+    hop): frames_for(n) at 44.1 kHz (n_fft 2048, hop 441); 1 + (n - 1) // 160 at 16 kHz, where n_fft 743 is odd."""
+    if rate == 16000:
+        return 1 + (n_samples - 1) // 160
+    if rate == 44100:
+        return frames_for(n_samples)
+    raise ValueError(f"Bad Samplerate: {rate} Hz")
+
+
 def padded_frames(t: int) -> int:
     """unet.py:75-77: time axis zero-padded up to a multiple of 64."""
     return ((t + DOWNSAMPLE - 1) // DOWNSAMPLE) * DOWNSAMPLE

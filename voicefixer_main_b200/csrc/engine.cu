@@ -664,7 +664,8 @@ VF_API void vf_destroy(vf_ctx* ctx) {
     if (s->p) cudaFree(s->p);
     if (s->order.ev) cudaEventDestroy(s->order.ev);
   }
-  if (ctx->d_stoi_tables) cudaFree(ctx->d_stoi_tables);
+  for (double* t : ctx->d_stoi_tables)
+    if (t) cudaFree(t);
   delete ctx;
 }
 

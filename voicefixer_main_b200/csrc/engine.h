@@ -189,6 +189,12 @@ struct Scratch {
   StreamOrder order;
 };
 
+// A mel filterbank in its sparse form: filter m = val[ofs[m] .. ofs[m] + len[m]) on bins f0[m] .. (val null: not loaded)
+struct SparseFb {
+  int *f0 = nullptr, *len = nullptr, *ofs = nullptr;
+  float* val = nullptr;
+};
+
 }  // namespace vf
 
 using namespace vf;
@@ -216,11 +222,16 @@ struct vf_ctx {
   double* d_window64 = nullptr;    // metric STFT (vf_metric_spectrogram, vf_score_varlen): float64 window and twiddles
   double2* d_tw1024d = nullptr;
   double2* d_tw2048d = nullptr;
+  double* d_window743 = nullptr;   // its 16 kHz geometry: float64 window [743] and twiddles e^{-2 pi i j / 743}
+  double2* d_tw743 = nullptr;
+  SparseFb fb16k;                  // AudioMetrics' mel_16k [372, 80] (optional key "metrics.mel_16k.fb")
   // scratch of the packed-set calls of standalone.cu: vf_score_varlen (two spectrograms, two mels, SSIM tile sums),
   // vf_score_time_varlen (resampled signals, frame and band values, tile sums, kept-frame indices) and
   // vf_sosfiltfilt_varlen (the call's filter tables, then the scan's extended rows and chunk states)
   Scratch score, time_score, iir;
-  double* d_stoi_tables = nullptr;   // vf_score_time_varlen's float64 tables (resampling taps, window, twiddles; first use)
+  // vf_score_time_varlen's float64 tables (resampling taps, window, twiddles), one per rate (44.1, 16 kHz; first use)
+  double* d_stoi_tables[2] = {nullptr, nullptr};
+  int stoi_half[2] = {0, 0};         // their resampling filters' half lengths
   // UNet weights: the mel-domain analysis module of VoiceFixer (prefix generator.analysis_module.) and the
   // linear-spectrogram unet_v2 of SSR_UNet / GSR_UNet (prefix generator.unet.); either may be absent
   UnetW gsr, ssr;

@@ -106,40 +106,43 @@ cudaError_t launch_istft_ola(const IstftOlaParams& p, cudaStream_t stream) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// MelScale.forward: one CTA = 8 time steps of one outer index; the [1025 x 8] spectrogram tile is staged in shared
-// memory (whole 32-byte sectors along whichever axis is contiguous), then 128 mels x 8 steps from the sparse filterbank.
+// MelScale.forward: one CTA = 8 time steps of one outer index; the [NF x 8] spectrogram tile is staged in shared
+// memory (whole 32-byte sectors along whichever axis is contiguous), then NM mels x 8 steps from the sparse filterbank.
 constexpr int MEL_TT = 8;
+template <int NF, int NM>
 __global__ void __launch_bounds__(256) mel_kernel(MelParams p) {
-  __shared__ float tile[1025][MEL_TT + 1];
+  __shared__ float tile[NF][MEL_TT + 1];
   const long o = blockIdx.y;
   const long t0 = (long)blockIdx.x * MEL_TT;
   const int nt = (int)min((long)MEL_TT, p.T - t0);
   const float* base = p.in + o * p.so + t0 * p.st;
   if (p.st == 1) {           // [..., freq, time] contiguous: time fastest
-    for (int idx = threadIdx.x; idx < 1025 * MEL_TT; idx += 256) {
+    for (int idx = threadIdx.x; idx < NF * MEL_TT; idx += 256) {
       const int f = idx / MEL_TT, tt = idx % MEL_TT;
       tile[f][tt] = tt < nt ? __ldg(base + (long)f * p.sf + tt) : 0.f;
     }
   } else {                   // e.g. the permuted view of a [.., time, freq] tensor: frequency fastest
-    for (int idx = threadIdx.x; idx < 1025 * MEL_TT; idx += 256) {
-      const int tt = idx / 1025, f = idx % 1025;
+    for (int idx = threadIdx.x; idx < NF * MEL_TT; idx += 256) {
+      const int tt = idx / NF, f = idx % NF;
       tile[f][tt] = tt < nt ? __ldg(base + (long)f * p.sf + (long)tt * p.st) : 0.f;
     }
   }
   __syncthreads();
-  for (int idx = threadIdx.x; idx < 128 * MEL_TT; idx += 256) {
-    const int tt = idx >> 7, m = idx & 127;
+  for (int idx = threadIdx.x; idx < NM * MEL_TT; idx += 256) {
+    const int tt = idx / NM, m = idx % NM;
     if (tt >= nt) continue;
     const int f0 = __ldg(p.fb_f0 + m), len = __ldg(p.fb_len + m);
     const float* w = p.fb_val + __ldg(p.fb_ofs + m);
     float acc = 0.f;
     for (int j = 0; j < len; ++j) acc = fmaf(tile[f0 + j][tt], __ldg(w + j), acc);
-    p.out[(o * p.T + t0 + tt) * 128 + m] = acc;
+    p.out[(o * p.T + t0 + tt) * NM + m] = acc;
   }
 }
-cudaError_t launch_mel(const MelParams& p, cudaStream_t stream) {
+cudaError_t launch_mel(const MelParams& p, cudaStream_t stream, int n_freq, int n_mels) {
   dim3 grid((unsigned)((p.T + MEL_TT - 1) / MEL_TT), (unsigned)p.n_outer);
-  mel_kernel<<<grid, 256, 0, stream>>>(p);
+  if (n_freq == 1025 && n_mels == 128) mel_kernel<1025, 128><<<grid, 256, 0, stream>>>(p);
+  else if (n_freq == 372 && n_mels == 80) mel_kernel<372, 80><<<grid, 256, 0, stream>>>(p);
+  else return cudaErrorInvalidValue;
   return cudaGetLastError();
 }
 

@@ -201,18 +201,20 @@ cudaError_t launch_peak_normalise_varlen(float* wav, const int64_t* vl_off, int 
                                          cudaStream_t stream);
 
 // MelScale.forward (tools/pytorch/mel_scale.py:52-64) as a stand-alone op on any [..., freq, time] view:
-// out[o, t, m] = sum_f in[o * so + f * sf + t * st] * fb[f, m] with the filterbank in its sparse form.
+// out[o, t, m] = sum_f in[o * so + f * sf + t * st] * fb[f, m] with the filterbank in its sparse form.  Two geometries:
+// n_freq x n_mels = 1025 x 128 (44.1 kHz, the model's) and 372 x 80 (AudioMetrics' mel_16k); any other is
+// cudaErrorInvalidValue.
 struct MelParams {
   const float* in;
   long n_outer, T;
   long so, sf, st;       // input strides (elements) of the outer, frequency and time axes
-  float* out;            // [n_outer, T, 128] contiguous
+  float* out;            // [n_outer, T, n_mels] contiguous
   const int* fb_f0;
   const int* fb_len;
   const int* fb_ofs;
   const float* fb_val;
 };
-cudaError_t launch_mel(const MelParams& p, cudaStream_t stream);
+cudaError_t launch_mel(const MelParams& p, cudaStream_t stream, int n_freq = 1025, int n_mels = 128);
 
 // ISTFT (FDomainHelper.istft, fDomainHelper.py:30-32,127 -> torchlibrosa ISTFT: n_fft = win = 2048, hop 441, periodic
 // hann, center): stage 1 writes the windowed inverse-DFT frames, stage 2 overlap-adds them in a fixed order and divides
@@ -267,19 +269,24 @@ struct ImageSet {
 cudaError_t launch_lsd_varlen(const float* est, const float* tgt, int F, const ImageSet& s, double* out, int out_stride, cudaStream_t stream);
 cudaError_t launch_sispec_varlen(const float* est, const float* tgt, int F, const ImageSet& s, double* out, int out_stride, cudaStream_t stream);
 
-// metrics.cu: |librosa.stft(wav, n_fft=2048, hop_length=441)| (librosa 0.8: reflect padding, periodic hann, float64 FFT
-// stored as complex64) of up to two packed sources at once (blockIdx.y = source), one CTA per frame.
+// metrics.cu: |librosa.stft(wav, n_fft, hop_length)| (librosa 0.8: reflect padding by n_fft / 2, periodic hann, float64
+// DFT stored as complex64) of up to two packed sources at once (blockIdx.y = source), one CTA per frame.  Two geometries:
+// launch_metric_stft is n_fft 2048, hop 441 (44.1 kHz: radix FFT), launch_metric_dft743 is n_fft 743, hop 160 (16 kHz:
+// 743 is prime, a direct DFT).
 struct MetricStftParams {
   const float* wav[2];                       // packed samples; clip b of source z = wav[z][off[z][b] .. off[z][b + 1])
-  float* sp[2];                              // [sum T_b, 1025]: clip b's frames at rows frame_off[b] ..
-  const double* window;                      // [2048] periodic hann, float64
+  float* sp[2];                              // [sum T_b, 1 + n_fft / 2]: clip b's frames at rows frame_off[b] ..
+  const double* window;                      // [n_fft] periodic hann, float64
   const double2* tw1024;                     // e^{-2 pi i j / 1024}, float64
   const double2* tw2048;                     // e^{-2 pi i k / 2048}, k = 0..1024
+  const double2* tw743;                      // e^{-2 pi i j / 743}, j = 0..742 (metric_dft743_kernel)
   int batch, sources;
   int64_t off[2][SCORE_MAX_IMAGES + 1];
-  int64_t frame_off[SCORE_MAX_IMAGES + 1];   // T_b = 1 + n_b / 441 (the sources have equal frame counts)
+  // T_b = 1 + (n_b - n_fft % 2) / hop: 1 + n_b / 441, or 1 + (n_b - 1) / 160 (the sources have equal frame counts)
+  int64_t frame_off[SCORE_MAX_IMAGES + 1];
 };
 cudaError_t launch_metric_stft(const MetricStftParams& p, cudaStream_t stream);
+cudaError_t launch_metric_dft743(const MetricStftParams& p, cudaStream_t stream);
 
 // skimage.metrics.structural_similarity(x, y, win_size=7) of scikit-image <= 0.18 on float32 images (data_range 2, 7x7
 // uniform filter, sample covariance, mean over the image cropped by 3), in float64.  Stage 1: one CTA per tile of
@@ -301,18 +308,18 @@ inline int ssim_tiles(long T, int F) {
 cudaError_t launch_ssim(const SsimParams& p, double* out, int out_stride, cudaStream_t stream);
 
 // speech_metrics.cu: the time-domain keys of AudioMetrics.evaluation (metrics.py:58-64), speechmetrics' sisdr and stoi
-// (pystoi 0.3.3, extended=False) for pairs of packed 44.1 kHz clips, all in float64.  A pair is zero-padded at the end to
-// its longer clip (N_b samples) by index math.  STOI's pipeline runs at 10 kHz: resample (100/441, Octave's 31947-tap
-// window), the target's frame energies, the silent-frame mask and its kept-frame scan, the overlap-add of the kept frames
-// into a compacted buffer, a 512-point STFT with the 15 one-third-octave band values per frame, and the 30-frame segment
-// correlations, summed per tile and then per pair in a fixed order.  The silence removal makes the frame count of a pair
-// a device value (kept[b] - 1 STFT frames); the buffers and grids are sized by its host-known upper bound, and slots past
-// it are skipped.  Every value depends on its own pair only, so a pair's bits do not depend on its batch.
-constexpr int STOI_UP = 100, STOI_DOWN = 441;   // 44.1 kHz -> 10 kHz
-constexpr int STOI_HALF = 15973;               // half length of the resampling filter (2 * 15973 + 1 taps)
+// (pystoi 0.3.3, extended=False) for pairs of packed 44.1 kHz or 16 kHz clips, all in float64.  A pair is zero-padded at
+// the end to its longer clip (N_b samples) by index math.  STOI's pipeline runs at 10 kHz: resample (up / down = 100 / 441
+// with Octave's 31947-tap window, or 5 / 8 with its 581-tap window), the target's frame energies, the silent-frame mask and
+// its kept-frame scan, the overlap-add of the kept frames into a compacted buffer, a 512-point STFT with the 15
+// one-third-octave band values per frame, and the 30-frame segment correlations, summed per tile and then per pair in a
+// fixed order.  The silence removal makes the frame count of a pair a device value (kept[b] - 1 STFT frames); the buffers
+// and grids are sized by its host-known upper bound, and slots past it are skipped.  Every value depends on its own pair
+// only, so a pair's bits do not depend on its batch.
 constexpr int STOI_FRAME = 256, STOI_HOP = 128, STOI_BANDS = 15, STOI_SEG = 30;
-// 10 kHz samples of a pair of padded length n, and its frames before silence removal (starts range(0, n10 - 256, 128))
-inline int64_t stoi_len10(int64_t n) { return (n * STOI_UP + STOI_DOWN - 1) / STOI_DOWN; }
+// 10 kHz samples of a pair of padded length n resampled by up / down, and its frames before silence removal (starts
+// range(0, n10 - 256, 128))
+inline int64_t stoi_len10(int64_t n, int up, int down) { return (n * up + down - 1) / down; }
 inline int64_t stoi_frames(int64_t n10) { return n10 > STOI_FRAME ? (n10 - STOI_FRAME + STOI_HOP - 1) / STOI_HOP : 0; }
 // correlation tiles of 256 (segment, band) items for at most nF - 1 STFT frames (nF - 30 segments)
 inline int64_t stoi_tiles(int64_t nF) { return nF > STOI_SEG ? ((nF - STOI_SEG) * STOI_BANDS + 255) / 256 : 0; }
@@ -321,12 +328,13 @@ struct TimeScoreParams {
   const float* tgt;
   int batch;
   int64_t e_off[SCORE_MAX_IMAGES + 1], t_off[SCORE_MAX_IMAGES + 1];
-  int64_t r_off[SCORE_MAX_IMAGES + 1];       // 10 kHz samples: stoi_len10(N_b)
+  int64_t r_off[SCORE_MAX_IMAGES + 1];       // 10 kHz samples: stoi_len10(N_b, up, down)
   int64_t f_off[SCORE_MAX_IMAGES + 1];       // frame slots: stoi_frames
   int64_t tile_off[SCORE_MAX_IMAGES + 1];    // correlation tiles: stoi_tiles
   int band_lo[STOI_BANDS], band_hi[STOI_BANDS];   // band k = rfft bins [band_lo[k], band_hi[k])
   double clip;                               // 1 + 10^(15 / 20)
-  const double* taps;                        // [2 * STOI_HALF + 1] Octave's window / its sum * 100
+  int up, down, half;                        // the resampling ratio to 10 kHz and its filter's half length
+  const double* taps;                        // [2 * half + 1] Octave's window / its sum * up
   const double* window;                      // [256] np.hanning(258)[1:-1]
   const double2* tw256;                      // e^{-2 pi i j / 256}
   const double2* tw512;                      // e^{-2 pi i k / 512}, k = 0..256

@@ -2,6 +2,7 @@
 //   * metric STFT: np.abs(librosa.stft(wav, hop_length=441, n_fft=2048)) as librosa 0.8 computes it - reflect padding by
 //     n_fft / 2 (index math on the un-padded clip), float64 periodic hann x float32 samples, float64 FFT (the fp64 Stockham
 //     FFT of fft.cuh), the spectrum stored as complex64 and |.| of that.  No power clamp: digital silence gives exact zeros.
+//     At 16 kHz (hop_length=160, n_fft=743) the same with a direct float64 DFT of the prime length 743.
 //   * SSIM: scikit-image 0.18's structural_similarity(x, y, win_size=7) in float64, deterministic.
 // Both are HBM / launch bound; one launch covers a whole set of clips or images of different lengths.
 #include "fft.cuh"
@@ -46,6 +47,69 @@ __global__ void __launch_bounds__(256) metric_stft_kernel(MetricStftParams p) {
 }
 cudaError_t launch_metric_stft(const MetricStftParams& p, cudaStream_t stream) {
   metric_stft_kernel<<<dim3((unsigned)p.frame_off[p.batch], p.sources), 256, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+// The 16 kHz geometry (n_fft 743, hop 160, 372 bins).  743 is prime, so each bin is a direct float64 sum over the frame,
+// n ascending: X[k] = sum_n w[n] x[n] e^{-2 pi i k n / 743}, with the twiddle index j = k n mod 743 advanced by k per term
+// (exact integer arithmetic) into a table staged in shared memory.  One CTA per DFT743_FRAMES consecutive frames of the set
+// (each frame finds its clip by bisection, as above) and source, one thread per bin: each twiddle read serves all its
+// frames.  A frame's sums do not depend on the frames it is grouped with.
+constexpr int DFT743_N = 743, DFT743_BINS = 372, DFT743_THREADS = 384, DFT743_FRAMES = 4;
+__global__ void __launch_bounds__(DFT743_THREADS) metric_dft743_kernel(MetricStftParams p) {
+  __shared__ double xs[DFT743_FRAMES][DFT743_N];
+  __shared__ double2 tw[DFT743_N];
+  const int tid = threadIdx.x, z = blockIdx.y;
+  const int64_t total = p.frame_off[p.batch], g0 = (int64_t)blockIdx.x * DFT743_FRAMES;
+  for (int i = tid; i < DFT743_N; i += DFT743_THREADS) tw[i] = p.tw743[i];
+  for (int f = 0; f < DFT743_FRAMES; ++f) {
+    const int64_t g = g0 + f;
+    if (g >= total) {                                           // past the set: zeros, not stored
+      for (int i = tid; i < DFT743_N; i += DFT743_THREADS) xs[f][i] = 0.0;
+      continue;
+    }
+    int lo = 0, hi = p.batch;
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (p.frame_off[mid] <= g) lo = mid; else hi = mid;
+    }
+    const long t = (long)(g - p.frame_off[lo]);
+    const float* x = p.wav[z] + p.off[z][lo];
+    const long n = (long)(p.off[z][lo + 1] - p.off[z][lo]);
+    for (int i = tid; i < DFT743_N; i += DFT743_THREADS) {    // the reflect-padded frame times the float64 window
+      long s = t * 160 + i - DFT743_N / 2;
+      if (s < 0) s = -s;
+      if (s >= n) s = 2L * (n - 1) - s;
+      xs[f][i] = (double)__ldg(x + s) * __ldg(p.window + i);
+    }
+  }
+  __syncthreads();
+  if (tid >= DFT743_BINS) return;
+  const int k = tid;
+  double re[DFT743_FRAMES], im[DFT743_FRAMES];
+#pragma unroll
+  for (int f = 0; f < DFT743_FRAMES; ++f) re[f] = im[f] = 0.0;
+  int j = 0;
+  for (int i = 0; i < DFT743_N; ++i) {
+    const double2 w = tw[j];
+#pragma unroll
+    for (int f = 0; f < DFT743_FRAMES; ++f) {
+      re[f] = fma(xs[f][i], w.x, re[f]);
+      im[f] = fma(xs[f][i], w.y, im[f]);
+    }
+    j += k;
+    if (j >= DFT743_N) j -= DFT743_N;
+  }
+#pragma unroll
+  for (int f = 0; f < DFT743_FRAMES; ++f) {
+    if (g0 + f >= total) break;
+    const float fr = (float)re[f], fi = (float)im[f];           // complex64 storage
+    p.sp[z][(size_t)(g0 + f) * DFT743_BINS + k] = (float)sqrt((double)fr * fr + (double)fi * fi);
+  }
+}
+cudaError_t launch_metric_dft743(const MetricStftParams& p, cudaStream_t stream) {
+  const unsigned blocks = (unsigned)((p.frame_off[p.batch] + DFT743_FRAMES - 1) / DFT743_FRAMES);
+  metric_dft743_kernel<<<dim3(blocks, p.sources), DFT743_THREADS, 0, stream>>>(p);
   return cudaGetLastError();
 }
 

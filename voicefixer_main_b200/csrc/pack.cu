@@ -68,6 +68,15 @@ int build_tables(vf_ctx* ctx) {
   if (rc) return rc;
   rc = upload(ctx, &ctx->d_tw2048d, d2);
   if (rc) return rc;
+  // the 16 kHz geometry: get_window('hann', 743, fftbins=True) (a symmetric 744-point window truncated), twiddles of 743
+  std::vector<double> win743(743);
+  for (int i = 0; i < 743; ++i) win743[i] = 0.5 + 0.5 * std::cos(i * (2.0 * PI / 743.0) + -PI);
+  std::vector<double2> d743(743);
+  for (int j = 0; j < 743; ++j) d743[j] = make_double2(std::cos(2 * PI * j / 743.0), -std::sin(2 * PI * j / 743.0));
+  rc = upload(ctx, &ctx->d_window743, win743);
+  if (rc) return rc;
+  rc = upload(ctx, &ctx->d_tw743, d743);
+  if (rc) return rc;
   std::vector<float> mw(128);
   for (int i = 0; i < 128; ++i) mw[i] = (float)(ctx->cfg.voc_mel_weight_a * std::exp(ctx->cfg.voc_mel_weight_b * i));
   return upload(ctx, &ctx->d_melw, mw);
@@ -394,32 +403,44 @@ int analysis_kind(vf_ctx* ctx, const std::string& A, int* kind) {
 const char* const GSR_PREFIX = "generator.analysis_module.";   // models/gsr_voicefixer.py:50,139
 const char* const SSR_PREFIX = "generator.unet.";              // models/ssr_unet.py:49, models/gsr_unet.py:49
 
+// A mel filterbank [n_freq, n_mels] -> its sparse rows (each triangular filter is one contiguous run of bins)
+int upload_fb(vf_ctx* ctx, const HostT& fb, const char* key, int n_freq, int n_mels, SparseFb* out) {
+  if (fb.shape.size() != 2 || fb.shape[0] != n_freq || fb.shape[1] != n_mels)
+    return fail(ctx, VF_EINVAL, "%s must be [%d,%d]", key, n_freq, n_mels);
+  std::vector<int> f0(n_mels), len(n_mels), ofs(n_mels);
+  std::vector<float> val;
+  for (int m = 0; m < n_mels; ++m) {
+    int lo = -1, hi = -1;
+    for (int f = 0; f < n_freq; ++f)
+      if (fb.v[(size_t)f * n_mels + m] != 0.f) { if (lo < 0) lo = f; hi = f; }
+    if (lo < 0) { lo = 0; hi = -1; }
+    f0[m] = lo; len[m] = hi - lo + 1; ofs[m] = (int)val.size();
+    for (int f = lo; f <= hi; ++f) val.push_back(fb.v[(size_t)f * n_mels + m]);
+  }
+  if (val.empty()) val.push_back(0.f);
+  int rc = upload(ctx, &out->f0, f0); if (rc) return rc;
+  rc = upload(ctx, &out->len, len); if (rc) return rc;
+  rc = upload(ctx, &out->ofs, ofs); if (rc) return rc;
+  return upload(ctx, &out->val, val);
+}
+
 }  // namespace
 
 // Loads whichever of the three networks the descriptors hold (a VoiceFixer checkpoint: analysis module + vocoder;
 // an SSR_UNet / GSR_UNet checkpoint: generator.unet.*).  A network that is present must be complete.  With none, only the
 // filterbank is loaded: enough for scoring (vf_score_varlen) and the front end; the network entry points fail with VF_ESTATE.
+// The optional "metrics.mel_16k.fb" [372, 80] adds the 16 kHz scoring geometry.
 int load_all(vf_ctx* ctx) {
-  // mel filterbank -> sparse rows (each triangular filter is one contiguous run of bins)
   {
     NEED(fb, "mel.fb");
-    if (fb->shape.size() != 2 || fb->shape[0] != 1025 || fb->shape[1] != 128)
-      return fail(ctx, VF_EINVAL, "mel.fb must be [1025,128]");
-    std::vector<int> f0(128), len(128), ofs(128);
-    std::vector<float> val;
-    for (int m = 0; m < 128; ++m) {
-      int lo = -1, hi = -1;
-      for (int f = 0; f < 1025; ++f)
-        if (fb->v[(size_t)f * 128 + m] != 0.f) { if (lo < 0) lo = f; hi = f; }
-      if (lo < 0) { lo = 0; hi = -1; }
-      f0[m] = lo; len[m] = hi - lo + 1; ofs[m] = (int)val.size();
-      for (int f = lo; f <= hi; ++f) val.push_back(fb->v[(size_t)f * 128 + m]);
-    }
-    if (val.empty()) val.push_back(0.f);
-    int rc = upload(ctx, &ctx->d_fb_f0, f0); if (rc) return rc;
-    rc = upload(ctx, &ctx->d_fb_len, len); if (rc) return rc;
-    rc = upload(ctx, &ctx->d_fb_ofs, ofs); if (rc) return rc;
-    rc = upload(ctx, &ctx->d_fb_val, val); if (rc) return rc;
+    SparseFb s;
+    int rc = upload_fb(ctx, *fb, "mel.fb", 1025, 128, &s);
+    if (rc) return rc;
+    ctx->d_fb_f0 = s.f0; ctx->d_fb_len = s.len; ctx->d_fb_ofs = s.ofs; ctx->d_fb_val = s.val;
+  }
+  if (const HostT* fb16 = find(ctx, "metrics.mel_16k.fb")) {
+    const int rc = upload_fb(ctx, *fb16, "metrics.mel_16k.fb", 372, 80, &ctx->fb16k);
+    if (rc) return rc;
   }
   int kind = ANALYSIS_NONE;
   int rc = analysis_kind(ctx, GSR_PREFIX, &kind);

@@ -1,5 +1,6 @@
 // The time-domain keys of AudioMetrics.evaluation (evaluation_proc/metrics.py:58-64): speechmetrics' sisdr and pystoi
-// 0.3.3's stoi(target, estimate, 44100, extended=False), restated in oracle/speech_metrics.py.  Everything is float64:
+// 0.3.3's stoi(target, estimate, 44100 or 16000, extended=False), restated in oracle/speech_metrics.py (44.1 kHz) and
+// tests/oracle_16k.py (16 kHz).  Everything is float64:
 // STOI's silent-frame mask is a threshold decision that fp32 rounding could flip.  See kernels.cuh for the pipeline.
 #include "fft.cuh"
 #include "kernels.cuh"
@@ -48,7 +49,7 @@ __global__ void __launch_bounds__(256) sisdr_kernel(TimeScoreParams p) {
   if (threadIdx.x == 0) p.out[2 * b] = 10.0 * log10((EPS + ss) / (EPS + nn));
 }
 
-// scipy.signal.resample_poly(x, 100, 441, window=taps / 100) of the padded clip: y[m] = sum_j x[j] taps[441 m - 100 j + L]
+// scipy.signal.resample_poly(x, up, down, window=taps / up) of the padded clip: y[m] = sum_j x[j] taps[down m - up j + L]
 // over the taps in range, j ascending.  One thread per output sample; blockIdx.y = 0 target, 1 estimate.
 __global__ void __launch_bounds__(256) stoi_resample_kernel(TimeScoreParams p) {
   const int z = blockIdx.y;
@@ -59,13 +60,13 @@ __global__ void __launch_bounds__(256) stoi_resample_kernel(TimeScoreParams p) {
   const int64_t* off = z ? p.e_off : p.t_off;
   const float* x = (z ? p.est : p.tgt) + off[b];
   const int64_t nx = off[b + 1] - off[b];
-  const int64_t c = m * STOI_DOWN + STOI_HALF;               // taps index of x[0]
-  int64_t j0 = c - 2 * STOI_HALF;                              // first j with c - 100 j <= 2L
-  j0 = j0 > 0 ? (j0 + STOI_UP - 1) / STOI_UP : 0;
-  int64_t j1 = c / STOI_UP;                                     // last j with c - 100 j >= 0
+  const int64_t c = m * p.down + p.half;                      // taps index of x[0]
+  int64_t j0 = c - 2 * p.half;                                 // first j with c - up j <= 2L
+  j0 = j0 > 0 ? (j0 + p.up - 1) / p.up : 0;
+  int64_t j1 = c / p.up;                                        // last j with c - up j >= 0
   if (j1 > nx - 1) j1 = nx - 1;
   double acc = 0;
-  for (int64_t j = j0; j <= j1; ++j) acc += (double)__ldg(x + j) * __ldg(p.taps + (c - STOI_UP * j));
+  for (int64_t j = j0; j <= j1; ++j) acc += (double)__ldg(x + j) * __ldg(p.taps + (c - p.up * j));
   p.rs[(size_t)z * p.r_off[p.batch] + g] = acc;
 }
 

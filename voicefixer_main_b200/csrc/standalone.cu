@@ -82,45 +82,92 @@ int check_offsets(vf_ctx* ctx, const char* fn, const char* side, const char* ite
 
 constexpr long SCORE_CAP_FRAMES = 16384;   // vf_score_varlen sub-batch cap (frames per side), see b200vf.h
 
-long stft_frames(int64_t n) { return 1 + (long)(n / 441); }
+// The per-rate geometry of the scoring calls: AudioMetrics.wav_to_spectrogram's branch (metrics.py:38-47) and pystoi's
+// resampling ratio to 10 kHz, chosen once per call from its rate.
+struct Geometry {
+  int rate, n_fft, hop, bins, mels;
+  SparseFb fb;                                                   // the mel filterbank [bins, mels]
+  const double* window;                                          // the STFT's float64 window [n_fft]
+  cudaError_t (*stft)(const MetricStftParams&, cudaStream_t);
+  int stoi_up, stoi_down;                                        // rate -> 10 kHz, reduced by their gcd
+  int slot;                                                      // index of the rate's STOI tables
+  // librosa's center=True frame count 1 + (n + 2 (n_fft / 2) - n_fft) / hop: 1 + n / 441, or 1 + (n - 1) / 160
+  long frames(int64_t n) const { return 1 + (long)((n - n_fft % 2) / hop); }
+  int64_t min_samples() const { return n_fft / 2 + 1; }          // one reflection of the n_fft / 2 padding
+  int64_t len10(int64_t n) const { return stoi_len10(n, stoi_up, stoi_down); }
+};
 
-// d_stoi_tables layout (doubles): taps, window, tw256 (double2), tw512 (double2)
-constexpr size_t STOI_TAPS = 2 * STOI_HALF + 1, STOI_WIN_AT = STOI_TAPS + 1, STOI_TW256_AT = STOI_WIN_AT + 256,
-                 STOI_TW512_AT = STOI_TW256_AT + 2 * 256, STOI_TABLES = STOI_TW512_AT + 2 * 257;
+int geometry(vf_ctx* ctx, const char* fn, int rate, Geometry* g) {
+  if (rate == 44100) {
+    *g = {44100, 2048, 441, 1025, 128, {ctx->d_fb_f0, ctx->d_fb_len, ctx->d_fb_ofs, ctx->d_fb_val}, ctx->d_window64,
+          launch_metric_stft, 100, 441, 0};
+    return VF_OK;
+  }
+  if (rate == 16000) {
+    *g = {16000, 743, 160, 372, 80, ctx->fb16k, ctx->d_window743, launch_metric_dft743, 5, 8, 1};
+    return VF_OK;
+  }
+  return fail(ctx, VF_EINVAL, "%s: rate %d Hz (need 44100 or 16000)", fn, rate);
+}
 
-// The float64 tables of vf_score_time_varlen, designed once per context on the host:
-// * pystoi's resample_oct(x, 10000, 44100) window, Octave's resample filter for p / q = 100 / 441: L = ceil((60 - 8) /
-//   (28.714 * roll_off)) with cut-off 1 / 882 and roll_off = cut-off / 10, h = kaiser(2L + 1, 0.1102 * (60 - 8.7)) x
-//   2 * 100 * (1 / 882) * sinc(2 * (1 / 882) * t), t = -L..L; scipy's resample_poly uses window = h / sum(h), times up = 100.
+int need_fb(vf_ctx* ctx, const Geometry& g) {
+  if (g.fb.val) return VF_OK;
+  if (g.rate == 44100) return fail(ctx, VF_ESTATE, "mel filterbank not loaded (call vf_load_weights first)");
+  return fail(ctx, VF_ESTATE, "16 kHz mel filterbank not loaded (pass \"metrics.mel_16k.fb\" [372, 80] to vf_load_weights)");
+}
+
+void set_tables(vf_ctx* ctx, const Geometry& g, MetricStftParams& p) {
+  p.window = g.window; p.tw1024 = ctx->d_tw1024d; p.tw2048 = ctx->d_tw2048d; p.tw743 = ctx->d_tw743;
+}
+void set_fb(const Geometry& g, MelParams& m) {
+  m.fb_f0 = g.fb.f0; m.fb_len = g.fb.len; m.fb_ofs = g.fb.ofs; m.fb_val = g.fb.val;
+}
+
+// d_stoi_tables layout (doubles): taps (2 half + 1, an odd count), window, tw256 (double2), tw512 (double2)
+constexpr size_t stoi_win_at(int half) { return 2 * (size_t)half + 2; }
+constexpr size_t stoi_tw256_at(int half) { return stoi_win_at(half) + 256; }
+constexpr size_t stoi_tw512_at(int half) { return stoi_tw256_at(half) + 2 * 256; }
+constexpr size_t stoi_table_doubles(int half) { return stoi_tw512_at(half) + 2 * 257; }
+
+// The float64 tables of vf_score_time_varlen for the rate of `g`, designed once per context on the host:
+// * pystoi's resample_oct(x, 10000, rate) window, Octave's resample filter for p / q = up / down (100 / 441 or 5 / 8):
+//   L = ceil((60 - 8) / (28.714 * roll_off)) with cut-off 1 / (2 max(p, q)) and roll_off = cut-off / 10 (L = 15973 or 290),
+//   h = kaiser(2L + 1, 0.1102 * (60 - 8.7)) x 2 p cut-off sinc(2 cut-off t), t = -L..L; scipy's resample_poly uses
+//   window = h / sum(h), times up.
 // * np.hanning(258)[1:-1] (0.5 + 0.5 cos(pi n / 257), n = -255, -253, ..., 255) and the 256 / 512-point twiddles.
-int stoi_tables(vf_ctx* ctx) {
-  if (ctx->d_stoi_tables) return VF_OK;
+int stoi_tables(vf_ctx* ctx, const Geometry& g) {
+  if (ctx->d_stoi_tables[g.slot]) return VF_OK;
   const double PI = 3.14159265358979323846;
-  std::vector<double> t(STOI_TABLES, 0.0);
-  const double fc = 1.0 / (2 * 441.0), roll_off = fc / 10, rejection_db = 60.0;
+  const double fc = 1.0 / (2.0 * std::max(g.stoi_up, g.stoi_down)), roll_off = fc / 10, rejection_db = 60.0;
   const long L = (long)std::ceil((rejection_db - 8) / (28.714 * roll_off));
-  if (L != STOI_HALF) return fail(ctx, VF_EASSERT, "stoi filter half length %ld != %d", L, STOI_HALF);
+  std::vector<double> t(stoi_table_doubles((int)L), 0.0);
   const double beta = 0.1102 * (rejection_db - 8.7), alpha = (double)L, i0_beta = std::cyl_bessel_i(0.0, beta);
   double sum = 0;
   for (long i = 0; i <= 2 * L; ++i) {
     const double r = (i - alpha) / alpha;
     const double kaiser = std::cyl_bessel_i(0.0, beta * std::sqrt(1 - r * r)) / i0_beta;
     const double x = 2 * fc * (double)(i - L), y = PI * (x == 0 ? 1e-20 : x);     // np.sinc
-    t[i] = kaiser * (2 * 100.0 * fc * (std::sin(y) / y));
+    t[i] = kaiser * (2 * (double)g.stoi_up * fc * (std::sin(y) / y));
     sum += t[i];
   }
-  for (size_t i = 0; i < STOI_TAPS; ++i) t[i] = t[i] / sum * STOI_UP;
-  for (int i = 0; i < 256; ++i) t[STOI_WIN_AT + i] = 0.5 + 0.5 * std::cos(PI * (2 * i - 255) / 257.0);
+  for (long i = 0; i <= 2 * L; ++i) t[i] = t[i] / sum * g.stoi_up;
+  const size_t win = stoi_win_at((int)L), tw256 = stoi_tw256_at((int)L), tw512 = stoi_tw512_at((int)L);
+  for (int i = 0; i < 256; ++i) t[win + i] = 0.5 + 0.5 * std::cos(PI * (2 * i - 255) / 257.0);
   for (int j = 0; j < 256; ++j) {
-    t[STOI_TW256_AT + 2 * j] = std::cos(2 * PI * j / 256.0);
-    t[STOI_TW256_AT + 2 * j + 1] = -std::sin(2 * PI * j / 256.0);
+    t[tw256 + 2 * j] = std::cos(2 * PI * j / 256.0);
+    t[tw256 + 2 * j + 1] = -std::sin(2 * PI * j / 256.0);
   }
   for (int k = 0; k <= 256; ++k) {
-    t[STOI_TW512_AT + 2 * k] = std::cos(2 * PI * k / 512.0);
-    t[STOI_TW512_AT + 2 * k + 1] = -std::sin(2 * PI * k / 512.0);
+    t[tw512 + 2 * k] = std::cos(2 * PI * k / 512.0);
+    t[tw512 + 2 * k + 1] = -std::sin(2 * PI * k / 512.0);
   }
-  CK(cudaMalloc((void**)&ctx->d_stoi_tables, STOI_TABLES * sizeof(double)));
-  CK(cudaMemcpy(ctx->d_stoi_tables, t.data(), STOI_TABLES * sizeof(double), cudaMemcpyHostToDevice));
+  double* d = nullptr;
+  CK(cudaMalloc((void**)&d, t.size() * sizeof(double)));
+  const cudaError_t e = cudaMemcpy(d, t.data(), t.size() * sizeof(double), cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) cudaFree(d);
+  CK(e);
+  ctx->d_stoi_tables[g.slot] = d;
+  ctx->stoi_half[g.slot] = (int)L;
   return VF_OK;
 }
 
@@ -222,13 +269,15 @@ VF_API int vf_sispec(vf_ctx* ctx, const float* est, const float* target, int bat
 }
 
 // ---------------------------------------------------------------------------------------------------------------- scoring
-VF_API int vf_metric_spectrogram(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* sp_out, float* mel_out,
-                                 void* stream) {
+VF_API int vf_metric_spectrogram_ex(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* sp_out,
+                                    float* mel_out, int rate, void* stream) {
   static const char* fn = "vf_metric_spectrogram";
+  Geometry g;
   int rc = begin_call(ctx, fn, wav && sp_out && batch > 0);
-  if (!rc) rc = check_offsets(ctx, fn, "wav", "clip", offsets, batch, 1025, ITEM_MAX);   // one reflection of the STFT padding
+  if (!rc) rc = geometry(ctx, fn, rate, &g);
+  if (!rc) rc = check_offsets(ctx, fn, "wav", "clip", offsets, batch, g.min_samples(), ITEM_MAX);
+  if (!rc && mel_out) rc = need_fb(ctx, g);
   if (rc) return rc;
-  if (mel_out && !ctx->d_fb_val) return fail(ctx, VF_ESTATE, "mel filterbank not loaded (call vf_load_weights first)");
   cudaStream_t st = (cudaStream_t)stream;
   const std::vector<int> starts = split(batch, SCORE_MAX_IMAGES);
   long rows = 0;
@@ -238,23 +287,28 @@ VF_API int vf_metric_spectrogram(vf_ctx* ctx, const float* wav, const int64_t* o
     memset(&p, 0, sizeof p);
     p.batch = starts[k + 1] - s;
     p.sources = 1;
-    p.wav[0] = wav; p.sp[0] = sp_out + (size_t)rows * 1025;
-    p.window = ctx->d_window64; p.tw1024 = ctx->d_tw1024d; p.tw2048 = ctx->d_tw2048d;
+    p.wav[0] = wav; p.sp[0] = sp_out + (size_t)rows * g.bins;
+    set_tables(ctx, g, p);
     for (int i = 0; i <= p.batch; ++i) p.off[0][i] = offsets[s + i];
-    for (int i = 0; i < p.batch; ++i) p.frame_off[i + 1] = p.frame_off[i] + stft_frames(offsets[s + i + 1] - offsets[s + i]);
-    CK(launch_metric_stft(p, st));
+    for (int i = 0; i < p.batch; ++i) p.frame_off[i + 1] = p.frame_off[i] + g.frames(offsets[s + i + 1] - offsets[s + i]);
+    CK(g.stft(p, st));
     ctx->launches++;
     rows += (long)p.frame_off[p.batch];
   }
   if (mel_out) {
     MelParams m;
     memset(&m, 0, sizeof m);
-    m.in = sp_out; m.n_outer = 1; m.T = rows; m.so = 0; m.sf = 1; m.st = 1025;
-    m.out = mel_out; m.fb_f0 = ctx->d_fb_f0; m.fb_len = ctx->d_fb_len; m.fb_ofs = ctx->d_fb_ofs; m.fb_val = ctx->d_fb_val;
-    CK(launch_mel(m, st));
+    m.in = sp_out; m.n_outer = 1; m.T = rows; m.so = 0; m.sf = 1; m.st = g.bins;
+    m.out = mel_out;
+    set_fb(g, m);
+    CK(launch_mel(m, st, g.bins, g.mels));
     ctx->launches++;
   }
   return VF_OK;
+}
+VF_API int vf_metric_spectrogram(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* sp_out, float* mel_out,
+                                 void* stream) {
+  return vf_metric_spectrogram_ex(ctx, wav, offsets, batch, sp_out, mel_out, 44100, stream);
 }
 
 VF_API int vf_ssim(vf_ctx* ctx, const float* est, const float* target, int images, int frames, int bins, double* out, void* stream) {
@@ -283,27 +337,31 @@ VF_API int vf_ssim(vf_ctx* ctx, const float* est, const float* target, int image
   return VF_OK;
 }
 
-VF_API int vf_score_varlen(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target, const int64_t* target_offsets,
-                           int batch, double* out, void* stream) {
+VF_API int vf_score_varlen_ex(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target,
+                              const int64_t* target_offsets, int batch, double* out, int rate, void* stream) {
   static const char* fn = "vf_score_varlen";
+  Geometry g;
   int rc = begin_call(ctx, fn, est && target && out && batch > 0);
-  if (!rc) rc = check_offsets(ctx, fn, "est", "clip", est_offsets, batch, 1025, ITEM_MAX);
-  if (!rc) rc = check_offsets(ctx, fn, "target", "clip", target_offsets, batch, 1025, ITEM_MAX);
+  if (!rc) rc = geometry(ctx, fn, rate, &g);
+  if (!rc) rc = check_offsets(ctx, fn, "est", "clip", est_offsets, batch, g.min_samples(), ITEM_MAX);
+  if (!rc) rc = check_offsets(ctx, fn, "target", "clip", target_offsets, batch, g.min_samples(), ITEM_MAX);
   if (rc) return rc;
   std::vector<long> T(batch);
   for (int i = 0; i < batch; ++i) {
-    T[i] = stft_frames(est_offsets[i + 1] - est_offsets[i]);
-    const long tt = stft_frames(target_offsets[i + 1] - target_offsets[i]);
+    T[i] = g.frames(est_offsets[i + 1] - est_offsets[i]);
+    const long tt = g.frames(target_offsets[i + 1] - target_offsets[i]);
     if (T[i] != tt) return fail(ctx, VF_EINVAL, "vf_score_varlen: pair %d: est has %ld frames, target %ld", i, T[i], tt);
     if (T[i] < 7) return fail(ctx, VF_EINVAL, "vf_score_varlen: pair %d has %ld frames, fewer than SSIM's 7", i, T[i]);
   }
-  if (!ctx->d_fb_val) return fail(ctx, VF_ESTATE, "mel filterbank not loaded (call vf_load_weights first)");
+  rc = need_fb(ctx, g);
+  if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
+  const int B = g.bins, M = g.mels;
   // sub-batches of at most SCORE_MAX_IMAGES pairs and SCORE_CAP_FRAMES frames per side.  Scratch per pair: two
   // spectrograms, two mels, its SSIM tile sums.
   const std::vector<int> starts = split(batch, SCORE_MAX_IMAGES, SCORE_CAP_FRAMES, [&](int i) { return (int64_t)T[i]; });
   rc = acquire_scratch(ctx, ctx->score, max_bytes(starts, [&](int i) {
-    return (size_t)T[i] * (2 * 1025 + 2 * 128) * 4 + (size_t)(ssim_tiles(T[i], 1025) + ssim_tiles(T[i], 128)) * 8;
+    return (size_t)T[i] * (2 * B + 2 * M) * 4 + (size_t)(ssim_tiles(T[i], B) + ssim_tiles(T[i], M)) * 8;
   }), st);
   if (rc) return rc;
   cudaError_t e = cudaSuccess;
@@ -319,21 +377,22 @@ VF_API int vf_score_varlen(vf_ctx* ctx, const float* est, const int64_t* est_off
     for (int i = 0; i < nb; ++i) p.frame_off[i + 1] = set.frame_off[i + 1] = p.frame_off[i] + T[s + i];
     const long F = (long)p.frame_off[nb];
     float* sp_e = static_cast<float*>(ctx->score.p);
-    float* sp_t = sp_e + (size_t)F * 1025;
-    float* mel_e = sp_t + (size_t)F * 1025;
-    float* mel_t = mel_e + (size_t)F * 128;
-    double* partial = reinterpret_cast<double*>(mel_t + (size_t)F * 128);   // F * 2306 floats: 8-byte aligned
+    float* sp_t = sp_e + (size_t)F * B;
+    float* mel_e = sp_t + (size_t)F * B;
+    float* mel_t = mel_e + (size_t)F * M;
+    double* partial = reinterpret_cast<double*>(mel_t + (size_t)F * M);   // F * (2306 or 904) floats: 8-byte aligned
     p.wav[0] = est; p.wav[1] = target; p.sp[0] = sp_e; p.sp[1] = sp_t;
-    p.window = ctx->d_window64; p.tw1024 = ctx->d_tw1024d; p.tw2048 = ctx->d_tw2048d;
-    e = launch_metric_stft(p, st);
+    set_tables(ctx, g, p);
+    e = g.stft(p, st);
     MelParams m;                              // both spectrograms in one launch: outer index 0 = est, 1 = target
     memset(&m, 0, sizeof m);
-    m.in = sp_e; m.n_outer = 2; m.T = F; m.so = F * 1025; m.sf = 1; m.st = 1025;
-    m.out = mel_e; m.fb_f0 = ctx->d_fb_f0; m.fb_len = ctx->d_fb_len; m.fb_ofs = ctx->d_fb_ofs; m.fb_val = ctx->d_fb_val;
-    if (e == cudaSuccess) e = launch_mel(m, st);
+    m.in = sp_e; m.n_outer = 2; m.T = F; m.so = F * B; m.sf = 1; m.st = B;
+    m.out = mel_e;
+    set_fb(g, m);
+    if (e == cudaSuccess) e = launch_mel(m, st, B, M);
     double* o = out + (size_t)s * 8;
     const float* img[2][2] = {{sp_e, sp_t}, {mel_e, mel_t}};
-    const int bins[2] = {1025, 128};
+    const int bins[2] = {B, M};
     for (int r = 0; r < 2 && e == cudaSuccess; ++r) {        // keys 0-3 on the spectrogram, 4-7 on the mel
       e = launch_lsd_varlen(img[r][0], img[r][1], bins[r], set, o + 4 * r, 8, st);
       if (e == cudaSuccess) e = launch_sispec_varlen(img[r][0], img[r][1], bins[r], set, o + 4 * r + 1, 8, st);
@@ -350,29 +409,38 @@ VF_API int vf_score_varlen(vf_ctx* ctx, const float* est, const int64_t* est_off
   if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "score launch: %s", cudaGetErrorString(e));
   return rc;
 }
+VF_API int vf_score_varlen(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target, const int64_t* target_offsets,
+                           int batch, double* out, void* stream) {
+  return vf_score_varlen_ex(ctx, est, est_offsets, target, target_offsets, batch, out, 44100, stream);
+}
 
-VF_API int vf_score_time_varlen(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target,
-                                const int64_t* target_offsets, int batch, double* out, void* stream) {
+VF_API int vf_score_time_varlen_ex(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target,
+                                   const int64_t* target_offsets, int batch, double* out, int rate, void* stream) {
   static const char* fn = "vf_score_time_varlen";
+  Geometry g;
   int rc = begin_call(ctx, fn, est && target && out && batch > 0);
+  if (!rc) rc = geometry(ctx, fn, rate, &g);
   if (!rc) rc = check_offsets(ctx, fn, "est", "pair", est_offsets, batch, 1, ITEM_MAX);
   if (!rc) rc = check_offsets(ctx, fn, "target", "pair", target_offsets, batch, 1, ITEM_MAX);
   if (rc) return rc;
   std::vector<int64_t> N(batch);
   for (int i = 0; i < batch; ++i) {
     N[i] = std::max(est_offsets[i + 1] - est_offsets[i], target_offsets[i + 1] - target_offsets[i]);
-    if (stoi_len10(N[i]) <= STOI_FRAME)
+    if (g.len10(N[i]) <= STOI_FRAME)
       return fail(ctx, VF_EINVAL, "vf_score_time_varlen: pair %d: %ld samples give %ld at 10 kHz, STOI needs more than %d", i,
-                  (long)N[i], (long)stoi_len10(N[i]), STOI_FRAME);
+                  (long)N[i], (long)g.len10(N[i]), STOI_FRAME);
   }
-  rc = stoi_tables(ctx);
+  rc = stoi_tables(ctx, g);
   if (rc) return rc;
+  const int half = ctx->stoi_half[g.slot];
+  const double* tables = ctx->d_stoi_tables[g.slot];
   cudaStream_t st = (cudaStream_t)stream;
-  // sub-batches of at most SCORE_MAX_IMAGES pairs and SCORE_CAP_FRAMES * 441 padded samples.  Scratch per pair:
-  // resampled and compacted signals, energies, band values, tile sums (doubles), then kept-frame indices and a count (ints).
-  const std::vector<int> starts = split(batch, SCORE_MAX_IMAGES, SCORE_CAP_FRAMES * 441, [&](int i) { return N[i]; });
+  // sub-batches of at most SCORE_MAX_IMAGES pairs and SCORE_CAP_FRAMES * hop padded samples: at either rate at most
+  // SCORE_CAP_FRAMES * 100 samples at 10 kHz.  Scratch per pair: resampled and compacted signals, energies, band values,
+  // tile sums (doubles), then kept-frame indices and a count (ints).
+  const std::vector<int> starts = split(batch, SCORE_MAX_IMAGES, SCORE_CAP_FRAMES * g.hop, [&](int i) { return N[i]; });
   rc = acquire_scratch(ctx, ctx->time_score, max_bytes(starts, [&](int i) {
-    const int64_t n10 = stoi_len10(N[i]), nf = stoi_frames(n10);
+    const int64_t n10 = g.len10(N[i]), nf = stoi_frames(n10);
     return (size_t)(4 * n10 + (1 + 2 * STOI_BANDS) * nf + stoi_tiles(nf)) * 8 + (size_t)(nf + 1) * 4;
   }), st);
   if (rc) return rc;
@@ -389,17 +457,18 @@ VF_API int vf_score_time_varlen(vf_ctx* ctx, const float* est, const int64_t* es
       p.t_off[i] = target_offsets[s + i] - target_offsets[s];
     }
     for (int i = 0; i < nb; ++i) {
-      const int64_t n10 = stoi_len10(N[s + i]), nf = stoi_frames(n10);
+      const int64_t n10 = g.len10(N[s + i]), nf = stoi_frames(n10);
       p.r_off[i + 1] = p.r_off[i] + n10;
       p.f_off[i + 1] = p.f_off[i] + nf;
       p.tile_off[i + 1] = p.tile_off[i] + stoi_tiles(nf);
     }
     stoi_bands(p.band_lo, p.band_hi);
     p.clip = 1 + std::pow(10.0, 15.0 / 20);
-    p.taps = ctx->d_stoi_tables;
-    p.window = ctx->d_stoi_tables + STOI_WIN_AT;
-    p.tw256 = reinterpret_cast<const double2*>(ctx->d_stoi_tables + STOI_TW256_AT);
-    p.tw512 = reinterpret_cast<const double2*>(ctx->d_stoi_tables + STOI_TW512_AT);
+    p.up = g.stoi_up; p.down = g.stoi_down; p.half = half;
+    p.taps = tables;
+    p.window = tables + stoi_win_at(half);
+    p.tw256 = reinterpret_cast<const double2*>(tables + stoi_tw256_at(half));
+    p.tw512 = reinterpret_cast<const double2*>(tables + stoi_tw512_at(half));
     const int64_t Rs = p.r_off[nb], Fs = p.f_off[nb], Ts = p.tile_off[nb];
     double* d = static_cast<double*>(ctx->time_score.p);
     p.rs = d;
@@ -416,6 +485,10 @@ VF_API int vf_score_time_varlen(vf_ctx* ctx, const float* est, const int64_t* es
   rc = mark_use(ctx, ctx->time_score.order, st);
   if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "time score launch: %s", cudaGetErrorString(e));
   return rc;
+}
+VF_API int vf_score_time_varlen(vf_ctx* ctx, const float* est, const int64_t* est_offsets, const float* target,
+                                const int64_t* target_offsets, int batch, double* out, void* stream) {
+  return vf_score_time_varlen_ex(ctx, est, est_offsets, target, target_offsets, batch, out, 44100, stream);
 }
 
 // ------------------------------------------------------------------------------------------------------ SR degradations

@@ -10,7 +10,9 @@
 * `AudioMetrics.wav_to_spectrogram` / `.evaluation` / `.evaluation_batch`: scoring a restored file against its clean target
   (metrics.py:37-81), the second half of evaluation_proc/eval.py's evaluation().  The spectrogram is librosa 0.8's STFT
   (reflect padding; librosa >= 0.10 pads with zeros, not built) and SSIM is scikit-image <= 0.18's float64
-  structural_similarity with data_range 2 (>= 0.19 computes float32 and needs data_range, not built).
+  structural_similarity with data_range 2 (>= 0.19 computes float32 and needs data_range, not built).  Both of the
+  reference's geometries are built: 44.1 kHz (n_fft 2048, hop 441, 128 mels) and 16 kHz (n_fft 743, hop 160, 80 mels);
+  an instance scores targets at its own rate, as aggregate_score builds one per test set (eval.py:43-45).
 * `evaluation(..., time_domain=True)` / `evaluation_batch(..., time_domain=True)` add the sisdr and stoi keys, which the
   reference gets from the third-party speechmetrics package on the CPU (metrics.py:58-64): SI-SDR as speechmetrics
   computes it and pystoi 0.3.3's STOI, restated in oracle/speech_metrics.py and computed in float64 by
@@ -91,12 +93,19 @@ def first_channel(path) -> np.ndarray:
     return np.ascontiguousarray(data[:, 0].astype(np.float32) / np.float32(32768.0))
 
 
-def check_rate(rate: int, what) -> None:
-    """wav_to_spectrogram's rate branch (metrics.py:38-47): 44100 is built, 16000 (n_fft 743, hop 160, 80 mels) is not."""
-    if rate == 16000:
-        raise NotImplementedError(f"{what}: the 16 kHz metrics (n_fft 743, hop 160, 80 mels) are not built")
-    if rate != 44100:
-        raise ValueError(f"Bad Samplerate: {what} is {rate} Hz")
+RATES = (44100, 16000)      # wav_to_spectrogram's two branches (metrics.py:38-47)
+
+
+def check_rate(rate: int, what, built: int = 44100) -> None:
+    """wav_to_spectrogram's rate branch (metrics.py:38-47) for an AudioMetrics instance that scores at `built` Hz: a file at
+    the other rate of RATES raises NotImplementedError naming the `rate=` it needs (aggregate_score builds one AudioMetrics
+    per test set, evaluation_proc/eval.py:43-45), any other rate ValueError("Bad Samplerate ...")."""
+    if rate == built:
+        return
+    if rate in RATES:
+        raise NotImplementedError(f"{what} is at {rate} Hz: score it with AudioMetrics(..., rate={rate}), this instance "
+                                  f"scores {built} Hz targets")
+    raise ValueError(f"Bad Samplerate: {what} is {rate} Hz")
 
 
 class AudioMetrics:
@@ -148,12 +157,14 @@ class AudioMetrics:
         return eng.ssim(est.reshape(b * c, t, f), target.reshape(b * c, t, f)).view(b, c, 1, 1)
 
     def wav_to_spectrogram(self, wav, rate: int = 44100):
-        """metrics.py:37-51 for one signal (numpy or tensor, 1-D): (sp [1, 1, T, 1025], mel [1, 1, T, 128]) on the device."""
-        check_rate(rate, "wav")
+        """metrics.py:37-51 for one signal (numpy or tensor, 1-D): (sp [1, 1, T, 1025], mel [1, 1, T, 128]) on the device, or
+        at rate=16000 (sp [1, 1, T, 372], mel [1, 1, T, 80]); any instance computes both, as the reference's does."""
+        if rate not in RATES:
+            raise ValueError(f"Bad Samplerate: {rate} Hz")
         eng = self._eng()
         x = torch.as_tensor(np.ascontiguousarray(wav, dtype=np.float32) if not isinstance(wav, torch.Tensor) else wav)
         x = x.to(eng.device, torch.float32).reshape(-1).contiguous()
-        sp, mel = eng.metric_spectrogram(x, [x.numel()])
+        sp, mel = eng.metric_spectrogram(x, [x.numel()]) if rate == 44100 else eng.metric_spectrogram(x, [x.numel()], rate=rate)
         return sp[None, None], mel[None, None]
 
     def evaluation(self, est, target, time_domain: bool = False) -> dict:
@@ -163,28 +174,31 @@ class AudioMetrics:
 
     def evaluation_batch(self, pairs, time_domain: bool = False) -> list:
         """evaluation(est, target) of every pair, in order, in one vf_score_varlen call: each dict is float-identical to
-        evaluation() of that pair.  Every file is decoded and checked before any GPU work; a bad pair fails the whole call,
-        naming the file: a target at 16 kHz (NotImplementedError) or at another rate than 44.1 kHz (ValueError), an est
-        whose frame count differs from its target's or a pair of fewer than 7 frames (ValueError).
+        evaluation() of that pair.  The instance scores targets at its own rate, 44.1 kHz or 16 kHz (AudioMetrics(owner,
+        rate=16000): n_fft 743, hop 160, 80 mels); an est at another rate is resampled to it on the GPU first, as
+        librosa.load(sr=rate) does.  Every file is decoded and checked before any GPU work; a bad pair fails the whole call,
+        naming the file: a target at the other of the two rates (NotImplementedError naming the rate= it needs) or at any
+        other rate (ValueError), an est whose frame count differs from its target's or a pair of fewer than 7 frames
+        (ValueError).
 
         time_domain=True adds speechmetrics' sisdr and stoi (one more call, vf_score_time_varlen, on each file's first
         channel as speechmetrics reads it), and each dict is {"sisdr", "stoi", <the 8 spectral keys>} in metrics.py's
-        order, without pesq.  The spectral values are those of time_domain=False.  The est must then be at the target's
-        44.1 kHz (ValueError naming it): speechmetrics would compare samples at two rates, which is not reproduced."""
-        from .arch import frames_for
+        order, without pesq.  The spectral values are those of time_domain=False.  The est must then be at its target's
+        rate (ValueError naming it): speechmetrics would compare samples at two rates, which is not reproduced."""
+        from .arch import metric_frames
         from .handler import _rate_len, _to_rate, read_pcm16
-        eng = self._eng()
+        rate = self.rate
         decoded, channels = [], []
         for est, target in pairs:
             if target is None:
                 decoded.append(None)
                 continue
-            t, rate = read_pcm16(target)
-            check_rate(rate, target)
+            t, t_rate = read_pcm16(target)
+            check_rate(t_rate, target, rate)
             e, e_rate = read_pcm16(est)
             if time_domain and e_rate != rate:
                 raise ValueError(f"{est} is at {e_rate} Hz: sisdr / stoi need it at its target's {rate} Hz")
-            te, tt = frames_for(_rate_len(len(e), e_rate, rate)), frames_for(len(t))
+            te, tt = metric_frames(_rate_len(len(e), e_rate, rate), rate), metric_frames(len(t), rate)
             if te != tt:
                 raise ValueError(f"{est} has {te} frames at {rate} Hz, its target {target} {tt}")
             if tt < 7:
@@ -196,15 +210,17 @@ class AudioMetrics:
         results = [{} for _ in decoded]
         if not live:
             return results
-        ests = [_to_rate(path, e, e_rate, 44100, eng) for path, e, e_rate, _ in live]
+        eng = self._eng()
+        at = {} if rate == 44100 else {"rate": rate}     # the 44.1 kHz calls are the entry points without a rate
+        ests = [_to_rate(path, e, e_rate, rate, eng) for path, e, e_rate, _ in live]
         tgts = [t for _, _, _, t in live]
         scores = eng.score_varlen(torch.from_numpy(np.concatenate(ests)).to(eng.device), [len(e) for e in ests],
-                                  torch.from_numpy(np.concatenate(tgts)).to(eng.device), [len(t) for t in tgts]).cpu()
+                                  torch.from_numpy(np.concatenate(tgts)).to(eng.device), [len(t) for t in tgts], **at).cpu()
         rows = iter(scores.tolist())
         if time_domain:
             ests, tgts = [e for e, _ in channels], [t for _, t in channels]
             td = eng.score_time_varlen(torch.from_numpy(np.concatenate(ests)).to(eng.device), [len(e) for e in ests],
-                                       torch.from_numpy(np.concatenate(tgts)).to(eng.device), [len(t) for t in tgts])
+                                       torch.from_numpy(np.concatenate(tgts)).to(eng.device), [len(t) for t in tgts], **at)
             time_rows = iter(td.cpu().tolist())
         for i, d in enumerate(decoded):
             if d is not None:

@@ -29,7 +29,8 @@ import numpy as np
 import torch
 
 from . import _lib as L
-from .arch import SSR_PREFIX, UNET_PREFIX, VocoderConfig, bigru_keys, dnn_keys, frames_for, unet_keys, vocoder_keys
+from .arch import (SSR_PREFIX, UNET_PREFIX, VocoderConfig, bigru_keys, dnn_keys, frames_for, metric_frames, unet_keys,
+                   vocoder_keys)
 
 
 class HParams(dict):
@@ -70,6 +71,11 @@ def melscale_fbanks(n_freqs=1025, f_min=0.0, f_max=22050.0, n_mels=128, sample_r
     down_slopes = (-1.0 * slopes[:, :-2]) / f_diff[:-1]
     up_slopes = slopes[:, 2:] / f_diff[1:]
     return torch.max(torch.zeros(1), torch.min(down_slopes, up_slopes))
+
+
+def mel16k_fbanks():
+    """AudioMetrics' mel_16k filterbank: MelScale(n_mels=80, sample_rate=16000, n_stft=372).fb, [372, 80]."""
+    return melscale_fbanks(372, 0.0, 8000.0, 80, 16000)
 
 
 def _ptr(t: Optional[torch.Tensor]):
@@ -161,7 +167,8 @@ class Engine:
                 raise KeyError(f"state dict is missing {len(missing)} '{g}' tensors, e.g. {missing[:3]}{hint}")
             needed += groups[g]
         fb = state["mel.fb"] if "mel.fb" in state else melscale_fbanks()
-        items = [("mel.fb", fb)] + [(k, state[k]) for k in needed]
+        # AudioMetrics' mel_16k (metrics.py:30), so that any engine also scores 16 kHz test sets
+        items = [("mel.fb", fb), ("metrics.mel_16k.fb", mel16k_fbanks())] + [(k, state[k]) for k in needed]
         descs = (L.VfTensorDesc * len(items))()
         keep = []
         for d, (k, t) in zip(descs, items):
@@ -268,16 +275,26 @@ class Engine:
                                          ctypes.c_void_p(out[o0:].data_ptr()), _stream()))
         return out.view(*lead, t, 128).transpose(-1, -2)     # same memory layout as the reference's matmul result
 
-    def metric_spectrogram(self, wav_packed: torch.Tensor, lengths, want_mel: bool = True):
+    def metric_spectrogram(self, wav_packed: torch.Tensor, lengths, want_mel: bool = True, rate: int = 44100):
         """vf_metric_spectrogram: |librosa.stft(n_fft=2048, hop_length=441)| of each clip of wav_packed (clips back to back,
-        `lengths` samples each) -> (sp [sum T_i, 1025], mel [sum T_i, 128] or None), clip i at rows sum_{j<i} T_i."""
+        `lengths` samples each) -> (sp [sum T_i, 1025], mel [sum T_i, 128] or None), clip i at rows sum_{j<i} T_i.
+        rate=16000 (vf_metric_spectrogram_ex): n_fft 743, hop 160 -> sp [sum T_i, 372], mel [sum T_i, 80] with
+        T_i = arch.metric_frames(n_i, 16000)."""
         wav_packed, offsets = self._varlen_args(wav_packed, lengths)
-        rows = self._packed_rows(offsets)
-        sp = torch.empty(rows, 1025, device=self.device)
-        mel = torch.empty(rows, 128, device=self.device) if want_mel else None
+        if rate == 44100:
+            rows, bins, mels = self._packed_rows(offsets), 1025, 128
+        else:
+            rows, bins, mels = sum(metric_frames(offsets[i + 1] - offsets[i], 16000) for i in range(len(offsets) - 1)), 372, 80
+        sp = torch.empty(rows, bins, device=self.device)
+        mel = torch.empty(rows, mels, device=self.device) if want_mel else None
         with torch.cuda.device(self.device):
-            self._ck(self.lib.vf_metric_spectrogram(self.ctx, _ptr(wav_packed), offsets, len(offsets) - 1, _ptr(sp), _ptr(mel),
-                                                    _stream()))
+            if rate == 44100:
+                rc = self.lib.vf_metric_spectrogram(self.ctx, _ptr(wav_packed), offsets, len(offsets) - 1, _ptr(sp), _ptr(mel),
+                                                    _stream())
+            else:
+                rc = self.lib.vf_metric_spectrogram_ex(self.ctx, _ptr(wav_packed), offsets, len(offsets) - 1, _ptr(sp), _ptr(mel),
+                                                       int(rate), _stream())
+            self._ck(rc)
         return sp, mel
 
     def ssim(self, est: torch.Tensor, target: torch.Tensor) -> torch.Tensor:
@@ -291,30 +308,39 @@ class Engine:
             self._ck(self.lib.vf_ssim(self.ctx, _ptr(est), _ptr(target), n, t, f, _ptr(out), _stream()))
         return out
 
-    def score_varlen(self, est_packed: torch.Tensor, est_lengths, target_packed: torch.Tensor, target_lengths) -> torch.Tensor:
+    def score_varlen(self, est_packed: torch.Tensor, est_lengths, target_packed: torch.Tensor, target_lengths,
+                     rate: int = 44100) -> torch.Tensor:
         """vf_score_varlen: the spectral metrics of each (est, target) pair of two packed sets -> float64 [pairs, 8], columns
-        in the order of edges.SCORE_KEYS."""
+        in the order of edges.SCORE_KEYS.  rate=16000 scores with the 16 kHz geometry (vf_score_varlen_ex)."""
         est_packed, est_off = self._varlen_args(est_packed, est_lengths)
         target_packed, target_off = self._varlen_args(target_packed, target_lengths)
         if len(est_off) != len(target_off):
             raise ValueError("score_varlen: est and target must hold the same number of clips")
         out = torch.empty(len(est_off) - 1, 8, dtype=torch.float64, device=self.device)
+        args = (self.ctx, _ptr(est_packed), est_off, _ptr(target_packed), target_off, len(est_off) - 1, _ptr(out))
         with torch.cuda.device(self.device):
-            self._ck(self.lib.vf_score_varlen(self.ctx, _ptr(est_packed), est_off, _ptr(target_packed), target_off,
-                                              len(est_off) - 1, _ptr(out), _stream()))
+            if rate == 44100:
+                self._ck(self.lib.vf_score_varlen(*args, _stream()))
+            else:
+                self._ck(self.lib.vf_score_varlen_ex(*args, int(rate), _stream()))
         return out
 
-    def score_time_varlen(self, est_packed: torch.Tensor, est_lengths, target_packed: torch.Tensor, target_lengths) -> torch.Tensor:
-        """vf_score_time_varlen: speechmetrics' sisdr and stoi of each (est, target) pair of two packed 44.1 kHz sets ->
-        float64 [pairs, 2], columns sisdr, stoi.  The clips of a pair may differ in length (the shorter is zero-padded)."""
+    def score_time_varlen(self, est_packed: torch.Tensor, est_lengths, target_packed: torch.Tensor, target_lengths,
+                          rate: int = 44100) -> torch.Tensor:
+        """vf_score_time_varlen: speechmetrics' sisdr and stoi of each (est, target) pair of two packed sets at `rate`
+        (44100, or 16000 through vf_score_time_varlen_ex) -> float64 [pairs, 2], columns sisdr, stoi.  The clips of a pair
+        may differ in length (the shorter is zero-padded)."""
         est_packed, est_off = self._varlen_args(est_packed, est_lengths)
         target_packed, target_off = self._varlen_args(target_packed, target_lengths)
         if len(est_off) != len(target_off):
             raise ValueError("score_time_varlen: est and target must hold the same number of clips")
         out = torch.empty(len(est_off) - 1, 2, dtype=torch.float64, device=self.device)
+        args = (self.ctx, _ptr(est_packed), est_off, _ptr(target_packed), target_off, len(est_off) - 1, _ptr(out))
         with torch.cuda.device(self.device):
-            self._ck(self.lib.vf_score_time_varlen(self.ctx, _ptr(est_packed), est_off, _ptr(target_packed), target_off,
-                                                   len(est_off) - 1, _ptr(out), _stream()))
+            if rate == 44100:
+                self._ck(self.lib.vf_score_time_varlen(*args, _stream()))
+            else:
+                self._ck(self.lib.vf_score_time_varlen_ex(*args, int(rate), _stream()))
         return out
 
     def sosfiltfilt_varlen(self, x_packed: torch.Tensor, lengths, sos, zi, row_filter, row_f32=None) -> torch.Tensor:
