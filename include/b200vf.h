@@ -16,6 +16,8 @@
  *                                 pre -> model -> from_log -> vocoder -> peak normalise -> trim_center
  *   vf_restore_varlen             the same for clips of different lengths in one call (handler() run over a test set)
  *   vf_restore_varlen_mels        + each clip's stage A / B mels, the inputs of handler()'s metrics (handler_batch)
+ *   vf_restore_chunks             the chunks of many live streams, gathered from device rings and cropped on the device:
+ *                                 LambdaOverlapAdd (tools/dsp/overlapadd_boxcar.py:338-534) run incrementally
  *   vf_to_log / vf_from_log       tools/pytorch/pytorch_util.py:157-163
  *   vf_to_pcm16                   the int16 conversion of save_wave, tools/file/wav.py:22-24 (SURVEY.md 8(f) row 3)
  *   vf_mel                        MelScale.forward on any spectrogram, tools/pytorch/mel_scale.py:52-64
@@ -162,6 +164,30 @@ VF_API int vf_restore_varlen(vf_ctx* ctx, const float* wav, const int64_t* offse
  * sub-batch adds one copy kernel on `stream` (none when both are NULL: the call is then vf_restore_varlen). */
 VF_API int vf_restore_varlen_mels(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out,
                                   unsigned flags, float* mel_out, float* log_mel_out, void* stream);
+/* Chunks of live audio streams, restored in one call (chunked boxcar-margin streaming, voicefixer_main_b200/streaming.py).
+ * ring [n_streams, ring_len] (device) holds each stream's recent samples: absolute position p of stream s is at
+ * ring[s * ring_len + p mod ring_len].  chunks: HOST table of n_chunks entries (read during the call only).  Chunk c reads
+ * positions start .. start + length - 1 of stream `stream`; a position >= valid reads as 0 (valid = the stream's length once
+ * it has ended, INT64_MAX while it is open: BoxcarOverlapAdd's zero padding).  Its restored samples [crop_left, length -
+ * crop_right) are written to kept_out (device), chunk after chunk.  Chunk c's kept samples are bit-identical to vf_restore_ex
+ * (batch 1, same flags) on its zero-filled samples, cropped.  Every argument is checked before any work is queued (VF_EINVAL:
+ * a stream out of range, length > ring_len, a length vf_restore_ex rejects - 1024 samples or fewer, over 2^30, or one
+ * trim_center refuses -, crops that leave nothing, start < 0); the context stays usable.  One gather launch, the
+ * vf_restore_varlen chain and one crop launch per sub-batch; each sub-batch runs on the plan for the next power of two of its
+ * chunk count (the extra rows repeat its first chunk and are discarded), and holds at most the largest power of two P <= 256
+ * whose batch shapes 1, 2, .., P fit the plan budget together, so a session whose chunk count changes every step reuses a
+ * few cached plans.  The packed input and output scratch is owned by the context, grown on
+ * demand stream-ordered and freed by vf_destroy. */
+typedef struct vf_chunk {
+  int32_t stream;
+  int32_t length;
+  int32_t crop_left;
+  int32_t crop_right;
+  int64_t start;
+  int64_t valid;
+} vf_chunk;
+VF_API int vf_restore_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_chunk* chunks, int n_chunks,
+                             float* kept_out, unsigned flags, void* stream);
 /* The same for the SSR_UNet / GSR_UNet path: clips of different lengths, packed and with HOST offsets as in
  * vf_restore_varlen, no flags.  Clip i's output is bit-identical to vf_ssr_restore on that clip alone (batch 1, same
  * options).  Every clip needs more than 1024 samples and at most 2^30 (no trim_center constraint: there is no vocoder); a

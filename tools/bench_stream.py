@@ -1,0 +1,145 @@
+#!/usr/bin/env python
+"""Benchmark of live-stream restoration (StreamingRestorer / vf_restore_chunks) on one GPU.
+
+    python tools/bench_stream.py [--streams 1,8,64,256] [--windows 1,2] [--steps K] [--warmup W]
+
+For every window W (seconds) and stream count S: S streams of seeded speech-like audio each push W of samples per step, with
+M = W / 4 samples of context on each side of every window (BoxcarOverlapAdd geometry), so after the first step every step
+restores S middle chunks of W + 2M.  Two arms run alternately in one process on the same chunks:
+- "streaming": S pushes (device to device, one copy each) + StreamingRestorer.step(): one gather launch, the varlen restore
+  chain, one crop launch ("streaming_step_only": the step without the pushes);
+- "torch_slicing": what a server does without it: slices each stream's chunk out of its (device-resident) history, one
+  VoiceFixer.restore_batch call per GROUP streams (torch.cat of the slices + vf_restore_varlen), and crops every result.
+  Its histories are resident from the start, so it pays nothing for receiving the audio.
+Both must give the same bits.  A step is timed with CUDA events around it after a device synchronise; medians are
+reported.  A step is real time when it takes at most W seconds (it restores W of audio per stream).  Prints one JSON line:
+per (W, S) the step times, audio seconds restored per second and the plans built and evicted; per W the largest S that
+stays real time; the card's name and power limit, read in the same run.
+"""
+import argparse
+import json
+import os
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+
+import torch  # noqa: E402
+
+from bench import SR, synth_batch  # noqa: E402
+from bench_varlen import card_info  # noqa: E402
+
+BANK = 8            # distinct synthetic signals; stream s plays signal s % BANK shifted by s * 997 samples
+# restore_batch calls of the baseline take at most this many streams: the sub-batch the streaming arm's plan-shape rule picks
+# for 1 - 2 s windows on an 80 GB card, so both arms run on the same cached plans.  Left to its own split, restore_batch of 256
+# chunks picks other shapes, and the two arms' plans would evict each other on every alternation.
+GROUP = 64
+
+
+def timed(fn):
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    out = fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return out, e0, e1
+
+
+def run_case(state, bank, W, M, S, steps, warmup):
+    """One (W, S) case on a model of its own: a fresh plan cache, so that plans of earlier cases neither crowd the budget nor
+    enter its size estimates."""
+    from voicefixer_main_b200 import VoiceFixer
+    from voicefixer_main_b200.streaming import StreamingRestorer
+    model = VoiceFixer().load_state_dict(state).eval().to(bank.device)
+    eng = model._engine()
+    xs = [torch.roll(bank[s % BANK], s * 997) for s in range(S)]
+    sr = StreamingRestorer(model, W, M, max_streams=S)
+    ids = [sr.open() for _ in range(S)]
+
+    def chunk(i):
+        return (0, W + M, 0, M) if i == 0 else (i * W - M, W + 2 * M, M, M)
+
+    pushed = torch.cuda.Event(enable_timing=True)
+
+    def streaming(i):
+        lo, hi = (0, W + M) if i == 0 else (i * W + M, (i + 1) * W + M)
+        for sid, x in zip(ids, xs):
+            sr.push(sid, x[lo:hi])
+        pushed.record()
+        out = sr.step()
+        return [out[sid] for sid in ids]
+
+    def torch_slicing(i):
+        start, length, cl, cr = chunk(i)
+        outs = []
+        for g in range(0, S, GROUP):
+            outs += model.restore_batch([x[start:start + length] for x in xs[g:g + GROUP]])
+        return [o[cl:length - cr] for o in outs]
+
+    info0 = eng.plan_cache_info()
+    ms = {"streaming": [], "streaming_step_only": [], "torch_slicing": []}
+    same = True
+    for i in range(warmup + steps):
+        a, a0, a1 = timed(lambda: streaming(i))
+        b, b0, b1 = timed(lambda: torch_slicing(i))
+        same = same and all(torch.equal(p, q) for p, q in zip(a, b))
+        if i >= warmup:
+            ms["streaming"].append(a0.elapsed_time(a1))
+            ms["streaming_step_only"].append(pushed.elapsed_time(a1))
+            ms["torch_slicing"].append(b0.elapsed_time(b1))
+    eng.check_errors()
+    info1 = eng.plan_cache_info()
+    launches = eng.launch_count()
+    eng.close()
+    audio_s = S * W / SR                                      # kept audio per steady-state step
+    res = {}
+    for k, v in ms.items():
+        med = sorted(v)[len(v) // 2]
+        res[k] = {"ms_per_step_median": med, "ms_min": min(v), "ms_max": max(v), "audio_seconds_per_sec": audio_s / (med * 1e-3),
+                  "real_time": med <= 1e3 * W / SR}
+    return {"window_s": W / SR, "margin_s": M / SR, "streams": S, "arms": res,
+            "speedup_vs_torch_slicing": res["torch_slicing"]["ms_per_step_median"] / res["streaming"]["ms_per_step_median"],
+            "bit_identical": bool(same),
+            "plans_built": (info1["plans"] + info1["evicted"]) - (info0["plans"] + info0["evicted"]),
+            "plans_evicted": info1["evicted"] - info0["evicted"], "plan_cache": info1, "gpu_launches": launches}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--streams", default="1,8,64,256")
+    ap.add_argument("--windows", default="1,2", help="window lengths in seconds; the margin is a quarter of the window")
+    ap.add_argument("--steps", type=int, default=5, help="timed steady-state steps per case")
+    ap.add_argument("--warmup", type=int, default=2, help="untimed steps per case (the first is the streams' first chunk)")
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("tools/bench_stream.py needs a CUDA device")
+    from voicefixer_main_b200.weights import make_state
+    dev = torch.device("cuda", 0)
+    state = make_state(1234)
+    streams = [int(s) for s in args.streams.split(",")]
+    cases, best = [], {}
+    for w_s in [float(w) for w in args.windows.split(",")]:
+        W = int(round(w_s * SR)) // 2 * 2
+        M = W // 4
+        n = (args.warmup + args.steps + 1) * W + M
+        bank = synth_batch(BANK, n, 4242).to(dev)
+        for S in streams:
+            c = run_case(state, bank, W, M, S, args.steps, args.warmup)
+            cases.append(c)
+            if c["arms"]["streaming"]["real_time"]:
+                best[f"{w_s:g}"] = max(best.get(f"{w_s:g}", 0), S)
+        del bank
+    top = max(cases, key=lambda c: c["arms"]["streaming"]["audio_seconds_per_sec"])
+    line = {"metric": "stream_audio_seconds_per_sec", "value": top["arms"]["streaming"]["audio_seconds_per_sec"], "unit": "audio s/s",
+            "higher_is_better": True, "data": "synthetic", "steps": args.steps, "warmup": args.warmup,
+            "config": {"workload": "S streams of seeded speech-like audio, each pushing W per step, M = W / 4, 44.1 kHz; value = "
+                                   "the best streaming arm over the cases", "best_case": {"window_s": top["window_s"], "streams": top["streams"]}},
+            "largest_real_time_streams": {"window_s=" + k: v for k, v in best.items()},
+            "cases": cases, "card": card_info(0)}
+    print(json.dumps(line))
+
+
+if __name__ == "__main__":
+    main()

@@ -6,7 +6,7 @@ with VF_ENODEVICE.  Nothing here computes on the data path; it only marshals poi
 """
 import ctypes
 import os
-from ctypes import (POINTER, Structure, byref, c_char_p, c_double, c_float, c_int, c_int64, c_size_t, c_uint, c_void_p)
+from ctypes import (POINTER, Structure, byref, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_size_t, c_uint, c_void_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200vf.so")
@@ -23,7 +23,7 @@ EXPORTS = [
     "vf_restore_varlen", "vf_ssr_restore_varlen", "vf_restore_varlen_mels", "vf_metric_spectrogram", "vf_ssim", "vf_score_varlen",
     "vf_ssr_restore_varlen_mels", "vf_selftest_op", "vf_selftest_gru", "vf_score_time_varlen",
     "vf_sosfiltfilt_varlen", "vf_resample_poly_f64_varlen", "vf_metric_spectrogram_ex", "vf_score_varlen_ex",
-    "vf_score_time_varlen_ex",
+    "vf_score_time_varlen_ex", "vf_restore_chunks",
 ]
 VF_RESTORE_UNIFY_ENERGY = 1
 VF_SSR_PEAK_NORMALISE = 1
@@ -83,6 +83,12 @@ class VfGruCase(Structure):
                 ("relu", c_int), ("out", c_void_p)]
 
 
+class VfChunk(Structure):
+    """vf_chunk (include/b200vf.h): one chunk of a vf_restore_chunks call."""
+    _fields_ = [("stream", c_int32), ("length", c_int32), ("crop_left", c_int32), ("crop_right", c_int32),
+                ("start", c_int64), ("valid", c_int64)]
+
+
 class EngineError(RuntimeError):
     def __init__(self, code, msg):
         super().__init__(f"libb200vf error {code}: {msg}")
@@ -139,6 +145,7 @@ def load_library():
                                POINTER(c_int), POINTER(c_int), c_char_p, c_int, POINTER(c_double)]
     lib.vf_restore_ex.argtypes = [P, P, c_int, c_int64, P, c_uint, P]
     lib.vf_restore_varlen.argtypes = [P, P, POINTER(c_int64), c_int, P, c_uint, P]
+    lib.vf_restore_chunks.argtypes = [P, P, c_int, c_int64, POINTER(VfChunk), c_int, P, c_uint, P]
     lib.vf_restore_varlen_mels.argtypes = [P, P, POINTER(c_int64), c_int, P, c_uint, P, P, P]
     lib.vf_ssr_forward.argtypes = [P, P, P, c_int, c_int64, P, P]
     lib.vf_ssr_restore.argtypes = [P, P, c_int, c_int64, P, P]

@@ -44,6 +44,17 @@ int mark_use(vf_ctx* ctx, StreamOrder& o, cudaStream_t st) {
   return VF_OK;
 }
 
+int acquire_scratch(vf_ctx* ctx, Scratch& s, size_t need, cudaStream_t st) {
+  const int rc = order_use(ctx, s.order, st);
+  if (rc || need <= s.bytes) return rc;
+  if (s.p) CK(cudaFreeAsync(s.p, st));
+  s.p = nullptr;
+  s.bytes = 0;
+  CK(cudaMallocAsync(&s.p, need, st));
+  s.bytes = need;
+  return VF_OK;
+}
+
 }  // namespace vf
 
 namespace {
@@ -539,16 +550,22 @@ int gather_mels(vf_ctx* ctx, const Plan* plan, const std::vector<int64_t>& frame
 // vf_restore_varlen (`fn`) and vf_restore_varlen_mels.  With mel_out or log_mel_out, each sub-batch's restore is followed by
 // one gather of its clips' rows t < T_i into the packed outputs at frame offsets F_i = sum_{j<i} T_j, still inside the
 // plan's use on `stream` (mark_use again after it).
+// trim_center (eval_gsr_voicefixer.py:68-72) of the vocoder output of n samples back to n: that output is T + T % 2 +
+// tail_base frames of the vocoder's total upsampling, and the centre crop needs it to exceed n by 0 or by at least 2.  The
+// message names item i as `what` (clip, chunk).
+int check_trim_center(vf_ctx* ctx, const char* what, int i, int64_t n) {
+  long scale = 1;
+  for (int s = 0; s < ctx->cfg.voc_num_stages; ++s) scale *= ctx->cfg.voc_scales[s];
+  const int T = frames_of(ctx, (long)n);
+  const long d = (long)(T + T % 2 + ctx->cfg.voc_tail_base) * scale - (long)n;
+  if (d < 0 || d == 1) return fail(ctx, VF_EINVAL, "%s %d: vocoder output length %ld incompatible with input %ld (trim_center)", what, i, (long)n + d, (long)n);
+  return VF_OK;
+}
+
 int restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t* offsets, int batch, float* wav_out,
                    unsigned flags, float* mel_out, float* log_mel_out, cudaStream_t st) {
-  int rc = check_varlen_call(ctx, fn, PLAN_VARLEN, wav, offsets, batch, wav_out, flags, VF_RESTORE_UNIFY_ENERGY, [&](int i, int64_t n) {
-    long scale = 1;
-    for (int s = 0; s < ctx->cfg.voc_num_stages; ++s) scale *= ctx->cfg.voc_scales[s];
-    const int T = frames_of(ctx, (long)n);
-    const long d = (long)(T + T % 2 + ctx->cfg.voc_tail_base) * scale - (long)n;
-    if (d < 0 || d == 1) return fail(ctx, VF_EINVAL, "clip %d: vocoder output length %ld incompatible with input %ld (trim_center)", i, (long)n + d, (long)n);
-    return VF_OK;
-  });
+  int rc = check_varlen_call(ctx, fn, PLAN_VARLEN, wav, offsets, batch, wav_out, flags, VF_RESTORE_UNIFY_ENERGY,
+                             [&](int i, int64_t n) { return check_trim_center(ctx, "clip", i, n); });
   if (rc) return rc;
   const bool mels = mel_out || log_mel_out;
   const std::vector<int64_t> frame_off = mels ? frame_offsets(ctx, offsets, batch) : std::vector<int64_t>();
@@ -559,6 +576,100 @@ int restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t*
     if (r) return r;
     return mark_use(ctx, plan->order, st);
   });
+}
+
+// vf_restore_chunks: every check before anything is queued, then per sub-batch one gather from the rings into the packed
+// input scratch, the varlen restore chain into the packed output scratch, and one crop into kept_out.
+//
+// Plan shapes: a streaming session's chunk count changes from step to step, and varlen plans are keyed by (batch, bucket),
+// so each sub-batch runs on the next power of two of its chunk count.  A sub-batch holds at most the largest power of two P
+// (and VL_MAX_CLIPS) whose shapes 1, 2, 4, .., P fit the plan budget together (2P - 1 rows): a session then meets at most
+// nine batch shapes per bucket instead of one per chunk count, and they stay cached side by side instead of evicting one
+// another whenever the count crosses a power of two.  The rows past the chunks repeat the sub-batch's first chunk, whose results are discarded: rows are
+// independent, so they change no kept sample, and unlike a row of digital silence they put nothing through the chain that
+// the call's own audio does not.
+int restore_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_chunk* chunks, int n_chunks,
+                   float* kept_out, unsigned flags, cudaStream_t st) {
+  const char* fn = "vf_restore_chunks";
+  int rc = check_ready(ctx);
+  if (rc) return rc;
+  if (!ring || !chunks || !kept_out || n_streams <= 0 || ring_len <= 0 || n_chunks <= 0) return fail(ctx, VF_EINVAL, "%s: bad arguments", fn);
+  if (flags & ~(unsigned)VF_RESTORE_UNIFY_ENERGY) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
+  rc = check_networks(ctx, PLAN_VARLEN);
+  if (rc) return rc;
+  int64_t longest = 0;
+  for (int i = 0; i < n_chunks; ++i) {
+    const vf_chunk& c = chunks[i];
+    if (c.stream < 0 || c.stream >= n_streams)
+      return fail(ctx, VF_EINVAL, "%s: chunk %d: stream %d is not in 0 .. %d", fn, i, c.stream, n_streams - 1);
+    if (c.length > ring_len)
+      return fail(ctx, VF_EINVAL, "%s: chunk %d: %d samples do not fit a ring of %ld", fn, i, c.length, (long)ring_len);
+    if (c.length <= 1024)
+      return fail(ctx, VF_EINVAL, "chunk %d: reflect padding needs more than n_fft/2 = 1024 samples (got %d)", i, c.length);
+    if (c.length > 1 << 30) return fail(ctx, VF_EINVAL, "chunk %d: %d samples is too long for one restore", i, c.length);
+    rc = check_trim_center(ctx, "chunk", i, c.length);
+    if (rc) return rc;
+    if (c.crop_left < 0 || c.crop_right < 0 || (int64_t)c.crop_left + c.crop_right >= c.length)
+      return fail(ctx, VF_EINVAL, "%s: chunk %d: crops %d and %d leave nothing of %d samples", fn, i, c.crop_left, c.crop_right, c.length);
+    if (c.start < 0 || c.start > INT64_MAX - c.length) return fail(ctx, VF_EINVAL, "%s: chunk %d: start %ld is out of range", fn, i, (long)c.start);
+    longest = std::max<int64_t>(longest, c.length);
+  }
+  const int fit = choose_sub_batch(ctx, PLAN_VARLEN, 2 * VL_MAX_CLIPS, round_up(frames_of(ctx, (long)longest), 64));
+  int cap = 1;
+  while (cap < VL_MAX_CLIPS && 4 * cap - 1 <= fit) cap *= 2;     // shapes 1, 2, .., 2 cap: 4 cap - 1 rows in all
+  auto rows_of = [](int b) { int r = 1; while (r < b) r *= 2; return r; };
+  auto row_chunk = [&](int s, int b, int k) -> const vf_chunk& { return chunks[s + (k < b ? k : 0)]; };
+  int64_t max_samples = 0;
+  for (int s = 0; s < n_chunks; s += cap) {
+    const int b = std::min(cap, n_chunks - s);
+    int64_t n = 0;
+    for (int k = 0; k < rows_of(b); ++k) n += row_chunk(s, b, k).length;
+    max_samples = std::max(max_samples, n);
+  }
+  rc = acquire_scratch(ctx, ctx->chunks, (size_t)max_samples * 2 * sizeof(float), st);
+  if (rc) return rc;
+  float* in = static_cast<float*>(ctx->chunks.p);
+  float* out = in + max_samples;
+  auto run = [&]() -> int {
+    int64_t kept_off = 0;
+    for (int s = 0; s < n_chunks; s += cap) {
+      const int b = std::min(cap, n_chunks - s), rows = rows_of(b);
+      ChunkGatherParams g;
+      memset(&g, 0, sizeof g);
+      g.ring = ring; g.out = in; g.ring_len = ring_len; g.rows = rows;
+      int64_t n_max = 0;
+      for (int k = 0; k < rows; ++k) {
+        const vf_chunk& c = row_chunk(s, b, k);
+        g.off[k + 1] = g.off[k] + c.length;
+        g.src[k] = (int64_t)c.stream * ring_len;
+        g.phase[k] = c.start % ring_len;
+        g.n_valid[k] = c.valid <= c.start ? 0 : std::min<int64_t>(c.length, c.valid - c.start);
+        n_max = std::max<int64_t>(n_max, c.length);
+      }
+      Plan* plan;
+      int r = get_plan(ctx, PLAN_VARLEN, rows, round_up(frames_of(ctx, (long)n_max), 64), &plan);
+      if (r) return r;
+      CK(launch_stream_gather(g, st));
+      ctx->launches++;
+      r = restore_impl(ctx, plan, in, rows, n_max, out, flags, st, g.off);
+      if (r) return r;
+      ChunkCropParams cp;
+      memset(&cp, 0, sizeof cp);
+      cp.restored = out; cp.kept = kept_out + kept_off; cp.chunks = b;
+      for (int k = 0; k < b; ++k) {
+        const vf_chunk& c = chunks[s + k];
+        cp.src[k] = g.off[k] + c.crop_left;
+        cp.keep[k + 1] = cp.keep[k] + c.length - c.crop_left - c.crop_right;
+      }
+      CK(launch_stream_crop(cp, st));
+      ctx->launches++;
+      kept_off += cp.keep[b];
+    }
+    return VF_OK;
+  };
+  rc = run();
+  const int rm = mark_use(ctx, ctx->chunks.order, st);
+  return rc ? rc : rm;
 }
 
 // vf_ssr_restore_varlen (`fn`) and vf_ssr_restore_varlen_mels.  After each sub-batch's ISTFT, still inside the plan's use on
@@ -660,7 +771,7 @@ VF_API void vf_destroy(vf_ctx* ctx) {
     if (st) cudaStreamDestroy(st);
   for (auto& e : ctx->ev)
     if (e) cudaEventDestroy(e);
-  for (Scratch* s : {&ctx->score, &ctx->time_score, &ctx->iir}) {
+  for (Scratch* s : {&ctx->score, &ctx->time_score, &ctx->iir, &ctx->chunks}) {
     if (s->p) cudaFree(s->p);
     if (s->order.ev) cudaEventDestroy(s->order.ev);
   }
@@ -768,6 +879,11 @@ VF_API int vf_restore_varlen_mels(vf_ctx* ctx, const float* wav, const int64_t* 
                                   unsigned flags, float* mel_out, float* log_mel_out, void* stream) {
   return restore_varlen(ctx, "vf_restore_varlen_mels", wav, offsets, batch, wav_out, flags, mel_out, log_mel_out,
                         (cudaStream_t)stream);
+}
+
+VF_API int vf_restore_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_chunk* chunks, int n_chunks,
+                             float* kept_out, unsigned flags, void* stream) {
+  return restore_chunks(ctx, ring, n_streams, ring_len, chunks, n_chunks, kept_out, flags, (cudaStream_t)stream);
 }
 
 VF_API int vf_restore(vf_ctx* ctx, const float* wav, int batch, int64_t n, float* wav_out, void* stream) {

@@ -229,6 +229,8 @@ struct vf_ctx {
   // vf_score_time_varlen (resampled signals, frame and band values, tile sums, kept-frame indices) and
   // vf_sosfiltfilt_varlen (the call's filter tables, then the scan's extended rows and chunk states)
   Scratch score, time_score, iir;
+  // vf_restore_chunks: the packed input and output of its largest sub-batch, back to back
+  Scratch chunks;
   // vf_score_time_varlen's float64 tables (resampling taps, window, twiddles), one per rate (44.1, 16 kHz; first use)
   double* d_stoi_tables[2] = {nullptr, nullptr};
   int stoi_half[2] = {0, 0};         // their resampling filters' half lengths
@@ -295,6 +297,10 @@ inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 // have queued work on the buffer, or the next use on another stream would not wait for that work.
 int order_use(vf_ctx* ctx, StreamOrder& o, cudaStream_t st);
 int mark_use(vf_ctx* ctx, StreamOrder& o, cudaStream_t st);
+// Orders this use of `s` after its previous one and grows it to `need` bytes, stream-ordered (no host synchronisation).
+// Once this succeeds, mark_use(ctx, s.order, st) must run on every path, a failed launch included: the sub-batches
+// queued before it read the scratch.
+int acquire_scratch(vf_ctx* ctx, Scratch& s, size_t need, cudaStream_t st);
 
 // pack.cu
 int upload_gemm(vf_ctx* ctx, GemmW* w, const std::vector<float>& m, int N, int K, const std::vector<float>* bias);

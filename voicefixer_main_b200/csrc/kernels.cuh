@@ -59,6 +59,31 @@ struct MelGatherParams {
 };
 cudaError_t launch_gather_mels(const MelGatherParams& p, cudaStream_t stream);
 
+// vf_restore_chunks (stream.cu): the chunk tables of one sub-batch, kernel parameters like the lengths table's offsets.
+// Gather: packed sample off[c] + j (j < off[c + 1] - off[c]) of row c is ring[src[c] + (phase[c] + j) mod ring_len] when
+// j < n_valid[c], else 0 (src: the row's stream times ring_len; phase: start mod ring_len; n_valid: the samples before the
+// stream's end).  Crop: kept sample keep[c] + j (j < keep[c + 1] - keep[c]) of chunk c is restored[src[c] + j] (src: the
+// chunk's packed offset plus its crop_left).
+struct ChunkGatherParams {
+  const float* ring;
+  float* out;
+  int64_t ring_len;
+  int rows;
+  int64_t off[VL_MAX_CLIPS + 1];
+  int64_t src[VL_MAX_CLIPS];
+  int64_t phase[VL_MAX_CLIPS];
+  int64_t n_valid[VL_MAX_CLIPS];
+};
+cudaError_t launch_stream_gather(const ChunkGatherParams& p, cudaStream_t stream);
+struct ChunkCropParams {
+  const float* restored;
+  float* kept;
+  int chunks;
+  int64_t keep[VL_MAX_CLIPS + 1];
+  int64_t src[VL_MAX_CLIPS];
+};
+cudaError_t launch_stream_crop(const ChunkCropParams& p, cudaStream_t stream);
+
 struct PlanePtr {
   __half* hi;
   __half* lo;

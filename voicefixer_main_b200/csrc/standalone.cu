@@ -18,20 +18,6 @@ int begin_call(vf_ctx* ctx, const char* fn, bool ok, const char* why = "") {
   return VF_OK;
 }
 
-// Orders this use of `s` after its previous one and grows it to `need` bytes, stream-ordered (no host synchronisation).
-// Once this succeeds, mark_use(ctx, s.order, st) must run on every path, a failed launch included: the sub-batches
-// queued before it read the scratch.
-int acquire_scratch(vf_ctx* ctx, Scratch& s, size_t need, cudaStream_t st) {
-  const int rc = order_use(ctx, s.order, st);
-  if (rc || need <= s.bytes) return rc;
-  if (s.p) CK(cudaFreeAsync(s.p, st));
-  s.p = nullptr;
-  s.bytes = 0;
-  CK(cudaMallocAsync(&s.p, need, st));
-  s.bytes = need;
-  return VF_OK;
-}
-
 // Consecutive sub-batches of a packed set of `batch` items: a sub-batch takes items until it holds max_rows, or until the
 // next item's size_of(i) would take its size past `cap`; an item larger than cap runs alone.  -> the first item of every
 // sub-batch, then `batch`.

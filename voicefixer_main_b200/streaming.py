@@ -1,0 +1,181 @@
+"""Restore many live audio streams at once: chunked boxcar-margin streaming over the engine's vf_restore_chunks.
+
+`StreamingRestorer` runs `BoxcarOverlapAdd(RestoreNet(model, unify_energy), 1, W, M)` (longform.py, the reference's
+tools/dsp/overlapadd_boxcar.py LambdaOverlapAdd) incrementally over streams whose samples arrive while they are restored:
+
+    sr = StreamingRestorer(model, window_size=44100, in_margin=11025)
+    a = sr.open()
+    sr.push(a, samples)             # any number of samples, any split, host or device
+    out = sr.step()                 # {id: the samples restored since the last step}
+    sr.close(a)                     # the rest comes out of the following step()
+
+The chunks and crops are exactly `BoxcarOverlapAdd.plan(n)`'s for a stream of n samples.  Chunk i is restored as soon as
+it is known to be a middle chunk of that plan, i.e. once (i + 1) W + M samples have been pushed (W + M for the first), and
+whatever is left after `close`.  So a stream's concatenated outputs are BoxcarOverlapAdd's result bit for bit, n samples in
+all, however its pushes were split and whichever streams shared its steps: vf_restore_chunks gives each chunk the bits of a
+one-clip restore().
+
+Each stream owns one row of a device ring of 2 (W + 2M) samples.  After a step the ring holds less than W + 2M samples
+still needed by the stream's next chunk, so a push of up to W + 2M samples always fits; a push that would overwrite needed
+samples raises, and the caller must step() first.  Each step is one vf_restore_chunks call: one gather launch builds the
+packed chunks from the rings and one crop launch packs the kept samples, whatever the number of streams.
+"""
+import itertools
+from typing import Dict, List, Optional, Tuple
+
+import torch
+
+from .arch import frames_for, vocoder_out_len
+from .longform import BoxcarOverlapAdd
+
+OPEN = (1 << 63) - 1              # `valid` of a chunk whose stream is still open: no position reads as zero padding
+MAX_CHUNK = 1 << 30               # samples of one clip of vf_restore_varlen (engine.cu check_varlen_call)
+
+
+def restore_rejects(engine, n: int) -> Optional[str]:
+    """Why restore() refuses a clip of n samples (the checks of vf_restore_ex / vf_restore_chunks), or None."""
+    if n <= 1024:
+        return f"{n} samples (reflect padding needs more than 1024)"
+    if n > MAX_CHUNK:
+        return f"{n} samples (one restore takes at most 2^30)"
+    d = vocoder_out_len(frames_for(n), engine.voc_cfg) - n
+    if d < 0 or d == 1:
+        return f"{n} samples (a vocoder output of {n + d} samples, which trim_center cannot cut to {n})"
+    return None
+
+
+class _Stream:
+    __slots__ = ("slot", "pushed", "next", "n")
+
+    def __init__(self, slot: int):
+        self.slot = slot
+        self.pushed = 0           # samples pushed so far (absolute position of the next one)
+        self.next = 0             # index of the next chunk to restore
+        self.n: Optional[int] = None    # total length once closed
+
+
+class StreamingRestorer:
+    """Live streams restored chunk by chunk with `in_margin` samples of context on each side of every `window_size` window.
+
+    model: a VoiceFixer on a CUDA device with weights loaded.  max_streams: the streams that may be open at once (one ring
+    row each).  unify_energy: as restore(unify_energy=...)."""
+
+    def __init__(self, model, window_size: int, in_margin: int, max_streams: int = 64, unify_energy: bool = False):
+        W, M = int(window_size), int(in_margin)
+        if W % 2:
+            raise ValueError("window_size must be even")
+        if not 0 < M < W:
+            raise ValueError("in_margin must be in (0, window_size)")
+        if max_streams < 1:
+            raise ValueError("max_streams must be at least 1")
+        self.engine = model._engine()
+        for n in (W + M, W + 2 * M):            # the first and middle chunks
+            why = restore_rejects(self.engine, n)
+            if why:
+                raise ValueError(f"window_size {W} and in_margin {M} give chunks of {why}")
+        self.window_size, self.in_margin, self.unify_energy = W, M, unify_energy
+        self._ola = BoxcarOverlapAdd(None, 1, W, M)      # plan() is the chunk geometry of a closed stream
+        self.ring_len = 2 * (W + 2 * M)
+        self.ring = torch.zeros(max_streams, self.ring_len, device=self.engine.device)
+        self._free = list(range(max_streams - 1, -1, -1))
+        self._streams: Dict[int, _Stream] = {}
+        self._ids = itertools.count()
+
+    def open(self) -> int:
+        """A new stream; its id is never reused."""
+        if not self._free:
+            raise RuntimeError(f"all {self.ring.shape[0]} streams are open (max_streams)")
+        sid = next(self._ids)
+        self._streams[sid] = _Stream(self._free.pop())
+        return sid
+
+    def _get(self, sid: int, what: str) -> _Stream:
+        st = self._streams.get(sid)
+        if st is None:
+            raise KeyError(f"{what}: no open stream {sid}")
+        if st.n is not None:
+            raise ValueError(f"{what}: stream {sid} is closed")
+        return st
+
+    def _keep_from(self, st: _Stream) -> int:
+        """First absolute position the stream's next chunk reads."""
+        return 0 if st.next == 0 else st.next * self.window_size - self.in_margin
+
+    def push(self, sid: int, samples: torch.Tensor):
+        """Appends 1-D float32 samples (host or device) to stream `sid`'s ring."""
+        st = self._get(sid, "push")
+        if not isinstance(samples, torch.Tensor) or samples.dtype != torch.float32 or samples.dim() != 1:
+            raise TypeError(f"push: stream {sid}: samples must be a 1-D float32 tensor")
+        k, L = samples.numel(), self.ring_len
+        held = st.pushed - self._keep_from(st)
+        if held + k > L:
+            raise OverflowError(f"push: stream {sid}: {k} samples do not fit its ring ({L - held} of {L} free); call step() first")
+        row, p = self.ring[st.slot], st.pushed % L
+        first = min(k, L - p)
+        row[p:p + first].copy_(samples[:first])
+        if k > first:
+            row[:k - first].copy_(samples[first:])
+        st.pushed += k
+
+    def _final_chunks(self, st: _Stream) -> List[Tuple[int, int, int, int]]:
+        """(start, length, crop_left, crop_right) of the chunks of a closed stream not restored yet: BoxcarOverlapAdd.plan(n)
+        from st.next on, the only chunk of a stream of at most W samples cropped to n as ola_forward's final cut does."""
+        plan, _ = self._ola.plan(st.n)
+        out = []
+        for i in range(st.next, len(plan)):
+            start, stop, cl, cr = plan[i]
+            if len(plan) == 1:
+                cr = stop - st.n
+            out.append((start, stop - start, cl, cr))
+        return out
+
+    def _ready_chunks(self, st: _Stream) -> List[Tuple[int, int, int, int]]:
+        """The chunks of an open stream that are middle chunks of its final plan whatever its length: chunk i once (i + 1) W + M
+        samples are in, as the plan's (i W - M, (i + 1) W + M, M, M), or (0, W + M, 0, M) for the first."""
+        W, M = self.window_size, self.in_margin
+        out = []
+        i = st.next
+        while st.pushed >= (i + 1) * W + M:
+            out.append((0, W + M, 0, M) if i == 0 else (i * W - M, W + 2 * M, M, M))
+            i += 1
+        return out
+
+    def close(self, sid: int):
+        """Ends stream `sid`; its remaining samples come out of the next step().  Raises ValueError, and leaves the stream
+        open, when its last chunk is one restore() would refuse (push more samples, then close again)."""
+        st = self._get(sid, "close")
+        st.n = st.pushed
+        for start, length, _, _ in self._final_chunks(st):
+            why = restore_rejects(self.engine, length)
+            if why:
+                st.n = None
+                raise ValueError(f"close: stream {sid}: its last chunk (samples {start} .. {start + length - 1}) has {why}")
+        if st.n == 0:                           # nothing was pushed: nothing to restore
+            self._release(sid)
+
+    def _release(self, sid: int):
+        self._free.append(self._streams.pop(sid).slot)
+
+    def step(self) -> Dict[int, torch.Tensor]:
+        """Restores every ready chunk of every stream in one vf_restore_chunks call -> {id: 1-D device tensor of the samples
+        restored since the last step} for the streams that have any.  A closed stream is gone once its last samples are out."""
+        table, owners = [], []
+        for sid, st in self._streams.items():
+            chunks = self._final_chunks(st) if st.n is not None else self._ready_chunks(st)
+            valid = OPEN if st.n is None else st.n
+            for start, length, cl, cr in chunks:
+                table.append((st.slot, length, cl, cr, start, valid))
+            if chunks:
+                owners.append((sid, len(chunks), sum(length - cl - cr for _, length, cl, cr in chunks)))
+        if not table:
+            return {}
+        kept = self.engine.restore_chunks(self.ring, table, unify_energy=self.unify_energy)
+        out, off = {}, 0
+        for sid, n_chunks, n_kept in owners:
+            out[sid] = kept[off:off + n_kept]
+            off += n_kept
+            st = self._streams[sid]
+            st.next += n_chunks
+            if st.n is not None:
+                self._release(sid)              # a closed stream's step emits all its remaining chunks
+        return out
