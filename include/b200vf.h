@@ -29,6 +29,8 @@
  *   vf_ssr_restore_varlen         the same for clips of different lengths in one call (eval_ssr_unet.py:handler()'s test set)
  *   vf_ssr_restore_varlen_mels    + each clip's output mel and peak normalise, the rest of eval_gsr_unet.py:handler()'s
  *                                 segment loop (handler_unet.handler_batch)
+ *   vf_ssr_restore_chunks         vf_restore_chunks for SSR_UNet / GSR_UNet: live streams of the denoising, declipping,
+ *                                 dereverberation and super-resolution models
  *   vf_istft                      FDomainHelper.istft tools/pytorch/modules/fDomainHelper.py:30-32,127 (torchlibrosa ISTFT)
  *   vf_resample_poly              load_wav's rate conversion, tools/utils.py:46-48
  *   vf_lsd / vf_sispec            AudioMetrics.lsd / .sispec evaluation_proc/metrics.py:83-95 (handler's mel metrics,
@@ -209,6 +211,17 @@ VF_API int vf_ssr_restore_varlen(vf_ctx* ctx, const float* wav, const int64_t* o
 #define VF_SSR_PEAK_NORMALISE 1u
 VF_API int vf_ssr_restore_varlen_mels(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out,
                                       unsigned flags, float* mel_out, void* stream);
+/* vf_restore_chunks for the SSR_UNet / GSR_UNet path: the same ring, vf_chunk table, `valid` zero fill and crops, no flags.
+ * Chunk c's kept samples are bit-identical to vf_ssr_restore (batch 1, same options) on its zero-filled samples, cropped.
+ * Every argument is checked before any work is queued (VF_EINVAL: a stream out of range, length > ring_len, 1024 samples or
+ * fewer, over 2^30, crops that leave nothing, start < 0; there is no trim_center constraint, so a length vf_restore_chunks
+ * refuses only for trim_center is accepted), and a context without the unet_v2 weights (generator.unet.*) fails with
+ * VF_ESTATE; the context stays usable.  One gather launch, the vf_ssr_restore_varlen chain and one crop launch per
+ * sub-batch, with vf_restore_chunks' power-of-two plan shapes and repeated first chunk; the largest sub-batch follows the SSR
+ * plan size per frame, larger than VoiceFixer's.  No peak normalisation: divide a stream by its peak, if at all, after it
+ * has ended.  The scratch is the one vf_restore_chunks uses. */
+VF_API int vf_ssr_restore_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_chunk* chunks,
+                                 int n_chunks, float* kept_out, void* stream);
 /* Same through HOST buffers (pinned for true asynchrony).  The copies and the compute run on library-owned streams with
  * two staging buffer pairs, so back-to-back calls overlap (the H2D of call i+1 and the D2H of call i-1 run under the
  * compute of call i); `stream` only receives a wait on this call's D2H.  Contract: wav_host holds its data when the

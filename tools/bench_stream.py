@@ -1,7 +1,10 @@
 #!/usr/bin/env python
-"""Benchmark of live-stream restoration (StreamingRestorer / vf_restore_chunks) on one GPU.
+"""Benchmark of live-stream restoration (StreamingRestorer / vf_restore_chunks, vf_ssr_restore_chunks) on one GPU.
 
-    python tools/bench_stream.py [--streams 1,8,64,256] [--windows 1,2] [--steps K] [--warmup W]
+    python tools/bench_stream.py [--workload gsr|ssr] [--streams 1,8,64,256] [--windows 1,2] [--steps K] [--warmup W]
+
+--workload gsr (the default) streams through VoiceFixer (ResUNet + vocoder, vf_restore_chunks); ssr through SSR_UNet
+(unet_v2 + ISTFT, vf_ssr_restore_chunks), whose baseline arm calls SSR_UNet.restore_batch (vf_ssr_restore_varlen).
 
 For every window W (seconds) and stream count S: S streams of seeded speech-like audio each push W of samples per step, with
 M = W / 4 samples of context on each side of every window (BoxcarOverlapAdd geometry), so after the first step every step
@@ -9,7 +12,7 @@ restores S middle chunks of W + 2M.  Two arms run alternately in one process on 
 - "streaming": S pushes (device to device, one copy each) + StreamingRestorer.step(): one gather launch, the varlen restore
   chain, one crop launch ("streaming_step_only": the step without the pushes);
 - "torch_slicing": what a server does without it: slices each stream's chunk out of its (device-resident) history, one
-  VoiceFixer.restore_batch call per GROUP streams (torch.cat of the slices + vf_restore_varlen), and crops every result.
+  restore_batch call per GROUP streams (torch.cat of the slices + the varlen restore), and crops every result.
   Its histories are resident from the start, so it pays nothing for receiving the audio.
 Both must give the same bits.  A step is timed with CUDA events around it after a device synchronise; medians are
 reported.  A step is real time when it takes at most W seconds (it restores W of audio per stream).  Prints one JSON line:
@@ -31,10 +34,12 @@ from bench import SR, synth_batch  # noqa: E402
 from bench_varlen import card_info  # noqa: E402
 
 BANK = 8            # distinct synthetic signals; stream s plays signal s % BANK shifted by s * 997 samples
-# restore_batch calls of the baseline take at most this many streams: the sub-batch the streaming arm's plan-shape rule picks
-# for 1 - 2 s windows on an 80 GB card, so both arms run on the same cached plans.  Left to its own split, restore_batch of 256
-# chunks picks other shapes, and the two arms' plans would evict each other on every alternation.
-GROUP = 64
+# restore_batch calls of the baseline take at most this many streams.  gsr: the sub-batch the streaming arm's plan-shape rule
+# picks for 1 - 2 s windows on an 80 GB card, so both arms run on the same cached plans.  ssr (about 1.4 times the plan bytes
+# per frame): a group whose plans stay cached beside the streaming arm's at 1 s windows (at S = 64 on an 80 GB H100, one plan
+# was evicted in the whole run: the first step's).  Left to its own split, restore_batch of 256 chunks picks other shapes,
+# and the two arms' plans would evict each other on every alternation.
+GROUP = {"gsr": 64, "ssr": 16}
 
 
 def timed(fn):
@@ -47,12 +52,13 @@ def timed(fn):
     return out, e0, e1
 
 
-def run_case(state, bank, W, M, S, steps, warmup):
+def run_case(workload, state, bank, W, M, S, steps, warmup):
     """One (W, S) case on a model of its own: a fresh plan cache, so that plans of earlier cases neither crowd the budget nor
     enter its size estimates."""
-    from voicefixer_main_b200 import VoiceFixer
+    from voicefixer_main_b200 import SSR_UNet, VoiceFixer
     from voicefixer_main_b200.streaming import StreamingRestorer
-    model = VoiceFixer().load_state_dict(state).eval().to(bank.device)
+    model = (SSR_UNet if workload == "ssr" else VoiceFixer)().load_state_dict(state).eval().to(bank.device)
+    group = GROUP[workload]
     eng = model._engine()
     xs = [torch.roll(bank[s % BANK], s * 997) for s in range(S)]
     sr = StreamingRestorer(model, W, M, max_streams=S)
@@ -74,8 +80,8 @@ def run_case(state, bank, W, M, S, steps, warmup):
     def torch_slicing(i):
         start, length, cl, cr = chunk(i)
         outs = []
-        for g in range(0, S, GROUP):
-            outs += model.restore_batch([x[start:start + length] for x in xs[g:g + GROUP]])
+        for g in range(0, S, group):
+            outs += model.restore_batch([x[start:start + length] for x in xs[g:g + group]])
         return [o[cl:length - cr] for o in outs]
 
     info0 = eng.plan_cache_info()
@@ -101,13 +107,15 @@ def run_case(state, bank, W, M, S, steps, warmup):
                   "real_time": med <= 1e3 * W / SR}
     return {"window_s": W / SR, "margin_s": M / SR, "streams": S, "arms": res,
             "speedup_vs_torch_slicing": res["torch_slicing"]["ms_per_step_median"] / res["streaming"]["ms_per_step_median"],
-            "bit_identical": bool(same),
+            "bit_identical": bool(same), "baseline_group": group,
             "plans_built": (info1["plans"] + info1["evicted"]) - (info0["plans"] + info0["evicted"]),
             "plans_evicted": info1["evicted"] - info0["evicted"], "plan_cache": info1, "gpu_launches": launches}
 
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--workload", choices=("gsr", "ssr"), default="gsr",
+                    help="gsr: VoiceFixer (vf_restore_chunks); ssr: SSR_UNet (vf_ssr_restore_chunks)")
     ap.add_argument("--streams", default="1,8,64,256")
     ap.add_argument("--windows", default="1,2", help="window lengths in seconds; the margin is a quarter of the window")
     ap.add_argument("--steps", type=int, default=5, help="timed steady-state steps per case")
@@ -115,9 +123,9 @@ def main():
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("tools/bench_stream.py needs a CUDA device")
-    from voicefixer_main_b200.weights import make_state
+    from voicefixer_main_b200.weights import make_ssr_state, make_state
     dev = torch.device("cuda", 0)
-    state = make_state(1234)
+    state = (make_ssr_state if args.workload == "ssr" else make_state)(1234)
     streams = [int(s) for s in args.streams.split(",")]
     cases, best = [], {}
     for w_s in [float(w) for w in args.windows.split(",")]:
@@ -126,7 +134,7 @@ def main():
         n = (args.warmup + args.steps + 1) * W + M
         bank = synth_batch(BANK, n, 4242).to(dev)
         for S in streams:
-            c = run_case(state, bank, W, M, S, args.steps, args.warmup)
+            c = run_case(args.workload, state, bank, W, M, S, args.steps, args.warmup)
             cases.append(c)
             if c["arms"]["streaming"]["real_time"]:
                 best[f"{w_s:g}"] = max(best.get(f"{w_s:g}", 0), S)
@@ -135,7 +143,8 @@ def main():
     line = {"metric": "stream_audio_seconds_per_sec", "value": top["arms"]["streaming"]["audio_seconds_per_sec"], "unit": "audio s/s",
             "higher_is_better": True, "data": "synthetic", "steps": args.steps, "warmup": args.warmup,
             "config": {"workload": "S streams of seeded speech-like audio, each pushing W per step, M = W / 4, 44.1 kHz; value = "
-                                   "the best streaming arm over the cases", "best_case": {"window_s": top["window_s"], "streams": top["streams"]}},
+                                   "the best streaming arm over the cases", "best_case": {"window_s": top["window_s"], "streams": top["streams"]},
+                       "model": "SSR_UNet (vf_ssr_restore_chunks)" if args.workload == "ssr" else "VoiceFixer (vf_restore_chunks)"},
             "largest_real_time_streams": {"window_s=" + k: v for k, v in best.items()},
             "cases": cases, "card": card_info(0)}
     print(json.dumps(line))

@@ -23,7 +23,7 @@ EXPORTS = [
     "vf_restore_varlen", "vf_ssr_restore_varlen", "vf_restore_varlen_mels", "vf_metric_spectrogram", "vf_ssim", "vf_score_varlen",
     "vf_ssr_restore_varlen_mels", "vf_selftest_op", "vf_selftest_gru", "vf_score_time_varlen",
     "vf_sosfiltfilt_varlen", "vf_resample_poly_f64_varlen", "vf_metric_spectrogram_ex", "vf_score_varlen_ex",
-    "vf_score_time_varlen_ex", "vf_restore_chunks",
+    "vf_score_time_varlen_ex", "vf_restore_chunks", "vf_ssr_restore_chunks",
 ]
 VF_RESTORE_UNIFY_ENERGY = 1
 VF_SSR_PEAK_NORMALISE = 1
@@ -152,6 +152,7 @@ def load_library():
     lib.vf_ssr_restore_host.argtypes = [P, P, c_int, c_int64, P, P]
     lib.vf_ssr_restore_varlen.argtypes = [P, P, POINTER(c_int64), c_int, P, P]
     lib.vf_ssr_restore_varlen_mels.argtypes = [P, P, POINTER(c_int64), c_int, P, c_uint, P, P]
+    lib.vf_ssr_restore_chunks.argtypes = [P, P, c_int, c_int64, POINTER(VfChunk), c_int, P, P]
     lib.vf_ssr_unet.argtypes = [P, P, c_int, c_int, P, P]
     lib.vf_ssr_stages.argtypes = [P, c_int, c_int64, P, P, P]
     lib.vf_istft.argtypes = [P, P, P, c_int, c_int, c_int64, P, P]

@@ -578,8 +578,10 @@ int restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t*
   });
 }
 
-// vf_restore_chunks: every check before anything is queued, then per sub-batch one gather from the rings into the packed
-// input scratch, the varlen restore chain into the packed output scratch, and one crop into kept_out.
+// vf_restore_chunks (`fn`, kind PLAN_VARLEN) and vf_ssr_restore_chunks (PLAN_SSR_VARLEN): every check before anything is
+// queued (per_chunk(i, length) for the entry point's own, after the length checks), then per sub-batch one gather from the
+// rings into the packed input scratch, chain(plan, in, rows, n_max, out, off) - the varlen chain of `kind` on the packed
+// chunks at host offsets off[0..rows] - into the packed output scratch, and one crop into kept_out.
 //
 // Plan shapes: a streaming session's chunk count changes from step to step, and varlen plans are keyed by (batch, bucket),
 // so each sub-batch runs on the next power of two of its chunk count.  A sub-batch holds at most the largest power of two P
@@ -587,15 +589,17 @@ int restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t*
 // nine batch shapes per bucket instead of one per chunk count, and they stay cached side by side instead of evicting one
 // another whenever the count crosses a power of two.  The rows past the chunks repeat the sub-batch's first chunk, whose results are discarded: rows are
 // independent, so they change no kept sample, and unlike a row of digital silence they put nothing through the chain that
-// the call's own audio does not.
-int restore_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_chunk* chunks, int n_chunks,
-                   float* kept_out, unsigned flags, cudaStream_t st) {
-  const char* fn = "vf_restore_chunks";
+// the call's own audio does not.  The cap follows the plan size per frame of `kind` (choose_sub_batch): an SSR varlen plan
+// holds about 1.4 times a VoiceFixer one per padded frame, so its cap is reached at shorter chunks.
+template <typename PerChunk, typename Chain>
+int restore_chunks(vf_ctx* ctx, const char* fn, int kind, const float* ring, int n_streams, int64_t ring_len,
+                   const vf_chunk* chunks, int n_chunks, float* kept_out, unsigned flags, unsigned known_flags, cudaStream_t st,
+                   PerChunk per_chunk, Chain chain) {
   int rc = check_ready(ctx);
   if (rc) return rc;
   if (!ring || !chunks || !kept_out || n_streams <= 0 || ring_len <= 0 || n_chunks <= 0) return fail(ctx, VF_EINVAL, "%s: bad arguments", fn);
-  if (flags & ~(unsigned)VF_RESTORE_UNIFY_ENERGY) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
-  rc = check_networks(ctx, PLAN_VARLEN);
+  if (flags & ~known_flags) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
+  rc = check_networks(ctx, kind);
   if (rc) return rc;
   int64_t longest = 0;
   for (int i = 0; i < n_chunks; ++i) {
@@ -607,14 +611,14 @@ int restore_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_l
     if (c.length <= 1024)
       return fail(ctx, VF_EINVAL, "chunk %d: reflect padding needs more than n_fft/2 = 1024 samples (got %d)", i, c.length);
     if (c.length > 1 << 30) return fail(ctx, VF_EINVAL, "chunk %d: %d samples is too long for one restore", i, c.length);
-    rc = check_trim_center(ctx, "chunk", i, c.length);
+    rc = per_chunk(i, (int64_t)c.length);
     if (rc) return rc;
     if (c.crop_left < 0 || c.crop_right < 0 || (int64_t)c.crop_left + c.crop_right >= c.length)
       return fail(ctx, VF_EINVAL, "%s: chunk %d: crops %d and %d leave nothing of %d samples", fn, i, c.crop_left, c.crop_right, c.length);
     if (c.start < 0 || c.start > INT64_MAX - c.length) return fail(ctx, VF_EINVAL, "%s: chunk %d: start %ld is out of range", fn, i, (long)c.start);
     longest = std::max<int64_t>(longest, c.length);
   }
-  const int fit = choose_sub_batch(ctx, PLAN_VARLEN, 2 * VL_MAX_CLIPS, round_up(frames_of(ctx, (long)longest), 64));
+  const int fit = choose_sub_batch(ctx, kind, 2 * VL_MAX_CLIPS, round_up(frames_of(ctx, (long)longest), 64));
   int cap = 1;
   while (cap < VL_MAX_CLIPS && 4 * cap - 1 <= fit) cap *= 2;     // shapes 1, 2, .., 2 cap: 4 cap - 1 rows in all
   auto rows_of = [](int b) { int r = 1; while (r < b) r *= 2; return r; };
@@ -647,11 +651,11 @@ int restore_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_l
         n_max = std::max<int64_t>(n_max, c.length);
       }
       Plan* plan;
-      int r = get_plan(ctx, PLAN_VARLEN, rows, round_up(frames_of(ctx, (long)n_max), 64), &plan);
+      int r = get_plan(ctx, kind, rows, round_up(frames_of(ctx, (long)n_max), 64), &plan);
       if (r) return r;
       CK(launch_stream_gather(g, st));
       ctx->launches++;
-      r = restore_impl(ctx, plan, in, rows, n_max, out, flags, st, g.off);
+      r = chain(plan, in, rows, n_max, out, g.off);
       if (r) return r;
       ChunkCropParams cp;
       memset(&cp, 0, sizeof cp);
@@ -883,7 +887,12 @@ VF_API int vf_restore_varlen_mels(vf_ctx* ctx, const float* wav, const int64_t* 
 
 VF_API int vf_restore_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_chunk* chunks, int n_chunks,
                              float* kept_out, unsigned flags, void* stream) {
-  return restore_chunks(ctx, ring, n_streams, ring_len, chunks, n_chunks, kept_out, flags, (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  return restore_chunks(ctx, "vf_restore_chunks", PLAN_VARLEN, ring, n_streams, ring_len, chunks, n_chunks, kept_out, flags,
+                        VF_RESTORE_UNIFY_ENERGY, st, [&](int i, int64_t n) { return check_trim_center(ctx, "chunk", i, n); },
+                        [&](Plan* plan, const float* in, int rows, int64_t n_max, float* out, const int64_t* off) {
+                          return restore_impl(ctx, plan, in, rows, n_max, out, flags, st, off);
+                        });
 }
 
 VF_API int vf_restore(vf_ctx* ctx, const float* wav, int batch, int64_t n, float* wav_out, void* stream) {
@@ -927,6 +936,16 @@ VF_API int vf_ssr_restore_varlen_mels(vf_ctx* ctx, const float* wav, const int64
                                       unsigned flags, float* mel_out, void* stream) {
   return ssr_restore_varlen(ctx, "vf_ssr_restore_varlen_mels", wav, offsets, batch, wav_out, flags, mel_out,
                             (cudaStream_t)stream);
+}
+
+VF_API int vf_ssr_restore_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_chunk* chunks,
+                                 int n_chunks, float* kept_out, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  return restore_chunks(ctx, "vf_ssr_restore_chunks", PLAN_SSR_VARLEN, ring, n_streams, ring_len, chunks, n_chunks, kept_out,
+                        0u, 0u, st, [](int, int64_t) { return VF_OK; },
+                        [&](Plan* plan, const float* in, int rows, int64_t n_max, float* out, const int64_t* off) {
+                          return ssr_impl(ctx, plan, nullptr, in, rows, n_max, out, st, off);
+                        });
 }
 
 VF_API int vf_ssr_restore_host(vf_ctx* ctx, const float* wav_host, int batch, int64_t n, float* out_host, void* stream) {

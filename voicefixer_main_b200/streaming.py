@@ -19,6 +19,12 @@ Each stream owns one row of a device ring of 2 (W + 2M) samples.  After a step t
 still needed by the stream's next chunk, so a push of up to W + 2M samples always fits; a push that would overwrite needed
 samples raises, and the caller must step() first.  Each step is one vf_restore_chunks call: one gather launch builds the
 packed chunks from the rings and one crop launch packs the kept samples, whatever the number of streams.
+
+The SSR_UNet / GSR_UNet models (denoising, declipping, dereverberation, super-resolution) stream the same way: with one of
+them each step is one vf_ssr_restore_chunks call, the same gather and crop around the unet_v2 + ISTFT chain, and a stream's
+outputs are `BoxcarOverlapAdd(RestoreNet(ssr_model), 1, W, M)`'s.  That path has no unify_energy, and none of the SSR
+handler's peak normalisation either: the handler divides a whole segment by its peak, which a live stream only knows once it
+has ended.
 """
 import itertools
 from typing import Dict, List, Optional, Tuple
@@ -27,17 +33,21 @@ import torch
 
 from .arch import frames_for, vocoder_out_len
 from .longform import BoxcarOverlapAdd
+from .model import SSR_UNet
 
 OPEN = (1 << 63) - 1              # `valid` of a chunk whose stream is still open: no position reads as zero padding
 MAX_CHUNK = 1 << 30               # samples of one clip of vf_restore_varlen (engine.cu check_varlen_call)
 
 
-def restore_rejects(engine, n: int) -> Optional[str]:
-    """Why restore() refuses a clip of n samples (the checks of vf_restore_ex / vf_restore_chunks), or None."""
+def restore_rejects(engine, n: int, ssr: bool = False) -> Optional[str]:
+    """Why restore() refuses a clip of n samples (the checks of vf_restore_ex / vf_restore_chunks), or None.  ssr: the
+    SSR_UNet / GSR_UNet restore() (vf_ssr_restore_chunks), which has no vocoder and so no trim_center constraint."""
     if n <= 1024:
         return f"{n} samples (reflect padding needs more than 1024)"
     if n > MAX_CHUNK:
         return f"{n} samples (one restore takes at most 2^30)"
+    if ssr:
+        return None
     d = vocoder_out_len(frames_for(n), engine.voc_cfg) - n
     if d < 0 or d == 1:
         return f"{n} samples (a vocoder output of {n + d} samples, which trim_center cannot cut to {n})"
@@ -57,8 +67,9 @@ class _Stream:
 class StreamingRestorer:
     """Live streams restored chunk by chunk with `in_margin` samples of context on each side of every `window_size` window.
 
-    model: a VoiceFixer on a CUDA device with weights loaded.  max_streams: the streams that may be open at once (one ring
-    row each).  unify_energy: as restore(unify_energy=...)."""
+    model: a VoiceFixer, SSR_UNet or GSR_UNet on a CUDA device with weights loaded.  max_streams: the streams that may be open
+    at once (one ring row each).  unify_energy: as VoiceFixer.restore(unify_energy=...); an SSR / GSR-UNet model has no such
+    flag, and asking for it raises ValueError."""
 
     def __init__(self, model, window_size: int, in_margin: int, max_streams: int = 64, unify_energy: bool = False):
         W, M = int(window_size), int(in_margin)
@@ -68,9 +79,12 @@ class StreamingRestorer:
             raise ValueError("in_margin must be in (0, window_size)")
         if max_streams < 1:
             raise ValueError("max_streams must be at least 1")
+        self.ssr = isinstance(model, SSR_UNet)          # GSR_UNet too
+        if self.ssr and unify_energy:
+            raise ValueError("unify_energy is a VoiceFixer option; SSR_UNet / GSR_UNet restore without it")
         self.engine = model._engine()
         for n in (W + M, W + 2 * M):            # the first and middle chunks
-            why = restore_rejects(self.engine, n)
+            why = restore_rejects(self.engine, n, self.ssr)
             if why:
                 raise ValueError(f"window_size {W} and in_margin {M} give chunks of {why}")
         self.window_size, self.in_margin, self.unify_energy = W, M, unify_energy
@@ -146,7 +160,7 @@ class StreamingRestorer:
         st = self._get(sid, "close")
         st.n = st.pushed
         for start, length, _, _ in self._final_chunks(st):
-            why = restore_rejects(self.engine, length)
+            why = restore_rejects(self.engine, length, self.ssr)
             if why:
                 st.n = None
                 raise ValueError(f"close: stream {sid}: its last chunk (samples {start} .. {start + length - 1}) has {why}")
@@ -157,8 +171,9 @@ class StreamingRestorer:
         self._free.append(self._streams.pop(sid).slot)
 
     def step(self) -> Dict[int, torch.Tensor]:
-        """Restores every ready chunk of every stream in one vf_restore_chunks call -> {id: 1-D device tensor of the samples
-        restored since the last step} for the streams that have any.  A closed stream is gone once its last samples are out."""
+        """Restores every ready chunk of every stream in one vf_restore_chunks call (vf_ssr_restore_chunks for an SSR / GSR-UNet
+        model) -> {id: 1-D device tensor of the samples restored since the last step} for the streams that have any.  A
+        closed stream is gone once its last samples are out."""
         table, owners = [], []
         for sid, st in self._streams.items():
             chunks = self._final_chunks(st) if st.n is not None else self._ready_chunks(st)
@@ -169,7 +184,10 @@ class StreamingRestorer:
                 owners.append((sid, len(chunks), sum(length - cl - cr for _, length, cl, cr in chunks)))
         if not table:
             return {}
-        kept = self.engine.restore_chunks(self.ring, table, unify_energy=self.unify_energy)
+        if self.ssr:
+            kept = self.engine.ssr_restore_chunks(self.ring, table)
+        else:
+            kept = self.engine.restore_chunks(self.ring, table, unify_energy=self.unify_energy)
         out, off = {}, 0
         for sid, n_chunks, n_kept in owners:
             out[sid] = kept[off:off + n_kept]
