@@ -31,6 +31,10 @@
  *                                 segment loop (handler_unet.handler_batch)
  *   vf_ssr_restore_chunks         vf_restore_chunks for SSR_UNet / GSR_UNet: live streams of the denoising, declipping,
  *                                 dereverberation and super-resolution models
+ *   vf_restore_windows            the windows of many live streams, gathered from device rings, weighted by a synthesis
+ *                                 window and overlap-added into caller-owned accumulators on the device: the windowed
+ *                                 LambdaOverlapAdd (tools/dsp/overlapadd.py:338-484) run incrementally
+ *   vf_ssr_restore_windows        vf_restore_windows for SSR_UNet / GSR_UNet
  *   vf_istft                      FDomainHelper.istft tools/pytorch/modules/fDomainHelper.py:30-32,127 (torchlibrosa ISTFT)
  *   vf_resample_poly              load_wav's rate conversion, tools/utils.py:46-48
  *   vf_lsd / vf_sispec            AudioMetrics.lsd / .sispec evaluation_proc/metrics.py:83-95 (handler's mel metrics,
@@ -222,6 +226,44 @@ VF_API int vf_ssr_restore_varlen_mels(vf_ctx* ctx, const float* wav, const int64
  * has ended.  The scratch is the one vf_restore_chunks uses. */
 VF_API int vf_ssr_restore_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_chunk* chunks,
                                  int n_chunks, float* kept_out, void* stream);
+/* Windows of live audio streams, restored, weighted and overlap-added in one call (windowed streaming,
+ * voicefixer_main_b200/streaming.py WindowedStreamingRestorer).  ring / ring_len / n_streams as in vf_restore_chunks.
+ * windows: HOST table of n_windows entries (read during the call only); window w reads positions start .. start + W - 1 of
+ * stream `stream` (W = window_len), where positions below 0 and at or past `valid` read as 0 (start may be as low as -W: the
+ * W zeros F.unfold(padding=W) puts before the signal).  synthesis: [W] device fp32 (the synthesis window, or W times
+ * 1 / (W / hop) for the unweighted average).  acc [n_streams, acc_len] (device, caller-owned, zero where nothing is pending):
+ * output position t of stream s accumulates at acc[s * acc_len + t mod acc_len].  For every window, in table order, each
+ * position t in [max(0, start), min(valid, start + W)) gets acc += fl(synthesis[t - start] * restored[t - start]) (the product
+ * rounded, then the add), restored being vf_restore_ex (batch 1, same flags) of the window's zero-filled samples: with one
+ * stream's windows in ascending start, each position sums its windows in ascending order from 0, as F.fold does on CUDA.
+ * Then emits: HOST table of n_emits ranges, at most one per stream; range e copies positions start .. start + count - 1 of
+ * its stream out of acc to `out` (device; may be NULL when no range holds samples), range after range, and zeroes their
+ * slots.  A stream's pending span is
+ * [start, start + acc_len) of its emission range; every window needs one for its stream.  Every argument is checked before
+ * any work is queued (VF_EINVAL: a stream out of range; W > ring_len; a W vf_restore_ex refuses; no synthesis table; a
+ * window start below -W; windows of one stream not in strictly ascending start; a window with no emission range for its
+ * stream, or writing outside the stream's pending span; a second range for a stream, start < 0, count < 0 or count >
+ * acc_len); the context stays usable.  One gather launch, the vf_restore_varlen chain and one overlap-add launch per
+ * sub-batch (sub-batches, plan shapes and scratch as in vf_restore_chunks), then one emission launch per 256 ranges that
+ * hold samples.  The library keeps no stream state: the rings and accumulators are the caller's. */
+typedef struct vf_window {
+  int32_t stream;
+  int64_t start;
+  int64_t valid;
+} vf_window;
+typedef struct vf_emit {
+  int32_t stream;
+  int64_t start;
+  int64_t count;
+} vf_emit;
+VF_API int vf_restore_windows(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_window* windows,
+                              int n_windows, int window_len, const float* synthesis, float* acc, int64_t acc_len,
+                              const vf_emit* emits, int n_emits, float* out, unsigned flags, void* stream);
+/* vf_restore_windows for the SSR_UNet / GSR_UNet path: no flags, the window's restored samples are vf_ssr_restore's (batch
+ * 1), no trim_center constraint on W, and a context without the unet_v2 weights fails with VF_ESTATE. */
+VF_API int vf_ssr_restore_windows(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_window* windows,
+                                  int n_windows, int window_len, const float* synthesis, float* acc, int64_t acc_len,
+                                  const vf_emit* emits, int n_emits, float* out, void* stream);
 /* Same through HOST buffers (pinned for true asynchrony).  The copies and the compute run on library-owned streams with
  * two staging buffer pairs, so back-to-back calls overlap (the H2D of call i+1 and the D2H of call i-1 run under the
  * compute of call i); `stream` only receives a wait on this call's D2H.  Contract: wav_host holds its data when the

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Benchmark of live-stream restoration (StreamingRestorer / vf_restore_chunks, vf_ssr_restore_chunks) on one GPU.
 
-    python tools/bench_stream.py [--workload gsr|ssr] [--streams 1,8,64,256] [--windows 1,2] [--steps K] [--warmup W]
+    python tools/bench_stream.py [--workload gsr|ssr] [--ola boxcar|windowed [--hop-div 2]] [--streams 1,8,64,256]
+                                 [--windows 1,2] [--steps K] [--warmup W]
 
 --workload gsr (the default) streams through VoiceFixer (ResUNet + vocoder, vf_restore_chunks); ssr through SSR_UNet
 (unet_v2 + ISTFT, vf_ssr_restore_chunks), whose baseline arm calls SSR_UNet.restore_batch (vf_ssr_restore_varlen).
@@ -14,6 +15,11 @@ restores S middle chunks of W + 2M.  Two arms run alternately in one process on 
 - "torch_slicing": what a server does without it: slices each stream's chunk out of its (device-resident) history, one
   restore_batch call per GROUP streams (torch.cat of the slices + the varlen restore), and crops every result.
   Its histories are resident from the start, so it pays nothing for receiving the audio.
+With --ola windowed the streams run WindowedStreamingRestorer (vf_restore_windows / vf_ssr_restore_windows) instead:
+hann-weighted windows of W every hop = W / hop_div, each stream still pushing W per step, so a steady-state step restores
+hop_div windows per stream and emits W samples of each.  Its baseline arm ("torch_windowed") slices the ready windows out of
+the zero-led resident histories, restores them with restore_batch GROUP at a time, multiplies them by the synthesis window
+and adds them into per-stream output buffers in ascending window order with torch, then cuts out the finished samples.
 Both must give the same bits.  A step is timed with CUDA events around it after a device synchronise; medians are
 reported.  A step is real time when it takes at most W seconds (it restores W of audio per stream).  Prints one JSON line:
 per (W, S) the step times, audio seconds restored per second and the plans built and evicted; per W the largest S that
@@ -112,10 +118,81 @@ def run_case(workload, state, bank, W, M, S, steps, warmup):
             "plans_evicted": info1["evicted"] - info0["evicted"], "plan_cache": info1, "gpu_launches": launches}
 
 
+def run_case_windowed(workload, state, bank, W, hop, S, steps, warmup):
+    """One (W, S) case of the windowed scheme on a model of its own (see run_case)."""
+    import torch.nn.functional as F
+    from voicefixer_main_b200 import SSR_UNet, VoiceFixer
+    from voicefixer_main_b200.streaming import WindowedStreamingRestorer
+    model = (SSR_UNet if workload == "ssr" else VoiceFixer)().load_state_dict(state).eval().to(bank.device)
+    group = GROUP[workload]
+    eng = model._engine()
+    xs = [torch.roll(bank[s % BANK], s * 997) for s in range(S)]
+    sr = WindowedStreamingRestorer(model, W, hop, max_streams=S)
+    ids = [sr.open() for _ in range(S)]
+    syn = sr.synthesis
+    xps = [F.pad(x, (W, 0)) for x in xs]                    # window k = xp[k hop : k hop + W]
+    accs = [torch.zeros(x.numel(), device=bank.device) for x in xs]
+    state_b = {"next": 1, "emitted": 0}
+    pushed = torch.cuda.Event(enable_timing=True)
+
+    def streaming(i):
+        for sid, x in zip(ids, xs):
+            sr.push(sid, x[i * W:(i + 1) * W])
+        pushed.record()
+        out = sr.step()
+        return [out[sid] for sid in ids]
+
+    def torch_windowed(i):
+        k0, k1 = state_b["next"], (i + 1) * W // hop + 1           # the windows ready once (i + 1) W samples are in
+        slices = [xp[k * hop:k * hop + W] for xp in xps for k in range(k0, k1)]
+        ys = []
+        for g in range(0, len(slices), group):
+            ys += model.restore_batch(slices[g:g + group])
+        nk = k1 - k0
+        for s in range(S):
+            for j, k in enumerate(range(k0, k1)):
+                lo, hi = max(0, k * hop - W), k * hop
+                y = ys[s * nk + j] * syn
+                accs[s][lo:hi] = accs[s][lo:hi] + y[lo - (k * hop - W):]
+        a, b = state_b["emitted"], max(0, k1 * hop - W)
+        state_b["next"], state_b["emitted"] = k1, b
+        return [acc[a:b] for acc in accs]
+
+    info0 = eng.plan_cache_info()
+    ms = {"streaming": [], "streaming_step_only": [], "torch_windowed": []}
+    same = True
+    for i in range(warmup + steps):
+        a, a0, a1 = timed(lambda: streaming(i))
+        b, b0, b1 = timed(lambda: torch_windowed(i))
+        same = same and all(torch.equal(p, q) for p, q in zip(a, b))
+        if i >= warmup:
+            ms["streaming"].append(a0.elapsed_time(a1))
+            ms["streaming_step_only"].append(pushed.elapsed_time(a1))
+            ms["torch_windowed"].append(b0.elapsed_time(b1))
+    eng.check_errors()
+    info1 = eng.plan_cache_info()
+    launches = eng.launch_count()
+    eng.close()
+    audio_s = S * W / SR                                      # emitted audio per steady-state step
+    res = {}
+    for k, v in ms.items():
+        med = sorted(v)[len(v) // 2]
+        res[k] = {"ms_per_step_median": med, "ms_min": min(v), "ms_max": max(v), "audio_seconds_per_sec": audio_s / (med * 1e-3),
+                  "real_time": med <= 1e3 * W / SR}
+    return {"window_s": W / SR, "hop_s": hop / SR, "streams": S, "arms": res,
+            "speedup_vs_torch_windowed": res["torch_windowed"]["ms_per_step_median"] / res["streaming"]["ms_per_step_median"],
+            "bit_identical": bool(same), "baseline_group": group,
+            "plans_built": (info1["plans"] + info1["evicted"]) - (info0["plans"] + info0["evicted"]),
+            "plans_evicted": info1["evicted"] - info0["evicted"], "plan_cache": info1, "gpu_launches": launches}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--workload", choices=("gsr", "ssr"), default="gsr",
                     help="gsr: VoiceFixer (vf_restore_chunks); ssr: SSR_UNet (vf_ssr_restore_chunks)")
+    ap.add_argument("--ola", choices=("boxcar", "windowed"), default="boxcar",
+                    help="boxcar: StreamingRestorer, M = W / 4; windowed: WindowedStreamingRestorer, hann, hop = W / hop-div")
+    ap.add_argument("--hop-div", type=int, default=2, help="windowed: hop = W / hop-div")
     ap.add_argument("--streams", default="1,8,64,256")
     ap.add_argument("--windows", default="1,2", help="window lengths in seconds; the margin is a quarter of the window")
     ap.add_argument("--steps", type=int, default=5, help="timed steady-state steps per case")
@@ -134,7 +211,10 @@ def main():
         n = (args.warmup + args.steps + 1) * W + M
         bank = synth_batch(BANK, n, 4242).to(dev)
         for S in streams:
-            c = run_case(args.workload, state, bank, W, M, S, args.steps, args.warmup)
+            if args.ola == "windowed":
+                c = run_case_windowed(args.workload, state, bank, W, W // args.hop_div, S, args.steps, args.warmup)
+            else:
+                c = run_case(args.workload, state, bank, W, M, S, args.steps, args.warmup)
             cases.append(c)
             if c["arms"]["streaming"]["real_time"]:
                 best[f"{w_s:g}"] = max(best.get(f"{w_s:g}", 0), S)
@@ -142,9 +222,12 @@ def main():
     top = max(cases, key=lambda c: c["arms"]["streaming"]["audio_seconds_per_sec"])
     line = {"metric": "stream_audio_seconds_per_sec", "value": top["arms"]["streaming"]["audio_seconds_per_sec"], "unit": "audio s/s",
             "higher_is_better": True, "data": "synthetic", "steps": args.steps, "warmup": args.warmup,
-            "config": {"workload": "S streams of seeded speech-like audio, each pushing W per step, M = W / 4, 44.1 kHz; value = "
-                                   "the best streaming arm over the cases", "best_case": {"window_s": top["window_s"], "streams": top["streams"]},
-                       "model": "SSR_UNet (vf_ssr_restore_chunks)" if args.workload == "ssr" else "VoiceFixer (vf_restore_chunks)"},
+            "config": {"workload": "S streams of seeded speech-like audio, each pushing W per step, "
+                                   + (f"hann windows every W / {args.hop_div}" if args.ola == "windowed" else "M = W / 4")
+                                   + ", 44.1 kHz; value = the best streaming arm over the cases",
+                       "best_case": {"window_s": top["window_s"], "streams": top["streams"]}, "ola": args.ola,
+                       "model": ("SSR_UNet (vf_ssr_restore_" if args.workload == "ssr" else "VoiceFixer (vf_restore_")
+                                + ("windows)" if args.ola == "windowed" else "chunks)")},
             "largest_real_time_streams": {"window_s=" + k: v for k, v in best.items()},
             "cases": cases, "card": card_info(0)}
     print(json.dumps(line))

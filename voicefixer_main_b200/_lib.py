@@ -23,7 +23,7 @@ EXPORTS = [
     "vf_restore_varlen", "vf_ssr_restore_varlen", "vf_restore_varlen_mels", "vf_metric_spectrogram", "vf_ssim", "vf_score_varlen",
     "vf_ssr_restore_varlen_mels", "vf_selftest_op", "vf_selftest_gru", "vf_score_time_varlen",
     "vf_sosfiltfilt_varlen", "vf_resample_poly_f64_varlen", "vf_metric_spectrogram_ex", "vf_score_varlen_ex",
-    "vf_score_time_varlen_ex", "vf_restore_chunks", "vf_ssr_restore_chunks",
+    "vf_score_time_varlen_ex", "vf_restore_chunks", "vf_ssr_restore_chunks", "vf_restore_windows", "vf_ssr_restore_windows",
 ]
 VF_RESTORE_UNIFY_ENERGY = 1
 VF_SSR_PEAK_NORMALISE = 1
@@ -87,6 +87,16 @@ class VfChunk(Structure):
     """vf_chunk (include/b200vf.h): one chunk of a vf_restore_chunks call."""
     _fields_ = [("stream", c_int32), ("length", c_int32), ("crop_left", c_int32), ("crop_right", c_int32),
                 ("start", c_int64), ("valid", c_int64)]
+
+
+class VfWindow(Structure):
+    """vf_window (include/b200vf.h): one window of a vf_restore_windows call."""
+    _fields_ = [("stream", c_int32), ("start", c_int64), ("valid", c_int64)]
+
+
+class VfEmit(Structure):
+    """vf_emit (include/b200vf.h): one stream's emission range of a vf_restore_windows call."""
+    _fields_ = [("stream", c_int32), ("start", c_int64), ("count", c_int64)]
 
 
 class EngineError(RuntimeError):
@@ -153,6 +163,10 @@ def load_library():
     lib.vf_ssr_restore_varlen.argtypes = [P, P, POINTER(c_int64), c_int, P, P]
     lib.vf_ssr_restore_varlen_mels.argtypes = [P, P, POINTER(c_int64), c_int, P, c_uint, P, P]
     lib.vf_ssr_restore_chunks.argtypes = [P, P, c_int, c_int64, POINTER(VfChunk), c_int, P, P]
+    lib.vf_restore_windows.argtypes = [P, P, c_int, c_int64, POINTER(VfWindow), c_int, c_int, P, P, c_int64, POINTER(VfEmit),
+                                       c_int, P, c_uint, P]
+    lib.vf_ssr_restore_windows.argtypes = [P, P, c_int, c_int64, POINTER(VfWindow), c_int, c_int, P, P, c_int64,
+                                           POINTER(VfEmit), c_int, P, P]
     lib.vf_ssr_unet.argtypes = [P, P, c_int, c_int, P, P]
     lib.vf_ssr_stages.argtypes = [P, c_int, c_int64, P, P, P]
     lib.vf_istft.argtypes = [P, P, P, c_int, c_int, c_int64, P, P]

@@ -578,19 +578,177 @@ int restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t*
   });
 }
 
-// vf_restore_chunks (`fn`, kind PLAN_VARLEN) and vf_ssr_restore_chunks (PLAN_SSR_VARLEN): every check before anything is
-// queued (per_chunk(i, length) for the entry point's own, after the length checks), then per sub-batch one gather from the
-// rings into the packed input scratch, chain(plan, in, rows, n_max, out, off) - the varlen chain of `kind` on the packed
-// chunks at host offsets off[0..rows] - into the packed output scratch, and one crop into kept_out.
+// One row of a streaming call: `length` samples of stream `stream` from position `start` on; positions below 0 (a window's
+// leading padding) and at or past `valid` (the stream's end) read as 0.
+struct StreamRow {
+  int stream;
+  int64_t length, start, valid;
+};
+
+// The output stage of vf_restore_chunks: per sub-batch, one crop of its chunks' kept samples into kept_out, chunk after chunk.
+struct CropStage {
+  const vf_chunk* chunks;
+  float* kept_out;
+  int64_t kept_off;
+  int sub_batch(vf_ctx* ctx, int s, int b, const int64_t* off, const float* restored, cudaStream_t st) {
+    ChunkCropParams cp;
+    memset(&cp, 0, sizeof cp);
+    cp.restored = restored; cp.kept = kept_out + kept_off; cp.chunks = b;
+    for (int k = 0; k < b; ++k) {
+      const vf_chunk& c = chunks[s + k];
+      cp.src[k] = off[k] + c.crop_left;
+      cp.keep[k + 1] = cp.keep[k] + c.length - c.crop_left - c.crop_right;
+    }
+    CK(launch_stream_crop(cp, st));
+    ctx->launches++;
+    kept_off += cp.keep[b];
+    return VF_OK;
+  }
+  int finish(vf_ctx*, cudaStream_t) { return VF_OK; }
+};
+
+// The output stage of vf_restore_windows: per sub-batch, one overlap-add of its windows into the accumulators, the windows of
+// each stream one run in table order (ascending start: the checks saw to it), windows that read only padding left out (they
+// change no output); after the last sub-batch, the emission of the finished ranges, one launch per VL_MAX_CLIPS ranges that
+// hold samples.
+struct OlaStage {
+  const vf_window* windows;
+  int W;
+  const float* synth;
+  float* acc;
+  int64_t acc_len;
+  const vf_emit* emits;
+  int n_emits;
+  float* out;
+  int sub_batch(vf_ctx* ctx, int s, int b, const int64_t* off, const float* restored, cudaStream_t st) {
+    std::vector<int> order(b);
+    for (int k = 0; k < b; ++k) order[k] = k;
+    std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return windows[s + x].stream < windows[s + y].stream; });
+    WindowOlaParams p;
+    memset(&p, 0, sizeof p);
+    p.restored = restored; p.synth = synth; p.acc = acc; p.acc_len = acc_len; p.W = W;
+    int n = 0, cur = -1;
+    for (int k : order) {
+      const vf_window& w = windows[s + k];
+      const int64_t lo = std::max<int64_t>(0, w.start), hi = std::min<int64_t>(w.valid, w.start + W);
+      if (lo >= hi) continue;
+      if (w.stream != cur) {                        // the stream's run begins at its first contributing window
+        cur = w.stream;
+        p.first[p.runs] = n;
+        p.lo[p.runs] = lo;
+        p.acc_row[p.runs] = (int64_t)w.stream * acc_len;
+        p.acc_phase[p.runs] = lo % acc_len;
+        p.pos[p.runs + 1] = p.pos[p.runs];
+        p.runs++;
+      }
+      const int r = p.runs - 1;
+      p.start[n] = w.start; p.end[n] = hi; p.src[n] = off[k];
+      p.first[r + 1] = ++n;
+      p.pos[r + 1] = std::max(p.pos[r + 1], p.pos[r] + hi - p.lo[r]);
+    }
+    if (p.runs == 0) return VF_OK;
+    CK(launch_window_ola(p, st));
+    ctx->launches++;
+    return VF_OK;
+  }
+  int finish(vf_ctx* ctx, cudaStream_t st) {
+    WindowEmitParams p;
+    memset(&p, 0, sizeof p);
+    p.acc = acc; p.out = out; p.acc_len = acc_len;
+    auto flush = [&]() -> int {
+      if (p.n == 0) return VF_OK;
+      CK(launch_window_emit(p, st));
+      ctx->launches++;
+      p.out += p.off[p.n];
+      p.n = 0;
+      return VF_OK;
+    };
+    for (int e = 0; e < n_emits; ++e) {
+      if (emits[e].count == 0) continue;
+      p.row[p.n] = (int64_t)emits[e].stream * acc_len;
+      p.phase[p.n] = emits[e].start % acc_len;
+      p.off[p.n + 1] = p.off[p.n] + emits[e].count;
+      if (++p.n == VL_MAX_CLIPS) {
+        const int r = flush();
+        if (r) return r;
+      }
+    }
+    return flush();
+  }
+};
+
+// The streaming calls after their checks: per sub-batch one gather from the rings into the packed input scratch, chain(plan,
+// in, rows, n_max, out, off) - the varlen chain of `kind` on the packed rows at host offsets off[0..rows] - into the packed
+// output scratch, and stage.sub_batch on the restored rows; then stage.finish.
 //
-// Plan shapes: a streaming session's chunk count changes from step to step, and varlen plans are keyed by (batch, bucket),
-// so each sub-batch runs on the next power of two of its chunk count.  A sub-batch holds at most the largest power of two P
+// Plan shapes: a streaming session's row count changes from step to step, and varlen plans are keyed by (batch, bucket),
+// so each sub-batch runs on the next power of two of its row count.  A sub-batch holds at most the largest power of two P
 // (and VL_MAX_CLIPS) whose shapes 1, 2, 4, .., P fit the plan budget together (2P - 1 rows): a session then meets at most
-// nine batch shapes per bucket instead of one per chunk count, and they stay cached side by side instead of evicting one
-// another whenever the count crosses a power of two.  The rows past the chunks repeat the sub-batch's first chunk, whose results are discarded: rows are
-// independent, so they change no kept sample, and unlike a row of digital silence they put nothing through the chain that
-// the call's own audio does not.  The cap follows the plan size per frame of `kind` (choose_sub_batch): an SSR varlen plan
-// holds about 1.4 times a VoiceFixer one per padded frame, so its cap is reached at shorter chunks.
+// nine batch shapes per bucket instead of one per row count, and they stay cached side by side instead of evicting one
+// another whenever the count crosses a power of two.  The rows past the sub-batch's own repeat its first row, whose results
+// are discarded: rows are independent, so they change no output sample, and unlike a row of digital silence they put nothing
+// through the chain that the call's own audio does not.  The cap follows the plan size per frame of `kind`
+// (choose_sub_batch): an SSR varlen plan holds about 1.4 times a VoiceFixer one per padded frame, so its cap is reached at
+// shorter rows.
+template <typename Stage, typename Chain>
+int run_stream_rows(vf_ctx* ctx, int kind, const float* ring, int64_t ring_len, const std::vector<StreamRow>& rows_in,
+                    Stage& stage, cudaStream_t st, Chain chain) {
+  const int n_rows = (int)rows_in.size();
+  int64_t longest = 0;
+  for (const StreamRow& r : rows_in) longest = std::max(longest, r.length);
+  const int fit = choose_sub_batch(ctx, kind, 2 * VL_MAX_CLIPS, round_up(frames_of(ctx, (long)longest), 64));
+  int cap = 1;
+  while (cap < VL_MAX_CLIPS && 4 * cap - 1 <= fit) cap *= 2;     // shapes 1, 2, .., 2 cap: 4 cap - 1 rows in all
+  auto rows_of = [](int b) { int r = 1; while (r < b) r *= 2; return r; };
+  auto row_at = [&](int s, int b, int k) -> const StreamRow& { return rows_in[s + (k < b ? k : 0)]; };
+  int64_t max_samples = 0;
+  for (int s = 0; s < n_rows; s += cap) {
+    const int b = std::min(cap, n_rows - s);
+    int64_t n = 0;
+    for (int k = 0; k < rows_of(b); ++k) n += row_at(s, b, k).length;
+    max_samples = std::max(max_samples, n);
+  }
+  int rc = acquire_scratch(ctx, ctx->chunks, (size_t)max_samples * 2 * sizeof(float), st);
+  if (rc) return rc;
+  float* in = static_cast<float*>(ctx->chunks.p);
+  float* out = in + max_samples;
+  auto run = [&]() -> int {
+    for (int s = 0; s < n_rows; s += cap) {
+      const int b = std::min(cap, n_rows - s), rows = rows_of(b);
+      ChunkGatherParams g;
+      memset(&g, 0, sizeof g);
+      g.ring = ring; g.out = in; g.ring_len = ring_len; g.rows = rows;
+      int64_t n_max = 0;
+      for (int k = 0; k < rows; ++k) {
+        const StreamRow& c = row_at(s, b, k);
+        g.off[k + 1] = g.off[k] + c.length;
+        g.src[k] = (int64_t)c.stream * ring_len;
+        g.phase[k] = (c.start % ring_len + ring_len) % ring_len;
+        g.lead[k] = c.start < 0 ? std::min<int64_t>(c.length, -c.start) : 0;
+        // valid - start would overflow for an open stream (valid = INT64_MAX) and a window start below 0
+        g.n_valid[k] = c.valid <= c.start ? 0 : c.valid - c.length >= c.start ? c.length : c.valid - c.start;
+        n_max = std::max<int64_t>(n_max, c.length);
+      }
+      Plan* plan;
+      int r = get_plan(ctx, kind, rows, round_up(frames_of(ctx, (long)n_max), 64), &plan);
+      if (r) return r;
+      CK(launch_stream_gather(g, st));
+      ctx->launches++;
+      r = chain(plan, in, rows, n_max, out, g.off);
+      if (r) return r;
+      r = stage.sub_batch(ctx, s, b, g.off, out, st);
+      if (r) return r;
+    }
+    return stage.finish(ctx, st);
+  };
+  rc = run();
+  const int rm = mark_use(ctx, ctx->chunks.order, st);
+  return rc ? rc : rm;
+}
+
+// vf_restore_chunks (`fn`, kind PLAN_VARLEN) and vf_ssr_restore_chunks (PLAN_SSR_VARLEN): every check before anything is
+// queued (per_chunk(i, length) for the entry point's own, after the length checks), then run_stream_rows with the crop into
+// kept_out.
 template <typename PerChunk, typename Chain>
 int restore_chunks(vf_ctx* ctx, const char* fn, int kind, const float* ring, int n_streams, int64_t ring_len,
                    const vf_chunk* chunks, int n_chunks, float* kept_out, unsigned flags, unsigned known_flags, cudaStream_t st,
@@ -601,7 +759,7 @@ int restore_chunks(vf_ctx* ctx, const char* fn, int kind, const float* ring, int
   if (flags & ~known_flags) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
   rc = check_networks(ctx, kind);
   if (rc) return rc;
-  int64_t longest = 0;
+  std::vector<StreamRow> rows(n_chunks);
   for (int i = 0; i < n_chunks; ++i) {
     const vf_chunk& c = chunks[i];
     if (c.stream < 0 || c.stream >= n_streams)
@@ -616,64 +774,68 @@ int restore_chunks(vf_ctx* ctx, const char* fn, int kind, const float* ring, int
     if (c.crop_left < 0 || c.crop_right < 0 || (int64_t)c.crop_left + c.crop_right >= c.length)
       return fail(ctx, VF_EINVAL, "%s: chunk %d: crops %d and %d leave nothing of %d samples", fn, i, c.crop_left, c.crop_right, c.length);
     if (c.start < 0 || c.start > INT64_MAX - c.length) return fail(ctx, VF_EINVAL, "%s: chunk %d: start %ld is out of range", fn, i, (long)c.start);
-    longest = std::max<int64_t>(longest, c.length);
+    rows[i] = StreamRow{c.stream, c.length, c.start, c.valid};
   }
-  const int fit = choose_sub_batch(ctx, kind, 2 * VL_MAX_CLIPS, round_up(frames_of(ctx, (long)longest), 64));
-  int cap = 1;
-  while (cap < VL_MAX_CLIPS && 4 * cap - 1 <= fit) cap *= 2;     // shapes 1, 2, .., 2 cap: 4 cap - 1 rows in all
-  auto rows_of = [](int b) { int r = 1; while (r < b) r *= 2; return r; };
-  auto row_chunk = [&](int s, int b, int k) -> const vf_chunk& { return chunks[s + (k < b ? k : 0)]; };
-  int64_t max_samples = 0;
-  for (int s = 0; s < n_chunks; s += cap) {
-    const int b = std::min(cap, n_chunks - s);
-    int64_t n = 0;
-    for (int k = 0; k < rows_of(b); ++k) n += row_chunk(s, b, k).length;
-    max_samples = std::max(max_samples, n);
-  }
-  rc = acquire_scratch(ctx, ctx->chunks, (size_t)max_samples * 2 * sizeof(float), st);
+  CropStage stage{chunks, kept_out, 0};
+  return run_stream_rows(ctx, kind, ring, ring_len, rows, stage, st, chain);
+}
+
+// vf_restore_windows (`fn`, kind PLAN_VARLEN) and vf_ssr_restore_windows (PLAN_SSR_VARLEN): every check before anything is
+// queued (per_len(W) for the entry point's own, after the length checks), then run_stream_rows with the overlap-add and
+// the emission.  A stream's pending span is [start, start + acc_len) of its emission range: every accumulator slot a window
+// writes or the emission reads must lie in it, so no live partial sum of another position is overwritten.
+template <typename PerLen, typename Chain>
+int restore_windows(vf_ctx* ctx, const char* fn, int kind, const float* ring, int n_streams, int64_t ring_len,
+                    const vf_window* windows, int n_windows, int W, const float* synthesis, float* acc, int64_t acc_len,
+                    const vf_emit* emits, int n_emits, float* out, unsigned flags, unsigned known_flags, cudaStream_t st,
+                    PerLen per_len, Chain chain) {
+  int rc = check_ready(ctx);
   if (rc) return rc;
-  float* in = static_cast<float*>(ctx->chunks.p);
-  float* out = in + max_samples;
-  auto run = [&]() -> int {
-    int64_t kept_off = 0;
-    for (int s = 0; s < n_chunks; s += cap) {
-      const int b = std::min(cap, n_chunks - s), rows = rows_of(b);
-      ChunkGatherParams g;
-      memset(&g, 0, sizeof g);
-      g.ring = ring; g.out = in; g.ring_len = ring_len; g.rows = rows;
-      int64_t n_max = 0;
-      for (int k = 0; k < rows; ++k) {
-        const vf_chunk& c = row_chunk(s, b, k);
-        g.off[k + 1] = g.off[k] + c.length;
-        g.src[k] = (int64_t)c.stream * ring_len;
-        g.phase[k] = c.start % ring_len;
-        g.n_valid[k] = c.valid <= c.start ? 0 : std::min<int64_t>(c.length, c.valid - c.start);
-        n_max = std::max<int64_t>(n_max, c.length);
-      }
-      Plan* plan;
-      int r = get_plan(ctx, kind, rows, round_up(frames_of(ctx, (long)n_max), 64), &plan);
-      if (r) return r;
-      CK(launch_stream_gather(g, st));
-      ctx->launches++;
-      r = chain(plan, in, rows, n_max, out, g.off);
-      if (r) return r;
-      ChunkCropParams cp;
-      memset(&cp, 0, sizeof cp);
-      cp.restored = out; cp.kept = kept_out + kept_off; cp.chunks = b;
-      for (int k = 0; k < b; ++k) {
-        const vf_chunk& c = chunks[s + k];
-        cp.src[k] = g.off[k] + c.crop_left;
-        cp.keep[k + 1] = cp.keep[k] + c.length - c.crop_left - c.crop_right;
-      }
-      CK(launch_stream_crop(cp, st));
-      ctx->launches++;
-      kept_off += cp.keep[b];
-    }
-    return VF_OK;
-  };
-  rc = run();
-  const int rm = mark_use(ctx, ctx->chunks.order, st);
-  return rc ? rc : rm;
+  if (!ring || !windows || !acc || !emits || n_streams <= 0 || ring_len <= 0 || n_windows <= 0 || acc_len <= 0 ||
+      n_emits <= 0)
+    return fail(ctx, VF_EINVAL, "%s: bad arguments", fn);
+  if (!synthesis) return fail(ctx, VF_EINVAL, "%s: no synthesis window table", fn);
+  if (flags & ~known_flags) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
+  rc = check_networks(ctx, kind);
+  if (rc) return rc;
+  if (W > ring_len) return fail(ctx, VF_EINVAL, "%s: windows of %d samples do not fit a ring of %ld", fn, W, (long)ring_len);
+  if (W <= 1024) return fail(ctx, VF_EINVAL, "%s: reflect padding needs more than n_fft/2 = 1024 samples (windows of %d)", fn, W);
+  if (W > 1 << 30) return fail(ctx, VF_EINVAL, "%s: windows of %d samples are too long for one restore", fn, W);
+  rc = per_len((int64_t)W);
+  if (rc) return rc;
+  std::vector<int64_t> from(n_streams, -1);         // each stream's pending span begins at its emission range
+  for (int e = 0; e < n_emits; ++e) {
+    const vf_emit& r = emits[e];
+    if (r.stream < 0 || r.stream >= n_streams)
+      return fail(ctx, VF_EINVAL, "%s: emission %d: stream %d is not in 0 .. %d", fn, e, r.stream, n_streams - 1);
+    if (from[r.stream] >= 0) return fail(ctx, VF_EINVAL, "%s: emission %d: stream %d has a second emission range", fn, e, r.stream);
+    if (r.start < 0 || r.start > INT64_MAX - acc_len || r.count < 0 || r.count > acc_len)
+      return fail(ctx, VF_EINVAL, "%s: emission %d: %ld samples from %ld leave stream %d's pending span of %ld", fn, e,
+                  (long)r.count, (long)r.start, r.stream, (long)acc_len);
+    from[r.stream] = r.start;
+    if (r.count > 0 && !out) return fail(ctx, VF_EINVAL, "%s: bad arguments (no output for emission %d)", fn, e);
+  }
+  std::vector<int64_t> last(n_streams, INT64_MIN);
+  std::vector<StreamRow> rows(n_windows);
+  for (int i = 0; i < n_windows; ++i) {
+    const vf_window& w = windows[i];
+    if (w.stream < 0 || w.stream >= n_streams)
+      return fail(ctx, VF_EINVAL, "%s: window %d: stream %d is not in 0 .. %d", fn, i, w.stream, n_streams - 1);
+    if (w.start < -(int64_t)W || w.start > INT64_MAX - W)
+      return fail(ctx, VF_EINVAL, "%s: window %d: start %ld is out of range", fn, i, (long)w.start);
+    if (w.start <= last[w.stream])
+      return fail(ctx, VF_EINVAL, "%s: window %d: start %ld of stream %d does not follow its previous window's %ld", fn, i,
+                  (long)w.start, w.stream, (long)last[w.stream]);
+    last[w.stream] = w.start;
+    if (from[w.stream] < 0) return fail(ctx, VF_EINVAL, "%s: window %d: stream %d has no emission range", fn, i, w.stream);
+    const int64_t lo = std::max<int64_t>(0, w.start), hi = std::min<int64_t>(w.valid, w.start + W);
+    if (lo < hi && (lo < from[w.stream] || hi - from[w.stream] > acc_len))
+      return fail(ctx, VF_EINVAL, "%s: window %d: samples %ld .. %ld leave stream %d's pending span %ld .. %ld", fn, i,
+                  (long)lo, (long)hi - 1, w.stream, (long)from[w.stream], (long)(from[w.stream] + acc_len - 1));
+    rows[i] = StreamRow{w.stream, W, w.start, w.valid};
+  }
+  OlaStage stage{windows, W, synthesis, acc, acc_len, emits, n_emits, out};
+  return run_stream_rows(ctx, kind, ring, ring_len, rows, stage, st, chain);
 }
 
 // vf_ssr_restore_varlen (`fn`) and vf_ssr_restore_varlen_mels.  After each sub-batch's ISTFT, still inside the plan's use on
@@ -895,6 +1057,18 @@ VF_API int vf_restore_chunks(vf_ctx* ctx, const float* ring, int n_streams, int6
                         });
 }
 
+VF_API int vf_restore_windows(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_window* windows,
+                              int n_windows, int window_len, const float* synthesis, float* acc, int64_t acc_len,
+                              const vf_emit* emits, int n_emits, float* out, unsigned flags, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  return restore_windows(ctx, "vf_restore_windows", PLAN_VARLEN, ring, n_streams, ring_len, windows, n_windows, window_len,
+                         synthesis, acc, acc_len, emits, n_emits, out, flags, VF_RESTORE_UNIFY_ENERGY, st,
+                         [&](int64_t n) { return check_trim_center(ctx, "window", 0, n); },
+                         [&](Plan* plan, const float* in, int rows, int64_t n_max, float* o, const int64_t* off) {
+                           return restore_impl(ctx, plan, in, rows, n_max, o, flags, st, off);
+                         });
+}
+
 VF_API int vf_restore(vf_ctx* ctx, const float* wav, int batch, int64_t n, float* wav_out, void* stream) {
   return vf_restore_ex(ctx, wav, batch, n, wav_out, ctx && ctx->unify_energy ? VF_RESTORE_UNIFY_ENERGY : 0u, stream);
 }
@@ -946,6 +1120,17 @@ VF_API int vf_ssr_restore_chunks(vf_ctx* ctx, const float* ring, int n_streams, 
                         [&](Plan* plan, const float* in, int rows, int64_t n_max, float* out, const int64_t* off) {
                           return ssr_impl(ctx, plan, nullptr, in, rows, n_max, out, st, off);
                         });
+}
+
+VF_API int vf_ssr_restore_windows(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_window* windows,
+                                  int n_windows, int window_len, const float* synthesis, float* acc, int64_t acc_len,
+                                  const vf_emit* emits, int n_emits, float* out, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  return restore_windows(ctx, "vf_ssr_restore_windows", PLAN_SSR_VARLEN, ring, n_streams, ring_len, windows, n_windows,
+                         window_len, synthesis, acc, acc_len, emits, n_emits, out, 0u, 0u, st, [](int64_t) { return VF_OK; },
+                         [&](Plan* plan, const float* in, int rows, int64_t n_max, float* o, const int64_t* off) {
+                           return ssr_impl(ctx, plan, nullptr, in, rows, n_max, o, st, off);
+                         });
 }
 
 VF_API int vf_ssr_restore_host(vf_ctx* ctx, const float* wav_host, int batch, int64_t n, float* out_host, void* stream) {

@@ -59,11 +59,12 @@ struct MelGatherParams {
 };
 cudaError_t launch_gather_mels(const MelGatherParams& p, cudaStream_t stream);
 
-// vf_restore_chunks (stream.cu): the chunk tables of one sub-batch, kernel parameters like the lengths table's offsets.
-// Gather: packed sample off[c] + j (j < off[c + 1] - off[c]) of row c is ring[src[c] + (phase[c] + j) mod ring_len] when
-// j < n_valid[c], else 0 (src: the row's stream times ring_len; phase: start mod ring_len; n_valid: the samples before the
-// stream's end).  Crop: kept sample keep[c] + j (j < keep[c + 1] - keep[c]) of chunk c is restored[src[c] + j] (src: the
-// chunk's packed offset plus its crop_left).
+// vf_restore_chunks and vf_restore_windows (stream.cu): the tables of one sub-batch, kernel parameters like the lengths
+// table's offsets.  Gather: packed sample off[c] + j (j < off[c + 1] - off[c]) of row c is ring[src[c] + (phase[c] + j) mod
+// ring_len] when lead[c] <= j < n_valid[c], else 0 (src: the row's stream times ring_len; phase: start mod ring_len, in
+// [0, ring_len); lead: the samples before position 0, 0 for a chunk; n_valid: the samples before the stream's end).  Crop:
+// kept sample keep[c] + j (j < keep[c + 1] - keep[c]) of chunk c is restored[src[c] + j] (src: the chunk's packed offset
+// plus its crop_left).
 struct ChunkGatherParams {
   const float* ring;
   float* out;
@@ -72,6 +73,7 @@ struct ChunkGatherParams {
   int64_t off[VL_MAX_CLIPS + 1];
   int64_t src[VL_MAX_CLIPS];
   int64_t phase[VL_MAX_CLIPS];
+  int64_t lead[VL_MAX_CLIPS];
   int64_t n_valid[VL_MAX_CLIPS];
 };
 cudaError_t launch_stream_gather(const ChunkGatherParams& p, cudaStream_t stream);
@@ -83,6 +85,39 @@ struct ChunkCropParams {
   int64_t src[VL_MAX_CLIPS];
 };
 cudaError_t launch_stream_crop(const ChunkCropParams& p, cudaStream_t stream);
+// vf_restore_windows' overlap-add of one sub-batch.  Its windows are grouped into runs, one per stream, each run's windows in
+// ascending start.  Thread pos[r] + i handles output position t = lo[r] + i of run r: for every window w in first[r] ..
+// first[r + 1] - 1 with start[w] <= t < end[w], in that order, acc[acc_row[r] + t mod acc_len] += fl(synth[t - start[w]] *
+// restored[src[w] + t - start[w]]) (acc_row: the stream times acc_len; acc_phase: lo mod acc_len; end: min(start + W, the
+// stream's valid); src: the window's packed offset).
+struct WindowOlaParams {
+  const float* restored;
+  const float* synth;
+  float* acc;
+  int64_t acc_len;
+  int W, runs;
+  int64_t pos[VL_MAX_CLIPS + 1];
+  int64_t lo[VL_MAX_CLIPS];
+  int64_t acc_row[VL_MAX_CLIPS];
+  int64_t acc_phase[VL_MAX_CLIPS];
+  int first[VL_MAX_CLIPS + 1];
+  int64_t start[VL_MAX_CLIPS];
+  int64_t end[VL_MAX_CLIPS];
+  int64_t src[VL_MAX_CLIPS];
+};
+cudaError_t launch_window_ola(const WindowOlaParams& p, cudaStream_t stream);
+// vf_restore_windows' emission: packed sample off[e] + j (j < off[e + 1] - off[e]) is acc[row[e] + (phase[e] + j) mod
+// acc_len], which is then zeroed (row: the stream times acc_len; phase: the range's start mod acc_len).
+struct WindowEmitParams {
+  float* acc;
+  float* out;
+  int64_t acc_len;
+  int n;
+  int64_t off[VL_MAX_CLIPS + 1];
+  int64_t row[VL_MAX_CLIPS];
+  int64_t phase[VL_MAX_CLIPS];
+};
+cudaError_t launch_window_emit(const WindowEmitParams& p, cudaStream_t stream);
 
 struct PlanePtr {
   __half* hi;

@@ -1,9 +1,11 @@
-// The two data-movement kernels of vf_restore_chunks (include/b200vf.h): the gather that builds a step's packed input from
-// the streams' device rings, and the crop that keeps each chunk's centre of the packed restored output.  Between them runs
-// the varlen restore chain (engine.cu).  Each is one launch per sub-batch of at most VL_MAX_CLIPS chunks, whatever the
-// number of streams: the chunk table is a __grid_constant__ kernel parameter (about 8 KB for the gather at 256 rows), so
-// no host memory is read after the call returns and no copy of the table is queued.  One thread per packed sample; a
-// warp's threads nearly always fall into one chunk, so the table lookups broadcast.
+// The data-movement kernels of vf_restore_chunks and vf_restore_windows (include/b200vf.h): the gather that builds a step's
+// packed input from the streams' device rings, and either the crop that keeps each chunk's centre of the packed restored
+// output (chunks) or the overlap-add of each synthesis-weighted window into the caller's per-stream accumulators followed by
+// the emission of the finished samples (windows).  Between the gather and the output stage runs the varlen restore chain
+// (engine.cu).  Each is one launch per sub-batch of at most VL_MAX_CLIPS rows (the emission: per VL_MAX_CLIPS streams),
+// whatever the number of streams: the tables are __grid_constant__ kernel parameters (about 10 KB for the gather, 13 KB for
+// the overlap-add at 256 rows), so no host memory is read after the call returns and no copy of a table is queued.  One
+// thread per packed or accumulated sample; a warp's threads nearly always fall into one row, so the table lookups broadcast.
 #include "kernels.cuh"
 
 namespace vf {
@@ -29,8 +31,8 @@ __global__ void __launch_bounds__(STREAM_THREADS) stream_gather_kernel(const __g
   if (i >= p.off[p.rows]) return;
   const int c = find_row(p.off, p.rows, i);
   const int64_t j = i - p.off[c];
-  float v = 0.f;                                   // past the stream's end: BoxcarOverlapAdd's zero padding
-  if (j < p.n_valid[c]) {
+  float v = 0.f;                                   // before position 0 or past the stream's end: the zero padding
+  if (j >= p.lead[c] && j < p.n_valid[c]) {
     int64_t r = p.phase[c] + j;                    // j < length <= ring_len, so one subtraction wraps it
     if (r >= p.ring_len) r -= p.ring_len;
     v = __ldg(p.ring + p.src[c] + r);
@@ -45,6 +47,42 @@ __global__ void __launch_bounds__(STREAM_THREADS) stream_crop_kernel(const __gri
   p.kept[i] = __ldg(p.restored + p.src[c] + (i - p.keep[c]));
 }
 
+// Ascending window order per position, and the product rounded before the add (no FMA contraction): the bits of F.fold
+// (CUDA col2im: each output starts at 0 and adds the windows in ascending order) of the rounded `frames * window` tensor.
+// The accumulator carries the partial sum from call to call, so the order holds across sub-batches and steps too.
+__global__ void __launch_bounds__(STREAM_THREADS) window_ola_kernel(const __grid_constant__ WindowOlaParams p) {
+  const int64_t i = (int64_t)blockIdx.x * STREAM_THREADS + threadIdx.x;
+  if (i >= p.pos[p.runs]) return;
+  const int r = find_row(p.pos, p.runs, i);
+  const int64_t t = p.lo[r] + (i - p.pos[r]);
+  int lo = p.first[r], hi = p.first[r + 1];        // the first window with start + W > t: the earliest that covers t
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (p.start[mid] + p.W <= t) lo = mid + 1; else hi = mid;
+  }
+  int64_t slot = p.acc_phase[r] + (i - p.pos[r]);  // a run spans at most acc_len positions, so one subtraction wraps it
+  if (slot >= p.acc_len) slot -= p.acc_len;
+  float* a = p.acc + p.acc_row[r] + slot;
+  float v = *a;
+  for (int w = lo; w < p.first[r + 1] && p.start[w] <= t; ++w) {
+    if (t >= p.end[w]) continue;                   // past the stream's end
+    const int64_t j = t - p.start[w];
+    v = __fadd_rn(v, __fmul_rn(__ldg(p.synth + j), __ldg(p.restored + p.src[w] + j)));
+  }
+  *a = v;
+}
+
+__global__ void __launch_bounds__(STREAM_THREADS) window_emit_kernel(const __grid_constant__ WindowEmitParams p) {
+  const int64_t i = (int64_t)blockIdx.x * STREAM_THREADS + threadIdx.x;
+  if (i >= p.off[p.n]) return;
+  const int e = find_row(p.off, p.n, i);
+  int64_t r = p.phase[e] + (i - p.off[e]);         // count <= acc_len, so one subtraction wraps it
+  if (r >= p.acc_len) r -= p.acc_len;
+  float* a = p.acc + p.row[e] + r;
+  p.out[i] = *a;
+  *a = 0.f;                                        // the slot is free for a later position, or a later stream
+}
+
 cudaError_t launch_stream_gather(const ChunkGatherParams& p, cudaStream_t stream) {
   const int64_t n = p.off[p.rows];
   stream_gather_kernel<<<(unsigned)((n + STREAM_THREADS - 1) / STREAM_THREADS), STREAM_THREADS, 0, stream>>>(p);
@@ -54,6 +92,18 @@ cudaError_t launch_stream_gather(const ChunkGatherParams& p, cudaStream_t stream
 cudaError_t launch_stream_crop(const ChunkCropParams& p, cudaStream_t stream) {
   const int64_t n = p.keep[p.chunks];
   stream_crop_kernel<<<(unsigned)((n + STREAM_THREADS - 1) / STREAM_THREADS), STREAM_THREADS, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_window_ola(const WindowOlaParams& p, cudaStream_t stream) {
+  const int64_t n = p.pos[p.runs];
+  window_ola_kernel<<<(unsigned)((n + STREAM_THREADS - 1) / STREAM_THREADS), STREAM_THREADS, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_window_emit(const WindowEmitParams& p, cudaStream_t stream) {
+  const int64_t n = p.off[p.n];
+  window_emit_kernel<<<(unsigned)((n + STREAM_THREADS - 1) / STREAM_THREADS), STREAM_THREADS, 0, stream>>>(p);
   return cudaGetLastError();
 }
 

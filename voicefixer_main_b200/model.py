@@ -261,6 +261,50 @@ class Engine:
                                                     _ptr(out), _stream()))
         return out
 
+    def restore_windows(self, ring: torch.Tensor, windows, window_len: int, synthesis: torch.Tensor, acc: torch.Tensor,
+                        emits, unify_energy: bool = False) -> torch.Tensor:
+        """Windows of live streams restored, weighted and overlap-added in one call (vf_restore_windows).  ring as in
+        restore_chunks; windows is a sequence of (stream, start, valid): positions start .. start + window_len - 1, those below
+        0 or >= valid read as 0.  Each window's restore() output times `synthesis` ([window_len] float32) is added, rounded
+        product by product, into acc [n_streams, acc_len] (stream s's position t at acc[s, t % acc_len]) over positions
+        [max(0, start), min(valid, start + window_len)).  Then emits, a sequence of (stream, start, count), copies each
+        stream's finished positions out of acc and zeroes them.  Returns the emitted samples, packed in emits order."""
+        ring, acc, synthesis, rows, ems, out = self._windows_args(ring, windows, window_len, synthesis, acc, emits)
+        flags = L.VF_RESTORE_UNIFY_ENERGY if unify_energy else 0
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_restore_windows(self.ctx, _ptr(ring), ring.shape[0], ring.shape[1], rows, len(windows),
+                                                 int(window_len), _ptr(synthesis), _ptr(acc), acc.shape[1], ems, len(emits),
+                                                 _ptr(out), flags, _stream()))
+        return out
+
+    def ssr_restore_windows(self, ring: torch.Tensor, windows, window_len: int, synthesis: torch.Tensor, acc: torch.Tensor,
+                            emits) -> torch.Tensor:
+        """restore_windows for the SSR / GSR-UNet path (vf_ssr_restore_windows): each window's output is
+        ssr_forward(None, window[None])[0] of the zero-filled window."""
+        ring, acc, synthesis, rows, ems, out = self._windows_args(ring, windows, window_len, synthesis, acc, emits)
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_ssr_restore_windows(self.ctx, _ptr(ring), ring.shape[0], ring.shape[1], rows, len(windows),
+                                                     int(window_len), _ptr(synthesis), _ptr(acc), acc.shape[1], ems,
+                                                     len(emits), _ptr(out), _stream()))
+        return out
+
+    def _windows_args(self, ring, windows, window_len, synthesis, acc, emits):
+        """Checked ring, accumulators and synthesis table, the host vf_window / vf_emit tables and the packed output of a
+        windows call."""
+        ring = _check_in(ring, self.device, "ring")
+        _check_in(acc, self.device, "acc")
+        if not acc.is_contiguous():
+            raise ValueError("acc must be contiguous: the call updates it in place")
+        if ring.dim() != 2 or acc.dim() != 2 or acc.shape[0] != ring.shape[0]:
+            raise ValueError("ring must be [n_streams, ring_len] and acc [n_streams, acc_len]")
+        if synthesis is not None:
+            synthesis = _check_in(synthesis, self.device, "synthesis")
+            if synthesis.dim() != 1 or synthesis.numel() != int(window_len):
+                raise ValueError("synthesis must be [window_len]")
+        rows = (L.VfWindow * max(1, len(windows)))(*[L.VfWindow(*map(int, t)) for t in windows])
+        ems = (L.VfEmit * max(1, len(emits)))(*[L.VfEmit(*map(int, t)) for t in emits])
+        return ring, acc, synthesis, rows, ems, torch.empty(sum(max(0, int(t[2])) for t in emits), device=self.device)
+
     def _chunks_args(self, ring: torch.Tensor, table):
         """Checked ring, the host vf_chunk table and the packed output of a chunks call."""
         ring = _check_in(ring, self.device, "ring")

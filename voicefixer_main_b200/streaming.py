@@ -25,6 +25,12 @@ them each step is one vf_ssr_restore_chunks call, the same gather and crop aroun
 outputs are `BoxcarOverlapAdd(RestoreNet(ssr_model), 1, W, M)`'s.  That path has no unify_energy, and none of the SSR
 handler's peak normalisation either: the handler divides a whole segment by its peak, which a live stream only knows once it
 has ended.
+
+`WindowedStreamingRestorer` runs the reference's other long-form scheme, `WindowedOverlapAdd(RestoreNet(model, unify_energy),
+1, W, hop, window)` (longform.py, tools/dsp/overlapadd.py's LambdaOverlapAdd), incrementally the same way: windows of W
+samples every hop, each restored, multiplied by the synthesis window and overlap-added, so adjacent windows cross-fade.
+Each step is one vf_restore_windows call (vf_ssr_restore_windows): the gather, the restore chain, one overlap-add launch
+per sub-batch into per-stream device accumulators, and one launch that emits the finished samples.
 """
 import itertools
 from typing import Dict, List, Optional, Tuple
@@ -32,7 +38,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from .arch import frames_for, vocoder_out_len
-from .longform import BoxcarOverlapAdd
+from .longform import BoxcarOverlapAdd, WindowedOverlapAdd
 from .model import SSR_UNet
 
 OPEN = (1 << 63) - 1              # `valid` of a chunk whose stream is still open: no position reads as zero padding
@@ -55,42 +61,33 @@ def restore_rejects(engine, n: int, ssr: bool = False) -> Optional[str]:
 
 
 class _Stream:
-    __slots__ = ("slot", "pushed", "next", "n")
+    __slots__ = ("slot", "pushed", "next", "n", "emitted")
 
-    def __init__(self, slot: int):
+    def __init__(self, slot: int, first: int = 0):
         self.slot = slot
         self.pushed = 0           # samples pushed so far (absolute position of the next one)
-        self.next = 0             # index of the next chunk to restore
+        self.next = first         # index of the next chunk / window to restore
         self.n: Optional[int] = None    # total length once closed
+        self.emitted = 0          # windowed: samples emitted so far
 
 
-class StreamingRestorer:
-    """Live streams restored chunk by chunk with `in_margin` samples of context on each side of every `window_size` window.
+class _RingStreams:
+    """The stream lifecycle and device ring shared by the streaming restorers: open / push / close bookkeeping, one ring row of
+    ring_len samples per stream.  A subclass says from which position a stream's samples are still needed (_keep_from)."""
+    _first = 0                    # _Stream.next of a new stream
 
-    model: a VoiceFixer, SSR_UNet or GSR_UNet on a CUDA device with weights loaded.  max_streams: the streams that may be open
-    at once (one ring row each).  unify_energy: as VoiceFixer.restore(unify_energy=...); an SSR / GSR-UNet model has no such
-    flag, and asking for it raises ValueError."""
-
-    def __init__(self, model, window_size: int, in_margin: int, max_streams: int = 64, unify_energy: bool = False):
-        W, M = int(window_size), int(in_margin)
-        if W % 2:
-            raise ValueError("window_size must be even")
-        if not 0 < M < W:
-            raise ValueError("in_margin must be in (0, window_size)")
+    def _init_model(self, model, unify_energy: bool, max_streams: int):
         if max_streams < 1:
             raise ValueError("max_streams must be at least 1")
         self.ssr = isinstance(model, SSR_UNet)          # GSR_UNet too
         if self.ssr and unify_energy:
             raise ValueError("unify_energy is a VoiceFixer option; SSR_UNet / GSR_UNet restore without it")
         self.engine = model._engine()
-        for n in (W + M, W + 2 * M):            # the first and middle chunks
-            why = restore_rejects(self.engine, n, self.ssr)
-            if why:
-                raise ValueError(f"window_size {W} and in_margin {M} give chunks of {why}")
-        self.window_size, self.in_margin, self.unify_energy = W, M, unify_energy
-        self._ola = BoxcarOverlapAdd(None, 1, W, M)      # plan() is the chunk geometry of a closed stream
-        self.ring_len = 2 * (W + 2 * M)
-        self.ring = torch.zeros(max_streams, self.ring_len, device=self.engine.device)
+        self.unify_energy = unify_energy
+
+    def _init_ring(self, ring_len: int, max_streams: int):
+        self.ring_len = ring_len
+        self.ring = torch.zeros(max_streams, ring_len, device=self.engine.device)
         self._free = list(range(max_streams - 1, -1, -1))
         self._streams: Dict[int, _Stream] = {}
         self._ids = itertools.count()
@@ -100,7 +97,7 @@ class StreamingRestorer:
         if not self._free:
             raise RuntimeError(f"all {self.ring.shape[0]} streams are open (max_streams)")
         sid = next(self._ids)
-        self._streams[sid] = _Stream(self._free.pop())
+        self._streams[sid] = _Stream(self._free.pop(), self._first)
         return sid
 
     def _get(self, sid: int, what: str) -> _Stream:
@@ -112,8 +109,7 @@ class StreamingRestorer:
         return st
 
     def _keep_from(self, st: _Stream) -> int:
-        """First absolute position the stream's next chunk reads."""
-        return 0 if st.next == 0 else st.next * self.window_size - self.in_margin
+        raise NotImplementedError
 
     def push(self, sid: int, samples: torch.Tensor):
         """Appends 1-D float32 samples (host or device) to stream `sid`'s ring."""
@@ -130,6 +126,36 @@ class StreamingRestorer:
         if k > first:
             row[:k - first].copy_(samples[first:])
         st.pushed += k
+
+    def _release(self, sid: int):
+        self._free.append(self._streams.pop(sid).slot)
+
+
+class StreamingRestorer(_RingStreams):
+    """Live streams restored chunk by chunk with `in_margin` samples of context on each side of every `window_size` window.
+
+    model: a VoiceFixer, SSR_UNet or GSR_UNet on a CUDA device with weights loaded.  max_streams: the streams that may be open
+    at once (one ring row each).  unify_energy: as VoiceFixer.restore(unify_energy=...); an SSR / GSR-UNet model has no such
+    flag, and asking for it raises ValueError."""
+
+    def __init__(self, model, window_size: int, in_margin: int, max_streams: int = 64, unify_energy: bool = False):
+        W, M = int(window_size), int(in_margin)
+        if W % 2:
+            raise ValueError("window_size must be even")
+        if not 0 < M < W:
+            raise ValueError("in_margin must be in (0, window_size)")
+        self._init_model(model, unify_energy, max_streams)
+        for n in (W + M, W + 2 * M):            # the first and middle chunks
+            why = restore_rejects(self.engine, n, self.ssr)
+            if why:
+                raise ValueError(f"window_size {W} and in_margin {M} give chunks of {why}")
+        self.window_size, self.in_margin = W, M
+        self._ola = BoxcarOverlapAdd(None, 1, W, M)      # plan() is the chunk geometry of a closed stream
+        self._init_ring(2 * (W + 2 * M), max_streams)
+
+    def _keep_from(self, st: _Stream) -> int:
+        """First absolute position the stream's next chunk reads."""
+        return 0 if st.next == 0 else st.next * self.window_size - self.in_margin
 
     def _final_chunks(self, st: _Stream) -> List[Tuple[int, int, int, int]]:
         """(start, length, crop_left, crop_right) of the chunks of a closed stream not restored yet: BoxcarOverlapAdd.plan(n)
@@ -167,9 +193,6 @@ class StreamingRestorer:
         if st.n == 0:                           # nothing was pushed: nothing to restore
             self._release(sid)
 
-    def _release(self, sid: int):
-        self._free.append(self._streams.pop(sid).slot)
-
     def step(self) -> Dict[int, torch.Tensor]:
         """Restores every ready chunk of every stream in one vf_restore_chunks call (vf_ssr_restore_chunks for an SSR / GSR-UNet
         model) -> {id: 1-D device tensor of the samples restored since the last step} for the streams that have any.  A
@@ -196,4 +219,98 @@ class StreamingRestorer:
             st.next += n_chunks
             if st.n is not None:
                 self._release(sid)              # a closed stream's step emits all its remaining chunks
+        return out
+
+
+class WindowedStreamingRestorer(_RingStreams):
+    """Live streams restored as `WindowedOverlapAdd(RestoreNet(model, unify_energy), 1, window_size, hop_size, window=window,
+    reorder_chunks=False)` restores a whole signal: window k reads positions [k hop - W, k hop) (zero before 0 and past the
+    stream's end), is restored, weighted by the synthesis window (or by 1 / (W / hop) when window is None) and overlap-added.
+
+    Window k is ready once k hop samples are in; it is then a window of the final plan whatever the stream's length.  Window
+    0 reads only padding and the last one, when hop divides n + W, only samples past n: neither contributes to any output,
+    so neither is restored.  Output sample t is final once the windows up to floor((t + W) / hop) (or the last) are added,
+    so a sample leaves at most W samples after it arrives.  Each sample goes through the network W / hop times.
+
+    Each stream owns one row of a device ring of 2W samples and one row of an accumulator of 2W partial sums.  After a step a
+    stream holds fewer than W samples still needed by its next window, so a push of up to W samples always fits; a push
+    that would overwrite needed samples raises OverflowError, and the caller must step() first.  model, max_streams and
+    unify_energy as for StreamingRestorer."""
+    _first = 1                    # window 0 contributes nothing
+
+    def __init__(self, model, window_size: int, hop_size: Optional[int] = None, window="hanning", max_streams: int = 64,
+                 unify_energy: bool = False):
+        W = int(window_size)
+        hop = W // 2 if hop_size is None else int(hop_size)
+        if W % 2:
+            raise ValueError("window_size must be even")
+        if not 0 < hop <= W:
+            raise ValueError("hop_size must be in (0, window_size]")
+        self._init_model(model, unify_energy, max_streams)
+        why = restore_rejects(self.engine, W, self.ssr)
+        if why:
+            raise ValueError(f"window_size {W} gives windows of {why}")
+        self.window_size, self.hop_size = W, hop
+        ola = WindowedOverlapAdd(None, 1, W, hop, window=window, reorder_chunks=False)
+        if ola.use_window:
+            synth = ola.window
+        else:                     # frames / (W / hop) on the device: a product with the fp32 reciprocal of the fp32 divisor
+            synth = torch.full((W,), float(torch.tensor(1.0) / torch.tensor(W / hop, dtype=torch.float32)))
+        self.synthesis = synth.to(self.engine.device)
+        self._init_ring(2 * W, max_streams)
+        self.acc = torch.zeros(max_streams, 2 * W, device=self.engine.device)
+
+    def _keep_from(self, st: _Stream) -> int:
+        """First absolute position the stream's next window reads; also the stream's first sample not emitted yet."""
+        return max(0, st.next * self.hop_size - self.window_size)
+
+    def _windows(self, st: _Stream) -> List[int]:
+        """Indices of the windows to add now: on an open stream the ready ones (k hop <= pushed), on a closed one all that
+        are left and contribute (k hop - W < n)."""
+        W, hop = self.window_size, self.hop_size
+        k, out = st.next, []
+        while (k * hop <= st.pushed) if st.n is None else (k * hop - W < st.n):
+            out.append(k)
+            k += 1
+        return out
+
+    def close(self, sid: int):
+        """Ends stream `sid`; its remaining samples come out of the next step()."""
+        st = self._get(sid, "close")
+        st.n = st.pushed
+        if not self._windows(st):                # nothing left to add: everything is out already
+            self._release(sid)
+
+    def step(self) -> Dict[int, torch.Tensor]:
+        """Restores every window ready to be added of every stream, adds it into the stream's accumulator and emits the
+        samples that are final, in one vf_restore_windows call (vf_ssr_restore_windows for an SSR / GSR-UNet model) ->
+        {id: 1-D device tensor of the samples finished since the last step} for the streams that have any.  A closed stream
+        is gone once its last samples are out."""
+        W, hop = self.window_size, self.hop_size
+        windows, emits, owners = [], [], []
+        for sid, st in self._streams.items():
+            ks = self._windows(st)
+            if not ks:
+                continue
+            valid = OPEN if st.n is None else st.n
+            windows += [(st.slot, k * hop - W, valid) for k in ks]
+            end = st.n if st.n is not None else max(0, (ks[-1] + 1) * hop - W)
+            emits.append((st.slot, st.emitted, end - st.emitted))
+            owners.append((sid, ks[-1] + 1, end))
+        if not windows:
+            return {}
+        if self.ssr:
+            done = self.engine.ssr_restore_windows(self.ring, windows, W, self.synthesis, self.acc, emits)
+        else:
+            done = self.engine.restore_windows(self.ring, windows, W, self.synthesis, self.acc, emits,
+                                               unify_energy=self.unify_energy)
+        out, off = {}, 0
+        for sid, nxt, end in owners:
+            st = self._streams[sid]
+            if end > st.emitted:
+                out[sid] = done[off:off + end - st.emitted]
+                off += end - st.emitted
+            st.next, st.emitted = nxt, end
+            if st.n is not None:
+                self._release(sid)              # a closed stream's step adds its last windows and emits the rest
         return out
