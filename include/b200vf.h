@@ -458,7 +458,8 @@ VF_API int vf_op_info(vf_ctx* ctx, int i, float* ms, double* flops, double* byte
  * Activation operands are fp16 bit patterns in the kernels' layout: [plane (hi, lo)][n_img][img_rows][C], rows of a 2-D
  * layer flattened (h, w) with one pad column (row pitch W + 1).  Output buffers are read AND written: they are uploaded
  * before the launch, so what the layer must not touch comes back unchanged. */
-enum { VF_LAYER_CONV2D = 0, VF_LAYER_CONVT2D = 1, VF_LAYER_CONV1D = 2, VF_LAYER_CONVT1D = 3, VF_LAYER_PAIR = 4 };
+enum { VF_LAYER_CONV2D = 0, VF_LAYER_CONVT2D = 1, VF_LAYER_CONV1D = 2, VF_LAYER_CONVT1D = 3, VF_LAYER_PAIR = 4,
+       VF_LAYER_LINEAR = 5 };
 enum { VF_LAYER_PRODUCT = 0, VF_LAYER_SIMT = 1 };
 enum { VF_RESID_NONE = 0, VF_RESID_FP32 = 1, VF_RESID_PLANES = 2, VF_RESID_AR = 3, VF_RESID_IDENTITY = 4 };
 typedef struct vf_layer_case {
@@ -505,19 +506,35 @@ typedef struct vf_layer_case {
   const int* head_valid;    /* [n_img] or NULL */
   float pair_slope_h, pair_slope_out;   /* PAIR: activation of h, and of x_new (the stage slope after the last pair) */
   int pair_last;            /* PAIR: no correction plane out (last pair of a stack) */
+  /* LINEAR: one nn.Linear of the bi_gru / dnn modules on L rows per image (x_row0 = 0, x_img_rows = L), packed and set up as
+   * the loader and the plan builder do it: w [cout][cin], b [cout]; in_bn (or NULL) = (weight, bias, running_mean,
+   * running_var) of a BatchNorm2d(1) applied to the input, folded into w and b.  With b_hh the layer is a GRU input
+   * projection: w = W_ih [2][768][cin] and b = b_ih, b_hh [2][768] of both directions (cout = 1536, no in_bn). */
+  const float* in_bn;
+  const float* b_hh;
   /* reported: the launch configuration the builder chose */
   int bn, bk, stages, resid_tma, tma_out, grid;
   int64_t tiles;
   int div_fallback;         /* a tile decode divides (its multiply-high magic would not be exact) */
+  char sig[160];            /* PRODUCT: the configuration signature of the launch (the one vf_selftest_plan_gemms reports) */
 } vf_layer_case;
 VF_API int vf_selftest_layer(vf_ctx* ctx, vf_layer_case* lc);
+
+/* TEST ONLY.  Builds a plan of `plan_kind` (0 GSR, 1 SSR, 2 GSR varlen, 3 SSR varlen) for (batch, frames) with the loaded
+ * weights and the context's options, launches nothing, and reports each GEMM and fused-pair launch: its label and the
+ * configuration signature vf_selftest_layer reports for a layer.  Records past `cap` are dropped; *count = all of them. */
+typedef struct vf_plan_gemm {
+  char label[48];
+  char sig[160];
+} vf_plan_gemm;
+VF_API int vf_selftest_plan_gemms(vf_ctx* ctx, int plan_kind, int batch, int frames, vf_plan_gemm* records, int cap, int* count);
 
 /* TEST ONLY.  One non-GEMM op of the launch chains, set up by the same helpers the plan builders and restore paths use and
  * launched as they launch it (run_ops or the same launch_* call), then copied back.  Synchronous; every pointer is a host
  * pointer, and output buffers are read AND written as in vf_selftest_layer.  fp16 planes are bit patterns [2][batch][rows][C].
  * Fields a kind does not use are zero.  The mel-weight table, window and twiddles are the context's own. */
 enum { VF_OP_FIRST = 0, VF_OP_POOL = 1, VF_OP_COND = 2, VF_OP_REFLECT = 3, VF_OP_TAIL = 4, VF_OP_FINALIZE = 5, VF_OP_ISTFT = 6,
-       VF_OP_PEAK_NORM = 7, VF_OP_FRONTEND = 8 };
+       VF_OP_PEAK_NORM = 7, VF_OP_FRONTEND = 8, VF_OP_PLANES = 9 };
 typedef struct vf_op_case {
   int kind, batch;
   /* Clips of different lengths (any kind; PEAK_NORM needs them): host sample offsets [batch + 1], clip b = [off[b], off[b + 1]).
@@ -587,6 +604,8 @@ typedef struct vf_op_case {
   float* sp_out;
   float* cos_out;
   float* sin_out;
+  /* PLANES (T): the bi_gru / dnn input planes of x [batch][T][128] floats, fma(x, bn1_scale, bn1_shift) split hi/lo into planes
+   * [2][batch][T][128]; with clip_off, rows t >= the clip's frames are zeros */
 } vf_op_case;
 VF_API int vf_selftest_op(vf_ctx* ctx, vf_op_case* oc);
 

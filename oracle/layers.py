@@ -141,6 +141,76 @@ def pair(xa, x, wa, ba, wb, bb, dil, slope_h, fp16_h=False):
     return x.to(D) + conv1d(h, wb, bb, 1), h
 
 
+BN_EPS = 1e-5
+
+
+def linear(x, w, b):
+    """nn.Linear on the last axis in float64: x [..., K], w [N, K], b [N]."""
+    return torch.as_tensor(x, dtype=D) @ torch.as_tensor(w, dtype=D).T + torch.as_tensor(b, dtype=D)
+
+
+def bn_scalar(bn):
+    """Eval-mode BatchNorm2d(1) of (weight, bias, running_mean, running_var) as (s, t) in float64: bn(x) = s x + t."""
+    w, b, m, v = (float(q) for q in np.asarray(bn, np.float64))
+    s = w / np.sqrt(v + BN_EPS)
+    return s, b - m * s
+
+
+def bn_fold(w, b, bn, shift_sum=True):
+    """Linear(bn(x)) = x W'^T + b' with W' = s W, b' = b + t * sum_k W[:, k], in float64 (the loader's pack_linear with its
+    input affine).  shift_sum=False is a known-wrong fold (b' = b + t), for tests of the GPU test's bar."""
+    s, t = bn_scalar(bn)
+    w, b = torch.as_tensor(w, dtype=D), torch.as_tensor(b, dtype=D)
+    return s * w, b + t * (w.sum(1) if shift_sum else 1.0)
+
+
+def gru_ih_bias(b_ih, b_hh, hidden=256, merge_n=False):
+    """The input projection's bias of a bidirectional GRU layer, [2 * 3 H] (forward, reverse): b_ih + (b_hr, b_hz, 0).
+    merge_n=True also adds b_hn (known-wrong: torch.nn.GRU applies it inside r * (W_hn h + b_hn))."""
+    b = torch.as_tensor(b_ih, dtype=D).reshape(2, 3 * hidden).clone()
+    bh = torch.as_tensor(b_hh, dtype=D).reshape(2, 3 * hidden)
+    n = 3 * hidden if merge_n else 2 * hidden
+    b[:, :n] += bh[:, :n]
+    return b.reshape(-1)
+
+
+def fma32(x, s, t):
+    """fmaf(x, s, t) for float32 arrays: x s + t rounded once to float32.  x s is exact in float64; the float64 sum is
+    corrected with its exact error (two-sum), which decides the float32 rounding when the sum sits on a float32 midpoint."""
+    x, s, t = (np.asarray(q, np.float32).astype(np.float64) for q in (x, s, t))
+    p = x * s
+    hi = p + t
+    bp = hi - t
+    err = (p - bp) + (t - (hi - bp))
+    y = hi.astype(np.float32)
+    # hi on a float32 midpoint: the nearer neighbour on err's side, not the tie-to-even astype picked
+    lo_n = np.nextafter(y, np.float32(-np.inf)).astype(np.float64)
+    hi_n = np.nextafter(y, np.float32(np.inf)).astype(np.float64)
+    y64 = y.astype(np.float64)
+    below = (hi == (y64 + lo_n) / 2) & (err < 0)
+    above = (hi == (y64 + hi_n) / 2) & (err > 0)
+    y = np.where(below, np.nextafter(y, np.float32(-np.inf)), y)
+    y = np.where(above, np.nextafter(y, np.float32(np.inf)), y)
+    return y.astype(np.float32)
+
+
+def affine_planes(x, scale, shift, valid_rows=None, fused=True):
+    """The bi_gru / dnn input planes (gru_tc.cu affine_planes_kernel) of x [n, T, C] float32: y = fmaf(x, scale, shift),
+    hi = fp16(y), lo = fp16(y - hi) as uint16 bits [2, n, T, C]; rows t >= valid_rows[b] are zeros.  fused=False rounds the
+    product before the add (known-wrong, for tests of the GPU test's bar)."""
+    x = np.asarray(x, np.float32)
+    if fused:
+        y = fma32(x, np.float32(scale), np.float32(shift))
+    else:
+        y = (x * np.float32(scale)).astype(np.float32) + np.float32(shift)
+    if valid_rows is not None:
+        for b, v in enumerate(valid_rows):
+            y[b, int(v):] = 0
+    hi = y.astype(np.float16)
+    lo = (y - hi.astype(np.float32)).astype(np.float16)
+    return np.stack([hi.view(np.uint16), lo.view(np.uint16)])
+
+
 # ------------------------------------------------------------------ write sets
 def write_rows_plain(n_img, out_img_rows, ld, out_row0, rows, c_off, cout):
     """MAP_PLAIN: GEMM row r of every image -> output row out_row0 + r, channels [c_off, c_off + cout)."""

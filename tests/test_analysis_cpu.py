@@ -155,3 +155,86 @@ def test_module_state_loads_with_its_keys(kind, make):
     eng.load_state(sd, need=(kind, "vocoder"))
     sent = [k for k in eng.lib.names if k.startswith(UNET_PREFIX)]
     assert sent == [k for k in sd if k.startswith(UNET_PREFIX) and not k.endswith("num_batches_tracked")]
+
+
+# ------------------------------------------------------------------------- the Linear layers' float64 references
+def test_linear_bn_fold_and_merged_gru_bias_match_the_modules():
+    """oracle/layers.py's float64 Linear, BatchNorm2d(1) fold and merged GRU input bias (the GPU layer suite's references
+    of the analysis launches) restate the torch modules of oracle/analysis.py: dnn's BatchNorm2d(1) + Linear pairs, and the
+    input projection of torch.nn.GRU's layers."""
+    import torch.nn.functional as F
+    from oracle import layers as R
+    s = {k[len(UNET_PREFIX):]: v.double() for k, v in make_dnn_state(1234).items() if k.startswith(UNET_PREFIX)}
+    g = torch.Generator().manual_seed(5)
+    x = torch.randn(2, 1, 7, 256, generator=g, dtype=torch.float64).relu()
+    for bn, li in (("2", "3"), ("5", "6"), ("8", "9"), ("11", "12")):
+        xi = x if s[li + ".weight"].shape[1] == 256 else torch.randn(2, 1, 7, s[li + ".weight"].shape[1], generator=g,
+                                                                       dtype=torch.float64).relu()
+        s[bn + ".running_mean"].fill_(0.3)           # a non-trivial affine: the seeded state's BatchNorm may be the identity
+        s[bn + ".running_var"].fill_(1.7)
+        s[bn + ".bias"].fill_(-0.45)
+        want = F.linear(A._bn(xi, s, bn), s[li + ".weight"], s[li + ".bias"])
+        params = [float(s[bn + k]) for k in (".weight", ".bias", ".running_mean", ".running_var")]
+        w, b = R.bn_fold(s[li + ".weight"], s[li + ".bias"], params)
+        got = R.linear(xi, w, b)
+        assert float((got - want).abs().max()) <= 1e-12 * float(want.abs().max())
+        wrong = R.linear(xi, *R.bn_fold(s[li + ".weight"], s[li + ".bias"], params, shift_sum=False))
+        assert float((wrong - want).abs().max()) > 1e-3
+    gru = torch.nn.GRU(256, 256, bidirectional=True, batch_first=True).double()
+    with torch.no_grad():
+        for p in gru.parameters():
+            p.copy_(torch.randn(p.shape, generator=g, dtype=torch.float64) / 8)
+    xg = torch.randn(3, 9, 256, generator=g, dtype=torch.float64)
+    G, _, _ = A.gru_input(xg, gru, 0)
+    w_ih = torch.cat([gru.weight_ih_l0, gru.weight_ih_l0_reverse]).detach()
+    b_ih = torch.cat([gru.bias_ih_l0, gru.bias_ih_l0_reverse]).detach()
+    b_hh = torch.cat([gru.bias_hh_l0, gru.bias_hh_l0_reverse]).detach()
+    assert float((R.linear(xg, w_ih, R.gru_ih_bias(b_ih, b_hh)) - G).abs().max()) <= 1e-12 * float(G.abs().max())
+    # and the float64 GRU layer built on it is torch.nn.GRU's first layer
+    y = gru(xg)[0].detach()
+    h = A.gru_layer(G, torch.stack([gru.weight_hh_l0, gru.weight_hh_l0_reverse]).detach(),
+                    torch.stack([gru.bias_hh_l0[512:], gru.bias_hh_l0_reverse[512:]]).detach())
+    assert float((h - y).abs().max()) <= 1e-12
+
+
+# ------------------------------------------------------------------------- the input planes (VF_OP_PLANES)
+def test_fma32_is_the_exactly_rounded_fused_multiply_add():
+    """R.fma32 against rational arithmetic: random operands, and sums constructed on float32 midpoints."""
+    from fractions import Fraction
+    from oracle import layers as R
+    g = np.random.default_rng(9)
+    x = (g.standard_normal(4000) * 3).astype(np.float32)
+    s = (g.standard_normal(4000) * 2).astype(np.float32)
+    t = (g.standard_normal(4000) * 4).astype(np.float32)
+    # midpoints: x s = m + half an ulp32 of m exactly, t = 0 or a float32 that keeps the sum on a midpoint ~ 2^-30 apart
+    s[:1000] = np.float32(1.0 + 2.0 ** -12)
+    x[:1000] = (np.round(x[:1000].astype(np.float64) * 2 ** 11) / 2 ** 11 * (1 + 2.0 ** -12)).astype(np.float32)
+    t[:500] = np.float32(2.0 ** -30)
+    t[500:1000] = np.float32(-(2.0 ** -30))
+    got = R.fma32(x, s, t)
+    for i in range(len(x)):
+        v = Fraction(float(x[i])) * Fraction(float(s[i])) + Fraction(float(t[i]))
+        lo = np.float32(float(v))                       # within one float32 ulp of v; pick the nearest neighbour exactly
+        cands = [np.nextafter(lo, np.float32(-np.inf)), lo, np.nextafter(lo, np.float32(np.inf))]
+        d = [abs(Fraction(float(c)) - v) for c in cands]
+        best = min(d)
+        ok = [c for c, e in zip(cands, d) if e == best]
+        want = ok[0] if len(ok) == 1 else [c for c in ok if not (c.view(np.uint32) & 1)][0]
+        assert got[i] == want, (i, x[i], s[i], t[i], got[i], want)
+    assert not np.array_equal(got, (x * s).astype(np.float32) + t)
+
+
+def test_separate_multiply_and_add_breaks_the_planes_bar():
+    """The GPU test compares the planes bit for bit: rounding x * scale before adding shift changes bits of the cases with
+    an affine that is not 1 / 0; and every pad row of the varlen cases is zero in the expected planes."""
+    import test_gpu_aux as X
+    from oracle import layers as R
+    for name, spec in X.PLANES_CASES.items():
+        x, scale, shift, Ts, off = X.planes_inputs(name)
+        want = R.affine_planes(x, scale, shift, Ts if off is not None else None)
+        if off is not None:
+            for b, T in enumerate(Ts):
+                assert not want[:, b, T:].any()
+        if spec["scale"] != 1.0 and not spec.get("ties"):
+            wrong = R.affine_planes(x, scale, shift, Ts if off is not None else None, fused=False)
+            assert (wrong != want).sum() > 10, name

@@ -129,6 +129,38 @@ def test_gru_mixed_lengths_with_relu(bigru_model):
     _check_gru(got, A.gru_layer(G, w, b, lengths, relu=True), lengths, T)
 
 
+# The recurrence's edges: a last clip group holding 1 of GRU_CLIPS = 4 clips (B = 5), one-frame sequences, gates driven far
+# past saturation (expf(-x) overflows to inf for x < -88.7, tanhf reaches +-1), and 35 clusters x 2 directions of 8 CTAs: 560
+# CTAs of one per SM, more than 132 SMs run at once.
+GRU_EDGES = {
+    "last_group_1_of_4": dict(B=5, T=64, lengths=[64, 17, 64, 3, 50], cin=256, relu=False),
+    "T1": dict(B=6, T=1, lengths=None, cin=512, relu=True),
+    "all_lengths_1": dict(B=5, T=16, lengths=[1] * 5, cin=256, relu=False),
+    "saturated_gates": dict(B=4, T=96, lengths=[96, 80, 1, 33], cin=256, relu=False, saturate=True),
+    "B140_T64": dict(B=140, T=64, lengths="mixed", cin=512, relu=True),
+}
+
+
+@pytest.mark.parametrize("name", list(GRU_EDGES))
+def test_gru_edges(bigru_model, name):
+    spec = GRU_EDGES[name]
+    B, T = spec["B"], spec["T"]
+    lengths = spec["lengths"]
+    if lengths == "mixed":
+        lengths = [int(v) for v in np.random.default_rng(140).integers(1, T + 1, B)]
+        lengths[::7] = [T] * len(lengths[::7])
+    G, w, b = _gru_inputs(B, T, seed=len(name) * 31 + B, cin=spec["cin"])
+    if spec.get("saturate"):
+        g = torch.Generator().manual_seed(77)
+        big = torch.rand(G.shape, generator=g, dtype=torch.float64) < 0.4
+        mag = 100 + 200 * torch.rand(G.shape, generator=g, dtype=torch.float64)
+        sign = torch.where(torch.rand(G.shape, generator=g, dtype=torch.float64) < 0.5, -1.0, 1.0)
+        G = torch.where(big, sign * mag, G)
+        assert float(G.abs().max()) > 89                    # expf(-x) of a gate overflows
+    got, G, w, b = _run_gru(bigru_model._engine(), G, w, b, lengths, spec["relu"], T)
+    _check_gru(got, A.gru_layer(G, w, b, lengths, relu=spec["relu"]), lengths, T)
+
+
 # ------------------------------------------------------------------------------------------------------ whole restores
 def test_restore_matches_oracle(model):
     wav = O.synth_clips(2, 44100, seed=31)

@@ -645,6 +645,71 @@ def test_peak_normalise_varlen_is_exact(eng):
     WORST["peak_norm"] = 0.0
 
 
+# ------------------------------------------------------------------ PLANES: affine_planes_kernel (bi_gru / dnn input)
+PLANES = 9            # VF_OP_PLANES
+PLANES_CASES = {
+    "planes.dnn_T101": dict(Ts=[101, 101], scale=1.0, shift=0.0),
+    "planes.bn0_T101": dict(Ts=[101, 101], scale=1.3718, shift=-0.4521),
+    "planes.bn0_T3": dict(Ts=[3], scale=0.8125, shift=2.375),
+    "planes.bn0_varlen": dict(Ts=[64, 3, 40, 1, 63], scale=1.3718, shift=-0.4521, varlen=True),
+    "planes.dnn_varlen": dict(Ts=[3, 128], scale=1.0, shift=0.0, varlen=True),
+    "planes.ties": dict(Ts=[16, 16], scale=2.0, shift=0.375, ties=True),
+}
+
+
+def fp16_ties(g, shape):
+    """float32 values on fp16 rounding ties: half of them halfway between two fp16 values (hi = fp16(y) is a tie), the other
+    half hi + d with d halfway between two fp16 values (lo = fp16(y - hi) is a tie); magnitudes 2 .. 2^7, both signs."""
+    k = g.integers(1, 7, shape)
+    m = g.integers(1024, 2048, shape)                      # hi = m 2^(k - 10): an fp16 value with lsb 2^(k - 10)
+    hi = m * 2.0 ** (k - 10)
+    hi_tie = hi + 2.0 ** (k - 11)                          # half an fp16 ulp above hi
+    lo_tie = hi + (2 * g.integers(1024, 2048, shape) + 1) * 2.0 ** (k - 23)   # d: 12 significant bits, d < ulp / 2
+    y = np.where(g.random(shape) < 0.5, hi_tie, lo_tie) * np.where(g.random(shape) < 0.5, -1.0, 1.0)
+    assert np.array_equal(y.astype(np.float32).astype(np.float64), y)
+    return y.astype(np.float32)
+
+
+def planes_inputs(name):
+    """(x [B, T, 128] float32, scale, shift, per clip frames, clip offsets or None) of a PLANES case."""
+    spec = PLANES_CASES[name]
+    g = _rng(name)
+    Ts = spec["Ts"]
+    B, T = len(Ts), max(Ts)
+    if spec.get("ties"):
+        y = fp16_ties(g, (B, T, 128))
+        x = ((y.astype(np.float64) - spec["shift"]) / spec["scale"]).astype(np.float32)
+        # x is exact except where y - shift leaves y's binade: nearly every fmaf(x, scale, shift) is the tie
+        assert (R.fma32(x, np.float32(spec["scale"]), np.float32(spec["shift"])) == y).mean() > 0.95
+    else:
+        x = (g.standard_normal((B, T, 128)) * 2 - 3).astype(np.float32)          # log10 mel
+    off = offsets([n_for_frames(t) for t in Ts]) if spec.get("varlen") else None
+    return x, np.float32(spec["scale"]), np.float32(spec["shift"]), Ts, off
+
+
+@pytest.mark.parametrize("name", list(PLANES_CASES))
+def test_input_planes_are_exact(eng, name):
+    """hi = fp16(fmaf(x, scale, shift)), lo = fp16(y - hi) bit for bit, zeros at every row past a clip's end, every element
+    written.  The fused multiply-add is evaluated exactly on the host (oracle/layers.py fma32)."""
+    x, scale, shift, Ts, off = planes_inputs(name)
+    B, T = x.shape[:2]
+    out = planes16((B, T, 128))
+    Case(PLANES, B, off, T=T, x=x, bn1_scale=scale, bn1_shift=shift, planes=out).run(eng, name)
+    want = R.affine_planes(x, scale, shift, Ts if off is not None else None)
+    bad = np.argwhere(out != want)
+    assert not len(bad), (name, f"{len(bad)} elements differ, first [plane, clip, row, channel] {bad[:4].tolist()}")
+    if PLANES_CASES[name].get("ties"):
+        y = R.fma32(x, scale, shift)
+        hi = y.astype(np.float16)
+        on_tie = (np.abs(y.astype(np.float64) - hi.astype(np.float64)) == np.spacing(np.abs(hi)).astype(np.float64) / 2)
+        lo = (y - hi.astype(np.float32))
+        lo_tie = lo.astype(np.float16).astype(np.float64) != lo.astype(np.float64)
+        print(f"{name}: {on_tie.mean():.2f} of the hi and {lo_tie.mean():.2f} of the lo roundings are inexact / ties")
+        assert on_tie.mean() > 0.2 and lo_tie.mean() > 0.2
+    WORST[name] = 0.0
+    print(f"{name}: bit-exact")
+
+
 # ------------------------------------------------------------------ the lengths table, the range flag, coverage
 def test_lengths_table_matches_the_host_formula(eng):
     """Every row of the table (kernels.cuh) for both UNets' bins, clips from one frame to a 60 s clip."""
@@ -677,6 +742,7 @@ def test_cases_cover_every_kind_both_tails_and_every_varlen_table(eng):
     want = {(k, 0, v) for k in (FIRST, POOL, COND, REFLECT) for v in (False, True)}
     want |= {(TAIL, t, v) for t in (1, 3) for v in (False, True)}
     want |= {(FINALIZE, 0, False), (FINALIZE, 0, True), (ISTFT, 0, False), (ISTFT, 0, True), (PEAK_NORM, 0, True)}
+    want |= {(PLANES, 0, False), (PLANES, 0, True)}
     if not want <= COVER:            # run on its own: run every case once
         for name in FIRST_CASES:
             test_first_layer_matches_float64(eng, name)
@@ -694,6 +760,8 @@ def test_cases_cover_every_kind_both_tails_and_every_varlen_table(eng):
         test_fused_istft_varlen_matches_float64(eng)
         test_fused_istft_uniform_matches_float64(eng, 1025)
         test_peak_normalise_varlen_is_exact(eng)
+        for name in PLANES_CASES:
+            test_input_planes_are_exact(eng, name)
     assert want <= COVER, sorted(want - COVER)
     for k, v in sorted(WORST.items()):
         print(f"worst {k}: {v:.3e}")

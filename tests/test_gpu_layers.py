@@ -21,7 +21,7 @@ SENT32 = np.uint32(0x7FC0BEEF)
 TOL = {3: 2.0 ** -16, 1: 2.0 ** -14}
 FLOOR = 2.0 ** -24                # fp16 subnormal spacing: the absolute floor of every plane bound
 RES_SLOPE, STAGE_SLOPE, UNET_SLOPE = 0.01, 0.2, 0.01
-CONV2D, CONVT2D, CONV1D, CONVT1D, PAIR = range(5)                            # vf_layer_case kinds (include/b200vf.h)
+CONV2D, CONVT2D, CONV1D, CONVT1D, PAIR, LINEAR = range(6)                    # vf_layer_case kinds (include/b200vf.h)
 RESID = {"fp32": 1, "planes": 2, "ar": 3, "identity": 4}
 
 REPORTS = {}          # case name -> reported launch configuration (product kernel)
@@ -30,6 +30,19 @@ REPORTS = {}          # case name -> reported launch configuration (product kern
 def C(name, kind, **kw):
     kw["name"], kw["kind"] = name, kind
     return kw
+
+
+def lin(name, cin, cout, L=101, n_img=2, **kw):
+    """One nn.Linear of bi_gru / dnn as plan.cu's linear() builds it (3-term, one tap, L frames per clip)."""
+    return C(name, LINEAR, terms=3, n_img=n_img, L=L, cin=cin, cout=cout, **kw)
+
+
+# the epilogues of plan.cu's analysis launches: BN_GRU.bn with no activation, the GRU input projection's fp32 G, a ReLU,
+# and linear_out's fp32 log-mel residual
+BN_NO_ACT = dict(outs="a", affine=True, act=0)
+GRU_IH = dict(outs="raw", gru=True)
+RELU = dict(outs="a", act=1, slope=0.0)
+LIN_OUT = dict(outs="raw", resid="fp32")
 
 
 def unet_conv1(name, H, W, cin, cout, n_img=1, row_valid=None):
@@ -108,6 +121,76 @@ CASES = [
     C("pair.varlen", PAIR, n_img=3, L=1000, dilation=9, row_valid=[1000, 378, 127]),
     C("pair.last", PAIR, L=1000, dilation=243, last=True, out_row0=3, out_slack=6),
     C("pair.d2187", PAIR, L=5000, dilation=2187),
+    # ---- configurations only the varlen plans, the 32-channel level or the last layer of a stack reach (the plan sweep)
+    unet_conv1("conv1.mel_l0_varlen", 8, 127, 32, 32, n_img=2, row_valid=[1024, 384]),
+    unet_conv1("conv1.dec6_b2", 4, 127, 64, 32),
+    unet_conv1("conv1.dec6_b2_varlen", 4, 127, 64, 32, n_img=2, row_valid=[512, 128]),
+    unet_conv1("conv1.enc2_b1", 4, 63, 32, 64),
+    unet_conv1("conv1.enc2_b1_varlen", 4, 63, 32, 64, n_img=2, row_valid=[256, 64]),
+    C("conv2_sc.enc2_b1_varlen", CONV2D, terms=3, n_img=2, H=4, W=63, cin=64, cout=64, sc_cin=32, outs="raw,a", affine=True,
+      act=1, slope=UNET_SLOPE, row_valid=[256, 64]),
+    C("conv2_sc.dec6_b2", CONV2D, terms=3, H=4, W=127, cin=32, cout=32, sc_cin=64, outs="raw,a", affine=True, act=1,
+      slope=UNET_SLOPE),
+    C("conv2_sc.dec6_b2_varlen", CONV2D, terms=3, n_img=2, H=4, W=127, cin=32, cout=32, sc_cin=64, outs="raw,a", affine=True,
+      act=1, slope=UNET_SLOPE, row_valid=[512, 128]),
+    C("conv2_res.c32_varlen", CONV2D, terms=3, n_img=2, H=8, W=127, cin=32, cout=32, resid="fp32", outs="raw,a", affine=True,
+      act=1, slope=UNET_SLOPE, row_valid=[1024, 384]),
+    C("conv2_res.dec_b5_relu", CONV2D, terms=3, H=4, W=63, cin=64, cout=64, resid="fp32", outs="a", affine=True, act=1,
+      slope=0.0),
+    C("conv2_res.dec_b5_relu_varlen", CONV2D, terms=3, n_img=2, H=4, W=63, cin=64, cout=64, resid="fp32", outs="a",
+      affine=True, act=1, slope=0.0, row_valid=[256, 64]),
+    C("skip_concat.enc1_b4", CONV2D, terms=3, H=4, W=127, cin=32, cout=32, resid="fp32", outs="raw,r,a", concat=True,
+      affine=True, act=1, slope=UNET_SLOPE),
+    C("skip_concat.enc1_b4_varlen", CONV2D, terms=3, n_img=2, H=4, W=127, cin=32, cout=32, resid="fp32", outs="raw,r,a",
+      concat=True, affine=True, act=1, slope=UNET_SLOPE, row_valid=[512, 128]),
+    C("skip_concat.enc_b4_varlen", CONV2D, terms=3, n_img=2, H=4, W=63, cin=64, cout=64, resid="fp32", outs="raw,r,a",
+      concat=True, affine=True, act=1, slope=UNET_SLOPE, row_valid=[256, 64]),
+    C("head.mel_varlen", CONV2D, terms=3, n_img=2, H=8, W=127, cin=32, cout=32, resid="fp32", head=True, head_in=True,
+      head_T=7, head_valid=[7, 3], row_valid=[1024, 384]),
+    C("cond.varlen_t1", CONV1D, terms=1, n_img=2, L=130, cin=128, cout=512, k=3, outs="a", act=2, row_valid=[130, 9]),
+    C("cond.varlen_t3", CONV1D, terms=3, n_img=2, L=130, cin=128, cout=512, k=3, outs="a", act=2, row_valid=[130, 9]),
+    C("res_a.d3_c256_varlen", CONV1D, terms=1, n_img=2, L=600, cin=256, cout=256, k=3, dilation=3, outs="a", act=1,
+      slope=RES_SLOPE, row_valid=[600, 3]),
+    C("up.s7_ar_tma_varlen", CONVT1D, terms=1, n_img=2, L=42, cin=1024, cout=512, stride=7, outs="a", out_ar=True,
+      row_valid=[294, 21]),
+    C("up.s3_ar_tma_c64", CONVT1D, terms=1, L=200, cin=128, cout=64, stride=3, outs="a", out_ar=True),
+    C("up.s3_t3_varlen", CONVT1D, terms=3, n_img=2, L=300, cin=128, cout=64, stride=3, outs="r,a", act=1, slope=RES_SLOPE,
+      row_valid=[900, 10]),
+    C("res_b.last_of_stack_varlen", CONV1D, terms=1, n_img=2, L=500, cin=128, cout=128, k=3, resid="ar", outs="a", act=1,
+      slope=STAGE_SLOPE, out_row0=3, out_slack=6, row_valid=[500, 77]),
+    C("res_b.planes_last_c256_t3", CONV1D, terms=3, L=300, cin=256, cout=256, k=3, resid="planes", outs="a", act=1,
+      slope=STAGE_SLOPE),
+    C("res_b.planes_last_c256_t3_varlen", CONV1D, terms=3, n_img=2, L=300, cin=256, cout=256, k=3, resid="planes", outs="a",
+      act=1, slope=STAGE_SLOPE, row_valid=[300, 3]),
+    C("res_b.planes_c256_t3_varlen", CONV1D, terms=3, n_img=2, L=300, cin=256, cout=256, k=3, resid="planes", outs="r,a",
+      act=1, slope=RES_SLOPE, row_valid=[300, 3]),
+    C("res_b.identity_last_c128_t3", CONV1D, terms=3, L=500, cin=128, cout=128, k=3, resid="identity", outs="a", act=1,
+      slope=STAGE_SLOPE),
+    C("res_b.identity_last_c128_t3_varlen", CONV1D, terms=3, n_img=2, L=500, cin=128, cout=128, k=3, resid="identity",
+      outs="a", act=1, slope=STAGE_SLOPE, row_valid=[500, 3]),
+    C("res_b.identity_c64_t3_varlen", CONV1D, terms=3, n_img=2, L=500, cin=64, cout=64, k=3, resid="identity", outs="r,a",
+      act=1, slope=RES_SLOPE, row_valid=[500, 3]),
+    C("pair.last_varlen", PAIR, n_img=2, L=1000, dilation=243, last=True, out_row0=3, out_slack=6, row_valid=[1000, 127]),
+    # ---- the analysis modules' Linear layers (plan.cu: build_bigru / build_dnn), at the plans' shapes
+    lin("bigru.lin1", 128, 256, **BN_NO_ACT),
+    lin("bigru.gru0.ih", 256, 1536, **GRU_IH),
+    lin("bigru.gru1.ih", 512, 1536, **GRU_IH),
+    lin("bigru.lin4", 512, 256, **RELU),
+    lin("bigru.lin6", 256, 128, **LIN_OUT),
+    lin("dnn.lin0", 128, 256, **RELU),
+    lin("dnn.lin1_bn", 256, 512, in_bn=True, **RELU),
+    lin("dnn.lin2_bn", 512, 1024, in_bn=True, **RELU),
+    lin("dnn.lin3_bn_k1024", 1024, 512, in_bn=True, **RELU),
+    lin("dnn.lin4_bn", 512, 256, in_bn=True, **RELU),
+    lin("dnn.lin5", 256, 128, **LIN_OUT),
+    # varlen plans: a 3-frame clip next to a long one (125 pad rows in its only tile), five clips, and T = 3 uniform
+    lin("bigru.lin1.varlen", 128, 256, L=128, row_valid=[3, 128], **BN_NO_ACT),
+    lin("bigru.gru0.ih.varlen", 256, 1536, L=64, n_img=5, row_valid=[64, 3, 40, 1, 63], **GRU_IH),
+    lin("bigru.gru1.ih.T3", 512, 1536, L=3, n_img=1, **GRU_IH),
+    lin("bigru.lin4.varlen", 512, 256, L=192, row_valid=[190, 3], **RELU),
+    lin("bigru.lin6.varlen", 256, 128, L=64, n_img=5, row_valid=[3, 64, 1, 40, 63], **LIN_OUT),
+    lin("dnn.lin3_bn_k1024.varlen", 1024, 512, L=128, row_valid=[3, 128], in_bn=True, **RELU),
+    lin("dnn.lin5.T3", 256, 128, L=3, n_img=1, **LIN_OUT),
     # ---- the tile decode's division fallback: SSR 60 s level 0 (6016 x 1025 rows, two images), windows only
     C("decode_fallback", CONV1D, terms=1, n_img=2, L=6016 * 1025, cin=32, cout=32, k=1, outs="a", act=1, slope=RES_SLOPE,
       windows=True),
@@ -246,6 +329,24 @@ def build(c, impl):
         lc.w = _ptr(w)
         lc.b = _ptr(bias())
         b.b = torch.from_numpy(keep[-1]).to(torch.float64)
+    elif kind == LINEAR:
+        w = (g.standard_normal((cout, cin)) / np.sqrt(cin)).astype(np.float32)
+        keep.append(w)
+        lc.w, lc.b = _ptr(w), _ptr(bias())
+        b_in = keep[-1]
+        b.w, b.b = torch.from_numpy(w).to(torch.float64), torch.from_numpy(b_in).to(torch.float64)
+        b.bn, b.b_hh = None, None
+        if c.get("gru"):                          # W_ih of both directions [2][768][cin], b_ih, b_hh
+            b.b_hh = bias()
+            lc.b_hh = _ptr(b.b_hh)
+            b.b = R.gru_ih_bias(b_in, b.b_hh)
+        elif c.get("in_bn"):                      # the BatchNorm2d(1) between the previous ReLU and this Linear
+            b.bn = np.array([g.uniform(0.5, 2.0), g.standard_normal() * 0.5, g.standard_normal() * 0.5,
+                             g.uniform(0.3, 2.0)], np.float32)
+            keep.append(b.bn)
+            lc.in_bn = _ptr(b.bn)
+            b.w, b.b = R.bn_fold(w, b_in, b.bn)
+        b.w_raw, b.b_raw = w, b_in
     else:
         lc.terms = b.terms = terms = 1
         lc.dilation = c["dilation"]
@@ -371,6 +472,8 @@ def reference(b, abs_=False):
         y = R.nchw_to_rows(R.conv_transpose2d(ab(x), ab(b.w), c["both"]))
     elif kind == CONV1D:
         y = R.ncl_to_rows(R.conv1d(ab(R.rows_to_ncl(b.x)), ab(b.w), ab(b.b), c.get("dilation", 1), c.get("centered", 1)))
+    elif kind == LINEAR:
+        y = R.linear(ab(b.x), ab(b.w), ab(b.b))
     else:
         y = R.ncl_to_rows(R.conv_transpose1d(ab(R.rows_to_ncl(b.x)), ab(b.w), ab(b.b), c["stride"]))
     if b.resid is not None:
@@ -404,7 +507,7 @@ def zero_rows_mask(b):
 
 def write_mask(b, ld, c_off, cout):
     c, kind = b.c, b.c["kind"]
-    if kind in (CONV2D, CONV1D, PAIR):
+    if kind in (CONV2D, CONV1D, PAIR, LINEAR):
         return R.write_rows_plain(b.n, b.out_img_rows, ld, b.out_row0, _out_geometry(b)[0], c_off, cout)
     if kind == CONVT2D:
         _, ow = _out_geometry(b)
@@ -462,6 +565,7 @@ def run_and_check(eng, c, impl):
     lc = b.lc
     rep = {k: getattr(lc, k) for k in ("bn", "bk", "stages", "resid_tma", "tma_out", "grid", "tiles", "div_fallback")}
     rep["terms"] = b.terms
+    rep["sig"] = lc.sig.decode()
     ck = Checker(c["name"] + ("/simt" if impl else ""))
     if c["kind"] == PAIR:
         check_pair(b, ck)
@@ -651,10 +755,56 @@ def test_fp16_overflow_is_reported_and_the_next_case_passes(eng):
     run_and_check(eng, BY_NAME["res_a.d243_c64"], 0)
 
 
+PLAN_FRAMES = {0: 101, 1: 101, 2: 128, 3: 128}        # plan kind (vf_selftest_plan_gemms) -> frames of the swept plan
+PLAN_NAMES = {0: "gsr", 1: "ssr", 2: "gsr_varlen", 3: "ssr_varlen"}
+
+
+def plan_sweep():
+    """[(plan, label, signature)] of every GEMM / fused-pair launch of the plans: each analysis module (unet, bi_gru, dnn) with
+    the vocoder at 1 and 3 terms, uniform and varlen, and the SSR plans, uniform and varlen.  Plans are built, not run."""
+    from voicefixer_main_b200.model import Engine
+    from voicefixer_main_b200.weights import make_bigru_state, make_dnn_state, make_ssr_state, make_state, make_vocoder_state
+    e = Engine("cuda:0")
+    out = []
+    try:
+        for module, make in (("unet", make_state), ("bi_gru", make_bigru_state), ("dnn", make_dnn_state)):
+            sd = make(1234)
+            if module != "unet":
+                sd.update(make_vocoder_state(seed=1235))
+            e.load_state(sd, need=(module, "vocoder"))
+            for terms in (1, 3):
+                e.set_option("vocoder_terms", terms)
+                for kind in (0, 2):
+                    out += [(f"{module}.{PLAN_NAMES[kind]}.voc{terms}", lb, sg) for lb, sg in e.selftest_plan_gemms(kind, 2, PLAN_FRAMES[kind])]
+        e.load_state(make_ssr_state(1234), need=("ssr",))
+        for kind in (1, 3):
+            out += [(PLAN_NAMES[kind], lb, sg) for lb, sg in e.selftest_plan_gemms(kind, 2, PLAN_FRAMES[kind])]
+        e.check_errors()
+    finally:
+        e.close()
+    return out
+
+
 def test_cases_cover_every_kernel_configuration(eng):
+    """Every GEMM and fused-pair launch the plans build has the configuration signature (plan.cu: op_signature) of some
+    case above, so each kernel configuration a restore runs is checked against float64 here."""
     for c in CASES:
         if c["name"] not in REPORTS:
             REPORTS[c["name"]] = run_and_check(eng, c, 0)[1]
+    by_sig = {}
+    for name, r in REPORTS.items():
+        by_sig.setdefault(r["sig"], name)
+    sweep = plan_sweep()
+    assert len(sweep) > 100 and all(sg for _, _, sg in sweep)
+    table, uncovered = {}, {}
+    for plan, label, sig in sweep:
+        table.setdefault(sig, (by_sig.get(sig), []))[1].append(f"{plan}:{label}")
+        if sig not in by_sig:
+            uncovered.setdefault(sig, []).append(f"{plan}:{label}")
+    for sig, (case, labels) in sorted(table.items()):
+        print(f"{sig}\n    case {case}\n    ops ({len(labels)}): {', '.join(labels[:6])}{' ...' if len(labels) > 6 else ''}")
+    assert not uncovered, "plan launches whose configuration no case checks:\n" + "\n".join(
+        f"{sig}\n    {', '.join(labels)}" for sig, labels in sorted(uncovered.items()))
     reps = [r for k, r in REPORTS.items() if BY_NAME[k]["kind"] != PAIR]
     assert {32, 64, 128} <= {r["bn"] for r in reps}
     assert {32, 64} <= {r["bk"] for r in reps}

@@ -171,3 +171,65 @@ def test_bar_catches_one_row_of_one_image_replaced_by_its_neighbours():
     y = G.reference(b).numpy().copy()
     y[1, 150] = y[1, 151]
     assert _bar_ratio(b, y) > 1
+
+
+# ------------------------------------------------------------------ the analysis modules' Linear layers
+def _act_ratio(b, y_mut):
+    """max |act(y_mut) - act(y64)| / bound with the bound the GPU test applies to the case's 3-term outputs (out_a after
+    its affine and activation, or the raw fp32 output), rows the layer zeroes excluded."""
+    c = b.c
+    y, M = G.reference(b).numpy(), G.reference(b, abs_=True).numpy()
+    keep = ~G.zero_rows_mask(b)[..., None]
+    tol = G.TOL[b.terms]
+    if c["outs"] == "raw":
+        want, got, bound = y, np.asarray(y_mut), tol * M + G.FLOOR
+    else:
+        sc = np.abs(b.scale) if c.get("affine") else 1.0
+        f = lambda v: R.activate(torch.as_tensor(v * b.scale + b.shift if c.get("affine") else v), c["act"],
+                                 c.get("slope", 0.0)).numpy()
+        want, got = f(y), f(np.asarray(y_mut))
+        bound = sc * tol * M + 2.0 ** -21 * np.abs(want) + G.FLOOR
+    return float((np.abs(got - want) / bound * keep).max())
+
+
+def test_linear_cases_pass_their_own_reference():
+    for c in G.CASES:
+        if c["kind"] == G.LINEAR:
+            b = _case(c["name"])
+            assert _act_ratio(b, G.reference(b).numpy()) == 0.0
+
+
+def test_bar_catches_the_bn_fold_without_the_weight_sums():
+    for name in ("dnn.lin1_bn", "dnn.lin3_bn_k1024", "dnn.lin3_bn_k1024.varlen"):
+        b = _case(name)
+        _, bias = R.bn_fold(b.w_raw, b.b_raw, b.bn, shift_sum=False)
+        assert _act_ratio(b, _mutated(b, b=bias)) > 1, name
+
+
+def test_bar_catches_b_hn_merged_into_the_gru_input_projection():
+    for name in ("bigru.gru0.ih", "bigru.gru1.ih", "bigru.gru0.ih.varlen"):
+        b = _case(name)
+        assert _act_ratio(b, _mutated(b, b=R.gru_ih_bias(b.b_raw, b.b_hh, merge_n=True))) > 1, name
+
+
+def test_bar_catches_the_log_mel_residual_on_the_first_n_tile_only():
+    """linear_out's N = 128 is two 64-column tiles in 3-term mode; the residual left off the second one."""
+    for name in ("bigru.lin6", "dnn.lin5", "bigru.lin6.varlen", "dnn.lin5.T3"):
+        b = _case(name)
+        resid = b.resid.clone()
+        resid[..., 64:] = 0
+        assert _act_ratio(b, _mutated(b, resid=resid)) > 1, name
+
+
+def test_pad_rows_of_a_3_frame_clip_are_nonzero_unless_written_as_zeros():
+    """The GPU test demands exact zeros at rows t >= 3 of the 3-frame clips: the GEMM's value there (the bias, with the
+    residual and the activation) is not zero, so a pad row left as computed fails it."""
+    for name in ("bigru.lin1.varlen", "bigru.gru0.ih.varlen", "bigru.lin4.varlen", "bigru.lin6.varlen", "dnn.lin3_bn_k1024.varlen"):
+        b = _case(name)
+        img = list(b.rv).index(3)
+        y = G.reference(b).numpy()[img, 3:]
+        c = b.c
+        if c["outs"] == "a":
+            v = y * b.scale + b.shift if c.get("affine") else y
+            y = R.activate(torch.as_tensor(v), c["act"], c.get("slope", 0.0)).numpy()
+        assert G.zero_rows_mask(b)[img, 3:].all() and (y != 0).any(axis=-1).all(), name

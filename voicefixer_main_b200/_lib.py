@@ -6,7 +6,7 @@ with VF_ENODEVICE.  Nothing here computes on the data path; it only marshals poi
 """
 import ctypes
 import os
-from ctypes import (POINTER, Structure, byref, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_size_t, c_uint, c_void_p)
+from ctypes import (POINTER, Structure, byref, c_char, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_size_t, c_uint, c_void_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200vf.so")
@@ -24,6 +24,7 @@ EXPORTS = [
     "vf_ssr_restore_varlen_mels", "vf_selftest_op", "vf_selftest_gru", "vf_score_time_varlen",
     "vf_sosfiltfilt_varlen", "vf_resample_poly_f64_varlen", "vf_metric_spectrogram_ex", "vf_score_varlen_ex",
     "vf_score_time_varlen_ex", "vf_restore_chunks", "vf_ssr_restore_chunks", "vf_restore_windows", "vf_ssr_restore_windows",
+    "vf_selftest_plan_gemms",
 ]
 VF_RESTORE_UNIFY_ENERGY = 1
 VF_SSR_PEAK_NORMALISE = 1
@@ -55,9 +56,10 @@ class VfLayerCase(Structure):
                 ("a_scale", c_void_p), ("a_shift", c_void_p), ("act", c_int), ("slope", c_float), ("out_row0", c_int),
                 ("out_img_rows", c_int), ("head_w", c_void_p), ("head_b", c_float), ("head_in", c_void_p),
                 ("head_out", c_void_p), ("head_T", c_int), ("row_valid", c_void_p), ("head_valid", c_void_p),
-                ("pair_slope_h", c_float), ("pair_slope_out", c_float), ("pair_last", c_int)] + \
+                ("pair_slope_h", c_float), ("pair_slope_out", c_float), ("pair_last", c_int), ("in_bn", c_void_p),
+                ("b_hh", c_void_p)] + \
                [(f, c_int) for f in ("bn", "bk", "stages", "resid_tma", "tma_out", "grid")] + \
-               [("tiles", c_int64), ("div_fallback", c_int)]
+               [("tiles", c_int64), ("div_fallback", c_int), ("sig", c_char * 160)]
 
 
 class VfOpCase(Structure):
@@ -75,6 +77,11 @@ class VfOpCase(Structure):
                [(f, c_void_p) for f in ("in_wav", "mag", "frames", "out")] + \
                [("Tp", c_int), ("Wpo", c_int), ("Tv", c_int), ("skip", c_int64), ("tail_smem", c_int64)] + \
                [(f, c_void_p) for f in ("mel_out", "logmel_out", "sp_out", "cos_out", "sin_out")]     # VF_OP_FRONTEND
+
+
+class VfPlanGemm(Structure):
+    """vf_plan_gemm (include/b200vf.h): one GEMM / fused-pair launch of a plan for vf_selftest_plan_gemms (tests only)."""
+    _fields_ = [("label", c_char * 48), ("sig", c_char * 160)]
 
 
 class VfGruCase(Structure):
@@ -149,6 +156,7 @@ def load_library():
     lib.vf_selftest_layer.argtypes = [P, POINTER(VfLayerCase)]
     lib.vf_selftest_op.argtypes = [P, POINTER(VfOpCase)]
     lib.vf_selftest_gru.argtypes = [P, POINTER(VfGruCase)]
+    lib.vf_selftest_plan_gemms.argtypes = [P, c_int, c_int, c_int, POINTER(VfPlanGemm), c_int, POINTER(c_int)]
     lib.vf_enable_op_timing.argtypes = [P, c_int]
     lib.vf_op_count.argtypes = [P]
     lib.vf_op_info.argtypes = [P, c_int, POINTER(c_float), POINTER(c_double), POINTER(c_double), POINTER(c_int),

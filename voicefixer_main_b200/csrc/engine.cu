@@ -1377,6 +1377,24 @@ int run_layer_case(vf_ctx* ctx, Builder& b, vf_layer_case& c) {
       rc = pack_conv1d(ctx, &W, host_tensor(c.w, {c.cout, c.cin, 3}), host_tensor(c.b, {c.cout}), false);
       if (!rc) rc = pack_conv1d(ctx, &W2, host_tensor(c.w2, {c.cout, c.cout, 3}), host_tensor(c.b2, {c.cout}), ident);
       break;
+    case VF_LAYER_LINEAR:
+      if (c.b_hh) {     // load_bigru: the layer's W_ih of both directions, b_ih + (b_hr, b_hz, 0)
+        const int G3 = 3 * GRU_HIDDEN;
+        HostT wi[2], bi[2], bh[2];
+        const HostT *pw[2], *pb[2], *ph[2];
+        for (int d = 0; d < 2; ++d) {
+          wi[d] = host_tensor(c.w + (size_t)d * G3 * c.cin, {G3, c.cin});
+          bi[d] = host_tensor(c.b + d * G3, {G3});
+          bh[d] = host_tensor(c.b_hh + d * G3, {G3});
+          pw[d] = &wi[d]; pb[d] = &bi[d]; ph[d] = &bh[d];
+        }
+        rc = pack_gru_ih(ctx, &W, pw, pb, ph);
+      } else {          // load_bigru / load_dnn: pack_linear, the input BatchNorm2d(1) folded as scalar_bn folds it
+        double st[2];
+        if (c.in_bn) scalar_bn_affine(c.in_bn, st);
+        rc = pack_linear(ctx, &W, host_tensor(c.w, {c.cout, c.cin}), host_tensor(c.b, {c.cout}), c.in_bn ? st : nullptr);
+      }
+      break;
   }
   if (rc) return rc;
 
@@ -1399,6 +1417,7 @@ int run_layer_case(vf_ctx* ctx, Builder& b, vf_layer_case& c) {
     c.bn = 64; c.bk = 64; c.stages = 0; c.resid_tma = 0; c.tma_out = 1; c.grid = op->pair.grid;
     c.tiles = (int64_t)n * op->pair.tiles_per_img;
     c.div_fallback = op->pair.magic_t == 0xffffffffu;
+    snprintf(c.sig, sizeof c.sig, "%s", op_signature(*op).c_str());
   } else {
     GemmEpilogue e;
     memset(&e, 0, sizeof e);
@@ -1437,6 +1456,9 @@ int run_layer_case(vf_ctx* ctx, Builder& b, vf_layer_case& c) {
         e.ct_stride = c.stride; e.ct_pad = c.stride / 2 + c.stride % 2;
         taps = taps_convt1d(c.cin);
         break;
+      case VF_LAYER_LINEAR:      // epi_plain(T, 0, N, T) + linear_gemm below
+        e.map = MAP_PLAIN;
+        break;
     }
     if (c.resid_kind == VF_RESID_FP32) {
       e.resid = dev_floats((const float*)c.resid, (size_t)n * rows * c.cout);
@@ -1473,7 +1495,8 @@ int run_layer_case(vf_ctx* ctx, Builder& b, vf_layer_case& c) {
       e.head_valid = dev_ints(c.head_valid);
     }
     if (b.rc) return b.rc;
-    b.gemm(ops, W, xs, has_s1 ? &s1 : nullptr, taps, e, n, c.terms);
+    if (c.kind == VF_LAYER_LINEAR) linear_gemm(b, ops, W, X, c.L, n, row_valid, e, c.terms);
+    else b.gemm(ops, W, xs, has_s1 ? &s1 : nullptr, taps, e, n, c.terms);
     if (b.rc) return b.rc;
     op = &ops.back();
     c.bn = op->bn; c.bk = op->bk;
@@ -1482,11 +1505,13 @@ int run_layer_case(vf_ctx* ctx, Builder& b, vf_layer_case& c) {
       c.grid = op->simt.prob.n_img * op->simt.prob.m_tiles * (op->simt.prob.N / 32);
       c.tiles = c.grid;
       c.div_fallback = 0;
+      c.sig[0] = 0;
     } else {
       const GemmTcParams& tp = op->tc;
       c.stages = tp.stages; c.resid_tma = tp.resid_tma; c.tma_out = tp.prob.epi.tma_out; c.grid = tp.grid;
       c.tiles = (int64_t)n * tp.prob.m_tiles * (tp.prob.N / op->bn);
       c.div_fallback = tp.magic_n == 0xffffffffu || tp.magic_m == 0xffffffffu;
+      snprintf(c.sig, sizeof c.sig, "%s", op_signature(*op).c_str());
     }
   }
   rc = run_ops(ctx, ops, 0);
@@ -1514,12 +1539,14 @@ extern "C" {
 VF_API int vf_selftest_layer(vf_ctx* ctx, vf_layer_case* lc) {
   if (!ctx || !lc) return VF_EINVAL;
   vf_layer_case& c = *lc;
-  const bool pair = c.kind == VF_LAYER_PAIR;
-  if (c.kind < VF_LAYER_CONV2D || c.kind > VF_LAYER_PAIR || (c.impl != VF_LAYER_PRODUCT && c.impl != VF_LAYER_SIMT) ||
+  const bool pair = c.kind == VF_LAYER_PAIR, lin = c.kind == VF_LAYER_LINEAR;
+  if (c.kind < VF_LAYER_CONV2D || c.kind > VF_LAYER_LINEAR || (c.impl != VF_LAYER_PRODUCT && c.impl != VF_LAYER_SIMT) ||
       (c.terms != 1 && c.terms != 3) || c.n_img <= 0 || !c.x || !c.w || c.cin <= 0 || c.cout <= 0 || c.x_row0 < 0 ||
       c.out_img_rows <= 0 || c.resid_kind < VF_RESID_NONE || c.resid_kind > VF_RESID_IDENTITY ||
       (c.resid_kind != VF_RESID_NONE && !c.resid) || (c.sc_cin && (c.kind != VF_LAYER_CONV2D || !c.sc_w || !c.sc_b || !c.sc_x)) ||
-      ((c.kind == VF_LAYER_CONV1D || c.kind == VF_LAYER_CONVT1D || pair) && !c.b) ||
+      ((c.kind == VF_LAYER_CONV1D || c.kind == VF_LAYER_CONVT1D || pair || lin) && !c.b) ||
+      ((c.in_bn || c.b_hh) && !lin) || (c.in_bn && c.b_hh) || (c.b_hh && c.cout != 6 * GRU_HIDDEN) ||
+      (lin && (c.L <= 0 || c.x_row0 != 0 || c.x_img_rows != c.L || c.resid_kind > VF_RESID_FP32 || c.head_w)) ||
       ((c.kind == VF_LAYER_CONV2D || c.kind == VF_LAYER_CONVT2D) && (c.H <= 0 || c.W <= 0 || c.b)) ||
       (c.kind == VF_LAYER_CONV1D && (c.k <= 0 || c.dilation <= 0)) || (c.kind == VF_LAYER_CONVT1D && c.stride <= 0) ||
       (c.head_w && (!c.head_out || c.head_T <= 0)) ||
@@ -1704,6 +1731,13 @@ int run_op_case(vf_ctx* ctx, Builder& b, vf_op_case& c) {
       if (rc) return rc;
       break;
     }
+    case VF_OP_PLANES: {         // the first op of build_bigru (BN0's scale and shift) and build_dnn (1, 0)
+      const size_t n = (size_t)B * c.T * 128;
+      const float* x = fl(c.x, n);
+      const PlanePtr o = planes_out(c.planes, n);
+      ops.push_back(planes_op(x, B, c.T, c.bn1_scale, c.bn1_shift, o, plan.vl(VL_T)));
+      break;
+    }
   }
   if (b.rc) return b.rc;
   rc = run_ops(ctx, ops, 0);
@@ -1755,7 +1789,7 @@ VF_API int vf_selftest_gru(vf_ctx* ctx, vf_gru_case* gc) {
 VF_API int vf_selftest_op(vf_ctx* ctx, vf_op_case* oc) {
   if (!ctx || !oc) return VF_EINVAL;
   vf_op_case& c = *oc;
-  const bool bad_kind = c.kind < VF_OP_FIRST || c.kind > VF_OP_FRONTEND;
+  const bool bad_kind = c.kind < VF_OP_FIRST || c.kind > VF_OP_PLANES;
   const bool bad_shape =
       (c.kind == VF_OP_FIRST && (c.T <= 0 || c.W <= 0 || !c.x || !c.w1 || !c.bn2_scale || !c.bn2_shift || !c.w_sc || !c.b_sc)) ||
       (c.kind == VF_OP_POOL && (c.H < 2 || c.W <= 0 || c.C <= 0 || c.C % 8 || !c.pin || !c.a_scale || !c.a_shift || c.level < 0 || c.level > 5)) ||
@@ -1766,7 +1800,8 @@ VF_API int vf_selftest_op(vf_ctx* ctx, vf_op_case* oc) {
       (c.kind == VF_OP_FINALIZE && (c.L <= 0 || c.n <= 0 || !c.in_wav || !c.peak_bits || !c.out)) ||
       (c.kind == VF_OP_ISTFT && (c.T <= 0 || c.n <= 1024 || !c.mag || !c.in_wav || !c.frames || !c.out)) ||
       (c.kind == VF_OP_PEAK_NORM && (!c.clip_off || c.n <= 0 || !c.wav || !c.peak_bits)) ||
-      (c.kind == VF_OP_FRONTEND && (c.n <= 0 || !c.in_wav || (c.clip_off && c.T <= 0) || !c.cos_out != !c.sin_out || (c.cos_out && !c.sp_out)));
+      (c.kind == VF_OP_FRONTEND && (c.n <= 0 || !c.in_wav || (c.clip_off && c.T <= 0) || !c.cos_out != !c.sin_out || (c.cos_out && !c.sp_out))) ||
+      (c.kind == VF_OP_PLANES && (c.T <= 0 || !c.x || !c.planes));
   if (bad_kind || c.batch <= 0 || bad_shape || (c.clip_off && (c.batch > VL_MAX_CLIPS || c.clip_off[0] != 0)))
     return fail(ctx, VF_EINVAL, "vf_selftest_op: bad case");
   CK(cudaSetDevice(ctx->device));
@@ -1780,6 +1815,35 @@ VF_API int vf_selftest_op(vf_ctx* ctx, vf_op_case* oc) {
   ctx->allocs.resize(n_weight_allocs);
   ctx->weight_bytes = weight_bytes;
   if (!rc && se != cudaSuccess) rc = fail(ctx, VF_ECUDA, "vf_selftest_op: %s", cudaGetErrorString(se));
+  return rc;
+}
+
+VF_API int vf_selftest_plan_gemms(vf_ctx* ctx, int plan_kind, int batch, int frames, vf_plan_gemm* records, int cap, int* count) {
+  if (!ctx || !count || cap < 0 || (cap && !records)) return VF_EINVAL;
+  if (plan_kind < PLAN_GSR || plan_kind > PLAN_SSR_VARLEN || batch <= 0 || frames <= 0 ||
+      (is_varlen_plan(plan_kind) && batch > VL_MAX_CLIPS))
+    return fail(ctx, VF_EINVAL, "vf_selftest_plan_gemms: bad plan");
+  if (ctx->validate_simt) return fail(ctx, VF_EINVAL, "vf_selftest_plan_gemms: validate_simt plans run no tensor-core launches");
+  if (!ctx->loaded) return fail(ctx, VF_ESTATE, "weights not loaded");
+  int rc = check_networks(ctx, plan_kind);
+  if (rc) return rc;
+  CK(cudaSetDevice(ctx->device));
+  Plan plan;
+  plan.kind = plan_kind; plan.batch = batch; plan.T = frames;
+  rc = build_plan(ctx, &plan);
+  int n = 0;
+  for (const std::vector<Op>* list : {&plan.frontend, &plan.unet, &plan.vocoder, &plan.tail})
+    for (const Op& op : *list) {
+      const std::string s = rc ? std::string() : op_signature(op);
+      if (s.empty()) continue;
+      if (n < cap) {
+        snprintf(records[n].label, sizeof records[n].label, "%s", op.label);
+        snprintf(records[n].sig, sizeof records[n].sig, "%s", s.c_str());
+      }
+      ++n;
+    }
+  *count = n;
+  free_plan(&plan);
   return rc;
 }
 

@@ -313,6 +313,14 @@ int pack_conv1d(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT& b, bool id
 int pack_convT1d(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT& b, int s);
 // the tail Conv1d(C -> 1, k7) weight [1][C][7] -> the tail kernel's [7][C]
 int pack_tail(vf_ctx* ctx, float** out, const HostT& w);
+// nn.Linear [N][K] + bias [N] -> packed GEMM operand; with `in_affine` (s, t) the input is s * x + t (a BatchNorm2d(1)
+// between the previous ReLU and this Linear): W' = s W, b' = b + t * sum_k W[n][k], folded in double
+int pack_linear(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT& b, const double* in_affine);
+// eval-mode BatchNorm2d(1) of (weight, bias, running_mean, running_var) -> (scale, shift) in double (eps 1e-5)
+void scalar_bn_affine(const float bn[4], double st[2]);
+// One bi_gru layer's input projection: per direction W_ih [768][K], b_ih and b_hh [768] -> both directions stacked, N = 1536,
+// bias b_ih + (b_hr, b_hz, 0)
+int pack_gru_ih(vf_ctx* ctx, GemmW* out, const HostT* const wi[2], const HostT* const bi[2], const HostT* const bh[2]);
 // Residual add of a vocoder stack as an identity tap (through the accumulator, no epilogue loads) up to this channel count;
 // above it the epilogue adds the hi/lo planes.  The packer appends the identity block and the plan builder adds the tap.
 constexpr int IDENT_MAX_C = 128;
@@ -379,6 +387,15 @@ void istft_params(vf_ctx* ctx, IstftFramesParams* fp, IstftOlaParams* op, const 
                   int T, float* frames, float* out, const int64_t* vl_off, const int* vl_T);
 // One bidirectional GRU layer (gru_tc.cu) on G [batch, T, 1536] into the [batch, T, 512] planes `out`, with its profile record
 Op gru_op(const float* G, const GruDirW (&dirs)[2], PlanePtr out, int batch, int T, int relu, const int* vl_T, const char* label);
+// The first GEMM operand of bi_gru / dnn: planes of scale * in + shift over [batch, T, 128] (zeros at t >= vl_T[b])
+Op planes_op(const float* in, int batch, int T, float scale, float shift, PlanePtr out, const int* vl_T);
+// One nn.Linear of an analysis module on [n_img, T, in.C] planes: a one-tap GEMM with W's bias; `e` carries the outputs, rows
+// t >= row_valid[img] are zeros
+void linear_gemm(Builder& b, std::vector<Op>& ops, const GemmW& W, const Planes& in, int T, int n_img, const int* row_valid,
+                 GemmEpilogue e, int terms);
+// The choices of a built OP_GEMM (tensor-core path) or OP_PAIR that select kernel code, as one string; "" for other ops.  Sizes
+// that only change occupancy (stages, grid) are left out.
+std::string op_signature(const Op& op);
 int build_plan(vf_ctx* ctx, Plan* plan);
 
 }  // namespace vf

@@ -296,33 +296,57 @@ int load_vocoder(vf_ctx* ctx) {
   return VF_OK;
 }
 
-// nn.Linear [N][K] (+ bias [N]) -> packed GEMM operand; with `in_affine` (s, t) the input is s * x + t (a BatchNorm2d(1)
-// between the previous ReLU and this Linear): W' = s W, b' = b + t * sum_k W[n][k], folded in double
-int pack_linear(vf_ctx* ctx, GemmW* out, const std::string& p, const double* in_affine = nullptr) {
-  NEED(w, p + ".weight");
-  NEED(b, p + ".bias");
-  if (w->shape.size() != 2 || b->v.size() != (size_t)w->shape[0]) return fail(ctx, VF_EINVAL, "%s: not a Linear layer", p.c_str());
-  const int N = (int)w->shape[0], K = (int)w->shape[1];
-  std::vector<float> m(w->v), bias(b->v);
+}  // namespace
+
+int pack_linear(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT& b, const double* in_affine) {
+  const int N = (int)w.shape[0], K = (int)w.shape[1];
+  std::vector<float> m(w.v), bias(b.v);
   if (in_affine) {
     for (int n = 0; n < N; ++n) {
       double rs = 0;
       for (int k = 0; k < K; ++k) {
-        rs += (double)w->v[(size_t)n * K + k];
-        m[(size_t)n * K + k] = (float)(in_affine[0] * (double)w->v[(size_t)n * K + k]);
+        rs += (double)w.v[(size_t)n * K + k];
+        m[(size_t)n * K + k] = (float)(in_affine[0] * (double)w.v[(size_t)n * K + k]);
       }
-      bias[n] = (float)((double)b->v[n] + in_affine[1] * rs);
+      bias[n] = (float)((double)b.v[n] + in_affine[1] * rs);
     }
   }
   return upload_gemm(ctx, out, m, N, K, &bias);
 }
 
-// eval-mode BatchNorm2d(1) -> (scale, shift) in double
+void scalar_bn_affine(const float bn[4], double st[2]) {
+  st[0] = (double)bn[0] / std::sqrt((double)bn[3] + 1e-5);
+  st[1] = (double)bn[1] - (double)bn[2] * st[0];
+}
+
+int pack_gru_ih(vf_ctx* ctx, GemmW* out, const HostT* const wi[2], const HostT* const bi[2], const HostT* const bh[2]) {
+  const int G3 = 3 * GRU_HIDDEN;
+  const int K = (int)(wi[0]->v.size() / G3);
+  std::vector<float> wih((size_t)2 * G3 * K), bias(2 * G3);
+  for (int d = 0; d < 2; ++d) {
+    std::copy(wi[d]->v.begin(), wi[d]->v.end(), wih.begin() + (size_t)d * G3 * K);
+    // b_hr and b_hz add to the input projection; b_hn stays inside r * (W_hn h + b_hn)
+    for (int j = 0; j < G3; ++j) bias[d * G3 + j] = j < 2 * GRU_HIDDEN ? bi[d]->v[j] + bh[d]->v[j] : bi[d]->v[j];
+  }
+  return upload_gemm(ctx, out, wih, 2 * G3, K, &bias);
+}
+
+namespace {
+
+// nn.Linear `p` of the state dict (pack_linear)
+int pack_linear(vf_ctx* ctx, GemmW* out, const std::string& p, const double* in_affine = nullptr) {
+  NEED(w, p + ".weight");
+  NEED(b, p + ".bias");
+  if (w->shape.size() != 2 || b->v.size() != (size_t)w->shape[0]) return fail(ctx, VF_EINVAL, "%s: not a Linear layer", p.c_str());
+  return pack_linear(ctx, out, *w, *b, in_affine);
+}
+
+// eval-mode BatchNorm2d(1) `p` of the state dict -> (scale, shift) in double (scalar_bn_affine)
 int scalar_bn(vf_ctx* ctx, const std::string& p, double* st) {
   NEED(w, p + ".weight"); NEED(b, p + ".bias"); NEED(m, p + ".running_mean"); NEED(v, p + ".running_var");
   if (w->v.size() != 1) return fail(ctx, VF_EINVAL, "%s: expected BatchNorm2d(1)", p.c_str());
-  st[0] = (double)w->v[0] / std::sqrt((double)v->v[0] + 1e-5);
-  st[1] = (double)b->v[0] - (double)m->v[0] * st[0];
+  const float bn[4] = {w->v[0], b->v[0], m->v[0], v->v[0]};
+  scalar_bn_affine(bn, st);
   return VF_OK;
 }
 
@@ -338,7 +362,7 @@ int load_bigru(vf_ctx* ctx, const std::string& A, BigruW* g) {
   const int G3 = 3 * GRU_HIDDEN;
   for (int l = 0; l < 2; ++l) {
     const int K = l ? 2 * GRU_HIDDEN : GRU_HIDDEN;
-    std::vector<float> wih((size_t)2 * G3 * K), bias(2 * G3);
+    const HostT *wis[2], *bis[2], *bhs[2];
     for (int d = 0; d < 2; ++d) {
       const std::string sfx = std::to_string(l) + (d ? "_reverse" : "");
       NEED(wi, A + "2.gru.weight_ih_l" + sfx); NEED(wh, A + "2.gru.weight_hh_l" + sfx);
@@ -346,13 +370,11 @@ int load_bigru(vf_ctx* ctx, const std::string& A, BigruW* g) {
       if (wi->v.size() != (size_t)G3 * K || wh->v.size() != (size_t)G3 * GRU_HIDDEN || bi->v.size() != (size_t)G3 ||
           bh->v.size() != (size_t)G3)
         return fail(ctx, VF_EINVAL, "%s2.gru layer %d: expected hidden size %d", A.c_str(), l, GRU_HIDDEN);
-      std::copy(wi->v.begin(), wi->v.end(), wih.begin() + (size_t)d * G3 * K);
-      // b_hr and b_hz add to the input projection; b_hn stays inside r * (W_hn h + b_hn)
-      for (int j = 0; j < G3; ++j) bias[d * G3 + j] = j < 2 * GRU_HIDDEN ? bi->v[j] + bh->v[j] : bi->v[j];
+      wis[d] = wi; bis[d] = bi; bhs[d] = bh;
       rc = upload(ctx, &g->dir[l][d].w_hh, wh->v); if (rc) return rc;
       rc = upload(ctx, &g->dir[l][d].b_hn, std::vector<float>(bh->v.begin() + 2 * GRU_HIDDEN, bh->v.end())); if (rc) return rc;
     }
-    rc = upload_gemm(ctx, &g->w_ih[l], wih, 2 * G3, K, &bias); if (rc) return rc;
+    rc = pack_gru_ih(ctx, &g->w_ih[l], wis, bis, bhs); if (rc) return rc;
   }
   rc = pack_linear(ctx, &g->lin_mid, A + "4"); if (rc) return rc;
   return pack_linear(ctx, &g->lin_out, A + "6");

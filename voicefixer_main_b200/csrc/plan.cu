@@ -781,6 +781,8 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
   return b.rc;
 }
 
+}  // namespace
+
 // The first GEMM operand of bi_gru / dnn: planes of scale * log-mel + shift (rows past a varlen clip's end are zeros)
 Op planes_op(const float* in, int batch, int T, float scale, float shift, PlanePtr out, const int* vl_T) {
   Op op; op.kind = OP_PLANES;
@@ -792,13 +794,45 @@ Op planes_op(const float* in, int batch, int T, float scale, float shift, PlaneP
   return op;
 }
 
-// One nn.Linear of an analysis module on [B, T, cin] planes: a one-tap GEMM with bias (taps1d(1, 1, cin, true)); `e` carries
-// the outputs.  Varlen rows past a clip's end are zeros.
-void linear(vf_ctx* ctx, Builder& b, Plan* plan, const GemmW& W, const Planes& in, GemmEpilogue e, const char* label) {
+// One nn.Linear: a one-tap GEMM with bias (taps1d(1, 1, cin, true))
+void linear_gemm(Builder& b, std::vector<Op>& ops, const GemmW& W, const Planes& in, int T, int n_img, const int* row_valid,
+                 GemmEpilogue e, int terms) {
   e.bias = W.bias;
-  e.row_valid = plan->vl(VL_T);
+  e.row_valid = row_valid;
+  b.gemm(ops, W, ASrc{in, T, 0}, nullptr, taps1d(1, 1, in.C, true), e, n_img, terms);
+}
+
+std::string op_signature(const Op& op) {
+  char s[160];
+  if (op.kind == OP_PAIR) {
+    snprintf(s, sizeof s, "pair last=%d varlen=%d", op.pair.ar_out == 0 ? 1 : 0, op.pair.row_valid ? 1 : 0);
+    return s;
+  }
+  if (op.kind != OP_GEMM) return "";
+  const GemmTcParams& tp = op.tc;
+  const GemmEpilogue& e = tp.prob.epi;
+  int sc = 0, ident = 0;
+  for (int i = 0; i < tp.prob.ntaps; ++i)
+    if (tp.prob.taps[i].src == 1) (tp.prob.taps[i].both ? ident : sc) = 1;
+  static const char* const maps[3] = {"plain", "convt2d", "convt1d"};
+  const char* resid = e.resid ? "fp32" : !e.resid_hi ? "none" : e.resid_ar ? "ar" : "planes";
+  std::string outs;
+  if (e.out_raw) outs += "raw,";
+  if (e.out_r.hi) outs += "r,";
+  if (e.out_a.hi) outs += e.out_ar ? "ar," : "a,";
+  if (!outs.empty()) outs.pop_back();
+  snprintf(s, sizeof s, "gemm map=%s terms=%d bn=%d bk=%d sc=%d identity=%d resid=%s resid_tma=%d out=%s tma_out=%d affine=%d act=%d head=%d varlen=%d",
+           maps[e.map], tp.prob.terms, op.bn, op.bk, sc, ident, resid, tp.resid_tma, outs.empty() ? "-" : outs.c_str(), e.tma_out,
+           e.a_scale ? 1 : 0, e.out_a.hi ? e.act : -1, e.head_w ? 1 : 0, e.row_valid ? 1 : 0);
+  return s;
+}
+
+namespace {
+
+// One nn.Linear of an analysis module on the plan's [B, T, cin] planes (linear_gemm); varlen rows past a clip's end are zeros
+void linear(vf_ctx* ctx, Builder& b, Plan* plan, const GemmW& W, const Planes& in, GemmEpilogue e, const char* label) {
   b.label = label;
-  b.gemm(plan->unet, W, ASrc{in, plan->T, 0}, nullptr, taps1d(1, 1, in.C, true), e, plan->batch, ctx->unet_terms);
+  linear_gemm(b, plan->unet, W, in, plan->T, plan->batch, plan->vl(VL_T), e, ctx->unet_terms);
 }
 
 // The module's last Linear: out_raw = d_logmel_out = Linear(x) + log-mel (gsr_voicefixer.py:90)

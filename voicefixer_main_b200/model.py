@@ -645,6 +645,17 @@ class Engine:
         with torch.cuda.device(self.device):
             self._ck(self.lib.vf_selftest_op(self.ctx, ctypes.byref(case)))
 
+    def selftest_plan_gemms(self, plan_kind: int, batch: int, frames: int):
+        """[(label, signature)] of every GEMM / fused-pair launch of a plan of plan_kind (0 GSR, 1 SSR, 2 GSR varlen, 3 SSR
+        varlen) built with the loaded weights and the current options; nothing is launched (vf_selftest_plan_gemms; tests
+        only)."""
+        cap, n = 2048, ctypes.c_int()
+        recs = (L.VfPlanGemm * cap)()
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_selftest_plan_gemms(self.ctx, plan_kind, batch, frames, recs, cap, ctypes.byref(n)))
+        assert n.value <= cap, n.value
+        return [(r.label.decode(), r.sig.decode()) for r in recs[:n.value]]
+
 
 # --------------------------------------------------------------------------------------------------------------
 class FDomainHelper:
