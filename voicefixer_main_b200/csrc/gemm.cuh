@@ -139,7 +139,7 @@ struct GemmTcParams {
 struct PairParams {
   CUtensorMap a_map;             // activated input plane lrelu(x), hi: [C, L, clips], box 64 x 128 x 1, SWIZZLE_128B
   CUtensorMap wa_map, wb_map;    // packed K-major hi weights [K >= 3C, C], box 64 x C
-  CUtensorMap xin_map[2];        // the activated and the correction plane of the source (box 64 x 126 x 1)
+  CUtensorMap xin_map;           // the correction plane of the source (box 64 x 126 x 1); its activated plane comes with the centre tap
   CUtensorMap xo_map;            // the correction plane of the destination (box 64 x 126 x 1); unused when ar_out == 0
   CUtensorMap ao_map;            // lrelu(x_new, slope_out), hi plane [C, out_row0 + L, clips] (box 64 x 126 x 1)
   const float* bias_a;

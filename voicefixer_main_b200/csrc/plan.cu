@@ -292,10 +292,9 @@ int pair_setup(vf_ctx* ctx, PairParams* pp, const Planes& src, const Planes& dst
   int rc = map_a(ctx, &pp->a_map, ASrc{src, L, 0}, src.p.hi, n_img, 64, false);
   if (!rc) rc = map_weights(ctx, &pp->wa_map, wa, wa.hi, 64, C, false);
   if (!rc) rc = map_weights(ctx, &pp->wb_map, wb, wb.hi, 64, C, false);
-  // the residual is rebuilt from the activated plane (an L2 hit: the centre tap just read these rows) and the correction
-  // plane; the new pair leaves as the two planes of `dst`
-  if (!rc) rc = map_rows(ctx, &pp->xin_map[0], src.p.hi, 2, C, L, (size_t)src.img_rows, n_img, 64, 126);
-  if (!rc) rc = map_rows(ctx, &pp->xin_map[1], src.p.lo, 2, C, L, (size_t)src.img_rows, n_img, 64, 126);
+  // the residual is rebuilt from the activated plane (the kernel takes it from the centre tap it has loaded) and the
+  // correction plane; the new pair leaves as the two planes of `dst`
+  if (!rc) rc = map_rows(ctx, &pp->xin_map, src.p.lo, 2, C, L, (size_t)src.img_rows, n_img, 64, 126);
   pp->ar_in = ar;
   if (!rc && !last) {
     pp->ar_out = ar;
