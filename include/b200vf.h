@@ -47,6 +47,8 @@
  *   vf_sosfiltfilt_varlen         the IIR types of tools/dsp/lowpass.py lowpass() / bandpass() (scipy sosfiltfilt)
  *   vf_resample_poly_f64_varlen   its "stft" type (resample_poly down and up), collate_fn_val's SR inputs
  *                                 dataloaders/data_module.py:130-150
+ *   vf_resample_sinc_varlen       librosa.load(sr=...)'s resampling as librosa 0.8 does it (resampy kaiser_best /
+ *                                 kaiser_fast), tools/utils.py:46-48 and metrics.py:33-34; opt-in (res_type)
  *
  * Conventions: every function returns 0 on success or a negative VF_E* code and never throws; the message is
  * available from vf_last_error().  All tensor arguments are contiguous fp32.  Unless a name ends in `_host`,
@@ -407,6 +409,22 @@ VF_API int vf_sosfiltfilt_varlen(vf_ctx* ctx, const double* x, const int64_t* of
 VF_API int vf_resample_poly_f64_varlen(vf_ctx* ctx, const double* x, const int64_t* in_offsets, int batch, const double* taps,
                                        const int64_t* tap_offsets, const int* up, const int* down, int n_filters,
                                        const int* row_filter, double* y, const int64_t* out_offsets, void* stream);
+/* librosa 0.8 resample(x, orig_sr, target_sr, res_type, fix=True) for res_type kaiser_best / kaiser_fast (resampy's sinc
+ * interpolation) of `batch` packed float32 rows: x packed with HOST in_offsets (every row at least 1 sample), y with HOST
+ * out_offsets.  Row i uses filter row_filter[i] (host) of `n_filters`: its table is tables[2 table_offsets[f] .. 2
+ * table_offsets[f + 1]) (device, 16-byte aligned; host table_offsets, in entries), nwin interleaved (win, delta) float64
+ * pairs as resampy hands them to its loop (win already multiplied by sample_ratio when it is below 1, delta = diff(win)
+ * with a last entry 0), for sample_ratio[f] = target_sr / orig_sr (host) and num_table[f] = 2^precision table entries per
+ * zero crossing (host).  Row i writes out_offsets[i + 1] - out_offsets[i] samples: resampy's first int(n sample_ratio) (a
+ * float64 product) and zeros past them, librosa's fix_length pad (a shorter output cuts).  The arithmetic is resampy's:
+ * float64 time register t / sample_ratio, float64 weights and products without FMA contraction, the output rounded to
+ * float32 after every tap.  A row's bits do not depend on its batch or position.  Every argument is checked before any work
+ * is queued (VF_EINVAL): a sample_ratio that is not positive, num_table < 1, an index step int(min(1, ratio) num_table) of
+ * 0, a table of at most num_table entries, a row filter out of range, a row whose int(n sample_ratio) is 0.  No scratch, no
+ * host synchronisation; one launch per 512 rows. */
+VF_API int vf_resample_sinc_varlen(vf_ctx* ctx, const float* x, const int64_t* in_offsets, int batch, const double* tables,
+                                   const int64_t* table_offsets, const double* sample_ratio, const int* num_table, int n_filters,
+                                   const int* row_filter, float* y, const int64_t* out_offsets, void* stream);
 
 VF_API int vf_to_log(vf_ctx* ctx, const float* in, float* out, int64_t n, void* stream);
 VF_API int vf_from_log(vf_ctx* ctx, const float* in, float* out, int64_t n, void* stream);

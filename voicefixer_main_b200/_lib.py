@@ -24,7 +24,7 @@ EXPORTS = [
     "vf_ssr_restore_varlen_mels", "vf_selftest_op", "vf_selftest_gru", "vf_score_time_varlen",
     "vf_sosfiltfilt_varlen", "vf_resample_poly_f64_varlen", "vf_metric_spectrogram_ex", "vf_score_varlen_ex",
     "vf_score_time_varlen_ex", "vf_restore_chunks", "vf_ssr_restore_chunks", "vf_restore_windows", "vf_ssr_restore_windows",
-    "vf_selftest_plan_gemms",
+    "vf_selftest_plan_gemms", "vf_resample_sinc_varlen",
 ]
 VF_RESTORE_UNIFY_ENERGY = 1
 VF_SSR_PEAK_NORMALISE = 1
@@ -197,6 +197,8 @@ def load_library():
                                           c_int, POINTER(c_int), POINTER(c_int), P, P]
     lib.vf_resample_poly_f64_varlen.argtypes = [P, P, POINTER(c_int64), c_int, P, POINTER(c_int64), POINTER(c_int),
                                                 POINTER(c_int), c_int, POINTER(c_int), P, POINTER(c_int64), P]
+    lib.vf_resample_sinc_varlen.argtypes = [P, P, POINTER(c_int64), c_int, P, POINTER(c_int64), POINTER(c_double),
+                                            POINTER(c_int), c_int, POINTER(c_int), P, POINTER(c_int64), P]
     _lib = lib
     return lib
 

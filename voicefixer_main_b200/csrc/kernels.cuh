@@ -463,4 +463,22 @@ struct ResampleF64Params {
 };
 cudaError_t launch_resample_f64(const ResampleF64Params& p, cudaStream_t stream);
 
+// sinc.cu: resampy's resample (librosa 0.8 resample, res_type kaiser_best / kaiser_fast) of packed float32 rows, one thread
+// per output sample.  Row b reads table tables[tab_at[b] ..][nwin[b]] of (win, delta) pairs, already scaled for its
+// sample_ratio ratio[b]; it writes out_off[b + 1] - out_off[b] samples, resampy's first n_valid[b] = int(n ratio) and
+// zeros past them (librosa's fix_length).  Everything travels in the parameters: no scratch, one launch per
+// SINC_MAX_ROWS rows.
+constexpr int SINC_MAX_ROWS = 512;                        // keeps SincParams under the 32 KiB kernel-parameter limit
+struct SincParams {
+  const float* x;
+  float* y;
+  const double2* tables;
+  int batch;
+  int64_t in_off[SINC_MAX_ROWS + 1], out_off[SINC_MAX_ROWS + 1];
+  int64_t tab_at[SINC_MAX_ROWS], nwin[SINC_MAX_ROWS], n_valid[SINC_MAX_ROWS];
+  double ratio[SINC_MAX_ROWS];
+  int num_table[SINC_MAX_ROWS];
+};
+cudaError_t launch_sinc_resample(const SincParams& p, cudaStream_t stream);
+
 }  // namespace vf

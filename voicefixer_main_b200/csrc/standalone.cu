@@ -602,6 +602,64 @@ VF_API int vf_resample_poly_f64_varlen(vf_ctx* ctx, const double* x, const int64
   return VF_OK;
 }
 
+// ------------------------------------------------------------------------------------------- librosa.load's resampling
+VF_API int vf_resample_sinc_varlen(vf_ctx* ctx, const float* x, const int64_t* in_offsets, int batch, const double* tables,
+                                   const int64_t* table_offsets, const double* sample_ratio, const int* num_table, int n_filters,
+                                   const int* row_filter, float* y, const int64_t* out_offsets, void* stream) {
+  static const char* fn = "vf_resample_sinc_varlen";
+  int rc = begin_call(ctx, fn, x && tables && table_offsets && sample_ratio && num_table && row_filter && y && batch > 0 &&
+                               n_filters > 0);
+  if (!rc && reinterpret_cast<uintptr_t>(tables) % alignof(double2) != 0)
+    rc = fail(ctx, VF_EINVAL, "%s: tables must be 16-byte aligned (interleaved double2)", fn);
+  if (!rc) rc = check_offsets(ctx, fn, "x", "row", in_offsets, batch, 1);
+  if (!rc) rc = check_offsets(ctx, fn, "y", "row", out_offsets, batch, 0);
+  if (rc) return rc;
+  if (table_offsets[0] != 0) return fail(ctx, VF_EINVAL, "%s: table offsets must start at 0", fn);
+  for (int f = 0; f < n_filters; ++f) {
+    const int64_t nwin = table_offsets[f + 1] - table_offsets[f];
+    const double r = sample_ratio[f];
+    if (!(r > 0.0) || !std::isfinite(r)) return fail(ctx, VF_EINVAL, "%s: filter %d: sample_ratio %g (need > 0)", fn, f, r);
+    if (num_table[f] < 1) return fail(ctx, VF_EINVAL, "%s: filter %d: num_table %d (need >= 1)", fn, f, num_table[f]);
+    if ((int64_t)(std::min(r, 1.0) * num_table[f]) < 1)
+      return fail(ctx, VF_EINVAL, "%s: filter %d: index step int(%g * %d) is 0", fn, f, std::min(r, 1.0), num_table[f]);
+    if (nwin <= num_table[f] || nwin > (int64_t(1) << 30))
+      return fail(ctx, VF_EINVAL, "%s: filter %d has %ld entries (need more than num_table %d)", fn, f, (long)nwin, num_table[f]);
+  }
+  std::vector<int64_t> n_valid(batch);
+  for (int i = 0; i < batch; ++i) {
+    const int f = row_filter[i];
+    if (f < 0 || f >= n_filters) return fail(ctx, VF_EINVAL, "%s: row %d: filter %d of %d", fn, i, f, n_filters);
+    const int64_t n = in_offsets[i + 1] - in_offsets[i];
+    n_valid[i] = (int64_t)((double)n * sample_ratio[f]);          // resampy's int(n * sample_ratio)
+    if (n_valid[i] < 1) return fail(ctx, VF_EINVAL, "%s: row %d has %ld samples, too few to resample by %g", fn, i, (long)n, sample_ratio[f]);
+  }
+  const std::vector<int> starts = split(batch, SINC_MAX_ROWS);
+  cudaError_t e = cudaSuccess;
+  for (size_t k = 0; k + 1 < starts.size() && e == cudaSuccess; ++k) {
+    const int s = starts[k], nb = starts[k + 1] - starts[k];
+    SincParams p;
+    memset(&p, 0, sizeof p);
+    p.batch = nb;
+    p.x = x + in_offsets[s];
+    p.y = y + out_offsets[s];
+    p.tables = reinterpret_cast<const double2*>(tables);
+    for (int i = 0; i < nb; ++i) {
+      const int f = row_filter[s + i];
+      p.in_off[i + 1] = in_offsets[s + i + 1] - in_offsets[s];
+      p.out_off[i + 1] = out_offsets[s + i + 1] - out_offsets[s];
+      p.tab_at[i] = table_offsets[f];
+      p.nwin[i] = table_offsets[f + 1] - table_offsets[f];
+      p.n_valid[i] = n_valid[s + i];
+      p.ratio[i] = sample_ratio[f];
+      p.num_table[i] = num_table[f];
+    }
+    e = launch_sinc_resample(p, (cudaStream_t)stream);
+    ctx->launches += 1;
+  }
+  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "sinc resample launch: %s", cudaGetErrorString(e));
+  return VF_OK;
+}
+
 // ------------------------------------------------------------------------------------------- finalize and conversions
 VF_API int vf_finalize(vf_ctx* ctx, const float* wav, int batch, int64_t len, int64_t n, float* wav_out, void* stream) {
   const int rc = begin_call(ctx, "vf_finalize", wav && wav_out && batch > 0 && len > 0 && n > 0);

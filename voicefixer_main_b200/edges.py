@@ -2,9 +2,12 @@
 
 * `resample_poly` / `resample_to`: zero-phase polyphase FIR rate conversion with the arithmetic of
   scipy.signal.resample_poly (Kaiser beta = 5 low-pass of 20 * max(up, down) + 1 taps), which is what the reference
-  itself uses to change rates (tools/dsp/lowpass.py:138-141).  The reference's `load_wav` (tools/utils.py:46-48) calls
-  librosa.load(sr=44100), whose resampler depends on the installed librosa (soxr_hq / kaiser_best) and is not available
-  offline; the FIR here is of the same class (windowed-sinc, > 60 dB stop band) and is checked against scipy.
+  itself uses to change rates (tools/dsp/lowpass.py:138-141).  This is the default (res_type=None) everywhere.
+* `resample` / `resample_to(..., res_type=...)`: what the reference's `load_wav` (tools/utils.py:46-48) and
+  AudioMetrics.read (metrics.py:33-34) actually do, librosa.load(sr=...) with librosa 0.8, whose default resampler is
+  resampy's "kaiser_best" sinc interpolation ("kaiser_fast" is its other filter).  Opt-in by res_type, named after
+  librosa's argument; vf_resample_sinc_varlen computes it.  Parity status: restated, unpinned (oracle/resampy.py lists
+  every choice; neither librosa nor resampy was available to check it against).  librosa >= 0.10's soxr_hq is not built.
 * `AudioMetrics.lsd` / `.sispec` / `.ssim`: evaluation_proc/metrics.py:83-106 for [B, C, T, F] tensors on the device, the
   metrics handler() logs per segment when a target is given (eval_gsr_voicefixer.py:56-64).
 * `AudioMetrics.wav_to_spectrogram` / `.evaluation` / `.evaluation_batch`: scoring a restored file against its clean target
@@ -70,10 +73,90 @@ def resample_poly(eng: Engine, x: torch.Tensor, up: int, down: int) -> torch.Ten
     return out
 
 
-def resample_to(eng: Engine, x: torch.Tensor, rate_in: int, rate_out: int = 44100) -> torch.Tensor:
-    """load_wav's rate conversion (tools/utils.py:46-48: librosa.load(path, sr=44100)) for a decoded signal."""
+def resample_to(eng: Engine, x: torch.Tensor, rate_in: int, rate_out: int = 44100, res_type: str = None) -> torch.Tensor:
+    """load_wav's rate conversion (tools/utils.py:46-48: librosa.load(path, sr=44100)) for decoded signals x [B, N]:
+    resample_poly (res_type=None), or librosa 0.8's resample with `res_type` (see resample)."""
+    if res_type is not None:
+        return torch.stack(resample(eng, list(x), rate_in, rate_out, res_type))
     fr = Fraction(int(rate_out), int(rate_in))
     return resample_poly(eng, x, fr.numerator, fr.denominator)
+
+
+# resampy's filters (resampy.filters.sinc_window parameters): res_type -> (num_zeros, precision, rolloff, Kaiser beta)
+RES_TYPES = {
+    "kaiser_best": (64, 9, 0.9475937167399596, 14.769656459379492),
+    "kaiser_fast": (16, 7, 0.85, 8.555504641634386),
+}
+
+
+def check_res_type(res_type) -> None:
+    """None (resample_poly) or one of RES_TYPES, else ValueError naming it."""
+    if res_type is not None and res_type not in RES_TYPES:
+        raise ValueError(f"unknown res_type {res_type!r}: need None, {' or '.join(map(repr, RES_TYPES))}")
+
+
+def sinc_lengths(n: int, orig_sr: int, target_sr: int):
+    """(resampy's int(n * ratio), librosa 0.8 resample's fix_length int(ceil(n * ratio))) for n samples, with the float64
+    ratio = target_sr / orig_sr.  ValueError, as resampy raises it, when the first is 0."""
+    ratio = float(target_sr) / orig_sr
+    n_valid = int(n * ratio)
+    if n_valid < 1:
+        raise ValueError(f"Input signal length={n} is too small to resample from {orig_sr}->{target_sr}")
+    return n_valid, int(np.ceil(n * ratio))
+
+
+def sinc_table(res_type: str, sample_ratio: float) -> np.ndarray:
+    """The float64 [nwin, 2] (win, delta) table resampy's loop reads for `res_type` at `sample_ratio`: resampy.filters'
+    sinc_window(num_zeros, precision, rolloff, window=kaiser(beta)) = kaiser(2 n + 1)[n:] * (rolloff * sinc(rolloff *
+    linspace(0, num_zeros, n + 1))) with n = 2^precision num_zeros, times sample_ratio when it is below 1; delta =
+    diff(win) with a last entry 0."""
+    from scipy.signal.windows import kaiser
+    num_zeros, precision, rolloff, beta = RES_TYPES[res_type]
+    n = 2 ** precision * num_zeros
+    win = kaiser(2 * n + 1, beta)[n:] * (rolloff * np.sinc(rolloff * np.linspace(0, num_zeros, num=n + 1, endpoint=True)))
+    if sample_ratio < 1:
+        win = win * sample_ratio
+    delta = np.zeros_like(win)
+    delta[:-1] = np.diff(win)
+    return np.stack([win, delta], axis=1)
+
+
+def _sinc_filter(eng: Engine, res_type: str, orig_sr: int, target_sr: int):
+    """(device table, sample_ratio, num_table) of Engine.resample_sinc_varlen, cached on the engine per (res_type, ratio)."""
+    ratio = float(target_sr) / orig_sr
+    cache = eng.__dict__.setdefault("_sinc_tables", {})
+    if (res_type, ratio) not in cache:
+        cache[res_type, ratio] = torch.from_numpy(sinc_table(res_type, ratio)).to(eng.device)
+    return cache[res_type, ratio], ratio, 2 ** RES_TYPES[res_type][1]
+
+
+def resample(eng: Engine, ys, orig_sr, target_sr: int, res_type: str = "kaiser_best") -> list:
+    """librosa 0.8 resample(y, orig_sr, target_sr, res_type, fix=True) of every 1-D float32 signal of `ys` (numpy arrays or
+    tensors), all in one vf_resample_sinc_varlen call: orig_sr is one rate for all, or one per signal.  -> list of float32
+    tensors on the engine's device; a signal already at target_sr comes back unchanged (on the device), as librosa returns
+    it.  resampy's int(n * ratio) samples, then zeros up to int(ceil(n * ratio)).  An unknown res_type, or a signal too short
+    for int(n * ratio) >= 1, raises ValueError before any GPU work."""
+    if res_type is None:
+        raise ValueError("resample: res_type None is resample_poly: call resample_to")
+    check_res_type(res_type)
+    rates = [int(orig_sr)] * len(ys) if np.ndim(orig_sr) == 0 else [int(r) for r in orig_sr]
+    if len(rates) != len(ys):
+        raise ValueError(f"resample: {len(rates)} rates for {len(ys)} signals")
+    todo = [i for i, r in enumerate(rates) if r != target_sr]
+    out_lengths = [sinc_lengths(int(np.prod(np.shape(ys[i]))), rates[i], target_sr)[1] for i in todo]
+    xs = [torch.as_tensor(y).to(eng.device, torch.float32).reshape(-1) for y in ys]
+    if not todo:
+        return xs
+    filters, keys, rows = [], {}, []
+    for i in todo:
+        if rates[i] not in keys:
+            keys[rates[i]] = len(filters)
+            filters.append(_sinc_filter(eng, res_type, rates[i], target_sr))
+        rows.append(keys[rates[i]])
+    y = eng.resample_sinc_varlen(torch.cat([xs[i] for i in todo]), [xs[i].numel() for i in todo], filters, rows, out_lengths)
+    for i, part in zip(todo, torch.split(y, out_lengths)):
+        xs[i] = part
+    return xs
 
 
 # AudioMetrics.evaluation's keys (metrics.py:70-78) in the column order of Engine.score_varlen
@@ -112,8 +195,10 @@ class AudioMetrics:
     """evaluation_proc/metrics.py:25-106 on the GPU: lsd, sispec and ssim of device tensors, the spectrogram and mel of a
     signal, and evaluation() of restored files against their targets."""
 
-    def __init__(self, owner, rate: int = 44100):
+    def __init__(self, owner, rate: int = 44100, res_type: str = None):
+        check_res_type(res_type)
         self.rate = rate
+        self.res_type = res_type
         self._owner = owner
 
     def _eng(self) -> Engine:
@@ -179,7 +264,8 @@ class AudioMetrics:
         librosa.load(sr=rate) does.  Every file is decoded and checked before any GPU work; a bad pair fails the whole call,
         naming the file: a target at the other of the two rates (NotImplementedError naming the rate= it needs) or at any
         other rate (ValueError), an est whose frame count differs from its target's or a pair of fewer than 7 frames
-        (ValueError).
+        (ValueError).  The instance's res_type (None: resample_poly) picks how an est at another rate is resampled; with
+        one, every such est goes through one edges.resample call, and the frame check uses librosa's resampled length.
 
         time_domain=True adds speechmetrics' sisdr and stoi (one more call, vf_score_time_varlen, on each file's first
         channel as speechmetrics reads it), and each dict is {"sisdr", "stoi", <the 8 spectral keys>} in metrics.py's
@@ -198,7 +284,7 @@ class AudioMetrics:
             e, e_rate = read_pcm16(est)
             if time_domain and e_rate != rate:
                 raise ValueError(f"{est} is at {e_rate} Hz: sisdr / stoi need it at its target's {rate} Hz")
-            te, tt = metric_frames(_rate_len(len(e), e_rate, rate), rate), metric_frames(len(t), rate)
+            te, tt = metric_frames(_rate_len(len(e), e_rate, rate, self.res_type), rate), metric_frames(len(t), rate)
             if te != tt:
                 raise ValueError(f"{est} has {te} frames at {rate} Hz, its target {target} {tt}")
             if tt < 7:
@@ -212,9 +298,14 @@ class AudioMetrics:
             return results
         eng = self._eng()
         at = {} if rate == 44100 else {"rate": rate}     # the 44.1 kHz calls are the entry points without a rate
-        ests = [_to_rate(path, e, e_rate, rate, eng) for path, e, e_rate, _ in live]
+        if self.res_type is None:
+            ests = [_to_rate(path, e, e_rate, rate, eng) for path, e, e_rate, _ in live]
+            est_packed = torch.from_numpy(np.concatenate(ests)).to(eng.device)
+        else:
+            ests = resample(eng, [e for _, e, _, _ in live], [e_rate for _, _, e_rate, _ in live], rate, self.res_type)
+            est_packed = torch.cat(ests)
         tgts = [t for _, _, _, t in live]
-        scores = eng.score_varlen(torch.from_numpy(np.concatenate(ests)).to(eng.device), [len(e) for e in ests],
+        scores = eng.score_varlen(est_packed, [len(e) for e in ests],
                                   torch.from_numpy(np.concatenate(tgts)).to(eng.device), [len(t) for t in tgts], **at).cpu()
         rows = iter(scores.tolist())
         if time_domain:

@@ -4,7 +4,8 @@ Same signature and contract as the reference handler that evaluation_proc/eval.p
     handler(input, output, target, ckpt, device, needrefresh=False, meta={}) -> dict of metrics
 It writes a 16-bit wav at `output`.  Differences, all outside the hot path: audio decoding uses the stdlib `wave`
 module (librosa / soundfile are not in this image): PCM16 wav of ANY sample rate, converted to 44.1 kHz on the GPU by
-the polyphase resampler (edges.py; load_wav -> librosa.load(sr=44100), tools/utils.py:46-48).  With a `target` the
+the polyphase resampler (edges.py; load_wav -> librosa.load(sr=44100), tools/utils.py:46-48), or with meta["res_type"]
+("kaiser_best" / "kaiser_fast") by librosa 0.8's own resampy filter, as the reference's load_wav does it.  With a `target` the
 per-segment mel metrics of eval_gsr_voicefixer.py:56-64 are computed on the GPU (lsd, sispec, non-log sispec, and with
 meta["mel_ssim"] the reference's `mel-ssim`, evaluation_proc/metrics.py:97-106).
 The segment loop, from_log, peak normalisation, trim_center, concat and the int16 conversion of
@@ -36,26 +37,33 @@ def read_pcm16(path):
     return (data.astype(np.float32) / 32768.0).mean(axis=1).astype(np.float32), rate
 
 
-def load_wav(path, sample_rate=44100, engine=None):
+def load_wav(path, sample_rate=44100, engine=None, res_type=None):
     """tools/utils.py:46-48 (librosa.load(path, sr=sample_rate)): decode + convert to `sample_rate`.  Rate conversion
-    runs on the GPU (`engine`, edges.resample_to); a file already at the target rate needs no engine."""
-    return _to_rate(path, *read_pcm16(path), sample_rate, engine)
+    runs on the GPU (`engine`, edges.resample_to): resample_poly, or librosa 0.8's resampy filter `res_type`
+    ("kaiser_best", "kaiser_fast"); a file already at the target rate needs no engine."""
+    from .edges import check_res_type
+    check_res_type(res_type)
+    return _to_rate(path, *read_pcm16(path), sample_rate, engine, res_type)
 
 
-def _to_rate(path, wav, rate, sample_rate, engine):
+def _to_rate(path, wav, rate, sample_rate, engine, res_type=None):
     """load_wav's conversion of decoded samples `wav` at `rate` to `sample_rate`."""
     if rate == sample_rate:
         return wav
     if engine is None:
         raise ValueError(f"{path}: {rate} Hz input needs an engine for the GPU resampler (pass engine=model._engine())")
     from .edges import resample_to
-    return resample_to(engine, torch.from_numpy(wav)[None].to(engine.device), rate, sample_rate)[0].cpu().numpy()
+    return resample_to(engine, torch.from_numpy(wav)[None].to(engine.device), rate, sample_rate, res_type)[0].cpu().numpy()
 
 
-def _rate_len(n, rate, sample_rate=44100):
-    """Length of what load_wav returns for n samples at `rate`: resample_poly's ceil(n * up / down)."""
+def _rate_len(n, rate, sample_rate=44100, res_type=None):
+    """Length of what load_wav returns for n samples at `rate`: resample_poly's ceil(n * up / down), or with a res_type
+    librosa 0.8's float int(ceil(n * (sample_rate / rate))) (ValueError when resampy's int(n * ratio) is 0)."""
     if rate == sample_rate:
         return n
+    if res_type is not None:
+        from .edges import sinc_lengths
+        return sinc_lengths(n, rate, sample_rate)[1]
     fr = Fraction(sample_rate, rate)
     return (n * fr.numerator + fr.denominator - 1) // fr.denominator
 
@@ -162,8 +170,9 @@ def handler(input, output, target, ckpt, device, needrefresh=False, meta={}):
     global model
     model = model.to(device)
     metrics = {}
-    wav_10k = load_wav(input, sample_rate=44100, engine=model._engine())
-    tgt = load_wav(target, sample_rate=44100, engine=model._engine()) if target is not None else None
+    res_type = meta.get("res_type")
+    wav_10k = load_wav(input, sample_rate=44100, engine=model._engine(), res_type=res_type)
+    tgt = load_wav(target, sample_rate=44100, engine=model._engine(), res_type=res_type) if target is not None else None
     out = restore_array(model, wav_10k, model.device, unify_energy=bool(meta.get("unify_energy", False)), target=tgt, metrics=metrics,
                         mel_ssim=bool(meta.get("mel_ssim", False)))
     # save_wave's float -> int16 conversion runs on the GPU (its `max <= 1` condition always holds after the
@@ -182,7 +191,8 @@ def handler_batch(items, ckpt, device, needrefresh=False, meta={}):
     (and one plan per distinct length) per segment.  Every file is decoded and checked before any GPU work: an item
     handler() would reject fails the whole call with handler()'s exception class, naming the file, and no file is written.
     needrefresh reloads the model once.  All segments and their mels are held on the device at once: split a test set too
-    large for that into several calls."""
+    large for that into several calls.  With meta["res_type"], every input and target not at 44.1 kHz is resampled in one
+    vf_resample_sinc_varlen call."""
     if needrefresh:
         refresh_model(ckpt)
     global model
@@ -192,16 +202,20 @@ def handler_batch(items, ckpt, device, needrefresh=False, meta={}):
     return restore_test_set(
         model, items, 2, mel_ssim, bool(meta.get("saturate", False)),
         lambda x, lengths, mel, log_mel: eng.restore_varlen(x, lengths, unify_energy=unify, mel_out=mel, log_mel_out=log_mel),
-        lambda tseg, mel, log_mel: _mel_metrics(model, tseg, mel, log_mel, unify, mel_ssim))
+        lambda tseg, mel, log_mel: _mel_metrics(model, tseg, mel, log_mel, unify, mel_ssim), meta.get("res_type"))
 
 
-def restore_test_set(mdl, items, n_mels, mel_ssim, saturate, restore, score):
+def restore_test_set(mdl, items, n_mels, mel_ssim, saturate, restore, score, res_type=None):
     """The body of handler_batch and handler_unet.handler_batch, which differ only in `restore` and `score`: the list of
     handler()'s dicts for `items`, and handler()'s output files, from batched restores.  Every item is decoded and checked
     (_check_file, with `mel_ssim`) before any GPU work.  Segments go longest first through
     restore(packed, lengths, *mel_bufs) -> the packed restored samples, where mel_bufs are `n_mels` packed [rows, 128]
     outputs when some item has a target and Nones otherwise.  score(tseg, *mels) -> dict scores a file's last segment: tseg
-    [1, 1, n] its target slice on the device, mels its [1, 1, T, 128] rows of each buffer.  Files are written last."""
+    [1, 1, n] its target slice on the device, mels its [1, 1, T, 128] rows of each buffer.  Files are written last.
+    res_type None converts every file with its own _to_rate; a res_type converts all inputs and targets in one
+    edges.resample call."""
+    from .edges import check_res_type, resample
+    check_res_type(res_type)
     eng = mdl._engine()
     items = [tuple(it) for it in items]
     if not items:
@@ -210,10 +224,19 @@ def restore_test_set(mdl, items, n_mels, mel_ssim, saturate, restore, score):
     for inp, _, tgt in items:
         x = read_pcm16(inp)
         t = read_pcm16(tgt) if tgt is not None else None
-        _check_file(inp, _rate_len(len(x[0]), x[1]), None if t is None else _rate_len(len(t[0]), t[1]), mel_ssim=mel_ssim)
+        _check_file(inp, _rate_len(len(x[0]), x[1], 44100, res_type),
+                    None if t is None else _rate_len(len(t[0]), t[1], 44100, res_type), mel_ssim=mel_ssim)
         decoded.append((x, t))
-    sigs = [_to_rate(inp, *x, 44100, eng) for (inp, _, _), (x, _) in zip(items, decoded)]
-    tgts = [None if t is None else _to_rate(tgt, *t, 44100, eng) for (_, _, tgt), (_, t) in zip(items, decoded)]
+    if res_type is None:
+        sigs = [_to_rate(inp, *x, 44100, eng) for (inp, _, _), (x, _) in zip(items, decoded)]
+        tgts = [None if t is None else _to_rate(tgt, *t, 44100, eng) for (_, _, tgt), (_, t) in zip(items, decoded)]
+    else:                       # inputs, then the targets there are, in one call; back to the host as _to_rate leaves them
+        ins = [x for x, t in decoded] + [t for x, t in decoded if t is not None]
+        rows = resample(eng, [w for w, _ in ins], [r for _, r in ins], 44100, res_type)
+        host = torch.cat(rows).cpu().numpy()
+        rows = np.split(host, np.cumsum([r.numel() for r in rows])[:-1])
+        sigs, rest = rows[:len(items)], iter(rows[len(items):])
+        tgts = [None if t is None else next(rest) for _, t in decoded]
     segs = [(f, s, e) for f, x in enumerate(sigs) for s, e in segment_bounds(len(x))]    # (file, start, end), file order
     want_mels = any(t is not None for t in tgts)
     pcm, mels = [None] * len(segs), [None] * len(segs)   # per segment: int16 samples; its [1, 1, T, 128] mel views

@@ -8,7 +8,7 @@ evaluation_proc/eval.py:128-132 calls:
 Per 60 s segment: restore; the linear mel of the restored output; with a target, the dict is replaced by the four mel metrics
 of that output against the target's mel (so the last segment's values come back); peak normalise when max|out| > 1.  The
 segments are concatenated and written as 16-bit PCM.  There is no unify_energy and no vocoder on this path; of `meta` only
-"saturate" is read (as handler.handler does).  Decoding, resampling and the file writes are handler.py's.
+"saturate" and "res_type" are read (as handler.handler reads them).  Decoding, resampling and the file writes are handler.py's.
 handler_batch(items, ...) is handler() over a whole list of files, with the same files and dicts, as batched restores.
 """
 import numpy as np
@@ -58,8 +58,9 @@ def handler(input, output, target, ckpt, device, needrefresh=False, meta={}):
     model = model.to(device)
     eng = model._engine()
     metrics = {}
-    wav_10k = load_wav(input, sample_rate=44100, engine=eng)
-    tgt = load_wav(target, sample_rate=44100, engine=eng) if target is not None else None
+    res_type = meta.get("res_type")
+    wav_10k = load_wav(input, sample_rate=44100, engine=eng, res_type=res_type)
+    tgt = load_wav(target, sample_rate=44100, engine=eng, res_type=res_type) if target is not None else None
     res = []
     for s, e in segment_bounds(wav_10k.shape[0]):
         seg = torch.from_numpy(np.ascontiguousarray(wav_10k[s:e]))[None, :].to(model.device)
@@ -96,4 +97,4 @@ def handler_batch(items, ckpt, device, needrefresh=False, meta={}):
     return restore_test_set(
         model, items, 1, True, bool(meta.get("saturate", False)),
         lambda x, lengths, mel: eng.ssr_restore_varlen(x, lengths, mel_out=mel, peak_normalise=True),
-        lambda tseg, mel: _mel_metrics(model, mel, tseg))
+        lambda tseg, mel: _mel_metrics(model, mel, tseg), meta.get("res_type"))

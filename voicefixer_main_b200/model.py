@@ -460,6 +460,25 @@ class Engine:
                                                           down, len(filters), rows, _ptr(out), out_off, _stream()))
         return out
 
+    def resample_sinc_varlen(self, x_packed: torch.Tensor, lengths, filters, row_filter, out_lengths) -> torch.Tensor:
+        """vf_resample_sinc_varlen: resampy's sinc resampling (librosa 0.8 resample, res_type kaiser_best / kaiser_fast) of
+        each float32 row of x_packed, row i with filter filters[row_filter[i]] = (table: float64 [nwin, 2] (win, delta) pairs
+        as edges.sinc_table designs them, sample_ratio, num_table) -> float32 rows of out_lengths[i] samples packed back to
+        back (resampy's int(n * sample_ratio), then zeros)."""
+        x_packed, off = self._varlen_args(x_packed, lengths)
+        out_lengths = [int(n) for n in out_lengths]
+        out_off = _offsets(out_lengths)
+        tables = torch.cat([t.to(self.device, torch.float64).reshape(-1, 2) for t, _, _ in filters]).contiguous()
+        table_off = _offsets([t.numel() // 2 for t, _, _ in filters])
+        ratio = (ctypes.c_double * len(filters))(*[float(r) for _, r, _ in filters])
+        num_table = (ctypes.c_int * len(filters))(*[int(k) for _, _, k in filters])
+        rows = (ctypes.c_int * len(row_filter))(*[int(f) for f in row_filter])
+        out = torch.empty(sum(out_lengths), device=self.device)
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_resample_sinc_varlen(self.ctx, _ptr(x_packed), off, len(off) - 1, _ptr(tables), table_off,
+                                                      ratio, num_table, len(filters), rows, _ptr(out), out_off, _stream()))
+        return out
+
     def amp_to_original_f(self, mel_est: torch.Tensor, mel_target: torch.Tensor) -> torch.Tensor:
         """tools/utils.py:50-55 on linear mels [B,T,128]: the estimate scaled to the target's low-band energy."""
         mel_est, mel_target = _check_in(mel_est, self.device, "mel_est"), _check_in(mel_target, self.device, "mel_target")
