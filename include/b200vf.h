@@ -151,7 +151,9 @@ VF_API int64_t vf_vocoder_out_len(vf_ctx* ctx, int frames);
 
 /* Fused stages A -> B -> C + peak normalise + centre trim: wav [B,N] -> wav_out [B,N] (device pointers). */
 VF_API int vf_restore(vf_ctx* ctx, const float* wav, int batch, int64_t n_samples, float* wav_out, void* stream);
-/* vf_restore with per-call behaviour flags (re-entrant: nothing is stored in the context). */
+/* vf_restore with per-call behaviour flags (re-entrant: nothing is stored in the context).  Every clip needs more than 1024
+ * samples and a length trim_center accepts; a bad argument fails before any work is queued, and a context without the
+ * analysis module or the vocoder with VF_ESTATE. */
 #define VF_RESTORE_UNIFY_ENERGY 1u   /* amp_to_original_f (tools/utils.py:50-55) as handler() applies it when
                                         meta["unify_energy"] is set, eval_gsr_voicefixer.py:54-55 */
 VF_API int vf_restore_ex(vf_ctx* ctx, const float* wav, int batch, int64_t n_samples, float* wav_out, unsigned flags,

@@ -120,7 +120,7 @@ def _raw_call(eng, packed, offsets, flags=0):
 
 def test_bad_calls_fail_and_leave_the_context_usable(model, state):
     from voicefixer_main_b200 import VoiceFixer
-    from voicefixer_main_b200._lib import VF_EINVAL
+    from voicefixer_main_b200._lib import VF_EINVAL, EngineError
     from voicefixer_main_b200.arch import VocoderConfig
     eng = model._engine()
     clips = _clips([5000, 20000], seed=900)
@@ -133,13 +133,24 @@ def test_bad_calls_fail_and_leave_the_context_usable(model, state):
     assert _raw_call(eng, packed, [0, 5000, 25000], flags=2) == VF_EINVAL          # unknown flag bits
     with pytest.raises(ValueError):
         model.restore_batch([clips[0], clips[1][:1000]])
+
+    def rejected_before_any_plan(eng, call):
+        # a fixed-shape call checks its arguments first: it builds no plan and launches nothing
+        plans, launches = eng.plan_cache_info()["plans"], eng.launch_count()
+        with pytest.raises(EngineError) as e:
+            call()
+        assert e.value.code == VF_EINVAL
+        assert (eng.plan_cache_info()["plans"], eng.launch_count()) == (plans, launches)
+
+    short = _clips([1024], seed=960)[0][None].contiguous()
+    rejected_before_any_plan(eng, lambda: model.restore(short))
+    rejected_before_any_plan(eng, lambda: model.restore_host(short.cpu().pin_memory(), torch.empty(1, 1024).pin_memory()))
     # trim_center's d == 1 case: no tail frames and an even frame count T with n = 441 (T - 1) + 440 samples
     m0 = VoiceFixer(vocoder_config=dataclasses.replace(VocoderConfig(), tail_pad_base=0)).load_state_dict(state).eval().to("cuda:0")
     e0 = m0._engine()
     bad = _clips([441 * 9 + 440], seed=990)[0]                                     # T = 10, L = 4410, d = 1
     assert _raw_call(e0, torch.cat([clips[0], bad]), [0, 5000, 5000 + bad.numel()]) == VF_EINVAL
-    with pytest.raises(Exception):
-        m0.restore(bad[None].contiguous())
+    rejected_before_any_plan(e0, lambda: m0.restore(bad[None].contiguous()))
     torch.cuda.synchronize()
     e0.check_errors()
     # nothing was launched by the rejected calls: the next call restores the same bits

@@ -44,15 +44,31 @@ int mark_use(vf_ctx* ctx, StreamOrder& o, cudaStream_t st) {
   return VF_OK;
 }
 
-int acquire_scratch(vf_ctx* ctx, Scratch& s, size_t need, cudaStream_t st) {
-  const int rc = order_use(ctx, s.order, st);
-  if (rc || need <= s.bytes) return rc;
+// Grows `s` to `need` bytes on `st`, stream-ordered (no host synchronisation), inside a use of it
+int grow_scratch(vf_ctx* ctx, Scratch& s, size_t need, cudaStream_t st) {
+  if (need <= s.bytes) return VF_OK;
   if (s.p) CK(cudaFreeAsync(s.p, st));
   s.p = nullptr;
   s.bytes = 0;
   CK(cudaMallocAsync(&s.p, need, st));
   s.bytes = need;
   return VF_OK;
+}
+
+// One use on `st` of a buffer that calls on any stream share: ordered after its previous use, then body(), then marked
+// on every path - a failed body included, whose earlier launches still read the buffer.  The body's error comes first.
+template <typename F>
+int with_use(vf_ctx* ctx, StreamOrder& o, cudaStream_t st, F body) {
+  int rc = order_use(ctx, o, st);
+  if (rc) return rc;
+  rc = body();
+  const int rm = mark_use(ctx, o, st);
+  return rc ? rc : rm;
+}
+
+int acquire_scratch(vf_ctx* ctx, Scratch& s, size_t need, cudaStream_t st) {
+  const int rc = order_use(ctx, s.order, st);
+  return rc ? rc : grow_scratch(ctx, s, need, st);
 }
 
 }  // namespace vf
@@ -183,15 +199,13 @@ int choose_sub_batch(vf_ctx* ctx, int kind, int batch, int frames) {
 
 // staging buffers for the host-pointer entry point, grown on demand
 int ensure_io(vf_ctx* ctx, Plan* plan, long n) {
-  if (plan->n_samples >= n && plan->d_wav) return VF_OK;
+  if (plan->n_samples >= n && plan->d_io[0][0]) return VF_OK;
   const size_t before = plan->bytes;
   Builder b{ctx, plan};
   for (int k = 0; k < 2; ++k) {
     plan->d_io[k][0] = b.alloc<float>((size_t)plan->batch * n);
     plan->d_io[k][1] = b.alloc<float>((size_t)plan->batch * n);
   }
-  plan->d_wav = plan->d_io[0][0];
-  plan->d_out = plan->d_io[0][1];
   plan->n_samples = n;
   ctx->plan_bytes += plan->bytes - before;
   return b.rc;
@@ -207,10 +221,10 @@ int host_roundtrip(vf_ctx* ctx, Plan* plan, const float* in_host, float* out_hos
   if (rc) return rc;
   const size_t bytes = (size_t)plan->batch * n * 4;
   if (!ctx->host_pipeline) {
-    CK(cudaMemcpyAsync(plan->d_wav, in_host, bytes, cudaMemcpyHostToDevice, st));
-    rc = body(plan->d_wav, plan->d_out, st);
+    CK(cudaMemcpyAsync(plan->d_io[0][0], in_host, bytes, cudaMemcpyHostToDevice, st));
+    rc = body(plan->d_io[0][0], plan->d_io[0][1], st);
     if (rc) return rc;
-    CK(cudaMemcpyAsync(out_host, plan->d_out, bytes, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(out_host, plan->d_io[0][1], bytes, cudaMemcpyDeviceToHost, st));
     return VF_OK;
   }
   if (!ctx->s_in) {
@@ -327,16 +341,10 @@ int run_chain(vf_ctx* ctx, Plan* plan, int slot, cudaStream_t st, int64_t n_laun
 
 int frames_of(vf_ctx* ctx, long n) { return 1 + (int)(n / ctx->cfg.hop); }
 
-int check_reflect(vf_ctx* ctx, long n) {
-  if (n <= 1024) return fail(ctx, VF_EINVAL, "reflect padding needs more than n_fft/2 = 1024 samples (got %ld)", n);
-  return VF_OK;
-}
-
 // vl_plan: a varlen plan whose lengths table holds the clips of `wav` (n is then the longest clip, T the plan's frames)
 int run_frontend(vf_ctx* ctx, const float* wav, int batch, long n, float* mel, float* logmel, float* sp, float* co,
                  float* si, cudaStream_t st, const Plan* vl_plan = nullptr) {
-  int rc = check_reflect(ctx, n);
-  if (rc) return rc;
+  if (n <= 1024) return fail(ctx, VF_EINVAL, "reflect padding needs more than n_fft/2 = 1024 samples (got %ld)", n);
   FrontendParams p;
   memset(&p, 0, sizeof p);
   p.wav = wav; p.n = n; p.batch = batch; p.T = frames_of(ctx, n);
@@ -384,21 +392,31 @@ int write_lengths_table(vf_ctx* ctx, Plan* plan, const int64_t* off, int batch, 
   return VF_OK;
 }
 
-// One restore chain on `plan`.  off == nullptr: `batch` clips of n samples (PLAN_GSR).  Otherwise clips of different
-// lengths (vf_restore_varlen): clip i = wav[off[i] .. off[i + 1]) (host offsets, off[0] = 0, validated by the caller), n = the
-// longest clip, `plan` the PLAN_VARLEN plan for the bucket of its frames; the output is packed like the input.
-int restore_impl(vf_ctx* ctx, Plan* plan, const float* wav, int batch, int64_t n, float* wav_out, unsigned flags, cudaStream_t st,
-                 const int64_t* off = nullptr) {
-  const int frames = plan->T;
+int no_post() { return VF_OK; }
+
+// One restore on `plan` inside one use of it: stage mark 0, the lengths table of a packed call (off: its clips' host
+// offsets rebased to the sub-batch, w0 the UNet's valid frequency bins), chain() - stages 1 to 3 -, stage mark 4, then
+// post(), the steps a packed call adds on the restored clips.
+template <typename Chain, typename Post = int (*)()>
+int run_restore(vf_ctx* ctx, Plan* plan, int w0, int batch, const int64_t* off, cudaStream_t st, Chain chain,
+                Post post = no_post) {
   if (ctx->op_timing) ctx->prof.clear();
-  int rc = order_use(ctx, plan->order, st);
-  if (rc) return rc;
-  rc = stage_mark(ctx, 0, st); if (rc) return rc;
-  if (off) {
-    rc = write_lengths_table(ctx, plan, off, batch, 127, st);
-    if (rc) return rc;
-  }
-  rc = run_frontend(ctx, wav, batch, (long)n, plan->d_mel, plan->d_logmel_in, nullptr, nullptr, nullptr, st, off ? plan : nullptr);
+  return with_use(ctx, plan->order, st, [&]() -> int {
+    int rc = stage_mark(ctx, 0, st);
+    if (!rc && off) rc = write_lengths_table(ctx, plan, off, batch, w0, st);
+    if (!rc) rc = chain();
+    if (!rc) rc = stage_mark(ctx, 4, st);
+    return rc ? rc : post();
+  });
+}
+
+// VoiceFixer's chain (run_restore's stages 1 to 3).  off == nullptr: `batch` clips of n samples (PLAN_GSR).  Otherwise
+// clips of different lengths (vf_restore_varlen): clip i = wav[off[i] .. off[i + 1]), n = the longest clip, `plan` the
+// PLAN_VARLEN plan for the bucket of its frames; the output is packed like the input.
+int restore_impl(vf_ctx* ctx, Plan* plan, const float* wav, int batch, int64_t n, float* wav_out, unsigned flags, cudaStream_t st,
+                 const int64_t* off) {
+  const int frames = plan->T;
+  int rc = run_frontend(ctx, wav, batch, (long)n, plan->d_mel, plan->d_logmel_in, nullptr, nullptr, nullptr, st, off ? plan : nullptr);
   if (rc) return rc;
   rc = stage_mark(ctx, 1, st); if (rc) return rc;
   const bool unify = (flags & VF_RESTORE_UNIFY_ENERGY) != 0;
@@ -427,24 +445,16 @@ int restore_impl(vf_ctx* ctx, Plan* plan, const float* wav, int batch, int64_t n
   if (rc) return rc;
   CK(launch_finalize(f, st));
   ctx->launches++;
-  rc = stage_mark(ctx, 4, st); if (rc) return rc;
-  return mark_use(ctx, plan->order, st);
+  return VF_OK;
 }
 
-// One SSR / GSR-UNet chain on `plan`: `batch` clips of n samples, magnitudes from the clips themselves (sp == nullptr) or sp.
-// off != nullptr: clips of different lengths (vf_ssr_restore_varlen) as in restore_impl, sp == nullptr, `plan` the
-// PLAN_SSR_VARLEN plan for the bucket of the longest clip's frames; rows t >= T_i of d_sp, d_mag and d_frames are never read.
+// The SSR / GSR-UNet chain: `batch` clips of n samples, magnitudes from the clips themselves (sp == nullptr) or sp.  off:
+// clips of different lengths (vf_ssr_restore_varlen) as in restore_impl, sp == nullptr, `plan` the PLAN_SSR_VARLEN plan for
+// the bucket of the longest clip's frames; rows t >= T_i of d_sp, d_mag and d_frames are never read.
 int ssr_impl(vf_ctx* ctx, Plan* plan, const float* sp, const float* wav, int batch, int64_t n, float* wav_out, cudaStream_t st,
-             const int64_t* off = nullptr) {
+             const int64_t* off) {
   const int frames = plan->T;
-  if (ctx->op_timing) ctx->prof.clear();
-  int rc = order_use(ctx, plan->order, st);
-  if (rc) return rc;
-  rc = stage_mark(ctx, 0, st); if (rc) return rc;
-  if (off) {
-    rc = write_lengths_table(ctx, plan, off, batch, 1024, st);
-    if (rc) return rc;
-  }
+  int rc = VF_OK;
   if (!sp) {     // SSR_UNet.pre (ssr_unet.py:140-143): the magnitude of the input itself
     rc = run_frontend(ctx, wav, batch, (long)n, nullptr, nullptr, plan->d_sp, nullptr, nullptr, st, off ? plan : nullptr);
     if (rc) return rc;
@@ -462,9 +472,54 @@ int ssr_impl(vf_ctx* ctx, Plan* plan, const float* sp, const float* wav, int bat
   CK(launch_istft_frames(fp, st));
   CK(launch_istft_ola(op, st));
   ctx->launches += 2;
-  rc = stage_mark(ctx, 3, st); if (rc) return rc;
-  rc = stage_mark(ctx, 4, st); if (rc) return rc;
-  return mark_use(ctx, plan->order, st);
+  return stage_mark(ctx, 3, st);
+}
+
+// What the restore calls of one model family need to know about it
+struct Family {
+  int fixed_kind, varlen_kind;   // plan kinds of its fixed-shape calls and of its packed ones
+  // the flag bits its calls accept; SSR_UNet's (VF_SSR_PEAK_NORMALISE) are vf_ssr_restore_varlen_mels', its other calls
+  // take no flags and pass 0
+  unsigned known_flags;
+  bool trim_center;              // the vocoder output is centre-cropped back to the input (eval_gsr_voicefixer.py:68-72)
+  int w0;                        // valid frequency bins of its UNet (lengths table): 127 (mel UNet) or 1024 (unet_v2)
+  // its chain for run_restore
+  int (*chain)(vf_ctx*, Plan*, const float* wav, int batch, int64_t n, float* out, unsigned flags, cudaStream_t st,
+               const int64_t* off);
+};
+const Family VOICEFIXER{PLAN_GSR, PLAN_VARLEN, VF_RESTORE_UNIFY_ENERGY, true, 127, restore_impl};
+const Family SSR_UNET{PLAN_SSR, PLAN_SSR_VARLEN, VF_SSR_PEAK_NORMALISE, false, 1024,
+                      [](vf_ctx* ctx, Plan* plan, const float* wav, int batch, int64_t n, float* out, unsigned, cudaStream_t st,
+                         const int64_t* off) { return ssr_impl(ctx, plan, nullptr, wav, batch, n, out, st, off); }};
+
+// run_restore of family f's chain
+template <typename Post = int (*)()>
+int restore_on(vf_ctx* ctx, const Family& f, Plan* plan, const float* wav, int batch, int64_t n, float* out, unsigned flags,
+               cudaStream_t st, const int64_t* off = nullptr, Post post = no_post) {
+  return run_restore(ctx, plan, f.w0, batch, off, st, [&] { return f.chain(ctx, plan, wav, batch, n, out, flags, st, off); }, post);
+}
+
+// For a family whose output is trim_center'ed, a vocoder output of n samples' input (T + T % 2 + tail_base frames of its
+// total upsampling) must exceed n by 0 or by at least 2.  `at` prefixes the message.
+int check_trim_center(vf_ctx* ctx, const Family& f, const char* at, int64_t n) {
+  if (!f.trim_center) return VF_OK;
+  long scale = 1;
+  for (int s = 0; s < ctx->cfg.voc_num_stages; ++s) scale *= ctx->cfg.voc_scales[s];
+  const int T = frames_of(ctx, (long)n);
+  const long d = (long)(T + T % 2 + ctx->cfg.voc_tail_base) * scale - (long)n;
+  if (d < 0 || d == 1)
+    return fail(ctx, VF_EINVAL, "%svocoder output length %ld incompatible with input %ld (trim_center)", at, (long)n + d, (long)n);
+  return VF_OK;
+}
+
+// The length checks of one item of n samples: more than n_fft/2 = 1024 (reflect padding), at most 2^30 in a packed call
+// (`item` names the item, null in a fixed-shape call), then check_trim_center.
+int check_length(vf_ctx* ctx, const Family& f, const char* item, int i, int64_t n) {
+  char at[32] = "";
+  if (item) snprintf(at, sizeof at, "%s %d: ", item, i);
+  if (n <= 1024) return fail(ctx, VF_EINVAL, "%sreflect padding needs more than n_fft/2 = 1024 samples (got %ld)", at, (long)n);
+  if (item && n > (int64_t)1 << 30) return fail(ctx, VF_EINVAL, "%s%ld samples is too long for one restore", at, (long)n);
+  return check_trim_center(ctx, f, at, n);
 }
 
 // A batched call as consecutive sub-batches of at most max_cb clips that fit the plan budget (choose_sub_batch, sized for
@@ -483,54 +538,30 @@ int run_sub_batches(vf_ctx* ctx, int kind, int batch, Frames frames, F body, int
   return VF_OK;
 }
 
-// Argument checks of a varlen entry point (`fn`) on plans of `kind`, all before anything is launched, so a rejected call
-// leaves no partial output and no work queued: a ready context, the pointers and batch, no flag bits outside `known_flags`,
-// offsets[0] == 0, the networks, then every clip (offsets increase, more than n_fft/2 samples, at most 2^30, and
-// per_clip(i, n) for checks of the entry point's own).
+// The fixed-shape calls of family f: `batch` clips of n samples as sub-batches, run(plan, off, b) restoring [off, off + b).
+// Every check comes first, so a rejected call builds no plan and queues no work.  VoiceFixer's networks are checked before
+// the length, whose trim_center bound is its vocoder's; SSR_UNet's after it, by the plan lookup.  Messages name `fn`, and
+// `flags_fn` for the flags.
 template <typename F>
-int check_varlen_call(vf_ctx* ctx, const char* fn, int kind, const float* wav, const int64_t* offsets, int batch,
-                      const float* wav_out, unsigned flags, unsigned known_flags, F per_clip) {
+int fixed_call(vf_ctx* ctx, const Family& f, const char* fn, const char* flags_fn, const void* in, int batch, int64_t n,
+               const void* out, unsigned flags, F run) {
   int rc = check_ready(ctx);
   if (rc) return rc;
-  if (!wav || !wav_out || !offsets || batch <= 0) return fail(ctx, VF_EINVAL, "%s: bad arguments", fn);
-  if (flags & ~known_flags) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
-  if (offsets[0] != 0) return fail(ctx, VF_EINVAL, "%s: offsets[0] must be 0 (got %ld)", fn, (long)offsets[0]);
-  rc = check_networks(ctx, kind);
+  if (!in || !out || batch <= 0) return fail(ctx, VF_EINVAL, "%s: bad arguments", fn);
+  if (flags & ~f.known_flags) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", flags_fn, flags);
+  if (f.trim_center && (rc = check_networks(ctx, f.fixed_kind))) return rc;
+  rc = check_length(ctx, f, nullptr, 0, n);
   if (rc) return rc;
-  for (int i = 0; i < batch; ++i) {
-    const int64_t n = offsets[i + 1] - offsets[i];
-    if (n <= 0) return fail(ctx, VF_EINVAL, "%s: offsets must increase (clip %d: %ld -> %ld)", fn, i, (long)offsets[i], (long)offsets[i + 1]);
-    if (n <= 1024) return fail(ctx, VF_EINVAL, "clip %d: reflect padding needs more than n_fft/2 = 1024 samples (got %ld)", i, (long)n);
-    if (n > (int64_t)1 << 30) return fail(ctx, VF_EINVAL, "clip %d: %ld samples is too long for one restore", i, (long)n);
-    rc = per_clip(i, n);
-    if (rc) return rc;
-  }
-  return VF_OK;
+  return run_sub_batches(ctx, f.fixed_kind, batch, [&](int, int) { return frames_of(ctx, (long)n); }, run);
 }
 
-// A varlen call (offsets validated by check_varlen_call) as consecutive sub-batches on plans of `kind` (plan budget, and the
-// lengths table's per-launch cap), each with its own bucket: body(plan, s, b, rel, n_max) runs clips [s, s + b), whose
-// offsets rebased to the sub-batch are rel[0..b] and whose longest clip has n_max samples.
-template <typename F>
-int run_varlen_sub_batches(vf_ctx* ctx, int kind, const int64_t* offsets, int batch, F body) {
-  auto longest = [&](int s, int b) {
-    int64_t n_max = 0;
-    for (int i = s; i < s + b; ++i) n_max = std::max(n_max, offsets[i + 1] - offsets[i]);
-    return n_max;
-  };
-  auto bucket = [&](int s, int b) { return round_up(frames_of(ctx, (long)longest(s, b)), 64); };
-  return run_sub_batches(ctx, kind, batch, bucket, [&](Plan* plan, int s, int b) {
-    int64_t rel[VL_MAX_CLIPS + 1];
-    for (int i = 0; i <= b; ++i) rel[i] = offsets[s + i] - offsets[s];
-    return body(plan, s, b, rel, longest(s, b));
-  }, VL_MAX_CLIPS);
-}
-
-// Packed frame offsets F_i = sum_{j<i} T_j of a varlen call's clips
-std::vector<int64_t> frame_offsets(vf_ctx* ctx, const int64_t* offsets, int batch) {
-  std::vector<int64_t> f(batch + 1, 0);
-  for (int i = 0; i < batch; ++i) f[i + 1] = f[i] + frames_of(ctx, (long)(offsets[i + 1] - offsets[i]));
-  return f;
+// vf_restore_host and vf_ssr_restore_host: fixed_call through the plans' host staging buffers
+int restore_host(vf_ctx* ctx, const Family& f, const char* fn, const float* wav_host, int batch, int64_t n, float* out_host,
+                 unsigned flags, cudaStream_t st) {
+  return fixed_call(ctx, f, fn, fn, wav_host, batch, n, out_host, flags, [&](Plan* plan, int off, int b) {
+    return host_roundtrip(ctx, plan, wav_host + (size_t)off * n, out_host + (size_t)off * n, (long)n, st,
+                          [&](const float* d_in, float* d_out, cudaStream_t s) { return restore_on(ctx, f, plan, d_in, b, n, d_out, flags, s); });
+  });
 }
 
 // One launch that gathers rows t < T_i of the sub-batch's [b, plan->T, 128] mel / logmel (either may be null with its
@@ -547,35 +578,52 @@ int gather_mels(vf_ctx* ctx, const Plan* plan, const std::vector<int64_t>& frame
   return VF_OK;
 }
 
-// vf_restore_varlen (`fn`) and vf_restore_varlen_mels.  With mel_out or log_mel_out, each sub-batch's restore is followed by
-// one gather of its clips' rows t < T_i into the packed outputs at frame offsets F_i = sum_{j<i} T_j, still inside the
-// plan's use on `stream` (mark_use again after it).
-// trim_center (eval_gsr_voicefixer.py:68-72) of the vocoder output of n samples back to n: that output is T + T % 2 +
-// tail_base frames of the vocoder's total upsampling, and the centre crop needs it to exceed n by 0 or by at least 2.  The
-// message names item i as `what` (clip, chunk).
-int check_trim_center(vf_ctx* ctx, const char* what, int i, int64_t n) {
-  long scale = 1;
-  for (int s = 0; s < ctx->cfg.voc_num_stages; ++s) scale *= ctx->cfg.voc_scales[s];
-  const int T = frames_of(ctx, (long)n);
-  const long d = (long)(T + T % 2 + ctx->cfg.voc_tail_base) * scale - (long)n;
-  if (d < 0 || d == 1) return fail(ctx, VF_EINVAL, "%s %d: vocoder output length %ld incompatible with input %ld (trim_center)", what, i, (long)n + d, (long)n);
-  return VF_OK;
+// The packed calls of family f (`fn`).  Every check comes before anything is launched, so a rejected call leaves no partial
+// output and no work queued.  Then per sub-batch the family's restore on its plan and post(plan, s, b, n_max, frame_off)
+// inside the same use of the plan, frame_off being the clips' packed frame offsets F_i = sum_{j<i} T_j.
+template <typename Post>
+int varlen_call(vf_ctx* ctx, const Family& f, const char* fn, const float* wav, const int64_t* offsets, int batch, float* wav_out,
+                unsigned flags, cudaStream_t st, Post post) {
+  int rc = check_ready(ctx);
+  if (rc) return rc;
+  if (!wav || !wav_out || !offsets || batch <= 0) return fail(ctx, VF_EINVAL, "%s: bad arguments", fn);
+  if (flags & ~f.known_flags) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
+  if (offsets[0] != 0) return fail(ctx, VF_EINVAL, "%s: offsets[0] must be 0 (got %ld)", fn, (long)offsets[0]);
+  rc = check_networks(ctx, f.varlen_kind);
+  if (rc) return rc;
+  for (int i = 0; i < batch; ++i) {
+    const int64_t n = offsets[i + 1] - offsets[i];
+    if (n <= 0) return fail(ctx, VF_EINVAL, "%s: offsets must increase (clip %d: %ld -> %ld)", fn, i, (long)offsets[i], (long)offsets[i + 1]);
+    rc = check_length(ctx, f, "clip", i, n);
+    if (rc) return rc;
+  }
+  std::vector<int64_t> frame_off(batch + 1, 0);
+  for (int i = 0; i < batch; ++i) frame_off[i + 1] = frame_off[i] + frames_of(ctx, (long)(offsets[i + 1] - offsets[i]));
+  auto longest = [&](int s, int b) {
+    int64_t n_max = 0;
+    for (int i = s; i < s + b; ++i) n_max = std::max(n_max, offsets[i + 1] - offsets[i]);
+    return n_max;
+  };
+  // sub-batches under the plan budget and the lengths table's per-launch cap, each on the bucket of its longest clip
+  auto bucket = [&](int s, int b) { return round_up(frames_of(ctx, (long)longest(s, b)), 64); };
+  return run_sub_batches(ctx, f.varlen_kind, batch, bucket, [&](Plan* plan, int s, int b) {
+    int64_t rel[VL_MAX_CLIPS + 1];      // the sub-batch's offsets, rebased
+    for (int i = 0; i <= b; ++i) rel[i] = offsets[s + i] - offsets[s];
+    const int64_t n_max = longest(s, b);
+    return restore_on(ctx, f, plan, wav + offsets[s], b, n_max, wav_out + offsets[s], flags, st, rel,
+                      [&] { return post(plan, s, b, n_max, frame_off); });
+  }, VL_MAX_CLIPS);
 }
 
+// vf_restore_varlen (`fn`) and vf_restore_varlen_mels.  With mel_out or log_mel_out, each sub-batch's restore is followed by
+// one gather of its clips' rows t < T_i into the packed outputs at frame offsets F_i = sum_{j<i} T_j.
 int restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t* offsets, int batch, float* wav_out,
                    unsigned flags, float* mel_out, float* log_mel_out, cudaStream_t st) {
-  int rc = check_varlen_call(ctx, fn, PLAN_VARLEN, wav, offsets, batch, wav_out, flags, VF_RESTORE_UNIFY_ENERGY,
-                             [&](int i, int64_t n) { return check_trim_center(ctx, "clip", i, n); });
-  if (rc) return rc;
-  const bool mels = mel_out || log_mel_out;
-  const std::vector<int64_t> frame_off = mels ? frame_offsets(ctx, offsets, batch) : std::vector<int64_t>();
-  return run_varlen_sub_batches(ctx, PLAN_VARLEN, offsets, batch, [&](Plan* plan, int s, int b, const int64_t* rel, int64_t n_max) {
-    int r = restore_impl(ctx, plan, wav + offsets[s], b, n_max, wav_out + offsets[s], flags, st, rel);
-    if (r || !mels) return r;
-    r = gather_mels(ctx, plan, frame_off, s, b, plan->d_mel, plan->d_logmel_out, mel_out, log_mel_out, st);
-    if (r) return r;
-    return mark_use(ctx, plan->order, st);
-  });
+  return varlen_call(ctx, VOICEFIXER, fn, wav, offsets, batch, wav_out, flags, st,
+                     [&](Plan* plan, int s, int b, int64_t, const std::vector<int64_t>& frame_off) {
+                       if (!mel_out && !log_mel_out) return VF_OK;
+                       return gather_mels(ctx, plan, frame_off, s, b, plan->d_mel, plan->d_logmel_out, mel_out, log_mel_out, st);
+                     });
 }
 
 // One row of a streaming call: `length` samples of stream `stream` from position `start` on; positions below 0 (a window's
@@ -677,9 +725,9 @@ struct OlaStage {
   }
 };
 
-// The streaming calls after their checks: per sub-batch one gather from the rings into the packed input scratch, chain(plan,
-// in, rows, n_max, out, off) - the varlen chain of `kind` on the packed rows at host offsets off[0..rows] - into the packed
-// output scratch, and stage.sub_batch on the restored rows; then stage.finish.
+// The streaming calls of family f after their checks: per sub-batch one gather from the rings into the packed input scratch,
+// the family's packed restore of the rows into the packed output scratch, and stage.sub_batch on the restored rows; then
+// stage.finish.
 //
 // Plan shapes: a streaming session's row count changes from step to step, and varlen plans are keyed by (batch, bucket),
 // so each sub-batch runs on the next power of two of its row count.  A sub-batch holds at most the largest power of two P
@@ -687,16 +735,16 @@ struct OlaStage {
 // nine batch shapes per bucket instead of one per row count, and they stay cached side by side instead of evicting one
 // another whenever the count crosses a power of two.  The rows past the sub-batch's own repeat its first row, whose results
 // are discarded: rows are independent, so they change no output sample, and unlike a row of digital silence they put nothing
-// through the chain that the call's own audio does not.  The cap follows the plan size per frame of `kind`
+// through the chain that the call's own audio does not.  The cap follows the plan size per frame of the family
 // (choose_sub_batch): an SSR varlen plan holds about 1.4 times a VoiceFixer one per padded frame, so its cap is reached at
 // shorter rows.
-template <typename Stage, typename Chain>
-int run_stream_rows(vf_ctx* ctx, int kind, const float* ring, int64_t ring_len, const std::vector<StreamRow>& rows_in,
-                    Stage& stage, cudaStream_t st, Chain chain) {
+template <typename Stage>
+int run_stream_rows(vf_ctx* ctx, const Family& f, const float* ring, int64_t ring_len, const std::vector<StreamRow>& rows_in,
+                    Stage& stage, unsigned flags, cudaStream_t st) {
   const int n_rows = (int)rows_in.size();
   int64_t longest = 0;
   for (const StreamRow& r : rows_in) longest = std::max(longest, r.length);
-  const int fit = choose_sub_batch(ctx, kind, 2 * VL_MAX_CLIPS, round_up(frames_of(ctx, (long)longest), 64));
+  const int fit = choose_sub_batch(ctx, f.varlen_kind, 2 * VL_MAX_CLIPS, round_up(frames_of(ctx, (long)longest), 64));
   int cap = 1;
   while (cap < VL_MAX_CLIPS && 4 * cap - 1 <= fit) cap *= 2;     // shapes 1, 2, .., 2 cap: 4 cap - 1 rows in all
   auto rows_of = [](int b) { int r = 1; while (r < b) r *= 2; return r; };
@@ -708,11 +756,11 @@ int run_stream_rows(vf_ctx* ctx, int kind, const float* ring, int64_t ring_len, 
     for (int k = 0; k < rows_of(b); ++k) n += row_at(s, b, k).length;
     max_samples = std::max(max_samples, n);
   }
-  int rc = acquire_scratch(ctx, ctx->chunks, (size_t)max_samples * 2 * sizeof(float), st);
-  if (rc) return rc;
-  float* in = static_cast<float*>(ctx->chunks.p);
-  float* out = in + max_samples;
-  auto run = [&]() -> int {
+  return with_use(ctx, ctx->chunks.order, st, [&]() -> int {
+    int rc = grow_scratch(ctx, ctx->chunks, (size_t)max_samples * 2 * sizeof(float), st);
+    if (rc) return rc;
+    float* in = static_cast<float*>(ctx->chunks.p);
+    float* out = in + max_samples;
     for (int s = 0; s < n_rows; s += cap) {
       const int b = std::min(cap, n_rows - s), rows = rows_of(b);
       ChunkGatherParams g;
@@ -730,34 +778,28 @@ int run_stream_rows(vf_ctx* ctx, int kind, const float* ring, int64_t ring_len, 
         n_max = std::max<int64_t>(n_max, c.length);
       }
       Plan* plan;
-      int r = get_plan(ctx, kind, rows, round_up(frames_of(ctx, (long)n_max), 64), &plan);
+      int r = get_plan(ctx, f.varlen_kind, rows, round_up(frames_of(ctx, (long)n_max), 64), &plan);
       if (r) return r;
       CK(launch_stream_gather(g, st));
       ctx->launches++;
-      r = chain(plan, in, rows, n_max, out, g.off);
+      r = restore_on(ctx, f, plan, in, rows, n_max, out, flags, st, g.off);
       if (r) return r;
       r = stage.sub_batch(ctx, s, b, g.off, out, st);
       if (r) return r;
     }
     return stage.finish(ctx, st);
-  };
-  rc = run();
-  const int rm = mark_use(ctx, ctx->chunks.order, st);
-  return rc ? rc : rm;
+  });
 }
 
-// vf_restore_chunks (`fn`, kind PLAN_VARLEN) and vf_ssr_restore_chunks (PLAN_SSR_VARLEN): every check before anything is
-// queued (per_chunk(i, length) for the entry point's own, after the length checks), then run_stream_rows with the crop into
-// kept_out.
-template <typename PerChunk, typename Chain>
-int restore_chunks(vf_ctx* ctx, const char* fn, int kind, const float* ring, int n_streams, int64_t ring_len,
-                   const vf_chunk* chunks, int n_chunks, float* kept_out, unsigned flags, unsigned known_flags, cudaStream_t st,
-                   PerChunk per_chunk, Chain chain) {
+// vf_restore_chunks and vf_ssr_restore_chunks (`fn`) of family f: every check before anything is queued, then
+// run_stream_rows with the crop into kept_out.
+int restore_chunks(vf_ctx* ctx, const Family& f, const char* fn, const float* ring, int n_streams, int64_t ring_len,
+                   const vf_chunk* chunks, int n_chunks, float* kept_out, unsigned flags, cudaStream_t st) {
   int rc = check_ready(ctx);
   if (rc) return rc;
   if (!ring || !chunks || !kept_out || n_streams <= 0 || ring_len <= 0 || n_chunks <= 0) return fail(ctx, VF_EINVAL, "%s: bad arguments", fn);
-  if (flags & ~known_flags) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
-  rc = check_networks(ctx, kind);
+  if (flags & ~f.known_flags) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
+  rc = check_networks(ctx, f.varlen_kind);
   if (rc) return rc;
   std::vector<StreamRow> rows(n_chunks);
   for (int i = 0; i < n_chunks; ++i) {
@@ -766,10 +808,7 @@ int restore_chunks(vf_ctx* ctx, const char* fn, int kind, const float* ring, int
       return fail(ctx, VF_EINVAL, "%s: chunk %d: stream %d is not in 0 .. %d", fn, i, c.stream, n_streams - 1);
     if (c.length > ring_len)
       return fail(ctx, VF_EINVAL, "%s: chunk %d: %d samples do not fit a ring of %ld", fn, i, c.length, (long)ring_len);
-    if (c.length <= 1024)
-      return fail(ctx, VF_EINVAL, "chunk %d: reflect padding needs more than n_fft/2 = 1024 samples (got %d)", i, c.length);
-    if (c.length > 1 << 30) return fail(ctx, VF_EINVAL, "chunk %d: %d samples is too long for one restore", i, c.length);
-    rc = per_chunk(i, (int64_t)c.length);
+    rc = check_length(ctx, f, "chunk", i, c.length);
     if (rc) return rc;
     if (c.crop_left < 0 || c.crop_right < 0 || (int64_t)c.crop_left + c.crop_right >= c.length)
       return fail(ctx, VF_EINVAL, "%s: chunk %d: crops %d and %d leave nothing of %d samples", fn, i, c.crop_left, c.crop_right, c.length);
@@ -777,31 +816,29 @@ int restore_chunks(vf_ctx* ctx, const char* fn, int kind, const float* ring, int
     rows[i] = StreamRow{c.stream, c.length, c.start, c.valid};
   }
   CropStage stage{chunks, kept_out, 0};
-  return run_stream_rows(ctx, kind, ring, ring_len, rows, stage, st, chain);
+  return run_stream_rows(ctx, f, ring, ring_len, rows, stage, flags, st);
 }
 
-// vf_restore_windows (`fn`, kind PLAN_VARLEN) and vf_ssr_restore_windows (PLAN_SSR_VARLEN): every check before anything is
-// queued (per_len(W) for the entry point's own, after the length checks), then run_stream_rows with the overlap-add and
-// the emission.  A stream's pending span is [start, start + acc_len) of its emission range: every accumulator slot a window
-// writes or the emission reads must lie in it, so no live partial sum of another position is overwritten.
-template <typename PerLen, typename Chain>
-int restore_windows(vf_ctx* ctx, const char* fn, int kind, const float* ring, int n_streams, int64_t ring_len,
+// vf_restore_windows and vf_ssr_restore_windows (`fn`) of family f: every check before anything is queued, then
+// run_stream_rows with the overlap-add and the emission.  A stream's pending span is [start, start + acc_len) of its
+// emission range: every accumulator slot a window writes or the emission reads must lie in it, so no live partial sum of
+// another position is overwritten.
+int restore_windows(vf_ctx* ctx, const Family& f, const char* fn, const float* ring, int n_streams, int64_t ring_len,
                     const vf_window* windows, int n_windows, int W, const float* synthesis, float* acc, int64_t acc_len,
-                    const vf_emit* emits, int n_emits, float* out, unsigned flags, unsigned known_flags, cudaStream_t st,
-                    PerLen per_len, Chain chain) {
+                    const vf_emit* emits, int n_emits, float* out, unsigned flags, cudaStream_t st) {
   int rc = check_ready(ctx);
   if (rc) return rc;
   if (!ring || !windows || !acc || !emits || n_streams <= 0 || ring_len <= 0 || n_windows <= 0 || acc_len <= 0 ||
       n_emits <= 0)
     return fail(ctx, VF_EINVAL, "%s: bad arguments", fn);
   if (!synthesis) return fail(ctx, VF_EINVAL, "%s: no synthesis window table", fn);
-  if (flags & ~known_flags) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
-  rc = check_networks(ctx, kind);
+  if (flags & ~f.known_flags) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
+  rc = check_networks(ctx, f.varlen_kind);
   if (rc) return rc;
   if (W > ring_len) return fail(ctx, VF_EINVAL, "%s: windows of %d samples do not fit a ring of %ld", fn, W, (long)ring_len);
   if (W <= 1024) return fail(ctx, VF_EINVAL, "%s: reflect padding needs more than n_fft/2 = 1024 samples (windows of %d)", fn, W);
   if (W > 1 << 30) return fail(ctx, VF_EINVAL, "%s: windows of %d samples are too long for one restore", fn, W);
-  rc = per_len((int64_t)W);
+  rc = check_trim_center(ctx, f, "window 0: ", W);
   if (rc) return rc;
   std::vector<int64_t> from(n_streams, -1);         // each stream's pending span begins at its emission range
   for (int e = 0; e < n_emits; ++e) {
@@ -835,7 +872,7 @@ int restore_windows(vf_ctx* ctx, const char* fn, int kind, const float* ring, in
     rows[i] = StreamRow{w.stream, W, w.start, w.valid};
   }
   OlaStage stage{windows, W, synthesis, acc, acc_len, emits, n_emits, out};
-  return run_stream_rows(ctx, kind, ring, ring_len, rows, stage, st, chain);
+  return run_stream_rows(ctx, f, ring, ring_len, rows, stage, flags, st);
 }
 
 // vf_ssr_restore_varlen (`fn`) and vf_ssr_restore_varlen_mels.  After each sub-batch's ISTFT, still inside the plan's use on
@@ -843,19 +880,14 @@ int restore_windows(vf_ctx* ctx, const char* fn, int kind, const float* ring, in
 // VF_SSR_PEAK_NORMALISE, the per-clip peak normalise of wav_out, after the mel is taken.
 int ssr_restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t* offsets, int batch, float* wav_out,
                        unsigned flags, float* mel_out, cudaStream_t st) {
-  int rc = check_varlen_call(ctx, fn, PLAN_SSR_VARLEN, wav, offsets, batch, wav_out, flags, VF_SSR_PEAK_NORMALISE,
-                             [](int, int64_t) { return VF_OK; });
-  if (rc) return rc;
   const bool peak = (flags & VF_SSR_PEAK_NORMALISE) != 0;
-  const std::vector<int64_t> frame_off = mel_out ? frame_offsets(ctx, offsets, batch) : std::vector<int64_t>();
-  return run_varlen_sub_batches(ctx, PLAN_SSR_VARLEN, offsets, batch, [&](Plan* plan, int s, int b, const int64_t* rel, int64_t n_max) {
+  return varlen_call(ctx, SSR_UNET, fn, wav, offsets, batch, wav_out, flags, st,
+                     [&](Plan* plan, int s, int b, int64_t n_max, const std::vector<int64_t>& frame_off) -> int {
     float* out = wav_out + offsets[s];
-    int r = ssr_impl(ctx, plan, nullptr, wav + offsets[s], b, n_max, out, st, rel);
-    if (r || (!mel_out && !peak)) return r;
     if (mel_out) {
       // mel(wav_to_spectrogram_phase(out)[0]) (eval_gsr_unet.py:54-55).  The ISTFT frames are dead once the overlap-add
       // has run, so they hold the mels at the bucket's row stride ([b, T, 128] of the [b, T, 2048] buffer).
-      r = run_frontend(ctx, out, b, (long)n_max, plan->d_frames, nullptr, nullptr, nullptr, nullptr, st, plan);
+      int r = run_frontend(ctx, out, b, (long)n_max, plan->d_frames, nullptr, nullptr, nullptr, nullptr, st, plan);
       if (r) return r;
       r = gather_mels(ctx, plan, frame_off, s, b, plan->d_frames, nullptr, mel_out, nullptr, st);
       if (r) return r;
@@ -865,7 +897,7 @@ int ssr_restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int6
       CK(launch_peak_normalise_varlen(out, plan->d_vl_off, b, (long)n_max, plan->d_peak, st));
       ctx->launches += 2;
     }
-    return mark_use(ctx, plan->order, st);
+    return VF_OK;
   });
 }
 
@@ -989,14 +1021,14 @@ VF_API int vf_unet_mel(vf_ctx* ctx, const float* mel_lin, int batch, int frames,
   rc = get_plan(ctx, PLAN_GSR, batch, frames, &plan);
   if (rc) return rc;
   const size_t n = (size_t)batch * frames * 128;
-  rc = order_use(ctx, plan->order, st);
-  if (rc) return rc;
-  CK(launch_to_log(mel_lin, plan->d_logmel_in, n, ctx->d_err + 1, st));
-  ctx->launches++;
-  rc = run_ops(ctx, plan->unet, st);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(logmel_out, plan->d_logmel_out, n * 4, cudaMemcpyDeviceToDevice, st));
-  return mark_use(ctx, plan->order, st);
+  return with_use(ctx, plan->order, st, [&]() -> int {
+    CK(launch_to_log(mel_lin, plan->d_logmel_in, n, ctx->d_err + 1, st));
+    ctx->launches++;
+    const int r = run_ops(ctx, plan->unet, st);
+    if (r) return r;
+    CK(cudaMemcpyAsync(logmel_out, plan->d_logmel_out, n * 4, cudaMemcpyDeviceToDevice, st));
+    return VF_OK;
+  });
 }
 
 VF_API int64_t vf_vocoder_out_len(vf_ctx* ctx, int frames) {
@@ -1012,27 +1044,23 @@ VF_API int vf_vocoder(vf_ctx* ctx, const float* mel_lin, int batch, int frames, 
   Plan* plan;
   rc = get_plan(ctx, PLAN_GSR, batch, frames, &plan);
   if (rc) return rc;
-  rc = order_use(ctx, plan->order, st);
-  if (rc) return rc;
-  Op& cop = plan->vocoder[plan->cond_op];
-  cop.cond.mel = mel_lin;
-  cop.cond.is_log = 0;
-  cop.cond.band_sums = nullptr;
-  rc = run_ops(ctx, plan->vocoder, st);
-  cop.cond.mel = plan->d_logmel_out;
-  cop.cond.is_log = 1;
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(wav_out, plan->d_voc_wav, (size_t)batch * plan->L * 4, cudaMemcpyDeviceToDevice, st));
-  return mark_use(ctx, plan->order, st);
+  return with_use(ctx, plan->order, st, [&]() -> int {
+    Op& cop = plan->vocoder[plan->cond_op];
+    cop.cond.mel = mel_lin;
+    cop.cond.is_log = 0;
+    cop.cond.band_sums = nullptr;
+    const int r = run_ops(ctx, plan->vocoder, st);
+    cop.cond.mel = plan->d_logmel_out;
+    cop.cond.is_log = 1;
+    if (r) return r;
+    CK(cudaMemcpyAsync(wav_out, plan->d_voc_wav, (size_t)batch * plan->L * 4, cudaMemcpyDeviceToDevice, st));
+    return VF_OK;
+  });
 }
 
 VF_API int vf_restore_ex(vf_ctx* ctx, const float* wav, int batch, int64_t n, float* wav_out, unsigned flags, void* stream) {
-  int rc = check_ready(ctx);
-  if (rc) return rc;
-  if (!wav || !wav_out || batch <= 0) return fail(ctx, VF_EINVAL, "vf_restore: bad arguments");
-  if (flags & ~(unsigned)VF_RESTORE_UNIFY_ENERGY) return fail(ctx, VF_EINVAL, "vf_restore_ex: unknown flag bits 0x%x", flags);
-  return run_sub_batches(ctx, PLAN_GSR, batch, [&](int, int) { return frames_of(ctx, (long)n); }, [&](Plan* plan, int off, int b) {
-    return restore_impl(ctx, plan, wav + (size_t)off * n, b, n, wav_out + (size_t)off * n, flags, (cudaStream_t)stream);
+  return fixed_call(ctx, VOICEFIXER, "vf_restore", "vf_restore_ex", wav, batch, n, wav_out, flags, [&](Plan* plan, int off, int b) {
+    return restore_on(ctx, VOICEFIXER, plan, wav + (size_t)off * n, b, n, wav_out + (size_t)off * n, flags, (cudaStream_t)stream);
   });
 }
 
@@ -1049,24 +1077,15 @@ VF_API int vf_restore_varlen_mels(vf_ctx* ctx, const float* wav, const int64_t* 
 
 VF_API int vf_restore_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_chunk* chunks, int n_chunks,
                              float* kept_out, unsigned flags, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  return restore_chunks(ctx, "vf_restore_chunks", PLAN_VARLEN, ring, n_streams, ring_len, chunks, n_chunks, kept_out, flags,
-                        VF_RESTORE_UNIFY_ENERGY, st, [&](int i, int64_t n) { return check_trim_center(ctx, "chunk", i, n); },
-                        [&](Plan* plan, const float* in, int rows, int64_t n_max, float* out, const int64_t* off) {
-                          return restore_impl(ctx, plan, in, rows, n_max, out, flags, st, off);
-                        });
+  return restore_chunks(ctx, VOICEFIXER, "vf_restore_chunks", ring, n_streams, ring_len, chunks, n_chunks, kept_out, flags,
+                        (cudaStream_t)stream);
 }
 
 VF_API int vf_restore_windows(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_window* windows,
                               int n_windows, int window_len, const float* synthesis, float* acc, int64_t acc_len,
                               const vf_emit* emits, int n_emits, float* out, unsigned flags, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  return restore_windows(ctx, "vf_restore_windows", PLAN_VARLEN, ring, n_streams, ring_len, windows, n_windows, window_len,
-                         synthesis, acc, acc_len, emits, n_emits, out, flags, VF_RESTORE_UNIFY_ENERGY, st,
-                         [&](int64_t n) { return check_trim_center(ctx, "window", 0, n); },
-                         [&](Plan* plan, const float* in, int rows, int64_t n_max, float* o, const int64_t* off) {
-                           return restore_impl(ctx, plan, in, rows, n_max, o, flags, st, off);
-                         });
+  return restore_windows(ctx, VOICEFIXER, "vf_restore_windows", ring, n_streams, ring_len, windows, n_windows, window_len,
+                         synthesis, acc, acc_len, emits, n_emits, out, flags, (cudaStream_t)stream);
 }
 
 VF_API int vf_restore(vf_ctx* ctx, const float* wav, int batch, int64_t n, float* wav_out, void* stream) {
@@ -1074,27 +1093,18 @@ VF_API int vf_restore(vf_ctx* ctx, const float* wav, int batch, int64_t n, float
 }
 
 VF_API int vf_restore_host(vf_ctx* ctx, const float* wav_host, int batch, int64_t n, float* out_host, void* stream) {
-  int rc = check_ready(ctx);
-  if (rc) return rc;
-  if (!wav_host || !out_host || batch <= 0) return fail(ctx, VF_EINVAL, "vf_restore_host: bad arguments");
-  cudaStream_t st = (cudaStream_t)stream;
-  const unsigned flags = ctx->unify_energy ? VF_RESTORE_UNIFY_ENERGY : 0u;
-  return run_sub_batches(ctx, PLAN_GSR, batch, [&](int, int) { return frames_of(ctx, (long)n); }, [&](Plan* plan, int off, int b) {
-    return host_roundtrip(ctx, plan, wav_host + (size_t)off * n, out_host + (size_t)off * n, (long)n, st,
-                          [&](const float* d_in, float* d_out, cudaStream_t s) { return restore_impl(ctx, plan, d_in, b, n, d_out, flags, s); });
-  });
+  return restore_host(ctx, VOICEFIXER, "vf_restore_host", wav_host, batch, n, out_host,
+                      ctx && ctx->unify_energy ? VF_RESTORE_UNIFY_ENERGY : 0u, (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------------------------------------- SSR / GSR-UNet path
 VF_API int vf_ssr_forward(vf_ctx* ctx, const float* sp, const float* wav, int batch, int64_t n, float* wav_out, void* stream) {
-  int rc = check_ready(ctx);
-  if (rc) return rc;
-  if (!wav || !wav_out || batch <= 0) return fail(ctx, VF_EINVAL, "vf_ssr_forward: bad arguments");
-  rc = check_reflect(ctx, (long)n);
-  if (rc) return rc;
-  const int frames = frames_of(ctx, (long)n);
-  return run_sub_batches(ctx, PLAN_SSR, batch, [=](int, int) { return frames; }, [&](Plan* plan, int off, int b) {
-    return ssr_impl(ctx, plan, sp ? sp + (size_t)off * frames * 1025 : nullptr, wav + (size_t)off * n, b, n, wav_out + (size_t)off * n, (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  return fixed_call(ctx, SSR_UNET, "vf_ssr_forward", "vf_ssr_forward", wav, batch, n, wav_out, 0u, [&](Plan* plan, int off, int b) {
+    return run_restore(ctx, plan, SSR_UNET.w0, b, nullptr, st, [&] {   // a caller's sp: SSR_UNET.chain with it
+      return ssr_impl(ctx, plan, sp ? sp + (size_t)off * plan->T * 1025 : nullptr, wav + (size_t)off * n, b, n,
+                      wav_out + (size_t)off * n, st, nullptr);
+    });
   });
 }
 
@@ -1114,36 +1124,19 @@ VF_API int vf_ssr_restore_varlen_mels(vf_ctx* ctx, const float* wav, const int64
 
 VF_API int vf_ssr_restore_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_chunk* chunks,
                                  int n_chunks, float* kept_out, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  return restore_chunks(ctx, "vf_ssr_restore_chunks", PLAN_SSR_VARLEN, ring, n_streams, ring_len, chunks, n_chunks, kept_out,
-                        0u, 0u, st, [](int, int64_t) { return VF_OK; },
-                        [&](Plan* plan, const float* in, int rows, int64_t n_max, float* out, const int64_t* off) {
-                          return ssr_impl(ctx, plan, nullptr, in, rows, n_max, out, st, off);
-                        });
+  return restore_chunks(ctx, SSR_UNET, "vf_ssr_restore_chunks", ring, n_streams, ring_len, chunks, n_chunks, kept_out, 0u,
+                        (cudaStream_t)stream);
 }
 
 VF_API int vf_ssr_restore_windows(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_window* windows,
                                   int n_windows, int window_len, const float* synthesis, float* acc, int64_t acc_len,
                                   const vf_emit* emits, int n_emits, float* out, void* stream) {
-  cudaStream_t st = (cudaStream_t)stream;
-  return restore_windows(ctx, "vf_ssr_restore_windows", PLAN_SSR_VARLEN, ring, n_streams, ring_len, windows, n_windows,
-                         window_len, synthesis, acc, acc_len, emits, n_emits, out, 0u, 0u, st, [](int64_t) { return VF_OK; },
-                         [&](Plan* plan, const float* in, int rows, int64_t n_max, float* o, const int64_t* off) {
-                           return ssr_impl(ctx, plan, nullptr, in, rows, n_max, o, st, off);
-                         });
+  return restore_windows(ctx, SSR_UNET, "vf_ssr_restore_windows", ring, n_streams, ring_len, windows, n_windows, window_len,
+                         synthesis, acc, acc_len, emits, n_emits, out, 0u, (cudaStream_t)stream);
 }
 
 VF_API int vf_ssr_restore_host(vf_ctx* ctx, const float* wav_host, int batch, int64_t n, float* out_host, void* stream) {
-  int rc = check_ready(ctx);
-  if (rc) return rc;
-  if (!wav_host || !out_host || batch <= 0) return fail(ctx, VF_EINVAL, "vf_ssr_restore_host: bad arguments");
-  rc = check_reflect(ctx, (long)n);
-  if (rc) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  return run_sub_batches(ctx, PLAN_SSR, batch, [&](int, int) { return frames_of(ctx, (long)n); }, [&](Plan* plan, int off, int b) {
-    return host_roundtrip(ctx, plan, wav_host + (size_t)off * n, out_host + (size_t)off * n, (long)n, st,
-                          [&](const float* d_in, float* d_out, cudaStream_t s) { return ssr_impl(ctx, plan, nullptr, d_in, b, n, d_out, s); });
-  });
+  return restore_host(ctx, SSR_UNET, "vf_ssr_restore_host", wav_host, batch, n, out_host, 0u, (cudaStream_t)stream);
 }
 
 VF_API int vf_ssr_unet(vf_ctx* ctx, const float* sp, int batch, int frames, float* mag_out, void* stream) {
@@ -1155,13 +1148,13 @@ VF_API int vf_ssr_unet(vf_ctx* ctx, const float* sp, int batch, int frames, floa
   rc = get_plan(ctx, PLAN_SSR, batch, frames, &plan);
   if (rc) return rc;
   if (ctx->op_timing) ctx->prof.clear();
-  rc = order_use(ctx, plan->order, st);
-  if (rc) return rc;
-  plan->unet[0].first.logmel = sp;
-  rc = run_ops(ctx, plan->unet, st);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(mag_out, plan->d_mag, (size_t)batch * frames * 1025 * 4, cudaMemcpyDeviceToDevice, st));
-  return mark_use(ctx, plan->order, st);
+  return with_use(ctx, plan->order, st, [&]() -> int {
+    plan->unet[0].first.logmel = sp;
+    const int r = run_ops(ctx, plan->unet, st);
+    if (r) return r;
+    CK(cudaMemcpyAsync(mag_out, plan->d_mag, (size_t)batch * frames * 1025 * 4, cudaMemcpyDeviceToDevice, st));
+    return VF_OK;
+  });
 }
 
 VF_API int vf_ssr_stages(vf_ctx* ctx, int batch, int64_t n, float* sp_out, float* mag_out, void* stream) {
@@ -1172,11 +1165,12 @@ VF_API int vf_ssr_stages(vf_ctx* ctx, int batch, int64_t n, float* sp_out, float
   rc = get_plan(ctx, PLAN_SSR, batch, frames, &plan);
   if (rc) return rc;
   const size_t bytes = (size_t)batch * frames * 1025 * 4;
-  rc = order_use(ctx, plan->order, (cudaStream_t)stream);
-  if (rc) return rc;
-  if (sp_out) CK(cudaMemcpyAsync(sp_out, plan->d_sp, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  if (mag_out) CK(cudaMemcpyAsync(mag_out, plan->d_mag, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  return mark_use(ctx, plan->order, (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  return with_use(ctx, plan->order, st, [&]() -> int {
+    if (sp_out) CK(cudaMemcpyAsync(sp_out, plan->d_sp, bytes, cudaMemcpyDeviceToDevice, st));
+    if (mag_out) CK(cudaMemcpyAsync(mag_out, plan->d_mag, bytes, cudaMemcpyDeviceToDevice, st));
+    return VF_OK;
+  });
 }
 
 VF_API int vf_restore_stages(vf_ctx* ctx, int batch, int64_t n, float* mel_lin_out, float* log_mel_out, void* stream) {
@@ -1187,11 +1181,12 @@ VF_API int vf_restore_stages(vf_ctx* ctx, int batch, int64_t n, float* mel_lin_o
   rc = get_plan(ctx, PLAN_GSR, batch, frames, &plan);
   if (rc) return rc;
   const size_t bytes = (size_t)batch * frames * 128 * 4;
-  rc = order_use(ctx, plan->order, (cudaStream_t)stream);
-  if (rc) return rc;
-  if (mel_lin_out) CK(cudaMemcpyAsync(mel_lin_out, plan->d_mel, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  if (log_mel_out) CK(cudaMemcpyAsync(log_mel_out, plan->d_logmel_out, bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  return mark_use(ctx, plan->order, (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  return with_use(ctx, plan->order, st, [&]() -> int {
+    if (mel_lin_out) CK(cudaMemcpyAsync(mel_lin_out, plan->d_mel, bytes, cudaMemcpyDeviceToDevice, st));
+    if (log_mel_out) CK(cudaMemcpyAsync(log_mel_out, plan->d_logmel_out, bytes, cudaMemcpyDeviceToDevice, st));
+    return VF_OK;
+  });
 }
 
 VF_API int vf_workspace_bytes(vf_ctx* ctx, int batch, int64_t n, size_t* bytes) {
@@ -1832,7 +1827,7 @@ VF_API int vf_selftest_plan_gemms(vf_ctx* ctx, int plan_kind, int batch, int fra
   plan.kind = plan_kind; plan.batch = batch; plan.T = frames;
   rc = build_plan(ctx, &plan);
   int n = 0;
-  for (const std::vector<Op>* list : {&plan.frontend, &plan.unet, &plan.vocoder, &plan.tail})
+  for (const std::vector<Op>* list : {&plan.unet, &plan.vocoder})
     for (const Op& op : *list) {
       const std::string s = rc ? std::string() : op_signature(op);
       if (s.empty()) continue;

@@ -156,9 +156,7 @@ struct Plan {
   long n_samples = 0;
   std::vector<void*> allocs;
   size_t bytes = 0;
-  std::vector<Op> frontend, unet, vocoder, tail;
-  float* d_wav = nullptr;        // [B, N]   staged input of the host entry points (buffer 0)
-  float* d_out = nullptr;        // [B, N]
+  std::vector<Op> unet, vocoder;
   float* d_io[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};   // [buffer][in / out]: double-buffered host staging
   cudaEvent_t io_ev[2][4] = {{nullptr, nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr, nullptr}};   // h2d done, input consumed, compute done, d2h done
   unsigned io_seq = 0;
@@ -178,8 +176,7 @@ struct Plan {
   // captured on the second use of the plan (the first runs eagerly and sets the kernels' function attributes)
   cudaGraphExec_t graph[2] = {nullptr, nullptr};
   int uses = 0;
-  // op slots patched per call
-  int fe_op = -1, cond_op = -1, fin_op = -1;
+  int cond_op = -1;              // the vocoder's conditioning op, patched per call
 };
 
 // Scratch of a plan-free entry point (standalone.cu): a stream-ordered allocation grown on demand and freed by vf_destroy
@@ -241,7 +238,6 @@ struct vf_ctx {
   BigruW bigru;
   DnnW dnn;
   bool voc_loaded = false;
-  float* d_win_sq_inv = nullptr;   // ISTFT: 1 / clamp(overlap-added squared window, 1e-11), period hop (steady state)
   // vocoder weights
   std::vector<GemmW> voc_cond;
   GemmW voc_stem;
@@ -249,7 +245,6 @@ struct vf_ctx {
   std::vector<std::vector<GemmW>> voc_res_a, voc_res_b;
   float* d_tail_w = nullptr;
   float tail_b = 0;
-  int voc_last_c = 64;
   std::map<std::tuple<int, int, long>, std::unique_ptr<Plan>> plans;   // (kind, batch, frames)
   uint64_t use_clock = 0;
   size_t plan_bytes = 0;               // device bytes held by cached plans

@@ -290,7 +290,6 @@ int load_vocoder(vf_ctx* ctx) {
     NEED(w, "vocoder.tail.weight"); NEED(b, "vocoder.tail.bias");
     rc = pack_tail(ctx, &ctx->d_tail_w, *w); if (rc) return rc;
     ctx->tail_b = b->v[0];
-    ctx->voc_last_c = (int)w->shape[1];
   }
   ctx->voc_loaded = true;
   return VF_OK;
