@@ -466,7 +466,7 @@ VF_API int vf_stage_times(vf_ctx* ctx, float ms[4]);
 /* Per-launch profile: with op timing enabled, the next vf_restore records a CUDA event before every kernel of
  * the UNet and vocoder launch chains.  vf_op_info(i) synchronises and returns the device time of launch i
  * together with its ALGORITHMIC flops / minimum HBM bytes (the reference op's own counts), the flops the tensor
- * cores actually executed for it (3 MMAs per product in 3-term mode, tile / phase padding, identity taps), the tensor-core tile
+ * cores actually executed for it (3 MMAs per product in 3-term mode, tile / phase padding), the tensor-core tile
  * (bn, bk, fp16 split terms; 0 for non-GEMM kernels) and a label such as "enc3.b2.conv1".  For roofline reporting only. */
 VF_API int vf_enable_op_timing(vf_ctx* ctx, int enable);
 VF_API int vf_op_count(vf_ctx* ctx);
@@ -481,7 +481,7 @@ VF_API int vf_op_info(vf_ctx* ctx, int i, float* ms, double* flops, double* byte
 enum { VF_LAYER_CONV2D = 0, VF_LAYER_CONVT2D = 1, VF_LAYER_CONV1D = 2, VF_LAYER_CONVT1D = 3, VF_LAYER_PAIR = 4,
        VF_LAYER_LINEAR = 5 };
 enum { VF_LAYER_PRODUCT = 0, VF_LAYER_SIMT = 1 };
-enum { VF_RESID_NONE = 0, VF_RESID_FP32 = 1, VF_RESID_PLANES = 2, VF_RESID_AR = 3, VF_RESID_IDENTITY = 4 };
+enum { VF_RESID_NONE = 0, VF_RESID_FP32 = 1, VF_RESID_PLANES = 2, VF_RESID_AR = 3 };
 typedef struct vf_layer_case {
   int kind, impl, terms;    /* VF_LAYER_*, VF_LAYER_PRODUCT / SIMT (no (a, r) support: VF_EINVAL), 1 or 3 */
   int n_img;
@@ -502,7 +502,7 @@ typedef struct vf_layer_case {
                                (PAIR: the (a, r) planes of x) */
   int x_img_rows, x_row0;
   const uint16_t* sc_x;     /* [2][n_img][rows][sc_cin] */
-  int resid_kind;           /* VF_RESID_*: FP32 [n_img][rows][cout] floats; PLANES / AR / IDENTITY [2][n_img][rows][cout] fp16 */
+  int resid_kind;           /* VF_RESID_*: FP32 [n_img][rows][cout] floats; PLANES / AR [2][n_img][rows][cout] fp16 */
   const void* resid;
   float ar_slope;           /* AR (input and output streams): the LeakyReLU slope whose fp16 inverse the stream uses */
   float* out_raw;           /* [n_img][out_img_rows][raw_ld] or NULL */

@@ -22,7 +22,7 @@ TOL = {3: 2.0 ** -16, 1: 2.0 ** -14}
 FLOOR = 2.0 ** -24                # fp16 subnormal spacing: the absolute floor of every plane bound
 RES_SLOPE, STAGE_SLOPE, UNET_SLOPE = 0.01, 0.2, 0.01
 CONV2D, CONVT2D, CONV1D, CONVT1D, PAIR, LINEAR = range(6)                    # vf_layer_case kinds (include/b200vf.h)
-RESID = {"fp32": 1, "planes": 2, "ar": 3, "identity": 4}
+RESID = {"fp32": 1, "planes": 2, "ar": 3}
 
 REPORTS = {}          # case name -> reported launch configuration (product kernel)
 
@@ -108,8 +108,8 @@ CASES = [
     C("res_b.ar_c256", CONV1D, terms=1, L=2058, cin=256, cout=256, k=3, resid="ar", outs="a", out_ar=True),
     C("res_b.ar_c128_varlen", CONV1D, terms=1, n_img=3, L=700, cin=128, cout=128, k=3, resid="ar", outs="a", out_ar=True,
       row_valid=[700, 300, 50]),
-    C("res_b.identity_c128", CONV1D, terms=1, L=1000, cin=128, cout=128, k=3, resid="identity", outs="r,a", act=1, slope=RES_SLOPE),
-    C("res_b.identity_c64_t3", CONV1D, terms=3, L=500, cin=64, cout=64, k=3, resid="identity", outs="r,a", act=1, slope=RES_SLOPE),
+    C("res_b.planes_c128", CONV1D, terms=1, L=1000, cin=128, cout=128, k=3, resid="planes", outs="r,a", act=1, slope=RES_SLOPE),
+    C("res_b.planes_c64_t3", CONV1D, terms=3, L=500, cin=64, cout=64, k=3, resid="planes", outs="r,a", act=1, slope=RES_SLOPE),
     C("res_b.planes_c256", CONV1D, terms=1, L=800, cin=256, cout=256, k=3, resid="planes", outs="r,a", act=1, slope=RES_SLOPE),
     C("res_b.planes_c512_t3", CONV1D, terms=3, L=300, cin=512, cout=512, k=3, resid="planes", outs="r,a", act=1, slope=RES_SLOPE),
     C("res_b.last_of_stack", CONV1D, terms=1, L=500, cin=128, cout=128, k=3, resid="ar", outs="a", act=1, slope=STAGE_SLOPE,
@@ -164,11 +164,11 @@ CASES = [
       act=1, slope=STAGE_SLOPE, row_valid=[300, 3]),
     C("res_b.planes_c256_t3_varlen", CONV1D, terms=3, n_img=2, L=300, cin=256, cout=256, k=3, resid="planes", outs="r,a",
       act=1, slope=RES_SLOPE, row_valid=[300, 3]),
-    C("res_b.identity_last_c128_t3", CONV1D, terms=3, L=500, cin=128, cout=128, k=3, resid="identity", outs="a", act=1,
+    C("res_b.planes_last_c128_t3", CONV1D, terms=3, L=500, cin=128, cout=128, k=3, resid="planes", outs="a", act=1,
       slope=STAGE_SLOPE),
-    C("res_b.identity_last_c128_t3_varlen", CONV1D, terms=3, n_img=2, L=500, cin=128, cout=128, k=3, resid="identity",
+    C("res_b.planes_last_c128_t3_varlen", CONV1D, terms=3, n_img=2, L=500, cin=128, cout=128, k=3, resid="planes",
       outs="a", act=1, slope=STAGE_SLOPE, row_valid=[500, 3]),
-    C("res_b.identity_c64_t3_varlen", CONV1D, terms=3, n_img=2, L=500, cin=64, cout=64, k=3, resid="identity", outs="r,a",
+    C("res_b.planes_c64_t3_varlen", CONV1D, terms=3, n_img=2, L=500, cin=64, cout=64, k=3, resid="planes", outs="r,a",
       act=1, slope=RES_SLOPE, row_valid=[500, 3]),
     C("pair.last_varlen", PAIR, n_img=2, L=1000, dilation=243, last=True, out_row0=3, out_slack=6, row_valid=[1000, 127]),
     # ---- the analysis modules' Linear layers (plan.cu: build_bigru / build_dnn), at the plans' shapes
@@ -727,8 +727,9 @@ def test_layer_simt_matches_float64(eng, name):
 
 @pytest.mark.parametrize("name", [c["name"] for c in CASES if c["kind"] == PAIR])
 def test_pair_two_launch_path_matches_float64(eng, name):
-    """The same residual pair as the two launches the plans use without the fused kernel: res.a (CONV1D, dilation d),
-    then res.b (CONV1D + the (a, r) residual, (a, r) out); each checked against float64 on its own."""
+    """The (a, r) launch kind of the C >= 128 stacks, res.a (CONV1D, dilation d) then res.b (CONV1D + the (a, r) residual,
+    (a, r) out), at the fused pair's edge shapes (no plan builds a C = 64 pair as two launches); each checked against
+    float64 on its own."""
     c = BY_NAME[name]
     L, n = c["L"], c.get("n_img", 1)
     common = dict(n_img=n, L=L, cin=64, cout=64, k=3, terms=1, row_valid=c.get("row_valid"))

@@ -1351,8 +1351,6 @@ int run_layer_case(vf_ctx* ctx, Builder& b, vf_layer_case& c) {
   // weights, through the loaders' packers
   GemmW W, W2;
   int rc = VF_OK;
-  const bool ident = (c.resid_kind == VF_RESID_PLANES || c.resid_kind == VF_RESID_AR || c.resid_kind == VF_RESID_IDENTITY ||
-                      c.kind == VF_LAYER_PAIR) && c.cout <= IDENT_MAX_C;      // load_vocoder: res.b of the C <= 128 stacks
   switch (c.kind) {
     case VF_LAYER_CONV2D: {
       const HostT w = host_tensor(c.w, {c.cout, c.cin, 3, 3});
@@ -1363,14 +1361,14 @@ int run_layer_case(vf_ctx* ctx, Builder& b, vf_layer_case& c) {
     }
     case VF_LAYER_CONVT2D: rc = pack_convT2d(ctx, &W, host_tensor(c.w, {c.cin, c.cout, 3, 3})); break;
     case VF_LAYER_CONV1D:
-      rc = pack_conv1d(ctx, &W, host_tensor(c.w, {c.cout, c.cin, c.k}), host_tensor(c.b, {c.cout}), ident);
+      rc = pack_conv1d(ctx, &W, host_tensor(c.w, {c.cout, c.cin, c.k}), host_tensor(c.b, {c.cout}));
       break;
     case VF_LAYER_CONVT1D:
       rc = pack_convT1d(ctx, &W, host_tensor(c.w, {c.cin, c.cout, 2 * c.stride}), host_tensor(c.b, {c.cout}), c.stride);
       break;
     case VF_LAYER_PAIR:
-      rc = pack_conv1d(ctx, &W, host_tensor(c.w, {c.cout, c.cin, 3}), host_tensor(c.b, {c.cout}), false);
-      if (!rc) rc = pack_conv1d(ctx, &W2, host_tensor(c.w2, {c.cout, c.cout, 3}), host_tensor(c.b2, {c.cout}), ident);
+      rc = pack_conv1d(ctx, &W, host_tensor(c.w, {c.cout, c.cin, 3}), host_tensor(c.b, {c.cout}));
+      if (!rc) rc = pack_conv1d(ctx, &W2, host_tensor(c.w2, {c.cout, c.cout, 3}), host_tensor(c.b2, {c.cout}));
       break;
     case VF_LAYER_LINEAR:
       if (c.b_hh) {     // load_bigru: the layer's W_ih of both directions, b_ih + (b_hr, b_hz, 0)
@@ -1462,10 +1460,6 @@ int run_layer_case(vf_ctx* ctx, Builder& b, vf_layer_case& c) {
       const Planes R = dev_planes(c.resid, rows, c.cout);
       e.resid_hi = R.p.hi; e.resid_lo = R.p.lo; e.resid_ld = c.cout;
       if (c.resid_kind == VF_RESID_AR) e.resid_ar = ar;
-    } else if (c.resid_kind == VF_RESID_IDENTITY) {
-      taps.push_back(GemmTap{0, 1, 0, 0, c.cout, 1});
-      s1 = ASrc{dev_planes(c.resid, rows, c.cout), rows, 0};
-      has_s1 = true;
     }
     if (c.out_raw) { e.out_raw = dev_floats(c.out_raw, out_n * c.raw_ld); e.raw_ld = c.raw_ld; }
     if (c.out_r) {
@@ -1537,7 +1531,7 @@ VF_API int vf_selftest_layer(vf_ctx* ctx, vf_layer_case* lc) {
   const bool pair = c.kind == VF_LAYER_PAIR, lin = c.kind == VF_LAYER_LINEAR;
   if (c.kind < VF_LAYER_CONV2D || c.kind > VF_LAYER_LINEAR || (c.impl != VF_LAYER_PRODUCT && c.impl != VF_LAYER_SIMT) ||
       (c.terms != 1 && c.terms != 3) || c.n_img <= 0 || !c.x || !c.w || c.cin <= 0 || c.cout <= 0 || c.x_row0 < 0 ||
-      c.out_img_rows <= 0 || c.resid_kind < VF_RESID_NONE || c.resid_kind > VF_RESID_IDENTITY ||
+      c.out_img_rows <= 0 || c.resid_kind < VF_RESID_NONE || c.resid_kind > VF_RESID_AR ||
       (c.resid_kind != VF_RESID_NONE && !c.resid) || (c.sc_cin && (c.kind != VF_LAYER_CONV2D || !c.sc_w || !c.sc_b || !c.sc_x)) ||
       ((c.kind == VF_LAYER_CONV1D || c.kind == VF_LAYER_CONVT1D || pair || lin) && !c.b) ||
       ((c.in_bn || c.b_hh) && !lin) || (c.in_bn && c.b_hh) || (c.b_hh && c.cout != 6 * GRU_HIDDEN) ||

@@ -21,7 +21,7 @@
 
 namespace vf {
 cudaError_t launch_gemm_tc(const GemmTcParams& p, int bn, int bk, cudaStream_t stream);
-size_t gemm_tc_smem_bytes(int bn, int bk, int stages, int planes_a, int terms, int tile_chunks, int resid_tma);
+size_t gemm_tc_smem_bytes(int bn, int bk, int stages, int terms, int tile_chunks, int resid_tma);
 int gemm_tc_max_bn(int terms);
 cudaError_t launch_pair_tc(const PairParams& p, cudaStream_t stream);
 size_t pair_tc_smem_bytes(int C);
@@ -38,7 +38,6 @@ struct GemmW {
   __half* lo = nullptr;
   float* bias = nullptr;
   int N = 0, K = 0;
-  int k_tail = 0;      // trailing identity block (pack_conv1d): a GEMM may contract the K - k_tail columns before it only
 };
 struct Affine {
   float* scale = nullptr;
@@ -66,8 +65,8 @@ struct Op {
   OpKind kind;
   int bn = 0, bk = 0;
   double flops = 0, bytes = 0;   // algorithmic work of this launch (reference op counts), for the roofline
-  double exec_flops = 0;         // tensor-core flops actually issued (3 MMAs per product in 3-term mode, K / phase padding,
-                                 // identity taps): numerator of the "executed" tensor fraction
+  double exec_flops = 0;         // tensor-core flops actually issued (3 MMAs per product in 3-term mode, K / phase
+                                 // padding): numerator of the "executed" tensor fraction
   char label[48] = {0};
   GemmTcParams tc;
   GemmSimtParams simt;
@@ -304,7 +303,7 @@ int load_all(vf_ctx* ctx);
 // PyTorch weight layouts -> packed GEMM operands (upload_gemm), as the loaders pack every conv of the networks
 int pack_conv3x3(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT* sc_w, const HostT* sc_b);
 int pack_convT2d(vf_ctx* ctx, GemmW* out, const HostT& w);
-int pack_conv1d(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT& b, bool identity = false);
+int pack_conv1d(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT& b);
 int pack_convT1d(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT& b, int s);
 // the tail Conv1d(C -> 1, k7) weight [1][C][7] -> the tail kernel's [7][C]
 int pack_tail(vf_ctx* ctx, float** out, const HostT& w);
@@ -316,9 +315,6 @@ void scalar_bn_affine(const float bn[4], double st[2]);
 // One bi_gru layer's input projection: per direction W_ih [768][K], b_ih and b_hh [768] -> both directions stacked, N = 1536,
 // bias b_ih + (b_hr, b_hz, 0)
 int pack_gru_ih(vf_ctx* ctx, GemmW* out, const HostT* const wi[2], const HostT* const bi[2], const HostT* const bh[2]);
-// Residual add of a vocoder stack as an identity tap (through the accumulator, no epilogue loads) up to this channel count;
-// above it the epilogue adds the hi/lo planes.  The packer appends the identity block and the plan builder adds the tap.
-constexpr int IDENT_MAX_C = 128;
 
 // plan.cu
 struct Builder {

@@ -39,8 +39,6 @@ struct GemmTap {
   int c_off;   // first channel inside the source
   int k_off;   // first column of the tap's segment in the packed weight matrix
   int nch;     // channels contracted by the tap (multiple of the kernel's BK)
-  int both;    // 1: contract hi AND lo planes of A even in 1-term mode (identity tap carrying the fp32-grade
-               //    residual stream through the accumulator)
 };
 
 struct OutPlane {
@@ -64,8 +62,8 @@ struct GemmEpilogue {
   const float* bias;   // [N] or null
   const float* resid;  // fp32 [n_img * rows_in, resid_ld] or null (MAP_PLAIN only)
   int resid_ld;
-  const __half* resid_hi;  // residual given as hi/lo planes [n_img * rows_in, resid_ld] (vocoder stacks whose
-  const __half* resid_lo;  // GEMM is MMA-bound: cheaper to add in the epilogue than as an identity tap)
+  const __half* resid_hi;  // residual given as hi/lo planes [n_img * rows_in, resid_ld] (the residual stream of the
+  const __half* resid_lo;  // vocoder stacks: separate hi/lo planes of x, or the (a, r) pair below)
   float* out_raw;      // fp32 or null
   int raw_ld;
   OutPlane out_r;      // raw value split hi/lo (consumed by 1x1 shortcut taps)
@@ -118,7 +116,7 @@ struct GemmProblem {
 };
 
 struct GemmTcParams {
-  CUtensorMap a_hi[2], a_lo[2];   // [C, rows, n_img] fp16
+  CUtensorMap a_hi[2];            // [C, rows, n_img] fp16 (3-term: [C, rows, n_img, 2], the hi and lo planes)
   CUtensorMap b_hi, b_lo;         // [Ktot, N] fp16 (K-major)
   CUtensorMap i_res;              // epilogue residual by TMA load (MAP_PLAIN only): fp32 [resid_ld, rows_in, n_img] box 32 x 32 x 1
                                   // SWIZZLE_128B (3-term), or fp16 planes [resid_ld, rows_in, n_img, 2] box 32 x 32 x 1 x 2 SWIZZLE_64B
@@ -128,7 +126,6 @@ struct GemmTcParams {
   int stages;
   int tile_chunks; // BK-wide K chunks per output tile
   int seg_chunks;  // 3-term mode: chunks per accumulation segment (promotion to registers in between)
-  int planes_a;    // smem slots per stage for A: 2 when any tap contracts the lo plane
   int grid;        // persistent CTAs
   uint32_t magic_n, magic_m;   // gemm_tc_magic() of N / BN and m_tiles: division-free tile decoding
   GemmProblem prob;

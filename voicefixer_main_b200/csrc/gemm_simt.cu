@@ -41,7 +41,7 @@ __global__ void __launch_bounds__(128) gemm_simt_kernel(const GemmSimtParams P) 
       if (in) {
         for (int k = 0; k < cw; ++k) {
           float a = __half2float(P.a_hi[tap.src][abase + c0 + k]);
-          if (three || tap.both) a += __half2float(P.a_lo[tap.src][abase + c0 + k]);
+          if (three) a += __half2float(P.a_lo[tap.src][abase + c0 + k]);
 #pragma unroll
           for (int n = 0; n < 32; ++n) acc[n] = fmaf(a, w_s[n][k], acc[n]);
         }

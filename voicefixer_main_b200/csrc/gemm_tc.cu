@@ -53,7 +53,7 @@ struct ChunkDesc {
   int a_c;          // channel coordinate of the A box
   int a_off;        // row offset of the A box relative to the tile's first row
   uint32_t kk;      // K coordinate of the weight tile
-  uint32_t flags;   // bit 0 src, bit 4 (hi-only kernels) the A tile is the lo plane: the second pass of an identity tap
+  uint32_t flags;   // bit 0 src
 };
 
 // Tile coordinates without loop-carried state: tile = (img * m_tiles + mi) * n_tiles + nt, decoded per tile with the
@@ -123,11 +123,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
   // 1024-byte alignment by offset arithmetic (keeps the pointer in the shared address space: LDS/STS, not generic)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int stages = P.stages;
-  const int planes_a = P.planes_a;                      // 2 when any tap contracts the lo plane of A
   constexpr int B_SLOT = (THREE ? 2 : 1) * B_BYTES;      // [B_hi][B_lo] of one tap, contiguous
   constexpr int A_BOX_BYTES = GEMM_BM * ROW_BYTES;      // bytes one A TMA box delivers: a whole number of 1 KB swizzle atoms
-  const int off_b = planes_a * A_BOX_BYTES;
-  const int stage_bytes = off_b + B_SLOT;
+  constexpr int off_b = (THREE ? 2 : 1) * A_BOX_BYTES;   // [A_hi][A_lo] in 3-term mode, A_hi alone otherwise
+  constexpr int stage_bytes = off_b + B_SLOT;
   uint8_t* stg_base = smem + (size_t)stages * stage_bytes;          // EPI_WARPS x 4 KB staging
   uint8_t* rstg_base = stg_base + EPI_WARPS * 4096;                  // resid_tma: EPI_WARPS x 4 KB residual tiles (TMA destination)
   uint8_t* tail = rstg_base + (size_t)P.resid_tma * EPI_WARPS * 4096;  // P.resid_tma = tiles in flight per warp (0, 1 or 2)
@@ -159,27 +158,22 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     fence_mbar_init();
     tma_prefetch_desc(&P.a_hi[0]);
     tma_prefetch_desc(&P.b_hi);
-    if (!THREE) tma_prefetch_desc(&P.a_lo[0]);
   }
-  // flatten taps x K chunks (see ChunkDesc).  In hi-only kernels a `both` tap (identity weights carrying the hi/lo residual
-  // stream) is two passes over the same weight chunks, the second with the lo plane of A as its A tile: every chunk is then one
-  // and the same MMA body (a data-dependent extra MMA per chunk would make the compiler serialise the wgmma pipeline).
+  // flatten taps x K chunks (see ChunkDesc)
   for (int ci = threadIdx.x; ci < tile_chunks; ci += blockDim.x) {
     int t = 0, first = 0;
     for (; t < pr.ntaps - 1; ++t) {
-      const int n = pr.taps[t].nch / BK * ((!THREE && pr.taps[t].both) ? 2 : 1);
+      const int n = pr.taps[t].nch / BK;
       if (ci < first + n) break;
       first += n;
     }
     const GemmTap& tap = pr.taps[t];
-    const int nk = tap.nch / BK;
-    const bool lo_pass = !THREE && tap.both && ci - first >= nk;
-    const int c = (ci - first - (lo_pass ? nk : 0)) * BK;
+    const int c = (ci - first) * BK;
     ChunkDesc cd;
     cd.a_c = tap.c_off + c;
     cd.a_off = tap.a_off;
     cd.kk = (uint32_t)(tap.k_off + c);
-    cd.flags = (uint32_t)(tap.src & 1) | (lo_pass ? 16u : 0u);
+    cd.flags = (uint32_t)(tap.src & 1);
     s_tab[ci] = cd;
   }
   __syncthreads();
@@ -204,7 +198,6 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         const ChunkDesc cur = cd;
         cd = s_tab[ci + 1 < tile_chunks ? ci + 1 : 0];     // next entry: its load latency hides behind the wait
         if (!mbar_wait(empty_bar + s, ph ^ 1, e.err, ERR_PIPE_PRODUCER)) { ok = false; break; }
-        const bool lo_pass = (cur.flags & 16u) != 0;
         const int src = cur.flags & 1u;
         uint8_t* st = smem + (size_t)s * stage_bytes;
         mbar_expect_tx(full_bar + s, (THREE ? 2u : 1u) * A_BOX_BYTES + B_SLOT);
@@ -213,7 +206,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           tma_load_4d(st, &P.a_hi[src], full_bar + s, cur.a_c, m0 + cur.a_off, img, 0);
           tma_load_3d(st + off_b, &P.b_hi, full_bar + s, k0, n0, 0);
         } else {
-          tma_load_3d(st, lo_pass ? &P.a_lo[src] : &P.a_hi[src], full_bar + s, cur.a_c, m0 + cur.a_off, img);
+          tma_load_3d(st, &P.a_hi[src], full_bar + s, cur.a_c, m0 + cur.a_off, img);
           tma_load_2d(st + off_b, &P.b_hi, full_bar + s, k0, n0);
         }
         if (++s == stages) { s = 0; ph ^= 1; }
@@ -634,15 +627,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 }
 
 // ---------------------------------------------------------------------------------------------- host side
-size_t gemm_tc_smem_bytes(int bn, int bk, int stages, int planes_a, int terms, int tile_chunks, int resid_tma) {
-  const size_t stage = (size_t)planes_a * GEMM_BM * bk * 2 + (size_t)(terms == 3 ? 2 : 1) * bn * bk * 2;
+size_t gemm_tc_smem_bytes(int bn, int bk, int stages, int terms, int tile_chunks, int resid_tma) {
+  const size_t stage = (size_t)(terms == 3 ? 2 : 1) * (GEMM_BM + bn) * bk * 2;
   return stages * stage + EPI_WARPS * 4096 * (1 + resid_tma) + (2 * stages + 16) * 8 + (3 * bn + 32) * 4 + EPI_WARPS * 32 * 8 +
          (size_t)tile_chunks * 16 + 1024;
 }
 
 template <int BN, int BK, bool THREE>
 static cudaError_t launch_cfg(const GemmTcParams& p, cudaStream_t stream) {
-  const size_t smem = gemm_tc_smem_bytes(BN, BK, p.stages, p.planes_a, p.prob.terms, p.tile_chunks, p.resid_tma);
+  const size_t smem = gemm_tc_smem_bytes(BN, BK, p.stages, p.prob.terms, p.tile_chunks, p.resid_tma);
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BN, BK, THREE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);

@@ -146,18 +146,14 @@ int pack_convT2d(vf_ctx* ctx, GemmW* out, const HostT& w) {
   return upload_gemm(ctx, out, m, N, K, nullptr);
 }
 
-// Conv1d [Cout][Cin][k] -> [Cout][k*Cin (+ Cout)]; with `identity` an identity block is appended so the
-// residual stream x (kept as fp16 hi/lo planes) is added inside the same accumulator: x' = x + conv(...)
-int pack_conv1d(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT& b, bool identity) {
+// Conv1d [Cout][Cin][k] -> [Cout][k*Cin]
+int pack_conv1d(vf_ctx* ctx, GemmW* out, const HostT& w, const HostT& b) {
   const int cout = (int)w.shape[0], cin = (int)w.shape[1], k = (int)w.shape[2];
-  const int K = k * cin + (identity ? cout : 0);
+  const int K = k * cin;
   std::vector<float> m((size_t)cout * K, 0.f);
-  for (int n = 0; n < cout; ++n) {
+  for (int n = 0; n < cout; ++n)
     for (int c = 0; c < cin; ++c)
       for (int t = 0; t < k; ++t) m[(size_t)n * K + t * cin + c] = w.v[((size_t)n * cin + c) * k + t];
-    if (identity) m[(size_t)n * K + k * cin + n] = 1.f;
-  }
-  out->k_tail = identity ? cout : 0;
   return upload_gemm(ctx, out, m, cout, K, &b.v);
 }
 
@@ -283,7 +279,7 @@ int load_vocoder(vf_ctx* ctx) {
       const std::string p = "vocoder.res." + std::to_string(s) + "." + std::to_string(i);
       NEED(wa, p + ".a.weight"); NEED(ba, p + ".a.bias"); NEED(wb, p + ".b.weight"); NEED(bb, p + ".b.bias");
       rc = pack_conv1d(ctx, &ctx->voc_res_a[s][i], *wa, *ba); if (rc) return rc;
-      rc = pack_conv1d(ctx, &ctx->voc_res_b[s][i], *wb, *bb, (int)wb->shape[0] <= IDENT_MAX_C); if (rc) return rc;
+      rc = pack_conv1d(ctx, &ctx->voc_res_b[s][i], *wb, *bb); if (rc) return rc;
     }
   }
   {

@@ -1,7 +1,6 @@
 // Plan building: every buffer of a (kind, batch, frames) shape is allocated and every TMA tensor map encoded here, once,
 // and each network becomes a list of launches with their arguments resolved (engine.h: Plan, Op).
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 
 #include "engine.h"
@@ -115,7 +114,7 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
     k += padded;
     if (ctx->validate_simt == 0) t.nch = padded;
   }
-  if (k != W.K && k != W.K - W.k_tail) { rc = fail(ctx, VF_EINVAL, "GEMM K mismatch: taps cover %d, packed weight has %d", k, W.K); return; }
+  if (k != W.K) { rc = fail(ctx, VF_EINVAL, "GEMM K mismatch: taps cover %d, packed weight has %d", k, W.K); return; }
   GemmProblem pr;
   memset(&pr, 0, sizeof pr);
   pr.n_img = n_img;
@@ -154,7 +153,6 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
         if (!rc) rc = map_a(ctx, &tp.a_hi[i], *srcs[i], srcs[i]->pl.p.hi, n_img, bk, true);
       } else {
         rc = map_a(ctx, &tp.a_hi[i], *srcs[i], srcs[i]->pl.p.hi, n_img, bk, false);
-        if (!rc) rc = map_a(ctx, &tp.a_lo[i], *srcs[i], srcs[i]->pl.p.lo, n_img, bk, false);
       }
     }
     if (terms == 3) {
@@ -165,20 +163,18 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
     }
     // accumulation segments (see gemm_tc.cu): a bounded chain of truncating MMAs, then promotion to registers
     tp.tile_chunks = 0;
-    for (auto& t : taps) tp.tile_chunks += t.nch / bk * ((terms == 1 && t.both) ? 2 : 1);   // ring slots per tile (a hi-only
-                                                                  // identity tap is a hi pass and a lo pass, gemm_tc.cu)
+    for (auto& t : taps) tp.tile_chunks += t.nch / bk;   // ring slots per tile
     // K steps per accumulation chain before promotion: longer chains = fewer promotion drains, shorter ones = less
     // drift of the tensor core's fp32 accumulation (the 3-term UNet carries a 1e-4 log-mel bar).
     const int seg_mmas = 24;
     tp.seg_chunks = std::max(1, seg_mmas / (bk / 16));
-    tp.planes_a = terms == 3 ? 2 : 1;
     // occupancy: small-K tiles are bound by loads/stores -> several persistent CTAs per SM; large-K -> one
     // one persistent CTA of 384 threads per SM (the accumulators take the register file): the deepest operand ring that fits
     const size_t smem_cap = (size_t)227 * 1024 - 1024;
     auto fit = [&](int ring) {
       int st = 8;
       for (; st >= 2; --st)
-        if (gemm_tc_smem_bytes(bn, bk, st, tp.planes_a, terms, tp.tile_chunks, ring) <= smem_cap) break;
+        if (gemm_tc_smem_bytes(bn, bk, st, terms, tp.tile_chunks, ring) <= smem_cap) break;
       return st;
     };
     // The residual and the fp32 output follow the GEMM rows, which only MAP_PLAIN layers store in order (gemm_tc.cu).
@@ -237,18 +233,15 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
   }
   {   // algorithmic work: the reference op's own MAC count and the minimum HBM traffic of this launch
     double kreal = 0;
-    for (auto& t : taps) if (!t.both) kreal += (double)std::min(t.nch, (t.src ? s1 : &s0)->pl.C);
+    for (auto& t : taps) kreal += (double)std::min(t.nch, (t.src ? s1 : &s0)->pl.C);
     const double wfrac = (epi.Wp > 1) ? double(epi.Wp - 1) / epi.Wp : 1.0;
     double rows = (double)n_img * (epi.map == MAP_CONVT1D ? epi.rows_in - 1 : epi.rows_in) * wfrac;
     op.flops = 2.0 * rows * N * kreal * (epi.map == MAP_CONVT2D ? 9.0 / 16.0 : 1.0);
-    // bytes per source element: both fp16 planes in 3-term mode, and for a source that an identity tap contracts
-    // with `both` (the hi/lo residual stream of the C <= 128 vocoder stacks); the hi plane alone otherwise
-    bool s1_both = false;
-    for (auto& t : taps) s1_both |= (t.src == 1 && t.both);
+    // bytes per source element: both fp16 planes in 3-term mode, the hi plane alone otherwise
     double a_bytes = (double)n_img * s0.rows * s0.pl.C * (terms == 3 ? 4 : 2);
-    if (s1) a_bytes += (double)n_img * s1->rows * s1->pl.C * ((terms == 3 || s1_both) ? 4 : 2);
+    if (s1) a_bytes += (double)n_img * s1->rows * s1->pl.C * (terms == 3 ? 4 : 2);
     double kexec = 0;
-    for (auto& t : taps) kexec += (double)round_up(t.nch, bk) * (terms == 3 ? 3 : (t.both ? 2 : 1));
+    for (auto& t : taps) kexec += (double)round_up(t.nch, bk) * (terms == 3 ? 3 : 1);
     op.exec_flops = 2.0 * (double)n_img * pr.m_tiles * GEMM_BM * N * kexec;
     const double out_elems = (double)n_img * (epi.map == MAP_CONVT1D ? (double)epi.out_rows_valid * epi.cout
                                               : (epi.map == MAP_CONVT2D ? 4.0 * epi.rows_in * epi.cout : (double)epi.rows_in * N));
@@ -674,10 +667,9 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
     // hi/lo planes of x.
     const uint32_t ar = (!ctx->validate_simt && terms == 1) ? ar_inv_word(c.voc_res_slope) : 0u;
     // C = 64 stacks of the hi-only mode with the (a, r) stream: one kernel per residual pair (pair_tc.cu), the intermediate h
-    // stays in shared memory; VF_TUNE_FUSED_PAIR=0 selects the two-launch path.  A pair's activated input and output planes
-    // must differ (a tile reads rows up to `dil` away from the ones another CTA is writing): the pairs ping-pong between xa and xa2.
-    const char* fenv = getenv("VF_TUNE_FUSED_PAIR");
-    const bool fused = !(fenv && atoi(fenv) == 0) && ar != 0 && cout == 64 && pair_tc_smem_bytes(cout) != 0;
+    // stays in shared memory.  A pair's activated input and output planes must differ (a tile reads rows up to `dil` away from
+    // the ones another CTA is writing): the pairs ping-pong between xa and xa2.
+    const bool fused = ar != 0 && cout == 64 && pair_tc_smem_bytes(cout) != 0;
     // residual stream x as hi/lo planes (ping-pong)
     Planes xr[2] = {ar ? Planes() : b.planes(B, (int)L, cout), ar ? Planes() : b.planes(B, (int)L, cout)};
     Planes xa = b.planes(B, (int)L, cout), ha = fused ? Planes() : b.planes(B, (int)L, cout);
@@ -743,23 +735,15 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
         }
         set_out_a(e, dst, 0, nullptr, nullptr, ACT_LRELU, last ? c.voc_stage_slope : c.voc_res_slope);
         b.label = "voc.res" + std::to_string(s) + "." + std::to_string(i) + ".b";
-        std::vector<GemmTap> taps = taps1d(3, 1, cout, true);
-        ASrc xsrc{xr[curx], (int)L, 0};
         if (ar) {
           // x = U(a) + r from the two planes of xa, rewritten in place: a tile reads exactly the rows it writes, and only
           // the "a" conv of the next pair (a later launch) looks at neighbouring rows
-          e.resid_hi = xa.p.hi; e.resid_lo = xa.p.lo; e.resid_ld = cout; e.resid_ar = ar;
-          b.gemm(ops, ctx->voc_res_b[s][i], ASrc{ha, (int)L, 0}, nullptr, taps, e, B, terms);
-        } else if (cout <= IDENT_MAX_C) {
-          // load/store-bound stacks: x rides through the accumulator (identity weights, both planes) and the
-          // epilogue issues no global loads
-          taps.push_back(GemmTap{0, 1, 0, 0, cout, 1});
-          b.gemm(ops, ctx->voc_res_b[s][i], ASrc{ha, (int)L, 0}, &xsrc, taps, e, B, terms);
+          e.resid_hi = xa.p.hi; e.resid_lo = xa.p.lo; e.resid_ar = ar;
         } else {
-          // MMA-bound stacks: the identity tap would add ~40% tensor work; add the planes in the epilogue instead
-          e.resid_hi = xr[curx].p.hi; e.resid_lo = xr[curx].p.lo; e.resid_ld = cout;
-          b.gemm(ops, ctx->voc_res_b[s][i], ASrc{ha, (int)L, 0}, nullptr, taps, e, B, terms);
+          e.resid_hi = xr[curx].p.hi; e.resid_lo = xr[curx].p.lo;
         }
+        e.resid_ld = cout;
+        b.gemm(ops, ctx->voc_res_b[s][i], ASrc{ha, (int)L, 0}, nullptr, taps1d(3, 1, cout, true), e, B, terms);
         curx = 1 - curx;
       }
     }
@@ -810,9 +794,9 @@ std::string op_signature(const Op& op) {
   if (op.kind != OP_GEMM) return "";
   const GemmTcParams& tp = op.tc;
   const GemmEpilogue& e = tp.prob.epi;
-  int sc = 0, ident = 0;
+  int sc = 0;
   for (int i = 0; i < tp.prob.ntaps; ++i)
-    if (tp.prob.taps[i].src == 1) (tp.prob.taps[i].both ? ident : sc) = 1;
+    if (tp.prob.taps[i].src == 1) sc = 1;
   static const char* const maps[3] = {"plain", "convt2d", "convt1d"};
   const char* resid = e.resid ? "fp32" : !e.resid_hi ? "none" : e.resid_ar ? "ar" : "planes";
   std::string outs;
@@ -820,8 +804,8 @@ std::string op_signature(const Op& op) {
   if (e.out_r.hi) outs += "r,";
   if (e.out_a.hi) outs += e.out_ar ? "ar," : "a,";
   if (!outs.empty()) outs.pop_back();
-  snprintf(s, sizeof s, "gemm map=%s terms=%d bn=%d bk=%d sc=%d identity=%d resid=%s resid_tma=%d out=%s tma_out=%d affine=%d act=%d head=%d varlen=%d",
-           maps[e.map], tp.prob.terms, op.bn, op.bk, sc, ident, resid, tp.resid_tma, outs.empty() ? "-" : outs.c_str(), e.tma_out,
+  snprintf(s, sizeof s, "gemm map=%s terms=%d bn=%d bk=%d sc=%d resid=%s resid_tma=%d out=%s tma_out=%d affine=%d act=%d head=%d varlen=%d",
+           maps[e.map], tp.prob.terms, op.bn, op.bk, sc, resid, tp.resid_tma, outs.empty() ? "-" : outs.c_str(), e.tma_out,
            e.a_scale ? 1 : 0, e.out_a.hi ? e.act : -1, e.head_w ? 1 : 0, e.row_valid ? 1 : 0);
   return s;
 }
