@@ -541,11 +541,16 @@ typedef struct vf_layer_case {
 VF_API int vf_selftest_layer(vf_ctx* ctx, vf_layer_case* lc);
 
 /* TEST ONLY.  Builds a plan of `plan_kind` (0 GSR, 1 SSR, 2 GSR varlen, 3 SSR varlen) for (batch, frames) with the loaded
- * weights and the context's options, launches nothing, and reports each GEMM and fused-pair launch: its label and the
- * configuration signature vf_selftest_layer reports for a layer.  Records past `cap` are dropped; *count = all of them. */
+ * weights and the context's options, launches nothing, and reports each GEMM and fused-pair launch: its label, the
+ * configuration signature vf_selftest_layer reports for a layer, and the size of its persistent tile loop (tiles and grid,
+ * as vf_selftest_layer reports them, and the column tiles among which a CTA's consecutive tiles move).  Records past `cap`
+ * are dropped; *count = all of them. */
 typedef struct vf_plan_gemm {
   char label[48];
   char sig[160];
+  int64_t tiles;            /* output tiles of the launch */
+  int grid;                 /* persistent CTAs: min(tiles, SMs) */
+  int col_tiles;            /* column (N) tiles per row block: tiles of a CTA change column block unless it divides grid */
 } vf_plan_gemm;
 VF_API int vf_selftest_plan_gemms(vf_ctx* ctx, int plan_kind, int batch, int frames, vf_plan_gemm* records, int cap, int* count);
 

@@ -81,7 +81,7 @@ class VfOpCase(Structure):
 
 class VfPlanGemm(Structure):
     """vf_plan_gemm (include/b200vf.h): one GEMM / fused-pair launch of a plan for vf_selftest_plan_gemms (tests only)."""
-    _fields_ = [("label", c_char * 48), ("sig", c_char * 160)]
+    _fields_ = [("label", c_char * 48), ("sig", c_char * 160), ("tiles", c_int64), ("grid", c_int), ("col_tiles", c_int)]
 
 
 class VfGruCase(Structure):

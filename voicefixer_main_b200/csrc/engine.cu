@@ -1407,8 +1407,9 @@ int run_layer_case(vf_ctx* ctx, Builder& b, vf_layer_case& c) {
     if (rc) return rc;
     ops.push_back(pop);
     op = &ops.back();
-    c.bn = 64; c.bk = 64; c.stages = 0; c.resid_tma = 0; c.tma_out = 1; c.grid = op->pair.grid;
-    c.tiles = (int64_t)n * op->pair.tiles_per_img;
+    c.bn = 64; c.bk = 64; c.stages = 0; c.resid_tma = 0; c.tma_out = 1;
+    int col_tiles;
+    op_tile_loop(*op, &c.tiles, &c.grid, &col_tiles);
     c.div_fallback = op->pair.magic_t == 0xffffffffu;
     snprintf(c.sig, sizeof c.sig, "%s", op_signature(*op).c_str());
   } else {
@@ -1497,8 +1498,9 @@ int run_layer_case(vf_ctx* ctx, Builder& b, vf_layer_case& c) {
       c.sig[0] = 0;
     } else {
       const GemmTcParams& tp = op->tc;
-      c.stages = tp.stages; c.resid_tma = tp.resid_tma; c.tma_out = tp.prob.epi.tma_out; c.grid = tp.grid;
-      c.tiles = (int64_t)n * tp.prob.m_tiles * (tp.prob.N / op->bn);
+      c.stages = tp.stages; c.resid_tma = tp.resid_tma; c.tma_out = tp.prob.epi.tma_out;
+      int col_tiles;
+      op_tile_loop(*op, &c.tiles, &c.grid, &col_tiles);
       c.div_fallback = tp.magic_n == 0xffffffffu || tp.magic_m == 0xffffffffu;
       snprintf(c.sig, sizeof c.sig, "%s", op_signature(*op).c_str());
     }
@@ -1828,6 +1830,7 @@ VF_API int vf_selftest_plan_gemms(vf_ctx* ctx, int plan_kind, int batch, int fra
       if (n < cap) {
         snprintf(records[n].label, sizeof records[n].label, "%s", op.label);
         snprintf(records[n].sig, sizeof records[n].sig, "%s", s.c_str());
+        op_tile_loop(op, &records[n].tiles, &records[n].grid, &records[n].col_tiles);
       }
       ++n;
     }

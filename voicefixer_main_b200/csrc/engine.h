@@ -387,6 +387,9 @@ void linear_gemm(Builder& b, std::vector<Op>& ops, const GemmW& W, const Planes&
 // The choices of a built OP_GEMM (tensor-core path) or OP_PAIR that select kernel code, as one string; "" for other ops.  Sizes
 // that only change occupancy (stages, grid) are left out.
 std::string op_signature(const Op& op);
+// The persistent tile loop of a built OP_GEMM (tensor-core path) or OP_PAIR: tiles in all, CTAs launched and column tiles per
+// row block (0, 0, 0 for other ops)
+void op_tile_loop(const Op& op, int64_t* tiles, int* grid, int* col_tiles);
 int build_plan(vf_ctx* ctx, Plan* plan);
 
 }  // namespace vf

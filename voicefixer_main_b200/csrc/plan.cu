@@ -810,6 +810,20 @@ std::string op_signature(const Op& op) {
   return s;
 }
 
+void op_tile_loop(const Op& op, int64_t* tiles, int* grid, int* col_tiles) {
+  *tiles = 0; *grid = 0; *col_tiles = 0;
+  if (op.kind == OP_PAIR) {
+    *tiles = (int64_t)op.pair.n_img * op.pair.tiles_per_img;
+    *grid = op.pair.grid;
+    *col_tiles = 1;
+  } else if (op.kind == OP_GEMM) {
+    const GemmProblem& pr = op.tc.prob;
+    *col_tiles = pr.N / op.bn;
+    *tiles = (int64_t)pr.n_img * pr.m_tiles * *col_tiles;
+    *grid = op.tc.grid;
+  }
+}
+
 namespace {
 
 // One nn.Linear of an analysis module on the plan's [B, T, cin] planes (linear_gemm); varlen rows past a clip's end are zeros

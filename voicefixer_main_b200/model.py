@@ -664,15 +664,17 @@ class Engine:
         with torch.cuda.device(self.device):
             self._ck(self.lib.vf_selftest_op(self.ctx, ctypes.byref(case)))
 
-    def selftest_plan_gemms(self, plan_kind: int, batch: int, frames: int):
+    def selftest_plan_gemms(self, plan_kind: int, batch: int, frames: int, tile_loop: bool = False):
         """[(label, signature)] of every GEMM / fused-pair launch of a plan of plan_kind (0 GSR, 1 SSR, 2 GSR varlen, 3 SSR
         varlen) built with the loaded weights and the current options; nothing is launched (vf_selftest_plan_gemms; tests
-        only)."""
+        only).  With tile_loop, [(label, signature, tiles, grid, col_tiles)]: each launch's persistent tile loop as well."""
         cap, n = 2048, ctypes.c_int()
         recs = (L.VfPlanGemm * cap)()
         with torch.cuda.device(self.device):
             self._ck(self.lib.vf_selftest_plan_gemms(self.ctx, plan_kind, batch, frames, recs, cap, ctypes.byref(n)))
         assert n.value <= cap, n.value
+        if tile_loop:
+            return [(r.label.decode(), r.sig.decode(), r.tiles, r.grid, r.col_tiles) for r in recs[:n.value]]
         return [(r.label.decode(), r.sig.decode()) for r in recs[:n.value]]
 
 
