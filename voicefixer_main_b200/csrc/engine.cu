@@ -1,6 +1,6 @@
 // Host side of libb200vf.so: the context, the plan cache, the run machinery and the C ABI (include/b200vf.h) of the restore
-// paths, options, profiling and self-tests.  Weight packing is in pack.cu, plan building in plan.cu, the entry points
-// that use no plan in standalone.cu, and the declarations they share in engine.h.
+// paths, options and profiling.  Weight packing is in pack.cu, plan building in plan.cu, the entry points that use no plan
+// in standalone.cu, the test-only hooks in selftest.cu, and the declarations they share in engine.h.
 //
 // A plan is the full, pre-resolved launch list for one (batch, frames) shape: every activation buffer is
 // allocated once, every TMA tensor map is encoded once, and running a stage is a loop of kernel launches on
@@ -16,6 +16,17 @@
 namespace {
 
 std::string g_create_error;
+
+int prof_mark(vf_ctx* ctx, cudaStream_t st) {
+  const size_t i = ctx->prof.size();     // event i closes record i-1 and opens record i
+  while (ctx->prof_ev.size() <= i) {
+    cudaEvent_t ev;
+    if (cudaEventCreate(&ev) != cudaSuccess) return fail(ctx, VF_ECUDA, "cudaEventCreate failed");
+    ctx->prof_ev.push_back(ev);
+  }
+  if (cudaEventRecord(ctx->prof_ev[i], st) != cudaSuccess) return fail(ctx, VF_ECUDA, "cudaEventRecord failed");
+  return VF_OK;
+}
 
 }  // namespace
 
@@ -71,10 +82,6 @@ int acquire_scratch(vf_ctx* ctx, Scratch& s, size_t need, cudaStream_t st) {
   return rc ? rc : grow_scratch(ctx, s, need, st);
 }
 
-}  // namespace vf
-
-namespace {
-
 void free_plan(Plan* plan) {
   for (auto& g : plan->graph)
     if (g) { cudaGraphExecDestroy(g); g = nullptr; }
@@ -85,6 +92,85 @@ void free_plan(Plan* plan) {
   for (void* p : plan->allocs) cudaFree(p);
   plan->allocs.clear();
 }
+
+// The networks a plan of `kind` runs must have been loaded
+int check_networks(vf_ctx* ctx, int kind) {
+  if (!is_ssr_plan(kind) && !(ctx->analysis != ANALYSIS_NONE && ctx->voc_loaded))
+    return fail(ctx, VF_ESTATE, "this entry point needs the analysis module (generator.analysis_module.*) and the vocoder (vocoder.*) weights");
+  if (is_ssr_plan(kind) && !ctx->ssr.loaded)
+    return fail(ctx, VF_ESTATE, "this entry point needs the unet_v2 weights (generator.unet.*)");
+  return VF_OK;
+}
+
+int run_ops(vf_ctx* ctx, std::vector<Op>& ops, cudaStream_t st) {
+  for (Op& op : ops) {
+    cudaError_t e = cudaSuccess;
+    if (ctx->op_timing) {
+      int rc = prof_mark(ctx, st);
+      if (rc) return rc;
+      const char* kinds[] = {"gemm", "unet_first", "pool", "voc_condition", "reflect_fill", "voc_tail", "finalize", "memset", "pair",
+                             "gru", "affine_planes"};
+      ctx->prof.push_back({op.label[0] ? std::string(op.label) : std::string(kinds[op.kind]), op.flops, op.bytes, op.exec_flops, op.bn, op.bk, op.kind == OP_GEMM ? op.tc.prob.terms : 0});
+    }
+    switch (op.kind) {
+      case OP_GEMM:
+        e = ctx->validate_simt ? launch_gemm_simt(op.simt, st) : launch_gemm_tc(op.tc, op.bn, op.bk, st);
+        break;
+      case OP_FIRST: e = launch_unet_first(op.first, st); break;
+      case OP_POOL: e = launch_pool(op.pool, st); break;
+      case OP_COND: e = launch_voc_condition(op.cond, st); break;
+      case OP_REFLECT: e = launch_reflect_fill(op.refl.pl, op.refl.batch, op.refl.L, op.refl.C, op.refl.pad, st, op.refl.vl_L); break;
+      case OP_TAIL: e = launch_voc_tail(op.tail, st); break;
+      case OP_FINALIZE: e = launch_finalize(op.fin, st); break;
+      case OP_MEMSET32: e = cudaMemsetAsync(op.ms.p, 0, op.ms.bytes, st); break;
+      case OP_PAIR: e = launch_pair_tc(op.pair, st); break;
+      case OP_GRU: e = launch_gru(op.gru, st); break;
+      case OP_PLANES: e = launch_affine_planes(op.planes, st); break;
+    }
+    if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "kernel launch (op kind %d): %s", (int)op.kind, cudaGetErrorString(e));
+    ctx->launches++;
+  }
+  if (ctx->op_timing) return prof_mark(ctx, st);   // closing event of the last record
+  return VF_OK;
+}
+
+int frames_of(vf_ctx* ctx, long n) { return 1 + (int)(n / ctx->cfg.hop); }
+
+// vl_plan: a varlen plan whose lengths table holds the clips of `wav` (n is then the longest clip, T the plan's frames)
+int run_frontend(vf_ctx* ctx, const float* wav, int batch, long n, float* mel, float* logmel, float* sp, float* co,
+                 float* si, cudaStream_t st, const Plan* vl_plan) {
+  if (n <= 1024) return fail(ctx, VF_EINVAL, "reflect padding needs more than n_fft/2 = 1024 samples (got %ld)", n);
+  FrontendParams p;
+  memset(&p, 0, sizeof p);
+  p.wav = wav; p.n = n; p.batch = batch; p.T = frames_of(ctx, n);
+  if (vl_plan) { p.T = vl_plan->T; p.vl_off = vl_plan->d_vl_off; }
+  p.window = ctx->d_window; p.tw1024 = ctx->d_tw1024; p.tw2048 = ctx->d_tw2048;
+  p.fb_f0 = ctx->d_fb_f0; p.fb_len = ctx->d_fb_len; p.fb_ofs = ctx->d_fb_ofs; p.fb_val = ctx->d_fb_val;
+  p.sp_out = sp; p.cos_out = co; p.sin_out = si; p.mel_out = mel; p.logmel_out = logmel;
+  cudaError_t e = launch_frontend(p, st);
+  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "frontend launch: %s", cudaGetErrorString(e));
+  ctx->launches++;
+  return VF_OK;
+}
+
+// This call's lengths -> the lengths table of a varlen plan (host offsets off[0..batch]), in stream order ahead of every
+// kernel that reads it.  w0: the valid frequency bins of the plan's UNet, 127 (mel UNet) or 1024 (unet_v2).
+int write_lengths_table(vf_ctx* ctx, Plan* plan, const int64_t* off, int batch, int w0, cudaStream_t st) {
+  VarlenSetupParams vp;
+  memset(&vp, 0, sizeof vp);
+  for (int i = 0; i <= batch; ++i) vp.off[i] = off[i];
+  vp.batch = batch; vp.hop = ctx->cfg.hop; vp.tail_base = ctx->cfg.voc_tail_base; vp.w0 = w0;
+  vp.n_stages = ctx->cfg.voc_num_stages;
+  for (int s = 0; s < vp.n_stages; ++s) vp.scales[s] = ctx->cfg.voc_scales[s];
+  vp.d_off = plan->d_vl_off; vp.d_rows = plan->d_vl_rows;
+  CK(launch_varlen_setup(vp, st));
+  ctx->launches++;
+  return VF_OK;
+}
+
+}  // namespace vf
+
+namespace {
 
 void drop_all_plans(vf_ctx* ctx) {
   cudaSetDevice(ctx->device);
@@ -130,15 +216,6 @@ int evict_plans(vf_ctx* ctx, size_t incoming, const Plan* keep) {
     ctx->plans.erase(victim);
     ctx->plans_evicted++;
   }
-  return VF_OK;
-}
-
-// The networks a plan of `kind` runs must have been loaded
-int check_networks(vf_ctx* ctx, int kind) {
-  if (!is_ssr_plan(kind) && !(ctx->analysis != ANALYSIS_NONE && ctx->voc_loaded))
-    return fail(ctx, VF_ESTATE, "this entry point needs the analysis module (generator.analysis_module.*) and the vocoder (vocoder.*) weights");
-  if (is_ssr_plan(kind) && !ctx->ssr.loaded)
-    return fail(ctx, VF_ESTATE, "this entry point needs the unet_v2 weights (generator.unet.*)");
   return VF_OK;
 }
 
@@ -255,49 +332,6 @@ int host_roundtrip(vf_ctx* ctx, Plan* plan, const float* in_host, float* out_hos
   return VF_OK;
 }
 
-int prof_mark(vf_ctx* ctx, cudaStream_t st) {
-  const size_t i = ctx->prof.size();     // event i closes record i-1 and opens record i
-  while (ctx->prof_ev.size() <= i) {
-    cudaEvent_t ev;
-    if (cudaEventCreate(&ev) != cudaSuccess) return fail(ctx, VF_ECUDA, "cudaEventCreate failed");
-    ctx->prof_ev.push_back(ev);
-  }
-  if (cudaEventRecord(ctx->prof_ev[i], st) != cudaSuccess) return fail(ctx, VF_ECUDA, "cudaEventRecord failed");
-  return VF_OK;
-}
-
-int run_ops(vf_ctx* ctx, std::vector<Op>& ops, cudaStream_t st) {
-  for (Op& op : ops) {
-    cudaError_t e = cudaSuccess;
-    if (ctx->op_timing) {
-      int rc = prof_mark(ctx, st);
-      if (rc) return rc;
-      const char* kinds[] = {"gemm", "unet_first", "pool", "voc_condition", "reflect_fill", "voc_tail", "finalize", "memset", "pair",
-                             "gru", "affine_planes"};
-      ctx->prof.push_back({op.label[0] ? std::string(op.label) : std::string(kinds[op.kind]), op.flops, op.bytes, op.exec_flops, op.bn, op.bk, op.kind == OP_GEMM ? op.tc.prob.terms : 0});
-    }
-    switch (op.kind) {
-      case OP_GEMM:
-        e = ctx->validate_simt ? launch_gemm_simt(op.simt, st) : launch_gemm_tc(op.tc, op.bn, op.bk, st);
-        break;
-      case OP_FIRST: e = launch_unet_first(op.first, st); break;
-      case OP_POOL: e = launch_pool(op.pool, st); break;
-      case OP_COND: e = launch_voc_condition(op.cond, st); break;
-      case OP_REFLECT: e = launch_reflect_fill(op.refl.pl, op.refl.batch, op.refl.L, op.refl.C, op.refl.pad, st, op.refl.vl_L); break;
-      case OP_TAIL: e = launch_voc_tail(op.tail, st); break;
-      case OP_FINALIZE: e = launch_finalize(op.fin, st); break;
-      case OP_MEMSET32: e = cudaMemsetAsync(op.ms.p, 0, op.ms.bytes, st); break;
-      case OP_PAIR: e = launch_pair_tc(op.pair, st); break;
-      case OP_GRU: e = launch_gru(op.gru, st); break;
-      case OP_PLANES: e = launch_affine_planes(op.planes, st); break;
-    }
-    if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "kernel launch (op kind %d): %s", (int)op.kind, cudaGetErrorString(e));
-    ctx->launches++;
-  }
-  if (ctx->op_timing) return prof_mark(ctx, st);   // closing event of the last record
-  return VF_OK;
-}
-
 // The middle of a restore - every launch between the front end and the tail kernel - reads and writes plan-owned
 // buffers only, so it is the same work every call: replay it as ONE graph launch instead of ~190 kernel launches
 // (SURVEY.md 7 step 6).  `body` enqueues the chain on a stream; it runs eagerly on the first use of the plan, is
@@ -339,25 +373,6 @@ int run_chain(vf_ctx* ctx, Plan* plan, int slot, cudaStream_t st, int64_t n_laun
   return VF_OK;
 }
 
-int frames_of(vf_ctx* ctx, long n) { return 1 + (int)(n / ctx->cfg.hop); }
-
-// vl_plan: a varlen plan whose lengths table holds the clips of `wav` (n is then the longest clip, T the plan's frames)
-int run_frontend(vf_ctx* ctx, const float* wav, int batch, long n, float* mel, float* logmel, float* sp, float* co,
-                 float* si, cudaStream_t st, const Plan* vl_plan = nullptr) {
-  if (n <= 1024) return fail(ctx, VF_EINVAL, "reflect padding needs more than n_fft/2 = 1024 samples (got %ld)", n);
-  FrontendParams p;
-  memset(&p, 0, sizeof p);
-  p.wav = wav; p.n = n; p.batch = batch; p.T = frames_of(ctx, n);
-  if (vl_plan) { p.T = vl_plan->T; p.vl_off = vl_plan->d_vl_off; }
-  p.window = ctx->d_window; p.tw1024 = ctx->d_tw1024; p.tw2048 = ctx->d_tw2048;
-  p.fb_f0 = ctx->d_fb_f0; p.fb_len = ctx->d_fb_len; p.fb_ofs = ctx->d_fb_ofs; p.fb_val = ctx->d_fb_val;
-  p.sp_out = sp; p.cos_out = co; p.sin_out = si; p.mel_out = mel; p.logmel_out = logmel;
-  cudaError_t e = launch_frontend(p, st);
-  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "frontend launch: %s", cudaGetErrorString(e));
-  ctx->launches++;
-  return VF_OK;
-}
-
 int check_ready(vf_ctx* ctx) {
   if (!ctx) return VF_EINVAL;
   if (!ctx->loaded) return fail(ctx, VF_ESTATE, "weights not loaded (call vf_load_weights first)");
@@ -374,21 +389,6 @@ int stage_mark(vf_ctx* ctx, int i, cudaStream_t st) {
       if (!e) CK(cudaEventCreate(&e));
   CK(cudaEventRecord(ctx->ev[i], st));
   if (i == 4) ctx->ev_valid = true;
-  return VF_OK;
-}
-
-// This call's lengths -> the lengths table of a varlen plan (host offsets off[0..batch]), in stream order ahead of every
-// kernel that reads it.  w0: the valid frequency bins of the plan's UNet, 127 (mel UNet) or 1024 (unet_v2).
-int write_lengths_table(vf_ctx* ctx, Plan* plan, const int64_t* off, int batch, int w0, cudaStream_t st) {
-  VarlenSetupParams vp;
-  memset(&vp, 0, sizeof vp);
-  for (int i = 0; i <= batch; ++i) vp.off[i] = off[i];
-  vp.batch = batch; vp.hop = ctx->cfg.hop; vp.tail_base = ctx->cfg.voc_tail_base; vp.w0 = w0;
-  vp.n_stages = ctx->cfg.voc_num_stages;
-  for (int s = 0; s < vp.n_stages; ++s) vp.scales[s] = ctx->cfg.voc_scales[s];
-  vp.d_off = plan->d_vl_off; vp.d_rows = plan->d_vl_rows;
-  CK(launch_varlen_setup(vp, st));
-  ctx->launches++;
   return VF_OK;
 }
 
@@ -1303,541 +1303,5 @@ VF_API int vf_op_info(vf_ctx* ctx, int i, float* ms, double* flops, double* byte
   if (label && label_cap > 0) snprintf(label, label_cap, "%s", ctx->prof[i].label.c_str());
   return VF_OK;
 }
-
-}  // extern "C"
-
-namespace {
-
-HostT host_tensor(const float* p, std::vector<int64_t> shape) {
-  size_t n = 1;
-  for (int64_t d : shape) n *= (size_t)d;
-  return HostT{std::vector<float>(p, p + n), shape};
-}
-
-// Builds and runs one vf_layer_case on plan `b.plan`; the device copies of the outputs are copied back into the case's
-// host buffers.  Weights are packed into ctx->allocs (the caller frees them).
-int run_layer_case(vf_ctx* ctx, Builder& b, vf_layer_case& c) {
-  const bool two_d = c.kind == VF_LAYER_CONV2D || c.kind == VF_LAYER_CONVT2D;
-  const int Wp = two_d ? c.W + 1 : 0;
-  const int rows = two_d ? c.H * Wp : c.L;          // GEMM input rows per image (the pair's and CONVT1D's input rows)
-  const int n = c.n_img;
-  auto up = [&](auto* dst, const void* src, size_t bytes) {
-    if (!b.rc && bytes) {
-      const cudaError_t e = cudaMemcpy(dst, src, bytes, cudaMemcpyHostToDevice);
-      if (e != cudaSuccess) b.rc = fail(ctx, VF_ECUDA, "selftest upload: %s", cudaGetErrorString(e));
-    }
-  };
-  auto dev_planes = [&](const void* host, int img_rows, int C) {   // [2][n][img_rows][C] fp16, uploaded
-    Planes pl = b.planes(n, img_rows, C);
-    if (host) up(pl.p.hi, host, pl.plane_stride * 2 * sizeof(__half));
-    return pl;
-  };
-  auto dev_floats = [&](const float* host, size_t count) -> float* {
-    if (!host) return nullptr;
-    float* d = b.alloc<float>(count);
-    up(d, host, count * sizeof(float));
-    return d;
-  };
-  auto dev_ints = [&](const int* host) -> const int* {
-    if (!host) return nullptr;
-    int* d = b.alloc<int>(n);
-    up(d, host, n * sizeof(int));
-    return d;
-  };
-  const uint32_t ar = ar_inv_word(c.ar_slope);
-  if ((c.resid_kind == VF_RESID_AR || c.out_ar || c.kind == VF_LAYER_PAIR) && !ar)
-    return fail(ctx, VF_EINVAL, "vf_selftest_layer: ar_slope %g has no fp16 inverse", c.ar_slope);
-
-  // weights, through the loaders' packers
-  GemmW W, W2;
-  int rc = VF_OK;
-  switch (c.kind) {
-    case VF_LAYER_CONV2D: {
-      const HostT w = host_tensor(c.w, {c.cout, c.cin, 3, 3});
-      HostT sw, sb;
-      if (c.sc_cin) { sw = host_tensor(c.sc_w, {c.cout, c.sc_cin}); sb = host_tensor(c.sc_b, {c.cout}); }
-      rc = pack_conv3x3(ctx, &W, w, c.sc_cin ? &sw : nullptr, c.sc_cin ? &sb : nullptr);
-      break;
-    }
-    case VF_LAYER_CONVT2D: rc = pack_convT2d(ctx, &W, host_tensor(c.w, {c.cin, c.cout, 3, 3})); break;
-    case VF_LAYER_CONV1D:
-      rc = pack_conv1d(ctx, &W, host_tensor(c.w, {c.cout, c.cin, c.k}), host_tensor(c.b, {c.cout}));
-      break;
-    case VF_LAYER_CONVT1D:
-      rc = pack_convT1d(ctx, &W, host_tensor(c.w, {c.cin, c.cout, 2 * c.stride}), host_tensor(c.b, {c.cout}), c.stride);
-      break;
-    case VF_LAYER_PAIR:
-      rc = pack_conv1d(ctx, &W, host_tensor(c.w, {c.cout, c.cin, 3}), host_tensor(c.b, {c.cout}));
-      if (!rc) rc = pack_conv1d(ctx, &W2, host_tensor(c.w2, {c.cout, c.cout, 3}), host_tensor(c.b2, {c.cout}));
-      break;
-    case VF_LAYER_LINEAR:
-      if (c.b_hh) {     // load_bigru: the layer's W_ih of both directions, b_ih + (b_hr, b_hz, 0)
-        const int G3 = 3 * GRU_HIDDEN;
-        HostT wi[2], bi[2], bh[2];
-        const HostT *pw[2], *pb[2], *ph[2];
-        for (int d = 0; d < 2; ++d) {
-          wi[d] = host_tensor(c.w + (size_t)d * G3 * c.cin, {G3, c.cin});
-          bi[d] = host_tensor(c.b + d * G3, {G3});
-          bh[d] = host_tensor(c.b_hh + d * G3, {G3});
-          pw[d] = &wi[d]; pb[d] = &bi[d]; ph[d] = &bh[d];
-        }
-        rc = pack_gru_ih(ctx, &W, pw, pb, ph);
-      } else {          // load_bigru / load_dnn: pack_linear, the input BatchNorm2d(1) folded as scalar_bn folds it
-        double st[2];
-        if (c.in_bn) scalar_bn_affine(c.in_bn, st);
-        rc = pack_linear(ctx, &W, host_tensor(c.w, {c.cout, c.cin}), host_tensor(c.b, {c.cout}), c.in_bn ? st : nullptr);
-      }
-      break;
-  }
-  if (rc) return rc;
-
-  const Planes X = dev_planes(c.x, c.x_img_rows, c.cin);
-  const ASrc xs{X, c.x_img_rows - c.x_row0, c.x_row0};
-  const int* row_valid = dev_ints(c.row_valid);
-  const size_t out_n = (size_t)n * c.out_img_rows;
-  const Planes OA = c.out_a ? dev_planes(c.out_a, c.out_img_rows, c.a_ld) : Planes();
-  if (b.rc) return b.rc;
-  std::vector<Op> ops;
-  Op* op = nullptr;
-  if (c.kind == VF_LAYER_PAIR) {
-    Op pop;
-    pop.kind = OP_PAIR;
-    rc = pair_setup(ctx, &pop.pair, X, OA, W, W2, n, c.L, c.dilation, ar, c.pair_last != 0, c.out_row0, c.pair_slope_h,
-                    c.pair_slope_out, row_valid);
-    if (rc) return rc;
-    ops.push_back(pop);
-    op = &ops.back();
-    c.bn = 64; c.bk = 64; c.stages = 0; c.resid_tma = 0; c.tma_out = 1;
-    int col_tiles;
-    op_tile_loop(*op, &c.tiles, &c.grid, &col_tiles);
-    c.div_fallback = op->pair.magic_t == 0xffffffffu;
-    snprintf(c.sig, sizeof c.sig, "%s", op_signature(*op).c_str());
-  } else {
-    GemmEpilogue e;
-    memset(&e, 0, sizeof e);
-    std::vector<GemmTap> taps;
-    ASrc s1{};
-    bool has_s1 = false;
-    e.rows_in = rows;
-    e.cout = c.cout;
-    e.out_img_rows = c.out_img_rows;
-    e.out_rows_valid = c.out_img_rows;
-    e.out_row0 = c.out_row0;
-    e.row_valid = row_valid;
-    e.bias = W.bias;
-    switch (c.kind) {
-      case VF_LAYER_CONV2D:
-        e.map = MAP_PLAIN; e.Wp = Wp;
-        taps = taps3x3(Wp, c.cin);
-        if (c.sc_cin) {
-          taps.push_back(GemmTap{0, 1, 0, 0, c.sc_cin});
-          s1 = ASrc{dev_planes(c.sc_x, rows, c.sc_cin), rows, 0};
-          has_s1 = true;
-        }
-        break;
-      case VF_LAYER_CONVT2D:
-        e.map = MAP_CONVT2D; e.Wp = Wp;
-        e.ct_out_wp = c.both ? 2 * Wp - 1 : 2 * Wp;
-        taps = taps_convt2d(Wp, c.cin);
-        break;
-      case VF_LAYER_CONV1D:
-        e.map = MAP_PLAIN;
-        taps = taps1d(c.k, c.dilation, c.cin, c.centered != 0);
-        break;
-      case VF_LAYER_CONVT1D:
-        e.map = MAP_CONVT1D;
-        e.rows_in = c.L + 1;
-        e.ct_stride = c.stride; e.ct_pad = c.stride / 2 + c.stride % 2;
-        taps = taps_convt1d(c.cin);
-        break;
-      case VF_LAYER_LINEAR:      // epi_plain(T, 0, N, T) + linear_gemm below
-        e.map = MAP_PLAIN;
-        break;
-    }
-    if (c.resid_kind == VF_RESID_FP32) {
-      e.resid = dev_floats((const float*)c.resid, (size_t)n * rows * c.cout);
-      e.resid_ld = c.cout;
-    } else if (c.resid_kind == VF_RESID_PLANES || c.resid_kind == VF_RESID_AR) {
-      const Planes R = dev_planes(c.resid, rows, c.cout);
-      e.resid_hi = R.p.hi; e.resid_lo = R.p.lo; e.resid_ld = c.cout;
-      if (c.resid_kind == VF_RESID_AR) e.resid_ar = ar;
-    }
-    if (c.out_raw) { e.out_raw = dev_floats(c.out_raw, out_n * c.raw_ld); e.raw_ld = c.raw_ld; }
-    if (c.out_r) {
-      const Planes R = dev_planes(c.out_r, c.out_img_rows, c.r_ld);
-      e.out_r = OutPlane{R.p.hi, R.p.lo, c.r_ld, c.r_c_off};
-    }
-    if (c.out_a) {
-      e.out_a = OutPlane{OA.p.hi, OA.p.lo, c.a_ld, c.a_c_off};
-      e.a_scale = dev_floats(c.a_scale, c.cout);
-      e.a_shift = dev_floats(c.a_shift, c.cout);
-      e.act = c.act;
-      e.slope = c.slope;
-      if (c.out_ar) e.out_ar = ar;
-    }
-    if (c.head_w) {
-      const size_t hn = (size_t)n * c.head_T * Wp;
-      e.head_w = dev_floats(c.head_w, 32);
-      e.head_b = c.head_b;
-      e.head_in = dev_floats(c.head_in, hn);
-      e.head_out = dev_floats(c.head_out, hn);
-      e.head_T = c.head_T;
-      e.head_valid = dev_ints(c.head_valid);
-    }
-    if (b.rc) return b.rc;
-    if (c.kind == VF_LAYER_LINEAR) linear_gemm(b, ops, W, X, c.L, n, row_valid, e, c.terms);
-    else b.gemm(ops, W, xs, has_s1 ? &s1 : nullptr, taps, e, n, c.terms);
-    if (b.rc) return b.rc;
-    op = &ops.back();
-    c.bn = op->bn; c.bk = op->bk;
-    if (c.impl == VF_LAYER_SIMT) {
-      c.stages = 0; c.resid_tma = 0; c.tma_out = 0;
-      c.grid = op->simt.prob.n_img * op->simt.prob.m_tiles * (op->simt.prob.N / 32);
-      c.tiles = c.grid;
-      c.div_fallback = 0;
-      c.sig[0] = 0;
-    } else {
-      const GemmTcParams& tp = op->tc;
-      c.stages = tp.stages; c.resid_tma = tp.resid_tma; c.tma_out = tp.prob.epi.tma_out;
-      int col_tiles;
-      op_tile_loop(*op, &c.tiles, &c.grid, &col_tiles);
-      c.div_fallback = tp.magic_n == 0xffffffffu || tp.magic_m == 0xffffffffu;
-      snprintf(c.sig, sizeof c.sig, "%s", op_signature(*op).c_str());
-    }
-  }
-  rc = run_ops(ctx, ops, 0);
-  if (rc) return rc;
-  CK(cudaDeviceSynchronize());
-  // outputs back into the host buffers
-  auto down = [&](void* dst, const void* src, size_t bytes) -> int {
-    CK(cudaMemcpy(dst, src, bytes, cudaMemcpyDeviceToHost));
-    return VF_OK;
-  };
-  if (c.out_a) rc = down(c.out_a, OA.p.hi, OA.plane_stride * 2 * sizeof(__half));
-  if (op->kind == OP_GEMM) {
-    const GemmEpilogue& e = c.impl == VF_LAYER_SIMT ? op->simt.prob.epi : op->tc.prob.epi;
-    if (!rc && c.out_raw) rc = down(c.out_raw, e.out_raw, out_n * c.raw_ld * sizeof(float));
-    if (!rc && c.out_r) rc = down(c.out_r, e.out_r.hi, out_n * c.r_ld * 2 * sizeof(__half));
-    if (!rc && c.head_w) rc = down(c.head_out, e.head_out, (size_t)n * c.head_T * Wp * sizeof(float));
-  }
-  return rc;
-}
-
-}  // namespace
-
-extern "C" {
-
-VF_API int vf_selftest_layer(vf_ctx* ctx, vf_layer_case* lc) {
-  if (!ctx || !lc) return VF_EINVAL;
-  vf_layer_case& c = *lc;
-  const bool pair = c.kind == VF_LAYER_PAIR, lin = c.kind == VF_LAYER_LINEAR;
-  if (c.kind < VF_LAYER_CONV2D || c.kind > VF_LAYER_LINEAR || (c.impl != VF_LAYER_PRODUCT && c.impl != VF_LAYER_SIMT) ||
-      (c.terms != 1 && c.terms != 3) || c.n_img <= 0 || !c.x || !c.w || c.cin <= 0 || c.cout <= 0 || c.x_row0 < 0 ||
-      c.out_img_rows <= 0 || c.resid_kind < VF_RESID_NONE || c.resid_kind > VF_RESID_AR ||
-      (c.resid_kind != VF_RESID_NONE && !c.resid) || (c.sc_cin && (c.kind != VF_LAYER_CONV2D || !c.sc_w || !c.sc_b || !c.sc_x)) ||
-      ((c.kind == VF_LAYER_CONV1D || c.kind == VF_LAYER_CONVT1D || pair || lin) && !c.b) ||
-      ((c.in_bn || c.b_hh) && !lin) || (c.in_bn && c.b_hh) || (c.b_hh && c.cout != 6 * GRU_HIDDEN) ||
-      (lin && (c.L <= 0 || c.x_row0 != 0 || c.x_img_rows != c.L || c.resid_kind > VF_RESID_FP32 || c.head_w)) ||
-      ((c.kind == VF_LAYER_CONV2D || c.kind == VF_LAYER_CONVT2D) && (c.H <= 0 || c.W <= 0 || c.b)) ||
-      (c.kind == VF_LAYER_CONV1D && (c.k <= 0 || c.dilation <= 0)) || (c.kind == VF_LAYER_CONVT1D && c.stride <= 0) ||
-      (c.head_w && (!c.head_out || c.head_T <= 0)) ||
-      (pair && (!c.w2 || !c.b2 || !c.out_a || c.terms != 1 || c.resid_kind != VF_RESID_NONE || c.dilation <= 0)))
-    return fail(ctx, VF_EINVAL, "vf_selftest_layer: bad case");
-  // the SIMT kernel's epilogue (gemm.cuh: epilogue_chunk) has no (a, r) stream and there is no SIMT pair
-  if (c.impl == VF_LAYER_SIMT && (pair || c.out_ar || c.resid_kind == VF_RESID_AR))
-    return fail(ctx, VF_EINVAL, "vf_selftest_layer: the SIMT kernel has no (a, r) stream");
-  CK(cudaSetDevice(ctx->device));
-  const size_t n_weight_allocs = ctx->allocs.size(), weight_bytes = ctx->weight_bytes;
-  const int saved = ctx->validate_simt;
-  ctx->validate_simt = c.impl == VF_LAYER_SIMT;
-  Plan plan;
-  Builder b{ctx, &plan};
-  int rc = run_layer_case(ctx, b, c);
-  ctx->validate_simt = saved;
-  const cudaError_t se = cudaDeviceSynchronize();
-  for (void* p : plan.allocs) cudaFree(p);
-  for (size_t i = n_weight_allocs; i < ctx->allocs.size(); ++i) cudaFree(ctx->allocs[i]);
-  ctx->allocs.resize(n_weight_allocs);
-  ctx->weight_bytes = weight_bytes;
-  if (!rc && se != cudaSuccess) rc = fail(ctx, VF_ECUDA, "vf_selftest_layer: %s", cudaGetErrorString(se));
-  return rc;
-}
-
-}  // extern "C"
-
-namespace {
-
-// Builds and runs one vf_op_case with its buffers in `b.plan`; each op's parameter block comes from the helper the plans
-// use, and the buffers are sized from what that helper derived.  Outputs are copied back into the case's host buffers.
-int run_op_case(vf_ctx* ctx, Builder& b, vf_op_case& c) {
-  Plan& plan = *b.plan;
-  const int B = c.batch;
-  plan.batch = B;
-  struct Down { void* host; const void* dev; size_t bytes; };
-  std::vector<Down> downs;
-  auto dev = [&](const void* host, size_t bytes) -> void* {        // device copy of a host buffer (or of nothing)
-    uint8_t* d = b.alloc<uint8_t>(bytes);
-    if (!b.rc && host && bytes) {
-      const cudaError_t e = cudaMemcpy(d, host, bytes, cudaMemcpyHostToDevice);
-      if (e != cudaSuccess) b.rc = fail(ctx, VF_ECUDA, "selftest upload: %s", cudaGetErrorString(e));
-    }
-    return d;
-  };
-  auto out = [&](void* host, size_t bytes) -> void* {             // in/out: uploaded now, copied back after the launch
-    if (!host) return nullptr;
-    void* d = dev(host, bytes);
-    downs.push_back({host, d, bytes});
-    return d;
-  };
-  auto planes_out = [&](uint16_t* host, size_t n) -> PlanePtr {  // [2][n] fp16 planes
-    __half* d = static_cast<__half*>(out(host, 2 * n * sizeof(__half)));
-    return PlanePtr{d, d ? d + n : nullptr};
-  };
-  auto fl = [&](const float* host, size_t n) { return static_cast<float*>(dev(host, n * sizeof(float))); };
-  const int last = VL_VOC + ctx->cfg.voc_num_stages - 1;
-  const int64_t packed = c.clip_off ? c.clip_off[B] : 0;            // samples of all clips when they are packed
-  int rc = VF_OK;
-  if (c.clip_off) {
-    plan.d_vl_off = b.alloc<int64_t>((size_t)B + 1);
-    plan.d_vl_rows = b.alloc<int>((size_t)VL_ROWS * B);
-    if (b.rc) return b.rc;
-    rc = write_lengths_table(ctx, &plan, c.clip_off, B, c.unet_w0, 0);
-    if (rc) return rc;
-  }
-  std::vector<Op> ops;
-  switch (c.kind) {
-    case VF_OP_FIRST: {
-      UnetW U;
-      ConvBlockW blk;
-      U.first_bn1_scale = c.bn1_scale; U.first_bn1_shift = c.bn1_shift;
-      U.d_first_w1 = fl(c.w1, 32 * 9); U.d_first_wsc = fl(c.w_sc, 32); U.d_first_bsc = fl(c.b_sc, 32);
-      blk.bn2 = Affine{fl(c.bn2_scale, 32), fl(c.bn2_shift, 32)};
-      Op op = first_op(ctx, U, blk, fl(c.x, (size_t)B * c.T * (c.W + 1)), B, c.T, c.W, PlanePtr{nullptr, nullptr}, nullptr,
-                       plan.vl(VL_T), plan.vl(VL_TP));
-      UnetFirstParams& f = op.first;
-      const size_t n = (size_t)B * f.Tp * (f.W + 1) * 32;
-      f.a2 = planes_out(c.a2, n);
-      f.sc_raw = static_cast<float*>(out(c.sc_raw, n * sizeof(float)));
-      c.Tp = f.Tp;
-      ops.push_back(op);
-      break;
-    }
-    case VF_OP_POOL: {
-      const Affine bn1{fl(c.a_scale, c.C), fl(c.a_shift, c.C)};
-      Op op = pool_op(ctx, fl(c.pin, (size_t)B * c.H * (c.W + 1) * c.C), B, c.H, c.W, c.C, bn1, PlanePtr{nullptr, nullptr},
-                      PlanePtr{nullptr, nullptr}, nullptr, plan.vl(VL_UNET + c.level + 1));
-      PoolParams& p = op.pool;
-      const size_t n = (size_t)B * (p.H / 2) * p.Wpo * p.C;
-      p.out_r = planes_out(c.out_r, n);
-      p.out_a = planes_out(c.out_a, n);
-      p.out_raw = static_cast<float*>(out(c.out_raw, n * sizeof(float)));
-      c.Wpo = p.Wpo;
-      ops.push_back(op);
-      break;
-    }
-    case VF_OP_COND: {
-      const size_t mel_n = (size_t)B * c.T * 128;
-      Op op = cond_op(ctx, fl(c.mel, mel_n), B, c.T, PlanePtr{nullptr, nullptr}, plan.vl(VL_T), plan.vl(VL_TV));
-      VocCondParams& p = op.cond;
-      p.is_log = c.is_log;
-      p.out = planes_out(c.cond, (size_t)B * p.Tv * 128);
-      c.Tv = p.Tv;
-      if (c.unify) {     // restore_impl: the band sums of the linear input mel and the restored log-mel, then the conditioning
-        float* sums = static_cast<float*>(out(c.band_sums, 2 * (size_t)B * sizeof(float)));
-        if (b.rc) return b.rc;
-        CK(unify_energy(fl(c.mel_target, mel_n), p.mel, B, c.T, sums, plan.vl(VL_T), &p, 0));
-      }
-      ops.push_back(op);
-      break;
-    }
-    case VF_OP_REFLECT:
-      ops.push_back(reflect_op(planes_out(c.planes, (size_t)B * (c.L + 6) * c.C), B, (int)c.L, c.C,
-                               c.cond_pad ? plan.vl(VL_TV) : plan.vl(last)));
-      break;
-    case VF_OP_TAIL: {
-      float* w = nullptr;
-      rc = pack_tail(ctx, &w, host_tensor(c.tail_w, {1, c.C, 7}));
-      if (rc) return rc;
-      const size_t n = (size_t)B * (c.L + 6) * c.C;
-      __half* in = static_cast<__half*>(dev(c.tail_in, 2 * n * sizeof(__half)));
-      float* wav = static_cast<float*>(out(c.wav, (size_t)B * c.L * sizeof(float)));
-      unsigned int* peak = static_cast<unsigned int*>(out(c.peak_bits, (size_t)B * sizeof(unsigned int)));
-      ops.push_back(memset_op(peak, (size_t)B * 4));
-      ops.push_back(tail_op(PlanePtr{in, in + n}, B, c.L, c.C, c.terms, w, c.tail_b, c.tanh_out, wav, peak, plan.vl(last)));
-      c.tail_smem = (int64_t)voc_tail_smem_bytes(c.C, c.terms);
-      break;
-    }
-    case VF_OP_FINALIZE: {
-      Op op;
-      op.kind = OP_FINALIZE;
-      float* o = static_cast<float*>(out(c.out, (c.clip_off ? packed : (int64_t)B * c.n) * sizeof(float)));
-      if (b.rc) return b.rc;
-      rc = finalize_params(ctx, &op.fin, fl(c.in_wav, (size_t)B * c.L), static_cast<unsigned int*>(dev(c.peak_bits, B * 4)), B,
-                           c.L, c.n, o, plan.d_vl_off, plan.vl(last));
-      if (rc) return rc;
-      c.skip = op.fin.skip;
-      ops.push_back(op);
-      break;
-    }
-    case VF_OP_ISTFT: {
-      const int64_t wav_n = c.clip_off ? packed : (int64_t)B * c.n;
-      float* frames = static_cast<float*>(out(c.frames, (size_t)B * c.T * 2048 * sizeof(float)));
-      float* o = static_cast<float*>(out(c.out, wav_n * sizeof(float)));
-      const float* mag = fl(c.mag, (size_t)B * c.T * 1025);
-      const float* wav = fl(c.in_wav, wav_n);
-      if (b.rc) return b.rc;
-      IstftFramesParams fp;
-      IstftOlaParams op;
-      istft_params(ctx, &fp, &op, mag, wav, B, c.n, c.T, frames, o, plan.d_vl_off, plan.vl(VL_T));
-      CK(launch_istft_frames(fp, 0));
-      CK(launch_istft_ola(op, 0));
-      break;
-    }
-    case VF_OP_PEAK_NORM: {      // ssr_restore_varlen's VF_SSR_PEAK_NORMALISE
-      float* wav = static_cast<float*>(out(c.wav, packed * sizeof(float)));
-      unsigned int* peak = static_cast<unsigned int*>(out(c.peak_bits, (size_t)B * sizeof(unsigned int)));
-      if (b.rc) return b.rc;
-      CK(cudaMemsetAsync(peak, 0, (size_t)B * sizeof(unsigned int), 0));
-      CK(launch_peak_normalise_varlen(wav, plan.d_vl_off, B, (long)c.n, peak, 0));
-      break;
-    }
-    case VF_OP_FRONTEND: {       // run_frontend as restore_impl, ssr_impl, ssr_restore_varlen and vf_frontend call it
-      if (!ctx->d_fb_val) return fail(ctx, VF_ESTATE, "vf_selftest_op: mel filterbank not loaded");
-      if (!c.clip_off) c.T = frames_of(ctx, (long)c.n);
-      for (int i = 0; c.clip_off && i < B; ++i) {
-        const long nb = (long)(c.clip_off[i + 1] - c.clip_off[i]);
-        if (nb <= 1024 || nb > c.n || frames_of(ctx, nb) > c.T)
-          return fail(ctx, VF_EINVAL, "vf_selftest_op: clip %d has %ld samples (need 1025 .. n, at most T = %d frames)", i, nb, c.T);
-      }
-      const size_t rows = (size_t)B * c.T;
-      float* mel = static_cast<float*>(out(c.mel_out, rows * 128 * sizeof(float)));
-      float* logmel = static_cast<float*>(out(c.logmel_out, rows * 128 * sizeof(float)));
-      float* sp = static_cast<float*>(out(c.sp_out, rows * 1025 * sizeof(float)));
-      float* co = static_cast<float*>(out(c.cos_out, rows * 1025 * sizeof(float)));
-      float* si = static_cast<float*>(out(c.sin_out, rows * 1025 * sizeof(float)));
-      const float* wav = fl(c.in_wav, c.clip_off ? packed : (int64_t)B * c.n);
-      if (b.rc) return b.rc;
-      plan.T = c.T;
-      rc = run_frontend(ctx, wav, B, (long)c.n, mel, logmel, sp, co, si, 0, c.clip_off ? &plan : nullptr);
-      if (rc) return rc;
-      break;
-    }
-    case VF_OP_PLANES: {         // the first op of build_bigru (BN0's scale and shift) and build_dnn (1, 0)
-      const size_t n = (size_t)B * c.T * 128;
-      const float* x = fl(c.x, n);
-      const PlanePtr o = planes_out(c.planes, n);
-      ops.push_back(planes_op(x, B, c.T, c.bn1_scale, c.bn1_shift, o, plan.vl(VL_T)));
-      break;
-    }
-  }
-  if (b.rc) return b.rc;
-  rc = run_ops(ctx, ops, 0);
-  if (rc) return rc;
-  CK(cudaDeviceSynchronize());
-  for (const Down& d : downs) CK(cudaMemcpy(d.host, d.dev, d.bytes, cudaMemcpyDeviceToHost));
-  if (c.vl_rows && plan.d_vl_rows) CK(cudaMemcpy(c.vl_rows, plan.d_vl_rows, (size_t)VL_ROWS * B * sizeof(int), cudaMemcpyDeviceToHost));
-  return VF_OK;
-}
-
-}  // namespace
-
-extern "C" {
-
-VF_API int vf_selftest_gru(vf_ctx* ctx, vf_gru_case* gc) {
-  if (!ctx || !gc) return VF_EINVAL;
-  const vf_gru_case& c = *gc;
-  if (c.batch <= 0 || c.T <= 0 || !c.G || !c.w_hh || !c.b_hn || !c.out) return fail(ctx, VF_EINVAL, "vf_selftest_gru: bad case");
-  for (int b = 0; c.lengths && b < c.batch; ++b)
-    if (c.lengths[b] < 1 || c.lengths[b] > c.T) return fail(ctx, VF_EINVAL, "vf_selftest_gru: clip %d has %d of %d frames", b, c.lengths[b], c.T);
-  CK(cudaSetDevice(ctx->device));
-  Plan plan;
-  Builder b{ctx, &plan};
-  const size_t H = GRU_HIDDEN, rows = (size_t)c.batch * c.T;
-  auto dev = [&](const void* host, size_t bytes) -> void* {
-    void* d = b.alloc<uint8_t>(bytes);
-    if (!b.rc && cudaMemcpy(d, host, bytes, cudaMemcpyHostToDevice) != cudaSuccess) b.rc = fail(ctx, VF_ECUDA, "vf_selftest_gru: upload");
-    return d;
-  };
-  const float* G = static_cast<const float*>(dev(c.G, rows * 6 * H * 4));
-  const float* w = static_cast<const float*>(dev(c.w_hh, 2 * 3 * H * H * 4));
-  const float* bhn = static_cast<const float*>(dev(c.b_hn, 2 * H * 4));
-  const int* len = c.lengths ? static_cast<const int*>(dev(c.lengths, (size_t)c.batch * 4)) : nullptr;
-  __half* out = static_cast<__half*>(dev(c.out, 2 * rows * 2 * H * 2));
-  int rc = b.rc;
-  if (!rc) {
-    const GruDirW dirs[2] = {{const_cast<float*>(w), const_cast<float*>(bhn)}, {const_cast<float*>(w) + 3 * H * H, const_cast<float*>(bhn) + H}};
-    std::vector<Op> ops{gru_op(G, dirs, PlanePtr{out, out + rows * 2 * H}, c.batch, c.T, c.relu != 0, len, "gru")};
-    rc = run_ops(ctx, ops, 0);
-  }
-  const cudaError_t se = cudaDeviceSynchronize();
-  if (!rc && se != cudaSuccess) rc = fail(ctx, VF_ECUDA, "vf_selftest_gru: %s", cudaGetErrorString(se));
-  if (!rc && cudaMemcpy(c.out, out, 2 * rows * 2 * H * 2, cudaMemcpyDeviceToHost) != cudaSuccess)
-    rc = fail(ctx, VF_ECUDA, "vf_selftest_gru: download");
-  for (void* p : plan.allocs) cudaFree(p);
-  return rc;
-}
-
-VF_API int vf_selftest_op(vf_ctx* ctx, vf_op_case* oc) {
-  if (!ctx || !oc) return VF_EINVAL;
-  vf_op_case& c = *oc;
-  const bool bad_kind = c.kind < VF_OP_FIRST || c.kind > VF_OP_PLANES;
-  const bool bad_shape =
-      (c.kind == VF_OP_FIRST && (c.T <= 0 || c.W <= 0 || !c.x || !c.w1 || !c.bn2_scale || !c.bn2_shift || !c.w_sc || !c.b_sc)) ||
-      (c.kind == VF_OP_POOL && (c.H < 2 || c.W <= 0 || c.C <= 0 || c.C % 8 || !c.pin || !c.a_scale || !c.a_shift || c.level < 0 || c.level > 5)) ||
-      (c.kind == VF_OP_COND && (c.T <= 0 || !c.mel || !c.cond || (c.unify && (!c.mel_target || !c.band_sums)))) ||
-      (c.kind == VF_OP_REFLECT && (c.L < 4 || c.C <= 0 || c.C % 8 || !c.planes)) ||
-      (c.kind == VF_OP_TAIL && (c.L <= 0 || c.C <= 0 || c.C % 8 || (c.terms != 1 && c.terms != 3) || !c.tail_in || !c.tail_w ||
-                                !c.wav || !c.peak_bits)) ||
-      (c.kind == VF_OP_FINALIZE && (c.L <= 0 || c.n <= 0 || !c.in_wav || !c.peak_bits || !c.out)) ||
-      (c.kind == VF_OP_ISTFT && (c.T <= 0 || c.n <= 1024 || !c.mag || !c.in_wav || !c.frames || !c.out)) ||
-      (c.kind == VF_OP_PEAK_NORM && (!c.clip_off || c.n <= 0 || !c.wav || !c.peak_bits)) ||
-      (c.kind == VF_OP_FRONTEND && (c.n <= 0 || !c.in_wav || (c.clip_off && c.T <= 0) || !c.cos_out != !c.sin_out || (c.cos_out && !c.sp_out))) ||
-      (c.kind == VF_OP_PLANES && (c.T <= 0 || !c.x || !c.planes));
-  if (bad_kind || c.batch <= 0 || bad_shape || (c.clip_off && (c.batch > VL_MAX_CLIPS || c.clip_off[0] != 0)))
-    return fail(ctx, VF_EINVAL, "vf_selftest_op: bad case");
-  CK(cudaSetDevice(ctx->device));
-  const size_t n_weight_allocs = ctx->allocs.size(), weight_bytes = ctx->weight_bytes;
-  Plan plan;
-  Builder b{ctx, &plan};
-  int rc = run_op_case(ctx, b, c);
-  const cudaError_t se = cudaDeviceSynchronize();
-  for (void* p : plan.allocs) cudaFree(p);
-  for (size_t i = n_weight_allocs; i < ctx->allocs.size(); ++i) cudaFree(ctx->allocs[i]);
-  ctx->allocs.resize(n_weight_allocs);
-  ctx->weight_bytes = weight_bytes;
-  if (!rc && se != cudaSuccess) rc = fail(ctx, VF_ECUDA, "vf_selftest_op: %s", cudaGetErrorString(se));
-  return rc;
-}
-
-VF_API int vf_selftest_plan_gemms(vf_ctx* ctx, int plan_kind, int batch, int frames, vf_plan_gemm* records, int cap, int* count) {
-  if (!ctx || !count || cap < 0 || (cap && !records)) return VF_EINVAL;
-  if (plan_kind < PLAN_GSR || plan_kind > PLAN_SSR_VARLEN || batch <= 0 || frames <= 0 ||
-      (is_varlen_plan(plan_kind) && batch > VL_MAX_CLIPS))
-    return fail(ctx, VF_EINVAL, "vf_selftest_plan_gemms: bad plan");
-  if (ctx->validate_simt) return fail(ctx, VF_EINVAL, "vf_selftest_plan_gemms: validate_simt plans run no tensor-core launches");
-  if (!ctx->loaded) return fail(ctx, VF_ESTATE, "weights not loaded");
-  int rc = check_networks(ctx, plan_kind);
-  if (rc) return rc;
-  CK(cudaSetDevice(ctx->device));
-  Plan plan;
-  plan.kind = plan_kind; plan.batch = batch; plan.T = frames;
-  rc = build_plan(ctx, &plan);
-  int n = 0;
-  for (const std::vector<Op>* list : {&plan.unet, &plan.vocoder})
-    for (const Op& op : *list) {
-      const std::string s = rc ? std::string() : op_signature(op);
-      if (s.empty()) continue;
-      if (n < cap) {
-        snprintf(records[n].label, sizeof records[n].label, "%s", op.label);
-        snprintf(records[n].sig, sizeof records[n].sig, "%s", s.c_str());
-        op_tile_loop(op, &records[n].tiles, &records[n].grid, &records[n].col_tiles);
-      }
-      ++n;
-    }
-  *count = n;
-  free_plan(&plan);
-  return rc;
-}
-
 
 }  // extern "C"

@@ -1,6 +1,6 @@
 // Declarations shared by the host translation units of libb200vf.so: engine.cu (context, plan cache, run machinery, C ABI),
-// pack.cu (weight ingestion and packing), plan.cu (launch plans) and standalone.cu (the plan-free entry points).  No
-// kernels are declared or defined here.
+// pack.cu (weight ingestion and packing), plan.cu (launch plans), standalone.cu (the plan-free entry points) and selftest.cu
+// (the test-only hooks).  No kernels are declared or defined here.
 #pragma once
 
 #include <cuda.h>
@@ -295,6 +295,14 @@ int mark_use(vf_ctx* ctx, StreamOrder& o, cudaStream_t st);
 // Once this succeeds, mark_use(ctx, s.order, st) must run on every path, a failed launch included: the sub-batches
 // queued before it read the scratch.
 int acquire_scratch(vf_ctx* ctx, Scratch& s, size_t need, cudaStream_t st);
+// engine.cu: the run machinery the self-tests (selftest.cu) share with the restore paths
+void free_plan(Plan* plan);
+int check_networks(vf_ctx* ctx, int kind);
+int run_ops(vf_ctx* ctx, std::vector<Op>& ops, cudaStream_t st);
+int frames_of(vf_ctx* ctx, long n);
+int run_frontend(vf_ctx* ctx, const float* wav, int batch, long n, float* mel, float* logmel, float* sp, float* co,
+                 float* si, cudaStream_t st, const Plan* vl_plan = nullptr);
+int write_lengths_table(vf_ctx* ctx, Plan* plan, const int64_t* off, int batch, int w0, cudaStream_t st);
 
 // pack.cu
 int upload_gemm(vf_ctx* ctx, GemmW* w, const std::vector<float>& m, int N, int K, const std::vector<float>* bias);
@@ -336,6 +344,13 @@ struct Builder {
             GemmEpilogue epi, int n_img, int terms);
 };
 GemmEpilogue epi_plain(int rows_in, int Wp, int cout, int out_img_rows);
+// ConvTranspose2d k3 s2 (pack_convT2d) of rows_in rows of pitch Wp into output rows of pitch out_wp
+GemmEpilogue epi_convt2d(int rows_in, int Wp, int cout, int out_img_rows, int out_wp);
+// ConvTranspose1d of stride s, padding s / 2 + s % 2 (pack_convT1d) of rows_in rows: GEMM rows q = 0 .. rows_in produce s
+// phases each
+GemmEpilogue epi_convt1d(int rows_in, int stride, int cout, int out_rows);
+// The activated output: act(scale * v + shift) into `pl` from channel c_off (scale, shift null: identity)
+void set_out_a(GemmEpilogue& e, const Planes& pl, int c_off, const float* scale, const float* shift, int act, float slope);
 // (a, r) residual stream (gemm.cuh): fp16(1 / slope) in both halves of a word, 0 when the LeakyReLU is not invertible that way
 uint32_t ar_inv_word(float slope);
 // Tap lists of the plans' convs: Conv2d 3x3 pad 1 on rows of pitch Wp; the four (dh, dw) input shifts of ConvTranspose2d

@@ -323,6 +323,29 @@ GemmEpilogue epi_plain(int rows_in, int Wp, int cout, int out_img_rows) {
   return e;
 }
 
+GemmEpilogue epi_convt2d(int rows_in, int Wp, int cout, int out_img_rows, int out_wp) {
+  GemmEpilogue e = epi_plain(rows_in, Wp, cout, out_img_rows);
+  e.map = MAP_CONVT2D;
+  e.ct_out_wp = out_wp;
+  return e;
+}
+
+GemmEpilogue epi_convt1d(int rows_in, int stride, int cout, int out_rows) {
+  GemmEpilogue e = epi_plain(rows_in + 1, 0, cout, out_rows);
+  e.map = MAP_CONVT1D;
+  e.ct_stride = stride;
+  e.ct_pad = stride / 2 + stride % 2;
+  return e;
+}
+
+void set_out_a(GemmEpilogue& e, const Planes& pl, int c_off, const float* scale, const float* shift, int act, float slope) {
+  e.out_a = OutPlane{pl.p.hi, pl.p.lo, pl.C, c_off};
+  e.a_scale = scale;
+  e.a_shift = shift;
+  e.act = act;
+  e.slope = slope;
+}
+
 Op first_op(vf_ctx* ctx, const UnetW& U, const ConvBlockW& blk, const float* in, int batch, int T, int W0, PlanePtr a2,
             float* sc_raw, const int* vl_T, const int* vl_Tp) {
   Op op; op.kind = OP_FIRST;
@@ -432,14 +455,6 @@ namespace {
 const int ENC_C[6] = {32, 64, 128, 256, 384, 384};
 const int DEC_CIN[6] = {384, 384, 384, 256, 128, 64};
 const int DEC_COUT[6] = {384, 384, 256, 128, 64, 32};
-
-void set_out_a(GemmEpilogue& e, const Planes& pl, int c_off, const float* scale, const float* shift, int act, float slope) {
-  e.out_a = OutPlane{pl.p.hi, pl.p.lo, pl.C, c_off};
-  e.a_scale = scale;
-  e.a_shift = shift;
-  e.act = act;
-  e.slope = slope;
-}
 
 struct Level {
   int H, W, Wp, C, rows;
@@ -570,12 +585,9 @@ int build_unet(vf_ctx* ctx, Builder& b, Plan* plan, const UnetW& U, const UnetGe
     Level& Lin = lv[6 - k];
     const int cin = DEC_CIN[k], cout = DEC_COUT[k];
     {   // ConvTranspose2d k3 s2 + prune + concat placement (modules.py:213-215)
-      GemmEpilogue e;
-      memset(&e, 0, sizeof e);
-      e.map = MAP_CONVT2D; e.rows_in = Lin.rows; e.Wp = Lin.Wp; e.cout = cout; e.out_img_rows = L.rows;
-      e.out_rows_valid = L.rows;
+      // output pitch L.Wp: 2 * Lin.Wp (time-only prune, modules.py:209) or 2 * Lin.Wp - 1 (both=True, modules.py:207-208)
+      GemmEpilogue e = epi_convt2d(Lin.rows, Lin.Wp, cout, L.rows, L.Wp);
       e.row_valid = Lin.valid;
-      e.ct_out_wp = L.Wp;      // 2 * Lin.Wp (time-only prune, modules.py:209) or 2 * Lin.Wp - 1 (both=True, modules.py:207-208)
       const ConvBlockW& blk = U.dec[k][0];
       e.out_r = OutPlane{L.cat_r.p.hi, L.cat_r.p.lo, 2 * L.C, 0};
       set_out_a(e, L.cat_a, 0, blk.bn1.scale, blk.bn1.shift, ACT_LRELU, S);
@@ -677,10 +689,7 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
     if (last_stage) tail_in = b.planes(B, (int)L + 6, cout);
     if (b.rc) return b.rc;
     {   // ConvTranspose1d: rows q = 0..Lprev produce s phases each
-      GemmEpilogue e;
-      memset(&e, 0, sizeof e);
-      e.map = MAP_CONVT1D; e.rows_in = (int)Lprev + 1; e.cout = cout; e.out_img_rows = (int)L; e.out_rows_valid = (int)L;
-      e.ct_stride = sc; e.ct_pad = sc / 2 + sc % 2;
+      GemmEpilogue e = epi_convt1d((int)Lprev, sc, cout, (int)L);
       e.row_valid = plan->vl(VL_VOC + s);
       e.bias = ctx->voc_up[s].bias;
       if (ar) e.out_ar = ar;

@@ -1,0 +1,480 @@
+// The test-only hooks of include/b200vf.h (vf_selftest_*): one conv layer, one non-GEMM op or one GRU layer set up the way
+// the plans set it up and run on buffers the caller chose, and the GEMM launches a plan builds.  Each hook runs its case in
+// run_case, on a temporary plan that stages the caller's host buffers, and leaves the context as it found it.
+#include <cstdio>
+
+#include "engine.h"
+
+namespace {
+
+HostT host_tensor(const float* p, std::vector<int64_t> shape) {
+  size_t n = 1;
+  for (int64_t d : shape) n *= (size_t)d;
+  return HostT{std::vector<float>(p, p + n), shape};
+}
+
+// The buffers of one case: a temporary plan, its builder, and the caller's host buffers staged on it.  in() returns a device
+// copy of `count` elements of `host` (null for null); inout() also copies them back once the case has run.  The _planes
+// forms stage fp16 planes [2][n_img][img_rows][C].
+struct Case {
+  vf_ctx* ctx;
+  Plan plan;
+  Builder b;
+  struct Back { void* host; const void* dev; size_t bytes; };
+  std::vector<Back> backs;
+
+  explicit Case(vf_ctx* c) : ctx(c), b{c, &plan} {}
+
+  void upload(void* dev, const void* host, size_t bytes) {
+    if (b.rc || !bytes) return;
+    const cudaError_t e = cudaMemcpy(dev, host, bytes, cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) b.rc = fail(ctx, VF_ECUDA, "selftest upload: %s", cudaGetErrorString(e));
+  }
+  // `bytes` of `dev` go back into `host` once the case has run
+  void back(void* host, const void* dev, size_t bytes) {
+    if (dev) backs.push_back({host, dev, bytes});
+  }
+  template <typename T>
+  T* in(const T* host, size_t count) {
+    if (!host) return nullptr;
+    T* d = b.alloc<T>(count);
+    upload(d, host, count * sizeof(T));
+    return d;
+  }
+  template <typename T>
+  T* inout(T* host, size_t count) {
+    T* d = in<T>(host, count);
+    back(host, d, count * sizeof(T));
+    return d;
+  }
+  Planes in_planes(const uint16_t* host, size_t n_img, int img_rows, int C) {
+    if (!host) return Planes();
+    const Planes pl = b.planes(n_img, img_rows, C);
+    upload(pl.p.hi, host, 2 * pl.plane_stride * sizeof(__half));
+    return pl;
+  }
+  Planes inout_planes(uint16_t* host, size_t n_img, int img_rows, int C) {
+    const Planes pl = in_planes(host, n_img, img_rows, C);
+    back(host, pl.p.hi, 2 * pl.plane_stride * sizeof(__half));
+    return pl;
+  }
+};
+
+// One case of `hook`: sets the device, records the context's weight allocations and runs body(case) with the option
+// validate_simt set to `validate_simt`.  Then, on every path: a hook that launches synchronises and copies the inout()
+// buffers back; the plan's buffers and the weights the case packed are freed; weight_bytes and validate_simt are restored.
+template <typename F>
+int run_case(vf_ctx* ctx, const char* hook, bool launches, int validate_simt, F body) {
+  CK(cudaSetDevice(ctx->device));
+  const size_t n_weight_allocs = ctx->allocs.size(), weight_bytes = ctx->weight_bytes;
+  const int saved_simt = ctx->validate_simt;
+  ctx->validate_simt = validate_simt;
+  Case s(ctx);
+  int rc = body(s);
+  ctx->validate_simt = saved_simt;
+  if (launches) {
+    const cudaError_t se = cudaDeviceSynchronize();
+    if (!rc && se != cudaSuccess) rc = fail(ctx, VF_ECUDA, "%s: %s", hook, cudaGetErrorString(se));
+    for (size_t i = 0; !rc && i < s.backs.size(); ++i) {
+      const cudaError_t e = cudaMemcpy(s.backs[i].host, s.backs[i].dev, s.backs[i].bytes, cudaMemcpyDeviceToHost);
+      if (e != cudaSuccess) rc = fail(ctx, VF_ECUDA, "selftest copy back: %s", cudaGetErrorString(e));
+    }
+  }
+  free_plan(&s.plan);
+  for (size_t i = n_weight_allocs; i < ctx->allocs.size(); ++i) cudaFree(ctx->allocs[i]);
+  ctx->allocs.resize(n_weight_allocs);
+  ctx->weight_bytes = weight_bytes;
+  return rc;
+}
+
+// What the hooks report of a built OP_GEMM (tensor-core path) or OP_PAIR: its configuration signature, its persistent tile
+// loop, and whether a tile decode divides (its multiply-high magic would not be exact)
+template <size_t N>
+void report_launch(const Op& op, char (&sig)[N], int64_t* tiles, int* grid, int* col_tiles, int* div_fallback) {
+  snprintf(sig, N, "%s", op_signature(op).c_str());
+  op_tile_loop(op, tiles, grid, col_tiles);
+  *div_fallback = op.kind == OP_PAIR ? op.pair.magic_t == 0xffffffffu : op.tc.magic_n == 0xffffffffu || op.tc.magic_m == 0xffffffffu;
+}
+
+// Builds and runs one vf_layer_case on the case's plan.  Weights are packed into ctx->allocs.
+int run_layer_case(vf_ctx* ctx, Case& s, vf_layer_case& c) {
+  Builder& b = s.b;
+  const bool two_d = c.kind == VF_LAYER_CONV2D || c.kind == VF_LAYER_CONVT2D;
+  const int Wp = two_d ? c.W + 1 : 0;
+  const int rows = two_d ? c.H * Wp : c.L;          // GEMM input rows per image (the pair's and CONVT1D's input rows)
+  const int n = c.n_img;
+  const uint32_t ar = ar_inv_word(c.ar_slope);
+  if ((c.resid_kind == VF_RESID_AR || c.out_ar || c.kind == VF_LAYER_PAIR) && !ar)
+    return fail(ctx, VF_EINVAL, "vf_selftest_layer: ar_slope %g has no fp16 inverse", c.ar_slope);
+
+  // weights, through the loaders' packers
+  GemmW W, W2;
+  int rc = VF_OK;
+  switch (c.kind) {
+    case VF_LAYER_CONV2D: {
+      const HostT w = host_tensor(c.w, {c.cout, c.cin, 3, 3});
+      HostT sw, sb;
+      if (c.sc_cin) { sw = host_tensor(c.sc_w, {c.cout, c.sc_cin}); sb = host_tensor(c.sc_b, {c.cout}); }
+      rc = pack_conv3x3(ctx, &W, w, c.sc_cin ? &sw : nullptr, c.sc_cin ? &sb : nullptr);
+      break;
+    }
+    case VF_LAYER_CONVT2D: rc = pack_convT2d(ctx, &W, host_tensor(c.w, {c.cin, c.cout, 3, 3})); break;
+    case VF_LAYER_CONV1D:
+      rc = pack_conv1d(ctx, &W, host_tensor(c.w, {c.cout, c.cin, c.k}), host_tensor(c.b, {c.cout}));
+      break;
+    case VF_LAYER_CONVT1D:
+      rc = pack_convT1d(ctx, &W, host_tensor(c.w, {c.cin, c.cout, 2 * c.stride}), host_tensor(c.b, {c.cout}), c.stride);
+      break;
+    case VF_LAYER_PAIR:
+      rc = pack_conv1d(ctx, &W, host_tensor(c.w, {c.cout, c.cin, 3}), host_tensor(c.b, {c.cout}));
+      if (!rc) rc = pack_conv1d(ctx, &W2, host_tensor(c.w2, {c.cout, c.cout, 3}), host_tensor(c.b2, {c.cout}));
+      break;
+    case VF_LAYER_LINEAR:
+      if (c.b_hh) {     // load_bigru: the layer's W_ih of both directions, b_ih + (b_hr, b_hz, 0)
+        const int G3 = 3 * GRU_HIDDEN;
+        HostT wi[2], bi[2], bh[2];
+        const HostT *pw[2], *pb[2], *ph[2];
+        for (int d = 0; d < 2; ++d) {
+          wi[d] = host_tensor(c.w + (size_t)d * G3 * c.cin, {G3, c.cin});
+          bi[d] = host_tensor(c.b + d * G3, {G3});
+          bh[d] = host_tensor(c.b_hh + d * G3, {G3});
+          pw[d] = &wi[d]; pb[d] = &bi[d]; ph[d] = &bh[d];
+        }
+        rc = pack_gru_ih(ctx, &W, pw, pb, ph);
+      } else {          // load_bigru / load_dnn: pack_linear, the input BatchNorm2d(1) folded as scalar_bn folds it
+        double st[2];
+        if (c.in_bn) scalar_bn_affine(c.in_bn, st);
+        rc = pack_linear(ctx, &W, host_tensor(c.w, {c.cout, c.cin}), host_tensor(c.b, {c.cout}), c.in_bn ? st : nullptr);
+      }
+      break;
+  }
+  if (rc) return rc;
+
+  const Planes X = s.in_planes(c.x, n, c.x_img_rows, c.cin);
+  const ASrc xs{X, c.x_img_rows - c.x_row0, c.x_row0};
+  const int* row_valid = s.in(c.row_valid, n);
+  const Planes OA = s.inout_planes(c.out_a, n, c.out_img_rows, c.a_ld);
+  if (b.rc) return b.rc;
+  std::vector<Op> ops;
+  if (c.kind == VF_LAYER_PAIR) {
+    Op pop;
+    pop.kind = OP_PAIR;
+    rc = pair_setup(ctx, &pop.pair, X, OA, W, W2, n, c.L, c.dilation, ar, c.pair_last != 0, c.out_row0, c.pair_slope_h,
+                    c.pair_slope_out, row_valid);
+    if (rc) return rc;
+    ops.push_back(pop);
+    c.bn = 64; c.bk = 64; c.stages = 0; c.resid_tma = 0; c.tma_out = 1;
+    int col_tiles;
+    report_launch(pop, c.sig, &c.tiles, &c.grid, &col_tiles, &c.div_fallback);
+  } else {
+    GemmEpilogue e = c.kind == VF_LAYER_CONVT2D ? epi_convt2d(rows, Wp, c.cout, c.out_img_rows, c.both ? 2 * Wp - 1 : 2 * Wp)
+                     : c.kind == VF_LAYER_CONVT1D ? epi_convt1d(c.L, c.stride, c.cout, c.out_img_rows)
+                                                  : epi_plain(rows, Wp, c.cout, c.out_img_rows);
+    e.out_row0 = c.out_row0;
+    e.row_valid = row_valid;
+    e.bias = W.bias;
+    std::vector<GemmTap> taps;     // LINEAR: linear_gemm's
+    ASrc s1{};
+    switch (c.kind) {
+      case VF_LAYER_CONV2D:
+        taps = taps3x3(Wp, c.cin);
+        if (c.sc_cin) {
+          taps.push_back(GemmTap{0, 1, 0, 0, c.sc_cin});
+          s1 = ASrc{s.in_planes(c.sc_x, n, rows, c.sc_cin), rows, 0};
+        }
+        break;
+      case VF_LAYER_CONVT2D: taps = taps_convt2d(Wp, c.cin); break;
+      case VF_LAYER_CONV1D: taps = taps1d(c.k, c.dilation, c.cin, c.centered != 0); break;
+      case VF_LAYER_CONVT1D: taps = taps_convt1d(c.cin); break;
+    }
+    if (c.resid_kind == VF_RESID_FP32) {
+      e.resid = s.in((const float*)c.resid, (size_t)n * rows * c.cout);
+      e.resid_ld = c.cout;
+    } else if (c.resid_kind == VF_RESID_PLANES || c.resid_kind == VF_RESID_AR) {
+      const Planes R = s.in_planes((const uint16_t*)c.resid, n, rows, c.cout);
+      e.resid_hi = R.p.hi; e.resid_lo = R.p.lo; e.resid_ld = c.cout;
+      if (c.resid_kind == VF_RESID_AR) e.resid_ar = ar;
+    }
+    if (c.out_raw) { e.out_raw = s.inout(c.out_raw, (size_t)n * c.out_img_rows * c.raw_ld); e.raw_ld = c.raw_ld; }
+    if (c.out_r) {
+      const Planes R = s.inout_planes(c.out_r, n, c.out_img_rows, c.r_ld);
+      e.out_r = OutPlane{R.p.hi, R.p.lo, c.r_ld, c.r_c_off};
+    }
+    if (c.out_a) {
+      set_out_a(e, OA, c.a_c_off, s.in(c.a_scale, c.cout), s.in(c.a_shift, c.cout), c.act, c.slope);
+      if (c.out_ar) e.out_ar = ar;
+    }
+    if (c.head_w) {
+      const size_t hn = (size_t)n * c.head_T * Wp;
+      e.head_w = s.in(c.head_w, 32);
+      e.head_b = c.head_b;
+      e.head_in = s.in(c.head_in, hn);
+      e.head_out = s.inout(c.head_out, hn);
+      e.head_T = c.head_T;
+      e.head_valid = s.in(c.head_valid, n);
+    }
+    if (b.rc) return b.rc;
+    if (c.kind == VF_LAYER_LINEAR) linear_gemm(b, ops, W, X, c.L, n, row_valid, e, c.terms);
+    else b.gemm(ops, W, xs, c.sc_cin ? &s1 : nullptr, taps, e, n, c.terms);
+    if (b.rc) return b.rc;
+    const Op& op = ops.back();
+    c.bn = op.bn; c.bk = op.bk;
+    if (c.impl == VF_LAYER_SIMT) {
+      c.stages = 0; c.resid_tma = 0; c.tma_out = 0;
+      c.grid = op.simt.prob.n_img * op.simt.prob.m_tiles * (op.simt.prob.N / 32);
+      c.tiles = c.grid;
+      c.div_fallback = 0;
+      c.sig[0] = 0;
+    } else {
+      c.stages = op.tc.stages; c.resid_tma = op.tc.resid_tma; c.tma_out = op.tc.prob.epi.tma_out;
+      int col_tiles;
+      report_launch(op, c.sig, &c.tiles, &c.grid, &col_tiles, &c.div_fallback);
+    }
+  }
+  return run_ops(ctx, ops, 0);
+}
+
+// Builds and runs one vf_op_case on the case's plan; each op's parameter block comes from the helper the plans use, and the
+// buffers are sized from what that helper derived.
+int run_op_case(vf_ctx* ctx, Case& s, vf_op_case& c) {
+  Builder& b = s.b;
+  Plan& plan = s.plan;
+  const int B = c.batch;
+  plan.batch = B;
+  const int last = VL_VOC + ctx->cfg.voc_num_stages - 1;
+  const int64_t packed = c.clip_off ? c.clip_off[B] : 0;            // samples of all clips when they are packed
+  int rc = VF_OK;
+  if (c.clip_off) {
+    plan.d_vl_off = b.alloc<int64_t>((size_t)B + 1);
+    plan.d_vl_rows = b.alloc<int>((size_t)VL_ROWS * B);
+    if (b.rc) return b.rc;
+    rc = write_lengths_table(ctx, &plan, c.clip_off, B, c.unet_w0, 0);
+    if (rc) return rc;
+    if (c.vl_rows) s.back(c.vl_rows, plan.d_vl_rows, (size_t)VL_ROWS * B * sizeof(int));
+  }
+  std::vector<Op> ops;
+  switch (c.kind) {
+    case VF_OP_FIRST: {
+      UnetW U;
+      ConvBlockW blk;
+      U.first_bn1_scale = c.bn1_scale; U.first_bn1_shift = c.bn1_shift;
+      U.d_first_w1 = s.in(c.w1, 32 * 9); U.d_first_wsc = s.in(c.w_sc, 32); U.d_first_bsc = s.in(c.b_sc, 32);
+      blk.bn2 = Affine{s.in(c.bn2_scale, 32), s.in(c.bn2_shift, 32)};
+      Op op = first_op(ctx, U, blk, s.in(c.x, (size_t)B * c.T * (c.W + 1)), B, c.T, c.W, PlanePtr{nullptr, nullptr}, nullptr,
+                       plan.vl(VL_T), plan.vl(VL_TP));
+      UnetFirstParams& f = op.first;
+      const int rows = f.Tp * (f.W + 1);
+      f.a2 = s.inout_planes(c.a2, B, rows, 32).p;
+      f.sc_raw = s.inout(c.sc_raw, (size_t)B * rows * 32);
+      c.Tp = f.Tp;
+      ops.push_back(op);
+      break;
+    }
+    case VF_OP_POOL: {
+      const Affine bn1{s.in(c.a_scale, c.C), s.in(c.a_shift, c.C)};
+      Op op = pool_op(ctx, s.in(c.pin, (size_t)B * c.H * (c.W + 1) * c.C), B, c.H, c.W, c.C, bn1, PlanePtr{nullptr, nullptr},
+                      PlanePtr{nullptr, nullptr}, nullptr, plan.vl(VL_UNET + c.level + 1));
+      PoolParams& p = op.pool;
+      const int rows = (p.H / 2) * p.Wpo;
+      p.out_r = s.inout_planes(c.out_r, B, rows, p.C).p;
+      p.out_a = s.inout_planes(c.out_a, B, rows, p.C).p;
+      p.out_raw = s.inout(c.out_raw, (size_t)B * rows * p.C);
+      c.Wpo = p.Wpo;
+      ops.push_back(op);
+      break;
+    }
+    case VF_OP_COND: {
+      const size_t mel_n = (size_t)B * c.T * 128;
+      Op op = cond_op(ctx, s.in(c.mel, mel_n), B, c.T, PlanePtr{nullptr, nullptr}, plan.vl(VL_T), plan.vl(VL_TV));
+      VocCondParams& p = op.cond;
+      p.is_log = c.is_log;
+      p.out = s.inout_planes(c.cond, B, p.Tv, 128).p;
+      c.Tv = p.Tv;
+      if (c.unify) {     // restore_impl: the band sums of the linear input mel and the restored log-mel, then the conditioning
+        float* sums = s.inout(c.band_sums, 2 * (size_t)B);
+        const float* target = s.in(c.mel_target, mel_n);
+        if (b.rc) return b.rc;
+        CK(unify_energy(target, p.mel, B, c.T, sums, plan.vl(VL_T), &p, 0));
+      }
+      ops.push_back(op);
+      break;
+    }
+    case VF_OP_REFLECT:
+      ops.push_back(reflect_op(s.inout_planes(c.planes, B, (int)c.L + 6, c.C).p, B, (int)c.L, c.C,
+                               c.cond_pad ? plan.vl(VL_TV) : plan.vl(last)));
+      break;
+    case VF_OP_TAIL: {
+      float* w = nullptr;
+      rc = pack_tail(ctx, &w, host_tensor(c.tail_w, {1, c.C, 7}));
+      if (rc) return rc;
+      const PlanePtr in = s.in_planes(c.tail_in, B, (int)c.L + 6, c.C).p;
+      float* wav = s.inout(c.wav, (size_t)B * c.L);
+      unsigned int* peak = s.inout(c.peak_bits, (size_t)B);
+      ops.push_back(memset_op(peak, (size_t)B * 4));
+      ops.push_back(tail_op(in, B, c.L, c.C, c.terms, w, c.tail_b, c.tanh_out, wav, peak, plan.vl(last)));
+      c.tail_smem = (int64_t)voc_tail_smem_bytes(c.C, c.terms);
+      break;
+    }
+    case VF_OP_FINALIZE: {
+      Op op;
+      op.kind = OP_FINALIZE;
+      float* o = s.inout(c.out, (size_t)(c.clip_off ? packed : (int64_t)B * c.n));
+      if (b.rc) return b.rc;
+      rc = finalize_params(ctx, &op.fin, s.in(c.in_wav, (size_t)B * c.L), s.in(c.peak_bits, (size_t)B), B, c.L, c.n, o,
+                           plan.d_vl_off, plan.vl(last));
+      if (rc) return rc;
+      c.skip = op.fin.skip;
+      ops.push_back(op);
+      break;
+    }
+    case VF_OP_ISTFT: {
+      const int64_t wav_n = c.clip_off ? packed : (int64_t)B * c.n;
+      float* frames = s.inout(c.frames, (size_t)B * c.T * 2048);
+      float* o = s.inout(c.out, (size_t)wav_n);
+      const float* mag = s.in(c.mag, (size_t)B * c.T * 1025);
+      const float* wav = s.in(c.in_wav, (size_t)wav_n);
+      if (b.rc) return b.rc;
+      IstftFramesParams fp;
+      IstftOlaParams op;
+      istft_params(ctx, &fp, &op, mag, wav, B, c.n, c.T, frames, o, plan.d_vl_off, plan.vl(VL_T));
+      CK(launch_istft_frames(fp, 0));
+      CK(launch_istft_ola(op, 0));
+      break;
+    }
+    case VF_OP_PEAK_NORM: {      // ssr_restore_varlen's VF_SSR_PEAK_NORMALISE
+      float* wav = s.inout(c.wav, (size_t)packed);
+      unsigned int* peak = s.inout(c.peak_bits, (size_t)B);
+      if (b.rc) return b.rc;
+      CK(cudaMemsetAsync(peak, 0, (size_t)B * sizeof(unsigned int), 0));
+      CK(launch_peak_normalise_varlen(wav, plan.d_vl_off, B, (long)c.n, peak, 0));
+      break;
+    }
+    case VF_OP_FRONTEND: {       // run_frontend as restore_impl, ssr_impl, ssr_restore_varlen and vf_frontend call it
+      if (!ctx->d_fb_val) return fail(ctx, VF_ESTATE, "vf_selftest_op: mel filterbank not loaded");
+      if (!c.clip_off) c.T = frames_of(ctx, (long)c.n);
+      for (int i = 0; c.clip_off && i < B; ++i) {
+        const long nb = (long)(c.clip_off[i + 1] - c.clip_off[i]);
+        if (nb <= 1024 || nb > c.n || frames_of(ctx, nb) > c.T)
+          return fail(ctx, VF_EINVAL, "vf_selftest_op: clip %d has %ld samples (need 1025 .. n, at most T = %d frames)", i, nb, c.T);
+      }
+      const size_t rows = (size_t)B * c.T;
+      float* mel = s.inout(c.mel_out, rows * 128);
+      float* logmel = s.inout(c.logmel_out, rows * 128);
+      float* sp = s.inout(c.sp_out, rows * 1025);
+      float* co = s.inout(c.cos_out, rows * 1025);
+      float* si = s.inout(c.sin_out, rows * 1025);
+      const float* wav = s.in(c.in_wav, (size_t)(c.clip_off ? packed : (int64_t)B * c.n));
+      if (b.rc) return b.rc;
+      plan.T = c.T;
+      rc = run_frontend(ctx, wav, B, (long)c.n, mel, logmel, sp, co, si, 0, c.clip_off ? &plan : nullptr);
+      if (rc) return rc;
+      break;
+    }
+    case VF_OP_PLANES: {         // the first op of build_bigru (BN0's scale and shift) and build_dnn (1, 0)
+      const float* x = s.in(c.x, (size_t)B * c.T * 128);
+      const PlanePtr o = s.inout_planes(c.planes, B, c.T, 128).p;
+      ops.push_back(planes_op(x, B, c.T, c.bn1_scale, c.bn1_shift, o, plan.vl(VL_T)));
+      break;
+    }
+  }
+  if (b.rc) return b.rc;
+  return run_ops(ctx, ops, 0);
+}
+
+}  // namespace
+
+extern "C" {
+
+VF_API int vf_selftest_layer(vf_ctx* ctx, vf_layer_case* lc) {
+  if (!ctx || !lc) return VF_EINVAL;
+  vf_layer_case& c = *lc;
+  const bool pair = c.kind == VF_LAYER_PAIR, lin = c.kind == VF_LAYER_LINEAR;
+  if (c.kind < VF_LAYER_CONV2D || c.kind > VF_LAYER_LINEAR || (c.impl != VF_LAYER_PRODUCT && c.impl != VF_LAYER_SIMT) ||
+      (c.terms != 1 && c.terms != 3) || c.n_img <= 0 || !c.x || !c.w || c.cin <= 0 || c.cout <= 0 || c.x_row0 < 0 ||
+      c.out_img_rows <= 0 || c.resid_kind < VF_RESID_NONE || c.resid_kind > VF_RESID_AR ||
+      (c.resid_kind != VF_RESID_NONE && !c.resid) || (c.sc_cin && (c.kind != VF_LAYER_CONV2D || !c.sc_w || !c.sc_b || !c.sc_x)) ||
+      ((c.kind == VF_LAYER_CONV1D || c.kind == VF_LAYER_CONVT1D || pair || lin) && !c.b) ||
+      ((c.in_bn || c.b_hh) && !lin) || (c.in_bn && c.b_hh) || (c.b_hh && c.cout != 6 * GRU_HIDDEN) ||
+      (lin && (c.L <= 0 || c.x_row0 != 0 || c.x_img_rows != c.L || c.resid_kind > VF_RESID_FP32 || c.head_w)) ||
+      ((c.kind == VF_LAYER_CONV2D || c.kind == VF_LAYER_CONVT2D) && (c.H <= 0 || c.W <= 0 || c.b)) ||
+      (c.kind == VF_LAYER_CONV1D && (c.k <= 0 || c.dilation <= 0)) || (c.kind == VF_LAYER_CONVT1D && c.stride <= 0) ||
+      (c.head_w && (!c.head_out || c.head_T <= 0)) ||
+      (pair && (!c.w2 || !c.b2 || !c.out_a || c.terms != 1 || c.resid_kind != VF_RESID_NONE || c.dilation <= 0)))
+    return fail(ctx, VF_EINVAL, "vf_selftest_layer: bad case");
+  // the SIMT kernel's epilogue (gemm.cuh: epilogue_chunk) has no (a, r) stream and there is no SIMT pair
+  if (c.impl == VF_LAYER_SIMT && (pair || c.out_ar || c.resid_kind == VF_RESID_AR))
+    return fail(ctx, VF_EINVAL, "vf_selftest_layer: the SIMT kernel has no (a, r) stream");
+  return run_case(ctx, "vf_selftest_layer", true, c.impl == VF_LAYER_SIMT, [&](Case& s) { return run_layer_case(ctx, s, c); });
+}
+
+VF_API int vf_selftest_gru(vf_ctx* ctx, vf_gru_case* gc) {
+  if (!ctx || !gc) return VF_EINVAL;
+  const vf_gru_case& c = *gc;
+  if (c.batch <= 0 || c.T <= 0 || !c.G || !c.w_hh || !c.b_hn || !c.out) return fail(ctx, VF_EINVAL, "vf_selftest_gru: bad case");
+  for (int b = 0; c.lengths && b < c.batch; ++b)
+    if (c.lengths[b] < 1 || c.lengths[b] > c.T) return fail(ctx, VF_EINVAL, "vf_selftest_gru: clip %d has %d of %d frames", b, c.lengths[b], c.T);
+  return run_case(ctx, "vf_selftest_gru", true, ctx->validate_simt, [&](Case& s) {
+    const size_t H = GRU_HIDDEN, rows = (size_t)c.batch * c.T;
+    const float* G = s.in(c.G, rows * 6 * H);
+    float* w = s.in(c.w_hh, 2 * 3 * H * H);
+    float* bhn = s.in(c.b_hn, 2 * H);
+    const int* len = s.in(c.lengths, (size_t)c.batch);
+    const PlanePtr out = s.inout_planes(c.out, c.batch, c.T, 2 * GRU_HIDDEN).p;
+    if (s.b.rc) return s.b.rc;
+    const GruDirW dirs[2] = {{w, bhn}, {w + 3 * H * H, bhn + H}};
+    std::vector<Op> ops{gru_op(G, dirs, out, c.batch, c.T, c.relu != 0, len, "gru")};
+    return run_ops(ctx, ops, 0);
+  });
+}
+
+VF_API int vf_selftest_op(vf_ctx* ctx, vf_op_case* oc) {
+  if (!ctx || !oc) return VF_EINVAL;
+  vf_op_case& c = *oc;
+  const bool bad_kind = c.kind < VF_OP_FIRST || c.kind > VF_OP_PLANES;
+  const bool bad_shape =
+      (c.kind == VF_OP_FIRST && (c.T <= 0 || c.W <= 0 || !c.x || !c.w1 || !c.bn2_scale || !c.bn2_shift || !c.w_sc || !c.b_sc)) ||
+      (c.kind == VF_OP_POOL && (c.H < 2 || c.W <= 0 || c.C <= 0 || c.C % 8 || !c.pin || !c.a_scale || !c.a_shift || c.level < 0 || c.level > 5)) ||
+      (c.kind == VF_OP_COND && (c.T <= 0 || !c.mel || !c.cond || (c.unify && (!c.mel_target || !c.band_sums)))) ||
+      (c.kind == VF_OP_REFLECT && (c.L < 4 || c.C <= 0 || c.C % 8 || !c.planes)) ||
+      (c.kind == VF_OP_TAIL && (c.L <= 0 || c.C <= 0 || c.C % 8 || (c.terms != 1 && c.terms != 3) || !c.tail_in || !c.tail_w ||
+                                !c.wav || !c.peak_bits)) ||
+      (c.kind == VF_OP_FINALIZE && (c.L <= 0 || c.n <= 0 || !c.in_wav || !c.peak_bits || !c.out)) ||
+      (c.kind == VF_OP_ISTFT && (c.T <= 0 || c.n <= 1024 || !c.mag || !c.in_wav || !c.frames || !c.out)) ||
+      (c.kind == VF_OP_PEAK_NORM && (!c.clip_off || c.n <= 0 || !c.wav || !c.peak_bits)) ||
+      (c.kind == VF_OP_FRONTEND && (c.n <= 0 || !c.in_wav || (c.clip_off && c.T <= 0) || !c.cos_out != !c.sin_out || (c.cos_out && !c.sp_out))) ||
+      (c.kind == VF_OP_PLANES && (c.T <= 0 || !c.x || !c.planes));
+  if (bad_kind || c.batch <= 0 || bad_shape || (c.clip_off && (c.batch > VL_MAX_CLIPS || c.clip_off[0] != 0)))
+    return fail(ctx, VF_EINVAL, "vf_selftest_op: bad case");
+  return run_case(ctx, "vf_selftest_op", true, ctx->validate_simt, [&](Case& s) { return run_op_case(ctx, s, c); });
+}
+
+VF_API int vf_selftest_plan_gemms(vf_ctx* ctx, int plan_kind, int batch, int frames, vf_plan_gemm* records, int cap, int* count) {
+  if (!ctx || !count || cap < 0 || (cap && !records)) return VF_EINVAL;
+  if (plan_kind < PLAN_GSR || plan_kind > PLAN_SSR_VARLEN || batch <= 0 || frames <= 0 ||
+      (is_varlen_plan(plan_kind) && batch > VL_MAX_CLIPS))
+    return fail(ctx, VF_EINVAL, "vf_selftest_plan_gemms: bad plan");
+  if (ctx->validate_simt) return fail(ctx, VF_EINVAL, "vf_selftest_plan_gemms: validate_simt plans run no tensor-core launches");
+  if (!ctx->loaded) return fail(ctx, VF_ESTATE, "weights not loaded");
+  int rc = check_networks(ctx, plan_kind);
+  if (rc) return rc;
+  return run_case(ctx, "vf_selftest_plan_gemms", false, 0, [&](Case& s) {
+    Plan& plan = s.plan;
+    plan.kind = plan_kind; plan.batch = batch; plan.T = frames;
+    const int built = build_plan(ctx, &plan);
+    int n = 0;
+    for (const std::vector<Op>* list : {&plan.unet, &plan.vocoder})
+      for (const Op& op : *list) {
+        if (built || (op.kind != OP_GEMM && op.kind != OP_PAIR)) continue;
+        if (n < cap) {
+          int div_fallback;
+          snprintf(records[n].label, sizeof records[n].label, "%s", op.label);
+          report_launch(op, records[n].sig, &records[n].tiles, &records[n].grid, &records[n].col_tiles, &div_fallback);
+        }
+        ++n;
+      }
+    *count = n;
+    return built;
+  });
+}
+
+}  // extern "C"
