@@ -21,7 +21,7 @@ D = torch.float64
 def nchw_to_rows(x):
     """[n, C, H, W] -> [n, H * (W + 1), C]: (h, w) pixels flattened with one zero pad column per image row (gemm.cuh)."""
     n, c, h, w = x.shape
-    r = torch.zeros(n, h, w + 1, c, dtype=x.dtype)
+    r = torch.zeros(n, h, w + 1, c, dtype=x.dtype, device=x.device)
     r[:, :, :w] = x.permute(0, 2, 3, 1)
     return r.reshape(n, h * (w + 1), c)
 

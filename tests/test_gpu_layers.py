@@ -451,7 +451,8 @@ def _set_outputs(b):
         b.head_out = np.full((n, T, Wp), SENT32, np.uint32)
         b.head_valid = None if c.get("head_valid") is None else np.asarray(c["head_valid"], np.int32)
         b.keep += [b.head_w, b.head_in, b.head_out, b.head_valid]
-        lc.head_w, lc.head_b, lc.head_T = _ptr(b.head_w), 0.375, T
+        b.head_b = 0.375
+        lc.head_w, lc.head_b, lc.head_T = _ptr(b.head_w), b.head_b, T
         lc.head_in, lc.head_out, lc.head_valid = _ptr(b.head_in), _ptr(b.head_out), _ptr(b.head_valid)
 
 
@@ -570,11 +571,32 @@ def run_and_check(eng, c, impl):
     if c["kind"] == PAIR:
         check_pair(b, ck)
         return ck.worst, rep
-    tol = TOL[b.terms]
-    cout = lc.cout
     wins = windows_of(b)
     y = reference(b) if wins is None else None
     M = reference(b, abs_=True) if wins is None else None
+    check_outputs(b, ck, y, M, impl)
+    return ck.worst, rep
+
+
+def check_write_set(name, what, bits, mask, sentinel, before=None):
+    """check_sentinels, or with `before` (the buffer as it was before the launch): every element outside the write set
+    still holds its old value."""
+    if before is None:
+        return check_sentinels(name, what, bits, mask, sentinel)
+    moved = (bits != before) & ~mask
+    if moved.any():
+        bad = np.argwhere(moved)
+        raise AssertionError((name, what, f"{len(bad)} elements outside the write set changed, first {bad[:4].tolist()}"))
+
+
+def check_outputs(b, ck, y, M, impl, before=None):
+    """Every output of a conv layer (b.buf): its write set, the exact zeros and every value against float64 (y, M =
+    reference(b) and reference(b, abs_=True)).  before: the output buffers as they were before the launch (the plan
+    replay, whose buffers carry no sentinels), keyed as b.buf."""
+    c, lc = b.c, b.lc
+    tol = TOL[b.terms]
+    cout = lc.cout
+    wins = windows_of(b)
     zr = zero_rows_mask(b)
 
     def views():
@@ -589,12 +611,14 @@ def run_and_check(eng, c, impl):
         ld = buf.shape[-1]
         off = b.c_off if key != "raw" else 0
         m = write_mask(b, ld, off, cout)
+        prev = None if before is None else before[key]
         if key == "raw":
-            check_sentinels(ck.name, key, buf, m, SENT32)
+            check_write_set(ck.name, key, buf, m, SENT32, prev)
         else:
-            check_sentinels(ck.name, key + ".hi", buf[0], m, SENT16)
+            check_write_set(ck.name, key + ".hi", buf[0], m, SENT16, None if prev is None else prev[0])
             lo_written = key == "r" or b.terms == 3 or lc.out_ar or impl == 1
-            check_sentinels(ck.name, key + ".lo", buf[1], m if lo_written else np.zeros_like(m), SENT16)
+            check_write_set(ck.name, key + ".lo", buf[1], m if lo_written else np.zeros_like(m), SENT16,
+                            None if prev is None else prev[1])
         del m
         for si, r0, r1, yy, mm in views():
             yy, mm = np.asarray(yy), np.asarray(mm)
@@ -622,8 +646,7 @@ def run_and_check(eng, c, impl):
                 else:
                     ck.values("a", hi, a_ref, sc * tol * mm + 2.0 ** -11 * np.abs(a_ref) + FLOOR, z)
     if c.get("head"):
-        check_head(b, ck, y, M, zr, tol)
-    return ck.worst, rep
+        check_head(b, ck, y, M, zr, tol, None if before is None else before["head"])
 
 
 def _ulp16(v):
@@ -640,7 +663,7 @@ def window_reference(b, img, r0, r1):
     return y[None].numpy(), m[None].numpy()
 
 
-def check_head(b, ck, y, M, zr, tol):
+def check_head(b, ck, y, M, zr, tol, before=None):
     c = b.c
     T, Wp = c["head_T"], c["W"] + 1
     got = _f32(b.head_out)
@@ -648,28 +671,31 @@ def check_head(b, ck, y, M, zr, tol):
     v = torch.where(torch.from_numpy(zr)[..., None], torch.zeros(()), y.clone() if torch.is_tensor(y) else torch.as_tensor(y))
     h = (v @ hw).reshape(b.n, -1, Wp)[:, :T]
     hm = (M @ hw.abs()).reshape(b.n, -1, Wp)[:, :T]
-    h[:, :, :Wp - 1] += 0.375
+    h[:, :, :Wp - 1] += b.head_b
     h[:, :, Wp - 1] = 0
-    bound = tol * (hm + 0.375)
+    bound = tol * (hm + abs(b.head_b))
     if b.head_in is not None:
         h = h + torch.from_numpy(b.head_in).double()
         bound = bound + 2.0 ** -23 * torch.from_numpy(np.abs(b.head_in)).double()
     mask = np.zeros((b.n, T, Wp), bool)
     for i in range(b.n):
         mask[i, :T if b.head_valid is None else b.head_valid[i]] = True
-    check_sentinels(ck.name, "head", b.head_out, mask, SENT32)
+    check_write_set(ck.name, "head", b.head_out, mask, SENT32, before)
     ck.values("head", np.where(mask, got, 0), np.where(mask, h.numpy(), 0), bound.numpy() + FLOOR, np.zeros(1, bool))
 
 
-def check_pair(b, ck):
+def check_pair(b, ck, before=None):
+    """The fused pair's (a, r) output planes against float64 (R.pair); before: as in check_outputs."""
     c = b.c
     L, n = c["L"], b.n
     a = b.buf["a"]
     orow0 = b.out_row0
     mask = R.write_rows_plain(n, b.out_img_rows, 64, orow0, L, 0, 64)
-    check_sentinels(ck.name, "a", a[0], mask, SENT16)
+    prev = (None, None) if before is None else before["a"]
+    check_write_set(ck.name, "a", a[0], mask, SENT16, prev[0])
     last = bool(c.get("last"))
-    check_sentinels(ck.name, "r", a[1], np.zeros_like(mask) if last else R.write_rows_plain(n, b.out_img_rows, 64, 0, L, 0, 64), SENT16)
+    check_write_set(ck.name, "r", a[1], np.zeros_like(mask) if last else R.write_rows_plain(n, b.out_img_rows, 64, 0, L, 0, 64),
+                    SENT16, prev[1])
     tol = TOL[1]
     slope_out = STAGE_SLOPE if last else RES_SLOPE
     for i in range(n):
@@ -681,7 +707,7 @@ def check_pair(b, ck):
         conv_h = R.conv1d(h.abs(), b.wb.abs(), None, 1)
         M = xs.abs() + conv_h + b.bb.abs()[None, :, None] + R.conv1d(mh, b.wb.abs(), None, 1)
         bound = tol * M + 2.0 ** -11 * conv_h
-        y, bound = R.ncl_to_rows(y)[0].numpy(), R.ncl_to_rows(bound)[0].numpy()
+        y, bound = R.ncl_to_rows(y)[0].cpu().numpy(), R.ncl_to_rows(bound)[0].cpu().numpy()
         hi = R.from_bits(a[0, i, orow0:orow0 + L])
         zero = np.zeros((L, 1), bool)
         zero[Lv:] = True

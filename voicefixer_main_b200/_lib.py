@@ -6,7 +6,7 @@ with VF_ENODEVICE.  Nothing here computes on the data path; it only marshals poi
 """
 import ctypes
 import os
-from ctypes import (POINTER, Structure, byref, c_char, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_size_t, c_uint, c_void_p)
+from ctypes import (POINTER, Structure, byref, c_char, c_char_p, c_double, c_float, c_int, c_int32, c_int64, c_size_t, c_uint, c_uint64, c_void_p)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200vf.so")
@@ -24,7 +24,7 @@ EXPORTS = [
     "vf_ssr_restore_varlen_mels", "vf_selftest_op", "vf_selftest_gru", "vf_score_time_varlen",
     "vf_sosfiltfilt_varlen", "vf_resample_poly_f64_varlen", "vf_metric_spectrogram_ex", "vf_score_varlen_ex",
     "vf_score_time_varlen_ex", "vf_restore_chunks", "vf_ssr_restore_chunks", "vf_restore_windows", "vf_ssr_restore_windows",
-    "vf_selftest_plan_gemms", "vf_resample_sinc_varlen",
+    "vf_selftest_plan_gemms", "vf_resample_sinc_varlen", "vf_selftest_plan_trace",
 ]
 VF_RESTORE_UNIFY_ENERGY = 1
 VF_SSR_PEAK_NORMALISE = 1
@@ -82,6 +82,17 @@ class VfOpCase(Structure):
 class VfPlanGemm(Structure):
     """vf_plan_gemm (include/b200vf.h): one GEMM / fused-pair launch of a plan for vf_selftest_plan_gemms (tests only)."""
     _fields_ = [("label", c_char * 48), ("sig", c_char * 160), ("tiles", c_int64), ("grid", c_int), ("col_tiles", c_int)]
+
+
+class VfTraceOp(Structure):
+    """vf_trace_op (include/b200vf.h): one launch of a plan as vf_selftest_plan_trace describes it (tests only)."""
+    _fields_ = [("list", c_int), ("index", c_int), ("kind", c_int), ("label", c_char * 48), ("layer", VfLayerCase),
+                ("op", VfOpCase), ("vl_rows", c_void_p), ("n_out", c_int), ("out_ptr", c_uint64 * 4),
+                ("out_bytes", c_uint64 * 4), ("n_allocs", c_int), ("alloc_ptr", POINTER(c_uint64)),
+                ("alloc_bytes", POINTER(c_uint64))]
+
+
+VF_TRACE_FN = ctypes.CFUNCTYPE(c_int, c_void_p, c_int, POINTER(VfTraceOp))
 
 
 class VfGruCase(Structure):
@@ -157,6 +168,7 @@ def load_library():
     lib.vf_selftest_op.argtypes = [P, POINTER(VfOpCase)]
     lib.vf_selftest_gru.argtypes = [P, POINTER(VfGruCase)]
     lib.vf_selftest_plan_gemms.argtypes = [P, c_int, c_int, c_int, POINTER(VfPlanGemm), c_int, POINTER(c_int)]
+    lib.vf_selftest_plan_trace.argtypes = [P, c_int, P, POINTER(c_int64), c_int, c_int64, c_uint, P, VF_TRACE_FN, P]
     lib.vf_enable_op_timing.argtypes = [P, c_int]
     lib.vf_op_count.argtypes = [P]
     lib.vf_op_info.argtypes = [P, c_int, POINTER(c_float), POINTER(c_double), POINTER(c_double), POINTER(c_int),

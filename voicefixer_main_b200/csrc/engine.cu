@@ -91,6 +91,7 @@ void free_plan(Plan* plan) {
   if (plan->order.ev) { cudaEventDestroy(plan->order.ev); plan->order.ev = nullptr; }
   for (void* p : plan->allocs) cudaFree(p);
   plan->allocs.clear();
+  plan->alloc_bytes.clear();
 }
 
 // The networks a plan of `kind` runs must have been loaded

@@ -80,6 +80,11 @@ struct Op {
   struct { void* p; size_t bytes; } ms;
   GruParams gru;
   AffinePlanesParams planes;
+  // OP_GEMM: its A sources (the TMA maps hold them only encoded); OP_PAIR: src[0] is the (a, r) planes it reads and pair_dst
+  // the planes it writes.  Recorded by the builder for the plan trace (selftest.cu); no launch reads them.
+  ASrc src[2] = {};
+  int n_src = 0;
+  Planes pair_dst;
 };
 
 struct ConvBlockW {
@@ -154,6 +159,7 @@ struct Plan {
   const int* vl(int row) const { return d_vl_rows ? d_vl_rows + (size_t)row * batch : nullptr; }
   long n_samples = 0;
   std::vector<void*> allocs;
+  std::vector<size_t> alloc_bytes;   // the size of each of allocs (Builder::alloc)
   size_t bytes = 0;
   std::vector<Op> unet, vocoder;
   float* d_io[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};   // [buffer][in / out]: double-buffered host staging
@@ -336,6 +342,7 @@ struct Builder {
     T* p = nullptr;
     if (rc) return nullptr;
     rc = dev_alloc(ctx, plan->allocs, plan->bytes, &p, count);
+    if (!rc) plan->alloc_bytes.push_back(std::max<size_t>(count * sizeof(T), 256));
     return p;
   }
   Planes planes(size_t n_img, int img_rows, int C);

@@ -79,6 +79,9 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
   if (rc) return;
   Op op;
   op.kind = OP_GEMM;
+  op.src[0] = s0;
+  if (s1) op.src[1] = *s1;
+  op.n_src = s1 ? 2 : 1;
   // K chunk width: 64 wherever the taps allow it.  Every chunk costs the two single-thread issue loops a fixed ~0.5 us
   // round (barrier wait, TMA / MMA operand set-up), so wide chunks win even where narrow ones would allow one more
   // co-resident CTA (measured: voc.res3.a 1.43 -> 0.96 ms)
@@ -716,6 +719,9 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
                                    (last && last_stage) ? 3 : 0, c.voc_res_slope, last ? c.voc_stage_slope : c.voc_res_slope,
                                    plan->vl(VL_VOC + s));
         if (mrc) return mrc;
+        op.src[0] = ASrc{src, (int)L, 0};
+        op.n_src = 1;
+        op.pair_dst = dst;
         op.flops = 2.0 * 2.0 * (double)B * L * cout * 3.0 * cout;
         op.exec_flops = 2.0 * 2.0 * (double)B * pp.tiles_per_img * GEMM_BM * cout * 3.0 * cout;
         op.bytes = (double)B * L * cout * (2 + 2 + (last ? 0 : 2) + 2);    // act in (operand and residual), r in, r out, act out

@@ -381,6 +381,298 @@ int run_op_case(vf_ctx* ctx, Case& s, vf_op_case& c) {
   return run_ops(ctx, ops, 0);
 }
 
+// vf_selftest_plan_trace: one launch of a plan at a time, each described in the hooks' case vocabulary and handed to the
+// caller's function before and after it runs.
+struct Tracer {
+  vf_ctx* ctx;
+  Plan& plan;
+  vf_trace_fn fn;
+  void* user;
+  std::vector<int> vl;                  // host copy of the plan's lengths table (varlen plans)
+  std::vector<uint64_t> aptr, abytes;   // the plan's buffers
+
+  const int* host_rows(const int* d) const { return d ? vl.data() + (d - plan.d_vl_rows) : nullptr; }
+  template <typename P>
+  void out(vf_trace_op* t, const P* p, size_t bytes) const {
+    if (p && t->n_out < 4) { t->out_ptr[t->n_out] = (uint64_t)(uintptr_t)p; t->out_bytes[t->n_out++] = bytes; }
+  }
+  // fp16 planes the builder allocated as [hi plane][lo plane] of n_img x rows x ld
+  int adjacent(const char* what, const __half* hi, const __half* lo, size_t plane, const char* label) const {
+    if (hi && lo != hi + plane) return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: %s: %s planes are not adjacent", label, what);
+    return VF_OK;
+  }
+
+  int describe_gemm(const Op& op, vf_trace_op* t) const {
+    const GemmProblem& pr = ctx->validate_simt ? op.simt.prob : op.tc.prob;
+    const GemmEpilogue& e = pr.epi;
+    vf_layer_case& c = t->layer;
+    const int n = pr.n_img;
+    const ASrc& s0 = op.src[0];
+    if (s0.rows != s0.pl.img_rows - s0.row0)
+      return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: %s reads %d of rows %d .. %d", op.label, s0.rows, s0.row0, s0.pl.img_rows);
+    c.impl = ctx->validate_simt ? VF_LAYER_SIMT : VF_LAYER_PRODUCT;
+    c.terms = pr.terms;
+    c.n_img = n;
+    c.cin = s0.pl.C;
+    c.cout = e.cout;
+    c.x = (const uint16_t*)s0.pl.p.hi;
+    c.x_img_rows = s0.pl.img_rows;
+    c.x_row0 = s0.row0;
+    int k = 0;
+    for (int i = 0; i < pr.ntaps; ++i) k += pr.taps[i].src == 0;
+    if (e.map == MAP_CONVT2D) {
+      c.kind = VF_LAYER_CONVT2D;
+      c.H = e.rows_in / e.Wp; c.W = e.Wp - 1;
+      c.both = e.ct_out_wp == 2 * e.Wp - 1;
+    } else if (e.map == MAP_CONVT1D) {
+      c.kind = VF_LAYER_CONVT1D;
+      c.L = e.rows_in - 1;
+      c.stride = e.ct_stride;
+    } else if (e.Wp > 0) {
+      c.kind = VF_LAYER_CONV2D;
+      c.H = e.rows_in / e.Wp; c.W = e.Wp - 1;
+      if (op.n_src == 2) { c.sc_cin = op.src[1].pl.C; c.sc_x = (const uint16_t*)op.src[1].pl.p.hi; }
+    } else {
+      c.kind = VF_LAYER_CONV1D;
+      c.L = e.rows_in;
+      c.k = k;
+      c.dilation = k > 1 ? pr.taps[1].a_off - pr.taps[0].a_off : 1;
+      c.centered = pr.taps[0].a_off < 0 || k == 1;
+    }
+    c.b = e.bias;
+    if (e.resid) {
+      c.resid_kind = VF_RESID_FP32;
+      c.resid = e.resid;
+    } else if (e.resid_hi) {
+      c.resid_kind = e.resid_ar ? VF_RESID_AR : VF_RESID_PLANES;
+      c.resid = e.resid_hi;
+      int rc = adjacent("residual", e.resid_hi, e.resid_lo, (size_t)n * e.rows_in * e.resid_ld, op.label);
+      if (rc) return rc;
+    }
+    if (e.resid_ar || e.out_ar) c.ar_slope = ctx->cfg.voc_res_slope;
+    const size_t out_elems = (size_t)n * e.out_img_rows;
+    if (e.out_raw) {
+      c.out_raw = e.out_raw; c.raw_ld = e.raw_ld;
+      out(t, e.out_raw, out_elems * e.raw_ld * 4);
+    }
+    if (e.out_r.hi) {
+      c.out_r = (uint16_t*)e.out_r.hi; c.r_ld = e.out_r.ld; c.r_c_off = e.out_r.c_off;
+      int rc = adjacent("out_r", e.out_r.hi, e.out_r.lo, out_elems * e.out_r.ld, op.label);
+      if (rc) return rc;
+      out(t, e.out_r.hi, 2 * out_elems * e.out_r.ld * 2);
+    }
+    if (e.out_a.hi) {
+      c.out_a = (uint16_t*)e.out_a.hi; c.a_ld = e.out_a.ld; c.a_c_off = e.out_a.c_off;
+      c.out_ar = e.out_ar != 0;
+      c.a_scale = e.a_scale; c.a_shift = e.a_shift;
+      c.act = e.act; c.slope = e.slope;
+      int rc = adjacent("out_a", e.out_a.hi, e.out_a.lo, out_elems * e.out_a.ld, op.label);
+      if (rc) return rc;
+      out(t, e.out_a.hi, 2 * out_elems * e.out_a.ld * 2);
+    }
+    c.out_row0 = e.out_row0;
+    c.out_img_rows = e.out_img_rows;
+    c.row_valid = host_rows(e.row_valid);
+    if (e.head_w) {
+      c.head_w = e.head_w; c.head_b = e.head_b;
+      c.head_in = e.head_in; c.head_out = e.head_out; c.head_T = e.head_T;
+      c.head_valid = host_rows(e.head_valid);
+      out(t, e.head_out, (size_t)n * e.head_T * e.Wp * 4);
+    }
+    return VF_OK;
+  }
+
+  int describe(const Op& op, int list, int index, vf_trace_op* t) const {
+    memset(t, 0, sizeof *t);
+    t->list = list; t->index = index;
+    static const char* const names[] = {"gemm", "unet_first", "pool", "voc_condition", "reflect_fill", "voc_tail", "finalize",
+                                        "memset", "pair", "gru", "affine_planes"};
+    snprintf(t->label, sizeof t->label, "%s", op.label[0] ? op.label : names[op.kind]);
+    t->vl_rows = plan.d_vl_rows ? vl.data() : nullptr;
+    t->n_allocs = (int)aptr.size();
+    t->alloc_ptr = aptr.data();
+    t->alloc_bytes = abytes.data();
+    vf_op_case& c = t->op;
+    c.batch = plan.batch;
+    if (!ctx->validate_simt) snprintf(t->layer.sig, sizeof t->layer.sig, "%s", op_signature(op).c_str());
+    switch (op.kind) {
+      case OP_GEMM: t->kind = VF_TRACE_GEMM; return describe_gemm(op, t);
+      case OP_PAIR: {
+        t->kind = VF_TRACE_PAIR;
+        const PairParams& p = op.pair;
+        const Planes& src = op.src[0].pl;
+        const Planes& dst = op.pair_dst;
+        vf_layer_case& l = t->layer;
+        l.kind = VF_LAYER_PAIR; l.impl = VF_LAYER_PRODUCT; l.terms = 1;
+        l.n_img = p.n_img; l.L = p.L; l.cin = l.cout = p.C; l.dilation = p.dil; l.k = 3;
+        l.b = p.bias_a; l.b2 = p.bias_b;
+        l.x = (const uint16_t*)src.p.hi; l.x_img_rows = src.img_rows;
+        l.out_a = (uint16_t*)dst.p.hi; l.a_ld = dst.C;
+        l.out_row0 = p.out_row0; l.out_img_rows = p.out_img_rows;
+        l.pair_slope_h = p.slope_h; l.pair_slope_out = p.slope_out; l.pair_last = p.ar_out == 0;
+        l.ar_slope = ctx->cfg.voc_res_slope;
+        l.row_valid = host_rows(p.row_valid);
+        out(t, dst.p.hi, 2 * dst.plane_stride * 2);
+        return VF_OK;
+      }
+      case OP_FIRST: {
+        t->kind = VF_TRACE_FIRST;
+        const UnetFirstParams& f = op.first;
+        c.kind = VF_OP_FIRST;
+        c.T = f.T; c.W = f.W; c.Tp = f.Tp;
+        c.bn1_scale = f.bn1_scale; c.bn1_shift = f.bn1_shift;
+        c.x = f.logmel; c.w1 = f.w1; c.bn2_scale = f.bn2_scale; c.bn2_shift = f.bn2_shift; c.w_sc = f.w_sc; c.b_sc = f.b_sc;
+        c.a2 = (uint16_t*)f.a2.hi; c.sc_raw = f.sc_raw;
+        const size_t rows = (size_t)f.batch * f.Tp * (f.W + 1);
+        int rc = adjacent("a2", f.a2.hi, f.a2.lo, rows * 32, "unet_first");
+        if (rc) return rc;
+        out(t, f.a2.hi, 2 * rows * 32 * 2);
+        out(t, f.sc_raw, rows * 32 * 4);
+        return VF_OK;
+      }
+      case OP_POOL: {
+        t->kind = VF_TRACE_POOL;
+        const PoolParams& p = op.pool;
+        c.kind = VF_OP_POOL;
+        c.H = p.H; c.W = p.Wp - 1; c.C = p.C; c.Wpo = p.Wpo;
+        const int Tp = round_up(plan.T, 64);
+        for (int l = 0; l < 6; ++l)
+          if ((Tp >> l) == p.H) c.level = l;
+        c.pin = p.in; c.a_scale = p.a_scale; c.a_shift = p.a_shift;
+        c.out_r = (uint16_t*)p.out_r.hi; c.out_a = (uint16_t*)p.out_a.hi; c.out_raw = p.out_raw;
+        const size_t elems = (size_t)p.batch * (p.H / 2) * p.Wpo * p.C;
+        int rc = adjacent("out_r", p.out_r.hi, p.out_r.lo, elems, "pool");
+        if (!rc) rc = adjacent("out_a", p.out_a.hi, p.out_a.lo, elems, "pool");
+        if (rc) return rc;
+        out(t, p.out_r.hi, 2 * elems * 2);
+        out(t, p.out_a.hi, 2 * elems * 2);
+        out(t, p.out_raw, elems * 4);
+        return VF_OK;
+      }
+      case OP_COND: {
+        t->kind = VF_TRACE_COND;
+        const VocCondParams& p = op.cond;
+        c.kind = VF_OP_COND;
+        c.T = p.T; c.Tv = p.Tv; c.is_log = p.is_log;
+        c.mel = p.mel; c.cond = (uint16_t*)p.out.hi;
+        if (p.band_sums) { c.unify = 1; c.band_sums = const_cast<float*>(p.band_sums); c.mel_target = plan.d_mel; }
+        const size_t elems = (size_t)p.batch * p.Tv * 128;
+        int rc = adjacent("cond", p.out.hi, p.out.lo, elems, "voc_condition");
+        if (rc) return rc;
+        out(t, p.out.hi, 2 * elems * 2);
+        return VF_OK;
+      }
+      case OP_REFLECT: {
+        t->kind = VF_TRACE_REFLECT;
+        c.kind = VF_OP_REFLECT;
+        c.L = op.refl.L; c.C = op.refl.C;
+        c.cond_pad = op.refl.L == voc_frames(ctx->cfg, plan.T);
+        c.planes = (uint16_t*)op.refl.pl.hi;
+        const size_t elems = (size_t)op.refl.batch * (op.refl.L + 6) * op.refl.C;
+        int rc = adjacent("reflect", op.refl.pl.hi, op.refl.pl.lo, elems, "reflect_fill");
+        if (rc) return rc;
+        out(t, op.refl.pl.hi, 2 * elems * 2);
+        return VF_OK;
+      }
+      case OP_MEMSET32:
+        t->kind = VF_TRACE_MEMSET;
+        c.planes = (uint16_t*)op.ms.p; c.n = (int64_t)op.ms.bytes;
+        out(t, (const char*)op.ms.p, op.ms.bytes);
+        return VF_OK;
+      case OP_TAIL: {
+        t->kind = VF_TRACE_TAIL;
+        const VocTailParams& p = op.tail;
+        c.kind = VF_OP_TAIL;
+        c.L = p.L; c.C = p.C; c.terms = p.terms; c.tanh_out = p.tanh_out;
+        c.tail_in = (const uint16_t*)p.in.hi; c.tail_w = p.w; c.tail_b = p.bias;
+        c.wav = p.wav; c.peak_bits = p.peak_bits;
+        c.tail_smem = (int64_t)voc_tail_smem_bytes(p.C, p.terms);
+        int rc = adjacent("tail_in", p.in.hi, p.in.lo, (size_t)p.batch * (p.L + 6) * p.C, "voc_tail");
+        if (rc) return rc;
+        out(t, p.wav, (size_t)p.batch * p.L * 4);
+        out(t, p.peak_bits, (size_t)p.batch * 4);
+        return VF_OK;
+      }
+      case OP_FINALIZE: {
+        t->kind = VF_TRACE_FINALIZE;
+        const FinalizeParams& f = op.fin;
+        c.kind = VF_OP_FINALIZE;
+        c.L = f.L; c.n = f.n; c.skip = f.skip;
+        c.in_wav = f.wav; c.peak_bits = (uint32_t*)f.peak_bits; c.out = f.out;
+        int64_t samples = 0;
+        if (f.vl_off) CK(cudaMemcpy(&samples, f.vl_off + f.batch, sizeof samples, cudaMemcpyDeviceToHost));
+        else samples = (int64_t)f.batch * f.n;
+        out(t, f.out, (size_t)samples * 4);
+        return VF_OK;
+      }
+      default: return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: op kind %d is not traced", (int)op.kind);
+    }
+  }
+
+  // Describes `op`, hands it to fn, runs it alone, hands it to fn again
+  int step(const Op& op, int list, int index) {
+    vf_trace_op t;
+    int rc = describe(op, list, index, &t);
+    if (rc) return rc;
+    CK(cudaDeviceSynchronize());
+    if (fn(user, 0, &t)) return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: stopped before %s", t.label);
+    std::vector<Op> one{op};
+    rc = run_ops(ctx, one, 0);
+    if (rc) return rc;
+    CK(cudaDeviceSynchronize());
+    if (fn(user, 1, &t)) return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: stopped after %s", t.label);
+    return VF_OK;
+  }
+};
+
+// The restore of vf_selftest_plan_trace on the case's plan, step for step as restore_impl and ssr_impl run it
+int run_trace(vf_ctx* ctx, Case& s, int kind, const float* wav, const int64_t* off, int batch, int64_t n, int T, unsigned flags,
+              float* wav_out, vf_trace_fn fn, void* user) {
+  Plan& plan = s.plan;
+  plan.kind = kind; plan.batch = batch; plan.T = T;
+  int rc = build_plan(ctx, &plan);
+  if (rc) return rc;
+  const bool ssr = is_ssr_plan(kind);
+  Tracer tr{ctx, plan, fn, user, {}, {}, {}};
+  for (size_t i = 0; i < plan.allocs.size(); ++i) {
+    tr.aptr.push_back((uint64_t)(uintptr_t)plan.allocs[i]);
+    tr.abytes.push_back(plan.alloc_bytes[i]);
+  }
+  if (off && (rc = write_lengths_table(ctx, &plan, off, batch, ssr ? 1024 : 127, 0))) return rc;
+  rc = run_frontend(ctx, wav, batch, (long)n, ssr ? nullptr : plan.d_mel, ssr ? nullptr : plan.d_logmel_in, ssr ? plan.d_sp : nullptr,
+                    nullptr, nullptr, 0, off ? &plan : nullptr);
+  if (rc) return rc;
+  CK(cudaDeviceSynchronize());
+  if (off) {
+    tr.vl.resize((size_t)VL_ROWS * batch);
+    CK(cudaMemcpy(tr.vl.data(), plan.d_vl_rows, tr.vl.size() * sizeof(int), cudaMemcpyDeviceToHost));
+  }
+  if (ssr) plan.unet[0].first.logmel = plan.d_sp;
+  for (size_t i = 0; i < plan.unet.size(); ++i)
+    if ((rc = tr.step(plan.unet[i], 0, (int)i))) return rc;
+  if (ssr) {
+    IstftFramesParams fp;
+    IstftOlaParams op;
+    istft_params(ctx, &fp, &op, plan.d_mag, wav, batch, (long)n, T, plan.d_frames, wav_out, plan.d_vl_off, plan.vl(VL_T));
+    CK(launch_istft_frames(fp, 0));
+    CK(launch_istft_ola(op, 0));
+    return VF_OK;
+  }
+  Op& cop = plan.vocoder[plan.cond_op];
+  cop.cond.mel = plan.d_logmel_out;
+  cop.cond.is_log = 1;
+  cop.cond.band_sums = nullptr;
+  if (flags & VF_RESTORE_UNIFY_ENERGY)
+    CK(unify_energy(plan.d_mel, plan.d_logmel_out, batch, T, plan.d_band, plan.vl(VL_T), &cop.cond, 0));
+  for (size_t i = 0; i < plan.vocoder.size(); ++i)
+    if ((rc = tr.step(plan.vocoder[i], 1, (int)i))) return rc;
+  Op fop;
+  fop.kind = OP_FINALIZE;
+  rc = finalize_params(ctx, &fop.fin, plan.d_voc_wav, plan.d_peak, batch, plan.L, (long)n, wav_out, off ? plan.d_vl_off : nullptr,
+                       off ? plan.vl(VL_VOC + ctx->cfg.voc_num_stages - 1) : nullptr);
+  return rc ? rc : tr.step(fop, 2, 0);
+}
+
 }  // namespace
 
 extern "C" {
@@ -474,6 +766,29 @@ VF_API int vf_selftest_plan_gemms(vf_ctx* ctx, int plan_kind, int batch, int fra
       }
     *count = n;
     return built;
+  });
+}
+
+VF_API int vf_selftest_plan_trace(vf_ctx* ctx, int plan_kind, const float* wav, const int64_t* offsets, int batch, int64_t n,
+                                  unsigned flags, float* wav_out, vf_trace_fn fn, void* user) {
+  if (!ctx || !wav || !wav_out || !fn || batch <= 0) return VF_EINVAL;
+  if (plan_kind < PLAN_GSR || plan_kind > PLAN_SSR_VARLEN || is_varlen_plan(plan_kind) != (offsets != nullptr) ||
+      (flags & ~(unsigned)VF_RESTORE_UNIFY_ENERGY) || (flags && is_ssr_plan(plan_kind)) ||
+      (offsets && (batch > VL_MAX_CLIPS || offsets[0] != 0)))
+    return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: bad call");
+  if (!ctx->loaded) return fail(ctx, VF_ESTATE, "weights not loaded");
+  int rc = check_networks(ctx, plan_kind);
+  if (rc) return rc;
+  if (offsets) {
+    n = 0;
+    for (int i = 0; i < batch; ++i) n = std::max<int64_t>(n, offsets[i + 1] - offsets[i]);
+    for (int i = 0; i < batch; ++i)
+      if (offsets[i + 1] - offsets[i] <= 1024) return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: clip %d has 1024 samples or fewer", i);
+  }
+  if (n <= 1024) return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: clips of 1024 samples or fewer");
+  const int T = offsets ? round_up(frames_of(ctx, (long)n), 64) : frames_of(ctx, (long)n);
+  return run_case(ctx, "vf_selftest_plan_trace", true, ctx->validate_simt, [&](Case& s) {
+    return run_trace(ctx, s, plan_kind, wav, offsets, batch, n, T, flags, wav_out, fn, user);
   });
 }
 

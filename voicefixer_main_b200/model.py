@@ -677,6 +677,37 @@ class Engine:
             return [(r.label.decode(), r.sig.decode(), r.tiles, r.grid, r.col_tiles) for r in recs[:n.value]]
         return [(r.label.decode(), r.sig.decode()) for r in recs[:n.value]]
 
+    def selftest_plan_trace(self, plan_kind: int, wav: torch.Tensor, lengths=None, on_op=None, unify_energy: bool = False):
+        """One restore on a fresh plan of plan_kind (0 GSR, 1 SSR: wav [B, n]; 2 GSR varlen, 3 SSR varlen: wav packed,
+        lengths per clip), one launch at a time: on_op(after, op) runs before (after = False) and after (True) each launch
+        with its L.VfTraceOp (vf_selftest_plan_trace; tests only).  An exception in on_op stops the run and is raised here.
+        Returns the restored output, shaped as the matching restore call returns it."""
+        wav = _check_in(wav, self.device, "wav")
+        out = torch.empty_like(wav)
+        caught = []
+
+        def cb(_user, after, op):
+            try:
+                on_op(bool(after), op.contents)
+                return 0
+            except BaseException as e:          # noqa: BLE001 - handed back to the caller below
+                caught.append(e)
+                return 1
+
+        fn = L.VF_TRACE_FN(cb)
+        if lengths is not None:
+            batch, n, offp = len(lengths), 0, _offsets(lengths)
+        else:
+            batch, n, offp = wav.shape[0], wav.shape[1], None
+        flags = L.VF_RESTORE_UNIFY_ENERGY if unify_energy else 0
+        with torch.cuda.device(self.device):
+            torch.cuda.synchronize()            # the hook runs on the legacy default stream
+            rc = self.lib.vf_selftest_plan_trace(self.ctx, plan_kind, _ptr(wav), offp, batch, n, flags, _ptr(out), fn, None)
+        if caught:
+            raise caught[0]
+        self._ck(rc)
+        return out
+
 
 # --------------------------------------------------------------------------------------------------------------
 class FDomainHelper:
