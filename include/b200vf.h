@@ -12,6 +12,10 @@
  *   vf_unet_mel                   VoiceFixer.forward models/gsr_voicefixer.py:183-193 -> Generator.forward :86-91
  *                                 -> UNetResComplex_100Mb.forward models/components/unet.py:60-103
  *   vf_vocoder                    model.vocoder(mel) eval_gsr_voicefixer.py:66 (third-party voicefixer.Vocoder)
+ *   vf_vocoder_varlen             the stand-alone vocoder (pip voicefixer's Vocoder.forward) on mels of different lengths
+ *                                 in one call; needs only the vocoder's weights and mel.fb
+ *   vf_resynth / vf_resynth_varlen  vocoder resynthesis: handler()'s segment step without the analysis module,
+ *                                 pre -> vocoder on the linear mel -> peak normalise -> trim_center (vocoder weights only)
  *   vf_restore / vf_restore_host  one iteration of the segment loop of handler(), eval_gsr_voicefixer.py:49-74:
  *                                 pre -> model -> from_log -> vocoder -> peak normalise -> trim_center
  *   vf_restore_varlen             the same for clips of different lengths in one call (handler() run over a test set)
@@ -148,6 +152,23 @@ VF_API int vf_unet_mel(vf_ctx* ctx, const float* mel_lin, int batch, int frames,
 /* mel_lin [B,T,128] -> wav_out [B,L], L = vf_vocoder_out_len(ctx, T). */
 VF_API int vf_vocoder(vf_ctx* ctx, const float* mel_lin, int batch, int frames, float* wav_out, void* stream);
 VF_API int64_t vf_vocoder_out_len(vf_ctx* ctx, int frames);
+/* The vocoder on linear mels of different lengths in one call, on a context that holds the vocoder's weights ("vocoder.*"
+ * and "mel.fb"; an analysis module may be loaded or not).  mel: packed device buffer [sum T_i, 128], clip i = rows
+ * frame_offsets[i] .. frame_offsets[i+1]; frame_offsets: HOST array of batch + 1 increasing int64, frame_offsets[0] = 0
+ * (read during the call only).  wav_out (device) receives each clip's full vocoder output, L_i = vf_vocoder_out_len(ctx,
+ * T_i) samples at sum_{j<i} L_j: no peak normalise and no trim, as vf_vocoder.  Clip i is bit-identical to vf_vocoder on
+ * that clip alone (batch 1, same options).  A clip may have any T_i >= 1 up to 2^30 / hop + 1 frames; an empty or
+ * decreasing range fails with VF_EINVAL and a context without the vocoder with VF_ESTATE, before any work is queued.
+ * Sub-batches, plans per (batch, bucket) and their CUDA graphs as vf_restore_varlen; the plans hold the vocoder's
+ * buffers only.  Each sub-batch adds one scatter of its mels into the plan and one pack of its outputs on `stream`. */
+VF_API int vf_vocoder_varlen(vf_ctx* ctx, const float* mel, const int64_t* frame_offsets, int batch, float* wav_out, void* stream);
+/* Vocoder resynthesis, wav [B,N] -> wav_out [B,N]: vf_frontend's linear mel -> the vocoder -> peak normalise ->
+ * trim_center, needing only the vocoder's weights.  Bit-identical to vf_frontend -> vf_vocoder -> vf_finalize.  Length
+ * rules as vf_restore_ex. */
+VF_API int vf_resynth(vf_ctx* ctx, const float* wav, int batch, int64_t n_samples, float* wav_out, void* stream);
+/* vf_resynth for clips of different lengths, packed with HOST offsets as vf_restore_varlen (no flags).  Clip i is
+ * bit-identical to vf_resynth on that clip alone (batch 1). */
+VF_API int vf_resynth_varlen(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out, void* stream);
 
 /* Fused stages A -> B -> C + peak normalise + centre trim: wav [B,N] -> wav_out [B,N] (device pointers). */
 VF_API int vf_restore(vf_ctx* ctx, const float* wav, int batch, int64_t n_samples, float* wav_out, void* stream);
@@ -540,7 +561,8 @@ typedef struct vf_layer_case {
 } vf_layer_case;
 VF_API int vf_selftest_layer(vf_ctx* ctx, vf_layer_case* lc);
 
-/* TEST ONLY.  Builds a plan of `plan_kind` (0 GSR, 1 SSR, 2 GSR varlen, 3 SSR varlen) for (batch, frames) with the loaded
+/* TEST ONLY.  Builds a plan of `plan_kind` (0 GSR, 1 SSR, 2 GSR varlen, 3 SSR varlen, 4 vocoder-only, 5 vocoder-only
+ * varlen) for (batch, frames) with the loaded
  * weights and the context's options, launches nothing, and reports each GEMM and fused-pair launch: its label, the
  * configuration signature vf_selftest_layer reports for a layer, and the size of its persistent tile loop (tiles and grid,
  * as vf_selftest_layer reports them, and the column tiles among which a CTA's consecutive tiles move).  Records past `cap`
@@ -553,6 +575,9 @@ typedef struct vf_plan_gemm {
   int col_tiles;            /* column (N) tiles per row block: tiles of a CTA change column block unless it divides grid */
 } vf_plan_gemm;
 VF_API int vf_selftest_plan_gemms(vf_ctx* ctx, int plan_kind, int batch, int frames, vf_plan_gemm* records, int cap, int* count);
+/* TEST ONLY.  The sub-batch a call of `batch` clips on plans of `plan_kind` (as vf_selftest_plan_gemms) with `frames` frames
+ * would run in under the plan budget, as the context stands (cached plans refine the per-frame size); builds nothing. */
+VF_API int vf_selftest_sub_batch(vf_ctx* ctx, int plan_kind, int batch, int frames);
 
 /* TEST ONLY.  One non-GEMM op of the launch chains, set up by the same helpers the plan builders and restore paths use and
  * launched as they launch it (run_ops or the same launch_* call), then copied back.  Synchronous; every pointer is a host
@@ -652,7 +677,8 @@ typedef struct vf_gru_case {
 } vf_gru_case;
 VF_API int vf_selftest_gru(vf_ctx* ctx, vf_gru_case* gc);
 
-/* TEST ONLY.  One restore on a plan of `plan_kind` (0 GSR, 1 SSR, 2 GSR varlen, 3 SSR varlen) built for this call with the
+/* TEST ONLY.  One restore on a plan of `plan_kind` (0 GSR, 1 SSR, 2 GSR varlen, 3 SSR varlen, 4 / 5 vocoder-only as
+ * vf_resynth / vf_resynth_varlen) built for this call with the
  * loaded weights and the context's options, run as the restore entry points run it (front end, lengths table, the UNet's
  * launches, the band sums of VF_RESTORE_UNIFY_ENERGY, the vocoder's, then the finalize or the ISTFT) but eagerly, one
  * launch at a time, synchronising around each launch of the UNet and vocoder lists and around the finalize.  wav and

@@ -24,7 +24,8 @@ EXPORTS = [
     "vf_ssr_restore_varlen_mels", "vf_selftest_op", "vf_selftest_gru", "vf_score_time_varlen",
     "vf_sosfiltfilt_varlen", "vf_resample_poly_f64_varlen", "vf_metric_spectrogram_ex", "vf_score_varlen_ex",
     "vf_score_time_varlen_ex", "vf_restore_chunks", "vf_ssr_restore_chunks", "vf_restore_windows", "vf_ssr_restore_windows",
-    "vf_selftest_plan_gemms", "vf_resample_sinc_varlen", "vf_selftest_plan_trace",
+    "vf_selftest_plan_gemms", "vf_resample_sinc_varlen", "vf_selftest_plan_trace", "vf_vocoder_varlen", "vf_resynth",
+    "vf_resynth_varlen", "vf_selftest_sub_batch",
 ]
 VF_RESTORE_UNIFY_ENERGY = 1
 VF_SSR_PEAK_NORMALISE = 1
@@ -151,6 +152,10 @@ def load_library():
     lib.vf_vocoder.argtypes = [P, P, c_int, c_int, P, P]
     lib.vf_vocoder_out_len.argtypes = [P, c_int]
     lib.vf_vocoder_out_len.restype = c_int64
+    lib.vf_vocoder_varlen.argtypes = [P, P, POINTER(c_int64), c_int, P, P]
+    lib.vf_resynth.argtypes = [P, P, c_int, c_int64, P, P]
+    lib.vf_resynth_varlen.argtypes = [P, P, POINTER(c_int64), c_int, P, P]
+    lib.vf_selftest_sub_batch.argtypes = [P, c_int, c_int, c_int]
     lib.vf_restore.argtypes = [P, P, c_int, c_int64, P, P]
     lib.vf_restore_host.argtypes = [P, P, c_int, c_int64, P, P]
     lib.vf_restore_stages.argtypes = [P, c_int, c_int64, P, P, P]

@@ -459,6 +459,21 @@ cudaError_t launch_gather_mels(const MelGatherParams& p, cudaStream_t stream) {
   return cudaGetLastError();
 }
 
+// One thread per value of clip b (blockIdx.y); blocks past its values return.
+__global__ void clip_copy_kernel(const __grid_constant__ ClipCopyParams p) {
+  const int b = blockIdx.y;
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= p.off[b + 1] - p.off[b]) return;
+  const int64_t packed = p.off[b] + i, plan = (int64_t)b * p.stride + i;
+  p.dst[p.to_packed ? packed : plan] = p.src[p.to_packed ? plan : packed];
+}
+cudaError_t launch_clip_copy(const ClipCopyParams& p, cudaStream_t stream) {
+  int64_t most = 0;
+  for (int b = 0; b < p.batch; ++b) most = std::max<int64_t>(most, p.off[b + 1] - p.off[b]);
+  clip_copy_kernel<<<dim3((unsigned)((most + 255) / 256), p.batch), 256, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
 // Segmented peak normalise (kernels.cuh): clip b = wav[off[b] .. off[b + 1]).  The max is order-free and the scale divides as
 // finalize_kernel does, so each clip gets the bits of a one-clip vf_finalize(len = n, n = n).
 __global__ void __launch_bounds__(256) peak_varlen_kernel(const float* __restrict__ wav, const int64_t* __restrict__ off,

@@ -96,6 +96,8 @@ void free_plan(Plan* plan) {
 
 // The networks a plan of `kind` runs must have been loaded
 int check_networks(vf_ctx* ctx, int kind) {
+  if (is_voc_plan(kind))     // the vocoder alone: whatever analysis module there is, or none
+    return ctx->voc_loaded ? VF_OK : fail(ctx, VF_ESTATE, "this entry point needs the vocoder (vocoder.*) weights");
   if (!is_ssr_plan(kind) && !(ctx->analysis != ANALYSIS_NONE && ctx->voc_loaded))
     return fail(ctx, VF_ESTATE, "this entry point needs the analysis module (generator.analysis_module.*) and the vocoder (vocoder.*) weights");
   if (is_ssr_plan(kind) && !ctx->ssr.loaded)
@@ -190,12 +192,14 @@ bool init_plan_budget(vf_ctx* ctx) {
   return true;
 }
 
-// The cached plan that size estimates for `kind` scale from (bytes scale with batch * padded frames), or null.  An SSR varlen
-// plan without a cached plan of its kind scales from an SSR plan: the same network and buffers per padded frame.
+// The cached plan that size estimates for `kind` scale from (bytes scale with batch * padded frames), or null.  An SSR or
+// vocoder-only varlen plan without a cached plan of its kind scales from a fixed-shape plan of its network: the same
+// buffers per padded frame.
 const Plan* size_reference(vf_ctx* ctx, int kind) {
   for (auto& kv : ctx->plans)
     if (std::get<0>(kv.first) == kind) return kv.second.get();
   if (kind == PLAN_SSR_VARLEN) return size_reference(ctx, PLAN_SSR);
+  if (kind == PLAN_VOC_VARLEN) return size_reference(ctx, PLAN_VOC);
   return nullptr;
 }
 
@@ -257,14 +261,21 @@ int get_plan(vf_ctx* ctx, int kind, int batch, int frames, Plan** out) {
   return evict_plans(ctx, 0, raw);
 }
 
+}  // namespace
+
+namespace vf {
+
 // A batch whose plan would not fit the plan budget is processed in sub-batches through one smaller plan (rows are
 // independent, so the result does not change): SSR at 64 x 10 s (143 GB) or a long file's stack of windows then run in two
 // or more passes instead of failing with an out-of-memory plan.  Workspace scales with batch x padded frames; the per-frame
-// figure is taken from a cached plan of the same path when there is one, else from the measured sizes (DESIGN.md 5).
+// figure is taken from a cached plan of the same path when there is one, else from the measured sizes (DESIGN.md 5).  A
+// vocoder-only plan holds the vocoder's buffers only: its figure depends on the vocoder mode (the 3-term mode keeps the
+// residual stream in separate planes and runs no fused pairs).
 int choose_sub_batch(vf_ctx* ctx, int kind, int batch, int frames) {
   init_plan_budget(ctx);
   const double tp = (frames + 63) / 64 * 64;
-  double per_frame = is_ssr_plan(kind) ? 2.4e6 : 1.7e6;     // bytes per clip and padded frame (measured 2.19e6 / 1.52e6) + margin
+  // bytes per clip and padded frame (measured 2.19e6 / 1.52e6; vocoder-only 0.63e6 / 1.14e6 at 1 / 3 terms) + margin
+  double per_frame = is_ssr_plan(kind) ? 2.4e6 : !is_voc_plan(kind) ? 1.7e6 : ctx->voc_terms == 3 ? 1.25e6 : 0.7e6;
   if (const Plan* ref = size_reference(ctx, kind))
     per_frame = 1.05 * (double)ref->bytes / ((double)ref->batch * ((ref->T + 63) / 64 * 64));
   const double fit = (double)ctx->plan_budget / (per_frame * tp);
@@ -274,6 +285,10 @@ int choose_sub_batch(vf_ctx* ctx, int kind, int batch, int frames) {
     if (batch % d == 0) return d;
   return cb;
 }
+
+}  // namespace vf
+
+namespace {
 
 // staging buffers for the host-pointer entry point, grown on demand
 int ensure_io(vf_ctx* ctx, Plan* plan, long n) {
@@ -411,6 +426,23 @@ int run_restore(vf_ctx* ctx, Plan* plan, int w0, int batch, const int64_t* off, 
   });
 }
 
+// eval_gsr_voicefixer.py:68-72: peak normalise + trim_center of the plan's vocoder output into wav_out (off: packed as
+// restore_impl's input)
+int finalize_on(vf_ctx* ctx, Plan* plan, int batch, int64_t n, float* wav_out, const int64_t* off, cudaStream_t st) {
+  FinalizeParams f;
+  const int rc = finalize_params(ctx, &f, plan->d_voc_wav, plan->d_peak, batch, plan->L, (long)n, wav_out,
+                                 off ? plan->d_vl_off : nullptr, off ? plan->vl(VL_VOC + ctx->cfg.voc_num_stages - 1) : nullptr);
+  if (rc) return rc;
+  CK(launch_finalize(f, st));
+  ctx->launches++;
+  return VF_OK;
+}
+
+// The launch list of a vocoder-only plan, from its d_mel to d_voc_wav and d_peak: fixed pointers, replayed as a graph
+int run_vocoder_chain(vf_ctx* ctx, Plan* plan, cudaStream_t st) {
+  return run_chain(ctx, plan, 0, st, (int64_t)plan->vocoder.size(), [&](cudaStream_t s) { return run_ops(ctx, plan->vocoder, s); });
+}
+
 // VoiceFixer's chain (run_restore's stages 1 to 3).  off == nullptr: `batch` clips of n samples (PLAN_GSR).  Otherwise
 // clips of different lengths (vf_restore_varlen): clip i = wav[off[i] .. off[i + 1]), n = the longest clip, `plan` the
 // PLAN_VARLEN plan for the bucket of its frames; the output is packed like the input.
@@ -439,14 +471,20 @@ int restore_impl(vf_ctx* ctx, Plan* plan, const float* wav, int batch, int64_t n
   rc = run_chain(ctx, plan, unify ? 1 : 0, st, (int64_t)plan->unet.size() + (int64_t)plan->vocoder.size() + (unify ? 1 : 0), chain);
   if (rc) return rc;
   rc = stage_mark(ctx, 3, st); if (rc) return rc;
-  // eval_gsr_voicefixer.py:68-72: peak normalise + trim_center
-  FinalizeParams f;
-  rc = finalize_params(ctx, &f, plan->d_voc_wav, plan->d_peak, batch, plan->L, (long)n, wav_out, off ? plan->d_vl_off : nullptr,
-                       off ? plan->vl(VL_VOC + ctx->cfg.voc_num_stages - 1) : nullptr);
+  return finalize_on(ctx, plan, batch, n, wav_out, off, st);
+}
+
+// The vocoder-only chain (vf_resynth, vf_resynth_varlen): restore_impl without the analysis module and without unify_energy.
+// The front end's linear mel d_mel conditions the vocoder directly (the plan's conditioning op reads it with is_log 0).
+int resynth_impl(vf_ctx* ctx, Plan* plan, const float* wav, int batch, int64_t n, float* wav_out, unsigned, cudaStream_t st,
+                 const int64_t* off) {
+  int rc = run_frontend(ctx, wav, batch, (long)n, plan->d_mel, nullptr, nullptr, nullptr, nullptr, st, off ? plan : nullptr);
   if (rc) return rc;
-  CK(launch_finalize(f, st));
-  ctx->launches++;
-  return VF_OK;
+  rc = stage_mark(ctx, 1, st);
+  if (!rc) rc = stage_mark(ctx, 2, st);
+  if (!rc) rc = run_vocoder_chain(ctx, plan, st);
+  if (!rc) rc = stage_mark(ctx, 3, st);
+  return rc ? rc : finalize_on(ctx, plan, batch, n, wav_out, off, st);
 }
 
 // The SSR / GSR-UNet chain: `batch` clips of n samples, magnitudes from the clips themselves (sp == nullptr) or sp.  off:
@@ -492,6 +530,9 @@ const Family VOICEFIXER{PLAN_GSR, PLAN_VARLEN, VF_RESTORE_UNIFY_ENERGY, true, 12
 const Family SSR_UNET{PLAN_SSR, PLAN_SSR_VARLEN, VF_SSR_PEAK_NORMALISE, false, 1024,
                       [](vf_ctx* ctx, Plan* plan, const float* wav, int batch, int64_t n, float* out, unsigned, cudaStream_t st,
                          const int64_t* off) { return ssr_impl(ctx, plan, nullptr, wav, batch, n, out, st, off); }};
+// Vocoder resynthesis: handler()'s segment step without the analysis module (w0 only fills the lengths table's UNet rows,
+// which no vocoder launch reads)
+const Family RESYNTH{PLAN_VOC, PLAN_VOC_VARLEN, 0, true, 127, resynth_impl};
 
 // run_restore of family f's chain
 template <typename Post = int (*)()>
@@ -625,6 +666,59 @@ int restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t*
                        if (!mel_out && !log_mel_out) return VF_OK;
                        return gather_mels(ctx, plan, frame_off, s, b, plan->d_mel, plan->d_logmel_out, mel_out, log_mel_out, st);
                      });
+}
+
+// vf_vocoder_varlen: every check before anything is queued, then per sub-batch of at most VL_MAX_CLIPS clips under the plan
+// budget, on the PLAN_VOC_VARLEN plan of the bucket of its longest clip, inside one use of it: the lengths table, one
+// scatter of the clips' mels into d_mel, the vocoder chain and one pack of each clip's L_i = vf_vocoder_out_len(T_i)
+// samples into wav_out at sum_{j<i} L_j.  The lengths table is written from sample offsets of clips of (T_i - 1) * hop
+// samples, which have T_i frames.
+int vocoder_varlen(vf_ctx* ctx, const float* mel, const int64_t* frame_offsets, int batch, float* wav_out, cudaStream_t st) {
+  const char* fn = "vf_vocoder_varlen";
+  int rc = check_ready(ctx);
+  if (rc) return rc;
+  if (!mel || !wav_out || !frame_offsets || batch <= 0) return fail(ctx, VF_EINVAL, "%s: bad arguments", fn);
+  if (frame_offsets[0] != 0) return fail(ctx, VF_EINVAL, "%s: frame_offsets[0] must be 0 (got %ld)", fn, (long)frame_offsets[0]);
+  rc = check_networks(ctx, PLAN_VOC_VARLEN);
+  if (rc) return rc;
+  const int hop = ctx->cfg.hop;
+  const int64_t max_frames = ((int64_t)1 << 30) / hop + 1;     // the packed restores' 2^30 samples
+  std::vector<int64_t> wav_off(batch + 1, 0);
+  for (int i = 0; i < batch; ++i) {
+    const int64_t T = frame_offsets[i + 1] - frame_offsets[i];
+    if (T <= 0)
+      return fail(ctx, VF_EINVAL, "%s: frame offsets must increase (clip %d: %ld -> %ld)", fn, i, (long)frame_offsets[i],
+                  (long)frame_offsets[i + 1]);
+    if (T > max_frames) return fail(ctx, VF_EINVAL, "%s: clip %d: %ld frames is too long for one call (at most %ld)", fn, i, (long)T, (long)max_frames);
+    wav_off[i + 1] = wav_off[i] + vf_vocoder_out_len(ctx, (int)T);
+  }
+  auto bucket = [&](int s, int b) {
+    int64_t t_max = 0;
+    for (int i = s; i < s + b; ++i) t_max = std::max(t_max, frame_offsets[i + 1] - frame_offsets[i]);
+    return round_up((int)t_max, 64);
+  };
+  return run_sub_batches(ctx, PLAN_VOC_VARLEN, batch, bucket, [&](Plan* plan, int s, int b) {
+    int64_t rel[VL_MAX_CLIPS + 1];
+    for (int i = 0; i <= b; ++i) rel[i] = (frame_offsets[s + i] - frame_offsets[s] - i) * hop;
+    return run_restore(ctx, plan, RESYNTH.w0, b, rel, st, [&]() -> int {
+      ClipCopyParams c;
+      memset(&c, 0, sizeof c);
+      c.src = mel + frame_offsets[s] * 128; c.dst = plan->d_mel; c.batch = b; c.to_packed = 0; c.stride = (int64_t)plan->T * 128;
+      for (int i = 0; i <= b; ++i) c.off[i] = (frame_offsets[s + i] - frame_offsets[s]) * 128;
+      CK(launch_clip_copy(c, st));
+      ctx->launches++;
+      int r = stage_mark(ctx, 1, st);
+      if (!r) r = stage_mark(ctx, 2, st);
+      if (!r) r = run_vocoder_chain(ctx, plan, st);
+      if (!r) r = stage_mark(ctx, 3, st);
+      if (r) return r;
+      c.src = plan->d_voc_wav; c.dst = wav_out + wav_off[s]; c.to_packed = 1; c.stride = plan->L;
+      for (int i = 0; i <= b; ++i) c.off[i] = wav_off[s + i] - wav_off[s];
+      CK(launch_clip_copy(c, st));
+      ctx->launches++;
+      return VF_OK;
+    });
+  }, VL_MAX_CLIPS);
 }
 
 // One row of a streaming call: `length` samples of stream `stream` from position `start` on; positions below 0 (a window's
@@ -1057,6 +1151,21 @@ VF_API int vf_vocoder(vf_ctx* ctx, const float* mel_lin, int batch, int frames, 
     CK(cudaMemcpyAsync(wav_out, plan->d_voc_wav, (size_t)batch * plan->L * 4, cudaMemcpyDeviceToDevice, st));
     return VF_OK;
   });
+}
+
+VF_API int vf_vocoder_varlen(vf_ctx* ctx, const float* mel, const int64_t* frame_offsets, int batch, float* wav_out, void* stream) {
+  return vocoder_varlen(ctx, mel, frame_offsets, batch, wav_out, (cudaStream_t)stream);
+}
+
+VF_API int vf_resynth(vf_ctx* ctx, const float* wav, int batch, int64_t n, float* wav_out, void* stream) {
+  return fixed_call(ctx, RESYNTH, "vf_resynth", "vf_resynth", wav, batch, n, wav_out, 0u, [&](Plan* plan, int off, int b) {
+    return restore_on(ctx, RESYNTH, plan, wav + (size_t)off * n, b, n, wav_out + (size_t)off * n, 0u, (cudaStream_t)stream);
+  });
+}
+
+VF_API int vf_resynth_varlen(vf_ctx* ctx, const float* wav, const int64_t* offsets, int batch, float* wav_out, void* stream) {
+  return varlen_call(ctx, RESYNTH, "vf_resynth_varlen", wav, offsets, batch, wav_out, 0u, (cudaStream_t)stream,
+                     [](Plan*, int, int, int64_t, const std::vector<int64_t>&) { return VF_OK; });
 }
 
 VF_API int vf_restore_ex(vf_ctx* ctx, const float* wav, int batch, int64_t n, float* wav_out, unsigned flags, void* stream) {

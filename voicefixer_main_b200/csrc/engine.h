@@ -134,12 +134,15 @@ struct DnnW {
 
 // PLAN_VARLEN: the GSR path for clips of different lengths (vf_restore_varlen), keyed by (batch, bucket): T = the bucket, a
 // multiple of 64 frames (the UNet's time granularity) that holds the call's longest clip.  PLAN_SSR_VARLEN: the same for
-// the SSR / GSR-UNet path (vf_ssr_restore_varlen)
-enum PlanKind { PLAN_GSR = 0, PLAN_SSR = 1, PLAN_VARLEN = 2, PLAN_SSR_VARLEN = 3 };
-// Plans of these kinds run unet_v2 + ISTFT (build_ssr); the others run the mel UNet + vocoder
+// the SSR / GSR-UNet path (vf_ssr_restore_varlen).  PLAN_VOC / PLAN_VOC_VARLEN: the vocoder alone on a linear mel
+// (vf_resynth, vf_resynth_varlen, vf_vocoder_varlen), fixed-shape and bucketed; they hold no analysis network
+enum PlanKind { PLAN_GSR = 0, PLAN_SSR = 1, PLAN_VARLEN = 2, PLAN_SSR_VARLEN = 3, PLAN_VOC = 4, PLAN_VOC_VARLEN = 5 };
+// Plans of these kinds run unet_v2 + ISTFT (build_ssr); the others run the vocoder, after the mel analysis module unless
+// is_voc_plan
 inline bool is_ssr_plan(int kind) { return kind == PLAN_SSR || kind == PLAN_SSR_VARLEN; }
+inline bool is_voc_plan(int kind) { return kind == PLAN_VOC || kind == PLAN_VOC_VARLEN; }
 // Plans of these kinds own a lengths table (kernels.cuh)
-inline bool is_varlen_plan(int kind) { return kind == PLAN_VARLEN || kind == PLAN_SSR_VARLEN; }
+inline bool is_varlen_plan(int kind) { return kind == PLAN_VARLEN || kind == PLAN_SSR_VARLEN || kind == PLAN_VOC_VARLEN; }
 
 // The previous use of a device buffer that calls on any stream share (a plan's workspace, a scratch): order_use makes
 // this use wait for it when it ran on another stream, mark_use records this one
@@ -166,11 +169,11 @@ struct Plan {
   cudaEvent_t io_ev[2][4] = {{nullptr, nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr, nullptr}};   // h2d done, input consumed, compute done, d2h done
   unsigned io_seq = 0;
   StreamOrder order;             // a plan's buffers are shared by every call of its shape
-  float* d_mel = nullptr;        // [B, T, 128] linear mel
-  float* d_logmel_in = nullptr;  // [B, T, 128] log10 mel (UNet input)
-  float* d_logmel_out = nullptr; // [B, T, 128]
+  float* d_mel = nullptr;        // [B, T, 128] linear mel (the vocoder's input in a vocoder-only plan)
+  float* d_logmel_in = nullptr;  // [B, T, 128] log10 mel (UNet input); null in a vocoder-only plan
+  float* d_logmel_out = nullptr; // [B, T, 128]; null in a vocoder-only plan
   float* d_voc_wav = nullptr;    // [B, L]
-  float* d_band = nullptr;       // [B][2] low-band energy sums (unify_energy)
+  float* d_band = nullptr;       // [B][2] low-band energy sums (unify_energy); null in a vocoder-only plan
   unsigned int* d_peak = nullptr;
   long L = 0;
   // SSR plans (unet_v2 + ISTFT)
@@ -380,8 +383,9 @@ Op first_op(vf_ctx* ctx, const UnetW& U, const ConvBlockW& blk, const float* in,
 // avg_pool2d(2,2) of an [batch, H * (W + 1), C] level + the consumer's bn1 + LeakyReLU: output pitch (W >> 1) + 1
 Op pool_op(vf_ctx* ctx, const float* in, int batch, int H, int W, int C, const Affine& next_bn1, PlanePtr out_r, PlanePtr out_a,
            float* out_raw, const int* row_valid);
-// vocoder conditioning of the restored log-mel [batch, T, 128]: Tv = T + T % 2 + voc_tail_base rows per clip
-Op cond_op(vf_ctx* ctx, const float* logmel, int batch, int T, PlanePtr out, const int* vl_T, const int* vl_Tv);
+// vocoder conditioning of the restored log-mel [batch, T, 128] (is_log 1) or of a linear mel (is_log 0): Tv = T + T % 2 +
+// voc_tail_base rows per clip
+Op cond_op(vf_ctx* ctx, const float* logmel, int batch, int T, PlanePtr out, const int* vl_T, const int* vl_Tv, int is_log = 1);
 inline int voc_frames(const vf_config& c, int T) { return T + T % 2 + c.voc_tail_base; }
 // amp_to_original_f (VF_RESTORE_UNIFY_ENERGY): zeroes `sums` and launches the low-band reduction on the stream, then points
 // the conditioning op at it
@@ -413,5 +417,7 @@ std::string op_signature(const Op& op);
 // row block (0, 0, 0 for other ops)
 void op_tile_loop(const Op& op, int64_t* tiles, int* grid, int* col_tiles);
 int build_plan(vf_ctx* ctx, Plan* plan);
+// engine.cu: the sub-batch a call of `batch` clips on plans of `kind` with `frames` (padded) frames runs in (the plan budget)
+int choose_sub_batch(vf_ctx* ctx, int kind, int batch, int frames);
 
 }  // namespace vf

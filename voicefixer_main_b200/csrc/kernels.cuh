@@ -58,6 +58,18 @@ struct MelGatherParams {
   int64_t frame_off[VL_MAX_CLIPS + 1];
 };
 cudaError_t launch_gather_mels(const MelGatherParams& p, cudaStream_t stream);
+// vf_vocoder_varlen: clip b's first off[b + 1] - off[b] values between a packed buffer (from element off[b]) and row b of a
+// plan buffer of `stride` elements per clip.  to_packed 0 scatters the packed mels into the plan's [batch, T, 128] d_mel
+// (off: frame offsets times 128, stride T * 128; rows t >= T_b are not written, the vocoder never reads them); 1 packs
+// each clip's first L_b samples of d_voc_wav [batch, L] (off: sample offsets, stride L).
+struct ClipCopyParams {
+  const float* src;
+  float* dst;
+  int batch, to_packed;
+  int64_t stride;
+  int64_t off[VL_MAX_CLIPS + 1];
+};
+cudaError_t launch_clip_copy(const ClipCopyParams& p, cudaStream_t stream);
 
 // vf_restore_chunks and vf_restore_windows (stream.cu): the tables of one sub-batch, kernel parameters like the lengths
 // table's offsets.  Gather: packed sample off[c] + j (j < off[c + 1] - off[c]) of row c is ring[src[c] + (phase[c] + j) mod

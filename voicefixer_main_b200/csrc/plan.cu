@@ -375,12 +375,12 @@ Op pool_op(vf_ctx* ctx, const float* in, int batch, int H, int W, int C, const A
   return op;
 }
 
-Op cond_op(vf_ctx* ctx, const float* logmel, int batch, int T, PlanePtr out, const int* vl_T, const int* vl_Tv) {
+Op cond_op(vf_ctx* ctx, const float* logmel, int batch, int T, PlanePtr out, const int* vl_T, const int* vl_Tv, int is_log) {
   const vf_config& c = ctx->cfg;
   Op op; op.kind = OP_COND;
   VocCondParams& p = op.cond;
   memset(&p, 0, sizeof p);
-  p.mel = logmel; p.is_log = 1; p.batch = batch; p.T = T; p.Tv = voc_frames(c, T); p.weight = ctx->d_melw;
+  p.mel = logmel; p.is_log = is_log; p.batch = batch; p.T = T; p.Tv = voc_frames(c, T); p.weight = ctx->d_melw;
   p.amp_floor = c.voc_amp_floor; p.ref_db = c.voc_ref_db; p.min_db = c.voc_min_db; p.tail_value = c.voc_tail_value;
   p.out = out;
   p.vl_T = vl_T; p.vl_Tv = vl_Tv;
@@ -646,7 +646,9 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
   Planes stem = b.planes(B, Tv, c.voc_channels);
   if (b.rc) return b.rc;
   plan->cond_op = (int)ops.size();
-  ops.push_back(cond_op(ctx, plan->d_logmel_out, B, T, cond.p, plan->vl(VL_T), plan->vl(VL_TV)));
+  // a vocoder-only plan conditions on its linear mel d_mel (vf_vocoder's is_log = 0), the others on the restored log-mel
+  const bool voc = is_voc_plan(plan->kind);
+  ops.push_back(cond_op(ctx, voc ? plan->d_mel : plan->d_logmel_out, B, T, cond.p, plan->vl(VL_T), plan->vl(VL_TV), voc ? 0 : 1));
   Planes cur = cond;
   for (int i = 0; i < c.voc_cond_layers; ++i) {
     const bool last = i == c.voc_cond_layers - 1;
@@ -929,7 +931,11 @@ int build_plan(vf_ctx* ctx, Plan* plan) {
     plan->d_vl_off = b.alloc<int64_t>((size_t)batch + 1);
     plan->d_vl_rows = b.alloc<int>((size_t)VL_ROWS * batch);
   }
-  if (!is_ssr_plan(kind)) {
+  if (is_voc_plan(kind)) {
+    // the vocoder alone: its linear mel input, its activations, d_voc_wav and d_peak (build_vocoder), the lengths table
+    plan->d_mel = b.alloc<float>((size_t)batch * frames * 128);
+    rc = b.rc ? b.rc : build_vocoder(ctx, b, plan);
+  } else if (!is_ssr_plan(kind)) {
     const size_t mel_n = (size_t)batch * frames * 128;
     plan->d_mel = b.alloc<float>(mel_n);
     plan->d_logmel_in = b.alloc<float>(mel_n);

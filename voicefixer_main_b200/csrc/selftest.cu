@@ -625,21 +625,21 @@ struct Tracer {
   }
 };
 
-// The restore of vf_selftest_plan_trace on the case's plan, step for step as restore_impl and ssr_impl run it
+// The restore of vf_selftest_plan_trace on the case's plan, step for step as restore_impl, ssr_impl and resynth_impl run it
 int run_trace(vf_ctx* ctx, Case& s, int kind, const float* wav, const int64_t* off, int batch, int64_t n, int T, unsigned flags,
               float* wav_out, vf_trace_fn fn, void* user) {
   Plan& plan = s.plan;
   plan.kind = kind; plan.batch = batch; plan.T = T;
   int rc = build_plan(ctx, &plan);
   if (rc) return rc;
-  const bool ssr = is_ssr_plan(kind);
+  const bool ssr = is_ssr_plan(kind), voc = is_voc_plan(kind);
   Tracer tr{ctx, plan, fn, user, {}, {}, {}};
   for (size_t i = 0; i < plan.allocs.size(); ++i) {
     tr.aptr.push_back((uint64_t)(uintptr_t)plan.allocs[i]);
     tr.abytes.push_back(plan.alloc_bytes[i]);
   }
   if (off && (rc = write_lengths_table(ctx, &plan, off, batch, ssr ? 1024 : 127, 0))) return rc;
-  rc = run_frontend(ctx, wav, batch, (long)n, ssr ? nullptr : plan.d_mel, ssr ? nullptr : plan.d_logmel_in, ssr ? plan.d_sp : nullptr,
+  rc = run_frontend(ctx, wav, batch, (long)n, ssr ? nullptr : plan.d_mel, plan.d_logmel_in, ssr ? plan.d_sp : nullptr,
                     nullptr, nullptr, 0, off ? &plan : nullptr);
   if (rc) return rc;
   CK(cudaDeviceSynchronize());
@@ -659,9 +659,11 @@ int run_trace(vf_ctx* ctx, Case& s, int kind, const float* wav, const int64_t* o
     return VF_OK;
   }
   Op& cop = plan.vocoder[plan.cond_op];
-  cop.cond.mel = plan.d_logmel_out;
-  cop.cond.is_log = 1;
-  cop.cond.band_sums = nullptr;
+  if (!voc) {      // a vocoder-only plan's conditioning op reads its d_mel as built
+    cop.cond.mel = plan.d_logmel_out;
+    cop.cond.is_log = 1;
+    cop.cond.band_sums = nullptr;
+  }
   if (flags & VF_RESTORE_UNIFY_ENERGY)
     CK(unify_energy(plan.d_mel, plan.d_logmel_out, batch, T, plan.d_band, plan.vl(VL_T), &cop.cond, 0));
   for (size_t i = 0; i < plan.vocoder.size(); ++i)
@@ -742,7 +744,7 @@ VF_API int vf_selftest_op(vf_ctx* ctx, vf_op_case* oc) {
 
 VF_API int vf_selftest_plan_gemms(vf_ctx* ctx, int plan_kind, int batch, int frames, vf_plan_gemm* records, int cap, int* count) {
   if (!ctx || !count || cap < 0 || (cap && !records)) return VF_EINVAL;
-  if (plan_kind < PLAN_GSR || plan_kind > PLAN_SSR_VARLEN || batch <= 0 || frames <= 0 ||
+  if (plan_kind < PLAN_GSR || plan_kind > PLAN_VOC_VARLEN || batch <= 0 || frames <= 0 ||
       (is_varlen_plan(plan_kind) && batch > VL_MAX_CLIPS))
     return fail(ctx, VF_EINVAL, "vf_selftest_plan_gemms: bad plan");
   if (ctx->validate_simt) return fail(ctx, VF_EINVAL, "vf_selftest_plan_gemms: validate_simt plans run no tensor-core launches");
@@ -769,11 +771,18 @@ VF_API int vf_selftest_plan_gemms(vf_ctx* ctx, int plan_kind, int batch, int fra
   });
 }
 
+VF_API int vf_selftest_sub_batch(vf_ctx* ctx, int plan_kind, int batch, int frames) {
+  if (!ctx) return VF_EINVAL;
+  if (plan_kind < PLAN_GSR || plan_kind > PLAN_VOC_VARLEN || batch <= 0 || frames <= 0)
+    return fail(ctx, VF_EINVAL, "vf_selftest_sub_batch: bad plan");
+  return choose_sub_batch(ctx, plan_kind, batch, frames);
+}
+
 VF_API int vf_selftest_plan_trace(vf_ctx* ctx, int plan_kind, const float* wav, const int64_t* offsets, int batch, int64_t n,
                                   unsigned flags, float* wav_out, vf_trace_fn fn, void* user) {
   if (!ctx || !wav || !wav_out || !fn || batch <= 0) return VF_EINVAL;
-  if (plan_kind < PLAN_GSR || plan_kind > PLAN_SSR_VARLEN || is_varlen_plan(plan_kind) != (offsets != nullptr) ||
-      (flags & ~(unsigned)VF_RESTORE_UNIFY_ENERGY) || (flags && is_ssr_plan(plan_kind)) ||
+  if (plan_kind < PLAN_GSR || plan_kind > PLAN_VOC_VARLEN || is_varlen_plan(plan_kind) != (offsets != nullptr) ||
+      (flags & ~(unsigned)VF_RESTORE_UNIFY_ENERGY) || (flags && (is_ssr_plan(plan_kind) || is_voc_plan(plan_kind))) ||
       (offsets && (batch > VL_MAX_CLIPS || offsets[0] != 0)))
     return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: bad call");
   if (!ctx->loaded) return fail(ctx, VF_ESTATE, "weights not loaded");

@@ -30,7 +30,7 @@ import torch
 
 from . import _lib as L
 from .arch import (SSR_PREFIX, UNET_PREFIX, VocoderConfig, bigru_keys, dnn_keys, frames_for, metric_frames, unet_keys,
-                   vocoder_keys)
+                   vocoder_keys, vocoder_out_len)
 
 
 class HParams(dict):
@@ -212,6 +212,43 @@ class Engine:
         out = torch.empty(b, self.lib.vf_vocoder_out_len(self.ctx, t), device=self.device)
         with torch.cuda.device(self.device):
             self._ck(self.lib.vf_vocoder(self.ctx, _ptr(mel_lin), b, t, _ptr(out), _stream()))
+        return out
+
+    def vocoder_varlen(self, mel_packed: torch.Tensor, frames, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The vocoder on linear mels of different lengths in one call (vf_vocoder_varlen): mel_packed [sum(frames), 128]
+        holds the clips' frames back to back; returns each clip's full vocoder output, arch.vocoder_out_len(T_i) samples,
+        packed in clip order (no peak normalise, no trim).  Clip i is bit-identical to vocoder(mel_i[None])[0].  Needs only
+        the vocoder's weights."""
+        if not isinstance(mel_packed, torch.Tensor) or mel_packed.dtype != torch.float32 or mel_packed.device != self.device:
+            raise TypeError(f"mel_packed must be a float32 CUDA tensor on {self.device}")
+        frames = [int(t) for t in frames]
+        if mel_packed.dim() != 2 or mel_packed.shape[1] != 128 or not frames or sum(frames) != mel_packed.shape[0]:
+            raise ValueError("mel_packed must be [sum(frames), 128] and hold the frames of at least one clip")
+        offsets = _offsets(frames)
+        n_out = sum(vocoder_out_len(t, self.voc_cfg) for t in frames) if min(frames) > 0 else 0
+        out = torch.empty(n_out, device=self.device) if out is None else out
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_vocoder_varlen(self.ctx, _ptr(mel_packed.contiguous()), offsets, len(frames), _ptr(out),
+                                                _stream()))
+        return out
+
+    def resynth(self, wav: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Vocoder resynthesis (vf_resynth): wav [B,N] -> the vocoder on its linear mel, peak normalised and trimmed to [B,N]
+        (restore() without the analysis module).  Needs only the vocoder's weights."""
+        wav = _check_in(wav, self.device, "wav")
+        b, n = wav.shape
+        out = torch.empty_like(wav) if out is None else out
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_resynth(self.ctx, _ptr(wav), b, n, _ptr(out), _stream()))
+        return out
+
+    def resynth_varlen(self, wav_packed: torch.Tensor, lengths, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """resynth for clips of different lengths in one call (vf_resynth_varlen), packed as restore_varlen: clip i of the
+        result is bit-identical to resynth(clip_i[None])[0]."""
+        wav_packed, offsets = self._varlen_args(wav_packed, lengths)
+        out = torch.empty_like(wav_packed) if out is None else out
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_resynth_varlen(self.ctx, _ptr(wav_packed), offsets, len(offsets) - 1, _ptr(out), _stream()))
         return out
 
     def restore(self, wav: torch.Tensor, out: Optional[torch.Tensor] = None, unify_energy: bool = False) -> torch.Tensor:
@@ -666,7 +703,7 @@ class Engine:
 
     def selftest_plan_gemms(self, plan_kind: int, batch: int, frames: int, tile_loop: bool = False):
         """[(label, signature)] of every GEMM / fused-pair launch of a plan of plan_kind (0 GSR, 1 SSR, 2 GSR varlen, 3 SSR
-        varlen) built with the loaded weights and the current options; nothing is launched (vf_selftest_plan_gemms; tests
+        varlen, 4 vocoder-only, 5 vocoder-only varlen) built with the loaded weights and the current options; nothing is launched (vf_selftest_plan_gemms; tests
         only).  With tile_loop, [(label, signature, tiles, grid, col_tiles)]: each launch's persistent tile loop as well."""
         cap, n = 2048, ctypes.c_int()
         recs = (L.VfPlanGemm * cap)()
@@ -677,9 +714,17 @@ class Engine:
             return [(r.label.decode(), r.sig.decode(), r.tiles, r.grid, r.col_tiles) for r in recs[:n.value]]
         return [(r.label.decode(), r.sig.decode()) for r in recs[:n.value]]
 
+    def selftest_sub_batch(self, plan_kind: int, batch: int, frames: int) -> int:
+        """The sub-batch a call of `batch` clips of `frames` frames on plans of plan_kind runs in under the plan budget
+        (vf_selftest_sub_batch; tests only)."""
+        rc = self.lib.vf_selftest_sub_batch(self.ctx, plan_kind, batch, frames)
+        if rc < 0:
+            self._ck(rc)
+        return rc
+
     def selftest_plan_trace(self, plan_kind: int, wav: torch.Tensor, lengths=None, on_op=None, unify_energy: bool = False):
-        """One restore on a fresh plan of plan_kind (0 GSR, 1 SSR: wav [B, n]; 2 GSR varlen, 3 SSR varlen: wav packed,
-        lengths per clip), one launch at a time: on_op(after, op) runs before (after = False) and after (True) each launch
+        """One restore on a fresh plan of plan_kind (0 GSR, 1 SSR, 4 vocoder-only resynthesis: wav [B, n]; 2 GSR varlen,
+        3 SSR varlen, 5 vocoder-only varlen: wav packed, lengths per clip), one launch at a time: on_op(after, op) runs before (after = False) and after (True) each launch
         with its L.VfTraceOp (vf_selftest_plan_trace; tests only).  An exception in on_op stops the run and is raised here.
         Returns the restored output, shaped as the matching restore call returns it."""
         wav = _check_in(wav, self.device, "wav")
