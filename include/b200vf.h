@@ -22,6 +22,8 @@
  *   vf_restore_varlen_mels        + each clip's stage A / B mels, the inputs of handler()'s metrics (handler_batch)
  *   vf_restore_chunks             the chunks of many live streams, gathered from device rings and cropped on the device:
  *                                 LambdaOverlapAdd (tools/dsp/overlapadd_boxcar.py:338-534) run incrementally
+ *   vf_vocoder_chunks             the chunks of many live mel streams (a TTS or voice-conversion model's output),
+ *                                 gathered from device frame rings, vocoded and cropped on the device
  *   vf_to_log / vf_from_log       tools/pytorch/pytorch_util.py:157-163
  *   vf_to_pcm16                   the int16 conversion of save_wave, tools/file/wav.py:22-24 (SURVEY.md 8(f) row 3)
  *   vf_mel                        MelScale.forward on any spectrogram, tools/pytorch/mel_scale.py:52-64
@@ -219,6 +221,22 @@ typedef struct vf_chunk {
 } vf_chunk;
 VF_API int vf_restore_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_len, const vf_chunk* chunks, int n_chunks,
                              float* kept_out, unsigned flags, void* stream);
+/* Chunks of live mel streams, vocoded in one call (voicefixer_main_b200/streaming.py StreamingVocoder), on a context that
+ * holds the vocoder's weights (as vf_vocoder_varlen).  ring [n_streams, ring_frames, 128] (device) holds each stream's recent
+ * linear mel frames: absolute frame p of stream s is row s * ring_frames + p mod ring_frames.  chunks: HOST table of
+ * n_chunks vf_chunk entries (read during the call only), as in vf_restore_chunks except that start, length and valid
+ * count frames and crop_left / crop_right count samples of the chunk's vf_vocoder_out_len(length) output: chunk c vocodes
+ * frames start .. start + length - 1 of stream `stream`, a frame >= valid reading as zeros, and its output samples
+ * [crop_left, vf_vocoder_out_len(length) - crop_right) are written to kept_out (device), chunk after chunk.  Chunk c's kept
+ * samples are bit-identical to vf_vocoder_varlen on its (zero-filled) frames alone, cropped.  Every argument is checked
+ * before any work is queued (VF_EINVAL: a stream out of range, length < 1, > ring_frames or over vf_vocoder_varlen's 2^30 /
+ * hop + 1 frames, crops that leave nothing, start < 0; VF_ESTATE: a context without "vocoder.*"); the context stays usable.
+ * Per sub-batch, on its PLAN_VOC_VARLEN plan: the lengths table, one gather launch of the chunks' frames from the rings
+ * straight into the plan's mel rows, the vocoder chain (replayed as a CUDA graph) and one crop launch straight out of the
+ * plan's output rows.  Sub-batches and plan shapes as vf_restore_chunks (next power of two of the chunk count, the extra
+ * rows repeating the first chunk; the largest sub-batch follows the vocoder-only plan size per frame).  No scratch. */
+VF_API int vf_vocoder_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_frames, const vf_chunk* chunks,
+                             int n_chunks, float* kept_out, void* stream);
 /* The same for the SSR_UNet / GSR_UNet path: clips of different lengths, packed and with HOST offsets as in
  * vf_restore_varlen, no flags.  Clip i's output is bit-identical to vf_ssr_restore on that clip alone (batch 1, same
  * options).  Every clip needs more than 1024 samples and at most 2^30 (no trim_center constraint: there is no vocoder); a

@@ -25,7 +25,7 @@ EXPORTS = [
     "vf_sosfiltfilt_varlen", "vf_resample_poly_f64_varlen", "vf_metric_spectrogram_ex", "vf_score_varlen_ex",
     "vf_score_time_varlen_ex", "vf_restore_chunks", "vf_ssr_restore_chunks", "vf_restore_windows", "vf_ssr_restore_windows",
     "vf_selftest_plan_gemms", "vf_resample_sinc_varlen", "vf_selftest_plan_trace", "vf_vocoder_varlen", "vf_resynth",
-    "vf_resynth_varlen", "vf_selftest_sub_batch",
+    "vf_resynth_varlen", "vf_selftest_sub_batch", "vf_vocoder_chunks",
 ]
 VF_RESTORE_UNIFY_ENERGY = 1
 VF_SSR_PEAK_NORMALISE = 1
@@ -103,7 +103,8 @@ class VfGruCase(Structure):
 
 
 class VfChunk(Structure):
-    """vf_chunk (include/b200vf.h): one chunk of a vf_restore_chunks call."""
+    """vf_chunk (include/b200vf.h): one chunk of a vf_restore_chunks call (of a vf_vocoder_chunks call: start, length and
+    valid in frames, the crops in output samples)."""
     _fields_ = [("stream", c_int32), ("length", c_int32), ("crop_left", c_int32), ("crop_right", c_int32),
                 ("start", c_int64), ("valid", c_int64)]
 
@@ -181,6 +182,7 @@ def load_library():
     lib.vf_restore_ex.argtypes = [P, P, c_int, c_int64, P, c_uint, P]
     lib.vf_restore_varlen.argtypes = [P, P, POINTER(c_int64), c_int, P, c_uint, P]
     lib.vf_restore_chunks.argtypes = [P, P, c_int, c_int64, POINTER(VfChunk), c_int, P, c_uint, P]
+    lib.vf_vocoder_chunks.argtypes = [P, P, c_int, c_int64, POINTER(VfChunk), c_int, P, P]
     lib.vf_restore_varlen_mels.argtypes = [P, P, POINTER(c_int64), c_int, P, c_uint, P, P, P]
     lib.vf_ssr_forward.argtypes = [P, P, P, c_int, c_int64, P, P]
     lib.vf_ssr_restore.argtypes = [P, P, c_int, c_int64, P, P]

@@ -179,3 +179,32 @@ def padded_frames(t: int) -> int:
 
 def vocoder_out_len(t: int, cfg: VocoderConfig) -> int:
     return (t + t % 2 + cfg.tail_pad_base) * cfg.hop
+
+
+def vocoder_receptive_field(cfg: VocoderConfig = None) -> int:
+    """R, in frames: the smallest margin such that mel frames outside [a - R, b + R) cannot change the vocoder's output
+    samples of frames [a, b) (frame t's samples are [t hop, (t + 1) hop)).  A chunk with R frames of context on each side of
+    its kept frames therefore gives those frames the samples of the whole mel; 576 frames (5.76 s) for the default config.
+
+    Derived layer by layer: the interval a perturbation of one frame p reaches, in the units of each layer's output -
+      - each of the cond_layers k3 convs (padding 1): +-1 frame;
+      - the k7 reflect-padded stem: +-(stem_kernel // 2) frames;
+      - each stage's ConvTranspose1d (stride s, kernel 2s, padding s // 2 + s % 2 = P): input [lo, hi] reaches output
+        samples [lo s - P, hi s - P + 2s - 1] at the stage's rate;
+      - each of the stage's resstack_depth residual pairs: the dilated k3 conv (dilation 3^i) +-3^i, the k3 conv after it
+        +-1, in that stage's samples;
+      - the k7 reflect-padded tail: +-(stem_kernel // 2) output samples.
+    The frames of the samples reached, [floor(lo / hop), floor(hi / hop)], are then p - left .. p + right, and R =
+    max(left, right).  Reflect and zero padding at a clip's edges and the constant tail frames only fold or drop what this
+    interval holds, so no edge reaches farther; with every tap of the seeded weights non-zero the bound is tight."""
+    cfg = cfg or VocoderConfig()
+    h = cfg.resstack_kernel // 2
+    hi = cfg.cond_layers + cfg.stem_kernel // 2          # frame p = 0 through the cond-net and the stem
+    lo = -hi
+    for scale, depth in zip(cfg.upsample_scales, cfg.resstack_depth):
+        pad = scale // 2 + scale % 2
+        lo, hi = lo * scale - pad, hi * scale - pad + 2 * scale - 1
+        reach = sum(cfg.dilation(i) * h + h for i in range(depth))
+        lo, hi = lo - reach, hi + reach
+    lo, hi = lo - cfg.stem_kernel // 2, hi + cfg.stem_kernel // 2
+    return max(-(lo // cfg.hop), hi // cfg.hop)

@@ -673,6 +673,8 @@ int restore_varlen(vf_ctx* ctx, const char* fn, const float* wav, const int64_t*
 // scatter of the clips' mels into d_mel, the vocoder chain and one pack of each clip's L_i = vf_vocoder_out_len(T_i)
 // samples into wav_out at sum_{j<i} L_j.  The lengths table is written from sample offsets of clips of (T_i - 1) * hop
 // samples, which have T_i frames.
+int64_t vocoder_max_frames(vf_ctx* ctx) { return ((int64_t)1 << 30) / ctx->cfg.hop + 1; }     // the packed restores' 2^30 samples
+
 int vocoder_varlen(vf_ctx* ctx, const float* mel, const int64_t* frame_offsets, int batch, float* wav_out, cudaStream_t st) {
   const char* fn = "vf_vocoder_varlen";
   int rc = check_ready(ctx);
@@ -682,7 +684,7 @@ int vocoder_varlen(vf_ctx* ctx, const float* mel, const int64_t* frame_offsets, 
   rc = check_networks(ctx, PLAN_VOC_VARLEN);
   if (rc) return rc;
   const int hop = ctx->cfg.hop;
-  const int64_t max_frames = ((int64_t)1 << 30) / hop + 1;     // the packed restores' 2^30 samples
+  const int64_t max_frames = vocoder_max_frames(ctx);
   std::vector<int64_t> wav_off(batch + 1, 0);
   for (int i = 0; i < batch; ++i) {
     const int64_t T = frame_offsets[i + 1] - frame_offsets[i];
@@ -820,35 +822,49 @@ struct OlaStage {
   }
 };
 
-// The streaming calls of family f after their checks: per sub-batch one gather from the rings into the packed input scratch,
-// the family's packed restore of the rows into the packed output scratch, and stage.sub_batch on the restored rows; then
-// stage.finish.
-//
-// Plan shapes: a streaming session's row count changes from step to step, and varlen plans are keyed by (batch, bucket),
-// so each sub-batch runs on the next power of two of its row count.  A sub-batch holds at most the largest power of two P
-// (and VL_MAX_CLIPS) whose shapes 1, 2, 4, .., P fit the plan budget together (2P - 1 rows): a session then meets at most
-// nine batch shapes per bucket instead of one per row count, and they stay cached side by side instead of evicting one
-// another whenever the count crosses a power of two.  The rows past the sub-batch's own repeat its first row, whose results
-// are discarded: rows are independent, so they change no output sample, and unlike a row of digital silence they put nothing
-// through the chain that the call's own audio does not.  The cap follows the plan size per frame of the family
-// (choose_sub_batch): an SSR varlen plan holds about 1.4 times a VoiceFixer one per padded frame, so its cap is reached at
-// shorter rows.
+// Plan shapes of the streaming calls (vf_restore_chunks, vf_restore_windows, vf_vocoder_chunks): a streaming session's row
+// count changes from step to step, and varlen plans are keyed by (batch, bucket), so each sub-batch runs on the next power of
+// two of its row count.  A sub-batch holds at most the largest power of two P (and VL_MAX_CLIPS) whose shapes 1, 2, 4, .., P
+// fit the plan budget together (2P - 1 rows): a session then meets at most nine batch shapes per bucket instead of one per
+// row count, and they stay cached side by side instead of evicting one another whenever the count crosses a power of two.
+// The rows past the sub-batch's own repeat its first row, whose results are discarded: rows are independent, so they change
+// no output sample, and unlike a row of digital silence they put nothing through the chain that the call's own audio does
+// not.  The cap follows the plan size per frame of the plan kind (choose_sub_batch) at the bucket of the call's longest row:
+// an SSR varlen plan holds about 1.4 times a VoiceFixer one per padded frame, so its cap is reached at shorter rows.
+struct StreamShapes {
+  int n, cap;                                     // the call's rows, the sub-batch cap P
+  int size(int s) const { return std::min(cap, n - s); }                     // rows of the sub-batch from row s
+  static int rows(int b) { int r = 1; while (r < b) r *= 2; return r; }      // its plan's batch
+  int at(int s, int k) const { return s + (k < size(s) ? k : 0); }           // the call's row in plan row k
+};
+
+StreamShapes stream_shapes(vf_ctx* ctx, int kind, int n_rows, int bucket) {
+  const int fit = choose_sub_batch(ctx, kind, 2 * VL_MAX_CLIPS, bucket);
+  int cap = 1;
+  while (cap < VL_MAX_CLIPS && 4 * cap - 1 <= fit) cap *= 2;     // shapes 1, 2, .., 2 cap: 4 cap - 1 rows in all
+  return StreamShapes{n_rows, cap};
+}
+
+// The frames of a stream row before its stream's end: `length` from `start` on, none at or past `valid`.  valid - start
+// would overflow for an open stream (valid = INT64_MAX) and a window start below 0.
+int64_t valid_count(int64_t start, int64_t length, int64_t valid) {
+  return valid <= start ? 0 : valid - length >= start ? length : valid - start;
+}
+
+// The streaming calls of family f after their checks: per sub-batch (stream_shapes) one gather from the rings into the
+// packed input scratch, the family's packed restore of the rows into the packed output scratch, and stage.sub_batch on the
+// restored rows; then stage.finish.
 template <typename Stage>
 int run_stream_rows(vf_ctx* ctx, const Family& f, const float* ring, int64_t ring_len, const std::vector<StreamRow>& rows_in,
                     Stage& stage, unsigned flags, cudaStream_t st) {
   const int n_rows = (int)rows_in.size();
   int64_t longest = 0;
   for (const StreamRow& r : rows_in) longest = std::max(longest, r.length);
-  const int fit = choose_sub_batch(ctx, f.varlen_kind, 2 * VL_MAX_CLIPS, round_up(frames_of(ctx, (long)longest), 64));
-  int cap = 1;
-  while (cap < VL_MAX_CLIPS && 4 * cap - 1 <= fit) cap *= 2;     // shapes 1, 2, .., 2 cap: 4 cap - 1 rows in all
-  auto rows_of = [](int b) { int r = 1; while (r < b) r *= 2; return r; };
-  auto row_at = [&](int s, int b, int k) -> const StreamRow& { return rows_in[s + (k < b ? k : 0)]; };
+  const StreamShapes sh = stream_shapes(ctx, f.varlen_kind, n_rows, round_up(frames_of(ctx, (long)longest), 64));
   int64_t max_samples = 0;
-  for (int s = 0; s < n_rows; s += cap) {
-    const int b = std::min(cap, n_rows - s);
+  for (int s = 0; s < n_rows; s += sh.cap) {
     int64_t n = 0;
-    for (int k = 0; k < rows_of(b); ++k) n += row_at(s, b, k).length;
+    for (int k = 0; k < StreamShapes::rows(sh.size(s)); ++k) n += rows_in[sh.at(s, k)].length;
     max_samples = std::max(max_samples, n);
   }
   return with_use(ctx, ctx->chunks.order, st, [&]() -> int {
@@ -856,20 +872,19 @@ int run_stream_rows(vf_ctx* ctx, const Family& f, const float* ring, int64_t rin
     if (rc) return rc;
     float* in = static_cast<float*>(ctx->chunks.p);
     float* out = in + max_samples;
-    for (int s = 0; s < n_rows; s += cap) {
-      const int b = std::min(cap, n_rows - s), rows = rows_of(b);
+    for (int s = 0; s < n_rows; s += sh.cap) {
+      const int b = sh.size(s), rows = StreamShapes::rows(b);
       ChunkGatherParams g;
       memset(&g, 0, sizeof g);
       g.ring = ring; g.out = in; g.ring_len = ring_len; g.rows = rows;
       int64_t n_max = 0;
       for (int k = 0; k < rows; ++k) {
-        const StreamRow& c = row_at(s, b, k);
+        const StreamRow& c = rows_in[sh.at(s, k)];
         g.off[k + 1] = g.off[k] + c.length;
         g.src[k] = (int64_t)c.stream * ring_len;
         g.phase[k] = (c.start % ring_len + ring_len) % ring_len;
         g.lead[k] = c.start < 0 ? std::min<int64_t>(c.length, -c.start) : 0;
-        // valid - start would overflow for an open stream (valid = INT64_MAX) and a window start below 0
-        g.n_valid[k] = c.valid <= c.start ? 0 : c.valid - c.length >= c.start ? c.length : c.valid - c.start;
+        g.n_valid[k] = valid_count(c.start, c.length, c.valid);
         n_max = std::max<int64_t>(n_max, c.length);
       }
       Plan* plan;
@@ -968,6 +983,85 @@ int restore_windows(vf_ctx* ctx, const Family& f, const char* fn, const float* r
   }
   OlaStage stage{windows, W, synthesis, acc, acc_len, emits, n_emits, out};
   return run_stream_rows(ctx, f, ring, ring_len, rows, stage, flags, st);
+}
+
+// vf_vocoder_chunks: every check before anything is queued, then per sub-batch (stream_shapes on PLAN_VOC_VARLEN at the
+// bucket of the call's longest chunk; each sub-batch on the bucket of its own), inside one use of its plan: the lengths
+// table as vocoder_varlen writes it, one gather of the chunks' frames from the rings straight into d_mel at the bucket's row
+// stride, the vocoder chain, and one crop of each chunk's kept samples straight out of d_voc_wav (row stride plan->L) into
+// kept_out, chunk after chunk.  The plan's own buffers are the packed input and output: no scratch.
+int vocoder_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_frames, const vf_chunk* chunks, int n_chunks,
+                   float* kept_out, cudaStream_t st) {
+  const char* fn = "vf_vocoder_chunks";
+  int rc = check_ready(ctx);
+  if (rc) return rc;
+  if (!ring || !chunks || !kept_out || n_streams <= 0 || ring_frames <= 0 || n_chunks <= 0)
+    return fail(ctx, VF_EINVAL, "%s: bad arguments", fn);
+  rc = check_networks(ctx, PLAN_VOC_VARLEN);
+  if (rc) return rc;
+  const int64_t max_frames = vocoder_max_frames(ctx);
+  int longest = 0;
+  for (int i = 0; i < n_chunks; ++i) {
+    const vf_chunk& c = chunks[i];
+    if (c.stream < 0 || c.stream >= n_streams)
+      return fail(ctx, VF_EINVAL, "%s: chunk %d: stream %d is not in 0 .. %d", fn, i, c.stream, n_streams - 1);
+    if (c.length < 1 || c.length > ring_frames)
+      return fail(ctx, VF_EINVAL, "%s: chunk %d: %d frames do not fit a ring of %ld", fn, i, c.length, (long)ring_frames);
+    if (c.length > max_frames)
+      return fail(ctx, VF_EINVAL, "%s: chunk %d: %d frames is too long for one call (at most %ld)", fn, i, c.length, (long)max_frames);
+    const int64_t n_out = vf_vocoder_out_len(ctx, c.length);
+    if (c.crop_left < 0 || c.crop_right < 0 || (int64_t)c.crop_left + c.crop_right >= n_out)
+      return fail(ctx, VF_EINVAL, "%s: chunk %d: crops %d and %d leave nothing of %ld samples", fn, i, c.crop_left, c.crop_right, (long)n_out);
+    if (c.start < 0 || c.start > INT64_MAX - c.length) return fail(ctx, VF_EINVAL, "%s: chunk %d: start %ld is out of range", fn, i, (long)c.start);
+    longest = std::max(longest, (int)c.length);
+  }
+  const StreamShapes sh = stream_shapes(ctx, PLAN_VOC_VARLEN, n_chunks, round_up(longest, 64));
+  const int hop = ctx->cfg.hop;
+  int64_t kept_off = 0;
+  for (int s = 0; s < n_chunks; s += sh.cap) {
+    const int b = sh.size(s), rows = StreamShapes::rows(b);
+    FrameGatherParams g;
+    memset(&g, 0, sizeof g);
+    g.ring = ring; g.ring_frames = ring_frames; g.rows = rows;
+    int64_t rel[VL_MAX_CLIPS + 1] = {0};      // the lengths table's sample offsets: clips of (T - 1) * hop samples
+    int n_max = 0;
+    for (int k = 0; k < rows; ++k) {
+      const vf_chunk& c = chunks[sh.at(s, k)];
+      g.off[k + 1] = g.off[k] + c.length;
+      g.src[k] = (int64_t)c.stream * ring_frames;
+      g.phase[k] = c.start % ring_frames;
+      g.n_valid[k] = valid_count(c.start, c.length, c.valid);
+      rel[k + 1] = rel[k] + (int64_t)(c.length - 1) * hop;
+      n_max = std::max(n_max, (int)c.length);
+    }
+    Plan* plan;
+    rc = get_plan(ctx, PLAN_VOC_VARLEN, rows, round_up(n_max, 64), &plan);
+    if (rc) return rc;
+    g.out = plan->d_mel; g.stride = plan->T;
+    ChunkCropParams cp;
+    memset(&cp, 0, sizeof cp);
+    cp.restored = plan->d_voc_wav; cp.kept = kept_out + kept_off; cp.chunks = b;
+    for (int k = 0; k < b; ++k) {
+      const vf_chunk& c = chunks[s + k];
+      cp.src[k] = (int64_t)k * plan->L + c.crop_left;
+      cp.keep[k + 1] = cp.keep[k] + vf_vocoder_out_len(ctx, c.length) - c.crop_left - c.crop_right;
+    }
+    rc = run_restore(ctx, plan, RESYNTH.w0, rows, rel, st, [&]() -> int {
+      CK(launch_frame_gather(g, st));
+      ctx->launches++;
+      int r = stage_mark(ctx, 1, st);
+      if (!r) r = stage_mark(ctx, 2, st);
+      if (!r) r = run_vocoder_chain(ctx, plan, st);
+      if (!r) r = stage_mark(ctx, 3, st);
+      if (r) return r;
+      CK(launch_stream_crop(cp, st));
+      ctx->launches++;
+      return VF_OK;
+    });
+    if (rc) return rc;
+    kept_off += cp.keep[b];
+  }
+  return VF_OK;
 }
 
 // vf_ssr_restore_varlen (`fn`) and vf_ssr_restore_varlen_mels.  After each sub-batch's ISTFT, still inside the plan's use on
@@ -1155,6 +1249,11 @@ VF_API int vf_vocoder(vf_ctx* ctx, const float* mel_lin, int batch, int frames, 
 
 VF_API int vf_vocoder_varlen(vf_ctx* ctx, const float* mel, const int64_t* frame_offsets, int batch, float* wav_out, void* stream) {
   return vocoder_varlen(ctx, mel, frame_offsets, batch, wav_out, (cudaStream_t)stream);
+}
+
+VF_API int vf_vocoder_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_frames, const vf_chunk* chunks,
+                             int n_chunks, float* kept_out, void* stream) {
+  return vocoder_chunks(ctx, ring, n_streams, ring_frames, chunks, n_chunks, kept_out, (cudaStream_t)stream);
 }
 
 VF_API int vf_resynth(vf_ctx* ctx, const float* wav, int batch, int64_t n, float* wav_out, void* stream) {

@@ -97,6 +97,23 @@ struct ChunkCropParams {
   int64_t src[VL_MAX_CLIPS];
 };
 cudaError_t launch_stream_crop(const ChunkCropParams& p, cudaStream_t stream);
+// vf_vocoder_chunks' gather of one sub-batch (stream.cu), straight into a PLAN_VOC_VARLEN plan's d_mel: frame t < off[c + 1]
+// - off[c] of chunk c is the 128 floats out[(c * stride + t) * 128 ..] (stride: the plan's frames per row, its bucket), read
+// from ring[(src[c] + (phase[c] + t) mod ring_frames) * 128 ..] when t < n_valid[c], else 0 (src: the chunk's stream times
+// ring_frames; phase: start mod ring_frames; n_valid: the frames before the stream's end).  Rows t >= the chunk's length
+// are not written: the lengths table keeps every launch of the chain off them, as in vf_vocoder_varlen.  Its crop is
+// launch_stream_crop on d_voc_wav.
+struct FrameGatherParams {
+  const float* ring;
+  float* out;
+  int64_t ring_frames, stride;
+  int rows;
+  int64_t off[VL_MAX_CLIPS + 1];
+  int64_t src[VL_MAX_CLIPS];
+  int64_t phase[VL_MAX_CLIPS];
+  int64_t n_valid[VL_MAX_CLIPS];
+};
+cudaError_t launch_frame_gather(const FrameGatherParams& p, cudaStream_t stream);
 // vf_restore_windows' overlap-add of one sub-batch.  Its windows are grouped into runs, one per stream, each run's windows in
 // ascending start.  Thread pos[r] + i handles output position t = lo[r] + i of run r: for every window w in first[r] ..
 // first[r + 1] - 1 with start[w] <= t < end[w], in that order, acc[acc_row[r] + t mod acc_len] += fl(synth[t - start[w]] *

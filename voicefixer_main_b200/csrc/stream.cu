@@ -2,7 +2,7 @@
 // packed input from the streams' device rings, and either the crop that keeps each chunk's centre of the packed restored
 // output (chunks) or the overlap-add of each synthesis-weighted window into the caller's per-stream accumulators followed by
 // the emission of the finished samples (windows).  Between the gather and the output stage runs the varlen restore chain
-// (engine.cu).  Each is one launch per sub-batch of at most VL_MAX_CLIPS rows (the emission: per VL_MAX_CLIPS streams),
+// (engine.cu).  vf_vocoder_chunks has its own frame gather, straight into a vocoder plan's mel rows, and the same crop.  Each is one launch per sub-batch of at most VL_MAX_CLIPS rows (the emission: per VL_MAX_CLIPS streams),
 // whatever the number of streams: the tables are __grid_constant__ kernel parameters (about 10 KB for the gather, 13 KB for
 // the overlap-add at 256 rows), so no host memory is read after the call returns and no copy of a table is queued.  One
 // thread per packed or accumulated sample; a warp's threads nearly always fall into one row, so the table lookups broadcast.
@@ -38,6 +38,23 @@ __global__ void __launch_bounds__(STREAM_THREADS) stream_gather_kernel(const __g
     v = __ldg(p.ring + p.src[c] + r);
   }
   p.out[i] = v;
+}
+
+// One thread per float of the packed frames: 128 consecutive threads copy one frame, so a warp reads 128 contiguous bytes
+// of one ring row and writes them to one d_mel row.
+__global__ void __launch_bounds__(STREAM_THREADS) frame_gather_kernel(const __grid_constant__ FrameGatherParams p) {
+  const int64_t i = (int64_t)blockIdx.x * STREAM_THREADS + threadIdx.x;
+  if (i >= p.off[p.rows] * 128) return;
+  const int64_t f = i >> 7;
+  const int c = find_row(p.off, p.rows, f);
+  const int64_t t = f - p.off[c];
+  float v = 0.f;                                   // at or past the stream's end: the zero fill
+  if (t < p.n_valid[c]) {
+    int64_t r = p.phase[c] + t;                    // t < length <= ring_frames, so one subtraction wraps it
+    if (r >= p.ring_frames) r -= p.ring_frames;
+    v = __ldg(p.ring + (p.src[c] + r) * 128 + (i & 127));
+  }
+  p.out[((int64_t)c * p.stride + t) * 128 + (i & 127)] = v;
 }
 
 __global__ void __launch_bounds__(STREAM_THREADS) stream_crop_kernel(const __grid_constant__ ChunkCropParams p) {
@@ -86,6 +103,12 @@ __global__ void __launch_bounds__(STREAM_THREADS) window_emit_kernel(const __gri
 cudaError_t launch_stream_gather(const ChunkGatherParams& p, cudaStream_t stream) {
   const int64_t n = p.off[p.rows];
   stream_gather_kernel<<<(unsigned)((n + STREAM_THREADS - 1) / STREAM_THREADS), STREAM_THREADS, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_frame_gather(const FrameGatherParams& p, cudaStream_t stream) {
+  const int64_t n = p.off[p.rows] * 128;
+  frame_gather_kernel<<<(unsigned)((n + STREAM_THREADS - 1) / STREAM_THREADS), STREAM_THREADS, 0, stream>>>(p);
   return cudaGetLastError();
 }
 

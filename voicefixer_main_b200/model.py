@@ -289,6 +289,19 @@ class Engine:
                                                 flags, _stream()))
         return out
 
+    def vocoder_chunks(self, ring: torch.Tensor, table) -> torch.Tensor:
+        """Chunks of live mel streams vocoded in one call (vf_vocoder_chunks): ring [n_streams, ring_frames, 128] float32 on
+        the device holds stream s's absolute frame p at ring[s, p % ring_frames]; table is a sequence of (stream, length,
+        crop_left, crop_right, start, valid) tuples, start / length / valid in frames and the crops in output samples.
+        Returns the kept samples out_c[crop_left : vocoder_out_len(length) - crop_right] of every chunk, packed in table
+        order, where out_c is vocoder_varlen of frames start .. start + length - 1 with those >= valid read as zeros.  Needs
+        only the vocoder's weights."""
+        ring, rows, out = self._chunks_args(ring, table, lambda n: vocoder_out_len(n, self.voc_cfg) if n > 0 else 0)
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_vocoder_chunks(self.ctx, _ptr(ring), ring.shape[0], ring.shape[1], rows, len(table), _ptr(out),
+                                                _stream()))
+        return out
+
     def ssr_restore_chunks(self, ring: torch.Tensor, table) -> torch.Tensor:
         """restore_chunks for the SSR / GSR-UNet path (vf_ssr_restore_chunks): the same ring and table, and out_c is
         ssr_forward(None, chunk[None])[0] of the zero-filled chunk."""
@@ -342,13 +355,17 @@ class Engine:
         ems = (L.VfEmit * max(1, len(emits)))(*[L.VfEmit(*map(int, t)) for t in emits])
         return ring, acc, synthesis, rows, ems, torch.empty(sum(max(0, int(t[2])) for t in emits), device=self.device)
 
-    def _chunks_args(self, ring: torch.Tensor, table):
-        """Checked ring, the host vf_chunk table and the packed output of a chunks call."""
+    def _chunks_args(self, ring: torch.Tensor, table, out_len=None):
+        """Checked ring, the host vf_chunk table and the packed output of a chunks call.  out_len: the output samples of a
+        chunk of `length` positions, for a ring of mel frames ([n_streams, ring_frames, 128]); None: a ring of samples."""
         ring = _check_in(ring, self.device, "ring")
-        if ring.dim() != 2:
+        if out_len is None and ring.dim() != 2:
             raise ValueError("ring must be [n_streams, ring_len]")
+        if out_len is not None and (ring.dim() != 3 or ring.shape[2] != 128):
+            raise ValueError("ring must be [n_streams, ring_frames, 128]")
+        out_len = out_len or (lambda n: n)
         rows = (L.VfChunk * max(1, len(table)))(*[L.VfChunk(*map(int, t)) for t in table])
-        kept = sum(max(0, int(t[1]) - int(t[2]) - int(t[3])) for t in table)
+        kept = sum(max(0, out_len(int(t[1])) - int(t[2]) - int(t[3])) for t in table)
         return ring, rows, torch.empty(kept, device=self.device)
 
     def _varlen_args(self, packed: torch.Tensor, lengths, dtype=torch.float32):

@@ -26,6 +26,9 @@ outputs are `BoxcarOverlapAdd(RestoreNet(ssr_model), 1, W, M)`'s.  That path has
 handler's peak normalisation either: the handler divides a whole segment by its peak, which a live stream only knows once it
 has ended.
 
+`StreamingVocoder` vocodes live mel streams the same way, chunk by chunk from device frame rings: each step is one
+vf_vocoder_chunks call (the geometry is vocoder.chunk_plan's, the composition its outputs equal vocoder.vocode_chunked).
+
 `WindowedStreamingRestorer` runs the reference's other long-form scheme, `WindowedOverlapAdd(RestoreNet(model, unify_energy),
 1, W, hop, window)` (longform.py, tools/dsp/overlapadd.py's LambdaOverlapAdd), incrementally the same way: windows of W
 samples every hop, each restored, multiplied by the synthesis window and overlap-added, so adjacent windows cross-fade.
@@ -40,6 +43,7 @@ import torch
 from .arch import frames_for, vocoder_out_len
 from .longform import BoxcarOverlapAdd, WindowedOverlapAdd
 from .model import SSR_UNet
+from .vocoder import check_chunking, chunk_plan
 
 OPEN = (1 << 63) - 1              # `valid` of a chunk whose stream is still open: no position reads as zero padding
 MAX_CHUNK = 1 << 30               # samples of one clip of vf_restore_varlen (engine.cu check_varlen_call)
@@ -72,9 +76,13 @@ class _Stream:
 
 
 class _RingStreams:
-    """The stream lifecycle and device ring shared by the streaming restorers: open / push / close bookkeeping, one ring row of
-    ring_len samples per stream.  A subclass says from which position a stream's samples are still needed (_keep_from)."""
+    """The stream lifecycle and device ring shared by the streaming restorers and the streaming vocoder: open / push / close
+    bookkeeping, one ring row of ring_len positions per stream, each position a sample (row shape ()) or a mel frame ((128,)).
+    A subclass says from which position a stream's input is still needed (_keep_from)."""
     _first = 0                    # _Stream.next of a new stream
+    _row = ()                     # the shape of one position
+    _push_what = "samples must be a 1-D float32 tensor"
+    _unit = "samples"
 
     def _init_model(self, model, unify_energy: bool, max_streams: int):
         if max_streams < 1:
@@ -87,7 +95,7 @@ class _RingStreams:
 
     def _init_ring(self, ring_len: int, max_streams: int):
         self.ring_len = ring_len
-        self.ring = torch.zeros(max_streams, ring_len, device=self.engine.device)
+        self.ring = torch.zeros(max_streams, ring_len, *self._row, device=self.engine.device)
         self._free = list(range(max_streams - 1, -1, -1))
         self._streams: Dict[int, _Stream] = {}
         self._ids = itertools.count()
@@ -112,14 +120,15 @@ class _RingStreams:
         raise NotImplementedError
 
     def push(self, sid: int, samples: torch.Tensor):
-        """Appends 1-D float32 samples (host or device) to stream `sid`'s ring."""
+        """Appends 1-D float32 samples (host or device) to stream `sid`'s ring (StreamingVocoder: [k, 128] mel frames)."""
         st = self._get(sid, "push")
-        if not isinstance(samples, torch.Tensor) or samples.dtype != torch.float32 or samples.dim() != 1:
-            raise TypeError(f"push: stream {sid}: samples must be a 1-D float32 tensor")
-        k, L = samples.numel(), self.ring_len
+        if (not isinstance(samples, torch.Tensor) or samples.dtype != torch.float32 or samples.dim() != 1 + len(self._row)
+                or tuple(samples.shape[1:]) != self._row):
+            raise TypeError(f"push: stream {sid}: {self._push_what}")
+        k, L = samples.shape[0], self.ring_len
         held = st.pushed - self._keep_from(st)
         if held + k > L:
-            raise OverflowError(f"push: stream {sid}: {k} samples do not fit its ring ({L - held} of {L} free); call step() first")
+            raise OverflowError(f"push: stream {sid}: {k} {self._unit} do not fit its ring ({L - held} of {L} free); call step() first")
         row, p = self.ring[st.slot], st.pushed % L
         first = min(k, L - p)
         row[p:p + first].copy_(samples[:first])
@@ -313,4 +322,99 @@ class WindowedStreamingRestorer(_RingStreams):
             st.next, st.emitted = nxt, end
             if st.n is not None:
                 self._release(sid)              # a closed stream's step adds its last windows and emits the rest
+        return out
+
+
+class StreamingVocoder(_RingStreams):
+    """Live mel streams - a TTS or voice-conversion model's output, a few frames at a time - vocoded chunk by chunk with
+    `margin_frames` frames of context on each side of every `window_frames` frames:
+
+        sv = StreamingVocoder(vocoder, window_frames=64, margin_frames=16)
+        a = sv.open()
+        sv.push(a, mel)                 # [k, 128] float32 linear mel frames, any k, any split, host or device
+        out = sv.step()                 # {id: the samples vocoded since the last step}
+        sv.close(a)                     # the rest comes out of the following step()
+
+    vocoder: a vocoder.Vocoder or a VoiceFixer (whose engine holds the vocoder) on a CUDA device with weights loaded.  W =
+    window_frames and M = margin_frames must be even, W >= 2, M >= 0.  The chunks and crops of a stream of T frames are
+    vocoder.chunk_plan(T, W, M)'s, so its concatenated outputs are vocoder.vocode_chunked(vocoder, mel, W, M) bit for bit,
+    vocoder_out_len(T) samples in all, however its pushes were split and whichever streams shared its steps:
+    vf_vocoder_chunks gives each chunk the bits of a one-mel forward on its frames.  A stream of at most W frames is one chunk,
+    forward(mel) itself; with M >= arch.vocoder_receptive_field(cfg) (576 frames for the default config) every kept frame has
+    the whole mel's context and the stream is forward(mel) on the whole mel.  A smaller M is an approximation whose error
+    falls as M grows (DESIGN.md 5).
+
+    Chunk i is vocoded once (i + 1) W + M frames have been pushed (with M = 0 one frame more: until then the stream could end
+    at (i + 1) W, and then chunk i is the last one and keeps the tail padding's samples); its range is then final whatever
+    the stream's length.  So the samples of frame t leave once M to W + M - 1 more frames have arrived after it (1 to W when
+    M = 0), and the remaining chunks of a closed stream in the next step().
+
+    Each stream owns one row of a device ring of 2 (W + 2M) frames.  After a step the ring holds fewer than W + 2M frames
+    still needed by the stream's next chunk (at most W when M = 0), so a push of up to W + 2M frames always fits; a push
+    that would overwrite needed frames raises OverflowError, and the caller must step() first.  Each step is one
+    vf_vocoder_chunks call: per sub-batch one gather launch writes the chunks' frames from the rings straight into the
+    vocoder plan and one crop launch reads the kept samples straight out of it, whatever the number of streams."""
+    _row = (128,)
+    _push_what = "mel must be a [k, 128] float32 tensor"
+    _unit = "frames"
+
+    def __init__(self, vocoder, window_frames: int, margin_frames: int, max_streams: int = 64):
+        W, M = check_chunking(window_frames, margin_frames)
+        if max_streams < 1:
+            raise ValueError("max_streams must be at least 1")
+        self.engine = vocoder._engine()
+        self.voc_cfg = self.engine.voc_cfg
+        self.window_frames, self.margin_frames = W, M
+        self._init_ring(2 * (W + 2 * M), max_streams)
+
+    def _keep_from(self, st: _Stream) -> int:
+        """First absolute frame the stream's next chunk reads."""
+        return max(0, st.next * self.window_frames - self.margin_frames)
+
+    def _ready_chunks(self, st: _Stream) -> List[Tuple[int, int, int, int]]:
+        """The chunks of an open stream whose range and crops are final whatever its length: chunk i once (i + 1) W + M
+        frames are in (and more than (i + 1) W, so that it cannot be the last one), as chunk_plan gives it then."""
+        W, M, hop = self.window_frames, self.margin_frames, self.voc_cfg.hop
+        out = []
+        i = st.next
+        while st.pushed >= (i + 1) * W + max(M, 1):
+            s = max(0, i * W - M)
+            length = (i + 1) * W + M - s
+            out.append((s, length, (i * W - s) * hop, vocoder_out_len(length, self.voc_cfg) - ((i + 1) * W - s) * hop))
+            i += 1
+        return out
+
+    def close(self, sid: int):
+        """Ends stream `sid`; its remaining samples come out of the next step()."""
+        st = self._get(sid, "close")
+        st.n = st.pushed
+        if st.n == 0:                           # nothing was pushed: nothing to vocode
+            self._release(sid)
+
+    def step(self) -> Dict[int, torch.Tensor]:
+        """Vocodes every ready chunk of every stream in one vf_vocoder_chunks call -> {id: 1-D device tensor of the samples
+        vocoded since the last step} for the streams that have any.  A closed stream is gone once its last samples are out."""
+        table, owners = [], []
+        for sid, st in self._streams.items():
+            if st.n is None:
+                chunks = self._ready_chunks(st)
+            else:
+                chunks = chunk_plan(st.n, self.window_frames, self.margin_frames, self.voc_cfg)[st.next:]
+            valid = OPEN if st.n is None else st.n
+            for start, length, cl, cr in chunks:
+                table.append((st.slot, length, cl, cr, start, valid))
+            if chunks:
+                n_kept = sum(vocoder_out_len(length, self.voc_cfg) - cl - cr for _, length, cl, cr in chunks)
+                owners.append((sid, len(chunks), n_kept))
+        if not table:
+            return {}
+        kept = self.engine.vocoder_chunks(self.ring, table)
+        out, off = {}, 0
+        for sid, n_chunks, n_kept in owners:
+            out[sid] = kept[off:off + n_kept]
+            off += n_kept
+            st = self._streams[sid]
+            st.next += n_chunks
+            if st.n is not None:
+                self._release(sid)              # a closed stream's step emits all its remaining chunks
         return out

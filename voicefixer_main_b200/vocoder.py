@@ -8,6 +8,9 @@
       .resynth_batch([wav_i]) -> [out_i]                     vocoder resynthesis of clips of different lengths
       .oracle(fpath, out_path, cuda=True) / .oracle_batch([(fpath, out_path)])
 
+Live mel streams (a TTS or voice-conversion model's frames, a few at a time) are vocoded chunk by chunk by
+streaming.StreamingVocoder; chunk_plan holds its geometry and vocode_chunked the composition its outputs equal.
+
 Its engine holds the vocoder and the built-in mel filterbank (model.melscale_fbanks) only: no restorer checkpoint and no
 analysis network is needed, and the plans hold the vocoder's buffers only (vf_vocoder_varlen, vf_resynth_varlen).
 model.Vocoder, the restorer's own `model.vocoder`, is a view onto a VoiceFixer's engine and stays as it is.
@@ -21,7 +24,7 @@ the GPU), cut into handler()'s 60 s segments, and each segment is resynthesised 
 normalise -> trim_center) and written as 16-bit PCM by save_wave.  It is the usual upper bound when scoring a restorer:
 what is left of a clean file after the vocoder alone.
 """
-from typing import List, Sequence
+from typing import List, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -54,6 +57,46 @@ def length_groups(frames: Sequence[int]) -> List[List[int]]:
         else:
             groups.append([i])
     return groups
+
+
+def check_chunking(window_frames: int, margin_frames: int):
+    """The chunk geometry's argument check: W >= 2 and M >= 0, both even (so every chunk's length has the parity of the
+    whole mel, and the chunks' outputs add up to its output length)."""
+    W, M = int(window_frames), int(margin_frames)
+    if W < 2 or W % 2:
+        raise ValueError(f"window_frames must be even and at least 2 (got {W})")
+    if M < 0 or M % 2:
+        raise ValueError(f"margin_frames must be even and at least 0 (got {M})")
+    return W, M
+
+
+def chunk_plan(T: int, window_frames: int, margin_frames: int, cfg: VocoderConfig = None) -> List[Tuple[int, int, int, int]]:
+    """The chunks that vocode a mel of T frames with W = window_frames frames kept per chunk and M = margin_frames frames of
+    context on each side: (start, length, crop_left, crop_right) per chunk, start and length in frames, the crops in samples
+    of the chunk's vocoder_out_len(length) output.  Chunk i (i < ceil(T / W)) reads frames [s, e), s = max(0, i W - M), e =
+    min(T, (i + 1) W + M), and keeps its samples [(i W - s) hop, (min(T, (i + 1) W) - s) hop); the last chunk keeps everything
+    from (i W - s) hop to the end of its output, the vocoder's tail padding included.  The kept samples add up to
+    vocoder_out_len(T), forward's length.  T = 0 has no chunks."""
+    cfg = cfg or VocoderConfig()
+    W, M = check_chunking(window_frames, margin_frames)
+    n = -(-int(T) // W)
+    out = []
+    for i in range(n):
+        s, e = max(0, i * W - M), min(T, (i + 1) * W + M)
+        right = 0 if i == n - 1 else vocoder_out_len(e - s, cfg) - ((i + 1) * W - s) * cfg.hop
+        out.append((s, e - s, (i * W - s) * cfg.hop, right))
+    return out
+
+
+def vocode_chunked(vocoder, mel: torch.Tensor, window_frames: int, margin_frames: int) -> torch.Tensor:
+    """The reference composition of a chunked stream: chunk_plan(T, W, M)'s chunks of mel [T, 128], each through
+    vocoder.forward on its torch slice alone, cropped and concatenated.  A StreamingVocoder stream's outputs are these bits."""
+    cfg = getattr(vocoder, "voc_cfg", None) or VocoderConfig()
+    kept = []
+    for s, length, left, right in chunk_plan(int(mel.shape[0]), window_frames, margin_frames, cfg):
+        out = vocoder.forward(mel[s:s + length][None, None])[0, 0]
+        kept.append(out[left:out.numel() - right])
+    return torch.cat(kept) if kept else mel.new_zeros(0)
 
 
 def _grouped(frames, items, call, out_len):
