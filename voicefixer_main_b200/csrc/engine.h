@@ -21,7 +21,7 @@
 
 namespace vf {
 cudaError_t launch_gemm_tc(const GemmTcParams& p, int bn, int bk, cudaStream_t stream);
-size_t gemm_tc_smem_bytes(int bn, int bk, int stages, int terms, int tile_chunks, int resid_tma);
+size_t gemm_tc_smem_bytes(int bn, int bk, int stages, int terms, int tile_chunks, int stg_warp, int resid_tma);
 int gemm_tc_max_bn(int terms);
 cudaError_t launch_pair_tc(const PairParams& p, cudaStream_t stream);
 size_t pair_tc_smem_bytes(int C);

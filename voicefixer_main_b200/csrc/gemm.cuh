@@ -120,9 +120,13 @@ struct GemmTcParams {
   CUtensorMap b_hi, b_lo;         // [Ktot, N] fp16 (K-major)
   CUtensorMap i_res;              // epilogue residual by TMA load (MAP_PLAIN only): fp32 [resid_ld, rows_in, n_img] box 32 x 32 x 1
                                   // SWIZZLE_128B (3-term), or fp16 planes [resid_ld, rows_in, n_img, 2] box 32 x 32 x 1 x 2 SWIZZLE_64B
-  int resid_tma;                  // residual tiles in flight per epilogue warp (4 KB and an mbarrier each): 1 or 2; 0 without a residual
+                                  // (3-term) / box min(BN, 64) x 16 x 1 x 2 (hi-only: one warp's fragment rows, gemm_tc.cu)
+  int resid_tma;                  // separate residual tiles in flight per 3-term epilogue warp (4 KB and an mbarrier each): 1 or 2;
+                                  // 0 without a residual and in hi-only kernels (the residual lands in the staging tile)
+  int stg_warp;                   // staging bytes per epilogue warp: 4096, or 16 rows x BN x planes fp16 for a hi-only MAP_PLAIN layer
   CUtensorMap o_raw;              // MAP_PLAIN epilogue TMA stores: fp32 [raw_ld, rows, n_img], box 32 x 32 x 1, SWIZZLE_128B
-  CUtensorMap o_r, o_a;           // fp16 [ld, rows, n_img, planes], box 32 x 32 x 1 x planes, SWIZZLE_64B (o_a: also see tma_out)
+  CUtensorMap o_r, o_a;           // fp16 [ld, rows, n_img, planes], box 32 x 32 x 1 x planes, SWIZZLE_64B (o_a: also see tma_out);
+                                  // hi-only MAP_PLAIN: box min(BN, 64) x 16 x 1 x planes, as i_res
   int stages;
   int tile_chunks; // BK-wide K chunks per output tile
   int seg_chunks;  // 3-term mode: chunks per accumulation segment (promotion to registers in between)

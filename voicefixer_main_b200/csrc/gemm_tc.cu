@@ -17,7 +17,8 @@
 // against the stacked [B_hi; B_lo] tile, lo*hi is a second MMA of width BN into the correction half, so the two small
 // correction products never mix into the main chain.
 //
-// Epilogue I/O.  A thread owns a row; a warp's 32 rows x 32 columns pass through its swizzled shared-memory staging tile.
+// Epilogue I/O.  Hi-only MAP_PLAIN layers finish the accumulator in its fragment layout, in place in the warp's staging tile
+// (see f_word below).  Every other layer: a thread owns a row; a warp's 32 rows x 32 columns pass through its swizzled shared-memory staging tile.
 // Residual tiles arrive there by TMA load, and MAP_PLAIN outputs leave by TMA store.  The transposed convs scatter their
 // rows, so the whole warp stores them row-major from the staging tile, every STG touching whole 64-byte row segments.
 // The accumulator fragments reach the row-per-thread layout through the same staging tiles (64 columns of the warp
@@ -127,9 +128,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
   constexpr int A_BOX_BYTES = GEMM_BM * ROW_BYTES;      // bytes one A TMA box delivers: a whole number of 1 KB swizzle atoms
   constexpr int off_b = (THREE ? 2 : 1) * A_BOX_BYTES;   // [A_hi][A_lo] in 3-term mode, A_hi alone otherwise
   constexpr int stage_bytes = off_b + B_SLOT;
-  uint8_t* stg_base = smem + (size_t)stages * stage_bytes;          // EPI_WARPS x 4 KB staging
-  uint8_t* rstg_base = stg_base + EPI_WARPS * 4096;                  // resid_tma: EPI_WARPS x 4 KB residual tiles (TMA destination)
-  uint8_t* tail = rstg_base + (size_t)P.resid_tma * EPI_WARPS * 4096;  // P.resid_tma = tiles in flight per warp (0, 1 or 2)
+  uint8_t* stg_base = smem + (size_t)stages * stage_bytes;          // EPI_WARPS x 4 KB (hi-only: P.stg_warp) staging
+  uint8_t* rstg_base = stg_base + EPI_WARPS * (THREE ? 4096 : P.stg_warp);   // 3-term: EPI_WARPS x 4 KB residual tiles (TMA destination)
+  uint8_t* tail = rstg_base + (size_t)(THREE ? P.resid_tma : 0) * EPI_WARPS * 4096;   // P.resid_tma = tiles in flight per warp (0, 1 or 2)
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(tail);
   uint64_t* empty_bar = full_bar + stages;
   uint64_t* resid_bar = empty_bar + stages;              // [8][2] per epilogue warp and ring slot: the residual tile has landed
@@ -222,7 +223,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     const int wq = ew & 3;              // warp inside its group: fragment rows [16 wq, 16 wq + 16) of the group's 64
     const int q = 2 * wg + (wq & 1);    // row quarter of the tile this warp's epilogue owns
     const int half = wq >> 1;           // which column chunk of each 64-column round it takes
-    float4* stg_f = reinterpret_cast<float4*>(stg_base) + (size_t)ew * 256;            // 4 KB per warp
+    const int stg_warp = THREE ? 4096 : P.stg_warp;    // staging bytes per epilogue warp
+    float4* stg_f = reinterpret_cast<float4*>(stg_base) + (size_t)ew * (stg_warp / 16);
     uint4* stg_h = reinterpret_cast<uint4*>(stg_f);                                    // halves alias the same 4 KB
     uint4* stg_l = stg_h + 128;
     RowInfo* rows = s_rows + ew * 32;
@@ -268,7 +270,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
     // requests run P.resid_tma (1 or 2) chunks ahead ACROSS tiles: a warp's chunk sequence is known up front (persistent tile
     // loop), and a request issued only at the start of its own tile exposes one HBM round trip per tile (ncu on voc.res2.*.b:
     // 4.8 us per 2-chunk tile, every unit below 62 %).
-    const int resid_ring = P.resid_tma;
+    const int resid_ring = THREE ? P.resid_tma : 0;
     uint8_t* rstg = rstg_base + (size_t)ew * resid_ring * 4096;
     uint64_t* rbar = resid_bar + ew * 2;
     uint32_t r_cons = 0, r_issued = 0;       // chunks consumed / requested by this warp
@@ -287,8 +289,27 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       pf_j += CHUNK_STEP;
       if (pf_j >= BN / 32) { pf_j = half; pf_tile += gridDim.x; }
     };
-    if (half < BN / 32)
+    if (THREE && half < BN / 32)
       for (int i = 0; i < resid_ring; ++i) issue_resid();
+    // Hi-only MAP_PLAIN layers finish the accumulator in its fragment layout: the warp's 16 rows x BN columns go through its
+    // staging tile as BN / FBW boxes of [plane][16 rows][FBW fp16 columns] (SWIZZLE_128B for 64 columns, SWIZZLE_64B for
+    // 32).  The tile's residual planes arrive there by TMA while its MMAs run, each thread rewrites the words it has read
+    // with its outputs, and the boxes leave by TMA store.  The thread's word of columns 8 k + 2 (lane & 3) (+1), fragment row
+    // lane / 4 + 8 hh, plane p, is f_off[hh] + box * f_box + p * F_PLANE + ((k % (FBW / 8)) << 4 ^ f_sw), worked out once (the
+    // empty asm keeps the offsets in registers instead of being worked out again at every use).
+    constexpr int FBW = BN < 64 ? BN : 64, F_PLANE = 16 * FBW * 2;
+    const int f_box = stg_warp / (BN / FBW);
+    uint32_t f_off[2], f_sw = (uint32_t)(FBW == 64 ? (lane >> 2) & 7 : (lane >> 3) & 3) << 4;
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) f_off[hh] = (uint32_t)(((lane >> 2) + 8 * hh) * FBW * 2 + 4 * (lane & 3));
+    if constexpr (!THREE) asm volatile("" : "+r"(f_off[0]), "+r"(f_off[1]), "+r"(f_sw));
+    uint8_t* const f_tile = stg_base + (size_t)ew * stg_warp;
+    auto f_word = [&](const int i, const int p) -> uint32_t* {     // the word of fragment elements i, i + 1 in plane p
+      const int k = i >> 2;
+      return reinterpret_cast<uint32_t*>(f_tile + (k / (FBW / 8)) * f_box + p * F_PLANE + f_off[(i >> 1) & 1] +
+                                         ((uint32_t)((k % (FBW / 8)) << 4) ^ f_sw));
+    };
+    uint32_t f_par = 0;                  // parity of the warp's residual barrier
     int prev_n0 = -1, s = 0;            // operand ring slot and its phase bit (the same sequence the producer walks)
     uint32_t ph = 0;
     float amax = 0.f;
@@ -320,16 +341,29 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       uint32_t orow = 0, flags = 0;
       // MAP_PLAIN (everything but the transposed convs): output rows follow the GEMM rows, and the TMA stores clip the rows
       // past rows_in; only the pad flag is needed
-      if (map == MAP_PLAIN) {
+      if (THREE && map == MAP_PLAIN) {
         if (row_ok) flags = kRowValid | (((Wp > 0 && (r % Wp) == Wp - 1) || r >= valid_rows(e.row_valid, img)) ? kRowPad : 0);
       } else if (map == MAP_CONVT2D) {
         cth = r / Wp;
         ctw = r - cth * Wp;
       }
+      // hi-only MAP_PLAIN: the flags of the thread's two fragment rows, worked out before the MMAs hide the row_valid load
+      const int frow = m0 + 64 * wg + 16 * wq;   // first of the warp's 16 GEMM rows
+      bool f_ok[2] = {false, false}, f_pad[2] = {false, false}, f_live = false;
+      if (!THREE && map == MAP_PLAIN) {
+        f_live = !tile_is_empty(e, img, m0);     // an empty tile issues no residual load and stores zeros
+        const int vrows = valid_rows(e.row_valid, img);
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int rr = frow + (lane >> 2) + 8 * hh;
+          f_ok[hh] = rr < rows_in;
+          f_pad[hh] = f_ok[hh] && ((Wp > 0 && (rr % Wp) == Wp - 1) || rr >= vrows);
+        }
+      }
       // store this warp's staged 32 rows x 32 columns of fp16 (hi [+ lo]): by TMA through the map `tm` of a MAP_PLAIN output,
       // else row-major to the rows published in `rows`, 8 rows x 64 B per instruction
       auto store_rows_h = [&](const OutPlane& op, const int co0, const bool two, const CUtensorMap* tm) {
-        if (map == MAP_PLAIN) {           // staged tile(s) -> TMA store; rows past rows_in are clipped by the tensor map
+        if (THREE && map == MAP_PLAIN) {  // staged tile(s) -> TMA store; rows past rows_in are clipped by the tensor map
           fence_proxy_async();
           __syncwarp();
           if (lane == 0) {
@@ -403,7 +437,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           __syncwarp();                   // every lane has read the tile: it may be refilled
           issue_resid();                  // the slot just read is free again: request the chunk `resid_ring` ahead
         }
-        if (has_resid_planes) {
+        if (THREE && has_resid_planes) {
           const uint32_t slot = r_cons & (uint32_t)(resid_ring - 1);
           if (ok && !mbar_wait(rbar + slot, (r_cons >> (resid_ring >> 1)) & 1u, e.err, ERR_PIPE_EPILOGUE)) ok = false;
           ++r_cons;
@@ -559,6 +593,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           }
           wgmma_commit();
           started = 1;
+          if (!THREE && ci == 0 && map == MAP_PLAIN && has_resid_planes) {   // the warp's residual planes, under the tile's MMAs
+            stg_release();                // the previous tile's stores have read the staging tile
+            if (lane == 0) {
+              mbar_expect_tx(rbar, BN * 64);                                    // 16 rows x BN columns x 2 planes of fp16
+#pragma unroll
+              for (int b = 0; b < BN / FBW; ++b)
+                tma_load_4d(f_tile + b * f_box, &P.i_res, rbar, n0 + b * FBW, m0 + 64 * wg + 16 * wq, img, 0);
+            }
+          }
           const bool close_seg = THREE ? (--left_in_seg == 0) : (ci + 1 == tile_chunks);
           // the group of the previous chunk has completed: its slot may be refilled (and this one at a segment's end)
           if (close_seg) {
@@ -588,6 +631,90 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
         }
         wgmma_wait<0>();                  // already drained at the tile's last chunk; states it for the compiler
         wgmma_fence_regs(acc, ACC_N / 2);
+      }
+      if (!THREE && map == MAP_PLAIN) {
+        // ---- hi-only MAP_PLAIN epilogue on the fragments: per element the arithmetic of process_chunk, in its order.  Each
+        // branch on the layer's configuration encloses a whole loop over the fragment: no branch per element.
+        const bool f_resid = has_resid_planes && f_live;
+        if (f_resid && ok && !mbar_wait(rbar, f_par, e.err, ERR_PIPE_EPILOGUE)) ok = false;
+        f_par ^= f_resid ? 1u : 0u;
+        auto bias2 = [&](const int i) { return *reinterpret_cast<const float2*>(s_bias + 8 * (i >> 2) + 2 * (lane & 3)); };
+        if (f_resid) {
+#pragma unroll
+          for (int i = 0; i < BN / 2; i += 2) {
+            float v0 = acc[i], v1 = acc[i + 1];
+            const float2 b2 = bias2(i);
+            if (has_bias) { v0 += b2.x; v1 += b2.y; }
+            add_planes(v0, v1, *f_word(i, 0), *f_word(i, 1), resid_ar);
+            const bool pad = f_pad[(i >> 1) & 1];
+            acc[i] = pad ? 0.f : v0; acc[i + 1] = pad ? 0.f : v1;
+          }
+        } else {
+#pragma unroll
+          for (int i = 0; i < BN / 2; i += 2) {
+            float v0 = acc[i], v1 = acc[i + 1];
+            const float2 b2 = bias2(i);
+            if (has_bias) { v0 += b2.x; v1 += b2.y; }
+            const bool pad = f_pad[(i >> 1) & 1];
+            acc[i] = pad ? 0.f : v0; acc[i + 1] = pad ? 0.f : v1;
+          }
+        }
+        stg_release();                    // the previous tile's stores have read the staging tile
+        // boxes of the staging tile -> TMA store through `tm` (rows past rows_in are clipped by the tensor map)
+        auto store_boxes = [&](const CUtensorMap* tm, const int c_off) {
+          fence_proxy_async();
+          __syncwarp();
+          if (lane == 0) {
+#pragma unroll
+            for (int b = 0; b < BN / FBW; ++b) tma_store_4d(tm, f_tile + b * f_box, c_off + n0 + b * FBW, e.out_row0 + frow, img, 0);
+            tma_store_commit();
+          }
+          st_pending = true;
+        };
+        if (want_r) {                     // raw hi/lo planes, over the residual words each thread has read
+#pragma unroll
+          for (int i = 0; i < BN / 2; i += 2) {
+            const __half2 h2 = __floats2half2_rn(acc[i], acc[i + 1]);
+            const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h2);
+            *f_word(i, 0) = hb;
+            *f_word(i, 1) = residual_h2(acc[i], acc[i + 1], hb);
+          }
+          store_boxes(&P.o_r, e.out_r.c_off);
+        }
+        if (want_a) {                     // activated planes: (a, r) or the hi plane
+          stg_release();                  // the raw planes' store has read the tile
+          // the hi plane of activated values: pad rows to zero, |value| into amax on rows inside the image
+          auto put_hi = [&](const int i, float v0, float v1) {
+            const int hh = (i >> 1) & 1;
+            if (f_pad[hh]) { v0 = 0.f; v1 = 0.f; }
+            if (f_ok[hh]) amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
+            const __half2 h2 = __floats2half2_rn(v0, v1);
+            *f_word(i, 0) = *reinterpret_cast<const uint32_t*>(&h2);
+          };
+          if (out_ar) {
+#pragma unroll
+            for (int i = 0; i < BN / 2; i += 2) {
+              const float v0 = acc[i], v1 = acc[i + 1];
+              if (f_ok[(i >> 1) & 1]) amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
+              uint32_t ab, rb;
+              ar_split(v0, v1, fmaxf(v0, v0 * slope), fmaxf(v1, v1 * slope), out_ar, ab, rb);
+              *f_word(i, 0) = ab;
+              *f_word(i, 1) = rb;
+            }
+          } else if (act == ACT_LRELU) {
+#pragma unroll
+            for (int i = 0; i < BN / 2; i += 2) put_hi(i, fmaxf(acc[i], acc[i] * slope), fmaxf(acc[i + 1], acc[i + 1] * slope));
+          } else if (act == ACT_ELU) {
+#pragma unroll
+            for (int i = 0; i < BN / 2; i += 2)
+              put_hi(i, acc[i] > 0.f ? acc[i] : expm1f(acc[i]), acc[i + 1] > 0.f ? acc[i + 1] : expm1f(acc[i + 1]));
+          } else {
+#pragma unroll
+            for (int i = 0; i < BN / 2; i += 2) put_hi(i, acc[i], acc[i + 1]);
+          }
+          store_boxes(&P.o_a, e.out_a.c_off);
+        }
+        continue;
       }
       // ---- accumulator fragments -> row-per-thread chunks, 64 columns per round through the group's staging tiles
       const float* fin = THREE ? tot : acc;
@@ -627,15 +754,15 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 }
 
 // ---------------------------------------------------------------------------------------------- host side
-size_t gemm_tc_smem_bytes(int bn, int bk, int stages, int terms, int tile_chunks, int resid_tma) {
+size_t gemm_tc_smem_bytes(int bn, int bk, int stages, int terms, int tile_chunks, int stg_warp, int resid_tma) {
   const size_t stage = (size_t)(terms == 3 ? 2 : 1) * (GEMM_BM + bn) * bk * 2;
-  return stages * stage + EPI_WARPS * 4096 * (1 + resid_tma) + (2 * stages + 16) * 8 + (3 * bn + 32) * 4 + EPI_WARPS * 32 * 8 +
+  return stages * stage + EPI_WARPS * ((size_t)stg_warp + 4096 * resid_tma) + (2 * stages + 16) * 8 + (3 * bn + 32) * 4 + EPI_WARPS * 32 * 8 +
          (size_t)tile_chunks * 16 + 1024;
 }
 
 template <int BN, int BK, bool THREE>
 static cudaError_t launch_cfg(const GemmTcParams& p, cudaStream_t stream) {
-  const size_t smem = gemm_tc_smem_bytes(BN, BK, p.stages, p.prob.terms, p.tile_chunks, p.resid_tma);
+  const size_t smem = gemm_tc_smem_bytes(BN, BK, p.stages, p.prob.terms, p.tile_chunks, p.stg_warp, p.resid_tma);
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<BN, BK, THREE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);

@@ -47,10 +47,12 @@ int map_weights(vf_ctx* ctx, CUtensorMap* m, const GemmW& W, const __half* pl, i
   const cuuint32_t box[3] = {(cuuint32_t)box_k, (cuuint32_t)box_n, 2};
   return encode_map(ctx, m, both ? 3 : 2, 2, pl, dims, strides, box, box_k == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B);
 }
-// epilogue TMA stores: fp16 plane(s) [ld, rows, image, plane], box 32 channels x 32 rows x 1 x planes
-int map_out_planes(vf_ctx* ctx, CUtensorMap* m, const __half* hi, const __half* lo, int planes, int ld, int rows, size_t img_rows, int n_img) {
+// epilogue TMA loads / stores: fp16 plane(s) [ld, rows, image, plane], box box_c channels x box_rows rows x 1 x planes
+// (3-term: 32 x 32, a warp's rows of one column chunk; hi-only: min(BN, 64) x 16, a warp's fragment rows, gemm_tc.cu)
+int map_out_planes(vf_ctx* ctx, CUtensorMap* m, const __half* hi, const __half* lo, int planes, int ld, int rows, size_t img_rows, int n_img,
+                   int box_c, int box_rows) {
   const size_t pstride = planes == 2 ? (size_t)(lo - hi) : (size_t)n_img * img_rows * ld;
-  return map_rows(ctx, m, hi, 2, ld, rows, img_rows, n_img, 32, 32, planes, pstride);
+  return map_rows(ctx, m, hi, 2, ld, rows, img_rows, n_img, box_c, box_rows, planes, pstride);
 }
 // activated planes of a transposed 1-D conv: output row t = s * q + p as [ld, p, q, image, plane], box 32 x 1 x 32 x 1 x planes
 int map_convt1d_out(vf_ctx* ctx, CUtensorMap* m, const __half* hi, const __half* lo, int planes, int ld, int s, long L, int n_img) {
@@ -174,12 +176,6 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
     // occupancy: small-K tiles are bound by loads/stores -> several persistent CTAs per SM; large-K -> one
     // one persistent CTA of 384 threads per SM (the accumulators take the register file): the deepest operand ring that fits
     const size_t smem_cap = (size_t)227 * 1024 - 1024;
-    auto fit = [&](int ring) {
-      int st = 8;
-      for (; st >= 2; --st)
-        if (gemm_tc_smem_bytes(bn, bk, st, terms, tp.tile_chunks, ring) <= smem_cap) break;
-      return st;
-    };
     // The residual and the fp32 output follow the GEMM rows, which only MAP_PLAIN layers store in order (gemm_tc.cu).
     GemmEpilogue& pe = pr.epi;
     const bool has_resid = pe.resid || pe.resid_hi;
@@ -188,9 +184,20 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
       return;
     }
     if (pe.resid && pe.resid_hi) { rc = fail(ctx, VF_EINVAL, "GEMM with both an fp32 and a hi/lo residual"); return; }
-    // The epilogue reads its residual by TMA, one or two 4 KB tiles per epilogue warp requested that many chunks ahead:
-    // two where the operand ring keeps its depth.
-    tp.resid_tma = has_resid ? 1 : 0;
+    // Staging per epilogue warp: a hi-only MAP_PLAIN layer finishes its accumulator fragments in place, 16 rows x BN columns
+    // in as many fp16 planes as its residual or widest output has; every other layer passes 32 x 32 fp32 through 4 KB.
+    const bool frag = terms == 1 && pe.map == MAP_PLAIN;
+    const int fbw = std::min(bn, 64);
+    tp.stg_warp = frag ? 16 * bn * 2 * ((has_resid || pe.out_r.hi || pe.out_ar) ? 2 : 1) : 4096;
+    auto fit = [&](int ring) {
+      int st = 8;
+      for (; st >= 2; --st)
+        if (gemm_tc_smem_bytes(bn, bk, st, terms, tp.tile_chunks, tp.stg_warp, ring) <= smem_cap) break;
+      return st;
+    };
+    // The 3-term epilogue reads its residual by TMA, one or two 4 KB tiles per epilogue warp requested that many chunks
+    // ahead: two where the operand ring keeps its depth.  The hi-only one reads it into its staging tile.
+    tp.resid_tma = (has_resid && !frag) ? 1 : 0;
     int stages = fit(tp.resid_tma);
     if (tp.resid_tma) {
       const int st2 = fit(2);
@@ -198,9 +205,11 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
     }
     if (stages < 2) { rc = fail(ctx, VF_EINVAL, "no wgmma tile configuration fits (bn=%d bk=%d terms=%d)", bn, bk, terms); return; }
     tp.stages = stages;
-    if (tp.resid_tma) {
+    // TMA boxes of the epilogue's fp16 planes: a warp's 16 fragment rows x min(BN, 64) columns (hi-only MAP_PLAIN), else 32 x 32
+    const int box_c = frag ? fbw : 32, box_rows = frag ? 16 : 32;
+    if (has_resid) {
       if (pe.resid) rc = map_rows(ctx, &tp.i_res, pe.resid, 4, pe.resid_ld, pe.rows_in, (size_t)pe.rows_in, n_img, 32, 32);
-      else rc = map_out_planes(ctx, &tp.i_res, pe.resid_hi, pe.resid_lo, 2, pe.resid_ld, pe.rows_in, (size_t)pe.rows_in, n_img);
+      else rc = map_out_planes(ctx, &tp.i_res, pe.resid_hi, pe.resid_lo, 2, pe.resid_ld, pe.rows_in, (size_t)pe.rows_in, n_img, box_c, box_rows);
       if (rc) return;
     }
     // Every MAP_PLAIN output leaves the epilogue's staging tiles by TMA store (gemm_tc.cu), and so does the activated output
@@ -220,11 +229,12 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
         if (rc) return;
       }
       if (pe.out_r.hi) {
-        rc = map_out_planes(ctx, &tp.o_r, pe.out_r.hi, pe.out_r.lo, 2, pe.out_r.ld, orows, (size_t)pe.out_img_rows, n_img);
+        rc = map_out_planes(ctx, &tp.o_r, pe.out_r.hi, pe.out_r.lo, 2, pe.out_r.ld, orows, (size_t)pe.out_img_rows, n_img, box_c, box_rows);
         if (rc) return;
       }
       if (pe.out_a.hi) {
-        rc = map_out_planes(ctx, &tp.o_a, pe.out_a.hi, pe.out_a.lo, (terms == 3 || pe.out_ar) ? 2 : 1, pe.out_a.ld, orows, (size_t)pe.out_img_rows, n_img);
+        rc = map_out_planes(ctx, &tp.o_a, pe.out_a.hi, pe.out_a.lo, (terms == 3 || pe.out_ar) ? 2 : 1, pe.out_a.ld, orows, (size_t)pe.out_img_rows, n_img,
+                            box_c, box_rows);
         if (rc) return;
       }
     }
