@@ -483,12 +483,11 @@ VF_API int vf_workspace_bytes(vf_ctx* ctx, int batch, int64_t n_samples, size_t*
 /* Synchronises `stream`, reads and clears the sticky device flags.  VF_OK, VF_EDEVICE or VF_EASSERT. */
 VF_API int vf_check_errors(vf_ctx* ctx, void* stream);
 
-/* Options: "vocoder_terms" (1 or 3 fp16 split terms; "unet_terms" accepts only 3), "unify_energy" (default flag of
+/* Options: "vocoder_terms" (1 or 3 fp16 split terms), "unify_energy" (default flag of
  * vf_restore / vf_restore_host; prefer vf_restore_ex's per-call flag), "plan_cache_mb" (cap on the device memory
  * held by cached per-shape plans, least recently used evicted first; 0 = half of the free device memory),
  * "graphs" (default 1: the fixed-pointer launch chain of a plan is captured on its second use and replayed as one CUDA graph from then on),
- * "host_pipeline" (default 1, see vf_restore_host),
- * "validate_simt" (1: run every GEMM on the SIMT validation kernel instead of the wgmma kernel - tests only). */
+ * "host_pipeline" (default 1, see vf_restore_host). */
 VF_API int vf_set_option(vf_ctx* ctx, const char* key, int value);
 /* Plans are cached per (path, batch, frames) - vf_restore_varlen and vf_ssr_restore_varlen: (path, batch, bucket) - ; the cache is bounded (see "plan_cache_mb").  A batch whose plan would not fit
  * the budget is processed in sub-batches through a smaller plan (same results: rows are independent); the *_stages accessors
@@ -519,10 +518,9 @@ VF_API int vf_op_info(vf_ctx* ctx, int i, float* ms, double* flops, double* byte
  * before the launch, so what the layer must not touch comes back unchanged. */
 enum { VF_LAYER_CONV2D = 0, VF_LAYER_CONVT2D = 1, VF_LAYER_CONV1D = 2, VF_LAYER_CONVT1D = 3, VF_LAYER_PAIR = 4,
        VF_LAYER_LINEAR = 5 };
-enum { VF_LAYER_PRODUCT = 0, VF_LAYER_SIMT = 1 };
 enum { VF_RESID_NONE = 0, VF_RESID_FP32 = 1, VF_RESID_PLANES = 2, VF_RESID_AR = 3 };
 typedef struct vf_layer_case {
-  int kind, impl, terms;    /* VF_LAYER_*, VF_LAYER_PRODUCT / SIMT (no (a, r) support: VF_EINVAL), 1 or 3 */
+  int kind, terms;          /* VF_LAYER_*, 1 or 3 */
   int n_img;
   int H, W;                 /* CONV2D / CONVT2D input pixels; GEMM rows per image H * (W + 1) */
   int L;                    /* CONV1D / CONVT1D / PAIR input rows per image */

@@ -252,7 +252,7 @@ def run_deep(eng, name, sms):
     make, claims = DEEP_BY_NAME[name]
     c = make(sms)
     t0, p0 = time.perf_counter(), time.process_time()
-    worst, rep = run_and_check(eng, c, 0)
+    worst, rep = run_and_check(eng, c)
     wall, cpu = time.perf_counter() - t0, time.process_time() - p0
     REPORTS[name] = (c, rep)
     return c, rep, worst, claims, wall, cpu

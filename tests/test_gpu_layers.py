@@ -224,15 +224,15 @@ def _ptr(a):
     return None if a is None else a.ctypes.data_as(ctypes.c_void_p)
 
 
-def build(c, impl):
+def build(c):
     """Inputs, the ctypes case and the float64 expectations of case c."""
     g = _rng(c["name"])
     b = Built()
     kind, terms, n = c["kind"], c.get("terms", 1), c.get("n_img", 1)
     cin, cout = c.get("cin", 64), c.get("cout", 64)
-    b.c, b.n, b.terms, b.impl = c, n, terms, impl
+    b.c, b.n, b.terms = c, n, terms
     lc = VL.VfLayerCase()
-    lc.kind, lc.impl, lc.terms, lc.n_img = kind, impl, terms, n
+    lc.kind, lc.terms, lc.n_img = kind, terms, n
     lc.cin, lc.cout = cin, cout
     keep = []                                     # host arrays the case points at
     rv = c.get("row_valid")
@@ -559,22 +559,22 @@ def check_sentinels(name, what, bits, mask, sentinel):
                               "touched outside" if written[tuple(bad[0])] else "not written inside"))
 
 
-def run_and_check(eng, c, impl):
-    b = build(c, impl)
+def run_and_check(eng, c):
+    b = build(c)
     eng.selftest_layer(b.lc)
     eng.check_errors()
     lc = b.lc
     rep = {k: getattr(lc, k) for k in ("bn", "bk", "stages", "resid_tma", "tma_out", "grid", "tiles", "div_fallback")}
     rep["terms"] = b.terms
     rep["sig"] = lc.sig.decode()
-    ck = Checker(c["name"] + ("/simt" if impl else ""))
+    ck = Checker(c["name"])
     if c["kind"] == PAIR:
         check_pair(b, ck)
         return ck.worst, rep
     wins = windows_of(b)
     y = reference(b) if wins is None else None
     M = reference(b, abs_=True) if wins is None else None
-    check_outputs(b, ck, y, M, impl)
+    check_outputs(b, ck, y, M)
     return ck.worst, rep
 
 
@@ -589,7 +589,7 @@ def check_write_set(name, what, bits, mask, sentinel, before=None):
         raise AssertionError((name, what, f"{len(bad)} elements outside the write set changed, first {bad[:4].tolist()}"))
 
 
-def check_outputs(b, ck, y, M, impl, before=None):
+def check_outputs(b, ck, y, M, before=None):
     """Every output of a conv layer (b.buf): its write set, the exact zeros and every value against float64 (y, M =
     reference(b) and reference(b, abs_=True)).  before: the output buffers as they were before the launch (the plan
     replay, whose buffers carry no sentinels), keyed as b.buf."""
@@ -616,7 +616,7 @@ def check_outputs(b, ck, y, M, impl, before=None):
             check_write_set(ck.name, key, buf, m, SENT32, prev)
         else:
             check_write_set(ck.name, key + ".hi", buf[0], m, SENT16, None if prev is None else prev[0])
-            lo_written = key == "r" or b.terms == 3 or lc.out_ar or impl == 1
+            lo_written = key == "r" or b.terms == 3 or lc.out_ar
             check_write_set(ck.name, key + ".lo", buf[1], m if lo_written else np.zeros_like(m), SENT16,
                             None if prev is None else prev[1])
         del m
@@ -733,22 +733,12 @@ def eng():
     e.close()
 
 
-def _simt_ok(c):
-    return c["kind"] != PAIR and not c.get("out_ar") and c.get("resid") != "ar"
-
-
 @pytest.mark.parametrize("name", [c["name"] for c in CASES])
 def test_layer_matches_float64(eng, name):
     c = BY_NAME[name]
-    worst, rep = run_and_check(eng, c, 0)
+    worst, rep = run_and_check(eng, c)
     REPORTS[name] = rep
     print(f"{name}: max err / bound = {worst:.3e} (tol {TOL[rep['terms']]:.1e})  config {rep}")
-
-
-@pytest.mark.parametrize("name", [c["name"] for c in CASES if _simt_ok(c)])
-def test_layer_simt_matches_float64(eng, name):
-    worst, _ = run_and_check(eng, BY_NAME[name], 1)
-    print(f"{name}/simt: max err / bound = {worst:.3e}")
 
 
 @pytest.mark.parametrize("name", [c["name"] for c in CASES if c["kind"] == PAIR])
@@ -764,14 +754,14 @@ def test_pair_two_launch_path_matches_float64(eng, name):
                **(dict(outs="a", act=1, slope=STAGE_SLOPE, out_row0=c.get("out_row0", 0), out_slack=c.get("out_slack", 0))
                   if c.get("last") else dict(outs="a", out_ar=True)), **common)
     for cc in (a_case, b_case):
-        worst, _ = run_and_check(eng, cc, 0)
+        worst, _ = run_and_check(eng, cc)
         print(f"{cc['name']}: max err / bound = {worst:.3e}")
 
 
 def test_fp16_overflow_is_reported_and_the_next_case_passes(eng):
     from voicefixer_main_b200._lib import EngineError
     c = dict(BY_NAME["res_a.d243_c64"], name="overflow")
-    b = build(c, 0)
+    b = build(c)
     xb = np.stack([np.full_like(b.keep[0][0], 0x7800), np.zeros_like(b.keep[0][1])])   # x = 32768 everywhere
     b.lc.x = _ptr(xb)
     b.keep.append(xb)
@@ -779,7 +769,7 @@ def test_fp16_overflow_is_reported_and_the_next_case_passes(eng):
     with pytest.raises(EngineError) as ei:
         eng.check_errors()
     assert ei.value.code == VL.VF_EDEVICE
-    run_and_check(eng, BY_NAME["res_a.d243_c64"], 0)
+    run_and_check(eng, BY_NAME["res_a.d243_c64"])
 
 
 PLAN_FRAMES = {0: 101, 1: 101, 2: 128, 3: 128}        # plan kind (vf_selftest_plan_gemms) -> frames of the swept plan
@@ -817,7 +807,7 @@ def test_cases_cover_every_kernel_configuration(eng):
     case above, so each kernel configuration a restore runs is checked against float64 here."""
     for c in CASES:
         if c["name"] not in REPORTS:
-            REPORTS[c["name"]] = run_and_check(eng, c, 0)[1]
+            REPORTS[c["name"]] = run_and_check(eng, c)[1]
     by_sig = {}
     for name, r in REPORTS.items():
         by_sig.setdefault(r["sig"], name)

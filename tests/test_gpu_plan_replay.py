@@ -469,7 +469,7 @@ def check_gemm(rp, t, label, ck):
         b.head_valid = rows_of(lc.head_valid, n)
     y = G.reference(b).cpu()
     M = G.reference(b, abs_=True).cpu()
-    G.check_outputs(b, ck, y, M, 0, before)
+    G.check_outputs(b, ck, y, M, before)
 
 
 def check_pair(rp, t, label, ck):

@@ -1,6 +1,6 @@
-"""The vf_selftest_* hooks leave the engine as they found them.  A case packs weights into the context, allocates buffers,
-may switch validate_simt on and may fail half way; the engine's cached plans, weights, options and launch count must not
-show it afterwards, whichever way the case ended."""
+"""The vf_selftest_* hooks leave the engine as they found them.  A case packs weights into the context, allocates buffers
+and may fail half way; the engine's cached plans, weights, options and launch count must not show it afterwards, whichever
+way the case ended."""
 import pytest
 import torch
 
@@ -29,13 +29,13 @@ def test_cases_leave_the_engine_as_they_found_it():
         n0 = e.launch_count()
 
         # a layer rejected after its weights were packed: the loaders' packer takes N = 48, Builder::gemm does not
-        bad = LAY.build(LAY.C("scope.cout48", LAY.CONV1D, L=64, cin=64, cout=48, k=3), 0)
+        bad = LAY.build(LAY.C("scope.cout48", LAY.CONV1D, L=64, cin=64, cout=48, k=3))
         with pytest.raises(VL.EngineError) as ei:
             e.selftest_layer(bad.lc)
         assert ei.value.code == VL.VF_EINVAL and "N=48 not a multiple of 32" in str(ei.value)
 
-        # a SIMT layer (the case switches validate_simt on), one launch
-        LAY.run_and_check(e, LAY.BY_NAME["conv1.mel_l0"], 1)
+        # a layer, one launch
+        LAY.run_and_check(e, LAY.BY_NAME["conv1.mel_l0"])
 
         # a tail case, which packs the tail weights: the peak memset and the tail conv
         name = "tail.L300_lt_one_tile"
@@ -51,7 +51,7 @@ def test_cases_leave_the_engine_as_they_found_it():
         AN._check_gru(got, A.gru_layer(G, w, b, lengths), lengths, T)
         launches = e.launch_count() - n0
 
-        # validate_simt is off again: a plan sweep refuses to run under it, and launches nothing
+        # a plan sweep still runs, and launches nothing
         assert e.selftest_plan_gemms(0, 2, 101)
         # no weights or plan buffers left behind
         assert e.workspace_bytes(2, N) == ws

@@ -120,20 +120,6 @@ def test_sub_batches_give_the_same_bits(ssr_state):
         assert torch.equal(g, f)
 
 
-def test_simt_validation_path(ssr_model):
-    eng = ssr_model._engine()
-    clips = _clips([5000, 1025, 20000], seed=1800)
-    eng.set_option("validate_simt", 1)
-    try:
-        got = ssr_model.restore_batch(clips)
-        want = _per_clip(ssr_model, clips)
-        eng.check_errors()
-    finally:
-        eng.set_option("validate_simt", 0)
-    for g, w in zip(got, want):
-        assert torch.equal(g, w)
-
-
 def _raw_call(eng, fn, packed, offsets, *flags):
     offs = (ctypes.c_int64 * len(offsets))(*offsets)
     out = torch.empty_like(packed)

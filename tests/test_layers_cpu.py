@@ -119,7 +119,7 @@ def _mutated(case, **kw):
 
 
 def _case(name):
-    return G.build(G.BY_NAME[name], 0)
+    return G.build(G.BY_NAME[name])
 
 
 def test_bar_catches_a_dropped_tap():

@@ -48,8 +48,8 @@ class VfTensorDesc(Structure):
 
 class VfLayerCase(Structure):
     """vf_layer_case (include/b200vf.h): one conv layer for vf_selftest_layer (tests only)."""
-    _fields_ = [(f, c_int) for f in ("kind", "impl", "terms", "n_img", "H", "W", "L", "cin", "cout", "sc_cin", "k",
-                                      "dilation", "centered", "stride", "both")] + \
+    _fields_ = [(f, c_int) for f in ("kind", "terms", "n_img", "H", "W", "L", "cin", "cout", "sc_cin", "k", "dilation",
+                                      "centered", "stride", "both")] + \
                [(f, c_void_p) for f in ("w", "b", "sc_w", "sc_b", "w2", "b2", "x")] + \
                [("x_img_rows", c_int), ("x_row0", c_int), ("sc_x", c_void_p), ("resid_kind", c_int), ("resid", c_void_p),
                 ("ar_slope", c_float), ("out_raw", c_void_p), ("raw_ld", c_int), ("out_r", c_void_p), ("r_ld", c_int),

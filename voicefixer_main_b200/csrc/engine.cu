@@ -117,7 +117,7 @@ int run_ops(vf_ctx* ctx, std::vector<Op>& ops, cudaStream_t st) {
     }
     switch (op.kind) {
       case OP_GEMM:
-        e = ctx->validate_simt ? launch_gemm_simt(op.simt, st) : launch_gemm_tc(op.tc, op.bn, op.bk, st);
+        e = launch_gemm_tc(op.tc, op.bn, op.bk, st);
         break;
       case OP_FIRST: e = launch_unet_first(op.first, st); break;
       case OP_POOL: e = launch_pool(op.pool, st); break;
@@ -354,7 +354,7 @@ int host_roundtrip(vf_ctx* ctx, Plan* plan, const float* in_host, float* out_hos
 // captured on the second, and replayed from then on.  Profiling modes always run eagerly.
 template <typename F>
 int run_chain(vf_ctx* ctx, Plan* plan, int slot, cudaStream_t st, int64_t n_launches, F body) {
-  const bool eager = !ctx->use_graphs || ctx->op_timing || ctx->timing || ctx->validate_simt;
+  const bool eager = !ctx->use_graphs || ctx->op_timing || ctx->timing;
   if (eager || plan->uses++ == 0) return body(st);
   if (!plan->graph[slot]) {
     if (!ctx->cap_stream && cudaStreamCreateWithFlags(&ctx->cap_stream, cudaStreamNonBlocking) != cudaSuccess)
@@ -1424,19 +1424,16 @@ VF_API int vf_check_errors(vf_ctx* ctx, void* stream) {
 VF_API int vf_set_option(vf_ctx* ctx, const char* key, int value) {
   if (!ctx || !key) return VF_EINVAL;
   const std::string k = key;
-  int* slot = nullptr;
-  if (k == "unet_terms" || k == "vocoder_terms") {
+  if (k == "vocoder_terms") {
     if (value != 1 && value != 3) return fail(ctx, VF_EINVAL, "%s must be 1 or 3", key);
-    // the UNet's fp32 skip streams, BN affines and fused head exist in the 3-term kernels only (the 1e-4 log-mel
-    // bar needs fp32-grade products anyway)
-    if (k == "unet_terms" && value != 3) return fail(ctx, VF_EINVAL, "unet_terms: only 3 is supported");
-    slot = k == "unet_terms" ? &ctx->unet_terms : &ctx->voc_terms;
+    if (ctx->voc_terms != value) {   // plans bake the option in: drop them
+      drop_all_plans(ctx);
+      ctx->voc_terms = value;
+    }
+    return VF_OK;
   } else if (k == "unify_energy") {
     ctx->unify_energy = value ? 1 : 0;     // per-call behaviour, no plan rebuild needed
     return VF_OK;
-  } else if (k == "validate_simt") {
-    slot = &ctx->validate_simt;
-    value = value ? 1 : 0;
   } else if (k == "host_pipeline") {
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
@@ -1450,14 +1447,8 @@ VF_API int vf_set_option(vf_ctx* ctx, const char* key, int value) {
     ctx->plan_budget = (size_t)value << 20;
     if (value) return evict_plans(ctx, 0, nullptr);
     return VF_OK;
-  } else {
-    return fail(ctx, VF_EINVAL, "unknown option '%s'", key);
   }
-  if (*slot != value) {   // plans bake the option in: drop them
-    drop_all_plans(ctx);
-    *slot = value;
-  }
-  return VF_OK;
+  return fail(ctx, VF_EINVAL, "unknown option '%s'", key);
 }
 
 VF_API int64_t vf_launch_count(vf_ctx* ctx) { return ctx ? ctx->launches : -1; }

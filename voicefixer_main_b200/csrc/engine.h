@@ -26,7 +26,6 @@ int gemm_tc_max_bn(int terms);
 cudaError_t launch_pair_tc(const PairParams& p, cudaStream_t stream);
 size_t pair_tc_smem_bytes(int C);
 uint32_t gemm_tc_magic(uint32_t d, uint64_t nmax);
-cudaError_t launch_gemm_simt(const GemmSimtParams& p, cudaStream_t stream);
 
 struct HostT {
   std::vector<float> v;
@@ -51,7 +50,7 @@ struct Planes {
 };
 struct ASrc {
   Planes pl;
-  int rows;           // valid rows per image (TMA bound / SIMT bound)
+  int rows;           // valid rows per image (the TMA bound)
   int row0;           // first valid row inside the allocation (reflection slack), usually 0
 };
 
@@ -69,7 +68,6 @@ struct Op {
                                  // padding): numerator of the "executed" tensor fraction
   char label[48] = {0};
   GemmTcParams tc;
-  GemmSimtParams simt;
   PairParams pair;
   UnetFirstParams first;
   PoolParams pool;
@@ -214,7 +212,7 @@ struct vf_ctx {
   bool loaded = false;
   EncodeTiledFn encode = nullptr;
   int sm_count = 132;
-  int unet_terms = 3, voc_terms = 1, validate_simt = 0, unify_energy = 0;
+  int voc_terms = 1, unify_energy = 0;
   int64_t launches = 0;
   int* d_err = nullptr;      // [0] device error code, [1] negative-input count
   // tables
@@ -410,10 +408,10 @@ Op planes_op(const float* in, int batch, int T, float scale, float shift, PlaneP
 // t >= row_valid[img] are zeros
 void linear_gemm(Builder& b, std::vector<Op>& ops, const GemmW& W, const Planes& in, int T, int n_img, const int* row_valid,
                  GemmEpilogue e, int terms);
-// The choices of a built OP_GEMM (tensor-core path) or OP_PAIR that select kernel code, as one string; "" for other ops.  Sizes
+// The choices of a built OP_GEMM or OP_PAIR that select kernel code, as one string; "" for other ops.  Sizes
 // that only change occupancy (stages, grid) are left out.
 std::string op_signature(const Op& op);
-// The persistent tile loop of a built OP_GEMM (tensor-core path) or OP_PAIR: tiles in all, CTAs launched and column tiles per
+// The persistent tile loop of a built OP_GEMM or OP_PAIR: tiles in all, CTAs launched and column tiles per
 // row block (0, 0, 0 for other ops)
 void op_tile_loop(const Op& op, int64_t* tiles, int* grid, int* col_tiles);
 int build_plan(vf_ctx* ctx, Plan* plan);

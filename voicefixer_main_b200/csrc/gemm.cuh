@@ -160,16 +160,6 @@ __device__ __forceinline__ uint32_t fast_div(uint32_t n, uint32_t d, uint32_t ma
   return __umulhi(n, magic);
 }
 
-struct GemmSimtParams {            // validation kernel: same contract, plain pointers
-  const __half* a_hi[2];
-  const __half* a_lo[2];
-  int a_ld[2], a_rows[2], a_img_rows[2];
-  const __half* b_hi;
-  const __half* b_lo;
-  int ktot;
-  GemmProblem prob;
-};
-
 __device__ __forceinline__ void split_store8(__half* hi, __half* lo, size_t idx, const float* a) {
   __align__(16) __half h[8];
   __align__(16) __half l[8];
@@ -180,89 +170,6 @@ __device__ __forceinline__ void split_store8(__half* hi, __half* lo, size_t idx,
   }
   *reinterpret_cast<uint4*>(hi + idx) = *reinterpret_cast<const uint4*>(h);
   *reinterpret_cast<uint4*>(lo + idx) = *reinterpret_cast<const uint4*>(l);
-}
-
-// One thread owns GEMM row `r` of image `img`; v holds columns [n_base, n_base + 32).
-__device__ __forceinline__ void epilogue_chunk(const GemmEpilogue& e, int img, int r, int n_base, float (&v)[32],
-                                               float& head_acc) {
-  if (r >= e.rows_in) return;
-  int co0 = n_base, phase = 0;
-  if (e.map != MAP_PLAIN) {
-    phase = n_base / e.cout;
-    co0 = n_base - phase * e.cout;
-  }
-  size_t orow;
-  bool pad = false;
-  const int vrows = valid_rows(e.row_valid, img);
-  if (e.map == MAP_PLAIN) {
-    orow = (size_t)img * e.out_img_rows + e.out_row0 + r;
-    if (e.Wp > 0) pad = (r % e.Wp) == e.Wp - 1;
-    pad |= r >= vrows;
-  } else if (e.map == MAP_CONVT2D) {
-    const int h = r / e.Wp, w = r - h * e.Wp;
-    const int ph = phase >> 1, pw = phase & 1;
-    const int col = 2 * w + pw;
-    if (col >= e.ct_out_wp) return;          // both=True prune: column past the output pitch
-    orow = (size_t)img * e.out_img_rows + (size_t)(2 * h + ph) * e.ct_out_wp + col;
-    pad = col == e.ct_out_wp - 1 || r >= vrows;
-  } else {
-    const long t = (long)r * e.ct_stride + phase - e.ct_pad;
-    if (t < 0 || t >= e.out_rows_valid) return;
-    orow = (size_t)img * e.out_img_rows + e.out_row0 + t;
-    pad = t >= vrows;
-  }
-  if (e.bias) {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] += __ldg(e.bias + n_base + i);
-  }
-  if (e.resid) {
-    const float4* rp = reinterpret_cast<const float4*>(e.resid + ((size_t)img * e.rows_in + r) * e.resid_ld + co0);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float4 q = __ldg(rp + i);
-      v[4 * i] += q.x; v[4 * i + 1] += q.y; v[4 * i + 2] += q.z; v[4 * i + 3] += q.w;
-    }
-  }
-  if (e.resid_hi) {
-    const size_t ro = ((size_t)img * e.rows_in + r) * e.resid_ld + co0;
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] += __half2float(e.resid_hi[ro + i]) + __half2float(e.resid_lo[ro + i]);
-  }
-  if (pad) {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = 0.f;
-  }
-  if (e.out_raw) {
-    float4* op = reinterpret_cast<float4*>(e.out_raw + orow * e.raw_ld + co0);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) op[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-  }
-  if (e.out_r.hi) {
-    const size_t base = orow * e.out_r.ld + e.out_r.c_off + co0;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) split_store8(e.out_r.hi, e.out_r.lo, base + 8 * i, v + 8 * i);
-  }
-  if (e.head_w) {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) head_acc = fmaf(v[i], __ldg(e.head_w + co0 + i), head_acc);
-  }
-  if (e.out_a.hi) {
-    bool ovf = false;
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      float a = v[i];
-      if (e.a_scale) a = fmaf(a, __ldg(e.a_scale + co0 + i), __ldg(e.a_shift + co0 + i));
-      if (e.act == ACT_LRELU) a = a > 0.f ? a : a * e.slope;
-      else if (e.act == ACT_ELU) a = a > 0.f ? a : expm1f(a);
-      if (pad) a = 0.f;
-      ovf |= !(fabsf(a) <= 65504.f);
-      v[i] = a;
-    }
-    if (ovf && e.err) atomicCAS(e.err, 0, ERR_FP16_OVERFLOW);
-    const size_t base = orow * e.out_a.ld + e.out_a.c_off + co0;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) split_store8(e.out_a.hi, e.out_a.lo, base + 8 * i, v + 8 * i);
-  }
 }
 
 // unet.py:96-100 + gsr_voicefixer.py:90: out = head(x) padded with a zero bin, plus the input log-mel;

@@ -115,9 +115,8 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
   int k = 0;
   for (auto& t : taps) {
     t.k_off = k;
-    const int padded = round_up(t.nch, bk);
-    k += padded;
-    if (ctx->validate_simt == 0) t.nch = padded;
+    t.nch = round_up(t.nch, bk);
+    k += t.nch;
   }
   if (k != W.K) { rc = fail(ctx, VF_EINVAL, "GEMM K mismatch: taps cover %d, packed weight has %d", k, W.K); return; }
   GemmProblem pr;
@@ -133,117 +132,100 @@ void Builder::gemm(std::vector<Op>& ops, const GemmW& W, const ASrc& s0, const A
   pr.epi = epi;
   op.bn = bn;
   op.bk = bk;
-  if (ctx->validate_simt) {
-    GemmSimtParams& sp = op.simt;
-    memset(&sp, 0, sizeof sp);
-    const ASrc* srcs[2] = {&s0, s1};
-    for (int i = 0; i < 2; ++i) {
-      if (!srcs[i]) continue;
-      const size_t off = (size_t)srcs[i]->row0 * srcs[i]->pl.C;
-      sp.a_hi[i] = srcs[i]->pl.p.hi + off;
-      sp.a_lo[i] = srcs[i]->pl.p.lo + off;
-      sp.a_ld[i] = srcs[i]->pl.C;
-      sp.a_rows[i] = srcs[i]->rows;
-      sp.a_img_rows[i] = srcs[i]->pl.img_rows;
-    }
-    sp.b_hi = W.hi; sp.b_lo = W.lo; sp.ktot = W.K;
-    sp.prob = pr;
-  } else {
-    GemmTcParams& tp = op.tc;
-    memset(&tp, 0, sizeof tp);
-    const ASrc* srcs[2] = {&s0, s1 ? s1 : &s0};
-    for (int i = 0; i < 2 && !rc; ++i) {
-      if (terms == 3) {
-        if (srcs[i]->pl.plane_stride == 0) rc = fail(ctx, VF_EINVAL, "3-term GEMM source without adjacent hi/lo planes");
-        if (!rc) rc = map_a(ctx, &tp.a_hi[i], *srcs[i], srcs[i]->pl.p.hi, n_img, bk, true);
-      } else {
-        rc = map_a(ctx, &tp.a_hi[i], *srcs[i], srcs[i]->pl.p.hi, n_img, bk, false);
-      }
-    }
+  GemmTcParams& tp = op.tc;
+  memset(&tp, 0, sizeof tp);
+  const ASrc* srcs[2] = {&s0, s1 ? s1 : &s0};
+  for (int i = 0; i < 2 && !rc; ++i) {
     if (terms == 3) {
-      if (!rc) rc = map_weights(ctx, &tp.b_hi, W, W.hi, bk, bn, true);
+      if (srcs[i]->pl.plane_stride == 0) rc = fail(ctx, VF_EINVAL, "3-term GEMM source without adjacent hi/lo planes");
+      if (!rc) rc = map_a(ctx, &tp.a_hi[i], *srcs[i], srcs[i]->pl.p.hi, n_img, bk, true);
     } else {
-      if (!rc) rc = map_weights(ctx, &tp.b_hi, W, W.hi, bk, bn, false);
-      if (!rc) rc = map_weights(ctx, &tp.b_lo, W, W.lo, bk, bn, false);
+      rc = map_a(ctx, &tp.a_hi[i], *srcs[i], srcs[i]->pl.p.hi, n_img, bk, false);
     }
-    // accumulation segments (see gemm_tc.cu): a bounded chain of truncating MMAs, then promotion to registers
-    tp.tile_chunks = 0;
-    for (auto& t : taps) tp.tile_chunks += t.nch / bk;   // ring slots per tile
-    // K steps per accumulation chain before promotion: longer chains = fewer promotion drains, shorter ones = less
-    // drift of the tensor core's fp32 accumulation (the 3-term UNet carries a 1e-4 log-mel bar).
-    const int seg_mmas = 24;
-    tp.seg_chunks = std::max(1, seg_mmas / (bk / 16));
-    // occupancy: small-K tiles are bound by loads/stores -> several persistent CTAs per SM; large-K -> one
-    // one persistent CTA of 384 threads per SM (the accumulators take the register file): the deepest operand ring that fits
-    const size_t smem_cap = (size_t)227 * 1024 - 1024;
-    // The residual and the fp32 output follow the GEMM rows, which only MAP_PLAIN layers store in order (gemm_tc.cu).
-    GemmEpilogue& pe = pr.epi;
-    const bool has_resid = pe.resid || pe.resid_hi;
-    if (pe.map != MAP_PLAIN && (has_resid || pe.out_raw)) {
-      rc = fail(ctx, VF_EINVAL, "GEMM residual or fp32 output on a transposed conv (MAP_PLAIN layers only)");
-      return;
-    }
-    if (pe.resid && pe.resid_hi) { rc = fail(ctx, VF_EINVAL, "GEMM with both an fp32 and a hi/lo residual"); return; }
-    // Staging per epilogue warp: a hi-only MAP_PLAIN layer finishes its accumulator fragments in place, 16 rows x BN columns
-    // in as many fp16 planes as its residual or widest output has; every other layer passes 32 x 32 fp32 through 4 KB.
-    const bool frag = terms == 1 && pe.map == MAP_PLAIN;
-    const int fbw = std::min(bn, 64);
-    tp.stg_warp = frag ? 16 * bn * 2 * ((has_resid || pe.out_r.hi || pe.out_ar) ? 2 : 1) : 4096;
-    auto fit = [&](int ring) {
-      int st = 8;
-      for (; st >= 2; --st)
-        if (gemm_tc_smem_bytes(bn, bk, st, terms, tp.tile_chunks, tp.stg_warp, ring) <= smem_cap) break;
-      return st;
-    };
-    // The 3-term epilogue reads its residual by TMA, one or two 4 KB tiles per epilogue warp requested that many chunks
-    // ahead: two where the operand ring keeps its depth.  The hi-only one reads it into its staging tile.
-    tp.resid_tma = (has_resid && !frag) ? 1 : 0;
-    int stages = fit(tp.resid_tma);
-    if (tp.resid_tma) {
-      const int st2 = fit(2);
-      if (st2 >= 2 && (st2 == stages || st2 >= 4)) { tp.resid_tma = 2; stages = st2; }
-    }
-    if (stages < 2) { rc = fail(ctx, VF_EINVAL, "no wgmma tile configuration fits (bn=%d bk=%d terms=%d)", bn, bk, terms); return; }
-    tp.stages = stages;
-    // TMA boxes of the epilogue's fp16 planes: a warp's 16 fragment rows x min(BN, 64) columns (hi-only MAP_PLAIN), else 32 x 32
-    const int box_c = frag ? fbw : 32, box_rows = frag ? 16 : 32;
-    if (has_resid) {
-      if (pe.resid) rc = map_rows(ctx, &tp.i_res, pe.resid, 4, pe.resid_ld, pe.rows_in, (size_t)pe.rows_in, n_img, 32, 32);
-      else rc = map_out_planes(ctx, &tp.i_res, pe.resid_hi, pe.resid_lo, 2, pe.resid_ld, pe.rows_in, (size_t)pe.rows_in, n_img, box_c, box_rows);
-      if (rc) return;
-    }
-    // Every MAP_PLAIN output leaves the epilogue's staging tiles by TMA store (gemm_tc.cu), and so does the activated output
-    // of a transposed 1-D conv that fills its output rows exactly; the other transposed-conv outputs are scattered by STG.
-    pe.tma_out = 0;
-    if (pe.map == MAP_CONVT1D && pe.out_a.hi && !pe.out_r.hi && pe.out_row0 == 0 &&
-        pe.out_rows_valid == pe.out_img_rows && pe.out_img_rows % pe.ct_stride == 0 && pe.out_a.ld % 8 == 0) {
-      rc = map_convt1d_out(ctx, &tp.o_a, pe.out_a.hi, pe.out_a.lo, (terms == 3 || pe.out_ar) ? 2 : 1, pe.out_a.ld, pe.ct_stride, pe.out_img_rows, n_img);
-      if (rc) return;
-      pe.tma_out = 1;
-    }
-    if (pe.map == MAP_PLAIN) {
-      const int orows = pe.out_row0 + pe.rows_in;
-      if (pe.out_raw) {
-        if (pe.raw_ld % 4) { rc = fail(ctx, VF_EINVAL, "fp32 GEMM output row of %d floats: the TMA store needs 16-byte rows", pe.raw_ld); return; }
-        rc = map_rows(ctx, &tp.o_raw, pe.out_raw, 4, pe.raw_ld, orows, (size_t)pe.out_img_rows, n_img, 32, 32);
-        if (rc) return;
-      }
-      if (pe.out_r.hi) {
-        rc = map_out_planes(ctx, &tp.o_r, pe.out_r.hi, pe.out_r.lo, 2, pe.out_r.ld, orows, (size_t)pe.out_img_rows, n_img, box_c, box_rows);
-        if (rc) return;
-      }
-      if (pe.out_a.hi) {
-        rc = map_out_planes(ctx, &tp.o_a, pe.out_a.hi, pe.out_a.lo, (terms == 3 || pe.out_ar) ? 2 : 1, pe.out_a.ld, orows, (size_t)pe.out_img_rows, n_img,
-                            box_c, box_rows);
-        if (rc) return;
-      }
-    }
-    const long total_tiles = (long)n_img * pr.m_tiles * (N / bn);
-    tp.grid = (int)std::min<long>(total_tiles, (long)ctx->sm_count);
-    tp.magic_n = gemm_tc_magic((uint32_t)(N / bn), (uint64_t)total_tiles);
-    tp.magic_m = gemm_tc_magic((uint32_t)pr.m_tiles, (uint64_t)n_img * pr.m_tiles);
-    tp.prob = pr;
   }
+  if (terms == 3) {
+    if (!rc) rc = map_weights(ctx, &tp.b_hi, W, W.hi, bk, bn, true);
+  } else {
+    if (!rc) rc = map_weights(ctx, &tp.b_hi, W, W.hi, bk, bn, false);
+    if (!rc) rc = map_weights(ctx, &tp.b_lo, W, W.lo, bk, bn, false);
+  }
+  // accumulation segments (see gemm_tc.cu): a bounded chain of truncating MMAs, then promotion to registers
+  tp.tile_chunks = 0;
+  for (auto& t : taps) tp.tile_chunks += t.nch / bk;   // ring slots per tile
+  // K steps per accumulation chain before promotion: longer chains = fewer promotion drains, shorter ones = less
+  // drift of the tensor core's fp32 accumulation (the 3-term UNet carries a 1e-4 log-mel bar).
+  const int seg_mmas = 24;
+  tp.seg_chunks = std::max(1, seg_mmas / (bk / 16));
+  // occupancy: small-K tiles are bound by loads/stores -> several persistent CTAs per SM; large-K -> one
+  // one persistent CTA of 384 threads per SM (the accumulators take the register file): the deepest operand ring that fits
+  const size_t smem_cap = (size_t)227 * 1024 - 1024;
+  // The residual and the fp32 output follow the GEMM rows, which only MAP_PLAIN layers store in order (gemm_tc.cu).
+  GemmEpilogue& pe = pr.epi;
+  const bool has_resid = pe.resid || pe.resid_hi;
+  if (pe.map != MAP_PLAIN && (has_resid || pe.out_raw)) {
+    rc = fail(ctx, VF_EINVAL, "GEMM residual or fp32 output on a transposed conv (MAP_PLAIN layers only)");
+    return;
+  }
+  if (pe.resid && pe.resid_hi) { rc = fail(ctx, VF_EINVAL, "GEMM with both an fp32 and a hi/lo residual"); return; }
+  // Staging per epilogue warp: a hi-only MAP_PLAIN layer finishes its accumulator fragments in place, 16 rows x BN columns
+  // in as many fp16 planes as its residual or widest output has; every other layer passes 32 x 32 fp32 through 4 KB.
+  const bool frag = terms == 1 && pe.map == MAP_PLAIN;
+  const int fbw = std::min(bn, 64);
+  tp.stg_warp = frag ? 16 * bn * 2 * ((has_resid || pe.out_r.hi || pe.out_ar) ? 2 : 1) : 4096;
+  auto fit = [&](int ring) {
+    int st = 8;
+    for (; st >= 2; --st)
+      if (gemm_tc_smem_bytes(bn, bk, st, terms, tp.tile_chunks, tp.stg_warp, ring) <= smem_cap) break;
+    return st;
+  };
+  // The 3-term epilogue reads its residual by TMA, one or two 4 KB tiles per epilogue warp requested that many chunks
+  // ahead: two where the operand ring keeps its depth.  The hi-only one reads it into its staging tile.
+  tp.resid_tma = (has_resid && !frag) ? 1 : 0;
+  int stages = fit(tp.resid_tma);
+  if (tp.resid_tma) {
+    const int st2 = fit(2);
+    if (st2 >= 2 && (st2 == stages || st2 >= 4)) { tp.resid_tma = 2; stages = st2; }
+  }
+  if (stages < 2) { rc = fail(ctx, VF_EINVAL, "no wgmma tile configuration fits (bn=%d bk=%d terms=%d)", bn, bk, terms); return; }
+  tp.stages = stages;
+  // TMA boxes of the epilogue's fp16 planes: a warp's 16 fragment rows x min(BN, 64) columns (hi-only MAP_PLAIN), else 32 x 32
+  const int box_c = frag ? fbw : 32, box_rows = frag ? 16 : 32;
+  if (has_resid) {
+    if (pe.resid) rc = map_rows(ctx, &tp.i_res, pe.resid, 4, pe.resid_ld, pe.rows_in, (size_t)pe.rows_in, n_img, 32, 32);
+    else rc = map_out_planes(ctx, &tp.i_res, pe.resid_hi, pe.resid_lo, 2, pe.resid_ld, pe.rows_in, (size_t)pe.rows_in, n_img, box_c, box_rows);
+    if (rc) return;
+  }
+  // Every MAP_PLAIN output leaves the epilogue's staging tiles by TMA store (gemm_tc.cu), and so does the activated output
+  // of a transposed 1-D conv that fills its output rows exactly; the other transposed-conv outputs are scattered by STG.
+  pe.tma_out = 0;
+  if (pe.map == MAP_CONVT1D && pe.out_a.hi && !pe.out_r.hi && pe.out_row0 == 0 &&
+      pe.out_rows_valid == pe.out_img_rows && pe.out_img_rows % pe.ct_stride == 0 && pe.out_a.ld % 8 == 0) {
+    rc = map_convt1d_out(ctx, &tp.o_a, pe.out_a.hi, pe.out_a.lo, (terms == 3 || pe.out_ar) ? 2 : 1, pe.out_a.ld, pe.ct_stride, pe.out_img_rows, n_img);
+    if (rc) return;
+    pe.tma_out = 1;
+  }
+  if (pe.map == MAP_PLAIN) {
+    const int orows = pe.out_row0 + pe.rows_in;
+    if (pe.out_raw) {
+      if (pe.raw_ld % 4) { rc = fail(ctx, VF_EINVAL, "fp32 GEMM output row of %d floats: the TMA store needs 16-byte rows", pe.raw_ld); return; }
+      rc = map_rows(ctx, &tp.o_raw, pe.out_raw, 4, pe.raw_ld, orows, (size_t)pe.out_img_rows, n_img, 32, 32);
+      if (rc) return;
+    }
+    if (pe.out_r.hi) {
+      rc = map_out_planes(ctx, &tp.o_r, pe.out_r.hi, pe.out_r.lo, 2, pe.out_r.ld, orows, (size_t)pe.out_img_rows, n_img, box_c, box_rows);
+      if (rc) return;
+    }
+    if (pe.out_a.hi) {
+      rc = map_out_planes(ctx, &tp.o_a, pe.out_a.hi, pe.out_a.lo, (terms == 3 || pe.out_ar) ? 2 : 1, pe.out_a.ld, orows, (size_t)pe.out_img_rows, n_img,
+                          box_c, box_rows);
+      if (rc) return;
+    }
+  }
+  const long total_tiles = (long)n_img * pr.m_tiles * (N / bn);
+  tp.grid = (int)std::min<long>(total_tiles, (long)ctx->sm_count);
+  tp.magic_n = gemm_tc_magic((uint32_t)(N / bn), (uint64_t)total_tiles);
+  tp.magic_m = gemm_tc_magic((uint32_t)pr.m_tiles, (uint64_t)n_img * pr.m_tiles);
+  tp.prob = pr;
   {   // algorithmic work: the reference op's own MAC count and the minimum HBM traffic of this launch
     double kreal = 0;
     for (auto& t : taps) kreal += (double)std::min(t.nch, (t.src ? s1 : &s0)->pl.C);
@@ -492,7 +474,9 @@ int build_unet(vf_ctx* ctx, Builder& b, Plan* plan, const UnetW& U, const UnetGe
   const int B = plan->batch, T = plan->T;
   const int Tp = (T + 63) / 64 * 64;
   std::vector<Op>& ops = plan->unet;
-  const int terms = ctx->unet_terms;
+  // the UNet's fp32 skip streams, BN affines and fused head exist in the 3-term kernels only (the 1e-4 log-mel bar needs
+  // fp32-grade products anyway)
+  const int terms = 3;
   const float S = UNET_SLOPE;
   Level lv[7];
   for (int l = 0; l < 7; ++l) {
@@ -692,7 +676,7 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
     // fp16 correction plane (the otherwise unused lo plane of the same allocation), updated in place by every residual layer:
     // 10 instead of 12 bytes per element through a residual pair.  A slope with no fp16 inverse (ar_inv_word) keeps separate
     // hi/lo planes of x.
-    const uint32_t ar = (!ctx->validate_simt && terms == 1) ? ar_inv_word(c.voc_res_slope) : 0u;
+    const uint32_t ar = terms == 1 ? ar_inv_word(c.voc_res_slope) : 0u;
     // C = 64 stacks of the hi-only mode with the (a, r) stream: one kernel per residual pair (pair_tc.cu), the intermediate h
     // stays in shared memory.  A pair's activated input and output planes must differ (a tile reads rows up to `dil` away from
     // the ones another CTA is writing): the pairs ping-pong between xa and xa2.
@@ -854,17 +838,17 @@ void op_tile_loop(const Op& op, int64_t* tiles, int* grid, int* col_tiles) {
 namespace {
 
 // One nn.Linear of an analysis module on the plan's [B, T, cin] planes (linear_gemm); varlen rows past a clip's end are zeros
-void linear(vf_ctx* ctx, Builder& b, Plan* plan, const GemmW& W, const Planes& in, GemmEpilogue e, const char* label) {
+void linear(Builder& b, Plan* plan, const GemmW& W, const Planes& in, GemmEpilogue e, const char* label) {
   b.label = label;
-  linear_gemm(b, plan->unet, W, in, plan->T, plan->batch, plan->vl(VL_T), e, ctx->unet_terms);
+  linear_gemm(b, plan->unet, W, in, plan->T, plan->batch, plan->vl(VL_T), e, 3);
 }
 
 // The module's last Linear: out_raw = d_logmel_out = Linear(x) + log-mel (gsr_voicefixer.py:90)
-void linear_out(vf_ctx* ctx, Builder& b, Plan* plan, const GemmW& W, const Planes& in, const char* label) {
+void linear_out(Builder& b, Plan* plan, const GemmW& W, const Planes& in, const char* label) {
   GemmEpilogue e = epi_plain(plan->T, 0, 128, plan->T);
   e.out_raw = plan->d_logmel_out; e.raw_ld = 128;
   e.resid = plan->d_logmel_in; e.resid_ld = 128;
-  linear(ctx, b, plan, W, in, e, label);
+  linear(b, plan, W, in, e, label);
 }
 
 // bi_gru (gsr_voicefixer.py:54-64): d_logmel_in -> d_logmel_out
@@ -878,21 +862,21 @@ int build_bigru(vf_ctx* ctx, Builder& b, Plan* plan) {
   {   // Linear 128 -> 256, then BN_GRU.bn (no activation in between: the epilogue's affine)
     GemmEpilogue e = epi_plain(T, 0, 256, T);
     set_out_a(e, x1, 0, g.gru_bn.scale, g.gru_bn.shift, ACT_NONE, 0.f);
-    linear(ctx, b, plan, g.lin_in, x0, e, "bigru.lin1");
+    linear(b, plan, g.lin_in, x0, e, "bigru.lin1");
   }
   for (int l = 0; l < 2; ++l) {
     GemmEpilogue e = epi_plain(T, 0, 6 * GRU_HIDDEN, T);
     e.out_raw = G; e.raw_ld = 6 * GRU_HIDDEN;
-    linear(ctx, b, plan, g.w_ih[l], l ? y : x1, e, l ? "bigru.gru1.ih" : "bigru.gru0.ih");
+    linear(b, plan, g.w_ih[l], l ? y : x1, e, l ? "bigru.gru1.ih" : "bigru.gru0.ih");
     // layer 0 writes y, which layer 1's input projection above has read by the time layer 1 overwrites it
     plan->unet.push_back(gru_op(G, g.dir[l], y.p, B, T, l, plan->vl(VL_T), l ? "bigru.gru1" : "bigru.gru0"));
   }
   {   // ReLU (on the GRU's output, in gru_op) -> Linear 512 -> 256 -> ReLU
     GemmEpilogue e = epi_plain(T, 0, 256, T);
     set_out_a(e, m, 0, nullptr, nullptr, ACT_LRELU, 0.f);
-    linear(ctx, b, plan, g.lin_mid, y, e, "bigru.lin4");
+    linear(b, plan, g.lin_mid, y, e, "bigru.lin4");
   }
-  linear_out(ctx, b, plan, g.lin_out, m, "bigru.lin6");
+  linear_out(b, plan, g.lin_out, m, "bigru.lin6");
   return b.rc;
 }
 
@@ -908,10 +892,10 @@ int build_dnn(vf_ctx* ctx, Builder& b, Plan* plan) {
     if (b.rc) return b.rc;
     GemmEpilogue e = epi_plain(T, 0, d.lin[i].N, T);
     set_out_a(e, o, 0, nullptr, nullptr, ACT_LRELU, 0.f);
-    linear(ctx, b, plan, d.lin[i], x, e, ("dnn.lin" + std::to_string(i)).c_str());
+    linear(b, plan, d.lin[i], x, e, ("dnn.lin" + std::to_string(i)).c_str());
     x = o;
   }
-  linear_out(ctx, b, plan, d.lin[5], x, "dnn.lin5");
+  linear_out(b, plan, d.lin[5], x, "dnn.lin5");
   return b.rc;
 }
 

@@ -60,18 +60,15 @@ struct Case {
   }
 };
 
-// One case of `hook`: sets the device, records the context's weight allocations and runs body(case) with the option
-// validate_simt set to `validate_simt`.  Then, on every path: a hook that launches synchronises and copies the inout()
-// buffers back; the plan's buffers and the weights the case packed are freed; weight_bytes and validate_simt are restored.
+// One case of `hook`: sets the device, records the context's weight allocations and runs body(case).  Then, on every path:
+// a hook that launches synchronises and copies the inout() buffers back; the plan's buffers and the weights the case packed
+// are freed; weight_bytes is restored.
 template <typename F>
-int run_case(vf_ctx* ctx, const char* hook, bool launches, int validate_simt, F body) {
+int run_case(vf_ctx* ctx, const char* hook, bool launches, F body) {
   CK(cudaSetDevice(ctx->device));
   const size_t n_weight_allocs = ctx->allocs.size(), weight_bytes = ctx->weight_bytes;
-  const int saved_simt = ctx->validate_simt;
-  ctx->validate_simt = validate_simt;
   Case s(ctx);
   int rc = body(s);
-  ctx->validate_simt = saved_simt;
   if (launches) {
     const cudaError_t se = cudaDeviceSynchronize();
     if (!rc && se != cudaSuccess) rc = fail(ctx, VF_ECUDA, "%s: %s", hook, cudaGetErrorString(se));
@@ -87,7 +84,7 @@ int run_case(vf_ctx* ctx, const char* hook, bool launches, int validate_simt, F 
   return rc;
 }
 
-// What the hooks report of a built OP_GEMM (tensor-core path) or OP_PAIR: its configuration signature, its persistent tile
+// What the hooks report of a built OP_GEMM or OP_PAIR: its configuration signature, its persistent tile
 // loop, and whether a tile decode divides (its multiply-high magic would not be exact)
 template <size_t N>
 void report_launch(const Op& op, char (&sig)[N], int64_t* tiles, int* grid, int* col_tiles, int* div_fallback) {
@@ -219,17 +216,9 @@ int run_layer_case(vf_ctx* ctx, Case& s, vf_layer_case& c) {
     if (b.rc) return b.rc;
     const Op& op = ops.back();
     c.bn = op.bn; c.bk = op.bk;
-    if (c.impl == VF_LAYER_SIMT) {
-      c.stages = 0; c.resid_tma = 0; c.tma_out = 0;
-      c.grid = op.simt.prob.n_img * op.simt.prob.m_tiles * (op.simt.prob.N / 32);
-      c.tiles = c.grid;
-      c.div_fallback = 0;
-      c.sig[0] = 0;
-    } else {
-      c.stages = op.tc.stages; c.resid_tma = op.tc.resid_tma; c.tma_out = op.tc.prob.epi.tma_out;
-      int col_tiles;
-      report_launch(op, c.sig, &c.tiles, &c.grid, &col_tiles, &c.div_fallback);
-    }
+    c.stages = op.tc.stages; c.resid_tma = op.tc.resid_tma; c.tma_out = op.tc.prob.epi.tma_out;
+    int col_tiles;
+    report_launch(op, c.sig, &c.tiles, &c.grid, &col_tiles, &c.div_fallback);
   }
   return run_ops(ctx, ops, 0);
 }
@@ -403,14 +392,13 @@ struct Tracer {
   }
 
   int describe_gemm(const Op& op, vf_trace_op* t) const {
-    const GemmProblem& pr = ctx->validate_simt ? op.simt.prob : op.tc.prob;
+    const GemmProblem& pr = op.tc.prob;
     const GemmEpilogue& e = pr.epi;
     vf_layer_case& c = t->layer;
     const int n = pr.n_img;
     const ASrc& s0 = op.src[0];
     if (s0.rows != s0.pl.img_rows - s0.row0)
       return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: %s reads %d of rows %d .. %d", op.label, s0.rows, s0.row0, s0.pl.img_rows);
-    c.impl = ctx->validate_simt ? VF_LAYER_SIMT : VF_LAYER_PRODUCT;
     c.terms = pr.terms;
     c.n_img = n;
     c.cin = s0.pl.C;
@@ -494,7 +482,7 @@ struct Tracer {
     t->alloc_bytes = abytes.data();
     vf_op_case& c = t->op;
     c.batch = plan.batch;
-    if (!ctx->validate_simt) snprintf(t->layer.sig, sizeof t->layer.sig, "%s", op_signature(op).c_str());
+    snprintf(t->layer.sig, sizeof t->layer.sig, "%s", op_signature(op).c_str());
     switch (op.kind) {
       case OP_GEMM: t->kind = VF_TRACE_GEMM; return describe_gemm(op, t);
       case OP_PAIR: {
@@ -503,7 +491,7 @@ struct Tracer {
         const Planes& src = op.src[0].pl;
         const Planes& dst = op.pair_dst;
         vf_layer_case& l = t->layer;
-        l.kind = VF_LAYER_PAIR; l.impl = VF_LAYER_PRODUCT; l.terms = 1;
+        l.kind = VF_LAYER_PAIR; l.terms = 1;
         l.n_img = p.n_img; l.L = p.L; l.cin = l.cout = p.C; l.dilation = p.dil; l.k = 3;
         l.b = p.bias_a; l.b2 = p.bias_b;
         l.x = (const uint16_t*)src.p.hi; l.x_img_rows = src.img_rows;
@@ -683,8 +671,8 @@ VF_API int vf_selftest_layer(vf_ctx* ctx, vf_layer_case* lc) {
   if (!ctx || !lc) return VF_EINVAL;
   vf_layer_case& c = *lc;
   const bool pair = c.kind == VF_LAYER_PAIR, lin = c.kind == VF_LAYER_LINEAR;
-  if (c.kind < VF_LAYER_CONV2D || c.kind > VF_LAYER_LINEAR || (c.impl != VF_LAYER_PRODUCT && c.impl != VF_LAYER_SIMT) ||
-      (c.terms != 1 && c.terms != 3) || c.n_img <= 0 || !c.x || !c.w || c.cin <= 0 || c.cout <= 0 || c.x_row0 < 0 ||
+  if (c.kind < VF_LAYER_CONV2D || c.kind > VF_LAYER_LINEAR || (c.terms != 1 && c.terms != 3) ||
+      c.n_img <= 0 || !c.x || !c.w || c.cin <= 0 || c.cout <= 0 || c.x_row0 < 0 ||
       c.out_img_rows <= 0 || c.resid_kind < VF_RESID_NONE || c.resid_kind > VF_RESID_AR ||
       (c.resid_kind != VF_RESID_NONE && !c.resid) || (c.sc_cin && (c.kind != VF_LAYER_CONV2D || !c.sc_w || !c.sc_b || !c.sc_x)) ||
       ((c.kind == VF_LAYER_CONV1D || c.kind == VF_LAYER_CONVT1D || pair || lin) && !c.b) ||
@@ -695,10 +683,7 @@ VF_API int vf_selftest_layer(vf_ctx* ctx, vf_layer_case* lc) {
       (c.head_w && (!c.head_out || c.head_T <= 0)) ||
       (pair && (!c.w2 || !c.b2 || !c.out_a || c.terms != 1 || c.resid_kind != VF_RESID_NONE || c.dilation <= 0)))
     return fail(ctx, VF_EINVAL, "vf_selftest_layer: bad case");
-  // the SIMT kernel's epilogue (gemm.cuh: epilogue_chunk) has no (a, r) stream and there is no SIMT pair
-  if (c.impl == VF_LAYER_SIMT && (pair || c.out_ar || c.resid_kind == VF_RESID_AR))
-    return fail(ctx, VF_EINVAL, "vf_selftest_layer: the SIMT kernel has no (a, r) stream");
-  return run_case(ctx, "vf_selftest_layer", true, c.impl == VF_LAYER_SIMT, [&](Case& s) { return run_layer_case(ctx, s, c); });
+  return run_case(ctx, "vf_selftest_layer", true, [&](Case& s) { return run_layer_case(ctx, s, c); });
 }
 
 VF_API int vf_selftest_gru(vf_ctx* ctx, vf_gru_case* gc) {
@@ -707,7 +692,7 @@ VF_API int vf_selftest_gru(vf_ctx* ctx, vf_gru_case* gc) {
   if (c.batch <= 0 || c.T <= 0 || !c.G || !c.w_hh || !c.b_hn || !c.out) return fail(ctx, VF_EINVAL, "vf_selftest_gru: bad case");
   for (int b = 0; c.lengths && b < c.batch; ++b)
     if (c.lengths[b] < 1 || c.lengths[b] > c.T) return fail(ctx, VF_EINVAL, "vf_selftest_gru: clip %d has %d of %d frames", b, c.lengths[b], c.T);
-  return run_case(ctx, "vf_selftest_gru", true, ctx->validate_simt, [&](Case& s) {
+  return run_case(ctx, "vf_selftest_gru", true, [&](Case& s) {
     const size_t H = GRU_HIDDEN, rows = (size_t)c.batch * c.T;
     const float* G = s.in(c.G, rows * 6 * H);
     float* w = s.in(c.w_hh, 2 * 3 * H * H);
@@ -739,7 +724,7 @@ VF_API int vf_selftest_op(vf_ctx* ctx, vf_op_case* oc) {
       (c.kind == VF_OP_PLANES && (c.T <= 0 || !c.x || !c.planes));
   if (bad_kind || c.batch <= 0 || bad_shape || (c.clip_off && (c.batch > VL_MAX_CLIPS || c.clip_off[0] != 0)))
     return fail(ctx, VF_EINVAL, "vf_selftest_op: bad case");
-  return run_case(ctx, "vf_selftest_op", true, ctx->validate_simt, [&](Case& s) { return run_op_case(ctx, s, c); });
+  return run_case(ctx, "vf_selftest_op", true, [&](Case& s) { return run_op_case(ctx, s, c); });
 }
 
 VF_API int vf_selftest_plan_gemms(vf_ctx* ctx, int plan_kind, int batch, int frames, vf_plan_gemm* records, int cap, int* count) {
@@ -747,11 +732,10 @@ VF_API int vf_selftest_plan_gemms(vf_ctx* ctx, int plan_kind, int batch, int fra
   if (plan_kind < PLAN_GSR || plan_kind > PLAN_VOC_VARLEN || batch <= 0 || frames <= 0 ||
       (is_varlen_plan(plan_kind) && batch > VL_MAX_CLIPS))
     return fail(ctx, VF_EINVAL, "vf_selftest_plan_gemms: bad plan");
-  if (ctx->validate_simt) return fail(ctx, VF_EINVAL, "vf_selftest_plan_gemms: validate_simt plans run no tensor-core launches");
   if (!ctx->loaded) return fail(ctx, VF_ESTATE, "weights not loaded");
   int rc = check_networks(ctx, plan_kind);
   if (rc) return rc;
-  return run_case(ctx, "vf_selftest_plan_gemms", false, 0, [&](Case& s) {
+  return run_case(ctx, "vf_selftest_plan_gemms", false, [&](Case& s) {
     Plan& plan = s.plan;
     plan.kind = plan_kind; plan.batch = batch; plan.T = frames;
     const int built = build_plan(ctx, &plan);
@@ -796,7 +780,7 @@ VF_API int vf_selftest_plan_trace(vf_ctx* ctx, int plan_kind, const float* wav, 
   }
   if (n <= 1024) return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: clips of 1024 samples or fewer");
   const int T = offsets ? round_up(frames_of(ctx, (long)n), 64) : frames_of(ctx, (long)n);
-  return run_case(ctx, "vf_selftest_plan_trace", true, ctx->validate_simt, [&](Case& s) {
+  return run_case(ctx, "vf_selftest_plan_trace", true, [&](Case& s) {
     return run_trace(ctx, s, plan_kind, wav, offsets, batch, n, T, flags, wav_out, fn, user);
   });
 }
