@@ -101,7 +101,9 @@ __global__ void __launch_bounds__(256) pool_kernel(PoolParams p) {
       a[i] = v[i];
       if (p.a_scale) a[i] = fmaf(a[i], __ldg(p.a_scale + g * 8 + i), __ldg(p.a_shift + g * 8 + i));
       a[i] = lrelu(a[i], p.slope);
-      if (!(fabsf(a[i]) <= 65504.f) && p.err) atomicCAS(p.err, 0, ERR_FP16_OVERFLOW);
+      // both split planes are range-checked: a, and the raw r = v (with slope 0.01 a can be in range while v is not)
+      const bool bad = !(fabsf(a[i]) <= 65504.f) || (p.out_r.hi && !(fabsf(v[i]) <= 65504.f));
+      if (bad && p.err) atomicCAS(p.err, 0, ERR_FP16_OVERFLOW);
     }
   }
   const size_t o = opix * p.C + g * 8;

@@ -1416,6 +1416,7 @@ VF_API int vf_check_errors(vf_ctx* ctx, void* stream) {
   CK(cudaMemcpy(h, ctx->d_err, 8, cudaMemcpyDeviceToHost));
   if (h[0] || h[1]) CK(cudaMemset(ctx->d_err, 0, 8));
   if (h[0] == ERR_FP16_OVERFLOW) return fail(ctx, VF_EDEVICE, "activation outside the fp16 range (|a| > 65504) in a hi/lo split");
+  if (h[0] == ERR_NAN_PHASE) return fail(ctx, VF_EDEVICE, "NaN phase in the ISTFT: a NaN or infinite input sample");
   if (h[0]) return fail(ctx, VF_EDEVICE, "device pipeline error code %d (201 producer / 202 mma / 203 epilogue time-out)", h[0]);
   if (h[1]) return fail(ctx, VF_EASSERT, "input has negative values counts %d", h[1]);
   return VF_OK;

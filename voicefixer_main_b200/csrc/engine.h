@@ -401,9 +401,9 @@ int finalize_params(vf_ctx* ctx, FinalizeParams* f, const float* wav, const unsi
 void istft_params(vf_ctx* ctx, IstftFramesParams* fp, IstftOlaParams* op, const float* mag, const float* wav, int batch, long n,
                   int T, float* frames, float* out, const int64_t* vl_off, const int* vl_T);
 // One bidirectional GRU layer (gru_tc.cu) on G [batch, T, 1536] into the [batch, T, 512] planes `out`, with its profile record
-Op gru_op(const float* G, const GruDirW (&dirs)[2], PlanePtr out, int batch, int T, int relu, const int* vl_T, const char* label);
+Op gru_op(vf_ctx* ctx, const float* G, const GruDirW (&dirs)[2], PlanePtr out, int batch, int T, int relu, const int* vl_T, const char* label);
 // The first GEMM operand of bi_gru / dnn: planes of scale * in + shift over [batch, T, 128] (zeros at t >= vl_T[b])
-Op planes_op(const float* in, int batch, int T, float scale, float shift, PlanePtr out, const int* vl_T);
+Op planes_op(vf_ctx* ctx, const float* in, int batch, int T, float scale, float shift, PlanePtr out, const int* vl_T);
 // One nn.Linear of an analysis module on [n_img, T, in.C] planes: a one-tap GEMM with W's bias; `e` carries the outputs, rows
 // t >= row_valid[img] are zeros
 void linear_gemm(Builder& b, std::vector<Op>& ops, const GemmW& W, const Planes& in, int T, int n_img, const int* row_valid,

@@ -31,7 +31,7 @@ constexpr int GEMM_MAX_TAPS = 12;
 
 enum { ACT_NONE = 0, ACT_LRELU = 1, ACT_ELU = 2 };
 enum { MAP_PLAIN = 0, MAP_CONVT2D = 1, MAP_CONVT1D = 2 };
-enum { ERR_FP16_OVERFLOW = 100, ERR_PIPE_PRODUCER = 201, ERR_PIPE_MMA = 202, ERR_PIPE_EPILOGUE = 203 };
+enum { ERR_FP16_OVERFLOW = 100, ERR_NAN_PHASE = 101, ERR_PIPE_PRODUCER = 201, ERR_PIPE_MMA = 202, ERR_PIPE_EPILOGUE = 203 };
 
 struct GemmTap {
   int a_off;   // row offset of the tap's window relative to the output row
@@ -152,6 +152,14 @@ struct PairParams {
   const int* row_valid;          // varlen plans: per clip valid rows (<= L); rows past it are written as zeros.  nullptr: L
   int* err;
 };
+
+// The fp16 range guard's running max |v|: max.NaN.f32 returns NaN when either operand is NaN (fmaxf would return the other
+// one), so one NaN output keeps the running max NaN and the final !(amax <= 65504) flags it as it flags an overflow
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
 
 // n / d with the host's multiply-high magic number (gemm_tc_magic): a handful of instructions instead of an integer division
 __device__ __forceinline__ uint32_t fast_div(uint32_t n, uint32_t d, uint32_t magic) {

@@ -456,6 +456,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           issue_resid();                  // the slot just read is free again: request the chunk `resid_ring` ahead
         }
         const bool pad = (flags & kRowPad) != 0;
+        // the range check covers the rows this chunk stores: a transposed conv's rows outside its output (t < 0, t past the
+        // output, the column past a both=True pitch) are computed but never stored, and cannot make a valid call fail
+        const bool stored = (flags & kRowValid) != 0;
         if (pad) {
 #pragma unroll
           for (int i = 0; i < 32; ++i) v[i] = 0.f;
@@ -473,7 +476,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           }
           st_pending = true;
         }
-        if (want_r) {                     // raw hi/lo planes
+        if (want_r) {                     // raw hi/lo planes: |v| itself is range-checked
+          if (stored) {
+#pragma unroll
+            for (int i = 0; i < 32; ++i) amax = fmax_nan(amax, fabsf(v[i]));
+          }
           stg_release();
           __syncwarp();
 #pragma unroll
@@ -502,9 +509,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
             }
           }
           if (out_ar) {                     // (a, r) stream: hi plane = fp16(lrelu(v)), lo plane = fp16(v - U(a)); |v| itself is range-checked
-            if (row_ok) {
+            if (stored) {
 #pragma unroll
-              for (int i = 0; i < 32; ++i) amax = fmaxf(amax, fabsf(v[i]));
+              for (int i = 0; i < 32; ++i) amax = fmax_nan(amax, fabsf(v[i]));
             }
             stg_release();
             __syncwarp();
@@ -531,9 +538,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 #pragma unroll
               for (int i = 0; i < 32; ++i) v[i] = 0.f;
             }
-            if (row_ok) {
+            if (stored) {
 #pragma unroll
-              for (int i = 0; i < 32; ++i) amax = fmaxf(amax, fabsf(v[i]));
+              for (int i = 0; i < 32; ++i) amax = fmax_nan(amax, fabsf(v[i]));
             }
             stg_release();
             __syncwarp();
@@ -671,9 +678,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           }
           st_pending = true;
         };
-        if (want_r) {                     // raw hi/lo planes, over the residual words each thread has read
+        if (want_r) {                     // raw hi/lo planes, over the residual words each thread has read; |v| is range-checked
 #pragma unroll
           for (int i = 0; i < BN / 2; i += 2) {
+            if (f_ok[(i >> 1) & 1]) amax = fmax_nan(amax, fmax_nan(fabsf(acc[i]), fabsf(acc[i + 1])));
             const __half2 h2 = __floats2half2_rn(acc[i], acc[i + 1]);
             const uint32_t hb = *reinterpret_cast<const uint32_t*>(&h2);
             *f_word(i, 0) = hb;
@@ -687,7 +695,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
           auto put_hi = [&](const int i, float v0, float v1) {
             const int hh = (i >> 1) & 1;
             if (f_pad[hh]) { v0 = 0.f; v1 = 0.f; }
-            if (f_ok[hh]) amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
+            if (f_ok[hh]) amax = fmax_nan(amax, fmax_nan(fabsf(v0), fabsf(v1)));
             const __half2 h2 = __floats2half2_rn(v0, v1);
             *f_word(i, 0) = *reinterpret_cast<const uint32_t*>(&h2);
           };
@@ -695,7 +703,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 #pragma unroll
             for (int i = 0; i < BN / 2; i += 2) {
               const float v0 = acc[i], v1 = acc[i + 1];
-              if (f_ok[(i >> 1) & 1]) amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
+              if (f_ok[(i >> 1) & 1]) amax = fmax_nan(amax, fmax_nan(fabsf(v0), fabsf(v1)));
               uint32_t ab, rb;
               ar_split(v0, v1, fmaxf(v0, v0 * slope), fmaxf(v1, v1 * slope), out_ar, ab, rb);
               *f_word(i, 0) = ab;
@@ -748,7 +756,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
       if (THREE && half == 0) epilogue_head(e, img, r, head_acc);
     }
     if ((map == MAP_PLAIN || convt1d_tma) && lane == 0) tma_store_wait_all();      // this thread's bulk stores have completed before the CTA exits
-    // NaN compares false against everything, inf exceeds the bound
+    // amax is NaN if any checked value was (fmax_nan), and NaN compares false against everything; inf exceeds the bound
     if (!(amax <= 65504.f) && e.err) atomicCAS(e.err, 0, ERR_FP16_OVERFLOW);
   }
 }

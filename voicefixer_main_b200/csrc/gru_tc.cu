@@ -12,6 +12,7 @@
 
 #include <algorithm>
 
+#include "gemm.cuh"
 #include "kernels.cuh"
 
 namespace cg = cooperative_groups;
@@ -45,6 +46,10 @@ __device__ __forceinline__ void store_split(const PlanePtr& o, size_t i, float y
   const __half hi = __float2half_rn(y);
   o.hi[i] = hi;
   o.lo[i] = __float2half_rn(y - __half2float(hi));
+}
+// the fp16 range guard of a split value (NaN fails the compare)
+__device__ __forceinline__ void check_range(float y, int* err) {
+  if (!(fabsf(y) <= 65504.f) && err) atomicCAS(err, 0, ERR_FP16_OVERFLOW);
 }
 
 }  // namespace
@@ -141,6 +146,7 @@ __global__ void __cluster_dims__(GRU_CTAS, 1, 1) __launch_bounds__(THREADS, 1) g
       float* mine = &s.h[cur ^ 1][gc][hidx(U)];
 #pragma unroll
       for (int q = 0; q < GRU_CTAS; ++q) *cluster.map_shared_rank(mine, q) = hn;
+      check_range(hn, p.err);          // |h| < 1 unless G holds a NaN or an infinity; h itself, as relu(NaN) would read 0
       store_split(p.out, ((size_t)gb * p.T + frame(st)) * (2 * H) + dir * H + U, p.relu ? fmaxf(hn, 0.f) : hn);
     }
     cluster.sync();        // release / acquire: the next h tile is complete in every CTA
@@ -157,7 +163,9 @@ __global__ void affine_planes_kernel(const AffinePlanesParams p) {
     const size_t row = i / p.C;
     const int b = (int)(row / p.T), t = (int)(row % p.T);
     const bool valid = !p.vl_T || t < __ldg(p.vl_T + b);
-    store_split(p.out, i, valid ? fmaf(__ldg(p.in + i), p.scale, p.shift) : 0.f);
+    const float y = valid ? fmaf(__ldg(p.in + i), p.scale, p.shift) : 0.f;
+    check_range(y, p.err);
+    store_split(p.out, i, y);
   }
 }
 

@@ -12,6 +12,7 @@
 #include <algorithm>
 
 #include "fft.cuh"
+#include "gemm.cuh"
 #include "kernels.cuh"
 
 namespace vf {
@@ -37,6 +38,8 @@ __global__ void __launch_bounds__(256) istft_frames_kernel(IstftFramesParams p) 
       const float2 xk = rfft_split(Z, p.tw2048, k);
       const float m = sqrtf(fmaxf(xk.x * xk.x + xk.y * xk.y, 1e-8f));     // fDomainHelper.py:62
       const float cs = xk.x / m, sn = xk.y / m;                              // fDomainHelper.py:63-64
+      // the magnitude's clamp maps a NaN power to 1e-4, but the phase keeps the NaN and would carry it to the output
+      if ((cs != cs || sn != sn) && p.err) atomicCAS(p.err, 0, ERR_NAN_PHASE);
       const float om = __ldg(p.mag + frame * 1025 + k);
       Y[k] = make_float2(om * cs, om * sn);                                  // unet_v2.py:136-137
     }

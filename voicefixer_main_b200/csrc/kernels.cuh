@@ -204,6 +204,7 @@ struct GruParams {
   int relu;                  // 1: the planes hold relu(h) (the module's ReLU after the last layer); the recurrence keeps h
   const int* vl_T;           // varlen: clip b has vl_T[b] frames (the reverse direction starts at its own last frame, rows past
                              // it are written as zeros); or null: T for every clip
+  int* err;                  // fp16 range flag: raised when an h of a clip's frames is not finite
 };
 int gru_groups(int batch);
 cudaError_t launch_gru(const GruParams& p, cudaStream_t stream);
@@ -215,6 +216,7 @@ struct AffinePlanesParams {
   float scale, shift;
   PlanePtr out;
   const int* vl_T;
+  int* err;              // fp16 range flag: raised when a written value is NaN or above 65504 in magnitude
 };
 cudaError_t launch_affine_planes(const AffinePlanesParams& p, cudaStream_t stream);
 
@@ -325,6 +327,7 @@ struct IstftFramesParams {
   // first vl_T[b] frames are computed (mag and frames keep the row stride T, the rows past vl_T[b] are not touched)
   const int64_t* vl_off;
   const int* vl_T;
+  int* err;              // with mag: raised (ERR_NAN_PHASE) when a frame's phase is NaN - a NaN or infinite input sample
 };
 cudaError_t launch_istft_frames(const IstftFramesParams& p, cudaStream_t stream);
 struct IstftOlaParams {

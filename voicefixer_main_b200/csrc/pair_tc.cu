@@ -247,7 +247,7 @@ __global__ void __launch_bounds__(PAIR_THREADS, 1) pair_tc_kernel(const __grid_c
         float a0 = acc1[i] + bias[i >> 2].x, a1 = acc1[i + 1] + bias[i >> 2].y;
         a0 = fmaxf(a0, a0 * slope_h); a1 = fmaxf(a1, a1 * slope_h);
         if (tm < 0 || tm >= L) { a0 = 0.f; a1 = 0.f; }        // conv_b pads h with zeros outside the clip
-        amax = fmaxf(amax, fmaxf(fabsf(a0), fabsf(a1)));
+        amax = fmax_nan(amax, fmax_nan(fabsf(a0), fabsf(a1)));
         const __half2 hv = __floats2half2_rn(a0, a1);
         const uint32_t bits = *reinterpret_cast<const uint32_t*>(&hv);
 #pragma unroll
@@ -310,14 +310,14 @@ __global__ void __launch_bounds__(PAIR_THREADS, 1) pair_tc_kernel(const __grid_c
           uint32_t a_bits, r_bits = 0u;
           float m;
           if (AR) {
-            m = fmaxf(fabsf(v0), fabsf(v1));   // |x| bounds |a| and keeps U(a) in range
+            m = fmax_nan(fabsf(v0), fabsf(v1));   // |x| bounds |a| and keeps U(a) in range
             ar_split(v0, v1, a0, a1, ar_out, a_bits, r_bits);
           } else {
-            m = fmaxf(fabsf(a0), fabsf(a1));
+            m = fmax_nan(fabsf(a0), fabsf(a1));
             const __half2 hh = __floats2half2_rn(a0, a1);
             a_bits = *reinterpret_cast<const uint32_t*>(&hh);
           }
-          amax = live[hh] ? fmaxf(amax, m) : amax;
+          amax = live[hh] ? fmax_nan(amax, m) : amax;
           if (kept[hh]) {
             if (AR) *reinterpret_cast<uint32_t*>(xr + off) = live[hh] ? r_bits : 0u;   // each thread rewrites exactly the word it has read
             *reinterpret_cast<uint32_t*>(act_base + off) = live[hh] ? a_bits : 0u;
@@ -332,6 +332,7 @@ __global__ void __launch_bounds__(PAIR_THREADS, 1) pair_tc_kernel(const __grid_c
       wgmma_fence_regs(acc1, C / 2);
       if (ahead) finish_p1();
     }
+    // amax covers h and the output planes, and is NaN if any of them was (fmax_nan)
     if (!(amax <= 65504.f) && P.err) atomicCAS(P.err, 0, ERR_FP16_OVERFLOW);
   }
 }

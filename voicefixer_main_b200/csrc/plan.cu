@@ -425,18 +425,18 @@ void istft_params(vf_ctx* ctx, IstftFramesParams* fp, IstftOlaParams* op, const 
   memset(fp, 0, sizeof *fp);
   fp->mag = mag; fp->wav = wav; fp->n = n; fp->batch = batch; fp->T = T;
   fp->window = ctx->d_window; fp->tw1024 = ctx->d_tw1024; fp->tw2048 = ctx->d_tw2048; fp->frames = frames;
-  fp->vl_off = vl_off; fp->vl_T = vl_T;
+  fp->vl_off = vl_off; fp->vl_T = vl_T; fp->err = ctx->d_err;
   memset(op, 0, sizeof *op);
   op->frames = frames; op->batch = batch; op->T = T; op->length = n; op->window = ctx->d_window;
   op->out = out; op->out_ld = n;
   op->vl_off = vl_off; op->vl_T = vl_T;
 }
 
-Op gru_op(const float* G, const GruDirW (&dirs)[2], PlanePtr out, int batch, int T, int relu, const int* vl_T, const char* label) {
+Op gru_op(vf_ctx* ctx, const float* G, const GruDirW (&dirs)[2], PlanePtr out, int batch, int T, int relu, const int* vl_T, const char* label) {
   Op op; op.kind = OP_GRU;
   GruParams& p = op.gru;
   memset(&p, 0, sizeof p);
-  p.G = G; p.out = out; p.batch = batch; p.T = T; p.relu = relu; p.vl_T = vl_T;
+  p.G = G; p.out = out; p.batch = batch; p.T = T; p.relu = relu; p.vl_T = vl_T; p.err = ctx->d_err;
   for (int d = 0; d < 2; ++d) { p.w_hh[d] = dirs[d].w_hh; p.b_hn[d] = dirs[d].b_hn; }
   const double H = GRU_HIDDEN, steps = 2.0 * batch * T;      // (direction, clip, frame) steps
   op.flops = steps * (2.0 * 3 * H * H + 12 * H);             // W_hh h, then the gates
@@ -778,11 +778,11 @@ int build_vocoder(vf_ctx* ctx, Builder& b, Plan* plan) {
 }  // namespace
 
 // The first GEMM operand of bi_gru / dnn: planes of scale * log-mel + shift (rows past a varlen clip's end are zeros)
-Op planes_op(const float* in, int batch, int T, float scale, float shift, PlanePtr out, const int* vl_T) {
+Op planes_op(vf_ctx* ctx, const float* in, int batch, int T, float scale, float shift, PlanePtr out, const int* vl_T) {
   Op op; op.kind = OP_PLANES;
   AffinePlanesParams& p = op.planes;
   memset(&p, 0, sizeof p);
-  p.in = in; p.batch = batch; p.T = T; p.C = 128; p.scale = scale; p.shift = shift; p.out = out; p.vl_T = vl_T;
+  p.in = in; p.batch = batch; p.T = T; p.C = 128; p.scale = scale; p.shift = shift; p.out = out; p.vl_T = vl_T; p.err = ctx->d_err;
   op.bytes = (double)batch * T * 128 * (4 + 4);
   snprintf(op.label, sizeof op.label, "analysis.in_planes");
   return op;
@@ -858,7 +858,7 @@ int build_bigru(vf_ctx* ctx, Builder& b, Plan* plan) {
   Planes x0 = b.planes(B, T, 128), x1 = b.planes(B, T, 256), y = b.planes(B, T, 512), m = b.planes(B, T, 256);
   float* G = b.alloc<float>((size_t)B * T * 6 * GRU_HIDDEN);
   if (b.rc) return b.rc;
-  plan->unet.push_back(planes_op(plan->d_logmel_in, B, T, g.bn0_scale, g.bn0_shift, x0.p, plan->vl(VL_T)));
+  plan->unet.push_back(planes_op(ctx, plan->d_logmel_in, B, T, g.bn0_scale, g.bn0_shift, x0.p, plan->vl(VL_T)));
   {   // Linear 128 -> 256, then BN_GRU.bn (no activation in between: the epilogue's affine)
     GemmEpilogue e = epi_plain(T, 0, 256, T);
     set_out_a(e, x1, 0, g.gru_bn.scale, g.gru_bn.shift, ACT_NONE, 0.f);
@@ -869,7 +869,7 @@ int build_bigru(vf_ctx* ctx, Builder& b, Plan* plan) {
     e.out_raw = G; e.raw_ld = 6 * GRU_HIDDEN;
     linear(b, plan, g.w_ih[l], l ? y : x1, e, l ? "bigru.gru1.ih" : "bigru.gru0.ih");
     // layer 0 writes y, which layer 1's input projection above has read by the time layer 1 overwrites it
-    plan->unet.push_back(gru_op(G, g.dir[l], y.p, B, T, l, plan->vl(VL_T), l ? "bigru.gru1" : "bigru.gru0"));
+    plan->unet.push_back(gru_op(ctx, G, g.dir[l], y.p, B, T, l, plan->vl(VL_T), l ? "bigru.gru1" : "bigru.gru0"));
   }
   {   // ReLU (on the GRU's output, in gru_op) -> Linear 512 -> 256 -> ReLU
     GemmEpilogue e = epi_plain(T, 0, 256, T);
@@ -886,7 +886,7 @@ int build_dnn(vf_ctx* ctx, Builder& b, Plan* plan) {
   const int B = plan->batch, T = plan->T;
   Planes x = b.planes(B, T, 128);
   if (b.rc) return b.rc;
-  plan->unet.push_back(planes_op(plan->d_logmel_in, B, T, 1.f, 0.f, x.p, plan->vl(VL_T)));
+  plan->unet.push_back(planes_op(ctx, plan->d_logmel_in, B, T, 1.f, 0.f, x.p, plan->vl(VL_T)));
   for (int i = 0; i < 5; ++i) {
     Planes o = b.planes(B, T, d.lin[i].N);
     if (b.rc) return b.rc;

@@ -362,7 +362,7 @@ int run_op_case(vf_ctx* ctx, Case& s, vf_op_case& c) {
     case VF_OP_PLANES: {         // the first op of build_bigru (BN0's scale and shift) and build_dnn (1, 0)
       const float* x = s.in(c.x, (size_t)B * c.T * 128);
       const PlanePtr o = s.inout_planes(c.planes, B, c.T, 128).p;
-      ops.push_back(planes_op(x, B, c.T, c.bn1_scale, c.bn1_shift, o, plan.vl(VL_T)));
+      ops.push_back(planes_op(ctx, x, B, c.T, c.bn1_scale, c.bn1_shift, o, plan.vl(VL_T)));
       break;
     }
   }
@@ -701,7 +701,7 @@ VF_API int vf_selftest_gru(vf_ctx* ctx, vf_gru_case* gc) {
     const PlanePtr out = s.inout_planes(c.out, c.batch, c.T, 2 * GRU_HIDDEN).p;
     if (s.b.rc) return s.b.rc;
     const GruDirW dirs[2] = {{w, bhn}, {w + 3 * H * H, bhn + H}};
-    std::vector<Op> ops{gru_op(G, dirs, out, c.batch, c.T, c.relu != 0, len, "gru")};
+    std::vector<Op> ops{gru_op(ctx, G, dirs, out, c.batch, c.T, c.relu != 0, len, "gru")};
     return run_ops(ctx, ops, 0);
   });
 }
