@@ -697,34 +697,57 @@ VF_API int vf_selftest_gru(vf_ctx* ctx, vf_gru_case* gc);
  * vf_resynth / vf_resynth_varlen) built for this call with the
  * loaded weights and the context's options, run as the restore entry points run it (front end, lengths table, the UNet's
  * launches, the band sums of VF_RESTORE_UNIFY_ENERGY, the vocoder's, then the finalize or the ISTFT) but eagerly, one
- * launch at a time, synchronising around each launch of the UNet and vocoder lists and around the finalize.  wav and
- * wav_out are device buffers as vf_restore (offsets NULL: batch clips of n samples) or vf_restore_varlen (offsets [batch + 1],
- * host; n is ignored) take them; flags are vf_restore_ex's (GSR plans only).  Synchronous; the plan is freed on return and
- * the plan cache is not touched.
+ * launch at a time, synchronising around each traced step.  The traced steps are the launches of the UNet and vocoder
+ * lists and the finalize; with VF_TRACE_DIRECT_STEPS also the launches the restore makes itself (list 3: the front end,
+ * the band sums, the ISTFT), so that only the lengths table of a varlen plan is written untraced, ahead of the first
+ * step.  wav and wav_out are device buffers as vf_restore (offsets NULL: batch clips of n samples) or vf_restore_varlen
+ * (offsets [batch + 1], host; n is ignored) take them; flags are vf_restore_ex's (GSR plans only) and
+ * VF_TRACE_DIRECT_STEPS (any plan).  Synchronous; the plan is freed on return and the plan cache is not touched.
  *
- * fn(user, after, op) runs before (after = 0) and after (after = 1) each traced launch; a nonzero return stops the run
- * (VF_EINVAL).  op describes the launch as the builder set it up, with DEVICE pointers: a GEMM or a fused pair (kind 0 / 8)
+ * fn(user, after, op) runs before (after = 0) and after (after = 1) each traced step; a nonzero return stops the run
+ * (VF_EINVAL).  op describes the step as the builder set it up, with DEVICE pointers: a GEMM or a fused pair (kind 0 / 8)
  * in vf_layer_case's terms (layer; x / sc_x / resid / out_* / head_* / a_scale / a_shift point at the plan's buffers, fp16
  * planes [2][n_img][img_rows][C] with the lo plane right after the hi plane; sig: the signature vf_selftest_plan_gemms
- * reports), the other kinds in vf_op_case's (op).
- * row_valid / head_valid and vl_rows are HOST pointers into a copy of the plan's lengths table [18][batch] (NULL: uniform).
- * out_ptr / out_bytes are the byte ranges the launch may write; allocs are every device buffer of the plan. */
+ * reports), a GRU layer in vf_trace_gru's (gru), the other kinds in vf_op_case's (op).
+ * row_valid / head_valid / gru.lengths and vl_rows are HOST pointers into a copy of the plan's lengths table [18][batch]
+ * (NULL: uniform).  out_ptr / out_bytes are the byte ranges the step may write (the ISTFT's and the finalize's output is
+ * the caller's wav_out, outside the plan); allocs are every device buffer of the plan.  launches (valid when after = 1) is
+ * what the step added to vf_launch_count. */
 enum { VF_TRACE_GEMM = 0, VF_TRACE_FIRST = 1, VF_TRACE_POOL = 2, VF_TRACE_COND = 3, VF_TRACE_REFLECT = 4, VF_TRACE_TAIL = 5,
-       VF_TRACE_FINALIZE = 6, VF_TRACE_MEMSET = 7, VF_TRACE_PAIR = 8 };
+       VF_TRACE_FINALIZE = 6, VF_TRACE_MEMSET = 7, VF_TRACE_PAIR = 8, VF_TRACE_PLANES = 9, VF_TRACE_GRU = 10,
+       VF_TRACE_FRONTEND = 11, VF_TRACE_BAND = 12, VF_TRACE_ISTFT = 13 };
+/* One bidirectional GRU layer of a bi_gru plan, as vf_gru_case describes it, with each direction's weights where the loader
+ * put them: G [batch][T][1536] fp32; w_hh[d] [768][256] and b_hn[d] [256] fp32; out planes [2][batch][T][512] */
+typedef struct vf_trace_gru {
+  int batch, T, relu;
+  const float* G;
+  const float* w_hh[2];
+  const float* b_hn[2];
+  const int* lengths;       /* host: the lengths table's frames row, or NULL (T each) */
+  uint16_t* out;
+} vf_trace_gru;
 typedef struct vf_trace_op {
-  int list, index, kind;    /* list 0: the UNet's launches, 1: the vocoder's, 2: the finalize; kind: VF_TRACE_* */
+  int list, index, kind;    /* list 0: the analysis module's launches, 1: the vocoder's, 2: the finalize, 3: the steps the
+                               restore launches itself (front end, band sums, ISTFT); kind: VF_TRACE_* */
   char label[48];
   vf_layer_case layer;      /* GEMM / PAIR (the pair: x = the (a, r) planes it reads, out_a = the planes it writes) */
   vf_op_case op;            /* FIRST, POOL, COND (mel_target, band_sums: the unify inputs and sums, else NULL), REFLECT,
-                               TAIL, FINALIZE; MEMSET: planes = the cleared buffer, n = its bytes */
+                               TAIL, FINALIZE; MEMSET: planes = the cleared buffer, n = its bytes; PLANES (x, planes, T,
+                               bn1_scale / bn1_shift); FRONTEND (in_wav, n, T, the outputs it writes; clip_off: the host
+                               offsets of a varlen call); BAND: the memset and band_energy of unify_energy, in COND's unify
+                               fields (mel: the restored log-mel, mel_target, band_sums, T); ISTFT: the frames and
+                               overlap-add launches (mag, in_wav, frames, out, n, T, clip_off) */
   const int* vl_rows;       /* [18][batch] host, or NULL */
   int n_out;
   uint64_t out_ptr[4], out_bytes[4];
   int n_allocs;
   const uint64_t* alloc_ptr;
   const uint64_t* alloc_bytes;
+  vf_trace_gru gru;         /* GRU */
+  int launches;
 } vf_trace_op;
 typedef int (*vf_trace_fn)(void* user, int after, const vf_trace_op* op);
+#define VF_TRACE_DIRECT_STEPS 0x100u   /* vf_selftest_plan_trace: trace the front end, band sums and ISTFT as list 3 */
 VF_API int vf_selftest_plan_trace(vf_ctx* ctx, int plan_kind, const float* wav, const int64_t* offsets, int batch, int64_t n,
                                   unsigned flags, float* wav_out, vf_trace_fn fn, void* user);
 

@@ -1,24 +1,30 @@
 """Every launch of the restore plans, replayed against float64 on the plans' own weights and activations.
 
-vf_selftest_plan_trace runs one restore on a fresh plan one launch at a time and describes each launch as the builder set it
-up.  Around every launch this file
-  1. snapshots every buffer of the plan, and afterwards checks that no byte outside the launch's declared outputs changed
+vf_selftest_plan_trace runs one restore on a fresh plan one step at a time and describes each step as the builder or the
+restore path set it up: every launch of the analysis module's and the vocoder's lists, the finalize, and the launches the
+restore makes itself (the front end, unify_energy's band sums, the SSR ISTFT).  Around every step this file
+  1. snapshots every buffer of the plan, and afterwards checks that no byte outside the step's declared outputs changed
      (inside a GEMM's or a pair's outputs, no element outside its write set either);
-  2. checks every output value against the float64 reference of the same op, computed from the launch's own inputs as they
-     were just before it ran, with the weights the test maps from the launch's label to the state dict.  Each op starts from
+  2. checks every output value against the float64 reference of the same op, computed from the step's own inputs as they
+     were just before it ran, with the weights the test maps from the step's label to the state dict.  Each op starts from
      the engine's inputs, so errors do not carry from op to op and every op is held to the bound the layer suite
-     (test_gpu_layers.py) or the non-GEMM suite (test_gpu_aux.py) derives for it, at every element;
-  3. checks each GEMM's and pair's wiring: every operand, shortcut operand and residual was last written by the launch the
-     network's dataflow names (expected_producers), and in a varlen plan its row_valid is the lengths-table row of its
-     geometry, computed from the clip lengths;
+     (test_gpu_layers.py), the non-GEMM suite (test_gpu_aux.py), the front-end suite (test_gpu_frontend.py) or the GRU
+     suite (test_gpu_analysis.py) derives for it, at every element;
+  3. checks each step's wiring: every operand, shortcut operand and residual of a GEMM or pair, and what the GRU, the
+     input planes, the conditioning, the band sums, the UNet's first layer and the ISTFT read, was last written by the
+     step the network's dataflow names (expected_producers, expected_reads), and in a varlen plan a GEMM's row_valid is
+     the lengths-table row of its geometry, computed from the clip lengths;
   4. in a varlen plan, checks that the rows past each clip of every GEMM and pair input are zeros (of either sign), the
      precondition of the layer suite's varlen cases (rows past a clip in each output are checked as exact zeros by step 2).
 Then the traced output must equal the product call's bit for bit (eager and graph replay), and every op kind and every
-GEMM / pair configuration of the plan must have been replayed.
+GEMM / pair configuration of the plan must have been replayed.  The accounting test traces every plan kind each context
+builds and checks that the traced steps are every launch the product call makes, but for the lengths table.
 
 Inputs: seeded synthetic speech and one clip that widens the activations' range (digital silence, a full-scale click and
 a DC offset).  The UNet launches are the same for every vocoder mode, so the GSR plans pair the vocoder's 1- and 3-term
-modes with unify_energy off and on once each, uniform and varlen."""
+modes with unify_energy off and on once each, uniform and varlen; the bi_gru and dnn plans do the same with the other
+pairings.  Their varlen calls hold five clips, so that the GRU's groups of four clips split 4 + 1, and the shortest clip
+is 3 frames of a 128-frame bucket."""
 import ctypes
 import time
 import types
@@ -27,30 +33,63 @@ import numpy as np
 import pytest
 import torch
 
+import test_gpu_analysis as AN
 import test_gpu_aux as A
+import test_gpu_frontend as FE
 import test_gpu_layers as G
+from oracle import analysis as AO
 from oracle import layers as R
 from oracle import vf_oracle as O
 from voicefixer_main_b200 import _lib as VL
-from voicefixer_main_b200.arch import SSR_PREFIX, UNET_PREFIX
+from voicefixer_main_b200.arch import DNN_LINEARS, SSR_PREFIX, UNET_PREFIX
 
 pytestmark = pytest.mark.gpu
 
-GEMM, FIRST, POOL, COND, REFLECT, TAIL, FINALIZE, MEMSET, PAIR = range(9)       # VF_TRACE_* (include/b200vf.h)
-KIND_NAMES = ["gemm", "first", "pool", "cond", "reflect", "tail", "finalize", "memset", "pair"]
+# VF_TRACE_* (include/b200vf.h)
+GEMM, FIRST, POOL, COND, REFLECT, TAIL, FINALIZE, MEMSET, PAIR, PLANES, GRU, FRONTEND, BAND, ISTFT = range(14)
+KIND_NAMES = ["gemm", "first", "pool", "cond", "reflect", "tail", "finalize", "memset", "pair", "planes", "gru", "frontend",
+              "band", "istft"]
 SR, HOP = 44100, 441
 # 1 s, 0.5 s and the shortest clip a restore takes: a varlen bucket of 128 frames pads two of its three clips
 N_LONG, N_MID, N_MIN = SR, SR // 2, 1025
 CLAMP = np.float32(np.log10(np.float32(1e-8)))     # the front end's log10(max(mel, 1e-8))
-PLANS = {                                          # name -> (plan kind, vocoder terms, unify_energy)
-    "gsr.voc1": (0, 1, False),
-    "gsr.voc3.unify": (0, 3, True),
-    "gsr_varlen.voc1.unify": (2, 1, True),
-    "gsr_varlen.voc3": (2, 3, False),
-    "ssr": (1, 3, False),
-    "ssr_varlen": (3, 3, False),
+PLANS = {                                          # name -> (plan kind, vocoder terms, unify_energy, analysis module)
+    "gsr.voc1": (0, 1, False, "unet"),
+    "gsr.voc3.unify": (0, 3, True, "unet"),
+    "gsr_varlen.voc1.unify": (2, 1, True, "unet"),
+    "gsr_varlen.voc3": (2, 3, False, "unet"),
+    "ssr": (1, 3, False, "unet"),
+    "ssr_varlen": (3, 3, False, "unet"),
+    "bigru.voc1": (0, 1, False, "bi_gru"),
+    "bigru_varlen.voc3.unify": (2, 3, True, "bi_gru"),
+    "dnn.voc3.unify": (0, 3, True, "dnn"),
+    "dnn_varlen.voc1": (2, 1, False, "dnn"),
 }
 RESULTS = {}          # plan -> (kinds replayed, signatures replayed)
+# what the plan's conditioning (and the band sums) read as the restored mel: the analysis module's last launch, or the front
+# end's linear mel in a vocoder-only plan
+MEL_PRODUCER = {"unet": "post.conv2", "bi_gru": "bigru.lin6", "dnn": "dnn.lin5", "voc": "frontend"}
+
+
+def module_of(name):
+    """The network a replay's plan name stands for: "unet", "bi_gru", "dnn", "ssr" or "voc" (vocoder only)."""
+    for prefix, module in (("bigru", "bi_gru"), ("dnn", "dnn"), ("ssr", "ssr"), ("voc", "voc")):
+        if name.startswith(prefix):
+            return module
+    return "unet"
+
+
+def want_kinds(module, terms, unify):
+    """The step kinds a traced plan of `module` must go through."""
+    if module == "ssr":
+        return {FRONTEND, GEMM, FIRST, POOL, ISTFT}
+    kinds = {FRONTEND, GEMM, COND, REFLECT, MEMSET, TAIL, FINALIZE}
+    kinds |= {"unet": {FIRST, POOL}, "bi_gru": {PLANES, GRU}, "dnn": {PLANES}, "voc": set()}[module]
+    if terms == 1:
+        kinds.add(PAIR)
+    if unify:
+        kinds.add(BAND)
+    return kinds
 
 
 # ------------------------------------------------------------------ inputs
@@ -63,12 +102,15 @@ def wide_clip(n, seed):
     return x.clamp(-1, 1).float()
 
 
-def inputs(kind):
-    """(wav on the device, lengths or None)."""
-    if kind in (0, 1):
+def inputs(kind, five=False):
+    """(wav on the device, lengths or None).  five: the varlen call of the bi_gru / dnn plans, two more clips (a GRU
+    cluster takes four)."""
+    if kind in (0, 1, 4):
         wav = torch.stack([O.synth_clips(1, N_LONG, seed=11)[0].float(), wide_clip(N_LONG, 12)])
         return wav.cuda(), None
     clips = [O.synth_clips(1, N_MIN, seed=13)[0].float(), wide_clip(N_MID, 14), O.synth_clips(1, N_LONG, seed=15)[0].float()]
+    if five:
+        clips += [O.synth_clips(1, 30001, seed=16)[0].float(), wide_clip(20000, 17)]
     return torch.cat(clips).cuda(), [len(c) for c in clips]
 
 
@@ -171,7 +213,47 @@ def voc_spec(label, sd, cfg):
                 slope=cfg.voc_stage_slope if (ab == "b" and last) else cfg.voc_res_slope)
 
 
+def scalar_bn(sd, key):
+    """A BatchNorm2d(1) of the state dict as (weight, bias, running_mean, running_var) float32, the layer suite's in_bn."""
+    return np.array([float(sd[f"{key}.{k}"].reshape(-1)[0]) for k in ("weight", "bias", "running_mean", "running_var")],
+                    np.float32)
+
+
+def analysis_spec(label, sd):
+    """What plan.cu's build_bigru / build_dnn give the Linear `label`, as pack.cu packs it: weights [cout, cin, 1] (a one-tap
+    GEMM), bias, the epilogue's affine and activation.  A BatchNorm2d(1) before a dnn Linear is folded as pack_linear folds
+    it (R.bn_fold, rounded to the fp32 weights the loader uploads); BN_GRU.bn is bigru.lin1's epilogue affine, its fp32
+    scalar repeated over the channels."""
+    P = lambda k: sd[UNET_PREFIX + k].double()
+    spec = {}
+    if label.startswith("bigru.gru"):
+        l = int(label[len("bigru.gru")])
+        g = lambda n: torch.cat([P(f"2.gru.{n}_l{l}"), P(f"2.gru.{n}_l{l}_reverse")])
+        w, b = g("weight_ih"), R.gru_ih_bias(g("bias_ih"), g("bias_hh"))
+    elif label.startswith("bigru."):
+        idx = {"bigru.lin1": 1, "bigru.lin4": 4, "bigru.lin6": 6}[label]
+        w, b = P(f"{idx}.weight"), P(f"{idx}.bias")
+        if idx == 1:
+            s, t = R.bn_scalar(scalar_bn(sd, UNET_PREFIX + "2.bn"))
+            spec.update(bn=(np.full(w.shape[0], s, np.float32), np.full(w.shape[0], t, np.float32)), act=0, slope=0.0)
+        elif idx == 4:
+            spec.update(act=1, slope=0.0)
+    else:
+        i = int(label[len("dnn.lin"):])
+        idx = DNN_LINEARS[i]
+        w, b = P(f"{idx}.weight"), P(f"{idx}.bias")
+        if 1 <= i <= 4:
+            w, b = R.bn_fold(w.float(), b.float(), scalar_bn(sd, UNET_PREFIX + str(idx - 1)))
+            w = w.float().double()
+        if i < 5:
+            spec.update(act=1, slope=0.0)
+    spec.update(w=w[:, :, None], b=b)
+    return spec
+
+
 def spec_of(label, sd, cfg, C):
+    if label.startswith(("bigru.", "dnn.")):
+        return analysis_spec(label, sd)
     if label.startswith("voc."):
         return voc_spec(label, sd, cfg)
     if label.startswith("ssr."):
@@ -195,8 +277,10 @@ class Replay:
         self.t_ref = self.t_snap = 0.0
         self.arena = 0
         self.clamped = []
-        self.writers = []         # (first byte, end, label) of every launch's outputs so far, in launch order
+        self.writers = []         # (first byte, end, label) of every step's outputs so far, in launch order
         self.lengths = None
+        self.module = module_of(name)
+        self.launches = 0         # what the traced steps added to vf_launch_count
 
     # ---- containment
     def on_op(self, after, t):
@@ -232,6 +316,7 @@ class Replay:
         self.t_ref += time.perf_counter() - t1
         self.writers += [(t.out_ptr[i], t.out_ptr[i] + t.out_bytes[i], label) for i in range(t.n_out)]
         self.ops += 1
+        self.launches += t.launches
         self.kinds.add(t.kind)
         if t.kind in (GEMM, PAIR):
             self.sigs.add(t.layer.sig.decode())
@@ -263,6 +348,25 @@ class Replay:
         elif t.kind == FIRST:
             o = t.op
             cap["x"] = host(o.x, np.float32, (o.batch, o.T, o.W + 1))
+        elif t.kind == PLANES:
+            o = t.op
+            cap["x"] = host(o.x, np.float32, (o.batch, o.T, 128))
+        elif t.kind == GRU:
+            g = t.gru
+            cap["G"] = host(g.G, np.float32, (g.batch, g.T, 1536))
+        elif t.kind == FRONTEND:
+            o = t.op
+            cap["wav"] = host(o.in_wav, np.float32, (self.samples(o),))
+            cap["before"] = {k: host(getattr(o, k), np.uint32, (o.batch, o.T, FE.WIDTH[k])) for k in FE.OUTS if getattr(o, k)}
+        elif t.kind == BAND:
+            o = t.op
+            cap["mel"] = host(o.mel, np.float32, (o.batch, o.T, 128))
+            cap["tgt"] = host(o.mel_target, np.float32, (o.batch, o.T, 128))
+        elif t.kind == ISTFT:
+            o = t.op
+            cap["mag"] = host(o.mag, np.float32, (o.batch, o.T, 1025))
+            cap["wav"] = host(o.in_wav, np.float32, (self.samples(o),))
+            cap["frames"] = host(o.frames, np.uint32, (o.batch, o.T, 2048))
         elif t.kind == POOL:
             o = t.op
             cap["x"] = host(o.pin, np.float32, (o.batch, o.H, o.W + 1, o.C))
@@ -281,7 +385,33 @@ class Replay:
             o = t.op
             cap["wav"] = host(o.in_wav, np.float32, (o.batch, o.L))
             cap["peak"] = host(o.peak_bits, np.uint32, (o.batch,))
+        if t.kind not in (GEMM, PAIR):
+            self.check_reads(t, label)
         return cap
+
+    def samples(self, o):
+        """Samples of the call's input (and of the ISTFT's output): packed clips, or batch x n."""
+        return sum(self.lengths) if self.lengths else o.batch * o.n
+
+    def clips(self, wav, o):
+        """The call's input as a list of clips."""
+        if not self.lengths:
+            return [wav[i * o.n:(i + 1) * o.n] for i in range(o.batch)]
+        off = np.concatenate([[0], np.cumsum(self.lengths)])
+        return [wav[off[i]:off[i + 1]] for i in range(len(self.lengths))]
+
+    def check_reads(self, t, label):
+        """What a step other than a GEMM or a pair reads was last written by the step the plan's dataflow names
+        (expected_reads)."""
+        o = t.op
+        ptrs = {PLANES: lambda: {"x": o.x}, GRU: lambda: {"G": t.gru.G}, FIRST: lambda: {"x": o.x},
+                COND: lambda: {"mel": o.mel, **({"band_sums": o.band_sums} if o.unify else {})},
+                BAND: lambda: {"mel": o.mel, "mel_target": o.mel_target}, ISTFT: lambda: {"mag": o.mag}}
+        if t.kind not in ptrs:
+            return
+        got = {k: self.producer(p) for k, p in ptrs[t.kind]().items()}
+        want = expected_reads(t.kind, label, self.module, t.kind == COND and bool(o.unify))
+        assert got == want, (self.name, label, "reads", got, "expected", want)
 
     def outputs(self, t):
         """The GEMM's / pair's output buffers, keyed as test_gpu_layers' b.buf."""
@@ -322,7 +452,9 @@ class Replay:
             return
         off = np.concatenate([[0], np.cumsum(self.lengths)])
         table = A.lengths_rows(off, 1024 if self.name.startswith("ssr") else 127)
-        if label.startswith("voc.cond") or label == "voc.stem":
+        if label.startswith(("bigru.", "dnn.")):
+            row = 0
+        elif label.startswith("voc.cond") or label == "voc.stem":
             row = 9
         elif label.startswith("voc."):
             row = 10 + int(label.split(".")[1][-1])
@@ -336,10 +468,14 @@ class Replay:
     def check_zero_input(self, t, label, cap):
         """The layer suite's varlen precondition (test_gpu_layers.build): the operand and the residual are zeros past each
         clip's rows (CONVT1D: past its input rows).  The stem's input rows past a clip hold the reflection padding and rows
-        no launch writes; it reads rows t .. t + 6 of valid output rows t only, and is not held to it."""
+        no launch writes; it reads rows t .. t + 6 of valid output rows t only, and is not held to it.  Nor is the front
+        end's log-mel, the residual of an analysis module's last Linear: the front end leaves the rows past a clip as they
+        were, and the epilogue writes zeros to those output rows whatever it adds there (checked by the replay)."""
         lc = t.layer
         if lc.kind == G.CONV1D and not lc.centered:
             return
+        if "resid" in cap and self.producer(lc.resid) == "frontend":
+            cap = {k: v for k, v in cap.items() if k != "resid"}
         rv = rows_of(lc.row_valid, lc.n_img)
         lim = rv if lc.kind != G.CONVT1D else (rv + lc.stride - 1) // lc.stride
         for i in range(lc.n_img):
@@ -350,10 +486,34 @@ class Replay:
                 assert not r.any(), (self.name, label, "residual rows past clip", i, "are not zero")
 
 
+def expected_reads(kind, label, module, unify=False):
+    """{input: label of the step that must have written it last} for a step other than a GEMM or a pair: the input planes
+    and the UNet's first layer read the front end's log-mel (SSR: its magnitudes), each GRU layer the G of its own input
+    projection (both layers share one G buffer), the conditioning and the band sums the restored log-mel (a vocoder-only
+    plan: the front end's linear mel), the band sums also the front end's linear mel, the ISTFT the SSR UNet's magnitudes."""
+    if kind in (PLANES, FIRST):
+        return {"x": "frontend"}
+    if kind == GRU:
+        return {"G": label + ".ih"}
+    if kind == COND:
+        return {"mel": MEL_PRODUCER[module], **({"band_sums": "band_energy"} if unify else {})}
+    if kind == BAND:
+        return {"mel": MEL_PRODUCER[module], "mel_target": "frontend"}
+    return {"mag": "ssr.post.conv2"}
+
+
 def expected_producers(label, cfg):
     """{input: label of the launch that must have written it last} for the GEMM or pair `label` (plan.cu's dataflow: each
     block's conv1 reads the previous block's activated output, conv2 reads its conv1, the residual stream runs from block
-    to block; the non-GEMM producers carry their kind's name)."""
+    to block; the non-GEMM producers carry their kind's name).  The analysis modules' Linear layers read the previous
+    launch's output; their last one adds the front end's log-mel."""
+    if label.startswith("bigru."):
+        x = {"bigru.lin1": "analysis.in_planes", "bigru.gru0.ih": "bigru.lin1", "bigru.gru1.ih": "bigru.gru0",
+             "bigru.lin4": "bigru.gru1", "bigru.lin6": "bigru.lin4"}[label]
+        return {"x": x, **({"resid": "frontend"} if label == "bigru.lin6" else {})}
+    if label.startswith("dnn."):
+        i = int(label[len("dnn.lin"):])
+        return {"x": "analysis.in_planes" if i == 0 else f"dnn.lin{i - 1}", **({"resid": "frontend"} if i == 5 else {})}
     if label.startswith("voc."):
         p = label.split(".")
         if p[1].startswith("cond"):
@@ -583,23 +743,135 @@ def check_finalize(rp, t, label, ck):
         assert np.array_equal(out[off[i]:off[i + 1]], want), (ck.name, i)
 
 
+def clip_frames(rp, t, B, T):
+    vl = vl_table(t, B)
+    return [T] * B if vl is None else [int(v) for v in vl[0]]
+
+
+def check_planes(rp, t, label, ck):
+    """Bit-exact, as test_gpu_aux.test_input_planes_are_exact: BN0's scale and shift as load_bigru folds them (dnn: 1, 0)."""
+    o = t.op
+    B = o.batch
+    s, sh = (R.bn_scalar(scalar_bn(rp.sd, UNET_PREFIX + "0")) if rp.module == "bi_gru" else (1.0, 0.0))
+    assert (o.bn1_scale, o.bn1_shift) == (np.float32(s), np.float32(sh)), (ck.name, o.bn1_scale, o.bn1_shift)
+    Ts = clip_frames(rp, t, B, o.T)
+    want = R.affine_planes(rp.cap["x"], o.bn1_scale, o.bn1_shift, Ts if rp.varlen else None)
+    bad = np.argwhere(planes(o.planes, B, o.T, 128) != want)
+    assert not len(bad), (ck.name, f"{len(bad)} elements differ, first [plane, clip, row, channel] {bad[:4].tolist()}")
+
+
+def check_gru(rp, t, label, ck):
+    """oracle/analysis.gru_layer from the captured G with the state dict's weight_hh / bias_hh (the device copies must be
+    those fp32 tensors bit for bit), ReLU on layer 1 only, each clip over its own frames: |err| < GRU_TOL
+    (test_gpu_analysis.py) and exact zeros past each clip."""
+    g = t.gru
+    l = int(label[len("bigru.gru")])
+    key = lambda n, d: UNET_PREFIX + f"2.gru.{n}_l{l}" + ("_reverse" if d else "")
+    w = torch.stack([rp.sd[key("weight_hh", d)].float() for d in range(2)])
+    bh = torch.stack([rp.sd[key("bias_hh", d)].float()[512:] for d in range(2)])
+    for d in range(2):
+        assert np.array_equal(host(g.w_hh[d], np.uint32, (768, 256)), w[d].numpy().view(np.uint32)), (ck.name, "w_hh", d)
+        assert np.array_equal(host(g.b_hn[d], np.uint32, (256,)), bh[d].numpy().view(np.uint32)), (ck.name, "b_hn", d)
+    assert g.relu == l, (ck.name, "relu", g.relu)
+    B, T = g.batch, g.T
+    Ts = clip_frames(rp, t, B, T)
+    if rp.varlen:
+        assert list(rows_of(g.lengths, B)) == Ts, (ck.name, "lengths are not the frames row")
+    else:
+        assert not g.lengths, ck.name
+    want = AO.gru_layer(torch.from_numpy(rp.cap["G"]).double(), w.double(), bh.double(), Ts, relu=bool(l)).numpy()
+    got = A.hi_lo(planes(g.out, B, T, 512))
+    zero = np.zeros((B, T, 1), bool)
+    for i, Tb in enumerate(Ts):
+        zero[i, Tb:] = True
+    ck.values("gru", got, want, np.full(got.shape, AN.GRU_TOL), zero)
+
+
+def check_frontend(rp, t, label, ck):
+    """test_gpu_frontend.check_frontend's bounds on every output the restore asks for; rows past a varlen clip are not
+    written."""
+    o = t.op
+    outs = {}
+    for k in FE.OUTS:
+        full = np.full((o.batch, o.T, FE.WIDTH[k]), G.SENT32, np.uint32)
+        if getattr(o, k):
+            got = host(getattr(o, k), np.uint32, full.shape)
+            for b, x in enumerate(rp.clips(rp.cap["wav"], o)):
+                Tb = 1 + len(x) // HOP
+                assert np.array_equal(got[b, Tb:], rp.cap["before"][k][b, Tb:]), (ck.name, k, b, "rows past the clip written")
+                full[b, :Tb] = got[b, :Tb]
+        outs[k] = full
+    want = [k for k in FE.OUTS if getattr(o, k)]
+    res = FE.check_frontend(ck.name, rp.clips(rp.cap["wav"], o), outs, O.mel_filterbank().numpy(), want)
+    ck.worst = max(ck.worst, res.worst)
+
+
+def check_band(rp, t, label, ck):
+    """unify_energy's sums against R.band_sums within test_gpu_aux.band_bound."""
+    o = t.op
+    sums = host(o.band_sums, np.float32, (o.batch, 2)).astype(np.float64)
+    for b, Tb in enumerate(clip_frames(rp, t, o.batch, o.T)):
+        s64 = R.band_sums(rp.cap["tgt"][b:b + 1], rp.cap["mel"][b:b + 1], [Tb])
+        ck.values("band", sums[b], s64[0], A.band_bound(rp.cap["tgt"][b], rp.cap["mel"][b], Tb) + G.FLOOR, np.zeros(1, bool))
+
+
+def check_istft(rp, t, label, ck):
+    """The fused ISTFT's frames and overlap-add within test_gpu_aux.fused_istft's bounds, from the captured magnitudes and
+    the input's phase; frames past a varlen clip are not written."""
+    o = t.op
+    wav, mag = rp.cap["wav"], rp.cap["mag"]
+    frames = host(o.frames, np.uint32, (o.batch, o.T, 2048))
+    out = host(o.out, np.uint32, (rp.samples(o),))
+    c_fft = 4 * A.U * np.log2(2048)
+    win = R.hann()
+    start = 0
+    for b, x in enumerate(rp.clips(wav, o)):
+        nb, Tb = len(x), 1 + len(x) // HOP
+        X, S = R.stft64(x, Tb)
+        cs, sn = R.phase(X)
+        mg = mag[b, :Tb].astype(np.float64)
+        f64 = R.inverse_frames(mg * (cs + 1j * sn))
+        E = A.istft_frame_error(mg, np.minimum(2.0, c_fft * S[:, None] / np.maximum(np.abs(X), 1e-4)))
+        ck.values("frames", frames[b, :Tb].view(np.float32).astype(np.float64), f64,
+                  win[None] * E[:, None] + A.gamma(3) * np.abs(f64) + G.FLOOR, (S == 0)[:, None])
+        assert np.array_equal(frames[b, Tb:], rp.cap["frames"][b, Tb:]), (ck.name, b, "frames past the clip written")
+        y, bnd = A.ola_bound(f64, E, nb)
+        ck.values("out", out[start:start + nb].view(np.float32).astype(np.float64), y, bnd, np.zeros(1, bool))
+        start += nb
+
+
 CHECKS = {GEMM: check_gemm, PAIR: check_pair, FIRST: check_first, POOL: check_pool, COND: check_cond, REFLECT: check_reflect,
-          MEMSET: check_memset, TAIL: check_tail, FINALIZE: check_finalize}
+          MEMSET: check_memset, TAIL: check_tail, FINALIZE: check_finalize, PLANES: check_planes, GRU: check_gru,
+          FRONTEND: check_frontend, BAND: check_band, ISTFT: check_istft}
 
 
 # ------------------------------------------------------------------ tests
 @pytest.fixture(scope="module")
 def setup():
+    """engine(module) -> (Engine, state dict, config): one context per analysis module, loaded once.  "unet" also holds the
+    SSR UNet; "bi_gru" and "dnn" hold their module and the vocoder (test_gpu_analysis.py's states)."""
     from voicefixer_main_b200.model import Engine
-    from voicefixer_main_b200.weights import make_ssr_state, make_state
-    sd = {**make_state(1234), **make_ssr_state(1234)}
-    e = Engine("cuda:0")
-    e.load_state(sd, need=("unet", "vocoder", "ssr"))
+    from voicefixer_main_b200.weights import make_bigru_state, make_dnn_state, make_ssr_state, make_state, make_vocoder_state
     cfg = VL.VfConfig()
     VL.load_library().vf_default_config(ctypes.byref(cfg))
-    yield e, sd, cfg
-    e.check_errors()
-    e.close()
+    engines = {}
+
+    def engine(module):
+        if module not in engines:
+            if module == "unet":
+                sd, need = {**make_state(1234), **make_ssr_state(1234)}, ("unet", "vocoder", "ssr")
+            else:
+                sd = {**(make_bigru_state if module == "bi_gru" else make_dnn_state)(1234), **make_vocoder_state(seed=1235)}
+                need = (module, "vocoder")
+            e = Engine("cuda:0")
+            e.load_state(sd, need=need)
+            engines[module] = (e, sd, cfg)
+        return engines[module]
+
+    yield engine
+    for e, _, _ in engines.values():
+        e.check_errors()
+        e.close()
 
 
 def product(e, kind, wav, lengths, unify):
@@ -609,21 +881,23 @@ def product(e, kind, wav, lengths, unify):
         return e.ssr_forward(None, wav)
     if kind == 2:
         return e.restore_varlen(wav, lengths, unify_energy=unify)
-    return e.ssr_restore_varlen(wav, lengths)
+    if kind == 3:
+        return e.ssr_restore_varlen(wav, lengths)
+    return e.resynth(wav) if kind == 4 else e.resynth_varlen(wav, lengths)
 
 
 def replay(setup, name):
-    e, sd, cfg = setup
-    kind, terms, unify = PLANS[name]
+    kind, terms, unify, module = PLANS[name]
+    e, sd, cfg = setup(module)
     e.set_option("vocoder_terms", terms)
-    wav, lengths = inputs(kind)
+    wav, lengths = inputs(kind, five=module != "unet")
     rp = Replay(name, sd, cfg, lengths is not None)
     rp.lengths = lengths
     PAIR_STAGE.clear()
     if terms == 1:
         PAIR_STAGE[cfg.voc_num_stages - 1] = True          # the C = 64 stack of the (a, r) stream (plan.cu: fused)
     t0 = time.perf_counter()
-    got = e.selftest_plan_trace(kind, wav, lengths, rp.on_op, unify_energy=unify)
+    got = e.selftest_plan_trace(kind, wav, lengths, rp.on_op, unify_energy=unify, direct_steps=True)
     wall = time.perf_counter() - t0
     e.check_errors()
     # the product call on the same input, eager then from its graph, equals the traced run bit for bit
@@ -636,8 +910,7 @@ def replay(setup, name):
     T = (1 + max(lengths) // HOP + 63) // 64 * 64 if lengths else 1 + wav.shape[1] // HOP
     sigs = {sg for _, sg in e.selftest_plan_gemms(kind, n, T)}
     assert sigs == rp.sigs, (name, "configurations not replayed", sigs - rp.sigs)
-    assert rp.kinds == ({GEMM, FIRST, POOL} if kind in (1, 3) else {GEMM, FIRST, POOL, COND, REFLECT, MEMSET, TAIL, FINALIZE, PAIR}
-                        if terms == 1 else {GEMM, FIRST, POOL, COND, REFLECT, MEMSET, TAIL, FINALIZE}), (name, rp.kinds)
+    assert rp.kinds == want_kinds("ssr" if kind in (1, 3) else module, terms, unify), (name, sorted(rp.kinds))
     RESULTS[name] = (rp.kinds, rp.sigs)
     print(f"{name}: {rp.ops} ops, worst err / bound {rp.worst:.3e} at {rp.worst_op}; arena {rp.arena / 2 ** 20:.1f} MiB; "
           f"snapshots + containment {rp.t_snap:.1f} s, float64 references + checks {rp.t_ref:.1f} s, wall {wall:.1f} s")
@@ -661,3 +934,59 @@ def test_replays_cover_every_op_kind(setup):
     sigs = set().union(*(s for _, s in RESULTS.values()))
     assert any("resid=ar" in s for s in sigs) and any("resid=planes" in s for s in sigs)
     assert any("varlen=1" in s for s in sigs) and any(s.startswith("pair") for s in sigs)
+
+
+# the plan kinds each context builds: GSR 0 / 2 (with unify_energy), SSR 1 / 3, vocoder-only 4 / 5
+ACCOUNTING = [("unet", k, u) for k, u in ((0, True), (2, True), (1, False), (3, False), (4, False), (5, False))] + \
+             [(m, k, k in (0, 2)) for m in ("bi_gru", "dnn") for k in (0, 2, 4, 5)]
+SETUP_LAUNCHES = {"lengths table": lambda varlen: int(varlen)}     # launches a call makes that the trace does not replay
+
+
+def test_traced_steps_are_every_launch_of_the_product_call(setup):
+    """For every plan kind of every context: the trace runs to completion and goes through every GEMM / pair configuration
+    vf_selftest_plan_gemms reports, and with graphs off the product call's launch count is the traced steps' plus
+    SETUP_LAUNCHES.  Without direct_steps the trace goes through the same steps but those of list 3.  Every step kind the
+    plans have is among CHECKS."""
+    seen = set()
+    for module, kind, unify in ACCOUNTING:
+        e, _, _ = setup(module)
+        e.set_option("vocoder_terms", 1)
+        wav, lengths = inputs(kind, five=module != "unet")
+        steps = {"kinds": set(), "sigs": set(), "launches": 0, "order": []}
+
+        def on_op(after, t):
+            if after:
+                steps["order"].append((t.list, t.label.decode()))
+                steps["kinds"].add(t.kind)
+                steps["launches"] += t.launches
+                if t.kind in (GEMM, PAIR):
+                    steps["sigs"].add(t.layer.sig.decode())
+
+        got = e.selftest_plan_trace(kind, wav, lengths, on_op, unify_energy=unify, direct_steps=True)
+        listed = []
+        plain = e.selftest_plan_trace(kind, wav, lengths, lambda after, t: listed.append((t.list, t.label.decode())) if after
+                                      else None, unify_energy=unify)
+        e.set_option("graphs", 0)
+        try:
+            n0 = e.launch_count()
+            want = product(e, kind, wav, lengths, unify)
+            torch.cuda.synchronize()
+            launches = e.launch_count() - n0
+        finally:
+            e.set_option("graphs", 1)
+        e.check_errors()
+        tag = (module, kind, unify)
+        assert torch.equal(got.view(torch.int32), want.view(torch.int32)), tag
+        assert torch.equal(plain.view(torch.int32), want.view(torch.int32)), tag
+        assert listed == [s for s in steps["order"] if s[0] != 3], (tag, "steps without direct_steps")
+        n = len(lengths) if lengths else wav.shape[0]
+        T = (1 + max(lengths) // HOP + 63) // 64 * 64 if lengths else 1 + wav.shape[1] // HOP
+        assert {sg for _, sg in e.selftest_plan_gemms(kind, n, T)} == steps["sigs"], tag
+        setup_launches = sum(f(lengths is not None) for f in SETUP_LAUNCHES.values())
+        assert launches == steps["launches"] + setup_launches, (tag, launches, steps["launches"], setup_launches)
+        mod = "ssr" if kind in (1, 3) else "voc" if kind in (4, 5) else module
+        assert steps["kinds"] == want_kinds(mod, 1, unify), (tag, sorted(steps["kinds"]))
+        print(f"{module} plan {kind}{' unify' if unify else ''}: {launches} launches = {steps['launches']} traced + "
+              f"{setup_launches} set-up")
+        seen |= steps["kinds"]
+    assert seen == set(CHECKS), sorted(seen)

@@ -230,7 +230,7 @@ def test_vocoder_plans_replay_against_float64(replay_setup, name):
     if terms == 1:
         PR.PAIR_STAGE[cfg.voc_num_stages - 1] = True
     try:
-        got = e.selftest_plan_trace(kind, wav, lengths, rp.on_op)
+        got = e.selftest_plan_trace(kind, wav, lengths, rp.on_op, direct_steps=True)
         e.check_errors()
         for _ in range(2):          # eager, then from the plan's graph
             want = e.resynth(wav) if lengths is None else e.resynth_varlen(wav, lengths)
@@ -241,8 +241,7 @@ def test_vocoder_plans_replay_against_float64(replay_setup, name):
         gemms = e.selftest_plan_gemms(kind, n, T)
         assert gemms and all(label.startswith("voc.") for label, _ in gemms), name
         assert {sg for _, sg in gemms} == rp.sigs, (name, "configurations not replayed")
-        want_kinds = {PR.GEMM, PR.COND, PR.REFLECT, PR.MEMSET, PR.TAIL, PR.FINALIZE} | ({PR.PAIR} if terms == 1 else set())
-        assert rp.kinds == want_kinds, (name, rp.kinds)
+        assert rp.kinds == PR.want_kinds("voc", terms, False), (name, rp.kinds)
         print(f"{name}: {rp.ops} ops, worst err / bound {rp.worst:.3e} at {rp.worst_op}; arena {rp.arena / 2 ** 20:.1f} MiB")
     finally:
         e.set_option("vocoder_terms", 1)

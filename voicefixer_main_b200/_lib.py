@@ -28,6 +28,7 @@ EXPORTS = [
     "vf_resynth_varlen", "vf_selftest_sub_batch", "vf_vocoder_chunks",
 ]
 VF_RESTORE_UNIFY_ENERGY = 1
+VF_TRACE_DIRECT_STEPS = 0x100
 VF_SSR_PEAK_NORMALISE = 1
 
 
@@ -85,12 +86,18 @@ class VfPlanGemm(Structure):
     _fields_ = [("label", c_char * 48), ("sig", c_char * 160), ("tiles", c_int64), ("grid", c_int), ("col_tiles", c_int)]
 
 
+class VfTraceGru(Structure):
+    """vf_trace_gru (include/b200vf.h): one GRU layer of a traced bi_gru plan (tests only)."""
+    _fields_ = [("batch", c_int), ("T", c_int), ("relu", c_int), ("G", c_void_p), ("w_hh", c_void_p * 2),
+                ("b_hn", c_void_p * 2), ("lengths", c_void_p), ("out", c_void_p)]
+
+
 class VfTraceOp(Structure):
-    """vf_trace_op (include/b200vf.h): one launch of a plan as vf_selftest_plan_trace describes it (tests only)."""
+    """vf_trace_op (include/b200vf.h): one step of a plan as vf_selftest_plan_trace describes it (tests only)."""
     _fields_ = [("list", c_int), ("index", c_int), ("kind", c_int), ("label", c_char * 48), ("layer", VfLayerCase),
                 ("op", VfOpCase), ("vl_rows", c_void_p), ("n_out", c_int), ("out_ptr", c_uint64 * 4),
                 ("out_bytes", c_uint64 * 4), ("n_allocs", c_int), ("alloc_ptr", POINTER(c_uint64)),
-                ("alloc_bytes", POINTER(c_uint64))]
+                ("alloc_bytes", POINTER(c_uint64)), ("gru", VfTraceGru), ("launches", c_int)]
 
 
 VF_TRACE_FN = ctypes.CFUNCTYPE(c_int, c_void_p, c_int, POINTER(VfTraceOp))

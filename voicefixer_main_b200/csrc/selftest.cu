@@ -370,8 +370,9 @@ int run_op_case(vf_ctx* ctx, Case& s, vf_op_case& c) {
   return run_ops(ctx, ops, 0);
 }
 
-// vf_selftest_plan_trace: one launch of a plan at a time, each described in the hooks' case vocabulary and handed to the
-// caller's function before and after it runs.
+// vf_selftest_plan_trace: one step of a plan at a time - a launch of its lists, or a launch group the restore paths make
+// themselves (list 3) - each described in the hooks' case vocabulary and handed to the caller's function before and after
+// it runs.
 struct Tracer {
   vf_ctx* ctx;
   Plan& plan;
@@ -593,8 +594,64 @@ struct Tracer {
         out(t, f.out, (size_t)samples * 4);
         return VF_OK;
       }
+      case OP_PLANES: {
+        t->kind = VF_TRACE_PLANES;
+        const AffinePlanesParams& p = op.planes;
+        c.kind = VF_OP_PLANES;
+        c.T = p.T; c.x = p.in; c.bn1_scale = p.scale; c.bn1_shift = p.shift; c.planes = (uint16_t*)p.out.hi;
+        const size_t elems = (size_t)p.batch * p.T * p.C;
+        int rc = adjacent("out", p.out.hi, p.out.lo, elems, op.label);
+        if (rc) return rc;
+        out(t, p.out.hi, 2 * elems * 2);
+        return VF_OK;
+      }
+      case OP_GRU: {
+        t->kind = VF_TRACE_GRU;
+        const GruParams& p = op.gru;
+        vf_trace_gru& g = t->gru;
+        g.batch = p.batch; g.T = p.T; g.relu = p.relu; g.G = p.G; g.out = (uint16_t*)p.out.hi;
+        for (int d = 0; d < 2; ++d) { g.w_hh[d] = p.w_hh[d]; g.b_hn[d] = p.b_hn[d]; }
+        g.lengths = host_rows(p.vl_T);
+        const size_t elems = (size_t)p.batch * p.T * 2 * GRU_HIDDEN;
+        int rc = adjacent("out", p.out.hi, p.out.lo, elems, op.label);
+        if (rc) return rc;
+        out(t, p.out.hi, 2 * elems * 2);
+        return VF_OK;
+      }
       default: return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: op kind %d is not traced", (int)op.kind);
     }
+  }
+
+  // The steps of list 3: launches the restore paths make themselves rather than through a launch list
+  void describe_direct(int kind, const char* label, vf_trace_op* t) {
+    memset(t, 0, sizeof *t);
+    t->list = 3; t->index = n_direct++; t->kind = kind;
+    snprintf(t->label, sizeof t->label, "%s", label);
+    t->vl_rows = plan.d_vl_rows ? vl.data() : nullptr;
+    t->n_allocs = (int)aptr.size();
+    t->alloc_ptr = aptr.data();
+    t->alloc_bytes = abytes.data();
+    t->op.batch = plan.batch;
+  }
+
+  // Hands `t` to fn, runs launch() (which counts its launches in ctx->launches as the product path does), hands t to fn again
+  template <typename F>
+  int run_step(vf_trace_op& t, F launch) {
+    CK(cudaDeviceSynchronize());
+    if (fn(user, 0, &t)) return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: stopped before %s", t.label);
+    const int64_t launches = ctx->launches;
+    int rc = launch();
+    if (rc) return rc;
+    t.launches = (int)(ctx->launches - launches);
+    CK(cudaDeviceSynchronize());
+    if (fn(user, 1, &t)) return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: stopped after %s", t.label);
+    return VF_OK;
+  }
+
+  // A step of list 3: traced with VF_TRACE_DIRECT_STEPS, else launched as the restore launches it
+  template <typename F>
+  int direct_step(vf_trace_op& t, F launch) {
+    return direct ? run_step(t, launch) : launch();
   }
 
   // Describes `op`, hands it to fn, runs it alone, hands it to fn again
@@ -602,18 +659,19 @@ struct Tracer {
     vf_trace_op t;
     int rc = describe(op, list, index, &t);
     if (rc) return rc;
-    CK(cudaDeviceSynchronize());
-    if (fn(user, 0, &t)) return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: stopped before %s", t.label);
-    std::vector<Op> one{op};
-    rc = run_ops(ctx, one, 0);
-    if (rc) return rc;
-    CK(cudaDeviceSynchronize());
-    if (fn(user, 1, &t)) return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: stopped after %s", t.label);
-    return VF_OK;
+    return run_step(t, [&] {
+      std::vector<Op> one{op};
+      return run_ops(ctx, one, 0);
+    });
   }
+
+  bool direct = false;       // VF_TRACE_DIRECT_STEPS
+  int n_direct = 0;
 };
 
-// The restore of vf_selftest_plan_trace on the case's plan, step for step as restore_impl, ssr_impl and resynth_impl run it
+// The restore of vf_selftest_plan_trace on the case's plan, step for step as restore_impl, ssr_impl and resynth_impl run it:
+// the same launches with the same arguments in the same order, each step counted in ctx->launches as they count it.  Only
+// the lengths table of a varlen plan is written untraced.
 int run_trace(vf_ctx* ctx, Case& s, int kind, const float* wav, const int64_t* off, int batch, int64_t n, int T, unsigned flags,
               float* wav_out, vf_trace_fn fn, void* user) {
   Plan& plan = s.plan;
@@ -622,29 +680,53 @@ int run_trace(vf_ctx* ctx, Case& s, int kind, const float* wav, const int64_t* o
   if (rc) return rc;
   const bool ssr = is_ssr_plan(kind), voc = is_voc_plan(kind);
   Tracer tr{ctx, plan, fn, user, {}, {}, {}};
+  tr.direct = (flags & VF_TRACE_DIRECT_STEPS) != 0;
   for (size_t i = 0; i < plan.allocs.size(); ++i) {
     tr.aptr.push_back((uint64_t)(uintptr_t)plan.allocs[i]);
     tr.abytes.push_back(plan.alloc_bytes[i]);
   }
   if (off && (rc = write_lengths_table(ctx, &plan, off, batch, ssr ? 1024 : 127, 0))) return rc;
-  rc = run_frontend(ctx, wav, batch, (long)n, ssr ? nullptr : plan.d_mel, plan.d_logmel_in, ssr ? plan.d_sp : nullptr,
-                    nullptr, nullptr, 0, off ? &plan : nullptr);
-  if (rc) return rc;
   CK(cudaDeviceSynchronize());
   if (off) {
     tr.vl.resize((size_t)VL_ROWS * batch);
     CK(cudaMemcpy(tr.vl.data(), plan.d_vl_rows, tr.vl.size() * sizeof(int), cudaMemcpyDeviceToHost));
   }
+  const size_t rows = (size_t)batch * T;
+  const int64_t samples = off ? off[batch] : (int64_t)batch * n;
+  {   // the front end: restore_impl's and resynth_impl's mels, ssr_impl's magnitudes
+    vf_trace_op t;
+    tr.describe_direct(VF_TRACE_FRONTEND, "frontend", &t);
+    vf_op_case& c = t.op;
+    c.kind = VF_OP_FRONTEND; c.clip_off = off; c.n = n; c.T = T; c.in_wav = wav;
+    c.mel_out = ssr ? nullptr : plan.d_mel; c.logmel_out = plan.d_logmel_in; c.sp_out = ssr ? plan.d_sp : nullptr;
+    tr.out(&t, c.mel_out, rows * 128 * 4);
+    tr.out(&t, c.logmel_out, rows * 128 * 4);
+    tr.out(&t, c.sp_out, rows * 1025 * 4);
+    rc = tr.direct_step(t, [&] {
+      return run_frontend(ctx, wav, batch, (long)n, c.mel_out, c.logmel_out, c.sp_out, nullptr, nullptr, 0, off ? &plan : nullptr);
+    });
+    if (rc) return rc;
+  }
   if (ssr) plan.unet[0].first.logmel = plan.d_sp;
   for (size_t i = 0; i < plan.unet.size(); ++i)
     if ((rc = tr.step(plan.unet[i], 0, (int)i))) return rc;
   if (ssr) {
-    IstftFramesParams fp;
-    IstftOlaParams op;
-    istft_params(ctx, &fp, &op, plan.d_mag, wav, batch, (long)n, T, plan.d_frames, wav_out, plan.d_vl_off, plan.vl(VL_T));
-    CK(launch_istft_frames(fp, 0));
-    CK(launch_istft_ola(op, 0));
-    return VF_OK;
+    vf_trace_op t;
+    tr.describe_direct(VF_TRACE_ISTFT, "istft", &t);
+    vf_op_case& c = t.op;
+    c.kind = VF_OP_ISTFT; c.clip_off = off; c.n = n; c.T = T;
+    c.mag = plan.d_mag; c.in_wav = wav; c.frames = plan.d_frames; c.out = wav_out;
+    tr.out(&t, plan.d_frames, rows * 2048 * 4);
+    tr.out(&t, wav_out, (size_t)samples * 4);
+    return tr.direct_step(t, [&] {
+      IstftFramesParams fp;
+      IstftOlaParams op;
+      istft_params(ctx, &fp, &op, plan.d_mag, wav, batch, (long)n, T, plan.d_frames, wav_out, plan.d_vl_off, plan.vl(VL_T));
+      CK(launch_istft_frames(fp, 0));
+      CK(launch_istft_ola(op, 0));
+      ctx->launches += 2;
+      return VF_OK;
+    });
   }
   Op& cop = plan.vocoder[plan.cond_op];
   if (!voc) {      // a vocoder-only plan's conditioning op reads its d_mel as built
@@ -652,8 +734,20 @@ int run_trace(vf_ctx* ctx, Case& s, int kind, const float* wav, const int64_t* o
     cop.cond.is_log = 1;
     cop.cond.band_sums = nullptr;
   }
-  if (flags & VF_RESTORE_UNIFY_ENERGY)
-    CK(unify_energy(plan.d_mel, plan.d_logmel_out, batch, T, plan.d_band, plan.vl(VL_T), &cop.cond, 0));
+  if (flags & VF_RESTORE_UNIFY_ENERGY) {     // restore_impl's band sums
+    vf_trace_op t;
+    tr.describe_direct(VF_TRACE_BAND, "band_energy", &t);
+    vf_op_case& c = t.op;
+    c.kind = VF_OP_COND; c.unify = 1; c.is_log = 1; c.T = T;
+    c.mel = plan.d_logmel_out; c.mel_target = plan.d_mel; c.band_sums = plan.d_band;
+    tr.out(&t, plan.d_band, 2 * (size_t)batch * 4);
+    rc = tr.direct_step(t, [&] {
+      CK(unify_energy(plan.d_mel, plan.d_logmel_out, batch, T, plan.d_band, plan.vl(VL_T), &cop.cond, 0));
+      ctx->launches++;
+      return VF_OK;
+    });
+    if (rc) return rc;
+  }
   for (size_t i = 0; i < plan.vocoder.size(); ++i)
     if ((rc = tr.step(plan.vocoder[i], 1, (int)i))) return rc;
   Op fop;
@@ -766,7 +860,8 @@ VF_API int vf_selftest_plan_trace(vf_ctx* ctx, int plan_kind, const float* wav, 
                                   unsigned flags, float* wav_out, vf_trace_fn fn, void* user) {
   if (!ctx || !wav || !wav_out || !fn || batch <= 0) return VF_EINVAL;
   if (plan_kind < PLAN_GSR || plan_kind > PLAN_VOC_VARLEN || is_varlen_plan(plan_kind) != (offsets != nullptr) ||
-      (flags & ~(unsigned)VF_RESTORE_UNIFY_ENERGY) || (flags && (is_ssr_plan(plan_kind) || is_voc_plan(plan_kind))) ||
+      (flags & ~(unsigned)(VF_RESTORE_UNIFY_ENERGY | VF_TRACE_DIRECT_STEPS)) ||
+      ((flags & VF_RESTORE_UNIFY_ENERGY) && (is_ssr_plan(plan_kind) || is_voc_plan(plan_kind))) ||
       (offsets && (batch > VL_MAX_CLIPS || offsets[0] != 0)))
     return fail(ctx, VF_EINVAL, "vf_selftest_plan_trace: bad call");
   if (!ctx->loaded) return fail(ctx, VF_ESTATE, "weights not loaded");

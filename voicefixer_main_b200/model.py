@@ -739,10 +739,12 @@ class Engine:
             self._ck(rc)
         return rc
 
-    def selftest_plan_trace(self, plan_kind: int, wav: torch.Tensor, lengths=None, on_op=None, unify_energy: bool = False):
+    def selftest_plan_trace(self, plan_kind: int, wav: torch.Tensor, lengths=None, on_op=None, unify_energy: bool = False,
+                            direct_steps: bool = False):
         """One restore on a fresh plan of plan_kind (0 GSR, 1 SSR, 4 vocoder-only resynthesis: wav [B, n]; 2 GSR varlen,
         3 SSR varlen, 5 vocoder-only varlen: wav packed, lengths per clip), one launch at a time: on_op(after, op) runs before (after = False) and after (True) each launch
         with its L.VfTraceOp (vf_selftest_plan_trace; tests only).  An exception in on_op stops the run and is raised here.
+        direct_steps: also trace the launches the restore makes itself (front end, band sums, ISTFT) as list 3.
         Returns the restored output, shaped as the matching restore call returns it."""
         wav = _check_in(wav, self.device, "wav")
         out = torch.empty_like(wav)
@@ -761,7 +763,7 @@ class Engine:
             batch, n, offp = len(lengths), 0, _offsets(lengths)
         else:
             batch, n, offp = wav.shape[0], wav.shape[1], None
-        flags = L.VF_RESTORE_UNIFY_ENERGY if unify_energy else 0
+        flags = (L.VF_RESTORE_UNIFY_ENERGY if unify_energy else 0) | (L.VF_TRACE_DIRECT_STEPS if direct_steps else 0)
         with torch.cuda.device(self.device):
             torch.cuda.synchronize()            # the hook runs on the legacy default stream
             rc = self.lib.vf_selftest_plan_trace(self.ctx, plan_kind, _ptr(wav), offp, batch, n, flags, _ptr(out), fn, None)
