@@ -55,6 +55,8 @@
  *                                 dataloaders/data_module.py:130-150
  *   vf_resample_sinc_varlen       librosa.load(sr=...)'s resampling as librosa 0.8 does it (resampy kaiser_best /
  *                                 kaiser_fast), tools/utils.py:46-48 and metrics.py:33-34; opt-in (res_type)
+ *   vf_resample_rings             either resampler on live streams, incrementally from device rings: the input
+ *                                 conversion of load_wav for audio that arrives while it is restored
  *
  * Conventions: every function returns 0 on success or a negative VF_E* code and never throws; the message is
  * available from vf_last_error().  All tensor arguments are contiguous fp32.  Unless a name ends in `_host`,
@@ -466,6 +468,46 @@ VF_API int vf_resample_poly_f64_varlen(vf_ctx* ctx, const double* x, const int64
 VF_API int vf_resample_sinc_varlen(vf_ctx* ctx, const float* x, const int64_t* in_offsets, int batch, const double* tables,
                                    const int64_t* table_offsets, const double* sample_ratio, const int* num_table, int n_filters,
                                    const int* row_filter, float* y, const int64_t* out_offsets, void* stream);
+
+/* Live streams resampled from device rings in one call (voicefixer_main_b200/streaming.py StreamingResampler, and the
+ * restorers' streams at other rates).  in_ring [n_streams, in_len] (device) holds each stream's recent float32 samples at
+ * its own rate: absolute input i of stream s is at in_ring[s * in_len + i mod in_len].  rows: HOST table of n_rows entries
+ * (read during the call only).  Row r computes outputs m0 .. m1 - 1 of its stream's signal of n inputs (n =
+ * VF_RESAMPLE_OPEN while the stream is open: no output is clamped to its end) with the arithmetic of a whole-signal call, so
+ * each output is bit-identical to that output of vf_resample_poly (family VF_RESAMPLE_POLY: up, down and taps = the
+ * 20 max(up, down) + 1 float32 taps of resample_poly's FIR, device) or of vf_resample_sinc_varlen (VF_RESAMPLE_SINC:
+ * table = nwin (win, delta) float64 pairs, device, 16-byte aligned, for sample_ratio `ratio` and num_table entries per zero
+ * crossing) on the whole signal; a closed sinc row's slots at or past int(n ratio) are zeros (librosa's fix_length).  Only
+ * inputs below `avail` have been written, and the ring holds those from avail - in_len on.  The outputs go to row
+ * out_stream of `out` as a ring of out_len positions (output m at out[out_stream * out_len + m mod out_len], n_out_streams
+ * rows), or with out_stream = -1 to out[out_offset + m - m0] (packed).  Every argument is checked before any work is
+ * queued (VF_EINVAL, naming the row): a stream or out_stream out of range, m0 < 0 or m1 < m0, an input window that reaches
+ * past avail or below what the ring holds (a sinc row may read from max(0, int(m0 / ratio) - K + 1) on, K = nwin / step,
+ * step = int(min(1, ratio) num_table)), a closed row's range past ceil(n up / down) or ceil(n ratio) outputs or with
+ * int(n ratio) = 0, more outputs than out_len, an unknown family or a filter that does not match it (a poly row with no
+ * taps or a table, a sinc row with no table, taps, a ratio that is not positive, num_table < 1, a step of 0 or a table of at
+ * most num_table entries); the context stays usable.  Empty rows (m0 = m1) are checked and launch nothing.  One launch per
+ * family present, per 256 rows of it, whatever the number of streams; no scratch, no host synchronisation. */
+#define VF_RESAMPLE_POLY 0
+#define VF_RESAMPLE_SINC 1
+#define VF_RESAMPLE_OPEN INT64_MAX
+typedef struct vf_resample_row {
+  int32_t stream;           /* row of in_ring */
+  int32_t family;           /* VF_RESAMPLE_POLY or VF_RESAMPLE_SINC */
+  int64_t m0, m1;           /* absolute output range [m0, m1) */
+  int64_t n;                /* the stream's input count once closed, VF_RESAMPLE_OPEN while open */
+  int64_t avail;            /* inputs written to the ring so far (at most n) */
+  int32_t up, down;         /* poly */
+  const float* taps;        /* poly: device, NULL for sinc */
+  const double* table;      /* sinc: device, NULL for poly */
+  int64_t nwin;             /* sinc: table entries */
+  double ratio;             /* sinc: target_sr / orig_sr */
+  int32_t num_table;        /* sinc */
+  int32_t out_stream;       /* row of the output ring, or -1: packed */
+  int64_t out_offset;       /* packed: where output m0 goes */
+} vf_resample_row;
+VF_API int vf_resample_rings(vf_ctx* ctx, const float* in_ring, int n_streams, int64_t in_len, const vf_resample_row* rows,
+                             int n_rows, float* out, int n_out_streams, int64_t out_len, void* stream);
 
 VF_API int vf_to_log(vf_ctx* ctx, const float* in, float* out, int64_t n, void* stream);
 VF_API int vf_from_log(vf_ctx* ctx, const float* in, float* out, int64_t n, void* stream);

@@ -3,6 +3,7 @@
 
     python tools/bench_stream.py [--workload gsr|ssr] [--ola boxcar|windowed [--hop-div 2]] [--streams 1,8,64,256]
                                  [--windows 1,2] [--steps K] [--warmup W]
+    python tools/bench_stream.py --input-rate 8000,16000,48000 [--res-type kaiser_best] [--streams 64] [--windows 1]
 
 --workload gsr (the default) streams through VoiceFixer (ResUNet + vocoder, vf_restore_chunks); ssr through SSR_UNet
 (unet_v2 + ISTFT, vf_ssr_restore_chunks), whose baseline arm calls SSR_UNet.restore_batch (vf_ssr_restore_varlen).
@@ -24,6 +25,14 @@ Both must give the same bits.  A step is timed with CUDA events around it after 
 reported.  A step is real time when it takes at most W seconds (it restores W of audio per stream).  Prints one JSON line:
 per (W, S) the step times, audio seconds restored per second and the plans built and evicted; per W the largest S that
 stays real time; the card's name and power limit, read in the same run.
+
+With --input-rate R (a comma-separated list), each case is S streams at R Hz through StreamingRestorer (VoiceFixer, boxcar,
+M = W / 4; --res-type picks the resampler, default resample_poly): each step pushes W R / 44100 samples per stream and the
+step first resamples the newly final samples into the 44.1 kHz rings (one vf_resample_rings launch), then restores.  Its
+baseline arm ("pre_resampled") is the same audio resampled whole beforehand with edges.resample_to and pushed at 44.1 kHz,
+exactly the samples the first arm made final in that step, so both restore the same chunks and must give the same bits.
+Only step() is timed in both arms.  A third pass, run separately under torch.profiler, sums the device time of
+stream_resample_kernel per step and its share of the step's kernel time.
 """
 import argparse
 import json
@@ -186,6 +195,85 @@ def run_case_windowed(workload, state, bank, W, hop, S, steps, warmup):
             "plans_evicted": info1["evicted"] - info0["evicted"], "plan_cache": info1, "gpu_launches": launches}
 
 
+def run_case_rates(state, W, M, S, rate, res_type, steps, warmup, seed=4242):
+    """S streams at `rate` Hz (see the module docstring) on a VoiceFixer of its own."""
+    from torch.profiler import ProfilerActivity, profile
+    from voicefixer_main_b200 import VoiceFixer
+    from voicefixer_main_b200.edges import resample_to
+    from voicefixer_main_b200.streaming import StreamingRestorer
+    dev = torch.device("cuda", 0)
+    model = VoiceFixer().load_state_dict(state).eval().to(dev)
+    eng = model._engine()
+    P = W * rate // SR                                        # input samples per stream per step
+    rounds = warmup + 2 * steps + 2
+    bank = synth_batch(BANK, rounds * P + 1, seed).to(dev)
+    xs = [torch.roll(bank[s % BANK], s * 997) for s in range(S)]
+    x44 = [resample_to(eng, x[None], rate, SR, res_type)[0] for x in xs]
+    a = StreamingRestorer(model, W, M, max_streams=S, res_type=res_type)
+    b = StreamingRestorer(model, W, M, max_streams=S)
+    ia, ib = [a.open(rate) for _ in range(S)], [b.open() for _ in range(S)]
+    assert P <= a.max_push(rate)
+
+    def step_pair(i):
+        for sid, x in zip(ia, xs):
+            a.push(sid, x[i * P:(i + 1) * P])
+        out_a, a0, a1 = timed(a.step)
+        for j, (sid, x) in enumerate(zip(ib, x44)):
+            done = a._streams[ia[j]].pushed                   # the 44.1 kHz samples arm a has made final
+            b.push(sid, x[b._streams[sid].pushed:done])
+        out_b, b0, b1 = timed(b.step)
+        same = all((p in out_a) == (q in out_b) and (p not in out_a or torch.equal(out_a[p], out_b[q])) for p, q in zip(ia, ib))
+        return same, a0.elapsed_time(a1), b0.elapsed_time(b1)
+
+    ms_a, ms_b, same = [], [], True
+    for i in range(warmup + steps):
+        ok, ta, tb = step_pair(i)
+        same = same and ok
+        if i >= warmup:
+            ms_a.append(ta)
+            ms_b.append(tb)
+    # the resample kernel's share, in a pass of its own under the profiler
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for i in range(warmup + steps, warmup + 2 * steps):
+            for sid, x in zip(ia, xs):
+                a.push(sid, x[i * P:(i + 1) * P])
+            a.step()
+        torch.cuda.synchronize()
+    kern = [e for e in prof.events() if e.device_type.name == "CUDA"]
+    rs_us = sum(e.device_time for e in kern if "stream_resample_kernel" in e.name)
+    all_us = sum(e.device_time for e in kern)
+    eng.check_errors()
+    eng.close()
+    med = lambda v: sorted(v)[len(v) // 2]
+    return {"input_rate": rate, "res_type": res_type, "window_s": W / SR, "margin_s": M / SR, "streams": S,
+            "input_samples_per_stream_per_step": P,
+            "arms": {"streaming_at_input_rate": {"step_ms_median": med(ms_a), "ms_min": min(ms_a), "ms_max": max(ms_a)},
+                     "pre_resampled": {"step_ms_median": med(ms_b), "ms_min": min(ms_b), "ms_max": max(ms_b)}},
+            "step_ms_ratio": med(ms_a) / med(ms_b), "bit_identical": bool(same),
+            "resample_kernel_us_per_step": rs_us / steps, "resample_share_of_step_kernel_time": rs_us / all_us if all_us else None,
+            "profiled_steps": steps}
+
+
+def main_rates(args):
+    from voicefixer_main_b200.weights import make_state
+    state = make_state(1234)
+    streams = [int(s) for s in args.streams.split(",")]
+    cases = []
+    for w_s in [float(w) for w in args.windows.split(",")]:
+        W = int(round(w_s * SR)) // 2 * 2
+        for rate in [int(r) for r in args.input_rate.split(",")]:
+            for S in streams:
+                cases.append(run_case_rates(state, W, W // 4, S, rate, args.res_type, args.steps, args.warmup))
+    line = {"metric": "stream_resample_step_ms_ratio", "value": max(c["step_ms_ratio"] for c in cases),
+            "unit": "step time at the input rate / step time pre-resampled", "higher_is_better": False, "data": "synthetic",
+            "steps": args.steps, "warmup": args.warmup,
+            "config": {"workload": "S streams of seeded speech-like audio at the input rate, each pushing W of audio per step, "
+                                   "M = W / 4, VoiceFixer (vf_resample_rings + vf_restore_chunks); value = the worst case",
+                       "res_type": args.res_type},
+            "cases": cases, "card": card_info(0)}
+    print(json.dumps(line))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--workload", choices=("gsr", "ssr"), default="gsr",
@@ -197,9 +285,14 @@ def main():
     ap.add_argument("--windows", default="1,2", help="window lengths in seconds; the margin is a quarter of the window")
     ap.add_argument("--steps", type=int, default=5, help="timed steady-state steps per case")
     ap.add_argument("--warmup", type=int, default=2, help="untimed steps per case (the first is the streams' first chunk)")
+    ap.add_argument("--input-rate", default=None, help="streams at these rates (Hz, comma-separated) through the resampler")
+    ap.add_argument("--res-type", default=None, choices=("kaiser_best", "kaiser_fast"),
+                    help="with --input-rate: librosa 0.8's resampy filter instead of resample_poly")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("tools/bench_stream.py needs a CUDA device")
+    if args.input_rate:
+        return main_rates(args)
     from voicefixer_main_b200.weights import make_ssr_state, make_state
     dev = torch.device("cuda", 0)
     state = (make_ssr_state if args.workload == "ssr" else make_state)(1234)

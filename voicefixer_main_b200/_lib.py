@@ -25,11 +25,13 @@ EXPORTS = [
     "vf_sosfiltfilt_varlen", "vf_resample_poly_f64_varlen", "vf_metric_spectrogram_ex", "vf_score_varlen_ex",
     "vf_score_time_varlen_ex", "vf_restore_chunks", "vf_ssr_restore_chunks", "vf_restore_windows", "vf_ssr_restore_windows",
     "vf_selftest_plan_gemms", "vf_resample_sinc_varlen", "vf_selftest_plan_trace", "vf_vocoder_varlen", "vf_resynth",
-    "vf_resynth_varlen", "vf_selftest_sub_batch", "vf_vocoder_chunks",
+    "vf_resynth_varlen", "vf_selftest_sub_batch", "vf_vocoder_chunks", "vf_resample_rings",
 ]
 VF_RESTORE_UNIFY_ENERGY = 1
 VF_TRACE_DIRECT_STEPS = 0x100
 VF_SSR_PEAK_NORMALISE = 1
+VF_RESAMPLE_POLY, VF_RESAMPLE_SINC = 0, 1
+VF_RESAMPLE_OPEN = (1 << 63) - 1
 
 
 class VfConfig(Structure):
@@ -124,6 +126,13 @@ class VfWindow(Structure):
 class VfEmit(Structure):
     """vf_emit (include/b200vf.h): one stream's emission range of a vf_restore_windows call."""
     _fields_ = [("stream", c_int32), ("start", c_int64), ("count", c_int64)]
+
+
+class VfResampleRow(Structure):
+    """vf_resample_row (include/b200vf.h): one stream's output range of a vf_resample_rings call."""
+    _fields_ = [("stream", c_int32), ("family", c_int32), ("m0", c_int64), ("m1", c_int64), ("n", c_int64), ("avail", c_int64),
+                ("up", c_int32), ("down", c_int32), ("taps", c_void_p), ("table", c_void_p), ("nwin", c_int64),
+                ("ratio", c_double), ("num_table", c_int32), ("out_stream", c_int32), ("out_offset", c_int64)]
 
 
 class EngineError(RuntimeError):
@@ -225,6 +234,7 @@ def load_library():
                                                 POINTER(c_int), c_int, POINTER(c_int), P, POINTER(c_int64), P]
     lib.vf_resample_sinc_varlen.argtypes = [P, P, POINTER(c_int64), c_int, P, POINTER(c_int64), POINTER(c_double),
                                             POINTER(c_int), c_int, POINTER(c_int), P, POINTER(c_int64), P]
+    lib.vf_resample_rings.argtypes = [P, P, c_int, c_int64, POINTER(VfResampleRow), c_int, P, c_int, c_int64, P]
     _lib = lib
     return lib
 

@@ -5,25 +5,19 @@
 //     AudioMetrics.lsd / .sispec (evaluation_proc/metrics.py:83-95, energy_unify evaluation_proc/utils.py:81-101)
 #include "kernels.cuh"
 #include "reduce.cuh"
+#include "resample.cuh"
 
 namespace vf {
 
 // out[b, m] = sum_i h[m * down - i * up + half] * x[b, i]: zero-phase polyphase resampling by up / down with a symmetric
-// FIR of 2 * half + 1 taps (designed on the host: firwin(.., 1 / max(up, down), window = ('kaiser', 5.0)) * up).
+// FIR of 2 * half + 1 taps (designed on the host: firwin(.., 1 / max(up, down), window = ('kaiser', 5.0)) * up).  The body
+// is poly_output (resample.cuh), which the streaming resampler shares.
 __global__ void __launch_bounds__(256) resample_poly_kernel(const float* __restrict__ x, long n, int up, int down, const float* __restrict__ h,
                                                             int half, float* __restrict__ out, long n_out) {
   const long m = (long)blockIdx.x * blockDim.x + threadIdx.x;
   const int b = blockIdx.y;
   if (m >= n_out) return;
-  const long c = m * down;
-  long i_lo = (c - half + up - 1) / up;          // ceil((c - half) / up) for a non-negative numerator
-  if (c - half < 0) i_lo = 0;
-  long i_hi = (c + half) / up;
-  if (i_hi > n - 1) i_hi = n - 1;
-  const float* xb = x + (size_t)b * n;
-  float acc = 0.f;
-  for (long i = i_lo; i <= i_hi; ++i) acc = fmaf(__ldg(h + (c - i * up + half)), __ldg(xb + i), acc);
-  out[(size_t)b * n_out + m] = acc;
+  out[(size_t)b * n_out + m] = poly_output(FlatInput{x + (size_t)b * n}, m, n, up, down, h, half);
 }
 cudaError_t launch_resample_poly(const float* x, int batch, long n, int up, int down, const float* h, int half, float* out, long n_out,
                                  cudaStream_t stream) {

@@ -513,4 +513,36 @@ struct SincParams {
 };
 cudaError_t launch_sinc_resample(const SincParams& p, cudaStream_t stream);
 
+// vf_resample_rings (stream.cu): the rows of one family of one launch, kernel parameters like the chunk gather's.  Thread
+// off[r] + j (j < off[r + 1] - off[r]) computes output m = m0[r] + j of row r from the input ring row at ring + src[r]
+// (absolute input i at (a_ph[r] + i - a0[r]) mod in_len, a0: the first input the row may read) for a signal of n[r] inputs
+// (INT64_MAX while open), and writes it to out[dst[r] + (d_ph[r] + j) mod out_len] (a ring row: dst = its stream times
+// out_len, d_ph = m0 mod out_len) or, with d_ph[r] < 0, to out[dst[r] + j] (packed).  Poly rows read their own taps, sinc
+// rows their own (win, delta) table, with slots at or past n_valid[r] = int(n ratio) written as zeros.
+constexpr int RING_RESAMPLE_ROWS = 256;                   // keeps either struct under the 32 KiB kernel-parameter limit
+struct RingResampleRows {
+  const float* ring;
+  float* out;
+  int64_t in_len, out_len;
+  int rows;
+  int64_t off[RING_RESAMPLE_ROWS + 1];
+  int64_t src[RING_RESAMPLE_ROWS], a0[RING_RESAMPLE_ROWS], a_ph[RING_RESAMPLE_ROWS];
+  int64_t m0[RING_RESAMPLE_ROWS], n[RING_RESAMPLE_ROWS];
+  int64_t dst[RING_RESAMPLE_ROWS], d_ph[RING_RESAMPLE_ROWS];
+};
+struct PolyRingParams {
+  RingResampleRows r;
+  const float* taps[RING_RESAMPLE_ROWS];
+  int up[RING_RESAMPLE_ROWS], down[RING_RESAMPLE_ROWS];
+};
+struct SincRingParams {
+  RingResampleRows r;
+  const double2* tab[RING_RESAMPLE_ROWS];
+  int64_t nwin[RING_RESAMPLE_ROWS], n_valid[RING_RESAMPLE_ROWS];
+  double ratio[RING_RESAMPLE_ROWS];
+  int num_table[RING_RESAMPLE_ROWS];
+};
+cudaError_t launch_stream_resample(const PolyRingParams& p, cudaStream_t stream);
+cudaError_t launch_stream_resample(const SincRingParams& p, cudaStream_t stream);
+
 }  // namespace vf

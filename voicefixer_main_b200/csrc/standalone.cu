@@ -174,6 +174,105 @@ void stoi_bands(int* lo, int* hi) {
   }
 }
 
+// The input windows of the float32 resamplers as resample.cuh computes them, on the host: [*first, *last] are the inputs
+// output m reads of an n-input signal (n = VF_RESAMPLE_OPEN while a stream is open: no clamp at its end); first > last when
+// it reads none.  The sinc arithmetic is the kernel's float64 arithmetic, operation for operation.
+void poly_window(int64_t m, int64_t n, int up, int down, int64_t* first, int64_t* last) {
+  const int64_t half = 10 * (int64_t)std::max(up, down), c = m * down;
+  *first = c - half < 0 ? 0 : (c - half + up - 1) / up;
+  *last = std::min((c + half) / up, n - 1);
+}
+struct SincGeom {
+  double ratio, scale, num_table;
+  int64_t step, nwin;
+  int64_t wing(double frac) const { return (nwin - (int64_t)(frac * num_table)) / step; }    // a wing's length bound
+  int64_t kmax() const { return nwin / step; }                                              // its largest value
+  void window(int64_t t, int64_t n, int64_t* first, int64_t* last) const {
+    const double tr = (double)t / ratio;
+    const int64_t nt = (int64_t)tr;
+    const double frac = scale * (tr - (double)nt);
+    const int64_t kl = std::min(nt + 1, wing(frac)), kr = std::min(n - nt - 1, wing(scale - frac));
+    *first = kl > 0 ? nt - kl + 1 : nt + 1;
+    *last = kr > 0 ? nt + kr : kl > 0 ? nt : nt - 1;
+  }
+};
+
+// vf_resample_rings' checks of one row.  -> why it is refused, or nullptr with the first input it may read (a0) and, for a
+// sinc row, its count of non-zero outputs.
+struct RingRow {
+  int64_t a0, n_valid;
+};
+const char* ring_row(const vf_resample_row& w, int n_streams, int64_t in_len, int n_out_streams, int64_t out_len, RingRow* c) {
+  static thread_local char msg[192];
+  if (w.stream < 0 || w.stream >= n_streams) return "stream out of range";
+  if (w.m0 < 0 || w.m1 < w.m0) return "bad output range (need 0 <= m0 <= m1)";
+  const bool open = w.n == VF_RESAMPLE_OPEN;
+  if (!open && (w.n < 1 || w.n > (int64_t(1) << 40))) return "input count n must be 1 .. 2^40, or VF_RESAMPLE_OPEN";
+  if (w.avail < 0 || (!open && w.avail > w.n)) return "avail must be 0 .. n";
+  if (w.out_stream >= 0) {
+    if (w.out_stream >= n_out_streams || out_len < 1) return "out_stream is not a row of the output ring";
+    if (w.m1 - w.m0 > out_len) return "more outputs than the output ring holds";
+  } else if (w.out_stream != -1 || w.out_offset < 0) {
+    return "out_stream must be a ring row or -1 (packed, out_offset >= 0)";
+  }
+  int64_t out_n = INT64_MAX;                         // the signal's output length once closed
+  int64_t first = 0, last = -1;                      // the inputs the row reads
+  c->n_valid = INT64_MAX;
+  if (w.family == VF_RESAMPLE_POLY) {
+    if (!w.taps || w.table || w.up < 1 || w.down < 1 || w.up > (1 << 20) || w.down > (1 << 20))
+      return "a poly row needs taps, no table and up, down in 1 .. 2^20";
+    if (!open) out_n = (w.n * w.up + w.down - 1) / w.down;
+    if (w.m1 > out_n) return "output range past the signal's ceil(n up / down) outputs";
+    if (w.m1 > w.m0) {
+      int64_t f, l;
+      poly_window(w.m0, w.n, w.up, w.down, &first, &l);
+      poly_window(w.m1 - 1, w.n, w.up, w.down, &f, &last);
+    }
+  } else if (w.family == VF_RESAMPLE_SINC) {
+    if (!w.table || w.taps || reinterpret_cast<uintptr_t>(w.table) % alignof(double2) != 0)
+      return "a sinc row needs a 16-byte aligned table and no taps";
+    if (!(w.ratio > 0.0) || !std::isfinite(w.ratio) || w.num_table < 1 || w.nwin <= w.num_table || w.nwin > (int64_t(1) << 30))
+      return "a sinc row needs ratio > 0, num_table >= 1 and more than num_table table entries";
+    const double scale = std::min(w.ratio, 1.0);
+    const SincGeom g{w.ratio, scale, (double)w.num_table, (int64_t)(scale * (double)w.num_table), w.nwin};
+    if (g.step < 1) return "the sinc index step int(min(1, ratio) num_table) is 0";
+    if (!open) {
+      c->n_valid = (int64_t)((double)w.n * w.ratio);
+      out_n = (int64_t)std::ceil((double)w.n * w.ratio);
+      if (c->n_valid < 1) return "too few inputs to resample (int(n ratio) is 0)";
+    }
+    if (w.m1 > out_n) return "output range past the signal's ceil(n ratio) outputs";
+    const int64_t m_end = std::min(w.m1, c->n_valid);          // outputs that read inputs
+    if (m_end > w.m0) {
+      first = std::max<int64_t>(0, (int64_t)((double)w.m0 / w.ratio) - (g.kmax() - 1));
+      // the last input: exact per output from the end down, until no earlier output can read further
+      for (int64_t t = m_end - 1; t >= w.m0; --t) {
+        int64_t f, l;
+        g.window(t, w.n, &f, &l);
+        last = std::max(last, l);
+        if ((int64_t)((double)t / w.ratio) + g.kmax() <= last) break;
+      }
+      if (last < first) last = first - 1;
+    }
+  } else {
+    return "unknown family";
+  }
+  if (first <= last) {
+    if (last > w.avail - 1) {
+      snprintf(msg, sizeof msg, "outputs %ld .. %ld read input %ld, past the %ld inputs in the ring", (long)w.m0, (long)w.m1 - 1,
+               (long)last, (long)w.avail);
+      return msg;
+    }
+    if (first < w.avail - in_len) {
+      snprintf(msg, sizeof msg, "outputs from %ld read input %ld, which the ring of %ld no longer holds", (long)w.m0, (long)first,
+               (long)in_len);
+      return msg;
+    }
+  }
+  c->a0 = std::max<int64_t>(first, 0);
+  return nullptr;
+}
+
 }  // namespace
 
 extern "C" {
@@ -657,6 +756,71 @@ VF_API int vf_resample_sinc_varlen(vf_ctx* ctx, const float* x, const int64_t* i
     ctx->launches += 1;
   }
   if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "sinc resample launch: %s", cudaGetErrorString(e));
+  return VF_OK;
+}
+
+// ----------------------------------------------------------------------------------------- live streams' rate conversion
+VF_API int vf_resample_rings(vf_ctx* ctx, const float* in_ring, int n_streams, int64_t in_len, const vf_resample_row* rows,
+                             int n_rows, float* out, int n_out_streams, int64_t out_len, void* stream) {
+  static const char* fn = "vf_resample_rings";
+  const int rc = begin_call(ctx, fn, in_ring && rows && out && n_streams > 0 && in_len > 0 && n_rows > 0 && n_out_streams >= 0 &&
+                                         out_len >= 0);
+  if (rc) return rc;
+  std::vector<RingRow> checked(n_rows);
+  for (int i = 0; i < n_rows; ++i) {
+    const char* why = ring_row(rows[i], n_streams, in_len, n_out_streams, out_len, &checked[i]);
+    if (why) return fail(ctx, VF_EINVAL, "%s: row %d: %s", fn, i, why);
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  cudaError_t e = cudaSuccess;
+  for (int family = VF_RESAMPLE_POLY; family <= VF_RESAMPLE_SINC && e == cudaSuccess; ++family) {
+    std::vector<int> mine;
+    for (int i = 0; i < n_rows; ++i)
+      if (rows[i].family == family && rows[i].m1 > rows[i].m0) mine.push_back(i);
+    for (size_t s = 0; s < mine.size() && e == cudaSuccess; s += RING_RESAMPLE_ROWS) {
+      const int nb = (int)std::min<size_t>(RING_RESAMPLE_ROWS, mine.size() - s);
+      auto fill = [&](RingResampleRows& q) {
+        q.ring = in_ring; q.out = out; q.in_len = in_len; q.out_len = out_len; q.rows = nb;
+        for (int k = 0; k < nb; ++k) {
+          const vf_resample_row& w = rows[mine[s + k]];
+          const RingRow& c = checked[mine[s + k]];
+          q.off[k + 1] = q.off[k] + (w.m1 - w.m0);
+          q.src[k] = (int64_t)w.stream * in_len;
+          q.a0[k] = c.a0;
+          q.a_ph[k] = c.a0 % in_len;
+          q.m0[k] = w.m0;
+          q.n[k] = w.n;
+          q.dst[k] = w.out_stream >= 0 ? (int64_t)w.out_stream * out_len : w.out_offset;
+          q.d_ph[k] = w.out_stream >= 0 ? w.m0 % out_len : -1;
+        }
+      };
+      if (family == VF_RESAMPLE_POLY) {
+        PolyRingParams p;
+        memset(&p, 0, sizeof p);
+        fill(p.r);
+        for (int k = 0; k < nb; ++k) {
+          const vf_resample_row& w = rows[mine[s + k]];
+          p.taps[k] = w.taps; p.up[k] = w.up; p.down[k] = w.down;
+        }
+        e = launch_stream_resample(p, st);
+      } else {
+        SincRingParams p;
+        memset(&p, 0, sizeof p);
+        fill(p.r);
+        for (int k = 0; k < nb; ++k) {
+          const vf_resample_row& w = rows[mine[s + k]];
+          p.tab[k] = reinterpret_cast<const double2*>(w.table);
+          p.nwin[k] = w.nwin;
+          p.n_valid[k] = checked[mine[s + k]].n_valid;
+          p.ratio[k] = w.ratio;
+          p.num_table[k] = w.num_table;
+        }
+        e = launch_stream_resample(p, st);
+      }
+      ctx->launches += 1;
+    }
+  }
+  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "ring resample launch: %s", cudaGetErrorString(e));
   return VF_OK;
 }
 

@@ -7,6 +7,7 @@
 // the overlap-add at 256 rows), so no host memory is read after the call returns and no copy of a table is queued.  One
 // thread per packed or accumulated sample; a warp's threads nearly always fall into one row, so the table lookups broadcast.
 #include "kernels.cuh"
+#include "resample.cuh"
 
 namespace vf {
 
@@ -99,6 +100,44 @@ __global__ void __launch_bounds__(STREAM_THREADS) window_emit_kernel(const __gri
   p.out[i] = *a;
   *a = 0.f;                                        // the slot is free for a later position, or a later stream
 }
+
+// vf_resample_rings resamples live streams from their own input rings into the restore rings (or a packed buffer): one
+// launch per filter family per RING_RESAMPLE_ROWS rows, its table a __grid_constant__ parameter (about 20 KB for poly, 25 KB
+// for sinc at 256 rows), one thread per output sample of the rows of one filter family.  The arithmetic is poly_output /
+// sinc_output (resample.cuh), the bodies of the whole-signal kernels, reading the stream's ring row instead of a flat row.
+__device__ __forceinline__ float ring_output(const PolyRingParams& p, int r, const RingInput& x, int64_t m) {
+  const int up = p.up[r], down = p.down[r];
+  return poly_output(x, m, p.r.n[r], up, down, p.taps[r], 10 * (up > down ? up : down));
+}
+__device__ __forceinline__ float ring_output(const SincRingParams& p, int r, const RingInput& x, int64_t m) {
+  if (m >= p.n_valid[r]) return 0.f;              // a closed stream's fix_length zeros
+  return sinc_output(x, m, p.r.n[r], p.ratio[r], p.num_table[r], p.tab[r], p.nwin[r]);
+}
+
+template <class P>
+__global__ void __launch_bounds__(STREAM_THREADS) stream_resample_kernel(const __grid_constant__ P p) {
+  const RingResampleRows& q = p.r;
+  const int64_t i = (int64_t)blockIdx.x * STREAM_THREADS + threadIdx.x;
+  if (i >= q.off[q.rows]) return;
+  const int r = find_row(q.off, q.rows, i);
+  const int64_t j = i - q.off[r];
+  const float y = ring_output(p, r, RingInput{q.ring + q.src[r], q.in_len, q.a0[r], q.a_ph[r]}, q.m0[r] + j);
+  int64_t d = j;
+  if (q.d_ph[r] >= 0) {                            // a ring row: j < out_len, so one subtraction wraps it
+    d = q.d_ph[r] + j;
+    if (d >= q.out_len) d -= q.out_len;
+  }
+  q.out[q.dst[r] + d] = y;
+}
+
+template <class P>
+cudaError_t launch_ring_resample(const P& p, cudaStream_t stream) {
+  const int64_t n = p.r.off[p.r.rows];
+  if (n > 0) stream_resample_kernel<P><<<(unsigned)((n + STREAM_THREADS - 1) / STREAM_THREADS), STREAM_THREADS, 0, stream>>>(p);
+  return cudaGetLastError();
+}
+cudaError_t launch_stream_resample(const PolyRingParams& p, cudaStream_t stream) { return launch_ring_resample(p, stream); }
+cudaError_t launch_stream_resample(const SincRingParams& p, cudaStream_t stream) { return launch_ring_resample(p, stream); }
 
 cudaError_t launch_stream_gather(const ChunkGatherParams& p, cudaStream_t stream) {
   const int64_t n = p.off[p.rows];

@@ -130,6 +130,32 @@ def _sinc_filter(eng: Engine, res_type: str, orig_sr: int, target_sr: int):
     return cache[res_type, ratio], ratio, 2 ** RES_TYPES[res_type][1]
 
 
+class StreamFilter:
+    """The filter of vf_resample_rings for one (rate_in, rate_out, res_type): family VF_RESAMPLE_POLY with up, down
+    (reduced by their gcd) and taps (design_filter's float32 taps on the device), or VF_RESAMPLE_SINC with table (the
+    float64 [nwin, 2] sinc_table on the device), ratio and num_table."""
+    __slots__ = ("family", "up", "down", "taps", "table", "ratio", "num_table")
+
+
+def stream_filter(eng: Engine, rate_in: int, rate_out: int, res_type: str = None) -> StreamFilter:
+    """The StreamFilter converting rate_in to rate_out with res_type (None: resample_poly), cached on the engine per
+    (rate_in, rate_out, res_type)."""
+    check_res_type(res_type)
+    cache = eng.__dict__.setdefault("_stream_filters", {})
+    key = (int(rate_in), int(rate_out), res_type)
+    if key not in cache:
+        f = StreamFilter()
+        if res_type is None:
+            fr = Fraction(int(rate_out), int(rate_in))
+            f.family, f.up, f.down = L.VF_RESAMPLE_POLY, fr.numerator, fr.denominator
+            f.taps = torch.from_numpy(design_filter(f.up, f.down)).to(eng.device)
+        else:
+            f.family = L.VF_RESAMPLE_SINC
+            f.table, f.ratio, f.num_table = _sinc_filter(eng, res_type, int(rate_in), int(rate_out))
+        cache[key] = f
+    return cache[key]
+
+
 def resample(eng: Engine, ys, orig_sr, target_sr: int, res_type: str = "kaiser_best") -> list:
     """librosa 0.8 resample(y, orig_sr, target_sr, res_type, fix=True) of every 1-D float32 signal of `ys` (numpy arrays or
     tensors), all in one vf_resample_sinc_varlen call: orig_sr is one rate for all, or one per signal.  -> list of float32

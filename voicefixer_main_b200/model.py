@@ -533,6 +533,33 @@ class Engine:
                                                       ratio, num_table, len(filters), rows, _ptr(out), out_off, _stream()))
         return out
 
+    def resample_rings(self, in_ring: torch.Tensor, rows, out: torch.Tensor) -> torch.Tensor:
+        """Live streams resampled from a device ring in one call (vf_resample_rings).  in_ring [n_streams, in_len] float32
+        holds stream s's absolute input i at in_ring[s, i % in_len].  rows is a sequence of (stream, filter, m0, m1, n, avail,
+        out_stream, out_offset): outputs m0 .. m1 - 1 of the stream's signal of n inputs (_lib.VF_RESAMPLE_OPEN while it is
+        open), of which the first `avail` have been pushed, with `filter` an edges.StreamFilter; each output has the bits of
+        that output of the whole-signal resample.  out is the output ring [n_out_streams, out_len] (output m of a row to
+        out[out_stream, m % out_len]) or a 1-D packed tensor (out_stream -1: output m to out[out_offset + m - m0]).
+        Returns out."""
+        in_ring = _check_in(in_ring, self.device, "in_ring")
+        if in_ring.dim() != 2 or not isinstance(out, torch.Tensor) or out.dtype != torch.float32 or out.device != self.device \
+                or not out.is_contiguous() or out.dim() not in (1, 2):
+            raise TypeError("resample_rings: in_ring [n_streams, in_len] and out [n_out_streams, out_len] or [n] float32 "
+                            f"contiguous tensors on {self.device}")
+        table = (L.VfResampleRow * len(rows))()
+        for t, (s, f, m0, m1, n, avail, os_, oo) in zip(table, rows):
+            t.stream, t.m0, t.m1, t.n, t.avail, t.out_stream, t.out_offset = s, m0, m1, n, avail, os_, oo
+            t.family = f.family
+            if f.family == L.VF_RESAMPLE_POLY:
+                t.up, t.down, t.taps = f.up, f.down, f.taps.data_ptr()
+            else:
+                t.table, t.nwin, t.ratio, t.num_table = f.table.data_ptr(), f.table.shape[0], f.ratio, f.num_table
+        n_out, out_len = (out.shape[0], out.shape[1]) if out.dim() == 2 else (0, 0)
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_resample_rings(self.ctx, _ptr(in_ring), in_ring.shape[0], in_ring.shape[1], table, len(rows),
+                                                _ptr(out), n_out, out_len, _stream()))
+        return out
+
     def amp_to_original_f(self, mel_est: torch.Tensor, mel_target: torch.Tensor) -> torch.Tensor:
         """tools/utils.py:50-55 on linear mels [B,T,128]: the estimate scaled to the target's low-band energy."""
         mel_est, mel_target = _check_in(mel_est, self.device, "mel_est"), _check_in(mel_target, self.device, "mel_target")
