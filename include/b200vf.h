@@ -57,6 +57,7 @@
  *                                 kaiser_fast), tools/utils.py:46-48 and metrics.py:33-34; opt-in (res_type)
  *   vf_resample_rings             either resampler on live streams, incrementally from device rings: the input
  *                                 conversion of load_wav for audio that arrives while it is restored
+ *   vf_remove_higher_frequency_varlen  the pip package's mode-1 pre-filter, remove_higher_frequency, before a restore
  *
  * Conventions: every function returns 0 on success or a negative VF_E* code and never throws; the message is
  * available from vf_last_error().  All tensor arguments are contiguous fp32.  Unless a name ends in `_host`,
@@ -468,6 +469,26 @@ VF_API int vf_resample_poly_f64_varlen(vf_ctx* ctx, const double* x, const int64
 VF_API int vf_resample_sinc_varlen(vf_ctx* ctx, const float* x, const int64_t* in_offsets, int batch, const double* tables,
                                    const int64_t* table_offsets, const double* sample_ratio, const int* num_table, int n_filters,
                                    const int* row_filter, float* y, const int64_t* out_offsets, void* stream);
+/* The VoiceFixer pip package's pre-filter, remove_higher_frequency(wav, ratio) (restore_inmem's mode 1), of `batch` packed
+ * float32 rows: x packed with HOST in_offsets (every row 1 .. 2^30 samples), y with HOST out_offsets, row i holding 512 (n_i
+ * // 512) samples (librosa 0.8's istft with length None; a row under 512 samples gives an empty output).  cutoff (device,
+ * int32 [batch]) receives each row's first removed bin.  Per row, in float64: librosa 0.8's stft (n_fft 2048, hop 512,
+ * periodic hann, reflect padding as np.pad makes it for any length), per-bin energies sum over frames of max(log10(|X| +
+ * 1e-8), 0), the package's sequential scan for the first bin whose running sum reaches ratio times their total, the bins
+ * below it scaled by |X| / (|X| + 1e-8) and the others zeroed, librosa's istft (overlap-add divided by the window sum of
+ * squares where that exceeds float32 tiny); the output is rounded to float32 once.  Only bins with |X| >= 1 carry energy: a
+ * quiet row has cutoff 0 and an all-zero output.  Where rounding makes the last running sum miss the threshold (the
+ * package would raise IndexError) every bin is kept, cutoff 1025.  A row's bits do not depend on its batch, its position
+ * or the sub-batching.  Every argument is checked before any work is queued (VF_EINVAL, naming the row): 0 < ratio <= 1,
+ * the row lengths, out_offsets matching them.  A NaN or infinite sample raises the device flag (VF_EDEVICE at
+ * vf_check_errors).  Sub-batches of at most 256 rows and 16384 frames (a longer row runs alone), four launches each, on a
+ * context-owned scratch of 16.4 KB per frame, allocated stream-ordered; no host synchronisation, no weights needed.  The
+ * scratch holds every frame of the largest sub-batch and is kept until vf_destroy: at most 269 MB for rows of up to 16384
+ * frames (190 s), but a longer row runs alone with all its frames resident, about 5.1 GB per hour of audio (34 GB for a
+ * 2^30-sample row); a call whose scratch cannot be allocated fails with VF_ECUDA before any kernel is queued.
+ * Split long recordings into segments, as the package's 30 s segmentation does. */
+VF_API int vf_remove_higher_frequency_varlen(vf_ctx* ctx, const float* x, const int64_t* in_offsets, int batch, double ratio,
+                                             float* y, const int64_t* out_offsets, int* cutoff, void* stream);
 
 /* Live streams resampled from device rings in one call (voicefixer_main_b200/streaming.py StreamingResampler, and the
  * restorers' streams at other rates).  in_ring [n_streams, in_len] (device) holds each stream's recent float32 samples at

@@ -26,6 +26,7 @@ EXPORTS = [
     "vf_score_time_varlen_ex", "vf_restore_chunks", "vf_ssr_restore_chunks", "vf_restore_windows", "vf_ssr_restore_windows",
     "vf_selftest_plan_gemms", "vf_resample_sinc_varlen", "vf_selftest_plan_trace", "vf_vocoder_varlen", "vf_resynth",
     "vf_resynth_varlen", "vf_selftest_sub_batch", "vf_vocoder_chunks", "vf_resample_rings",
+    "vf_remove_higher_frequency_varlen",
 ]
 VF_RESTORE_UNIFY_ENERGY = 1
 VF_TRACE_DIRECT_STEPS = 0x100
@@ -235,6 +236,7 @@ def load_library():
     lib.vf_resample_sinc_varlen.argtypes = [P, P, POINTER(c_int64), c_int, P, POINTER(c_int64), POINTER(c_double),
                                             POINTER(c_int), c_int, POINTER(c_int), P, POINTER(c_int64), P]
     lib.vf_resample_rings.argtypes = [P, P, c_int, c_int64, POINTER(VfResampleRow), c_int, P, c_int, c_int64, P]
+    lib.vf_remove_higher_frequency_varlen.argtypes = [P, P, POINTER(c_int64), c_int, c_double, P, POINTER(c_int64), P, P]
     _lib = lib
     return lib
 

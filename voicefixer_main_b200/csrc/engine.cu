@@ -1158,7 +1158,7 @@ VF_API void vf_destroy(vf_ctx* ctx) {
     if (st) cudaStreamDestroy(st);
   for (auto& e : ctx->ev)
     if (e) cudaEventDestroy(e);
-  for (Scratch* s : {&ctx->score, &ctx->time_score, &ctx->iir, &ctx->chunks}) {
+  for (Scratch* s : {&ctx->score, &ctx->time_score, &ctx->iir, &ctx->chunks, &ctx->prefilter}) {
     if (s->p) cudaFree(s->p);
     if (s->order.ev) cudaEventDestroy(s->order.ev);
   }
@@ -1417,6 +1417,7 @@ VF_API int vf_check_errors(vf_ctx* ctx, void* stream) {
   if (h[0] || h[1]) CK(cudaMemset(ctx->d_err, 0, 8));
   if (h[0] == ERR_FP16_OVERFLOW) return fail(ctx, VF_EDEVICE, "activation outside the fp16 range (|a| > 65504) in a hi/lo split");
   if (h[0] == ERR_NAN_PHASE) return fail(ctx, VF_EDEVICE, "NaN phase in the ISTFT: a NaN or infinite input sample");
+  if (h[0] == ERR_NONFINITE_INPUT) return fail(ctx, VF_EDEVICE, "a NaN or infinite input sample in vf_remove_higher_frequency_varlen");
   if (h[0]) return fail(ctx, VF_EDEVICE, "device pipeline error code %d (201 producer / 202 mma / 203 epilogue time-out)", h[0]);
   if (h[1]) return fail(ctx, VF_EASSERT, "input has negative values counts %d", h[1]);
   return VF_OK;

@@ -31,7 +31,7 @@ constexpr int GEMM_MAX_TAPS = 12;
 
 enum { ACT_NONE = 0, ACT_LRELU = 1, ACT_ELU = 2 };
 enum { MAP_PLAIN = 0, MAP_CONVT2D = 1, MAP_CONVT1D = 2 };
-enum { ERR_FP16_OVERFLOW = 100, ERR_NAN_PHASE = 101, ERR_PIPE_PRODUCER = 201, ERR_PIPE_MMA = 202, ERR_PIPE_EPILOGUE = 203 };
+enum { ERR_FP16_OVERFLOW = 100, ERR_NAN_PHASE = 101, ERR_NONFINITE_INPUT = 102, ERR_PIPE_PRODUCER = 201, ERR_PIPE_MMA = 202, ERR_PIPE_EPILOGUE = 203 };
 
 struct GemmTap {
   int a_off;   // row offset of the tap's window relative to the output row

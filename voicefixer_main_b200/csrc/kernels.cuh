@@ -545,4 +545,24 @@ struct SincRingParams {
 cudaError_t launch_stream_resample(const PolyRingParams& p, cudaStream_t stream);
 cudaError_t launch_stream_resample(const SincRingParams& p, cudaStream_t stream);
 
+// prefilter.cu: the pip package's remove_higher_frequency (vf_remove_higher_frequency_varlen) of one sub-batch of packed
+// float32 rows, four launches: STFT, per-row cutoff, masked inverse frames, overlap-add.  Row b has T_b = 1 + n_b / 512
+// frames at frame_off[b] of the scratch `spec`, 1025 double2 per frame (the spectrum, then the frame's 2048 doubles).
+constexpr int PREFILTER_MAX_ROWS = 256;                   // rows per sub-batch
+constexpr int64_t PREFILTER_CAP_FRAMES = 16384;           // frames per sub-batch (16.4 KB of scratch each); a longer row runs alone
+struct PrefilterParams {
+  const float* x;                            // row b = x[in_off[b] .. in_off[b + 1])
+  float* y;                                  // row b = y[out_off[b] .. out_off[b + 1]), 512 (n_b / 512) samples
+  double2* spec;                             // [frame_off[batch]][1025]
+  const double* window;                      // [2048] periodic hann, float64
+  const double2* tw1024;                     // e^{-2 pi i j / 1024}
+  const double2* tw2048;                     // e^{-2 pi i k / 2048}, k = 0..1024
+  int* cutoff;                               // [batch] first removed bin (1025: none)
+  int* err;                                  // raised (ERR_NONFINITE_INPUT) by a NaN or infinite sample
+  double ratio;
+  int batch;
+  int64_t in_off[PREFILTER_MAX_ROWS + 1], out_off[PREFILTER_MAX_ROWS + 1], frame_off[PREFILTER_MAX_ROWS + 1];
+};
+cudaError_t launch_prefilter(const PrefilterParams& p, cudaStream_t stream);
+
 }  // namespace vf

@@ -759,6 +759,55 @@ VF_API int vf_resample_sinc_varlen(vf_ctx* ctx, const float* x, const int64_t* i
   return VF_OK;
 }
 
+// ------------------------------------------------------------------------------------- the pip package's mode-1 pre-filter
+VF_API int vf_remove_higher_frequency_varlen(vf_ctx* ctx, const float* x, const int64_t* in_offsets, int batch, double ratio,
+                                             float* y, const int64_t* out_offsets, int* cutoff, void* stream) {
+  static const char* fn = "vf_remove_higher_frequency_varlen";
+  int rc = begin_call(ctx, fn, x && cutoff && batch > 0);
+  if (!rc && !(ratio > 0.0 && ratio <= 1.0)) rc = fail(ctx, VF_EINVAL, "%s: ratio %g (need 0 < ratio <= 1)", fn, ratio);
+  if (!rc) rc = check_offsets(ctx, fn, "x", "row", in_offsets, batch, 1, ITEM_MAX);
+  if (!rc && (!out_offsets || out_offsets[0] != 0)) rc = fail(ctx, VF_EINVAL, "%s: y offsets must start at 0", fn);
+  if (rc) return rc;
+  std::vector<int64_t> T(batch);
+  for (int i = 0; i < batch; ++i) {
+    const int64_t n = in_offsets[i + 1] - in_offsets[i], m = out_offsets[i + 1] - out_offsets[i];
+    if (m != 512 * (n / 512))
+      return fail(ctx, VF_EINVAL, "%s: y row %d has %ld samples (need 512 * (%ld // 512) = %ld)", fn, i, (long)m, (long)n,
+                  (long)(512 * (n / 512)));
+    T[i] = 1 + n / 512;
+  }
+  if (!y && out_offsets[batch] > 0) return fail(ctx, VF_EINVAL, "%s: no output for %ld samples", fn, (long)out_offsets[batch]);
+  cudaStream_t st = (cudaStream_t)stream;
+  // sub-batches of at most PREFILTER_MAX_ROWS rows and PREFILTER_CAP_FRAMES frames; scratch per row: its frames' spectra
+  const std::vector<int> starts = split(batch, PREFILTER_MAX_ROWS, PREFILTER_CAP_FRAMES, [&](int i) { return T[i]; });
+  rc = acquire_scratch(ctx, ctx->prefilter, max_bytes(starts, [&](int i) { return (size_t)T[i] * 1025 * sizeof(double2); }), st);
+  if (rc) return rc;
+  cudaError_t e = cudaSuccess;
+  for (size_t k = 0; k + 1 < starts.size() && e == cudaSuccess; ++k) {
+    const int s = starts[k], nb = starts[k + 1] - starts[k];
+    PrefilterParams p;
+    memset(&p, 0, sizeof p);
+    p.batch = nb;
+    p.x = x + in_offsets[s];
+    p.y = y ? y + out_offsets[s] : nullptr;
+    p.spec = static_cast<double2*>(ctx->prefilter.p);
+    p.window = ctx->d_window64; p.tw1024 = ctx->d_tw1024d; p.tw2048 = ctx->d_tw2048d;
+    p.cutoff = cutoff + s;
+    p.err = ctx->d_err;
+    p.ratio = ratio;
+    for (int i = 0; i < nb; ++i) {
+      p.in_off[i + 1] = in_offsets[s + i + 1] - in_offsets[s];
+      p.out_off[i + 1] = out_offsets[s + i + 1] - out_offsets[s];
+      p.frame_off[i + 1] = p.frame_off[i] + T[s + i];
+    }
+    e = launch_prefilter(p, st);
+    ctx->launches += p.out_off[nb] > 0 ? 4 : 3;
+  }
+  rc = mark_use(ctx, ctx->prefilter.order, st);
+  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "prefilter launch: %s", cudaGetErrorString(e));
+  return rc;
+}
+
 // ----------------------------------------------------------------------------------------- live streams' rate conversion
 VF_API int vf_resample_rings(vf_ctx* ctx, const float* in_ring, int n_streams, int64_t in_len, const vf_resample_row* rows,
                              int n_rows, float* out, int n_out_streams, int64_t out_len, void* stream) {

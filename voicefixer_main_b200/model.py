@@ -533,6 +533,23 @@ class Engine:
                                                       ratio, num_table, len(filters), rows, _ptr(out), out_off, _stream()))
         return out
 
+    def remove_higher_frequency_varlen(self, x_packed: torch.Tensor, lengths, ratio: float = 0.95):
+        """vf_remove_higher_frequency_varlen: the pip package's pre-filter remove_higher_frequency(wav, ratio) of each float32
+        row of x_packed (rows back to back, `lengths` samples each, 1 .. 2^30) -> (packed float32 output, its row lengths
+        512 * (n // 512), int32 device tensor of each row's first removed bin).  A quiet row (no bin with |X| >= 1) has cutoff
+        0 and zeros; a row under 512 samples an empty output.  A NaN or infinite sample raises VF_EDEVICE at check_errors.
+        Device scratch: 16.4 KB per frame (1 + n // 512) of the call's largest sub-batch, kept by the engine; a row longer than
+        16384 frames (190 s) runs alone with all its frames resident, about 5.1 GB per hour of audio."""
+        x_packed, off = self._varlen_args(x_packed, lengths)
+        out_lengths = [512 * ((off[i + 1] - off[i]) // 512) for i in range(len(off) - 1)]
+        out = torch.empty(sum(out_lengths), device=self.device)
+        cutoff = torch.empty(len(off) - 1, dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_remove_higher_frequency_varlen(self.ctx, _ptr(x_packed), off, len(off) - 1, float(ratio),
+                                                                _ptr(out) if out.numel() else None, _offsets(out_lengths),
+                                                                _ptr(cutoff), _stream()))
+        return out, out_lengths, cutoff
+
     def resample_rings(self, in_ring: torch.Tensor, rows, out: torch.Tensor) -> torch.Tensor:
         """Live streams resampled from a device ring in one call (vf_resample_rings).  in_ring [n_streams, in_len] float32
         holds stream s's absolute input i at in_ring[s, i % in_len].  rows is a sequence of (stream, filter, m0, m1, n, avail,
@@ -1065,6 +1082,35 @@ class VoiceFixer(_EngineModel):
         eng, lengths = self._batch_engine(wavs)
         out = eng.restore_varlen(torch.cat(wavs), lengths, unify_energy=unify_energy)
         return list(torch.split(out, lengths))
+
+    def remove_higher_frequency(self, wav, ratio=0.95) -> np.ndarray:
+        """The pip package's pre-filter (VoiceFixer.remove_higher_frequency, the first step of restore_inmem's mode 1) of one
+        1-D clip: bins from the first one where the running sum of per-bin energies sum_t max(log10(|X| + 1e-8), 0) reaches
+        ratio times their total are removed, the rest scaled by |X| / (|X| + 1e-8), in librosa 0.8's stft / istft (n_fft 2048,
+        hop 512).  -> 1-D float32 numpy of 512 * (len(wav) // 512) samples (istft with length None); a quiet clip, with no
+        bin of |X| >= 1, comes back as zeros.  One remove_higher_frequency_batch call."""
+        outs, _ = self.remove_higher_frequency_batch([wav], ratio)
+        return outs[0].cpu().numpy()
+
+    def remove_higher_frequency_batch(self, wavs, ratio=0.95):
+        """remove_higher_frequency of every 1-D clip of `wavs` (numpy arrays or tensors, on the host or the device, any
+        lengths from 1 to 2^30 samples) in one vf_remove_higher_frequency_varlen call -> (list of float32 tensors on the
+        model's device, 512 * (n // 512) samples each: empty under 512; int32 device tensor of each clip's first removed bin,
+        0 for a quiet clip, which comes back as zeros).  Each clip gets the bits it gets alone.  A ratio outside (0, 1], an
+        empty list, or a clip that is not 1-D or is empty raises ValueError before any GPU work; a NaN or infinite sample
+        raises VF_EDEVICE at the engine's check_errors."""
+        if not isinstance(ratio, (int, float, np.floating, np.integer)) or not 0 < float(ratio) <= 1:
+            raise ValueError(f"remove_higher_frequency: ratio {ratio!r} (need 0 < ratio <= 1)")
+        if not isinstance(wavs, (list, tuple)) or not wavs:
+            raise ValueError("remove_higher_frequency_batch: expected a non-empty list of 1-D clips")
+        for i, w in enumerate(wavs):
+            if np.ndim(w) != 1 or not 1 <= np.shape(w)[0] <= 1 << 30:
+                raise ValueError(f"remove_higher_frequency_batch: clip {i} must be 1-D with 1 .. 2^30 samples "
+                                 f"(got shape {tuple(np.shape(w))})")
+        eng = self._engine()
+        xs = [torch.as_tensor(w).to(eng.device, torch.float32) for w in wavs]
+        out, lengths, cutoff = eng.remove_higher_frequency_varlen(torch.cat(xs), [x.numel() for x in xs], float(ratio))
+        return list(torch.split(out, lengths)), cutoff
 
     def restore_inmem(self, wav_10k, cuda=True, mode=0, your_vocoder_func=None):
         """The pip package's in-memory entry point: 44.1 kHz samples -> restored [1, N] numpy (handler.restore_inmem)."""
