@@ -178,12 +178,18 @@ def test_null_outputs_behave_as_restore_varlen(model):
     ref, n_ref = _raw(eng, "vf_restore_varlen", clips)
     got, n_got = _raw(eng, "vf_restore_varlen_mels", clips, None, None)
     assert torch.equal(got, ref) and n_got == n_ref
-    _, mel, _ = _mels_call(eng, clips)
+    _, mel, log_mel = _mels_call(eng, clips)
     mel_only = torch.empty_like(mel)
     got2, n_mels = _raw(eng, "vf_restore_varlen_mels", clips, ctypes.c_void_p(mel_only.data_ptr()), None)
     eng.check_errors()
     assert torch.equal(got2, ref) and n_mels == n_ref + 1          # one copy kernel for the one sub-batch
     assert torch.equal(mel_only, mel)
+    mel_both, log_both = torch.full_like(mel, float("nan")), torch.full_like(log_mel, float("nan"))   # unwritten rows stay NaN
+    got3, n_both = _raw(eng, "vf_restore_varlen_mels", clips, ctypes.c_void_p(mel_both.data_ptr()),
+                        ctypes.c_void_p(log_both.data_ptr()))
+    eng.check_errors()
+    assert torch.equal(got3, ref) and n_both == n_ref + 1          # both outputs: still one copy kernel
+    assert torch.equal(mel_both, mel) and torch.equal(log_both, log_mel)
 
 
 def test_graph_replay_gives_the_first_calls_bits(fresh_model):

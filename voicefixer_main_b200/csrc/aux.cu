@@ -2,6 +2,7 @@
 // maps, vocoder conditioning, reflection padding, the Cout = 1 tail conv + tanh + peak, peak-normalise + trim.
 // All of them are one-pass, vectorised (16-byte accesses on the channel-innermost planes) and write the
 // fp16 hi/lo planes the next tensor-core GEMM consumes, so no tensor is re-read for an elementwise step.
+// Then the packed calls' lengths table and per-clip peak normalise; their row copies are stream.cu's.
 #include "gemm.cuh"
 #include "kernels.cuh"
 
@@ -444,35 +445,6 @@ __global__ void varlen_setup_kernel(const __grid_constant__ VarlenSetupParams p)
 }
 cudaError_t launch_varlen_setup(const VarlenSetupParams& p, cudaStream_t stream) {
   varlen_setup_kernel<<<(p.batch + 128) / 128, 128, 0, stream>>>(p);
-  return cudaGetLastError();
-}
-
-// One thread per mel value of the packed outputs; blocks past clip b's frames return.
-__global__ void gather_mels_kernel(const __grid_constant__ MelGatherParams p) {
-  const int b = blockIdx.y;
-  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= (size_t)(p.frame_off[b + 1] - p.frame_off[b]) * 128) return;
-  const size_t src = (size_t)b * p.T * 128 + i, dst = (size_t)p.frame_off[b] * 128 + i;
-  if (p.mel_out) p.mel_out[dst] = p.mel[src];
-  if (p.logmel_out) p.logmel_out[dst] = p.logmel[src];
-}
-cudaError_t launch_gather_mels(const MelGatherParams& p, cudaStream_t stream) {
-  gather_mels_kernel<<<dim3((unsigned)(((size_t)p.T * 128 + 255) / 256), p.batch), 256, 0, stream>>>(p);
-  return cudaGetLastError();
-}
-
-// One thread per value of clip b (blockIdx.y); blocks past its values return.
-__global__ void clip_copy_kernel(const __grid_constant__ ClipCopyParams p) {
-  const int b = blockIdx.y;
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= p.off[b + 1] - p.off[b]) return;
-  const int64_t packed = p.off[b] + i, plan = (int64_t)b * p.stride + i;
-  p.dst[p.to_packed ? packed : plan] = p.src[p.to_packed ? plan : packed];
-}
-cudaError_t launch_clip_copy(const ClipCopyParams& p, cudaStream_t stream) {
-  int64_t most = 0;
-  for (int b = 0; b < p.batch; ++b) most = std::max<int64_t>(most, p.off[b + 1] - p.off[b]);
-  clip_copy_kernel<<<dim3((unsigned)((most + 255) / 256), p.batch), 256, 0, stream>>>(p);
   return cudaGetLastError();
 }
 

@@ -5,6 +5,7 @@
 // A plan is the full, pre-resolved launch list for one (batch, frames) shape: every activation buffer is
 // allocated once, every TMA tensor map is encoded once, and running a stage is a loop of kernel launches on
 // the caller's stream - no allocation, no host synchronisation, no CPU arithmetic on the data path.
+#include <cassert>
 #include <climits>
 #include <cmath>
 #include <cstdarg>
@@ -438,9 +439,13 @@ int finalize_on(vf_ctx* ctx, Plan* plan, int batch, int64_t n, float* wav_out, c
   return VF_OK;
 }
 
-// The launch list of a vocoder-only plan, from its d_mel to d_voc_wav and d_peak: fixed pointers, replayed as a graph
+// Stages 1 to 3 of a vocoder-only plan: the launch list from its d_mel to d_voc_wav and d_peak, with fixed pointers, replayed
+// as a graph.  Stage 1 (the front end or the mel copy) ends before it, and stage 2 (the analysis module) is empty.
 int run_vocoder_chain(vf_ctx* ctx, Plan* plan, cudaStream_t st) {
-  return run_chain(ctx, plan, 0, st, (int64_t)plan->vocoder.size(), [&](cudaStream_t s) { return run_ops(ctx, plan->vocoder, s); });
+  int rc = stage_mark(ctx, 1, st);
+  if (!rc) rc = stage_mark(ctx, 2, st);
+  if (!rc) rc = run_chain(ctx, plan, 0, st, (int64_t)plan->vocoder.size(), [&](cudaStream_t s) { return run_ops(ctx, plan->vocoder, s); });
+  return rc ? rc : stage_mark(ctx, 3, st);
 }
 
 // VoiceFixer's chain (run_restore's stages 1 to 3).  off == nullptr: `batch` clips of n samples (PLAN_GSR).  Otherwise
@@ -479,11 +484,7 @@ int restore_impl(vf_ctx* ctx, Plan* plan, const float* wav, int batch, int64_t n
 int resynth_impl(vf_ctx* ctx, Plan* plan, const float* wav, int batch, int64_t n, float* wav_out, unsigned, cudaStream_t st,
                  const int64_t* off) {
   int rc = run_frontend(ctx, wav, batch, (long)n, plan->d_mel, nullptr, nullptr, nullptr, nullptr, st, off ? plan : nullptr);
-  if (rc) return rc;
-  rc = stage_mark(ctx, 1, st);
-  if (!rc) rc = stage_mark(ctx, 2, st);
   if (!rc) rc = run_vocoder_chain(ctx, plan, st);
-  if (!rc) rc = stage_mark(ctx, 3, st);
   return rc ? rc : finalize_on(ctx, plan, batch, n, wav_out, off, st);
 }
 
@@ -606,18 +607,43 @@ int restore_host(vf_ctx* ctx, const Family& f, const char* fn, const float* wav_
   });
 }
 
+// The table of one row_copy_kernel launch (kernels.cuh), built row by row in launch order.  Flat sources unless a ring
+// length is given.
+struct RowCopy {
+  RowCopyParams p;
+  explicit RowCopy(int64_t ring = INT64_MAX) {
+    memset(&p, 0, sizeof p);
+    p.ring = ring;
+  }
+  // dst[j] = src[(phase + j) mod ring] for lead <= j < n_valid, else 0, for j < count
+  void add(const float* src, float* dst, int64_t count, int64_t phase = 0, int64_t lead = 0, int64_t n_valid = INT64_MAX) {
+    assert(p.rows < ROW_COPY_ROWS);
+    const int c = p.rows++;
+    p.src[c] = src; p.dst[c] = dst;
+    p.phase[c] = phase; p.lead[c] = lead; p.n_valid[c] = n_valid;
+    p.off[c + 1] = p.off[c] + count;
+  }
+  int64_t total() const { return p.off[p.rows]; }
+  int launch(vf_ctx* ctx, cudaStream_t st) const {
+    CK(launch_row_copy(p, st));
+    ctx->launches++;
+    return VF_OK;
+  }
+};
+
 // One launch that gathers rows t < T_i of the sub-batch's [b, plan->T, 128] mel / logmel (either may be null with its
-// output) into the packed outputs at the frame offsets frame_off[s .. s + b] of its clips.
+// output) into the packed outputs at the frame offsets frame_off[s .. s + b] of its clips: b rows per output.
 int gather_mels(vf_ctx* ctx, const Plan* plan, const std::vector<int64_t>& frame_off, int s, int b, const float* mel,
                 const float* logmel, float* mel_out, float* logmel_out, cudaStream_t st) {
-  MelGatherParams g;
-  memset(&g, 0, sizeof g);
-  g.mel = mel; g.logmel = logmel; g.mel_out = mel_out; g.logmel_out = logmel_out;
-  g.batch = b; g.T = plan->T;
-  for (int i = 0; i <= b; ++i) g.frame_off[i] = frame_off[s + i];
-  CK(launch_gather_mels(g, st));
-  ctx->launches++;
-  return VF_OK;
+  RowCopy g;
+  auto rows = [&](const float* src, float* out) {
+    if (!out) return;
+    for (int i = 0; i < b; ++i)
+      g.add(src + (int64_t)i * plan->T * 128, out + frame_off[s + i] * 128, (frame_off[s + i + 1] - frame_off[s + i]) * 128);
+  };
+  rows(mel, mel_out);
+  rows(logmel, logmel_out);
+  return g.launch(ctx, st);
 }
 
 // The packed calls of family f (`fn`).  Every check comes before anything is launched, so a rejected call leaves no partial
@@ -702,23 +728,17 @@ int vocoder_varlen(vf_ctx* ctx, const float* mel, const int64_t* frame_offsets, 
   return run_sub_batches(ctx, PLAN_VOC_VARLEN, batch, bucket, [&](Plan* plan, int s, int b) {
     int64_t rel[VL_MAX_CLIPS + 1];
     for (int i = 0; i <= b; ++i) rel[i] = (frame_offsets[s + i] - frame_offsets[s] - i) * hop;
+    // rows t >= T_i of d_mel are not written: the lengths table keeps every launch of the chain off them
+    RowCopy scatter, pack;
+    for (int i = 0; i < b; ++i) {
+      scatter.add(mel + frame_offsets[s + i] * 128, plan->d_mel + (int64_t)i * plan->T * 128,
+                  (frame_offsets[s + i + 1] - frame_offsets[s + i]) * 128);
+      pack.add(plan->d_voc_wav + (int64_t)i * plan->L, wav_out + wav_off[s + i], wav_off[s + i + 1] - wav_off[s + i]);
+    }
     return run_restore(ctx, plan, RESYNTH.w0, b, rel, st, [&]() -> int {
-      ClipCopyParams c;
-      memset(&c, 0, sizeof c);
-      c.src = mel + frame_offsets[s] * 128; c.dst = plan->d_mel; c.batch = b; c.to_packed = 0; c.stride = (int64_t)plan->T * 128;
-      for (int i = 0; i <= b; ++i) c.off[i] = (frame_offsets[s + i] - frame_offsets[s]) * 128;
-      CK(launch_clip_copy(c, st));
-      ctx->launches++;
-      int r = stage_mark(ctx, 1, st);
-      if (!r) r = stage_mark(ctx, 2, st);
+      int r = scatter.launch(ctx, st);
       if (!r) r = run_vocoder_chain(ctx, plan, st);
-      if (!r) r = stage_mark(ctx, 3, st);
-      if (r) return r;
-      c.src = plan->d_voc_wav; c.dst = wav_out + wav_off[s]; c.to_packed = 1; c.stride = plan->L;
-      for (int i = 0; i <= b; ++i) c.off[i] = wav_off[s + i] - wav_off[s];
-      CK(launch_clip_copy(c, st));
-      ctx->launches++;
-      return VF_OK;
+      return r ? r : pack.launch(ctx, st);
     });
   }, VL_MAX_CLIPS);
 }
@@ -736,18 +756,13 @@ struct CropStage {
   float* kept_out;
   int64_t kept_off;
   int sub_batch(vf_ctx* ctx, int s, int b, const int64_t* off, const float* restored, cudaStream_t st) {
-    ChunkCropParams cp;
-    memset(&cp, 0, sizeof cp);
-    cp.restored = restored; cp.kept = kept_out + kept_off; cp.chunks = b;
+    RowCopy crop;
     for (int k = 0; k < b; ++k) {
       const vf_chunk& c = chunks[s + k];
-      cp.src[k] = off[k] + c.crop_left;
-      cp.keep[k + 1] = cp.keep[k] + c.length - c.crop_left - c.crop_right;
+      crop.add(restored + off[k] + c.crop_left, kept_out + kept_off + crop.total(), c.length - c.crop_left - c.crop_right);
     }
-    CK(launch_stream_crop(cp, st));
-    ctx->launches++;
-    kept_off += cp.keep[b];
-    return VF_OK;
+    kept_off += crop.total();
+    return crop.launch(ctx, st);
   }
   int finish(vf_ctx*, cudaStream_t) { return VF_OK; }
 };
@@ -874,35 +889,51 @@ int run_stream_rows(vf_ctx* ctx, const Family& f, const float* ring, int64_t rin
     float* out = in + max_samples;
     for (int s = 0; s < n_rows; s += sh.cap) {
       const int b = sh.size(s), rows = StreamShapes::rows(b);
-      ChunkGatherParams g;
-      memset(&g, 0, sizeof g);
-      g.ring = ring; g.out = in; g.ring_len = ring_len; g.rows = rows;
+      RowCopy g(ring_len);
       int64_t n_max = 0;
       for (int k = 0; k < rows; ++k) {
         const StreamRow& c = rows_in[sh.at(s, k)];
-        g.off[k + 1] = g.off[k] + c.length;
-        g.src[k] = (int64_t)c.stream * ring_len;
-        g.phase[k] = (c.start % ring_len + ring_len) % ring_len;
-        g.lead[k] = c.start < 0 ? std::min<int64_t>(c.length, -c.start) : 0;
-        g.n_valid[k] = valid_count(c.start, c.length, c.valid);
+        g.add(ring + (int64_t)c.stream * ring_len, in + g.total(), c.length, (c.start % ring_len + ring_len) % ring_len,
+              c.start < 0 ? std::min<int64_t>(c.length, -c.start) : 0, valid_count(c.start, c.length, c.valid));
         n_max = std::max<int64_t>(n_max, c.length);
       }
       Plan* plan;
       int r = get_plan(ctx, f.varlen_kind, rows, round_up(frames_of(ctx, (long)n_max), 64), &plan);
+      if (!r) r = g.launch(ctx, st);
       if (r) return r;
-      CK(launch_stream_gather(g, st));
-      ctx->launches++;
-      r = restore_on(ctx, f, plan, in, rows, n_max, out, flags, st, g.off);
+      r = restore_on(ctx, f, plan, in, rows, n_max, out, flags, st, g.p.off);
       if (r) return r;
-      r = stage.sub_batch(ctx, s, b, g.off, out, st);
+      r = stage.sub_batch(ctx, s, b, g.p.off, out, st);
       if (r) return r;
     }
     return stage.finish(ctx, st);
   });
 }
 
+// The checks of a streaming call's chunk table (`fn`), chunk by chunk and in this order: its stream; its length, from min_len
+// to the ring's ring_len `unit`s; the call's length rule, length_rule(i, length); crops that leave something of its
+// out_len(length) output samples; a start that its length does not carry past INT64_MAX.
+template <typename Rule, typename OutLen>
+int check_chunks(vf_ctx* ctx, const char* fn, const vf_chunk* chunks, int n_chunks, int n_streams, int64_t ring_len,
+                 const char* unit, int min_len, Rule length_rule, OutLen out_len) {
+  for (int i = 0; i < n_chunks; ++i) {
+    const vf_chunk& c = chunks[i];
+    if (c.stream < 0 || c.stream >= n_streams)
+      return fail(ctx, VF_EINVAL, "%s: chunk %d: stream %d is not in 0 .. %d", fn, i, c.stream, n_streams - 1);
+    if (c.length < min_len || c.length > ring_len)
+      return fail(ctx, VF_EINVAL, "%s: chunk %d: %d %s do not fit a ring of %ld", fn, i, c.length, unit, (long)ring_len);
+    const int rc = length_rule(i, c.length);
+    if (rc) return rc;
+    const int64_t n_out = out_len(c.length);
+    if (c.crop_left < 0 || c.crop_right < 0 || (int64_t)c.crop_left + c.crop_right >= n_out)
+      return fail(ctx, VF_EINVAL, "%s: chunk %d: crops %d and %d leave nothing of %ld samples", fn, i, c.crop_left, c.crop_right, (long)n_out);
+    if (c.start < 0 || c.start > INT64_MAX - c.length) return fail(ctx, VF_EINVAL, "%s: chunk %d: start %ld is out of range", fn, i, (long)c.start);
+  }
+  return VF_OK;
+}
+
 // vf_restore_chunks and vf_ssr_restore_chunks (`fn`) of family f: every check before anything is queued, then
-// run_stream_rows with the crop into kept_out.
+// run_stream_rows with the crop into kept_out.  A chunk's length below 1 fails the family's length rule.
 int restore_chunks(vf_ctx* ctx, const Family& f, const char* fn, const float* ring, int n_streams, int64_t ring_len,
                    const vf_chunk* chunks, int n_chunks, float* kept_out, unsigned flags, cudaStream_t st) {
   int rc = check_ready(ctx);
@@ -911,20 +942,11 @@ int restore_chunks(vf_ctx* ctx, const Family& f, const char* fn, const float* ri
   if (flags & ~f.known_flags) return fail(ctx, VF_EINVAL, "%s: unknown flag bits 0x%x", fn, flags);
   rc = check_networks(ctx, f.varlen_kind);
   if (rc) return rc;
+  rc = check_chunks(ctx, fn, chunks, n_chunks, n_streams, ring_len, "samples", INT_MIN,
+                    [&](int i, int length) { return check_length(ctx, f, "chunk", i, length); }, [](int length) { return (int64_t)length; });
+  if (rc) return rc;
   std::vector<StreamRow> rows(n_chunks);
-  for (int i = 0; i < n_chunks; ++i) {
-    const vf_chunk& c = chunks[i];
-    if (c.stream < 0 || c.stream >= n_streams)
-      return fail(ctx, VF_EINVAL, "%s: chunk %d: stream %d is not in 0 .. %d", fn, i, c.stream, n_streams - 1);
-    if (c.length > ring_len)
-      return fail(ctx, VF_EINVAL, "%s: chunk %d: %d samples do not fit a ring of %ld", fn, i, c.length, (long)ring_len);
-    rc = check_length(ctx, f, "chunk", i, c.length);
-    if (rc) return rc;
-    if (c.crop_left < 0 || c.crop_right < 0 || (int64_t)c.crop_left + c.crop_right >= c.length)
-      return fail(ctx, VF_EINVAL, "%s: chunk %d: crops %d and %d leave nothing of %d samples", fn, i, c.crop_left, c.crop_right, c.length);
-    if (c.start < 0 || c.start > INT64_MAX - c.length) return fail(ctx, VF_EINVAL, "%s: chunk %d: start %ld is out of range", fn, i, (long)c.start);
-    rows[i] = StreamRow{c.stream, c.length, c.start, c.valid};
-  }
+  for (int i = 0; i < n_chunks; ++i) rows[i] = StreamRow{chunks[i].stream, chunks[i].length, chunks[i].start, chunks[i].valid};
   CropStage stage{chunks, kept_out, 0};
   return run_stream_rows(ctx, f, ring, ring_len, rows, stage, flags, st);
 }
@@ -1000,66 +1022,49 @@ int vocoder_chunks(vf_ctx* ctx, const float* ring, int n_streams, int64_t ring_f
   rc = check_networks(ctx, PLAN_VOC_VARLEN);
   if (rc) return rc;
   const int64_t max_frames = vocoder_max_frames(ctx);
+  rc = check_chunks(ctx, fn, chunks, n_chunks, n_streams, ring_frames, "frames", 1, [&](int i, int length) {
+    if (length > max_frames)
+      return fail(ctx, VF_EINVAL, "%s: chunk %d: %d frames is too long for one call (at most %ld)", fn, i, length, (long)max_frames);
+    return VF_OK;
+  }, [&](int length) { return vf_vocoder_out_len(ctx, length); });
+  if (rc) return rc;
   int longest = 0;
-  for (int i = 0; i < n_chunks; ++i) {
-    const vf_chunk& c = chunks[i];
-    if (c.stream < 0 || c.stream >= n_streams)
-      return fail(ctx, VF_EINVAL, "%s: chunk %d: stream %d is not in 0 .. %d", fn, i, c.stream, n_streams - 1);
-    if (c.length < 1 || c.length > ring_frames)
-      return fail(ctx, VF_EINVAL, "%s: chunk %d: %d frames do not fit a ring of %ld", fn, i, c.length, (long)ring_frames);
-    if (c.length > max_frames)
-      return fail(ctx, VF_EINVAL, "%s: chunk %d: %d frames is too long for one call (at most %ld)", fn, i, c.length, (long)max_frames);
-    const int64_t n_out = vf_vocoder_out_len(ctx, c.length);
-    if (c.crop_left < 0 || c.crop_right < 0 || (int64_t)c.crop_left + c.crop_right >= n_out)
-      return fail(ctx, VF_EINVAL, "%s: chunk %d: crops %d and %d leave nothing of %ld samples", fn, i, c.crop_left, c.crop_right, (long)n_out);
-    if (c.start < 0 || c.start > INT64_MAX - c.length) return fail(ctx, VF_EINVAL, "%s: chunk %d: start %ld is out of range", fn, i, (long)c.start);
-    longest = std::max(longest, (int)c.length);
-  }
+  for (int i = 0; i < n_chunks; ++i) longest = std::max(longest, (int)chunks[i].length);
   const StreamShapes sh = stream_shapes(ctx, PLAN_VOC_VARLEN, n_chunks, round_up(longest, 64));
   const int hop = ctx->cfg.hop;
   int64_t kept_off = 0;
   for (int s = 0; s < n_chunks; s += sh.cap) {
     const int b = sh.size(s), rows = StreamShapes::rows(b);
-    FrameGatherParams g;
-    memset(&g, 0, sizeof g);
-    g.ring = ring; g.ring_frames = ring_frames; g.rows = rows;
     int64_t rel[VL_MAX_CLIPS + 1] = {0};      // the lengths table's sample offsets: clips of (T - 1) * hop samples
     int n_max = 0;
     for (int k = 0; k < rows; ++k) {
       const vf_chunk& c = chunks[sh.at(s, k)];
-      g.off[k + 1] = g.off[k] + c.length;
-      g.src[k] = (int64_t)c.stream * ring_frames;
-      g.phase[k] = c.start % ring_frames;
-      g.n_valid[k] = valid_count(c.start, c.length, c.valid);
       rel[k + 1] = rel[k] + (int64_t)(c.length - 1) * hop;
       n_max = std::max(n_max, (int)c.length);
     }
     Plan* plan;
     rc = get_plan(ctx, PLAN_VOC_VARLEN, rows, round_up(n_max, 64), &plan);
     if (rc) return rc;
-    g.out = plan->d_mel; g.stride = plan->T;
-    ChunkCropParams cp;
-    memset(&cp, 0, sizeof cp);
-    cp.restored = plan->d_voc_wav; cp.kept = kept_out + kept_off; cp.chunks = b;
+    // the frame rings as rings of 128 ring_frames floats; rows t >= a chunk's length of d_mel are not written, as in
+    // vf_vocoder_varlen
+    RowCopy gather(ring_frames * 128), crop;
+    for (int k = 0; k < rows; ++k) {
+      const vf_chunk& c = chunks[sh.at(s, k)];
+      gather.add(ring + (int64_t)c.stream * ring_frames * 128, plan->d_mel + (int64_t)k * plan->T * 128, (int64_t)c.length * 128,
+                 c.start % ring_frames * 128, 0, valid_count(c.start, c.length, c.valid) * 128);
+    }
     for (int k = 0; k < b; ++k) {
       const vf_chunk& c = chunks[s + k];
-      cp.src[k] = (int64_t)k * plan->L + c.crop_left;
-      cp.keep[k + 1] = cp.keep[k] + vf_vocoder_out_len(ctx, c.length) - c.crop_left - c.crop_right;
+      crop.add(plan->d_voc_wav + (int64_t)k * plan->L + c.crop_left, kept_out + kept_off + crop.total(),
+               vf_vocoder_out_len(ctx, c.length) - c.crop_left - c.crop_right);
     }
     rc = run_restore(ctx, plan, RESYNTH.w0, rows, rel, st, [&]() -> int {
-      CK(launch_frame_gather(g, st));
-      ctx->launches++;
-      int r = stage_mark(ctx, 1, st);
-      if (!r) r = stage_mark(ctx, 2, st);
+      int r = gather.launch(ctx, st);
       if (!r) r = run_vocoder_chain(ctx, plan, st);
-      if (!r) r = stage_mark(ctx, 3, st);
-      if (r) return r;
-      CK(launch_stream_crop(cp, st));
-      ctx->launches++;
-      return VF_OK;
+      return r ? r : crop.launch(ctx, st);
     });
     if (rc) return rc;
-    kept_off += cp.keep[b];
+    kept_off += crop.total();
   }
   return VF_OK;
 }

@@ -46,74 +46,26 @@ struct VarlenSetupParams {
   int* d_rows;                     // [VL_ROWS][batch]
 };
 cudaError_t launch_varlen_setup(const VarlenSetupParams& p, cudaStream_t stream);
-// vf_restore_varlen_mels: rows t < T_b of clip b in a varlen plan's [batch, T, 128] mel buffers (row stride T = the bucket)
-// -> rows [frame_off[b], frame_off[b + 1]) of packed caller buffers (either output may be null).  The frame offsets are a
-// kernel parameter, as the lengths table's sample offsets are.
-struct MelGatherParams {
-  const float* mel;
-  const float* logmel;
-  float* mel_out;
-  float* logmel_out;
-  int batch, T;
-  int64_t frame_off[VL_MAX_CLIPS + 1];
+// The row copy (stream.cu) of every packed and streaming call: the mel gathers of vf_restore_varlen_mels and
+// vf_ssr_restore_varlen_mels, vf_vocoder_varlen's scatter into d_mel and pack of d_voc_wav, and the streaming calls' gathers
+// from the device rings and crops of the kept samples.  Row c writes dst[c][j] for j < off[c + 1] - off[c]: src[c][(phase[c]
+// + j) mod ring] when lead[c] <= j < n_valid[c], else 0.  ring: the source's wrap length in floats, INT64_MAX for a flat
+// source, phase 0.  A ring of R mel frames is a ring of 128 R floats, its phase, lead and n_valid scaled by 128.  Callers
+// keep phase < ring and no row longer than ring, so one subtraction wraps.  The table is a kernel parameter, like the
+// lengths table's offsets; it holds two rows per clip of a sub-batch, so the gather of both of a sub-batch's mel outputs is
+// one launch.
+constexpr int ROW_COPY_ROWS = 2 * VL_MAX_CLIPS;
+struct RowCopyParams {
+  int64_t ring;
+  int rows;
+  int64_t off[ROW_COPY_ROWS + 1];
+  const float* src[ROW_COPY_ROWS];
+  float* dst[ROW_COPY_ROWS];
+  int64_t phase[ROW_COPY_ROWS], lead[ROW_COPY_ROWS], n_valid[ROW_COPY_ROWS];
 };
-cudaError_t launch_gather_mels(const MelGatherParams& p, cudaStream_t stream);
-// vf_vocoder_varlen: clip b's first off[b + 1] - off[b] values between a packed buffer (from element off[b]) and row b of a
-// plan buffer of `stride` elements per clip.  to_packed 0 scatters the packed mels into the plan's [batch, T, 128] d_mel
-// (off: frame offsets times 128, stride T * 128; rows t >= T_b are not written, the vocoder never reads them); 1 packs
-// each clip's first L_b samples of d_voc_wav [batch, L] (off: sample offsets, stride L).
-struct ClipCopyParams {
-  const float* src;
-  float* dst;
-  int batch, to_packed;
-  int64_t stride;
-  int64_t off[VL_MAX_CLIPS + 1];
-};
-cudaError_t launch_clip_copy(const ClipCopyParams& p, cudaStream_t stream);
+static_assert(sizeof(RowCopyParams) <= 32764, "the row copy table must fit the kernel parameter space");
+cudaError_t launch_row_copy(const RowCopyParams& p, cudaStream_t stream);
 
-// vf_restore_chunks and vf_restore_windows (stream.cu): the tables of one sub-batch, kernel parameters like the lengths
-// table's offsets.  Gather: packed sample off[c] + j (j < off[c + 1] - off[c]) of row c is ring[src[c] + (phase[c] + j) mod
-// ring_len] when lead[c] <= j < n_valid[c], else 0 (src: the row's stream times ring_len; phase: start mod ring_len, in
-// [0, ring_len); lead: the samples before position 0, 0 for a chunk; n_valid: the samples before the stream's end).  Crop:
-// kept sample keep[c] + j (j < keep[c + 1] - keep[c]) of chunk c is restored[src[c] + j] (src: the chunk's packed offset
-// plus its crop_left).
-struct ChunkGatherParams {
-  const float* ring;
-  float* out;
-  int64_t ring_len;
-  int rows;
-  int64_t off[VL_MAX_CLIPS + 1];
-  int64_t src[VL_MAX_CLIPS];
-  int64_t phase[VL_MAX_CLIPS];
-  int64_t lead[VL_MAX_CLIPS];
-  int64_t n_valid[VL_MAX_CLIPS];
-};
-cudaError_t launch_stream_gather(const ChunkGatherParams& p, cudaStream_t stream);
-struct ChunkCropParams {
-  const float* restored;
-  float* kept;
-  int chunks;
-  int64_t keep[VL_MAX_CLIPS + 1];
-  int64_t src[VL_MAX_CLIPS];
-};
-cudaError_t launch_stream_crop(const ChunkCropParams& p, cudaStream_t stream);
-// vf_vocoder_chunks' gather of one sub-batch (stream.cu), straight into a PLAN_VOC_VARLEN plan's d_mel: frame t < off[c + 1]
-// - off[c] of chunk c is the 128 floats out[(c * stride + t) * 128 ..] (stride: the plan's frames per row, its bucket), read
-// from ring[(src[c] + (phase[c] + t) mod ring_frames) * 128 ..] when t < n_valid[c], else 0 (src: the chunk's stream times
-// ring_frames; phase: start mod ring_frames; n_valid: the frames before the stream's end).  Rows t >= the chunk's length
-// are not written: the lengths table keeps every launch of the chain off them, as in vf_vocoder_varlen.  Its crop is
-// launch_stream_crop on d_voc_wav.
-struct FrameGatherParams {
-  const float* ring;
-  float* out;
-  int64_t ring_frames, stride;
-  int rows;
-  int64_t off[VL_MAX_CLIPS + 1];
-  int64_t src[VL_MAX_CLIPS];
-  int64_t phase[VL_MAX_CLIPS];
-  int64_t n_valid[VL_MAX_CLIPS];
-};
-cudaError_t launch_frame_gather(const FrameGatherParams& p, cudaStream_t stream);
 // vf_restore_windows' overlap-add of one sub-batch.  Its windows are grouped into runs, one per stream, each run's windows in
 // ascending start.  Thread pos[r] + i handles output position t = lo[r] + i of run r: for every window w in first[r] ..
 // first[r + 1] - 1 with start[w] <= t < end[w], in that order, acc[acc_row[r] + t mod acc_len] += fl(synth[t - start[w]] *

@@ -1,11 +1,12 @@
-// The data-movement kernels of vf_restore_chunks and vf_restore_windows (include/b200vf.h): the gather that builds a step's
-// packed input from the streams' device rings, and either the crop that keeps each chunk's centre of the packed restored
-// output (chunks) or the overlap-add of each synthesis-weighted window into the caller's per-stream accumulators followed by
-// the emission of the finished samples (windows).  Between the gather and the output stage runs the varlen restore chain
-// (engine.cu).  vf_vocoder_chunks has its own frame gather, straight into a vocoder plan's mel rows, and the same crop.  Each is one launch per sub-batch of at most VL_MAX_CLIPS rows (the emission: per VL_MAX_CLIPS streams),
-// whatever the number of streams: the tables are __grid_constant__ kernel parameters (about 10 KB for the gather, 13 KB for
-// the overlap-add at 256 rows), so no host memory is read after the call returns and no copy of a table is queued.  One
-// thread per packed or accumulated sample; a warp's threads nearly always fall into one row, so the table lookups broadcast.
+// The data-movement kernels of the packed and streaming calls (include/b200vf.h).  The row copy moves rows of floats
+// between packed buffers, plan buffers and the streams' device rings: the streaming calls' gather of a step's input from
+// the rings and crop of each chunk's kept centre, vf_vocoder_varlen's scatter and pack, and the varlen restores' mel
+// gathers.  vf_restore_windows instead overlap-adds each synthesis-weighted window into the caller's per-stream accumulators
+// and then emits the finished samples; vf_resample_rings resamples the streams' input rings into the restore rings.  Each
+// is one launch per sub-batch (the emission: per VL_MAX_CLIPS streams), whatever the number of streams: the tables are
+// __grid_constant__ kernel parameters (about 24.6 KB for the row copy, 13 KB for the overlap-add at 256 rows), so no host
+// memory is read after the call returns and no copy of a table is queued.  One thread per float copied, accumulated or
+// resampled; a warp's threads nearly always fall into one row, so the table lookups broadcast.
 #include "kernels.cuh"
 #include "resample.cuh"
 
@@ -27,42 +28,18 @@ __device__ __forceinline__ int find_row(const int64_t* bounds, int n, int64_t i)
 
 }  // namespace
 
-__global__ void __launch_bounds__(STREAM_THREADS) stream_gather_kernel(const __grid_constant__ ChunkGatherParams p) {
+__global__ void __launch_bounds__(STREAM_THREADS) row_copy_kernel(const __grid_constant__ RowCopyParams p) {
   const int64_t i = (int64_t)blockIdx.x * STREAM_THREADS + threadIdx.x;
   if (i >= p.off[p.rows]) return;
   const int c = find_row(p.off, p.rows, i);
   const int64_t j = i - p.off[c];
-  float v = 0.f;                                   // before position 0 or past the stream's end: the zero padding
+  float v = 0.f;                                   // before the lead or past the valid count: the zero padding
   if (j >= p.lead[c] && j < p.n_valid[c]) {
-    int64_t r = p.phase[c] + j;                    // j < length <= ring_len, so one subtraction wraps it
-    if (r >= p.ring_len) r -= p.ring_len;
-    v = __ldg(p.ring + p.src[c] + r);
+    int64_t r = p.phase[c] + j;
+    if (r >= p.ring) r -= p.ring;
+    v = __ldg(p.src[c] + r);
   }
-  p.out[i] = v;
-}
-
-// One thread per float of the packed frames: 128 consecutive threads copy one frame, so a warp reads 128 contiguous bytes
-// of one ring row and writes them to one d_mel row.
-__global__ void __launch_bounds__(STREAM_THREADS) frame_gather_kernel(const __grid_constant__ FrameGatherParams p) {
-  const int64_t i = (int64_t)blockIdx.x * STREAM_THREADS + threadIdx.x;
-  if (i >= p.off[p.rows] * 128) return;
-  const int64_t f = i >> 7;
-  const int c = find_row(p.off, p.rows, f);
-  const int64_t t = f - p.off[c];
-  float v = 0.f;                                   // at or past the stream's end: the zero fill
-  if (t < p.n_valid[c]) {
-    int64_t r = p.phase[c] + t;                    // t < length <= ring_frames, so one subtraction wraps it
-    if (r >= p.ring_frames) r -= p.ring_frames;
-    v = __ldg(p.ring + (p.src[c] + r) * 128 + (i & 127));
-  }
-  p.out[((int64_t)c * p.stride + t) * 128 + (i & 127)] = v;
-}
-
-__global__ void __launch_bounds__(STREAM_THREADS) stream_crop_kernel(const __grid_constant__ ChunkCropParams p) {
-  const int64_t i = (int64_t)blockIdx.x * STREAM_THREADS + threadIdx.x;
-  if (i >= p.keep[p.chunks]) return;
-  const int c = find_row(p.keep, p.chunks, i);
-  p.kept[i] = __ldg(p.restored + p.src[c] + (i - p.keep[c]));
+  p.dst[c][j] = v;
 }
 
 // Ascending window order per position, and the product rounded before the add (no FMA contraction): the bits of F.fold
@@ -139,21 +116,9 @@ cudaError_t launch_ring_resample(const P& p, cudaStream_t stream) {
 cudaError_t launch_stream_resample(const PolyRingParams& p, cudaStream_t stream) { return launch_ring_resample(p, stream); }
 cudaError_t launch_stream_resample(const SincRingParams& p, cudaStream_t stream) { return launch_ring_resample(p, stream); }
 
-cudaError_t launch_stream_gather(const ChunkGatherParams& p, cudaStream_t stream) {
+cudaError_t launch_row_copy(const RowCopyParams& p, cudaStream_t stream) {
   const int64_t n = p.off[p.rows];
-  stream_gather_kernel<<<(unsigned)((n + STREAM_THREADS - 1) / STREAM_THREADS), STREAM_THREADS, 0, stream>>>(p);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_frame_gather(const FrameGatherParams& p, cudaStream_t stream) {
-  const int64_t n = p.off[p.rows] * 128;
-  frame_gather_kernel<<<(unsigned)((n + STREAM_THREADS - 1) / STREAM_THREADS), STREAM_THREADS, 0, stream>>>(p);
-  return cudaGetLastError();
-}
-
-cudaError_t launch_stream_crop(const ChunkCropParams& p, cudaStream_t stream) {
-  const int64_t n = p.keep[p.chunks];
-  stream_crop_kernel<<<(unsigned)((n + STREAM_THREADS - 1) / STREAM_THREADS), STREAM_THREADS, 0, stream>>>(p);
+  row_copy_kernel<<<(unsigned)((n + STREAM_THREADS - 1) / STREAM_THREADS), STREAM_THREADS, 0, stream>>>(p);
   return cudaGetLastError();
 }
 
