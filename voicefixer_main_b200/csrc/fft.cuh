@@ -1,159 +1,111 @@
-// Shared-memory 1024-point complex FFT used by the STFT front end (frontend.cu) and the ISTFT back end (istft.cu) in fp32,
-// and by the metric STFT (metrics.cu) in fp64 through the double2 overloads at the end of this file.  256 threads, five
-// radix-4 Stockham passes, natural-order output.  A 2048-point REAL transform is one such FFT on the even/odd-packed frame z[n] = x[2n] + i x[2n+1] plus the real-FFT split (forward) or its inverse (backward).
+// Shared-memory radix-4 Stockham FFT and the real-FFT splits of the STFT kernels, templated on the complex type: float2
+// for the front end (frontend.cu) and the ISTFT (istft.cu), double2 for the metric STFT (metrics.cu), STOI (speech_metrics.cu)
+// and the pre-filter (prefilter.cu).  A 2N-point REAL transform is one N-point complex FFT on the even/odd-packed frame
+// z[n] = x[2n] + i x[2n+1] plus the real-FFT split (forward) or its inverse (backward).  Also the frame loads' two
+// centre-padding rules.
 #pragma once
 #include <cuda_runtime.h>
 
 namespace vf {
 
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) {
-  return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x);
+template <class C>
+using real_of = decltype(C::x);
+
+template <class C>
+__device__ __forceinline__ C cmul(C a, C b) {
+  return C{a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x};
 }
 
-// In: buf0[0..1023] (synchronised).  Out: returned pointer (== buf1) holds the forward DFT, e^{-2 pi i jk/1024};
-// the block is synchronised on return.  tw1024[j] = e^{-2 pi i j / 1024}.
-__device__ __forceinline__ float2* fft1024_forward(float2* buf0, float2* buf1, const float2* __restrict__ tw1024, int tid) {
-  float2* src = buf0;
-  float2* dst = buf1;
+// N = 4^PASSES points on N / 4 threads (tid 0 .. N/4 - 1), natural-order output.  Several transforms may share a block,
+// since every thread of the block runs the passes and their __syncthreads.  In: buf0[0..N) (synchronised).  Out: the
+// returned pointer (buf1 after an odd number of passes, buf0 after an even one) holds the forward DFT, e^{-2 pi i jk/N};
+// the block is synchronised on return.  tw[j] = e^{-2 pi i j / N}.
+template <int PASSES, class C>
+__device__ __forceinline__ C* fft_forward(C* buf0, C* buf1, const C* __restrict__ tw, int tid) {
+  constexpr int Q = 1 << (2 * PASSES - 2);
+  C* src = buf0;
+  C* dst = buf1;
 #pragma unroll
-  for (int pass = 0; pass < 5; ++pass) {
+  for (int pass = 0; pass < PASSES; ++pass) {
     const int ns = 1 << (2 * pass);
     const int k = tid & (ns - 1);
-    const int tw_step = k * (256 / ns);
-    float2 a = src[tid];
-    float2 bq = src[tid + 256];
-    float2 c = src[tid + 512];
-    float2 d = src[tid + 768];
+    const int tw_step = k * (Q / ns);
+    C a = src[tid];
+    C bq = src[tid + Q];
+    C c = src[tid + 2 * Q];
+    C d = src[tid + 3 * Q];
     if (pass > 0) {
-      bq = cmul(bq, __ldg(tw1024 + tw_step));
-      c = cmul(c, __ldg(tw1024 + 2 * tw_step));
-      d = cmul(d, __ldg(tw1024 + 3 * tw_step));
+      bq = cmul(bq, __ldg(tw + tw_step));
+      c = cmul(c, __ldg(tw + 2 * tw_step));
+      d = cmul(d, __ldg(tw + 3 * tw_step));
     }
-    const float2 s0 = make_float2(a.x + c.x, a.y + c.y), s1 = make_float2(a.x - c.x, a.y - c.y);
-    const float2 s2 = make_float2(bq.x + d.x, bq.y + d.y), s3 = make_float2(bq.x - d.x, bq.y - d.y);
+    const C s0 = C{a.x + c.x, a.y + c.y}, s1 = C{a.x - c.x, a.y - c.y};
+    const C s2 = C{bq.x + d.x, bq.y + d.y}, s3 = C{bq.x - d.x, bq.y - d.y};
     const int o = ((tid - k) << 2) + k;
-    dst[o] = make_float2(s0.x + s2.x, s0.y + s2.y);
-    dst[o + ns] = make_float2(s1.x + s3.y, s1.y - s3.x);          // s1 - i*s3
-    dst[o + 2 * ns] = make_float2(s0.x - s2.x, s0.y - s2.y);
-    dst[o + 3 * ns] = make_float2(s1.x - s3.y, s1.y + s3.x);      // s1 + i*s3
+    dst[o] = C{s0.x + s2.x, s0.y + s2.y};
+    dst[o + ns] = C{s1.x + s3.y, s1.y - s3.x};          // s1 - i*s3
+    dst[o + 2 * ns] = C{s0.x - s2.x, s0.y - s2.y};
+    dst[o + 3 * ns] = C{s1.x - s3.y, s1.y + s3.x};      // s1 + i*s3
     __syncthreads();
-    float2* tmp = src; src = dst; dst = tmp;
-  }
-  return src;   // five passes: buf1
-}
-
-// Bin k (0..1024) of the 2048-point real DFT from the packed 1024-point spectrum Z: X[k] = E[k] + e^{-2 pi i k/2048} O[k].
-__device__ __forceinline__ float2 rfft_split(const float2* Z, const float2* __restrict__ tw2048, int k) {
-  const float2 zk = Z[k & 1023];
-  const float2 zr = Z[(1024 - k) & 1023];
-  const float2 e = make_float2(0.5f * (zk.x + zr.x), 0.5f * (zk.y - zr.y));      // (Zk + conj Zr)/2
-  const float2 o = make_float2(0.5f * (zk.y + zr.y), -0.5f * (zk.x - zr.x));     // -i (Zk - conj Zr)/2
-  const float2 wo = cmul(o, __ldg(tw2048 + k));
-  return make_float2(e.x + wo.x, e.y + wo.y);
-}
-
-// Windowed, reflect-padded (center=True, pad n_fft/2) frame t of x[0..n), packed z[j] = x[2j] + i x[2j+1] into buf.
-__device__ __forceinline__ void load_frame_packed(float2* buf, const float* __restrict__ x, long n, int t,
-                                                  const float* __restrict__ window, int tid) {
-  for (int j = tid; j < 1024; j += 256) {
-    float v[2];
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      long g = (long)t * 441 + 2 * j + e - 1024;
-      if (g < 0) g = -g;
-      if (g >= n) g = 2L * (n - 1) - g;
-      v[e] = __ldg(x + g) * __ldg(window + 2 * j + e);
-    }
-    buf[j] = make_float2(v[0], v[1]);
-  }
-}
-
-// ---- fp64 twins of fft1024_forward / rfft_split for the metric STFT (metrics.cu), which has librosa's float64 FFT.
-// Same passes and data flow; the fp32 functions above stay as they are (the front end keeps its bits).
-__device__ __forceinline__ double2 cmul(double2 a, double2 b) {
-  return make_double2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x);
-}
-
-__device__ __forceinline__ double2* fft1024_forward(double2* buf0, double2* buf1, const double2* __restrict__ tw1024, int tid) {
-  double2* src = buf0;
-  double2* dst = buf1;
-#pragma unroll
-  for (int pass = 0; pass < 5; ++pass) {
-    const int ns = 1 << (2 * pass);
-    const int k = tid & (ns - 1);
-    const int tw_step = k * (256 / ns);
-    double2 a = src[tid];
-    double2 bq = src[tid + 256];
-    double2 c = src[tid + 512];
-    double2 d = src[tid + 768];
-    if (pass > 0) {
-      bq = cmul(bq, __ldg(tw1024 + tw_step));
-      c = cmul(c, __ldg(tw1024 + 2 * tw_step));
-      d = cmul(d, __ldg(tw1024 + 3 * tw_step));
-    }
-    const double2 s0 = make_double2(a.x + c.x, a.y + c.y), s1 = make_double2(a.x - c.x, a.y - c.y);
-    const double2 s2 = make_double2(bq.x + d.x, bq.y + d.y), s3 = make_double2(bq.x - d.x, bq.y - d.y);
-    const int o = ((tid - k) << 2) + k;
-    dst[o] = make_double2(s0.x + s2.x, s0.y + s2.y);
-    dst[o + ns] = make_double2(s1.x + s3.y, s1.y - s3.x);          // s1 - i*s3
-    dst[o + 2 * ns] = make_double2(s0.x - s2.x, s0.y - s2.y);
-    dst[o + 3 * ns] = make_double2(s1.x - s3.y, s1.y + s3.x);      // s1 + i*s3
-    __syncthreads();
-    double2* tmp = src; src = dst; dst = tmp;
+    C* tmp = src; src = dst; dst = tmp;
   }
   return src;
 }
 
-__device__ __forceinline__ double2 rfft_split(const double2* Z, const double2* __restrict__ tw2048, int k) {
-  const double2 zk = Z[k & 1023];
-  const double2 zr = Z[(1024 - k) & 1023];
-  const double2 e = make_double2(0.5 * (zk.x + zr.x), 0.5 * (zk.y - zr.y));
-  const double2 o = make_double2(0.5 * (zk.y + zr.y), -0.5 * (zk.x - zr.x));
-  const double2 wo = cmul(o, __ldg(tw2048 + k));
-  return make_double2(e.x + wo.x, e.y + wo.y);
+// Bin k (0..H) of the 2H-point real DFT from the packed H-point spectrum Z: X[k] = E[k] + e^{-2 pi i k/2H} O[k].
+// tw[k] = e^{-2 pi i k / 2H}.
+template <int H, class C>
+__device__ __forceinline__ C rfft_split(const C* Z, const C* __restrict__ tw, int k) {
+  const real_of<C> half = 0.5;
+  const C zk = Z[k & (H - 1)];
+  const C zr = Z[(H - k) & (H - 1)];
+  const C e = C{half * (zk.x + zr.x), half * (zk.y - zr.y)};      // (Zk + conj Zr)/2
+  const C o = C{half * (zk.y + zr.y), -half * (zk.x - zr.x)};     // -i (Zk - conj Zr)/2
+  const C wo = cmul(o, __ldg(tw + k));
+  return C{e.x + wo.x, e.y + wo.y};
 }
 
-// ---- fp64 256-point complex FFT and the 512-point real split, for STOI's STFT (speech_metrics.cu).  The same radix-4
-// Stockham passes with 64 threads per transform (tid 0..63); several transforms may share a block, since every thread of
-// the block runs the four passes and their __syncthreads.  tw256[j] = e^{-2 pi i j / 256}.
-__device__ __forceinline__ double2* fft256_forward(double2* buf0, double2* buf1, const double2* __restrict__ tw256, int tid) {
-  double2* src = buf0;
-  double2* dst = buf1;
-#pragma unroll
-  for (int pass = 0; pass < 4; ++pass) {
-    const int ns = 1 << (2 * pass);
-    const int k = tid & (ns - 1);
-    const int tw_step = k * (64 / ns);
-    double2 a = src[tid];
-    double2 bq = src[tid + 64];
-    double2 c = src[tid + 128];
-    double2 d = src[tid + 192];
-    if (pass > 0) {
-      bq = cmul(bq, __ldg(tw256 + tw_step));
-      c = cmul(c, __ldg(tw256 + 2 * tw_step));
-      d = cmul(d, __ldg(tw256 + 3 * tw_step));
-    }
-    const double2 s0 = make_double2(a.x + c.x, a.y + c.y), s1 = make_double2(a.x - c.x, a.y - c.y);
-    const double2 s2 = make_double2(bq.x + d.x, bq.y + d.y), s3 = make_double2(bq.x - d.x, bq.y - d.y);
-    const int o = ((tid - k) << 2) + k;
-    dst[o] = make_double2(s0.x + s2.x, s0.y + s2.y);
-    dst[o + ns] = make_double2(s1.x + s3.y, s1.y - s3.x);          // s1 - i*s3
-    dst[o + 2 * ns] = make_double2(s0.x - s2.x, s0.y - s2.y);
-    dst[o + 3 * ns] = make_double2(s1.x - s3.y, s1.y + s3.x);      // s1 + i*s3
-    __syncthreads();
-    double2* tmp = src; src = dst; dst = tmp;
+// The last step of the packed 2048-point real inverse (istft.cu describes it): z = FFT(conj Z) of the packed spectrum Z, and
+// the frame's samples 2j, 2j + 1 are conj(z[j]) / 1024 times the window; 256 threads
+template <class C>
+__device__ __forceinline__ void irfft_unpack(C* out, const C* z, const C* __restrict__ win, int tid) {
+  const real_of<C> scale = real_of<C>(1) / real_of<C>(1024);
+  for (int j = tid; j < 1024; j += 256) {
+    const C v = z[j], w = __ldg(win + j);
+    out[j] = C{v.x * scale * w.x, -v.y * scale * w.y};
   }
-  return src;   // four passes: buf0
 }
 
-// Bin k (0..256) of the 512-point real DFT from the packed 256-point spectrum Z.  tw512[k] = e^{-2 pi i k / 512}.
-__device__ __forceinline__ double2 rfft512_split(const double2* Z, const double2* __restrict__ tw512, int k) {
-  const double2 zk = Z[k & 255];
-  const double2 zr = Z[(256 - k) & 255];
-  const double2 e = make_double2(0.5 * (zk.x + zr.x), 0.5 * (zk.y - zr.y));
-  const double2 o = make_double2(0.5 * (zk.y + zr.y), -0.5 * (zk.x - zr.x));
-  const double2 wo = cmul(o, __ldg(tw512 + k));
-  return make_double2(e.x + wo.x, e.y + wo.y);
+// Centre padding, as an index s (-pad <= s < n + pad) into a clip of n samples.  reflect_once: one reflection at each end
+// (torch's and librosa's reflect padding, n > pad).
+__device__ __forceinline__ long reflect_once(long s, long n) {
+  if (s < 0) s = -s;
+  if (s >= n) s = 2L * (n - 1) - s;
+  return s;
+}
+
+// np.pad(x, 1024, mode="reflect") at padded position s + 1024: the even periodic extension of period 2 (n - 1), which
+// is what numpy's repeated reflection makes of a clip of n <= 1024 samples; a one-sample clip pads with itself
+__device__ __forceinline__ int64_t reflect_repeated(int64_t s, int64_t n) {
+  if (n == 1) return 0;
+  const int64_t P = 2 * (n - 1);
+  s %= P;
+  if (s < 0) s += P;
+  return s >= n ? P - s : s;
+}
+
+// Windowed, reflect-padded (center=True, pad n_fft/2) frame t (the caller's int or long frame index) of x[0..n) at hop
+// HOP, packed z[j] = w[2j] x[2j] + i w[2j+1] x[2j+1] into buf; 256 threads
+template <int HOP, class C, class I>
+__device__ __forceinline__ void load_frame_packed(C* buf, const float* __restrict__ x, long n, I t,
+                                                  const real_of<C>* __restrict__ window, int tid) {
+  for (int j = tid; j < 1024; j += 256) {
+    real_of<C> v[2];
+#pragma unroll
+    for (int e = 0; e < 2; ++e)
+      v[e] = (real_of<C>)__ldg(x + reflect_once((long)t * HOP + 2 * j + e - 1024, n)) * __ldg(window + 2 * j + e);
+    buf[j] = C{v[0], v[1]};
+  }
 }
 
 }  // namespace vf

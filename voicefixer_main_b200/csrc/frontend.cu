@@ -29,14 +29,14 @@ __global__ void __launch_bounds__(256) frontend_kernel(FrontendParams p) {
   }
 
   // windowed, reflect-padded frame packed as z[n] = x[2n] + i x[2n+1]; 1024-point FFT (fft.cuh)
-  load_frame_packed(buf0, x, n, t, p.window, tid);
+  load_frame_packed<441>(buf0, x, n, t, p.window, tid);
   __syncthreads();
-  const float2* src = fft1024_forward(buf0, buf1, p.tw1024, tid);
+  const float2* src = fft_forward<5>(buf0, buf1, p.tw1024, tid);
   // src == buf1 now holds Z[0..1023]; buf0 is free and becomes the magnitude row
   float* mag = reinterpret_cast<float*>(buf0);
   const size_t frame = (size_t)b * p.T + t;
   for (int k = tid; k <= 1024; k += 256) {
-    const float2 xk = rfft_split(src, p.tw2048, k);
+    const float2 xk = rfft_split<1024>(src, p.tw2048, k);
     const float re = xk.x, im = xk.y;
     const float m = sqrtf(fmaxf(re * re + im * im, 1e-8f));       // fDomainHelper.py:62, eps = 1e-8
     mag[k] = m;

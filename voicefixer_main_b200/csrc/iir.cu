@@ -5,15 +5,6 @@
 namespace vf {
 namespace {
 
-__device__ __forceinline__ int row_of(const int64_t* off, int batch, int64_t g) {
-  int lo = 0, hi = batch;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (off[mid] <= g) lo = mid; else hi = mid;
-  }
-  return lo;
-}
-
 // Sample i of row b's input to this pass.  Forward: the odd extension 2 x[0] - x[edge - i] / x[i - edge] /
 // 2 x[n-1] - x[n - 2 - (i - edge - n)] (scipy's odd_ext, computed in the input's dtype: rounded to float32 for a
 // float32 row).  Backward: the forward result reversed.
@@ -35,7 +26,7 @@ template <bool BACK, bool PHASE_C>
 __global__ void __launch_bounds__(128) sos_chunk_kernel(SosParams p) {
   const int64_t g = (int64_t)blockIdx.x * 128 + threadIdx.x;
   if (g >= p.chunk_off[p.batch]) return;
-  const int b = row_of(p.chunk_off, p.batch, g);
+  const int b = packed_row(p.chunk_off, p.batch, g);
   const int64_t k = g - p.chunk_off[b];
   const int64_t nc = p.chunk_off[b + 1] - p.chunk_off[b];
   if (!PHASE_C && k == nc - 1) return;
@@ -149,7 +140,7 @@ __global__ void __launch_bounds__(32) iir_design_kernel(IirDesignParams p) {
 __global__ void __launch_bounds__(256) resample_f64_kernel(ResampleF64Params p) {
   const int64_t g = (int64_t)blockIdx.x * 256 + threadIdx.x;
   if (g >= p.out_off[p.batch]) return;
-  const int b = row_of(p.out_off, p.batch, g);
+  const int b = packed_row(p.out_off, p.batch, g);
   const int64_t m = g - p.out_off[b], n = p.in_off[b + 1] - p.in_off[b];
   const int64_t up = p.up[b], down = p.down[b], half = p.half[b];
   double acc = 0.0;

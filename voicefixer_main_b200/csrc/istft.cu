@@ -31,11 +31,11 @@ __global__ void __launch_bounds__(256) istft_frames_kernel(IstftFramesParams p) 
       x = p.wav + __ldg(p.vl_off + b);
       n = (long)(__ldg(p.vl_off + b + 1) - __ldg(p.vl_off + b));
     }
-    load_frame_packed(buf0, x, n, t, p.window, tid);
+    load_frame_packed<441>(buf0, x, n, t, p.window, tid);
     __syncthreads();
-    const float2* Z = fft1024_forward(buf0, buf1, p.tw1024, tid);
+    const float2* Z = fft_forward<5>(buf0, buf1, p.tw1024, tid);
     for (int k = tid; k <= 1024; k += 256) {
-      const float2 xk = rfft_split(Z, p.tw2048, k);
+      const float2 xk = rfft_split<1024>(Z, p.tw2048, k);
       const float m = sqrtf(fmaxf(xk.x * xk.x + xk.y * xk.y, 1e-8f));     // fDomainHelper.py:62
       const float cs = xk.x / m, sn = xk.y / m;                              // fDomainHelper.py:63-64
       // the magnitude's clamp maps a NaN power to 1e-4, but the phase keeps the NaN and would carry it to the output
@@ -59,14 +59,8 @@ __global__ void __launch_bounds__(256) istft_frames_kernel(IstftFramesParams p) 
     buf0[k] = make_float2(e.x - o.y, -(e.y + o.x));
   }
   __syncthreads();
-  const float2* z = fft1024_forward(buf0, buf1, p.tw1024, tid);
-  float2* out = reinterpret_cast<float2*>(p.frames + frame * 2048);
-  const float2* win = reinterpret_cast<const float2*>(p.window);
-  for (int j = tid; j < 1024; j += 256) {
-    const float2 v = z[j];
-    const float2 w = __ldg(win + j);
-    out[j] = make_float2(v.x * (1.f / 1024.f) * w.x, -v.y * (1.f / 1024.f) * w.y);
-  }
+  const float2* z = fft_forward<5>(buf0, buf1, p.tw1024, tid);
+  irfft_unpack(reinterpret_cast<float2*>(p.frames + frame * 2048), z, reinterpret_cast<const float2*>(p.window), tid);
 }
 cudaError_t launch_istft_frames(const IstftFramesParams& p, cudaStream_t stream) {
   dim3 grid(p.T, p.batch);

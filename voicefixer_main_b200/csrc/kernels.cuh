@@ -1,4 +1,4 @@
-// Parameter blocks and launchers of the non-GEMM kernels on the hot path.
+// Parameter blocks and launchers of the non-GEMM kernels on the hot path, and the packed sets' row lookup.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -46,6 +46,18 @@ struct VarlenSetupParams {
   int* d_rows;                     // [VL_ROWS][batch]
 };
 cudaError_t launch_varlen_setup(const VarlenSetupParams& p, cudaStream_t stream);
+
+// The row of a packed set that holds element i (i < off[n]): the c with off[c] <= i < off[c + 1], off[0..n] increasing,
+// the convention of the offsets tables below.
+__device__ __forceinline__ int packed_row(const int64_t* off, int n, int64_t i) {
+  int lo = 0, hi = n;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (off[mid] <= i) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
 // The row copy (stream.cu) of every packed and streaming call: the mel gathers of vf_restore_varlen_mels and
 // vf_ssr_restore_varlen_mels, vf_vocoder_varlen's scatter into d_mel and pack of d_voc_wav, and the streaming calls' gathers
 // from the device rings and crops of the kept samples.  Row c writes dst[c][j] for j < off[c + 1] - off[c]: src[c][(phase[c]

@@ -17,30 +17,16 @@ __global__ void __launch_bounds__(256) metric_stft_kernel(MetricStftParams p) {
   __shared__ double2 buf1[1024];
   const int tid = threadIdx.x, z = blockIdx.y;
   const int64_t g = blockIdx.x;
-  int lo = 0, hi = p.batch;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (p.frame_off[mid] <= g) lo = mid; else hi = mid;
-  }
-  const long t = (long)(g - p.frame_off[lo]);
-  const float* x = p.wav[z] + p.off[z][lo];
-  const long n = (long)(p.off[z][lo + 1] - p.off[z][lo]);
-  for (int j = tid; j < 1024; j += 256) {       // z[j] = w[2j] x[2j] + i w[2j+1] x[2j+1] of the reflect-padded frame
-    double v[2];
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      long s = t * 441 + 2 * j + e - 1024;
-      if (s < 0) s = -s;
-      if (s >= n) s = 2L * (n - 1) - s;
-      v[e] = (double)__ldg(x + s) * __ldg(p.window + 2 * j + e);
-    }
-    buf0[j] = make_double2(v[0], v[1]);
-  }
+  const int b = packed_row(p.frame_off, p.batch, g);
+  const long t = (long)(g - p.frame_off[b]);
+  const float* x = p.wav[z] + p.off[z][b];
+  const long n = (long)(p.off[z][b + 1] - p.off[z][b]);
+  load_frame_packed<441>(buf0, x, n, t, p.window, tid);
   __syncthreads();
-  const double2* Z = fft1024_forward(buf0, buf1, p.tw1024, tid);
+  const double2* Z = fft_forward<5>(buf0, buf1, p.tw1024, tid);
   float* out = p.sp[z] + (size_t)g * 1025;
   for (int k = tid; k <= 1024; k += 256) {
-    const double2 X = rfft_split(Z, p.tw2048, k);
+    const double2 X = rfft_split<1024>(Z, p.tw2048, k);
     const float re = (float)X.x, im = (float)X.y;                // complex64 storage
     out[k] = (float)sqrt((double)re * re + (double)im * im);     // numpy's complex64 abs (hypotf); the products are exact
   }
@@ -68,20 +54,12 @@ __global__ void __launch_bounds__(DFT743_THREADS) metric_dft743_kernel(MetricStf
       for (int i = tid; i < DFT743_N; i += DFT743_THREADS) xs[f][i] = 0.0;
       continue;
     }
-    int lo = 0, hi = p.batch;
-    while (hi - lo > 1) {
-      const int mid = (lo + hi) >> 1;
-      if (p.frame_off[mid] <= g) lo = mid; else hi = mid;
-    }
-    const long t = (long)(g - p.frame_off[lo]);
-    const float* x = p.wav[z] + p.off[z][lo];
-    const long n = (long)(p.off[z][lo + 1] - p.off[z][lo]);
-    for (int i = tid; i < DFT743_N; i += DFT743_THREADS) {    // the reflect-padded frame times the float64 window
-      long s = t * 160 + i - DFT743_N / 2;
-      if (s < 0) s = -s;
-      if (s >= n) s = 2L * (n - 1) - s;
-      xs[f][i] = (double)__ldg(x + s) * __ldg(p.window + i);
-    }
+    const int b = packed_row(p.frame_off, p.batch, g);
+    const long t = (long)(g - p.frame_off[b]);
+    const float* x = p.wav[z] + p.off[z][b];
+    const long n = (long)(p.off[z][b + 1] - p.off[z][b]);
+    for (int i = tid; i < DFT743_N; i += DFT743_THREADS)     // the reflect-padded frame times the float64 window
+      xs[f][i] = (double)__ldg(x + reflect_once(t * 160 + i - DFT743_N / 2, n)) * __ldg(p.window + i);
   }
   __syncthreads();
   if (tid >= DFT743_BINS) return;

@@ -21,32 +21,13 @@ namespace {
 constexpr double PF_EPS = 1e-8;
 constexpr int PF_BINS = 1025, PF_HOP = 512, PF_CUTOFF_THREADS = 1024;
 
-__device__ __forceinline__ int pf_row_of(const int64_t* off, int batch, int64_t g) {
-  int lo = 0, hi = batch;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (off[mid] <= g) lo = mid; else hi = mid;
-  }
-  return lo;
-}
-
-// np.pad(x, 1024, mode="reflect") at padded position s + 1024: the even periodic extension of period 2 (n - 1), which
-// is what numpy's repeated reflection makes of a clip of n <= 1024 samples; a one-sample clip pads with itself
-__device__ __forceinline__ int64_t pf_reflect(int64_t s, int64_t n) {
-  if (n == 1) return 0;
-  const int64_t P = 2 * (n - 1);
-  s %= P;
-  if (s < 0) s += P;
-  return s >= n ? P - s : s;
-}
-
 // One CTA per frame of the sub-batch
 __global__ void __launch_bounds__(256) prefilter_stft_kernel(const PrefilterParams p) {
   __shared__ double2 buf0[1024];
   __shared__ double2 buf1[1024];
   const int tid = threadIdx.x;
   const int64_t g = blockIdx.x;
-  const int b = pf_row_of(p.frame_off, p.batch, g);
+  const int b = packed_row(p.frame_off, p.batch, g);
   const int64_t t = g - p.frame_off[b];
   const float* x = p.x + p.in_off[b];
   const int64_t n = p.in_off[b + 1] - p.in_off[b];
@@ -55,7 +36,7 @@ __global__ void __launch_bounds__(256) prefilter_stft_kernel(const PrefilterPara
     double v[2];
 #pragma unroll
     for (int e = 0; e < 2; ++e) {
-      const float s = __ldg(x + pf_reflect(t * PF_HOP + 2 * j + e - 1024, n));
+      const float s = __ldg(x + reflect_repeated(t * PF_HOP + 2 * j + e - 1024, n));
       finite = finite && isfinite(s);
       v[e] = (double)s * __ldg(p.window + 2 * j + e);
     }
@@ -63,9 +44,9 @@ __global__ void __launch_bounds__(256) prefilter_stft_kernel(const PrefilterPara
   }
   if (!finite && p.err) atomicCAS(p.err, 0, ERR_NONFINITE_INPUT);
   __syncthreads();
-  const double2* Z = fft1024_forward(buf0, buf1, p.tw1024, tid);
+  const double2* Z = fft_forward<5>(buf0, buf1, p.tw1024, tid);
   double2* out = p.spec + (size_t)g * PF_BINS;
-  for (int k = tid; k < PF_BINS; k += 256) out[k] = rfft_split(Z, p.tw2048, k);
+  for (int k = tid; k < PF_BINS; k += 256) out[k] = rfft_split<1024>(Z, p.tw2048, k);
 }
 
 // max(log10(|X| + EPS), 0): log10 is negative exactly below 1
@@ -122,7 +103,7 @@ __global__ void __launch_bounds__(256) prefilter_istft_kernel(const PrefilterPar
   __shared__ double2 buf1[1024];
   const int tid = threadIdx.x;
   const int64_t g = blockIdx.x;
-  const int b = pf_row_of(p.frame_off, p.batch, g);
+  const int b = packed_row(p.frame_off, p.batch, g);
   const int cutoff = p.cutoff[b];
   double2* slot = p.spec + (size_t)g * PF_BINS;
   for (int k = tid; k < 1024; k += 256) {
@@ -135,13 +116,8 @@ __global__ void __launch_bounds__(256) prefilter_istft_kernel(const PrefilterPar
     buf0[k] = make_double2(e.x - o.y, -(e.y + o.x));                               // conj(E + i O)
   }
   __syncthreads();                              // every read of the slot is done before the frame overwrites it
-  const double2* z = fft1024_forward(buf0, buf1, p.tw1024, tid);
-  double2* out = reinterpret_cast<double2*>(slot);
-  const double2* win = reinterpret_cast<const double2*>(p.window);
-  for (int j = tid; j < 1024; j += 256) {
-    const double2 v = z[j], w = __ldg(win + j);
-    out[j] = make_double2(v.x * (1.0 / 1024.0) * w.x, -v.y * (1.0 / 1024.0) * w.y);
-  }
+  const double2* z = fft_forward<5>(buf0, buf1, p.tw1024, tid);
+  irfft_unpack(slot, z, reinterpret_cast<const double2*>(p.window), tid);
 }
 
 // One thread per output sample j of the sub-batch: padded position j + 1024 gathers its (at most four) frames in
@@ -150,7 +126,7 @@ __global__ void __launch_bounds__(256) prefilter_istft_kernel(const PrefilterPar
 __global__ void __launch_bounds__(256) prefilter_ola_kernel(const PrefilterParams p) {
   const int64_t g = (int64_t)blockIdx.x * 256 + threadIdx.x;
   if (g >= p.out_off[p.batch]) return;
-  const int b = pf_row_of(p.out_off, p.batch, g);
+  const int b = packed_row(p.out_off, p.batch, g);
   const int64_t pos = g - p.out_off[b] + 1024;
   const int64_t T = p.frame_off[b + 1] - p.frame_off[b];
   const int64_t t_lo = pos > 2047 ? (pos - 2047 + PF_HOP - 1) / PF_HOP : 0;

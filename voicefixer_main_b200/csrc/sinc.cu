@@ -7,21 +7,12 @@
 namespace vf {
 namespace {
 
-__device__ __forceinline__ int sinc_row_of(const int64_t* off, int batch, int64_t g) {
-  int lo = 0, hi = batch;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (off[mid] <= g) lo = mid; else hi = mid;
-  }
-  return lo;
-}
-
 // One thread per output sample g of the packed output; row b's slots past n_valid[b] = int(n sample_ratio) are zeros.  The
 // body is sinc_output (resample.cuh), which the streaming resampler shares.
 __global__ void __launch_bounds__(256) sinc_resample_kernel(const SincParams p) {
   const int64_t g = (int64_t)blockIdx.x * 256 + threadIdx.x;
   if (g >= p.out_off[p.batch]) return;
-  const int b = sinc_row_of(p.out_off, p.batch, g);
+  const int b = packed_row(p.out_off, p.batch, g);
   const int64_t t = g - p.out_off[b];
   float y = 0.f;
   if (t < p.n_valid[b])

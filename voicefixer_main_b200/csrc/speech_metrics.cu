@@ -11,15 +11,6 @@ namespace {
 
 constexpr double EPS = 2.220446049250313e-16;   // np.finfo(np.float64).eps
 
-__device__ __forceinline__ int pair_of(const int64_t* off, int batch, int64_t g) {
-  int lo = 0, hi = batch;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (off[mid] <= g) lo = mid; else hi = mid;
-  }
-  return lo;
-}
-
 // SI-SDR of pair blockIdx.x, r = target, e = estimate, both zero-padded to N: a = (eps + r.e) / (r.r + eps), then
 // Sss = sum (a r)^2 and Snn = sum (e - a r)^2 in a second pass (no expansion: it would cancel when e ~ r).
 __global__ void __launch_bounds__(256) sisdr_kernel(TimeScoreParams p) {
@@ -55,7 +46,7 @@ __global__ void __launch_bounds__(256) stoi_resample_kernel(TimeScoreParams p) {
   const int z = blockIdx.y;
   const int64_t g = (int64_t)blockIdx.x * 256 + threadIdx.x;
   if (g >= p.r_off[p.batch]) return;
-  const int b = pair_of(p.r_off, p.batch, g);
+  const int b = packed_row(p.r_off, p.batch, g);
   const int64_t m = g - p.r_off[b];
   const int64_t* off = z ? p.e_off : p.t_off;
   const float* x = (z ? p.est : p.tgt) + off[b];
@@ -75,7 +66,7 @@ __global__ void __launch_bounds__(256) stoi_energy_kernel(TimeScoreParams p) {
   const int64_t g = ((int64_t)blockIdx.x * 256 + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (g >= p.f_off[p.batch]) return;
-  const int b = pair_of(p.f_off, p.batch, g);
+  const int b = packed_row(p.f_off, p.batch, g);
   const double* x = p.rs + p.r_off[b] + (g - p.f_off[b]) * STOI_HOP;
   double acc = 0;
 #pragma unroll
@@ -128,7 +119,7 @@ __global__ void __launch_bounds__(256) stoi_compact_kernel(TimeScoreParams p) {
   const int z = blockIdx.y;
   const int64_t g = (int64_t)blockIdx.x * 256 + threadIdx.x;
   if (g >= p.r_off[p.batch]) return;
-  const int b = pair_of(p.r_off, p.batch, g);
+  const int b = packed_row(p.r_off, p.batch, g);
   const int64_t s = g - p.r_off[b];
   const int K = p.kept[b];
   if (s >= (int64_t)(K + 1) * STOI_HOP) return;
@@ -155,7 +146,7 @@ __global__ void __launch_bounds__(256) stoi_bands_kernel(TimeScoreParams p) {
   int b = 0;
   int64_t k = 0;
   if (active) {
-    b = pair_of(p.f_off, p.batch, g);
+    b = packed_row(p.f_off, p.batch, g);
     k = g - p.f_off[b];
     active = k < (int64_t)p.kept[b] - 1;
   }
@@ -168,9 +159,9 @@ __global__ void __launch_bounds__(256) stoi_bands_kernel(TimeScoreParams p) {
       buf[grp][0][j] = v;
     }
     __syncthreads();
-    const double2* Z = fft256_forward(buf[grp][0], buf[grp][1], p.tw256, tid);
+    const double2* Z = fft_forward<4>(buf[grp][0], buf[grp][1], p.tw256, tid);
     for (int q = tid; q <= 256; q += 64) {
-      const double2 X = rfft512_split(Z, p.tw512, q);
+      const double2 X = rfft_split<256>(Z, p.tw512, q);
       const double m = sqrt(X.x * X.x + X.y * X.y);      // np.square(np.abs(X))
       pw[grp][q] = m * m;
     }
@@ -189,7 +180,7 @@ __global__ void __launch_bounds__(256) stoi_bands_kernel(TimeScoreParams p) {
 __global__ void __launch_bounds__(256) stoi_corr_kernel(TimeScoreParams p) {
   __shared__ double sh[8];
   const int t = blockIdx.x;
-  const int b = pair_of(p.tile_off, p.batch, t);
+  const int b = packed_row(p.tile_off, p.batch, t);
   const int64_t item = (t - p.tile_off[b]) * 256 + threadIdx.x;
   const int64_t J = (int64_t)p.kept[b] - 1 - (STOI_SEG - 1);
   double rho = 0;

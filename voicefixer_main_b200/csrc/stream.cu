@@ -16,22 +16,12 @@ namespace {
 
 constexpr int STREAM_THREADS = 256;
 
-// The row c of a packed table with bounds[c] <= i < bounds[c + 1] (bounds increasing, i < bounds[n])
-__device__ __forceinline__ int find_row(const int64_t* bounds, int n, int64_t i) {
-  int lo = 0, hi = n;
-  while (hi - lo > 1) {
-    const int mid = (lo + hi) >> 1;
-    if (bounds[mid] <= i) lo = mid; else hi = mid;
-  }
-  return lo;
-}
-
 }  // namespace
 
 __global__ void __launch_bounds__(STREAM_THREADS) row_copy_kernel(const __grid_constant__ RowCopyParams p) {
   const int64_t i = (int64_t)blockIdx.x * STREAM_THREADS + threadIdx.x;
   if (i >= p.off[p.rows]) return;
-  const int c = find_row(p.off, p.rows, i);
+  const int c = packed_row(p.off, p.rows, i);
   const int64_t j = i - p.off[c];
   float v = 0.f;                                   // before the lead or past the valid count: the zero padding
   if (j >= p.lead[c] && j < p.n_valid[c]) {
@@ -48,7 +38,7 @@ __global__ void __launch_bounds__(STREAM_THREADS) row_copy_kernel(const __grid_c
 __global__ void __launch_bounds__(STREAM_THREADS) window_ola_kernel(const __grid_constant__ WindowOlaParams p) {
   const int64_t i = (int64_t)blockIdx.x * STREAM_THREADS + threadIdx.x;
   if (i >= p.pos[p.runs]) return;
-  const int r = find_row(p.pos, p.runs, i);
+  const int r = packed_row(p.pos, p.runs, i);
   const int64_t t = p.lo[r] + (i - p.pos[r]);
   int lo = p.first[r], hi = p.first[r + 1];        // the first window with start + W > t: the earliest that covers t
   while (lo < hi) {
@@ -70,7 +60,7 @@ __global__ void __launch_bounds__(STREAM_THREADS) window_ola_kernel(const __grid
 __global__ void __launch_bounds__(STREAM_THREADS) window_emit_kernel(const __grid_constant__ WindowEmitParams p) {
   const int64_t i = (int64_t)blockIdx.x * STREAM_THREADS + threadIdx.x;
   if (i >= p.off[p.n]) return;
-  const int e = find_row(p.off, p.n, i);
+  const int e = packed_row(p.off, p.n, i);
   int64_t r = p.phase[e] + (i - p.off[e]);         // count <= acc_len, so one subtraction wraps it
   if (r >= p.acc_len) r -= p.acc_len;
   float* a = p.acc + p.row[e] + r;
@@ -96,7 +86,7 @@ __global__ void __launch_bounds__(STREAM_THREADS) stream_resample_kernel(const _
   const RingResampleRows& q = p.r;
   const int64_t i = (int64_t)blockIdx.x * STREAM_THREADS + threadIdx.x;
   if (i >= q.off[q.rows]) return;
-  const int r = find_row(q.off, q.rows, i);
+  const int r = packed_row(q.off, q.rows, i);
   const int64_t j = i - q.off[r];
   const float y = ring_output(p, r, RingInput{q.ring + q.src[r], q.in_len, q.a0[r], q.a_ph[r]}, q.m0[r] + j);
   int64_t d = j;
