@@ -58,6 +58,8 @@
  *   vf_resample_rings             either resampler on live streams, incrementally from device rings: the input
  *                                 conversion of load_wav for audio that arrives while it is restored
  *   vf_remove_higher_frequency_varlen  the pip package's mode-1 pre-filter, remove_higher_frequency, before a restore
+ *   vf_decode_pcm_varlen          the decode and downmix of librosa.load(path, mono=True) (tools/utils.py:46-48,
+ *                                 metrics.py:33-34) for 8-, 16-, 24-, 32-bit and float WAV data of any channel count
  *
  * Conventions: every function returns 0 on success or a negative VF_E* code and never throws; the message is
  * available from vf_last_error().  All tensor arguments are contiguous fp32.  Unless a name ends in `_host`,
@@ -489,6 +491,36 @@ VF_API int vf_resample_sinc_varlen(vf_ctx* ctx, const float* x, const int64_t* i
  * Split long recordings into segments, as the package's 30 s segmentation does. */
 VF_API int vf_remove_higher_frequency_varlen(vf_ctx* ctx, const float* x, const int64_t* in_offsets, int batch, double ratio,
                                              float* y, const int64_t* out_offsets, int* cutoff, void* stream);
+
+/* librosa.load(path, sr=None, mono=True)'s samples of `n_rows` WAV data chunks (soundfile's float read, then librosa 0.8's
+ * to_mono), decoded on the device.  bytes: one device buffer holding every row's data chunk.  rows: HOST table (read during
+ * the call only); row i holds `frames` interleaved frames of `channels` (1 .. 64) samples of `format` from bytes +
+ * byte_offset; the caller keeps every row inside the buffer.  byte_offset is a multiple of the sample width for u8, s16,
+ * s32, f32 and f64 data (those are read with aligned loads); s24 frames may sit at any byte (byte loads).  Samples convert
+ * as libsndfile's float read does: u8 (b - 128) / 128, s16 v 2^-15, s24 v 2^-23 (sign-extended), s32 float32(v) 2^-31
+ * (rounded to nearest), f32 unchanged (NaN and Inf included), f64 rounded to float32.  mono_out (device, float32) receives
+ * the rows packed back to back, row i at sum_{j<i} frames_j: the channel itself for one channel (librosa leaves a 1-D
+ * signal alone), else numpy's float32 x.mean(axis=1) of the row's [frames, channels] samples, bit for bit: numpy's
+ * add.reduce order over the frame's channels (sequential below 8, its eight running sums from 8 on, added to the
+ * identity 0) and one float32 division by the channel count.  first_out (device, float64, packed the same; may be NULL)
+ * receives channel 0 as soundfile reads it in float64, speechmetrics' input: the exact quotient for the integer formats,
+ * the value itself for the float formats.  A row's bits do not depend on its batch, position or sub-batch.  Every
+ * argument is checked before any work is queued (VF_EINVAL, naming the row).  One thread per output frame, one launch per
+ * 1024 rows; no scratch, no host synchronisation. */
+#define VF_PCM_U8 0
+#define VF_PCM_S16 1
+#define VF_PCM_S24 2
+#define VF_PCM_S32 3
+#define VF_PCM_F32 4
+#define VF_PCM_F64 5
+typedef struct vf_pcm_row {
+  int64_t byte_offset;      /* of the row's first frame in `bytes` */
+  int64_t frames;           /* >= 0 */
+  int32_t channels;         /* 1 .. 64 */
+  int32_t format;           /* VF_PCM_* */
+} vf_pcm_row;
+VF_API int vf_decode_pcm_varlen(vf_ctx* ctx, const void* bytes, int n_rows, const vf_pcm_row* rows, float* mono_out,
+                                double* first_out, void* stream);
 
 /* Live streams resampled from device rings in one call (voicefixer_main_b200/streaming.py StreamingResampler, and the
  * restorers' streams at other rates).  in_ring [n_streams, in_len] (device) holds each stream's recent float32 samples at

@@ -26,7 +26,7 @@ EXPORTS = [
     "vf_score_time_varlen_ex", "vf_restore_chunks", "vf_ssr_restore_chunks", "vf_restore_windows", "vf_ssr_restore_windows",
     "vf_selftest_plan_gemms", "vf_resample_sinc_varlen", "vf_selftest_plan_trace", "vf_vocoder_varlen", "vf_resynth",
     "vf_resynth_varlen", "vf_selftest_sub_batch", "vf_vocoder_chunks", "vf_resample_rings",
-    "vf_remove_higher_frequency_varlen",
+    "vf_remove_higher_frequency_varlen", "vf_decode_pcm_varlen",
 ]
 VF_RESTORE_UNIFY_ENERGY = 1
 VF_TRACE_DIRECT_STEPS = 0x100
@@ -136,6 +136,11 @@ class VfResampleRow(Structure):
                 ("ratio", c_double), ("num_table", c_int32), ("out_stream", c_int32), ("out_offset", c_int64)]
 
 
+class VfPcmRow(Structure):
+    """vf_pcm_row (include/b200vf.h): one WAV data chunk of a vf_decode_pcm_varlen call."""
+    _fields_ = [("byte_offset", c_int64), ("frames", c_int64), ("channels", c_int32), ("format", c_int32)]
+
+
 class EngineError(RuntimeError):
     def __init__(self, code, msg):
         super().__init__(f"libb200vf error {code}: {msg}")
@@ -237,6 +242,7 @@ def load_library():
                                             POINTER(c_int), c_int, POINTER(c_int), P, POINTER(c_int64), P]
     lib.vf_resample_rings.argtypes = [P, P, c_int, c_int64, POINTER(VfResampleRow), c_int, P, c_int, c_int64, P]
     lib.vf_remove_higher_frequency_varlen.argtypes = [P, P, POINTER(c_int64), c_int, c_double, P, POINTER(c_int64), P, P]
+    lib.vf_decode_pcm_varlen.argtypes = [P, P, c_int, POINTER(VfPcmRow), P, P, P]
     _lib = lib
     return lib
 

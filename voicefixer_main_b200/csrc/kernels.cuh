@@ -529,4 +529,20 @@ struct PrefilterParams {
 };
 cudaError_t launch_prefilter(const PrefilterParams& p, cudaStream_t stream);
 
+// pcm.cu: vf_decode_pcm_varlen of one sub-batch of WAV data chunks, one thread per output frame.  Row b's frames start at
+// bytes + byte_off[b], channels[b] interleaved samples of format[b] (VF_PCM_*) each; its outputs are frames
+// out_off[b] .. out_off[b + 1] - 1 of mono (and of first, when not null).
+constexpr int PCM_MAX_ROWS = 1024;                        // keeps PcmParams under the 32 KiB kernel-parameter limit
+struct PcmParams {
+  const uint8_t* bytes;
+  float* mono;
+  double* first;
+  int batch;
+  int64_t out_off[PCM_MAX_ROWS + 1];
+  int64_t byte_off[PCM_MAX_ROWS];
+  int channels[PCM_MAX_ROWS], format[PCM_MAX_ROWS];
+};
+static_assert(sizeof(PcmParams) <= 32764, "the decode table must fit the kernel parameter space");
+cudaError_t launch_decode_pcm(const PcmParams& p, cudaStream_t stream);
+
 }  // namespace vf

@@ -808,6 +808,51 @@ VF_API int vf_remove_higher_frequency_varlen(vf_ctx* ctx, const float* x, const 
   return rc;
 }
 
+// ------------------------------------------------------------------------------------------------ librosa.load's decode
+VF_API int vf_decode_pcm_varlen(vf_ctx* ctx, const void* bytes, int n_rows, const vf_pcm_row* rows, float* mono_out,
+                                double* first_out, void* stream) {
+  static const char* fn = "vf_decode_pcm_varlen";
+  static const int width[] = {1, 2, 3, 4, 4, 8};   // bytes per sample of VF_PCM_U8 .. VF_PCM_F64
+  const int rc = begin_call(ctx, fn, bytes && rows && mono_out && n_rows > 0);
+  if (rc) return rc;
+  const uint8_t* base = static_cast<const uint8_t*>(bytes);
+  for (int i = 0; i < n_rows; ++i) {
+    const vf_pcm_row& r = rows[i];
+    if (r.format < VF_PCM_U8 || r.format > VF_PCM_F64) return fail(ctx, VF_EINVAL, "%s: row %d: format %d", fn, i, r.format);
+    if (r.channels < 1 || r.channels > 64)
+      return fail(ctx, VF_EINVAL, "%s: row %d: %d channels (need 1 .. 64)", fn, i, r.channels);
+    if (r.frames < 0 || r.byte_offset < 0 || r.frames > (INT64_MAX / 512))
+      return fail(ctx, VF_EINVAL, "%s: row %d: %ld frames at byte %ld", fn, i, (long)r.frames, (long)r.byte_offset);
+    const int align = r.format == VF_PCM_S24 ? 1 : width[r.format];
+    if (reinterpret_cast<uintptr_t>(base + r.byte_offset) % align != 0)
+      return fail(ctx, VF_EINVAL, "%s: row %d: %d-byte samples at a misaligned address", fn, i, width[r.format]);
+  }
+  const std::vector<int> starts = split(n_rows, PCM_MAX_ROWS);
+  cudaError_t e = cudaSuccess;
+  int64_t out_at = 0;                    // the first output frame of the sub-batch
+  for (size_t k = 0; k + 1 < starts.size() && e == cudaSuccess; ++k) {
+    const int s = starts[k], nb = starts[k + 1] - starts[k];
+    PcmParams p;
+    memset(&p, 0, sizeof p);
+    p.batch = nb;
+    p.bytes = base;
+    p.mono = mono_out + out_at;
+    p.first = first_out ? first_out + out_at : nullptr;
+    for (int i = 0; i < nb; ++i) {
+      const vf_pcm_row& r = rows[s + i];
+      p.out_off[i + 1] = p.out_off[i] + r.frames;
+      p.byte_off[i] = r.byte_offset;
+      p.channels[i] = r.channels;
+      p.format[i] = r.format;
+    }
+    e = launch_decode_pcm(p, (cudaStream_t)stream);
+    ctx->launches += p.out_off[nb] > 0 ? 1 : 0;
+    out_at += p.out_off[nb];
+  }
+  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "decode launch: %s", cudaGetErrorString(e));
+  return VF_OK;
+}
+
 // ----------------------------------------------------------------------------------------- live streams' rate conversion
 VF_API int vf_resample_rings(vf_ctx* ctx, const float* in_ring, int n_streams, int64_t in_len, const vf_resample_row* rows,
                              int n_rows, float* out, int n_out_streams, int64_t out_len, void* stream) {

@@ -25,7 +25,6 @@
 The filter design is host arithmetic (numpy); every sample / reduction is computed by libb200vf kernels (edges.cu).
 """
 import ctypes
-import wave
 from fractions import Fraction
 
 import numpy as np
@@ -192,16 +191,6 @@ SCORE_KEYS = ("lsd", "non_log_sispec", "sispec", "ssim", "final_mel_lsd", "final
 TIME_KEYS = ("sisdr", "stoi")
 
 
-def first_channel(path) -> np.ndarray:
-    """The first channel of a 16-bit PCM wav as speechmetrics reads it (soundfile, float64 int16 / 32768), held as float32,
-    which represents every such value exactly."""
-    with wave.open(path, "rb") as w:
-        if w.getsampwidth() != 2:
-            raise ValueError(f"{path}: need 16-bit PCM (got {8 * w.getsampwidth()} bit)")
-        data = np.frombuffer(w.readframes(w.getnframes()), dtype=np.int16).reshape(-1, w.getnchannels())
-    return np.ascontiguousarray(data[:, 0].astype(np.float32) / np.float32(32768.0))
-
-
 RATES = (44100, 16000)      # wav_to_spectrogram's two branches (metrics.py:38-47)
 
 
@@ -287,8 +276,8 @@ class AudioMetrics:
         """evaluation(est, target) of every pair, in order, in one vf_score_varlen call: each dict is float-identical to
         evaluation() of that pair.  The instance scores targets at its own rate, 44.1 kHz or 16 kHz (AudioMetrics(owner,
         rate=16000): n_fft 743, hop 160, 80 mels); an est at another rate is resampled to it on the GPU first, as
-        librosa.load(sr=rate) does.  Every file is decoded and checked before any GPU work; a bad pair fails the whole call,
-        naming the file: a target at the other of the two rates (NotImplementedError naming the rate= it needs) or at any
+        librosa.load(sr=rate) does.  Every file is decoded (files other than 16-bit PCM in one vf_decode_pcm_varlen call,
+        see handler.decode_wavs) and checked before any scoring; a bad pair fails the whole call, naming the file: a target at the other of the two rates (NotImplementedError naming the rate= it needs) or at any
         other rate (ValueError), an est whose frame count differs from its target's or a pair of fewer than 7 frames
         (ValueError).  The instance's res_type (None: resample_poly) picks how an est at another rate is resampled; with
         one, every such est goes through one edges.resample call, and the frame check uses librosa's resampled length.
@@ -298,16 +287,20 @@ class AudioMetrics:
         order, without pesq.  The spectral values are those of time_domain=False.  The est must then be at its target's
         rate (ValueError naming it): speechmetrics would compare samples at two rates, which is not reproduced."""
         from .arch import metric_frames
-        from .handler import _rate_len, _to_rate, read_pcm16
+        from .handler import _rate_len, _to_rate, decode_wavs
         rate = self.rate
+        pairs = list(pairs)                  # read twice below: any iterable of pairs
+        live_pairs = [(est, target) for est, target in pairs if target is not None]
+        files = iter(decode_wavs([p for pair in live_pairs for p in pair], self._eng() if live_pairs else None,
+                                 first=time_domain))
         decoded, channels = [], []
         for est, target in pairs:
             if target is None:
                 decoded.append(None)
                 continue
-            t, t_rate = read_pcm16(target)
+            e, e_rate, *e0 = next(files)
+            t, t_rate, *t0 = next(files)
             check_rate(t_rate, target, rate)
-            e, e_rate = read_pcm16(est)
             if time_domain and e_rate != rate:
                 raise ValueError(f"{est} is at {e_rate} Hz: sisdr / stoi need it at its target's {rate} Hz")
             te, tt = metric_frames(_rate_len(len(e), e_rate, rate, self.res_type), rate), metric_frames(len(t), rate)
@@ -317,7 +310,7 @@ class AudioMetrics:
                 raise ValueError(f"{est} / {target}: {tt} frames, fewer than SSIM's 7x7 window")
             decoded.append((est, e, e_rate, t))
             if time_domain:       # 7 frames are more than STOI's one frame at 10 kHz: no check of its own
-                channels.append((first_channel(est), first_channel(target)))
+                channels.append((e0[0], t0[0]))
         live = [d for d in decoded if d is not None]
         results = [{} for _ in decoded]
         if not live:

@@ -2,8 +2,9 @@
 
 Same signature and contract as the reference handler that evaluation_proc/eval.py:128-132 calls:
     handler(input, output, target, ckpt, device, needrefresh=False, meta={}) -> dict of metrics
-It writes a 16-bit wav at `output`.  Differences, all outside the hot path: audio decoding uses the stdlib `wave`
-module (librosa / soundfile are not in this image): PCM16 wav of ANY sample rate, converted to 44.1 kHz on the GPU by
+It writes a 16-bit wav at `output`.  Differences, all outside the hot path: files are read as librosa.load(mono=True)
+reads them through soundfile (which is not in this image): any PCM / IEEE-float WAV (wavfile.parse; 16-bit files decoded
+on the host, the others on the GPU by vf_decode_pcm_varlen) of ANY sample rate, converted to 44.1 kHz on the GPU by
 the polyphase resampler (edges.py; load_wav -> librosa.load(sr=44100), tools/utils.py:46-48), or with meta["res_type"]
 ("kaiser_best" / "kaiser_fast") by librosa 0.8's own resampy filter, as the reference's load_wav does it.  With a `target` the
 per-segment mel metrics of eval_gsr_voicefixer.py:56-64 are computed on the GPU (lsd, sispec, non-log sispec, and with
@@ -18,6 +19,7 @@ from fractions import Fraction
 import numpy as np
 import torch
 
+from . import wavfile
 from ._lib import VF_EINVAL, EngineError
 from .arch import frames_for
 from .model import VoiceFixer, default_hparams
@@ -27,23 +29,63 @@ hp = None
 SEG_LENGTH = 44100 * 60          # eval_gsr_voicefixer.py:47
 
 
+def _mono16(w) -> np.ndarray:
+    """read_pcm16's samples of a parsed 16-bit file (host numpy): int16 / 32768 per channel, then their float32 mean."""
+    data = np.frombuffer(w.data, dtype="<i2").reshape(-1, w.channels)
+    return (data.astype(np.float32) / 32768.0).mean(axis=1).astype(np.float32)
+
+
 def read_pcm16(path):
     """(mono float32 samples in [-1, 1), sample rate) of a 16-bit PCM wav."""
-    with wave.open(path, "rb") as w:
-        if w.getsampwidth() != 2:
-            raise ValueError(f"{path}: need 16-bit PCM (got {8 * w.getsampwidth()} bit)")
-        rate = w.getframerate()
-        data = np.frombuffer(w.readframes(w.getnframes()), dtype=np.int16).reshape(-1, w.getnchannels())
-    return (data.astype(np.float32) / 32768.0).mean(axis=1).astype(np.float32), rate
+    w = wavfile.parse(path)
+    if w.format != wavfile.S16:
+        raise ValueError(f"{path}: need 16-bit PCM (got {wavfile.NAMES[w.format]})")
+    return _mono16(w), w.rate
+
+
+def decode_wavs(paths, engine=None, first=False) -> list:
+    """librosa.load(path, sr=None, mono=True) of every file of `paths` (any WAV wavfile.parse accepts): a list of (mono
+    float32 numpy samples, rate).  16-bit files decode on the host, as read_pcm16 does; every other file of the list is
+    decoded on the GPU by one Engine.decode_pcm_varlen call, so those need an `engine` (ValueError naming engine= without
+    one).  first=True appends each file's channel 0 as speechmetrics reads it (soundfile's float64) held as float32, which
+    holds it exactly for u8, s16, s24 and f32 data; an s32 or f64 file raises ValueError instead.  Every file is parsed
+    and checked before any GPU work."""
+    infos = [wavfile.parse(p) for p in paths]
+    if first:
+        for w in infos:
+            if w.format in (wavfile.S32, wavfile.F64):
+                raise ValueError(f"{w.path}: {wavfile.NAMES[w.format]} samples do not fit float32 exactly; sisdr / stoi "
+                                 f"would score a rounded signal")
+    gpu = [w for w in infos if w.format != wavfile.S16]
+    if gpu and engine is None:
+        raise ValueError(f"{gpu[0].path}: {wavfile.NAMES[gpu[0].format]} WAV data decodes on the GPU (pass "
+                         f"engine=model._engine())")
+    decoded = iter(())
+    if gpu:
+        mono, ch0 = engine.decode_pcm_varlen(gpu, first=first)
+        cut = np.cumsum([w.frames for w in gpu])[:-1]
+        mono = np.split(mono.cpu().numpy(), cut)
+        ch0 = np.split(ch0.float().cpu().numpy(), cut) if first else [None] * len(gpu)
+        decoded = zip(mono, ch0)
+    out = []
+    for w in infos:
+        if w.format == wavfile.S16:
+            x = _mono16(w)
+            c = np.frombuffer(w.data, dtype="<i2")[::w.channels].astype(np.float32) / np.float32(32768.0) if first else None
+        else:
+            x, c = next(decoded)
+        out.append((x, w.rate, c) if first else (x, w.rate))
+    return out
 
 
 def load_wav(path, sample_rate=44100, engine=None, res_type=None):
-    """tools/utils.py:46-48 (librosa.load(path, sr=sample_rate)): decode + convert to `sample_rate`.  Rate conversion
-    runs on the GPU (`engine`, edges.resample_to): resample_poly, or librosa 0.8's resampy filter `res_type`
-    ("kaiser_best", "kaiser_fast"); a file already at the target rate needs no engine."""
+    """tools/utils.py:46-48 (librosa.load(path, sr=sample_rate)): decode + convert to `sample_rate`.  A 16-bit file decodes
+    on the host, any other WAV decode_wavs accepts on the GPU (`engine`).  Rate conversion runs on the GPU (`engine`,
+    edges.resample_to): resample_poly, or librosa 0.8's resampy filter `res_type` ("kaiser_best", "kaiser_fast"); a 16-bit
+    file already at the target rate needs no engine."""
     from .edges import check_res_type
     check_res_type(res_type)
-    return _to_rate(path, *read_pcm16(path), sample_rate, engine, res_type)
+    return _to_rate(path, *decode_wavs([path], engine)[0], sample_rate, engine, res_type)
 
 
 def _to_rate(path, wav, rate, sample_rate, engine, res_type=None):
@@ -220,10 +262,12 @@ def restore_test_set(mdl, items, n_mels, mel_ssim, saturate, restore, score, res
     items = [tuple(it) for it in items]
     if not items:
         return []
+    files = decode_wavs([inp for inp, _, _ in items] + [tgt for _, _, tgt in items if tgt is not None], eng)
+    ins, tgt_files = iter(files[:len(items)]), iter(files[len(items):])
     decoded = []
     for inp, _, tgt in items:
-        x = read_pcm16(inp)
-        t = read_pcm16(tgt) if tgt is not None else None
+        x = next(ins)
+        t = next(tgt_files) if tgt is not None else None
         _check_file(inp, _rate_len(len(x[0]), x[1], 44100, res_type),
                     None if t is None else _rate_len(len(t[0]), t[1], 44100, res_type), mel_ssim=mel_ssim)
         decoded.append((x, t))

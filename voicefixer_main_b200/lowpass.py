@@ -282,7 +282,7 @@ def sr_validation_inputs(eng, wavs, cutoffs=SR_CUTOFFS):
 
 
 def make_sr_testset(eng, clean_paths, out_dir, cutoffs=SR_CUTOFFS, list_type="cheby1"):
-    """Write sr_validation_inputs of 44.1 kHz 16-bit PCM clean files (read as read_pcm16 reads them) as
+    """Write sr_validation_inputs of 44.1 kHz clean WAV files (any format, decoded in one handler.decode_wavs call) as
     out_dir/<list_type>/<c>/<file name> (16-bit PCM as save_wave converts it) and, per cutoff, the pair list
     out_dir/<list_type>/pair_<list_type>_<c>.lst of "degraded clean" lines in evaluation_proc/config.py's format, which
     handler_batch and evaluation_batch items can be read from.  Returns {c: list path}.
@@ -293,9 +293,10 @@ def make_sr_testset(eng, clean_paths, out_dir, cutoffs=SR_CUTOFFS, list_type="ch
 
     Every file is checked before any GPU work or write: a path with white space, two clean files of one name (their
     degraded copies would overwrite each other) or a file not at 44.1 kHz raises ValueError naming it."""
-    from .handler import read_pcm16, save_pcm16
+    from .handler import decode_wavs, save_pcm16
     eng = _eng(eng)
-    clean, names = [], {}
+    clean_paths = list(clean_paths)          # read three times below: any iterable of paths
+    names = {}
     for path in clean_paths:
         if any(ch.isspace() for ch in str(path)) or any(ch.isspace() for ch in str(out_dir)):
             raise ValueError(f"{path}: the pair-list format cannot hold paths with white space")
@@ -303,7 +304,8 @@ def make_sr_testset(eng, clean_paths, out_dir, cutoffs=SR_CUTOFFS, list_type="ch
         if name in names:
             raise ValueError(f"{path} and {names[name]} share the file name {name}: their degraded copies would collide")
         names[name] = path
-        x, rate = read_pcm16(path)
+    clean = []
+    for path, (x, rate) in zip(clean_paths, decode_wavs(clean_paths, eng)):
         if rate != 44100:
             raise ValueError(f"{path} is at {rate} Hz: the SR recipe needs 44.1 kHz input")
         clean.append(x)

@@ -550,6 +550,29 @@ class Engine:
                                                                 _ptr(cutoff), _stream()))
         return out, out_lengths, cutoff
 
+    def decode_pcm_varlen(self, files, first: bool = False):
+        """vf_decode_pcm_varlen: librosa.load(path, sr=None, mono=True)'s samples of every wavfile.WavInfo of `files` ->
+        (mono float32 [sum frames], channel 0 float64 [sum frames] or None), file i at rows sum_{j<i} frames_j.  The data
+        chunks go to one pinned staging buffer, each at a 16-byte aligned offset, and to the device in one copy."""
+        files = list(files)
+        at, end = [], 0
+        for w in files:
+            at.append(end)
+            end += (len(w.data) + 15) // 16 * 16
+        staging = torch.empty(max(end, 16), dtype=torch.uint8, pin_memory=True)
+        host = staging.numpy()
+        for w, a in zip(files, at):
+            host[a:a + len(w.data)] = np.frombuffer(w.data, dtype=np.uint8)
+        dev = staging.to(self.device, non_blocking=True)
+        rows = (L.VfPcmRow * max(1, len(files)))(*[L.VfPcmRow(a, w.frames, w.channels, w.format) for w, a in zip(files, at)])
+        n = sum(w.frames for w in files)
+        mono = torch.empty(n, device=self.device)
+        ch0 = torch.empty(n, dtype=torch.float64, device=self.device) if first else None
+        if files:
+            with torch.cuda.device(self.device):
+                self._ck(self.lib.vf_decode_pcm_varlen(self.ctx, _ptr(dev), len(files), rows, _ptr(mono), _ptr(ch0), _stream()))
+        return mono, ch0
+
     def resample_rings(self, in_ring: torch.Tensor, rows, out: torch.Tensor) -> torch.Tensor:
         """Live streams resampled from a device ring in one call (vf_resample_rings).  in_ring [n_streams, in_len] float32
         holds stream s's absolute input i at in_ring[s, i % in_len].  rows is a sequence of (stream, filter, m0, m1, n, avail,
