@@ -60,6 +60,8 @@
  *   vf_remove_higher_frequency_varlen  the pip package's mode-1 pre-filter, remove_higher_frequency, before a restore
  *   vf_decode_pcm_varlen          the decode and downmix of librosa.load(path, mono=True) (tools/utils.py:46-48,
  *                                 metrics.py:33-34) for 8-, 16-, 24-, 32-bit and float WAV data of any channel count
+ *   vf_decode_flac_varlen         the same files as FLAC (8-, 16- and 24-bit, 1 .. 8 channels), decoded into the bytes of
+ *                                 a WAV data chunk holding the same samples, which vf_decode_pcm_varlen then converts
  *
  * Conventions: every function returns 0 on success or a negative VF_E* code and never throws; the message is
  * available from vf_last_error().  All tensor arguments are contiguous fp32.  Unless a name ends in `_host`,
@@ -521,6 +523,51 @@ typedef struct vf_pcm_row {
 } vf_pcm_row;
 VF_API int vf_decode_pcm_varlen(vf_ctx* ctx, const void* bytes, int n_rows, const vf_pcm_row* rows, float* mono_out,
                                 double* first_out, void* stream);
+
+/* The FLAC audio (RFC 9639) of `n_rows` files, decoded as libsndfile's read of a FLAC file returns it, into the bytes of
+ * a WAV data chunk holding the same samples: interleaved little-endian u8 (stored as v + 128), s16 or s24.  Those bytes
+ * are what vf_decode_pcm_varlen converts, so a FLAC file's samples are the WAV path's bit for bit.  bytes: one device
+ * buffer; rows: HOST table (read during the call only).  Row i's audio region (its frames, from the first frame's sync code
+ * to the end of the file, as voicefixer_main_b200/flacfile.py finds it) is `nbytes` bytes at bytes + byte_offset, which is
+ * a multiple of 8; the bytes up to the next multiple of 8 after the region must be readable.  Its STREAMINFO facts:
+ * total_samples (> 0) per channel, channels (1 .. 8), bits (8, 16, 24), rate, the blocking strategy (`variable`: 0 fixed,
+ * 1 variable) and first_block, the first frame's block size (the frame-number multiplier under fixed blocking).  Its
+ * total_samples x channels x bits / 8 output bytes go to pcm + pcm_offset.  Every subframe type, wasted bits, the four
+ * channel assignments, both Rice codings with escapes and partition orders 0 .. 15 are decoded.  status (device,
+ * n_rows): all ones for a row that decoded, else (byte << 8) | VF_FLAC_E* of its first bad frame, `byte` counted from
+ * the start of its region; the output of a row whose status is not all ones, and of the whole call, must not be used.
+ * Every argument is checked before any work is queued (VF_EINVAL, naming the row).  Sub-batches of at most 512 rows and
+ * 64 MiB of FLAC data (a larger file runs alone); per sub-batch, four kernel launches and a context-owned scratch of 4 bytes
+ * per FLAC byte, 13 bytes per 8 FLAC bytes (frame candidates, each row with its own share) and 4 bytes per decoded sample.  One thread per FLAC byte
+ * finds candidate frames (sync code, header, CRC-8, agreement with STREAMINFO), one per candidate walks its subframes to
+ * its end and checks CRC-16, one per row chains the frames from the first (a header-shaped pattern inside a frame never
+ * changes the result), then one per chained frame decodes it.  No host synchronisation. */
+#define VF_FLAC_ENOSYNC 1      /* no frame sync code where a frame must start */
+#define VF_FLAC_ERESERVED 2    /* a reserved or forbidden code in a frame header */
+#define VF_FLAC_EMISMATCH 3    /* a frame header disagrees with STREAMINFO (channels, bit depth, rate, blocking) */
+#define VF_FLAC_ECRC8 4        /* frame header CRC-8 mismatch */
+#define VF_FLAC_ESUBFRAME 5    /* a reserved or forbidden subframe code (type, LPC precision, negative shift, coding) */
+#define VF_FLAC_EPARTITION 6   /* invalid residual partitioning */
+#define VF_FLAC_ETRUNCATED 7   /* a frame runs past the end of the data */
+#define VF_FLAC_ECRC16 8       /* frame CRC-16 mismatch */
+#define VF_FLAC_ERANGE 9       /* a decoded sample (or residual) outside its bit depth's range */
+#define VF_FLAC_ESEQUENCE 10   /* a frame or sample number out of sequence, or a short fixed-blocking frame before the last */
+#define VF_FLAC_ELENGTH 11     /* the frames' sample counts do not add up to STREAMINFO's total */
+#define VF_FLAC_ECANDIDATES 12 /* more candidate frames in a row than one per 8 of its bytes */
+typedef struct vf_flac_row {
+  int64_t byte_offset;      /* of the row's first frame in `bytes`, a multiple of 8 */
+  int64_t nbytes;           /* of its audio region, > 0 */
+  int64_t total_samples;    /* per channel, > 0 */
+  int64_t pcm_offset;       /* of its first output byte in `pcm` */
+  int32_t channels;         /* 1 .. 8 */
+  int32_t bits;             /* 8, 16, 24 */
+  int32_t rate;             /* > 0 */
+  int32_t variable;         /* 0: fixed blocking, 1: variable blocking */
+  int32_t first_block;      /* 1 .. 65535 */
+  int32_t pad_;
+} vf_flac_row;
+VF_API int vf_decode_flac_varlen(vf_ctx* ctx, const void* bytes, int n_rows, const vf_flac_row* rows, void* pcm,
+                                 unsigned long long* status, void* stream);
 
 /* Live streams resampled from device rings in one call (voicefixer_main_b200/streaming.py StreamingResampler, and the
  * restorers' streams at other rates).  in_ring [n_streams, in_len] (device) holds each stream's recent float32 samples at

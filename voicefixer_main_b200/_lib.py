@@ -26,7 +26,7 @@ EXPORTS = [
     "vf_score_time_varlen_ex", "vf_restore_chunks", "vf_ssr_restore_chunks", "vf_restore_windows", "vf_ssr_restore_windows",
     "vf_selftest_plan_gemms", "vf_resample_sinc_varlen", "vf_selftest_plan_trace", "vf_vocoder_varlen", "vf_resynth",
     "vf_resynth_varlen", "vf_selftest_sub_batch", "vf_vocoder_chunks", "vf_resample_rings",
-    "vf_remove_higher_frequency_varlen", "vf_decode_pcm_varlen",
+    "vf_remove_higher_frequency_varlen", "vf_decode_pcm_varlen", "vf_decode_flac_varlen",
 ]
 VF_RESTORE_UNIFY_ENERGY = 1
 VF_TRACE_DIRECT_STEPS = 0x100
@@ -141,6 +141,13 @@ class VfPcmRow(Structure):
     _fields_ = [("byte_offset", c_int64), ("frames", c_int64), ("channels", c_int32), ("format", c_int32)]
 
 
+class VfFlacRow(Structure):
+    """vf_flac_row (include/b200vf.h): one FLAC file's audio region of a vf_decode_flac_varlen call."""
+    _fields_ = [("byte_offset", c_int64), ("nbytes", c_int64), ("total_samples", c_int64), ("pcm_offset", c_int64),
+                ("channels", c_int32), ("bits", c_int32), ("rate", c_int32), ("variable", c_int32), ("first_block", c_int32),
+                ("pad_", c_int32)]
+
+
 class EngineError(RuntimeError):
     def __init__(self, code, msg):
         super().__init__(f"libb200vf error {code}: {msg}")
@@ -243,6 +250,7 @@ def load_library():
     lib.vf_resample_rings.argtypes = [P, P, c_int, c_int64, POINTER(VfResampleRow), c_int, P, c_int, c_int64, P]
     lib.vf_remove_higher_frequency_varlen.argtypes = [P, P, POINTER(c_int64), c_int, c_double, P, POINTER(c_int64), P, P]
     lib.vf_decode_pcm_varlen.argtypes = [P, P, c_int, POINTER(VfPcmRow), P, P, P]
+    lib.vf_decode_flac_varlen.argtypes = [P, P, c_int, POINTER(VfFlacRow), P, P, P]
     _lib = lib
     return lib
 

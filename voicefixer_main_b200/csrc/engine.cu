@@ -1163,7 +1163,7 @@ VF_API void vf_destroy(vf_ctx* ctx) {
     if (st) cudaStreamDestroy(st);
   for (auto& e : ctx->ev)
     if (e) cudaEventDestroy(e);
-  for (Scratch* s : {&ctx->score, &ctx->time_score, &ctx->iir, &ctx->chunks, &ctx->prefilter}) {
+  for (Scratch* s : {&ctx->score, &ctx->time_score, &ctx->iir, &ctx->chunks, &ctx->prefilter, &ctx->flac}) {
     if (s->p) cudaFree(s->p);
     if (s->order.ev) cudaEventDestroy(s->order.ev);
   }

@@ -236,6 +236,8 @@ struct vf_ctx {
   Scratch chunks;
   // vf_remove_higher_frequency_varlen: the float64 spectra (then frames) of its largest sub-batch
   Scratch prefilter;
+  // vf_decode_flac_varlen: the frame search tables and the int32 samples of its largest sub-batch
+  Scratch flac;
   // vf_score_time_varlen's float64 tables (resampling taps, window, twiddles), one per rate (44.1, 16 kHz; first use)
   double* d_stoi_tables[2] = {nullptr, nullptr};
   int stoi_half[2] = {0, 0};         // their resampling filters' half lengths

@@ -545,4 +545,31 @@ struct PcmParams {
 static_assert(sizeof(PcmParams) <= 32764, "the decode table must fit the kernel parameter space");
 cudaError_t launch_decode_pcm(const PcmParams& p, cudaStream_t stream);
 
+// flac.cu: vf_decode_flac_varlen of one sub-batch of FLAC audio regions.  Row b's region is bytes + byte_off[b] (8-byte
+// aligned), scan_off[b + 1] - scan_off[b] bytes long; byte j of it is scan element scan_off[b] + j.  Its PCM output starts
+// at pcm + pcm_off[b]; its int32 working samples at smp + smp_off[b] (total[b] * channels[b] of them).  Scratch, per scan
+// element: ends; per candidate slot (cap of them, row b's from (scan_off[b] >> 3) + 2b): cand_at (scan element of its sync
+// code), cand_len (its length in bytes, or -FLAC_E*), chained (1 when the row's chain takes it); count[b]: row b's number of
+// candidates.  status[b]: (byte << 8) | code of the row's first error (atomicMin), all ones when there is none.
+constexpr int FLAC_MAX_ROWS = 512;                        // keeps FlacParams under the 32 KiB kernel-parameter limit
+struct FlacParams {
+  const uint8_t* bytes;
+  uint8_t* pcm;
+  unsigned long long* status;
+  int32_t* ends;
+  int32_t* smp;
+  int64_t* cand_at;
+  int32_t* cand_len;
+  uint8_t* chained;
+  int* count;
+  int64_t cap;
+  int batch;
+  int64_t scan_off[FLAC_MAX_ROWS + 1];
+  int64_t byte_off[FLAC_MAX_ROWS], total[FLAC_MAX_ROWS], pcm_off[FLAC_MAX_ROWS], smp_off[FLAC_MAX_ROWS];
+  int32_t channels[FLAC_MAX_ROWS], bits[FLAC_MAX_ROWS], rate[FLAC_MAX_ROWS], first_block[FLAC_MAX_ROWS];
+  uint8_t variable[FLAC_MAX_ROWS];
+};
+static_assert(sizeof(FlacParams) <= 32764, "the FLAC table must fit the kernel parameter space");
+cudaError_t launch_decode_flac(const FlacParams& p, cudaStream_t stream);
+
 }  // namespace vf

@@ -853,6 +853,86 @@ VF_API int vf_decode_pcm_varlen(vf_ctx* ctx, const void* bytes, int n_rows, cons
   return VF_OK;
 }
 
+// ------------------------------------------------------------------------------------------------- FLAC frames to PCM
+constexpr int64_t FLAC_CAP_BYTES = int64_t(64) << 20;   // FLAC bytes per sub-batch; a larger file runs alone
+
+VF_API int vf_decode_flac_varlen(vf_ctx* ctx, const void* bytes, int n_rows, const vf_flac_row* rows, void* pcm,
+                                 unsigned long long* status, void* stream) {
+  static const char* fn = "vf_decode_flac_varlen";
+  int rc = begin_call(ctx, fn, bytes && rows && pcm && status && n_rows > 0);
+  if (rc) return rc;
+  const uint8_t* base = static_cast<const uint8_t*>(bytes);
+  for (int i = 0; i < n_rows; ++i) {
+    const vf_flac_row& r = rows[i];
+    if (r.byte_offset < 0 || r.byte_offset % 8 || r.nbytes <= 0 || r.nbytes > (int64_t(1) << 40) ||
+        reinterpret_cast<uintptr_t>(base + r.byte_offset) % 8)
+      return fail(ctx, VF_EINVAL, "%s: row %d: %ld bytes at byte %ld (need > 0 bytes at a multiple of 8)", fn, i, (long)r.nbytes,
+                  (long)r.byte_offset);
+    if (r.channels < 1 || r.channels > 8) return fail(ctx, VF_EINVAL, "%s: row %d: %d channels (need 1 .. 8)", fn, i, r.channels);
+    if (r.bits != 8 && r.bits != 16 && r.bits != 24) return fail(ctx, VF_EINVAL, "%s: row %d: %d bits (need 8, 16 or 24)", fn, i, r.bits);
+    if (r.total_samples <= 0 || r.total_samples > (int64_t(1) << 36) || r.pcm_offset < 0 || r.rate <= 0)
+      return fail(ctx, VF_EINVAL, "%s: row %d: %ld samples at %d Hz to byte %ld", fn, i, (long)r.total_samples, r.rate,
+                  (long)r.pcm_offset);
+    if (r.variable != 0 && r.variable != 1) return fail(ctx, VF_EINVAL, "%s: row %d: blocking strategy %d", fn, i, r.variable);
+    if (r.first_block < 1 || r.first_block > 65535)
+      return fail(ctx, VF_EINVAL, "%s: row %d: first block size %d (need 1 .. 65535)", fn, i, r.first_block);
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  // scratch of a sub-batch: the per-row candidate counters, ends (int32 per FLAC byte), its working samples (int32), then
+  // the candidate tables, each 16-byte aligned.  A sub-batch has (sum of nbytes) / 8 + 2 nb candidate slots, which
+  // sum_i (nbytes_i / 8 + 3) bounds.
+  auto al = [](size_t n) { return (n + 15) / 16 * 16; };
+  auto cap_of = [&](int i) { return rows[i].nbytes / 8 + 3; };
+  const std::vector<int> starts = split(n_rows, FLAC_MAX_ROWS, FLAC_CAP_BYTES, [&](int i) { return rows[i].nbytes; });
+  rc = acquire_scratch(ctx, ctx->flac, al(4 * FLAC_MAX_ROWS) + max_bytes(starts, [&](int i) {
+    return al(4 * rows[i].nbytes) + al(4 * rows[i].total_samples * rows[i].channels) + 13 * cap_of(i) + 48;
+  }), st);
+  if (rc) return rc;
+  cudaError_t e = cudaMemsetAsync(status, 0xFF, sizeof(unsigned long long) * n_rows, st);
+  for (size_t k = 0; k + 1 < starts.size() && e == cudaSuccess; ++k) {
+    const int s = starts[k], nb = starts[k + 1] - starts[k];
+    FlacParams p;
+    memset(&p, 0, sizeof p);
+    p.batch = nb;
+    p.bytes = base;
+    p.pcm = static_cast<uint8_t*>(pcm);
+    p.status = status + s;
+    int64_t smp = 0;
+    for (int i = 0; i < nb; ++i) {
+      const vf_flac_row& r = rows[s + i];
+      p.scan_off[i + 1] = p.scan_off[i] + r.nbytes;
+      p.byte_off[i] = r.byte_offset;
+      p.total[i] = r.total_samples;
+      p.pcm_off[i] = r.pcm_offset;
+      p.smp_off[i] = smp;
+      smp += r.total_samples * r.channels;
+      p.channels[i] = r.channels;
+      p.bits[i] = r.bits;
+      p.rate[i] = r.rate;
+      p.first_block[i] = r.first_block;
+      p.variable[i] = (uint8_t)r.variable;
+    }
+    p.cap = (p.scan_off[nb] >> 3) + 2 * (int64_t)nb;      // row b's slots from (scan_off[b] >> 3) + 2 b (flac.cu)
+    char* at = static_cast<char*>(ctx->flac.p);
+    p.count = reinterpret_cast<int*>(at);
+    at += al(4 * FLAC_MAX_ROWS);
+    p.ends = reinterpret_cast<int32_t*>(at);
+    at += al(4 * p.scan_off[nb]);
+    p.smp = reinterpret_cast<int32_t*>(at);
+    at += al(4 * smp);
+    p.cand_at = reinterpret_cast<int64_t*>(at);
+    at += al(8 * p.cap);
+    p.cand_len = reinterpret_cast<int32_t*>(at);
+    at += al(4 * p.cap);
+    p.chained = reinterpret_cast<uint8_t*>(at);
+    e = launch_decode_flac(p, st);
+    ctx->launches += 4;
+  }
+  rc = mark_use(ctx, ctx->flac.order, st);
+  if (e != cudaSuccess) return fail(ctx, VF_ECUDA, "FLAC decode launch: %s", cudaGetErrorString(e));
+  return rc;
+}
+
 // ----------------------------------------------------------------------------------------- live streams' rate conversion
 VF_API int vf_resample_rings(vf_ctx* ctx, const float* in_ring, int n_streams, int64_t in_len, const vf_resample_row* rows,
                              int n_rows, float* out, int n_out_streams, int64_t out_len, void* stream) {

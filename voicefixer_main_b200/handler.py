@@ -4,7 +4,8 @@ Same signature and contract as the reference handler that evaluation_proc/eval.p
     handler(input, output, target, ckpt, device, needrefresh=False, meta={}) -> dict of metrics
 It writes a 16-bit wav at `output`.  Differences, all outside the hot path: files are read as librosa.load(mono=True)
 reads them through soundfile (which is not in this image): any PCM / IEEE-float WAV (wavfile.parse; 16-bit files decoded
-on the host, the others on the GPU by vf_decode_pcm_varlen) of ANY sample rate, converted to 44.1 kHz on the GPU by
+on the host, the others on the GPU by vf_decode_pcm_varlen) or 8-, 16- or 24-bit FLAC (flacfile.parse, decoded on the GPU by
+vf_decode_flac_varlen) of ANY sample rate, converted to 44.1 kHz on the GPU by
 the polyphase resampler (edges.py; load_wav -> librosa.load(sr=44100), tools/utils.py:46-48), or with meta["res_type"]
 ("kaiser_best" / "kaiser_fast") by librosa 0.8's own resampy filter, as the reference's load_wav does it.  With a `target` the
 per-segment mel metrics of eval_gsr_voicefixer.py:56-64 are computed on the GPU (lsd, sispec, non-log sispec, and with
@@ -19,7 +20,7 @@ from fractions import Fraction
 import numpy as np
 import torch
 
-from . import wavfile
+from . import flacfile, wavfile
 from ._lib import VF_EINVAL, EngineError
 from .arch import frames_for
 from .model import VoiceFixer, default_hparams
@@ -43,44 +44,62 @@ def read_pcm16(path):
     return _mono16(w), w.rate
 
 
+def _parse(path):
+    """wavfile.parse or flacfile.parse of `path`, chosen by its leading bytes as libsndfile chooses (`fLaC`, or an ID3v2
+    tag before it, is FLAC), not by its name."""
+    with open(path, "rb") as f:
+        head = f.read(4)
+    return flacfile.parse(path) if flacfile.is_flac(head) else wavfile.parse(path)
+
+
 def decode_wavs(paths, engine=None, first=False) -> list:
-    """librosa.load(path, sr=None, mono=True) of every file of `paths` (any WAV wavfile.parse accepts): a list of (mono
-    float32 numpy samples, rate).  16-bit files decode on the host, as read_pcm16 does; every other file of the list is
-    decoded on the GPU by one Engine.decode_pcm_varlen call, so those need an `engine` (ValueError naming engine= without
-    one).  first=True appends each file's channel 0 as speechmetrics reads it (soundfile's float64) held as float32, which
-    holds it exactly for u8, s16, s24 and f32 data; an s32 or f64 file raises ValueError instead.  Every file is parsed
-    and checked before any GPU work."""
-    infos = [wavfile.parse(p) for p in paths]
+    """librosa.load(path, sr=None, mono=True) of every file of `paths` (any WAV wavfile.parse accepts, any FLAC
+    flacfile.parse accepts): a list of (mono float32 numpy samples, rate).  16-bit WAV files decode on the host, as
+    read_pcm16 does; the other WAV files of the list are decoded on the GPU by one Engine.decode_pcm_varlen call and the
+    FLAC files by one Engine.decode_flac_varlen call, so those need an `engine` (ValueError naming engine= without one).
+    first=True appends each file's channel 0 as speechmetrics reads it (soundfile's float64) held as float32, which holds it
+    exactly for u8, s16, s24 and f32 data and for every FLAC; an s32 or f64 WAV raises ValueError instead.  Every file is
+    parsed and checked before any GPU work."""
+    infos = [_parse(p) for p in paths]
+    flac = [w for w in infos if isinstance(w, flacfile.FlacInfo)]
+    wavs = [w for w in infos if not isinstance(w, flacfile.FlacInfo)]
     if first:
-        for w in infos:
+        for w in wavs:
             if w.format in (wavfile.S32, wavfile.F64):
                 raise ValueError(f"{w.path}: {wavfile.NAMES[w.format]} samples do not fit float32 exactly; sisdr / stoi "
                                  f"would score a rounded signal")
-    gpu = [w for w in infos if w.format != wavfile.S16]
+    gpu = [w for w in wavs if w.format != wavfile.S16]
     if gpu and engine is None:
         raise ValueError(f"{gpu[0].path}: {wavfile.NAMES[gpu[0].format]} WAV data decodes on the GPU (pass "
                          f"engine=model._engine())")
-    decoded = iter(())
-    if gpu:
-        mono, ch0 = engine.decode_pcm_varlen(gpu, first=first)
-        cut = np.cumsum([w.frames for w in gpu])[:-1]
+    if flac and engine is None:
+        raise ValueError(f"{flac[0].path}: FLAC decodes on the GPU (pass engine=model._engine())")
+
+    def split(files, decoded, frames):
+        mono, ch0 = decoded
+        cut = np.cumsum(frames)[:-1]
         mono = np.split(mono.cpu().numpy(), cut)
-        ch0 = np.split(ch0.float().cpu().numpy(), cut) if first else [None] * len(gpu)
-        decoded = zip(mono, ch0)
+        ch0 = np.split(ch0.float().cpu().numpy(), cut) if first else [None] * len(files)
+        return zip(mono, ch0)
+
+    pcm_decoded = split(gpu, engine.decode_pcm_varlen(gpu, first=first), [w.frames for w in gpu]) if gpu else iter(())
+    flac_decoded = split(flac, engine.decode_flac_varlen(flac, first=first), [w.total for w in flac]) if flac else iter(())
     out = []
     for w in infos:
-        if w.format == wavfile.S16:
+        if isinstance(w, flacfile.FlacInfo):
+            x, c = next(flac_decoded)
+        elif w.format == wavfile.S16:
             x = _mono16(w)
             c = np.frombuffer(w.data, dtype="<i2")[::w.channels].astype(np.float32) / np.float32(32768.0) if first else None
         else:
-            x, c = next(decoded)
+            x, c = next(pcm_decoded)
         out.append((x, w.rate, c) if first else (x, w.rate))
     return out
 
 
 def load_wav(path, sample_rate=44100, engine=None, res_type=None):
     """tools/utils.py:46-48 (librosa.load(path, sr=sample_rate)): decode + convert to `sample_rate`.  A 16-bit file decodes
-    on the host, any other WAV decode_wavs accepts on the GPU (`engine`).  Rate conversion runs on the GPU (`engine`,
+    on the host, any other WAV or FLAC decode_wavs accepts on the GPU (`engine`).  Rate conversion runs on the GPU (`engine`,
     edges.resample_to): resample_poly, or librosa 0.8's resampy filter `res_type` ("kaiser_best", "kaiser_fast"); a 16-bit
     file already at the target rate needs no engine."""
     from .edges import check_res_type

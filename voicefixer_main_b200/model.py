@@ -550,28 +550,79 @@ class Engine:
                                                                 _ptr(cutoff), _stream()))
         return out, out_lengths, cutoff
 
+    def _stage(self, buffers, align: int = 16):
+        """The byte buffers `buffers` in one pinned staging buffer, each at an `align`-byte aligned offset, sent to the
+        device in one copy -> (device uint8 tensor, offsets)."""
+        at, end = [], 0
+        for b in buffers:
+            at.append(end)
+            end += (len(b) + align - 1) // align * align
+        staging = torch.empty(end + align, dtype=torch.uint8, pin_memory=True)
+        host = staging.numpy()
+        for b, a in zip(buffers, at):
+            host[a:a + len(b)] = np.frombuffer(b, dtype=np.uint8)
+        return staging.to(self.device, non_blocking=True), at
+
+    def _decode_pcm_rows(self, dev, rows, first: bool):
+        """vf_decode_pcm_varlen of the (byte offset, frames, channels, format) rows of the device bytes `dev`."""
+        table = (L.VfPcmRow * max(1, len(rows)))(*[L.VfPcmRow(*r) for r in rows])
+        n = sum(r[1] for r in rows)
+        mono = torch.empty(n, device=self.device)
+        ch0 = torch.empty(n, dtype=torch.float64, device=self.device) if first else None
+        if rows:
+            with torch.cuda.device(self.device):
+                self._ck(self.lib.vf_decode_pcm_varlen(self.ctx, _ptr(dev), len(rows), table, _ptr(mono), _ptr(ch0), _stream()))
+        return mono, ch0
+
     def decode_pcm_varlen(self, files, first: bool = False):
         """vf_decode_pcm_varlen: librosa.load(path, sr=None, mono=True)'s samples of every wavfile.WavInfo of `files` ->
         (mono float32 [sum frames], channel 0 float64 [sum frames] or None), file i at rows sum_{j<i} frames_j.  The data
         chunks go to one pinned staging buffer, each at a 16-byte aligned offset, and to the device in one copy."""
         files = list(files)
-        at, end = [], 0
+        dev, at = self._stage([w.data for w in files])
+        return self._decode_pcm_rows(dev, [(a, w.frames, w.channels, w.format) for w, a in zip(files, at)], first)
+
+    def flac_pcm(self, files):
+        """vf_decode_flac_varlen: the samples of every flacfile.FlacInfo of `files` as the bytes of a WAV data chunk
+        (interleaved little-endian u8 as v + 128, s16 or s24) -> (device uint8 buffer, byte offset of each file's bytes).
+        The audio regions go to the device in one copy.  A file the decoder rejects raises ValueError naming it, the reason
+        and the file offset of the first bad frame; this reads the per-file status back, the call's one synchronisation."""
+        from .flacfile import ERRORS
+        files = list(files)
+        if not files:
+            return torch.empty(0, dtype=torch.uint8, device=self.device), []
+        dev, at = self._stage([w.audio for w in files])
+        out, end = [], 0
         for w in files:
-            at.append(end)
-            end += (len(w.data) + 15) // 16 * 16
-        staging = torch.empty(max(end, 16), dtype=torch.uint8, pin_memory=True)
-        host = staging.numpy()
-        for w, a in zip(files, at):
-            host[a:a + len(w.data)] = np.frombuffer(w.data, dtype=np.uint8)
-        dev = staging.to(self.device, non_blocking=True)
-        rows = (L.VfPcmRow * max(1, len(files)))(*[L.VfPcmRow(a, w.frames, w.channels, w.format) for w, a in zip(files, at)])
-        n = sum(w.frames for w in files)
-        mono = torch.empty(n, device=self.device)
-        ch0 = torch.empty(n, dtype=torch.float64, device=self.device) if first else None
-        if files:
-            with torch.cuda.device(self.device):
-                self._ck(self.lib.vf_decode_pcm_varlen(self.ctx, _ptr(dev), len(files), rows, _ptr(mono), _ptr(ch0), _stream()))
-        return mono, ch0
+            out.append(end)
+            end += (w.total * w.channels * (w.bits // 8) + 15) // 16 * 16
+        pcm = torch.empty(max(end, 16), dtype=torch.uint8, device=self.device)
+        status = torch.empty(len(files), dtype=torch.int64, device=self.device)
+        rows = (L.VfFlacRow * len(files))(*[L.VfFlacRow(a, len(w.audio), w.total, o, w.channels, w.bits, w.rate, w.variable,
+                                                        w.first_block, 0) for w, a, o in zip(files, at, out)])
+        with torch.cuda.device(self.device):
+            self._ck(self.lib.vf_decode_flac_varlen(self.ctx, _ptr(dev), len(files), rows, _ptr(pcm), _ptr(status), _stream()))
+        for w, st in zip(files, status.cpu().tolist()):
+            if st != -1:
+                byte, code = (st & (1 << 64) - 1) >> 8, st & 0xFF
+                raise ValueError(f"{w.path}: {ERRORS.get(code, f'FLAC error {code}')} (frame at byte {w.audio_start + byte})")
+        return pcm, out
+
+    def decode_flac_varlen(self, files, first: bool = False):
+        """librosa.load(path, sr=None, mono=True)'s samples of every flacfile.FlacInfo of `files`, as decode_pcm_varlen
+        returns them: the FLAC frames decode to WAV data bytes on the device (flac_pcm), which vf_decode_pcm_varlen then
+        converts and downmixes, so the result is the WAV path's for the same samples, bit for bit."""
+        files = list(files)
+        pcm, out = self.flac_pcm(files)
+        fmt = {8: 0, 16: 1, 24: 2}                         # VF_PCM_U8, VF_PCM_S16, VF_PCM_S24
+        return self._decode_pcm_rows(pcm, [(o, w.total, w.channels, fmt[w.bits]) for w, o in zip(files, out)], first)
+
+    def decode_flac_pcm(self, files) -> list:
+        """The WAV data bytes of every flacfile.FlacInfo of `files` (flac_pcm), as host numpy uint8 arrays."""
+        files = list(files)
+        pcm, out = self.flac_pcm(files)
+        host = pcm.cpu().numpy()
+        return [host[o:o + w.total * w.channels * (w.bits // 8)] for w, o in zip(files, out)]
 
     def resample_rings(self, in_ring: torch.Tensor, rows, out: torch.Tensor) -> torch.Tensor:
         """Live streams resampled from a device ring in one call (vf_resample_rings).  in_ring [n_streams, in_len] float32
